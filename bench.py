@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 rANS hot path (BASELINE.json metric).
+"""bench.py -- headline benchmark of the rANS hot path on one H100 (BASELINE.json metric).
 
 Step      = one bit-exact round trip of the hot path over one batch: encode the
             batch (rb200_encode: encode kernel + directory scan + compaction), then
@@ -14,6 +14,8 @@ roofline  = the decode kernel (the north-star kernel) against measured HBM copy 
             the encode call is reported beside it.
 --impl reference times the reference's own CPU coders (oracle/_ref, built from the
 reference sources) on all host cores on a bounded sample of the same workload.
+--dump-outputs DIR writes what the last timed step of every measured workload returned (see
+dump_outputs) for output-for-output comparison of two builds; the inputs are seeded, so identical per run.
 """
 import argparse
 import json
@@ -60,6 +62,9 @@ def parse_args():
     ap.add_argument("--e2e-steps", type=int, default=5)
     ap.add_argument("--cpu-sample", type=int, default=256 << 20, help="bytes of the workload the in-line CPU baseline is timed on")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the last timed step's outputs of every measured workload to DIR: the headline workload's "
+                         "as DIR/<name>.npy, each other config's as DIR/<workload>__<name>.npy (at most 64 MB in all)")
     return ap.parse_args()
 
 
@@ -168,9 +173,9 @@ class ClockSampler:
 
 
 def ncu_traffic(workload, chunk, kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` on `workload`, from the committed
-    `ncu --set full` captures (profiles/ncu_traffic.json, regenerated by tools/ncu_traffic.py), or None when no capture
-    of this build's kernel exists for the workload / chunk size."""
+    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` on `workload`, from `ncu --set full`
+    captures of this machine (profiles/ncu_traffic.json, written by tools/ncu_traffic.py; not committed), or None when
+    no capture of this build's kernel exists for the workload / chunk size."""
     try:
         with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
             t = json.load(f)
@@ -187,7 +192,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback: H100 SXM data-sheet HBM3 bandwidth 3.35 TB/s (not a measured figure)"
 
 
 # ------------------------------------------------------------------ reference arm / cpu baseline
@@ -317,7 +322,7 @@ class Rig:
         return t.tolist()
 
 
-def measure(rig, workload, n, chunk, steps, warmup, e2e_steps, headline):
+def measure(rig, workload, n, chunk, steps, warmup, e2e_steps, headline, dump_dir=None, dump_prefix=""):
     """One workload on every rank: bit-exact check, K timed round trips (device-resident, CUDA events on the
     context's stream, max over ranks), the host-buffer e2e number, and -- for the headline -- the blob gather."""
     torch, rb, ctx, dev, world = rig.torch, rig.rb, rig.ctx, rig.dev, rig.world
@@ -392,6 +397,11 @@ def measure(rig, workload, n, chunk, steps, warmup, e2e_steps, headline):
     ctx.sync()
     if not torch.equal(out, data):
         raise SystemExit(f"bench.py: {workload}: timed round trip is NOT bit-exact")
+    if dump_dir:
+        named = {"decoded": out, "blob": blob[:blob_size], "offsets": offsets}
+        if blocks:
+            named["block_freqs"] = bfreqs
+        dump_outputs(dump_dir, {dump_prefix + k: v for k, v in named.items()})
     total_ms, enc_ms, dec_ms = rig.max_over_ranks([t_start.elapsed_time(t_end),
                                                    float(np.mean([e[0].elapsed_time(e[1]) for e in ev])),
                                                    float(np.mean([e[1].elapsed_time(e[2]) for e in ev]))])
@@ -437,6 +447,29 @@ def measure(rig, workload, n, chunk, steps, warmup, e2e_steps, headline):
         model.close()
     torch.cuda.empty_cache()
     return res
+
+
+# elements kept of a longer output: per workload at most 2 + 2 + 4 (+ 2 for per-block frequencies) MiB, so the five
+# workloads of a default run stay below 64 MB together
+DUMP_SAMPLE = 1 << 19
+
+
+def dump_outputs(path, named):
+    """--dump-outputs: the arrays the timed path handed its caller in the last step (decoded symbols, compressed blob,
+    chunk directory, per-block frequency tables), as DIR/<name>.npy -- float32, or float64 for the 64-bit directory.
+    An array longer than DUMP_SAMPLE is reduced to a fixed sample: the positions drawn by a generator seeded with the
+    array's name and length, plus its last element, in ascending order."""
+    import torch
+    os.makedirs(path, exist_ok=True)
+    for name, t in named.items():
+        t = t.reshape(-1)
+        n = t.numel()
+        if n > DUMP_SAMPLE:
+            rng = np.random.default_rng([n] + [ord(c) for c in name])
+            idx = np.unique(np.append(rng.integers(0, n, DUMP_SAMPLE - 1), n - 1))
+            t = t[torch.from_numpy(idx).to(t.device)]
+        dtype = np.float64 if t.dtype == torch.int64 else np.float32
+        np.save(os.path.join(path, name + ".npy"), t.cpu().numpy().astype(dtype))
 
 
 def measure_gather(rig, blob, blob_size, offsets, n_chunks, enc, steps):
@@ -528,8 +561,8 @@ def measure_e2e(rig, workload, data, n, chunk, cap, n_chunks, model, coder, sb, 
            "pcie_gbs_per_direction_per_rank": moved * e2e_steps / dt / 1e9,
            "note": ("rb200_blocks_model_encode + rb200_blocks_decode" if blocks else "rb200_encode + rb200_decode")
                    + " with RB200_MEM_HOST on pinned buffers, wall clock",
-           "bound": "PCIe: each call streams its input in and its output back concurrently; with both directions busy the "
-                    "slower one gets 43-47 GB/s on this box (tools/pcie_probe.py, profiles/r1_pcie_copies.log)"}
+           "bound": "PCIe: each call streams its input in and its output back concurrently (tools/pcie_probe.py measures "
+                    "what one direction gets while the other is busy)"}
     if dt_model is not None:
         res["with_model"] = {"value": rig.world * n * e2e_steps / dt_model / 1e9, "unit": UNIT,
                              "note": "the same plus rb200_model_from_data (one more pass of the input over PCIe for the histogram, "
@@ -539,14 +572,16 @@ def measure_e2e(rig, workload, data, n, chunk, cap, n_chunks, model, coder, sb, 
 
 def run_ours(args, rank, local_rank, world):
     rig = Rig(rank, local_rank, world)
-    head = measure(rig, args.workload, args.size, args.chunk, args.steps, args.warmup, args.e2e_steps, headline=True)
+    head = measure(rig, args.workload, args.size, args.chunk, args.steps, args.warmup, args.e2e_steps, headline=True,
+                   dump_dir=args.dump_outputs if rank == 0 else None)
     configs = {}
     want = args.configs == "all" or (args.configs == "auto" and args.workload == HEADLINE and args.size == 1 << 30)
     if want:
         for name in WORKLOADS:
             if name == args.workload:
                 continue
-            configs[name] = measure(rig, name, args.size, args.chunk, args.config_steps, 3, min(args.e2e_steps, 2), headline=False)
+            configs[name] = measure(rig, name, args.size, args.chunk, args.config_steps, 3, min(args.e2e_steps, 2), headline=False,
+                                    dump_dir=args.dump_outputs if rank == 0 else None, dump_prefix=name + "__")
     if rank != 0:
         if rig.dist:
             rig.dist.barrier()
@@ -561,7 +596,7 @@ def run_ours(args, rank, local_rank, world):
         "config": {"workload": args.workload, "stands_for": head["stands_for"], "symbols_per_gpu": head["symbols_per_gpu"],
                    "chunk_syms": args.chunk, "lanes": 32, "coder": coder_name, "scale_bits": head["scale_bits"],
                    "compressed_bytes_per_symbol": head["compressed_bytes_per_symbol"],
-                   "l2": "inputs (1 GiB symbols + ~1 GiB blob) exceed the 126 MB L2; no flush needed",
+                   "l2": "inputs (1 GiB symbols + ~1 GiB blob) exceed the 50 MB L2; no flush needed",
                    "step": "encode call (%d launch%s) + decode call (1 launch), device-resident, through the C-ABI"
                            % (per_step - 1, "" if per_step == 2 else "es")},
     }

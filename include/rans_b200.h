@@ -1,5 +1,5 @@
 /*
- * rans_b200.h -- bulk C-ABI of the B200-native interleaved rANS coder.
+ * rans_b200.h -- bulk C-ABI of the GPU-native (H100, sm_90a) interleaved rANS coder.
  *
  * The reference (rygorous/ryg_rans) is header-only: its hot path is the per-symbol
  * step functions of rans_byte.h / rans64.h / rans_word_sse41.h inlined into the

@@ -1,6 +1,6 @@
-// rans_byte.h -- byte-renormalising rANS step functions, host + sm_100a device.
+// rans_byte.h -- byte-renormalising rANS step functions, host + sm_90a device.
 //
-// Source-level API of the B200 rANS package.  Every name, type and signature below is
+// Source-level API of the GPU rANS package.  Every name, type and signature below is
 // the reference's (rygorous/ryg_rans rans_byte.h; line numbers cited per function) so
 // that main.cpp / main_alias.cpp-style callers compile against this header unchanged
 // (tests/test_dropin_drivers.py does exactly that), and the same functions are usable

@@ -1,4 +1,4 @@
-// rans_word_avx2.h -- 32-lane AVX2 decoder for the chunk streams the B200 encoder produces.
+// rans_word_avx2.h -- 32-lane AVX2 decoder for the chunk streams the GPU encoder produces.
 //
 // SURVEY 8f.4: "host SIMD decoders for CPU-side consumption of GPU streams" -- the 16-way AVX2 decoder
 // the reference's README mentions (README:120-122) but never shipped, taken to the interleave width the

@@ -4,7 +4,7 @@
 //
 // Names, types and signatures are the reference's (rygorous/ryg_rans rans_word_sse41.h;
 // lines cited) so main_simd.cpp compiles against this header unchanged.  This is the coder
-// the B200 kernels implement warp-wide (csrc/word_kernels.cuh): RansSimdDecRenorm's
+// the GPU kernels implement warp-wide (csrc/word_kernels.cuh): RansSimdDecRenorm's
 // "movemask -> shuffle the next k words to the k lanes that need them" is the 4-lane
 // version of the kernels' ballot + popc(mask & lanemask_lt).
 //

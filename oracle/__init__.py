@@ -6,7 +6,7 @@ legs may import this package.  Nothing under ryg_rans_b200/ does.
 Two libraries:
   * liboracle.so        -- oracle/rans_oracle.c, the plain-C restatement (prefix orc_)
   * _ref/libryg_ref.so  -- the reference's own headers/drivers compiled from
-                           /root/reference (prefix ref_); present only when built
+                           the reference checkout (prefix ref_); present only when built
                            in a container that has the reference checked out (the
                            built .so travels to the GPU box with the snapshot).
 """
@@ -24,14 +24,9 @@ CODER_WORD, CODER_BYTE, CODER_ALIAS, CODER_RANS64 = 0, 1, 2, 3
 
 
 def build(force=False):
-    """Compile liboracle.so (always) and _ref/ (only if /root/reference is present)."""
-    need = force or not os.path.exists(os.path.join(_HERE, "liboracle.so"))
-    src = os.path.join(_HERE, "rans_oracle.c")
-    lib = os.path.join(_HERE, "liboracle.so")
-    if not need and os.path.getmtime(src) > os.path.getmtime(lib):
-        need = True
-    if need or (os.path.isdir("/root/reference") and not os.path.exists(os.path.join(_HERE, "_ref", "libryg_ref.so"))):
-        subprocess.check_call(["make", "-C", _HERE, "all"], stdout=subprocess.DEVNULL)
+    """Compile liboracle.so (always) and _ref/ (oracle/Makefile builds it only where the reference sources are present).
+    make is asked every time: it rebuilds only what is stale, and writes nothing when everything is current."""
+    subprocess.check_call(["make", "-C", _HERE, *(["-B"] if force else []), "all"], stdout=subprocess.DEVNULL)
 
 
 def _p(a, t):

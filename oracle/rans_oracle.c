@@ -1,7 +1,7 @@
 /*
  * rans_oracle.c -- CPU restatement of the ryg_rans hot path.  TEST INFRASTRUCTURE ONLY.
  *
- * This file is the parity oracle for the B200 kernels.  It is plain C99, single
+ * This file is the parity oracle for the GPU kernels.  It is plain C99, single
  * threaded, and restates the reference algorithms in a deliberately simple
  * "array of lane states + one shared cursor" form, generalised from the
  * reference drivers' fixed N (1, 2, 8) to an arbitrary lane count N.

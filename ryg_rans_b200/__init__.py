@@ -1,6 +1,6 @@
-"""ryg_rans_b200 -- B200-native interleaved rANS coder behind ryg_rans's API surface.
+"""ryg_rans_b200 -- GPU-native (H100) interleaved rANS coder behind ryg_rans's API surface.
 
-The product is the C-ABI shared library ``librans_b200.so`` (CUDA kernels for sm_100a
+The product is the C-ABI shared library ``librans_b200.so`` (CUDA kernels for sm_90a
 + C++ host code, sources in ``csrc/``, interface in ``include/rans_b200.h``).  This
 Python package is only plumbing for tests and benchmarks: it builds the library
 in-tree with nvcc and exposes it through ctypes.  There is NO CPU fallback: if the

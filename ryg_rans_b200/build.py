@@ -1,4 +1,4 @@
-"""In-tree build of librans_b200.so (and the C++ example driver) with nvcc for sm_100a."""
+"""In-tree build of librans_b200.so (and the C++ example driver) with nvcc for sm_90a (H100)."""
 import os
 import shutil
 import subprocess
@@ -11,7 +11,7 @@ EXAM_PATH = os.path.join(_HERE, "exam_gpu")
 EXAM_MULTI_PATH = os.path.join(_HERE, "exam_gpu_multi")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-O2,-Wall", "-I" + os.path.join(_ROOT, "include"), "-I" + CSRC,
 ]
 

@@ -1,4 +1,4 @@
-// alias_kernels.cuh -- sm_100a kernels for the alias-table coder (main_alias.cpp semantics):
+// alias_kernels.cuh -- sm_90a kernels for the alias-table coder (main_alias.cpp semantics):
 // rans_byte.h state machine (31-bit state, byte renormalisation, L = 1 << 23) with the
 // alias-method symbol lookup of main_alias.cpp:252-267 (decode) and the slot remap of
 // main_alias.cpp:241-250 (encode).
@@ -194,7 +194,7 @@ constexpr uint32_t kAliasDecSmem = kAliasDecWarps * kRingBytes + 256 * kAliasDec
 // and pull chunk ids from the context's atomic counter; the 32 KiB replicated bucket table is built once per CTA; the
 // per-warp stream window is the cp.async ring with a mirror behind it, wrapped once per 8 steps, so the two ranked byte
 // reads of RansDecRenorm need no address masking (round 1's kernel spends 5 of its ~20 ALU-pipe instructions per step
-// on that, and the ALU pipe is what binds it: 85 % busy).  Experiments and ablations: profiles/r2_alias_decode_lab.md.
+// on that, and the ALU pipe is what binds it: 85 % busy).  Experiments and ablations: tools/decode_lab.cu --coder alias.
 // ---------------------------------------------------------------------------
 using AliasDecShip = DecPolicy<20, 2, 8, kRefillCpAsync, 9, 0, 0, 0, false, 256 * kAliasDecReplicas * 16>;
 
@@ -703,7 +703,7 @@ inline void configure_alias_pair()
                          kAliasEncFixedSmem + (ALIAS ? (2u << 16) : 0u));
 }
 // Build switch: 1 ships the repacked ("lean") bucket entry of alias_dec_step_p for the compile-time scale_bits
-// (A/B in profiles/r2_alias_decode_lab.md); a runtime scale_bits always takes the plain entry.
+// (A/B: tools/decode_lab.cu --coder alias); a runtime scale_bits always takes the plain entry.
 #ifndef RB200_ALIAS_LEAN
 #define RB200_ALIAS_LEAN 1
 #endif

@@ -69,11 +69,8 @@ histogram_kernel(const uint8_t* __restrict__ in, uint64_t n, unsigned long long*
     }
 }
 
-inline void launch_histogram(cudaStream_t stream, const uint8_t* d_in, uint64_t n, unsigned long long* d_counts)
+inline void launch_histogram(cudaStream_t stream, uint32_t sms, const uint8_t* d_in, uint64_t n, unsigned long long* d_counts)
 {
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const uint64_t want = (n / 16 + kHistWarps * 32 - 1) / (kHistWarps * 32);
     // keep each block's per-bin count below 2^32: >= 1 block per 2^31 bytes is plenty
     uint64_t grid = static_cast<uint64_t>(sms) * 8;

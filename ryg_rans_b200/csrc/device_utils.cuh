@@ -1,4 +1,4 @@
-// device_utils.cuh -- small sm_100a device helpers shared by the rANS kernels.
+// device_utils.cuh -- small sm_90a device helpers shared by the rANS kernels.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -133,7 +133,7 @@ __device__ __forceinline__ void stg_stream_u128(uint4* p, uint4 v)
 
 // ---- L2 residency hints (createpolicy + .L2::cache_hint).  The fused encoders park every finished stream in a
 // per-warp scratch slot until its final position is known; marking those lines evict_last and the one-pass streams
-// (symbols in, blob out) evict_first keeps the scratch in the 126 MB L2 instead of making an HBM round trip.
+// (symbols in, blob out) evict_first keeps as much of the scratch as fits in L2 (50 MB on H100) instead of making an HBM round trip.
 __device__ __forceinline__ uint64_t l2_policy_keep()
 {
     uint64_t p;

@@ -1,4 +1,4 @@
-// model_host.cpp -- host-side order-0 model construction for the B200 rANS coder.
+// model_host.cpp -- host-side order-0 model construction for the GPU rANS coder.
 //
 // Model construction is setup, not hot path, but it decides every table entry and
 // therefore every bit of the stream, so it has to reproduce the reference's

@@ -1,4 +1,4 @@
-// rans64_kernels.cuh -- sm_100a kernels for the rans64.h coder as main64.cpp drives it:
+// rans64_kernels.cuh -- sm_90a kernels for the rans64.h coder as main64.cpp drives it:
 // 64-bit state in [2^31, 2^63), 32-bit renormalisation units (never loops), cum2sym symbol lookup.
 //
 //   Rans64DecGet / cum2sym / Rans64DecAdvanceSymbolStep / Rans64DecRenorm   rans64.h:118-121, main64.cpp:202,

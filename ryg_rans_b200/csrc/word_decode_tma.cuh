@@ -1,4 +1,4 @@
-// word_decode_tma.cuh -- K1p: persistent 32-way word-coder decode with TMA-fed stream rings (sm_100a).
+// word_decode_tma.cuh -- K1p: persistent 32-way word-coder decode with TMA-fed stream rings (sm_90a).
 //
 // Same decode step as word_kernels.cuh (RansSimdDecSym + RansSimdDecRenorm, rans_word_sse41.h:151-227, as one
 // warp), different plumbing:
@@ -222,7 +222,7 @@ __device__ __forceinline__ void mul_wide_u32(uint32_t a, uint32_t b, uint32_t& l
 //   ptxas forms the table address with ONE LEA.HI; e * 2^12 likewise gives freq in the high word and bias << 20 in the
 //   low one.  Two IMAD.WIDE + one shift replace five shift/mask instructions (16 instead of 18 per step) -- but they run
 //   on the FMA-heavy pipe, which the four IMADs of the step already load, and measured slower than the shift form
-//   (profiles/r2_decode_lab.md); the shipped configuration uses shifts.
+//   (tools/decode_lab.cu); the shipped configuration uses shifts.
 template <class P, bool WIDE>
 __device__ __forceinline__ void tma_dec_step(uint32_t& x, uint32_t& cur, uint32_t tab, uint8_t* o, uint32_t lt, uint32_t lane,
                                              cudaTextureObject_t tex, bool via_tex, bool active)
@@ -457,7 +457,7 @@ word_decode_tma_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, con
     }
 }
 
-// The configuration the C-ABI launches (tools/decode_lab.cu measures the alternatives; profiles/r2_decode_lab.md):
+// The configuration the C-ABI launches (tools/decode_lab.cu measures the alternatives):
 // 2 CTAs of 32 warps per SM, fill check / ring wrap every 8 steps, ring of 4 x 512 B filled by cp.async (LDGSTS),
 // table by one TMA bulk copy, freq / bias by one IMAD.WIDE, slot and x >> 12 by shift / mask.
 using DecShip = DecPolicy<32, 2, 8, kRefillCpAsync, 9, 2, 0, 0, false>;

@@ -1,4 +1,4 @@
-// word_kernels.cuh -- sm_100a kernels for the word coder (rans_word_sse41.h semantics):
+// word_kernels.cuh -- sm_90a kernels for the word coder (rans_word_sse41.h semantics):
 // 32-bit state, 16-bit renormalisation, L = 1 << 16, scale_bits = 12.
 //
 // One warp = one chunk = one 32-way interleaved stream; lane k owns rANS state k.
@@ -577,7 +577,7 @@ __device__ __forceinline__ void fused_place(const uint64_t* look, uint32_t chunk
     // Warps do not progress evenly, so the scan front (the oldest unfinished chunk) can trail this warp by a chunk time
     // and more: the wait is real, and every poll costs ~12 issue slots that the encoding warps of the SM want.  Back off
     // exponentially (128 ns .. 4 us): round 1 polled every 100 ns and spent a fifth of the kernel's instructions here
-    // (ncu source view: 5.3 M poll iterations per GiB, profiles/r2_encode_experiments.md).
+    // (seen in the ncu source view as millions of poll iterations per GiB).
     uint64_t v = 0, since = 0;
     uint32_t ns = 128;
     for (;;) {
@@ -634,8 +634,7 @@ word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t ch
 
     // The previous chunk(s) are placed late on purpose.  Warps do not progress evenly (the issue arbiter favours high warp
     // ids), so the scan front -- the oldest unfinished chunk -- trails the fastest warps by about one chunk time: placing
-    // 32 steps into the next chunk instead was measured at 2.39 ms per GiB against 1.15 ms, 580 M polling instructions
-    // (profiles/r2_encode_experiments.md).
+    // 32 steps into the next chunk instead was measured to be about twice as slow: the workers spent their issue slots polling.
     uint32_t pend_chunk[kFusedSlots - 1], pend_size[kFusedSlots - 1];      // oldest first; registers (static indexing only)
     uint32_t n_pending = 0, cur = 0;                                        // cur = slot of the chunk being encoded
     for (;;) {

@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 def _gen(kind, n, seed):
@@ -48,10 +48,21 @@ def oracle_lib():
 
 
 @pytest.fixture(scope="session")
+def book1(oracle_lib):
+    """The reference's test file, recovered from its 32-way stream in tests/golden/book1_n32.npz."""
+    import oracle
+    g = np.load(os.path.join(ROOT, "tests", "golden", "book1_n32.npz"))
+    freqs = g["freqs"]
+    cum = np.concatenate([[0], np.cumsum(freqs)]).astype(np.uint32)
+    book, _ = oracle_lib.decode(oracle.CODER_WORD, g["stream"], int(g["n"]), freqs, cum, 32)
+    return book
+
+
+@pytest.fixture(scope="session")
 def ref_lib():
     import oracle
     if not oracle.Reference.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
+        pytest.skip("oracle/_ref not built (the reference sources were not available to build())")
     return oracle.Reference()
 
 

@@ -1,5 +1,5 @@
 // Function-level differential test of include/rans_byte.h, rans64.h, rans_word_sse41.h against the reference's headers.
-// REFDIR is replaced by the reference checkout's path at test time (tests/test_header_parity.py); nothing of the
+// REFDIR is replaced by the reference checkout's path at build time (oracle/Makefile); nothing of the
 // reference is copied here -- its headers are #included where they lie, inside namespace ref.
 #include <stdint.h>
 #include <stdlib.h>

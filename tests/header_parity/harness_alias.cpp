@@ -1,6 +1,6 @@
 // Differential test of include/rans_alias.h against the reference's own alias code, which lives in its driver
 // (main_alias.cpp: SymbolStats::make_alias_table, RansEncPutAlias, RansDecGetAlias).  REFDIR is replaced by the
-// reference checkout's path at test time; the driver is #included where it lies (its main renamed), nothing is copied.
+// reference checkout's path at build time (oracle/Makefile); the driver is #included where it lies (its main renamed), nothing is copied.
 // system headers first, outside the namespaces: their include guards then make the driver's own #includes no-ops
 #include <stdio.h>
 #include <stdarg.h>

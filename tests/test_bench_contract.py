@@ -14,7 +14,7 @@ BASE_KEYS = {"metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_ste
              "vs_baseline", "dtype", "data", "config", "e2e", "gpu_launches"}
 
 
-@pytest.mark.skipif(not os.path.exists(REF_LIB), reason="oracle/_ref is built only where /root/reference exists")
+@pytest.mark.skipif(not os.path.exists(REF_LIB), reason="oracle/_ref is built only where the reference sources are available")
 @pytest.mark.parametrize("workload", ["uniform_1GiB_word32", "zipf1.1_1GiB_alias32"])
 def test_reference_arm_prints_the_contract_line(workload):
     out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--workload", workload, "--steps", "2",

@@ -4,6 +4,8 @@ Mirrors the reference's own verification (decode-output memcmp, main_simd.cpp:34
 and strengthens it: the GPU blob must equal the oracle's container byte for byte, the
 GPU must decode the oracle's blob, and the oracle must decode the GPU's blob.
 """
+import os
+
 import numpy as np
 import pytest
 
@@ -12,6 +14,8 @@ import oracle as orc
 pytestmark = pytest.mark.gpu
 
 WORD, BYTE, ALIAS, RANS64 = 0, 1, 2, 3
+# the reference's own N = 32 streams of the seeded inputs below (made by tests/golden/make_ref_streams.py)
+REF_STREAMS = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_streams_n32.npz"))
 
 
 def _model(oracle_lib, data, scale_bits):
@@ -35,6 +39,22 @@ def _roundtrip(gpu_ctx, oracle_lib, data, coder, scale_bits, chunk):
     model.close()
 
 
+def _reference_stream_n32(gpu_ctx, oracle_lib, name, coder, ocoder, sb, data):
+    """The GPU's one-chunk container holds exactly the reference's N = 32 stream of `data` under the reference's model,
+    the GPU decodes it, and the stream is consumed to its end (the reference's decoder was checked on it when the
+    fixture was made)."""
+    freqs, ref_stream = REF_STREAMS[f"{name}/freqs"], REF_STREAMS[f"{name}/stream"]
+    f2, cum = oracle_lib.model(data, sb)
+    assert np.array_equal(f2, freqs)
+    model = gpu_ctx.model(coder, sb, freqs)
+    blob, offs = gpu_ctx.encode_host(model, data, 1 << 16)
+    assert np.array_equal(blob[int(offs[0]):], ref_stream)
+    assert np.array_equal(gpu_ctx.decode_host(model, blob, offs, data.size, 1 << 16), data)
+    dec, used = oracle_lib.decode(ocoder, ref_stream, data.size, freqs, cum, 32, sb)
+    assert np.array_equal(dec, data) and used == ref_stream.size
+    model.close()
+
+
 @pytest.mark.parametrize("kind", ["uniform", "zipf", "text", "two", "skew", "const"])
 @pytest.mark.parametrize("n,chunk", [(1, 32), (31, 32), (32, 32), (33, 64), (4096, 4096), (100003, 4096), (300000, 16384)])
 def test_word_parity(gpu_ctx, oracle_lib, gen, kind, n, chunk):
@@ -51,17 +71,9 @@ def test_word_empty(gpu_ctx, oracle_lib, gen):
     assert out.size == 0
 
 
-def test_word_reference_stream_n32(gpu_ctx, oracle_lib, ref_lib, gen):
+def test_word_reference_stream_n32(gpu_ctx, oracle_lib, gen):
     """A single chunk IS the reference's N-way stream with N = 32 (SURVEY 8a layout)."""
-    data = gen("text", 50000, 5)
-    freqs, cum = ref_lib.model(data, 12)
-    ref_stream = ref_lib.encode(orc.CODER_WORD, data, freqs, cum, 32)
-    model = gpu_ctx.model(WORD, 12, freqs)
-    blob, offs = gpu_ctx.encode_host(model, data, 1 << 16)
-    assert np.array_equal(blob[int(offs[0]):], ref_stream)
-    # and the reference's own primitives decode the GPU stream
-    dec, used = ref_lib.decode(orc.CODER_WORD, blob[int(offs[0]):], data.size, freqs, cum, 32)
-    assert np.array_equal(dec, data) and used == ref_stream.size
+    _reference_stream_n32(gpu_ctx, oracle_lib, "word", WORD, orc.CODER_WORD, 12, gen("text", 50000, 5))
 
 
 def test_book1_known_answer_through_the_gpu(gpu_ctx, oracle_lib):
@@ -146,15 +158,8 @@ def test_alias_parity(gpu_ctx, oracle_lib, gen, kind, n, chunk, sb):
     _roundtrip(gpu_ctx, oracle_lib, data, ALIAS, sb, chunk)
 
 
-def test_alias_reference_stream_n32(gpu_ctx, ref_lib, gen):
-    data = gen("zipf", 60000, 6)
-    freqs, cum = ref_lib.model(data, 16)
-    ref_stream = ref_lib.encode(orc.CODER_ALIAS, data, freqs, cum, 32, 16)
-    model = gpu_ctx.model(ALIAS, 16, freqs)
-    blob, offs = gpu_ctx.encode_host(model, data, 1 << 16)
-    assert np.array_equal(blob[int(offs[0]):], ref_stream)
-    dec, used = ref_lib.decode(orc.CODER_ALIAS, blob[int(offs[0]):], data.size, freqs, cum, 32, 16)
-    assert np.array_equal(dec, data) and used == ref_stream.size
+def test_alias_reference_stream_n32(gpu_ctx, oracle_lib, gen):
+    _reference_stream_n32(gpu_ctx, oracle_lib, "alias", ALIAS, orc.CODER_ALIAS, 16, gen("zipf", 60000, 6))
 
 
 def test_alias_corrupt_stream_is_reported(gpu_ctx, oracle_lib, gen):
@@ -200,17 +205,11 @@ def test_rans64_parity(gpu_ctx, oracle_lib, gen, kind, n, chunk, sb):
 
 
 @pytest.mark.parametrize("coder,ocoder,sb", [(BYTE, orc.CODER_BYTE, 14), (RANS64, orc.CODER_RANS64, 14)])
-def test_byte_and_rans64_reference_stream_n32(gpu_ctx, ref_lib, gen, coder, ocoder, sb):
+def test_byte_and_rans64_reference_stream_n32(gpu_ctx, oracle_lib, gen, coder, ocoder, sb):
     """The reference's own RansEncPutSymbol / Rans64EncPutSymbol loops (N = 32) produce the GPU's chunk stream,
     and the reference's decoders read the GPU stream."""
-    data = gen("text", 60000, 8)
-    freqs, cum = ref_lib.model(data, sb)
-    ref_stream = ref_lib.encode(ocoder, data, freqs, cum, 32, sb)
-    model = gpu_ctx.model(coder, sb, freqs)
-    blob, offs = gpu_ctx.encode_host(model, data, 1 << 16)
-    assert np.array_equal(blob[int(offs[0]):], ref_stream)
-    dec, used = ref_lib.decode(ocoder, blob[int(offs[0]):], data.size, freqs, cum, 32, sb)
-    assert np.array_equal(dec, data) and used == ref_stream.size
+    name = "byte" if coder == BYTE else "rans64"
+    _reference_stream_n32(gpu_ctx, oracle_lib, name, coder, ocoder, sb, gen("text", 60000, 8))
 
 
 # ---------------------------------------------------------------- device histogram / per-block models (config 5)

@@ -1,6 +1,6 @@
 """include/rans_word_avx2.h: the 32-lane AVX2 consumer for GPU chunk streams (SURVEY 8f.4).
 
-A host without a GPU must be able to read what the B200 encoder wrote.  The header decodes the word coder's
+A host without a GPU must be able to read what the GPU encoder wrote.  The header decodes the word coder's
 N = 32 streams with four __m256i of states; here it is checked against the reference's own N = 32 streams (golden
 fixtures made by the reference code), against oracle containers of every input shape, against corrupt streams, and
 -- on the GPU box -- against containers the CUDA encoder produced.

@@ -256,7 +256,7 @@ def _alias_step_lean(x, sb, divider, slot_adjust, slot_freqs, sym_id):
 def test_alias_lean_entry_is_equivalent(gen, sb, kind):
     """Every slot value x & ((1 << sb) - 1), under arbitrary upper state bits, decodes to the same symbol and the same
     next state through the repacked bucket entry as through the plain one (the GPU A/B of the two is in
-    profiles/r2_alias_decode_lab.md; the GPU parity tests cover whichever one the library was built with)."""
+    tools/decode_lab.cu --coder alias; the GPU parity tests cover whichever one the library was built with)."""
     if kind == "zipf":
         data = gen("zipf", 50000, sb)
     elif kind == "two_symbols":

@@ -7,7 +7,7 @@
 // read, no refill).  Ablated variants produce garbage; every other variant is verified byte for byte against the input.
 // One JSON line per variant on stdout.  Not part of the product: links librans_b200.so, includes the kernel headers.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Iinclude -Iryg_rans_b200/csrc \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Iinclude -Iryg_rans_b200/csrc \
 //        -o build/decode_lab tools/decode_lab.cu -Lryg_rans_b200 -lrans_b200 -Xlinker -rpath -Xlinker '$ORIGIN/../ryg_rans_b200'
 //   build/decode_lab [--n BYTES] [--chunk SYMS] [--reps K] [--dist uniform|text|zipf] [--only NAME] [--peak GBS]
 //                    [--coder word|alias]
@@ -284,7 +284,7 @@ int main(int argc, char** argv)
     uint32_t chunk = 8192;
     int reps = 5;
     std::string dist = "uniform", only, coder = "word";
-    double peak = 6481.8;
+    double peak = 3350.0;                       // GB/s: H100 SXM data-sheet HBM3 bandwidth; --peak for a measured one
     for (int i = 1; i < argc; i++) {
         auto arg = [&](const char* f) { return std::strcmp(argv[i], f) == 0 && i + 1 < argc; };
         if (arg("--n")) n = std::strtoull(argv[++i], nullptr, 0);

@@ -5,7 +5,7 @@ Launches are grouped by kernel name and by size class: the full-workload launche
 slice launches of the pipelined HOST path (the e2e leg) have the same kernel names but durations two orders of magnitude
 apart, so each name is split at a third of its longest launch.  Output: a markdown table on stdout.
 
-usage: tools/launch_summary.py profiles/r2_final_launches.csv
+usage: tools/launch_summary.py launches.csv
 """
 import collections
 import csv

@@ -39,7 +39,7 @@ def main():
     tag = sys.argv[2] if len(sys.argv) > 2 else "r2"
     traffic = {"source": "ncu --set full --clock-control none, one capture per kernel per workload (tools/profile_all.sh)",
                "workloads": {}}
-    md = [f"# {tag}: `ncu --set full --clock-control none` of every hot kernel on every BASELINE workload (B200, 1 GPU)", "",
+    md = [f"# {tag}: `ncu --set full --clock-control none` of every hot kernel on every BASELINE workload (1 GPU)", "",
           "Command: `tools/profile_all.sh` (bench.py --workload W --steps 1, chunk 8192).  The LAST captured launch of each kernel is "
           "shown.  `binds` = the busiest unit among LSU data pipe / issue slots / DRAM / FMA-heavy / ALU / XU.", ""]
     for rep in sorted(f for f in os.listdir(d) if f.endswith(".ncu-rep") or f.endswith(".csv")):
@@ -74,6 +74,7 @@ def main():
             md.append("")
         per["encode_call"] = enc_call          # every kernel of one encode call (model / encode / scan / compaction)
         traffic["workloads"][w] = {"chunk_syms": CHUNK, "dram_bytes_per_launch": per}
+    os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)      # git-ignored: captures are machine-specific records
     with open(os.path.join(ROOT, "profiles", "ncu_traffic.json"), "w") as f:
         json.dump(traffic, f, indent=1)
     with open(os.path.join(ROOT, "profiles", f"{tag}_ncu_summary.md"), "w") as f:

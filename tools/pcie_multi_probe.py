@@ -2,7 +2,7 @@
 time?  One child process per GPU (CUDA_VISIBLE_DEVICES), bidirectional 64 MiB pinned copies (H2D on one stream, D2H on
 another -- what a host-mode rb200_encode / rb200_decode call does) for about a second after a common start time.
 Placements: `local` = every GPU's buffers first-touched on its own NUMA node; `alt` = odd GPUs use the OTHER node.
-Run on the GPU box with all GPUs visible:  python tools/pcie_multi_probe.py  > gpurun_out/pcie_multi_probe.jsonl"""
+Run on the GPU box with all GPUs visible:  python tools/pcie_multi_probe.py  > pcie_multi_probe.jsonl"""
 import json
 import os
 import subprocess

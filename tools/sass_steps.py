@@ -1,6 +1,5 @@
 #!/usr/bin/env python
-"""Print one unrolled step of the hot loops from the built library's SASS (the listings committed as
-profiles/r1_final_sass_steps.md and profiles/r2_final_sass_steps.md), and the mnemonics that prove the asynchronous
+"""Print one unrolled step of the hot loops from the built library's SASS, and the mnemonics that prove the asynchronous
 staging (TMA bulk copy, cp.async, mbarrier) is in the shipped decoder.  Needs cuobjdump; no GPU.
 
     python tools/sass_steps.py [path/to/librans_b200.so]
