@@ -485,7 +485,7 @@ bool use_persistent_decode()
 uint32_t fused_word_grid(rb200_ctx* ctx, uint32_t n_chunks)
 {
     const uint32_t want = (n_chunks + 1 + kEncWarps - 1) / kEncWarps;       // + 1: one warp of the grid is the scanner
-    const uint32_t grid = static_cast<uint32_t>(ctx->sms) * RB200_ENC_MINBLOCKS;
+    const uint32_t grid = static_cast<uint32_t>(ctx->sms) * RB200_FUSED_MINBLOCKS;
     return grid > want ? want : grid;
 }
 

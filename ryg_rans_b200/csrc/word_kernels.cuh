@@ -211,15 +211,27 @@ word_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const u
 // that the 8 lanes of a quarter-warp always hit different 16-byte bank groups.
 // ---------------------------------------------------------------------------
 // build-time switches of the encoders (A/B runs: nvcc -DNAME=value into a second .so, loaded with RB200_LIB)
+// The fused word encoder's scratch is live data: (resident warps) x (slots per warp) x (one chunk's stream, 8.3 KB at
+// chunks of 8192).  2 CTAs x 16 warps per SM with two slots bring it down to about the 50 MB L2 of an H100 (3 x 16 warps
+// with three slots: 100-150 MB), and the evict_last hint then keeps most of it there, so a stream is not read back from
+// HBM before it is placed.  H100 SXM at 700 W, 1 GiB uniform bytes, chunks of 8192, ms per encode call
+// {CTAs per SM, slots, hint}: {3, 3, no} 1.79 | {3, 2, no} 1.76 | {3, 2, yes} 1.71 | {2, 3, no} 1.67 | {2, 2, no} 1.66 |
+// {2, 2, yes} 1.62.  Fewer warps lose more encode throughput than they save traffic (2 x 11 warps, {2, yes}: 1.71), and
+// 32-40 warps per SM in other shapes (3 x 12, 3 x 10, 2 x 20, 4 x 8) measured the same as 2 x 16 within noise (on a
+// 400 W card: 1.70-1.72 ms against 1.84-1.86 ms for {3, 3, no}).
+// Dropping a placed stream's lines from L2 (discard.global.L2, so they are never written back) was slower: 1.66 ms.
 #ifndef RB200_FUSED_SLOTS
-#define RB200_FUSED_SLOTS 3            // scratch slots per worker warp of the fused word encoder: a chunk is placed SLOTS - 1 chunks late (2, 3, 4 measured: 1.155 / 1.126 / 1.163 ms per GiB)
+#define RB200_FUSED_SLOTS 2            // scratch slots per worker warp of the fused word encoder: a chunk is placed SLOTS - 1 chunks late
 #endif
 constexpr uint32_t kFusedSlots = RB200_FUSED_SLOTS;
+#ifndef RB200_FUSED_MINBLOCKS
+#define RB200_FUSED_MINBLOCKS 2        // CTAs per SM of the fused word encoder (its grid is SMs x this)
+#endif
 #ifndef RB200_ENC_UNIFORM_FLUSH
 #define RB200_ENC_UNIFORM_FLUSH 1      // vote on the (warp-uniform) flush test so that ptxas emits a uniform branch
 #endif
 #ifndef RB200_ENC_KEEP_HINT
-#define RB200_ENC_KEEP_HINT false      // evict_last hint on the fused encoder's scratch stores (see word_enc_flush)
+#define RB200_ENC_KEEP_HINT true       // evict_last hint on the fused encoder's scratch stores (see word_enc_flush)
 #endif
 #ifndef RB200_ENC_ASM_RENORM
 #define RB200_ENC_ASM_RENORM 1
@@ -607,11 +619,11 @@ __device__ __forceinline__ void fused_place(const uint64_t* look, uint32_t chunk
     }
 }
 
-// Grid = resident capacity (SMs x RB200_ENC_MINBLOCKS CTAs).  Warp 0 of CTA 0 is the scanner, every other warp is
-// a worker with TWO scratch slots: it encodes chunk k+1 into one slot before it places chunk k from the other,
+// Grid = resident capacity (SMs x RB200_FUSED_MINBLOCKS CTAs).  Warp 0 of CTA 0 is the scanner, every other warp is
+// a worker with kFusedSlots scratch slots: it encodes chunk k+1 into one slot before it places chunk k from the other,
 // so by the time it asks for E_k the scanner has normally long passed k and nobody polls.
 template <bool R32>
-__global__ void __launch_bounds__(kEncWarps * 32, RB200_ENC_MINBLOCKS)
+__global__ void __launch_bounds__(kEncWarps * 32, RB200_FUSED_MINBLOCKS)
 word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
                          const WordEncEntry* __restrict__ g_table, uint8_t* __restrict__ scratch, uint32_t slot_bytes,
                          uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap,
