@@ -445,6 +445,7 @@ alias_decode_persist_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size
 // ---------------------------------------------------------------------------
 constexpr int kAliasEncWarps = 32;
 constexpr uint32_t kAliasEncFixedSmem = kAliasEncWarps * kEncWarpSmem + kEncTableBytes;   // 64 KiB + remap
+constexpr uint32_t kAliasFusedSlots = 2;        // scratch slots per worker warp in fused mode (a SlotQueue, placement.cuh)
 
 __device__ __forceinline__ uint32_t lds_u16_ro(uint32_t addr)
 {
@@ -619,8 +620,8 @@ __device__ __forceinline__ uint32_t alias_encode_stream(const uint8_t* __restric
 // Two modes (like the word encoder):
 //   look == nullptr: chunks strided over the persistent CTAs, each into its own worst-case slot of `scratch`,
 //                    sizes[] written for the tile scan + compaction that follow;
-//   look != nullptr: fused -- chunk ids from an atomic counter, two scratch slots per warp, warp 0 of CTA 0 is the
-//                    scanner, every worker places chunk k after encoding chunk k+1 (see word_kernels.cuh, K2f).
+//   look != nullptr: fused -- chunk ids from an atomic counter, kAliasFusedSlots scratch slots per warp, warp 0 of
+//                    CTA 0 is the scanner (placement.cuh).
 template <bool ALIAS, uint32_t SB>
 __global__ void __launch_bounds__(kAliasEncWarps * 32, 1)
 alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb_rt,
@@ -662,9 +663,8 @@ alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_s
         fused_scanner(look, n_chunks, lane, status);
         return;
     }
-    uint8_t* slots = scratch + (static_cast<uint64_t>(blockIdx.x) * kAliasEncWarps + warp) * 2 * slot_bytes;
-    uint32_t pend_chunk = 0, pend_size = 0, parity = 0;
-    bool pending = false;
+    const PlaceOut out = {look, n_chunks, blob, blob_cap, offsets, status};
+    SlotQueue<kAliasFusedSlots> q(scratch, blockIdx.x * kAliasEncWarps + warp, slot_bytes);
     for (;;) {
         uint32_t chunk = 0;
         if (lane == 0) chunk = atomicAdd(counter, 1u);
@@ -672,22 +672,10 @@ alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_s
         if (chunk >= n_chunks) break;
         const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
         const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-        const uint32_t produced = alias_encode_stream<ALIAS, SB>(in + first, m, tab, remap, wsm, sb,
-                                                             slots + (parity + 1) * static_cast<uint64_t>(slot_bytes), status);
-        if (lane == 0) st_relaxed_u64(look + chunk, kLookAgg | ((produced + 15u) & ~15u));
-        __syncwarp();
-        if (pending)
-            fused_place(look, pend_chunk, n_chunks, slots + (2 - parity) * static_cast<uint64_t>(slot_bytes), pend_size, blob, blob_cap,
-                        offsets, lane, status);
-        pend_chunk = chunk;
-        pend_size = produced;
-        pending = true;
-        parity ^= 1;
-        __syncwarp();
+        const uint32_t produced = alias_encode_stream<ALIAS, SB>(in + first, m, tab, remap, wsm, sb, q.next_end(), status);
+        q.finish(out, chunk, produced, lane);
     }
-    if (pending)
-        fused_place(look, pend_chunk, n_chunks, slots + (2 - parity) * static_cast<uint64_t>(slot_bytes), pend_size, blob, blob_cap,
-                    offsets, lane, status);
+    q.drain(out, lane);
 }
 
 // scale_bits the kernels are specialised for (main_alias.cpp:276 uses 16, main.cpp:136 / main64.cpp:136 use 14, the word
@@ -731,7 +719,7 @@ inline void configure_alias_kernels()
     }
 
 // remap == nullptr selects the rans_byte cum2sym coder.  look == nullptr: split mode (sizes[] out, one slot per
-// chunk); otherwise fused mode (two slots per resident warp; look/counter zeroed by the caller).
+// chunk); otherwise fused mode (kAliasFusedSlots slots per resident warp; look/counter zeroed by the caller).
 // sms = multiprocessors of the context's device (rb200_ctx keeps it; nothing process-wide is cached here).
 inline int launch_alias_encode(cudaStream_t stream, uint32_t sms, const uint8_t* d_in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
                                uint32_t sb, const AliasEncEntry* enc, const uint16_t* remap, uint8_t* scratch, uint32_t slot,
@@ -749,7 +737,6 @@ inline int launch_alias_encode(cudaStream_t stream, uint32_t sms, const uint8_t*
     }
     return 0;
 }
-inline uint32_t alias_fused_slots(uint32_t sms) { return sms * kAliasEncWarps * 2; }
 
 // work != nullptr: the persistent kernel (sms x 2 CTAs of 20 warps, chunk ids from the context's work counter)
 inline int launch_alias_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets, uint32_t sb,

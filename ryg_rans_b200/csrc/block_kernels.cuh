@@ -397,12 +397,13 @@ block_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, const u
 
 // K5f: per-block encode in ONE persistent launch -- model (optional), tables, encode, directory, placement.
 //
-// CTA 0 only hosts the scanner warp (word_kernels.cuh, K2f).  Every other CTA takes block ids from an atomic counter
+// CTA 0 only hosts the scanner warp (placement.cuh).  Every other CTA takes block ids from an atomic counter
 // (so chunks start in order), builds the block's model when BUILD (count_freqs + normalize_freqs, written to
 // block_freqs) or reads it, builds the encoder table in shared memory, and its warps encode the block's chunks into
-// per-warp scratch slots exactly as the fused word encoder does: publish the padded size, place the chunk of the
-// PREVIOUS block once the scanner has turned the published sizes into end offsets.  The second pass over the block's
-// 64 KiB (histogram first, then encode) is served by the L2.
+// kBlockFusedSlots per-warp scratch slots (a SlotQueue) exactly as the fused word encoder does: publish the padded size,
+// place the chunk of the PREVIOUS block once the scanner has turned the published sizes into end offsets.  The second
+// pass over the block's 64 KiB (histogram first, then encode) is served by the L2.
+constexpr uint32_t kBlockFusedSlots = 2;        // scratch slots per worker warp
 template <bool BUILD, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, WARPS <= 8 ? 5 : 1)
 block_encode_fused_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uint32_t block_size, uint16_t* __restrict__ block_freqs,
@@ -425,9 +426,8 @@ block_encode_fused_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uin
     }
     const uint32_t warps = blockDim.x >> 5;
     const uint32_t tab = smem_addr(s_enc), wsm = tab + kEncTableBytes + warp * kEncWarpSmem;
-    uint8_t* slots = scratch + (static_cast<uint64_t>(blockIdx.x - 1) * warps + warp) * 2 * slot_bytes;     // this warp's two slots
-    uint32_t pend_chunk = 0, pend_size = 0, parity = 0;
-    bool pending = false;
+    const PlaceOut out = {look, n_chunks, blob, blob_cap, offsets, status};
+    SlotQueue<kBlockFusedSlots> q(scratch, (blockIdx.x - 1) * warps + warp, slot_bytes);
     for (;;) {
         __syncthreads();                                   // the previous block's table is no longer in use
         if (tid == 0) s_block = atomicAdd(counter, 1u);
@@ -445,26 +445,13 @@ block_encode_fused_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uin
         }
         const bool r32 = block_build_enc_table(s_cum, ok, s_tab);
         if (warp < per_block) {
-            const uint32_t chunk = block * per_block + warp;
-            uint8_t* slot_end = slots + (parity + 1) * static_cast<uint64_t>(slot_bytes);
             const uint8_t* src = blk + static_cast<uint64_t>(warp) * chunk_syms;
-            const uint32_t produced = r32 ? word_encode_stream<true>(src, chunk_syms, tab, wsm, slot_end, status)
-                                          : word_encode_stream<false>(src, chunk_syms, tab, wsm, slot_end, status);
-            if (lane == 0) st_relaxed_u64(look + chunk, kLookAgg | ((produced + 15u) & ~15u));
-            __syncwarp();
-            if (pending)
-                fused_place(look, pend_chunk, n_chunks, slots + (2 - parity) * static_cast<uint64_t>(slot_bytes), pend_size, blob, blob_cap,
-                            offsets, lane, status);
-            pend_chunk = chunk;
-            pend_size = produced;
-            pending = true;
-            parity ^= 1;
-            __syncwarp();
+            const uint32_t produced = r32 ? word_encode_stream<true>(src, chunk_syms, tab, wsm, q.next_end(), status)
+                                          : word_encode_stream<false>(src, chunk_syms, tab, wsm, q.next_end(), status);
+            q.finish(out, block * per_block + warp, produced, lane);
         }
     }
-    if (pending)
-        fused_place(look, pend_chunk, n_chunks, slots + (2 - parity) * static_cast<uint64_t>(slot_bytes), pend_size, blob, blob_cap, offsets,
-                    lane, status);
+    q.drain(out, lane);
 }
 
 inline uint32_t block_threads(uint32_t block_size, uint32_t chunk_syms)

@@ -454,7 +454,7 @@ int reserve_encode_workspace(rb200_ctx* ctx, uint32_t n_chunks, uint32_t slot, u
 
 // Word-coder encode has two paths:
 //   fused: ONE persistent launch -- workers encode, a scanner warp turns published sizes into end offsets
-//          in chunk order, workers place chunk k after encoding chunk k+1 (word_kernels.cuh, K2f);
+//          in chunk order, workers place chunk k after encoding chunk k+1 (placement.cuh);
 //   split: three launches -- encode into per-chunk worst-case slots, tile scan, compaction.
 // fused is faster as long as the scanner keeps up, i.e. for chunks of >= 4096 symbols; below that the split path
 // is used (H100 SXM at a 400 W power limit, 1 GiB uniform bytes: 1.89 vs 2.21 ms per call at chunks of 8192, 2.10 vs
@@ -489,21 +489,51 @@ uint32_t fused_word_grid(rb200_ctx* ctx, uint32_t n_chunks)
     return grid > want ? want : grid;
 }
 
+// The fused encoders' workspace: `slots` scratch slots of `slot` bytes, and in ctx->sizes the chunk counter (16 bytes)
+// followed by look[n_chunks] (placement.cuh).
+struct FusedWorkspace {
+    uint8_t* scratch;
+    uint64_t* look;
+    uint32_t* counter;
+};
+
+int reserve_fused(rb200_ctx* ctx, size_t slots, uint32_t slot, uint32_t n_chunks)
+{
+    int rc = reserve(ctx, ctx->scratch, slots * slot + 16);
+    if (rc == RB200_OK) rc = reserve(ctx, ctx->sizes, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t));
+    return rc;
+}
+
+// reserve_fused, then zero the counter and look[] on the context's stream
+int fused_workspace(rb200_ctx* ctx, size_t slots, uint32_t slot, uint32_t n_chunks, FusedWorkspace* ws)
+{
+    int rc = reserve_fused(ctx, slots, slot, n_chunks);
+    if (rc != RB200_OK) return rc;
+    RB_CUDA(ctx, cudaMemsetAsync(ctx->sizes.p, 0, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t), ctx->stream));
+    ws->scratch = static_cast<uint8_t*>(ctx->scratch.p);
+    ws->counter = static_cast<uint32_t*>(ctx->sizes.p);
+    ws->look = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + 16);
+    return RB200_OK;
+}
+
+// scratch slots of the fused word or alias / byte encoder: slots per warp x the warps of its largest grid
+size_t fused_slot_count(rb200_ctx* ctx, int coder, uint32_t n_chunks)
+{
+    if (coder == RB200_CODER_WORD) return static_cast<size_t>(fused_word_grid(ctx, n_chunks)) * kEncWarps * kFusedSlots;
+    return static_cast<size_t>(ctx->sms) * kAliasEncWarps * kAliasFusedSlots;     // launch_alias_encode: <= one CTA per SM
+}
+
 int encode_word_fused(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_in, size_t n, uint32_t chunk_syms, uint32_t n_chunks,
                       uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets)
 {
     const uint32_t slot = slot_bytes_for(chunk_syms);
-    const uint32_t grid = fused_word_grid(ctx, n_chunks);
-    int rc = reserve(ctx, ctx->scratch, static_cast<size_t>(grid) * kEncWarps * kFusedSlots * slot + 16);  // kFusedSlots per resident warp
-    if (rc == RB200_OK) rc = reserve(ctx, ctx->sizes, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t));
+    FusedWorkspace ws = {};
+    int rc = fused_workspace(ctx, fused_slot_count(ctx, RB200_CODER_WORD, n_chunks), slot, n_chunks, &ws);
     if (rc != RB200_OK) return rc;
-    uint32_t* counter = static_cast<uint32_t*>(ctx->sizes.p);
-    uint64_t* look = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + 16);
-    RB_CUDA(ctx, cudaMemsetAsync(ctx->sizes.p, 0, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t), ctx->stream));
     auto kernel = model->enc_r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>;
-    kernel<<<grid, kEncWarps * 32, kEncSmemBytes, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->d_word_enc,
-                                                                 static_cast<uint8_t*>(ctx->scratch.p), slot, look, counter, d_blob,
-                                                                 blob_cap, d_offsets, ctx->d_status);
+    kernel<<<fused_word_grid(ctx, n_chunks), kEncWarps * 32, kEncSmemBytes, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->d_word_enc,
+                                                                                           ws.scratch, slot, ws.look, ws.counter, d_blob,
+                                                                                           blob_cap, d_offsets, ctx->d_status);
     return check_launch(ctx, "word_encode_fused_kernel");
 }
 
@@ -513,13 +543,8 @@ int reserve_encode(rb200_ctx* ctx, const rb200_model* model, uint32_t n_chunks, 
 {
     if (!n_chunks) return RB200_OK;
     const uint32_t slot = slot_bytes_for(chunk_syms);
-    if (use_fused_encode(chunk_syms) && model->coder != RB200_CODER_RANS64) {
-        const size_t slots = model->coder == RB200_CODER_WORD ? static_cast<size_t>(fused_word_grid(ctx, n_chunks)) * kEncWarps * kFusedSlots
-                                                              : static_cast<size_t>(alias_fused_slots(static_cast<uint32_t>(ctx->sms)));
-        int rc = reserve(ctx, ctx->scratch, slots * slot + 16);
-        if (rc == RB200_OK) rc = reserve(ctx, ctx->sizes, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t));
-        return rc;
-    }
+    if (use_fused_encode(chunk_syms) && model->coder != RB200_CODER_RANS64)
+        return reserve_fused(ctx, fused_slot_count(ctx, model->coder, n_chunks), slot, n_chunks);
     uint8_t* scratch; uint32_t* sizes; uint64_t* tile_sums;
     return reserve_encode_workspace(ctx, n_chunks, slot, &scratch, &sizes, &tile_sums);
 }
@@ -535,15 +560,12 @@ int encode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_in,
         return encode_word_fused(ctx, model, d_in, n, chunk_syms, n_chunks, d_blob, blob_cap, d_offsets);
     const uint32_t slot = slot_bytes_for(chunk_syms);
     if (fused && (model->coder == RB200_CODER_ALIAS || model->coder == RB200_CODER_BYTE)) {
-        int rc = reserve(ctx, ctx->scratch, static_cast<size_t>(alias_fused_slots(static_cast<uint32_t>(ctx->sms))) * slot + 16);
-        if (rc == RB200_OK) rc = reserve(ctx, ctx->sizes, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t));
+        FusedWorkspace ws = {};
+        int rc = fused_workspace(ctx, fused_slot_count(ctx, model->coder, n_chunks), slot, n_chunks, &ws);
         if (rc != RB200_OK) return rc;
-        uint32_t* counter = static_cast<uint32_t*>(ctx->sizes.p);
-        uint64_t* look = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + 16);
-        RB_CUDA(ctx, cudaMemsetAsync(ctx->sizes.p, 0, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t), ctx->stream));
         const bool alias = model->coder == RB200_CODER_ALIAS;
         launch_alias_encode(ctx->stream, static_cast<uint32_t>(ctx->sms), d_in, n, chunk_syms, n_chunks, model->scale_bits, alias ? model->d_alias_enc : model->d_byte_enc,
-                            alias ? model->d_alias_remap : nullptr, static_cast<uint8_t*>(ctx->scratch.p), slot, nullptr, look, counter,
+                            alias ? model->d_alias_remap : nullptr, ws.scratch, slot, nullptr, ws.look, ws.counter,
                             d_blob, blob_cap, d_offsets, ctx->d_status);
         return check_launch(ctx, alias ? "alias_encode_kernel(fused)" : "byte_encode_kernel(fused)");
     }
@@ -959,14 +981,11 @@ int blocks_encode_device(rb200_ctx* ctx, const uint8_t* d_in, uint32_t n_blocks,
     if (use_fused_encode(chunk_syms) || build_models) {
         const uint32_t threads = block_threads(block_size, chunk_syms);
         const uint32_t grid = block_fused_grid(static_cast<uint32_t>(ctx->sms), n_blocks, threads, build_models);
-        int rc = reserve(ctx, ctx->scratch, static_cast<size_t>(grid) * (threads / 32) * 2 * slot + 16);   // two slots per resident warp
-        if (rc == RB200_OK) rc = reserve(ctx, ctx->sizes, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t));
+        FusedWorkspace ws = {};
+        int rc = fused_workspace(ctx, static_cast<size_t>(grid) * (threads / 32) * kBlockFusedSlots, slot, n_chunks, &ws);
         if (rc != RB200_OK) return rc;
-        uint32_t* counter = static_cast<uint32_t*>(ctx->sizes.p);
-        uint64_t* look = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + 16);
-        RB_CUDA(ctx, cudaMemsetAsync(ctx->sizes.p, 0, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t), ctx->stream));
         launch_block_encode_fused(ctx->stream, grid, threads, build_models, d_in, n_blocks, block_size, d_freqs, chunk_syms,
-                                  static_cast<uint8_t*>(ctx->scratch.p), slot, look, counter, d_blob, blob_cap, d_offsets, ctx->d_status);
+                                  ws.scratch, slot, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status);
         return check_launch(ctx, "block_encode_fused_kernel");
     }
     uint8_t* scratch; uint32_t* sizes; uint64_t* tile_sums;

@@ -10,6 +10,7 @@
 //                                                     exact division by reciprocal multiply
 #pragma once
 #include "device_utils.cuh"
+#include "placement.cuh"
 #include "tables.h"
 
 namespace rb200 {
@@ -467,161 +468,10 @@ word_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_sy
 constexpr uint32_t kEncSmemBytes = kEncTableBytes + kEncWarps * kEncWarpSmem;
 
 // ---------------------------------------------------------------------------
-// K2f: persistent encode with the directory and the compaction fused in.
-//
-// Every worker warp fetches chunk ids from an atomic counter (so chunks start in order), encodes the
-// chunk into one of two scratch slots that belong to the WARP and publishes its padded size.  One
-// scanner warp turns the published sizes into end offsets in chunk order.  A worker places chunk k
-// (moves its stream to blob[E_k - size .. E_k) and writes the directory entry) only after it has
-// encoded chunk k+1, so its E_k is ready and no warp polls.  One launch, no CTA barrier in the loop.
-// (Two earlier variants -- per-CTA and per-warp decoupled look-back -- were correct but slower than the
-// split path because of polling; see DESIGN.md section 6.)
+// K2f: persistent encode with the directory and the compaction fused in (the protocol: placement.cuh).
 // ---------------------------------------------------------------------------
-constexpr uint64_t kLookAgg = 1ull << 62, kLookPrefix = 2ull << 62, kLookValue = (1ull << 62) - 1;
-constexpr uint64_t kLookStallNs = 8ull * 1000 * 1000 * 1000;   // a bug must not hang the GPU: after 8 s without progress give up and
-                                                               // flag kStatStall (time, not iterations: the waits are legitimate and
-                                                               // stretch by orders of magnitude under compute-sanitizer)
-
-__device__ __forceinline__ uint64_t ld_relaxed_u64(const uint64_t* p)
-{
-    uint64_t v;
-    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_relaxed_u64(uint64_t* p, uint64_t v)
-{
-    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ uint4 ldg_l2_u128(const uint4* p)      // L2-coherent: data this kernel wrote itself
-{
-    uint4 v;
-    asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-    return v;
-}
-
-// move one finished stream (it ends at src_end, 16-byte aligned) to blob[end - size .. end)
-__device__ __forceinline__ void place_stream(const uint8_t* src_end, uint32_t size, uint8_t* __restrict__ blob, uint64_t end, uint32_t lane)
-{
-    const uint32_t padded = (size + 15u) & ~15u;
-    const uint32_t gap = padded - size;
-    const uint8_t* src = src_end - size;
-    uint8_t* dst_vec0 = blob + (end - padded);
-    if (lane < 16) {
-        uint8_t v = 0;
-        if (lane >= gap) v = *reinterpret_cast<const volatile uint8_t*>(src + (lane - gap));
-        dst_vec0[lane] = v;
-    }
-    const uint4* s4 = reinterpret_cast<const uint4*>(src + (16 - gap));
-    uint4* d4 = reinterpret_cast<uint4*>(dst_vec0 + 16);
-    const uint32_t nvec = padded / 16 - 1;
-    uint32_t v = lane;
-    for (; v + 96 < nvec; v += 128) {                      // four loads in flight per lane
-        const uint4 a = ldg_l2_u128(s4 + v), b = ldg_l2_u128(s4 + v + 32), c = ldg_l2_u128(s4 + v + 64), d = ldg_l2_u128(s4 + v + 96);
-        stg_stream_u128(d4 + v, a);
-        stg_stream_u128(d4 + v + 32, b);
-        stg_stream_u128(d4 + v + 64, c);
-        stg_stream_u128(d4 + v + 96, d);
-    }
-    for (; v < nvec; v += 32) stg_stream_u128(d4 + v, ldg_l2_u128(s4 + v));
-}
-
-// The scanner: ONE warp of the grid walks the status array in chunk order and rewrites every published
-// size (kLookAgg | padded size) into the inclusive end offset E_c (kLookPrefix | E_c).  Chunks are handed
-// out in order, so the entry it waits for always belongs to a chunk some resident warp is encoding.
-__device__ __forceinline__ void fused_scanner(uint64_t* look, uint32_t n_chunks, uint32_t lane, uint32_t* status)
-{
-    constexpr int kPer = 8;                 // consecutive entries per lane: 256 entries per trip, one warp scan per trip
-    uint64_t run = 0, idle_since = 0;
-    uint32_t pos = 0;
-    while (pos < n_chunks) {
-        const uint32_t base = pos + kPer * lane;
-        uint64_t v[kPer];
-#pragma unroll
-        for (int j = 0; j < kPer; j++) v[j] = (base + j < n_chunks) ? ld_relaxed_u64(look + base + j) : 0;   // independent loads
-        // r = length of this lane's leading run of published entries; local inclusive sums over that run
-        uint32_t r = 0;
-        uint64_t sum[kPer];
-        uint64_t acc = 0;
-        bool open = true;
-#pragma unroll
-        for (int j = 0; j < kPer; j++) {
-            open = open && ((v[j] >> 62) == 1);
-            if (open) { acc += v[j] & kLookValue; r = j + 1; }
-            sum[j] = acc;
-        }
-        // the contiguous ready prefix of the whole window: all of lanes < f, the first r_f entries of lane f
-        const uint32_t full = __ballot_sync(0xffffffffu, r == kPer);
-        const uint32_t f = full == 0xffffffffu ? 32u : static_cast<uint32_t>(__ffs(~full)) - 1u;
-        const uint32_t cnt = lane < f ? kPer : (lane == f ? r : 0u);
-        const uint64_t mine = cnt ? sum[cnt - 1] : 0;
-        uint64_t incl = mine;
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint64_t t = __shfl_up_sync(0xffffffffu, incl, d);
-            if (lane >= static_cast<uint32_t>(d)) incl += t;
-        }
-        const uint64_t before = run + incl - mine;
-#pragma unroll
-        for (int j = 0; j < kPer; j++)
-            if (static_cast<uint32_t>(j) < cnt) st_relaxed_u64(look + base + j, kLookPrefix | (before + sum[j]));
-        run += __shfl_sync(0xffffffffu, incl, 31);
-        const uint32_t r_f = __shfl_sync(0xffffffffu, r, f & 31);
-        const uint32_t done = f == 32 ? 32u * kPer : f * kPer + r_f;
-        pos += done;
-        if (done == 0) {
-            const uint64_t now = global_timer_ns();
-            if (!idle_since) idle_since = now;
-            if (now - idle_since > kLookStallNs) {   // never hang the GPU: give up and flag
-                if (lane == 0) atomicOr(status, kStatStall);
-                return;
-            }
-            __nanosleep(100);
-        } else {
-            idle_since = 0;
-        }
-    }
-}
-
-// one warp: wait for the scanner to publish E_c of `chunk`, then move the stream and write the directory entry
-__device__ __forceinline__ void fused_place(const uint64_t* look, uint32_t chunk, uint32_t n_chunks, const uint8_t* slot_end,
-                                            uint32_t produced, uint8_t* __restrict__ blob, uint64_t blob_cap,
-                                            uint64_t* __restrict__ offsets, uint32_t lane, uint32_t* status)
-{
-    // Warps do not progress evenly, so the scan front (the oldest unfinished chunk) can trail this warp by a chunk time
-    // and more: the wait is real, and every poll costs ~12 issue slots that the encoding warps of the SM want.  Back off
-    // exponentially (128 ns .. 4 us): round 1 polled every 100 ns and spent a fifth of the kernel's instructions here
-    // (seen in the ncu source view as millions of poll iterations per GiB).
-    uint64_t v = 0, since = 0;
-    uint32_t ns = 128;
-    for (;;) {
-        if (lane == 0) v = ld_relaxed_u64(look + chunk);
-        v = __shfl_sync(0xffffffffu, v, 0);
-        if ((v >> 62) == 2) break;
-        if (ns >= 4096) {                                  // only once the back-off has topped out: keep the common path short
-            const uint64_t now = global_timer_ns();
-            if (!since) since = now;
-            if (now - since > kLookStallNs) {
-                if (lane == 0) atomicOr(status, kStatStall);
-                return;
-            }
-        }
-        __nanosleep(ns);
-        if (ns < 4096) ns <<= 1;
-    }
-    const uint64_t end = v & kLookValue;                   // E_c
-    if (lane == 0) {
-        offsets[chunk] = end - produced;
-        if (chunk == n_chunks - 1) offsets[n_chunks] = end;
-    }
-    if (end <= blob_cap) {
-        place_stream(slot_end, produced, blob, end, lane);
-    } else if (lane == 0) {
-        atomicOr(status, kStatSpace);
-    }
-}
-
 // Grid = resident capacity (SMs x RB200_FUSED_MINBLOCKS CTAs).  Warp 0 of CTA 0 is the scanner, every other warp is
-// a worker with kFusedSlots scratch slots: it encodes chunk k+1 into one slot before it places chunk k from the other,
-// so by the time it asks for E_k the scanner has normally long passed k and nobody polls.
+// a worker with kFusedSlots scratch slots (a SlotQueue).
 template <bool R32>
 __global__ void __launch_bounds__(kEncWarps * 32, RB200_FUSED_MINBLOCKS)
 word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
@@ -640,15 +490,8 @@ word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t ch
         return;
     }
     const uint32_t tab = smem_addr(s_enc), wsm = tab + kEncTableBytes + warp * kEncWarpSmem;
-    // this warp's kFusedSlots scratch slots: chunk j of this warp goes to slot j % kFusedSlots and is placed
-    // kFusedSlots - 1 chunks later
-    uint8_t* slots = scratch + (static_cast<uint64_t>(blockIdx.x) * kEncWarps + warp) * kFusedSlots * slot_bytes;
-
-    // The previous chunk(s) are placed late on purpose.  Warps do not progress evenly (the issue arbiter favours high warp
-    // ids), so the scan front -- the oldest unfinished chunk -- trails the fastest warps by about one chunk time: placing
-    // 32 steps into the next chunk instead was measured to be about twice as slow: the workers spent their issue slots polling.
-    uint32_t pend_chunk[kFusedSlots - 1], pend_size[kFusedSlots - 1];      // oldest first; registers (static indexing only)
-    uint32_t n_pending = 0, cur = 0;                                        // cur = slot of the chunk being encoded
+    const PlaceOut out = {look, n_chunks, blob, blob_cap, offsets, status};
+    SlotQueue<kFusedSlots> q(scratch, static_cast<uint64_t>(blockIdx.x) * kEncWarps + warp, slot_bytes);
     for (;;) {
         uint32_t chunk = 0;
         if (lane == 0) chunk = atomicAdd(counter, 1u);     // chunks start in order
@@ -656,39 +499,10 @@ word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t ch
         if (chunk >= n_chunks) break;
         const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
         const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-        uint8_t* slot_end = slots + (cur + 1) * static_cast<uint64_t>(slot_bytes);
-        const uint32_t produced = word_encode_stream<R32, RB200_ENC_KEEP_HINT>(in + first, m, tab, wsm, slot_end, status);
-        if (lane == 0) st_relaxed_u64(look + chunk, kLookAgg | ((produced + 15u) & ~15u));
-        __syncwarp();
-        if (n_pending == kFusedSlots - 1) {                // every other slot is taken: place the oldest, it sits in slot cur + 1
-            const uint32_t oldest = cur + 1 == kFusedSlots ? 0 : cur + 1;
-            fused_place(look, pend_chunk[0], n_chunks, slots + (oldest + 1) * static_cast<uint64_t>(slot_bytes), pend_size[0], blob, blob_cap,
-                        offsets, lane, status);
-#pragma unroll
-            for (int j = 0; j + 1 < kFusedSlots - 1; j++) {
-                pend_chunk[j] = pend_chunk[j + 1];
-                pend_size[j] = pend_size[j + 1];
-            }
-            n_pending--;
-        }
-#pragma unroll
-        for (int j = 0; j < kFusedSlots - 1; j++)
-            if (static_cast<uint32_t>(j) == n_pending) {
-                pend_chunk[j] = chunk;
-                pend_size[j] = produced;
-            }
-        n_pending++;
-        cur = cur + 1 == kFusedSlots ? 0 : cur + 1;
-        __syncwarp();
+        const uint32_t produced = word_encode_stream<R32, RB200_ENC_KEEP_HINT>(in + first, m, tab, wsm, q.next_end(), status);
+        q.finish(out, chunk, produced, lane);
     }
-    // drain, oldest first: the k-th pending chunk sits k slots behind the next free one
-#pragma unroll
-    for (int j = 0; j < kFusedSlots - 1; j++)
-        if (static_cast<uint32_t>(j) < n_pending) {
-            const uint32_t slot = (cur + kFusedSlots - n_pending + j) % kFusedSlots;
-            fused_place(look, pend_chunk[j], n_chunks, slots + (slot + 1) * static_cast<uint64_t>(slot_bytes), pend_size[j], blob, blob_cap,
-                        offsets, lane, status);
-        }
+    q.drain(out, lane);
 }
 
 // ---------------------------------------------------------------------------
@@ -813,21 +627,7 @@ compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const u
             if (end > blob_cap) atomicOr(status, kStatSpace);
         }
     }
-    if (end > blob_cap) return;
-    const uint32_t padded = (size + 15u) & ~15u;
-    const uint32_t gap = padded - size;                    // zero bytes in front of the stream, < 16
-    const uint8_t* src = scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes - size;
-    uint8_t* dst_vec0 = blob + (end - padded);             // 16-byte aligned
-
-    if (lane < 16) {                                       // first vector: gap zeros + stream head
-        uint8_t v = 0;
-        if (lane >= gap) v = src[lane - gap];
-        dst_vec0[lane] = v;
-    }
-    const uint4* s4 = reinterpret_cast<const uint4*>(src + (16 - gap));   // 16-byte aligned by construction
-    uint4* d4 = reinterpret_cast<uint4*>(dst_vec0 + 16);
-    const uint32_t nvec = padded / 16 - 1;
-    for (uint32_t v = lane; v < nvec; v += 32) stg_stream_u128(d4 + v, ldg_stream_u128(s4 + v));
+    if (end <= blob_cap) place_stream<false>(scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, size, blob, end, lane);
 }
 
 }  // namespace rb200

@@ -1,10 +1,12 @@
-"""The fused word encoder (K2f) over many more chunks than it has resident warps.
+"""The fused encoders over many more chunks than they have resident warps.
 
-Every worker warp of word_encode_fused_kernel cycles through a few scratch slots of its own and places a chunk a
-chunk late.  The fused test in test_gpu_parity.py encodes 3 M symbols, fewer chunks than there are workers, so no
+Every worker warp of word_encode_fused_kernel (K2f) and block_encode_fused_kernel (K5f) cycles through a few scratch
+slots of its own and places a chunk a chunk late (placement.cuh: SlotQueue).  The fused test in test_gpu_parity.py encodes 3 M symbols, fewer chunks than there are workers, so no
 slot is ever reused there.  Here 64 Mi symbols at chunks of 4096 / 8192 make every worker take several chunks, with
 three models: uniform, Zipf, and a two-symbol model {4095, 1} on data that is mostly the frequency-1 symbol (about
-11 bits per symbol, close to the worst case a chunk's scratch slot is sized for).
+11 bits per symbol, close to the worst case a chunk's scratch slot is sized for).  The per-block tests in
+test_gpu_parity.py encode at most 200 blocks, fewer than the worker CTAs of K5f (5 per SM, less the scanner's); here
+4096 blocks make every worker CTA take several blocks.
 """
 import numpy as np
 import pytest
@@ -63,3 +65,60 @@ def test_fused_encode_reuses_slots(gpu_ctx, oracle_lib, kind, chunk):
     gpu_ctx.sync()
     assert torch.equal(out, data)
     model.close()
+
+
+def test_fused_block_encode_reuses_slots(gpu_ctx, oracle_lib):
+    """K5f with and without the model build (rb200_blocks_model_encode, rb200_blocks_encode) on 4096 blocks of 64 KiB at
+    chunks of 8192: models, directory and blob match the oracle block by block, and the container decodes back."""
+    import torch
+    n_blocks, block_size, chunk = 4096, 65536, 8192
+    per = block_size // chunk
+    g = torch.Generator(device="cuda")
+    g.manual_seed(0xB10C)
+    # block b: Zipf over 256 symbols with exponent 0.6 + 0.1 * (b % 9), as in test_gpu_parity.py's per-block cases
+    expo = 0.6 + 0.1 * (torch.arange(n_blocks, dtype=torch.float64) % 9)
+    p = 1.0 / torch.arange(1, 257, dtype=torch.float64)[None, :] ** expo[:, None]
+    cdf = torch.cumsum(p / p.sum(1, keepdim=True), 1).to(device="cuda", dtype=torch.float32).contiguous()
+    u = torch.rand(n_blocks, block_size, device="cuda", generator=g)
+    data = torch.searchsorted(cdf, u).clamp_(max=255).to(torch.uint8).reshape(-1)
+    n = data.numel()
+    cap = gpu_ctx.encode_bound(n, chunk)
+
+    def encode(build):
+        freqs = torch.zeros((n_blocks, 256), dtype=torch.int16, device="cuda")    # u16 bit patterns
+        blob = torch.zeros(cap, dtype=torch.uint8, device="cuda")
+        offs = torch.zeros(n_blocks * per + 1, dtype=torch.int64, device="cuda")
+        if build:
+            gpu_ctx.blocks_model_encode_device(data.data_ptr(), n_blocks, block_size, freqs.data_ptr(), chunk, blob.data_ptr(), cap,
+                                               offs.data_ptr())
+        else:
+            gpu_ctx.blocks_build_models_device(data.data_ptr(), n_blocks, block_size, freqs.data_ptr())
+            gpu_ctx.blocks_encode_device(data.data_ptr(), n_blocks, block_size, freqs.data_ptr(), chunk, blob.data_ptr(), cap,
+                                         offs.data_ptr())
+        gpu_ctx.sync()
+        return freqs, blob, offs
+
+    freqs, blob, offs = encode(True)
+    freqs2, blob2, offs2 = encode(False)
+    assert torch.equal(freqs, freqs2) and torch.equal(offs, offs2) and torch.equal(blob, blob2)
+
+    h_data = data.cpu().numpy()
+    h_freqs = freqs.cpu().numpy().view(np.uint16)
+    h_offs = offs.cpu().numpy().astype(np.uint64)
+    size = int(h_offs[-1])
+    h_blob = blob[:size].cpu().numpy()
+    base = 0
+    for b in range(n_blocks):             # oracle: every block is its own container; they concatenate (16-byte aligned ends)
+        blk = h_data[b * block_size:(b + 1) * block_size]
+        f, c = oracle_lib.model(blk, 12)
+        assert np.array_equal(h_freqs[b].astype(np.uint32), f), b
+        ob, oo = oracle_lib.chunked_encode(orc.CODER_WORD, blk, f, c, chunk, nlanes=32, scale_bits=12)
+        assert np.array_equal(h_offs[b * per:(b + 1) * per], oo[:-1] + np.uint64(base)), b
+        assert np.array_equal(h_blob[base:base + ob.size], ob), b
+        base += ob.size
+    assert size == base
+
+    out = torch.zeros_like(data)
+    gpu_ctx.blocks_decode_device(blob.data_ptr(), size, offs.data_ptr(), freqs.data_ptr(), n_blocks, block_size, chunk, out.data_ptr())
+    gpu_ctx.sync()
+    assert torch.equal(out, data)
