@@ -282,11 +282,11 @@ class Context:
                                                               MEM_HOST), self.h)
         return freqs
 
-    def blocks_encode_host(self, data, n_blocks, block_size, block_freqs, chunk_syms):
+    def blocks_encode_host(self, data, n_blocks, block_size, block_freqs, chunk_syms, blob_cap=None):
         data = np.ascontiguousarray(data, dtype=np.uint8)
         block_freqs = np.ascontiguousarray(block_freqs, dtype=np.uint16)
         n_chunks = n_blocks * (block_size // chunk_syms)
-        cap = self.encode_bound(data.size, chunk_syms)
+        cap = self.encode_bound(data.size, chunk_syms) if blob_cap is None else blob_cap
         blob = np.zeros(max(cap, 16), np.uint8)
         offsets = np.zeros(n_chunks + 1, np.uint64)
         size = C.c_size_t(0)
@@ -295,12 +295,12 @@ class Context:
                                                         MEM_HOST), self.h)
         return blob[:size.value].copy(), offsets
 
-    def blocks_model_encode_host(self, data, n_blocks, block_size, chunk_syms):
+    def blocks_model_encode_host(self, data, n_blocks, block_size, chunk_syms, blob_cap=None):
         """models + encode in one call; returns (blob, offsets, block_freqs)"""
         data = np.ascontiguousarray(data, dtype=np.uint8)
         freqs = np.zeros((n_blocks, 256), np.uint16)
         n_chunks = n_blocks * (block_size // chunk_syms)
-        cap = self.encode_bound(data.size, chunk_syms)
+        cap = self.encode_bound(data.size, chunk_syms) if blob_cap is None else blob_cap
         blob = np.zeros(max(cap, 16), np.uint8)
         offsets = np.zeros(n_chunks + 1, np.uint64)
         size = C.c_size_t(0)

@@ -213,20 +213,8 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
         return RB200_E_CUDA;
     }
     // the decoders want the large shared-memory carve-out (tables + per-warp rings)
-    cudaFuncSetAttribute(word_decode_tma_kernel<DecShip, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_decode_tma_kernel<DecShip, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DecShip::kSmemBytes);
-    cudaFuncSetAttribute(word_decode_tma_kernel<DecShip, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_decode_tma_kernel<DecShip, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DecShip::kSmemBytes);
-    cudaFuncSetAttribute(word_decode_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_decode_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_encode_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_encode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
-    cudaFuncSetAttribute(word_encode_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_encode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
-    cudaFuncSetAttribute(word_encode_fused_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_encode_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
-    cudaFuncSetAttribute(word_encode_fused_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_encode_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+    configure_word_decode_tma();
+    configure_word_kernels();
     configure_alias_kernels();
     configure_block_kernels();
     configure_rans64_kernels();
@@ -641,8 +629,6 @@ int decode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_blo
     return rc;
 }
 
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 }  // namespace
 
 namespace {
@@ -668,37 +654,44 @@ int reserve_dir(rb200_ctx* ctx, size_t entries)
     return RB200_OK;
 }
 
-// An error exit of a host pipeline must not leave copies in flight: they target the caller's buffers and the context's
-// staging, which a later reserve() may free.  Also clears whatever the kernels flagged.
-int fail_pipeline(rb200_ctx* ctx, int rc)
+// Runs `enqueue`, the part of a host pipeline that puts work on the three streams.  An error exit must not leave copies
+// in flight: they target the caller's buffers and the context's staging, which a later reserve() may free.  So any
+// non-OK result first drains the streams, and clears whatever the kernels flagged.
+template <class Enqueue>
+int run_pipeline(rb200_ctx* ctx, Enqueue enqueue)
 {
-    cudaStreamSynchronize(ctx->s_in);
-    cudaStreamSynchronize(ctx->stream);
-    cudaStreamSynchronize(ctx->s_out);
-    cudaMemsetAsync(ctx->d_status, 0, sizeof(uint32_t), ctx->stream);
-    cudaMemsetAsync(ctx->d_work, 0, sizeof(DecodeWork), ctx->stream);
-    cudaStreamSynchronize(ctx->stream);
+    const int rc = enqueue();
+    if (rc != RB200_OK) {
+        cudaStreamSynchronize(ctx->s_in);
+        cudaStreamSynchronize(ctx->stream);
+        cudaStreamSynchronize(ctx->s_out);
+        cudaMemsetAsync(ctx->d_status, 0, sizeof(uint32_t), ctx->stream);
+        cudaMemsetAsync(ctx->d_work, 0, sizeof(DecodeWork), ctx->stream);
+        cudaStreamSynchronize(ctx->stream);
+    }
     return rc;
 }
 
-// One pipeline slice of a host-mode call: chunks [c0, c0 + cnt) = symbols [lo, lo + len).
+// One pipeline slice of a host-mode call: units [u0, u0 + units) = chunks [c0, c0 + cnt) = symbols [lo, lo + len).
+// A unit is one chunk for rb200_encode / rb200_decode and one block for the per-block calls.
 struct Slice {
-    size_t c0, cnt, lo, len;
+    size_t u0, units, c0, cnt, lo, len;
 };
 
 // Slice plan for the host pipeline.  Steady-state slices are `RB200_SLICE_MIB` (default 32 MiB) of symbols:
 // big enough that PCIe time dwarfs launch overhead and the per-slice host wake-up, small enough to overlap.
 // The first and last three slices ramp (1/8, 1/4, 1/2 of that) so that the pipeline fill (first H2D) and
 // drain (last D2H), which nothing overlaps, are short.  Returns the number of slices (<= kMaxSlices).
-size_t plan_slices(size_t n, uint32_t chunk_syms, Slice* out)
+// Slices hold whole units of `unit_syms` symbols and `unit_chunks` chunks.
+size_t plan_slices(size_t n, uint32_t unit_syms, uint32_t unit_chunks, Slice* out)
 {
     static const size_t tuned = [] {        // tuning knob for the host pipeline (1..1024 MiB)
         const char* e = std::getenv("RB200_SLICE_MIB");
         const long v = e ? std::atol(e) : 0;
         return (v >= 1 && v <= 1024) ? static_cast<size_t>(v) << 20 : static_cast<size_t>(32u << 20);
     }();
-    const size_t total = rb200_chunk_count(n, chunk_syms);
-    size_t tc = (tuned + chunk_syms - 1) / chunk_syms;                // chunks per steady-state slice
+    const size_t total = rb200_chunk_count(n, unit_syms);
+    size_t tc = (tuned + unit_syms - 1) / unit_syms;                  // units per steady-state slice
     if (tc == 0) tc = 1;
     const size_t room = rb200_ctx::kMaxSlices - 8;
     if (total / tc >= room) tc = total / room + 1;
@@ -708,9 +701,9 @@ size_t plan_slices(size_t n, uint32_t chunk_syms, Slice* out)
     auto push = [&](size_t cnt) {
         if (cnt == 0) return;
         if (cnt > total - c) cnt = total - c;
-        const size_t lo = c * chunk_syms;
-        const size_t len = (n - lo < cnt * chunk_syms) ? n - lo : cnt * chunk_syms;
-        out[k++] = Slice{c, cnt, lo, len};
+        const size_t lo = c * unit_syms;
+        const size_t len = (n - lo < cnt * unit_syms) ? n - lo : cnt * unit_syms;
+        out[k++] = Slice{c, cnt, c * unit_chunks, cnt * unit_chunks, lo, len};
         c += cnt;
     };
     const size_t tail = ramped ? ramp[0] + ramp[1] + ramp[2] : 0;
@@ -722,138 +715,187 @@ size_t plan_slices(size_t n, uint32_t chunk_syms, Slice* out)
     return k;
 }
 
+// A table of `unit_bytes` per unit that a host pipeline moves along with each slice (the per-block frequency tables),
+// staged in ctx->st_aux: copied in before the slice runs when `in` is set, or out after it when `out` is set.
+struct UnitTable {
+    const void* in;
+    void* out;
+    size_t unit_bytes;
+};
+
 // Host buffers -> blob, overlapped: slice i+1 is copied in while slice i is encoded and slice i-1 is
 // copied out.  Every slice is its own container in a staging region; because containers end 16-byte
 // aligned they concatenate, and the directory entries only need the running base added.  Directories are
 // staged in pinned memory (an async copy to a pageable `offsets` would block the issuing thread).
-int encode_host(rb200_ctx* ctx, const rb200_model* model, const uint8_t* in, size_t n, uint32_t chunk_syms, uint8_t* blob,
-                size_t blob_cap, uint64_t* offsets, size_t* blob_size)
+// `reserve_ws(units)` grows the encode workspace for a slice of that many units; it runs once, for the largest slice,
+// so that no slice stalls on a reallocation.  `encode_slice(slice, d_in, d_table, d_blob, cap, d_offsets)` enqueues
+// one slice's encode on ctx->stream.
+template <class ReserveWs, class EncodeSlice>
+int encode_pipeline(rb200_ctx* ctx, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t unit_chunks, UnitTable tab,
+                    ReserveWs reserve_ws, EncodeSlice encode_slice, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size)
 {
-    const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
     if (n == 0) {
         offsets[0] = 0;
         if (blob_size) *blob_size = 0;
         return RB200_OK;
     }
+    const uint32_t unit_syms = chunk_syms * unit_chunks;
+    const size_t n_units = rb200_chunk_count(n, unit_syms), n_chunks = n_units * unit_chunks;
     Slice sl[rb200_ctx::kMaxSlices];
-    const size_t n_slices = plan_slices(n, chunk_syms, sl);
-    size_t max_cnt = 0;
-    for (size_t i = 0; i < n_slices; i++) max_cnt = sl[i].cnt > max_cnt ? sl[i].cnt : max_cnt;
+    const size_t n_slices = plan_slices(n, unit_syms, unit_chunks, sl);
+    size_t max_units = 0;
+    for (size_t i = 0; i < n_slices; i++) max_units = sl[i].units > max_units ? sl[i].units : max_units;
+    const size_t slot = slot_bytes_for(chunk_syms);
     // slice i's container is built at bound(symbols before it); its directory at c0 + i (cnt + 1 entries)
     int rc = reserve(ctx, ctx->st_in, n + 16);
-    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_blob, n_chunks * static_cast<size_t>(slot_bytes_for(chunk_syms)) + 16);
+    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_blob, n_chunks * slot + 16);
     if (rc == RB200_OK) rc = reserve(ctx, ctx->st_offsets, (n_chunks + n_slices) * sizeof(uint64_t));
+    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_aux, n_units * tab.unit_bytes);
     if (rc == RB200_OK) rc = reserve_dir(ctx, n_chunks + n_slices);
-    if (rc == RB200_OK) rc = reserve_encode(ctx, model, static_cast<uint32_t>(max_cnt), chunk_syms);   // no regrowth mid-pipeline
+    if (rc == RB200_OK) rc = reserve_ws(max_units);
     if (rc != RB200_OK) return rc;
     uint8_t* d_in = static_cast<uint8_t*>(ctx->st_in.p);
     uint8_t* d_blob = static_cast<uint8_t*>(ctx->st_blob.p);
     uint64_t* d_off = static_cast<uint64_t*>(ctx->st_offsets.p);
-    const size_t slot = slot_bytes_for(chunk_syms);
+    uint8_t* d_tab = static_cast<uint8_t*>(ctx->st_aux.p);
+    const size_t tb = tab.unit_bytes;
 
-    RB_CUDA(ctx, cudaEventRecord(ctx->ev_start, ctx->stream));       // staging buffers may still be in use upstream
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_in, ctx->ev_start, 0));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_start, 0));
-
-    auto issue = [&](size_t i) -> int {      // H2D + kernels for slice i
-        const Slice& s = sl[i];
-        RB_CUDA(ctx, cudaMemcpyAsync(d_in + s.lo, in + s.lo, s.len, cudaMemcpyHostToDevice, ctx->s_in));
-        RB_CUDA(ctx, cudaEventRecord(ctx->ev_in[i], ctx->s_in));
-        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[i], 0));
-        uint64_t* so = d_off + s.c0 + i;
-        int r = encode_device(ctx, model, d_in + s.lo, s.len, chunk_syms, d_blob + s.c0 * slot, s.cnt * slot, so);
+    return run_pipeline(ctx, [&]() -> int {
+        RB_CUDA(ctx, cudaEventRecord(ctx->ev_start, ctx->stream));       // staging buffers may still be in use upstream
+        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_in, ctx->ev_start, 0));
+        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_start, 0));
+        auto issue = [&](size_t i) -> int {      // H2D + kernels for slice i
+            const Slice& s = sl[i];
+            RB_CUDA(ctx, cudaMemcpyAsync(d_in + s.lo, in + s.lo, s.len, cudaMemcpyHostToDevice, ctx->s_in));
+            if (tab.in)
+                RB_CUDA(ctx, cudaMemcpyAsync(d_tab + s.u0 * tb, static_cast<const uint8_t*>(tab.in) + s.u0 * tb, s.units * tb,
+                                             cudaMemcpyHostToDevice, ctx->s_in));
+            RB_CUDA(ctx, cudaEventRecord(ctx->ev_in[i], ctx->s_in));
+            RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[i], 0));
+            uint64_t* so = d_off + s.c0 + i;
+            const int r = encode_slice(s, d_in + s.lo, d_tab + s.u0 * tb, d_blob + s.c0 * slot, s.cnt * slot, so);
+            if (r != RB200_OK) return r;
+            RB_CUDA(ctx, cudaMemcpyAsync(&ctx->h_slice_total[i], so + s.cnt, sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
+            RB_CUDA(ctx, cudaEventRecord(ctx->ev_done[i], ctx->stream));
+            return RB200_OK;
+        };
+        int r = issue(0);
         if (r != RB200_OK) return r;
-        RB_CUDA(ctx, cudaMemcpyAsync(&ctx->h_slice_total[i], so + s.cnt, sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        RB_CUDA(ctx, cudaEventRecord(ctx->ev_done[i], ctx->stream));
+        size_t base = 0;
+        bool overflow = false;
+        for (size_t i = 0; i < n_slices; i++) {
+            if (i + 1 < n_slices) {
+                r = issue(i + 1);
+                if (r != RB200_OK) return r;
+            }
+            RB_CUDA(ctx, cudaEventSynchronize(ctx->ev_done[i]));          // slice i's size is now on the host
+            const size_t total = static_cast<size_t>(ctx->h_slice_total[i]);
+            const Slice& s = sl[i];
+            if (base + total > blob_cap) {
+                overflow = true;                                          // finish the slices, copy nothing more out
+            } else if (!overflow) {
+                RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_done[i], 0));
+                RB_CUDA(ctx, cudaMemcpyAsync(blob + base, d_blob + s.c0 * slot, total, cudaMemcpyDeviceToHost, ctx->s_out));
+                RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir + s.c0 + i, d_off + s.c0 + i, s.cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+                                             ctx->s_out));
+                if (tab.out)
+                    RB_CUDA(ctx, cudaMemcpyAsync(static_cast<uint8_t*>(tab.out) + s.u0 * tb, d_tab + s.u0 * tb, s.units * tb,
+                                                 cudaMemcpyDeviceToHost, ctx->s_out));
+            }
+            ctx->h_slice_total[i] = base;                                 // reuse as "base of slice i"
+            base += total;
+        }
+        RB_CUDA(ctx, cudaEventRecord(ctx->ev_out, ctx->s_out));
+        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_out, 0));
+        r = rb200_sync(ctx);
+        if (r != RB200_OK) return r;
+        if (overflow) return RB200_E_SPACE;
+        for (size_t i = 0; i < n_slices; i++) {                           // rebase the directory into the caller's array
+            const uint64_t add = ctx->h_slice_total[i];
+            const uint64_t* src = ctx->h_dir + sl[i].c0 + i;
+            uint64_t* dst = offsets + sl[i].c0;
+            for (size_t c = 0; c < sl[i].cnt; c++) dst[c] = src[c] + add;
+        }
+        offsets[n_chunks] = base;
+        if (blob_size) *blob_size = base;
         return RB200_OK;
-    };
-
-    rc = issue(0);
-    if (rc != RB200_OK) return fail_pipeline(ctx, rc);
-    size_t base = 0;
-    bool overflow = false;
-    for (size_t i = 0; i < n_slices; i++) {
-        if (i + 1 < n_slices) {
-            rc = issue(i + 1);
-            if (rc != RB200_OK) return fail_pipeline(ctx, rc);
-        }
-        RB_CUDA(ctx, cudaEventSynchronize(ctx->ev_done[i]));          // slice i's size is now on the host
-        const size_t total = static_cast<size_t>(ctx->h_slice_total[i]);
-        const Slice& s = sl[i];
-        if (base + total > blob_cap) {
-            overflow = true;
-        } else if (!overflow) {
-            RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_done[i], 0));
-            RB_CUDA(ctx, cudaMemcpyAsync(blob + base, d_blob + s.c0 * slot, total, cudaMemcpyDeviceToHost, ctx->s_out));
-            RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir + s.c0 + i, d_off + s.c0 + i, s.cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost,
-                                         ctx->s_out));
-        }
-        ctx->h_slice_total[i] = base;                                 // reuse as "base of slice i"
-        base += total;
-    }
-    RB_CUDA(ctx, cudaEventRecord(ctx->ev_out, ctx->s_out));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_out, 0));
-    rc = rb200_sync(ctx);
-    if (rc != RB200_OK) return rc;
-    if (overflow) return RB200_E_SPACE;
-    for (size_t i = 0; i < n_slices; i++) {                           // rebase the directory into the caller's array
-        const uint64_t add = ctx->h_slice_total[i];
-        const uint64_t* src = ctx->h_dir + sl[i].c0 + i;
-        uint64_t* dst = offsets + sl[i].c0;
-        for (size_t c = 0; c < sl[i].cnt; c++) dst[c] = src[c] + add;
-    }
-    offsets[n_chunks] = base;
-    if (blob_size) *blob_size = base;
-    return RB200_OK;
+    });
 }
 
 // blob -> host buffers, overlapped the same way; no host synchronisation until the end because the
 // directory (and therefore every slice's byte range) is already on the host.
-int decode_host(rb200_ctx* ctx, const rb200_model* model, const uint8_t* blob, size_t blob_size, const uint64_t* offsets,
-                uint32_t chunk_syms, uint8_t* out, size_t n)
+// `decode_slice(slice, d_blob, d_offsets, d_table, d_out)` enqueues one slice's decode on ctx->stream; d_offsets points
+// at the slice's first directory entry.
+template <class DecodeSlice>
+int decode_pipeline(rb200_ctx* ctx, const uint8_t* blob, size_t blob_size, const uint64_t* offsets, uint32_t chunk_syms,
+                    uint32_t unit_chunks, UnitTable tab, DecodeSlice decode_slice, uint8_t* out, size_t n)
 {
-    const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
     if (n == 0) return RB200_OK;
+    const uint32_t unit_syms = chunk_syms * unit_chunks;
+    const size_t n_units = rb200_chunk_count(n, unit_syms), n_chunks = n_units * unit_chunks;
     if (offsets[n_chunks] != blob_size) return RB200_E_STREAM;
     Slice sl[rb200_ctx::kMaxSlices];
-    const size_t n_slices = plan_slices(n, chunk_syms, sl);
+    const size_t n_slices = plan_slices(n, unit_syms, unit_chunks, sl);
     int rc = reserve(ctx, ctx->st_blob, blob_size + 16);
     if (rc == RB200_OK) rc = reserve(ctx, ctx->st_offsets, (n_chunks + 1) * sizeof(uint64_t));
     if (rc == RB200_OK) rc = reserve(ctx, ctx->st_out, n + 16);
+    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_aux, n_units * tab.unit_bytes);
     if (rc == RB200_OK) rc = reserve_dir(ctx, n_chunks + 1);
     if (rc != RB200_OK) return rc;
-    uint8_t* d_blob = static_cast<uint8_t*>(ctx->st_blob.p);
-    uint64_t* d_off = static_cast<uint64_t*>(ctx->st_offsets.p);
-    uint8_t* d_out = static_cast<uint8_t*>(ctx->st_out.p);
-
-    RB_CUDA(ctx, cudaEventRecord(ctx->ev_start, ctx->stream));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_in, ctx->ev_start, 0));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_start, 0));
     for (size_t c = 0; c < n_chunks; c++) {                          // the copies below trust these
         if (offsets[c] > offsets[c + 1] || offsets[c + 1] > blob_size) return RB200_E_STREAM;
         ctx->h_dir[c] = offsets[c];
     }
     ctx->h_dir[n_chunks] = offsets[n_chunks];
-    RB_CUDA(ctx, cudaMemcpyAsync(d_off, ctx->h_dir, (n_chunks + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->s_in));
-    for (size_t i = 0; i < n_slices; i++) {
-        const Slice& s = sl[i];
-        const size_t c1 = s.c0 + s.cnt;
-        // bytes of chunks [c0, c1): from the (aligned) end of chunk c0-1 to the end of chunk c1-1
-        const size_t b0 = s.c0 ? static_cast<size_t>(offsets[s.c0] & ~15ull) : 0;
-        const size_t b1 = static_cast<size_t>(offsets[c1] & ~15ull);
-        if (b1 > b0) RB_CUDA(ctx, cudaMemcpyAsync(d_blob + b0, blob + b0, b1 - b0, cudaMemcpyHostToDevice, ctx->s_in));
-        RB_CUDA(ctx, cudaEventRecord(ctx->ev_in[i], ctx->s_in));
-        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[i], 0));
-        rc = decode_device(ctx, model, d_blob, blob_size, d_off + s.c0, chunk_syms, d_out + s.lo, s.len);
-        if (rc != RB200_OK) return fail_pipeline(ctx, rc);
-        RB_CUDA(ctx, cudaEventRecord(ctx->ev_done[i], ctx->stream));
-        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_done[i], 0));
-        RB_CUDA(ctx, cudaMemcpyAsync(out + s.lo, d_out + s.lo, s.len, cudaMemcpyDeviceToHost, ctx->s_out));
-    }
-    RB_CUDA(ctx, cudaEventRecord(ctx->ev_out, ctx->s_out));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_out, 0));
-    return rb200_sync(ctx);
+    uint8_t* d_blob = static_cast<uint8_t*>(ctx->st_blob.p);
+    uint64_t* d_off = static_cast<uint64_t*>(ctx->st_offsets.p);
+    uint8_t* d_out = static_cast<uint8_t*>(ctx->st_out.p);
+    uint8_t* d_tab = static_cast<uint8_t*>(ctx->st_aux.p);
+    const size_t tb = tab.unit_bytes;
+
+    return run_pipeline(ctx, [&]() -> int {
+        RB_CUDA(ctx, cudaEventRecord(ctx->ev_start, ctx->stream));
+        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_in, ctx->ev_start, 0));
+        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_start, 0));
+        RB_CUDA(ctx, cudaMemcpyAsync(d_off, ctx->h_dir, (n_chunks + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->s_in));
+        for (size_t i = 0; i < n_slices; i++) {
+            const Slice& s = sl[i];
+            // bytes of chunks [c0, c1): from the (aligned) end of chunk c0-1 to the end of chunk c1-1
+            const size_t b0 = s.c0 ? static_cast<size_t>(offsets[s.c0] & ~15ull) : 0;
+            const size_t b1 = static_cast<size_t>(offsets[s.c0 + s.cnt] & ~15ull);
+            if (b1 > b0) RB_CUDA(ctx, cudaMemcpyAsync(d_blob + b0, blob + b0, b1 - b0, cudaMemcpyHostToDevice, ctx->s_in));
+            if (tab.in)
+                RB_CUDA(ctx, cudaMemcpyAsync(d_tab + s.u0 * tb, static_cast<const uint8_t*>(tab.in) + s.u0 * tb, s.units * tb,
+                                             cudaMemcpyHostToDevice, ctx->s_in));
+            RB_CUDA(ctx, cudaEventRecord(ctx->ev_in[i], ctx->s_in));
+            RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[i], 0));
+            const int r = decode_slice(s, d_blob, d_off + s.c0, d_tab + s.u0 * tb, d_out + s.lo);
+            if (r != RB200_OK) return r;
+            RB_CUDA(ctx, cudaEventRecord(ctx->ev_done[i], ctx->stream));
+            RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_done[i], 0));
+            RB_CUDA(ctx, cudaMemcpyAsync(out + s.lo, d_out + s.lo, s.len, cudaMemcpyDeviceToHost, ctx->s_out));
+        }
+        RB_CUDA(ctx, cudaEventRecord(ctx->ev_out, ctx->s_out));
+        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_out, 0));
+        return rb200_sync(ctx);
+    });
 }
+
+// Entry checks shared by the encode / decode calls.  RB200_MEM_DEVICE runs `device` once the blob (16 bytes) and the
+// directory (8 bytes) are aligned for the kernels; RB200_MEM_HOST runs `host`, a slice pipeline.
+template <class Device, class Host>
+int by_mem_kind(int mem_kind, const void* blob, const uint64_t* offsets, Device device, Host host)
+{
+    if (mem_kind == RB200_MEM_DEVICE) {
+        if ((reinterpret_cast<uintptr_t>(blob) & 15) || (reinterpret_cast<uintptr_t>(offsets) & 7)) return RB200_E_ARG;
+        return device();
+    }
+    if (mem_kind != RB200_MEM_HOST) return RB200_E_ARG;
+    return host();
+}
+
+// container invariant: the blob ends on a 16-byte boundary; the decoders index it in 16-byte vectors with 32 bits
+bool blob_size_ok(size_t blob_size) { return (blob_size & 15) == 0 && (blob_size >> 36) == 0; }
 
 }  // namespace
 
@@ -862,12 +904,17 @@ extern "C" int rb200_encode(rb200_ctx* ctx, const rb200_model* model, const uint
 {
     if (!ctx || !model || model->ctx != ctx || !blob || !offsets || (!in && n) || !chunk_ok(chunk_syms)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
-    if (mem_kind == RB200_MEM_DEVICE) {
-        if (!aligned16(blob) || (reinterpret_cast<uintptr_t>(offsets) & 7)) return RB200_E_ARG;
-        return encode_device(ctx, model, in, n, chunk_syms, blob, blob_cap, offsets);
-    }
-    if (mem_kind != RB200_MEM_HOST) return RB200_E_ARG;
-    return encode_host(ctx, model, in, n, chunk_syms, blob, blob_cap, offsets, blob_size);
+    return by_mem_kind(
+        mem_kind, blob, offsets, [&] { return encode_device(ctx, model, in, n, chunk_syms, blob, blob_cap, offsets); },
+        [&] {
+            return encode_pipeline(
+                ctx, in, n, chunk_syms, 1, UnitTable{},
+                [&](size_t units) { return reserve_encode(ctx, model, static_cast<uint32_t>(units), chunk_syms); },
+                [&](const Slice& s, const uint8_t* d_in, uint8_t*, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
+                    return encode_device(ctx, model, d_in, s.len, chunk_syms, d_blob, cap, d_off);
+                },
+                blob, blob_cap, offsets, blob_size);
+        });
 }
 
 extern "C" int rb200_decode(rb200_ctx* ctx, const rb200_model* model, const uint8_t* blob, size_t blob_size,
@@ -875,15 +922,18 @@ extern "C" int rb200_decode(rb200_ctx* ctx, const rb200_model* model, const uint
 {
     if (!ctx || !model || model->ctx != ctx || !offsets || (!out && n) || (!blob && blob_size) || !chunk_ok(chunk_syms))
         return RB200_E_ARG;
-    if (blob_size & 15) return RB200_E_ARG;     // container invariant: the blob ends on a 16-byte boundary
-    if (blob_size >> 36) return RB200_E_ARG;    // the decoders index the blob in 16-byte vectors with 32 bits
+    if (!blob_size_ok(blob_size)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
-    if (mem_kind == RB200_MEM_DEVICE) {
-        if (!aligned16(blob) || (reinterpret_cast<uintptr_t>(offsets) & 7)) return RB200_E_ARG;
-        return decode_device(ctx, model, blob, blob_size, offsets, chunk_syms, out, n);
-    }
-    if (mem_kind != RB200_MEM_HOST) return RB200_E_ARG;
-    return decode_host(ctx, model, blob, blob_size, offsets, chunk_syms, out, n);
+    return by_mem_kind(
+        mem_kind, blob, offsets, [&] { return decode_device(ctx, model, blob, blob_size, offsets, chunk_syms, out, n); },
+        [&] {
+            return decode_pipeline(
+                ctx, blob, blob_size, offsets, chunk_syms, 1, UnitTable{},
+                [&](const Slice& s, const uint8_t* d_blob, const uint64_t* d_off, uint8_t*, uint8_t* d_out) {
+                    return decode_device(ctx, model, d_blob, blob_size, d_off, chunk_syms, d_out, s.len);
+                },
+                out, n);
+        });
 }
 
 // ---------------------------------------------------------------------------
@@ -967,6 +1017,36 @@ extern "C" int rb200_blocks_build_models(rb200_ctx* ctx, const uint8_t* in, uint
 
 namespace {
 
+constexpr size_t kBlockFreqBytes = 256 * sizeof(uint16_t);     // one block's frequency table
+
+// The per-block encoder's launch shape over `n_blocks` blocks: the fused kernel on `grid` CTAs of `threads` threads with
+// `slots` scratch slots (slots per warp x the warps of its grid), or the split sequence when grid is 0.
+// blocks_encode_device and reserve_blocks_encode size the workspace from it.
+struct BlockEncodeShape {
+    uint32_t threads, grid;
+    size_t slots;
+};
+
+BlockEncodeShape block_encode_shape(rb200_ctx* ctx, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, bool build_models)
+{
+    if (!use_fused_encode(chunk_syms) && !build_models) return BlockEncodeShape{0, 0, 0};
+    const uint32_t threads = block_threads(block_size, chunk_syms);
+    const uint32_t grid = block_fused_grid(static_cast<uint32_t>(ctx->sms), n_blocks, threads, build_models);
+    return BlockEncodeShape{threads, grid, static_cast<size_t>(grid) * (threads / 32) * kBlockFusedSlots};
+}
+
+// Grows the encode workspaces to what a per-block encode over `n_blocks` blocks needs (the host pipeline does this once
+// for its largest slice, which holds far fewer than 2^31 chunks).
+int reserve_blocks_encode(rb200_ctx* ctx, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, bool build_models)
+{
+    const uint32_t n_chunks = n_blocks * (block_size / chunk_syms);
+    const uint32_t slot = slot_bytes_for(chunk_syms);
+    const BlockEncodeShape shape = block_encode_shape(ctx, n_blocks, block_size, chunk_syms, build_models);
+    if (shape.grid) return reserve_fused(ctx, shape.slots, slot, n_chunks);
+    uint8_t* scratch; uint32_t* sizes; uint64_t* tile_sums;
+    return reserve_encode_workspace(ctx, n_chunks, slot, &scratch, &sizes, &tile_sums);
+}
+
 // Per-block encode.  Default: ONE persistent launch (block_encode_fused_kernel: [model,] tables, encode, directory,
 // placement); build_models makes the kernel run count_freqs + normalize_freqs per block first and write d_freqs.
 // RB200_ENCODE_PATH=split keeps the round-1 sequence (encode into per-chunk slots, tile scan, compaction).
@@ -978,13 +1058,12 @@ int blocks_encode_device(rb200_ctx* ctx, const uint8_t* d_in, uint32_t n_blocks,
     if (n_chunks64 >= (1ull << 31)) return RB200_E_ARG;
     const uint32_t n_chunks = static_cast<uint32_t>(n_chunks64);
     const uint32_t slot = slot_bytes_for(chunk_syms);
-    if (use_fused_encode(chunk_syms) || build_models) {
-        const uint32_t threads = block_threads(block_size, chunk_syms);
-        const uint32_t grid = block_fused_grid(static_cast<uint32_t>(ctx->sms), n_blocks, threads, build_models);
+    const BlockEncodeShape shape = block_encode_shape(ctx, n_blocks, block_size, chunk_syms, build_models);
+    if (shape.grid) {
         FusedWorkspace ws = {};
-        int rc = fused_workspace(ctx, static_cast<size_t>(grid) * (threads / 32) * kBlockFusedSlots, slot, n_chunks, &ws);
+        int rc = fused_workspace(ctx, shape.slots, slot, n_chunks, &ws);
         if (rc != RB200_OK) return rc;
-        launch_block_encode_fused(ctx->stream, grid, threads, build_models, d_in, n_blocks, block_size, d_freqs, chunk_syms,
+        launch_block_encode_fused(ctx->stream, shape.grid, shape.threads, build_models, d_in, n_blocks, block_size, d_freqs, chunk_syms,
                                   ws.scratch, slot, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status);
         return check_launch(ctx, "block_encode_fused_kernel");
     }
@@ -1003,159 +1082,27 @@ bool blocks_geometry_ok(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_s
     return n_blocks && block_size && chunk_ok(chunk_syms) && block_size % chunk_syms == 0 && block_size / chunk_syms <= 32;
 }
 
-
-// Host buffers -> blob for the per-block path, overlapped like encode_host: slices of whole blocks; slice i+1 is
-// copied in (with its frequency tables when the caller supplies them) while slice i is encoded and slice i-1 is copied
-// out (blob, directory, and the frequency tables when the kernel built them).
-int blocks_encode_host(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint16_t* block_freqs, bool build,
-                       uint32_t chunk_syms, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size)
-{
-    const uint32_t per_block = block_size / chunk_syms;
-    const size_t n = static_cast<size_t>(n_blocks) * block_size;
-    const size_t n_chunks = static_cast<size_t>(n_blocks) * per_block;
-    Slice sl[rb200_ctx::kMaxSlices];                         // planned in units of blocks: c0 / cnt count blocks here
-    const size_t n_slices = plan_slices(n, block_size, sl);
-    const size_t slot = slot_bytes_for(chunk_syms);
-    const size_t fbytes = static_cast<size_t>(n_blocks) * 256 * sizeof(uint16_t);
-    int rc = reserve(ctx, ctx->st_in, n + 16);
-    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_blob, n_chunks * slot + 16);
-    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_offsets, (n_chunks + n_slices) * sizeof(uint64_t));
-    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_aux, fbytes);
-    if (rc == RB200_OK) rc = reserve_dir(ctx, n_chunks + n_slices);
-    if (rc != RB200_OK) return rc;
-    uint8_t* d_in = static_cast<uint8_t*>(ctx->st_in.p);
-    uint8_t* d_blob = static_cast<uint8_t*>(ctx->st_blob.p);
-    uint64_t* d_off = static_cast<uint64_t*>(ctx->st_offsets.p);
-    uint16_t* d_freqs = static_cast<uint16_t*>(ctx->st_aux.p);
-
-    RB_CUDA(ctx, cudaEventRecord(ctx->ev_start, ctx->stream));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_in, ctx->ev_start, 0));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_start, 0));
-
-    auto issue = [&](size_t i) -> int {
-        const Slice& s = sl[i];
-        const size_t c0 = s.c0 * per_block, cnt = s.cnt * per_block;          // chunks of this slice
-        RB_CUDA(ctx, cudaMemcpyAsync(d_in + s.lo, in + s.lo, s.len, cudaMemcpyHostToDevice, ctx->s_in));
-        if (!build)
-            RB_CUDA(ctx, cudaMemcpyAsync(d_freqs + s.c0 * 256, block_freqs + s.c0 * 256, s.cnt * 256 * sizeof(uint16_t),
-                                         cudaMemcpyHostToDevice, ctx->s_in));
-        RB_CUDA(ctx, cudaEventRecord(ctx->ev_in[i], ctx->s_in));
-        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[i], 0));
-        uint64_t* so = d_off + c0 + i;
-        int r = blocks_encode_device(ctx, d_in + s.lo, static_cast<uint32_t>(s.cnt), block_size, d_freqs + s.c0 * 256, build, chunk_syms,
-                                     d_blob + c0 * slot, cnt * slot, so);
-        if (r != RB200_OK) return r;
-        RB_CUDA(ctx, cudaMemcpyAsync(&ctx->h_slice_total[i], so + cnt, sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        RB_CUDA(ctx, cudaEventRecord(ctx->ev_done[i], ctx->stream));
-        return RB200_OK;
-    };
-    rc = issue(0);
-    if (rc != RB200_OK) return fail_pipeline(ctx, rc);
-    size_t base = 0;
-    bool overflow = false;
-    for (size_t i = 0; i < n_slices; i++) {
-        if (i + 1 < n_slices) {
-            rc = issue(i + 1);
-            if (rc != RB200_OK) return fail_pipeline(ctx, rc);
-        }
-        RB_CUDA(ctx, cudaEventSynchronize(ctx->ev_done[i]));
-        const size_t total = static_cast<size_t>(ctx->h_slice_total[i]);
-        const Slice& s = sl[i];
-        const size_t c0 = s.c0 * per_block, cnt = s.cnt * per_block;
-        if (base + total > blob_cap) {
-            overflow = true;
-        } else if (!overflow) {
-            RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_done[i], 0));
-            RB_CUDA(ctx, cudaMemcpyAsync(blob + base, d_blob + c0 * slot, total, cudaMemcpyDeviceToHost, ctx->s_out));
-            RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir + c0 + i, d_off + c0 + i, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->s_out));
-            if (build)
-                RB_CUDA(ctx, cudaMemcpyAsync(block_freqs + s.c0 * 256, d_freqs + s.c0 * 256, s.cnt * 256 * sizeof(uint16_t),
-                                             cudaMemcpyDeviceToHost, ctx->s_out));
-        }
-        ctx->h_slice_total[i] = base;
-        base += total;
-    }
-    RB_CUDA(ctx, cudaEventRecord(ctx->ev_out, ctx->s_out));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_out, 0));
-    rc = rb200_sync(ctx);
-    if (rc != RB200_OK) return rc;
-    if (overflow) return RB200_E_SPACE;
-    for (size_t i = 0; i < n_slices; i++) {                  // rebase the directory into the caller's array
-        const uint64_t add = ctx->h_slice_total[i];
-        const size_t c0 = sl[i].c0 * per_block, cnt = sl[i].cnt * per_block;
-        const uint64_t* src = ctx->h_dir + c0 + i;
-        uint64_t* dst = offsets + c0;
-        for (size_t c = 0; c < cnt; c++) dst[c] = src[c] + add;
-    }
-    offsets[n_chunks] = base;
-    if (blob_size) *blob_size = base;
-    return RB200_OK;
-}
-
-int blocks_decode_host(rb200_ctx* ctx, const uint8_t* blob, size_t blob_size, const uint64_t* offsets, const uint16_t* block_freqs,
-                       uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint8_t* out)
-{
-    const uint32_t per_block = block_size / chunk_syms;
-    const size_t n = static_cast<size_t>(n_blocks) * block_size;
-    const size_t n_chunks = static_cast<size_t>(n_blocks) * per_block;
-    if (offsets[n_chunks] != blob_size) return RB200_E_STREAM;
-    Slice sl[rb200_ctx::kMaxSlices];                         // units of blocks
-    const size_t n_slices = plan_slices(n, block_size, sl);
-    const size_t fbytes = static_cast<size_t>(n_blocks) * 256 * sizeof(uint16_t);
-    int rc = reserve(ctx, ctx->st_blob, blob_size + 16);
-    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_offsets, (n_chunks + 1) * sizeof(uint64_t));
-    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_out, n + 16);
-    if (rc == RB200_OK) rc = reserve(ctx, ctx->st_aux, fbytes);
-    if (rc == RB200_OK) rc = reserve_dir(ctx, n_chunks + 1);
-    if (rc != RB200_OK) return rc;
-    uint8_t* d_blob = static_cast<uint8_t*>(ctx->st_blob.p);
-    uint64_t* d_off = static_cast<uint64_t*>(ctx->st_offsets.p);
-    uint8_t* d_out = static_cast<uint8_t*>(ctx->st_out.p);
-    uint16_t* d_freqs = static_cast<uint16_t*>(ctx->st_aux.p);
-    for (size_t c = 0; c < n_chunks; c++) {                  // the copies below trust these
-        if (offsets[c] > offsets[c + 1] || offsets[c + 1] > blob_size) return RB200_E_STREAM;
-        ctx->h_dir[c] = offsets[c];
-    }
-    ctx->h_dir[n_chunks] = offsets[n_chunks];
-
-    RB_CUDA(ctx, cudaEventRecord(ctx->ev_start, ctx->stream));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_in, ctx->ev_start, 0));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_start, 0));
-    RB_CUDA(ctx, cudaMemcpyAsync(d_off, ctx->h_dir, (n_chunks + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->s_in));
-    for (size_t i = 0; i < n_slices; i++) {
-        const Slice& s = sl[i];
-        const size_t c0 = s.c0 * per_block, c1 = (s.c0 + s.cnt) * per_block;
-        const size_t b0 = c0 ? static_cast<size_t>(offsets[c0] & ~15ull) : 0;
-        const size_t b1 = static_cast<size_t>(offsets[c1] & ~15ull);
-        if (b1 > b0) RB_CUDA(ctx, cudaMemcpyAsync(d_blob + b0, blob + b0, b1 - b0, cudaMemcpyHostToDevice, ctx->s_in));
-        RB_CUDA(ctx, cudaMemcpyAsync(d_freqs + s.c0 * 256, block_freqs + s.c0 * 256, s.cnt * 256 * sizeof(uint16_t), cudaMemcpyHostToDevice,
-                                     ctx->s_in));
-        RB_CUDA(ctx, cudaEventRecord(ctx->ev_in[i], ctx->s_in));
-        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[i], 0));
-        launch_block_decode(ctx->stream, d_blob, blob_size, d_off + c0, d_freqs + s.c0 * 256, static_cast<uint32_t>(s.cnt), block_size,
-                            chunk_syms, d_out + s.lo, ctx->d_status);
-        rc = check_launch(ctx, "block_decode_kernel");
-        if (rc != RB200_OK) return fail_pipeline(ctx, rc);
-        RB_CUDA(ctx, cudaEventRecord(ctx->ev_done[i], ctx->stream));
-        RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_done[i], 0));
-        RB_CUDA(ctx, cudaMemcpyAsync(out + s.lo, d_out + s.lo, s.len, cudaMemcpyDeviceToHost, ctx->s_out));
-    }
-    RB_CUDA(ctx, cudaEventRecord(ctx->ev_out, ctx->s_out));
-    RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_out, 0));
-    return rb200_sync(ctx);
-}
-
+// Host mode runs the slice pipeline over whole blocks; the frequency tables go in with each slice when the caller supplies
+// them, and come back with it when the kernel builds them.
 int blocks_encode_entry(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint16_t* block_freqs, bool build,
                         uint32_t chunk_syms, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind)
 {
     if (!ctx || !in || !block_freqs || !blob || !offsets || !blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
-    if (mem_kind == RB200_MEM_DEVICE) {
-        if (!aligned16(blob) || (reinterpret_cast<uintptr_t>(offsets) & 7)) return RB200_E_ARG;
-        return blocks_encode_device(ctx, in, n_blocks, block_size, block_freqs, build, chunk_syms, blob, blob_cap, offsets);
-    }
-    if (mem_kind != RB200_MEM_HOST) return RB200_E_ARG;
-    return blocks_encode_host(ctx, in, n_blocks, block_size, block_freqs, build, chunk_syms, blob, blob_cap, offsets, blob_size);
+    return by_mem_kind(
+        mem_kind, blob, offsets,
+        [&] { return blocks_encode_device(ctx, in, n_blocks, block_size, block_freqs, build, chunk_syms, blob, blob_cap, offsets); },
+        [&] {
+            const UnitTable freqs = build ? UnitTable{nullptr, block_freqs, kBlockFreqBytes} : UnitTable{block_freqs, nullptr, kBlockFreqBytes};
+            return encode_pipeline(
+                ctx, in, static_cast<size_t>(n_blocks) * block_size, chunk_syms, block_size / chunk_syms, freqs,
+                [&](size_t units) { return reserve_blocks_encode(ctx, static_cast<uint32_t>(units), block_size, chunk_syms, build); },
+                [&](const Slice& s, const uint8_t* d_in, uint8_t* d_freqs, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
+                    return blocks_encode_device(ctx, d_in, static_cast<uint32_t>(s.units), block_size, reinterpret_cast<uint16_t*>(d_freqs),
+                                                build, chunk_syms, d_blob, cap, d_off);
+                },
+                blob, blob_cap, offsets, blob_size);
+        });
 }
 
 }  // namespace
@@ -1180,18 +1127,24 @@ extern "C" int rb200_blocks_decode(rb200_ctx* ctx, const uint8_t* blob, size_t b
                                    uint8_t* out, int mem_kind)
 {
     if (!ctx || !blob || !offsets || !block_freqs || !out || !blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
-    if (blob_size & 15) return RB200_E_ARG;
-    if (blob_size >> 36) return RB200_E_ARG;
+    if (!blob_size_ok(blob_size)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
-    const size_t n_chunks = static_cast<size_t>(n_blocks) * (block_size / chunk_syms);
-    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
-    if (mem_kind == RB200_MEM_DEVICE) {
-        if (!aligned16(blob) || (reinterpret_cast<uintptr_t>(offsets) & 7)) return RB200_E_ARG;
-        launch_block_decode(ctx->stream, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out, ctx->d_status);
+    const uint32_t per_block = block_size / chunk_syms;
+    if (static_cast<uint64_t>(n_blocks) * per_block >= (1ull << 31)) return RB200_E_ARG;
+    auto decode = [&](const uint8_t* d_blob, const uint64_t* d_off, const uint16_t* d_freqs, uint32_t blocks, uint8_t* d_out) {
+        launch_block_decode(ctx->stream, d_blob, blob_size, d_off, d_freqs, blocks, block_size, chunk_syms, d_out, ctx->d_status);
         return check_launch(ctx, "block_decode_kernel");
-    }
-    if (mem_kind != RB200_MEM_HOST) return RB200_E_ARG;
-    return blocks_decode_host(ctx, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out);
+    };
+    return by_mem_kind(
+        mem_kind, blob, offsets, [&] { return decode(blob, offsets, block_freqs, n_blocks, out); },
+        [&] {
+            return decode_pipeline(
+                ctx, blob, blob_size, offsets, chunk_syms, per_block, UnitTable{block_freqs, nullptr, kBlockFreqBytes},
+                [&](const Slice& s, const uint8_t* d_blob, const uint64_t* d_off, uint8_t* d_freqs, uint8_t* d_out) {
+                    return decode(d_blob, d_off, reinterpret_cast<const uint16_t*>(d_freqs), static_cast<uint32_t>(s.units), d_out);
+                },
+                out, static_cast<size_t>(n_blocks) * block_size);
+        });
 }
 
 // ---------------------------------------------------------------------------

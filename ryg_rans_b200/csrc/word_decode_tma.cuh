@@ -462,4 +462,12 @@ word_decode_tma_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, con
 // table by one TMA bulk copy, freq / bias by one IMAD.WIDE, slot and x >> 12 by shift / mask.
 using DecShip = DecPolicy<32, 2, 8, kRefillCpAsync, 9, 2, 0, 0, false>;
 
+inline void configure_word_decode_tma()
+{
+    cudaFuncSetAttribute(word_decode_tma_kernel<DecShip, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_decode_tma_kernel<DecShip, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DecShip::kSmemBytes);
+    cudaFuncSetAttribute(word_decode_tma_kernel<DecShip, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_decode_tma_kernel<DecShip, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DecShip::kSmemBytes);
+}
+
 }  // namespace rb200

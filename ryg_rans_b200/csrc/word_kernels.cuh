@@ -630,4 +630,18 @@ compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const u
     if (end <= blob_cap) place_stream<false>(scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, size, blob, end, lane);
 }
 
+inline void configure_word_kernels()
+{
+    cudaFuncSetAttribute(word_decode_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_decode_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_encode_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_encode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+    cudaFuncSetAttribute(word_encode_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_encode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+    cudaFuncSetAttribute(word_encode_fused_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_encode_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+    cudaFuncSetAttribute(word_encode_fused_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_encode_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+}
+
 }  // namespace rb200

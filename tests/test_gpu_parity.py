@@ -350,6 +350,44 @@ def _check_blocks(gpu_ctx, oracle_lib, data, n_blocks, block_size, chunk):
     return freqs16
 
 
+# 520 blocks of 64 KiB = 32.5 MiB: the host pipeline's default plan is two slices (512 blocks, then 8)
+_TWO_SLICE_BLOCKS = 520
+
+
+def test_block_encode_bound_is_tight_enough(gpu_ctx, gen):
+    """Per-block host encodes into a blob 16 bytes short of the container fail with E_SPACE (-3) once the second slice
+    does not fit; the context then encodes the same input at full capacity to the identical blob, directory and models."""
+    import ryg_rans_b200 as rb
+    n_blocks, block_size, chunk = _TWO_SLICE_BLOCKS, 65536, 8192
+    data = _block_data(gen, n_blocks, block_size)
+    blob, offs, freqs = gpu_ctx.blocks_model_encode_host(data, n_blocks, block_size, chunk)
+    calls = (lambda cap: gpu_ctx.blocks_model_encode_host(data, n_blocks, block_size, chunk, blob_cap=cap),
+             lambda cap: gpu_ctx.blocks_encode_host(data, n_blocks, block_size, freqs, chunk, blob_cap=cap) + (freqs,))
+    for call in calls:
+        with pytest.raises(rb.RansError) as ei:
+            call(blob.size - 16)
+        assert ei.value.code == -3
+        b2, o2, f2 = call(None)
+        assert np.array_equal(b2, blob) and np.array_equal(o2, offs) and np.array_equal(f2, freqs)
+
+
+def test_block_corrupt_stream_is_reported(gpu_ctx, gen):
+    """A per-block host decode of a container with one corrupted stream in its second slice fails with E_STREAM (-4);
+    the context then decodes the intact container to the input."""
+    import ryg_rans_b200 as rb
+    n_blocks, block_size, chunk = _TWO_SLICE_BLOCKS, 65536, 8192
+    data = _block_data(gen, n_blocks, block_size)
+    blob, offs, freqs = gpu_ctx.blocks_model_encode_host(data, n_blocks, block_size, chunk)
+    c = 517 * (block_size // chunk) + 3              # block 517 holds uniform bytes: a stream of about 8 KiB
+    assert int(offs[c + 1]) - int(offs[c]) > 4096
+    bad = blob.copy()
+    bad[int(offs[c]) + 128:int(offs[c]) + 400] ^= 0x5A
+    with pytest.raises(rb.RansError) as ei:
+        gpu_ctx.blocks_decode_host(bad, offs, freqs, n_blocks, block_size, chunk)
+    assert ei.value.code == -4
+    assert np.array_equal(gpu_ctx.blocks_decode_host(blob, offs, freqs, n_blocks, block_size, chunk), data)
+
+
 # ---------------------------------------------------------------- alternative paths, big sizes
 
 @pytest.mark.parametrize("path", ["fused", "split"])
