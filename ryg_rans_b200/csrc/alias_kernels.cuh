@@ -441,7 +441,7 @@ alias_decode_persist_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size
 // alias_remap (u16, 2 << scale_bits bytes = 128 KiB at scale_bits 16; SURVEY H8) lives in
 // shared memory next to the 8x replicated per-symbol table ({magic, freq, cum, shift}, one
 // conflict-free LDS.128 per step) and the per-warp 512 B symbol stage + 512 B output ring
-// (same staged, vectorised I/O as the word encoder).
+// of the shared chunk encoder (encode_stream.cuh).
 // ---------------------------------------------------------------------------
 constexpr int kAliasEncWarps = 32;
 constexpr uint32_t kAliasEncFixedSmem = kAliasEncWarps * kEncWarpSmem + kEncTableBytes;   // 64 KiB + remap
@@ -454,167 +454,97 @@ __device__ __forceinline__ uint32_t lds_u16_ro(uint32_t addr)
     return v;
 }
 
-struct AliasEncState {
-    uint32_t x;        // rANS state
-    uint32_t wpos;     // un-wrapped ring position of the next byte = 511 - bytes_emitted
-    uint32_t flags;
-};
-
-// One encode step of the byte-renormalising coders for the whole warp.
+// The byte-renormalising coders for encode_stream (encode_stream.cuh); wpos is the ring position of the next byte =
+// 511 - bytes_emitted.  step = one encode step for the whole warp:
 //   ALIAS:  RansEncPutAlias (main_alias.cpp:241-250); table {magic, freq, cum, shift}
 //   !ALIAS: RansEncPutSymbol (rans_byte.h:258-280);   table {x_max, rcp_freq, bias, cmpl_freq | rcp_shift << 16}
 //           = RansEncSymbol (rans_byte.h:159-165), bit 31 of the last word marks a symbol outside the model
-// FULL: all 32 lanes take part (active == true at compile time); only the ragged first step of a chunk does not.
-template <bool ALIAS, bool FULL, uint32_t SB>
-__device__ __forceinline__ void alias_enc_step(AliasEncState& st, uint32_t sym, uint32_t tab_lane, uint32_t remap, uint32_t ring,
-                                               uint32_t gt, uint32_t sb_rt, bool active)
-{
-    const uint32_t sb = SB ? SB : sb_rt;
-    bool n1 = false, n2 = false;
-    uint4 e = make_uint4(0, 1, 0, 0);
-    uint32_t x_max = 0;
-    if (active) {
-        e = lds_u128_ro(tab_lane + sym * (kEncReplicas * 16));
-        st.flags |= e.w;
-        x_max = ALIAS ? e.y << (31 - sb) : e.x;                   // ((L >> sb) << 8) * freq, rans_byte.h:64 / :197
-    }
-    if (FULL) {
-        // the renormalisation below as one PTX sequence: two predicates feed the votes, the ranked stores and
-        // the shifts (the compiler otherwise re-evaluates the comparisons and branches around the stores)
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p1, p2;\n\t"
-            ".reg .b32 m1, m2, r1, r2, a, b, xs;\n\t"
-            "shr.u32 xs, %0, 8;\n\t"
-            "setp.ge.u32 p1, %0, %2;\n\t"
-            "setp.ge.u32 p2, xs, %2;\n\t"
-            "vote.sync.ballot.b32 m1, p1, 0xffffffff;\n\t"
-            "vote.sync.ballot.b32 m2, p2, 0xffffffff;\n\t"
-            "and.b32 r1, m1, %3;\n\t"
-            "and.b32 r2, m2, %3;\n\t"
-            "popc.b32 r1, r1;\n\t"
-            "popc.b32 r2, r2;\n\t"
-            "sub.u32 a, %1, r1;\n\t"
-            "sub.u32 a, a, r2;\n\t"
-            "sub.u32 b, a, 1;\n\t"
-            "and.b32 a, a, %4;\n\t"
-            "and.b32 b, b, %4;\n\t"
-            "or.b32 a, a, %5;\n\t"
-            "or.b32 b, b, %5;\n\t"
-            "@p1 st.shared.u8 [a], %0;\n\t"
-            "@p2 st.shared.u8 [b], xs;\n\t"
-            "@p1 mov.b32 %0, xs;\n\t"
-            "@p2 shr.u32 %0, %0, 8;\n\t"
-            "popc.b32 m1, m1;\n\t"
-            "popc.b32 m2, m2;\n\t"
-            "sub.u32 %1, %1, m1;\n\t"
-            "sub.u32 %1, %1, m2;\n\t"
-            "}"
-            : "+r"(st.x), "+r"(st.wpos)
-            : "r"(x_max), "r"(gt), "n"(kEncRingBytes - 1), "r"(ring)
-            : "memory");
-    } else {
-        if (active) {
-            n1 = st.x >= x_max;                                   // :65 / :265
-            n2 = (st.x >> 8) >= x_max;                            // second trip of the do/while, :67-70
-        }
-        const uint32_t m1 = __ballot_sync(0xffffffffu, n1);
-        const uint32_t m2 = __ballot_sync(0xffffffffu, n2);
-        if (n1) {
-            // lanes are visited 31..0 (main_alias.cpp:365-370 generalised); each writes downwards
-            const uint32_t pos = st.wpos - __popc(m1 & gt) - __popc(m2 & gt);
-            sts_u8(ring | (pos & (kEncRingBytes - 1)), st.x);                          // :68
-            if (n2) sts_u8(ring | ((pos - 1) & (kEncRingBytes - 1)), st.x >> 8);
-            st.x >>= n2 ? 16 : 8;                                                      // :69
-        }
-        st.wpos -= __popc(m1) + __popc(m2);
-    }
-    if (active) {
-        if (ALIAS) {
-            // exact x / freq with the 33-bit round-up reciprocal 2^32 + magic, as in the word encoder; here
-            // x < 2^31 (rans_byte.h:26-28), so x + mulhi(x, magic) < 2^32 and there is no carry to fold in
-            const uint32_t q = funnel_shr_wrap(st.x + __umulhi(st.x, e.x), 0u, e.w);
-            const uint32_t r = st.x - q * e.y;                                     // x % freq
-            st.x = (q << sb) + lds_u16_ro(remap + 2u * (r + e.z));                 // main_alias.cpp:249
-        } else {
-            const uint32_t q = __umulhi(st.x, e.y) >> ((e.w >> 16) & 31u);         // rans_byte.h:278
-            st.x = st.x + e.z + q * (e.w & 0xffffu);                               // :279
-        }
-    }
-}
-
-// Encode m symbols (one warp) as one 32-way byte-renormalised stream ending at slot_end (16-byte aligned);
-// returns the stream size in bytes (warp-uniform).
 template <bool ALIAS, uint32_t SB>
-__device__ __forceinline__ uint32_t alias_encode_stream(const uint8_t* __restrict__ chunk_in, uint32_t m, uint32_t tab, uint32_t remap,
-                                                        uint32_t wsm, uint32_t sb, uint8_t* __restrict__ slot_end,
-                                                        uint32_t* __restrict__ status)
-{
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t stage = wsm, ring = wsm + kEncStageBytes;
-    const uint32_t tab_lane = tab + (lane & (kEncReplicas - 1)) * 16;
-    const uint32_t gt = lanemask_gt();
+struct AliasEncoder {
+    using X = uint32_t;
+    static constexpr uint32_t kUnit = 1, kMaxEmit = 2, kBadBit = kEncBadSymbol;
+    static constexpr X kInit = kByteL;                 // RansEncInit, rans_byte.h:56-59
+    uint32_t tab;                                      // shared address of the 8x replicated uint4 table
+    uint32_t remap;                                    // ALIAS: shared address of alias_remap (u16)
+    uint32_t sb_rt;                                    // scale_bits when SB == 0
 
-    AliasEncState st;
-    st.x = kByteL;                              // RansEncInit, rans_byte.h:56-59
-    st.wpos = kEncRingBytes - 1;
-    st.flags = 0;
-    uint32_t flushed = 0;
-    const uint32_t steps = m >> 5, rem = m & 31;
-    const uint32_t nblk = steps >> 4;
-    const bool vec_ok = (reinterpret_cast<uintptr_t>(chunk_in) & 15) == 0;
-
-    uint4 parked = make_uint4(0, 0, 0, 0);
-    if (nblk && vec_ok) parked = ldg_stream_u128(reinterpret_cast<const uint4*>(chunk_in + (nblk - 1) * kEncStageBytes) + lane);
-    if (rem) {
-        const bool active = lane < rem;
-        const uint32_t s = active ? chunk_in[static_cast<uint64_t>(steps) * 32 + lane] : 0;
-        alias_enc_step<ALIAS, false, SB>(st, s, tab_lane, remap, ring, gt, sb, active);
-    }
-    for (uint32_t g = steps; g > nblk * 16; g--) {
-        const uint32_t s = chunk_in[static_cast<uint64_t>(g - 1) * 32 + lane];
-        alias_enc_step<ALIAS, true, SB>(st, s, tab_lane, remap, ring, gt, sb, true);
-        if (((g - 1) & 3) == 0) word_enc_flush(kEncRingBytes - 1 - st.wpos, flushed, ring, slot_end, lane);
-    }
-    word_enc_flush(kEncRingBytes - 1 - st.wpos, flushed, ring, slot_end, lane);
-
-    for (uint32_t b = nblk; b-- > 0;) {
-        __syncwarp();
-        if (vec_ok) {
-            sts_u128(stage + lane * 16, parked);
-            if (b) parked = ldg_stream_u128(reinterpret_cast<const uint4*>(chunk_in + (b - 1) * kEncStageBytes) + lane);
+    template <bool FULL>
+    __device__ __forceinline__ void step(EncState<X>& st, uint32_t sym, uint32_t tab_lane, uint32_t ring, uint32_t gt, bool active) const
+    {
+        const uint32_t sb = SB ? SB : sb_rt;
+        bool n1 = false, n2 = false;
+        uint4 e = make_uint4(0, 1, 0, 0);
+        uint32_t x_max = 0;
+        if (active) {
+            e = lds_u128_ro(tab_lane + sym * (kEncReplicas * 16));
+            st.flags |= e.w;
+            x_max = ALIAS ? e.y << (31 - sb) : e.x;                   // ((L >> sb) << 8) * freq, rans_byte.h:64 / :197
+        }
+        if (FULL) {
+            // the renormalisation below as one PTX sequence: two predicates feed the votes, the ranked stores and
+            // the shifts (the compiler otherwise re-evaluates the comparisons and branches around the stores)
+            asm volatile(
+                "{\n\t"
+                ".reg .pred p1, p2;\n\t"
+                ".reg .b32 m1, m2, r1, r2, a, b, xs;\n\t"
+                "shr.u32 xs, %0, 8;\n\t"
+                "setp.ge.u32 p1, %0, %2;\n\t"
+                "setp.ge.u32 p2, xs, %2;\n\t"
+                "vote.sync.ballot.b32 m1, p1, 0xffffffff;\n\t"
+                "vote.sync.ballot.b32 m2, p2, 0xffffffff;\n\t"
+                "and.b32 r1, m1, %3;\n\t"
+                "and.b32 r2, m2, %3;\n\t"
+                "popc.b32 r1, r1;\n\t"
+                "popc.b32 r2, r2;\n\t"
+                "sub.u32 a, %1, r1;\n\t"
+                "sub.u32 a, a, r2;\n\t"
+                "sub.u32 b, a, 1;\n\t"
+                "and.b32 a, a, %4;\n\t"
+                "and.b32 b, b, %4;\n\t"
+                "or.b32 a, a, %5;\n\t"
+                "or.b32 b, b, %5;\n\t"
+                "@p1 st.shared.u8 [a], %0;\n\t"
+                "@p2 st.shared.u8 [b], xs;\n\t"
+                "@p1 mov.b32 %0, xs;\n\t"
+                "@p2 shr.u32 %0, %0, 8;\n\t"
+                "popc.b32 m1, m1;\n\t"
+                "popc.b32 m2, m2;\n\t"
+                "sub.u32 %1, %1, m1;\n\t"
+                "sub.u32 %1, %1, m2;\n\t"
+                "}"
+                : "+r"(st.x), "+r"(st.wpos)
+                : "r"(x_max), "r"(gt), "n"(kEncRingBytes - 1), "r"(ring)
+                : "memory");
         } else {
-            const uint8_t* p = chunk_in + b * kEncStageBytes + lane;
-#pragma unroll
-            for (int j = 0; j < 16; j++) sts_u8(stage + j * 32 + lane, p[j * 32]);
+            if (active) {
+                n1 = st.x >= x_max;                                   // :65 / :265
+                n2 = (st.x >> 8) >= x_max;                            // second trip of the do/while, :67-70
+            }
+            const uint32_t m1 = __ballot_sync(0xffffffffu, n1);
+            const uint32_t m2 = __ballot_sync(0xffffffffu, n2);
+            if (n1) {
+                // lanes are visited 31..0 (main_alias.cpp:365-370 generalised); each writes downwards
+                const uint32_t pos = st.wpos - __popc(m1 & gt) - __popc(m2 & gt);
+                sts_u8(ring | (pos & (kEncRingBytes - 1)), st.x);                          // :68
+                if (n2) sts_u8(ring | ((pos - 1) & (kEncRingBytes - 1)), st.x >> 8);
+                st.x >>= n2 ? 16 : 8;                                                      // :69
+            }
+            st.wpos -= __popc(m1) + __popc(m2);
         }
-        __syncwarp();
-#pragma unroll
-        for (int grp = 3; grp >= 0; grp--) {
-#pragma unroll
-            for (int j = 3; j >= 0; j--)
-                alias_enc_step<ALIAS, true, SB>(st, lds_u8(stage + (grp * 4 + j) * 32 + lane), tab_lane, remap, ring, gt, sb, true);
-            if (kEncRingBytes - 1 - st.wpos - flushed >= 256) word_enc_flush(kEncRingBytes - 1 - st.wpos, flushed, ring, slot_end, lane);
+        if (active) {
+            if (ALIAS) {
+                // exact x / freq with the 33-bit round-up reciprocal 2^32 + magic, as in the word encoder; here
+                // x < 2^31 (rans_byte.h:26-28), so x + mulhi(x, magic) < 2^32 and there is no carry to fold in
+                const uint32_t q = funnel_shr_wrap(st.x + __umulhi(st.x, e.x), 0u, e.w);
+                const uint32_t r = st.x - q * e.y;                                     // x % freq
+                st.x = (q << sb) + lds_u16_ro(remap + 2u * (r + e.z));                 // main_alias.cpp:249
+            } else {
+                const uint32_t q = __umulhi(st.x, e.y) >> ((e.w >> 16) & 31u);         // rans_byte.h:278
+                st.x = st.x + e.z + q * (e.w & 0xffffu);                               // :279
+            }
         }
     }
-
-    // RansEncFlush for lanes 31..0 (rans_byte.h:93-105): lane 31's most significant byte is the first byte
-    // written (highest address); lane 0's least significant byte ends up first in memory
-    word_enc_flush(kEncRingBytes - 1 - st.wpos, flushed, ring, slot_end, lane);     // < 16 bytes stay pending
-    const uint32_t hpos = st.wpos - 4u * (31 - lane);
-#pragma unroll
-    for (int j = 0; j < 4; j++) sts_u8(ring | ((hpos - (3 - j)) & (kEncRingBytes - 1)), st.x >> (8 * j));
-    st.wpos -= kHeaderBytes;
-    const uint32_t produced = kEncRingBytes - 1 - st.wpos;
-    word_enc_flush(produced, flushed, ring, slot_end, lane);
-    const uint32_t left = produced - flushed;                        // < 16 bytes: head of the stream
-    if (lane < left) {
-        const uint32_t off = flushed + lane + 1;
-        *(slot_end - off) = static_cast<uint8_t>(lds_u8(ring | ((0u - off) & (kEncRingBytes - 1))));
-    }
-    if (__any_sync(0xffffffffu, (st.flags & kEncBadSymbol) != 0) && lane == 0) atomicOr(status, kStatSymbol);
-    return produced;
-}
+};
 
 // !ALIAS: g_enc holds RansEncSymbol images {x_max, rcp_freq, bias, cmpl | shift << 16}, g_remap is unused
 // Two modes (like the word encoder):
@@ -648,13 +578,13 @@ alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_s
 
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t base = smem_addr(s_alias);
-    const uint32_t tab = base + kAliasEncWarps * kEncWarpSmem, remap = base + kAliasEncFixedSmem, wsm = base + warp * kEncWarpSmem;
+    const uint32_t wsm = base + warp * kEncWarpSmem;
+    const AliasEncoder<ALIAS, SB> coder = {base + kAliasEncWarps * kEncWarpSmem, base + kAliasEncFixedSmem, sb};
     if (!look) {
         for (uint32_t chunk = blockIdx.x * kAliasEncWarps + warp; chunk < n_chunks; chunk += gridDim.x * kAliasEncWarps) {
             const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
             const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-            const uint32_t produced = alias_encode_stream<ALIAS, SB>(in + first, m, tab, remap, wsm, sb,
-                                                                 scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, status);
+            const uint32_t produced = encode_stream(in + first, m, coder, wsm, scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, status);
             if (lane == 0) sizes[chunk] = produced;
         }
         return;
@@ -672,7 +602,7 @@ alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_s
         if (chunk >= n_chunks) break;
         const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
         const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-        const uint32_t produced = alias_encode_stream<ALIAS, SB>(in + first, m, tab, remap, wsm, sb, q.next_end(), status);
+        const uint32_t produced = encode_stream(in + first, m, coder, wsm, q.next_end(), status);
         q.finish(out, chunk, produced, lane);
     }
     q.drain(out, lane);

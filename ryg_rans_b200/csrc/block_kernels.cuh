@@ -446,8 +446,8 @@ block_encode_fused_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uin
         const bool r32 = block_build_enc_table(s_cum, ok, s_tab);
         if (warp < per_block) {
             const uint8_t* src = blk + static_cast<uint64_t>(warp) * chunk_syms;
-            const uint32_t produced = r32 ? word_encode_stream<true>(src, chunk_syms, tab, wsm, q.next_end(), status)
-                                          : word_encode_stream<false>(src, chunk_syms, tab, wsm, q.next_end(), status);
+            const uint32_t produced = r32 ? encode_stream(src, chunk_syms, WordEncoder<true>{tab}, wsm, q.next_end(), status)
+                                          : encode_stream(src, chunk_syms, WordEncoder<false>{tab}, wsm, q.next_end(), status);
             q.finish(out, block * per_block + warp, produced, lane);
         }
     }

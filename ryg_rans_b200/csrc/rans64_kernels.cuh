@@ -7,8 +7,9 @@
 //
 // Same mapping as the other coders (one warp = one chunk = one 32-way stream, one ballot per step
 // because a lane moves at most one u32 per step).  This is the "lets the GPU decode streams made by
-// the reference's fastest CPU encoder" row of SURVEY 8(f); it reuses the word coder's stream window,
-// symbol stage, output ring and flush, and is not tuned beyond that.
+// the reference's fastest CPU encoder" row of SURVEY 8(f); it reuses the word coder's stream window and
+// the chunk encoder every coder shares (encode_stream.cuh: symbol stage, output ring, flush), and is not
+// tuned beyond that.  Its encoder is split-only: per-chunk slots, then the tile scan and compaction.
 #pragma once
 #include "device_utils.cuh"
 #include "tables.h"
@@ -103,43 +104,46 @@ rans64_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const
     if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(status, kStatStream);
 }
 
-struct Rans64EncState {
-    uint64_t x;
-    uint32_t wpos;     // un-wrapped ring position of the next u32 = 508 - 4 * words_emitted
-    uint32_t flags;
-};
+// The rans64 coder for encode_stream (encode_stream.cuh); wpos is the ring position of the next u32 =
+// 508 - 4 * words_emitted.  step = Rans64EncPutSymbol for 32 lanes (rans64.h:262-278).  tab_lane = this lane's replica
+// of the 256-entry table {rcp_lo, rcp_hi, bias, cmpl_freq | rcp_shift << 20 | bad << 31}: one 16-byte Rans64EncSymbol
+// image per symbol (freq is M - cmpl_freq), replicated 8x so that the 8 lanes of a quarter-warp hit 8 different 16-byte
+// bank groups -- ONE conflict-free LDS.128 per step.  (Round 1 read the 32-byte image with two LDS.128 from an
+// unreplicated table: ~28 wavefronts per step, shared-memory data pipe 99 % busy, 3.8 ms per GiB.)
+struct Rans64Encoder {
+    using X = uint64_t;
+    static constexpr uint32_t kUnit = 4, kMaxEmit = 4, kBadBit = kEncBadSymbol;
+    static constexpr X kInit = kRans64L;               // Rans64EncInit, rans64.h:65-68
+    uint32_t tab;                                      // shared address of the 8x replicated uint4 table
+    uint32_t sb;
 
-// Rans64EncPutSymbol for 32 lanes (rans64.h:262-278).  tab_lane = this lane's replica of the 256-entry table
-// {rcp_lo, rcp_hi, bias, cmpl_freq | rcp_shift << 20 | bad << 31}: one 16-byte Rans64EncSymbol image per symbol (freq
-// is M - cmpl_freq), replicated 8x so that the 8 lanes of a quarter-warp hit 8 different 16-byte bank groups -- ONE
-// conflict-free LDS.128 per step.  (Round 1 read the 32-byte image with two LDS.128 from an unreplicated table: ~28
-// wavefronts per step, shared-memory data pipe 99 % busy, 3.8 ms per GiB.)
-__device__ __forceinline__ void rans64_enc_step(Rans64EncState& st, uint32_t sym, uint32_t tab_lane, uint32_t ring, uint32_t gt, uint32_t sb,
-                                                bool active)
-{
-    bool need = false;
-    uint4 e = make_uint4(0, 0, 0, 0);
-    if (active) {
-        e = lds_u128_ro(tab_lane + sym * (kEncReplicas * 16));
-        st.flags |= e.w;
-        const uint32_t freq = (1u << sb) - (e.w & 0xfffffu);
-        const uint64_t x_max = static_cast<uint64_t>(freq) << (63 - sb);               // ((L >> sb) << 32) * freq, :269
-        need = st.x >= x_max;
+    template <bool FULL>
+    __device__ __forceinline__ void step(EncState<X>& st, uint32_t sym, uint32_t tab_lane, uint32_t ring, uint32_t gt, bool active) const
+    {
+        bool need = false;
+        uint4 e = make_uint4(0, 0, 0, 0);
+        if (active) {
+            e = lds_u128_ro(tab_lane + sym * (kEncReplicas * 16));
+            st.flags |= e.w;
+            const uint32_t freq = (1u << sb) - (e.w & 0xfffffu);
+            const uint64_t x_max = static_cast<uint64_t>(freq) << (63 - sb);               // ((L >> sb) << 32) * freq, :269
+            need = st.x >= x_max;
+        }
+        const uint32_t mask = __ballot_sync(0xffffffffu, need);
+        if (need) {
+            asm volatile("st.shared.u32 [%0], %1;" ::"r"(ring | ((st.wpos - 4u * __popc(mask & gt)) & (kEncRingBytes - 1))),
+                         "r"(static_cast<uint32_t>(st.x))
+                         : "memory");                                                      // :271-272
+            st.x >>= 32;                                                                   // :273
+        }
+        st.wpos -= 4u * __popc(mask);
+        if (active) {
+            const uint64_t rcp = static_cast<uint64_t>(e.x) | (static_cast<uint64_t>(e.y) << 32);
+            const uint64_t q = __umul64hi(st.x, rcp) >> ((e.w >> 20) & 63u);               // :276
+            st.x = st.x + e.z + q * (e.w & 0xfffffu);                                      // :277
+        }
     }
-    const uint32_t mask = __ballot_sync(0xffffffffu, need);
-    if (need) {
-        asm volatile("st.shared.u32 [%0], %1;" ::"r"(ring | ((st.wpos - 4u * __popc(mask & gt)) & (kEncRingBytes - 1))),
-                     "r"(static_cast<uint32_t>(st.x))
-                     : "memory");                                                      // :271-272
-        st.x >>= 32;                                                                   // :273
-    }
-    st.wpos -= 4u * __popc(mask);
-    if (active) {
-        const uint64_t rcp = static_cast<uint64_t>(e.x) | (static_cast<uint64_t>(e.y) << 32);
-        const uint64_t q = __umul64hi(st.x, rcp) >> ((e.w >> 20) & 63u);               // :276
-        st.x = st.x + e.z + q * (e.w & 0xfffffu);                                      // :277
-    }
-}
+};
 
 __global__ void __launch_bounds__(kRans64Warps * 32, 2)
 rans64_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb,
@@ -154,79 +158,14 @@ rans64_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_
     }
     __syncthreads();
 
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t warp = threadIdx.x >> 5;
     const uint32_t chunk = blockIdx.x * kRans64Warps + warp;
     if (chunk >= n_chunks) return;
     const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
     const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-    const uint8_t* chunk_in = in + first;
-    const uint32_t wsm = smem_addr(s_r64e) + warp * kEncWarpSmem;
-    const uint32_t stage = wsm, ring = wsm + kEncStageBytes, tab = smem_addr(s_tab) + (lane & (kEncReplicas - 1)) * 16;
-    uint8_t* slot_end = scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes;
-    const uint32_t gt = lanemask_gt();
-
-    Rans64EncState st;
-    st.x = kRans64L;                            // Rans64EncInit, rans64.h:65-68
-    st.wpos = kEncRingBytes - 4;
-    st.flags = 0;
-    uint32_t flushed = 0;
-    const uint32_t steps = m >> 5, rem = m & 31;
-    const uint32_t nblk = steps >> 4;
-    const bool vec_ok = (reinterpret_cast<uintptr_t>(chunk_in) & 15) == 0;
-
-    uint4 parked = make_uint4(0, 0, 0, 0);
-    if (nblk && vec_ok) parked = ldg_stream_u128(reinterpret_cast<const uint4*>(chunk_in + (nblk - 1) * kEncStageBytes) + lane);
-    if (rem) {
-        const bool active = lane < rem;
-        const uint32_t s = active ? chunk_in[static_cast<uint64_t>(steps) * 32 + lane] : 0;
-        rans64_enc_step(st, s, tab, ring, gt, sb, active);
-    }
-    for (uint32_t g = steps; g > nblk * 16; g--) {
-        const uint32_t s = chunk_in[static_cast<uint64_t>(g - 1) * 32 + lane];
-        rans64_enc_step(st, s, tab, ring, gt, sb, true);
-        if (((g - 1) & 1) == 0) word_enc_flush(kEncRingBytes - 4 - st.wpos, flushed, ring, slot_end, lane);
-    }
-    word_enc_flush(kEncRingBytes - 4 - st.wpos, flushed, ring, slot_end, lane);
-
-    for (uint32_t b = nblk; b-- > 0;) {
-        __syncwarp();
-        if (vec_ok) {
-            sts_u128(stage + lane * 16, parked);
-            if (b) parked = ldg_stream_u128(reinterpret_cast<const uint4*>(chunk_in + (b - 1) * kEncStageBytes) + lane);
-        } else {
-            const uint8_t* p = chunk_in + b * kEncStageBytes + lane;
-#pragma unroll
-            for (int j = 0; j < 16; j++) sts_u8(stage + j * 32 + lane, p[j * 32]);
-        }
-        __syncwarp();
-#pragma unroll
-        for (int pr = 7; pr >= 0; pr--) {                    // <= 128 bytes per step: look at the ring every 2 steps
-            rans64_enc_step(st, lds_u8(stage + (pr * 2 + 1) * 32 + lane), tab, ring, gt, sb, true);
-            rans64_enc_step(st, lds_u8(stage + (pr * 2) * 32 + lane), tab, ring, gt, sb, true);
-            if (kEncRingBytes - 4 - st.wpos - flushed >= 256) word_enc_flush(kEncRingBytes - 4 - st.wpos, flushed, ring, slot_end, lane);
-        }
-    }
-
-    // Rans64EncFlush for lanes 31..0 (rans64.h:96-103): 256 bytes, in two halves so the 512-byte ring never overflows
-    word_enc_flush(kEncRingBytes - 4 - st.wpos, flushed, ring, slot_end, lane);         // < 16 bytes stay pending
-#pragma unroll
-    for (int half = 1; half >= 0; half--) {
-        if ((lane >> 4) == static_cast<uint32_t>(half)) {
-            const uint32_t hpos = st.wpos - 8u * (15 - (lane & 15));
-            asm volatile("st.shared.u32 [%0], %1;" ::"r"(ring | (hpos & (kEncRingBytes - 1))), "r"(static_cast<uint32_t>(st.x >> 32)) : "memory");
-            asm volatile("st.shared.u32 [%0], %1;" ::"r"(ring | ((hpos - 4) & (kEncRingBytes - 1))), "r"(static_cast<uint32_t>(st.x)) : "memory");
-        }
-        st.wpos -= 128;
-        word_enc_flush(kEncRingBytes - 4 - st.wpos, flushed, ring, slot_end, lane);
-    }
-    const uint32_t produced = kEncRingBytes - 4 - st.wpos;
-    const uint32_t left = produced - flushed;                  // < 16 bytes, multiple of 4: head of the stream
-    if (4 * lane < left) {
-        const uint32_t off = flushed + 4 * lane + 4;
-        *reinterpret_cast<uint32_t*>(slot_end - off) = lds_u32(ring | ((0u - off) & (kEncRingBytes - 1)));
-    }
-    if (lane == 0) sizes[chunk] = produced;
-    if (__any_sync(0xffffffffu, (st.flags & kEncBadSymbol) != 0) && lane == 0) atomicOr(status, kStatSymbol);
+    const uint32_t produced = encode_stream(in + first, m, Rans64Encoder{smem_addr(s_tab), sb},
+                                            smem_addr(s_r64e) + warp * kEncWarpSmem, scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, status);
+    if ((threadIdx.x & 31) == 0) sizes[chunk] = produced;
 }
 
 inline void configure_rans64_kernels()

@@ -10,6 +10,7 @@
 //                                                     exact division by reciprocal multiply
 #pragma once
 #include "device_utils.cuh"
+#include "encode_stream.cuh"
 #include "placement.cuh"
 #include "tables.h"
 
@@ -204,12 +205,7 @@ word_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const u
 
 // ---------------------------------------------------------------------------
 // K2: 32-way word-coder encode into per-chunk worst-case slots of a scratch buffer
-//
-// Per warp: 512 B input stage (16 steps of symbols, filled by one coalesced 128-bit load
-// per lane issued a block ahead) and a 512 B output ring (emitted words are placed with
-// ballot/popc compaction, flushed to HBM as whole 16-byte vectors).  The per-symbol
-// parameters come from ONE conflict-free LDS.128: the 256-entry table is replicated 8x so
-// that the 8 lanes of a quarter-warp always hit different 16-byte bank groups.
+// (stage, ring and flush: encode_stream.cuh; the word coder's step: WordEncoder below)
 // ---------------------------------------------------------------------------
 // build-time switches of the encoders (A/B runs: nvcc -DNAME=value into a second .so, loaded with RB200_LIB)
 // The fused word encoder's scratch is live data: (resident warps) x (slots per warp) x (one chunk's stream, 8.3 KB at
@@ -228,21 +224,13 @@ constexpr uint32_t kFusedSlots = RB200_FUSED_SLOTS;
 #ifndef RB200_FUSED_MINBLOCKS
 #define RB200_FUSED_MINBLOCKS 2        // CTAs per SM of the fused word encoder (its grid is SMs x this)
 #endif
-#ifndef RB200_ENC_UNIFORM_FLUSH
-#define RB200_ENC_UNIFORM_FLUSH 1      // vote on the (warp-uniform) flush test so that ptxas emits a uniform branch
-#endif
 #ifndef RB200_ENC_KEEP_HINT
-#define RB200_ENC_KEEP_HINT true       // evict_last hint on the fused encoder's scratch stores (see word_enc_flush)
+#define RB200_ENC_KEEP_HINT true       // evict_last hint on the fused encoder's scratch stores (see enc_flush)
 #endif
 #ifndef RB200_ENC_ASM_RENORM
 #define RB200_ENC_ASM_RENORM 1
 #endif
 constexpr int kEncWarps = 16;
-constexpr uint32_t kEncReplicas = 8;
-constexpr uint32_t kEncStageBytes = 512;     // 16 steps x 32 symbols
-constexpr uint32_t kEncRingBytes = 512;
-constexpr uint32_t kEncTableBytes = 256 * kEncReplicas * 16;                 // 32 KiB
-constexpr uint32_t kEncWarpSmem = kEncStageBytes + kEncRingBytes;            // 1 KiB per warp
 
 // {magic, x_max | shift, start, 4096 - freq}
 //   x_max = freq << 20 in 32-bit arithmetic (rans_word_sse41.h:85; wraps to 0 for freq 4096, as the
@@ -265,173 +253,75 @@ __device__ __forceinline__ uint32_t funnel_shr_wrap(uint32_t lo, uint32_t hi, ui
     return r;
 }
 
-struct WordEncState {
-    uint32_t x;        // rANS state
-    uint32_t wpos;     // ring byte position (relative to slot end, un-wrapped) of the next word = 510 - 2 * words_emitted
-    uint32_t flags;    // OR of the table's (4096 - freq) words: bit 12 set <=> a symbol with freq 0 was met
-};
+// The word coder for encode_stream (encode_stream.cuh).  step = RansWordEncPut for 32 lanes (rans_word_sse41.h:81-93);
+// wpos is the ring position of the next word = 510 - 2 * words_emitted; flags bit 12 set <=> a symbol with freq 0.
+template <bool R32>
+struct WordEncoder {
+    using X = uint32_t;
+    static constexpr uint32_t kUnit = 2, kMaxEmit = 2, kBadBit = kWordSlots;
+    static constexpr X kInit = kWordL;                 // RansWordEncInit, rans_word_sse41.h:75-78
+    uint32_t tab;                                      // shared address of the 8x replicated uint4 table
 
-// RansWordEncPut for 32 lanes (rans_word_sse41.h:81-93)
-// FULL: all 32 lanes take part (the caller passes active == true); the ragged first step of a chunk is the only
-// one that does not.
-template <bool R32, bool FULL>
-__device__ __forceinline__ void word_enc_step(WordEncState& st, uint32_t sym, uint32_t tab_lane, uint32_t ring, uint32_t gt, bool active)
-{
-    bool need = false;
-    uint4 e = make_uint4(0, 0, 0, 0);
-    if (active) {
-        e = lds_u128_ro(tab_lane + sym * (kEncReplicas * 16));
-        st.flags |= e.w;
-        need = (st.x | 31u) >= e.y;                                   // x >= ((L >> 12) << 16) * freq, :85
-    }
-#if RB200_ENC_ASM_RENORM
-    // the same renormalisation as below with ONE predicate feeding the vote, the store and the shift (the
-    // compiler otherwise evaluates the comparison twice and copies x before shifting it)
-    if (FULL) {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            ".reg .b32 m, r, a;\n\t"
-            "setp.ge.u32 p, %2, %3;\n\t"
-            "vote.sync.ballot.b32 m, p, 0xffffffff;\n\t"
-            "and.b32 r, m, %4;\n\t"
-            "popc.b32 r, r;\n\t"
-            "shl.b32 r, r, 1;\n\t"
-            "sub.u32 a, %1, r;\n\t"
-            "and.b32 a, a, %5;\n\t"
-            "or.b32 a, a, %6;\n\t"
-            "@p st.shared.u16 [a], %0;\n\t"
-            "@p shr.u32 %0, %0, 16;\n\t"
-            "popc.b32 m, m;\n\t"
-            "shl.b32 m, m, 1;\n\t"
-            "sub.u32 %1, %1, m;\n\t"
-            "}"
-            : "+r"(st.x), "+r"(st.wpos)
-            : "r"(st.x | 31u), "r"(e.y), "r"(gt), "n"(kEncRingBytes - 1), "r"(ring)
-            : "memory");
-    } else
-#endif
+    template <bool FULL>
+    __device__ __forceinline__ void step(EncState<X>& st, uint32_t sym, uint32_t tab_lane, uint32_t ring, uint32_t gt, bool active) const
     {
-    const uint32_t mask = __ballot_sync(0xffffffffu, need);
-    if (need) {
-        sts_u16(ring | ((st.wpos - 2u * __popc(mask & gt)) & (kEncRingBytes - 1)), st.x);   // :86-87, lanes 31..0 downwards
-        st.x >>= 16;                                                                        // :88
-    }
-    st.wpos -= 2u * __popc(mask);
-    }
-    if (active) {
-        uint32_t q;
-        if (R32) {
-            // x < freq << 20 here, where the 32-bit reciprocal is exact: q = mulhi(x, M32) >> shift
-            q = funnel_shr_wrap(__umulhi(st.x, e.x), 0u, e.y);
-        } else {
-            // q = x / freq exactly for any x: M = 2^32 + magic = ceil(2^(32+shift) / freq), q = (x + mulhi(x, magic)) >> shift
-            const uint32_t hi = __umulhi(st.x, e.x);
-            const uint32_t lo = st.x + hi;
-            q = funnel_shr_wrap(lo, lo < hi ? 1u : 0u, e.y);
+        bool need = false;
+        uint4 e = make_uint4(0, 0, 0, 0);
+        if (active) {
+            e = lds_u128_ro(tab_lane + sym * (kEncReplicas * 16));
+            st.flags |= e.w;
+            need = (st.x | 31u) >= e.y;                                   // x >= ((L >> 12) << 16) * freq, :85
         }
-        st.x = st.x + e.z + q * e.w;                       // ((x / freq) << 12) + x % freq + start, :92
-    }
-}
-
-// flush every complete 16-byte vector of the ring; *flushed = bytes already written below slot_end.
-// KEEP: the destination is a scratch slot that is read back soon (fused paths): ask the L2 to hold on to it.
-template <bool KEEP = false>
-__device__ __forceinline__ void word_enc_flush(uint32_t produced, uint32_t& flushed, uint32_t ring, uint8_t* slot_end, uint32_t lane)
-{
-    const uint32_t nvec = (produced - flushed) >> 4;
-    __syncwarp();
-    if (lane < nvec) {
-        const uint32_t v = (flushed >> 4) + lane + 1;                 // vector v ends 16 * (v - 1) bytes below slot_end
-        const uint4 q = lds_u128(ring + ((0u - 16u * v) & (kEncRingBytes - 1)));
-        if (KEEP) stg_hint_u128(reinterpret_cast<uint4*>(slot_end - 16ull * v), q, l2_policy_keep());
-        else stg_stream_u128(reinterpret_cast<uint4*>(slot_end - 16ull * v), q);
-    }
-    flushed += nvec << 4;
-    __syncwarp();
-}
-
-// Encode m symbols (one warp) as one 32-way stream that ENDS at slot_end (16-byte aligned) and grows
-// downwards; returns the stream size in bytes (warp-uniform).
-//   tab  = shared address of the 8x replicated uint4 table
-//   wsm  = shared address of this warp's 1 KiB (stage, then ring; 512-byte aligned)
-//   KEEP = the slot is scratch that is read back soon (see word_enc_flush)
-template <bool R32, bool KEEP = false>
-__device__ __forceinline__ uint32_t word_encode_stream(const uint8_t* __restrict__ chunk_in, uint32_t m, uint32_t tab, uint32_t wsm,
-                                                       uint8_t* __restrict__ slot_end, uint32_t* __restrict__ status)
-{
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t stage = wsm, ring = wsm + kEncStageBytes;
-    const uint32_t tab_lane = tab + (lane & (kEncReplicas - 1)) * 16;
-    const uint32_t gt = lanemask_gt();
-
-    WordEncState st;
-    st.x = kWordL;                              // RansWordEncInit, rans_word_sse41.h:75-78
-    st.wpos = kEncRingBytes - 2;
-    st.flags = 0;
-    uint32_t flushed = 0;
-    const uint32_t steps = m >> 5, rem = m & 31;
-    const uint32_t nblk = steps >> 4;           // full 16-step blocks, staged; the rest is read directly
-    const bool vec_ok = (reinterpret_cast<uintptr_t>(chunk_in) & 15) == 0;
-
-    // symbols are walked last to first (main_simd.cpp:294): ragged tail first
-    uint4 parked = make_uint4(0, 0, 0, 0);
-    if (nblk && vec_ok) parked = ldg_stream_u128(reinterpret_cast<const uint4*>(chunk_in + (nblk - 1) * kEncStageBytes) + lane);
-    if (rem) {
-        const bool active = lane < rem;
-        const uint32_t s = active ? chunk_in[static_cast<uint64_t>(steps) * 32 + lane] : 0;
-        word_enc_step<R32, false>(st, s, tab_lane, ring, gt, active);
-    }
-    for (uint32_t g = steps; g > nblk * 16; g--) {
-        const uint32_t s = chunk_in[static_cast<uint64_t>(g - 1) * 32 + lane];
-        word_enc_step<R32, true>(st, s, tab_lane, ring, gt, true);
-        if (((g - 1) & 3) == 0) word_enc_flush<KEEP>(kEncRingBytes - 2 - st.wpos, flushed, ring, slot_end, lane);
-    }
-    word_enc_flush<KEEP>(kEncRingBytes - 2 - st.wpos, flushed, ring, slot_end, lane);
-
-    for (uint32_t b = nblk; b-- > 0;) {
-        __syncwarp();
-        if (vec_ok) {
-            sts_u128(stage + lane * 16, parked);
-            if (b) parked = ldg_stream_u128(reinterpret_cast<const uint4*>(chunk_in + (b - 1) * kEncStageBytes) + lane);
-        } else {                                 // unaligned input: byte loads into the stage
-            const uint8_t* p = chunk_in + b * kEncStageBytes + lane;
-#pragma unroll
-            for (int j = 0; j < 16; j++) sts_u8(stage + j * 32 + lane, p[j * 32]);
-        }
-        __syncwarp();
-#pragma unroll
-        for (int grp = 3; grp >= 0; grp--) {
-#pragma unroll
-            for (int j = 3; j >= 0; j--)
-                word_enc_step<R32, true>(st, lds_u8(stage + (grp * 4 + j) * 32 + lane), tab_lane, ring, gt, true);
-            // <= 256 bytes per 4 steps; flushing whenever >= 256 are pending keeps the 512-byte ring safe.  The test is
-            // warp-uniform; voting on it tells ptxas so (a uniform branch: no convergence check before the next ballot)
-#if RB200_ENC_UNIFORM_FLUSH
-            if (__any_sync(0xffffffffu, kEncRingBytes - 2 - st.wpos - flushed >= 256))
-#else
-            if (kEncRingBytes - 2 - st.wpos - flushed >= 256)
+#if RB200_ENC_ASM_RENORM
+        // the same renormalisation as below with ONE predicate feeding the vote, the store and the shift (the
+        // compiler otherwise evaluates the comparison twice and copies x before shifting it)
+        if (FULL) {
+            asm volatile(
+                "{\n\t"
+                ".reg .pred p;\n\t"
+                ".reg .b32 m, r, a;\n\t"
+                "setp.ge.u32 p, %2, %3;\n\t"
+                "vote.sync.ballot.b32 m, p, 0xffffffff;\n\t"
+                "and.b32 r, m, %4;\n\t"
+                "popc.b32 r, r;\n\t"
+                "shl.b32 r, r, 1;\n\t"
+                "sub.u32 a, %1, r;\n\t"
+                "and.b32 a, a, %5;\n\t"
+                "or.b32 a, a, %6;\n\t"
+                "@p st.shared.u16 [a], %0;\n\t"
+                "@p shr.u32 %0, %0, 16;\n\t"
+                "popc.b32 m, m;\n\t"
+                "shl.b32 m, m, 1;\n\t"
+                "sub.u32 %1, %1, m;\n\t"
+                "}"
+                : "+r"(st.x), "+r"(st.wpos)
+                : "r"(st.x | 31u), "r"(e.y), "r"(gt), "n"(kEncRingBytes - 1), "r"(ring)
+                : "memory");
+        } else
 #endif
-                word_enc_flush<KEEP>(kEncRingBytes - 2 - st.wpos, flushed, ring, slot_end, lane);
+        {
+        const uint32_t mask = __ballot_sync(0xffffffffu, need);
+        if (need) {
+            sts_u16(ring | ((st.wpos - 2u * __popc(mask & gt)) & (kEncRingBytes - 1)), st.x);   // :86-87, lanes 31..0 downwards
+            st.x >>= 16;                                                                        // :88
+        }
+        st.wpos -= 2u * __popc(mask);
+        }
+        if (active) {
+            uint32_t q;
+            if (R32) {
+                // x < freq << 20 here, where the 32-bit reciprocal is exact: q = mulhi(x, M32) >> shift
+                q = funnel_shr_wrap(__umulhi(st.x, e.x), 0u, e.y);
+            } else {
+                // q = x / freq exactly for any x: M = 2^32 + magic = ceil(2^(32+shift) / freq), q = (x + mulhi(x, magic)) >> shift
+                const uint32_t hi = __umulhi(st.x, e.x);
+                const uint32_t lo = st.x + hi;
+                q = funnel_shr_wrap(lo, lo < hi ? 1u : 0u, e.y);
+            }
+            st.x = st.x + e.z + q * e.w;                       // ((x / freq) << 12) + x % freq + start, :92
         }
     }
-
-    // RansWordEncFlush for lanes 31..0 (main_simd.cpp:298-299): lane 31's hi word first (highest), lane 0's lo word last
-    word_enc_flush<KEEP>(kEncRingBytes - 2 - st.wpos, flushed, ring, slot_end, lane);     // < 16 bytes stay pending
-    const uint32_t hpos = st.wpos - 4u * (31 - lane);
-    sts_u16(ring | (hpos & (kEncRingBytes - 1)), st.x >> 16);
-    sts_u16(ring | ((hpos - 2) & (kEncRingBytes - 1)), st.x);
-    st.wpos -= kHeaderBytes;
-    const uint32_t produced = kEncRingBytes - 2 - st.wpos;           // total stream bytes
-    word_enc_flush<KEEP>(produced, flushed, ring, slot_end, lane);
-    const uint32_t left = produced - flushed;                        // < 16, even: head of the stream, not vector aligned
-    if (2 * lane < left) {
-        const uint32_t off = flushed + 2 * lane + 2;                 // bytes below slot_end
-        *reinterpret_cast<uint16_t*>(slot_end - off) = static_cast<uint16_t>(lds_u16(ring | ((0u - off) & (kEncRingBytes - 1))));
-    }
-    if (__any_sync(0xffffffffu, (st.flags & kWordSlots) != 0) && lane == 0) atomicOr(status, kStatSymbol);
-    return produced;
-}
+};
 
 // chunk `chunk` into the end of its own worst-case slot of `scratch`; size to sizes[chunk]
 template <bool R32>
@@ -439,7 +329,7 @@ __device__ __forceinline__ void word_encode_chunk(const uint8_t* __restrict__ ch
                                                   uint32_t tab, uint32_t wsm, uint8_t* __restrict__ scratch,
                                                   uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
 {
-    const uint32_t produced = word_encode_stream<R32>(chunk_in, m, tab, wsm, scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, status);
+    const uint32_t produced = encode_stream(chunk_in, m, WordEncoder<R32>{tab}, wsm, scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, status);
     if ((threadIdx.x & 31) == 0) sizes[chunk] = produced;
 }
 
@@ -499,7 +389,7 @@ word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t ch
         if (chunk >= n_chunks) break;
         const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
         const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-        const uint32_t produced = word_encode_stream<R32, RB200_ENC_KEEP_HINT>(in + first, m, tab, wsm, q.next_end(), status);
+        const uint32_t produced = encode_stream<RB200_ENC_KEEP_HINT>(in + first, m, WordEncoder<R32>{tab}, wsm, q.next_end(), status);
         q.finish(out, chunk, produced, lane);
     }
     q.drain(out, lane);

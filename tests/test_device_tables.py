@@ -21,7 +21,7 @@ HARNESS = r'''
 #include <random>
 using namespace rb200;
 
-// the kernels' arithmetic (word_kernels.cuh: word_enc_expand / word_enc_step)
+// the kernels' arithmetic (word_kernels.cuh: word_enc_expand / WordEncoder::step)
 static uint32_t mulhi(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) >> 32); }
 static uint32_t q33(uint32_t x, WordEncEntry e)
 {

@@ -136,6 +136,33 @@ def test_word_zero_freq_symbol_is_reported(gpu_ctx, oracle_lib, gen):
     assert ei.value.code == -7
 
 
+@pytest.mark.parametrize("coder,sb", [(WORD, 12), (BYTE, 14), (ALIAS, 16), (RANS64, 14)])
+@pytest.mark.parametrize("chunk", [1000, 5000])       # split path; fused path (word, byte, alias)
+@pytest.mark.parametrize("where", ["ragged", "unstaged", "staged"])
+def test_zero_freq_symbol_is_reported_by_every_coder(gpu_ctx, oracle_lib, gen, coder, sb, chunk, where):
+    """A symbol the model gives frequency 0 fails the encode with RB200_E_SYMBOL wherever the chunk encoder meets it:
+    in the ragged first step (the last chunk % 32 symbols), in a step read directly (the steps above the staged
+    16-step blocks) or in a staged block.  1000 = 31 steps + 8: one staged block, 15 direct steps; 5000 = 156 steps + 8:
+    nine staged blocks, 12 direct steps.  The symbol sits in the second chunk, which is not 16-byte aligned, so its
+    blocks are staged with byte loads; test_word_zero_freq_symbol_is_reported meets it in an aligned, vector-staged
+    block."""
+    import ryg_rans_b200 as rb
+    data = gen("text", 3 * chunk, 2)
+    freqs, cum = _model(oracle_lib, data, sb)
+    model = gpu_ctx.model(coder, sb, freqs)
+    steps = chunk // 32
+    local = {"ragged": chunk - 3, "unstaged": (steps // 16 * 16 + 1) * 32 + 5, "staged": 100}[where]
+    other = data.copy()
+    other[chunk + local] = int(np.flatnonzero(freqs == 0)[0])
+    with pytest.raises(rb.RansError) as ei:
+        gpu_ctx.encode_host(model, other, chunk)
+    assert ei.value.code == -7
+    blob, offs = gpu_ctx.encode_host(model, data, chunk)
+    oblob, ooffs = oracle_lib.chunked_encode(coder, data, freqs, cum, chunk, nlanes=32, scale_bits=sb)
+    assert np.array_equal(offs, ooffs) and np.array_equal(blob, oblob)
+    model.close()
+
+
 def test_encode_bound_is_tight_enough(gpu_ctx, oracle_lib, gen):
     data = gen("uniform", 70000, 9)
     freqs, cum = _model(oracle_lib, data, 12)
