@@ -225,6 +225,40 @@ int rb200_container_pack(int coder, uint32_t scale_bits, uint32_t chunk_syms, si
                          uint8_t* out, size_t out_cap, size_t* out_size);
 int rb200_container_open(const uint8_t* buf, size_t size, rb200_container_info* info);
 
+/* ---------------------------------------------------------------- wire format on the GPU */
+
+/* zlib's crc32 (IEEE, reflected, init and xor-out ~0; the container's checksum) of n bytes of a host or device
+ * buffer, computed on the GPU.  Any n and any alignment.  crc_in chains like zlib: crc(a || b) =
+ * rb200_crc32(b, rb200_crc32(a, 0)); pass 0 to start.  HOST mode stages the buffer through the context.  *crc_out is
+ * written to host memory; the call synchronises. */
+int rb200_crc32(rb200_ctx* ctx, const uint8_t* data, size_t n, uint32_t crc_in, uint32_t* crc_out, int mem_kind);
+
+/* rb200_encode + rb200_container_pack in one call: the directory and the blob are encoded straight into their place
+ * in `out`, and the bytes equal what rb200_container_pack writes for the same model, input, chunk_syms and flags.
+ * The model section is the model's own frequencies.  out_cap must hold rb200_container_size(n_chunks, blob size);
+ * rb200_container_size(rb200_chunk_count(n, chunk_syms), rb200_encode_bound(n, chunk_syms)) always does.
+ * flags: RB200_CONTAINER_CRC_BLOB adds the blob CRC, taken on the GPU.
+ * HOST mode: synchronous; out 8-byte aligned; *out_size (may be NULL) receives the container's size.
+ * DEVICE mode: out 16-byte aligned; work is only enqueued on the context stream (encode, CRCs, a header kernel) and
+ * out_size is not written: the size is rb200_container_size(n_chunks, blob_bytes) with blob_bytes from the header.
+ * A blob that does not fit out_cap is RB200_E_SPACE, from the call (HOST) or from rb200_sync (DEVICE, as for
+ * rb200_encode; the header is then not written).  out_cap below the header, model and directory is RB200_E_SPACE
+ * from the call in both modes. */
+int rb200_container_encode(rb200_ctx* ctx, const rb200_model* model, const uint8_t* in, size_t n, uint32_t chunk_syms,
+                           uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind);
+
+/* rb200_container_open + rb200_model_create + rb200_decode in one call, on a container in host or device memory.
+ * The container is validated by the same rules as rb200_container_open (RB200_E_STREAM on any failure); *n_symbols
+ * (may be NULL) then receives its n, and out_cap < n returns RB200_E_SPACE before any decoding, so a caller can
+ * allocate and call again.  The call synchronises and returns one status for the whole call.
+ * HOST mode: buf and out 8-byte aligned.  The header, model and directory are checked before decoding; the blob CRC
+ * is taken slice by slice while decoding, so on a blob CRC mismatch (RB200_E_STREAM) out has been written and its
+ * contents are unspecified.
+ * DEVICE mode: buf and out 16-byte aligned.  Both CRCs are taken on the GPU before anything is decoded: a container
+ * that fails any check leaves out untouched. */
+int rb200_container_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                           uint64_t* n_symbols, int mem_kind);
+
 #ifdef __cplusplus
 }
 #endif

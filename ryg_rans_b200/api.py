@@ -56,6 +56,10 @@ EXPORTS = [
     ("rb200_container_pack", C.c_int, [C.c_int, C.c_uint32, C.c_uint32, C.c_size_t, _u32p, C.c_void_p, C.c_void_p, C.c_size_t,
                                        C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("rb200_container_open", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_crc32", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, _u32p, C.c_int]),
+    ("rb200_container_encode", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p,
+                                         C.c_size_t, C.POINTER(C.c_size_t), C.c_int]),
+    ("rb200_container_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
 ]
 CONTAINER_CRC_BLOB = 1
 
@@ -257,6 +261,57 @@ class Context:
         counts = np.zeros(256, np.uint64)
         self.lib.check(self.lib.dll.rb200_histogram(self.h, ptr, n, counts.ctypes.data_as(_u64p), MEM_DEVICE), self.h)
         return counts
+
+    # ---- CRC-32 and the container in host or device memory
+    def crc32(self, data, crc_in=0):
+        """zlib.crc32 of a host array, computed on the GPU."""
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        out = C.c_uint32(0)
+        self.lib.check(self.lib.dll.rb200_crc32(self.h, _np_ptr(data), data.size, crc_in, C.byref(out), MEM_HOST), self.h)
+        return out.value
+
+    def crc32_device(self, ptr, n, crc_in=0):
+        out = C.c_uint32(0)
+        self.lib.check(self.lib.dll.rb200_crc32(self.h, ptr, n, crc_in, C.byref(out), MEM_DEVICE), self.h)
+        return out.value
+
+    def container_capacity(self, n, chunk_syms):
+        """bytes that always hold rb200_container_encode's output for n symbols"""
+        return int(self.lib.dll.rb200_container_size(self.chunk_count(n, chunk_syms), self.encode_bound(n, chunk_syms)))
+
+    def container_encode_host(self, model, data, chunk_syms, flags=0, out_cap=None):
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        cap = self.container_capacity(data.size, chunk_syms) if out_cap is None else out_cap
+        out = np.zeros(max(cap, 16), np.uint8)
+        size = C.c_size_t(0)
+        self.lib.check(self.lib.dll.rb200_container_encode(self.h, model.h, _np_ptr(data), data.size, chunk_syms, flags, _np_ptr(out),
+                                                           cap, C.byref(size), MEM_HOST), self.h)
+        return out[:size.value].copy()
+
+    def container_encode_device(self, model, in_ptr, n, chunk_syms, flags, out_ptr, out_cap):
+        """asynchronous; errors come from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_encode(self.h, model.h, in_ptr, n, chunk_syms, flags, out_ptr, out_cap, None,
+                                                           MEM_DEVICE), self.h)
+
+    def container_decode_host(self, buf, out_cap=None):
+        """returns the decoded symbols; out_cap defaults to the container's n"""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        n = C.c_uint64(0)
+        if out_cap is None:
+            rc = self.lib.dll.rb200_container_decode(self.h, _np_ptr(buf), buf.size, None, 0, C.byref(n), MEM_HOST)
+            if rc not in (0, -3):
+                self.lib.check(rc, self.h)
+            out_cap = n.value
+        out = np.zeros(max(out_cap, 1), np.uint8)
+        self.lib.check(self.lib.dll.rb200_container_decode(self.h, _np_ptr(buf), buf.size, _np_ptr(out), out_cap, C.byref(n),
+                                                           MEM_HOST), self.h)
+        return out[:n.value]
+
+    def container_decode_device(self, buf_ptr, size, out_ptr, out_cap):
+        """synchronous; returns the container's n"""
+        n = C.c_uint64(0)
+        self.lib.check(self.lib.dll.rb200_container_decode(self.h, buf_ptr, size, out_ptr, out_cap, C.byref(n), MEM_DEVICE), self.h)
+        return n.value
 
     # ---- per-block models, device pointers (asynchronous)
     def blocks_build_models_device(self, in_ptr, n_blocks, block_size, freqs_ptr):

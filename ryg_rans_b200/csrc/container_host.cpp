@@ -6,34 +6,18 @@
 //
 //   [ 64-byte header ][ freqs: 256 x u32 ][ offsets: (n_chunks + 1) x u64 ][ pad to 16 ][ blob ]
 //
-// Host-only, no GPU work.  All integers little-endian.  CRC-32 (IEEE, reflected) over header
-// (with the crc fields zeroed) + freqs + offsets always; over the blob when RB200_CONTAINER_CRC_BLOB
-// is set (1 GiB takes ~1 s on one core, so it is optional).
-#include "rans_b200.h"
+// All integers little-endian.  CRC-32 (zlib's: IEEE, reflected) over header (with the crc fields zeroed) + freqs +
+// offsets always; over the blob when RB200_CONTAINER_CRC_BLOB is set.  rb200_container_pack / _open here work on host
+// buffers with a host CRC (slicing-by-8, ~1 GB/s on one core: the blob CRC is optional for that reason).
+// rb200_container_encode / _decode (rans_b200.cu) write and read the same bytes in host or device memory with the
+// blob CRC on the GPU (crc_kernels.cuh); they validate through the parser below, so both sides apply one set of rules.
+#include "container_format.h"
 
 #include <cstring>
 
+namespace rb200 {
+
 namespace {
-
-constexpr uint32_t kMagic = 0x43324252u;   // "RB2C"
-constexpr uint16_t kVersion = 1;
-
-struct Header {                 // 64 bytes
-    uint32_t magic;
-    uint16_t version;
-    uint8_t coder;
-    uint8_t scale_bits;
-    uint32_t lanes;
-    uint32_t chunk_syms;
-    uint64_t n_symbols;
-    uint64_t n_chunks;
-    uint64_t blob_bytes;
-    uint32_t flags;
-    uint32_t meta_crc;          // header (crc fields zero) + freqs + offsets
-    uint32_t blob_crc;          // valid when flags & RB200_CONTAINER_CRC_BLOB
-    uint32_t reserved[3];
-};
-static_assert(sizeof(Header) == 64, "container header must stay 64 bytes");
 
 struct CrcTable {
     uint32_t t[8][256];
@@ -49,7 +33,9 @@ struct CrcTable {
     }
 };
 
-uint32_t crc32_update(uint32_t crc, const void* data, size_t len)     // slicing-by-8
+}  // namespace
+
+uint32_t container_crc32(uint32_t crc, const void* data, size_t len)     // slicing-by-8
 {
     static const CrcTable table;                                      // built once, thread-safe (C++11 static)
     const uint32_t (*T)[256] = table.t;
@@ -69,21 +55,22 @@ uint32_t crc32_update(uint32_t crc, const void* data, size_t len)     // slicing
     return ~crc;
 }
 
-size_t pad16(size_t v) { return (v + 15) & ~static_cast<size_t>(15); }
-size_t blob_offset(uint64_t n_chunks) { return pad16(sizeof(Header) + 256 * sizeof(uint32_t) + (n_chunks + 1) * sizeof(uint64_t)); }
-
-uint32_t meta_crc(const Header& h, const uint32_t* freqs, const uint64_t* offsets)
+uint32_t container_header_crc(const ContainerHeader& h)
 {
-    Header z = h;
+    ContainerHeader z = h;
     z.meta_crc = 0;
     z.blob_crc = 0;
-    uint32_t c = crc32_update(0, &z, sizeof z);
-    c = crc32_update(c, freqs, 256 * sizeof(uint32_t));
-    return crc32_update(c, offsets, (h.n_chunks + 1) * sizeof(uint64_t));
+    return container_crc32(0, &z, sizeof z);
 }
 
-// what rb200_model_create would accept: a known coder, its scale_bits range, frequencies that sum to 1 << scale_bits
-bool model_fields_ok(uint32_t coder, uint32_t scale_bits, const uint32_t* freqs)
+uint32_t container_meta_crc(const ContainerHeader& h, const uint32_t* freqs, const uint64_t* offsets)
+{
+    uint32_t c = container_header_crc(h);
+    c = container_crc32(c, freqs, 256 * sizeof(uint32_t));
+    return container_crc32(c, offsets, (h.n_chunks + 1) * sizeof(uint64_t));
+}
+
+bool container_model_ok(uint32_t coder, uint32_t scale_bits, const uint32_t* freqs)
 {
     if (coder > RB200_CODER_RANS64 || scale_bits < 8 || scale_bits > 16) return false;
     if (coder == RB200_CODER_WORD && scale_bits != 12) return false;
@@ -92,23 +79,12 @@ bool model_fields_ok(uint32_t coder, uint32_t scale_bits, const uint32_t* freqs)
     return sum == (1ull << scale_bits);
 }
 
-}  // namespace
-
-extern "C" size_t rb200_container_size(size_t n_chunks, size_t blob_bytes) { return blob_offset(n_chunks) + blob_bytes; }
-
-extern "C" int rb200_container_pack(int coder, uint32_t scale_bits, uint32_t chunk_syms, size_t n, const uint32_t freqs[256],
-                                    const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes, uint32_t flags, uint8_t* out,
-                                    size_t out_cap, size_t* out_size)
+ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_syms, uint64_t n, uint64_t n_chunks,
+                                 uint64_t blob_bytes, uint32_t flags)
 {
-    if (!freqs || !offsets || (!blob && blob_bytes) || !out || !chunk_syms) return RB200_E_ARG;
-    if (coder < 0 || !model_fields_ok(static_cast<uint32_t>(coder), scale_bits, freqs)) return RB200_E_MODEL;   // never write what open rejects
-    const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
-    if (offsets[n_chunks] != blob_bytes || (blob_bytes & 15)) return RB200_E_ARG;
-    const size_t total = rb200_container_size(n_chunks, blob_bytes);
-    if (total > out_cap) return RB200_E_SPACE;
-    Header h{};
-    h.magic = kMagic;
-    h.version = kVersion;
+    ContainerHeader h{};
+    h.magic = kContainerMagic;
+    h.version = kContainerVersion;
     h.coder = static_cast<uint8_t>(coder);
     h.scale_bits = static_cast<uint8_t>(scale_bits);
     h.lanes = RB200_LANES;
@@ -117,8 +93,61 @@ extern "C" int rb200_container_pack(int coder, uint32_t scale_bits, uint32_t chu
     h.n_chunks = n_chunks;
     h.blob_bytes = blob_bytes;
     h.flags = flags & RB200_CONTAINER_CRC_BLOB;
-    h.meta_crc = meta_crc(h, freqs, offsets);
-    if (h.flags & RB200_CONTAINER_CRC_BLOB) h.blob_crc = crc32_update(0, blob, blob_bytes);
+    return h;
+}
+
+int container_parse_header(const uint8_t* hdr, size_t size, ContainerHeader* out)
+{
+    if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
+    ContainerHeader h;
+    std::memcpy(&h, hdr, sizeof h);
+    if (h.magic != kContainerMagic || h.version != kContainerVersion || h.lanes != RB200_LANES || !h.chunk_syms) return RB200_E_STREAM;
+    if (h.n_chunks != h.n_symbols / h.chunk_syms + (h.n_symbols % h.chunk_syms != 0) || h.n_chunks >= (1ull << 31) ||
+        (h.blob_bytes & 15) || h.coder > RB200_CODER_RANS64 || h.scale_bits < 8 || h.scale_bits > 16)
+        return RB200_E_STREAM;
+    const size_t boff = container_blob_offset(h.n_chunks);
+    if (boff > size || h.blob_bytes > size - boff) return RB200_E_STREAM;
+    *out = h;
+    return RB200_OK;
+}
+
+int container_check_prefix(const ContainerHeader& h, const uint8_t* prefix, uint32_t meta_crc)
+{
+    const uint32_t* freqs = reinterpret_cast<const uint32_t*>(prefix + sizeof(ContainerHeader));
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(prefix + kContainerDirOffset);
+    if (meta_crc != h.meta_crc) return RB200_E_STREAM;
+    if (!container_model_ok(h.coder, h.scale_bits, freqs)) return RB200_E_STREAM;        // CRC-valid but inconsistent
+    if (offsets[h.n_chunks] != h.blob_bytes) return RB200_E_STREAM;
+    if (h.n_chunks && offsets[0] >= 16) return RB200_E_STREAM;                           // the first stream starts inside the first vector
+    for (uint64_t c = 0; c < h.n_chunks; c++)
+        if (offsets[c] > offsets[c + 1]) return RB200_E_STREAM;
+    return RB200_OK;
+}
+
+int container_check_blob(const ContainerHeader& h, uint32_t blob_crc)
+{
+    return (h.flags & RB200_CONTAINER_CRC_BLOB) && blob_crc != h.blob_crc ? RB200_E_STREAM : RB200_OK;
+}
+
+}  // namespace rb200
+
+using namespace rb200;
+
+extern "C" size_t rb200_container_size(size_t n_chunks, size_t blob_bytes) { return container_blob_offset(n_chunks) + blob_bytes; }
+
+extern "C" int rb200_container_pack(int coder, uint32_t scale_bits, uint32_t chunk_syms, size_t n, const uint32_t freqs[256],
+                                    const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes, uint32_t flags, uint8_t* out,
+                                    size_t out_cap, size_t* out_size)
+{
+    if (!freqs || !offsets || (!blob && blob_bytes) || !out || !chunk_syms) return RB200_E_ARG;
+    if (coder < 0 || !container_model_ok(static_cast<uint32_t>(coder), scale_bits, freqs)) return RB200_E_MODEL;   // never write what open rejects
+    const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
+    if (offsets[n_chunks] != blob_bytes || (blob_bytes & 15)) return RB200_E_ARG;
+    const size_t total = rb200_container_size(n_chunks, blob_bytes);
+    if (total > out_cap) return RB200_E_SPACE;
+    ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n, n_chunks, blob_bytes, flags);
+    h.meta_crc = container_meta_crc(h, freqs, offsets);
+    if (h.flags & RB200_CONTAINER_CRC_BLOB) h.blob_crc = container_crc32(0, blob, blob_bytes);
     uint8_t* p = out;
     std::memcpy(p, &h, sizeof h);
     p += sizeof h;
@@ -126,7 +155,7 @@ extern "C" int rb200_container_pack(int coder, uint32_t scale_bits, uint32_t chu
     p += 256 * sizeof(uint32_t);
     std::memcpy(p, offsets, (n_chunks + 1) * sizeof(uint64_t));
     p += (n_chunks + 1) * sizeof(uint64_t);
-    const size_t boff = blob_offset(n_chunks);
+    const size_t boff = container_blob_offset(n_chunks);
     std::memset(p, 0, out + boff - p);
     if (blob_bytes) std::memcpy(out + boff, blob, blob_bytes);
     if (out_size) *out_size = total;
@@ -136,26 +165,18 @@ extern "C" int rb200_container_pack(int coder, uint32_t scale_bits, uint32_t chu
 extern "C" int rb200_container_open(const uint8_t* buf, size_t size, rb200_container_info* info)
 {
     if (!buf || !info) return RB200_E_ARG;
-    if (size < sizeof(Header)) return RB200_E_STREAM;
-    Header h;
-    std::memcpy(&h, buf, sizeof h);
-    if (h.magic != kMagic || h.version != kVersion || h.lanes != RB200_LANES || !h.chunk_syms) return RB200_E_STREAM;
-    if (h.n_chunks != h.n_symbols / h.chunk_syms + (h.n_symbols % h.chunk_syms != 0) || h.n_chunks >= (1ull << 31) ||
-        (h.blob_bytes & 15) || h.coder > RB200_CODER_RANS64 || h.scale_bits < 8 || h.scale_bits > 16)
-        return RB200_E_STREAM;
-    const size_t boff = blob_offset(h.n_chunks);
-    if (boff > size || h.blob_bytes > size - boff) return RB200_E_STREAM;
+    ContainerHeader h;
+    int rc = container_parse_header(buf, size, &h);
+    if (rc != RB200_OK) return rc;
     // freqs/offsets sit at 4- and 8-byte aligned positions when buf itself is 8-byte aligned (callers map or malloc it)
-    const uint32_t* freqs = reinterpret_cast<const uint32_t*>(buf + sizeof(Header));
-    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + sizeof(Header) + 256 * sizeof(uint32_t));
+    const uint32_t* freqs = reinterpret_cast<const uint32_t*>(buf + sizeof(ContainerHeader));
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + kContainerDirOffset);
     if (reinterpret_cast<uintptr_t>(buf) & 7) return RB200_E_ARG;
-    if (meta_crc(h, freqs, offsets) != h.meta_crc) return RB200_E_STREAM;
-    if (!model_fields_ok(h.coder, h.scale_bits, freqs)) return RB200_E_STREAM;        // CRC-valid but inconsistent
-    if (offsets[h.n_chunks] != h.blob_bytes) return RB200_E_STREAM;
-    if (h.n_chunks && offsets[0] >= 16) return RB200_E_STREAM;                        // the first stream starts inside the first vector
-    for (uint64_t c = 0; c < h.n_chunks; c++)
-        if (offsets[c] > offsets[c + 1]) return RB200_E_STREAM;
-    if ((h.flags & RB200_CONTAINER_CRC_BLOB) && crc32_update(0, buf + boff, h.blob_bytes) != h.blob_crc) return RB200_E_STREAM;
+    rc = container_check_prefix(h, buf, container_meta_crc(h, freqs, offsets));
+    if (rc != RB200_OK) return rc;
+    const size_t boff = container_blob_offset(h.n_chunks);
+    if (h.flags & RB200_CONTAINER_CRC_BLOB) rc = container_check_blob(h, container_crc32(0, buf + boff, h.blob_bytes));
+    if (rc != RB200_OK) return rc;
     info->coder = h.coder;
     info->scale_bits = h.scale_bits;
     info->chunk_syms = h.chunk_syms;

@@ -1,0 +1,301 @@
+// crc_kernels.cuh -- zlib's CRC-32 (IEEE polynomial, reflected, init and xor-out ~0) on sm_90a, and the GF(2)
+// algebra that joins CRCs of adjacent pieces (zlib's crc32_combine), shared by the host and the kernels.
+//
+// The CRC register after a message is linear in (initial register, message): with R(c, D) the register after D
+// starting from c,   R(c, A || B) = R(R(c, A), B)   and   R(c, D) = shift(c, |D|) ^ R(0, D),
+// where shift(c, len) multiplies c by x^(8 len) mod P.  zlib's crc32(D, crc_in) = ~R(~crc_in, D).  So the kernel
+// cuts the buffer into one contiguous segment per thread, computes each segment's R(0, D_t) on its own, shifts it
+// by the bytes that follow the segment and XORs everything together; one thread then applies crc_in and the
+// xor-out.  Multiplying by x^(8 len) takes one product per set bit of len from the table of x^(8 2^k), k < 64,
+// so lengths past 2^32 cost nothing extra.
+//
+// Per-segment method: slicing-by-4 over 32-bit words with the four 256-entry tables in shared memory, each entry
+// replicated 32 times with lane l reading replica l.  The replica of entry i for lane l sits at word i * 32 + l,
+// i.e. always in bank l, so the random table indices of a warp never conflict (DESIGN.md section 4 has the
+// alternatives and the numbers).  The 128 KiB of tables leave one 1024-thread CTA per SM.
+#pragma once
+#include <cstdint>
+#include <cuda_runtime.h>
+
+#include "container_format.h"
+#include "device_utils.cuh"
+
+namespace rb200 {
+
+constexpr uint32_t kCrcPoly = 0xEDB88320u;   // reflected IEEE 802.3 polynomial
+constexpr uint32_t kCrcOne = 0x80000000u;    // x^0 in the reflected representation
+
+// a * b mod P (reflected): zlib's multmodp, with a fixed trip count so that a == 0 is fine
+__host__ __device__ constexpr uint32_t crc32_mulmod(uint32_t a, uint32_t b)
+{
+    uint32_t p = 0;
+    for (int i = 0; i < 32; i++) {
+        p ^= b & (0u - ((a >> (31 - i)) & 1u));
+        b = (b >> 1) ^ (kCrcPoly & (0u - (b & 1u)));
+    }
+    return p;
+}
+
+struct CrcPowers {
+    uint32_t p[64];   // x^(8 * 2^k) mod P
+};
+
+__host__ __device__ constexpr CrcPowers crc32_make_powers()
+{
+    CrcPowers t{};
+    uint32_t x = kCrcOne >> 8;                                  // x^8
+    for (int k = 0; k < 64; k++) {
+        t.p[k] = x;
+        x = crc32_mulmod(x, x);
+    }
+    return t;
+}
+
+constexpr CrcPowers kCrcPowersHost = crc32_make_powers();
+__constant__ CrcPowers kCrcPowersDev = crc32_make_powers();
+
+__host__ __device__ inline uint32_t crc32_power(int k)
+{
+#ifdef __CUDA_ARCH__
+    return kCrcPowersDev.p[k];
+#else
+    return kCrcPowersHost.p[k];
+#endif
+}
+
+// c * x^(8 len) mod P: the register c followed by len zero bytes
+__host__ __device__ inline uint32_t crc32_shift(uint32_t c, uint64_t len)
+{
+    for (int k = 0; len; k++, len >>= 1)
+        if (len & 1) c = crc32_mulmod(c, crc32_power(k));
+    return c;
+}
+
+// zlib's crc32_combine: crc32(A || B) from crc32(A), crc32(B) and |B|
+__host__ __device__ inline uint32_t crc32_combine(uint32_t crc_a, uint32_t crc_b, uint64_t len_b)
+{
+    return crc32_shift(crc_a, len_b) ^ crc_b;
+}
+
+// zlib's crc32(D, crc_in) from acc = R(0, D) and |D|
+__host__ __device__ inline uint32_t crc32_finish(uint32_t crc_in, uint64_t len, uint32_t acc)
+{
+    return ~(crc32_shift(~crc_in, len) ^ acc);
+}
+
+// One CRC result: what the kernel computed and over how many bytes (the host pipeline joins slices with it).
+struct CrcSlot {
+    uint64_t len;
+    uint32_t crc;
+    uint32_t pad;
+};
+
+// Accumulator and CTA counter of crc32_kernel.  Zero between launches: the last CTA resets them.
+struct CrcWork {
+    uint32_t acc;
+    uint32_t done;
+};
+
+constexpr int kCrcThreads = 1024;
+constexpr int kCrcTableWords = 4 * 256 * 32;
+constexpr size_t kCrcSmemBytes = (kCrcTableWords + 64) * sizeof(uint32_t);
+
+namespace crc_detail {
+
+// R(0, D) for the bytes of one thread's segment, bit by bit (the finalise kernel's 34-byte pieces)
+__device__ __forceinline__ uint32_t raw_bytes_bitwise(const uint8_t* p, uint32_t len)
+{
+    uint32_t c = 0;
+    for (uint32_t i = 0; i < len; i++) {
+        c ^= p[i];
+#pragma unroll
+        for (int k = 0; k < 8; k++) c = (c >> 1) ^ (kCrcPoly & (0u - (c & 1u)));
+    }
+    return c;
+}
+
+// c * x^(8 len) with the powers in shared memory (lanes index it divergently; __constant__ would serialise)
+__device__ __forceinline__ uint32_t shift_smem(uint32_t c, uint64_t len, const uint32_t* pow)
+{
+    for (int k = 0; len; k++, len >>= 1)
+        if (len & 1) c = crc32_mulmod(c, pow[k]);
+    return c;
+}
+
+// x^(8 len) mod P by the whole warp: lane l takes bits l and l + 32 of len, then a butterfly of products
+__device__ __forceinline__ uint32_t x8pow_warp(uint64_t len)
+{
+    const int l = threadIdx.x & 31;
+    uint32_t f = ((len >> l) & 1) ? kCrcPowersDev.p[l] : kCrcOne;
+    if ((len >> (l + 32)) & 1) f = crc32_mulmod(f, kCrcPowersDev.p[l + 32]);
+#pragma unroll
+    for (int m = 16; m; m >>= 1) f = crc32_mulmod(f, __shfl_xor_sync(0xffffffffu, f, m));
+    return f;
+}
+
+// crc32_finish by a whole warp (every lane returns the result)
+__device__ __forceinline__ uint32_t finish_warp(uint32_t crc_in, uint64_t len, uint32_t acc)
+{
+    return ~(crc32_mulmod(~crc_in, x8pow_warp(len)) ^ acc);
+}
+
+__device__ __forceinline__ uint32_t step_word(uint32_t c, uint32_t w, uint32_t tab)
+{
+    const uint32_t v = c ^ w;
+    // table j (entry = byte followed by j zero bytes) at tab + j * 32 KiB; entry i of this lane at + i * 128
+    return lds_u32_ro(tab + 3 * 32768 + ((v << 7) & 0x7f80u)) ^ lds_u32_ro(tab + 2 * 32768 + ((v >> 1) & 0x7f80u)) ^
+           lds_u32_ro(tab + 1 * 32768 + ((v >> 9) & 0x7f80u)) ^ lds_u32_ro(tab + ((v >> 17) & 0x7f80u));
+}
+
+__device__ __forceinline__ uint32_t step_vec(uint32_t c, uint4 v, uint32_t tab)
+{
+    c = step_word(c, v.x, tab);
+    c = step_word(c, v.y, tab);
+    c = step_word(c, v.z, tab);
+    return step_word(c, v.w, tab);
+}
+
+__device__ __forceinline__ uint32_t step_byte(uint32_t c, uint32_t b, uint32_t tab)
+{
+    return lds_u32_ro(tab + (((c ^ b) & 0xffu) << 7)) ^ (c >> 8);
+}
+
+}  // namespace crc_detail
+
+// zlib crc32(data[0, n), crc_in) -> slot.  With n_dev set the length is min(*n_dev, n): a length the device wrote
+// (a directory's last entry), bounded by the buffer.  Any n and any alignment of data.  work must be zero (it is left zero).
+__global__ void __launch_bounds__(kCrcThreads, 1)
+    crc32_kernel(const uint8_t* __restrict__ data, uint64_t n, const uint64_t* __restrict__ n_dev, uint32_t crc_in, CrcWork* work,
+                 CrcSlot* slot)
+{
+    using namespace crc_detail;
+    extern __shared__ uint4 crc_smem_v[];
+    uint32_t* tabs = reinterpret_cast<uint32_t*>(crc_smem_v);
+    uint32_t* pow = tabs + kCrcTableWords;
+    {   // entry i of table j: R(0, byte i then j zero bytes); 32 replicas, 128 contiguous bytes
+        const uint32_t j = threadIdx.x >> 8, i = threadIdx.x & 255;
+        uint32_t c = i;
+        for (uint32_t k = 0; k < 8 * (j + 1); k++) c = (c >> 1) ^ (kCrcPoly & (0u - (c & 1u)));
+        uint4* dst = reinterpret_cast<uint4*>(tabs + (j * 256 + i) * 32);
+#pragma unroll
+        for (int r = 0; r < 8; r++) dst[r] = make_uint4(c, c, c, c);
+        if (threadIdx.x < 64) pow[threadIdx.x] = kCrcPowersDev.p[threadIdx.x];
+    }
+    __syncthreads();
+    if (n_dev && *n_dev < n) n = *n_dev;
+
+    // thread t owns span bytes [t L, (t + 1) L) of the 16-aligned span that starts a0 bytes before data
+    const uint64_t a0 = reinterpret_cast<uintptr_t>(data) & 15;
+    const uint8_t* base = data - a0;
+    const uint64_t span = a0 + n;
+    const uint64_t threads = static_cast<uint64_t>(gridDim.x) * kCrcThreads;
+    uint64_t L = (span + threads - 1) / threads;
+    L = (L + 31) & ~31ull;
+    const uint64_t t = static_cast<uint64_t>(blockIdx.x) * kCrcThreads + threadIdx.x;
+    uint64_t p = t * L;
+    const uint64_t e = p + L < span ? p + L : span;
+    if (p < a0) p = a0;
+    uint32_t contrib = 0;
+    if (p < e) {
+        const uint32_t tab = smem_addr(tabs) + (threadIdx.x & 31) * 4;
+        uint32_t c = 0;
+        for (; p < e && (p & 15); p++) c = step_byte(c, base[p], tab);              // unaligned head (thread 0 only)
+        const uint4* v = reinterpret_cast<const uint4*>(base + p);
+        const uint64_t pairs = (e - p) >> 5;
+        if (pairs) {
+            uint4 x0 = __ldg(v), x1 = __ldg(v + 1);
+            for (uint64_t k = 1; k < pairs; k++) {
+                const uint4 y0 = __ldg(v + 2 * k), y1 = __ldg(v + 2 * k + 1);
+                c = step_vec(step_vec(c, x0, tab), x1, tab);
+                x0 = y0;
+                x1 = y1;
+            }
+            c = step_vec(step_vec(c, x0, tab), x1, tab);
+            p += pairs << 5;
+        }
+        if (e - p >= 16) {
+            c = step_vec(c, __ldg(reinterpret_cast<const uint4*>(base + p)), tab);
+            p += 16;
+        }
+        for (; p < e; p++) c = step_byte(c, base[p], tab);                          // ragged tail (last thread only)
+        contrib = shift_smem(c, span - e, pow);
+    }
+    contrib = __reduce_xor_sync(0xffffffffu, contrib);
+    if ((threadIdx.x & 31) == 0 && contrib) {
+        atomicXor(&work->acc, contrib);
+        __threadfence();
+    }
+    __syncthreads();
+    __shared__ uint32_t last;
+    if (threadIdx.x == 0) {
+        __threadfence();
+        last = atomicAdd(&work->done, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last || threadIdx.x >= 32) return;
+    __threadfence();
+    const uint32_t acc = threadIdx.x == 0 ? atomicExch(&work->acc, 0u) : 0u;
+    const uint32_t crc = finish_warp(crc_in, n, __shfl_sync(0xffffffffu, acc, 0));
+    if (threadIdx.x == 0) {
+        work->done = 0;
+        slot->len = n;
+        slot->crc = crc;
+    }
+}
+
+inline void configure_crc_kernels()
+{
+    cudaFuncSetAttribute(crc32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCrcSmemBytes));
+}
+
+// CTAs for a length known on the host: about 256 bytes per thread at least, at most one CTA per SM
+inline uint32_t crc32_grid(uint32_t sms, uint64_t n)
+{
+    const uint64_t want = (n + kCrcThreads * 256ull - 1) / (kCrcThreads * 256ull);
+    return want < 1 ? 1 : (want > sms ? sms : static_cast<uint32_t>(want));
+}
+
+// The last step of a device-memory rb200_container_encode, one warp: the encoder has written the directory at
+// out + 1088 and the blob at out + blob_off, crc32_kernel has put the directory's CRC in slots[0] and (with
+// RB200_CONTAINER_CRC_BLOB) the blob's in slots[1].  Reads blob_bytes from the directory, completes the header
+// (h arrives with blob_bytes and both CRCs zero), and writes header, model and the zero pad in front of the blob.
+__global__ void __launch_bounds__(32)
+    container_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t blob_off, uint64_t out_cap, const uint32_t* __restrict__ freqs,
+                            const CrcSlot* __restrict__ slots, uint32_t* status)
+{
+    using namespace crc_detail;
+    __shared__ uint4 sbuf_v[kContainerDirOffset / 16];
+    uint32_t* sbuf = reinterpret_cast<uint32_t*>(sbuf_v);
+    const uint32_t lane = threadIdx.x;
+    const uint64_t blob_bytes = reinterpret_cast<const uint64_t*>(out + kContainerDirOffset)[h.n_chunks];
+    if (blob_bytes > out_cap - blob_off) {            // the encoder has flagged it; leave the buffer as it is
+        if (lane == 0) atomicOr(status, kStatSpace);
+        return;
+    }
+    if (lane == 0) {
+        ContainerHeader* sh = reinterpret_cast<ContainerHeader*>(sbuf);
+        *sh = h;
+        sh->blob_bytes = blob_bytes;
+    }
+    for (uint32_t i = lane; i < 256; i += 32) sbuf[16 + i] = freqs[i];
+    __syncwarp();
+    // CRC of header || freqs: 34 bytes per lane, each shifted past the bytes after it
+    constexpr uint32_t kPiece = kContainerDirOffset / 32;
+    uint32_t c = raw_bytes_bitwise(reinterpret_cast<const uint8_t*>(sbuf) + lane * kPiece, kPiece);
+    c = __reduce_xor_sync(0xffffffffu, crc32_shift(c, kContainerDirOffset - kPiece * (lane + 1)));
+    const uint32_t head_crc = finish_warp(0, kContainerDirOffset, c);
+    const uint64_t dir_bytes = (h.n_chunks + 1) * sizeof(uint64_t);
+    const uint32_t meta = crc32_mulmod(head_crc, x8pow_warp(dir_bytes)) ^ slots[0].crc;      // crc32_combine
+    __syncwarp();
+    if (lane == 0) {
+        sbuf[offsetof(ContainerHeader, meta_crc) / 4] = meta;
+        sbuf[offsetof(ContainerHeader, blob_crc) / 4] = (h.flags & RB200_CONTAINER_CRC_BLOB) ? slots[1].crc : 0u;
+    }
+    __syncwarp();
+    uint4* dst = reinterpret_cast<uint4*>(out);
+    for (uint32_t i = lane; i < kContainerDirOffset / 16; i += 32) dst[i] = sbuf_v[i];
+    const uint64_t dir_end = kContainerDirOffset + dir_bytes;
+    if (lane == 0 && blob_off > dir_end) *reinterpret_cast<uint64_t*>(out + dir_end) = 0;   // the 8-byte pad
+}
+
+}  // namespace rb200

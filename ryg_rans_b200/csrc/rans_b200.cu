@@ -17,6 +17,8 @@
 
 #include "alias_kernels.cuh"
 #include "block_kernels.cuh"
+#include "container_format.h"
+#include "crc_kernels.cuh"
 #include "rans64_kernels.cuh"
 #include "tables.h"
 #include "word_kernels.cuh"
@@ -54,6 +56,10 @@ struct rb200_ctx {
     uint64_t* h_slice_total = nullptr;   // pinned, kMaxSlices entries
     uint64_t* h_dir = nullptr;           // pinned staging for directories (caller's `offsets` may be pageable)
     size_t h_dir_cap = 0;                // entries
+    // CRC-32 (crc_kernels.cuh): the kernel's self-resetting accumulator, one result per pipeline slice, pinned mirror
+    CrcWork* d_crc_work = nullptr;
+    CrcSlot* d_crc = nullptr;            // kMaxSlices entries
+    CrcSlot* h_crc = nullptr;
 };
 
 struct rb200_model {
@@ -71,6 +77,8 @@ struct rb200_model {
     AliasEncEntry* d_byte_enc = nullptr;     // 256 RansEncSymbol images
     uint8_t* d_r64_dec = nullptr;            // cum2sym[1 << scale_bits] + 256 x {start, freq}
     uint4* d_r64_enc = nullptr;              // 256 x 32 B Rans64EncSymbol images
+    uint32_t freqs[256] = {};                // the model's frequencies: the model section of a container
+    uint32_t* d_freqs = nullptr;             // device copy, for rb200_container_encode in device memory
 };
 
 namespace {
@@ -208,6 +216,10 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_done[i], cudaEventDisableTiming);
     }
     if (e == cudaSuccess) e = cudaMallocHost(&ctx->h_slice_total, rb200_ctx::kMaxSlices * sizeof(uint64_t));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_crc_work, sizeof(CrcWork));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_crc_work, 0, sizeof(CrcWork));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_crc, rb200_ctx::kMaxSlices * sizeof(CrcSlot));
+    if (e == cudaSuccess) e = cudaMallocHost(&ctx->h_crc, rb200_ctx::kMaxSlices * sizeof(CrcSlot));
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -218,6 +230,7 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     configure_alias_kernels();
     configure_block_kernels();
     configure_rans64_kernels();
+    configure_crc_kernels();
     cudaGetLastError();
     *out = ctx;
     return RB200_OK;
@@ -235,6 +248,9 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->h_status) cudaFreeHost(ctx->h_status);
     if (ctx->h_slice_total) cudaFreeHost(ctx->h_slice_total);
     if (ctx->h_dir) cudaFreeHost(ctx->h_dir);
+    if (ctx->d_crc_work) cudaFree(ctx->d_crc_work);
+    if (ctx->d_crc) cudaFree(ctx->d_crc);
+    if (ctx->h_crc) cudaFreeHost(ctx->h_crc);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -280,6 +296,7 @@ extern "C" void rb200_model_destroy(rb200_model* m)
     cudaFree(m->d_alias_dec); cudaFree(m->d_alias_enc); cudaFree(m->d_alias_remap);
     cudaFree(m->d_byte_dec); cudaFree(m->d_byte_enc);
     cudaFree(m->d_r64_dec); cudaFree(m->d_r64_enc);
+    cudaFree(m->d_freqs);
     delete m;
 }
 
@@ -362,6 +379,9 @@ extern "C" int rb200_model_create(rb200_ctx* ctx, int coder, uint32_t scale_bits
         delete m;
         return RB200_E_ARG;
     }
+    std::memcpy(m->freqs, freqs, sizeof m->freqs);
+    if (rc == RB200_OK && e == cudaSuccess) e = cudaMalloc(&m->d_freqs, sizeof m->freqs);
+    if (rc == RB200_OK && e == cudaSuccess) e = cudaMemcpy(m->d_freqs, m->freqs, sizeof m->freqs, cudaMemcpyHostToDevice);
     if (rc != RB200_OK || e != cudaSuccess) {
         if (e != cudaSuccess) rc = cuda_fail(ctx, e, "model upload");
         rb200_model_destroy(m);
@@ -723,6 +743,15 @@ struct UnitTable {
     size_t unit_bytes;
 };
 
+// Optional per-slice work of a host pipeline, enqueued on ctx->stream once the slice's bytes are on the device:
+// `(i, d_data, d_len, cap)` after slice i's encode, whose staged container is d_data[0, *d_len) with *d_len <= cap;
+// `(i, d_data, len)` before
+// slice i's decode, whose blob bytes are d_data[0, len).  rb200_container_encode / _decode CRC the blob with it.
+struct NoSliceHook {
+    int operator()(size_t, const uint8_t*, const uint64_t*, size_t) const { return RB200_OK; }
+    int operator()(size_t, const uint8_t*, size_t) const { return RB200_OK; }
+};
+
 // Host buffers -> blob, overlapped: slice i+1 is copied in while slice i is encoded and slice i-1 is
 // copied out.  Every slice is its own container in a staging region; because containers end 16-byte
 // aligned they concatenate, and the directory entries only need the running base added.  Directories are
@@ -730,9 +759,10 @@ struct UnitTable {
 // `reserve_ws(units)` grows the encode workspace for a slice of that many units; it runs once, for the largest slice,
 // so that no slice stalls on a reallocation.  `encode_slice(slice, d_in, d_table, d_blob, cap, d_offsets)` enqueues
 // one slice's encode on ctx->stream.
-template <class ReserveWs, class EncodeSlice>
+template <class ReserveWs, class EncodeSlice, class Hook = NoSliceHook>
 int encode_pipeline(rb200_ctx* ctx, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t unit_chunks, UnitTable tab,
-                    ReserveWs reserve_ws, EncodeSlice encode_slice, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size)
+                    ReserveWs reserve_ws, EncodeSlice encode_slice, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size,
+                    Hook hook = Hook{})
 {
     if (n == 0) {
         offsets[0] = 0;
@@ -773,7 +803,8 @@ int encode_pipeline(rb200_ctx* ctx, const uint8_t* in, size_t n, uint32_t chunk_
             RB_CUDA(ctx, cudaEventRecord(ctx->ev_in[i], ctx->s_in));
             RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[i], 0));
             uint64_t* so = d_off + s.c0 + i;
-            const int r = encode_slice(s, d_in + s.lo, d_tab + s.u0 * tb, d_blob + s.c0 * slot, s.cnt * slot, so);
+            int r = encode_slice(s, d_in + s.lo, d_tab + s.u0 * tb, d_blob + s.c0 * slot, s.cnt * slot, so);
+            if (r == RB200_OK) r = hook(i, d_blob + s.c0 * slot, so + s.cnt, s.cnt * slot);
             if (r != RB200_OK) return r;
             RB_CUDA(ctx, cudaMemcpyAsync(&ctx->h_slice_total[i], so + s.cnt, sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
             RB_CUDA(ctx, cudaEventRecord(ctx->ev_done[i], ctx->stream));
@@ -826,9 +857,9 @@ int encode_pipeline(rb200_ctx* ctx, const uint8_t* in, size_t n, uint32_t chunk_
 // directory (and therefore every slice's byte range) is already on the host.
 // `decode_slice(slice, d_blob, d_offsets, d_table, d_out)` enqueues one slice's decode on ctx->stream; d_offsets points
 // at the slice's first directory entry.
-template <class DecodeSlice>
+template <class DecodeSlice, class Hook = NoSliceHook>
 int decode_pipeline(rb200_ctx* ctx, const uint8_t* blob, size_t blob_size, const uint64_t* offsets, uint32_t chunk_syms,
-                    uint32_t unit_chunks, UnitTable tab, DecodeSlice decode_slice, uint8_t* out, size_t n)
+                    uint32_t unit_chunks, UnitTable tab, DecodeSlice decode_slice, uint8_t* out, size_t n, Hook hook = Hook{})
 {
     if (n == 0) return RB200_OK;
     const uint32_t unit_syms = chunk_syms * unit_chunks;
@@ -869,7 +900,8 @@ int decode_pipeline(rb200_ctx* ctx, const uint8_t* blob, size_t blob_size, const
                                              cudaMemcpyHostToDevice, ctx->s_in));
             RB_CUDA(ctx, cudaEventRecord(ctx->ev_in[i], ctx->s_in));
             RB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[i], 0));
-            const int r = decode_slice(s, d_blob, d_off + s.c0, d_tab + s.u0 * tb, d_out + s.lo);
+            int r = hook(i, d_blob + b0, b1 - b0);
+            if (r == RB200_OK) r = decode_slice(s, d_blob, d_off + s.c0, d_tab + s.u0 * tb, d_out + s.lo);
             if (r != RB200_OK) return r;
             RB_CUDA(ctx, cudaEventRecord(ctx->ev_done[i], ctx->stream));
             RB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_out, ctx->ev_done[i], 0));
@@ -897,6 +929,32 @@ int by_mem_kind(int mem_kind, const void* blob, const uint64_t* offsets, Device 
 // container invariant: the blob ends on a 16-byte boundary; the decoders index it in 16-byte vectors with 32 bits
 bool blob_size_ok(size_t blob_size) { return (blob_size & 15) == 0 && (blob_size >> 36) == 0; }
 
+// the host-buffer form of rb200_encode / rb200_decode (one chunk per pipeline unit)
+template <class Hook = NoSliceHook>
+int encode_host(rb200_ctx* ctx, const rb200_model* model, const uint8_t* in, size_t n, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap,
+                uint64_t* offsets, size_t* blob_size, Hook hook = Hook{})
+{
+    return encode_pipeline(
+        ctx, in, n, chunk_syms, 1, UnitTable{},
+        [&](size_t units) { return reserve_encode(ctx, model, static_cast<uint32_t>(units), chunk_syms); },
+        [&](const Slice& s, const uint8_t* d_in, uint8_t*, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
+            return encode_device(ctx, model, d_in, s.len, chunk_syms, d_blob, cap, d_off);
+        },
+        blob, blob_cap, offsets, blob_size, hook);
+}
+
+template <class Hook = NoSliceHook>
+int decode_host(rb200_ctx* ctx, const rb200_model* model, const uint8_t* blob, size_t blob_size, const uint64_t* offsets,
+                uint32_t chunk_syms, uint8_t* out, size_t n, Hook hook = Hook{})
+{
+    return decode_pipeline(
+        ctx, blob, blob_size, offsets, chunk_syms, 1, UnitTable{},
+        [&](const Slice& s, const uint8_t* d_blob, const uint64_t* d_off, uint8_t*, uint8_t* d_out) {
+            return decode_device(ctx, model, d_blob, blob_size, d_off, chunk_syms, d_out, s.len);
+        },
+        out, n, hook);
+}
+
 }  // namespace
 
 extern "C" int rb200_encode(rb200_ctx* ctx, const rb200_model* model, const uint8_t* in, size_t n, uint32_t chunk_syms,
@@ -906,15 +964,7 @@ extern "C" int rb200_encode(rb200_ctx* ctx, const rb200_model* model, const uint
     DeviceGuard g(ctx->device);
     return by_mem_kind(
         mem_kind, blob, offsets, [&] { return encode_device(ctx, model, in, n, chunk_syms, blob, blob_cap, offsets); },
-        [&] {
-            return encode_pipeline(
-                ctx, in, n, chunk_syms, 1, UnitTable{},
-                [&](size_t units) { return reserve_encode(ctx, model, static_cast<uint32_t>(units), chunk_syms); },
-                [&](const Slice& s, const uint8_t* d_in, uint8_t*, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
-                    return encode_device(ctx, model, d_in, s.len, chunk_syms, d_blob, cap, d_off);
-                },
-                blob, blob_cap, offsets, blob_size);
-        });
+        [&] { return encode_host(ctx, model, in, n, chunk_syms, blob, blob_cap, offsets, blob_size); });
 }
 
 extern "C" int rb200_decode(rb200_ctx* ctx, const rb200_model* model, const uint8_t* blob, size_t blob_size,
@@ -926,14 +976,7 @@ extern "C" int rb200_decode(rb200_ctx* ctx, const rb200_model* model, const uint
     DeviceGuard g(ctx->device);
     return by_mem_kind(
         mem_kind, blob, offsets, [&] { return decode_device(ctx, model, blob, blob_size, offsets, chunk_syms, out, n); },
-        [&] {
-            return decode_pipeline(
-                ctx, blob, blob_size, offsets, chunk_syms, 1, UnitTable{},
-                [&](const Slice& s, const uint8_t* d_blob, const uint64_t* d_off, uint8_t*, uint8_t* d_out) {
-                    return decode_device(ctx, model, d_blob, blob_size, d_off, chunk_syms, d_out, s.len);
-                },
-                out, n);
-        });
+        [&] { return decode_host(ctx, model, blob, blob_size, offsets, chunk_syms, out, n); });
 }
 
 // ---------------------------------------------------------------------------
@@ -1145,6 +1188,191 @@ extern "C" int rb200_blocks_decode(rb200_ctx* ctx, const uint8_t* blob, size_t b
                 },
                 out, static_cast<size_t>(n_blocks) * block_size);
         });
+}
+
+// ---------------------------------------------------------------------------
+// CRC-32 and the container in host or device memory: crc_kernels.cuh, container_host.cpp
+// ---------------------------------------------------------------------------
+
+namespace {
+
+// zlib crc32 of d[0, n) into `slot`, on ctx->stream; with n_dev set the length is min(*n_dev, n)
+int launch_crc(rb200_ctx* ctx, const uint8_t* d, uint64_t n, const uint64_t* n_dev, uint32_t crc_in, CrcSlot* slot)
+{
+    const uint32_t sms = static_cast<uint32_t>(ctx->sms);
+    crc32_kernel<<<n_dev ? sms : crc32_grid(sms, n), kCrcThreads, kCrcSmemBytes, ctx->stream>>>(d, n, n_dev, crc_in, ctx->d_crc_work, slot);
+    return check_launch(ctx, "crc32_kernel");
+}
+
+// brings slots [0, count) to ctx->h_crc and waits for them
+int fetch_crc(rb200_ctx* ctx, size_t count)
+{
+    if (!count) return RB200_OK;
+    RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_crc, ctx->d_crc, count * sizeof(CrcSlot), cudaMemcpyDeviceToHost, ctx->stream));
+    RB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return RB200_OK;
+}
+
+// the CRC of the whole blob from the per-slice CRCs a host pipeline left in slots [0, count), joined in slice order
+int joined_slice_crc(rb200_ctx* ctx, size_t count, uint32_t* crc)
+{
+    const int rc = fetch_crc(ctx, count);
+    if (rc != RB200_OK) return rc;
+    uint32_t c = 0;
+    for (size_t i = 0; i < count; i++) c = crc32_combine(c, ctx->h_crc[i].crc, ctx->h_crc[i].len);
+    *crc = c;
+    return RB200_OK;
+}
+
+// The per-slice hook of the container calls: CRC each slice's blob bytes into slot i when `on`.  Counts the slices.
+struct SliceCrc {
+    rb200_ctx* ctx;
+    bool on;
+    size_t* slices;
+    int operator()(size_t i, const uint8_t* d, const uint64_t* d_len, size_t cap) const
+    {
+        *slices = i + 1;
+        return on ? launch_crc(ctx, d, cap, d_len, 0, ctx->d_crc + i) : RB200_OK;
+    }
+    int operator()(size_t i, const uint8_t* d, size_t len) const
+    {
+        *slices = i + 1;
+        return on ? launch_crc(ctx, d, len, nullptr, 0, ctx->d_crc + i) : RB200_OK;
+    }
+};
+
+// rb200_container_decode once the buffers are checked: header, model and directory validated by the shared parser,
+// then the blob CRC, then a model and the decode.  DEVICE: the prefix is read through pinned memory, both CRCs
+// are taken on the GPU, and nothing is decoded unless every check passes.
+int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap, uint64_t* n_symbols,
+                          bool device)
+{
+    ContainerHeader h;
+    const uint8_t* prefix = buf;
+    int rc;
+    if (device) {
+        if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
+        rc = reserve_dir(ctx, sizeof(ContainerHeader) / sizeof(uint64_t));
+        if (rc != RB200_OK) return rc;
+        RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir, buf, sizeof(ContainerHeader), cudaMemcpyDeviceToHost, ctx->stream));
+        RB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        rc = container_parse_header(reinterpret_cast<const uint8_t*>(ctx->h_dir), size, &h);
+        if (rc != RB200_OK) return rc;
+        const size_t boff = container_blob_offset(h.n_chunks);
+        rc = reserve_dir(ctx, boff / sizeof(uint64_t));
+        if (rc != RB200_OK) return rc;
+        const uint64_t rest = boff - sizeof(ContainerHeader);     // model, directory and pad: what the CRC covers after the header
+        const uint64_t covered = kContainerDirOffset - sizeof(ContainerHeader) + (h.n_chunks + 1) * sizeof(uint64_t);
+        RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir, buf, sizeof(ContainerHeader) + rest, cudaMemcpyDeviceToHost, ctx->stream));
+        rc = launch_crc(ctx, buf + sizeof(ContainerHeader), covered, nullptr, 0, ctx->d_crc);
+        if (rc == RB200_OK) rc = fetch_crc(ctx, 1);
+        if (rc != RB200_OK) return rc;
+        prefix = reinterpret_cast<const uint8_t*>(ctx->h_dir);
+        rc = container_check_prefix(h, prefix, crc32_combine(container_header_crc(h), ctx->h_crc[0].crc, covered));
+    } else {
+        rc = container_parse_header(buf, size, &h);
+        if (rc == RB200_OK)
+            rc = container_check_prefix(h, buf, container_meta_crc(h, reinterpret_cast<const uint32_t*>(buf + sizeof(ContainerHeader)),
+                                                                   reinterpret_cast<const uint64_t*>(buf + kContainerDirOffset)));
+    }
+    if (rc != RB200_OK) return rc;
+    if (n_symbols) *n_symbols = h.n_symbols;
+    if (out_cap < h.n_symbols) return RB200_E_SPACE;
+    if (h.n_symbols && !out) return RB200_E_ARG;
+    if (!chunk_ok(h.chunk_syms) || !blob_size_ok(h.blob_bytes)) return RB200_E_ARG;     // what rb200_decode accepts
+    const uint8_t* blob = buf + container_blob_offset(h.n_chunks);
+    const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
+    if (device && blob_crc) {
+        rc = launch_crc(ctx, blob, h.blob_bytes, nullptr, 0, ctx->d_crc);
+        if (rc == RB200_OK) rc = fetch_crc(ctx, 1);
+        if (rc == RB200_OK) rc = container_check_blob(h, ctx->h_crc[0].crc);
+        if (rc != RB200_OK) return rc;
+    }
+    rb200_model* model = nullptr;
+    rc = rb200_model_create(ctx, h.coder, h.scale_bits, reinterpret_cast<const uint32_t*>(prefix + sizeof(ContainerHeader)), &model);
+    if (rc != RB200_OK) return rc;
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + kContainerDirOffset);
+    if (device) {
+        rc = decode_device(ctx, model, blob, h.blob_bytes, offsets, h.chunk_syms, out, h.n_symbols);
+        const int st = rb200_sync(ctx);
+        if (rc == RB200_OK) rc = st;
+    } else {
+        size_t slices = 0;
+        rc = decode_host(ctx, model, blob, h.blob_bytes, offsets, h.chunk_syms, out, h.n_symbols, SliceCrc{ctx, blob_crc, &slices});
+        uint32_t crc = 0;
+        if (rc == RB200_OK && blob_crc) rc = joined_slice_crc(ctx, slices, &crc);
+        if (rc == RB200_OK) rc = container_check_blob(h, crc);
+    }
+    rb200_model_destroy(model);
+    return rc;
+}
+
+}  // namespace
+
+extern "C" int rb200_crc32(rb200_ctx* ctx, const uint8_t* data, size_t n, uint32_t crc_in, uint32_t* crc_out, int mem_kind)
+{
+    if (!ctx || !crc_out || (!data && n) || (mem_kind != RB200_MEM_HOST && mem_kind != RB200_MEM_DEVICE)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    const uint8_t* d = data;
+    if (mem_kind == RB200_MEM_HOST) {
+        const int rc = reserve(ctx, ctx->st_in, n + 16);
+        if (rc != RB200_OK) return rc;
+        if (n) RB_CUDA(ctx, cudaMemcpyAsync(ctx->st_in.p, data, n, cudaMemcpyHostToDevice, ctx->stream));
+        d = static_cast<const uint8_t*>(ctx->st_in.p);
+    }
+    int rc = launch_crc(ctx, d, n, nullptr, crc_in, ctx->d_crc);
+    if (rc == RB200_OK) rc = fetch_crc(ctx, 1);
+    if (rc == RB200_OK) *crc_out = ctx->h_crc[0].crc;
+    return rc;
+}
+
+extern "C" int rb200_container_encode(rb200_ctx* ctx, const rb200_model* model, const uint8_t* in, size_t n, uint32_t chunk_syms,
+                                      uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind)
+{
+    if (!ctx || !model || model->ctx != ctx || !out || (!in && n) || !chunk_ok(chunk_syms)) return RB200_E_ARG;
+    const bool device = mem_kind == RB200_MEM_DEVICE;
+    if ((!device && mem_kind != RB200_MEM_HOST) || (reinterpret_cast<uintptr_t>(out) & (device ? 15 : 7))) return RB200_E_ARG;
+    if (!container_model_ok(static_cast<uint32_t>(model->coder), model->scale_bits, model->freqs)) return RB200_E_MODEL;
+    const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
+    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    const size_t boff = container_blob_offset(n_chunks);
+    if (out_cap < boff) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    ContainerHeader h = container_header(model->coder, model->scale_bits, chunk_syms, n, n_chunks, 0, flags);
+    const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + kContainerDirOffset);
+    const size_t dir_bytes = (n_chunks + 1) * sizeof(uint64_t);
+    if (device) {            // asynchronous: directory CRC, blob CRC, then the header from blob_bytes = dir[n_chunks]
+        int rc = encode_device(ctx, model, in, n, chunk_syms, out + boff, out_cap - boff, dir);
+        if (rc == RB200_OK) rc = launch_crc(ctx, out + kContainerDirOffset, dir_bytes, nullptr, 0, ctx->d_crc);
+        if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+        if (rc != RB200_OK) return rc;
+        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, boff, out_cap, model->d_freqs, ctx->d_crc, ctx->d_status);
+        return check_launch(ctx, "container_finish_kernel");
+    }
+    size_t blob_bytes = 0, slices = 0;
+    int rc = encode_host(ctx, model, in, n, chunk_syms, out + boff, out_cap - boff, dir, &blob_bytes, SliceCrc{ctx, blob_crc, &slices});
+    if (rc == RB200_OK && blob_crc) rc = joined_slice_crc(ctx, slices, &h.blob_crc);
+    if (rc != RB200_OK) return rc;
+    h.blob_bytes = blob_bytes;
+    h.meta_crc = container_meta_crc(h, model->freqs, dir);
+    std::memcpy(out, &h, sizeof h);
+    std::memcpy(out + sizeof h, model->freqs, sizeof model->freqs);
+    std::memset(out + kContainerDirOffset + dir_bytes, 0, boff - kContainerDirOffset - dir_bytes);
+    if (out_size) *out_size = boff + blob_bytes;
+    return RB200_OK;
+}
+
+extern "C" int rb200_container_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                      uint64_t* n_symbols, int mem_kind)
+{
+    if (!ctx || !buf || (!out && out_cap)) return RB200_E_ARG;
+    const bool device = mem_kind == RB200_MEM_DEVICE;
+    const uintptr_t align = device ? 15 : 7;
+    if ((!device && mem_kind != RB200_MEM_HOST) || (reinterpret_cast<uintptr_t>(buf) & align) || (reinterpret_cast<uintptr_t>(out) & align))
+        return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, device);
 }
 
 // ---------------------------------------------------------------------------

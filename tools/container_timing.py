@@ -1,0 +1,161 @@
+"""What the container costs on the GPU, on the headline workload (1 GiB of uniform bytes, word coder, chunks of 8192,
+device buffers):
+
+  rb200_crc32 over 1 GiB of device memory (ms, and the share of 3.35 TB/s, the H100 SXM data-sheet bandwidth);
+  rb200_encode against rb200_container_encode with flags 0 and RB200_CONTAINER_CRC_BLOB, alternated;
+  rb200_decode against rb200_container_decode;
+  host rb200_container_pack with RB200_CONTAINER_CRC_BLOB against rb200_crc32 in HOST mode, on the same blob.
+
+Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
+numbers.  Every output is checked against the plain calls plus rb200_container_pack.
+    python tools/container_timing.py [--reps 10] [--json out.json]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import ryg_rans_b200 as rb  # noqa: E402
+from ryg_rans_b200 import api  # noqa: E402
+
+HBM_BPS = 3.35e12
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        q = ""
+    import torch
+    return q or torch.cuda.get_device_name(0)
+
+
+def timed(fn, sync):
+    import torch
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    fn()
+    b.record()
+    sync()
+    b.synchronize()
+    return a.elapsed_time(b)
+
+
+def stats(ts):
+    ts = np.asarray(ts)
+    return {"median_ms": float(np.median(ts)), "min_ms": float(ts.min()), "max_ms": float(ts.max()), "n": int(ts.size)}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+    import torch
+    assert torch.cuda.is_available(), "needs a CUDA device"
+    n, chunk = 1 << 30, 8192
+    g = torch.Generator(device="cuda")
+    g.manual_seed(1234)
+    d_in = torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda", generator=g)
+    ctx = rb.Context(0)
+    model = rb.Model.from_data(ctx, rb.CODER_WORD, 12, device_ptr=d_in.data_ptr(), n=n)
+    n_chunks = ctx.chunk_count(n, chunk)
+    bound = ctx.encode_bound(n, chunk)
+    cap = ctx.container_capacity(n, chunk)
+    d_blob = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+    d_offs = torch.empty(n_chunks + 1, dtype=torch.int64, device="cuda")
+    d_cont = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_out = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+    sync = ctx.sync
+
+    calls = {
+        "encode": lambda: ctx.encode_device(model, d_in.data_ptr(), n, chunk, d_blob.data_ptr(), bound, d_offs.data_ptr()),
+        "container_encode": lambda: ctx.container_encode_device(model, d_in.data_ptr(), n, chunk, 0, d_cont.data_ptr(), cap),
+        "container_encode_crc": lambda: ctx.container_encode_device(model, d_in.data_ptr(), n, chunk, api.CONTAINER_CRC_BLOB,
+                                                                    d_cont.data_ptr(), cap),
+    }
+    times = {k: [] for k in calls}
+    for _ in range(args.warmup):
+        for f in calls.values():
+            timed(f, sync)
+    for _ in range(args.reps):
+        for k, f in calls.items():
+            times[k].append(timed(f, sync))
+
+    # outputs: the CRC_BLOB container (last call) equals pack of the plain encode's blob and directory
+    calls["encode"]()
+    sync()
+    blob_bytes = int(d_offs[n_chunks].item())
+    h_blob = d_blob[:blob_bytes].cpu().numpy()
+    h_offs = d_offs.cpu().numpy().view(np.uint64)
+    t0 = time.perf_counter()
+    want = api.container_pack(rb.CODER_WORD, 12, chunk, n, model.freqs, h_offs, h_blob, api.CONTAINER_CRC_BLOB)
+    t_pack = time.perf_counter() - t0
+    calls["container_encode_crc"]()
+    sync()
+    size = want.size
+    identical_encode = bool(np.array_equal(d_cont[:size].cpu().numpy(), want))
+    d_want = torch.from_numpy(want).cuda()
+
+    # rb200_crc32 over 1 GiB of device memory
+    crc_times = []
+    for i in range(args.warmup + args.reps):
+        t = timed(lambda: ctx.crc32_device(d_in.data_ptr(), n), sync)
+        if i >= args.warmup:
+            crc_times.append(t)
+    crc_ok = ctx.crc32_device(d_blob.data_ptr(), blob_bytes) == int(np.frombuffer(want[48:52].tobytes(), np.uint32)[0])
+
+    # decode: plain against container (the CRC_BLOB container, both checks on the GPU)
+    dec = {
+        "decode": lambda: ctx.decode_device(model, d_blob.data_ptr(), blob_bytes, d_offs.data_ptr(), chunk, d_out.data_ptr(), n),
+        "container_decode": lambda: ctx.container_decode_device(d_want.data_ptr(), size, d_out.data_ptr(), n),
+    }
+    dtimes = {k: [] for k in dec}
+    for _ in range(args.warmup):
+        for f in dec.values():
+            timed(f, sync)
+    for _ in range(args.reps):
+        for k, f in dec.items():
+            dtimes[k].append(timed(f, sync))
+    d_out.zero_()
+    dec["container_decode"]()
+    identical_decode = bool(torch.equal(d_out[:n], d_in))
+
+    # host: pack with the blob CRC (one core) against rb200_crc32 in HOST mode, same blob
+    host_crc = []
+    for i in range(1 + args.reps):
+        t0 = time.perf_counter()
+        c = ctx.crc32(h_blob)
+        if i:
+            host_crc.append((time.perf_counter() - t0) * 1e3)
+    host_crc_ok = c == int(np.frombuffer(want[48:52].tobytes(), np.uint32)[0])
+
+    res = {
+        "card": card(),
+        "workload": {"n": n, "coder": "word", "chunk_syms": chunk, "blob_bytes": blob_bytes, "container_bytes": size},
+        "crc32_device_1GiB": {**stats(crc_times), "share_of_3.35TBps": n / HBM_BPS * 1e3 / float(np.median(crc_times))},
+        "encode": {k: stats(v) for k, v in times.items()},
+        "decode": {k: stats(v) for k, v in dtimes.items()},
+        "host_blob": {"container_pack_crc_blob_ms": t_pack * 1e3, "rb200_crc32_host_mode": stats(host_crc)},
+        "checks": {"container_encode_equals_pack": identical_encode, "container_decode_equals_input": identical_decode,
+                   "crc32_device_equals_header": bool(crc_ok), "crc32_host_equals_header": bool(host_crc_ok)},
+    }
+    print(json.dumps(res, indent=1))
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump(res, f, indent=1)
+    ok = all(res["checks"].values())
+    model.close()
+    ctx.close()
+    sys.exit(0 if ok else 1)
+
+
+if __name__ == "__main__":
+    main()

@@ -53,6 +53,34 @@ def main():
     assert np.array_equal(ctx.blocks_decode_host(blob, offs, freqs, nb, bs, chunk), data)
     st = rb.SymbolStats().count_freqs(data)
     assert np.array_equal(ctx.histogram(data), st.freqs.astype(np.uint64))
+    # CRC-32 and the container calls: host mode over several pipeline slices, device mode, a rejected container
+    import zlib
+    import torch
+    from ryg_rans_b200 import api
+    for start in (0, 3):
+        assert ctx.crc32(data[start:]) == zlib.crc32(data[start:].tobytes())
+    f, c = orc.model(data, 12)
+    m = ctx.model(rb.CODER_WORD, 12, f)
+    cont = ctx.container_encode_host(m, data, 4096, api.CONTAINER_CRC_BLOB)
+    blob, offs = ctx.encode_host(m, data, 4096)
+    assert np.array_equal(cont, api.container_pack(rb.CODER_WORD, 12, 4096, data.size, f, offs, blob, api.CONTAINER_CRC_BLOB))
+    assert np.array_equal(ctx.container_decode_host(cont), data)
+    d_in = torch.from_numpy(data).cuda()
+    d_cont = torch.zeros(cont.size + 16, dtype=torch.uint8, device="cuda")
+    d_out = torch.zeros(data.size + 16, dtype=torch.uint8, device="cuda")
+    assert ctx.crc32_device(d_in.data_ptr() + 5, data.size - 5) == zlib.crc32(data[5:].tobytes())
+    ctx.container_encode_device(m, d_in.data_ptr(), data.size, 4096, api.CONTAINER_CRC_BLOB, d_cont.data_ptr(), cont.size)
+    ctx.sync()
+    assert np.array_equal(d_cont[:cont.size].cpu().numpy(), cont)
+    assert ctx.container_decode_device(d_cont.data_ptr(), cont.size, d_out.data_ptr(), data.size) == data.size
+    assert torch.equal(d_out[:data.size], d_in)
+    d_cont[cont.size - 20] ^= 1
+    try:
+        ctx.container_decode_device(d_cont.data_ptr(), cont.size, d_out.data_ptr(), data.size)
+        raise SystemExit("blob corruption not reported")
+    except rb.RansError:
+        pass
+    m.close()
     print("sanitize smoke ok:", ctx.launches, "launches")
 
 
