@@ -11,10 +11,10 @@
 // significant first (RansDecRenorm, rans_byte.h:307-318, called lane by lane at
 // main_alias.cpp:396-397).
 #pragma once
+#include "decode_stream.cuh"
 #include "device_utils.cuh"
 #include "tables.h"
-#include "word_kernels.cuh"   // StreamWindow
-#include "word_decode_tma.cuh"   // persistent decode plumbing: DecPolicy, TmaWindow, tma_issue / tma_advance
+#include "word_kernels.cuh"   // funnel_shr_wrap; encode_stream and placement for the encoder
 
 namespace rb200 {
 
@@ -22,179 +22,125 @@ constexpr uint32_t kByteL = 1u << 23;   // RANS_BYTE_L, rans_byte.h:50
 constexpr int kAliasDecWarps = 16;
 constexpr uint32_t kAliasDecReplicas = 8;    // quarter-warp lanes hit 8 different 16-byte bank groups
 
-// One decode step of the byte-renormalising coders for the whole warp.
-//   ALIAS:  RansDecGetAlias (main_alias.cpp:252-267); tab_lane = this lane's replica of the 256 x 16 B
-//           bucket table.
-//   !ALIAS: RansDecGet -> cum2sym -> RansDecAdvanceSymbolStep (rans_byte.h:125-128, main.cpp:200,
-//           rans_byte.h:291-304); tab_lane = shared address of cum2sym[1 << sb], followed by the
-//           256 x {start | freq << 16} table.
-// then RansDecRenorm (rans_byte.h:307-318) for both.
-// FULL: all 32 lanes take part (active == true at compile time); only the ragged last step of a chunk does not.
+// ---------------------------------------------------------------------------
+// K8: the rans_byte cum2sym decoder (main.cpp) on the stream window of decode_stream.cuh.
+// ---------------------------------------------------------------------------
+// The byte coder for decode_window_chunk: RansDecGet -> cum2sym -> RansDecAdvanceSymbolStep (rans_byte.h:125-128,
+// main.cpp:200, rans_byte.h:291-304), then RansDecRenorm (rans_byte.h:307-318).  tab = shared address of cum2sym[1 << sb],
+// followed by the 256 x {start | freq << 16} table.
 // SB: scale_bits as a compile-time constant (16, 14, 12: masks and shift counts become immediates), 0 = use `sb_rt`.
-template <bool ALIAS, bool FULL, uint32_t SB>
-__device__ __forceinline__ void alias_dec_step(uint32_t& x, uint32_t& cursor, uint32_t tab_lane, uint32_t ring, uint8_t* o,
-                                               uint32_t lt, uint32_t sb_rt, bool active)
-{
-    const uint32_t sb = SB ? SB : sb_rt;
-    bool n1 = false, n2 = false;
-    if (active) {
-        const uint32_t xm = x & ((1u << sb) - 1);                          // main_alias.cpp:258 / rans_byte.h:127
-        if (ALIAS) {
-            const uint32_t bucket = xm >> (sb - 8);                        // :259
-            const uint4 e = lds_u128_ro(mad_u32(bucket, kAliasDecReplicas * 16, tab_lane));
-            const bool own = xm < e.x;                                     // :261 (bucket2 = 2 * bucket + 1)
-            const uint32_t fs = own ? e.z : e.y;                           // slot_freqs << 8 | sym_id
-            const uint32_t adj = own ? (e.w >> 16) : (e.w & 0xffffu);
-            x = (fs >> 8) * (x >> sb) + ((xm - adj) & 0xffffu);            // :265
-            *o = static_cast<uint8_t>(fs);                                 // :266
-        } else {
-            const uint32_t s = lds_u8_ro(tab_lane + xm);                   // cum2sym, main.cpp:200
-            const uint32_t ds = lds_u32_ro(tab_lane + (1u << sb) + 4u * s);   // RansDecSymbol {start, freq}
-            x = (ds >> 16) * (x >> sb) + xm - (ds & 0xffffu);              // rans_byte.h:297
-            *o = static_cast<uint8_t>(s);
-        }
-        n1 = x < kByteL;
-        n2 = x < (kByteL >> 8);
-    }
-    if (FULL) {
-        // RansDecRenorm for the warp as one PTX sequence: two predicates feed the votes, the two ranked byte
-        // loads and the state updates (the C++ below costs six more instructions and a branch per step)
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p1, p2;\n\t"
-            ".reg .b32 m, r, a, b;\n\t"
-            "setp.lt.u32 p1, %0, %2;\n\t"
-            "setp.lt.u32 p2, %0, %3;\n\t"
-            "vote.sync.ballot.b32 m, p1, 0xffffffff;\n\t"
-            "and.b32 r, m, %4;\n\t"
-            "popc.b32 r, r;\n\t"
-            "add.u32 a, %1, r;\n\t"
-            "popc.b32 m, m;\n\t"
-            "add.u32 %1, %1, m;\n\t"
-            "vote.sync.ballot.b32 m, p2, 0xffffffff;\n\t"
-            "and.b32 r, m, %4;\n\t"
-            "popc.b32 r, r;\n\t"
-            "add.u32 a, a, r;\n\t"
-            "popc.b32 m, m;\n\t"
-            "add.u32 %1, %1, m;\n\t"
-            "add.u32 b, a, 1;\n\t"
-            "and.b32 a, a, %5;\n\t"
-            "and.b32 b, b, %5;\n\t"
-            "or.b32 a, a, %6;\n\t"
-            "or.b32 b, b, %6;\n\t"
-            "@p1 ld.shared.u8 a, [a];\n\t"
-            "@p2 ld.shared.u8 b, [b];\n\t"
-            "@p1 mad.lo.u32 %0, %0, 256, a;\n\t"
-            "@p2 mad.lo.u32 %0, %0, 256, b;\n\t"
-            "}"
-            : "+r"(x), "+r"(cursor)
-            : "n"(kByteL), "n"(kByteL >> 8), "r"(lt), "n"(kRingBytes - 1), "r"(ring)
-            : "memory");
-        return;
-    }
-    const uint32_t m1 = __ballot_sync(0xffffffffu, n1);
-    const uint32_t m2 = __ballot_sync(0xffffffffu, n2);
-    uint32_t a = cursor + __popc(m1 & lt);
-    if (m2) a += __popc(m2 & lt);                                          // warp-uniform: two-byte refills are the rarer case
-    const uint32_t b0 = lds_u8(ring | (a & (kRingBytes - 1)));
-    if (n1) x = (x << 8) | b0;                                             // rans_byte.h:313
-    cursor += __popc(m1);
-    if (m2) {
-        const uint32_t b1 = lds_u8(ring | ((a + 1) & (kRingBytes - 1)));
-        if (n2) x = (x << 8) | b1;
-        cursor += __popc(m2);
-    }
-}
+template <uint32_t SB>
+struct ByteDecoder {
+    using X = uint32_t;
+    static constexpr uint32_t kHeaderBytes = rb200::kHeaderBytes, kUnit = 1, kMaxBytes = 2;
+    static constexpr X kL = kByteL;                    // RansEncInit, rans_byte.h:56-59
+    uint32_t tab;
+    uint32_t sb_rt;
 
-// ALIAS: g_tab = 256 x AliasDecEntry.  !ALIAS: g_tab = cum2sym[1 << sb] followed by 256 x u32 {start | freq << 16}.
-template <bool ALIAS, uint32_t SB>
+    // RansDecInit x 32 (rans_byte.h:109-122): lane k's state is the k-th little-endian u32
+    template <class At>
+    __device__ __forceinline__ X read_header(At at, uint32_t lane) const
+    {
+        uint32_t x = 0;
+#pragma unroll
+        for (int b = 3; b >= 0; b--) x = (x << 8) | lds_u8(at(4 * lane + b));
+        return x;
+    }
+
+    template <bool FULL>
+    __device__ __forceinline__ void step(uint32_t& x, uint32_t& cursor, uint32_t ring, uint8_t* o, uint32_t lt, bool active) const
+    {
+        const uint32_t sb = SB ? SB : sb_rt;
+        bool n1 = false, n2 = false;
+        if (active) {
+            const uint32_t xm = x & ((1u << sb) - 1);                          // rans_byte.h:127
+            const uint32_t s = lds_u8_ro(tab + xm);                            // cum2sym, main.cpp:200
+            const uint32_t ds = lds_u32_ro(tab + (1u << sb) + 4u * s);         // RansDecSymbol {start, freq}
+            x = (ds >> 16) * (x >> sb) + xm - (ds & 0xffffu);                  // rans_byte.h:297
+            *o = static_cast<uint8_t>(s);
+            n1 = x < kByteL;
+            n2 = x < (kByteL >> 8);
+        }
+        if (FULL) {
+            // RansDecRenorm for the warp as one PTX sequence: two predicates feed the votes, the two ranked byte
+            // loads and the state updates (the C++ below costs six more instructions and a branch per step)
+            asm volatile(
+                "{\n\t"
+                ".reg .pred p1, p2;\n\t"
+                ".reg .b32 m, r, a, b;\n\t"
+                "setp.lt.u32 p1, %0, %2;\n\t"
+                "setp.lt.u32 p2, %0, %3;\n\t"
+                "vote.sync.ballot.b32 m, p1, 0xffffffff;\n\t"
+                "and.b32 r, m, %4;\n\t"
+                "popc.b32 r, r;\n\t"
+                "add.u32 a, %1, r;\n\t"
+                "popc.b32 m, m;\n\t"
+                "add.u32 %1, %1, m;\n\t"
+                "vote.sync.ballot.b32 m, p2, 0xffffffff;\n\t"
+                "and.b32 r, m, %4;\n\t"
+                "popc.b32 r, r;\n\t"
+                "add.u32 a, a, r;\n\t"
+                "popc.b32 m, m;\n\t"
+                "add.u32 %1, %1, m;\n\t"
+                "add.u32 b, a, 1;\n\t"
+                "and.b32 a, a, %5;\n\t"
+                "and.b32 b, b, %5;\n\t"
+                "or.b32 a, a, %6;\n\t"
+                "or.b32 b, b, %6;\n\t"
+                "@p1 ld.shared.u8 a, [a];\n\t"
+                "@p2 ld.shared.u8 b, [b];\n\t"
+                "@p1 mad.lo.u32 %0, %0, 256, a;\n\t"
+                "@p2 mad.lo.u32 %0, %0, 256, b;\n\t"
+                "}"
+                : "+r"(x), "+r"(cursor)
+                : "n"(kByteL), "n"(kByteL >> 8), "r"(lt), "n"(kRingBytes - 1), "r"(ring)
+                : "memory");
+            return;
+        }
+        const uint32_t m1 = __ballot_sync(0xffffffffu, n1);
+        const uint32_t m2 = __ballot_sync(0xffffffffu, n2);
+        uint32_t a = cursor + __popc(m1 & lt);
+        if (m2) a += __popc(m2 & lt);                                          // warp-uniform: two-byte refills are the rarer case
+        const uint32_t b0 = lds_u8(ring | (a & (kRingBytes - 1)));
+        if (n1) x = (x << 8) | b0;                                             // rans_byte.h:313
+        cursor += __popc(m1);
+        if (m2) {
+            const uint32_t b1 = lds_u8(ring | ((a + 1) & (kRingBytes - 1)));
+            if (n2) x = (x << 8) | b1;
+            cursor += __popc(m2);
+        }
+}
+};
+
+// g_tab = cum2sym[1 << sb] followed by 256 x u32 {start | freq << 16}
+template <uint32_t SB>
 __global__ void __launch_bounds__(kAliasDecWarps * 32, 4)
-alias_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets, uint32_t sb_rt,
-                    const void* __restrict__ g_tab, uint8_t* __restrict__ out, uint64_t n, uint32_t chunk_syms,
-                    uint32_t n_chunks, uint32_t* __restrict__ status)
+byte_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets, uint32_t sb_rt,
+                   const void* __restrict__ g_tab, uint8_t* __restrict__ out, uint64_t n, uint32_t chunk_syms,
+                   uint32_t n_chunks, uint32_t* __restrict__ status)
 {
     const uint32_t sb = SB ? SB : sb_rt;
     extern __shared__ __align__(1024) uint8_t s_adec[];       // [16 x 1 KiB rings][table]
     uint4* s_tab = reinterpret_cast<uint4*>(s_adec + kAliasDecWarps * kRingBytes);
-    if (ALIAS) {
-        const AliasDecEntry* g_dec = static_cast<const AliasDecEntry*>(g_tab);
-        for (uint32_t i = threadIdx.x; i < 256 * kAliasDecReplicas; i += blockDim.x) {
-            const AliasDecEntry e = g_dec[i / kAliasDecReplicas];
-            s_tab[i] = make_uint4(e.divider, e.alt0, e.alt1, e.adjust);
-        }
-    } else {
-        const uint32_t vecs = ((1u << sb) + 1024) / 16;
-        for (uint32_t i = threadIdx.x; i < vecs; i += blockDim.x) s_tab[i] = static_cast<const uint4*>(g_tab)[i];
-    }
+    const uint32_t vecs = ((1u << sb) + 1024) / 16;
+    for (uint32_t i = threadIdx.x; i < vecs; i += blockDim.x) s_tab[i] = static_cast<const uint4*>(g_tab)[i];
     __syncthreads();
 
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t warp = threadIdx.x >> 5;
     const uint32_t chunk = blockIdx.x * kAliasDecWarps + warp;
     if (chunk >= n_chunks) return;
-
     const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
     const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-    const uint64_t off = offsets[chunk];
-    const uint64_t end = offsets[chunk + 1] & ~static_cast<uint64_t>(15);
-    if (off + kHeaderBytes > end || end > blob_size) {
-        if (lane == 0) atomicOr(status, kStatStream);
-        return;
-    }
-
-    StreamWindow win;
-    win.open(blob, blob_size, off, smem_addr(s_adec) + warp * kRingBytes, lane);
-    uint32_t cursor = static_cast<uint32_t>(off);
-    // RansDecInit x 32 (rans_byte.h:109-122)
-    uint32_t x = 0;
-#pragma unroll
-    for (int b = 3; b >= 0; b--) x = (x << 8) | lds_u8(win.ring | ((cursor + 4 * lane + b) & (kRingBytes - 1)));
-    cursor += kHeaderBytes;
-
-    const uint32_t lt = lanemask_lt();
-    const uint32_t tab_lane = smem_addr_pinned(s_tab) + (ALIAS ? (lane & (kAliasDecReplicas - 1)) * 16 : 0);
-    uint8_t* o = out + first + lane;
-    const uint32_t steps = m >> 5, rem = m & 31;
-    uint32_t g = 0;
-    for (; g + 8 <= steps; g += 8) {
-        win.top_up(cursor, lane);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o, lt, sb, true);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 32, lt, sb, true);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 64, lt, sb, true);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 96, lt, sb, true);
-        win.top_up(cursor, lane);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 128, lt, sb, true);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 160, lt, sb, true);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 192, lt, sb, true);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 224, lt, sb, true);
-        o += 256;
-    }
-    if (g + 4 <= steps) {
-        win.top_up(cursor, lane);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o, lt, sb, true);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 32, lt, sb, true);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 64, lt, sb, true);
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o + 96, lt, sb, true);
-        o += 128;
-        g += 4;
-    }
-    win.top_up(cursor, lane);
-    for (; g < steps; g++) {
-        alias_dec_step<ALIAS, true, SB>(x, cursor, tab_lane, win.ring, o, lt, sb, true);
-        o += 32;
-    }
-    if (rem) alias_dec_step<ALIAS, false, SB>(x, cursor, tab_lane, win.ring, o, lt, sb, lane < rem);
-
-    const bool bad = (cursor != static_cast<uint32_t>(end)) || (x != kByteL);
-    if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(status, kStatStream);
+    decode_window_chunk(ByteDecoder<SB>{smem_addr_pinned(s_tab), sb}, blob, blob_size, offsets, chunk, smem_addr(s_adec) + warp * kRingBytes,
+                        out + first, m, status);
 }
-constexpr uint32_t kAliasDecSmem = kAliasDecWarps * kRingBytes + 256 * kAliasDecReplicas * 16;   // 48 KiB
 
 // ---------------------------------------------------------------------------
-// K3p: the alias decoder on the persistent plumbing of word_decode_tma.cuh -- 2 CTAs of 20 warps per SM stay resident
-// and pull chunk ids from the context's atomic counter; the 32 KiB replicated bucket table is built once per CTA; the
+// K3p: the alias decoder on the persistent window of decode_stream.cuh -- 2 CTAs of 20 warps per SM stay resident and
+// pull chunk ids from the context's atomic counter; the 32 KiB replicated bucket table is built once per CTA; the
 // per-warp stream window is the cp.async ring with a mirror behind it, wrapped once per 8 steps, so the two ranked byte
-// reads of RansDecRenorm need no address masking (round 1's kernel spends 5 of its ~20 ALU-pipe instructions per step
-// on that, and the ALU pipe is what binds it: 85 % busy).  Experiments and ablations: tools/decode_lab.cu --coder alias.
+// reads of RansDecRenorm need no address masking (round 1's kernel spent 5 of its ~20 ALU-pipe instructions per step
+// on that, and the ALU pipe is what bound it: 85 % busy).  Experiments and ablations: tools/decode_lab.cu --coder alias.
 // ---------------------------------------------------------------------------
 using AliasDecShip = DecPolicy<20, 2, 8, kRefillCpAsync, 9, 0, 0, 0, false, 256 * kAliasDecReplicas * 16>;
 
@@ -216,123 +162,125 @@ __device__ __forceinline__ uint4 alias_lean_entry(const AliasDecEntry& e, uint32
     return make_uint4(((own_count - 1u) << K) | adj_own, none ? e.alt0 : e.alt1, e.alt0, e.adjust & 0xffffu);
 }
 
-template <uint32_t SB, int ABL = 0, int LEAN = 0>
-__device__ __forceinline__ void alias_dec_step_p(uint32_t& x, uint32_t& cur, uint32_t tab_lane, uint8_t* o, uint32_t lt, uint32_t sb_rt,
-                                                 bool active)
-{
-    const uint32_t sb = SB ? SB : sb_rt;
-    if (active) {
-        if (LEAN && SB > 8) {
-            constexpr uint32_t LB = SB > 8 ? SB - 8 : 1;
-            // bucket id: byte 1 of x by one PRMT at scale_bits 16, otherwise masked in place and scaled by the IMAD
-            const uint32_t addr = LB == 8 ? mad_u32(__byte_perm(x, 0u, 0x4441u), kAliasDecReplicas * 16, tab_lane)
-                                          : mad_u32(x & (0xffu << LB), (kAliasDecReplicas * 16) >> (LB & 7), tab_lane);
-            const uint4 e = lds_u128_ro(addr);
-            const bool own = mad_u32(x, 1u << (32 - LB), 0u) <= e.x;           // main_alias.cpp:261 on the bucket-local bits
-            const uint32_t fs = own ? e.y : e.z;
-            const uint32_t adj = own ? e.x : e.w;
-            x = mad_u32(fs >> 8, x >> SB, (x - adj) & ((1u << SB) - 1));       // :265
-            if (!(ABL & kAblNoSymbolStore)) *o = static_cast<uint8_t>(fs);     // :266
-        } else {
-            const uint32_t xm = x & ((1u << sb) - 1);                              // main_alias.cpp:258
-            const uint32_t bucket = xm >> (sb - 8);                                // :259
-            const uint4 e = lds_u128_ro(mad_u32(bucket, kAliasDecReplicas * 16, tab_lane));
-            const bool own = xm < e.x;                                             // :261 (bucket2 = 2 * bucket + 1)
-            const uint32_t fs = own ? e.z : e.y;                                   // slot_freqs << 8 | sym_id
-            const uint32_t adj = __byte_perm(e.w, 0u, own ? 0x4432u : 0x4410u);    // the taken half of the packed adjusts
-            x = mad_u32(fs >> 8, x >> sb, (xm - adj) & 0xffffu);                   // :265
-            if (!(ABL & kAblNoSymbolStore)) *o = static_cast<uint8_t>(fs);         // :266
-        }
-    }
-    // RansDecRenorm (rans_byte.h:307-318) for the warp: 0, 1 or 2 bytes per lane, lane k's bytes before lane k+1's,
-    // most significant first.  Two predicates feed the votes, the ranked byte loads and the merges.
-    const uint32_t xr = active ? x : kByteL;
-    uint32_t xo = x;
-    if (ABL & kAblAliasOneByte) {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p1;\n\t"
-            ".reg .b32 m, r, a, b0;\n\t"
-            "setp.lt.u32 p1, %2, %4;\n\t"
-            "vote.sync.ballot.b32 m, p1, 0xffffffff;\n\t"
-            "and.b32 r, m, %3;\n\t"
-            "popc.b32 r, r;\n\t"
-            "add.u32 a, %1, r;\n\t"
-            "popc.b32 m, m;\n\t"
-            "add.u32 %1, %1, m;\n\t"
-            "ld.shared.u8 b0, [a];\n\t"
-            "@p1 mad.lo.u32 %0, %0, 256, b0;\n\t"
-            "}"
-            : "+r"(xo), "+r"(cur)
-            : "r"(xr), "r"(lt), "n"(kByteL));
-    } else if (ABL & kAblNoRingRead) {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p1, p2;\n\t"
-            ".reg .b32 m, r, a, b0;\n\t"
-            "setp.lt.u32 p1, %2, %4;\n\t"
-            "setp.lt.u32 p2, %2, %5;\n\t"
-            "vote.sync.ballot.b32 m, p1, 0xffffffff;\n\t"
-            "and.b32 r, m, %3;\n\t"
-            "popc.b32 r, r;\n\t"
-            "add.u32 a, %1, r;\n\t"
-            "popc.b32 m, m;\n\t"
-            "add.u32 %1, %1, m;\n\t"
-            "vote.sync.ballot.b32 m, p2, 0xffffffff;\n\t"
-            "and.b32 r, m, %3;\n\t"
-            "popc.b32 r, r;\n\t"
-            "add.u32 a, a, r;\n\t"
-            "popc.b32 m, m;\n\t"
-            "add.u32 %1, %1, m;\n\t"
-            "and.b32 b0, a, 255;\n\t"
-            "@p1 mad.lo.u32 %0, %0, 256, b0;\n\t"
-            "@p2 mad.lo.u32 %0, %0, 256, b0;\n\t"
-            "}"
-            : "+r"(xo), "+r"(cur)
-            : "r"(xr), "r"(lt), "n"(kByteL), "n"(kByteL >> 8));
-    } else {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p1, p2;\n\t"
-            ".reg .b32 m, r, a, b0, b1;\n\t"
-            "setp.lt.u32 p1, %2, %4;\n\t"
-            "setp.lt.u32 p2, %2, %5;\n\t"
-            "vote.sync.ballot.b32 m, p1, 0xffffffff;\n\t"
-            "and.b32 r, m, %3;\n\t"
-            "popc.b32 r, r;\n\t"
-            "add.u32 a, %1, r;\n\t"
-            "popc.b32 m, m;\n\t"
-            "add.u32 %1, %1, m;\n\t"
-            "vote.sync.ballot.b32 m, p2, 0xffffffff;\n\t"
-            "and.b32 r, m, %3;\n\t"
-            "popc.b32 r, r;\n\t"
-            "add.u32 a, a, r;\n\t"
-            "popc.b32 m, m;\n\t"
-            "add.u32 %1, %1, m;\n\t"
-            "ld.shared.u8 b0, [a];\n\t"              // unpredicated: ring + mirror make both reads safe for every lane
-            "ld.shared.u8 b1, [a+1];\n\t"
-            "@p1 mad.lo.u32 %0, %0, 256, b0;\n\t"
-            "@p2 mad.lo.u32 %0, %0, 256, b1;\n\t"
-            "}"
-            : "+r"(xo), "+r"(cur)
-            : "r"(xr), "r"(lt), "n"(kByteL), "n"(kByteL >> 8));
-    }
-    x = xo;
-}
+// The alias coder for decode_persistent: RansDecGetAlias (main_alias.cpp:252-267), then RansDecRenorm
+// (rans_byte.h:307-318).  tab_lane = this lane's replica of the 256 x 16 B bucket table.
+template <uint32_t SB, int LEAN = 0>
+struct AliasDecoder {
+    using X = uint32_t;
+    static constexpr uint32_t kHeaderBytes = rb200::kHeaderBytes, kUnit = 1, kMaxBytes = 2;
+    static constexpr X kL = kByteL;
+    uint32_t tab_lane;
+    uint32_t sb_rt;
 
-// kGroup steps: wrap (the mirror absorbed the previous group's overrun), fill check, steps
-template <uint32_t SB, class P, int LEAN>
-__device__ __forceinline__ void alias_dec_group(TmaWindow& win, uint32_t& x, uint32_t ring_end, uint32_t tab_lane, uint8_t* og, uint32_t lt,
-                                                uint32_t lane, uint32_t sb_rt, uint32_t* __restrict__ status)
-{
-    if (win.cur >= ring_end) {
-        win.cur -= P::kRing;
-        win.limit -= P::kRing;
+    template <class At>
+    __device__ __forceinline__ X read_header(At at, uint32_t lane) const
+    {
+        return ByteDecoder<SB>{0, 0}.read_header(at, lane);
     }
-    if (!(P::kAblate & kAblNoRefill) && __any_sync(0xffffffffu, win.cur > win.limit)) tma_advance<P>(win, lane, status);
-#pragma unroll
-    for (int j = 0; j < P::kGroup; j++) alias_dec_step_p<SB, P::kAblate, LEAN>(x, win.cur, tab_lane, og + 32 * j, lt, sb_rt, true);
-}
+
+    template <class P>
+    __device__ __forceinline__ void step_p(uint32_t& x, uint32_t& cur, uint8_t* o, uint32_t lt, uint32_t lane, int j, bool active) const
+    {
+        const uint32_t sb = SB ? SB : sb_rt;
+        if (active) {
+            if (LEAN && SB > 8) {
+                constexpr uint32_t LB = SB > 8 ? SB - 8 : 1;
+                // bucket id: byte 1 of x by one PRMT at scale_bits 16, otherwise masked in place and scaled by the IMAD
+                const uint32_t addr = LB == 8 ? mad_u32(__byte_perm(x, 0u, 0x4441u), kAliasDecReplicas * 16, tab_lane)
+                                              : mad_u32(x & (0xffu << LB), (kAliasDecReplicas * 16) >> (LB & 7), tab_lane);
+                const uint4 e = lds_u128_ro(addr);
+                const bool own = mad_u32(x, 1u << (32 - LB), 0u) <= e.x;           // main_alias.cpp:261 on the bucket-local bits
+                const uint32_t fs = own ? e.y : e.z;
+                const uint32_t adj = own ? e.x : e.w;
+                x = mad_u32(fs >> 8, x >> SB, (x - adj) & ((1u << SB) - 1));       // :265
+                if (!(P::kAblate & kAblNoSymbolStore)) *o = static_cast<uint8_t>(fs);     // :266
+            } else {
+                const uint32_t xm = x & ((1u << sb) - 1);                              // main_alias.cpp:258
+                const uint32_t bucket = xm >> (sb - 8);                                // :259
+                const uint4 e = lds_u128_ro(mad_u32(bucket, kAliasDecReplicas * 16, tab_lane));
+                const bool own = xm < e.x;                                             // :261 (bucket2 = 2 * bucket + 1)
+                const uint32_t fs = own ? e.z : e.y;                                   // slot_freqs << 8 | sym_id
+                const uint32_t adj = __byte_perm(e.w, 0u, own ? 0x4432u : 0x4410u);    // the taken half of the packed adjusts
+                x = mad_u32(fs >> 8, x >> sb, (xm - adj) & 0xffffu);                   // :265
+                if (!(P::kAblate & kAblNoSymbolStore)) *o = static_cast<uint8_t>(fs);         // :266
+            }
+        }
+        // RansDecRenorm (rans_byte.h:307-318) for the warp: 0, 1 or 2 bytes per lane, lane k's bytes before lane k+1's,
+        // most significant first.  Two predicates feed the votes, the ranked byte loads and the merges.
+        const uint32_t xr = active ? x : kByteL;
+        uint32_t xo = x;
+        if (P::kAblate & kAblAliasOneByte) {
+            asm volatile(
+                "{\n\t"
+                ".reg .pred p1;\n\t"
+                ".reg .b32 m, r, a, b0;\n\t"
+                "setp.lt.u32 p1, %2, %4;\n\t"
+                "vote.sync.ballot.b32 m, p1, 0xffffffff;\n\t"
+                "and.b32 r, m, %3;\n\t"
+                "popc.b32 r, r;\n\t"
+                "add.u32 a, %1, r;\n\t"
+                "popc.b32 m, m;\n\t"
+                "add.u32 %1, %1, m;\n\t"
+                "ld.shared.u8 b0, [a];\n\t"
+                "@p1 mad.lo.u32 %0, %0, 256, b0;\n\t"
+                "}"
+                : "+r"(xo), "+r"(cur)
+                : "r"(xr), "r"(lt), "n"(kByteL));
+        } else if (P::kAblate & kAblNoRingRead) {
+            asm volatile(
+                "{\n\t"
+                ".reg .pred p1, p2;\n\t"
+                ".reg .b32 m, r, a, b0;\n\t"
+                "setp.lt.u32 p1, %2, %4;\n\t"
+                "setp.lt.u32 p2, %2, %5;\n\t"
+                "vote.sync.ballot.b32 m, p1, 0xffffffff;\n\t"
+                "and.b32 r, m, %3;\n\t"
+                "popc.b32 r, r;\n\t"
+                "add.u32 a, %1, r;\n\t"
+                "popc.b32 m, m;\n\t"
+                "add.u32 %1, %1, m;\n\t"
+                "vote.sync.ballot.b32 m, p2, 0xffffffff;\n\t"
+                "and.b32 r, m, %3;\n\t"
+                "popc.b32 r, r;\n\t"
+                "add.u32 a, a, r;\n\t"
+                "popc.b32 m, m;\n\t"
+                "add.u32 %1, %1, m;\n\t"
+                "and.b32 b0, a, 255;\n\t"
+                "@p1 mad.lo.u32 %0, %0, 256, b0;\n\t"
+                "@p2 mad.lo.u32 %0, %0, 256, b0;\n\t"
+                "}"
+                : "+r"(xo), "+r"(cur)
+                : "r"(xr), "r"(lt), "n"(kByteL), "n"(kByteL >> 8));
+        } else {
+            asm volatile(
+                "{\n\t"
+                ".reg .pred p1, p2;\n\t"
+                ".reg .b32 m, r, a, b0, b1;\n\t"
+                "setp.lt.u32 p1, %2, %4;\n\t"
+                "setp.lt.u32 p2, %2, %5;\n\t"
+                "vote.sync.ballot.b32 m, p1, 0xffffffff;\n\t"
+                "and.b32 r, m, %3;\n\t"
+                "popc.b32 r, r;\n\t"
+                "add.u32 a, %1, r;\n\t"
+                "popc.b32 m, m;\n\t"
+                "add.u32 %1, %1, m;\n\t"
+                "vote.sync.ballot.b32 m, p2, 0xffffffff;\n\t"
+                "and.b32 r, m, %3;\n\t"
+                "popc.b32 r, r;\n\t"
+                "add.u32 a, a, r;\n\t"
+                "popc.b32 m, m;\n\t"
+                "add.u32 %1, %1, m;\n\t"
+                "ld.shared.u8 b0, [a];\n\t"              // unpredicated: ring + mirror make both reads safe for every lane
+                "ld.shared.u8 b1, [a+1];\n\t"
+                "@p1 mad.lo.u32 %0, %0, 256, b0;\n\t"
+                "@p2 mad.lo.u32 %0, %0, 256, b1;\n\t"
+                "}"
+                : "+r"(xo), "+r"(cur)
+                : "r"(xr), "r"(lt), "n"(kByteL), "n"(kByteL >> 8));
+        }
+        x = xo;
+    }
+};
 
 // P, LEAN: the shipped configuration unless tools/decode_lab.cu instantiates an experiment
 template <uint32_t SB, class P = AliasDecShip, int LEAN = 0>
@@ -341,6 +289,7 @@ alias_decode_persist_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size
                             const AliasDecEntry* __restrict__ g_dec, uint8_t* __restrict__ out, uint64_t n, uint32_t chunk_syms,
                             uint32_t n_chunks, DecodeWork* __restrict__ work, uint32_t* __restrict__ status)
 {
+    static_assert(P::kRefill == kRefillCpAsync, "the ring's mbarriers are not initialised here: cp.async refill only");
     extern __shared__ __align__(1024) uint8_t s_adec[];       // [32 KiB table][16 B][kWarps x (ring, mirror)]
     uint4* s_tab = reinterpret_cast<uint4*>(s_adec);
     for (uint32_t i = threadIdx.x; i < 256 * kAliasDecReplicas; i += blockDim.x) {
@@ -353,85 +302,10 @@ alias_decode_persist_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size
     const uint32_t base = smem_addr_pinned(s_adec);
     const uint32_t warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
     const uint32_t lane = threadIdx.x & 31;
-    const uint32_t tab_lane = base + (lane & (kAliasDecReplicas - 1)) * 16;
-    const uint32_t lt = lanemask_lt();
-    TmaWindow win;
-    win.ring = base + P::kWarpsOff + warp * P::kWarpStride;
-    win.seq_ready = kTmaSeqBase;
-
-    for (;;) {
-        uint32_t chunk = 0;
-        if (lane == 0) chunk = atomicAdd(&work->next_chunk, 1u);
-        chunk = __shfl_sync(0xffffffffu, chunk, 0);
-        if (chunk >= n_chunks) break;
-        const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
-        const uint64_t left = n - first;
-        const uint32_t m = left < chunk_syms ? static_cast<uint32_t>(left) : chunk_syms;
-        const uint64_t off = offsets[chunk];
-        const uint64_t end = offsets[chunk + 1] & ~static_cast<uint64_t>(15);
-        const bool dir_bad = off + kHeaderBytes > end || end > blob_size || end - off > (1u << 30);   // the directory is not trusted
-        if (__shfl_sync(0xffffffffu, dir_bad ? 1u : 0u, 0)) {
-            if (lane == 0) atomicOr(status, kStatStream);
-            continue;
-        }
-        const uint32_t off_in = __shfl_sync(0xffffffffu, static_cast<uint32_t>(off % P::kUnit), 0);
-        const uint32_t len = __shfl_sync(0xffffffffu, static_cast<uint32_t>(end - off), 0);
-        const uint32_t seq0 = win.seq_ready;
-        const uint32_t pos0 = seq0 * P::kUnit + off_in;
-        win.end_pos = pos0 + len;
-        win.src = reinterpret_cast<uint64_t>(blob) + (off - off_in) - static_cast<uint64_t>(seq0) * P::kUnit + lane * 16;
-        win.cur = win.ring + (pos0 & (P::kRing - 1));
-        win.limit = win.cur - off_in - P::kNeed;
-        if (!(P::kAblate & kAblNoRefill)) {
-            tma_issue<P>(win, seq0, lane);
-            asm volatile("cp.async.commit_group;" ::: "memory");
-            while (win.cur > win.limit) tma_advance<P>(win, lane, status);
-        }
-        __syncwarp();
-
-        // RansDecInit x 32 (rans_byte.h:109-122): lane k's state is the k-th little-endian u32; the mirror covers a wrap
-        uint32_t x = 0;
-#pragma unroll
-        for (int b = 3; b >= 0; b--) x = (x << 8) | lds_u8(win.cur + 4 * lane + b);
-        win.cur += kHeaderBytes;
-
-        uint8_t* o = out + first + lane;
-        const uint32_t ring_end = win.ring + P::kRing;
-        uint32_t todo = m >> 5;
-        for (; todo >= P::kGroup; todo -= P::kGroup) {
-            alias_dec_group<SB, P, LEAN>(win, x, ring_end, tab_lane, o, lt, lane, sb_rt, status);
-            o += 32 * P::kGroup;
-        }
-        if (win.cur >= ring_end) {
-            win.cur -= P::kRing;
-            win.limit -= P::kRing;
-        }
-        if (!(P::kAblate & kAblNoRefill) && __any_sync(0xffffffffu, win.cur > win.limit)) tma_advance<P>(win, lane, status);
-        for (; todo; todo--) {
-            alias_dec_step_p<SB, P::kAblate, LEAN>(x, win.cur, tab_lane, o, lt, sb_rt, true);
-            o += 32;
-        }
-        if (m & 31) alias_dec_step_p<SB, P::kAblate, LEAN>(x, win.cur, tab_lane, o, lt, sb_rt, lane < (m & 31));   // main_alias.cpp:399-404
-
-        const uint32_t pos = win.cur + (win.seq_ready * P::kUnit - P::kNeed - win.limit);
-        const bool bad = (pos != pos0 + len) || (x != kByteL);
-        if (!P::kAblate && __any_sync(0xffffffffu, bad) && lane == 0) atomicOr(status, kStatStream);
-        if (!(P::kAblate & kAblNoRefill)) {
-            const uint32_t seq_end = (win.end_pos + P::kUnit - 1) / P::kUnit;
-            asm volatile("cp.async.wait_group 0;" ::: "memory");
-            win.seq_ready = win.seq_ready < seq_end ? win.seq_ready + 1 : seq_end;
-        }
-        __syncwarp();
-    }
-    if (lane == 0) {
-        const uint32_t total = gridDim.x * P::kWarps;
-        if (atomicAdd(&work->warps_done, 1u) == total - 1) {
-            work->next_chunk = 0;
-            work->warps_done = 0;
-        }
-    }
+    const AliasDecoder<SB, LEAN> coder = {base + (lane & (kAliasDecReplicas - 1)) * 16, sb_rt};
+    decode_persistent<P>(coder, base + P::kWarpsOff + warp * P::kWarpStride, blob, blob_size, offsets, out, n, chunk_syms, n_chunks,
+                         work, lane, status);
 }
-
 
 // ---------------------------------------------------------------------------
 // K4: 32-way alias encode.  RansEncPutAlias (main_alias.cpp:241-250) = RansEncRenorm
@@ -611,16 +485,19 @@ alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_s
 // scale_bits the kernels are specialised for (main_alias.cpp:276 uses 16, main.cpp:136 / main64.cpp:136 use 14, the word
 // coder's 12); every other value runs the generic instantiation (SB = 0).
 template <bool ALIAS, uint32_t SB>
-inline void configure_alias_pair()
+inline void configure_alias_encode()
 {
-    const uint32_t dec_smem = ALIAS ? kAliasDecSmem : kAliasDecWarps * kRingBytes + 1024 + (1u << 16);
-    cudaFuncSetAttribute(alias_decode_kernel<ALIAS, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(alias_decode_kernel<ALIAS, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, dec_smem);
     cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          kAliasEncFixedSmem + (ALIAS ? (2u << 16) : 0u));
 }
-// Build switch: 1 ships the repacked ("lean") bucket entry of alias_dec_step_p for the compile-time scale_bits
+template <uint32_t SB>
+inline void configure_byte_decode()
+{
+    cudaFuncSetAttribute(byte_decode_kernel<SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(byte_decode_kernel<SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAliasDecWarps * kRingBytes + 1024 + (1u << 16));
+}
+// Build switch: 1 ships the repacked ("lean") bucket entry of AliasDecoder for the compile-time scale_bits
 // (A/B: tools/decode_lab.cu --coder alias); a runtime scale_bits always takes the plain entry.
 #ifndef RB200_ALIAS_LEAN
 #define RB200_ALIAS_LEAN 1
@@ -636,8 +513,9 @@ inline void configure_alias_persist()
 inline void configure_alias_kernels()
 {
     configure_alias_persist<0>(); configure_alias_persist<16>(); configure_alias_persist<14>(); configure_alias_persist<12>();
-    configure_alias_pair<true, 0>(); configure_alias_pair<true, 16>(); configure_alias_pair<true, 14>(); configure_alias_pair<true, 12>();
-    configure_alias_pair<false, 0>(); configure_alias_pair<false, 16>(); configure_alias_pair<false, 14>(); configure_alias_pair<false, 12>();
+    configure_byte_decode<0>(); configure_byte_decode<16>(); configure_byte_decode<14>(); configure_byte_decode<12>();
+    configure_alias_encode<true, 0>(); configure_alias_encode<true, 16>(); configure_alias_encode<true, 14>(); configure_alias_encode<true, 12>();
+    configure_alias_encode<false, 0>(); configure_alias_encode<false, 16>(); configure_alias_encode<false, 14>(); configure_alias_encode<false, 12>();
 }
 
 #define RB200_ALIAS_SB_DISPATCH(sb, CALL) \
@@ -668,33 +546,25 @@ inline int launch_alias_encode(cudaStream_t stream, uint32_t sms, const uint8_t*
     return 0;
 }
 
-// work != nullptr: the persistent kernel (sms x 2 CTAs of 20 warps, chunk ids from the context's work counter)
-inline int launch_alias_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets, uint32_t sb,
-                               const AliasDecEntry* dec, uint8_t* out, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
-                               uint32_t* status, DecodeWork* work = nullptr, uint32_t sms = 0)
+// the persistent kernel: sms x 2 CTAs of 20 warps, chunk ids from the context's work counter
+inline void launch_alias_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets, uint32_t sb,
+                                const AliasDecEntry* dec, uint8_t* out, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
+                                uint32_t* status, DecodeWork* work, uint32_t sms)
 {
-    if (work) {
-        using P = AliasDecShip;
-        const uint32_t want = (n_chunks + P::kWarps - 1) / P::kWarps, full = sms * P::kMinBlocks;
-        const uint32_t pgrid = want < full ? want : full;
-        RB200_ALIAS_SB_DISPATCH(sb, (alias_decode_persist_kernel<SB, P, kAliasLean><<<pgrid, P::kWarps * 32, P::kSmemBytes, stream>>>(
-            blob, blob_size, offsets, sb, dec, out, n, chunk_syms, n_chunks, work, status)))
-        return 0;
-    }
-    const uint32_t grid = (n_chunks + kAliasDecWarps - 1) / kAliasDecWarps;
-    RB200_ALIAS_SB_DISPATCH(sb, (alias_decode_kernel<true, SB><<<grid, kAliasDecWarps * 32, kAliasDecSmem, stream>>>(
-        blob, blob_size, offsets, sb, dec, out, n, chunk_syms, n_chunks, status)))
-    return 0;
+    using P = AliasDecShip;
+    const uint32_t want = (n_chunks + P::kWarps - 1) / P::kWarps, full = sms * P::kMinBlocks;
+    const uint32_t grid = want < full ? want : full;
+    RB200_ALIAS_SB_DISPATCH(sb, (alias_decode_persist_kernel<SB, P, kAliasLean><<<grid, P::kWarps * 32, P::kSmemBytes, stream>>>(
+        blob, blob_size, offsets, sb, dec, out, n, chunk_syms, n_chunks, work, status)))
 }
 
 // rans_byte cum2sym decode: table = cum2sym[1 << sb] followed by 256 x u32 {start | freq << 16}
-inline int launch_byte_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets, uint32_t sb,
-                              const uint8_t* table, uint8_t* out, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t* status)
+inline void launch_byte_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets, uint32_t sb,
+                               const uint8_t* table, uint8_t* out, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t* status)
 {
     const uint32_t grid = (n_chunks + kAliasDecWarps - 1) / kAliasDecWarps;
-    RB200_ALIAS_SB_DISPATCH(sb, (alias_decode_kernel<false, SB><<<grid, kAliasDecWarps * 32, kAliasDecWarps * kRingBytes + 1024 + (1u << sb), stream>>>(
+    RB200_ALIAS_SB_DISPATCH(sb, (byte_decode_kernel<SB><<<grid, kAliasDecWarps * 32, kAliasDecWarps * kRingBytes + 1024 + (1u << sb), stream>>>(
         blob, blob_size, offsets, sb, table, out, n, chunk_syms, n_chunks, status)))
-    return 0;
 }
 
 }  // namespace rb200

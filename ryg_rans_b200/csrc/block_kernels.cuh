@@ -12,6 +12,7 @@
 #pragma once
 #include "device_utils.cuh"
 #include "tables.h"
+#include "word_decode_tma.cuh"   // WordDecoder
 #include "word_kernels.cuh"
 
 namespace rb200 {
@@ -323,9 +324,9 @@ block_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const 
     uint8_t* dst = out + static_cast<uint64_t>(blockIdx.x) * block_size + static_cast<uint64_t>(warp) * chunk_syms;
     const uint32_t ring = smem_addr(s_dyn) + warp * kRingBytes;
     if (s_flag[1])
-        word_decode_chunk<true>(blob, blob_size, offsets, chunk, smem_addr_pinned(s_tab), ring, dst, chunk_syms, status);
+        decode_window_chunk(WordDecoder<true>{smem_addr_pinned(s_tab), 0}, blob, blob_size, offsets, chunk, ring, dst, chunk_syms, status);
     else
-        word_decode_chunk<false>(blob, blob_size, offsets, chunk, smem_addr_pinned(s_tab), ring, dst, chunk_syms, status);
+        decode_window_chunk(WordDecoder<false>{smem_addr_pinned(s_tab), 0}, blob, blob_size, offsets, chunk, ring, dst, chunk_syms, status);
 }
 
 // The block's encoder table (8x replicated {magic, x_max | shift, start, 4096 - freq}) from its cumulative table in

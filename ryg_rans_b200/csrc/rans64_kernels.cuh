@@ -7,13 +7,14 @@
 //
 // Same mapping as the other coders (one warp = one chunk = one 32-way stream, one ballot per step
 // because a lane moves at most one u32 per step).  This is the "lets the GPU decode streams made by
-// the reference's fastest CPU encoder" row of SURVEY 8(f); it reuses the word coder's stream window and
-// the chunk encoder every coder shares (encode_stream.cuh: symbol stage, output ring, flush), and is not
+// the reference's fastest CPU encoder" row of SURVEY 8(f); it runs on the chunk decoder and encoder every coder
+// shares (decode_stream.cuh: stream window; encode_stream.cuh: symbol stage, output ring, flush), and is not
 // tuned beyond that.  Its encoder is split-only: per-chunk slots, then the tile scan and compaction.
 #pragma once
+#include "decode_stream.cuh"
 #include "device_utils.cuh"
+#include "encode_stream.cuh"
 #include "tables.h"
-#include "word_kernels.cuh"
 
 namespace rb200 {
 
@@ -23,27 +24,43 @@ constexpr int kRans64Warps = 16;
 constexpr uint32_t kRans64DecReplicas = 16;        // an LDS.64 is served 16 lanes at a time: one {start, freq} copy per lane of a half-warp
 constexpr uint32_t kRans64DecSymBytes = 256 * kRans64DecReplicas * 8;      // 32 KiB
 
-// tab = shared address of cum2sym[1 << sb]; syms_lane = this lane's replica of the 256 x {start, freq} table that follows it
-// (16 replicas, entry s of replica r at (s * 16 + r) * 8: the 16 lanes of each LDS.64 phase hit 16 different 8-byte bank
-// groups whatever their symbols are)
-__device__ __forceinline__ void rans64_dec_step(uint64_t& x, uint32_t& cursor, uint32_t tab, uint32_t syms_lane, uint32_t ring, uint8_t* o,
-                                                uint32_t lt, uint32_t sb, bool active)
-{
-    bool need = false;
-    if (active) {
-        const uint32_t cf = static_cast<uint32_t>(x) & ((1u << sb) - 1);               // rans64.h:120
-        const uint32_t s = lds_u8_ro(tab + cf);                                        // main64.cpp:202
-        const uint2 ds = lds_u64_ro(syms_lane + s * (kRans64DecReplicas * 8));         // Rans64DecSymbol {start, freq}
-        x = static_cast<uint64_t>(ds.y) * (x >> sb) + cf - ds.x;                       // rans64.h:297
-        *o = static_cast<uint8_t>(s);
-        need = x < kRans64L;                                                           // :309
+// The rans64 coder for decode_window_chunk.  tab = shared address of cum2sym[1 << sb]; syms_lane = this lane's replica of
+// the 256 x {start, freq} table that follows it (16 replicas, entry s of replica r at (s * 16 + r) * 8: the 16 lanes of
+// each LDS.64 phase hit 16 different 8-byte bank groups whatever their symbols are)
+struct Rans64Decoder {
+    using X = uint64_t;
+    static constexpr uint32_t kHeaderBytes = kRans64HeaderBytes, kUnit = 4, kMaxBytes = 4;
+    static constexpr X kL = kRans64L;                  // Rans64EncInit, rans64.h:65-68
+    uint32_t tab;
+    uint32_t syms_lane;
+    uint32_t sb;
+
+    // Rans64DecInit x 32 (rans64.h:107-115): lane k's state is the k-th u64
+    template <class At>
+    __device__ __forceinline__ X read_header(At at, uint32_t lane) const
+    {
+        return lds_u32(at(8 * lane)) | (static_cast<uint64_t>(lds_u32(at(8 * lane + 4))) << 32);
     }
-    const uint32_t mask = __ballot_sync(0xffffffffu, need);
-    const uint32_t a = cursor + 4u * __popc(mask & lt);
-    const uint32_t w = lds_u32(ring | (a & (kRingBytes - 1)));
-    if (need) x = (x << 32) | w;                                                       // :310
-    cursor += 4u * __popc(mask);
-}
+
+    template <bool FULL>
+    __device__ __forceinline__ void step(uint64_t& x, uint32_t& cursor, uint32_t ring, uint8_t* o, uint32_t lt, bool active) const
+    {
+        bool need = false;
+        if (active) {
+            const uint32_t cf = static_cast<uint32_t>(x) & ((1u << sb) - 1);               // rans64.h:120
+            const uint32_t s = lds_u8_ro(tab + cf);                                        // main64.cpp:202
+            const uint2 ds = lds_u64_ro(syms_lane + s * (kRans64DecReplicas * 8));         // Rans64DecSymbol {start, freq}
+            x = static_cast<uint64_t>(ds.y) * (x >> sb) + cf - ds.x;                       // rans64.h:297
+            *o = static_cast<uint8_t>(s);
+            need = x < kRans64L;                                                           // :309
+        }
+        const uint32_t mask = __ballot_sync(0xffffffffu, need);
+        const uint32_t a = cursor + 4u * __popc(mask & lt);
+        const uint32_t w = lds_u32(ring | (a & (kRingBytes - 1)));
+        if (need) x = (x << 32) | w;                                                       // :310
+        cursor += 4u * __popc(mask);
+    }
+};
 
 __global__ void __launch_bounds__(kRans64Warps * 32, 2)
 rans64_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets, uint32_t sb,
@@ -66,42 +83,9 @@ rans64_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const
     if (chunk >= n_chunks) return;
     const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
     const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-    const uint64_t off = offsets[chunk];
-    const uint64_t end = offsets[chunk + 1] & ~static_cast<uint64_t>(15);
-    if ((off & 3) || off + kRans64HeaderBytes > end || end > blob_size) {
-        if (lane == 0) atomicOr(status, kStatStream);
-        return;
-    }
-
-    StreamWindow win;
-    win.open(blob, blob_size, off, smem_addr(s_r64) + warp * kRingBytes, lane);
-    uint32_t cursor = static_cast<uint32_t>(off);
-    // Rans64DecInit x 32 (rans64.h:107-115)
-    uint64_t x = lds_u32(win.ring | ((cursor + 8 * lane) & (kRingBytes - 1)));
-    x |= static_cast<uint64_t>(lds_u32(win.ring | ((cursor + 8 * lane + 4) & (kRingBytes - 1)))) << 32;
-    cursor += kRans64HeaderBytes;
-
-    const uint32_t lt = lanemask_lt();
     const uint32_t tab = smem_addr(s_tab);
-    const uint32_t syms_lane = tab + (1u << sb) + (lane & (kRans64DecReplicas - 1)) * 8;
-    uint8_t* o = out + first + lane;
-    const uint32_t steps = m >> 5, rem = m & 31;
-    uint32_t g = 0;
-    for (; g + 2 <= steps; g += 2) {                            // <= 128 bytes per step: top up every 2 steps
-        win.top_up(cursor, lane);
-        rans64_dec_step(x, cursor, tab, syms_lane, win.ring, o, lt, sb, true);
-        rans64_dec_step(x, cursor, tab, syms_lane, win.ring, o + 32, lt, sb, true);
-        o += 64;
-    }
-    win.top_up(cursor, lane);
-    if (g < steps) {
-        rans64_dec_step(x, cursor, tab, syms_lane, win.ring, o, lt, sb, true);
-        o += 32;
-    }
-    if (rem) rans64_dec_step(x, cursor, tab, syms_lane, win.ring, o, lt, sb, lane < rem);
-
-    const bool bad = (cursor != static_cast<uint32_t>(end)) || (x != kRans64L);
-    if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(status, kStatStream);
+    const Rans64Decoder coder = {tab, tab + (1u << sb) + (lane & (kRans64DecReplicas - 1)) * 8, sb};
+    decode_window_chunk(coder, blob, blob_size, offsets, chunk, smem_addr(s_r64) + warp * kRingBytes, out + first, m, status);
 }
 
 // The rans64 coder for encode_stream (encode_stream.cuh); wpos is the ring position of the next u32 =

@@ -479,17 +479,6 @@ bool use_fused_encode(uint32_t chunk_syms)
     return chunk_syms >= 4096;
 }
 
-// RB200_DECODE_PATH=classic selects the round-1 decoder (one CTA per 8 chunks, LDG -> STS window) for A/B runs;
-// the default is the persistent kernel of word_decode_tma.cuh (H100, 1 GiB uniform bytes: 1.15 vs 1.20 ms).
-bool use_persistent_decode()
-{
-    static const bool persistent = [] {
-        const char* e = std::getenv("RB200_DECODE_PATH");
-        return !(e && std::strcmp(e, "classic") == 0);
-    }();
-    return persistent;
-}
-
 uint32_t fused_word_grid(rb200_ctx* ctx, uint32_t n_chunks)
 {
     const uint32_t want = (n_chunks + 1 + kEncWarps - 1) / kEncWarps;       // + 1: one warp of the grid is the scanner
@@ -613,24 +602,14 @@ int decode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_blo
     const uint32_t n_chunks = static_cast<uint32_t>(n_chunks_sz);
     if (!n_chunks) return RB200_OK;
     if (model->coder == RB200_CODER_WORD) {
-        if (use_persistent_decode()) {
-            // persistent grid: 2 CTAs of 32 warps per SM, chunks handed out by an atomic counter (word_decode_tma.cuh)
-            const uint32_t want = (n_chunks + DecShip::kWarps - 1) / DecShip::kWarps;
-            const uint32_t full = static_cast<uint32_t>(ctx->sms) * DecShip::kMinBlocks;
-            const uint32_t grid = want < full ? want : full;
-            auto kernel = model->wide ? word_decode_tma_kernel<DecShip, true> : word_decode_tma_kernel<DecShip, false>;
-            kernel<<<grid, DecShip::kWarps * 32, DecShip::kSmemBytes, ctx->stream>>>(d_blob, blob_size, d_offsets, model->d_word_dec, d_out, n,
-                                                                                     chunk_syms, n_chunks, ctx->d_work, ctx->d_status, 0);
-            return check_launch(ctx, "word_decode_tma_kernel");
-        }
-        const uint32_t grid = (n_chunks + kDecWarps - 1) / kDecWarps;
-        if (model->wide)
-            word_decode_kernel<true><<<grid, kDecWarps * 32, 0, ctx->stream>>>(d_blob, blob_size, d_offsets, model->d_word_dec, d_out,
-                                                                                n, chunk_syms, n_chunks, ctx->d_status);
-        else
-            word_decode_kernel<false><<<grid, kDecWarps * 32, 0, ctx->stream>>>(d_blob, blob_size, d_offsets, model->d_word_dec, d_out,
-                                                                                 n, chunk_syms, n_chunks, ctx->d_status);
-        return check_launch(ctx, "word_decode_kernel");
+        // persistent grid: 2 CTAs of 32 warps per SM, chunks handed out by an atomic counter (word_decode_tma.cuh)
+        const uint32_t want = (n_chunks + DecShip::kWarps - 1) / DecShip::kWarps;
+        const uint32_t full = static_cast<uint32_t>(ctx->sms) * DecShip::kMinBlocks;
+        const uint32_t grid = want < full ? want : full;
+        auto kernel = model->wide ? word_decode_tma_kernel<DecShip, true> : word_decode_tma_kernel<DecShip, false>;
+        kernel<<<grid, DecShip::kWarps * 32, DecShip::kSmemBytes, ctx->stream>>>(d_blob, blob_size, d_offsets, model->d_word_dec, d_out, n,
+                                                                                 chunk_syms, n_chunks, ctx->d_work, ctx->d_status, 0);
+        return check_launch(ctx, "word_decode_tma_kernel");
     }
     if (model->coder == RB200_CODER_RANS64) {
         launch_rans64_decode(ctx->stream, d_blob, blob_size, d_offsets, model->scale_bits, model->d_r64_dec, d_out, n, chunk_syms,
@@ -642,11 +621,9 @@ int decode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_blo
                            n_chunks, ctx->d_status);
         return check_launch(ctx, "byte_decode_kernel");
     }
-    int rc = launch_alias_decode(ctx->stream, d_blob, blob_size, d_offsets, model->scale_bits, model->d_alias_dec, d_out, n,
-                                 chunk_syms, n_chunks, ctx->d_status, use_persistent_decode() ? ctx->d_work : nullptr,
-                                 static_cast<uint32_t>(ctx->sms));
-    if (rc == RB200_OK) rc = check_launch(ctx, "alias_decode_kernel");
-    return rc;
+    launch_alias_decode(ctx->stream, d_blob, blob_size, d_offsets, model->scale_bits, model->d_alias_dec, d_out, n, chunk_syms, n_chunks,
+                        ctx->d_status, ctx->d_work, static_cast<uint32_t>(ctx->sms));
+    return check_launch(ctx, "alias_decode_persist_kernel");
 }
 
 }  // namespace

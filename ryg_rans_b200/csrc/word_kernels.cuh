@@ -21,189 +21,6 @@ constexpr uint32_t kWordScaleBits = 12;     // RANS_WORD_SCALE_BITS, :37
 constexpr uint32_t kWordSlots = 1u << kWordScaleBits;
 
 // ---------------------------------------------------------------------------
-// Per-warp stream window: a 1 KiB shared-memory ring over the compressed stream,
-// refilled 512 B at a time with one coalesced 128-bit load per lane.  The load for
-// the next unit is issued one refill ahead and parked in registers, so its HBM
-// latency is hidden behind >= 8 decode steps.  The cursor never leaves the ring,
-// which also bounds every read a corrupt stream could cause.
-// ---------------------------------------------------------------------------
-constexpr uint32_t kRingBytes = 1024;
-constexpr uint32_t kUnitBytes = 512;
-
-struct StreamWindow {
-    uint32_t ring;          // shared-space address of this warp's ring, 1 KiB aligned
-    uint32_t fill_end;      // low 32 bits of the absolute blob byte offset filled so far
-    uint32_t next_vec;      // this lane's 16-byte vector of the next unit to fetch (index into the blob)
-    uint32_t limit_vec;     // blob_size / 16 (the C-ABI rejects blobs of 64 GiB and more)
-    const uint4* base;      // blob, warp-uniform
-    uint4 parked;           // unit in flight
-
-    // Past the end of the blob the last vector is fetched again instead: what lies beyond a stream's
-    // own end is never consumed by a valid stream, and a corrupt one may read any in-bounds bytes.
-    __device__ __forceinline__ uint4 fetch()
-    {
-        const uint4 v = ldg_stream_u128(base + min(next_vec, limit_vec - 1));
-        next_vec += 32;
-        return v;
-    }
-
-    // off = absolute byte offset of the stream start inside the blob
-    __device__ __forceinline__ void open(const uint8_t* blob, uint64_t blob_size, uint64_t off, uint32_t ring_addr, uint32_t lane)
-    {
-        ring = ring_addr;
-        base = reinterpret_cast<const uint4*>(blob);
-        const uint32_t unit0 = static_cast<uint32_t>(off / kUnitBytes);
-        next_vec = unit0 * 32 + lane;
-        limit_vec = static_cast<uint32_t>(blob_size / 16);
-        uint4 a = fetch();
-        uint4 b = fetch();
-        parked = fetch();
-        sts_u128(ring + ((unit0 & 1) * kUnitBytes) + lane * 16, a);
-        sts_u128(ring + (((unit0 + 1) & 1) * kUnitBytes) + lane * 16, b);
-        fill_end = (unit0 + 2) * kUnitBytes;
-        __syncwarp();
-    }
-
-    // Call before every group of steps that consumes at most 256 bytes.
-    __device__ __forceinline__ void top_up(uint32_t cursor, uint32_t lane)
-    {
-        if (fill_end - cursor <= kUnitBytes) {          // warp-uniform
-            __syncwarp();
-            sts_u128(ring + (fill_end & kUnitBytes) + lane * 16, parked);
-            fill_end += kUnitBytes;
-            parked = fetch();
-            __syncwarp();
-        }
-    }
-};
-
-// ---------------------------------------------------------------------------
-// K1: 32-way word-coder decode
-// ---------------------------------------------------------------------------
-constexpr int kDecWarps = 8;
-
-template <bool WIDE>
-__device__ __forceinline__ uint32_t word_table_freq(uint32_t e)
-{
-    uint32_t f = e >> 20;
-    if (WIDE) f = f ? f : kWordSlots;   // single-symbol model: freq 4096 stored as 0
-    return f;
-}
-
-// one decode step for the whole warp: RansWordDecSym + RansWordDecRenorm
-__device__ __forceinline__ uint32_t mad_u32(uint32_t a, uint32_t b, uint32_t c)
-{
-    uint32_t d;
-    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-    return d;
-}
-
-// one decode step for the whole warp: RansWordDecSym + RansWordDecRenorm.
-// tab = shared-space address of the packed table (kept live in a register by the caller).
-template <bool WIDE>
-__device__ __forceinline__ void word_dec_step(uint32_t& x, uint32_t& cursor, uint32_t tab, uint32_t ring,
-                                              uint8_t* o, uint32_t lt, bool active)
-{
-    bool need = false;
-    if (active) {
-        const uint32_t e = lds_u32_ro(mad_u32(x & (kWordSlots - 1), 4u, tab));  // rans_word_sse41.h:126
-        x = word_table_freq<WIDE>(e) * (x >> kWordScaleBits) + ((e >> 8) & 0xfffu);   // :129
-        *o = static_cast<uint8_t>(e);                                       // :130
-        need = x < kWordL;                                                  // :137
-    }
-    const uint32_t mask = __ballot_sync(0xffffffffu, need);
-    const uint32_t a = mad_u32(__popc(mask & lt), 2u, cursor);              // lane order within the step
-    const uint32_t w = lds_u16(ring | (a & (kRingBytes - 1)));
-    if (need) x = (x << 16) | w;                                            // :138
-    cursor = mad_u32(__popc(mask), 2u, cursor);                             // :139
-}
-
-// Decode chunk `chunk` (one warp).  tab = shared address of the 4096-entry packed table,
-// ring = shared address of this warp's 1 KiB stream window.
-template <bool WIDE>
-__device__ __forceinline__ void word_decode_chunk(const uint8_t* __restrict__ blob, uint64_t blob_size,
-                                                  const uint64_t* __restrict__ offsets, uint32_t chunk, uint32_t tab,
-                                                  uint32_t ring, uint8_t* __restrict__ chunk_out, uint32_t m,
-                                                  uint32_t* __restrict__ status)
-{
-    const uint32_t lane = threadIdx.x & 31;
-    const uint64_t off = offsets[chunk];
-    const uint64_t end = offsets[chunk + 1] & ~static_cast<uint64_t>(15);
-    if ((off & 1) || off + kHeaderBytes > end || end > blob_size) {      // directory is not trusted
-        if (lane == 0) atomicOr(status, kStatStream);
-        return;
-    }
-
-    StreamWindow win;
-    win.open(blob, blob_size, off, ring, lane);
-    uint32_t cursor = static_cast<uint32_t>(off);
-    // RansWordDecInit x 32 (rans_word_sse41.h:109-120): lane k's state is the k-th u32
-    uint32_t x = lds_u16(win.ring | ((cursor + 4 * lane) & (kRingBytes - 1)))
-               | (lds_u16(win.ring | ((cursor + 4 * lane + 2) & (kRingBytes - 1))) << 16);
-    cursor += kHeaderBytes;
-
-    const uint32_t lt = lanemask_lt();
-    uint8_t* o = chunk_out + lane;
-    const uint32_t steps = m >> 5, rem = m & 31;
-    uint32_t g = 0;
-    for (; g + 8 <= steps; g += 8) {
-        win.top_up(cursor, lane);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o, lt, true);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 32, lt, true);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 64, lt, true);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 96, lt, true);
-        win.top_up(cursor, lane);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 128, lt, true);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 160, lt, true);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 192, lt, true);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 224, lt, true);
-        o += 256;
-    }
-    if (g + 4 <= steps) {
-        win.top_up(cursor, lane);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o, lt, true);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 32, lt, true);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 64, lt, true);
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o + 96, lt, true);
-        o += 128;
-        g += 4;
-    }
-    win.top_up(cursor, lane);
-    for (; g < steps; g++) {
-        word_dec_step<WIDE>(x, cursor, tab, win.ring, o, lt, true);
-        o += 32;
-    }
-    if (rem) word_dec_step<WIDE>(x, cursor, tab, win.ring, o, lt, lane < rem);   // main_simd.cpp:328-332
-
-    // A valid stream is consumed exactly to its (aligned) end and leaves every lane
-    // in the encoder's initial state.
-    const bool bad = (cursor != static_cast<uint32_t>(end)) || (x != kWordL);
-    if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(status, kStatStream);
-}
-
-template <bool WIDE>
-__global__ void __launch_bounds__(kDecWarps * 32, 8)
-word_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets,
-                   const uint32_t* __restrict__ g_table,   // 4096 packed slots, one model for the whole buffer
-                   uint8_t* __restrict__ out, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
-                   uint32_t* __restrict__ status)
-{
-    __shared__ __align__(16) uint32_t s_tab[kWordSlots];
-    __shared__ __align__(1024) uint8_t s_ring[kDecWarps][kRingBytes];
-
-    for (uint32_t i = threadIdx.x; i < kWordSlots / 4; i += blockDim.x)
-        reinterpret_cast<uint4*>(s_tab)[i] = reinterpret_cast<const uint4*>(g_table)[i];
-    __syncthreads();
-
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint32_t chunk = blockIdx.x * kDecWarps + warp;
-    if (chunk >= n_chunks) return;
-    const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
-    const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-    word_decode_chunk<WIDE>(blob, blob_size, offsets, chunk, smem_addr_pinned(s_tab), smem_addr(&s_ring[warp][0]), out + first, m, status);
-}
-
-// ---------------------------------------------------------------------------
 // K2: 32-way word-coder encode into per-chunk worst-case slots of a scratch buffer
 // (stage, ring and flush: encode_stream.cuh; the word coder's step: WordEncoder below)
 // ---------------------------------------------------------------------------
@@ -522,8 +339,6 @@ compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const u
 
 inline void configure_word_kernels()
 {
-    cudaFuncSetAttribute(word_decode_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_decode_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(word_encode_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(word_encode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
     cudaFuncSetAttribute(word_encode_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);

@@ -449,12 +449,11 @@ print("fused ok", ctx.launches)
     assert out.returncode == 0 and "fused ok" in out.stdout, out.stderr[-2000:]
 
 
-@pytest.mark.parametrize("path", ["classic", "persistent"])
+@pytest.mark.parametrize("path", ["persistent"])   # one decoder per coder now; the parameter keeps the test id
 def test_forced_decode_paths(cuda_box, path):
-    """Both word decoders (RB200_DECODE_PATH=classic: one CTA per 8 chunks, LDG -> STS window; default: persistent grid,
-    TMA-staged table, cp.async ring, word_decode_tma.cuh) must decode oracle containers bit-exactly at every chunk size,
-    ragged tails and the single-symbol (freq 4096) model included, report corruption, and stay usable afterwards (the
-    persistent decoder's work counter re-arms itself)."""
+    """The word decoder (persistent grid, TMA-staged table, cp.async ring, word_decode_tma.cuh) must decode oracle
+    containers bit-exactly at every chunk size, ragged tails and the single-symbol (freq 4096) model included, report
+    corruption, and stay usable afterwards (its work counter re-arms itself)."""
     import os
     import subprocess
     import sys
@@ -490,8 +489,7 @@ for n in (1, 31, 32, 33, 4097, 1_000_003, 3_000_017):
         m.close()
 print("decode paths ok", ctx.launches)
 ''' % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, RB200_DECODE_PATH=path)
-    out = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=600)
+    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
     assert out.returncode == 0, out.stdout + out.stderr
     assert "decode paths ok" in out.stdout
 

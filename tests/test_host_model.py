@@ -232,7 +232,7 @@ def _alias_step_plain(x, sb, divider, slot_adjust, slot_freqs, sym_id):
 
 
 def _alias_step_lean(x, sb, divider, slot_adjust, slot_freqs, sym_id):
-    """The repacked entry of alias_kernels.cuh (alias_lean_entry / alias_dec_step_p<SB, ABL, LEAN = 1>): the own
+    """The repacked entry of alias_kernels.cuh (alias_lean_entry / AliasDecoder<SB, LEAN = 1>::step_p): the own
     count sits at the top of word 0 above the own adjust, the comparison is made on x << (40 - sb)."""
     lb, k = sb - 8, 40 - sb
     bucket = np.arange(256, dtype=np.uint32)

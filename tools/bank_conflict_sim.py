@@ -2,7 +2,7 @@
 """How many shared-memory wavefronts does the decode table gather of one warp cost, for different table layouts?
 
 The decode step's gather (`tab[x & 4095]`, 4-byte entries, 32 lanes with independent pseudo-random slots) is the
-largest term of the LSU budget that bounds `word_decode_kernel` (DESIGN.md section 6).  A wavefront serves one
+largest term of the LSU budget that bounds the round-1 word decode step (DESIGN.md section 6).  A wavefront serves one
 4-byte word per bank (32 banks); lanes reading the SAME word are a broadcast.  The cost of one LDS is the largest
 number of distinct words any bank has to deliver.  This Monte-Carlo compares candidate layouts; ncu
 measured ~3.7 wavefronts per gather for the shipped layout (1 + 2.76 replays per step), the first row's 3.5 is the

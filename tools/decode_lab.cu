@@ -376,18 +376,6 @@ int main(int argc, char** argv)
                 (unsigned long long)n, chunk, dist.c_str(), (unsigned long long)blob_size, sms, peak);
 
     std::vector<Variant> vs;
-    {
-        Variant v;
-        v.name = "r1_kernel";
-        v.verify = true;
-        v.note = "round-1 word_decode_kernel: 8 warps per CTA, one CTA per 8 chunks, LDG+STS ring";
-        v.launch = [](const Bench& b) {
-            const uint32_t grid = (b.n_chunks + kDecWarps - 1) / kDecWarps;
-            word_decode_kernel<false><<<grid, kDecWarps * 32>>>(b.blob, b.blob_size, b.offsets, b.table, b.out, b.n, b.chunk, b.n_chunks,
-                                                                  b.status);
-        };
-        vs.push_back(v);
-    }
     //                       warps, CTAs/SM, group, refill, log2(unit), wide-mul (1 state, 2 entry), tex-every, ablate, iadd3
     using Ship = DecShip;
     using Tma512 = DecPolicy<32, 2, 8, kRefillTma, 9, 2>;

@@ -41,7 +41,7 @@ def step_between(instrs, opcode, skip, max_len=60):
 def main():
     lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "ryg_rans_b200", "librans_b200.so")
     fns = functions(subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout)
-    dec = next(v for k, v in fns.items() if "word_decode_kernelILb0" in k)
+    dec = next(v for k, v in fns.items() if "block_decode_kernel" in k)
     enc = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1" in k)
     tma = next(v for k, v in fns.items() if "word_decode_tma_kernel" in k and k.endswith("Lb0EEEvPKhmPKmPKjPhmjjPNS_10DecodeWorkEPjy"))
     ali = next(v for k, v in fns.items() if "alias_decode_persist_kernelILj16E" in k)
@@ -49,7 +49,7 @@ def main():
                          step_between(tma, "STG.E.U8", 2)),
                         ("alias_decode_persist_kernel<16> (round 2, shipped): one step (symbol store to symbol store)",
                          step_between(ali, "STG.E.U8", 2)),
-                        ("word_decode_kernel<false> (round 1; still inside the per-block decoder): one step (vote to vote)",
+                        ("block_decode_kernel (round 1 window: decode_window_chunk with WordDecoder<false>): one step (vote to vote)",
                          step_between(dec, "VOTE.ANY", 5)),
                         ("word_encode_fused_kernel<R32>: one step (symbol load to symbol load)", step_between(enc, "LDS.U8", 8))):
         print("## %s: %d instructions" % (title, len(step)))
