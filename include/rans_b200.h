@@ -177,6 +177,50 @@ int rb200_blocks_model_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_bloc
                               uint16_t* block_freqs, uint32_t chunk_syms,
                               uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind);
 
+/* Per-block containers: the self-describing container (below) at version 2, holding every block's model.
+ *
+ *   [ 64-byte header ][ block_freqs: n_blocks x 256 x u16 ][ offsets: (n_chunks + 1) x u64 ][ pad to 16 ][ blob ]
+ *
+ * The header is version 1's with version = 2, the word coder, scale_bits 12, 32 lanes, block_size in the u32 at
+ * byte 52, n_blocks in the u32 at byte 56 and a zero u32 at byte 60; meta_crc covers header, block_freqs and offsets.
+ * The directory starts at 64 + 512 n_blocks.  rb200_container_blocks_open rejects with RB200_E_STREAM anything
+ * rb200_blocks_decode would not take (geometry as above, n_blocks >= 1, n_symbols == n_blocks * block_size,
+ * n_chunks == n_symbols / chunk_syms < 2^31), sections that do not fit `size`, a nonzero byte-60 word, an unknown
+ * flag, a CRC mismatch, a block whose frequencies do not sum to 4096, and a directory that breaks version 1's rules.
+ * rb200_container_open / _decode accept only version 1 and these calls only version 2.
+ *
+ * pack: host only; RB200_E_MODEL for a block that does not sum to 4096, RB200_E_ARG for bad geometry or a directory
+ * that disagrees with the blob.  open: as rb200_container_open (pointers INTO buf, which must be 8-byte aligned). */
+typedef struct rb200_container_blocks_info {
+    uint32_t n_blocks, block_size, chunk_syms, flags;
+    uint64_t n_symbols, n_chunks, blob_bytes;
+    const uint16_t* block_freqs;    /* n_blocks x 256 */
+    const uint64_t* offsets;        /* n_chunks + 1 */
+    const uint8_t* blob;
+} rb200_container_blocks_info;
+
+size_t rb200_container_blocks_size(uint32_t n_blocks, size_t n_chunks, size_t blob_bytes);
+int rb200_container_blocks_pack(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, const uint16_t* block_freqs,
+                                const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes, uint32_t flags,
+                                uint8_t* out, size_t out_cap, size_t* out_size);
+int rb200_container_blocks_open(const uint8_t* buf, size_t size, rb200_container_blocks_info* info);
+/* rb200_blocks_model_encode (block_freqs == NULL: every block's model is built on the GPU and written straight into
+ * the container's model section) or rb200_blocks_encode (the caller's tables, in host or device memory as mem_kind)
+ * + rb200_container_blocks_pack in one call, with the rules of rb200_container_encode: out 16-byte aligned (DEVICE)
+ * or 8-byte aligned (HOST); out_cap below header, model and directory is RB200_E_SPACE from the call; a blob past
+ * out_cap is RB200_E_SPACE from the call (HOST) or from rb200_sync (DEVICE, header then unwritten);
+ * rb200_container_blocks_size(n_blocks, n_chunks, rb200_encode_bound(n, chunk_syms)) always suffices.  A caller table
+ * that does not sum to 4096 is RB200_E_MODEL from the call in HOST mode; in DEVICE mode the block encoder codes such
+ * a block with an empty model, so rb200_sync returns RB200_E_SYMBOL and the header is not written. */
+int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                                  const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags,
+                                  uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind);
+/* rb200_container_blocks_open + rb200_blocks_decode in one call, with the rules of rb200_container_decode: *n_symbols
+ * written and out_cap < n RB200_E_SPACE before any decoding; DEVICE mode checks both CRCs on the GPU before any
+ * decode kernel runs (a rejected container leaves out untouched); HOST mode takes the blob CRC per slice. */
+int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                  uint64_t* n_symbols, int mem_kind);
+
 /* ---------------------------------------------------------------- multi-GPU: gathering the shards' blobs (NCCL) */
 
 /* Shards are independent (SURVEY 8e): every rank encodes / decodes its own contiguous range of symbols with no

@@ -47,6 +47,13 @@ EXPORTS = [
                                             C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t), C.c_int]),
     ("rb200_blocks_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
                                       C.c_uint32, C.c_void_p, C.c_int]),
+    ("rb200_container_blocks_size", C.c_size_t, [C.c_uint32, C.c_size_t, C.c_size_t]),
+    ("rb200_container_blocks_pack", C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                              C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("rb200_container_blocks_open", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_container_blocks_encode", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32,
+                                                C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int]),
+    ("rb200_container_blocks_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -97,6 +104,43 @@ def container_open(buf):
     offsets = buf[o_off:o_off + 8 * (info.n_chunks + 1)].view(np.uint64)
     blob = buf[b_off:b_off + info.blob_bytes]
     meta = {k: int(getattr(info, k)) for k in ("coder", "scale_bits", "chunk_syms", "flags", "n_symbols", "n_chunks", "blob_bytes")}
+    return meta, freqs, offsets, blob
+
+
+class ContainerBlocksInfo(C.Structure):
+    _fields_ = [("n_blocks", C.c_uint32), ("block_size", C.c_uint32), ("chunk_syms", C.c_uint32), ("flags", C.c_uint32),
+                ("n_symbols", C.c_uint64), ("n_chunks", C.c_uint64), ("blob_bytes", C.c_uint64),
+                ("block_freqs", _u16p), ("offsets", _u64p), ("blob", _u8p)]
+
+
+def container_blocks_pack(n_blocks, block_size, chunk_syms, block_freqs, offsets, blob, flags=0):
+    """rb200_container_blocks_pack: a per-block (version 2) container from the per-block calls' three arrays"""
+    lib = load()
+    block_freqs = np.ascontiguousarray(block_freqs, dtype=np.uint16)
+    offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+    blob = np.ascontiguousarray(blob, dtype=np.uint8)
+    total = int(lib.dll.rb200_container_blocks_size(n_blocks, offsets.size - 1, blob.size))
+    out = np.zeros(total, np.uint8)
+    size = C.c_size_t(0)
+    lib.check(lib.dll.rb200_container_blocks_pack(n_blocks, block_size, chunk_syms, block_freqs.ctypes.data, offsets.ctypes.data,
+                                                  blob.ctypes.data, blob.size, flags, out.ctypes.data, total, C.byref(size)))
+    return out[:size.value]
+
+
+def container_blocks_open(buf):
+    """Returns (info dict, block_freqs [n_blocks, 256], offsets, blob) as numpy views into buf."""
+    lib = load()
+    buf = np.ascontiguousarray(buf, dtype=np.uint8)
+    info = ContainerBlocksInfo()
+    lib.check(lib.dll.rb200_container_blocks_open(buf.ctypes.data, buf.size, C.byref(info)))
+    base = buf.ctypes.data
+    f_off = C.addressof(info.block_freqs.contents) - base
+    o_off = C.addressof(info.offsets.contents) - base
+    b_off = (C.addressof(info.blob.contents) - base) if info.blob_bytes else buf.size
+    freqs = buf[f_off:f_off + 512 * info.n_blocks].view(np.uint16).reshape(info.n_blocks, 256)
+    offsets = buf[o_off:o_off + 8 * (info.n_chunks + 1)].view(np.uint64)
+    blob = buf[b_off:b_off + info.blob_bytes]
+    meta = {k: int(getattr(info, k)) for k in ("n_blocks", "block_size", "chunk_syms", "flags", "n_symbols", "n_chunks", "blob_bytes")}
     return meta, freqs, offsets, blob
 
 
@@ -311,6 +355,50 @@ class Context:
         """synchronous; returns the container's n"""
         n = C.c_uint64(0)
         self.lib.check(self.lib.dll.rb200_container_decode(self.h, buf_ptr, size, out_ptr, out_cap, C.byref(n), MEM_DEVICE), self.h)
+        return n.value
+
+    # ---- per-block containers (version 2): every block's model, the directory and the blob in one buffer
+    def container_blocks_capacity(self, n_blocks, block_size, chunk_syms):
+        """bytes that always hold rb200_container_blocks_encode's output"""
+        n = n_blocks * block_size
+        return int(self.lib.dll.rb200_container_blocks_size(n_blocks, n // chunk_syms, self.encode_bound(n, chunk_syms)))
+
+    def container_blocks_encode_host(self, data, n_blocks, block_size, chunk_syms, block_freqs=None, flags=0, out_cap=None):
+        """block_freqs None: the models are built on the GPU; else the caller's [n_blocks, 256] u16 tables"""
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        freqs = None if block_freqs is None else np.ascontiguousarray(block_freqs, dtype=np.uint16)
+        cap = self.container_blocks_capacity(n_blocks, block_size, chunk_syms) if out_cap is None else out_cap
+        out = np.zeros(max(cap, 16), np.uint8)
+        size = C.c_size_t(0)
+        self.lib.check(self.lib.dll.rb200_container_blocks_encode(self.h, _np_ptr(data), n_blocks, block_size,
+                                                                  None if freqs is None else _np_ptr(freqs), chunk_syms, flags,
+                                                                  _np_ptr(out), cap, C.byref(size), MEM_HOST), self.h)
+        return out[:size.value].copy()
+
+    def container_blocks_encode_device(self, in_ptr, n_blocks, block_size, freqs_ptr, chunk_syms, flags, out_ptr, out_cap):
+        """asynchronous; freqs_ptr None builds the models; errors come from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_blocks_encode(self.h, in_ptr, n_blocks, block_size, freqs_ptr, chunk_syms, flags,
+                                                                  out_ptr, out_cap, None, MEM_DEVICE), self.h)
+
+    def container_blocks_decode_host(self, buf, out_cap=None):
+        """returns the decoded symbols; out_cap defaults to the container's n"""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        n = C.c_uint64(0)
+        if out_cap is None:
+            rc = self.lib.dll.rb200_container_blocks_decode(self.h, _np_ptr(buf), buf.size, None, 0, C.byref(n), MEM_HOST)
+            if rc not in (0, -3):
+                self.lib.check(rc, self.h)
+            out_cap = n.value
+        out = np.zeros(max(out_cap, 1), np.uint8)
+        self.lib.check(self.lib.dll.rb200_container_blocks_decode(self.h, _np_ptr(buf), buf.size, _np_ptr(out), out_cap, C.byref(n),
+                                                                  MEM_HOST), self.h)
+        return out[:n.value]
+
+    def container_blocks_decode_device(self, buf_ptr, size, out_ptr, out_cap):
+        """synchronous; returns the container's n"""
+        n = C.c_uint64(0)
+        self.lib.check(self.lib.dll.rb200_container_blocks_decode(self.h, buf_ptr, size, out_ptr, out_cap, C.byref(n), MEM_DEVICE),
+                       self.h)
         return n.value
 
     # ---- per-block models, device pointers (asynchronous)

@@ -1,5 +1,5 @@
 // container_format.h -- the layout of the self-describing container (container_host.cpp has the format comment) and
-// the one parser both rb200_container_open and rb200_container_decode go through.  Internal to the library.
+// the one parser every container call goes through.  Internal to the library.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -9,7 +9,8 @@
 namespace rb200 {
 
 constexpr uint32_t kContainerMagic = 0x43324252u;   // "RB2C"
-constexpr uint16_t kContainerVersion = 1;
+constexpr uint16_t kContainerVersion = 1;           // one model: 256 x u32
+constexpr uint16_t kContainerVersionBlocks = 2;     // one model per block: n_blocks x 256 x u16, word coder
 
 struct ContainerHeader {        // 64 bytes
     uint32_t magic;
@@ -22,36 +23,70 @@ struct ContainerHeader {        // 64 bytes
     uint64_t n_chunks;
     uint64_t blob_bytes;
     uint32_t flags;
-    uint32_t meta_crc;          // header (crc fields zero) + freqs + offsets
+    uint32_t meta_crc;          // header (crc fields zero) + model + offsets
     uint32_t blob_crc;          // valid when flags & RB200_CONTAINER_CRC_BLOB
-    uint32_t reserved[3];
+    uint32_t block_size;        // version 2: symbols per block (version 1: zero, not checked)
+    uint32_t n_blocks;          // version 2: blocks, >= 1 (version 1: zero, not checked)
+    uint32_t reserved;          // version 2: zero
 };
 static_assert(sizeof(ContainerHeader) == 64, "container header must stay 64 bytes");
 
-constexpr size_t kContainerDirOffset = sizeof(ContainerHeader) + 256 * sizeof(uint32_t);   // 1088, 16-aligned
+constexpr size_t kContainerDirOffset = sizeof(ContainerHeader) + 256 * sizeof(uint32_t);   // version 1: 1088, 16-aligned
+constexpr size_t kBlockModelBytes = 256 * sizeof(uint16_t);                                 // one block's frequencies
 
-inline size_t container_blob_offset(uint64_t n_chunks)
+// The layout, as functions of the (parsed) header: model section, directory, pad to 16, blob.  Version 1 keeps 1024
+// bytes of model, so its directory stays at 1088; version 2 has 512 bytes per block, so its directory starts at
+// 64 + 512 n_blocks, also 16-aligned.  64-bit throughout: n_blocks < 2^32 and n_chunks < 2^31 once parsed.
+inline uint64_t container_model_bytes(const ContainerHeader& h)
 {
-    return (kContainerDirOffset + (n_chunks + 1) * sizeof(uint64_t) + 15) & ~static_cast<size_t>(15);
+    return h.version == kContainerVersionBlocks ? kBlockModelBytes * h.n_blocks : 256 * sizeof(uint32_t);
+}
+inline uint64_t container_dir_offset(const ContainerHeader& h) { return sizeof(ContainerHeader) + container_model_bytes(h); }
+inline uint64_t container_dir_end(const ContainerHeader& h) { return container_dir_offset(h) + (h.n_chunks + 1) * sizeof(uint64_t); }
+inline uint64_t container_blob_offset(const ContainerHeader& h) { return (container_dir_end(h) + 15) & ~15ull; }
+
+// a header with only what the layout depends on: for sizes computed before there is a header
+inline ContainerHeader container_shape(uint16_t version, uint32_t n_blocks, uint64_t n_chunks)
+{
+    ContainerHeader h{};
+    h.version = version;
+    h.n_blocks = n_blocks;
+    h.n_chunks = n_chunks;
+    return h;
+}
+
+// the chunk sizes the kernels take (32 .. 2^24 symbols)
+inline bool container_chunk_ok(uint32_t chunk_syms) { return chunk_syms >= 32 && chunk_syms <= (1u << 24); }
+// per-block geometry: whole chunks per block, at most 32 (one CTA per block, one warp per chunk)
+inline bool container_blocks_geometry_ok(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms)
+{
+    return n_blocks && block_size && container_chunk_ok(chunk_syms) && block_size % chunk_syms == 0 && block_size / chunk_syms <= 32;
 }
 
 // the header rb200_container_pack writes (crc fields zero)
 ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_syms, uint64_t n, uint64_t n_chunks,
                                  uint64_t blob_bytes, uint32_t flags);
+// the header rb200_container_blocks_pack writes (crc fields zero)
+ContainerHeader container_blocks_header(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint64_t blob_bytes, uint32_t flags);
 // what rb200_model_create would accept: a known coder, its scale_bits range, frequencies that sum to 1 << scale_bits
 bool container_model_ok(uint32_t coder, uint32_t scale_bits, const uint32_t* freqs);
+// every block's 256 frequencies sum to 4096
+bool container_block_models_ok(const uint16_t* block_freqs, uint32_t n_blocks);
+// the directory rules: the first stream starts inside the first vector, monotone, last entry == blob_bytes
+bool container_directory_ok(const uint64_t* offsets, uint64_t n_chunks, uint64_t blob_bytes);
 // zlib crc32 on the host (slicing-by-8)
 uint32_t container_crc32(uint32_t crc, const void* data, size_t len);
 // CRC-32 of the header with its crc fields zeroed: the first 64 bytes of what meta_crc covers
 uint32_t container_header_crc(const ContainerHeader& h);
-// meta_crc over header, freqs and offsets, on the host
-uint32_t container_meta_crc(const ContainerHeader& h, const uint32_t* freqs, const uint64_t* offsets);
+// meta_crc over header, model section (container_model_bytes(h) bytes) and offsets, on the host
+uint32_t container_meta_crc(const ContainerHeader& h, const void* model, const uint64_t* offsets);
 
 // The parser, in the order rb200_container_open applies it.  Each step returns RB200_OK or RB200_E_STREAM; the CRC
 // values are the caller's, computed wherever the bytes live.
-//  1. the 64-byte header against the buffer size (`size` bytes in all; `hdr` holds at least 64 of them)
-int container_parse_header(const uint8_t* hdr, size_t size, ContainerHeader* h);
-//  2. header + model + directory (`prefix`: container_blob_offset(h.n_chunks) bytes), given their CRC
+//  1. the 64-byte header against the buffer size (`size` bytes in all; `hdr` holds at least 64 of them); `version`
+//     is the one the caller accepts (kContainerVersion or kContainerVersionBlocks), any other is rejected
+int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, ContainerHeader* h);
+//  2. header + model + directory (`prefix`: container_blob_offset(h) bytes), given their CRC
 int container_check_prefix(const ContainerHeader& h, const uint8_t* prefix, uint32_t meta_crc);
 //  3. the blob, given its CRC (only consulted when the header carries one)
 int container_check_blob(const ContainerHeader& h, uint32_t blob_crc);

@@ -4,13 +4,27 @@
 // (main.cpp:182-188).  The bulk API's natural output (blob + offsets + the caller's freqs) is enough
 // for in-process use; this file adds the versioned, checksummed envelope needed to ship it:
 //
-//   [ 64-byte header ][ freqs: 256 x u32 ][ offsets: (n_chunks + 1) x u64 ][ pad to 16 ][ blob ]
+//   version 1 (one model):       [ 64-byte header ][ freqs: 256 x u32 ][ offsets: (n_chunks + 1) x u64 ][ pad to 16 ][ blob ]
+//   version 2 (a model per block): [ 64-byte header ][ block_freqs: n_blocks x 256 x u16 ][ offsets ][ pad to 16 ][ blob ]
 //
-// All integers little-endian.  CRC-32 (zlib's: IEEE, reflected) over header (with the crc fields zeroed) + freqs +
-// offsets always; over the blob when RB200_CONTAINER_CRC_BLOB is set.  rb200_container_pack / _open here work on host
-// buffers with a host CRC (slicing-by-8, ~1 GB/s on one core: the blob CRC is optional for that reason).
-// rb200_container_encode / _decode (rans_b200.cu) write and read the same bytes in host or device memory with the
-// blob CRC on the GPU (crc_kernels.cuh); they validate through the parser below, so both sides apply one set of rules.
+// All integers little-endian.  CRC-32 (zlib's: IEEE, reflected) over header (with the crc fields zeroed) + model +
+// offsets always (meta_crc); over the blob when RB200_CONTAINER_CRC_BLOB is set.  The header layout is the same in
+// both versions.  Version 1 has its directory at 1088; version 2 (word coder, scale_bits 12, 32 lanes) carries
+// block_size at byte 52 and n_blocks at byte 56, its model section is 512 n_blocks bytes, so its directory starts at
+// 64 + 512 n_blocks, and the u32 at byte 60 is zero.  Its chunk order is the per-block calls': chunk = block *
+// (block_size / chunk_syms) + chunk-in-block, so each block's chunks are ordinary 32-way word streams under that
+// block's row of block_freqs.  A version 2 container is valid only if: chunk_syms and block_size are what
+// rb200_blocks_decode accepts (block_size % chunk_syms == 0, at most 32 chunks per block), n_blocks >= 1,
+// n_symbols == n_blocks * block_size, n_chunks == n_symbols / chunk_syms < 2^31, blob_bytes % 16 == 0, every section
+// fits the buffer, no flag but RB200_CONTAINER_CRC_BLOB, meta_crc matches, every block's frequencies sum to 4096, the
+// directory rules of version 1 hold (offsets[0] < 16, monotone, offsets[n_chunks] == blob_bytes), and the blob CRC
+// matches when present.  Each call accepts exactly one version: rb200_container_* version 1, rb200_container_blocks_*
+// version 2.
+//
+// rb200_container_pack / _open and the _blocks_ forms here work on host buffers with a host CRC (slicing-by-8, ~1 GB/s
+// on one core: the blob CRC is optional for that reason).  rb200_container_encode / _decode and the _blocks_ forms
+// (rans_b200.cu) write and read the same bytes in host or device memory with the blob CRC on the GPU
+// (crc_kernels.cuh); they validate through the parser below, so both sides apply one set of rules.
 #include "container_format.h"
 
 #include <cstring>
@@ -63,10 +77,10 @@ uint32_t container_header_crc(const ContainerHeader& h)
     return container_crc32(0, &z, sizeof z);
 }
 
-uint32_t container_meta_crc(const ContainerHeader& h, const uint32_t* freqs, const uint64_t* offsets)
+uint32_t container_meta_crc(const ContainerHeader& h, const void* model, const uint64_t* offsets)
 {
     uint32_t c = container_header_crc(h);
-    c = container_crc32(c, freqs, 256 * sizeof(uint32_t));
+    c = container_crc32(c, model, container_model_bytes(h));
     return container_crc32(c, offsets, (h.n_chunks + 1) * sizeof(uint64_t));
 }
 
@@ -77,6 +91,25 @@ bool container_model_ok(uint32_t coder, uint32_t scale_bits, const uint32_t* fre
     uint64_t sum = 0;
     for (int s = 0; s < 256; s++) sum += freqs[s];
     return sum == (1ull << scale_bits);
+}
+
+bool container_block_models_ok(const uint16_t* block_freqs, uint32_t n_blocks)
+{
+    for (uint64_t b = 0; b < n_blocks; b++) {
+        uint32_t sum = 0;
+        for (int s = 0; s < 256; s++) sum += block_freqs[b * 256 + s];
+        if (sum != 4096) return false;
+    }
+    return true;
+}
+
+bool container_directory_ok(const uint64_t* offsets, uint64_t n_chunks, uint64_t blob_bytes)
+{
+    if (offsets[n_chunks] != blob_bytes) return false;
+    if (n_chunks && offsets[0] >= 16) return false;                                       // the first stream starts inside the first vector
+    for (uint64_t c = 0; c < n_chunks; c++)
+        if (offsets[c] > offsets[c + 1]) return false;
+    return true;
 }
 
 ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_syms, uint64_t n, uint64_t n_chunks,
@@ -96,16 +129,34 @@ ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_
     return h;
 }
 
-int container_parse_header(const uint8_t* hdr, size_t size, ContainerHeader* out)
+ContainerHeader container_blocks_header(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint64_t blob_bytes, uint32_t flags)
+{
+    const uint64_t n = static_cast<uint64_t>(n_blocks) * block_size;
+    ContainerHeader h = container_header(RB200_CODER_WORD, 12, chunk_syms, n, n / chunk_syms, blob_bytes, flags);
+    h.version = kContainerVersionBlocks;
+    h.block_size = block_size;
+    h.n_blocks = n_blocks;
+    return h;
+}
+
+int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, ContainerHeader* out)
 {
     if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
     ContainerHeader h;
     std::memcpy(&h, hdr, sizeof h);
-    if (h.magic != kContainerMagic || h.version != kContainerVersion || h.lanes != RB200_LANES || !h.chunk_syms) return RB200_E_STREAM;
-    if (h.n_chunks != h.n_symbols / h.chunk_syms + (h.n_symbols % h.chunk_syms != 0) || h.n_chunks >= (1ull << 31) ||
-        (h.blob_bytes & 15) || h.coder > RB200_CODER_RANS64 || h.scale_bits < 8 || h.scale_bits > 16)
+    if (h.magic != kContainerMagic || h.version != version || h.lanes != RB200_LANES || !h.chunk_syms) return RB200_E_STREAM;
+    if (version == kContainerVersionBlocks) {
+        // what rb200_blocks_decode accepts; n_blocks * block_size cannot overflow 64 bits
+        if (h.coder != RB200_CODER_WORD || h.scale_bits != 12 || !container_blocks_geometry_ok(h.n_blocks, h.block_size, h.chunk_syms))
+            return RB200_E_STREAM;
+        if (h.n_symbols != static_cast<uint64_t>(h.n_blocks) * h.block_size || h.n_chunks != h.n_symbols / h.chunk_syms ||
+            h.n_chunks >= (1ull << 31) || (h.blob_bytes & 15) || h.reserved || (h.flags & ~RB200_CONTAINER_CRC_BLOB))
+            return RB200_E_STREAM;
+    } else if (h.n_chunks != h.n_symbols / h.chunk_syms + (h.n_symbols % h.chunk_syms != 0) || h.n_chunks >= (1ull << 31) ||
+               (h.blob_bytes & 15) || h.coder > RB200_CODER_RANS64 || h.scale_bits < 8 || h.scale_bits > 16) {
         return RB200_E_STREAM;
-    const size_t boff = container_blob_offset(h.n_chunks);
+    }
+    const uint64_t boff = container_blob_offset(h);                 // < 2^42: n_chunks < 2^31, n_blocks < 2^32
     if (boff > size || h.blob_bytes > size - boff) return RB200_E_STREAM;
     *out = h;
     return RB200_OK;
@@ -113,15 +164,14 @@ int container_parse_header(const uint8_t* hdr, size_t size, ContainerHeader* out
 
 int container_check_prefix(const ContainerHeader& h, const uint8_t* prefix, uint32_t meta_crc)
 {
-    const uint32_t* freqs = reinterpret_cast<const uint32_t*>(prefix + sizeof(ContainerHeader));
-    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(prefix + kContainerDirOffset);
+    const uint8_t* model = prefix + sizeof(ContainerHeader);
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(prefix + container_dir_offset(h));
     if (meta_crc != h.meta_crc) return RB200_E_STREAM;
-    if (!container_model_ok(h.coder, h.scale_bits, freqs)) return RB200_E_STREAM;        // CRC-valid but inconsistent
-    if (offsets[h.n_chunks] != h.blob_bytes) return RB200_E_STREAM;
-    if (h.n_chunks && offsets[0] >= 16) return RB200_E_STREAM;                           // the first stream starts inside the first vector
-    for (uint64_t c = 0; c < h.n_chunks; c++)
-        if (offsets[c] > offsets[c + 1]) return RB200_E_STREAM;
-    return RB200_OK;
+    const bool model_ok = h.version == kContainerVersionBlocks
+                              ? container_block_models_ok(reinterpret_cast<const uint16_t*>(model), h.n_blocks)
+                              : container_model_ok(h.coder, h.scale_bits, reinterpret_cast<const uint32_t*>(model));
+    if (!model_ok) return RB200_E_STREAM;                                                  // CRC-valid but inconsistent
+    return container_directory_ok(offsets, h.n_chunks, h.blob_bytes) ? RB200_OK : RB200_E_STREAM;
 }
 
 int container_check_blob(const ContainerHeader& h, uint32_t blob_crc)
@@ -129,11 +179,45 @@ int container_check_blob(const ContainerHeader& h, uint32_t blob_crc)
     return (h.flags & RB200_CONTAINER_CRC_BLOB) && blob_crc != h.blob_crc ? RB200_E_STREAM : RB200_OK;
 }
 
+namespace {
+
+// Both packs: header (CRCs filled in), model, directory, zero pad and blob into out[0, container_blob_offset(h) + blob).
+void container_write(ContainerHeader h, const void* model, const uint64_t* offsets, const uint8_t* blob, uint8_t* out)
+{
+    h.meta_crc = container_meta_crc(h, model, offsets);
+    if (h.flags & RB200_CONTAINER_CRC_BLOB) h.blob_crc = container_crc32(0, blob, h.blob_bytes);
+    const uint64_t dir = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
+    std::memcpy(out, &h, sizeof h);
+    std::memcpy(out + sizeof h, model, container_model_bytes(h));
+    std::memcpy(out + dir, offsets, dir_end - dir);
+    std::memset(out + dir_end, 0, boff - dir_end);
+    if (h.blob_bytes) std::memcpy(out + boff, blob, h.blob_bytes);
+}
+
+// Both opens: the parser's three steps on a host buffer (8-byte aligned) holding a container of `version`.
+int container_open_checked(const uint8_t* buf, size_t size, uint16_t version, ContainerHeader* h)
+{
+    int rc = container_parse_header(buf, size, version, h);
+    if (rc != RB200_OK) return rc;
+    // model and offsets sit at 4- and 8-byte aligned positions when buf itself is 8-byte aligned (callers map or malloc it)
+    if (reinterpret_cast<uintptr_t>(buf) & 7) return RB200_E_ARG;
+    rc = container_check_prefix(*h, buf, container_meta_crc(*h, buf + sizeof(ContainerHeader),
+                                                            reinterpret_cast<const uint64_t*>(buf + container_dir_offset(*h))));
+    if (rc == RB200_OK && (h->flags & RB200_CONTAINER_CRC_BLOB))
+        rc = container_check_blob(*h, container_crc32(0, buf + container_blob_offset(*h), h->blob_bytes));
+    return rc;
+}
+
+}  // namespace
+
 }  // namespace rb200
 
 using namespace rb200;
 
-extern "C" size_t rb200_container_size(size_t n_chunks, size_t blob_bytes) { return container_blob_offset(n_chunks) + blob_bytes; }
+extern "C" size_t rb200_container_size(size_t n_chunks, size_t blob_bytes)
+{
+    return container_blob_offset(container_shape(kContainerVersion, 0, n_chunks)) + blob_bytes;
+}
 
 extern "C" int rb200_container_pack(int coder, uint32_t scale_bits, uint32_t chunk_syms, size_t n, const uint32_t freqs[256],
                                     const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes, uint32_t flags, uint8_t* out,
@@ -145,19 +229,7 @@ extern "C" int rb200_container_pack(int coder, uint32_t scale_bits, uint32_t chu
     if (offsets[n_chunks] != blob_bytes || (blob_bytes & 15)) return RB200_E_ARG;
     const size_t total = rb200_container_size(n_chunks, blob_bytes);
     if (total > out_cap) return RB200_E_SPACE;
-    ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n, n_chunks, blob_bytes, flags);
-    h.meta_crc = container_meta_crc(h, freqs, offsets);
-    if (h.flags & RB200_CONTAINER_CRC_BLOB) h.blob_crc = container_crc32(0, blob, blob_bytes);
-    uint8_t* p = out;
-    std::memcpy(p, &h, sizeof h);
-    p += sizeof h;
-    std::memcpy(p, freqs, 256 * sizeof(uint32_t));
-    p += 256 * sizeof(uint32_t);
-    std::memcpy(p, offsets, (n_chunks + 1) * sizeof(uint64_t));
-    p += (n_chunks + 1) * sizeof(uint64_t);
-    const size_t boff = container_blob_offset(n_chunks);
-    std::memset(p, 0, out + boff - p);
-    if (blob_bytes) std::memcpy(out + boff, blob, blob_bytes);
+    container_write(container_header(coder, scale_bits, chunk_syms, n, n_chunks, blob_bytes, flags), freqs, offsets, blob, out);
     if (out_size) *out_size = total;
     return RB200_OK;
 }
@@ -166,16 +238,7 @@ extern "C" int rb200_container_open(const uint8_t* buf, size_t size, rb200_conta
 {
     if (!buf || !info) return RB200_E_ARG;
     ContainerHeader h;
-    int rc = container_parse_header(buf, size, &h);
-    if (rc != RB200_OK) return rc;
-    // freqs/offsets sit at 4- and 8-byte aligned positions when buf itself is 8-byte aligned (callers map or malloc it)
-    const uint32_t* freqs = reinterpret_cast<const uint32_t*>(buf + sizeof(ContainerHeader));
-    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + kContainerDirOffset);
-    if (reinterpret_cast<uintptr_t>(buf) & 7) return RB200_E_ARG;
-    rc = container_check_prefix(h, buf, container_meta_crc(h, freqs, offsets));
-    if (rc != RB200_OK) return rc;
-    const size_t boff = container_blob_offset(h.n_chunks);
-    if (h.flags & RB200_CONTAINER_CRC_BLOB) rc = container_check_blob(h, container_crc32(0, buf + boff, h.blob_bytes));
+    const int rc = container_open_checked(buf, size, kContainerVersion, &h);
     if (rc != RB200_OK) return rc;
     info->coder = h.coder;
     info->scale_bits = h.scale_bits;
@@ -184,8 +247,50 @@ extern "C" int rb200_container_open(const uint8_t* buf, size_t size, rb200_conta
     info->n_symbols = h.n_symbols;
     info->n_chunks = h.n_chunks;
     info->blob_bytes = h.blob_bytes;
-    info->freqs = freqs;
-    info->offsets = offsets;
-    info->blob = buf + boff;
+    info->freqs = reinterpret_cast<const uint32_t*>(buf + sizeof(ContainerHeader));
+    info->offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h));
+    info->blob = buf + container_blob_offset(h);
+    return RB200_OK;
+}
+
+extern "C" size_t rb200_container_blocks_size(uint32_t n_blocks, size_t n_chunks, size_t blob_bytes)
+{
+    return container_blob_offset(container_shape(kContainerVersionBlocks, n_blocks, n_chunks)) + blob_bytes;
+}
+
+extern "C" int rb200_container_blocks_pack(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, const uint16_t* block_freqs,
+                                           const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes, uint32_t flags, uint8_t* out,
+                                           size_t out_cap, size_t* out_size)
+{
+    if (!block_freqs || !offsets || (!blob && blob_bytes) || !out) return RB200_E_ARG;
+    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
+    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
+    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    if (!container_block_models_ok(block_freqs, n_blocks)) return RB200_E_MODEL;          // never write what open rejects
+    if ((blob_bytes & 15) || !container_directory_ok(offsets, n_chunks, blob_bytes)) return RB200_E_ARG;
+    const ContainerHeader h = container_blocks_header(n_blocks, block_size, chunk_syms, blob_bytes, flags);
+    const size_t total = container_blob_offset(h) + blob_bytes;
+    if (total > out_cap) return RB200_E_SPACE;
+    container_write(h, block_freqs, offsets, blob, out);
+    if (out_size) *out_size = total;
+    return RB200_OK;
+}
+
+extern "C" int rb200_container_blocks_open(const uint8_t* buf, size_t size, rb200_container_blocks_info* info)
+{
+    if (!buf || !info) return RB200_E_ARG;
+    ContainerHeader h;
+    const int rc = container_open_checked(buf, size, kContainerVersionBlocks, &h);
+    if (rc != RB200_OK) return rc;
+    info->n_blocks = h.n_blocks;
+    info->block_size = h.block_size;
+    info->chunk_syms = h.chunk_syms;
+    info->flags = h.flags;
+    info->n_symbols = h.n_symbols;
+    info->n_chunks = h.n_chunks;
+    info->blob_bytes = h.blob_bytes;
+    info->block_freqs = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));
+    info->offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h));
+    info->blob = buf + container_blob_offset(h);
     return RB200_OK;
 }

@@ -255,37 +255,44 @@ inline uint32_t crc32_grid(uint32_t sms, uint64_t n)
     return want < 1 ? 1 : (want > sms ? sms : static_cast<uint32_t>(want));
 }
 
-// The last step of a device-memory rb200_container_encode, one warp: the encoder has written the directory at
-// out + 1088 and the blob at out + blob_off, crc32_kernel has put the directory's CRC in slots[0] and (with
-// RB200_CONTAINER_CRC_BLOB) the blob's in slots[1].  Reads blob_bytes from the directory, completes the header
-// (h arrives with blob_bytes and both CRCs zero), and writes header, model and the zero pad in front of the blob.
+// The last step of a device-memory container encode, one warp.  The encoder has written the directory at
+// out + dir_off and the blob at out + blob_off.  crc32_kernel has put into slots[0] the CRC of out[head, dir_end),
+// where head is what this kernel writes in front of it: header and model `freqs` (version 1, head = 1088: the model
+// comes from the rb200_model and is CRC'd here) or the header alone (version 2, freqs == nullptr, head = 64: the
+// block encoder wrote the models in place, so slots[0] covers model and directory); with RB200_CONTAINER_CRC_BLOB
+// the blob's CRC is in slots[1].  Reads blob_bytes from the directory, completes the header (h arrives with
+// blob_bytes and both CRCs zero), and writes the head and the zero pad in front of the blob -- only when the status
+// word is clear (an encoder error leaves the buffer as it is) and the blob fits out_cap (else it flags kStatSpace).
 __global__ void __launch_bounds__(32)
-    container_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t blob_off, uint64_t out_cap, const uint32_t* __restrict__ freqs,
-                            const CrcSlot* __restrict__ slots, uint32_t* status)
+    container_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
+                            const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status)
 {
     using namespace crc_detail;
     __shared__ uint4 sbuf_v[kContainerDirOffset / 16];
     uint32_t* sbuf = reinterpret_cast<uint32_t*>(sbuf_v);
     const uint32_t lane = threadIdx.x;
-    const uint64_t blob_bytes = reinterpret_cast<const uint64_t*>(out + kContainerDirOffset)[h.n_chunks];
+    if (*status) return;                              // the encoder has flagged an error: rb200_sync reports it
+    const uint64_t blob_bytes = reinterpret_cast<const uint64_t*>(out + dir_off)[h.n_chunks];
     if (blob_bytes > out_cap - blob_off) {            // the encoder has flagged it; leave the buffer as it is
         if (lane == 0) atomicOr(status, kStatSpace);
         return;
     }
+    const uint32_t head = freqs ? static_cast<uint32_t>(kContainerDirOffset) : static_cast<uint32_t>(sizeof(ContainerHeader));
     if (lane == 0) {
         ContainerHeader* sh = reinterpret_cast<ContainerHeader*>(sbuf);
         *sh = h;
         sh->blob_bytes = blob_bytes;
     }
-    for (uint32_t i = lane; i < 256; i += 32) sbuf[16 + i] = freqs[i];
+    if (freqs)
+        for (uint32_t i = lane; i < 256; i += 32) sbuf[16 + i] = freqs[i];
     __syncwarp();
-    // CRC of header || freqs: 34 bytes per lane, each shifted past the bytes after it
-    constexpr uint32_t kPiece = kContainerDirOffset / 32;
-    uint32_t c = raw_bytes_bitwise(reinterpret_cast<const uint8_t*>(sbuf) + lane * kPiece, kPiece);
-    c = __reduce_xor_sync(0xffffffffu, crc32_shift(c, kContainerDirOffset - kPiece * (lane + 1)));
-    const uint32_t head_crc = finish_warp(0, kContainerDirOffset, c);
-    const uint64_t dir_bytes = (h.n_chunks + 1) * sizeof(uint64_t);
-    const uint32_t meta = crc32_mulmod(head_crc, x8pow_warp(dir_bytes)) ^ slots[0].crc;      // crc32_combine
+    // CRC of the head: head / 32 bytes per lane (34 or 2), each shifted past the bytes after it
+    const uint32_t piece = head / 32;
+    uint32_t c = raw_bytes_bitwise(reinterpret_cast<const uint8_t*>(sbuf) + lane * piece, piece);
+    c = __reduce_xor_sync(0xffffffffu, crc32_shift(c, head - piece * (lane + 1)));
+    const uint32_t head_crc = finish_warp(0, head, c);
+    const uint64_t dir_end = dir_off + (h.n_chunks + 1) * sizeof(uint64_t);
+    const uint32_t meta = crc32_mulmod(head_crc, x8pow_warp(dir_end - head)) ^ slots[0].crc;      // crc32_combine
     __syncwarp();
     if (lane == 0) {
         sbuf[offsetof(ContainerHeader, meta_crc) / 4] = meta;
@@ -293,8 +300,7 @@ __global__ void __launch_bounds__(32)
     }
     __syncwarp();
     uint4* dst = reinterpret_cast<uint4*>(out);
-    for (uint32_t i = lane; i < kContainerDirOffset / 16; i += 32) dst[i] = sbuf_v[i];
-    const uint64_t dir_end = kContainerDirOffset + dir_bytes;
+    for (uint32_t i = lane; i < head / 16; i += 32) dst[i] = sbuf_v[i];
     if (lane == 0 && blob_off > dir_end) *reinterpret_cast<uint64_t*>(out + dir_end) = 0;   // the 8-byte pad
 }
 

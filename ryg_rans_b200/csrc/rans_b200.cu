@@ -157,10 +157,7 @@ struct DeviceGuard {
     }
 };
 
-constexpr uint32_t kMinChunk = 32;
-constexpr uint32_t kMaxChunk = 1u << 24;
-
-bool chunk_ok(uint32_t chunk_syms) { return chunk_syms >= kMinChunk && chunk_syms <= kMaxChunk; }
+bool chunk_ok(uint32_t chunk_syms) { return container_chunk_ok(chunk_syms); }     // 32 .. 2^24 symbols
 
 }  // namespace
 
@@ -1096,33 +1093,53 @@ int blocks_encode_device(rb200_ctx* ctx, const uint8_t* d_in, uint32_t n_blocks,
     return finish_encode(ctx, scratch, slot, sizes, tile_sums, n_chunks, d_blob, blob_cap, d_offsets);
 }
 
-// one CTA per block, one warp per chunk of the block: at most 32 chunks per block
-bool blocks_geometry_ok(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms)
+// Host mode runs the slice pipeline over whole blocks; the frequency tables go in with each slice when the caller supplies
+// them, and come back with it when the kernel builds them.  `hook` as in encode_pipeline.
+template <class Hook = NoSliceHook>
+int blocks_encode_host(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint16_t* block_freqs, bool build,
+                       uint32_t chunk_syms, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size, Hook hook = Hook{})
 {
-    return n_blocks && block_size && chunk_ok(chunk_syms) && block_size % chunk_syms == 0 && block_size / chunk_syms <= 32;
+    const UnitTable freqs = build ? UnitTable{nullptr, block_freqs, kBlockFreqBytes} : UnitTable{block_freqs, nullptr, kBlockFreqBytes};
+    return encode_pipeline(
+        ctx, in, static_cast<size_t>(n_blocks) * block_size, chunk_syms, block_size / chunk_syms, freqs,
+        [&](size_t units) { return reserve_blocks_encode(ctx, static_cast<uint32_t>(units), block_size, chunk_syms, build); },
+        [&](const Slice& s, const uint8_t* d_in, uint8_t* d_freqs, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
+            return blocks_encode_device(ctx, d_in, static_cast<uint32_t>(s.units), block_size, reinterpret_cast<uint16_t*>(d_freqs),
+                                        build, chunk_syms, d_blob, cap, d_off);
+        },
+        blob, blob_cap, offsets, blob_size, hook);
 }
 
-// Host mode runs the slice pipeline over whole blocks; the frequency tables go in with each slice when the caller supplies
-// them, and come back with it when the kernel builds them.
 int blocks_encode_entry(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint16_t* block_freqs, bool build,
                         uint32_t chunk_syms, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind)
 {
-    if (!ctx || !in || !block_freqs || !blob || !offsets || !blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
+    if (!ctx || !in || !block_freqs || !blob || !offsets || !container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
     return by_mem_kind(
         mem_kind, blob, offsets,
         [&] { return blocks_encode_device(ctx, in, n_blocks, block_size, block_freqs, build, chunk_syms, blob, blob_cap, offsets); },
-        [&] {
-            const UnitTable freqs = build ? UnitTable{nullptr, block_freqs, kBlockFreqBytes} : UnitTable{block_freqs, nullptr, kBlockFreqBytes};
-            return encode_pipeline(
-                ctx, in, static_cast<size_t>(n_blocks) * block_size, chunk_syms, block_size / chunk_syms, freqs,
-                [&](size_t units) { return reserve_blocks_encode(ctx, static_cast<uint32_t>(units), block_size, chunk_syms, build); },
-                [&](const Slice& s, const uint8_t* d_in, uint8_t* d_freqs, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
-                    return blocks_encode_device(ctx, d_in, static_cast<uint32_t>(s.units), block_size, reinterpret_cast<uint16_t*>(d_freqs),
-                                                build, chunk_syms, d_blob, cap, d_off);
-                },
-                blob, blob_cap, offsets, blob_size);
-        });
+        [&] { return blocks_encode_host(ctx, in, n_blocks, block_size, block_freqs, build, chunk_syms, blob, blob_cap, offsets, blob_size); });
+}
+
+int blocks_decode_device(rb200_ctx* ctx, const uint8_t* d_blob, size_t blob_size, const uint64_t* d_off, const uint16_t* d_freqs,
+                         uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint8_t* d_out)
+{
+    launch_block_decode(ctx->stream, d_blob, blob_size, d_off, d_freqs, n_blocks, block_size, chunk_syms, d_out, ctx->d_status);
+    return check_launch(ctx, "block_decode_kernel");
+}
+
+// the host-buffer form of rb200_blocks_decode: the slice pipeline over whole blocks, each slice's tables copied in with it
+template <class Hook = NoSliceHook>
+int blocks_decode_host(rb200_ctx* ctx, const uint8_t* blob, size_t blob_size, const uint64_t* offsets, const uint16_t* block_freqs,
+                       uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint8_t* out, Hook hook = Hook{})
+{
+    return decode_pipeline(
+        ctx, blob, blob_size, offsets, chunk_syms, block_size / chunk_syms, UnitTable{block_freqs, nullptr, kBlockFreqBytes},
+        [&](const Slice& s, const uint8_t* d_blob, const uint64_t* d_off, uint8_t* d_freqs, uint8_t* d_out) {
+            return blocks_decode_device(ctx, d_blob, blob_size, d_off, reinterpret_cast<const uint16_t*>(d_freqs),
+                                        static_cast<uint32_t>(s.units), block_size, chunk_syms, d_out);
+        },
+        out, static_cast<size_t>(n_blocks) * block_size, hook);
 }
 
 }  // namespace
@@ -1146,25 +1163,15 @@ extern "C" int rb200_blocks_decode(rb200_ctx* ctx, const uint8_t* blob, size_t b
                                    const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
                                    uint8_t* out, int mem_kind)
 {
-    if (!ctx || !blob || !offsets || !block_freqs || !out || !blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
+    if (!ctx || !blob || !offsets || !block_freqs || !out || !container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
     if (!blob_size_ok(blob_size)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
     const uint32_t per_block = block_size / chunk_syms;
     if (static_cast<uint64_t>(n_blocks) * per_block >= (1ull << 31)) return RB200_E_ARG;
-    auto decode = [&](const uint8_t* d_blob, const uint64_t* d_off, const uint16_t* d_freqs, uint32_t blocks, uint8_t* d_out) {
-        launch_block_decode(ctx->stream, d_blob, blob_size, d_off, d_freqs, blocks, block_size, chunk_syms, d_out, ctx->d_status);
-        return check_launch(ctx, "block_decode_kernel");
-    };
     return by_mem_kind(
-        mem_kind, blob, offsets, [&] { return decode(blob, offsets, block_freqs, n_blocks, out); },
-        [&] {
-            return decode_pipeline(
-                ctx, blob, blob_size, offsets, chunk_syms, per_block, UnitTable{block_freqs, nullptr, kBlockFreqBytes},
-                [&](const Slice& s, const uint8_t* d_blob, const uint64_t* d_off, uint8_t* d_freqs, uint8_t* d_out) {
-                    return decode(d_blob, d_off, reinterpret_cast<const uint16_t*>(d_freqs), static_cast<uint32_t>(s.units), d_out);
-                },
-                out, static_cast<size_t>(n_blocks) * block_size);
-        });
+        mem_kind, blob, offsets,
+        [&] { return blocks_decode_device(ctx, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out); },
+        [&] { return blocks_decode_host(ctx, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out); });
 }
 
 // ---------------------------------------------------------------------------
@@ -1218,11 +1225,12 @@ struct SliceCrc {
     }
 };
 
-// rb200_container_decode once the buffers are checked: header, model and directory validated by the shared parser,
-// then the blob CRC, then a model and the decode.  DEVICE: the prefix is read through pinned memory, both CRCs
-// are taken on the GPU, and nothing is decoded unless every check passes.
+// rb200_container_decode / rb200_container_blocks_decode once the buffers are checked: header, model and directory
+// validated by the shared parser for `version`, then the blob CRC, then the decode (a model and rb200_decode's kernels
+// for version 1, the per-block decoder reading its tables in place for version 2).  DEVICE: the prefix is read through
+// pinned memory, both CRCs are taken on the GPU, and nothing is decoded unless every check passes.
 int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap, uint64_t* n_symbols,
-                          bool device)
+                          bool device, uint16_t version)
 {
     ContainerHeader h;
     const uint8_t* prefix = buf;
@@ -1233,31 +1241,31 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
         if (rc != RB200_OK) return rc;
         RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir, buf, sizeof(ContainerHeader), cudaMemcpyDeviceToHost, ctx->stream));
         RB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        rc = container_parse_header(reinterpret_cast<const uint8_t*>(ctx->h_dir), size, &h);
+        rc = container_parse_header(reinterpret_cast<const uint8_t*>(ctx->h_dir), size, version, &h);
         if (rc != RB200_OK) return rc;
-        const size_t boff = container_blob_offset(h.n_chunks);
+        const size_t boff = container_blob_offset(h);
         rc = reserve_dir(ctx, boff / sizeof(uint64_t));
         if (rc != RB200_OK) return rc;
-        const uint64_t rest = boff - sizeof(ContainerHeader);     // model, directory and pad: what the CRC covers after the header
-        const uint64_t covered = kContainerDirOffset - sizeof(ContainerHeader) + (h.n_chunks + 1) * sizeof(uint64_t);
-        RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir, buf, sizeof(ContainerHeader) + rest, cudaMemcpyDeviceToHost, ctx->stream));
+        const uint64_t covered = container_dir_end(h) - sizeof(ContainerHeader);     // model and directory: what the CRC covers after the header
+        RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir, buf, boff, cudaMemcpyDeviceToHost, ctx->stream));
         rc = launch_crc(ctx, buf + sizeof(ContainerHeader), covered, nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK) rc = fetch_crc(ctx, 1);
         if (rc != RB200_OK) return rc;
         prefix = reinterpret_cast<const uint8_t*>(ctx->h_dir);
         rc = container_check_prefix(h, prefix, crc32_combine(container_header_crc(h), ctx->h_crc[0].crc, covered));
     } else {
-        rc = container_parse_header(buf, size, &h);
+        rc = container_parse_header(buf, size, version, &h);
         if (rc == RB200_OK)
-            rc = container_check_prefix(h, buf, container_meta_crc(h, reinterpret_cast<const uint32_t*>(buf + sizeof(ContainerHeader)),
-                                                                   reinterpret_cast<const uint64_t*>(buf + kContainerDirOffset)));
+            rc = container_check_prefix(h, buf, container_meta_crc(h, buf + sizeof(ContainerHeader),
+                                                                   reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h))));
     }
     if (rc != RB200_OK) return rc;
     if (n_symbols) *n_symbols = h.n_symbols;
     if (out_cap < h.n_symbols) return RB200_E_SPACE;
     if (h.n_symbols && !out) return RB200_E_ARG;
     if (!chunk_ok(h.chunk_syms) || !blob_size_ok(h.blob_bytes)) return RB200_E_ARG;     // what rb200_decode accepts
-    const uint8_t* blob = buf + container_blob_offset(h.n_chunks);
+    const uint8_t* blob = buf + container_blob_offset(h);
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h));
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
     if (device && blob_crc) {
         rc = launch_crc(ctx, blob, h.blob_bytes, nullptr, 0, ctx->d_crc);
@@ -1265,23 +1273,43 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
         if (rc == RB200_OK) rc = container_check_blob(h, ctx->h_crc[0].crc);
         if (rc != RB200_OK) return rc;
     }
+    // the decode: DEVICE enqueues it and synchronises; HOST runs a slice pipeline that CRCs each slice's blob bytes
+    auto decode = [&](auto on_device, auto on_host) -> int {
+        if (device) {
+            const int r = on_device();
+            const int st = rb200_sync(ctx);
+            return r == RB200_OK ? st : r;
+        }
+        size_t slices = 0;
+        int r = on_host(SliceCrc{ctx, blob_crc, &slices});
+        uint32_t crc = 0;
+        if (r == RB200_OK && blob_crc) r = joined_slice_crc(ctx, slices, &crc);
+        if (r == RB200_OK) r = container_check_blob(h, crc);
+        return r;
+    };
+    if (version == kContainerVersionBlocks) {
+        const uint16_t* block_freqs = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));     // read in place
+        return decode(
+            [&] { return blocks_decode_device(ctx, blob, h.blob_bytes, offsets, block_freqs, h.n_blocks, h.block_size, h.chunk_syms, out); },
+            [&](SliceCrc hook) {
+                return blocks_decode_host(ctx, blob, h.blob_bytes, offsets, block_freqs, h.n_blocks, h.block_size, h.chunk_syms, out, hook);
+            });
+    }
     rb200_model* model = nullptr;
     rc = rb200_model_create(ctx, h.coder, h.scale_bits, reinterpret_cast<const uint32_t*>(prefix + sizeof(ContainerHeader)), &model);
     if (rc != RB200_OK) return rc;
-    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + kContainerDirOffset);
-    if (device) {
-        rc = decode_device(ctx, model, blob, h.blob_bytes, offsets, h.chunk_syms, out, h.n_symbols);
-        const int st = rb200_sync(ctx);
-        if (rc == RB200_OK) rc = st;
-    } else {
-        size_t slices = 0;
-        rc = decode_host(ctx, model, blob, h.blob_bytes, offsets, h.chunk_syms, out, h.n_symbols, SliceCrc{ctx, blob_crc, &slices});
-        uint32_t crc = 0;
-        if (rc == RB200_OK && blob_crc) rc = joined_slice_crc(ctx, slices, &crc);
-        if (rc == RB200_OK) rc = container_check_blob(h, crc);
-    }
+    rc = decode([&] { return decode_device(ctx, model, blob, h.blob_bytes, offsets, h.chunk_syms, out, h.n_symbols); },
+                [&](SliceCrc hook) { return decode_host(ctx, model, blob, h.blob_bytes, offsets, h.chunk_syms, out, h.n_symbols, hook); });
     rb200_model_destroy(model);
     return rc;
+}
+
+// Alignment of a container call's buffers: 16 bytes in DEVICE mode (the kernels' vector loads), 8 in HOST mode.
+bool container_mem_ok(int mem_kind, const void* a, const void* b)
+{
+    if (mem_kind != RB200_MEM_HOST && mem_kind != RB200_MEM_DEVICE) return false;
+    const uintptr_t align = mem_kind == RB200_MEM_DEVICE ? 15 : 7;
+    return !(reinterpret_cast<uintptr_t>(a) & align) && !(reinterpret_cast<uintptr_t>(b) & align);
 }
 
 }  // namespace
@@ -1307,24 +1335,23 @@ extern "C" int rb200_container_encode(rb200_ctx* ctx, const rb200_model* model, 
                                       uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind)
 {
     if (!ctx || !model || model->ctx != ctx || !out || (!in && n) || !chunk_ok(chunk_syms)) return RB200_E_ARG;
+    if (!container_mem_ok(mem_kind, out, nullptr)) return RB200_E_ARG;
     const bool device = mem_kind == RB200_MEM_DEVICE;
-    if ((!device && mem_kind != RB200_MEM_HOST) || (reinterpret_cast<uintptr_t>(out) & (device ? 15 : 7))) return RB200_E_ARG;
     if (!container_model_ok(static_cast<uint32_t>(model->coder), model->scale_bits, model->freqs)) return RB200_E_MODEL;
     const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
     if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
-    const size_t boff = container_blob_offset(n_chunks);
+    ContainerHeader h = container_header(model->coder, model->scale_bits, chunk_syms, n, n_chunks, 0, flags);
+    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
     if (out_cap < boff) return RB200_E_SPACE;
     DeviceGuard g(ctx->device);
-    ContainerHeader h = container_header(model->coder, model->scale_bits, chunk_syms, n, n_chunks, 0, flags);
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
-    uint64_t* dir = reinterpret_cast<uint64_t*>(out + kContainerDirOffset);
-    const size_t dir_bytes = (n_chunks + 1) * sizeof(uint64_t);
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
     if (device) {            // asynchronous: directory CRC, blob CRC, then the header from blob_bytes = dir[n_chunks]
         int rc = encode_device(ctx, model, in, n, chunk_syms, out + boff, out_cap - boff, dir);
-        if (rc == RB200_OK) rc = launch_crc(ctx, out + kContainerDirOffset, dir_bytes, nullptr, 0, ctx->d_crc);
+        if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
         if (rc != RB200_OK) return rc;
-        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, boff, out_cap, model->d_freqs, ctx->d_crc, ctx->d_status);
+        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, model->d_freqs, ctx->d_crc, ctx->d_status);
         return check_launch(ctx, "container_finish_kernel");
     }
     size_t blob_bytes = 0, slices = 0;
@@ -1335,7 +1362,7 @@ extern "C" int rb200_container_encode(rb200_ctx* ctx, const rb200_model* model, 
     h.meta_crc = container_meta_crc(h, model->freqs, dir);
     std::memcpy(out, &h, sizeof h);
     std::memcpy(out + sizeof h, model->freqs, sizeof model->freqs);
-    std::memset(out + kContainerDirOffset + dir_bytes, 0, boff - kContainerDirOffset - dir_bytes);
+    std::memset(out + dir_end, 0, boff - dir_end);
     if (out_size) *out_size = boff + blob_bytes;
     return RB200_OK;
 }
@@ -1344,12 +1371,62 @@ extern "C" int rb200_container_decode(rb200_ctx* ctx, const uint8_t* buf, size_t
                                       uint64_t* n_symbols, int mem_kind)
 {
     if (!ctx || !buf || (!out && out_cap)) return RB200_E_ARG;
-    const bool device = mem_kind == RB200_MEM_DEVICE;
-    const uintptr_t align = device ? 15 : 7;
-    if ((!device && mem_kind != RB200_MEM_HOST) || (reinterpret_cast<uintptr_t>(buf) & align) || (reinterpret_cast<uintptr_t>(out) & align))
-        return RB200_E_ARG;
+    if (!container_mem_ok(mem_kind, buf, out)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
-    return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, device);
+    return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, mem_kind == RB200_MEM_DEVICE, kContainerVersion);
+}
+
+// The per-block container: the block encoder writes every block's model (built, or the caller's tables copied in
+// first), the directory and the blob straight into their place in `out`; then as rb200_container_encode, except that
+// one CRC launch covers model and directory, which are contiguous.
+extern "C" int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                                             const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap,
+                                             size_t* out_size, int mem_kind)
+{
+    if (!ctx || !in || !out || !container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
+    if (!container_mem_ok(mem_kind, out, nullptr)) return RB200_E_ARG;
+    const bool device = mem_kind == RB200_MEM_DEVICE, build = block_freqs == nullptr;
+    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
+    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    if (!build && !device && !container_block_models_ok(block_freqs, n_blocks)) return RB200_E_MODEL;
+    ContainerHeader h = container_blocks_header(n_blocks, block_size, chunk_syms, 0, flags);
+    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
+    if (out_cap < boff) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
+    uint16_t* model = reinterpret_cast<uint16_t*>(out + sizeof(ContainerHeader));
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
+    const size_t model_bytes = dir_off - sizeof(ContainerHeader);
+    if (device) {            // asynchronous: model + directory CRC, blob CRC, then the header from blob_bytes = dir[n_chunks]
+        if (!build) RB_CUDA(ctx, cudaMemcpyAsync(model, block_freqs, model_bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+        int rc = blocks_encode_device(ctx, in, n_blocks, block_size, model, build, chunk_syms, out + boff, out_cap - boff, dir);
+        if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), nullptr, 0, ctx->d_crc);
+        if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+        if (rc != RB200_OK) return rc;
+        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, nullptr, ctx->d_crc, ctx->d_status);
+        return check_launch(ctx, "container_finish_kernel");
+    }
+    if (!build) std::memcpy(model, block_freqs, model_bytes);
+    size_t blob_bytes = 0, slices = 0;
+    int rc = blocks_encode_host(ctx, in, n_blocks, block_size, model, build, chunk_syms, out + boff, out_cap - boff, dir, &blob_bytes,
+                                SliceCrc{ctx, blob_crc, &slices});
+    if (rc == RB200_OK && blob_crc) rc = joined_slice_crc(ctx, slices, &h.blob_crc);
+    if (rc != RB200_OK) return rc;
+    h.blob_bytes = blob_bytes;
+    h.meta_crc = container_meta_crc(h, model, dir);
+    std::memcpy(out, &h, sizeof h);
+    std::memset(out + dir_end, 0, boff - dir_end);
+    if (out_size) *out_size = boff + blob_bytes;
+    return RB200_OK;
+}
+
+extern "C" int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                             uint64_t* n_symbols, int mem_kind)
+{
+    if (!ctx || !buf || (!out && out_cap)) return RB200_E_ARG;
+    if (!container_mem_ok(mem_kind, buf, out)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, mem_kind == RB200_MEM_DEVICE, kContainerVersionBlocks);
 }
 
 // ---------------------------------------------------------------------------

@@ -6,9 +6,16 @@ device buffers):
   rb200_decode against rb200_container_decode;
   host rb200_container_pack with RB200_CONTAINER_CRC_BLOB against rb200_crc32 in HOST mode, on the same blob.
 
+With --blocks, the per-block container on the per-GPU blocks workload (8192 blocks of 64 KiB, chunks of 8192, device
+buffers, per-block Zipf data with a permuted alphabet per block):
+
+  rb200_blocks_model_encode against rb200_container_blocks_encode (models built) with flags 0 and
+  RB200_CONTAINER_CRC_BLOB, alternated;
+  rb200_blocks_decode against rb200_container_blocks_decode (both CRCs checked).
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
-numbers.  Every output is checked against the plain calls plus rb200_container_pack.
-    python tools/container_timing.py [--reps 10] [--json out.json]"""
+numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
+    python tools/container_timing.py [--blocks] [--reps 10] [--json out.json]"""
 import argparse
 import json
 import os
@@ -52,14 +59,101 @@ def stats(ts):
     return {"median_ms": float(np.median(ts)), "min_ms": float(ts.min()), "max_ms": float(ts.max()), "n": int(ts.size)}
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--reps", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--json", default=None)
-    args = ap.parse_args()
+def alternate(calls, sync, warmup, reps):
+    """times every call `reps` times after `warmup` rounds, in alternation"""
+    times = {k: [] for k in calls}
+    for _ in range(warmup):
+        for f in calls.values():
+            timed(f, sync)
+    for _ in range(reps):
+        for k, f in calls.items():
+            times[k].append(timed(f, sync))
+    return {k: stats(v) for k, v in times.items()}
+
+
+def blocks_data(n_blocks, block_size, seed):
+    """per-block Zipf(0.6 + 0.1 (b % 9)) over a permuted alphabet per block, generated on the GPU"""
     import torch
-    assert torch.cuda.is_available(), "needs a CUDA device"
+    g = torch.Generator(device="cuda")
+    g.manual_seed(seed)
+    ranks = torch.arange(1, 257, device="cuda", dtype=torch.float64)
+    probs = torch.stack([1.0 / ranks ** (0.6 + 0.1 * e) for e in range(9)])
+    out = torch.empty(n_blocks * block_size, dtype=torch.uint8, device="cuda")
+    step = 256
+    for b0 in range(0, n_blocks, step):
+        nb = min(step, n_blocks - b0)
+        p = probs[torch.arange(b0, b0 + nb, device="cuda") % 9]
+        r = torch.multinomial(p, block_size, replacement=True, generator=g)
+        perm = torch.argsort(torch.rand(nb, 256, device="cuda", generator=g), dim=1)
+        out[b0 * block_size:(b0 + nb) * block_size] = torch.gather(perm, 1, r).to(torch.uint8).reshape(-1)
+    return out
+
+
+def blocks(args):
+    import torch
+    n_blocks, block_size, chunk = 8192, 65536, 8192
+    n = n_blocks * block_size
+    d_in = blocks_data(n_blocks, block_size, 1234)
+    ctx = rb.Context(0)
+    n_chunks = n // chunk
+    bound = ctx.encode_bound(n, chunk)
+    cap = ctx.container_blocks_capacity(n_blocks, block_size, chunk)
+    d_blob = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+    d_offs = torch.empty(n_chunks + 1, dtype=torch.int64, device="cuda")
+    d_freqs = torch.empty(n_blocks * 256, dtype=torch.int16, device="cuda")
+    d_cont = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_out = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+    sync = ctx.sync
+    calls = {
+        "blocks_model_encode": lambda: ctx.blocks_model_encode_device(d_in.data_ptr(), n_blocks, block_size, d_freqs.data_ptr(), chunk,
+                                                                      d_blob.data_ptr(), bound, d_offs.data_ptr()),
+        "container_blocks_encode": lambda: ctx.container_blocks_encode_device(d_in.data_ptr(), n_blocks, block_size, None, chunk, 0,
+                                                                              d_cont.data_ptr(), cap),
+        "container_blocks_encode_crc": lambda: ctx.container_blocks_encode_device(d_in.data_ptr(), n_blocks, block_size, None, chunk,
+                                                                                  api.CONTAINER_CRC_BLOB, d_cont.data_ptr(), cap),
+    }
+    enc = alternate(calls, sync, args.warmup, args.reps)
+
+    # outputs: both containers equal pack of the plain call's blob, directory and models
+    calls["blocks_model_encode"]()
+    sync()
+    blob_bytes = int(d_offs[n_chunks].item())
+    h_blob = d_blob[:blob_bytes].cpu().numpy()
+    h_offs = d_offs.cpu().numpy().view(np.uint64)
+    h_freqs = d_freqs.cpu().numpy().view(np.uint16).reshape(n_blocks, 256)
+    identical = {}
+    for flags, key in ((0, "container_blocks_encode"), (api.CONTAINER_CRC_BLOB, "container_blocks_encode_crc")):
+        want = api.container_blocks_pack(n_blocks, block_size, chunk, h_freqs, h_offs, h_blob, flags)
+        calls[key]()
+        sync()
+        identical[key + "_equals_pack"] = bool(np.array_equal(d_cont[:want.size].cpu().numpy(), want))
+    size = want.size                                                  # the CRC_BLOB container
+    d_want = torch.from_numpy(want).cuda()
+
+    dec = {
+        "blocks_decode": lambda: ctx.blocks_decode_device(d_blob.data_ptr(), blob_bytes, d_offs.data_ptr(), d_freqs.data_ptr(), n_blocks,
+                                                          block_size, chunk, d_out.data_ptr()),
+        "container_blocks_decode": lambda: ctx.container_blocks_decode_device(d_want.data_ptr(), size, d_out.data_ptr(), n),
+    }
+    dtimes = alternate(dec, sync, args.warmup, args.reps)
+    d_out.zero_()
+    dec["container_blocks_decode"]()
+    identical_decode = bool(torch.equal(d_out[:n], d_in))
+
+    res = {
+        "card": card(),
+        "workload": {"n_blocks": n_blocks, "block_size": block_size, "chunk_syms": chunk, "n": n, "blob_bytes": blob_bytes,
+                     "container_bytes": size, "prefix_bytes": size - blob_bytes},
+        "encode": enc,
+        "decode": dtimes,
+        "checks": {**identical, "container_blocks_decode_equals_input": identical_decode},
+    }
+    ctx.close()
+    return res
+
+
+def headline(args):
+    import torch
     n, chunk = 1 << 30, 8192
     g = torch.Generator(device="cuda")
     g.manual_seed(1234)
@@ -81,13 +175,7 @@ def main():
         "container_encode_crc": lambda: ctx.container_encode_device(model, d_in.data_ptr(), n, chunk, api.CONTAINER_CRC_BLOB,
                                                                     d_cont.data_ptr(), cap),
     }
-    times = {k: [] for k in calls}
-    for _ in range(args.warmup):
-        for f in calls.values():
-            timed(f, sync)
-    for _ in range(args.reps):
-        for k, f in calls.items():
-            times[k].append(timed(f, sync))
+    enc = alternate(calls, sync, args.warmup, args.reps)
 
     # outputs: the CRC_BLOB container (last call) equals pack of the plain encode's blob and directory
     calls["encode"]()
@@ -117,13 +205,7 @@ def main():
         "decode": lambda: ctx.decode_device(model, d_blob.data_ptr(), blob_bytes, d_offs.data_ptr(), chunk, d_out.data_ptr(), n),
         "container_decode": lambda: ctx.container_decode_device(d_want.data_ptr(), size, d_out.data_ptr(), n),
     }
-    dtimes = {k: [] for k in dec}
-    for _ in range(args.warmup):
-        for f in dec.values():
-            timed(f, sync)
-    for _ in range(args.reps):
-        for k, f in dec.items():
-            dtimes[k].append(timed(f, sync))
+    dtimes = alternate(dec, sync, args.warmup, args.reps)
     d_out.zero_()
     dec["container_decode"]()
     identical_decode = bool(torch.equal(d_out[:n], d_in))
@@ -141,20 +223,32 @@ def main():
         "card": card(),
         "workload": {"n": n, "coder": "word", "chunk_syms": chunk, "blob_bytes": blob_bytes, "container_bytes": size},
         "crc32_device_1GiB": {**stats(crc_times), "share_of_3.35TBps": n / HBM_BPS * 1e3 / float(np.median(crc_times))},
-        "encode": {k: stats(v) for k, v in times.items()},
-        "decode": {k: stats(v) for k, v in dtimes.items()},
+        "encode": enc,
+        "decode": dtimes,
         "host_blob": {"container_pack_crc_blob_ms": t_pack * 1e3, "rb200_crc32_host_mode": stats(host_crc)},
         "checks": {"container_encode_equals_pack": identical_encode, "container_decode_equals_input": identical_decode,
                    "crc32_device_equals_header": bool(crc_ok), "crc32_host_equals_header": bool(host_crc_ok)},
     }
+    model.close()
+    ctx.close()
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
+    ap.add_argument("--reps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+    import torch
+    assert torch.cuda.is_available(), "needs a CUDA device"
+    res = blocks(args) if args.blocks else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
             json.dump(res, f, indent=1)
-    ok = all(res["checks"].values())
-    model.close()
-    ctx.close()
-    sys.exit(0 if ok else 1)
+    sys.exit(0 if all(res["checks"].values()) else 1)
 
 
 if __name__ == "__main__":
