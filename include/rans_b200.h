@@ -220,6 +220,16 @@ int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_
  * decode kernel runs (a rejected container leaves out untouched); HOST mode takes the blob CRC per slice. */
 int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                   uint64_t* n_symbols, int mem_kind);
+/* rb200_container_blocks_decode for a container in DEVICE memory, with nothing done on the host: the header, every
+ * block's model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, then the block decoder
+ * runs -- all enqueued on the context stream; the call never synchronises, copies to the host or allocates, so it can
+ * be captured in a CUDA graph.  buf and out 16-byte aligned.  size = bytes available at buf (a shorter container is
+ * accepted, as by rb200_container_blocks_open).  d_n_symbols (device memory, may be NULL) receives n once header,
+ * models and directory pass.  The call returns only RB200_E_ARG (null / misaligned / bad mem) or RB200_E_CUDA;
+ * every verdict on the container comes from rb200_sync: RB200_E_STREAM for anything rb200_container_blocks_open
+ * rejects, RB200_E_SPACE for n > out_cap; in both cases out is untouched. */
+int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                        uint64_t* d_n_symbols);
 
 /* ---------------------------------------------------------------- multi-GPU: gathering the shards' blobs (NCCL) */
 

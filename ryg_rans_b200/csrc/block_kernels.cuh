@@ -280,6 +280,27 @@ __device__ __forceinline__ bool block_prefix(const F* freqs, uint32_t* s_cum, ui
     return *s_bad == 0;
 }
 
+// RansWordTablesInitSymbol for every slot (rans_word_sse41.h:64-72) from the cumulative table in s_cum.  Each thread
+// owns a run of consecutive slots: one binary search over the cumulative table for the first, then it walks forward,
+// so the work is balanced however skewed the model is.  Sets *s_wide when one symbol takes all 4096 slots.  The
+// caller puts a CTA barrier between this and the first read of s_tab.
+__device__ __forceinline__ void block_fill_slots(const uint32_t* s_cum, uint32_t* s_tab, uint32_t* s_wide)
+{
+    const uint32_t per = kWordSlots / blockDim.x;                // blockDim is a power of two between 128 and 1024
+    uint32_t slot = threadIdx.x * per;
+    uint32_t lo = 0, hi = 256;                                   // largest s with cum[s] <= slot
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (s_cum[mid] <= slot) lo = mid; else hi = mid;
+    }
+    for (uint32_t j = 0; j < per; j++, slot++) {
+        while (slot >= s_cum[lo + 1]) lo++;                      // also steps over zero-width symbols
+        const uint32_t f = s_cum[lo + 1] - s_cum[lo];
+        if (f == kWordSlots) *s_wide = 1;
+        s_tab[slot] = ((f & 0xfffu) << 20) | ((slot - s_cum[lo]) << 8) | lo;
+    }
+}
+
 __global__ void __launch_bounds__(kMaxBlockWarps * 32)
 block_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets,
                     const uint16_t* __restrict__ block_freqs, uint32_t block_size, uint32_t chunk_syms,
@@ -298,24 +319,7 @@ block_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const 
         if (tid == 0) atomicOr(status, kStatStream);
         return;
     }
-    // RansWordTablesInitSymbol for every slot (rans_word_sse41.h:64-72).  Each thread owns a run of
-    // consecutive slots: one binary search over the cumulative table for the first, then it walks
-    // forward, so the work is balanced however skewed the model is.
-    {
-        const uint32_t per = kWordSlots / blockDim.x;            // blockDim is a power of two between 128 and 1024
-        uint32_t slot = tid * per;
-        uint32_t lo = 0, hi = 256;                               // largest s with cum[s] <= slot
-        while (hi - lo > 1) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (s_cum[mid] <= slot) lo = mid; else hi = mid;
-        }
-        for (uint32_t j = 0; j < per; j++, slot++) {
-            while (slot >= s_cum[lo + 1]) lo++;                  // also steps over zero-width symbols
-            const uint32_t f = s_cum[lo + 1] - s_cum[lo];
-            if (f == kWordSlots) s_flag[1] = 1;
-            s_tab[slot] = ((f & 0xfffu) << 20) | ((slot - s_cum[lo]) << 8) | lo;
-        }
-    }
+    block_fill_slots(s_cum, s_tab, &s_flag[1]);
     __syncthreads();
 
     const uint32_t per_block = block_size / chunk_syms;

@@ -6,6 +6,14 @@
 
 #include "rans_b200.h"
 
+// The layout and the rules below are compiled for the host and, under nvcc, for the device too: the kernels of
+// rb200_container_blocks_decode_async (container_decode.cuh) apply the same functions as the host parser.
+#ifdef __CUDACC__
+#define RB200_HD __host__ __device__
+#else
+#define RB200_HD
+#endif
+
 namespace rb200 {
 
 constexpr uint32_t kContainerMagic = 0x43324252u;   // "RB2C"
@@ -37,13 +45,13 @@ constexpr size_t kBlockModelBytes = 256 * sizeof(uint16_t);                     
 // The layout, as functions of the (parsed) header: model section, directory, pad to 16, blob.  Version 1 keeps 1024
 // bytes of model, so its directory stays at 1088; version 2 has 512 bytes per block, so its directory starts at
 // 64 + 512 n_blocks, also 16-aligned.  64-bit throughout: n_blocks < 2^32 and n_chunks < 2^31 once parsed.
-inline uint64_t container_model_bytes(const ContainerHeader& h)
+RB200_HD inline uint64_t container_model_bytes(const ContainerHeader& h)
 {
     return h.version == kContainerVersionBlocks ? kBlockModelBytes * h.n_blocks : 256 * sizeof(uint32_t);
 }
-inline uint64_t container_dir_offset(const ContainerHeader& h) { return sizeof(ContainerHeader) + container_model_bytes(h); }
-inline uint64_t container_dir_end(const ContainerHeader& h) { return container_dir_offset(h) + (h.n_chunks + 1) * sizeof(uint64_t); }
-inline uint64_t container_blob_offset(const ContainerHeader& h) { return (container_dir_end(h) + 15) & ~15ull; }
+RB200_HD inline uint64_t container_dir_offset(const ContainerHeader& h) { return sizeof(ContainerHeader) + container_model_bytes(h); }
+RB200_HD inline uint64_t container_dir_end(const ContainerHeader& h) { return container_dir_offset(h) + (h.n_chunks + 1) * sizeof(uint64_t); }
+RB200_HD inline uint64_t container_blob_offset(const ContainerHeader& h) { return (container_dir_end(h) + 15) & ~15ull; }
 
 // a header with only what the layout depends on: for sizes computed before there is a header
 inline ContainerHeader container_shape(uint16_t version, uint32_t n_blocks, uint64_t n_chunks)
@@ -56,11 +64,47 @@ inline ContainerHeader container_shape(uint16_t version, uint32_t n_blocks, uint
 }
 
 // the chunk sizes the kernels take (32 .. 2^24 symbols)
-inline bool container_chunk_ok(uint32_t chunk_syms) { return chunk_syms >= 32 && chunk_syms <= (1u << 24); }
+RB200_HD inline bool container_chunk_ok(uint32_t chunk_syms) { return chunk_syms >= 32 && chunk_syms <= (1u << 24); }
 // per-block geometry: whole chunks per block, at most 32 (one CTA per block, one warp per chunk)
-inline bool container_blocks_geometry_ok(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms)
+RB200_HD inline bool container_blocks_geometry_ok(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms)
 {
     return n_blocks && block_size && container_chunk_ok(chunk_syms) && block_size % chunk_syms == 0 && block_size / chunk_syms <= 32;
+}
+
+// Every rule of a header (already read from the first 64 of `size` bytes) for the one `version` the caller accepts:
+// the fields agree with each other and with the geometry the decoders take, and every section fits `size`.
+RB200_HD inline bool container_header_ok(const ContainerHeader& h, uint64_t size, uint16_t version)
+{
+    if (h.magic != kContainerMagic || h.version != version || h.lanes != RB200_LANES || !h.chunk_syms) return false;
+    if (version == kContainerVersionBlocks) {
+        // what rb200_blocks_decode accepts; n_blocks * block_size cannot overflow 64 bits
+        if (h.coder != RB200_CODER_WORD || h.scale_bits != 12 || !container_blocks_geometry_ok(h.n_blocks, h.block_size, h.chunk_syms))
+            return false;
+        if (h.n_symbols != static_cast<uint64_t>(h.n_blocks) * h.block_size || h.n_chunks != h.n_symbols / h.chunk_syms ||
+            h.n_chunks >= (1ull << 31) || (h.blob_bytes & 15) || h.reserved || (h.flags & ~RB200_CONTAINER_CRC_BLOB))
+            return false;
+    } else if (h.n_chunks != h.n_symbols / h.chunk_syms + (h.n_symbols % h.chunk_syms != 0) || h.n_chunks >= (1ull << 31) ||
+               (h.blob_bytes & 15) || h.coder > RB200_CODER_RANS64 || h.scale_bits < 8 || h.scale_bits > 16) {
+        return false;
+    }
+    const uint64_t boff = container_blob_offset(h);                 // < 2^42: n_chunks < 2^31, n_blocks < 2^32
+    return boff <= size && h.blob_bytes <= size - boff;
+}
+
+// The per-element rules of a version 2 prefix, one block or one directory entry at a time.
+// one block's 256 frequencies sum to 4096
+RB200_HD inline bool container_block_model_ok(const uint16_t* freqs)
+{
+    uint32_t sum = 0;
+    for (int s = 0; s < 256; s++) sum += freqs[s];
+    return sum == 4096;
+}
+// entry c (< n_chunks) of the directory is not above the next one
+RB200_HD inline bool container_dir_step_ok(const uint64_t* offsets, uint64_t c) { return offsets[c] <= offsets[c + 1]; }
+// the first stream starts inside the first vector, the last entry is the blob size
+RB200_HD inline bool container_dir_ends_ok(const uint64_t* offsets, uint64_t n_chunks, uint64_t blob_bytes)
+{
+    return offsets[n_chunks] == blob_bytes && (!n_chunks || offsets[0] < 16);
 }
 
 // the header rb200_container_pack writes (crc fields zero)

@@ -25,6 +25,8 @@
 // on one core: the blob CRC is optional for that reason).  rb200_container_encode / _decode and the _blocks_ forms
 // (rans_b200.cu) write and read the same bytes in host or device memory with the blob CRC on the GPU
 // (crc_kernels.cuh); they validate through the parser below, so both sides apply one set of rules.
+// rb200_container_blocks_decode_async applies the same rules in kernels (container_decode.cuh): the header and
+// per-element rules are the __host__ __device__ functions of container_format.h that the parser below calls.
 #include "container_format.h"
 
 #include <cstring>
@@ -95,20 +97,16 @@ bool container_model_ok(uint32_t coder, uint32_t scale_bits, const uint32_t* fre
 
 bool container_block_models_ok(const uint16_t* block_freqs, uint32_t n_blocks)
 {
-    for (uint64_t b = 0; b < n_blocks; b++) {
-        uint32_t sum = 0;
-        for (int s = 0; s < 256; s++) sum += block_freqs[b * 256 + s];
-        if (sum != 4096) return false;
-    }
+    for (uint64_t b = 0; b < n_blocks; b++)
+        if (!container_block_model_ok(block_freqs + b * 256)) return false;
     return true;
 }
 
 bool container_directory_ok(const uint64_t* offsets, uint64_t n_chunks, uint64_t blob_bytes)
 {
-    if (offsets[n_chunks] != blob_bytes) return false;
-    if (n_chunks && offsets[0] >= 16) return false;                                       // the first stream starts inside the first vector
+    if (!container_dir_ends_ok(offsets, n_chunks, blob_bytes)) return false;
     for (uint64_t c = 0; c < n_chunks; c++)
-        if (offsets[c] > offsets[c + 1]) return false;
+        if (!container_dir_step_ok(offsets, c)) return false;
     return true;
 }
 
@@ -144,20 +142,7 @@ int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, Co
     if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
     ContainerHeader h;
     std::memcpy(&h, hdr, sizeof h);
-    if (h.magic != kContainerMagic || h.version != version || h.lanes != RB200_LANES || !h.chunk_syms) return RB200_E_STREAM;
-    if (version == kContainerVersionBlocks) {
-        // what rb200_blocks_decode accepts; n_blocks * block_size cannot overflow 64 bits
-        if (h.coder != RB200_CODER_WORD || h.scale_bits != 12 || !container_blocks_geometry_ok(h.n_blocks, h.block_size, h.chunk_syms))
-            return RB200_E_STREAM;
-        if (h.n_symbols != static_cast<uint64_t>(h.n_blocks) * h.block_size || h.n_chunks != h.n_symbols / h.chunk_syms ||
-            h.n_chunks >= (1ull << 31) || (h.blob_bytes & 15) || h.reserved || (h.flags & ~RB200_CONTAINER_CRC_BLOB))
-            return RB200_E_STREAM;
-    } else if (h.n_chunks != h.n_symbols / h.chunk_syms + (h.n_symbols % h.chunk_syms != 0) || h.n_chunks >= (1ull << 31) ||
-               (h.blob_bytes & 15) || h.coder > RB200_CODER_RANS64 || h.scale_bits < 8 || h.scale_bits > 16) {
-        return RB200_E_STREAM;
-    }
-    const uint64_t boff = container_blob_offset(h);                 // < 2^42: n_chunks < 2^31, n_blocks < 2^32
-    if (boff > size || h.blob_bytes > size - boff) return RB200_E_STREAM;
+    if (!container_header_ok(h, size, version)) return RB200_E_STREAM;
     *out = h;
     return RB200_OK;
 }

@@ -163,10 +163,12 @@ __device__ __forceinline__ uint32_t step_byte(uint32_t c, uint32_t b, uint32_t t
 }  // namespace crc_detail
 
 // zlib crc32(data[0, n), crc_in) -> slot.  With n_dev set the length is min(*n_dev, n): a length the device wrote
-// (a directory's last entry), bounded by the buffer.  Any n and any alignment of data.  work must be zero (it is left zero).
+// (a directory's last entry), bounded by the buffer.  With off_dev set the bytes start *off_dev bytes after data (a
+// position the device wrote), and n still bounds them from data.  Any n and any alignment of data.  work must be zero
+// (it is left zero).
 __global__ void __launch_bounds__(kCrcThreads, 1)
-    crc32_kernel(const uint8_t* __restrict__ data, uint64_t n, const uint64_t* __restrict__ n_dev, uint32_t crc_in, CrcWork* work,
-                 CrcSlot* slot)
+    crc32_kernel(const uint8_t* __restrict__ data, uint64_t n, const uint64_t* __restrict__ n_dev, const uint64_t* __restrict__ off_dev,
+                 uint32_t crc_in, CrcWork* work, CrcSlot* slot)
 {
     using namespace crc_detail;
     extern __shared__ uint4 crc_smem_v[];
@@ -182,6 +184,11 @@ __global__ void __launch_bounds__(kCrcThreads, 1)
         if (threadIdx.x < 64) pow[threadIdx.x] = kCrcPowersDev.p[threadIdx.x];
     }
     __syncthreads();
+    if (off_dev) {
+        const uint64_t skip = *off_dev < n ? *off_dev : n;
+        data += skip;
+        n -= skip;
+    }
     if (n_dev && *n_dev < n) n = *n_dev;
 
     // thread t owns span bytes [t L, (t + 1) L) of the 16-aligned span that starts a0 bytes before data

@@ -17,6 +17,7 @@
 
 #include "alias_kernels.cuh"
 #include "block_kernels.cuh"
+#include "container_decode.cuh"
 #include "container_format.h"
 #include "crc_kernels.cuh"
 #include "rans64_kernels.cuh"
@@ -60,6 +61,9 @@ struct rb200_ctx {
     CrcWork* d_crc_work = nullptr;
     CrcSlot* d_crc = nullptr;            // kMaxSlices entries
     CrcSlot* h_crc = nullptr;
+    // rb200_container_blocks_decode_async (container_decode.cuh): its fixed workspace and launch shapes
+    BlocksAsyncWork* d_blocks_async = nullptr;
+    BlocksAsyncShape blocks_async = {};
 };
 
 struct rb200_model {
@@ -217,6 +221,8 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     if (e == cudaSuccess) e = cudaMemset(ctx->d_crc_work, 0, sizeof(CrcWork));
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_crc, rb200_ctx::kMaxSlices * sizeof(CrcSlot));
     if (e == cudaSuccess) e = cudaMallocHost(&ctx->h_crc, rb200_ctx::kMaxSlices * sizeof(CrcSlot));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_blocks_async, sizeof(BlocksAsyncWork));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_async, 0, sizeof(BlocksAsyncWork));
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -228,6 +234,7 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     configure_block_kernels();
     configure_rans64_kernels();
     configure_crc_kernels();
+    ctx->blocks_async = configure_container_decode(static_cast<uint32_t>(ctx->sms));
     cudaGetLastError();
     *out = ctx;
     return RB200_OK;
@@ -248,6 +255,7 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->d_crc_work) cudaFree(ctx->d_crc_work);
     if (ctx->d_crc) cudaFree(ctx->d_crc);
     if (ctx->h_crc) cudaFreeHost(ctx->h_crc);
+    if (ctx->d_blocks_async) cudaFree(ctx->d_blocks_async);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -1184,7 +1192,8 @@ namespace {
 int launch_crc(rb200_ctx* ctx, const uint8_t* d, uint64_t n, const uint64_t* n_dev, uint32_t crc_in, CrcSlot* slot)
 {
     const uint32_t sms = static_cast<uint32_t>(ctx->sms);
-    crc32_kernel<<<n_dev ? sms : crc32_grid(sms, n), kCrcThreads, kCrcSmemBytes, ctx->stream>>>(d, n, n_dev, crc_in, ctx->d_crc_work, slot);
+    crc32_kernel<<<n_dev ? sms : crc32_grid(sms, n), kCrcThreads, kCrcSmemBytes, ctx->stream>>>(d, n, n_dev, nullptr, crc_in,
+                                                                                                ctx->d_crc_work, slot);
     return check_launch(ctx, "crc32_kernel");
 }
 
@@ -1427,6 +1436,40 @@ extern "C" int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf,
     if (!container_mem_ok(mem_kind, buf, out)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
     return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, mem_kind == RB200_MEM_DEVICE, kContainerVersionBlocks);
+}
+
+// The kernels of container_decode.cuh, with lengths and positions the host cannot know taken from the plan on the
+// device; the host passes only bounds it knows (size).  Six launches, no copy, no synchronisation, no allocation.
+extern "C" int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                                   uint64_t* d_n_symbols)
+{
+    if (!ctx || !buf || !out || (reinterpret_cast<uintptr_t>(d_n_symbols) & 7)) return RB200_E_ARG;
+    if (!container_mem_ok(RB200_MEM_DEVICE, buf, out)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    BlocksAsyncWork* w = ctx->d_blocks_async;
+    const BlocksAsyncShape& shape = ctx->blocks_async;
+    const uint32_t sms = static_cast<uint32_t>(ctx->sms);
+    const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
+    cudaStream_t s = ctx->stream;
+    container_plan_kernel<<<1, 32, 0, s>>>(buf, size, w);
+    int rc = check_launch(ctx, "container_plan_kernel");
+    if (rc != RB200_OK) return rc;
+    crc32_kernel<<<crc32_grid(sms, after_head), kCrcThreads, kCrcSmemBytes, s>>>(buf + sizeof(ContainerHeader), after_head, &w->plan.meta_len,
+                                                                                 nullptr, 0, &w->crc_work, &w->crc[0]);
+    rc = check_launch(ctx, "crc32_kernel(meta)");
+    if (rc != RB200_OK) return rc;
+    crc32_kernel<<<crc32_grid(sms, size), kCrcThreads, kCrcSmemBytes, s>>>(buf, size, &w->plan.blob_len, &w->plan.blob_off, 0,
+                                                                           &w->crc_work, &w->crc[1]);
+    rc = check_launch(ctx, "crc32_kernel(blob)");
+    if (rc != RB200_OK) return rc;
+    container_prefix_check_kernel<<<shape.check_grid, kPrefixWarps * 32, 0, s>>>(buf, w);
+    rc = check_launch(ctx, "container_prefix_check_kernel");
+    if (rc != RB200_OK) return rc;
+    container_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status);
+    rc = check_launch(ctx, "container_verdict_kernel");
+    if (rc != RB200_OK) return rc;
+    block_decode_planned_kernel<<<shape.decode_grid, kPlannedWarps * 32, 0, s>>>(buf, out, w, ctx->d_status);
+    return check_launch(ctx, "block_decode_planned_kernel");
 }
 
 // ---------------------------------------------------------------------------

@@ -11,7 +11,9 @@ buffers, per-block Zipf data with a permuted alphabet per block):
 
   rb200_blocks_model_encode against rb200_container_blocks_encode (models built) with flags 0 and
   RB200_CONTAINER_CRC_BLOB, alternated;
-  rb200_blocks_decode against rb200_container_blocks_decode (both CRCs checked).
+  rb200_blocks_decode against rb200_container_blocks_decode and rb200_container_blocks_decode_async, each container
+  call with flags 0 and RB200_CONTAINER_CRC_BLOB, alternated; and the host time each container decode call takes to
+  return.
 
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
@@ -122,23 +124,39 @@ def blocks(args):
     h_offs = d_offs.cpu().numpy().view(np.uint64)
     h_freqs = d_freqs.cpu().numpy().view(np.uint16).reshape(n_blocks, 256)
     identical = {}
+    d_want = {}                                                       # flags -> the container in device memory
     for flags, key in ((0, "container_blocks_encode"), (api.CONTAINER_CRC_BLOB, "container_blocks_encode_crc")):
         want = api.container_blocks_pack(n_blocks, block_size, chunk, h_freqs, h_offs, h_blob, flags)
         calls[key]()
         sync()
         identical[key + "_equals_pack"] = bool(np.array_equal(d_cont[:want.size].cpu().numpy(), want))
-    size = want.size                                                  # the CRC_BLOB container
-    d_want = torch.from_numpy(want).cuda()
+        d_want[flags] = torch.from_numpy(want).cuda()
+    size = want.size                                                  # both flags give the same size
+    crc = api.CONTAINER_CRC_BLOB
 
     dec = {
         "blocks_decode": lambda: ctx.blocks_decode_device(d_blob.data_ptr(), blob_bytes, d_offs.data_ptr(), d_freqs.data_ptr(), n_blocks,
                                                           block_size, chunk, d_out.data_ptr()),
-        "container_blocks_decode": lambda: ctx.container_blocks_decode_device(d_want.data_ptr(), size, d_out.data_ptr(), n),
+        "container_blocks_decode": lambda: ctx.container_blocks_decode_device(d_want[0].data_ptr(), size, d_out.data_ptr(), n),
+        "container_blocks_decode_crc": lambda: ctx.container_blocks_decode_device(d_want[crc].data_ptr(), size, d_out.data_ptr(), n),
+        "container_blocks_decode_async": lambda: ctx.container_blocks_decode_async(d_want[0].data_ptr(), size, d_out.data_ptr(), n),
+        "container_blocks_decode_async_crc": lambda: ctx.container_blocks_decode_async(d_want[crc].data_ptr(), size, d_out.data_ptr(), n),
     }
     dtimes = alternate(dec, sync, args.warmup, args.reps)
-    d_out.zero_()
-    dec["container_blocks_decode"]()
-    identical_decode = bool(torch.equal(d_out[:n], d_in))
+    # host time until each container decode call returns (the synchronous call waits for the GPU; the async one enqueues)
+    host = {k: [] for k in dec if k != "blocks_decode"}
+    for _ in range(args.reps):
+        for k in host:
+            t0 = time.perf_counter()
+            dec[k]()
+            host[k].append((time.perf_counter() - t0) * 1e3)
+            sync()
+    decode_ok = {}
+    for k in dec:
+        d_out.zero_()
+        dec[k]()
+        sync()
+        decode_ok[k + "_equals_input"] = bool(torch.equal(d_out[:n], d_in))
 
     res = {
         "card": card(),
@@ -146,7 +164,8 @@ def blocks(args):
                      "container_bytes": size, "prefix_bytes": size - blob_bytes},
         "encode": enc,
         "decode": dtimes,
-        "checks": {**identical, "container_blocks_decode_equals_input": identical_decode},
+        "decode_call_host_ms": {k: stats(v) for k, v in host.items()},
+        "checks": {**identical, **decode_ok},
     }
     ctx.close()
     return res

@@ -81,6 +81,29 @@ def main():
     except rb.RansError:
         pass
     m.close()
+    # the per-block container decoded by kernels alone: valid, then a corrupt model and a corrupt blob (both rejected
+    # before any decode)
+    cap = ctx.container_blocks_capacity(nb, bs, chunk)
+    d_cb = torch.zeros(cap + 16, dtype=torch.uint8, device="cuda")
+    d_n = torch.zeros(1, dtype=torch.int64, device="cuda")
+    ctx.container_blocks_encode_device(d_in.data_ptr(), nb, bs, None, chunk, api.CONTAINER_CRC_BLOB, d_cb.data_ptr(), cap)
+    d_out.zero_()
+    ctx.container_blocks_decode_async(d_cb.data_ptr(), cap, d_out.data_ptr(), data.size, d_n.data_ptr())
+    ctx.sync()
+    assert int(d_n.item()) == data.size and torch.equal(d_out[:data.size], d_in)
+    h_cb = d_cb[:cap].cpu().numpy()
+    boff = api.container_blocks_open(h_cb)[3].ctypes.data - h_cb.ctypes.data
+    for pos in (64 + 3, boff + 1000):
+        d_cb[pos] ^= 1
+        d_out.zero_()
+        ctx.container_blocks_decode_async(d_cb.data_ptr(), cap, d_out.data_ptr(), data.size, d_n.data_ptr())
+        try:
+            ctx.sync()
+            raise SystemExit("per-block container corruption not reported")
+        except rb.RansError:
+            pass
+        assert not d_out.any().item()
+        d_cb[pos] ^= 1
     print("sanitize smoke ok:", ctx.launches, "launches")
 
 
