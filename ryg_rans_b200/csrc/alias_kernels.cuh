@@ -450,46 +450,32 @@ alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_s
     }
     __syncthreads();
 
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t warp = threadIdx.x >> 5;
     const uint32_t base = smem_addr(s_alias);
     const uint32_t wsm = base + warp * kEncWarpSmem;
     const AliasEncoder<ALIAS, SB> coder = {base + kAliasEncWarps * kEncWarpSmem, base + kAliasEncFixedSmem, sb};
     if (!look) {
         for (uint32_t chunk = blockIdx.x * kAliasEncWarps + warp; chunk < n_chunks; chunk += gridDim.x * kAliasEncWarps) {
-            const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
-            const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-            const uint32_t produced = encode_stream(in + first, m, coder, wsm, scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, status);
-            if (lane == 0) sizes[chunk] = produced;
+            const ChunkRange r = chunk_range(chunk, chunk_syms, n);
+            encode_chunk_split(in + r.first, r.m, chunk, coder, wsm, scratch, slot_bytes, sizes, status);
         }
         return;
     }
-    if (blockIdx.x == 0 && warp == 0) {
-        fused_scanner(look, n_chunks, lane, status);
-        return;
-    }
-    const PlaceOut out = {look, n_chunks, blob, blob_cap, offsets, status};
-    SlotQueue<kAliasFusedSlots> q(scratch, blockIdx.x * kAliasEncWarps + warp, slot_bytes);
-    for (;;) {
-        uint32_t chunk = 0;
-        if (lane == 0) chunk = atomicAdd(counter, 1u);
-        chunk = __shfl_sync(0xffffffffu, chunk, 0);
-        if (chunk >= n_chunks) break;
-        const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
-        const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-        const uint32_t produced = encode_stream(in + first, m, coder, wsm, q.next_end(), status);
-        q.finish(out, chunk, produced, lane);
-    }
-    q.drain(out, lane);
+    encode_chunks_fused<kAliasFusedSlots, kAliasEncWarps, false>(in, n, chunk_syms, coder, wsm, scratch, slot_bytes,
+                                                                 PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
 }
 
+// dynamic shared memory of the alias (remap != nullptr) or byte encoder at scale_bits sb
+inline uint32_t alias_encode_smem(bool alias, uint32_t sb) { return kAliasEncFixedSmem + (alias ? (2u << sb) : 0u); }
+
 // scale_bits the kernels are specialised for (main_alias.cpp:276 uses 16, main.cpp:136 / main64.cpp:136 use 14, the word
-// coder's 12); every other value runs the generic instantiation (SB = 0).
+// coder's 12); every other value runs the generic instantiation (SB = 0).  Each is configured for scale_bits 16, the
+// most shared memory any of them is launched with.
 template <bool ALIAS, uint32_t SB>
 inline void configure_alias_encode()
 {
     cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         kAliasEncFixedSmem + (ALIAS ? (2u << 16) : 0u));
+    cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, alias_encode_smem(ALIAS, 16));
 }
 template <uint32_t SB>
 inline void configure_byte_decode()
@@ -527,23 +513,20 @@ inline void configure_alias_kernels()
     }
 
 // remap == nullptr selects the rans_byte cum2sym coder.  look == nullptr: split mode (sizes[] out, one slot per
-// chunk); otherwise fused mode (kAliasFusedSlots slots per resident warp; look/counter zeroed by the caller).
-// sms = multiprocessors of the context's device (rb200_ctx keeps it; nothing process-wide is cached here).
-inline int launch_alias_encode(cudaStream_t stream, uint32_t sms, const uint8_t* d_in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
-                               uint32_t sb, const AliasEncEntry* enc, const uint16_t* remap, uint8_t* scratch, uint32_t slot,
-                               uint32_t* sizes, uint64_t* look, uint32_t* counter, uint8_t* blob, uint64_t blob_cap, uint64_t* offsets,
-                               uint32_t* status)
+// chunk); otherwise fused mode (kAliasFusedSlots slots per worker warp; look/counter zeroed by the caller).
+// grid <= one CTA per SM (the kernel is persistent), smem = alias_encode_smem(remap != nullptr, sb).
+inline void launch_alias_encode(cudaStream_t stream, uint32_t grid, uint32_t smem, const uint8_t* d_in, uint64_t n, uint32_t chunk_syms,
+                                uint32_t n_chunks, uint32_t sb, const AliasEncEntry* enc, const uint16_t* remap, uint8_t* scratch,
+                                uint32_t slot, uint32_t* sizes, uint64_t* look, uint32_t* counter, uint8_t* blob, uint64_t blob_cap,
+                                uint64_t* offsets, uint32_t* status)
 {
-    uint32_t grid = (n_chunks + (look ? 1 : 0) + kAliasEncWarps - 1) / kAliasEncWarps;
-    if (grid > sms) grid = sms;                       // persistent: one CTA per SM
     if (remap) {
-        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_kernel<true, SB><<<grid, kAliasEncWarps * 32, kAliasEncFixedSmem + (2u << sb), stream>>>(
+        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_kernel<true, SB><<<grid, kAliasEncWarps * 32, smem, stream>>>(
             d_in, n, chunk_syms, n_chunks, sb, enc, remap, scratch, slot, sizes, look, counter, blob, blob_cap, offsets, status)))
     } else {
-        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_kernel<false, SB><<<grid, kAliasEncWarps * 32, kAliasEncFixedSmem, stream>>>(
+        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_kernel<false, SB><<<grid, kAliasEncWarps * 32, smem, stream>>>(
             d_in, n, chunk_syms, n_chunks, sb, enc, nullptr, scratch, slot, sizes, look, counter, blob, blob_cap, offsets, status)))
     }
-    return 0;
 }
 
 // the persistent kernel: sms x 2 CTAs of 20 warps, chunk ids from the context's work counter

@@ -395,9 +395,9 @@ block_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, const u
     const uint8_t* src = in + static_cast<uint64_t>(blockIdx.x) * block_size + static_cast<uint64_t>(warp) * chunk_syms;
     const uint32_t wsm = smem_addr(s_enc) + kEncTableBytes + warp * kEncWarpSmem;
     if (r32)
-        word_encode_chunk<true>(src, chunk_syms, chunk, smem_addr(s_enc), wsm, scratch, slot_bytes, sizes, status);
+        encode_chunk_split(src, chunk_syms, chunk, WordEncoder<true>{smem_addr(s_enc)}, wsm, scratch, slot_bytes, sizes, status);
     else
-        word_encode_chunk<false>(src, chunk_syms, chunk, smem_addr(s_enc), wsm, scratch, slot_bytes, sizes, status);
+        encode_chunk_split(src, chunk_syms, chunk, WordEncoder<false>{smem_addr(s_enc)}, wsm, scratch, slot_bytes, sizes, status);
 }
 
 // K5f: per-block encode in ONE persistent launch -- model (optional), tables, encode, directory, placement.
@@ -466,12 +466,15 @@ inline uint32_t block_threads(uint32_t block_size, uint32_t chunk_syms)
     return warps * 32;
 }
 
-template <bool BUILD, int WARPS>
-inline void configure_block_fused()
+// dynamic shared memory of both per-block encoders (K5, K5f) at `threads` threads: the table, then 1 KiB per warp
+inline uint32_t block_encode_smem(uint32_t threads) { return kEncTableBytes + (threads / 32) * kEncWarpSmem; }
+
+// the instance of the fused per-block encoder for blocks of block_threads() = `threads`
+using BlockEncodeFusedKernel = decltype(&block_encode_fused_kernel<true, 8>);
+inline BlockEncodeFusedKernel block_encode_fused_for(bool build, uint32_t threads)
 {
-    cudaFuncSetAttribute(block_encode_fused_kernel<BUILD, WARPS>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(block_encode_fused_kernel<BUILD, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         kEncTableBytes + WARPS * kEncWarpSmem);
+    if (threads <= 256) return build ? block_encode_fused_kernel<true, 8> : block_encode_fused_kernel<false, 8>;
+    return build ? block_encode_fused_kernel<true, 32> : block_encode_fused_kernel<false, 32>;
 }
 
 inline void configure_block_kernels()
@@ -480,53 +483,13 @@ inline void configure_block_kernels()
     // ~17.4 KiB static (table, cumulative, flag) + 1 KiB of ring per warp: above 48 KiB from 31 warps on, so opt in
     cudaFuncSetAttribute(block_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxBlockWarps * kRingBytes);
     cudaFuncSetAttribute(block_encode_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(block_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncTableBytes + kMaxBlockWarps * kEncWarpSmem);
-    configure_block_fused<true, 8>(); configure_block_fused<false, 8>(); configure_block_fused<true, 32>(); configure_block_fused<false, 32>();
-}
-
-// grid of the fused per-block encoder: CTA 0 (scanner) + as many worker CTAs as are resident at once
-inline uint32_t block_fused_grid(uint32_t sms, uint32_t n_blocks, uint32_t threads, bool build)
-{
-    int per_sm = 0;
-    const size_t smem = kEncTableBytes + (threads / 32) * kEncWarpSmem;
-    const int t = static_cast<int>(threads);
-    if (threads <= 256) {
-        if (build) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_encode_fused_kernel<true, 8>, t, smem);
-        else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_encode_fused_kernel<false, 8>, t, smem);
-    } else {
-        if (build) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_encode_fused_kernel<true, 32>, t, smem);
-        else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_encode_fused_kernel<false, 32>, t, smem);
-    }
-    if (per_sm < 1) per_sm = 1;
-    uint64_t workers = static_cast<uint64_t>(sms) * per_sm - 1;       // the scanner CTA takes one slot
-    if (workers > n_blocks) workers = n_blocks;
-    if (workers < 1) workers = 1;
-    return static_cast<uint32_t>(workers + 1);
-}
-
-inline void launch_block_encode_fused(cudaStream_t stream, uint32_t grid, uint32_t threads, bool build, const uint8_t* d_in, uint32_t n_blocks,
-                                      uint32_t block_size, uint16_t* d_freqs, uint32_t chunk_syms, uint8_t* scratch, uint32_t slot,
-                                      uint64_t* look, uint32_t* counter, uint8_t* blob, uint64_t blob_cap, uint64_t* offsets, uint32_t* status)
-{
-    const size_t smem = kEncTableBytes + (threads / 32) * kEncWarpSmem;
-#define RB200_BLOCK_FUSED_LAUNCH(B, W)                                                                                              \
-    block_encode_fused_kernel<B, W><<<grid, threads, smem, stream>>>(d_in, n_blocks, block_size, d_freqs, chunk_syms, scratch, slot, look, \
-                                                                     counter, blob, blob_cap, offsets, status)
-    if (threads <= 256) {
-        if (build) RB200_BLOCK_FUSED_LAUNCH(true, 8); else RB200_BLOCK_FUSED_LAUNCH(false, 8);
-    } else {
-        if (build) RB200_BLOCK_FUSED_LAUNCH(true, 32); else RB200_BLOCK_FUSED_LAUNCH(false, 32);
-    }
-#undef RB200_BLOCK_FUSED_LAUNCH
-}
-
-inline void launch_block_encode(cudaStream_t stream, const uint8_t* d_in, uint32_t n_blocks, uint32_t block_size,
-                                const uint16_t* d_freqs, uint32_t chunk_syms, uint8_t* scratch, uint32_t slot,
-                                uint32_t* sizes, uint32_t* status)
-{
-    const uint32_t threads = block_threads(block_size, chunk_syms);
-    block_encode_kernel<<<n_blocks, threads, kEncTableBytes + (threads / 32) * kEncWarpSmem, stream>>>(d_in, block_size, d_freqs, chunk_syms,
-                                                                                                       scratch, slot, sizes, status);
+    cudaFuncSetAttribute(block_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(kMaxBlockWarps * 32));
+    for (const bool build : {true, false})
+        for (const uint32_t threads : {8u * 32, 32u * 32}) {
+            cudaFuncSetAttribute(block_encode_fused_for(build, threads), cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 cudaSharedmemCarveoutMaxShared);
+            cudaFuncSetAttribute(block_encode_fused_for(build, threads), cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
+        }
 }
 
 inline void launch_block_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets,

@@ -160,4 +160,26 @@ __device__ __forceinline__ uint32_t encode_stream(const uint8_t* __restrict__ ch
     return produced;
 }
 
+// The symbols of chunk `chunk` of in[0, n): in[first, first + m), m = chunk_syms except for a ragged last chunk.
+struct ChunkRange {
+    uint64_t first;
+    uint32_t m;
+};
+__device__ __forceinline__ ChunkRange chunk_range(uint32_t chunk, uint32_t chunk_syms, uint64_t n)
+{
+    const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
+    return {first, static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first))};
+}
+
+// The split path's store (K6 compacts after it): encode chunk `chunk` (m symbols at chunk_in) into the end of its own
+// worst-case slot of `scratch` and record its size in sizes[chunk].
+template <class Coder>
+__device__ __forceinline__ void encode_chunk_split(const uint8_t* __restrict__ chunk_in, uint32_t m, uint32_t chunk, const Coder coder,
+                                                   uint32_t wsm, uint8_t* __restrict__ scratch, uint32_t slot_bytes,
+                                                   uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
+{
+    const uint32_t produced = encode_stream(chunk_in, m, coder, wsm, scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, status);
+    if ((threadIdx.x & 31) == 0) sizes[chunk] = produced;
+}
+
 }  // namespace rb200

@@ -1,5 +1,6 @@
 // placement.cuh -- how the fused encoders (word K2f, the fused mode of the alias / byte encoder, per-block K5f) turn
-// finished chunk streams into the container, and the stream copy the split path's compaction (K6) shares with them.
+// finished chunk streams into the container, the chunk loop K2f and the alias / byte encoder run it from, and the stream
+// copy the split path's compaction (K6) shares with them.
 //
 // Every worker warp fetches chunk ids in order, encodes a chunk into one of its own scratch slots and publishes the
 // padded size in look[chunk].  One scanner warp of the grid turns the published sizes into end offsets in chunk order.
@@ -9,6 +10,7 @@
 // than the split path because of polling; see DESIGN.md section 6.)
 #pragma once
 #include "device_utils.cuh"
+#include "encode_stream.cuh"
 
 namespace rb200 {
 
@@ -242,5 +244,32 @@ struct SlotQueue {
             }
     }
 };
+
+// The chunk loop of a fused encoder of WARPS warps per CTA (K2f, the fused alias / byte mode).  Warp 0 of CTA 0 is the
+// scanner; every other warp takes chunk ids from `counter` (zeroed by the host, so chunks start in order), encodes each
+// into its SlotQueue<SLOTS> and places it SLOTS - 1 chunks later.  No CTA barrier: warps are independent from here on.
+// wsm = this warp's 1 KiB of shared memory, KEEP as in encode_stream.
+template <uint32_t SLOTS, uint32_t WARPS, bool KEEP, class Coder>
+__device__ __forceinline__ void encode_chunks_fused(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, const Coder coder,
+                                                    uint32_t wsm, uint8_t* __restrict__ scratch, uint32_t slot_bytes, const PlaceOut& out,
+                                                    uint32_t* __restrict__ counter)
+{
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (blockIdx.x == 0 && warp == 0) {
+        fused_scanner(out.look, out.n_chunks, lane, out.status);
+        return;
+    }
+    SlotQueue<SLOTS> q(scratch, blockIdx.x * WARPS + warp, slot_bytes);
+    for (;;) {
+        uint32_t chunk = 0;
+        if (lane == 0) chunk = atomicAdd(counter, 1u);
+        chunk = __shfl_sync(0xffffffffu, chunk, 0);
+        if (chunk >= out.n_chunks) break;
+        const ChunkRange r = chunk_range(chunk, chunk_syms, n);
+        const uint32_t produced = encode_stream<KEEP>(in + r.first, r.m, coder, wsm, q.next_end(), out.status);
+        q.finish(out, chunk, produced, lane);
+    }
+    q.drain(out, lane);
+}
 
 }  // namespace rb200

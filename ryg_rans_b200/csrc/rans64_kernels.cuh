@@ -145,19 +145,18 @@ rans64_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_
     const uint32_t warp = threadIdx.x >> 5;
     const uint32_t chunk = blockIdx.x * kRans64Warps + warp;
     if (chunk >= n_chunks) return;
-    const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
-    const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-    const uint32_t produced = encode_stream(in + first, m, Rans64Encoder{smem_addr(s_tab), sb},
-                                            smem_addr(s_r64e) + warp * kEncWarpSmem, scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, status);
-    if ((threadIdx.x & 31) == 0) sizes[chunk] = produced;
+    const ChunkRange r = chunk_range(chunk, chunk_syms, n);
+    encode_chunk_split(in + r.first, r.m, chunk, Rans64Encoder{smem_addr(s_tab), sb}, smem_addr(s_r64e) + warp * kEncWarpSmem, scratch,
+                       slot_bytes, sizes, status);
 }
+constexpr uint32_t kRans64EncSmemBytes = kRans64Warps * kEncWarpSmem + kEncTableBytes;     // dynamic shared memory of the encoder
 
 inline void configure_rans64_kernels()
 {
     cudaFuncSetAttribute(rans64_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRans64Warps * kRingBytes + kRans64DecSymBytes + (1u << 16));
     cudaFuncSetAttribute(rans64_decode_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(rans64_encode_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(rans64_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRans64Warps * kEncWarpSmem + kEncTableBytes);
+    cudaFuncSetAttribute(rans64_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRans64EncSmemBytes);
 }
 
 inline void launch_rans64_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets, uint32_t sb,
@@ -166,14 +165,6 @@ inline void launch_rans64_decode(cudaStream_t stream, const uint8_t* blob, uint6
     const uint32_t grid = (n_chunks + kRans64Warps - 1) / kRans64Warps;
     rans64_decode_kernel<<<grid, kRans64Warps * 32, kRans64Warps * kRingBytes + kRans64DecSymBytes + (1u << sb), stream>>>(
         blob, blob_size, offsets, sb, table, out, n, chunk_syms, n_chunks, status);
-}
-
-inline void launch_rans64_encode(cudaStream_t stream, const uint8_t* d_in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb,
-                                 const uint4* enc, uint8_t* scratch, uint32_t slot, uint32_t* sizes, uint32_t* status)
-{
-    const uint32_t grid = (n_chunks + kRans64Warps - 1) / kRans64Warps;
-    rans64_encode_kernel<<<grid, kRans64Warps * 32, kRans64Warps * kEncWarpSmem + kEncTableBytes, stream>>>(d_in, n, chunk_syms, n_chunks, sb, enc,
-                                                                                                  scratch, slot, sizes, status);
 }
 
 }  // namespace rb200

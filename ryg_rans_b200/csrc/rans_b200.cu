@@ -9,6 +9,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -451,20 +452,6 @@ int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* siz
     return check_launch(ctx, "compact_kernel");
 }
 
-int reserve_encode_workspace(rb200_ctx* ctx, uint32_t n_chunks, uint32_t slot, uint8_t** scratch, uint32_t** sizes, uint64_t** tile_sums)
-{
-    int rc = reserve(ctx, ctx->scratch, static_cast<size_t>(n_chunks) * slot + 16);
-    if (rc != RB200_OK) return rc;
-    const size_t sizes_bytes = round16((static_cast<size_t>(n_chunks) + 1) * sizeof(uint32_t));
-    const size_t tiles = (static_cast<size_t>(n_chunks) + kScanTile - 1) / kScanTile + 1;
-    rc = reserve(ctx, ctx->sizes, sizes_bytes + tiles * sizeof(uint64_t));
-    if (rc != RB200_OK) return rc;
-    *scratch = static_cast<uint8_t*>(ctx->scratch.p);
-    *sizes = static_cast<uint32_t*>(ctx->sizes.p);
-    *tile_sums = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + sizes_bytes);
-    return RB200_OK;
-}
-
 // Word-coder encode has two paths:
 //   fused: ONE persistent launch -- workers encode, a scanner warp turns published sizes into end offsets
 //          in chunk order, workers place chunk k after encoding chunk k+1 (placement.cuh);
@@ -472,6 +459,7 @@ int reserve_encode_workspace(rb200_ctx* ctx, uint32_t n_chunks, uint32_t slot, u
 // fused is faster as long as the scanner keeps up, i.e. for chunks of >= 4096 symbols; below that the split path
 // is used (H100 SXM at a 400 W power limit, 1 GiB uniform bytes: 1.89 vs 2.21 ms per call at chunks of 8192, 2.10 vs
 // 2.25 ms at 4096, but 2.80 vs 2.36 ms at 2048).  RB200_ENCODE_PATH=split|fused forces one.
+// Only the encode plans (plan_encode, plan_blocks_encode) ask.
 bool use_fused_encode(uint32_t chunk_syms)
 {
     static const int forced = [] {           // read once; thread-safe static initialisation
@@ -484,71 +472,94 @@ bool use_fused_encode(uint32_t chunk_syms)
     return chunk_syms >= 4096;
 }
 
-uint32_t fused_word_grid(rb200_ctx* ctx, uint32_t n_chunks)
-{
-    const uint32_t want = (n_chunks + 1 + kEncWarps - 1) / kEncWarps;       // + 1: one warp of the grid is the scanner
-    const uint32_t grid = static_cast<uint32_t>(ctx->sms) * RB200_FUSED_MINBLOCKS;
-    return grid > want ? want : grid;
-}
-
-// The fused encoders' workspace: `slots` scratch slots of `slot` bytes, and in ctx->sizes the chunk counter (16 bytes)
-// followed by look[n_chunks] (placement.cuh).
-struct FusedWorkspace {
-    uint8_t* scratch;
-    uint64_t* look;
-    uint32_t* counter;
+// How one encode call over n_chunks chunks runs, decided once: the path, the encode launch's shape, and the workspace
+// both need.  Fused: one launch of `grid` CTAs with `slots` scratch slots (slots per worker warp x the warps of the grid);
+// in ctx->sizes the chunk counter (16 bytes), then look[n_chunks] (placement.cuh).  Split: the encode launch into one
+// slot per chunk, then finish_encode; in ctx->sizes sizes[n_chunks], then the scan's tile sums.
+struct EncodePlan {
+    bool fused;
+    uint32_t grid, threads, smem;      // the encode launch (dynamic shared memory in bytes)
+    size_t slots;
+    uint32_t slot_bytes;
+    uint32_t n_chunks;
 };
 
-int reserve_fused(rb200_ctx* ctx, size_t slots, uint32_t slot, uint32_t n_chunks)
+EncodePlan plan_encode(const rb200_ctx* ctx, const rb200_model* model, uint32_t n_chunks, uint32_t chunk_syms)
 {
-    int rc = reserve(ctx, ctx->scratch, slots * slot + 16);
-    if (rc == RB200_OK) rc = reserve(ctx, ctx->sizes, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t));
+    EncodePlan p = {};
+    p.n_chunks = n_chunks;
+    p.slot_bytes = slot_bytes_for(chunk_syms);
+    p.fused = n_chunks && model->coder != RB200_CODER_RANS64 && use_fused_encode(chunk_syms);
+    p.slots = n_chunks;
+    const uint32_t sms = static_cast<uint32_t>(ctx->sms);
+    if (model->coder == RB200_CODER_WORD) {
+        p.threads = kEncWarps * 32;
+        p.smem = kEncSmemBytes;
+        if (p.fused) {
+            const uint32_t want = (n_chunks + 1 + kEncWarps - 1) / kEncWarps;     // + 1: one warp of the grid is the scanner
+            p.grid = std::min(want, sms * RB200_FUSED_MINBLOCKS);
+            p.slots = static_cast<size_t>(p.grid) * kEncWarps * kFusedSlots;
+        } else {
+            p.grid = (n_chunks + kEncWarps - 1) / kEncWarps;
+        }
+    } else if (model->coder == RB200_CODER_RANS64) {
+        p.threads = kRans64Warps * 32;
+        p.smem = kRans64EncSmemBytes;
+        p.grid = (n_chunks + kRans64Warps - 1) / kRans64Warps;
+    } else {                           // alias / byte: persistent, at most one CTA per SM
+        p.threads = kAliasEncWarps * 32;
+        p.smem = alias_encode_smem(model->coder == RB200_CODER_ALIAS, model->scale_bits);
+        p.grid = std::min((n_chunks + (p.fused ? 1 : 0) + kAliasEncWarps - 1) / kAliasEncWarps, sms);
+        if (p.fused) p.slots = static_cast<size_t>(sms) * kAliasEncWarps * kAliasFusedSlots;
+    }
+    return p;
+}
+
+// Bytes of the u32 part of ctx->sizes (the fused path's counter, the split path's sizes[]); the u64 part follows.
+size_t plan_head_bytes(const EncodePlan& p)
+{
+    return p.fused ? 16 : round16((static_cast<size_t>(p.n_chunks) + 1) * sizeof(uint32_t));
+}
+
+// Grows ctx->scratch and ctx->sizes to what `p` needs (the host pipeline does this once for its largest slice so that
+// no slice has to stall on a reallocation).
+int reserve_plan(rb200_ctx* ctx, const EncodePlan& p)
+{
+    const size_t n = p.n_chunks;
+    const size_t longs = p.fused ? n : (n + kScanTile - 1) / kScanTile + 1;
+    int rc = reserve(ctx, ctx->scratch, p.slots * p.slot_bytes + 16);
+    if (rc == RB200_OK) rc = reserve(ctx, ctx->sizes, plan_head_bytes(p) + longs * sizeof(uint64_t));
     return rc;
 }
 
-// reserve_fused, then zero the counter and look[] on the context's stream
-int fused_workspace(rb200_ctx* ctx, size_t slots, uint32_t slot, uint32_t n_chunks, FusedWorkspace* ws)
+// The workspace of a plan, as the encode kernels take it; the pointers of the other path are null.
+struct EncodeWorkspace {
+    uint8_t* scratch;
+    uint32_t* counter;     // fused
+    uint64_t* look;        // fused
+    uint32_t* sizes;       // split
+    uint64_t* tile_sums;   // split
+};
+
+// Runs a plan: reserve its workspace; fused: zero the counter and look[], then `launch(ws)`, the one kernel; split:
+// `launch(ws)` encodes into the slots (when there are chunks), then finish_encode.  `launch` returns check_launch's code.
+template <class Launch>
+int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, Launch launch)
 {
-    int rc = reserve_fused(ctx, slots, slot, n_chunks);
+    int rc = reserve_plan(ctx, p);
     if (rc != RB200_OK) return rc;
-    RB_CUDA(ctx, cudaMemsetAsync(ctx->sizes.p, 0, 16 + static_cast<size_t>(n_chunks) * sizeof(uint64_t), ctx->stream));
-    ws->scratch = static_cast<uint8_t*>(ctx->scratch.p);
-    ws->counter = static_cast<uint32_t*>(ctx->sizes.p);
-    ws->look = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + 16);
-    return RB200_OK;
-}
-
-// scratch slots of the fused word or alias / byte encoder: slots per warp x the warps of its largest grid
-size_t fused_slot_count(rb200_ctx* ctx, int coder, uint32_t n_chunks)
-{
-    if (coder == RB200_CODER_WORD) return static_cast<size_t>(fused_word_grid(ctx, n_chunks)) * kEncWarps * kFusedSlots;
-    return static_cast<size_t>(ctx->sms) * kAliasEncWarps * kAliasFusedSlots;     // launch_alias_encode: <= one CTA per SM
-}
-
-int encode_word_fused(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_in, size_t n, uint32_t chunk_syms, uint32_t n_chunks,
-                      uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets)
-{
-    const uint32_t slot = slot_bytes_for(chunk_syms);
-    FusedWorkspace ws = {};
-    int rc = fused_workspace(ctx, fused_slot_count(ctx, RB200_CODER_WORD, n_chunks), slot, n_chunks, &ws);
-    if (rc != RB200_OK) return rc;
-    auto kernel = model->enc_r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>;
-    kernel<<<fused_word_grid(ctx, n_chunks), kEncWarps * 32, kEncSmemBytes, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->d_word_enc,
-                                                                                           ws.scratch, slot, ws.look, ws.counter, d_blob,
-                                                                                           blob_cap, d_offsets, ctx->d_status);
-    return check_launch(ctx, "word_encode_fused_kernel");
-}
-
-// Grows the encode workspaces to what a call over `n_chunks` chunks needs (the host pipeline does this once
-// for its largest slice so that no slice has to stall on a reallocation).
-int reserve_encode(rb200_ctx* ctx, const rb200_model* model, uint32_t n_chunks, uint32_t chunk_syms)
-{
-    if (!n_chunks) return RB200_OK;
-    const uint32_t slot = slot_bytes_for(chunk_syms);
-    if (use_fused_encode(chunk_syms) && model->coder != RB200_CODER_RANS64)
-        return reserve_fused(ctx, fused_slot_count(ctx, model->coder, n_chunks), slot, n_chunks);
-    uint8_t* scratch; uint32_t* sizes; uint64_t* tile_sums;
-    return reserve_encode_workspace(ctx, n_chunks, slot, &scratch, &sizes, &tile_sums);
+    uint8_t* scratch = static_cast<uint8_t*>(ctx->scratch.p);
+    uint32_t* head = static_cast<uint32_t*>(ctx->sizes.p);
+    uint64_t* tail = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + plan_head_bytes(p));
+    if (p.fused) {
+        RB_CUDA(ctx, cudaMemsetAsync(ctx->sizes.p, 0, 16 + static_cast<size_t>(p.n_chunks) * sizeof(uint64_t), ctx->stream));
+        return launch(EncodeWorkspace{scratch, head, tail, nullptr, nullptr});
+    }
+    if (p.n_chunks) {
+        rc = launch(EncodeWorkspace{scratch, nullptr, nullptr, head, tail});
+        if (rc != RB200_OK) return rc;
+    }
+    return finish_encode(ctx, scratch, p.slot_bytes, head, tail, p.n_chunks, d_blob, blob_cap, d_offsets);
 }
 
 int encode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_in, size_t n, uint32_t chunk_syms,
@@ -557,46 +568,31 @@ int encode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_in,
     const size_t n_chunks_sz = rb200_chunk_count(n, chunk_syms);
     if (n_chunks_sz >= (1ull << 31)) return RB200_E_ARG;
     const uint32_t n_chunks = static_cast<uint32_t>(n_chunks_sz);
-    const bool fused = n_chunks && use_fused_encode(chunk_syms);
-    if (fused && model->coder == RB200_CODER_WORD)
-        return encode_word_fused(ctx, model, d_in, n, chunk_syms, n_chunks, d_blob, blob_cap, d_offsets);
-    const uint32_t slot = slot_bytes_for(chunk_syms);
-    if (fused && (model->coder == RB200_CODER_ALIAS || model->coder == RB200_CODER_BYTE)) {
-        FusedWorkspace ws = {};
-        int rc = fused_workspace(ctx, fused_slot_count(ctx, model->coder, n_chunks), slot, n_chunks, &ws);
-        if (rc != RB200_OK) return rc;
-        const bool alias = model->coder == RB200_CODER_ALIAS;
-        launch_alias_encode(ctx->stream, static_cast<uint32_t>(ctx->sms), d_in, n, chunk_syms, n_chunks, model->scale_bits, alias ? model->d_alias_enc : model->d_byte_enc,
-                            alias ? model->d_alias_remap : nullptr, ws.scratch, slot, nullptr, ws.look, ws.counter,
-                            d_blob, blob_cap, d_offsets, ctx->d_status);
-        return check_launch(ctx, alias ? "alias_encode_kernel(fused)" : "byte_encode_kernel(fused)");
-    }
-    uint8_t* scratch; uint32_t* sizes; uint64_t* tile_sums;
-    int rc = reserve_encode_workspace(ctx, n_chunks, slot, &scratch, &sizes, &tile_sums);
-    if (rc != RB200_OK) return rc;
-    if (n_chunks) {
+    const EncodePlan p = plan_encode(ctx, model, n_chunks, chunk_syms);
+    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, [&](const EncodeWorkspace& ws) {
         if (model->coder == RB200_CODER_WORD) {
-            const uint32_t grid = (n_chunks + kEncWarps - 1) / kEncWarps;
+            if (p.fused) {
+                auto kernel = model->enc_r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>;
+                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->d_word_enc, ws.scratch, p.slot_bytes,
+                                                                   ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status);
+                return check_launch(ctx, "word_encode_fused_kernel");
+            }
             auto kernel = model->enc_r32 ? word_encode_kernel<true> : word_encode_kernel<false>;
-            kernel<<<grid, kEncWarps * 32, kEncSmemBytes, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->d_word_enc, scratch, slot,
-                                                                         sizes, ctx->d_status);
-            rc = check_launch(ctx, "word_encode_kernel");
-        } else if (model->coder == RB200_CODER_ALIAS) {
-            rc = launch_alias_encode(ctx->stream, static_cast<uint32_t>(ctx->sms), d_in, n, chunk_syms, n_chunks, model->scale_bits, model->d_alias_enc,
-                                     model->d_alias_remap, scratch, slot, sizes, nullptr, nullptr, nullptr, 0, nullptr, ctx->d_status);
-            if (rc == RB200_OK) rc = check_launch(ctx, "alias_encode_kernel");
-        } else if (model->coder == RB200_CODER_BYTE) {
-            rc = launch_alias_encode(ctx->stream, static_cast<uint32_t>(ctx->sms), d_in, n, chunk_syms, n_chunks, model->scale_bits, model->d_byte_enc, nullptr, scratch,
-                                     slot, sizes, nullptr, nullptr, nullptr, 0, nullptr, ctx->d_status);
-            if (rc == RB200_OK) rc = check_launch(ctx, "byte_encode_kernel");
-        } else {
-            launch_rans64_encode(ctx->stream, d_in, n, chunk_syms, n_chunks, model->scale_bits, model->d_r64_enc, scratch, slot, sizes,
-                                 ctx->d_status);
-            rc = check_launch(ctx, "rans64_encode_kernel");
+            kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->d_word_enc, ws.scratch, p.slot_bytes,
+                                                               ws.sizes, ctx->d_status);
+            return check_launch(ctx, "word_encode_kernel");
         }
-        if (rc != RB200_OK) return rc;
-    }
-    return finish_encode(ctx, scratch, slot, sizes, tile_sums, n_chunks, d_blob, blob_cap, d_offsets);
+        if (model->coder == RB200_CODER_RANS64) {
+            rans64_encode_kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->scale_bits, model->d_r64_enc,
+                                                                             ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status);
+            return check_launch(ctx, "rans64_encode_kernel");
+        }
+        const bool alias = model->coder == RB200_CODER_ALIAS;
+        launch_alias_encode(ctx->stream, p.grid, p.smem, d_in, n, chunk_syms, n_chunks, model->scale_bits, alias ? model->d_alias_enc : model->d_byte_enc,
+                            alias ? model->d_alias_remap : nullptr, ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob,
+                            blob_cap, d_offsets, ctx->d_status);
+        return check_launch(ctx, alias ? "alias_encode_kernel" : "byte_encode_kernel");
+    });
 }
 
 int decode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_blob, size_t blob_size, const uint64_t* d_offsets,
@@ -738,12 +734,12 @@ struct NoSliceHook {
 // copied out.  Every slice is its own container in a staging region; because containers end 16-byte
 // aligned they concatenate, and the directory entries only need the running base added.  Directories are
 // staged in pinned memory (an async copy to a pageable `offsets` would block the issuing thread).
-// `reserve_ws(units)` grows the encode workspace for a slice of that many units; it runs once, for the largest slice,
-// so that no slice stalls on a reallocation.  `encode_slice(slice, d_in, d_table, d_blob, cap, d_offsets)` enqueues
-// one slice's encode on ctx->stream.
-template <class ReserveWs, class EncodeSlice, class Hook = NoSliceHook>
+// `plan_slice(slice)` is the encode plan of a slice; the plan of the largest slice is reserved up front, so that no
+// slice stalls on a reallocation.  `encode_slice(slice, d_in, d_table, d_blob, cap, d_offsets)` enqueues one slice's
+// encode on ctx->stream.
+template <class PlanSlice, class EncodeSlice, class Hook = NoSliceHook>
 int encode_pipeline(rb200_ctx* ctx, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t unit_chunks, UnitTable tab,
-                    ReserveWs reserve_ws, EncodeSlice encode_slice, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size,
+                    PlanSlice plan_slice, EncodeSlice encode_slice, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size,
                     Hook hook = Hook{})
 {
     if (n == 0) {
@@ -755,8 +751,8 @@ int encode_pipeline(rb200_ctx* ctx, const uint8_t* in, size_t n, uint32_t chunk_
     const size_t n_units = rb200_chunk_count(n, unit_syms), n_chunks = n_units * unit_chunks;
     Slice sl[rb200_ctx::kMaxSlices];
     const size_t n_slices = plan_slices(n, unit_syms, unit_chunks, sl);
-    size_t max_units = 0;
-    for (size_t i = 0; i < n_slices; i++) max_units = sl[i].units > max_units ? sl[i].units : max_units;
+    const Slice* largest = &sl[0];
+    for (size_t i = 1; i < n_slices; i++) largest = sl[i].units > largest->units ? &sl[i] : largest;
     const size_t slot = slot_bytes_for(chunk_syms);
     // slice i's container is built at bound(symbols before it); its directory at c0 + i (cnt + 1 entries)
     int rc = reserve(ctx, ctx->st_in, n + 16);
@@ -764,7 +760,7 @@ int encode_pipeline(rb200_ctx* ctx, const uint8_t* in, size_t n, uint32_t chunk_
     if (rc == RB200_OK) rc = reserve(ctx, ctx->st_offsets, (n_chunks + n_slices) * sizeof(uint64_t));
     if (rc == RB200_OK) rc = reserve(ctx, ctx->st_aux, n_units * tab.unit_bytes);
     if (rc == RB200_OK) rc = reserve_dir(ctx, n_chunks + n_slices);
-    if (rc == RB200_OK) rc = reserve_ws(max_units);
+    if (rc == RB200_OK) rc = reserve_plan(ctx, plan_slice(*largest));
     if (rc != RB200_OK) return rc;
     uint8_t* d_in = static_cast<uint8_t*>(ctx->st_in.p);
     uint8_t* d_blob = static_cast<uint8_t*>(ctx->st_blob.p);
@@ -918,7 +914,7 @@ int encode_host(rb200_ctx* ctx, const rb200_model* model, const uint8_t* in, siz
 {
     return encode_pipeline(
         ctx, in, n, chunk_syms, 1, UnitTable{},
-        [&](size_t units) { return reserve_encode(ctx, model, static_cast<uint32_t>(units), chunk_syms); },
+        [&](const Slice& s) { return plan_encode(ctx, model, static_cast<uint32_t>(s.cnt), chunk_syms); },
         [&](const Slice& s, const uint8_t* d_in, uint8_t*, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
             return encode_device(ctx, model, d_in, s.len, chunk_syms, d_blob, cap, d_off);
         },
@@ -1044,32 +1040,28 @@ namespace {
 
 constexpr size_t kBlockFreqBytes = 256 * sizeof(uint16_t);     // one block's frequency table
 
-// The per-block encoder's launch shape over `n_blocks` blocks: the fused kernel on `grid` CTAs of `threads` threads with
-// `slots` scratch slots (slots per warp x the warps of its grid), or the split sequence when grid is 0.
-// blocks_encode_device and reserve_blocks_encode size the workspace from it.
-struct BlockEncodeShape {
-    uint32_t threads, grid;
-    size_t slots;
-};
-
-BlockEncodeShape block_encode_shape(rb200_ctx* ctx, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, bool build_models)
+// The plan of a per-block encode over n_blocks blocks (n_blocks x block_size / chunk_syms < 2^31 chunks): the fused
+// kernel (CTA 0 the scanner, then as many worker CTAs as are resident at once, at most one per block) whenever it builds
+// the models, or the split sequence (one CTA per block) when use_fused_encode says so.
+EncodePlan plan_blocks_encode(const rb200_ctx* ctx, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, bool build)
 {
-    if (!use_fused_encode(chunk_syms) && !build_models) return BlockEncodeShape{0, 0, 0};
-    const uint32_t threads = block_threads(block_size, chunk_syms);
-    const uint32_t grid = block_fused_grid(static_cast<uint32_t>(ctx->sms), n_blocks, threads, build_models);
-    return BlockEncodeShape{threads, grid, static_cast<size_t>(grid) * (threads / 32) * kBlockFusedSlots};
-}
-
-// Grows the encode workspaces to what a per-block encode over `n_blocks` blocks needs (the host pipeline does this once
-// for its largest slice, which holds far fewer than 2^31 chunks).
-int reserve_blocks_encode(rb200_ctx* ctx, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, bool build_models)
-{
-    const uint32_t n_chunks = n_blocks * (block_size / chunk_syms);
-    const uint32_t slot = slot_bytes_for(chunk_syms);
-    const BlockEncodeShape shape = block_encode_shape(ctx, n_blocks, block_size, chunk_syms, build_models);
-    if (shape.grid) return reserve_fused(ctx, shape.slots, slot, n_chunks);
-    uint8_t* scratch; uint32_t* sizes; uint64_t* tile_sums;
-    return reserve_encode_workspace(ctx, n_chunks, slot, &scratch, &sizes, &tile_sums);
+    EncodePlan p = {};
+    p.n_chunks = n_blocks * (block_size / chunk_syms);
+    p.slot_bytes = slot_bytes_for(chunk_syms);
+    p.fused = build || use_fused_encode(chunk_syms);
+    p.threads = block_threads(block_size, chunk_syms);
+    p.smem = block_encode_smem(p.threads);
+    if (!p.fused) {
+        p.grid = n_blocks;
+        p.slots = p.n_chunks;
+        return p;
+    }
+    int per_sm = 0;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_encode_fused_for(build, p.threads), static_cast<int>(p.threads), p.smem);
+    const uint64_t workers = static_cast<uint64_t>(ctx->sms) * std::max(per_sm, 1) - 1;      // the scanner CTA takes one slot
+    p.grid = static_cast<uint32_t>(std::max<uint64_t>(std::min<uint64_t>(workers, n_blocks), 1) + 1);
+    p.slots = static_cast<size_t>(p.grid) * (p.threads / 32) * kBlockFusedSlots;
+    return p;
 }
 
 // Per-block encode.  Default: ONE persistent launch (block_encode_fused_kernel: [model,] tables, encode, directory,
@@ -1078,27 +1070,19 @@ int reserve_blocks_encode(rb200_ctx* ctx, uint32_t n_blocks, uint32_t block_size
 int blocks_encode_device(rb200_ctx* ctx, const uint8_t* d_in, uint32_t n_blocks, uint32_t block_size, uint16_t* d_freqs,
                          bool build_models, uint32_t chunk_syms, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets)
 {
-    const uint32_t per_block = block_size / chunk_syms;
-    const uint64_t n_chunks64 = static_cast<uint64_t>(n_blocks) * per_block;
-    if (n_chunks64 >= (1ull << 31)) return RB200_E_ARG;
-    const uint32_t n_chunks = static_cast<uint32_t>(n_chunks64);
-    const uint32_t slot = slot_bytes_for(chunk_syms);
-    const BlockEncodeShape shape = block_encode_shape(ctx, n_blocks, block_size, chunk_syms, build_models);
-    if (shape.grid) {
-        FusedWorkspace ws = {};
-        int rc = fused_workspace(ctx, shape.slots, slot, n_chunks, &ws);
-        if (rc != RB200_OK) return rc;
-        launch_block_encode_fused(ctx->stream, shape.grid, shape.threads, build_models, d_in, n_blocks, block_size, d_freqs, chunk_syms,
-                                  ws.scratch, slot, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status);
-        return check_launch(ctx, "block_encode_fused_kernel");
-    }
-    uint8_t* scratch; uint32_t* sizes; uint64_t* tile_sums;
-    int rc = reserve_encode_workspace(ctx, n_chunks, slot, &scratch, &sizes, &tile_sums);
-    if (rc != RB200_OK) return rc;
-    launch_block_encode(ctx->stream, d_in, n_blocks, block_size, d_freqs, chunk_syms, scratch, slot, sizes, ctx->d_status);
-    rc = check_launch(ctx, "block_encode_kernel");
-    if (rc != RB200_OK) return rc;
-    return finish_encode(ctx, scratch, slot, sizes, tile_sums, n_chunks, d_blob, blob_cap, d_offsets);
+    if (static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) >= (1ull << 31)) return RB200_E_ARG;
+    const EncodePlan p = plan_blocks_encode(ctx, n_blocks, block_size, chunk_syms, build_models);
+    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, [&](const EncodeWorkspace& ws) {
+        if (p.fused) {
+            block_encode_fused_for(build_models, p.threads)<<<p.grid, p.threads, p.smem, ctx->stream>>>(
+                d_in, n_blocks, block_size, d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.look, ws.counter, d_blob, blob_cap, d_offsets,
+                ctx->d_status);
+            return check_launch(ctx, "block_encode_fused_kernel");
+        }
+        block_encode_kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, block_size, d_freqs, chunk_syms, ws.scratch, p.slot_bytes,
+                                                                        ws.sizes, ctx->d_status);
+        return check_launch(ctx, "block_encode_kernel");
+    });
 }
 
 // Host mode runs the slice pipeline over whole blocks; the frequency tables go in with each slice when the caller supplies
@@ -1110,7 +1094,7 @@ int blocks_encode_host(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uin
     const UnitTable freqs = build ? UnitTable{nullptr, block_freqs, kBlockFreqBytes} : UnitTable{block_freqs, nullptr, kBlockFreqBytes};
     return encode_pipeline(
         ctx, in, static_cast<size_t>(n_blocks) * block_size, chunk_syms, block_size / chunk_syms, freqs,
-        [&](size_t units) { return reserve_blocks_encode(ctx, static_cast<uint32_t>(units), block_size, chunk_syms, build); },
+        [&](const Slice& s) { return plan_blocks_encode(ctx, static_cast<uint32_t>(s.units), block_size, chunk_syms, build); },
         [&](const Slice& s, const uint8_t* d_in, uint8_t* d_freqs, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
             return blocks_encode_device(ctx, d_in, static_cast<uint32_t>(s.units), block_size, reinterpret_cast<uint16_t*>(d_freqs),
                                         build, chunk_syms, d_blob, cap, d_off);

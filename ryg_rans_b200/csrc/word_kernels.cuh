@@ -140,16 +140,6 @@ struct WordEncoder {
     }
 };
 
-// chunk `chunk` into the end of its own worst-case slot of `scratch`; size to sizes[chunk]
-template <bool R32>
-__device__ __forceinline__ void word_encode_chunk(const uint8_t* __restrict__ chunk_in, uint32_t m, uint32_t chunk,
-                                                  uint32_t tab, uint32_t wsm, uint8_t* __restrict__ scratch,
-                                                  uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
-{
-    const uint32_t produced = encode_stream(chunk_in, m, WordEncoder<R32>{tab}, wsm, scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, status);
-    if ((threadIdx.x & 31) == 0) sizes[chunk] = produced;
-}
-
 #ifndef RB200_ENC_MINBLOCKS
 #define RB200_ENC_MINBLOCKS 3
 #endif
@@ -167,18 +157,18 @@ word_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_sy
     const uint32_t warp = threadIdx.x >> 5;
     const uint32_t chunk = blockIdx.x * kEncWarps + warp;
     if (chunk >= n_chunks) return;
-    const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
-    const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-    word_encode_chunk<R32>(in + first, m, chunk, smem_addr(s_enc), smem_addr(s_enc) + kEncTableBytes + warp * kEncWarpSmem, scratch,
-                      slot_bytes, sizes, status);
+    const ChunkRange r = chunk_range(chunk, chunk_syms, n);
+    encode_chunk_split(in + r.first, r.m, chunk, WordEncoder<R32>{smem_addr(s_enc)}, smem_addr(s_enc) + kEncTableBytes + warp * kEncWarpSmem,
+                       scratch, slot_bytes, sizes, status);
 }
+// dynamic shared memory of both word encoders (K2, K2f)
 constexpr uint32_t kEncSmemBytes = kEncTableBytes + kEncWarps * kEncWarpSmem;
 
 // ---------------------------------------------------------------------------
 // K2f: persistent encode with the directory and the compaction fused in (the protocol: placement.cuh).
 // ---------------------------------------------------------------------------
-// Grid = resident capacity (SMs x RB200_FUSED_MINBLOCKS CTAs).  Warp 0 of CTA 0 is the scanner, every other warp is
-// a worker with kFusedSlots scratch slots (a SlotQueue).
+// Grid = resident capacity (SMs x RB200_FUSED_MINBLOCKS CTAs, sized by the host's encode plan).  Warp 0 of CTA 0 is the
+// scanner, every other warp is a worker with kFusedSlots scratch slots (encode_chunks_fused).
 template <bool R32>
 __global__ void __launch_bounds__(kEncWarps * 32, RB200_FUSED_MINBLOCKS)
 word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
@@ -191,25 +181,9 @@ word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t ch
     for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
     __syncthreads();
 
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (blockIdx.x == 0 && warp == 0) {                    // no CTA barrier below: warps are independent from here on
-        fused_scanner(look, n_chunks, lane, status);
-        return;
-    }
-    const uint32_t tab = smem_addr(s_enc), wsm = tab + kEncTableBytes + warp * kEncWarpSmem;
-    const PlaceOut out = {look, n_chunks, blob, blob_cap, offsets, status};
-    SlotQueue<kFusedSlots> q(scratch, static_cast<uint64_t>(blockIdx.x) * kEncWarps + warp, slot_bytes);
-    for (;;) {
-        uint32_t chunk = 0;
-        if (lane == 0) chunk = atomicAdd(counter, 1u);     // chunks start in order
-        chunk = __shfl_sync(0xffffffffu, chunk, 0);
-        if (chunk >= n_chunks) break;
-        const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
-        const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk_syms), n - first));
-        const uint32_t produced = encode_stream<RB200_ENC_KEEP_HINT>(in + first, m, WordEncoder<R32>{tab}, wsm, q.next_end(), status);
-        q.finish(out, chunk, produced, lane);
-    }
-    q.drain(out, lane);
+    const uint32_t tab = smem_addr(s_enc), wsm = tab + kEncTableBytes + (threadIdx.x >> 5) * kEncWarpSmem;
+    encode_chunks_fused<kFusedSlots, kEncWarps, RB200_ENC_KEEP_HINT>(in, n, chunk_syms, WordEncoder<R32>{tab}, wsm, scratch, slot_bytes,
+                                                                     PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
 }
 
 // ---------------------------------------------------------------------------

@@ -1,10 +1,12 @@
 """The fused encoders over many more chunks than they have resident warps.
 
-Every worker warp of word_encode_fused_kernel (K2f) and block_encode_fused_kernel (K5f) cycles through a few scratch
-slots of its own and places a chunk a chunk late (placement.cuh: SlotQueue).  The fused test in test_gpu_parity.py encodes 3 M symbols, fewer chunks than there are workers, so no
-slot is ever reused there.  Here 64 Mi symbols at chunks of 4096 / 8192 make every worker take several chunks, with
-three models: uniform, Zipf, and a two-symbol model {4095, 1} on data that is mostly the frequency-1 symbol (about
-11 bits per symbol, close to the worst case a chunk's scratch slot is sized for).  The per-block tests in
+Every worker warp of word_encode_fused_kernel (K2f), of the fused alias / byte encoder and of block_encode_fused_kernel
+(K5f) cycles through a few scratch slots of its own and places a chunk a chunk late (placement.cuh: SlotQueue).  The
+fused test in test_gpu_parity.py encodes 3 M symbols, fewer chunks than there are workers, so no slot is ever reused
+there.  Here 64 Mi symbols at chunks of 4096 / 8192 (up to 16 384 chunks, against at most SMs x 32 worker warps) make
+every worker take several chunks: the word coder with three models -- uniform, Zipf, and a two-symbol model {4095, 1}
+on data that is mostly the frequency-1 symbol (about 11 bits per symbol, close to the worst case a chunk's scratch slot
+is sized for) -- and the alias coder at scale_bits 16 and the byte coder at 14 with the uniform and Zipf models.  The per-block tests in
 test_gpu_parity.py encode at most 200 blocks, fewer than the worker CTAs of K5f (5 per SM, less the scanner's); here
 4096 blocks make every worker CTA take several blocks.
 """
@@ -33,11 +35,17 @@ def _data(kind):
     return (torch.rand(N, device="cuda", generator=g) < 0.9).to(torch.uint8)
 
 
+# (coder, scale_bits, kind); the word coder's cases keep their ids ("rare" needs scale_bits 12)
+CASES = [pytest.param("word", 12, kind, id=kind) for kind in ("uniform", "zipf", "rare")] + \
+        [pytest.param(coder, sb, kind, id=f"{coder}{sb}-{kind}") for coder, sb in (("alias", 16), ("byte", 14))
+         for kind in ("uniform", "zipf")]
+CODERS = {"word": orc.CODER_WORD, "alias": orc.CODER_ALIAS, "byte": orc.CODER_BYTE}    # the library's numbering too
+
+
 @pytest.mark.parametrize("chunk", [4096, 8192])
-@pytest.mark.parametrize("kind", ["uniform", "zipf", "rare"])
-def test_fused_encode_reuses_slots(gpu_ctx, oracle_lib, kind, chunk):
+@pytest.mark.parametrize("coder, sb, kind", CASES)
+def test_fused_encode_reuses_slots(gpu_ctx, oracle_lib, coder, sb, kind, chunk):
     import torch
-    import ryg_rans_b200 as rb
     data = _data(kind)
     h_data = data.cpu().numpy()
     if kind == "rare":
@@ -46,8 +54,8 @@ def test_fused_encode_reuses_slots(gpu_ctx, oracle_lib, kind, chunk):
         cum = np.zeros(257, np.uint32)
         cum[1:] = np.cumsum(freqs)
     else:
-        freqs, cum = oracle_lib.model(h_data, 12)
-    model = gpu_ctx.model(rb.CODER_WORD, 12, freqs)
+        freqs, cum = oracle_lib.model(h_data, sb)
+    model = gpu_ctx.model(CODERS[coder], sb, freqs)
     n_chunks = gpu_ctx.chunk_count(N, chunk)
     cap = gpu_ctx.encode_bound(N, chunk)
     blob = torch.empty(cap, dtype=torch.uint8, device="cuda")
@@ -56,7 +64,7 @@ def test_fused_encode_reuses_slots(gpu_ctx, oracle_lib, kind, chunk):
     gpu_ctx.encode_device(model, data.data_ptr(), N, chunk, blob.data_ptr(), cap, offsets.data_ptr())
     gpu_ctx.sync()
     size = int(offsets[-1])
-    oblob, ooffs = oracle_lib.chunked_encode(orc.CODER_WORD, h_data, freqs, cum, chunk, nlanes=32, scale_bits=12)
+    oblob, ooffs = oracle_lib.chunked_encode(CODERS[coder], h_data, freqs, cum, chunk, nlanes=32, scale_bits=sb)
     assert np.array_equal(offsets.cpu().numpy().astype(np.uint64), ooffs), "directory differs from the oracle container"
     assert size == oblob.size and np.array_equal(blob[:size].cpu().numpy(), oblob), "blob differs from the oracle container"
     if kind == "rare":
