@@ -230,6 +230,20 @@ int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf, size_t siz
  * rejects, RB200_E_SPACE for n > out_cap; in both cases out is untouched. */
 int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                         uint64_t* d_n_symbols);
+/* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
+ * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's
+ * decode table is built on the GPU into the context, and the decoder the header calls for is picked on the GPU -- all
+ * enqueued on the context stream.  The rules of rb200_container_blocks_decode_async apply: DEVICE memory only, buf and
+ * out 16-byte aligned, d_n_symbols 8-byte aligned or NULL; the call never synchronises, copies to the host or
+ * allocates, so it can be captured in a CUDA graph, and returns only RB200_E_ARG (nothing launched) or RB200_E_CUDA.
+ * *d_n_symbols receives n once header, model and directory pass (also when the blob CRC then fails).  rb200_sync gives
+ * the verdict: RB200_E_STREAM for anything rb200_container_open rejects, RB200_E_SPACE for n > out_cap, content errors
+ * first; in both cases out is untouched.  One difference from rb200_container_decode: a container that open accepts
+ * but the decoders refuse (chunk_syms outside 32 .. 2^24, a blob of 2^36 bytes or more, a byte-coder frequency of
+ * 65536), which that call reports as RB200_E_ARG or RB200_E_MODEL, is RB200_E_STREAM here, out untouched.  Version 2
+ * containers are rejected (RB200_E_STREAM). */
+int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                 uint64_t* d_n_symbols);
 
 /* ---------------------------------------------------------------- multi-GPU: gathering the shards' blobs (NCCL) */
 

@@ -55,6 +55,7 @@ EXPORTS = [
                                                 C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int]),
     ("rb200_container_blocks_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
     ("rb200_container_blocks_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_container_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -357,6 +358,11 @@ class Context:
         n = C.c_uint64(0)
         self.lib.check(self.lib.dll.rb200_container_decode(self.h, buf_ptr, size, out_ptr, out_cap, C.byref(n), MEM_DEVICE), self.h)
         return n.value
+
+    def container_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
+        """enqueue only (CUDA-graph capturable), any coder; n_ptr: device address of a u64 that receives n, or 0.  The
+        verdict on the container (-4 corrupt or not decodable, -3 out_cap too small, output untouched) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_decode_async(self.h, buf_ptr, size, out_ptr, out_cap, n_ptr or None), self.h)
 
     # ---- per-block containers (version 2): every block's model, the directory and the blob in one buffer
     def container_blocks_capacity(self, n_blocks, block_size, chunk_syms):

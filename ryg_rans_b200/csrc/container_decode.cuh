@@ -1,22 +1,33 @@
-// container_decode.cuh -- rb200_container_blocks_decode_async: a per-block (version 2) container in device memory,
-// checked and decoded by kernels alone, so that the call only enqueues work (and can be captured in a CUDA graph).
+// container_decode.cuh -- rb200_container_blocks_decode_async (version 2, per-block models) and
+// rb200_container_decode_async (version 1, one model, any coder): a container in device memory, checked and decoded by
+// kernels alone, so that the call only enqueues work (and can be captured in a CUDA graph).
 //
-// The stages run in stream order; each reads what the one before it left in the context's BlocksAsyncWork:
-//   container_plan_kernel          one warp: container_header_ok on buf[0, 64) against size -> the plan; clears the
-//                                  verdict words
+// The stages run in stream order; each reads what the one before it left in the context's BlocksAsyncWork (for
+// version 1 the first member of its SingleAsyncWork):
+//   container_plan_kernel          one warp: container_header_ok on buf[0, 64) against size for the call's version ->
+//                                  the plan (version 1 also coder and scale_bits); clears the verdict words and the
+//                                  call's work counters, so that a call never depends on how the previous one ended
 //   crc32_kernel x 2               meta CRC of buf + 64, length from the plan; blob CRC at buf + blob_off (both lengths
 //                                  are zero when the header is rejected, the blob's also when the flag is clear)
-//   container_prefix_check_kernel  container_block_model_ok for every block, container_dir_step_ok for every
-//                                  directory entry, container_dir_ends_ok once
+//   container_prefix_check_kernel  container_block_model_ok for every block (version 2), container_dir_step_ok for
+//                                  every directory entry, container_dir_ends_ok once
+//   container_table_kernel         version 1, one CTA: container_model_ok and container_model_decodable on the model,
+//                                  then the header coder's decode table, byte for byte what rb200_model_create uploads
 //   container_verdict_kernel       one warp: header CRC (crc fields zero) joined with the meta CRC, both CRCs compared;
 //                                  writes n_symbols, then sets go or ORs kStatStream / kStatSpace into the status word
-//   block_decode_planned_kernel    a fixed grid that exits at once unless go; CTAs take block ids from a counter, build
+//   version 2: block_decode_planned_kernel
+//                                  a fixed grid that exits at once unless go; CTAs take block ids from a counter, build
 //                                  the block's slot table in shared memory and decode its chunks
+//   version 1: one launch per decoder variant rb200_decode can pick (kDec*), each on a fixed grid; go holds the id of
+//              the one that runs, every other exits before it touches shared memory, TMA or its counter
 // The rules are the host parser's (container_format.h); they run in its order: content errors before kStatSpace.
 #pragma once
+#include "alias_kernels.cuh"
 #include "block_kernels.cuh"
 #include "container_format.h"
 #include "crc_kernels.cuh"
+#include "rans64_kernels.cuh"
+#include "word_decode_tma.cuh"
 
 namespace rb200 {
 
@@ -41,13 +52,36 @@ struct BlocksAsyncWork {
     uint32_t ctas_done;
 };
 
-__global__ void __launch_bounds__(32) container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, BlocksAsyncWork* w)
+// The decoders of a version 1 container, one per variant rb200_decode picks: the word coder narrow or WIDE (a frequency
+// of 4096), the alias and byte coders specialised for scale_bits 16, 14, 12 or generic (RB200_ALIAS_SB_DISPATCH), rans64.
+// The verdict stores the id of the one to run in go; kDecNone decodes nothing.
+constexpr uint32_t kDecNone = 0, kDecWord = 1, kDecWordWide = 2, kDecAlias = 3, kDecByte = 7, kDecRans64 = 11;
+// offset of a specialisation from kDecAlias / kDecByte
+__host__ __device__ constexpr uint32_t sb_variant(uint32_t sb) { return sb == 16 ? 0 : sb == 14 ? 1 : sb == 12 ? 2 : 3; }
+
+// the largest decode table: rans64's cum2sym at scale_bits 16 and its 256 x {start, freq}
+constexpr uint32_t kSingleTableBytes = (1u << 16) + 2048;
+
+// rb200_container_decode_async's workspace: fixed-size, allocated with the context.
+struct SingleAsyncWork {
+    BlocksAsyncWork c;          // plan (n_blocks 0: no block models), CRCs and verdict words; go is the decoder id
+    uint32_t coder, scale_bits; // from the header, when c.plan.ok
+    uint32_t wide;              // the word table has a slot of frequency 4096
+    uint32_t refused;           // the decoders refuse the model (container_model_decodable)
+    DecodeWork work;            // the decoder's chunk counter; zero between launches (the last warp out re-arms it)
+    alignas(16) uint8_t table[kSingleTableBytes];   // the decode table of the header's coder, as rb200_model_create's
+};
+
+// single: the version 1 call's workspace (w is then &single->c), or null for version 2
+__global__ void __launch_bounds__(32)
+    container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, BlocksAsyncWork* w, SingleAsyncWork* single)
 {
     if (threadIdx.x) return;
     BlocksPlan p = {};
+    uint32_t coder = 0, scale_bits = 0;
     if (size >= sizeof(ContainerHeader)) {                           // a shorter buffer is not read at all
         const ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(buf);
-        if (container_header_ok(h, size, kContainerVersionBlocks)) {
+        if (container_header_ok(h, size, static_cast<uint16_t>(version))) {
             p.ok = 1;
             p.n_symbols = h.n_symbols;
             p.n_chunks = h.n_chunks;
@@ -56,14 +90,27 @@ __global__ void __launch_bounds__(32) container_plan_kernel(const uint8_t* __res
             p.blob_bytes = h.blob_bytes;
             p.meta_len = container_dir_end(h) - sizeof(ContainerHeader);
             p.blob_len = (h.flags & RB200_CONTAINER_CRC_BLOB) ? h.blob_bytes : 0;
-            p.n_blocks = h.n_blocks;
-            p.block_size = h.block_size;
+            if (version == kContainerVersionBlocks) {                // version 1 does not check these fields
+                p.n_blocks = h.n_blocks;
+                p.block_size = h.block_size;
+            }
             p.chunk_syms = h.chunk_syms;
+            coder = h.coder;
+            scale_bits = h.scale_bits;
         }
     }
     w->plan = p;
     w->bad = 0;
     w->go = 0;
+    w->next_block = 0;
+    w->ctas_done = 0;
+    if (single) {
+        single->coder = coder;
+        single->scale_bits = scale_bits;
+        single->wide = 0;
+        single->refused = 0;
+        single->work = DecodeWork{0, 0};
+    }
 }
 
 // The per-element rules of the prefix.  Each warp stages 32 block models (16 KiB, coalesced) in shared memory with
@@ -104,11 +151,101 @@ __global__ void __launch_bounds__(kPrefixWarps * 32)
     if (!ok) w->bad = 1;
 }
 
+// The version 1 model (256 x u32 at buf + 64) checked and turned into the decode table of the header's coder in
+// s->table, byte for byte what rb200_model_create builds on the host (tables.h has the formats and the per-entry
+// formulas both sides call).  Slot-to-symbol is a binary search over cum, per slot (word) or per 4 slots (the cum2sym
+// bytes of the byte and rans64 coders, stored as one u32); the alias pairing runs on one thread.
+constexpr int kTableThreads = 512;
+
+__global__ void __launch_bounds__(kTableThreads) container_table_kernel(const uint8_t* __restrict__ buf, SingleAsyncWork* s)
+{
+    __shared__ uint32_t s_freq[256], s_cum[257];
+    __shared__ uint32_t s_divider[256], s_adjust[512], s_slot_freqs[512], s_rest[256], s_given[256];
+    __shared__ uint8_t s_sym_id[512];
+    __shared__ uint32_t s_build;
+    const uint32_t tid = threadIdx.x;
+    if (!s->c.plan.ok) return;
+    const uint32_t coder = s->coder, sb = s->scale_bits;
+    if (tid < 256) s_freq[tid] = reinterpret_cast<const uint32_t*>(buf + sizeof(ContainerHeader))[tid];
+    __syncthreads();
+    if (tid == 0) {
+        bool build = false;
+        if (!container_model_ok(coder, sb, s_freq)) {
+            s->c.bad = 1;                                            // what rb200_container_open rejects
+        } else if (!container_model_decodable(coder, s_freq)) {
+            s->refused = 1;                                          // what rb200_container_decode refuses
+        } else if (coder == RB200_CODER_ALIAS) {
+            build = alias_tables_core(s_freq, (1u << sb) / 256, s_divider, s_adjust, s_slot_freqs, s_sym_id, s_rest, s_given);
+            if (!build) s->refused = 1;                              // rb200_model_create: RB200_E_MODEL
+        } else {
+            build = true;
+        }
+        s_cum[0] = 0;
+        for (int i = 0; i < 256; i++) s_cum[i + 1] = s_cum[i] + s_freq[i];    // < 2^17 once the model is ok
+        s_build = build;
+    }
+    __syncthreads();
+    if (!s_build) return;
+    const uint32_t M = 1u << sb;
+    // the symbol whose range holds slot: the largest s with cum[s] <= slot (zero-width symbols hold none)
+    auto symbol_of = [&](uint32_t slot) {
+        uint32_t lo = 0, hi = 256;
+        while (hi - lo > 1) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (s_cum[mid] <= slot) lo = mid; else hi = mid;
+        }
+        return lo;
+    };
+    if (coder == RB200_CODER_WORD) {
+        uint32_t* tab = reinterpret_cast<uint32_t*>(s->table);
+        bool wide = false;
+        for (uint32_t slot = tid; slot < M; slot += kTableThreads) {
+            const uint32_t sym = symbol_of(slot), f = s_cum[sym + 1] - s_cum[sym];
+            wide |= f == M;
+            tab[slot] = word_dec_entry(sym, f, slot - s_cum[sym]);
+        }
+        if (wide) s->wide = 1;
+    } else if (coder == RB200_CODER_ALIAS) {
+        if (tid < 256) reinterpret_cast<AliasDecEntry*>(s->table)[tid] = alias_dec_entry(tid, s_divider, s_adjust, s_slot_freqs, s_sym_id);
+    } else {                                                         // byte, rans64: cum2sym[M], then 256 symbol entries
+        uint32_t* c2s = reinterpret_cast<uint32_t*>(s->table);
+        for (uint32_t q = tid; q < M / 4; q += kTableThreads) {
+            uint32_t sym = symbol_of(4 * q), packed = 0;
+            for (uint32_t k = 0; k < 4; k++) {
+                while (4 * q + k >= s_cum[sym + 1]) sym++;           // steps over zero-width symbols
+                packed |= sym << (8 * k);
+            }
+            c2s[q] = packed;
+        }
+        uint32_t* syms = reinterpret_cast<uint32_t*>(s->table + M);
+        if (tid < 256) {
+            const uint32_t f = s_cum[tid + 1] - s_cum[tid];
+            if (coder == RB200_CODER_BYTE) {
+                syms[tid] = byte_dec_symbol(s_cum[tid], f);
+            } else {                                                 // Rans64DecSymbol {start, freq}
+                syms[2 * tid] = s_cum[tid];
+                syms[2 * tid + 1] = f;
+            }
+        }
+    }
+}
+
+// the decoder a version 1 container needs: rb200_decode's choice of kernel (decode_device)
+__device__ inline uint32_t single_decoder(uint32_t coder, uint32_t scale_bits, uint32_t wide)
+{
+    if (coder == RB200_CODER_WORD) return wide ? kDecWordWide : kDecWord;
+    if (coder == RB200_CODER_ALIAS) return kDecAlias + sb_variant(scale_bits);
+    if (coder == RB200_CODER_BYTE) return kDecByte + sb_variant(scale_bits);
+    return kDecRans64;
+}
+
 // One warp.  meta_crc covers the header with its crc fields zeroed, then meta_len bytes whose CRC is in crc[0];
 // the header's CRC is taken here with container_finish_kernel's warp helpers and joined (crc32_combine).
+// single: as for container_plan_kernel.  Version 1 also refuses what the decoders do not take (container_format.h),
+// as content, and its go is the id of the decoder to run.
 __global__ void __launch_bounds__(32)
     container_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, BlocksAsyncWork* w,
-                             uint32_t* status)
+                             uint32_t* status, const SingleAsyncWork* single)
 {
     using namespace crc_detail;
     __shared__ uint4 s_head_v[sizeof(ContainerHeader) / 16];
@@ -138,12 +275,13 @@ __global__ void __launch_bounds__(32)
     if (lane) return;
     const bool prefix_ok = meta == meta_crc && !w->bad;
     if (prefix_ok && n_symbols) *n_symbols = p.n_symbols;
-    if (!prefix_ok || ((flags & RB200_CONTAINER_CRC_BLOB) && w->crc[1].crc != blob_crc))
+    const bool refused = single && (single->refused || !container_geometry_decodable(p.chunk_syms, p.blob_bytes));
+    if (!prefix_ok || refused || ((flags & RB200_CONTAINER_CRC_BLOB) && w->crc[1].crc != blob_crc))
         atomicOr(status, kStatStream);
     else if (p.n_symbols > out_cap)
         atomicOr(status, kStatSpace);
     else
-        w->go = 1;
+        w->go = single ? single_decoder(single->coder, single->scale_bits, single->wide) : 1;
 }
 
 // The per-block decoder for a geometry only the device knows: a fixed grid of kPlannedWarps-warp CTAs (resident all at
@@ -202,6 +340,144 @@ __global__ void __launch_bounds__(kPlannedWarps * 32, 8)
     }
 }
 
+// The version 1 decoders.  Each takes the geometry, the table and its counter from the call's SingleAsyncWork and runs
+// only when go is its id.  Word and alias: the shipped persistent kernels' CTA set-up around decode_persistent with the
+// shipped policies; byte and rans64: the shipped kernels' table staging around a counter-driven loop over
+// decode_window_chunk (their own kernels launch one warp per chunk, a grid only the host can size).
+
+template <bool WIDE>
+__global__ void __launch_bounds__(DecShip::kWarps * 32, DecShip::kMinBlocks)
+    word_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, SingleAsyncWork* __restrict__ w,
+                               uint32_t* __restrict__ status)
+{
+    using P = DecShip;
+    static_assert(P::kRefill == kRefillCpAsync, "the ring's mbarriers are not initialised here: cp.async refill only");
+    if (w->c.go != (WIDE ? kDecWordWide : kDecWord)) return;        // the same for the whole grid
+    const BlocksPlan p = w->c.plan;
+    extern __shared__ __align__(1024) uint8_t s_dec[];     // [16 KiB table][table mbarrier][kWarps x (ring, mirror, mbarriers)]
+    const uint32_t tab = smem_addr_pinned(s_dec);
+    const uint32_t bar_tab = tab + kWordSlots * 4;
+    const uint32_t warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);       // warp-uniform for ptxas
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t ring = tab + P::kWarpsOff + warp * P::kWarpStride;
+
+    if (threadIdx.x == 0) mbar_init(bar_tab, 1);
+    mbar_fence_init();
+    __syncthreads();
+    if (threadIdx.x == 0) {                                // the table for the whole CTA: one 16 KiB bulk copy
+        mbar_arrive_expect_tx(bar_tab, kWordSlots * 4);
+        bulk_g2s(tab, w->table, kWordSlots * 4, bar_tab);
+    }
+    {
+        uint32_t spins = 0;
+        while (!mbar_try_wait(bar_tab, 0))
+            if (++spins > kTmaSpinLimit) {
+                if (threadIdx.x == 0) atomicOr(status, kStatStall);
+                return;
+            }
+    }
+    __syncwarp();
+    decode_persistent<P>(WordDecoder<WIDE>{tab, 0}, ring, buf + p.blob_off, p.blob_bytes, reinterpret_cast<const uint64_t*>(buf + p.dir_off),
+                         out, p.n_symbols, p.chunk_syms, static_cast<uint32_t>(p.n_chunks), &w->work, lane, status);
+}
+
+template <uint32_t SB>
+__global__ void __launch_bounds__(AliasDecShip::kWarps * 32, AliasDecShip::kMinBlocks)
+    alias_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, SingleAsyncWork* __restrict__ w,
+                                uint32_t* __restrict__ status)
+{
+    using P = AliasDecShip;
+    if (w->c.go != kDecAlias + sb_variant(SB)) return;
+    const BlocksPlan p = w->c.plan;
+    const uint32_t sb_rt = w->scale_bits;
+    const AliasDecEntry* g_dec = reinterpret_cast<const AliasDecEntry*>(w->table);
+    extern __shared__ __align__(1024) uint8_t s_adec[];       // [32 KiB table][16 B][kWarps x (ring, mirror)]
+    uint4* s_tab = reinterpret_cast<uint4*>(s_adec);
+    for (uint32_t i = threadIdx.x; i < 256 * kAliasDecReplicas; i += blockDim.x) {
+        const AliasDecEntry e = g_dec[i / kAliasDecReplicas];
+        if (kAliasLean && SB > 8) s_tab[i] = alias_lean_entry<(SB > 8 ? SB : 9)>(e, i / kAliasDecReplicas);
+        else s_tab[i] = make_uint4(e.divider, e.alt0, e.alt1, e.adjust);
+    }
+    __syncthreads();
+
+    const uint32_t base = smem_addr_pinned(s_adec);
+    const uint32_t warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+    const uint32_t lane = threadIdx.x & 31;
+    const AliasDecoder<SB, kAliasLean> coder = {base + (lane & (kAliasDecReplicas - 1)) * 16, sb_rt};
+    decode_persistent<P>(coder, base + P::kWarpsOff + warp * P::kWarpStride, buf + p.blob_off, p.blob_bytes,
+                         reinterpret_cast<const uint64_t*>(buf + p.dir_off), out, p.n_symbols, p.chunk_syms, static_cast<uint32_t>(p.n_chunks),
+                         &w->work, lane, status);
+}
+
+// Every warp of the grid takes chunk ids from w->work until none is left and decodes each through its 1 KiB stream
+// window at shared address `ring`; the last warp out re-arms the counter.
+template <class C>
+__device__ __forceinline__ void decode_window_planned(const C& coder, const uint8_t* __restrict__ buf, uint8_t* __restrict__ out,
+                                                      SingleAsyncWork* __restrict__ w, uint32_t ring, uint32_t* __restrict__ status)
+{
+    const BlocksPlan p = w->c.plan;
+    const uint8_t* blob = buf + p.blob_off;
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + p.dir_off);
+    const uint32_t lane = threadIdx.x & 31, n_chunks = static_cast<uint32_t>(p.n_chunks);
+    for (;;) {
+        uint32_t chunk = 0;
+        if (lane == 0) chunk = atomicAdd(&w->work.next_chunk, 1u);
+        chunk = __shfl_sync(0xffffffffu, chunk, 0);       // also orders the previous chunk's ring reads before the next fill
+        if (chunk >= n_chunks) break;
+        const uint64_t first = static_cast<uint64_t>(chunk) * p.chunk_syms;
+        const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(p.chunk_syms), p.n_symbols - first));
+        decode_window_chunk(coder, blob, p.blob_bytes, offsets, chunk, ring, out + first, m, status);
+    }
+    if (lane == 0 && atomicAdd(&w->work.warps_done, 1u) == gridDim.x * (blockDim.x / 32) - 1) {
+        w->work.next_chunk = 0;
+        w->work.warps_done = 0;
+    }
+}
+
+// dynamic shared memory of the byte decoder: 16 rings, 256 symbol entries and cum2sym at the largest scale_bits the
+// variant decodes (the generic one: 15)
+__host__ __device__ constexpr uint32_t byte_planned_smem(uint32_t SB) { return kAliasDecWarps * kRingBytes + 1024 + (1u << (SB ? SB : 15)); }
+
+template <uint32_t SB>
+__global__ void __launch_bounds__(kAliasDecWarps * 32, 4)
+    byte_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, SingleAsyncWork* __restrict__ w,
+                               uint32_t* __restrict__ status)
+{
+    if (w->c.go != kDecByte + sb_variant(SB)) return;
+    const uint32_t sb = SB ? SB : w->scale_bits;
+    extern __shared__ __align__(1024) uint8_t s_adec[];       // [16 x 1 KiB rings][table]
+    uint4* s_tab = reinterpret_cast<uint4*>(s_adec + kAliasDecWarps * kRingBytes);
+    const uint32_t vecs = ((1u << sb) + 1024) / 16;
+    for (uint32_t i = threadIdx.x; i < vecs; i += blockDim.x) s_tab[i] = reinterpret_cast<const uint4*>(w->table)[i];
+    __syncthreads();
+    const uint32_t warp = threadIdx.x >> 5;
+    decode_window_planned(ByteDecoder<SB>{smem_addr_pinned(s_tab), sb}, buf, out, w, smem_addr(s_adec) + warp * kRingBytes, status);
+}
+
+constexpr uint32_t kRans64PlannedSmem = kRans64Warps * kRingBytes + kRans64DecSymBytes + (1u << 16);
+
+__global__ void __launch_bounds__(kRans64Warps * 32, 2)
+    rans64_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, SingleAsyncWork* __restrict__ w,
+                                 uint32_t* __restrict__ status)
+{
+    if (w->c.go != kDecRans64) return;
+    const uint32_t sb = w->scale_bits;
+    extern __shared__ __align__(1024) uint8_t s_r64[];        // [16 x 1 KiB rings][cum2sym][256 x 16 replicas x {start, freq}]
+    uint4* s_tab = reinterpret_cast<uint4*>(s_r64 + kRans64Warps * kRingBytes);
+    const uint32_t vecs = (1u << sb) / 16;
+    for (uint32_t i = threadIdx.x; i < vecs; i += blockDim.x) s_tab[i] = reinterpret_cast<const uint4*>(w->table)[i];
+    {
+        const uint2* g_syms = reinterpret_cast<const uint2*>(w->table + (1u << sb));
+        uint2* s_syms = reinterpret_cast<uint2*>(s_r64 + kRans64Warps * kRingBytes + (1u << sb));
+        for (uint32_t i = threadIdx.x; i < 256 * kRans64DecReplicas; i += blockDim.x) s_syms[i] = g_syms[i / kRans64DecReplicas];
+    }
+    __syncthreads();
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t tab = smem_addr(s_tab);
+    const Rans64Decoder coder = {tab, tab + (1u << sb) + (lane & (kRans64DecReplicas - 1)) * 8, sb};
+    decode_window_planned(coder, buf, out, w, smem_addr(s_r64) + warp * kRingBytes, status);
+}
+
 // The launch shapes, fixed per device: the decoder's grid is every CTA that is resident at once.
 struct BlocksAsyncShape {
     uint32_t decode_grid, check_grid;
@@ -213,6 +489,43 @@ inline BlocksAsyncShape configure_container_decode(uint32_t sms)
     int per_sm = 0;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_decode_planned_kernel, kPlannedWarps * 32, 0);
     return BlocksAsyncShape{sms * static_cast<uint32_t>(per_sm < 1 ? 1 : per_sm), sms * 8};
+}
+
+// One launch of a version 1 decoder: kernel, grid, threads, dynamic shared memory.
+struct SingleDecodeLaunch {
+    void (*kernel)(const uint8_t*, uint8_t*, SingleAsyncWork*, uint32_t*);
+    uint32_t grid, threads, smem;
+    const char* name;
+};
+constexpr int kSingleDecoders = 11;
+
+// The version 1 decoders in id order, each with every CTA that is resident at once (the word and alias grids are the
+// shipped kernels' full grids).
+inline void configure_single_decode(uint32_t sms, SingleDecodeLaunch* out)
+{
+    const SingleDecodeLaunch l[kSingleDecoders] = {
+        {word_decode_planned_kernel<false>, sms * DecShip::kMinBlocks, DecShip::kWarps * 32, DecShip::kSmemBytes, "word_decode_planned_kernel"},
+        {word_decode_planned_kernel<true>, sms * DecShip::kMinBlocks, DecShip::kWarps * 32, DecShip::kSmemBytes, "word_decode_planned_kernel(wide)"},
+        {alias_decode_planned_kernel<16>, sms * AliasDecShip::kMinBlocks, AliasDecShip::kWarps * 32, AliasDecShip::kSmemBytes, "alias_decode_planned_kernel<16>"},
+        {alias_decode_planned_kernel<14>, sms * AliasDecShip::kMinBlocks, AliasDecShip::kWarps * 32, AliasDecShip::kSmemBytes, "alias_decode_planned_kernel<14>"},
+        {alias_decode_planned_kernel<12>, sms * AliasDecShip::kMinBlocks, AliasDecShip::kWarps * 32, AliasDecShip::kSmemBytes, "alias_decode_planned_kernel<12>"},
+        {alias_decode_planned_kernel<0>, sms * AliasDecShip::kMinBlocks, AliasDecShip::kWarps * 32, AliasDecShip::kSmemBytes, "alias_decode_planned_kernel<0>"},
+        {byte_decode_planned_kernel<16>, 0, kAliasDecWarps * 32, byte_planned_smem(16), "byte_decode_planned_kernel<16>"},
+        {byte_decode_planned_kernel<14>, 0, kAliasDecWarps * 32, byte_planned_smem(14), "byte_decode_planned_kernel<14>"},
+        {byte_decode_planned_kernel<12>, 0, kAliasDecWarps * 32, byte_planned_smem(12), "byte_decode_planned_kernel<12>"},
+        {byte_decode_planned_kernel<0>, 0, kAliasDecWarps * 32, byte_planned_smem(0), "byte_decode_planned_kernel<0>"},
+        {rans64_decode_planned_kernel, 0, kRans64Warps * 32, kRans64PlannedSmem, "rans64_decode_planned_kernel"},
+    };
+    for (int i = 0; i < kSingleDecoders; i++) {
+        out[i] = l[i];
+        cudaFuncSetAttribute(l[i].kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(l[i].kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(l[i].smem));
+        if (!out[i].grid) {
+            int per_sm = 0;
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, l[i].kernel, static_cast<int>(l[i].threads), l[i].smem);
+            out[i].grid = sms * static_cast<uint32_t>(per_sm < 1 ? 1 : per_sm);
+        }
+    }
 }
 
 }  // namespace rb200

@@ -4,15 +4,12 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "hd.h"
 #include "rans_b200.h"
 
-// The layout and the rules below are compiled for the host and, under nvcc, for the device too: the kernels of
-// rb200_container_blocks_decode_async (container_decode.cuh) apply the same functions as the host parser.
-#ifdef __CUDACC__
-#define RB200_HD __host__ __device__
-#else
-#define RB200_HD
-#endif
+// The layout and the rules below are compiled for the host and, under nvcc, for the device too (RB200_HD): the kernels
+// of rb200_container_decode_async / rb200_container_blocks_decode_async (container_decode.cuh) apply the same functions
+// as the host parser.
 
 namespace rb200 {
 
@@ -91,6 +88,32 @@ RB200_HD inline bool container_header_ok(const ContainerHeader& h, uint64_t size
     return boff <= size && h.blob_bytes <= size - boff;
 }
 
+// what rb200_model_create would accept: a known coder, its scale_bits range, frequencies that sum to 1 << scale_bits
+RB200_HD inline bool container_model_ok(uint32_t coder, uint32_t scale_bits, const uint32_t* freqs)
+{
+    if (coder > RB200_CODER_RANS64 || scale_bits < 8 || scale_bits > 16) return false;
+    if (coder == RB200_CODER_WORD && scale_bits != 12) return false;
+    uint64_t sum = 0;
+    for (int s = 0; s < 256; s++) sum += freqs[s];
+    return sum == (1ull << scale_bits);
+}
+
+// What the decoders take beyond what rb200_container_open checks.  A version 1 container can pass open and still be
+// refused by the decode: rb200_container_decode returns RB200_E_ARG for the geometry and RB200_E_MODEL for the model.
+// chunks of 32 .. 2^24 symbols, and a blob below 2^36 bytes (the decoders index it in 16-byte vectors with 32 bits)
+RB200_HD inline bool container_geometry_decodable(uint32_t chunk_syms, uint64_t blob_bytes)
+{
+    return container_chunk_ok(chunk_syms) && (blob_bytes >> 36) == 0;
+}
+// the byte coder's frequencies are below 65536 (RansDecSymbol.freq is 16 bits wide, rans_byte.h:168-171)
+RB200_HD inline bool container_model_decodable(uint32_t coder, const uint32_t* freqs)
+{
+    if (coder != RB200_CODER_BYTE) return true;
+    for (int s = 0; s < 256; s++)
+        if (freqs[s] >= 65536u) return false;
+    return true;
+}
+
 // The per-element rules of a version 2 prefix, one block or one directory entry at a time.
 // one block's 256 frequencies sum to 4096
 RB200_HD inline bool container_block_model_ok(const uint16_t* freqs)
@@ -112,8 +135,6 @@ ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_
                                  uint64_t blob_bytes, uint32_t flags);
 // the header rb200_container_blocks_pack writes (crc fields zero)
 ContainerHeader container_blocks_header(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint64_t blob_bytes, uint32_t flags);
-// what rb200_model_create would accept: a known coder, its scale_bits range, frequencies that sum to 1 << scale_bits
-bool container_model_ok(uint32_t coder, uint32_t scale_bits, const uint32_t* freqs);
 // every block's 256 frequencies sum to 4096
 bool container_block_models_ok(const uint16_t* block_freqs, uint32_t n_blocks);
 // the directory rules: the first stream starts inside the first vector, monotone, last entry == blob_bytes

@@ -25,8 +25,9 @@
 // on one core: the blob CRC is optional for that reason).  rb200_container_encode / _decode and the _blocks_ forms
 // (rans_b200.cu) write and read the same bytes in host or device memory with the blob CRC on the GPU
 // (crc_kernels.cuh); they validate through the parser below, so both sides apply one set of rules.
-// rb200_container_blocks_decode_async applies the same rules in kernels (container_decode.cuh): the header and
-// per-element rules are the __host__ __device__ functions of container_format.h that the parser below calls.
+// rb200_container_decode_async and rb200_container_blocks_decode_async apply the same rules in kernels
+// (container_decode.cuh): the header, model and per-element rules are the __host__ __device__ functions of
+// container_format.h that the parser below calls.
 #include "container_format.h"
 
 #include <cstring>
@@ -84,15 +85,6 @@ uint32_t container_meta_crc(const ContainerHeader& h, const void* model, const u
     uint32_t c = container_header_crc(h);
     c = container_crc32(c, model, container_model_bytes(h));
     return container_crc32(c, offsets, (h.n_chunks + 1) * sizeof(uint64_t));
-}
-
-bool container_model_ok(uint32_t coder, uint32_t scale_bits, const uint32_t* freqs)
-{
-    if (coder > RB200_CODER_RANS64 || scale_bits < 8 || scale_bits > 16) return false;
-    if (coder == RB200_CODER_WORD && scale_bits != 12) return false;
-    uint64_t sum = 0;
-    for (int s = 0; s < 256; s++) sum += freqs[s];
-    return sum == (1ull << scale_bits);
 }
 
 bool container_block_models_ok(const uint16_t* block_freqs, uint32_t n_blocks)

@@ -93,55 +93,22 @@ extern "C" int rb200_alias_tables_build(const uint32_t freqs[256], const uint32_
     const uint32_t total = cum[256];
     if (total == 0 || total % 256u != 0) return RB200_E_MODEL;    // main_alias.cpp:151-152
     const uint32_t bucket = total / 256u;                         // :155
+    uint32_t rest[256], given[256];
+    const bool ok = rb200::alias_tables_core(freqs, bucket, divider, slot_adjust, slot_freqs, sym_id, rest, given);
 
-    // Phase 1 (main_alias.cpp:159-204): pair every under-full symbol with an
-    // over-full donor.  rest[] is what each symbol still has to hand out.
-    uint32_t rest[256];
+    // alias_remap (main_alias.cpp:225-228): bucket s gives its own part to symbol s and the rest to its partner, each
+    // after what earlier buckets gave that symbol -- the bases slot_adjust was formed from (:223-224)
     for (int s = 0; s < 256; s++) {
-        rest[s] = freqs[s];
-        divider[s] = bucket;
-        sym_id[2 * s] = sym_id[2 * s + 1] = static_cast<uint8_t>(s);
-    }
-    auto next_donor = [&](int from) { while (from < 256 && rest[from] < bucket) from++; return from; };
-    auto next_taker = [&](int from) { while (from < 256 && rest[from] >= bucket) from++; return from; };
-    int donor = next_donor(0);                                    // :172-173
-    int taker = next_taker(0);                                    // :174-175
-    int resume = taker + 1;                                       // :179
-    while (donor < 256 && taker < 256) {                          // :183
-        sym_id[2 * taker] = static_cast<uint8_t>(donor);          // :185
-        divider[taker] = rest[taker];                             // :186
-        rest[donor] -= bucket - divider[taker];                   // :189
-        if (rest[donor] >= bucket || resume <= donor) {           // :192
-            taker = next_taker(resume);
-            resume = taker + 1;
-        } else {
-            taker = donor;                                        // :199 (donor became a taker behind us)
-        }
-        donor = next_donor(donor);                                // :202-203
-    }
-
-    // Phase 2 (main_alias.cpp:207-232): hand out code slots bucket by bucket.
-    uint32_t given[256] = {0};
-    for (int s = 0; s < 256; s++) {
-        const int other = sym_id[2 * s];
-        const uint32_t own = divider[s], lent = bucket - own;
-        const uint32_t own_base = given[s], other_base = given[other];
         const uint32_t lo = static_cast<uint32_t>(s) * bucket;
-        divider[s] = lo + own;                                    // :219
-        slot_freqs[2 * s + 1] = freqs[s];                         // :221
-        slot_freqs[2 * s] = freqs[other];                         // :222
-        slot_adjust[2 * s + 1] = lo - own_base;                   // :223
-        slot_adjust[2 * s] = lo - (other_base - own);             // :224
-        uint32_t* dst_own = alias_remap + cum[s] + own_base;      // :225-226
+        const uint32_t own = divider[s] - lo, lent = bucket - own;
+        const int other = sym_id[2 * s];
+        const uint32_t own_base = lo - slot_adjust[2 * s + 1], other_base = lo + own - slot_adjust[2 * s];
+        uint32_t* dst_own = alias_remap + cum[s] + own_base;
         for (uint32_t k = 0; k < own; k++) dst_own[k] = lo + k;
-        uint32_t* dst_other = alias_remap + cum[other] + other_base;   // :227-228
+        uint32_t* dst_other = alias_remap + cum[other] + other_base;
         for (uint32_t k = 0; k < lent; k++) dst_other[k] = lo + own + k;
-        given[s] += own;                                          // :230-231
-        given[other] += lent;
     }
-    for (int s = 0; s < 256; s++)
-        if (given[s] != freqs[s]) return RB200_E_MODEL;           // :235-236
-    return RB200_OK;
+    return ok ? RB200_OK : RB200_E_MODEL;
 }
 
 // ---------------------------------------------------------------------------
@@ -172,7 +139,7 @@ int build_word_device_tables(const uint32_t freqs[256], WordDeviceTables& t)
         const uint32_t f = freqs[s];
         if (f == 4096) t.wide = 1;
         for (uint32_t k = 0; k < f; k++)                               // decode: one u32 per slot
-            t.dec[cum[s] + k] = ((f & 0xfffu) << 20) | (k << 8) | static_cast<uint32_t>(s);
+            t.dec[cum[s] + k] = word_dec_entry(static_cast<uint32_t>(s), f, k);
         // encode: exact x / f for any 32-bit x by the round-up reciprocal
         //   M = ceil(2^(32+sh) / f) = 2^32 + magic,  q = (x + mulhi(x, magic)) >> sh
         if (f == 0) {
@@ -217,10 +184,7 @@ int build_alias_device_tables(const uint32_t freqs[256], uint32_t scale_bits, Al
     int rc = rb200_alias_tables_build(freqs, cum, divider, slot_adjust, slot_freqs, sym_id, remap.data());
     if (rc != RB200_OK) return rc;
     t.scale_bits = scale_bits;
-    for (int b = 0; b < 256; b++)
-        t.dec[b] = {divider[b], (slot_freqs[2 * b] << 8) | sym_id[2 * b],
-                    (slot_freqs[2 * b + 1] << 8) | sym_id[2 * b + 1],
-                    (slot_adjust[2 * b] & 0xffffu) | (slot_adjust[2 * b + 1] << 16)};
+    for (uint32_t b = 0; b < 256; b++) t.dec[b] = alias_dec_entry(b, divider, slot_adjust, slot_freqs, sym_id);
     t.remap.resize(cum[256]);
     for (uint32_t i = 0; i < cum[256]; i++) t.remap[i] = static_cast<uint16_t>(remap[i]);
     for (int s = 0; s < 256; s++) {
@@ -254,7 +218,7 @@ int build_byte_device_tables(const uint32_t freqs[256], uint32_t scale_bits, Byt
     uint32_t* dsyms = reinterpret_cast<uint32_t*>(t.dec.data() + M);
     for (int s = 0; s < 256; s++) {
         std::memset(t.dec.data() + cum[s], s, freqs[s]);                // cum2sym, main.cpp:145-148
-        dsyms[s] = cum[s] | (freqs[s] << 16);                           // RansDecSymbolInit, rans_byte.h:246-252
+        dsyms[s] = byte_dec_symbol(cum[s], freqs[s]);                   // RansDecSymbolInit, rans_byte.h:246-252
         const uint32_t f = freqs[s];
         const uint32_t x_max = ((1u << 23 >> scale_bits) << 8) * (f ? f : 1);    // rans_byte.h:197
         if (f == 0) {           // never valid to encode (rans_byte.h:260): act like freq 1, flag it

@@ -65,6 +65,9 @@ struct rb200_ctx {
     // rb200_container_blocks_decode_async (container_decode.cuh): its fixed workspace and launch shapes
     BlocksAsyncWork* d_blocks_async = nullptr;
     BlocksAsyncShape blocks_async = {};
+    // rb200_container_decode_async: its fixed workspace (with the decode table) and its decoders' launches
+    SingleAsyncWork* d_single_async = nullptr;
+    SingleDecodeLaunch single_decoders[kSingleDecoders] = {};
 };
 
 struct rb200_model {
@@ -224,6 +227,8 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     if (e == cudaSuccess) e = cudaMallocHost(&ctx->h_crc, rb200_ctx::kMaxSlices * sizeof(CrcSlot));
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_blocks_async, sizeof(BlocksAsyncWork));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_async, 0, sizeof(BlocksAsyncWork));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_single_async, sizeof(SingleAsyncWork));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_single_async, 0, sizeof(SingleAsyncWork));
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -236,6 +241,7 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     configure_rans64_kernels();
     configure_crc_kernels();
     ctx->blocks_async = configure_container_decode(static_cast<uint32_t>(ctx->sms));
+    configure_single_decode(static_cast<uint32_t>(ctx->sms), ctx->single_decoders);
     cudaGetLastError();
     *out = ctx;
     return RB200_OK;
@@ -257,6 +263,7 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->d_crc) cudaFree(ctx->d_crc);
     if (ctx->h_crc) cudaFreeHost(ctx->h_crc);
     if (ctx->d_blocks_async) cudaFree(ctx->d_blocks_async);
+    if (ctx->d_single_async) cudaFree(ctx->d_single_async);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -1256,7 +1263,7 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
     if (n_symbols) *n_symbols = h.n_symbols;
     if (out_cap < h.n_symbols) return RB200_E_SPACE;
     if (h.n_symbols && !out) return RB200_E_ARG;
-    if (!chunk_ok(h.chunk_syms) || !blob_size_ok(h.blob_bytes)) return RB200_E_ARG;     // what rb200_decode accepts
+    if (!container_geometry_decodable(h.chunk_syms, h.blob_bytes)) return RB200_E_ARG;  // what rb200_decode accepts
     const uint8_t* blob = buf + container_blob_offset(h);
     const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h));
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
@@ -1288,8 +1295,10 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
                 return blocks_decode_host(ctx, blob, h.blob_bytes, offsets, block_freqs, h.n_blocks, h.block_size, h.chunk_syms, out, hook);
             });
     }
+    const uint32_t* freqs = reinterpret_cast<const uint32_t*>(prefix + sizeof(ContainerHeader));
+    if (!container_model_decodable(h.coder, freqs)) return RB200_E_MODEL;                 // what rb200_model_create accepts
     rb200_model* model = nullptr;
-    rc = rb200_model_create(ctx, h.coder, h.scale_bits, reinterpret_cast<const uint32_t*>(prefix + sizeof(ContainerHeader)), &model);
+    rc = rb200_model_create(ctx, h.coder, h.scale_bits, freqs, &model);
     if (rc != RB200_OK) return rc;
     rc = decode([&] { return decode_device(ctx, model, blob, h.blob_bytes, offsets, h.chunk_syms, out, h.n_symbols); },
                 [&](SliceCrc hook) { return decode_host(ctx, model, blob, h.blob_bytes, offsets, h.chunk_syms, out, h.n_symbols, hook); });
@@ -1422,20 +1431,19 @@ extern "C" int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf,
     return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, mem_kind == RB200_MEM_DEVICE, kContainerVersionBlocks);
 }
 
-// The kernels of container_decode.cuh, with lengths and positions the host cannot know taken from the plan on the
-// device; the host passes only bounds it knows (size).  Six launches, no copy, no synchronisation, no allocation.
-extern "C" int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
-                                                   uint64_t* d_n_symbols)
+namespace {
+
+// The async decodes' checks up to the verdict, for `version` (single: version 1's workspace, w == &single->c; null for
+// version 2): plan, meta CRC, blob CRC, the prefix check, version 1's model check and table build, then the verdict.
+// Lengths and positions the host cannot know come from the plan on the device; the host passes only bounds it knows
+// (size).
+int enqueue_container_checks(rb200_ctx* ctx, const uint8_t* buf, size_t size, size_t out_cap, uint64_t* d_n_symbols, uint16_t version,
+                             BlocksAsyncWork* w, SingleAsyncWork* single)
 {
-    if (!ctx || !buf || !out || (reinterpret_cast<uintptr_t>(d_n_symbols) & 7)) return RB200_E_ARG;
-    if (!container_mem_ok(RB200_MEM_DEVICE, buf, out)) return RB200_E_ARG;
-    DeviceGuard g(ctx->device);
-    BlocksAsyncWork* w = ctx->d_blocks_async;
-    const BlocksAsyncShape& shape = ctx->blocks_async;
     const uint32_t sms = static_cast<uint32_t>(ctx->sms);
     const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
     cudaStream_t s = ctx->stream;
-    container_plan_kernel<<<1, 32, 0, s>>>(buf, size, w);
+    container_plan_kernel<<<1, 32, 0, s>>>(buf, size, version, w, single);
     int rc = check_launch(ctx, "container_plan_kernel");
     if (rc != RB200_OK) return rc;
     crc32_kernel<<<crc32_grid(sms, after_head), kCrcThreads, kCrcSmemBytes, s>>>(buf + sizeof(ContainerHeader), after_head, &w->plan.meta_len,
@@ -1446,14 +1454,54 @@ extern "C" int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t
                                                                            &w->crc_work, &w->crc[1]);
     rc = check_launch(ctx, "crc32_kernel(blob)");
     if (rc != RB200_OK) return rc;
-    container_prefix_check_kernel<<<shape.check_grid, kPrefixWarps * 32, 0, s>>>(buf, w);
+    container_prefix_check_kernel<<<ctx->blocks_async.check_grid, kPrefixWarps * 32, 0, s>>>(buf, w);
     rc = check_launch(ctx, "container_prefix_check_kernel");
     if (rc != RB200_OK) return rc;
-    container_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status);
-    rc = check_launch(ctx, "container_verdict_kernel");
+    if (single) {
+        container_table_kernel<<<1, kTableThreads, 0, s>>>(buf, single);
+        rc = check_launch(ctx, "container_table_kernel");
+        if (rc != RB200_OK) return rc;
+    }
+    container_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status, single);
+    return check_launch(ctx, "container_verdict_kernel");
+}
+
+// the argument rules both async decodes share: device memory, buf and out 16-byte aligned, d_n_symbols 8-byte aligned
+bool async_args_ok(const rb200_ctx* ctx, const uint8_t* buf, const uint8_t* out, const uint64_t* d_n_symbols)
+{
+    return ctx && buf && out && !(reinterpret_cast<uintptr_t>(d_n_symbols) & 7) && container_mem_ok(RB200_MEM_DEVICE, buf, out);
+}
+
+}  // namespace
+
+// The kernels of container_decode.cuh.  Six launches, no copy, no synchronisation, no allocation.
+extern "C" int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                                   uint64_t* d_n_symbols)
+{
+    if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    BlocksAsyncWork* w = ctx->d_blocks_async;
+    int rc = enqueue_container_checks(ctx, buf, size, out_cap, d_n_symbols, kContainerVersionBlocks, w, nullptr);
     if (rc != RB200_OK) return rc;
-    block_decode_planned_kernel<<<shape.decode_grid, kPlannedWarps * 32, 0, s>>>(buf, out, w, ctx->d_status);
+    block_decode_planned_kernel<<<ctx->blocks_async.decode_grid, kPlannedWarps * 32, 0, ctx->stream>>>(buf, out, w, ctx->d_status);
     return check_launch(ctx, "block_decode_planned_kernel");
+}
+
+// The same checks for version 1, then every decoder variant on its fixed grid: the verdict's go names the one that
+// runs.  Seventeen launches, no copy, no synchronisation, no allocation.
+extern "C" int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                            uint64_t* d_n_symbols)
+{
+    if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    SingleAsyncWork* w = ctx->d_single_async;
+    int rc = enqueue_container_checks(ctx, buf, size, out_cap, d_n_symbols, kContainerVersion, &w->c, w);
+    for (int i = 0; i < kSingleDecoders && rc == RB200_OK; i++) {
+        const SingleDecodeLaunch& l = ctx->single_decoders[i];
+        l.kernel<<<l.grid, l.threads, l.smem, ctx->stream>>>(buf, out, w, ctx->d_status);
+        rc = check_launch(ctx, l.name);
+    }
+    return rc;
 }
 
 // ---------------------------------------------------------------------------

@@ -3,10 +3,19 @@
 #include <cstdint>
 #include <vector>
 
+#include "hd.h"
+
 namespace rb200 {
 
 // marks a symbol the model gives frequency 0; the encoder flags RB200_E_SYMBOL
 constexpr uint32_t kEncBadSymbol = 0x80000000u;
+
+// The per-entry formulas of the decode tables below.  The host builders (model_host.cpp) and the device build of
+// rb200_container_decode_async (container_decode.cuh) both call them, so both produce the same bytes.
+// word: slot k of symbol s with frequency f (4096 is stored as 0, see WordDeviceTables)
+RB200_HD inline uint32_t word_dec_entry(uint32_t s, uint32_t f, uint32_t k) { return ((f & 0xfffu) << 20) | (k << 8) | s; }
+// byte: symbol s's RansDecSymbol {start, freq} (freq < 65536)
+RB200_HD inline uint32_t byte_dec_symbol(uint32_t start, uint32_t f) { return start | (f << 16); }
 
 // ---- word coder (rans_word_sse41.h semantics, scale_bits 12)
 //
@@ -47,6 +56,66 @@ int build_word_device_tables(const uint32_t freqs[256], WordDeviceTables& t);
 //   alias_remap as u16 (values < 65536; SURVEY H8) = 128 KiB at scale_bits 16.
 struct AliasDecEntry { uint32_t divider, alt0, alt1, adjust; };
 struct AliasEncEntry { uint32_t magic, freq, cum, shift; };
+
+// bucket b's decode entry from the arrays of alias_tables_core
+RB200_HD inline AliasDecEntry alias_dec_entry(uint32_t b, const uint32_t* divider, const uint32_t* slot_adjust, const uint32_t* slot_freqs,
+                                              const uint8_t* sym_id)
+{
+    return {divider[b], (slot_freqs[2 * b] << 8) | sym_id[2 * b], (slot_freqs[2 * b + 1] << 8) | sym_id[2 * b + 1],
+            (slot_adjust[2 * b] & 0xffffu) | (slot_adjust[2 * b + 1] << 16)};
+}
+
+// make_alias_table (main_alias.cpp:147-237) up to what decode needs: divider[256], slot_adjust[512], slot_freqs[512] and
+// sym_id[512] for frequencies that sum to 256 * bucket.  alias_remap, which only the encoder needs, follows from these
+// (rb200_alias_tables_build).  rest and given are 256 words of scratch each.  False if the pairing does not hand out
+// exactly every symbol's frequency (main_alias.cpp:235-236).  Sequential by nature: one thread runs it.
+RB200_HD inline bool alias_tables_core(const uint32_t* freqs, uint32_t bucket, uint32_t* divider, uint32_t* slot_adjust,
+                                       uint32_t* slot_freqs, uint8_t* sym_id, uint32_t* rest, uint32_t* given)
+{
+    // Phase 1 (main_alias.cpp:159-204): pair every under-full symbol with an over-full donor.  rest[] is what each
+    // symbol still has to hand out.
+    for (int s = 0; s < 256; s++) {
+        rest[s] = freqs[s];
+        divider[s] = bucket;
+        sym_id[2 * s] = sym_id[2 * s + 1] = static_cast<uint8_t>(s);
+        given[s] = 0;
+    }
+    int donor = 0, taker = 0;
+    while (donor < 256 && rest[donor] < bucket) donor++;          // :172-173
+    while (taker < 256 && rest[taker] >= bucket) taker++;         // :174-175
+    int resume = taker + 1;                                       // :179
+    while (donor < 256 && taker < 256) {                          // :183
+        sym_id[2 * taker] = static_cast<uint8_t>(donor);          // :185
+        divider[taker] = rest[taker];                             // :186
+        rest[donor] -= bucket - divider[taker];                   // :189
+        if (rest[donor] >= bucket || resume <= donor) {           // :192
+            taker = resume;
+            while (taker < 256 && rest[taker] >= bucket) taker++;
+            resume = taker + 1;
+        } else {
+            taker = donor;                                        // :199 (donor became a taker behind us)
+        }
+        while (donor < 256 && rest[donor] < bucket) donor++;      // :202-203
+    }
+
+    // Phase 2 (main_alias.cpp:207-232): hand out code slots bucket by bucket.
+    for (int s = 0; s < 256; s++) {
+        const int other = sym_id[2 * s];
+        const uint32_t own = divider[s], lent = bucket - own;
+        const uint32_t own_base = given[s], other_base = given[other];
+        const uint32_t lo = static_cast<uint32_t>(s) * bucket;
+        divider[s] = lo + own;                                    // :219
+        slot_freqs[2 * s + 1] = freqs[s];                         // :221
+        slot_freqs[2 * s] = freqs[other];                         // :222
+        slot_adjust[2 * s + 1] = lo - own_base;                   // :223
+        slot_adjust[2 * s] = lo - (other_base - own);             // :224
+        given[s] += own;                                          // :230-231
+        given[other] += lent;
+    }
+    for (int s = 0; s < 256; s++)
+        if (given[s] != freqs[s]) return false;                   // :235-236
+    return true;
+}
 struct AliasDeviceTables {
     uint32_t scale_bits;
     AliasDecEntry dec[256];

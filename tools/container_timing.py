@@ -15,9 +15,17 @@ buffers, per-block Zipf data with a permuted alphabet per block):
   call with flags 0 and RB200_CONTAINER_CRC_BLOB, alternated; and the host time each container decode call takes to
   return.
 
+With --single, the single-model container's decode calls on three workloads of 1 GiB in device memory, chunks of 8192:
+the headline one (uniform, word), Zipf 1.1 with the alias coder at scale_bits 16, and uniform with rans64 at 14:
+
+  rb200_decode against rb200_container_decode and rb200_container_decode_async, each container call with flags 0 and
+  RB200_CONTAINER_CRC_BLOB, alternated; the host time each container decode call takes to return; and a torch.profiler
+  list of the kernels of rb200_decode and of the async call (median device time per kernel), which shows the planned
+  decoder against the shipped one and the launches the verdict gated out.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
-    python tools/container_timing.py [--blocks] [--reps 10] [--json out.json]"""
+    python tools/container_timing.py [--blocks | --single] [--reps 10] [--json out.json]"""
 import argparse
 import json
 import os
@@ -253,16 +261,112 @@ def headline(args):
     return res
 
 
+def zipf_data(n, seed, s=1.1):
+    """p(r) ~ r^-s over 256 symbols, generated on the GPU in pieces"""
+    import torch
+    g = torch.Generator(device="cuda")
+    g.manual_seed(seed)
+    p = 1.0 / torch.arange(1, 257, device="cuda", dtype=torch.float64) ** s
+    cdf = (torch.cumsum(p, 0) / p.sum()).to(torch.float32)
+    out = torch.empty(n, dtype=torch.uint8, device="cuda")
+    step = 1 << 26
+    for lo in range(0, n, step):
+        u = torch.rand(min(step, n - lo), device="cuda", generator=g)
+        out[lo:lo + u.numel()] = torch.searchsorted(cdf, u).clamp_(max=255).to(torch.uint8)
+    return out
+
+
+def kernel_times(fn, sync, reps):
+    """torch.profiler over `reps` calls of fn: {kernel name: median device time in us per call, launches per call}"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            fn()
+            sync()
+    per = {}
+    for e in prof.events():
+        if e.device_type == torch.autograd.DeviceType.CUDA and not e.name.startswith("Memcpy") and not e.name.startswith("Memset"):
+            per.setdefault(e.name, []).append(e.time_range.elapsed_us())
+    return {k: {"median_us": float(np.median(v)), "launches_per_call": len(v) / reps} for k, v in per.items()}
+
+
+def single(args):
+    import torch
+    n, chunk = 1 << 30, 8192
+    g = torch.Generator(device="cuda")
+    g.manual_seed(1234)
+    workloads = (("uniform word", rb.CODER_WORD, 12, lambda: torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda", generator=g)),
+                 ("Zipf 1.1 alias 16", rb.CODER_ALIAS, 16, lambda: zipf_data(n, 1235)),
+                 ("uniform rans64 14", rb.CODER_RANS64, 14, lambda: torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda", generator=g)))
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    crc = api.CONTAINER_CRC_BLOB
+    cap = ctx.container_capacity(n, chunk)
+    n_chunks = ctx.chunk_count(n, chunk)
+    dir_off = 64 + 1024
+    boff = (dir_off + 8 * (n_chunks + 1) + 15) & ~15
+    d_out = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+    d_cont = {0: torch.empty(cap + 16, dtype=torch.uint8, device="cuda"), crc: torch.empty(cap + 16, dtype=torch.uint8, device="cuda")}
+    res = {"card": card(), "workloads": {}, "checks": {}}
+    for name, coder, sb, make in workloads:
+        d_in = make()
+        model = rb.Model.from_data(ctx, coder, sb, device_ptr=d_in.data_ptr(), n=n)
+        for flags, d in d_cont.items():
+            ctx.container_encode_device(model, d_in.data_ptr(), n, chunk, flags, d.data_ptr(), cap)
+        sync()
+        head = d_cont[0][:64].cpu().numpy()
+        blob_bytes = int(head[32:40].view(np.uint64)[0])
+        size = boff + blob_bytes
+        b0, bc = d_cont[0].data_ptr(), d_cont[crc].data_ptr()
+        dec = {
+            "decode": lambda: ctx.decode_device(model, b0 + boff, blob_bytes, b0 + dir_off, chunk, d_out.data_ptr(), n),
+            "container_decode": lambda: ctx.container_decode_device(b0, size, d_out.data_ptr(), n),
+            "container_decode_crc": lambda: ctx.container_decode_device(bc, size, d_out.data_ptr(), n),
+            "container_decode_async": lambda: ctx.container_decode_async(b0, size, d_out.data_ptr(), n),
+            "container_decode_async_crc": lambda: ctx.container_decode_async(bc, size, d_out.data_ptr(), n),
+        }
+        dtimes = alternate(dec, sync, args.warmup, args.reps)
+        host = {k: [] for k in dec if k != "decode"}
+        for _ in range(args.reps):
+            for k in host:
+                t0 = time.perf_counter()
+                dec[k]()
+                host[k].append((time.perf_counter() - t0) * 1e3)
+                sync()
+        for k in dec:
+            d_out.zero_()
+            dec[k]()
+            sync()
+            res["checks"][f"{name}: {k}_equals_input"] = bool(torch.equal(d_out[:n], d_in))
+        kernels = {k: kernel_times(dec[k], sync, args.reps) for k in ("decode", "container_decode_async", "container_decode_async_crc")}
+        planned = {k: v for k, v in kernels["container_decode_async"].items() if "decode_planned_kernel" in k}
+        ran = max(planned, key=lambda k: planned[k]["median_us"])
+        res["workloads"][name] = {
+            "n": n, "chunk_syms": chunk, "blob_bytes": blob_bytes, "container_bytes": size,
+            "decode": dtimes,
+            "decode_call_host_ms": {k: stats(v) for k, v in host.items()},
+            "kernels": kernels,
+            "planned_decoder": ran,
+            "gated_out_launches": {"count": len(planned) - 1, "sum_us": sum(v["median_us"] for k, v in planned.items() if k != ran)},
+        }
+        model.close()
+        del d_in
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
+    ap.add_argument("--single", action="store_true", help="the single-model container's decode calls on three workloads")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else headline(args)
+    res = blocks(args) if args.blocks else single(args) if args.single else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:

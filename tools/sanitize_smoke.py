@@ -104,6 +104,39 @@ def main():
             pass
         assert not d_out.any().item()
         d_cb[pos] ^= 1
+    # the single-model container decoded by kernels alone: a valid container of each coder, then (alias) a corrupt
+    # model and a corrupt blob, rejected before any decode, and a corrupt stream with flags 0, which the decoder reports
+    for coder, sb in ((rb.CODER_WORD, 12), (rb.CODER_ALIAS, 16), (rb.CODER_BYTE, 14), (rb.CODER_RANS64, 12)):
+        f, _ = orc.model(data, sb)
+        m = ctx.model(coder, sb, f)
+        ccap = ctx.container_capacity(data.size, 4096)
+        d_c = torch.zeros(ccap + 16, dtype=torch.uint8, device="cuda")
+        for flags in (api.CONTAINER_CRC_BLOB, 0):
+            ctx.container_encode_device(m, d_in.data_ptr(), data.size, 4096, flags, d_c.data_ptr(), ccap)
+            d_out.zero_()
+            ctx.container_decode_async(d_c.data_ptr(), ccap, d_out.data_ptr(), data.size, d_n.data_ptr())
+            ctx.sync()
+            assert int(d_n.item()) == data.size and torch.equal(d_out[:data.size], d_in), (coder, flags)
+        m.close()
+        if coder != rb.CODER_ALIAS:
+            continue
+        h_c = d_c[:ccap].cpu().numpy()
+        boff = api.container_open(h_c)[3].ctypes.data - h_c.ctypes.data
+        for pos, flags in ((64 + 3, api.CONTAINER_CRC_BLOB), (boff + 1000, api.CONTAINER_CRC_BLOB), (boff + 1000, 0)):
+            m = ctx.model(coder, sb, f)
+            ctx.container_encode_device(m, d_in.data_ptr(), data.size, 4096, flags, d_c.data_ptr(), ccap)
+            ctx.sync()
+            m.close()
+            d_c[pos] ^= 1
+            d_out.zero_()
+            ctx.container_decode_async(d_c.data_ptr(), ccap, d_out.data_ptr(), data.size, d_n.data_ptr())
+            try:
+                ctx.sync()
+                raise SystemExit("single-model container corruption not reported")
+            except rb.RansError:
+                pass
+            if flags:
+                assert not d_out.any().item()
     print("sanitize smoke ok:", ctx.launches, "launches")
 
 

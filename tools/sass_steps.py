@@ -45,10 +45,16 @@ def main():
     enc = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1" in k)
     tma = next(v for k, v in fns.items() if "word_decode_tma_kernel" in k and k.endswith("Lb0EEEvPKhmPKmPKjPhmjjPNS_10DecodeWorkEPjy"))
     ali = next(v for k, v in fns.items() if "alias_decode_persist_kernelILj16E" in k)
+    tma_planned = next(v for k, v in fns.items() if "word_decode_planned_kernelILb0E" in k)
+    ali_planned = next(v for k, v in fns.items() if "alias_decode_planned_kernelILj16E" in k)
     for title, step in (("word_decode_tma_kernel<DecShip, false> (round 2, shipped): one step (symbol store to symbol store)",
                          step_between(tma, "STG.E.U8", 2)),
+                        ("word_decode_planned_kernel<false> (rb200_container_decode_async): one step (symbol store to symbol store)",
+                         step_between(tma_planned, "STG.E.U8", 2)),
                         ("alias_decode_persist_kernel<16> (round 2, shipped): one step (symbol store to symbol store)",
                          step_between(ali, "STG.E.U8", 2)),
+                        ("alias_decode_planned_kernel<16> (rb200_container_decode_async): one step (symbol store to symbol store)",
+                         step_between(ali_planned, "STG.E.U8", 2)),
                         ("block_decode_kernel (round 1 window: decode_window_chunk with WordDecoder<false>): one step (vote to vote)",
                          step_between(dec, "VOTE.ANY", 5)),
                         ("word_encode_fused_kernel<R32>: one step (symbol load to symbol load)", step_between(enc, "LDS.U8", 8))):
