@@ -245,6 +245,21 @@ int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t* buf, size
 int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                  uint64_t* d_n_symbols);
 
+/* The encode side of the same: rb200_model_from_data(ctx, coder, scale_bits, in, n, RB200_MEM_DEVICE, ...), then
+ * rb200_container_encode(..., RB200_MEM_DEVICE) with that model, then rb200_model_destroy -- the same container bytes,
+ * with the model built on the GPU, so that the call only enqueues work on the context's stream: it never synchronises
+ * or copies to the host, and it allocates nothing for the model.  `in` and `out` are device memory, `out` 16-byte
+ * aligned.  The encode workspace grows as in rb200_container_encode, so a call of the same geometry outside a CUDA
+ * graph capture must come first.  The call returns RB200_E_ARG (nothing launched) for a null ctx, in or out, a
+ * misaligned out, an unknown coder, the word coder with scale_bits != 12, scale_bits outside 8 .. 16, chunk_syms outside
+ * 32 .. 2^24, n >= 2^32 (counts of 32 bits, as rb200_model_from_data) or 2^31 chunks or more; RB200_E_MODEL for n == 0;
+ * RB200_E_SPACE when out_cap is below the blob offset.  rb200_sync returns RB200_E_MODEL when rb200_model_create would
+ * refuse the model (the byte coder at scale_bits 16 on data of one symbol: a frequency of 65536), RB200_E_SPACE when
+ * the blob does not fit out_cap, RB200_E_STALL as elsewhere.  On every error the header is not written.  The container
+ * is rb200_container_size(n_chunks, blob_bytes) bytes, blob_bytes from its header. */
+int rb200_container_model_encode_async(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, size_t n,
+                                       uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap);
+
 /* ---------------------------------------------------------------- multi-GPU: gathering the shards' blobs (NCCL) */
 
 /* Shards are independent (SURVEY 8e): every rank encodes / decodes its own contiguous range of symbols with no

@@ -56,6 +56,8 @@ EXPORTS = [
     ("rb200_container_blocks_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
     ("rb200_container_blocks_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_container_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_container_model_encode_async", C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_size_t, C.c_uint32,
+                                                     C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -363,6 +365,13 @@ class Context:
         """enqueue only (CUDA-graph capturable), any coder; n_ptr: device address of a u64 that receives n, or 0.  The
         verdict on the container (-4 corrupt or not decodable, -3 out_cap too small, output untouched) comes from sync()"""
         self.lib.check(self.lib.dll.rb200_container_decode_async(self.h, buf_ptr, size, out_ptr, out_cap, n_ptr or None), self.h)
+
+    def container_model_encode_async(self, coder, scale_bits, in_ptr, n, chunk_syms, flags, out_ptr, out_cap):
+        """enqueue only (CUDA-graph capturable once a call of the same geometry has grown the workspace): the model built
+        from the data on the GPU, then the container, as Model.from_data + container_encode_device.  The verdict (-2 a
+        model rb200_model_create refuses, -3 out_cap too small for the blob, header unwritten) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_model_encode_async(self.h, coder, scale_bits, in_ptr, n, chunk_syms, flags, out_ptr,
+                                                                       out_cap), self.h)
 
     # ---- per-block containers (version 2): every block's model, the directory and the blob in one buffer
     def container_blocks_capacity(self, n_blocks, block_size, chunk_syms):

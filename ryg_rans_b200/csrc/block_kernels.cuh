@@ -84,11 +84,14 @@ inline void launch_histogram(cudaStream_t stream, uint32_t sms, const uint8_t* d
 // ---------------------------------------------------------------------------
 constexpr int kModelWarps = 8;
 
-// calc_cum_freqs + normalize_freqs(4096) (main.cpp:68-129) on 256 counts in shared memory, run by ONE warp, bit-exact:
-// s_cnt = the block's histogram (sums to block_size), s_cum / s_w = 257 / 256 words of workspace; the normalised
-// frequencies end up in s_w and in dst[0..256).
-__device__ __forceinline__ void block_normalize(const uint32_t* s_cnt, uint32_t* s_cum, uint32_t* s_w, uint16_t* __restrict__ dst,
-                                                uint32_t* __restrict__ status)
+// calc_cum_freqs + normalize_freqs(target) (main.cpp:68-129) on 256 counts in shared memory, run by ONE warp, bit-exact:
+// s_cnt = the counts (their sum below 2^32), s_cum / s_w = 257 / 256 words of workspace (s_w 16-byte aligned); the
+// normalised frequencies end up in s_w and in dst[0..256).  target <= 65536: the resample product target * cum is below
+// 2^48 and the arg-min key (width << 8 | symbol) below 2^25.  When no symbol can give up a slot (main.cpp:104) it ORs
+// fail_bit into the status word.  The per-block callers pass compile-time constants (4096, kStatStream).
+template <class T>
+__device__ __forceinline__ void block_normalize(const uint32_t* s_cnt, uint32_t* s_cum, uint32_t* s_w, T* __restrict__ dst, uint32_t target,
+                                                uint32_t fail_bit, uint32_t* __restrict__ status)
 {
     const uint32_t lane = threadIdx.x & 31;
     // calc_cum_freqs (main.cpp:68-73): lane l owns symbols 8l .. 8l+7
@@ -105,8 +108,8 @@ __device__ __forceinline__ void block_normalize(const uint32_t* s_cnt, uint32_t*
     // resample, main.cpp:83-84 (cum[0] stays 0)
 #pragma unroll
     for (int j = 0; j < 8; j++)
-        s_cum[8 * lane + j] = static_cast<uint32_t>((static_cast<uint64_t>(kWordSlots) * (base + local[j])) / total);
-    if (lane == 31) s_cum[256] = kWordSlots;                       // 4096 * total / total
+        s_cum[8 * lane + j] = static_cast<uint32_t>((static_cast<uint64_t>(target) * (base + local[j])) / total);
+    if (lane == 31) s_cum[256] = target;                           // target * total / total
     __syncwarp();
 
     // main.cpp:90-116, symbols in order.  Moving the boundaries between donor and taker by one changes exactly
@@ -138,9 +141,9 @@ __device__ __forceinline__ void block_normalize(const uint32_t* s_cnt, uint32_t*
         }
         __syncwarp();
     }
-    if (failed && lane == 0) atomicOr(status, kStatStream);
+    if (failed && lane == 0) atomicOr(status, fail_bit);
 #pragma unroll
-    for (int j = 0; j < 8; j++) dst[8 * lane + j] = static_cast<uint16_t>(s_w[8 * lane + j]);     // main.cpp:127
+    for (int j = 0; j < 8; j++) dst[8 * lane + j] = static_cast<T>(s_w[8 * lane + j]);            // main.cpp:127
 }
 
 // Shared-memory workspace of the per-block model build.
@@ -185,7 +188,7 @@ __device__ __forceinline__ void block_model_build(const uint8_t* __restrict__ bl
         sm.cnt[s] = t;
     }
     __syncthreads();
-    if (warp == 0) block_normalize(sm.cnt, sm.cum, sm.h[0], dst, status);      // h[0] is reused for the 256 widths
+    if (warp == 0) block_normalize(sm.cnt, sm.cum, sm.h[0], dst, kWordSlots, kStatStream, status);      // h[0] is reused for the 256 widths
     __syncthreads();
 }
 
@@ -226,7 +229,7 @@ __device__ __forceinline__ void block_model_build_wide(const uint8_t* __restrict
         s_cnt[s] = t;
     }
     __syncthreads();
-    if (warp == 0) block_normalize(s_cnt, s_cum, s_w, dst, status);
+    if (warp == 0) block_normalize(s_cnt, s_cum, s_w, dst, kWordSlots, kStatStream, status);
     __syncthreads();
 }
 

@@ -10,6 +10,7 @@ constexpr uint32_t kStatStream = 1u;   // a chunk stream did not end where it mu
 constexpr uint32_t kStatSymbol = 2u;   // encoder saw a symbol with model frequency 0
 constexpr uint32_t kStatSpace  = 4u;   // compacted blob does not fit blob_cap
 constexpr uint32_t kStatStall  = 8u;   // a bounded wait inside a kernel expired (a bug or a wedged GPU, not bad input)
+constexpr uint32_t kStatModel  = 16u;  // the model built from the data is one rb200_model_create refuses
 
 constexpr uint32_t kHeaderBytes = 128; // 32 lanes x u32 final state (RansWordEncFlush / RansEncFlush x 32)
 

@@ -117,13 +117,6 @@ extern "C" int rb200_alias_tables_build(const uint32_t freqs[256], const uint32_
 
 namespace rb200 {
 
-static uint32_t ceil_log2(uint32_t v)
-{
-    uint32_t s = 0;
-    while ((1u << s) < v) s++;
-    return s;
-}
-
 int build_word_device_tables(const uint32_t freqs[256], WordDeviceTables& t)
 {
     uint32_t cum[257];
@@ -140,30 +133,9 @@ int build_word_device_tables(const uint32_t freqs[256], WordDeviceTables& t)
         if (f == 4096) t.wide = 1;
         for (uint32_t k = 0; k < f; k++)                               // decode: one u32 per slot
             t.dec[cum[s] + k] = word_dec_entry(static_cast<uint32_t>(s), f, k);
-        // encode: exact x / f for any 32-bit x by the round-up reciprocal
-        //   M = ceil(2^(32+sh) / f) = 2^32 + magic,  q = (x + mulhi(x, magic)) >> sh
-        if (f == 0) {
-            t.enc[s] = {0u, kEncBadSymbol};
-            t.enc32[s] = {0u, kEncBadSymbol};
-        } else {
-            const uint32_t sh = ceil_log2(f);
-            const unsigned __int128 one = 1;
-            const unsigned __int128 M = ((one << (32 + sh)) + f - 1) / f;
-            const uint32_t magic = static_cast<uint32_t>(M - (one << 32));
-            t.enc[s] = {magic, f | (cum[s] << 13) | (sh << 25)};
-            // 32-bit reciprocal, exact on x < f << 20 (see tables.h)
-            if (f == 1) {
-                t.enc32[s] = {0xffffffffu, f | (cum[s] << 13)};
-            } else {
-                const uint32_t s32 = sh - 1;
-                const uint64_t pow = 1ull << (32 + s32);
-                const uint64_t M32 = (pow + f - 1) / f;                    // < 2^32 because 2^s32 < f
-                const uint64_t err = M32 * f - pow;                        // < f
-                const uint64_t xmax = (static_cast<uint64_t>(f) << 20) - 1;
-                if (M32 >> 32 || xmax * err >= pow) t.enc32_ok = 0;
-                t.enc32[s] = {static_cast<uint32_t>(M32), f | (cum[s] << 13) | (s32 << 25)};
-            }
-        }
+        // encode: exact x / f by the round-up reciprocal, 33-bit (any x) and 32-bit (x < f << 20) forms (tables.h)
+        t.enc[s] = word_enc_entry(f, cum[s]);
+        t.enc32[s] = word_enc32_entry(f, cum[s], &t.enc32_ok);
     }
     return RB200_OK;
 }
@@ -187,18 +159,7 @@ int build_alias_device_tables(const uint32_t freqs[256], uint32_t scale_bits, Al
     for (uint32_t b = 0; b < 256; b++) t.dec[b] = alias_dec_entry(b, divider, slot_adjust, slot_freqs, sym_id);
     t.remap.resize(cum[256]);
     for (uint32_t i = 0; i < cum[256]; i++) t.remap[i] = static_cast<uint16_t>(remap[i]);
-    for (int s = 0; s < 256; s++) {
-        const uint32_t f = freqs[s];
-        if (f == 0) {
-            t.enc[s] = {0u, 0u, 0u, kEncBadSymbol};
-        } else {
-            // same round-up reciprocal as the word coder: exact for every 32-bit x
-            const uint32_t sh = ceil_log2(f);
-            const unsigned __int128 one = 1;
-            const unsigned __int128 M = ((one << (32 + sh)) + f - 1) / f;
-            t.enc[s] = {static_cast<uint32_t>(M - (one << 32)), f, cum[s], sh};
-        }
-    }
+    for (int s = 0; s < 256; s++) t.enc[s] = alias_enc_entry(freqs[s], cum[s]);
     return RB200_OK;
 }
 
@@ -219,17 +180,7 @@ int build_byte_device_tables(const uint32_t freqs[256], uint32_t scale_bits, Byt
     for (int s = 0; s < 256; s++) {
         std::memset(t.dec.data() + cum[s], s, freqs[s]);                // cum2sym, main.cpp:145-148
         dsyms[s] = byte_dec_symbol(cum[s], freqs[s]);                   // RansDecSymbolInit, rans_byte.h:246-252
-        const uint32_t f = freqs[s];
-        const uint32_t x_max = ((1u << 23 >> scale_bits) << 8) * (f ? f : 1);    // rans_byte.h:197
-        if (f == 0) {           // never valid to encode (rans_byte.h:260): act like freq 1, flag it
-            t.enc[s] = {x_max, 0xffffffffu, M - 1, ((M - 1) & 0xffffu) | kEncBadSymbol};
-        } else if (f == 1) {    // rans_byte.h:199-228
-            t.enc[s] = {x_max, 0xffffffffu, cum[s] + M - 1, (M - 1) & 0xffffu};
-        } else {                // rans_byte.h:229-242
-            const uint32_t sh = ceil_log2(f);
-            const uint32_t rcp = static_cast<uint32_t>(((1ull << (sh + 31)) + f - 1) / f);
-            t.enc[s] = {x_max, rcp, cum[s], ((M - f) & 0xffffu) | ((sh - 1) << 16)};
-        }
+        t.enc[s] = byte_enc_entry(freqs[s], cum[s], scale_bits);
     }
     return RB200_OK;
 }
@@ -252,24 +203,7 @@ int build_rans64_device_tables(const uint32_t freqs[256], uint32_t scale_bits, R
         std::memset(t.dec.data() + cum[s], s, freqs[s]);                // cum2sym, main64.cpp:145-148
         dsyms[2 * s] = cum[s];                                          // Rans64DecSymbolInit, rans64.h:250-256
         dsyms[2 * s + 1] = freqs[s];
-        const uint32_t f = freqs[s];
-        uint64_t rcp;
-        uint32_t shift, bias, flag = 0;
-        if (f < 2) {                                                    // rans64.h:199-228 (freq 0: same, flagged)
-            rcp = ~0ull;
-            shift = 0;
-            bias = (f ? cum[s] : 0) + M - 1;
-            if (f == 0) flag = kEncBadSymbol;
-        } else {                                                        // rans64.h:229-246
-            const uint32_t k = ceil_log2(f);
-            const unsigned __int128 one = 1;
-            rcp = static_cast<uint64_t>(((one << (k + 63)) + f - 1) / f);
-            shift = k - 1;
-            bias = cum[s];
-        }
-        const uint32_t fe = f ? f : 1;
-        const uint32_t e[8] = {static_cast<uint32_t>(rcp), static_cast<uint32_t>(rcp >> 32), fe, bias, M - fe, shift | flag, 0, 0};
-        std::memcpy(t.enc[s], e, sizeof e);
+        rans64_enc_entry(freqs[s], cum[s], scale_bits, t.enc[s]);
     }
     return RB200_OK;
 }

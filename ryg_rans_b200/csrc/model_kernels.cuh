@@ -1,0 +1,154 @@
+// model_kernels.cuh -- rb200_container_model_encode_async: a single-model (version 1) container whose model is built
+// from the data on the GPU, so that the whole encode only enqueues work (and can be captured in a CUDA graph).
+//
+// The stages run in stream order on the context's stream (rans_b200.cu); each reads what the one before it left in the
+// context's ModelAsyncWork:
+//   memset + histogram_kernel   the data's 256 counts into counts[]
+//   container_model_kernel      one CTA: calc_cum_freqs + normalize_freqs(1 << scale_bits) on the counts, bit-exact
+//                               (block_normalize); the checks of rb200_model_create (kStatModel on refusal); the coder's
+//                               encode tables, byte for byte what rb200_model_create uploads (tables.h formulas)
+//   the coder's encoder         the shipped kernel with its table pointers into the workspace.  The word coder runs
+//                               both instances of its gated wrappers below; r32 names the one that encodes, the other
+//                               exits before it touches the counter, look[] or scratch
+//   crc32_kernel x 1-2, container_finish_kernel
+//                               as rb200_container_encode in device memory, with the model section from freqs[]
+#pragma once
+#include "block_kernels.cuh"
+#include "container_format.h"
+#include "tables.h"
+#include "word_kernels.cuh"
+
+namespace rb200 {
+
+// The call's workspace: fixed-size (about 150 KiB), allocated with the context, so the call never allocates for the
+// model.  Every table has the layout of its rb200_model counterpart.
+struct ModelAsyncWork {
+    unsigned long long counts[256];               // the histogram; zeroed in stream order before each call
+    uint32_t freqs[256];                          // the normalised model: the container's model section
+    uint32_t r32;                                 // the word encoder to run: 1 the 32-bit reciprocal instance, 0 the 33-bit
+    alignas(16) WordEncEntry word_enc[256];       // word: 33-bit reciprocals (WordDeviceTables::enc)
+    alignas(16) WordEncEntry word_enc32[256];     // word: 32-bit reciprocals (WordDeviceTables::enc32)
+    alignas(16) AliasEncEntry alias_enc[256];
+    alignas(16) AliasEncEntry byte_enc[256];      // RansEncSymbol images
+    alignas(16) uint4 r64_enc[256 * 2];           // Rans64EncSymbol images, 32 bytes each
+    alignas(16) uint16_t alias_remap[1u << 16];   // the first 1 << scale_bits entries are the model's
+};
+
+constexpr int kModelThreads = 256;                // one thread per symbol
+
+// coder and scale_bits are valid (the host checks them); r32_allowed is word_r32_allowed().  A model
+// rb200_model_create refuses sets kStatModel, and the tables are written all the same (the encoders then run on
+// well-formed entries, and container_finish_kernel writes no header).  Normalisation itself cannot fail for targets
+// >= 256: a squashed symbol needs a donor of width > 1, and while any symbol is squashed the widths, which sum to the
+// target, cannot all be <= 1.  block_normalize keeps its check all the same, with kStatModel as the verdict.
+__global__ void __launch_bounds__(kModelThreads)
+    container_model_kernel(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w, uint32_t* __restrict__ status)
+{
+    __shared__ uint32_t s_cnt[256], s_cum[257];
+    __shared__ __align__(16) uint32_t s_w[256];
+    __shared__ uint32_t s_divider[256], s_adjust[512], s_slot_freqs[512], s_rest[256], s_given[256];
+    __shared__ uint8_t s_sym_id[512];
+    __shared__ uint32_t s_paired;
+    const uint32_t tid = threadIdx.x, M = 1u << sb;
+    s_cnt[tid] = static_cast<uint32_t>(w->counts[tid]);        // n < 2^32, so every count and their sum fit
+    __syncthreads();
+    if (tid < 32) block_normalize(s_cnt, s_cum, s_w, w->freqs, M, kStatModel, status);
+    __syncthreads();
+    if (tid == 0) {
+        bool ok = container_model_ok(coder, sb, s_w) && container_model_decodable(coder, s_w);
+        uint32_t c = 0;
+        for (int s = 0; s < 256; s++) {
+            s_cum[s] = c;
+            c += s_w[s];
+        }
+        s_cum[256] = c;
+        bool paired = false;
+        if (ok && coder == RB200_CODER_ALIAS) {
+            paired = alias_tables_core(s_w, M / 256, s_divider, s_adjust, s_slot_freqs, s_sym_id, s_rest, s_given);
+            ok = paired;
+        }
+        s_paired = paired;
+        if (!ok) atomicOr(status, kStatModel);
+    }
+    __syncthreads();
+    const uint32_t f = s_w[tid], cum = s_cum[tid];
+    if (coder == RB200_CODER_WORD) {
+        int exact = 1;
+        w->word_enc[tid] = word_enc_entry(f, cum);
+        w->word_enc32[tid] = word_enc32_entry(f, cum, &exact);
+        const bool r32 = __syncthreads_and(exact) != 0;
+        if (tid == 0) w->r32 = r32 && r32_allowed;
+    } else if (coder == RB200_CODER_ALIAS) {
+        w->alias_enc[tid] = alias_enc_entry(f, cum);
+        if (s_paired) {
+            // alias_remap as rb200_alias_tables_build fills it: bucket b gives its own part to symbol b and the rest to
+            // its partner, each after what earlier buckets gave that symbol; one thread per code slot
+            const uint32_t bucket = M / 256;
+            for (uint32_t i = tid; i < M; i += kModelThreads) {
+                const uint32_t b = i / bucket, k = i - b * bucket, lo = b * bucket, own = s_divider[b] - lo;
+                const uint32_t dst = k < own ? s_cum[b] + (lo - s_adjust[2 * b + 1]) + k
+                                             : s_cum[s_sym_id[2 * b]] + (lo + own - s_adjust[2 * b]) + (k - own);
+                w->alias_remap[dst] = static_cast<uint16_t>(lo + k);
+            }
+        }
+    } else if (coder == RB200_CODER_BYTE) {
+        w->byte_enc[tid] = byte_enc_entry(f, cum, sb);
+    } else {
+        uint32_t e[8];
+        rans64_enc_entry(f, cum, sb, e);
+        w->r64_enc[2 * tid] = make_uint4(e[0], e[1], e[2], e[3]);
+        w->r64_enc[2 * tid + 1] = make_uint4(e[4], e[5], e[6], e[7]);
+    }
+}
+
+// The word encoders behind the gate: word_encode_kernel / word_encode_fused_kernel, run only when *gate (the model
+// kernel's r32) names this instance.  The host launches both instances of the call's path.
+template <bool R32>
+__global__ void __launch_bounds__(kEncWarps * 32, RB200_ENC_MINBLOCKS)
+word_encode_gated_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
+                         const WordEncEntry* __restrict__ g_table, const uint32_t* __restrict__ gate, uint8_t* __restrict__ scratch,
+                         uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
+{
+    if (*gate != (R32 ? 1u : 0u)) return;                          // the same for the whole grid
+    extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
+    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
+    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
+    __syncthreads();
+
+    const uint32_t warp = threadIdx.x >> 5;
+    const uint32_t chunk = blockIdx.x * kEncWarps + warp;
+    if (chunk >= n_chunks) return;
+    const ChunkRange r = chunk_range(chunk, chunk_syms, n);
+    encode_chunk_split(in + r.first, r.m, chunk, WordEncoder<R32>{smem_addr(s_enc)}, smem_addr(s_enc) + kEncTableBytes + warp * kEncWarpSmem,
+                       scratch, slot_bytes, sizes, status);
+}
+
+template <bool R32>
+__global__ void __launch_bounds__(kEncWarps * 32, RB200_FUSED_MINBLOCKS)
+word_encode_fused_gated_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
+                               const WordEncEntry* __restrict__ g_table, const uint32_t* __restrict__ gate, uint8_t* __restrict__ scratch,
+                               uint32_t slot_bytes, uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob,
+                               uint64_t blob_cap, uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
+{
+    if (*gate != (R32 ? 1u : 0u)) return;                          // the same for the whole grid
+    extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
+    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
+    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
+    __syncthreads();
+
+    const uint32_t tab = smem_addr(s_enc), wsm = tab + kEncTableBytes + (threadIdx.x >> 5) * kEncWarpSmem;
+    encode_chunks_fused<kFusedSlots, kEncWarps, RB200_ENC_KEEP_HINT>(in, n, chunk_syms, WordEncoder<R32>{tab}, wsm, scratch, slot_bytes,
+                                                                     PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
+}
+
+inline void configure_model_kernels()
+{
+    for (const void* k : {reinterpret_cast<const void*>(word_encode_gated_kernel<false>), reinterpret_cast<const void*>(word_encode_gated_kernel<true>),
+                          reinterpret_cast<const void*>(word_encode_fused_gated_kernel<false>),
+                          reinterpret_cast<const void*>(word_encode_fused_gated_kernel<true>)}) {
+        cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+    }
+}
+
+}  // namespace rb200

@@ -21,6 +21,7 @@
 #include "container_decode.cuh"
 #include "container_format.h"
 #include "crc_kernels.cuh"
+#include "model_kernels.cuh"
 #include "rans64_kernels.cuh"
 #include "tables.h"
 #include "word_kernels.cuh"
@@ -68,6 +69,8 @@ struct rb200_ctx {
     // rb200_container_decode_async: its fixed workspace (with the decode table) and its decoders' launches
     SingleAsyncWork* d_single_async = nullptr;
     SingleDecodeLaunch single_decoders[kSingleDecoders] = {};
+    // rb200_container_model_encode_async (model_kernels.cuh): the counts, the model and its encode tables
+    ModelAsyncWork* d_model_async = nullptr;
 };
 
 struct rb200_model {
@@ -136,6 +139,7 @@ inline uint32_t slot_bytes_for(uint32_t chunk_syms) { return static_cast<uint32_
 
 int status_to_code(uint32_t bits)
 {
+    if (bits & kStatModel) return RB200_E_MODEL;
     if (bits & kStatSymbol) return RB200_E_SYMBOL;
     if (bits & kStatSpace) return RB200_E_SPACE;
     if (bits & kStatStream) return RB200_E_STREAM;
@@ -229,6 +233,8 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_async, 0, sizeof(BlocksAsyncWork));
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_single_async, sizeof(SingleAsyncWork));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_single_async, 0, sizeof(SingleAsyncWork));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_model_async, sizeof(ModelAsyncWork));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_model_async, 0, sizeof(ModelAsyncWork));
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -242,6 +248,7 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     configure_crc_kernels();
     ctx->blocks_async = configure_container_decode(static_cast<uint32_t>(ctx->sms));
     configure_single_decode(static_cast<uint32_t>(ctx->sms), ctx->single_decoders);
+    configure_model_kernels();
     cudaGetLastError();
     *out = ctx;
     return RB200_OK;
@@ -264,6 +271,7 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->h_crc) cudaFreeHost(ctx->h_crc);
     if (ctx->d_blocks_async) cudaFree(ctx->d_blocks_async);
     if (ctx->d_single_async) cudaFree(ctx->d_single_async);
+    if (ctx->d_model_async) cudaFree(ctx->d_model_async);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -491,15 +499,15 @@ struct EncodePlan {
     uint32_t n_chunks;
 };
 
-EncodePlan plan_encode(const rb200_ctx* ctx, const rb200_model* model, uint32_t n_chunks, uint32_t chunk_syms)
+EncodePlan plan_encode(const rb200_ctx* ctx, int coder, uint32_t scale_bits, uint32_t n_chunks, uint32_t chunk_syms)
 {
     EncodePlan p = {};
     p.n_chunks = n_chunks;
     p.slot_bytes = slot_bytes_for(chunk_syms);
-    p.fused = n_chunks && model->coder != RB200_CODER_RANS64 && use_fused_encode(chunk_syms);
+    p.fused = n_chunks && coder != RB200_CODER_RANS64 && use_fused_encode(chunk_syms);
     p.slots = n_chunks;
     const uint32_t sms = static_cast<uint32_t>(ctx->sms);
-    if (model->coder == RB200_CODER_WORD) {
+    if (coder == RB200_CODER_WORD) {
         p.threads = kEncWarps * 32;
         p.smem = kEncSmemBytes;
         if (p.fused) {
@@ -509,13 +517,13 @@ EncodePlan plan_encode(const rb200_ctx* ctx, const rb200_model* model, uint32_t 
         } else {
             p.grid = (n_chunks + kEncWarps - 1) / kEncWarps;
         }
-    } else if (model->coder == RB200_CODER_RANS64) {
+    } else if (coder == RB200_CODER_RANS64) {
         p.threads = kRans64Warps * 32;
         p.smem = kRans64EncSmemBytes;
         p.grid = (n_chunks + kRans64Warps - 1) / kRans64Warps;
     } else {                           // alias / byte: persistent, at most one CTA per SM
         p.threads = kAliasEncWarps * 32;
-        p.smem = alias_encode_smem(model->coder == RB200_CODER_ALIAS, model->scale_bits);
+        p.smem = alias_encode_smem(coder == RB200_CODER_ALIAS, scale_bits);
         p.grid = std::min((n_chunks + (p.fused ? 1 : 0) + kAliasEncWarps - 1) / kAliasEncWarps, sms);
         if (p.fused) p.slots = static_cast<size_t>(sms) * kAliasEncWarps * kAliasFusedSlots;
     }
@@ -569,35 +577,72 @@ int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob
     return finish_encode(ctx, scratch, p.slot_bytes, head, tail, p.n_chunks, d_blob, blob_cap, d_offsets);
 }
 
-int encode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_in, size_t n, uint32_t chunk_syms,
-                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets)
+// The encode tables of one encode call, in device memory.  Word: `word_gate` null runs the instance word_r32 names on
+// word[word_r32]; set, both gated instances run (model_kernels.cuh), each on its own table, and *word_gate picks one.
+struct EncodeTables {
+    int coder;
+    uint32_t scale_bits;
+    const WordEncEntry* word[2];       // the 33-bit and the 32-bit reciprocal tables
+    int word_r32;
+    const uint32_t* word_gate;
+    const AliasEncEntry* enc;          // alias / byte
+    const uint16_t* remap;             // alias
+    const uint4* r64;                  // rans64
+};
+
+EncodeTables model_tables(const rb200_model* m)
+{
+    return EncodeTables{m->coder, m->scale_bits, {m->d_word_enc, m->d_word_enc}, m->enc_r32, nullptr,
+                        m->coder == RB200_CODER_ALIAS ? m->d_alias_enc : m->d_byte_enc, m->d_alias_remap, m->d_r64_enc};
+}
+
+int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, size_t n, uint32_t chunk_syms, uint8_t* d_blob,
+                  size_t blob_cap, uint64_t* d_offsets)
 {
     const size_t n_chunks_sz = rb200_chunk_count(n, chunk_syms);
     if (n_chunks_sz >= (1ull << 31)) return RB200_E_ARG;
     const uint32_t n_chunks = static_cast<uint32_t>(n_chunks_sz);
-    const EncodePlan p = plan_encode(ctx, model, n_chunks, chunk_syms);
+    const EncodePlan p = plan_encode(ctx, t.coder, t.scale_bits, n_chunks, chunk_syms);
     return run_encode(ctx, p, d_blob, blob_cap, d_offsets, [&](const EncodeWorkspace& ws) {
-        if (model->coder == RB200_CODER_WORD) {
+        if (t.coder == RB200_CODER_WORD) {
+            if (t.word_gate) {
+                int rc = RB200_OK;
+                for (int r32 = 0; r32 < 2 && rc == RB200_OK; r32++) {
+                    if (p.fused) {
+                        auto kernel = r32 ? word_encode_fused_gated_kernel<true> : word_encode_fused_gated_kernel<false>;
+                        kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], t.word_gate, ws.scratch,
+                                                                           p.slot_bytes, ws.look, ws.counter, d_blob, blob_cap, d_offsets,
+                                                                           ctx->d_status);
+                        rc = check_launch(ctx, "word_encode_fused_gated_kernel");
+                    } else {
+                        auto kernel = r32 ? word_encode_gated_kernel<true> : word_encode_gated_kernel<false>;
+                        kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], t.word_gate, ws.scratch,
+                                                                           p.slot_bytes, ws.sizes, ctx->d_status);
+                        rc = check_launch(ctx, "word_encode_gated_kernel");
+                    }
+                }
+                return rc;
+            }
+            const WordEncEntry* table = t.word[t.word_r32 ? 1 : 0];
             if (p.fused) {
-                auto kernel = model->enc_r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>;
-                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->d_word_enc, ws.scratch, p.slot_bytes,
+                auto kernel = t.word_r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>;
+                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.scratch, p.slot_bytes,
                                                                    ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status);
                 return check_launch(ctx, "word_encode_fused_kernel");
             }
-            auto kernel = model->enc_r32 ? word_encode_kernel<true> : word_encode_kernel<false>;
-            kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->d_word_enc, ws.scratch, p.slot_bytes,
+            auto kernel = t.word_r32 ? word_encode_kernel<true> : word_encode_kernel<false>;
+            kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.scratch, p.slot_bytes,
                                                                ws.sizes, ctx->d_status);
             return check_launch(ctx, "word_encode_kernel");
         }
-        if (model->coder == RB200_CODER_RANS64) {
-            rans64_encode_kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, model->scale_bits, model->d_r64_enc,
+        if (t.coder == RB200_CODER_RANS64) {
+            rans64_encode_kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.scale_bits, t.r64,
                                                                              ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status);
             return check_launch(ctx, "rans64_encode_kernel");
         }
-        const bool alias = model->coder == RB200_CODER_ALIAS;
-        launch_alias_encode(ctx->stream, p.grid, p.smem, d_in, n, chunk_syms, n_chunks, model->scale_bits, alias ? model->d_alias_enc : model->d_byte_enc,
-                            alias ? model->d_alias_remap : nullptr, ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob,
-                            blob_cap, d_offsets, ctx->d_status);
+        const bool alias = t.coder == RB200_CODER_ALIAS;
+        launch_alias_encode(ctx->stream, p.grid, p.smem, d_in, n, chunk_syms, n_chunks, t.scale_bits, t.enc, alias ? t.remap : nullptr,
+                            ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status);
         return check_launch(ctx, alias ? "alias_encode_kernel" : "byte_encode_kernel");
     });
 }
@@ -921,9 +966,9 @@ int encode_host(rb200_ctx* ctx, const rb200_model* model, const uint8_t* in, siz
 {
     return encode_pipeline(
         ctx, in, n, chunk_syms, 1, UnitTable{},
-        [&](const Slice& s) { return plan_encode(ctx, model, static_cast<uint32_t>(s.cnt), chunk_syms); },
+        [&](const Slice& s) { return plan_encode(ctx, model->coder, model->scale_bits, static_cast<uint32_t>(s.cnt), chunk_syms); },
         [&](const Slice& s, const uint8_t* d_in, uint8_t*, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
-            return encode_device(ctx, model, d_in, s.len, chunk_syms, d_blob, cap, d_off);
+            return encode_device(ctx, model_tables(model), d_in, s.len, chunk_syms, d_blob, cap, d_off);
         },
         blob, blob_cap, offsets, blob_size, hook);
 }
@@ -948,7 +993,7 @@ extern "C" int rb200_encode(rb200_ctx* ctx, const rb200_model* model, const uint
     if (!ctx || !model || model->ctx != ctx || !blob || !offsets || (!in && n) || !chunk_ok(chunk_syms)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
     return by_mem_kind(
-        mem_kind, blob, offsets, [&] { return encode_device(ctx, model, in, n, chunk_syms, blob, blob_cap, offsets); },
+        mem_kind, blob, offsets, [&] { return encode_device(ctx, model_tables(model), in, n, chunk_syms, blob, blob_cap, offsets); },
         [&] { return encode_host(ctx, model, in, n, chunk_syms, blob, blob_cap, offsets, blob_size); });
 }
 
@@ -1349,7 +1394,7 @@ extern "C" int rb200_container_encode(rb200_ctx* ctx, const rb200_model* model, 
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
     uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
     if (device) {            // asynchronous: directory CRC, blob CRC, then the header from blob_bytes = dir[n_chunks]
-        int rc = encode_device(ctx, model, in, n, chunk_syms, out + boff, out_cap - boff, dir);
+        int rc = encode_device(ctx, model_tables(model), in, n, chunk_syms, out + boff, out_cap - boff, dir);
         if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
         if (rc != RB200_OK) return rc;
@@ -1502,6 +1547,44 @@ extern "C" int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, 
         rc = check_launch(ctx, l.name);
     }
     return rc;
+}
+
+// rb200_model_from_data + rb200_container_encode (device memory) + rb200_model_destroy with kernels alone
+// (model_kernels.cuh): histogram, model kernel, the coder's encoder, the CRCs and the header.  Five to seven launches and
+// one memset, no copy, no synchronisation; the encode workspace grows as in rb200_container_encode.
+extern "C" int rb200_container_model_encode_async(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, size_t n,
+                                                  uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    if (!ctx || !in || !out || !container_mem_ok(RB200_MEM_DEVICE, out, nullptr)) return RB200_E_ARG;
+    if (coder < RB200_CODER_WORD || coder > RB200_CODER_RANS64 || scale_bits < 8 || scale_bits > 16) return RB200_E_ARG;
+    if (coder == RB200_CODER_WORD && scale_bits != kWordScaleBits) return RB200_E_ARG;
+    if (!chunk_ok(chunk_syms) || (n >> 32)) return RB200_E_ARG;      // counts of 32 bits, as rb200_model_from_data
+    const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
+    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    if (n == 0) return RB200_E_MODEL;                                // normalize_freqs divides by the total
+    ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n, n_chunks, 0, flags);
+    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
+    if (out_cap < boff) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    ModelAsyncWork* w = ctx->d_model_async;
+    RB_CUDA(ctx, cudaMemsetAsync(w->counts, 0, sizeof w->counts, ctx->stream));
+    launch_histogram(ctx->stream, static_cast<uint32_t>(ctx->sms), in, n, w->counts);
+    int rc = check_launch(ctx, "histogram_kernel");
+    if (rc != RB200_OK) return rc;
+    container_model_kernel<<<1, kModelThreads, 0, ctx->stream>>>(static_cast<uint32_t>(coder), scale_bits, word_r32_allowed() ? 1u : 0u, w,
+                                                                 ctx->d_status);
+    rc = check_launch(ctx, "container_model_kernel");
+    if (rc != RB200_OK) return rc;
+    const EncodeTables t = {coder, scale_bits, {w->word_enc, w->word_enc32}, 0, &w->r32,
+                            coder == RB200_CODER_ALIAS ? w->alias_enc : w->byte_enc, w->alias_remap, w->r64_enc};
+    const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
+    rc = encode_device(ctx, t, in, n, chunk_syms, out + boff, out_cap - boff, dir);
+    if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, nullptr, 0, ctx->d_crc);
+    if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+    if (rc != RB200_OK) return rc;
+    container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, w->freqs, ctx->d_crc, ctx->d_status);
+    return check_launch(ctx, "container_finish_kernel");
 }
 
 // ---------------------------------------------------------------------------

@@ -17,6 +17,18 @@ RB200_HD inline uint32_t word_dec_entry(uint32_t s, uint32_t f, uint32_t k) { re
 // byte: symbol s's RansDecSymbol {start, freq} (freq < 65536)
 RB200_HD inline uint32_t byte_dec_symbol(uint32_t start, uint32_t f) { return start | (f << 16); }
 
+// The per-entry formulas of the encode tables below, shared the same way by the host builders and the device model
+// build of rb200_container_model_encode_async (model_kernels.cuh).  f <= 65536 and cum <= 65536 throughout.
+RB200_HD inline uint32_t ceil_log2(uint32_t v)
+{
+    uint32_t s = 0;
+    while ((1u << s) < v) s++;
+    return s;
+}
+// ceil(2^(32 + sh) / f), sh = ceil_log2(f): the round-up reciprocal of the word and alias encoders, in [2^32, 2^33)
+// (2^(32 + sh) <= 2^48, so 64 bits hold it exactly)
+RB200_HD inline uint64_t rcp33(uint32_t f, uint32_t sh) { return ((1ull << (32 + sh)) + f - 1) / f; }
+
 // ---- word coder (rans_word_sse41.h semantics, scale_bits 12)
 //
 // decode: one u32 per slot, 16 KiB: (freq & 0xfff) << 20 | bias << 8 | symbol.
@@ -33,6 +45,28 @@ RB200_HD inline uint32_t byte_dec_symbol(uint32_t start, uint32_t f) { return st
 //   fewer per symbol.  freq 1 uses M32 = 2^32 - 1, which yields x - 1; the kernel adds the missing
 //   1 * (4096 - 1) to `start`.  `enc32_ok` says every symbol of the model passed the check.
 struct WordEncEntry { uint32_t magic, packed; };
+
+// symbol s of frequency f starting at cum: its `enc` entry (33-bit reciprocal: exact for any 32-bit x)
+RB200_HD inline WordEncEntry word_enc_entry(uint32_t f, uint32_t cum)
+{
+    if (f == 0) return {0u, kEncBadSymbol};
+    const uint32_t sh = ceil_log2(f);
+    return {static_cast<uint32_t>(rcp33(f, sh)), f | (cum << 13) | (sh << 25)};     // magic = M - 2^32
+}
+// its `enc32` entry (32-bit reciprocal, exact on x < f << 20); clears *exact when the check fails for f
+RB200_HD inline WordEncEntry word_enc32_entry(uint32_t f, uint32_t cum, int* exact)
+{
+    if (f == 0) return {0u, kEncBadSymbol};
+    if (f == 1) return {0xffffffffu, f | (cum << 13)};
+    const uint32_t s32 = ceil_log2(f) - 1;
+    const uint64_t pow = 1ull << (32 + s32);
+    const uint64_t M32 = (pow + f - 1) / f;                    // < 2^32 because 2^s32 < f
+    const uint64_t err = M32 * f - pow;                        // < f
+    const uint64_t xmax = (static_cast<uint64_t>(f) << 20) - 1;
+    if (M32 >> 32 || xmax * err >= pow) *exact = 0;
+    return {static_cast<uint32_t>(M32), f | (cum << 13) | (s32 << 25)};
+}
+
 struct WordDeviceTables {
     uint32_t dec[4096];
     WordEncEntry enc[256];
@@ -56,6 +90,14 @@ int build_word_device_tables(const uint32_t freqs[256], WordDeviceTables& t);
 //   alias_remap as u16 (values < 65536; SURVEY H8) = 128 KiB at scale_bits 16.
 struct AliasDecEntry { uint32_t divider, alt0, alt1, adjust; };
 struct AliasEncEntry { uint32_t magic, freq, cum, shift; };
+
+// alias: symbol s's encode entry (the word coder's round-up reciprocal: exact for every 32-bit x)
+RB200_HD inline AliasEncEntry alias_enc_entry(uint32_t f, uint32_t cum)
+{
+    if (f == 0) return {0u, 0u, 0u, kEncBadSymbol};
+    const uint32_t sh = ceil_log2(f);
+    return {static_cast<uint32_t>(rcp33(f, sh)), f, cum, sh};
+}
 
 // bucket b's decode entry from the arrays of alias_tables_core
 RB200_HD inline AliasDecEntry alias_dec_entry(uint32_t b, const uint32_t* divider, const uint32_t* slot_adjust, const uint32_t* slot_freqs,
@@ -137,6 +179,18 @@ struct ByteDeviceTables {
 };
 int build_byte_device_tables(const uint32_t freqs[256], uint32_t scale_bits, ByteDeviceTables& t);
 
+// symbol s's RansEncSymbol image (RansEncSymbolInit, rans_byte.h:174-243)
+RB200_HD inline AliasEncEntry byte_enc_entry(uint32_t f, uint32_t cum, uint32_t scale_bits)
+{
+    const uint32_t M = 1u << scale_bits;
+    const uint32_t x_max = ((1u << 23 >> scale_bits) << 8) * (f ? f : 1);      // rans_byte.h:197
+    if (f == 0) return {x_max, 0xffffffffu, M - 1, ((M - 1) & 0xffffu) | kEncBadSymbol};   // never valid to encode (:260): freq 1, flagged
+    if (f == 1) return {x_max, 0xffffffffu, cum + M - 1, (M - 1) & 0xffffu};              // :199-228
+    const uint32_t sh = ceil_log2(f);                                                      // :229-242
+    const uint32_t rcp = static_cast<uint32_t>(((1ull << (sh + 31)) + f - 1) / f);
+    return {x_max, rcp, cum, ((M - f) & 0xffffu) | ((sh - 1) << 16)};
+}
+
 // ---- rans64 (main64.cpp semantics over rans64.h), scale_bits 8..16
 //
 // decode: cum2sym[1 << scale_bits] followed by 256 x {u32 start, u32 freq} (= Rans64DecSymbol, rans64.h:151-154)
@@ -148,5 +202,42 @@ struct Rans64DeviceTables {
     uint32_t enc[256][8];
 };
 int build_rans64_device_tables(const uint32_t freqs[256], uint32_t scale_bits, Rans64DeviceTables& t);
+
+// ceil(2^(k + 63) / f) for 2 <= f <= 2^16, k = ceil_log2(f): in [2^63, 2^64).  Long division in base 2^32 of
+// 2^(k - 1) * 2^64 (the top digit is below f), so that 64-bit arithmetic gives the exact quotient.
+RB200_HD inline uint64_t rcp64(uint32_t f, uint32_t k)
+{
+    const uint64_t t1 = (1ull << (k - 1)) << 32;              // < f * 2^32
+    const uint64_t q1 = t1 / f, t0 = (t1 % f) << 32;
+    const uint64_t q0 = t0 / f;
+    return ((q1 << 32) | q0) + (t0 % f != 0);
+}
+// symbol s's Rans64EncSymbol image, 8 words (Rans64EncSymbolInit, rans64.h:167-247)
+RB200_HD inline void rans64_enc_entry(uint32_t f, uint32_t cum, uint32_t scale_bits, uint32_t e[8])
+{
+    const uint32_t M = 1u << scale_bits;
+    uint64_t rcp;
+    uint32_t shift, bias, flag = 0;
+    if (f < 2) {                                                // rans64.h:199-228 (freq 0: same, flagged)
+        rcp = ~0ull;
+        shift = 0;
+        bias = (f ? cum : 0) + M - 1;
+        if (f == 0) flag = kEncBadSymbol;
+    } else {                                                    // rans64.h:229-246
+        const uint32_t k = ceil_log2(f);
+        rcp = rcp64(f, k);
+        shift = k - 1;
+        bias = cum;
+    }
+    const uint32_t fe = f ? f : 1;
+    e[0] = static_cast<uint32_t>(rcp);
+    e[1] = static_cast<uint32_t>(rcp >> 32);
+    e[2] = fe;
+    e[3] = bias;
+    e[4] = M - fe;
+    e[5] = shift | flag;
+    e[6] = 0;
+    e[7] = 0;
+}
 
 }  // namespace rb200

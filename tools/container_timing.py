@@ -23,9 +23,17 @@ the headline one (uniform, word), Zipf 1.1 with the alias coder at scale_bits 16
   list of the kernels of rb200_decode and of the async call (median device time per kernel), which shows the planned
   decoder against the shipped one and the launches the verdict gated out.
 
+With --model, the single-model container's encode on the same three workloads, each with flags 0 and
+RB200_CONTAINER_CRC_BLOB, alternated:
+
+  rb200_container_encode with a prebuilt model; rb200_model_from_data + rb200_container_encode + rb200_model_destroy
+  (what a caller without a model does); rb200_container_model_encode_async (the model built on the GPU); the host time
+  each call takes to return; and a torch.profiler list of the async call's kernels (histogram, model kernel, encoder,
+  the gated-out word encoder instance, CRCs, header).
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
-    python tools/container_timing.py [--blocks | --single] [--reps 10] [--json out.json]"""
+    python tools/container_timing.py [--blocks | --single | --model] [--reps 10] [--json out.json]"""
 import argparse
 import json
 import os
@@ -356,17 +364,75 @@ def single(args):
     return res
 
 
+def model_encode(args):
+    import torch
+    n, chunk = 1 << 30, 8192
+    g = torch.Generator(device="cuda")
+    g.manual_seed(1234)
+    workloads = (("uniform word", rb.CODER_WORD, 12, lambda: torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda", generator=g)),
+                 ("Zipf 1.1 alias 16", rb.CODER_ALIAS, 16, lambda: zipf_data(n, 1235)),
+                 ("uniform rans64 14", rb.CODER_RANS64, 14, lambda: torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda", generator=g)))
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    crc = api.CONTAINER_CRC_BLOB
+    cap = ctx.container_capacity(n, chunk)
+    d_ref = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_out = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    res = {"card": card(), "workloads": {}, "checks": {}}
+    for name, coder, sb, make in workloads:
+        d_in = make()
+        i, r, o = d_in.data_ptr(), d_ref.data_ptr(), d_out.data_ptr()
+        model = rb.Model.from_data(ctx, coder, sb, device_ptr=i, n=n)
+
+        def from_data(flags):
+            m = rb.Model.from_data(ctx, coder, sb, device_ptr=i, n=n)
+            ctx.container_encode_device(m, i, n, chunk, flags, r, cap)
+            m.close()
+
+        calls = {}
+        for tag, flags in (("", 0), ("_crc", crc)):
+            calls["encode_prebuilt" + tag] = lambda flags=flags: ctx.container_encode_device(model, i, n, chunk, flags, r, cap)
+            calls["from_data_encode" + tag] = lambda flags=flags: from_data(flags)
+            calls["model_encode_async" + tag] = lambda flags=flags: ctx.container_model_encode_async(coder, sb, i, n, chunk, flags, o, cap)
+        times = alternate(calls, sync, args.warmup, args.reps)
+        host = {k: [] for k in calls if not k.startswith("encode_prebuilt")}
+        for _ in range(args.reps):
+            for k in host:
+                t0 = time.perf_counter()
+                calls[k]()
+                host[k].append((time.perf_counter() - t0) * 1e3)
+                sync()
+        for tag in ("", "_crc"):
+            calls["encode_prebuilt" + tag]()
+            calls["model_encode_async" + tag]()
+            sync()
+            head = d_out[:64].cpu().numpy()
+            size = int(ctx.lib.dll.rb200_container_size(int(head[24:32].view(np.uint64)[0]), int(head[32:40].view(np.uint64)[0])))
+            res["checks"][f"{name}: model_encode_async{tag}_equals_prebuilt"] = bool(torch.equal(d_out[:size], d_ref[:size]))
+        res["workloads"][name] = {
+            "n": n, "chunk_syms": chunk,
+            "encode": times,
+            "call_host_ms": {k: stats(v) for k, v in host.items()},
+            "kernels": {k: kernel_times(calls[k], sync, args.reps) for k in ("model_encode_async", "model_encode_async_crc")},
+        }
+        model.close()
+        del d_in
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
     ap.add_argument("--single", action="store_true", help="the single-model container's decode calls on three workloads")
+    ap.add_argument("--model", action="store_true", help="the single-model container's encode with the model built from the data")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else single(args) if args.single else headline(args)
+    res = blocks(args) if args.blocks else single(args) if args.single else model_encode(args) if args.model else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:

@@ -137,6 +137,27 @@ def main():
                 pass
             if flags:
                 assert not d_out.any().item()
+    # the single-model container with its model built on the GPU: every coder, valid; then a model the library
+    # refuses (byte coder at scale_bits 16 on one symbol) and an argument error, which launches nothing
+    ccap = ctx.container_capacity(data.size, 4096)
+    d_c = torch.zeros(ccap + 16, dtype=torch.uint8, device="cuda")
+    for coder, sb in ((rb.CODER_WORD, 12), (rb.CODER_ALIAS, 16), (rb.CODER_BYTE, 14), (rb.CODER_RANS64, 12)):
+        ctx.container_model_encode_async(coder, sb, d_in.data_ptr(), data.size, 4096, api.CONTAINER_CRC_BLOB, d_c.data_ptr(), ccap)
+        d_out.zero_()
+        ctx.container_decode_async(d_c.data_ptr(), ccap, d_out.data_ptr(), data.size, d_n.data_ptr())
+        ctx.sync()
+        assert torch.equal(d_out[:data.size], d_in), coder
+    d_one = torch.full((data.size,), 0x41, dtype=torch.uint8, device="cuda")
+    ctx.container_model_encode_async(rb.CODER_BYTE, 16, d_one.data_ptr(), data.size, 4096, 0, d_c.data_ptr(), ccap)
+    try:
+        ctx.sync()
+        raise SystemExit("refused model not reported")
+    except rb.RansError as e:
+        assert e.code == -2, e
+    before = ctx.launches
+    assert ctx.lib.dll.rb200_container_model_encode_async(ctx.h, rb.CODER_WORD, 14, d_in.data_ptr(), data.size, 4096, 0,
+                                                          d_c.data_ptr(), ccap) == -1
+    assert ctx.launches == before
     print("sanitize smoke ok:", ctx.launches, "launches")
 
 

@@ -43,6 +43,7 @@ def main():
     fns = functions(subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout)
     dec = next(v for k, v in fns.items() if "block_decode_kernel" in k)
     enc = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1" in k)
+    enc_gated = next(v for k, v in fns.items() if "word_encode_fused_gated_kernelILb1" in k)
     tma = next(v for k, v in fns.items() if "word_decode_tma_kernel" in k and k.endswith("Lb0EEEvPKhmPKmPKjPhmjjPNS_10DecodeWorkEPjy"))
     ali = next(v for k, v in fns.items() if "alias_decode_persist_kernelILj16E" in k)
     tma_planned = next(v for k, v in fns.items() if "word_decode_planned_kernelILb0E" in k)
@@ -57,7 +58,9 @@ def main():
                          step_between(ali_planned, "STG.E.U8", 2)),
                         ("block_decode_kernel (round 1 window: decode_window_chunk with WordDecoder<false>): one step (vote to vote)",
                          step_between(dec, "VOTE.ANY", 5)),
-                        ("word_encode_fused_kernel<R32>: one step (symbol load to symbol load)", step_between(enc, "LDS.U8", 8))):
+                        ("word_encode_fused_kernel<R32>: one step (symbol load to symbol load)", step_between(enc, "LDS.U8", 8)),
+                        ("word_encode_fused_gated_kernel<R32> (rb200_container_model_encode_async): one step (symbol load to symbol load)",
+                         step_between(enc_gated, "LDS.U8", 8))):
         print("## %s: %d instructions" % (title, len(step)))
         print("```")
         for addr, ins in step:
