@@ -173,6 +173,30 @@ __device__ __forceinline__ void fused_place(const PlaceOut& out, uint32_t chunk,
     }
 }
 
+// one warp: wait for the scanner to publish E_c of `chunk`, with fused_place's back-off; returns kLookPrefix | E_c, or 0
+// once the wait has expired (kStatStall is then set).  fused_place keeps its own copy of the loop: calling this from
+// it changes the code ptxas makes for every fused encoder.
+__device__ __forceinline__ uint64_t wait_end_offset(const PlaceOut& out, uint32_t chunk, uint32_t lane)
+{
+    uint64_t v = 0, since = 0;
+    uint32_t ns = 128;
+    for (;;) {
+        if (lane == 0) v = ld_relaxed_u64(out.look + chunk);
+        v = __shfl_sync(0xffffffffu, v, 0);
+        if ((v >> 62) == 2) return v;
+        if (ns >= 4096) {
+            const uint64_t now = global_timer_ns();
+            if (!since) since = now;
+            if (now - since > kLookStallNs) {
+                if (lane == 0) atomicOr(out.status, kStatStall);
+                return 0;
+            }
+        }
+        __nanosleep(ns);
+        if (ns < 4096) ns <<= 1;
+    }
+}
+
 // One worker warp's SLOTS scratch slots, at scratch + worker * SLOTS * slot_bytes (the host sizes the scratch as
 // workers x SLOTS slots).  A chunk is encoded into the slot that ends at next_end(), published by finish() and placed
 // SLOTS - 1 chunks later; drain() places what is left once the warp runs out of chunks.

@@ -467,39 +467,59 @@ int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* siz
     return check_launch(ctx, "compact_kernel");
 }
 
-// Word-coder encode has two paths:
+// Word-coder encode has three paths:
 //   fused: ONE persistent launch -- workers encode, a scanner warp turns published sizes into end offsets
 //          in chunk order, workers place chunk k after encoding chunk k+1 (placement.cuh);
+//   ring:  the fused launch with every stream kept in its warp's shared-memory ring until it is placed with TMA bulk
+//          copies (K2r, encode_ring.cuh): no scratch; for chunks of <= kEncRingMaxChunk symbols, whose worst-case
+//          stream fits a ring, and models the host knows satisfy word_ring_model (so not for
+//          rb200_container_model_encode_async, whose model is built on the GPU);
 //   split: three launches -- encode into per-chunk worst-case slots, tile scan, compaction.
 // fused is faster as long as the scanner keeps up, i.e. for chunks of >= 4096 symbols; below that the split path
 // is used (H100 SXM at a 400 W power limit, 1 GiB uniform bytes: 1.89 vs 2.21 ms per call at chunks of 8192, 2.10 vs
-// 2.25 ms at 4096, but 2.80 vs 2.36 ms at 2048).  RB200_ENCODE_PATH=split|fused forces one.
-// Only the encode plans (plan_encode, plan_blocks_encode) ask.
-bool use_fused_encode(uint32_t chunk_syms)
+// 2.25 ms at 4096, but 2.80 vs 2.36 ms at 2048).  Where both fit, ring replaces fused (DESIGN.md section 4).
+// RB200_ENCODE_PATH=split|fused forces one of those two.  Only the encode plans (plan_encode, plan_blocks_encode) ask.
+int forced_encode_path()                     // RB200_ENCODE_PATH: 1 fused, 0 split, -1 not set
 {
     static const int forced = [] {           // read once; thread-safe static initialisation
         const char* e = std::getenv("RB200_ENCODE_PATH");
         return !e ? -1 : (std::strcmp(e, "fused") == 0 ? 1 : (std::strcmp(e, "split") == 0 ? 0 : -1));
     }();
+    return forced;
+}
+
+bool use_fused_encode(uint32_t chunk_syms)
+{
     // two worst-case slots per resident warp: keep that scratch below ~2 GB (chunks of <= 64 Ki symbols)
     if (chunk_syms > 65536) return false;
-    if (forced >= 0) return forced == 1;
+    if (forced_encode_path() >= 0) return forced_encode_path() == 1;
     return chunk_syms >= 4096;
 }
 
 // How one encode call over n_chunks chunks runs, decided once: the path, the encode launch's shape, and the workspace
-// both need.  Fused: one launch of `grid` CTAs with `slots` scratch slots (slots per worker warp x the warps of the grid);
+// both need.  Fused: one launch of `grid` CTAs with `slots` scratch slots (slots per worker warp x the warps of the grid; none for ring);
 // in ctx->sizes the chunk counter (16 bytes), then look[n_chunks] (placement.cuh).  Split: the encode launch into one
 // slot per chunk, then finish_encode; in ctx->sizes sizes[n_chunks], then the scan's tile sums.
 struct EncodePlan {
     bool fused;
+    bool ring;                         // word coder, fused: K2r instead of K2f (no scratch slots)
     uint32_t grid, threads, smem;      // the encode launch (dynamic shared memory in bytes)
     size_t slots;
     uint32_t slot_bytes;
     uint32_t n_chunks;
 };
 
-EncodePlan plan_encode(const rb200_ctx* ctx, int coder, uint32_t scale_bits, uint32_t n_chunks, uint32_t chunk_syms)
+// A word model whose streams fit K2r's ring: no symbol holds all 4096 slots.  Such a symbol's x_max wraps to 0
+// (word_enc_expand), so every step emits a word: 2 * chunk_syms + 128 bytes per chunk, more than kWordStreamMax.
+bool word_ring_model(const uint32_t freqs[256])
+{
+    for (int s = 0; s < 256; s++)
+        if (freqs[s] >= kWordSlots) return false;
+    return true;
+}
+
+// ring_model: the word model is known to satisfy word_ring_model (a model built on the GPU is not known to)
+EncodePlan plan_encode(const rb200_ctx* ctx, int coder, uint32_t scale_bits, uint32_t n_chunks, uint32_t chunk_syms, bool ring_model)
 {
     EncodePlan p = {};
     p.n_chunks = n_chunks;
@@ -510,7 +530,13 @@ EncodePlan plan_encode(const rb200_ctx* ctx, int coder, uint32_t scale_bits, uin
     if (coder == RB200_CODER_WORD) {
         p.threads = kEncWarps * 32;
         p.smem = kEncSmemBytes;
-        if (p.fused) {
+        p.ring = p.fused && ring_model && forced_encode_path() < 0 && chunk_syms <= kEncRingMaxChunk;
+        if (p.ring) {
+            p.threads = kEncRingWarps * 32;
+            p.smem = kEncRingSmemBytes;
+            p.grid = std::min((n_chunks + 1 + kEncRingWarps - 1) / kEncRingWarps, sms);
+            p.slots = 0;
+        } else if (p.fused) {
             const uint32_t want = (n_chunks + 1 + kEncWarps - 1) / kEncWarps;     // + 1: one warp of the grid is the scanner
             p.grid = std::min(want, sms * RB200_FUSED_MINBLOCKS);
             p.slots = static_cast<size_t>(p.grid) * kEncWarps * kFusedSlots;
@@ -588,12 +614,14 @@ struct EncodeTables {
     const AliasEncEntry* enc;          // alias / byte
     const uint16_t* remap;             // alias
     const uint4* r64;                  // rans64
+    bool word_ring = false;            // word: the model satisfies word_ring_model
 };
 
 EncodeTables model_tables(const rb200_model* m)
 {
     return EncodeTables{m->coder, m->scale_bits, {m->d_word_enc, m->d_word_enc}, m->enc_r32, nullptr,
-                        m->coder == RB200_CODER_ALIAS ? m->d_alias_enc : m->d_byte_enc, m->d_alias_remap, m->d_r64_enc};
+                        m->coder == RB200_CODER_ALIAS ? m->d_alias_enc : m->d_byte_enc, m->d_alias_remap, m->d_r64_enc,
+                        word_ring_model(m->freqs)};
 }
 
 int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, size_t n, uint32_t chunk_syms, uint8_t* d_blob,
@@ -602,7 +630,7 @@ int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, si
     const size_t n_chunks_sz = rb200_chunk_count(n, chunk_syms);
     if (n_chunks_sz >= (1ull << 31)) return RB200_E_ARG;
     const uint32_t n_chunks = static_cast<uint32_t>(n_chunks_sz);
-    const EncodePlan p = plan_encode(ctx, t.coder, t.scale_bits, n_chunks, chunk_syms);
+    const EncodePlan p = plan_encode(ctx, t.coder, t.scale_bits, n_chunks, chunk_syms, t.word_ring);
     return run_encode(ctx, p, d_blob, blob_cap, d_offsets, [&](const EncodeWorkspace& ws) {
         if (t.coder == RB200_CODER_WORD) {
             if (t.word_gate) {
@@ -624,6 +652,12 @@ int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, si
                 return rc;
             }
             const WordEncEntry* table = t.word[t.word_r32 ? 1 : 0];
+            if (p.ring) {
+                auto kernel = t.word_r32 ? word_encode_ring_kernel<true> : word_encode_ring_kernel<false>;
+                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.look, ws.counter, d_blob,
+                                                                   blob_cap, d_offsets, ctx->d_status);
+                return check_launch(ctx, "word_encode_ring_kernel");
+            }
             if (p.fused) {
                 auto kernel = t.word_r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>;
                 kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.scratch, p.slot_bytes,
@@ -966,7 +1000,9 @@ int encode_host(rb200_ctx* ctx, const rb200_model* model, const uint8_t* in, siz
 {
     return encode_pipeline(
         ctx, in, n, chunk_syms, 1, UnitTable{},
-        [&](const Slice& s) { return plan_encode(ctx, model->coder, model->scale_bits, static_cast<uint32_t>(s.cnt), chunk_syms); },
+        [&](const Slice& s) {
+            return plan_encode(ctx, model->coder, model->scale_bits, static_cast<uint32_t>(s.cnt), chunk_syms, word_ring_model(model->freqs));
+        },
         [&](const Slice& s, const uint8_t* d_in, uint8_t*, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
             return encode_device(ctx, model_tables(model), d_in, s.len, chunk_syms, d_blob, cap, d_off);
         },

@@ -10,6 +10,7 @@
 //                                                     exact division by reciprocal multiply
 #pragma once
 #include "device_utils.cuh"
+#include "encode_ring.cuh"
 #include "encode_stream.cuh"
 #include "placement.cuh"
 #include "tables.h"
@@ -187,6 +188,249 @@ word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t ch
 }
 
 // ---------------------------------------------------------------------------
+// K2r: the fused word encoder with its streams in shared memory (the chunk loop and placement: encode_ring.cuh).
+// Every warp encodes into its own shared-memory stream ring of RING bytes; a finished stream stays there until its end
+// offset is published and is then stored to the blob with TMA bulk copies, so no stream goes through global scratch.
+// The step loads its symbol 2 D steps and its table entry D steps ahead, so only the state arithmetic is on the chain.
+// ---------------------------------------------------------------------------
+constexpr uint32_t kWordStreamMax = 12480;   // worst-case stream of a chunk of 8192 symbols (DESIGN.md section 8)
+
+// shared address of ring position pos, pos in [-RING, RING) (as uint32_t)
+template <uint32_t RING>
+__device__ __forceinline__ uint32_t ring_addr(uint32_t ring, uint32_t pos)
+{
+    if constexpr ((RING & (RING - 1)) == 0) return ring + (pos & (RING - 1));
+    else return ring + min(pos, pos + RING);
+}
+
+// x = ((x / freq) << 12) + x % freq + start for a renormalised x (RansWordEncPut, rans_word_sse41.h:92), e = word_enc_expand
+template <bool R32>
+__device__ __forceinline__ uint32_t word_enc_fold(uint32_t x, const uint4 e)
+{
+    uint32_t q;
+    if (R32) {
+        q = funnel_shr_wrap(__umulhi(x, e.x), 0u, e.y);
+    } else {
+        const uint32_t hi = __umulhi(x, e.x);
+        const uint32_t lo = x + hi;
+        q = funnel_shr_wrap(lo, lo < hi ? 1u : 0u, e.y);
+    }
+    return x + e.z + q * e.w;
+}
+
+// one full-warp step on a prefetched table entry: WordEncoder::step's renormalisation, with the word stored at ring
+// position wpos - 2 * popc(mask & gt) modulo RING (wpos in [-RING, RING) on entry)
+template <bool R32, uint32_t RING>
+__device__ __forceinline__ void word_ring_step(uint32_t& x, uint32_t& wpos, uint32_t& flags, const uint4 e, uint32_t ring, uint32_t gt)
+{
+    flags |= e.w;
+    if constexpr ((RING & (RING - 1)) == 0) {
+        asm volatile(
+            "{\n\t"
+            ".reg .pred p;\n\t"
+            ".reg .b32 m, r, a;\n\t"
+            "setp.ge.u32 p, %2, %3;\n\t"
+            "vote.sync.ballot.b32 m, p, 0xffffffff;\n\t"
+            "and.b32 r, m, %4;\n\t"
+            "popc.b32 r, r;\n\t"
+            "shl.b32 r, r, 1;\n\t"
+            "sub.u32 a, %1, r;\n\t"
+            "and.b32 a, a, %5;\n\t"
+            "add.u32 a, a, %6;\n\t"
+            "@p st.shared.u16 [a], %0;\n\t"
+            "@p shr.u32 %0, %0, 16;\n\t"
+            "popc.b32 m, m;\n\t"
+            "shl.b32 m, m, 1;\n\t"
+            "sub.u32 %1, %1, m;\n\t"
+            "}"
+            : "+r"(x), "+r"(wpos)
+            : "r"(x | 31u), "r"(e.y), "r"(gt), "n"(RING - 1), "r"(ring)
+            : "memory");
+    } else {
+        asm volatile(
+            "{\n\t"
+            ".reg .pred p;\n\t"
+            ".reg .b32 m, r, a, b;\n\t"
+            "setp.ge.u32 p, %2, %3;\n\t"
+            "vote.sync.ballot.b32 m, p, 0xffffffff;\n\t"
+            "and.b32 r, m, %4;\n\t"
+            "popc.b32 r, r;\n\t"
+            "shl.b32 r, r, 1;\n\t"
+            "sub.u32 a, %1, r;\n\t"
+            "add.u32 b, a, %5;\n\t"
+            "min.u32 a, a, b;\n\t"
+            "add.u32 a, a, %6;\n\t"
+            "@p st.shared.u16 [a], %0;\n\t"
+            "@p shr.u32 %0, %0, 16;\n\t"
+            "popc.b32 m, m;\n\t"
+            "shl.b32 m, m, 1;\n\t"
+            "sub.u32 %1, %1, m;\n\t"
+            "}"
+            : "+r"(x), "+r"(wpos)
+            : "r"(x | 31u), "r"(e.y), "r"(gt), "n"(RING), "r"(ring)
+            : "memory");
+    }
+    x = word_enc_fold<R32>(x, e);
+}
+
+// Encode m symbols (one warp) as one 32-way stream that ends at ring position `top` (16-byte aligned) and grows
+// downwards, modulo RING; the bytes of encode_stream's stream, preceded by zeros up to a 16-byte boundary.  Returns the
+// stream size in bytes (warp-uniform); the stream then fills [top - round_up_16(size), top) of the ring.
+//   stage = this warp's 512 B input stage; tab = the shared address of the 8x replicated uint4 table
+//   space.reserve(emitted, need): returns once `need` more bytes below the `emitted` ones are free to write
+template <bool R32, uint32_t RING, uint32_t D, class Space>
+__device__ __forceinline__ uint32_t word_encode_stream_ring(const uint8_t* __restrict__ chunk_in, uint32_t m, uint32_t tab, uint32_t stage,
+                                                            uint32_t ring, uint32_t top, Space& space, uint32_t* __restrict__ status)
+{
+    static_assert(D == 1 || D == 2 || D == 4, "the prefetch registers rotate with the 16-step stage block");
+    static_assert(RING % 16 == 0 && RING >= kWordStreamMax + 16 && RING > 2048, "a worst-case stream fits the ring");
+    constexpr uint32_t D2 = 2 * D;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t tab_lane = tab + (lane & (kEncReplicas - 1)) * 16;
+    const uint32_t gt = lanemask_gt();
+    auto entry = [&](uint32_t s) { return lds_u128_ro(tab_lane + s * (kEncReplicas * 16)); };
+    auto emitted = [&](uint32_t w) { const uint32_t d = top - 2u - w; return min(d, d + RING); };
+    auto wrap = [](uint32_t w) { return min(w, w + RING); };      // back into [0, RING)
+
+    uint32_t x = kWordL, wpos = top - 2u, flags = 0;
+    const uint32_t steps = m >> 5, rem = m & 31;
+    const uint32_t nblk = steps >> 4;
+    const bool vec_ok = (reinterpret_cast<uintptr_t>(chunk_in) & 15) == 0;
+    uint4 parked = make_uint4(0, 0, 0, 0);
+    auto fetch = [&](uint32_t b) {               // block b's 512 symbols into registers, one 16-byte vector per lane
+        if (vec_ok) parked = ldg_stream_u128(reinterpret_cast<const uint4*>(chunk_in + b * kEncStageBytes) + lane);
+    };
+    auto fill = [&](uint32_t b) {                // block b into the stage (row j = step 16 b + j)
+        if (vec_ok) {
+            sts_u128(stage + lane * 16, parked);
+        } else {
+            const uint8_t* p = chunk_in + b * kEncStageBytes + lane;
+#pragma unroll
+            for (int j = 0; j < 16; j++) sts_u8(stage + j * 32 + lane, p[j * 32]);
+        }
+    };
+
+    // symbols are walked last to first (main_simd.cpp:294): the ragged tail first, read directly
+    if (nblk) fetch(nblk - 1);
+    space.reserve(0, (steps - nblk * 16 + 1) * 64);
+    if (rem) {
+        const bool active = lane < rem;
+        const uint4 e = active ? entry(chunk_in[static_cast<uint64_t>(steps) * 32 + lane]) : make_uint4(0, 0, 0, 0);
+        const bool need = active && (x | 31u) >= e.y;
+        const uint32_t mask = __ballot_sync(0xffffffffu, need);
+        if (need) {
+            sts_u16(ring_addr<RING>(ring, wpos - 2u * __popc(mask & gt)), x);
+            x >>= 16;
+        }
+        wpos -= 2u * __popc(mask);
+        if (active) {
+            flags |= e.w;
+            x = word_enc_fold<R32>(x, e);
+        }
+    }
+    for (uint32_t g = steps; g > nblk * 16; g--)
+        word_ring_step<R32, RING>(x, wpos, flags, entry(chunk_in[static_cast<uint64_t>(g - 1) * 32 + lane]), ring, gt);
+    wpos = wrap(wpos);
+
+    if (nblk) {
+        // the software pipeline: during step t the symbol of step t - 2D and the table entry of step t - D are loaded;
+        // sy[t % 2D] and en[t % D] hold them (16 % 2D == 0, so the rotation is the same in every block)
+        uint32_t sy[D2];
+        uint4 en[D];
+        __syncwarp();
+        fill(nblk - 1);
+        if (nblk > 1) fetch(nblk - 2);
+        __syncwarp();
+#pragma unroll
+        for (int j = 15; j >= 16 - static_cast<int>(D2); j--) sy[j % D2] = lds_u8(stage + j * 32 + lane);
+#pragma unroll
+        for (int j = 15; j >= 16 - static_cast<int>(D); j--) en[j % D] = entry(sy[j % D2]);
+        for (uint32_t b = nblk; b-- > 0;) {
+            space.reserve(emitted(wpos), 16 * 64);
+#pragma unroll
+            for (int j = 15; j >= 0; j--) {
+                const uint4 e = en[j % D];
+                if (j == static_cast<int>(D2) - 1 && b) {      // every row of block b has been read: the stage takes block b - 1
+                    __syncwarp();
+                    fill(b - 1);
+                    if (b > 1) fetch(b - 2);
+                    __syncwarp();
+                }
+                // in block 0 the rows below 0 read stale stage bytes: valid table indices, never used
+                sy[j % D2] = lds_u8(stage + ((j - static_cast<int>(D2)) & 15) * 32 + lane);
+                en[j % D] = entry(sy[(j - static_cast<int>(D)) & (D2 - 1)]);
+                word_ring_step<R32, RING>(x, wpos, flags, e, ring, gt);
+            }
+            wpos = wrap(wpos);
+        }
+    }
+
+    // the final states for lanes 31..0 (RansWordEncFlush, main_simd.cpp:298-299), then zeros down to a 16-byte boundary
+    space.reserve(emitted(wpos), 32 * 4 + 16);
+    const uint32_t hpos = wpos - 4u * (31u - lane);
+    sts_u16(ring_addr<RING>(ring, hpos), x >> 16);
+    sts_u16(ring_addr<RING>(ring, hpos - 2u), x);
+    const uint32_t produced = emitted(wpos) + 32 * 4;
+    const uint32_t gap = ((produced + 15u) & ~15u) - produced;
+    if (2u * lane < gap) sts_u16(ring_addr<RING>(ring, top - produced - 2u - 2u * lane), 0);
+    if (__any_sync(0xffffffffu, (flags & kWordSlots) != 0) && lane == 0) atomicOr(status, kStatSymbol);
+    return produced;
+}
+
+// K2r's shape: one CTA of RB200_RING_WARPS warps per SM, each with a ring of RB200_RING_BYTES and a 512 B stage, and the
+// table: 32 KiB + 15 x (12800 + 512) B = 227 KiB, all the shared memory a CTA can have.  A ring holds a worst-case stream
+// (12 480 B at chunks of 8192); with uniform bytes the pending stream (8.3 KB) leaves 4.5 KB for the next one.
+// H100 SXM at 400 W, 1 GiB uniform bytes, chunks of 8192, ms per call of the step alone (no placement:
+// tools/encode_ring_lab.cu), {ring bytes, warps, D}: {16384, 11, 1} 2.00 | {16384, 11, 2} 1.73 | {16384, 11, 4} 1.60 |
+// {14336, 13, 2} 1.32 | {14336, 13, 4} 1.33 | {13312, 14, 1} 1.23 | {13312, 14, 2} 1.24 | {13312, 14, 4} 1.26 |
+// {12800, 15, 1} 1.18 | {12800, 15, 2} 1.25 | {12800, 15, 4} 1.27; the split encoder (K2, 16 warps x 3 CTAs, streams
+// through global slots) 1.23, the shipped K2f with placement 1.71.  At 11 warps the step is latency bound and the
+// prefetch distance pays; at 14-15 warps the warps hide the latency and D = 1 issues least.  With placement
+// (encode_ring.cuh) the order changes: {12800, 15, 2} 1.37-1.38 | {12800, 15, 1} 1.59-1.75 | {13312, 14, 1} 1.41-1.42 |
+// {14336, 13, 2} 1.50-1.51 | {16384, 11, 4} 1.76-1.77, against 1.70-1.71 for K2f in the same runs (two sessions).
+#ifndef RB200_RING_BYTES
+#define RB200_RING_BYTES 12800
+#endif
+#ifndef RB200_RING_WARPS
+#define RB200_RING_WARPS 15
+#endif
+#ifndef RB200_RING_AHEAD
+#define RB200_RING_AHEAD 2             // D: table entries loaded D steps ahead, symbols 2 D steps ahead
+#endif
+constexpr uint32_t kEncRingStreamBytes = RB200_RING_BYTES, kEncRingWarps = RB200_RING_WARPS;
+constexpr uint32_t kEncRingMaxChunk = 8192;     // chunks of at most this many symbols have streams of at most kWordStreamMax bytes
+constexpr uint32_t kEncRingSmemBytes = kEncTableBytes + kEncRingWarps * (kEncRingStreamBytes + kEncStageBytes);
+
+// The body of K2r at a given shape (the kernels below use RB200_RING_*): dynamic shared memory
+// [32 KiB table][W rings of RING bytes][W stages of 512 B].  Returns this warp's ring waits (encode_ring.cuh).
+template <bool R32, uint32_t RING, uint32_t W, uint32_t D>
+__device__ __forceinline__ uint32_t word_encode_ring(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms,
+                                                     const WordEncEntry* __restrict__ g_table, const PlaceOut& out, uint32_t* __restrict__ counter)
+{
+    extern __shared__ __align__(1024) uint8_t s_enc[];
+    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
+    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
+    __syncthreads();
+    const uint32_t warp = threadIdx.x >> 5, tab = smem_addr(s_enc);
+    const uint32_t ring = tab + kEncTableBytes + warp * RING, stage = tab + kEncTableBytes + W * RING + warp * kEncStageBytes;
+    uint32_t* status = out.status;
+    return encode_chunks_ring<RING>(in, n, chunk_syms, ring, out, counter, [=](const uint8_t* chunk_in, uint32_t m, StreamRing<RING>& q) {
+        return word_encode_stream_ring<R32, RING, D>(chunk_in, m, tab, stage, ring, q.top, q, status);
+    });
+}
+
+// Grid = min(SMs, what the chunks need), sized by the host's encode plan; chunk_syms <= kEncRingMaxChunk.
+template <bool R32>
+__global__ void __launch_bounds__(kEncRingWarps * 32, 1)
+word_encode_ring_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
+                        const WordEncEntry* __restrict__ g_table, uint64_t* __restrict__ look, uint32_t* __restrict__ counter,
+                        uint8_t* __restrict__ blob, uint64_t blob_cap, uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
+{
+    word_encode_ring<R32, kEncRingStreamBytes, kEncRingWarps, RB200_RING_AHEAD>(in, n, chunk_syms, g_table,
+                                                                   PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
+}
+
+// ---------------------------------------------------------------------------
 // K6: directory + compaction of the per-chunk slots into the final blob
 //
 // offsets[c] = E_c - sizes[c], E_c = sum_{j<=c} round_up_16(sizes[j]); offsets[n_chunks] = E_last.
@@ -321,6 +565,10 @@ inline void configure_word_kernels()
     cudaFuncSetAttribute(word_encode_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
     cudaFuncSetAttribute(word_encode_fused_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(word_encode_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+    cudaFuncSetAttribute(word_encode_ring_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_encode_ring_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncRingSmemBytes);
+    cudaFuncSetAttribute(word_encode_ring_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(word_encode_ring_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncRingSmemBytes);
 }
 
 }  // namespace rb200
