@@ -260,6 +260,20 @@ int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size
 int rb200_container_model_encode_async(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, size_t n,
                                        uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap);
 
+/* rb200_container_model_encode_async with the length in device memory: the call reads n = *d_n when it executes (at
+ * every replay of a CUDA graph that captured it) and writes the bytes rb200_container_model_encode_async(ctx, coder,
+ * scale_bits, in, *d_n, chunk_syms, flags, out, out_cap) writes.  n_max is a host-side bound that fixes the launch
+ * shapes and the workspace, so one graph serves every 1 <= *d_n <= n_max; nothing is written at or past the container's
+ * end, rb200_container_size(n_chunks, blob_bytes).  d_n is device memory, 8-byte aligned.  The call returns
+ * RB200_E_ARG (nothing launched) by the fixed call's rules with n_max in place of n, and for a null or misaligned d_n
+ * or n_max == 0; RB200_E_SPACE when out_cap is below the blob offset for n_max.  rb200_sync returns RB200_E_MODEL for
+ * *d_n == 0 and RB200_E_ARG for *d_n > n_max (out is not written at all in either case), and otherwise what it returns
+ * for the fixed call.  On every error the header is not written.  The workspace grows for n_max as the fixed call's
+ * for n, so a call with the same (coder, chunk_syms, n_max) outside a capture must come first. */
+int rb200_container_model_encode_varlen_async(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in,
+                                              const uint64_t* d_n, size_t n_max, uint32_t chunk_syms, uint32_t flags,
+                                              uint8_t* out, size_t out_cap);
+
 /* ---------------------------------------------------------------- multi-GPU: gathering the shards' blobs (NCCL) */
 
 /* Shards are independent (SURVEY 8e): every rank encodes / decodes its own contiguous range of symbols with no

@@ -58,6 +58,8 @@ EXPORTS = [
     ("rb200_container_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_container_model_encode_async", C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_size_t, C.c_uint32,
                                                      C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_container_model_encode_varlen_async", C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                            C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -372,6 +374,14 @@ class Context:
         model rb200_model_create refuses, -3 out_cap too small for the blob, header unwritten) comes from sync()"""
         self.lib.check(self.lib.dll.rb200_container_model_encode_async(self.h, coder, scale_bits, in_ptr, n, chunk_syms, flags, out_ptr,
                                                                        out_cap), self.h)
+
+    def container_model_encode_varlen_async(self, coder, scale_bits, in_ptr, n_ptr, n_max, chunk_syms, flags, out_ptr, out_cap):
+        """container_model_encode_async with the length read from device memory when the work runs: n_ptr is the device
+        address of a u64 n, 1 <= n <= n_max.  n_max fixes the launch shapes and the workspace, so one captured call serves
+        every such n.  The verdict (-2 for n == 0, -1 for n > n_max, both with out untouched; otherwise as
+        container_model_encode_async) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_model_encode_varlen_async(self.h, coder, scale_bits, in_ptr, n_ptr, n_max, chunk_syms,
+                                                                              flags, out_ptr, out_cap), self.h)
 
     # ---- per-block containers (version 2): every block's model, the directory and the blob in one buffer
     def container_blocks_capacity(self, n_blocks, block_size, chunk_syms):

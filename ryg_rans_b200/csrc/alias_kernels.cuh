@@ -427,12 +427,11 @@ struct AliasEncoder {
 //   look != nullptr: fused -- chunk ids from an atomic counter, kAliasFusedSlots scratch slots per warp, warp 0 of
 //                    CTA 0 is the scanner (placement.cuh).
 template <bool ALIAS, uint32_t SB>
-__global__ void __launch_bounds__(kAliasEncWarps * 32, 1)
-alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb_rt,
-                    const AliasEncEntry* __restrict__ g_enc, const uint16_t* __restrict__ g_remap,
-                    uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
-                    uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap,
-                    uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
+__device__ __forceinline__ void alias_encode(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb_rt,
+                                             const AliasEncEntry* __restrict__ g_enc, const uint16_t* __restrict__ g_remap,
+                                             uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
+                                             uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob,
+                                             uint64_t blob_cap, uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
 {
     const uint32_t sb = SB ? SB : sb_rt;
     extern __shared__ __align__(1024) uint8_t s_alias[];      // [32 x 1.0 KiB stage+ring][32 KiB table][remap]
@@ -465,6 +464,35 @@ alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_s
                                                                  PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
 }
 
+template <bool ALIAS, uint32_t SB>
+__global__ void __launch_bounds__(kAliasEncWarps * 32, 1)
+alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb_rt,
+                    const AliasEncEntry* __restrict__ g_enc, const uint16_t* __restrict__ g_remap,
+                    uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
+                    uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap,
+                    uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
+{
+    alias_encode<ALIAS, SB>(in, n, chunk_syms, n_chunks, sb_rt, g_enc, g_remap, scratch, slot_bytes, sizes, look, counter, blob, blob_cap,
+                            offsets, status);
+}
+
+// rb200_container_model_encode_varlen_async: n, the chunk count, the blob's place in the container `out` and its
+// capacity from the record, on the grid the host sized for n_max.  In split mode a CTA past the real chunks exits before
+// it stages its tables; in fused mode every CTA runs (CTA 0 holds the scanner, the others find no chunk and leave).
+template <bool ALIAS, uint32_t SB>
+__global__ void __launch_bounds__(kAliasEncWarps * 32, 1)
+alias_encode_varlen_kernel(const uint8_t* __restrict__ in, uint32_t chunk_syms, const VarlenGeom* __restrict__ geom, uint32_t sb_rt,
+                           const AliasEncEntry* __restrict__ g_enc, const uint16_t* __restrict__ g_remap,
+                           uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
+                           uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ out,
+                           uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
+{
+    const uint32_t n_chunks = geom->n_chunks;
+    if (!geom->go || (!look && blockIdx.x * kAliasEncWarps >= n_chunks)) return;
+    alias_encode<ALIAS, SB>(in, geom->n, chunk_syms, n_chunks, sb_rt, g_enc, g_remap, scratch, slot_bytes, sizes, look, counter,
+                            out + geom->blob_off, geom->blob_cap, offsets, status);
+}
+
 // dynamic shared memory of the alias (remap != nullptr) or byte encoder at scale_bits sb
 inline uint32_t alias_encode_smem(bool alias, uint32_t sb) { return kAliasEncFixedSmem + (alias ? (2u << sb) : 0u); }
 
@@ -476,6 +504,8 @@ inline void configure_alias_encode()
 {
     cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, alias_encode_smem(ALIAS, 16));
+    cudaFuncSetAttribute(alias_encode_varlen_kernel<ALIAS, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(alias_encode_varlen_kernel<ALIAS, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, alias_encode_smem(ALIAS, 16));
 }
 template <uint32_t SB>
 inline void configure_byte_decode()
@@ -526,6 +556,22 @@ inline void launch_alias_encode(cudaStream_t stream, uint32_t grid, uint32_t sme
     } else {
         RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_kernel<false, SB><<<grid, kAliasEncWarps * 32, smem, stream>>>(
             d_in, n, chunk_syms, n_chunks, sb, enc, nullptr, scratch, slot, sizes, look, counter, blob, blob_cap, offsets, status)))
+    }
+}
+
+// launch_alias_encode for rb200_container_model_encode_varlen_async: n, n_chunks and the blob from `geom`, the blob in
+// `out`; grid and mode fixed by the host for n_max
+inline void launch_alias_encode_varlen(cudaStream_t stream, uint32_t grid, uint32_t smem, const uint8_t* d_in, uint32_t chunk_syms,
+                                       const VarlenGeom* geom, uint32_t sb, const AliasEncEntry* enc, const uint16_t* remap,
+                                       uint8_t* scratch, uint32_t slot, uint32_t* sizes, uint64_t* look, uint32_t* counter, uint8_t* out,
+                                       uint64_t* offsets, uint32_t* status)
+{
+    if (remap) {
+        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_varlen_kernel<true, SB><<<grid, kAliasEncWarps * 32, smem, stream>>>(
+            d_in, chunk_syms, geom, sb, enc, remap, scratch, slot, sizes, look, counter, out, offsets, status)))
+    } else {
+        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_varlen_kernel<false, SB><<<grid, kAliasEncWarps * 32, smem, stream>>>(
+            d_in, chunk_syms, geom, sb, enc, nullptr, scratch, slot, sizes, look, counter, out, offsets, status)))
     }
 }
 

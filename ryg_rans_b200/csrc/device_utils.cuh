@@ -11,8 +11,22 @@ constexpr uint32_t kStatSymbol = 2u;   // encoder saw a symbol with model freque
 constexpr uint32_t kStatSpace  = 4u;   // compacted blob does not fit blob_cap
 constexpr uint32_t kStatStall  = 8u;   // a bounded wait inside a kernel expired (a bug or a wedged GPU, not bad input)
 constexpr uint32_t kStatModel  = 16u;  // the model built from the data is one rb200_model_create refuses
+constexpr uint32_t kStatArg    = 32u;  // a length read from device memory is outside what the call was enqueued for
 
 constexpr uint32_t kHeaderBytes = 128; // 32 lanes x u32 final state (RansWordEncFlush / RansEncFlush x 32)
+
+// The geometry of rb200_container_model_encode_varlen_async, which reads the input length from device memory: written
+// by varlen_plan_kernel (model_kernels.cuh) from *d_n at every run, read at entry by every kernel after it, which all
+// exit when go == 0.  The launch shapes are the host's, sized for n_max; everything that depends on n is here.
+struct VarlenGeom {
+    uint64_t n;            // symbols, 1 <= n <= n_max
+    uint64_t dir_len;      // directory bytes, 8 (n_chunks + 1)
+    uint64_t blob_off;     // offset of the blob in the container, round16(1088 + dir_len)
+    uint64_t blob_cap;     // out_cap - blob_off
+    uint64_t blob_len;     // dir[n_chunks], copied after the encoder (the blob CRC's length)
+    uint32_t n_chunks;
+    uint32_t go;           // 1: *d_n passed the checks; 0: nothing after the plan runs (dir_len, blob_off, blob_len are 0)
+};
 
 __device__ __forceinline__ uint32_t lanemask_lt()
 {

@@ -12,6 +12,11 @@
 //                               exits before it touches the counter, look[] or scratch
 //   crc32_kernel x 1-2, container_finish_kernel
 //                               as rb200_container_encode in device memory, with the model section from freqs[]
+//
+// rb200_container_model_encode_varlen_async runs the same stages on launch shapes the host sizes for a bound n_max,
+// and reads the length from device memory: varlen_plan_kernel checks *d_n and writes the geometry record (VarlenGeom,
+// device_utils.cuh) into geom; every later kernel takes n, the chunk count and the blob's place from there and exits
+// at entry when the checks failed.  The encoders are the *_varlen_kernel instances, which call the same drivers.
 #pragma once
 #include "block_kernels.cuh"
 #include "container_format.h"
@@ -32,6 +37,7 @@ struct ModelAsyncWork {
     alignas(16) AliasEncEntry byte_enc[256];      // RansEncSymbol images
     alignas(16) uint4 r64_enc[256 * 2];           // Rans64EncSymbol images, 32 bytes each
     alignas(16) uint16_t alias_remap[1u << 16];   // the first 1 << scale_bits entries are the model's
+    VarlenGeom geom;                              // rb200_container_model_encode_varlen_async: the length and layout of this run
 };
 
 constexpr int kModelThreads = 256;                // one thread per symbol
@@ -41,8 +47,8 @@ constexpr int kModelThreads = 256;                // one thread per symbol
 // well-formed entries, and container_finish_kernel writes no header).  Normalisation itself cannot fail for targets
 // >= 256: a squashed symbol needs a donor of width > 1, and while any symbol is squashed the widths, which sum to the
 // target, cannot all be <= 1.  block_normalize keeps its check all the same, with kStatModel as the verdict.
-__global__ void __launch_bounds__(kModelThreads)
-    container_model_kernel(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w, uint32_t* __restrict__ status)
+__device__ __forceinline__ void container_model(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w,
+                                                uint32_t* __restrict__ status)
 {
     __shared__ uint32_t s_cnt[256], s_cum[257];
     __shared__ __align__(16) uint32_t s_w[256];
@@ -101,6 +107,54 @@ __global__ void __launch_bounds__(kModelThreads)
     }
 }
 
+__global__ void __launch_bounds__(kModelThreads)
+    container_model_kernel(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w, uint32_t* __restrict__ status)
+{
+    container_model(coder, sb, r32_allowed, w, status);
+}
+
+// The varlen call's instance: with *d_n == 0 the counts are all zero and normalisation has no total to scale, so it
+// runs only when the plan passed
+__global__ void __launch_bounds__(kModelThreads)
+    container_model_varlen_kernel(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w,
+                                  uint32_t* __restrict__ status)
+{
+    if (!w->geom.go) return;
+    container_model(coder, sb, r32_allowed, w, status);
+}
+
+// The first kernel of rb200_container_model_encode_varlen_async, one warp: reads n = *d_n, checks 1 <= n <= n_max
+// (n == 0 is kStatModel, as the fixed call's RB200_E_MODEL; n > n_max is kStatArg) and writes the geometry of a
+// version 1 container of n symbols into *g, with go = 1 when the checks pass.  On failure *g is zero: every later
+// kernel exits at entry and the CRC kernels, which read their lengths from *g, cover nothing.  out_cap is at least the
+// blob offset of n_max (the host checks it), so blob_cap does not wrap.
+__global__ void __launch_bounds__(32)
+    varlen_plan_kernel(const uint64_t* __restrict__ d_n, uint64_t n_max, uint32_t chunk_syms, uint64_t out_cap, VarlenGeom* __restrict__ g,
+                       uint32_t* __restrict__ status)
+{
+    if (threadIdx.x) return;
+    const uint64_t n = *d_n;
+    VarlenGeom r = {};
+    if (n == 0 || n > n_max) {
+        atomicOr(status, n == 0 ? kStatModel : kStatArg);
+    } else {
+        const uint64_t chunks = n / chunk_syms + (n % chunk_syms != 0);
+        r.n = n;
+        r.n_chunks = static_cast<uint32_t>(chunks);
+        r.dir_len = (chunks + 1) * sizeof(uint64_t);
+        r.blob_off = (kContainerDirOffset + r.dir_len + 15) & ~15ull;
+        r.blob_cap = out_cap - r.blob_off;
+        r.go = 1;
+    }
+    *g = r;
+}
+
+// After the encoder, one thread: blob_len = dir[n_chunks], the length of the blob CRC (crc32_kernel's n_dev)
+__global__ void __launch_bounds__(32) varlen_blob_len_kernel(const uint64_t* __restrict__ dir, VarlenGeom* __restrict__ g)
+{
+    if (threadIdx.x == 0 && g->go) g->blob_len = dir[g->n_chunks];
+}
+
 // The word encoders behind the gate: word_encode_kernel / word_encode_fused_kernel, run only when *gate (the model
 // kernel's r32) names this instance.  The host launches both instances of the call's path.
 template <bool R32>
@@ -141,11 +195,58 @@ word_encode_fused_gated_kernel(const uint8_t* __restrict__ in, uint64_t n, uint3
                                                                      PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
 }
 
+// The varlen call's word encoders: the gated wrappers above with n, the chunk count and the blob's place (in the
+// container `out`) from the record, on the grid the host sized for n_max.  A split-path CTA past the real chunks exits
+// before it stages its table.
+template <bool R32>
+__global__ void __launch_bounds__(kEncWarps * 32, RB200_ENC_MINBLOCKS)
+word_encode_gated_varlen_kernel(const uint8_t* __restrict__ in, uint32_t chunk_syms, const VarlenGeom* __restrict__ geom,
+                                const WordEncEntry* __restrict__ g_table, const uint32_t* __restrict__ gate, uint8_t* __restrict__ scratch,
+                                uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
+{
+    const uint32_t n_chunks = geom->n_chunks;
+    if (!geom->go || *gate != (R32 ? 1u : 0u) || blockIdx.x * kEncWarps >= n_chunks) return;   // the same for the whole CTA
+    extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
+    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
+    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
+    __syncthreads();
+
+    const uint32_t warp = threadIdx.x >> 5;
+    const uint32_t chunk = blockIdx.x * kEncWarps + warp;
+    if (chunk >= n_chunks) return;
+    const ChunkRange r = chunk_range(chunk, chunk_syms, geom->n);
+    encode_chunk_split(in + r.first, r.m, chunk, WordEncoder<R32>{smem_addr(s_enc)}, smem_addr(s_enc) + kEncTableBytes + warp * kEncWarpSmem,
+                       scratch, slot_bytes, sizes, status);
+}
+
+template <bool R32>
+__global__ void __launch_bounds__(kEncWarps * 32, RB200_FUSED_MINBLOCKS)
+word_encode_fused_gated_varlen_kernel(const uint8_t* __restrict__ in, uint32_t chunk_syms, const VarlenGeom* __restrict__ geom,
+                                      const WordEncEntry* __restrict__ g_table, const uint32_t* __restrict__ gate, uint8_t* __restrict__ scratch,
+                                      uint32_t slot_bytes, uint64_t* __restrict__ look, uint32_t* __restrict__ counter,
+                                      uint8_t* __restrict__ out, uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
+{
+    if (!geom->go || *gate != (R32 ? 1u : 0u)) return;             // the same for the whole grid
+    extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
+    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
+    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
+    __syncthreads();
+
+    const uint32_t tab = smem_addr(s_enc), wsm = tab + kEncTableBytes + (threadIdx.x >> 5) * kEncWarpSmem;
+    encode_chunks_fused<kFusedSlots, kEncWarps, RB200_ENC_KEEP_HINT>(
+        in, geom->n, chunk_syms, WordEncoder<R32>{tab}, wsm, scratch, slot_bytes,
+        PlaceOut{look, geom->n_chunks, out + geom->blob_off, geom->blob_cap, offsets, status}, counter);
+}
+
 inline void configure_model_kernels()
 {
     for (const void* k : {reinterpret_cast<const void*>(word_encode_gated_kernel<false>), reinterpret_cast<const void*>(word_encode_gated_kernel<true>),
                           reinterpret_cast<const void*>(word_encode_fused_gated_kernel<false>),
-                          reinterpret_cast<const void*>(word_encode_fused_gated_kernel<true>)}) {
+                          reinterpret_cast<const void*>(word_encode_fused_gated_kernel<true>),
+                          reinterpret_cast<const void*>(word_encode_gated_varlen_kernel<false>),
+                          reinterpret_cast<const void*>(word_encode_gated_varlen_kernel<true>),
+                          reinterpret_cast<const void*>(word_encode_fused_gated_varlen_kernel<false>),
+                          reinterpret_cast<const void*>(word_encode_fused_gated_varlen_kernel<true>)}) {
         cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
     }

@@ -139,6 +139,7 @@ inline uint32_t slot_bytes_for(uint32_t chunk_syms) { return static_cast<uint32_
 
 int status_to_code(uint32_t bits)
 {
+    if (bits & kStatArg) return RB200_E_ARG;
     if (bits & kStatModel) return RB200_E_MODEL;
     if (bits & kStatSymbol) return RB200_E_SYMBOL;
     if (bits & kStatSpace) return RB200_E_SPACE;
@@ -582,10 +583,8 @@ struct EncodeWorkspace {
     uint64_t* tile_sums;   // split
 };
 
-// Runs a plan: reserve its workspace; fused: zero the counter and look[], then `launch(ws)`, the one kernel; split:
-// `launch(ws)` encodes into the slots (when there are chunks), then finish_encode.  `launch` returns check_launch's code.
-template <class Launch>
-int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, Launch launch)
+// Reserves the workspace of a plan and lays it out; fused: zeroes the counter and look[] on the stream.
+int prepare_workspace(rb200_ctx* ctx, const EncodePlan& p, EncodeWorkspace* ws)
 {
     int rc = reserve_plan(ctx, p);
     if (rc != RB200_OK) return rc;
@@ -594,13 +593,27 @@ int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob
     uint64_t* tail = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + plan_head_bytes(p));
     if (p.fused) {
         RB_CUDA(ctx, cudaMemsetAsync(ctx->sizes.p, 0, 16 + static_cast<size_t>(p.n_chunks) * sizeof(uint64_t), ctx->stream));
-        return launch(EncodeWorkspace{scratch, head, tail, nullptr, nullptr});
+        *ws = EncodeWorkspace{scratch, head, tail, nullptr, nullptr};
+    } else {
+        *ws = EncodeWorkspace{scratch, nullptr, nullptr, head, tail};
     }
+    return RB200_OK;
+}
+
+// Runs a plan: prepare its workspace; fused: `launch(ws)`, the one kernel; split: `launch(ws)` encodes into the slots
+// (when there are chunks), then finish_encode.  `launch` returns check_launch's code.
+template <class Launch>
+int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, Launch launch)
+{
+    EncodeWorkspace ws = {};
+    int rc = prepare_workspace(ctx, p, &ws);
+    if (rc != RB200_OK) return rc;
+    if (p.fused) return launch(ws);
     if (p.n_chunks) {
-        rc = launch(EncodeWorkspace{scratch, nullptr, nullptr, head, tail});
+        rc = launch(ws);
         if (rc != RB200_OK) return rc;
     }
-    return finish_encode(ctx, scratch, p.slot_bytes, head, tail, p.n_chunks, d_blob, blob_cap, d_offsets);
+    return finish_encode(ctx, ws.scratch, p.slot_bytes, ws.sizes, ws.tile_sums, p.n_chunks, d_blob, blob_cap, d_offsets);
 }
 
 // The encode tables of one encode call, in device memory.  Word: `word_gate` null runs the instance word_r32 names on
@@ -679,6 +692,59 @@ int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, si
                             ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status);
         return check_launch(ctx, alias ? "alias_encode_kernel" : "byte_encode_kernel");
     });
+}
+
+// encode_device for rb200_container_model_encode_varlen_async, on a GPU-built model (t.word_gate set): the plan of
+// n_chunks_max chunks fixes the path and every launch shape, and each kernel reads n, the chunk count and the blob's
+// place in the container `out` from `geom`.  Split: the tile scan, the tile prefix when n_max's tiles pass the
+// threshold, and the compaction, all on the device's chunk count.
+int encode_device_varlen(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, uint32_t n_chunks_max, uint32_t chunk_syms,
+                         const VarlenGeom* geom, uint8_t* out, uint64_t* d_offsets)
+{
+    const EncodePlan p = plan_encode(ctx, t.coder, t.scale_bits, n_chunks_max, chunk_syms, false);
+    EncodeWorkspace ws = {};
+    int rc = prepare_workspace(ctx, p, &ws);
+    if (rc != RB200_OK) return rc;
+    cudaStream_t s = ctx->stream;
+    if (t.coder == RB200_CODER_WORD) {
+        for (int r32 = 0; r32 < 2 && rc == RB200_OK; r32++) {
+            if (p.fused) {
+                auto kernel = r32 ? word_encode_fused_gated_varlen_kernel<true> : word_encode_fused_gated_varlen_kernel<false>;
+                kernel<<<p.grid, p.threads, p.smem, s>>>(d_in, chunk_syms, geom, t.word[r32], t.word_gate, ws.scratch, p.slot_bytes, ws.look,
+                                                         ws.counter, out, d_offsets, ctx->d_status);
+                rc = check_launch(ctx, "word_encode_fused_gated_varlen_kernel");
+            } else {
+                auto kernel = r32 ? word_encode_gated_varlen_kernel<true> : word_encode_gated_varlen_kernel<false>;
+                kernel<<<p.grid, p.threads, p.smem, s>>>(d_in, chunk_syms, geom, t.word[r32], t.word_gate, ws.scratch, p.slot_bytes, ws.sizes,
+                                                         ctx->d_status);
+                rc = check_launch(ctx, "word_encode_gated_varlen_kernel");
+            }
+        }
+    } else if (t.coder == RB200_CODER_RANS64) {
+        rans64_encode_varlen_kernel<<<p.grid, p.threads, p.smem, s>>>(d_in, chunk_syms, geom, t.scale_bits, t.r64, ws.scratch, p.slot_bytes,
+                                                                      ws.sizes, ctx->d_status);
+        rc = check_launch(ctx, "rans64_encode_varlen_kernel");
+    } else {
+        const bool alias = t.coder == RB200_CODER_ALIAS;
+        launch_alias_encode_varlen(s, p.grid, p.smem, d_in, chunk_syms, geom, t.scale_bits, t.enc, alias ? t.remap : nullptr, ws.scratch,
+                                   p.slot_bytes, ws.sizes, ws.look, ws.counter, out, d_offsets, ctx->d_status);
+        rc = check_launch(ctx, "alias_encode_varlen_kernel");
+    }
+    if (rc != RB200_OK || p.fused) return rc;
+    const uint32_t tiles = (n_chunks_max + kScanTile - 1) / kScanTile;
+    scan_tiles_varlen_kernel<<<tiles, 1024, 0, s>>>(ws.sizes, geom, d_offsets, ws.tile_sums);
+    rc = check_launch(ctx, "scan_tiles_varlen_kernel");
+    if (rc != RB200_OK) return rc;
+    const uint32_t prefixed = tiles > kTilePrefixThreshold ? 1u : 0u;
+    if (prefixed) {
+        tile_prefix_varlen_kernel<<<1, 1024, 0, s>>>(ws.tile_sums, geom);
+        rc = check_launch(ctx, "tile_prefix_varlen_kernel");
+        if (rc != RB200_OK) return rc;
+    }
+    const uint32_t grid = (n_chunks_max + kCopyWarps - 1) / kCopyWarps;
+    compact_varlen_kernel<<<grid, kCopyWarps * 32, 0, s>>>(ws.scratch, p.slot_bytes, ws.sizes, d_offsets, ws.tile_sums, prefixed, geom, out,
+                                                           ctx->d_status);
+    return check_launch(ctx, "compact_varlen_kernel");
 }
 
 int decode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_blob, size_t blob_size, const uint64_t* d_offsets,
@@ -1260,11 +1326,13 @@ extern "C" int rb200_blocks_decode(rb200_ctx* ctx, const uint8_t* blob, size_t b
 
 namespace {
 
-// zlib crc32 of d[0, n) into `slot`, on ctx->stream; with n_dev set the length is min(*n_dev, n)
-int launch_crc(rb200_ctx* ctx, const uint8_t* d, uint64_t n, const uint64_t* n_dev, uint32_t crc_in, CrcSlot* slot)
+// zlib crc32 of d[0, n) into `slot`, on ctx->stream; with n_dev set the length is min(*n_dev, n); with off_dev set the
+// bytes start *off_dev bytes after d (crc32_kernel)
+int launch_crc(rb200_ctx* ctx, const uint8_t* d, uint64_t n, const uint64_t* n_dev, uint32_t crc_in, CrcSlot* slot,
+               const uint64_t* off_dev = nullptr)
 {
     const uint32_t sms = static_cast<uint32_t>(ctx->sms);
-    crc32_kernel<<<n_dev ? sms : crc32_grid(sms, n), kCrcThreads, kCrcSmemBytes, ctx->stream>>>(d, n, n_dev, nullptr, crc_in,
+    crc32_kernel<<<n_dev ? sms : crc32_grid(sms, n), kCrcThreads, kCrcSmemBytes, ctx->stream>>>(d, n, n_dev, off_dev, crc_in,
                                                                                                 ctx->d_crc_work, slot);
     return check_launch(ctx, "crc32_kernel");
 }
@@ -1585,18 +1653,36 @@ extern "C" int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, 
     return rc;
 }
 
+namespace {
+
+// the argument rules of both model encodes, with n the length (fixed call) or its bound n_max (varlen call)
+bool model_encode_args_ok(const rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, size_t n, uint32_t chunk_syms,
+                          const uint8_t* out)
+{
+    if (!ctx || !in || !out || !container_mem_ok(RB200_MEM_DEVICE, out, nullptr)) return false;
+    if (coder < RB200_CODER_WORD || coder > RB200_CODER_RANS64 || scale_bits < 8 || scale_bits > 16) return false;
+    if (coder == RB200_CODER_WORD && scale_bits != kWordScaleBits) return false;
+    if (!chunk_ok(chunk_syms) || (n >> 32)) return false;            // counts of 32 bits, as rb200_model_from_data
+    return rb200_chunk_count(n, chunk_syms) < (1ull << 31);
+}
+
+// the encode tables the model kernel builds in the workspace; the word coder's gate is its r32
+EncodeTables workspace_tables(ModelAsyncWork* w, int coder, uint32_t scale_bits)
+{
+    return EncodeTables{coder, scale_bits, {w->word_enc, w->word_enc32}, 0, &w->r32,
+                        coder == RB200_CODER_ALIAS ? w->alias_enc : w->byte_enc, w->alias_remap, w->r64_enc};
+}
+
+}  // namespace
+
 // rb200_model_from_data + rb200_container_encode (device memory) + rb200_model_destroy with kernels alone
 // (model_kernels.cuh): histogram, model kernel, the coder's encoder, the CRCs and the header.  Five to seven launches and
 // one memset, no copy, no synchronisation; the encode workspace grows as in rb200_container_encode.
 extern "C" int rb200_container_model_encode_async(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, size_t n,
                                                   uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
 {
-    if (!ctx || !in || !out || !container_mem_ok(RB200_MEM_DEVICE, out, nullptr)) return RB200_E_ARG;
-    if (coder < RB200_CODER_WORD || coder > RB200_CODER_RANS64 || scale_bits < 8 || scale_bits > 16) return RB200_E_ARG;
-    if (coder == RB200_CODER_WORD && scale_bits != kWordScaleBits) return RB200_E_ARG;
-    if (!chunk_ok(chunk_syms) || (n >> 32)) return RB200_E_ARG;      // counts of 32 bits, as rb200_model_from_data
+    if (!model_encode_args_ok(ctx, coder, scale_bits, in, n, chunk_syms, out)) return RB200_E_ARG;
     const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
-    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
     if (n == 0) return RB200_E_MODEL;                                // normalize_freqs divides by the total
     ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n, n_chunks, 0, flags);
     const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
@@ -1611,8 +1697,7 @@ extern "C" int rb200_container_model_encode_async(rb200_ctx* ctx, int coder, uin
                                                                  ctx->d_status);
     rc = check_launch(ctx, "container_model_kernel");
     if (rc != RB200_OK) return rc;
-    const EncodeTables t = {coder, scale_bits, {w->word_enc, w->word_enc32}, 0, &w->r32,
-                            coder == RB200_CODER_ALIAS ? w->alias_enc : w->byte_enc, w->alias_remap, w->r64_enc};
+    const EncodeTables t = workspace_tables(w, coder, scale_bits);
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
     uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
     rc = encode_device(ctx, t, in, n, chunk_syms, out + boff, out_cap - boff, dir);
@@ -1621,6 +1706,50 @@ extern "C" int rb200_container_model_encode_async(rb200_ctx* ctx, int coder, uin
     if (rc != RB200_OK) return rc;
     container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, w->freqs, ctx->d_crc, ctx->d_status);
     return check_launch(ctx, "container_finish_kernel");
+}
+
+// rb200_container_model_encode_async with the length read from device memory at every run (model_kernels.cuh): the plan
+// kernel, then the same stages on launch shapes sized for n_max, each taking the length from the plan's record.  Eight
+// to eleven launches and one or two memsets, no copy, no synchronisation; the workspace grows as the fixed call's for n_max.
+extern "C" int rb200_container_model_encode_varlen_async(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in,
+                                                         const uint64_t* d_n, size_t n_max, uint32_t chunk_syms, uint32_t flags,
+                                                         uint8_t* out, size_t out_cap)
+{
+    if (!d_n || (reinterpret_cast<uintptr_t>(d_n) & 7) || n_max == 0) return RB200_E_ARG;
+    if (!model_encode_args_ok(ctx, coder, scale_bits, in, n_max, chunk_syms, out)) return RB200_E_ARG;
+    const uint32_t n_chunks_max = static_cast<uint32_t>(rb200_chunk_count(n_max, chunk_syms));
+    ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n_max, n_chunks_max, 0, flags);
+    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h);
+    if (out_cap < container_blob_offset(h)) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    cudaStream_t s = ctx->stream;
+    ModelAsyncWork* w = ctx->d_model_async;
+    VarlenGeom* geom = &w->geom;
+    varlen_plan_kernel<<<1, 32, 0, s>>>(d_n, n_max, chunk_syms, out_cap, geom, ctx->d_status);
+    int rc = check_launch(ctx, "varlen_plan_kernel");
+    if (rc != RB200_OK) return rc;
+    RB_CUDA(ctx, cudaMemsetAsync(w->counts, 0, sizeof w->counts, s));
+    histogram_varlen_kernel<<<histogram_grid(static_cast<uint32_t>(ctx->sms), n_max), kHistWarps * 32, 0, s>>>(in, geom, w->counts);
+    rc = check_launch(ctx, "histogram_varlen_kernel");
+    if (rc != RB200_OK) return rc;
+    container_model_varlen_kernel<<<1, kModelThreads, 0, s>>>(static_cast<uint32_t>(coder), scale_bits, word_r32_allowed() ? 1u : 0u, w,
+                                                              ctx->d_status);
+    rc = check_launch(ctx, "container_model_varlen_kernel");
+    if (rc != RB200_OK) return rc;
+    const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
+    rc = encode_device_varlen(ctx, workspace_tables(w, coder, scale_bits), in, n_chunks_max, chunk_syms, geom, out, dir);
+    if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, &geom->dir_len, 0, ctx->d_crc);
+    if (rc == RB200_OK && blob_crc) {
+        varlen_blob_len_kernel<<<1, 32, 0, s>>>(dir, geom);
+        rc = check_launch(ctx, "varlen_blob_len_kernel");
+        if (rc == RB200_OK) rc = launch_crc(ctx, out, out_cap, &geom->blob_len, 0, ctx->d_crc + 1, &geom->blob_off);
+    }
+    if (rc != RB200_OK) return rc;
+    h.n_symbols = 0;                                   // the finish kernel fills in n and n_chunks from the record
+    h.n_chunks = 0;
+    container_finish_varlen_kernel<<<1, 32, 0, s>>>(out, h, geom, out_cap, w->freqs, ctx->d_crc, ctx->d_status);
+    return check_launch(ctx, "container_finish_varlen_kernel");
 }
 
 // ---------------------------------------------------------------------------

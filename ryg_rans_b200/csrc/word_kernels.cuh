@@ -440,9 +440,9 @@ word_encode_ring_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chu
 // ---------------------------------------------------------------------------
 constexpr uint32_t kScanTile = 4096;
 
-__global__ void __launch_bounds__(1024)
-scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
-                  uint64_t* __restrict__ tile_sums)
+// pass 1 for tile blockIdx.x (one CTA of 1024 threads)
+__device__ __forceinline__ void scan_tile(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
+                                          uint64_t* __restrict__ tile_sums)
 {
     __shared__ uint64_t s_warp[32];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -479,9 +479,16 @@ scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_
     if (tid == 1023) tile_sums[blockIdx.x] = s_warp[31];
 }
 
-// for very large directories: turn tile_sums into exclusive prefixes once, so compact CTAs read one value
 __global__ void __launch_bounds__(1024)
-tile_prefix_kernel(uint64_t* __restrict__ tile_sums, uint32_t n_tiles)
+scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
+                  uint64_t* __restrict__ tile_sums)
+{
+    scan_tile(sizes, n_chunks, offsets, tile_sums);
+}
+
+// for very large directories: turn tile_sums into exclusive prefixes once, so compact CTAs read one value (one CTA of
+// 1024 threads)
+__device__ __forceinline__ void tile_prefix(uint64_t* __restrict__ tile_sums, uint32_t n_tiles)
 {
     __shared__ uint64_t s_warp[32];
     __shared__ uint64_t s_carry;
@@ -515,14 +522,20 @@ tile_prefix_kernel(uint64_t* __restrict__ tile_sums, uint32_t n_tiles)
     }
 }
 
+__global__ void __launch_bounds__(1024)
+tile_prefix_kernel(uint64_t* __restrict__ tile_sums, uint32_t n_tiles)
+{
+    tile_prefix(tile_sums, n_tiles);
+}
+
 constexpr int kCopyWarps = 8;
 constexpr uint32_t kTilePrefixThreshold = 256;   // above this many tiles, tile_prefix_kernel runs first
 
 // one warp moves one chunk stream from the end of its scratch slot to blob[offsets[c]..E_c)
-__global__ void __launch_bounds__(kCopyWarps * 32)
-compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
-               uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
-               uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status)
+__device__ __forceinline__ void compact_chunks(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+                                               uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums,
+                                               uint32_t tiles_prefixed, uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap,
+                                               uint32_t* __restrict__ status)
 {
     __shared__ uint64_t s_base;
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -553,6 +566,45 @@ compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const u
         }
     }
     if (end <= blob_cap) place_stream<false>(scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, size, blob, end, lane);
+}
+
+__global__ void __launch_bounds__(kCopyWarps * 32)
+compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+               uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
+               uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status)
+{
+    compact_chunks(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, blob, blob_cap, status);
+}
+
+// The split path's directory and compaction for rb200_container_model_encode_varlen_async: grids sized for n_max, the
+// chunk count, the blob's place and its capacity from the record (VarlenGeom, device_utils.cuh).  CTAs past the real
+// tiles or chunks exit at entry.  The host fixes whether tile_prefix runs from n_max's tile count; the prefix and the
+// compaction then both use the device's, which gives the same sums as either choice.
+__global__ void __launch_bounds__(1024)
+scan_tiles_varlen_kernel(const uint32_t* __restrict__ sizes, const VarlenGeom* __restrict__ geom, uint64_t* __restrict__ offsets,
+                         uint64_t* __restrict__ tile_sums)
+{
+    const uint32_t n_chunks = geom->n_chunks;
+    if (!geom->go || blockIdx.x * kScanTile >= n_chunks) return;
+    scan_tile(sizes, n_chunks, offsets, tile_sums);
+}
+
+__global__ void __launch_bounds__(1024)
+tile_prefix_varlen_kernel(uint64_t* __restrict__ tile_sums, const VarlenGeom* __restrict__ geom)
+{
+    if (!geom->go) return;
+    tile_prefix(tile_sums, (geom->n_chunks + kScanTile - 1) / kScanTile);
+}
+
+// out = the container: the blob starts geom->blob_off bytes into it
+__global__ void __launch_bounds__(kCopyWarps * 32)
+compact_varlen_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+                      uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
+                      const VarlenGeom* __restrict__ geom, uint8_t* __restrict__ out, uint32_t* __restrict__ status)
+{
+    const uint32_t n_chunks = geom->n_chunks;
+    if (!geom->go || blockIdx.x * kCopyWarps >= n_chunks) return;
+    compact_chunks(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, out + geom->blob_off, geom->blob_cap, status);
 }
 
 inline void configure_word_kernels()

@@ -29,7 +29,9 @@ RB200_CONTAINER_CRC_BLOB, alternated:
   rb200_container_encode with a prebuilt model; rb200_model_from_data + rb200_container_encode + rb200_model_destroy
   (what a caller without a model does); rb200_container_model_encode_async (the model built on the GPU); the host time
   each call takes to return; and a torch.profiler list of the async call's kernels (histogram, model kernel, encoder,
-  the gated-out word encoder instance, CRCs, header).
+  the gated-out word encoder instance, CRCs, header).  The varlen arm: rb200_container_model_encode_varlen_async at
+  *d_n = n_max = 1 GiB against the fixed async call, and at *d_n = 64 MiB with n_max = 1 GiB against the fixed call at
+  64 MiB (the cost of launch shapes sized for n_max), with a torch.profiler list of the varlen call's kernels.
 
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
@@ -378,6 +380,9 @@ def model_encode(args):
     cap = ctx.container_capacity(n, chunk)
     d_ref = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
     d_out = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    small = 64 << 20
+    d_n = torch.tensor([n, small], dtype=torch.int64, device="cuda")
+    n_full, n_small = d_n.data_ptr(), d_n[1:].data_ptr()
     res = {"card": card(), "workloads": {}, "checks": {}}
     for name, coder, sb, make in workloads:
         d_in = make()
@@ -394,6 +399,12 @@ def model_encode(args):
             calls["encode_prebuilt" + tag] = lambda flags=flags: ctx.container_encode_device(model, i, n, chunk, flags, r, cap)
             calls["from_data_encode" + tag] = lambda flags=flags: from_data(flags)
             calls["model_encode_async" + tag] = lambda flags=flags: ctx.container_model_encode_async(coder, sb, i, n, chunk, flags, o, cap)
+            calls["varlen_n_max" + tag] = lambda flags=flags: ctx.container_model_encode_varlen_async(coder, sb, i, n_full, n, chunk, flags, o,
+                                                                                                      cap)
+            calls["model_encode_async_64m" + tag] = lambda flags=flags: ctx.container_model_encode_async(coder, sb, i, small, chunk, flags, r,
+                                                                                                        cap)
+            calls["varlen_64m_of_n_max" + tag] = lambda flags=flags: ctx.container_model_encode_varlen_async(coder, sb, i, n_small, n, chunk,
+                                                                                                             flags, o, cap)
         times = alternate(calls, sync, args.warmup, args.reps)
         host = {k: [] for k in calls if not k.startswith("encode_prebuilt")}
         for _ in range(args.reps):
@@ -409,11 +420,20 @@ def model_encode(args):
             head = d_out[:64].cpu().numpy()
             size = int(ctx.lib.dll.rb200_container_size(int(head[24:32].view(np.uint64)[0]), int(head[32:40].view(np.uint64)[0])))
             res["checks"][f"{name}: model_encode_async{tag}_equals_prebuilt"] = bool(torch.equal(d_out[:size], d_ref[:size]))
+            for nn, varlen in ((n, "varlen_n_max"), (small, "varlen_64m_of_n_max")):
+                d_out.zero_()
+                ctx.container_model_encode_async(coder, sb, i, nn, chunk, 0 if not tag else crc, r, cap)
+                calls[varlen + tag]()
+                sync()
+                head = d_out[:64].cpu().numpy()
+                size = int(ctx.lib.dll.rb200_container_size(int(head[24:32].view(np.uint64)[0]), int(head[32:40].view(np.uint64)[0])))
+                res["checks"][f"{name}: {varlen}{tag}_equals_fixed_call"] = bool(torch.equal(d_out[:size], d_ref[:size]))
         res["workloads"][name] = {
             "n": n, "chunk_syms": chunk,
             "encode": times,
             "call_host_ms": {k: stats(v) for k, v in host.items()},
-            "kernels": {k: kernel_times(calls[k], sync, args.reps) for k in ("model_encode_async", "model_encode_async_crc")},
+            "kernels": {k: kernel_times(calls[k], sync, args.reps) for k in ("model_encode_async", "model_encode_async_crc", "varlen_n_max_crc",
+                                                                             "varlen_64m_of_n_max_crc")},
         }
         model.close()
         del d_in

@@ -158,6 +158,32 @@ def main():
     assert ctx.lib.dll.rb200_container_model_encode_async(ctx.h, rb.CODER_WORD, 14, d_in.data_ptr(), data.size, 4096, 0,
                                                           d_c.data_ptr(), ccap) == -1
     assert ctx.launches == before
+    # the same with the length read from device memory (n_max = 3 n): valid, *d_n == n_max, then 0 and n_max + 1,
+    # which the plan kernel refuses before anything reads the input or writes the output
+    n_max = 3 * data.size
+    vcap = ctx.container_capacity(n_max, 4096)
+    d_v = torch.zeros(vcap + 16, dtype=torch.uint8, device="cuda")
+    d_big = torch.cat([d_in, d_in, d_in])
+    d_len = torch.zeros(1, dtype=torch.int64, device="cuda")
+    for coder, sb in ((rb.CODER_WORD, 12), (rb.CODER_ALIAS, 16), (rb.CODER_BYTE, 14), (rb.CODER_RANS64, 12)):
+        for length, src in ((data.size, d_in), (n_max, d_big)):
+            d_len.fill_(length)
+            ctx.container_model_encode_varlen_async(coder, sb, d_big.data_ptr(), d_len.data_ptr(), n_max, 4096, api.CONTAINER_CRC_BLOB,
+                                                    d_v.data_ptr(), vcap)
+            d_big_out = torch.zeros(n_max + 16, dtype=torch.uint8, device="cuda")
+            ctx.container_decode_async(d_v.data_ptr(), vcap, d_big_out.data_ptr(), n_max, d_n.data_ptr())
+            ctx.sync()
+            assert torch.equal(d_big_out[:length], src), (coder, length)
+    for length, code in ((0, -2), (n_max + 1, -1)):
+        d_len.fill_(length)
+        d_v.fill_(0x5C)
+        ctx.container_model_encode_varlen_async(rb.CODER_WORD, 12, d_in.data_ptr(), d_len.data_ptr(), n_max, 4096, 0, d_v.data_ptr(), vcap)
+        try:
+            ctx.sync()
+            raise SystemExit("refused length not reported")
+        except rb.RansError as e:
+            assert e.code == code, e
+        assert bool((d_v == 0x5C).all().item())
     print("sanitize smoke ok:", ctx.launches, "launches")
 
 

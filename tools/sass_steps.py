@@ -44,6 +44,7 @@ def main():
     dec = next(v for k, v in fns.items() if "block_decode_kernel" in k)
     enc = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1" in k)
     enc_gated = next(v for k, v in fns.items() if "word_encode_fused_gated_kernelILb1" in k)
+    enc_varlen = next(v for k, v in fns.items() if "word_encode_fused_gated_varlen_kernelILb1" in k)
     tma = next(v for k, v in fns.items() if "word_decode_tma_kernel" in k and k.endswith("Lb0EEEvPKhmPKmPKjPhmjjPNS_10DecodeWorkEPjy"))
     ali = next(v for k, v in fns.items() if "alias_decode_persist_kernelILj16E" in k)
     tma_planned = next(v for k, v in fns.items() if "word_decode_planned_kernelILb0E" in k)
@@ -60,7 +61,9 @@ def main():
                          step_between(dec, "VOTE.ANY", 5)),
                         ("word_encode_fused_kernel<R32>: one step (symbol load to symbol load)", step_between(enc, "LDS.U8", 8)),
                         ("word_encode_fused_gated_kernel<R32> (rb200_container_model_encode_async): one step (symbol load to symbol load)",
-                         step_between(enc_gated, "LDS.U8", 8))):
+                         step_between(enc_gated, "LDS.U8", 8)),
+                        ("word_encode_fused_gated_varlen_kernel<R32> (rb200_container_model_encode_varlen_async): one step (symbol load "
+                         "to symbol load)", step_between(enc_varlen, "LDS.U8", 8))):
         print("## %s: %d instructions" % (title, len(step)))
         print("```")
         for addr, ins in step:
