@@ -230,6 +230,55 @@ int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf, size_t siz
  * rejects, RB200_E_SPACE for n > out_cap; in both cases out is untouched. */
 int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                         uint64_t* d_n_symbols);
+/* ---------------------------------------------------------------- per-block models for the byte and rans64 coders */
+
+/* The per-block calls above for RB200_CODER_BYTE (main.cpp: rans_byte + cum2sym) and RB200_CODER_RANS64 (main64.cpp) at
+ * scale_bits 8..15, with the same geometry (block_size % chunk_syms == 0, at most 32 chunks per block, chunk = block *
+ * (block_size / chunk_syms) + chunk-in-block).  block_freqs is [n_blocks][256] u16, each row normalised to
+ * 1 << scale_bits; every chunk is the coder's ordinary 32-way stream under its block's row, as rb200_encode writes it
+ * with that model.  model_encode builds every block's model on the GPU (count_freqs + normalize_freqs(1 << scale_bits),
+ * main.cpp:59-129, bit-exact) and writes it to block_freqs.  HOST mode pipelines slices of whole blocks like
+ * rb200_blocks_encode; DEVICE mode only enqueues.  RB200_E_ARG (nothing launched) for a coder other than BYTE or RANS64,
+ * scale_bits outside 8..15, a bad geometry, a null pointer, a bad mem_kind or 2^31 chunks or more.  A caller table
+ * whose block does not sum to 1 << scale_bits is RB200_E_MODEL from the call in HOST mode; in DEVICE mode that block is
+ * coded with an empty model and rb200_sync returns RB200_E_SYMBOL.  A symbol of frequency 0 is RB200_E_SYMBOL; a decode
+ * table that does not sum, or a corrupt stream, is RB200_E_STREAM. */
+int rb200_blocks_coder_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
+                              uint32_t block_size, const uint16_t* block_freqs, uint32_t chunk_syms,
+                              uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind);
+int rb200_blocks_coder_model_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
+                                    uint32_t block_size, uint16_t* block_freqs, uint32_t chunk_syms,
+                                    uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind);
+int rb200_blocks_coder_decode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* blob, size_t blob_size,
+                              const uint64_t* offsets, const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size,
+                              uint32_t chunk_syms, uint8_t* out, int mem_kind);
+
+/* Their container, version 3: version 2's layout (rb200_container_blocks_size gives its size) with the header's own
+ * coder (byte 6: RB200_CODER_BYTE or RB200_CODER_RANS64) and scale_bits (byte 7: 8..15); every block's frequencies sum
+ * to 1 << scale_bits, and every other rule is version 2's.  The _coder_ calls accept only version 3, the other container
+ * calls reject it.  pack: host only; RB200_E_ARG for a bad coder or scale_bits and as rb200_container_blocks_pack,
+ * RB200_E_MODEL for a block that does not sum.  open: as rb200_container_blocks_open, with coder and scale_bits.
+ * encode: block_freqs == NULL builds the models on the GPU straight into the model section; otherwise the rules of
+ * rb200_container_blocks_encode with the total 1 << scale_bits.  decode: the rules of rb200_container_blocks_decode. */
+typedef struct rb200_container_blocks_coder_info {
+    uint32_t coder, scale_bits;
+    uint32_t n_blocks, block_size, chunk_syms, flags;
+    uint64_t n_symbols, n_chunks, blob_bytes;
+    const uint16_t* block_freqs;    /* n_blocks x 256 */
+    const uint64_t* offsets;        /* n_chunks + 1 */
+    const uint8_t* blob;
+} rb200_container_blocks_coder_info;
+
+int rb200_container_blocks_coder_pack(int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                      const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes,
+                                      uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size);
+int rb200_container_blocks_coder_open(const uint8_t* buf, size_t size, rb200_container_blocks_coder_info* info);
+int rb200_container_blocks_coder_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
+                                        uint32_t block_size, const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags,
+                                        uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind);
+int rb200_container_blocks_coder_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                        uint64_t* n_symbols, int mem_kind);
+
 /* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
  * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's
  * decode table is built on the GPU into the context, and the decoder the header calls for is picked on the GPU -- all

@@ -172,10 +172,11 @@ struct BlockModelSmem {
     uint32_t cum[257];
 };
 
-// count_freqs + calc_cum_freqs + normalize_freqs(4096) (main.cpp:59-129) of one block by the whole CTA, bit-exact.
+// count_freqs + calc_cum_freqs + normalize_freqs(target) (main.cpp:59-129) of one block by the whole CTA, bit-exact.
 // The CTA must call it convergently; on return (after a CTA barrier) dst[0..256) holds the normalised frequencies.
+// target <= 32768 (the frequencies are u16); the word coder's callers pass the constant 4096.
 __device__ __forceinline__ void block_model_build(const uint8_t* __restrict__ blk, uint32_t block_size, BlockModelSmem& sm,
-                                                  uint16_t* __restrict__ dst, uint32_t* __restrict__ status)
+                                                  uint16_t* __restrict__ dst, uint32_t* __restrict__ status, uint32_t target)
 {
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     for (uint32_t i = tid; i < kModelWarps * 256; i += blockDim.x) (&sm.h[0][0])[i] = 0;
@@ -207,16 +208,16 @@ __device__ __forceinline__ void block_model_build(const uint8_t* __restrict__ bl
         sm.cnt[s] = t;
     }
     __syncthreads();
-    if (warp == 0) block_normalize(sm.cnt, sm.cum, sm.h[0], dst, kWordSlots, kStatStream, status);      // h[0] is reused for the 256 widths
+    if (warp == 0) block_normalize(sm.cnt, sm.cum, sm.h[0], dst, target, kStatStream, status);      // h[0] is reused for the 256 widths
     __syncthreads();
 }
 
 // The same with the bank-private histogram of histogram_kernel (one copy per lane, 32 KiB at `hist`): no bank
 // conflicts and no hot-counter serialisation.  Used by the fused per-block encoder, where the 32 KiB are the (not yet
-// built) encoder table.  s_cnt / s_cum / s_w: 256 / 257 / 256 words.
+// built) encoder table.  s_cnt / s_cum / s_w: 256 / 257 / 256 words.  target as for block_model_build.
 __device__ __forceinline__ void block_model_build_wide(const uint8_t* __restrict__ blk, uint32_t block_size, uint32_t* hist, uint32_t* s_cnt,
                                                        uint32_t* s_cum, uint32_t* s_w, uint16_t* __restrict__ dst,
-                                                       uint32_t* __restrict__ status)
+                                                       uint32_t* __restrict__ status, uint32_t target)
 {
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     for (uint32_t i = tid; i < 256 * 32; i += blockDim.x) hist[i] = 0;
@@ -248,7 +249,7 @@ __device__ __forceinline__ void block_model_build_wide(const uint8_t* __restrict
         s_cnt[s] = t;
     }
     __syncthreads();
-    if (warp == 0) block_normalize(s_cnt, s_cum, s_w, dst, kWordSlots, kStatStream, status);
+    if (warp == 0) block_normalize(s_cnt, s_cum, s_w, dst, target, kStatStream, status);
     __syncthreads();
 }
 
@@ -260,7 +261,7 @@ block_model_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t
     __shared__ uint32_t s_cnt[256], s_cum[257];
     __shared__ __align__(16) uint32_t s_w[256];      // block_normalize reads it 16 bytes at a time
     block_model_build_wide(in + static_cast<uint64_t>(blockIdx.x) * block_size, block_size, s_hist, s_cnt, s_cum, s_w,
-                           block_freqs + static_cast<uint64_t>(blockIdx.x) * 256, status);
+                           block_freqs + static_cast<uint64_t>(blockIdx.x) * 256, status, kWordSlots);
 }
 
 inline void launch_block_models(cudaStream_t stream, const uint8_t* d_in, uint32_t n_blocks, uint32_t block_size,
@@ -275,9 +276,9 @@ inline void launch_block_models(cudaStream_t stream, const uint8_t* d_in, uint32
 constexpr int kMaxBlockWarps = 32;
 
 // cum[s] for the block's frequencies (u16 from global memory, or the u32 widths the model build left in shared
-// memory); returns false if they do not sum to 4096
+// memory); returns false if they do not sum to target (the word coder's callers pass the constant 4096)
 template <class F>
-__device__ __forceinline__ bool block_prefix(const F* freqs, uint32_t* s_cum, uint32_t* s_bad)
+__device__ __forceinline__ bool block_prefix(const F* freqs, uint32_t* s_cum, uint32_t* s_bad, uint32_t target)
 {
     const uint32_t tid = threadIdx.x, lane = tid & 31;
     if (tid == 0) *s_bad = 0;
@@ -295,7 +296,7 @@ __device__ __forceinline__ bool block_prefix(const F* freqs, uint32_t* s_cum, ui
         for (int j = 0; j < 8; j++) s_cum[8 * lane + j] = incl - run + local[j];
         if (lane == 31) {
             s_cum[256] = incl;
-            if (incl != kWordSlots) *s_bad = 1;
+            if (incl != target) *s_bad = 1;
         }
     }
     __syncthreads();
@@ -336,7 +337,7 @@ block_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const 
     const uint32_t tid = threadIdx.x, warp = tid >> 5;
     const uint16_t* freqs = block_freqs + static_cast<uint64_t>(blockIdx.x) * 256;
     if (tid == 0) s_flag[1] = 0;
-    const bool ok = block_prefix(freqs, s_cum, &s_flag[0]);
+    const bool ok = block_prefix(freqs, s_cum, &s_flag[0], kWordSlots);
     if (!ok) {
         if (tid == 0) atomicOr(status, kStatStream);
         return;
@@ -410,7 +411,7 @@ block_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, const u
     const uint32_t warp = threadIdx.x >> 5;
     const uint16_t* freqs = block_freqs + static_cast<uint64_t>(blockIdx.x) * 256;
     const uint32_t per_block = block_size / chunk_syms;
-    const bool ok = block_prefix(freqs, s_cum, &s_flag[0]);
+    const bool ok = block_prefix(freqs, s_cum, &s_flag[0], kWordSlots);
     const bool r32 = block_build_enc_table(s_cum, ok, s_tab);
     if (warp >= per_block) return;
     const uint32_t chunk = blockIdx.x * per_block + warp;
@@ -465,10 +466,10 @@ block_encode_fused_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uin
         uint16_t* freqs = block_freqs + static_cast<uint64_t>(block) * 256;
         bool ok;
         if (BUILD) {
-            block_model_build_wide(blk, block_size, reinterpret_cast<uint32_t*>(s_enc), s_cnt, s_cum, s_w, freqs, status);
-            ok = block_prefix(s_w, s_cum, &s_flag[0]);                // the widths are still in shared memory
+            block_model_build_wide(blk, block_size, reinterpret_cast<uint32_t*>(s_enc), s_cnt, s_cum, s_w, freqs, status, kWordSlots);
+            ok = block_prefix(s_w, s_cum, &s_flag[0], kWordSlots);    // the widths are still in shared memory
         } else {
-            ok = block_prefix(static_cast<const uint16_t*>(freqs), s_cum, &s_flag[0]);
+            ok = block_prefix(static_cast<const uint16_t*>(freqs), s_cum, &s_flag[0], kWordSlots);
         }
         const bool r32 = block_build_enc_table(s_cum, ok, s_tab);
         if (warp < per_block) {

@@ -316,7 +316,7 @@ __global__ void __launch_bounds__(kPlannedWarps * 32, 8)
             __syncthreads();
             const uint32_t block = s_block;
             if (block >= n_blocks) break;
-            if (!block_prefix(models + static_cast<uint64_t>(block) * 256, s_cum, &s_flag[0])) {   // checked before: not reached
+            if (!block_prefix(models + static_cast<uint64_t>(block) * 256, s_cum, &s_flag[0], kWordSlots)) {   // checked before: not reached
                 if (tid == 0) atomicOr(status, kStatStream);
                 continue;
             }

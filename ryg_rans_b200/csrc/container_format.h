@@ -16,6 +16,7 @@ namespace rb200 {
 constexpr uint32_t kContainerMagic = 0x43324252u;   // "RB2C"
 constexpr uint16_t kContainerVersion = 1;           // one model: 256 x u32
 constexpr uint16_t kContainerVersionBlocks = 2;     // one model per block: n_blocks x 256 x u16, word coder
+constexpr uint16_t kContainerVersionBlocksCoder = 3;  // version 2's layout with the byte or rans64 coder at scale_bits 8..15
 
 struct ContainerHeader {        // 64 bytes
     uint32_t magic;
@@ -30,9 +31,9 @@ struct ContainerHeader {        // 64 bytes
     uint32_t flags;
     uint32_t meta_crc;          // header (crc fields zero) + model + offsets
     uint32_t blob_crc;          // valid when flags & RB200_CONTAINER_CRC_BLOB
-    uint32_t block_size;        // version 2: symbols per block (version 1: zero, not checked)
-    uint32_t n_blocks;          // version 2: blocks, >= 1 (version 1: zero, not checked)
-    uint32_t reserved;          // version 2: zero
+    uint32_t block_size;        // versions 2, 3: symbols per block (version 1: zero, not checked)
+    uint32_t n_blocks;          // versions 2, 3: blocks, >= 1 (version 1: zero, not checked)
+    uint32_t reserved;          // versions 2, 3: zero
 };
 static_assert(sizeof(ContainerHeader) == 64, "container header must stay 64 bytes");
 
@@ -49,6 +50,25 @@ RB200_HD inline uint64_t container_model_bytes(const ContainerHeader& h)
 RB200_HD inline uint64_t container_dir_offset(const ContainerHeader& h) { return sizeof(ContainerHeader) + container_model_bytes(h); }
 RB200_HD inline uint64_t container_dir_end(const ContainerHeader& h) { return container_dir_offset(h) + (h.n_chunks + 1) * sizeof(uint64_t); }
 RB200_HD inline uint64_t container_blob_offset(const ContainerHeader& h) { return (container_dir_end(h) + 15) & ~15ull; }
+
+// Version 3 is version 2 with the header's own coder (byte or rans64) and scale_bits (8..15): the same layout, and every
+// rule of version 2 but the coder, scale_bits and the block total.  The layout functions above and container_header_ok
+// serve versions 1 and 2 (the kernels of container_decode.cuh call them); the host reads a version 3 header through
+// its version 2 shape.
+RB200_HD inline bool container_blocks_coder_ok(uint32_t coder, uint32_t scale_bits)
+{
+    return (coder == RB200_CODER_BYTE || coder == RB200_CODER_RANS64) && scale_bits >= 8 && scale_bits <= 15;
+}
+// the header the layout functions and version 2's rules read for h: h itself, or for version 3 its version 2 shape
+inline ContainerHeader container_layout(ContainerHeader h)
+{
+    if (h.version == kContainerVersionBlocksCoder) {
+        h.version = kContainerVersionBlocks;
+        h.coder = RB200_CODER_WORD;
+        h.scale_bits = 12;
+    }
+    return h;
+}
 
 // a header with only what the layout depends on: for sizes computed before there is a header
 inline ContainerHeader container_shape(uint16_t version, uint32_t n_blocks, uint64_t n_chunks)
@@ -115,13 +135,15 @@ RB200_HD inline bool container_model_decodable(uint32_t coder, const uint32_t* f
 }
 
 // The per-element rules of a version 2 prefix, one block or one directory entry at a time.
-// one block's 256 frequencies sum to 4096
-RB200_HD inline bool container_block_model_ok(const uint16_t* freqs)
+// one block's 256 frequencies sum to total (version 3: 1 << scale_bits)
+RB200_HD inline bool container_block_model_sums_to(const uint16_t* freqs, uint32_t total)
 {
     uint32_t sum = 0;
     for (int s = 0; s < 256; s++) sum += freqs[s];
-    return sum == 4096;
+    return sum == total;
 }
+// one block's 256 frequencies sum to 4096
+RB200_HD inline bool container_block_model_ok(const uint16_t* freqs) { return container_block_model_sums_to(freqs, 4096); }
 // entry c (< n_chunks) of the directory is not above the next one
 RB200_HD inline bool container_dir_step_ok(const uint64_t* offsets, uint64_t c) { return offsets[c] <= offsets[c + 1]; }
 // the first stream starts inside the first vector, the last entry is the blob size
@@ -135,8 +157,13 @@ ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_
                                  uint64_t blob_bytes, uint32_t flags);
 // the header rb200_container_blocks_pack writes (crc fields zero)
 ContainerHeader container_blocks_header(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint64_t blob_bytes, uint32_t flags);
+// the header rb200_container_blocks_coder_pack writes (crc fields zero)
+ContainerHeader container_blocks_coder_header(int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                              uint64_t blob_bytes, uint32_t flags);
 // every block's 256 frequencies sum to 4096
 bool container_block_models_ok(const uint16_t* block_freqs, uint32_t n_blocks);
+// every block's 256 frequencies sum to total
+bool container_block_models_sum_to(const uint16_t* block_freqs, uint32_t n_blocks, uint32_t total);
 // the directory rules: the first stream starts inside the first vector, monotone, last entry == blob_bytes
 bool container_directory_ok(const uint64_t* offsets, uint64_t n_chunks, uint64_t blob_bytes);
 // zlib crc32 on the host (slicing-by-8)
@@ -149,7 +176,8 @@ uint32_t container_meta_crc(const ContainerHeader& h, const void* model, const u
 // The parser, in the order rb200_container_open applies it.  Each step returns RB200_OK or RB200_E_STREAM; the CRC
 // values are the caller's, computed wherever the bytes live.
 //  1. the 64-byte header against the buffer size (`size` bytes in all; `hdr` holds at least 64 of them); `version`
-//     is the one the caller accepts (kContainerVersion or kContainerVersionBlocks), any other is rejected
+//     is the one the caller accepts (kContainerVersion, kContainerVersionBlocks or kContainerVersionBlocksCoder), any
+//     other is rejected
 int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, ContainerHeader* h);
 //  2. header + model + directory (`prefix`: container_blob_offset(h) bytes), given their CRC
 int container_check_prefix(const ContainerHeader& h, const uint8_t* prefix, uint32_t meta_crc);

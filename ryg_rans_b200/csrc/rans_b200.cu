@@ -17,6 +17,7 @@
 #include <string>
 
 #include "alias_kernels.cuh"
+#include "block_coder_kernels.cuh"
 #include "block_kernels.cuh"
 #include "container_decode.cuh"
 #include "container_format.h"
@@ -245,6 +246,7 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     configure_word_kernels();
     configure_alias_kernels();
     configure_block_kernels();
+    configure_block_coder_kernels();
     configure_rans64_kernels();
     configure_crc_kernels();
     ctx->blocks_async = configure_container_decode(static_cast<uint32_t>(ctx->sms));
@@ -1194,15 +1196,16 @@ namespace {
 
 constexpr size_t kBlockFreqBytes = 256 * sizeof(uint16_t);     // one block's frequency table
 
-// The plan of a per-block encode over n_blocks blocks (n_blocks x block_size / chunk_syms < 2^31 chunks): the fused
-// kernel (CTA 0 the scanner, then as many worker CTAs as are resident at once, at most one per block) whenever it builds
-// the models, or the split sequence (one CTA per block) when use_fused_encode says so.
-EncodePlan plan_blocks_encode(const rb200_ctx* ctx, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, bool build)
+// The plan of a per-block encode over n_blocks blocks (n_blocks x block_size / chunk_syms < 2^31 chunks).  The word
+// coder: the fused kernel (CTA 0 the scanner, then as many worker CTAs as are resident at once, at most one per block)
+// whenever it builds the models, or the split sequence (one CTA per block) when use_fused_encode says so.  The byte and
+// rans64 coders: the split sequence (block_coder_encode_kernel), in slots of the same worst case as plan_encode's.
+EncodePlan plan_blocks_encode(const rb200_ctx* ctx, int coder, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, bool build)
 {
     EncodePlan p = {};
     p.n_chunks = n_blocks * (block_size / chunk_syms);
     p.slot_bytes = slot_bytes_for(chunk_syms);
-    p.fused = build || use_fused_encode(chunk_syms);
+    p.fused = coder == RB200_CODER_WORD && (build || use_fused_encode(chunk_syms));
     p.threads = block_threads(block_size, chunk_syms);
     p.smem = block_encode_smem(p.threads);
     if (!p.fused) {
@@ -1218,15 +1221,21 @@ EncodePlan plan_blocks_encode(const rb200_ctx* ctx, uint32_t n_blocks, uint32_t 
     return p;
 }
 
-// Per-block encode.  Default: ONE persistent launch (block_encode_fused_kernel: [model,] tables, encode, directory,
-// placement); build_models makes the kernel run count_freqs + normalize_freqs per block first and write d_freqs.
-// RB200_ENCODE_PATH=split keeps the round-1 sequence (encode into per-chunk slots, tile scan, compaction).
-int blocks_encode_device(rb200_ctx* ctx, const uint8_t* d_in, uint32_t n_blocks, uint32_t block_size, uint16_t* d_freqs,
-                         bool build_models, uint32_t chunk_syms, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets)
+// Per-block encode.  The word coder (scale_bits 12), default: ONE persistent launch (block_encode_fused_kernel: [model,]
+// tables, encode, directory, placement); build_models makes the kernel run count_freqs + normalize_freqs per block first
+// and write d_freqs.  RB200_ENCODE_PATH=split keeps the round-1 sequence (encode into per-chunk slots, tile scan,
+// compaction), which the byte and rans64 coders always run (block_coder_encode_kernel, models of 1 << sb).
+int blocks_encode_device(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* d_in, uint32_t n_blocks, uint32_t block_size,
+                         uint16_t* d_freqs, bool build_models, uint32_t chunk_syms, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets)
 {
     if (static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) >= (1ull << 31)) return RB200_E_ARG;
-    const EncodePlan p = plan_blocks_encode(ctx, n_blocks, block_size, chunk_syms, build_models);
+    const EncodePlan p = plan_blocks_encode(ctx, coder, n_blocks, block_size, chunk_syms, build_models);
     return run_encode(ctx, p, d_blob, blob_cap, d_offsets, [&](const EncodeWorkspace& ws) {
+        if (coder != RB200_CODER_WORD) {
+            launch_block_coder_encode(ctx->stream, static_cast<uint32_t>(coder), sb, build_models, p.grid, p.threads, p.smem, d_in, block_size,
+                                      d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status);
+            return check_launch(ctx, "block_coder_encode_kernel");
+        }
         if (p.fused) {
             block_encode_fused_for(build_models, p.threads)<<<p.grid, p.threads, p.smem, ctx->stream>>>(
                 d_in, n_blocks, block_size, d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.look, ws.counter, d_blob, blob_cap, d_offsets,
@@ -1242,72 +1251,65 @@ int blocks_encode_device(rb200_ctx* ctx, const uint8_t* d_in, uint32_t n_blocks,
 // Host mode runs the slice pipeline over whole blocks; the frequency tables go in with each slice when the caller supplies
 // them, and come back with it when the kernel builds them.  `hook` as in encode_pipeline.
 template <class Hook = NoSliceHook>
-int blocks_encode_host(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint16_t* block_freqs, bool build,
-                       uint32_t chunk_syms, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size, Hook hook = Hook{})
+int blocks_encode_host(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                       uint16_t* block_freqs, bool build, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap, uint64_t* offsets,
+                       size_t* blob_size, Hook hook = Hook{})
 {
     const UnitTable freqs = build ? UnitTable{nullptr, block_freqs, kBlockFreqBytes} : UnitTable{block_freqs, nullptr, kBlockFreqBytes};
     return encode_pipeline(
         ctx, in, static_cast<size_t>(n_blocks) * block_size, chunk_syms, block_size / chunk_syms, freqs,
-        [&](const Slice& s) { return plan_blocks_encode(ctx, static_cast<uint32_t>(s.units), block_size, chunk_syms, build); },
+        [&](const Slice& s) { return plan_blocks_encode(ctx, coder, static_cast<uint32_t>(s.units), block_size, chunk_syms, build); },
         [&](const Slice& s, const uint8_t* d_in, uint8_t* d_freqs, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
-            return blocks_encode_device(ctx, d_in, static_cast<uint32_t>(s.units), block_size, reinterpret_cast<uint16_t*>(d_freqs),
+            return blocks_encode_device(ctx, coder, sb, d_in, static_cast<uint32_t>(s.units), block_size, reinterpret_cast<uint16_t*>(d_freqs),
                                         build, chunk_syms, d_blob, cap, d_off);
         },
         blob, blob_cap, offsets, blob_size, hook);
 }
 
-int blocks_encode_entry(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint16_t* block_freqs, bool build,
-                        uint32_t chunk_syms, uint8_t* blob, size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind)
+int blocks_encode_entry(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                        uint16_t* block_freqs, bool build, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap, uint64_t* offsets,
+                        size_t* blob_size, int mem_kind)
 {
     if (!ctx || !in || !block_freqs || !blob || !offsets || !container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
     return by_mem_kind(
         mem_kind, blob, offsets,
-        [&] { return blocks_encode_device(ctx, in, n_blocks, block_size, block_freqs, build, chunk_syms, blob, blob_cap, offsets); },
-        [&] { return blocks_encode_host(ctx, in, n_blocks, block_size, block_freqs, build, chunk_syms, blob, blob_cap, offsets, blob_size); });
+        [&] { return blocks_encode_device(ctx, coder, sb, in, n_blocks, block_size, block_freqs, build, chunk_syms, blob, blob_cap, offsets); },
+        [&] {
+            return blocks_encode_host(ctx, coder, sb, in, n_blocks, block_size, block_freqs, build, chunk_syms, blob, blob_cap, offsets,
+                                      blob_size);
+        });
 }
 
-int blocks_decode_device(rb200_ctx* ctx, const uint8_t* d_blob, size_t blob_size, const uint64_t* d_off, const uint16_t* d_freqs,
-                         uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint8_t* d_out)
+int blocks_decode_device(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* d_blob, size_t blob_size, const uint64_t* d_off,
+                         const uint16_t* d_freqs, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint8_t* d_out)
 {
+    if (coder != RB200_CODER_WORD) {
+        launch_block_coder_decode(ctx->stream, static_cast<uint32_t>(coder), sb, d_blob, blob_size, d_off, d_freqs, n_blocks, block_size,
+                                  chunk_syms, d_out, ctx->d_status);
+        return check_launch(ctx, "block_coder_decode_kernel");
+    }
     launch_block_decode(ctx->stream, d_blob, blob_size, d_off, d_freqs, n_blocks, block_size, chunk_syms, d_out, ctx->d_status);
     return check_launch(ctx, "block_decode_kernel");
 }
 
 // the host-buffer form of rb200_blocks_decode: the slice pipeline over whole blocks, each slice's tables copied in with it
 template <class Hook = NoSliceHook>
-int blocks_decode_host(rb200_ctx* ctx, const uint8_t* blob, size_t blob_size, const uint64_t* offsets, const uint16_t* block_freqs,
-                       uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint8_t* out, Hook hook = Hook{})
+int blocks_decode_host(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* blob, size_t blob_size, const uint64_t* offsets,
+                       const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint8_t* out,
+                       Hook hook = Hook{})
 {
     return decode_pipeline(
         ctx, blob, blob_size, offsets, chunk_syms, block_size / chunk_syms, UnitTable{block_freqs, nullptr, kBlockFreqBytes},
         [&](const Slice& s, const uint8_t* d_blob, const uint64_t* d_off, uint8_t* d_freqs, uint8_t* d_out) {
-            return blocks_decode_device(ctx, d_blob, blob_size, d_off, reinterpret_cast<const uint16_t*>(d_freqs),
+            return blocks_decode_device(ctx, coder, sb, d_blob, blob_size, d_off, reinterpret_cast<const uint16_t*>(d_freqs),
                                         static_cast<uint32_t>(s.units), block_size, chunk_syms, d_out);
         },
         out, static_cast<size_t>(n_blocks) * block_size, hook);
 }
 
-}  // namespace
-
-extern "C" int rb200_blocks_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
-                                   const uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap,
-                                   uint64_t* offsets, size_t* blob_size, int mem_kind)
-{
-    return blocks_encode_entry(ctx, in, n_blocks, block_size, const_cast<uint16_t*>(block_freqs), false, chunk_syms, blob, blob_cap, offsets,
-                               blob_size, mem_kind);
-}
-
-extern "C" int rb200_blocks_model_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
-                                         uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap,
-                                         uint64_t* offsets, size_t* blob_size, int mem_kind)
-{
-    return blocks_encode_entry(ctx, in, n_blocks, block_size, block_freqs, true, chunk_syms, blob, blob_cap, offsets, blob_size, mem_kind);
-}
-
-extern "C" int rb200_blocks_decode(rb200_ctx* ctx, const uint8_t* blob, size_t blob_size, const uint64_t* offsets,
-                                   const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
-                                   uint8_t* out, int mem_kind)
+int blocks_decode_entry(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* blob, size_t blob_size, const uint64_t* offsets,
+                        const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint8_t* out, int mem_kind)
 {
     if (!ctx || !blob || !offsets || !block_freqs || !out || !container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
     if (!blob_size_ok(blob_size)) return RB200_E_ARG;
@@ -1316,8 +1318,76 @@ extern "C" int rb200_blocks_decode(rb200_ctx* ctx, const uint8_t* blob, size_t b
     if (static_cast<uint64_t>(n_blocks) * per_block >= (1ull << 31)) return RB200_E_ARG;
     return by_mem_kind(
         mem_kind, blob, offsets,
-        [&] { return blocks_decode_device(ctx, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out); },
-        [&] { return blocks_decode_host(ctx, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out); });
+        [&] { return blocks_decode_device(ctx, coder, sb, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out); },
+        [&] { return blocks_decode_host(ctx, coder, sb, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out); });
+}
+
+// The byte / rans64 per-block calls' own checks before the shared entries: the coder, scale_bits 8..15 and fewer than
+// 2^31 chunks (RB200_E_ARG, nothing launched); a HOST-mode caller table that does not sum to 1 << sb (RB200_E_MODEL).
+int blocks_coder_args(int coder, uint32_t sb, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, const uint16_t* caller_freqs,
+                      int mem_kind)
+{
+    if (coder < 0 || !container_blocks_coder_ok(static_cast<uint32_t>(coder), sb)) return RB200_E_ARG;
+    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
+    if (static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) >= (1ull << 31)) return RB200_E_ARG;
+    if (caller_freqs && mem_kind == RB200_MEM_HOST && !container_block_models_sum_to(caller_freqs, n_blocks, 1u << sb)) return RB200_E_MODEL;
+    return RB200_OK;
+}
+
+}  // namespace
+
+extern "C" int rb200_blocks_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                                   const uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap,
+                                   uint64_t* offsets, size_t* blob_size, int mem_kind)
+{
+    return blocks_encode_entry(ctx, RB200_CODER_WORD, 12, in, n_blocks, block_size, const_cast<uint16_t*>(block_freqs), false, chunk_syms,
+                               blob, blob_cap, offsets, blob_size, mem_kind);
+}
+
+extern "C" int rb200_blocks_model_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                                         uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap,
+                                         uint64_t* offsets, size_t* blob_size, int mem_kind)
+{
+    return blocks_encode_entry(ctx, RB200_CODER_WORD, 12, in, n_blocks, block_size, block_freqs, true, chunk_syms, blob, blob_cap, offsets,
+                               blob_size, mem_kind);
+}
+
+extern "C" int rb200_blocks_decode(rb200_ctx* ctx, const uint8_t* blob, size_t blob_size, const uint64_t* offsets,
+                                   const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                   uint8_t* out, int mem_kind)
+{
+    return blocks_decode_entry(ctx, RB200_CODER_WORD, 12, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out,
+                               mem_kind);
+}
+
+extern "C" int rb200_blocks_coder_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
+                                         uint32_t block_size, const uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob,
+                                         size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind)
+{
+    if (!block_freqs) return RB200_E_ARG;
+    const int rc = blocks_coder_args(coder, scale_bits, n_blocks, block_size, chunk_syms, block_freqs, mem_kind);
+    if (rc != RB200_OK) return rc;
+    return blocks_encode_entry(ctx, coder, scale_bits, in, n_blocks, block_size, const_cast<uint16_t*>(block_freqs), false, chunk_syms,
+                               blob, blob_cap, offsets, blob_size, mem_kind);
+}
+
+extern "C" int rb200_blocks_coder_model_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
+                                               uint32_t block_size, uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob,
+                                               size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind)
+{
+    const int rc = blocks_coder_args(coder, scale_bits, n_blocks, block_size, chunk_syms, nullptr, mem_kind);
+    if (rc != RB200_OK) return rc;
+    return blocks_encode_entry(ctx, coder, scale_bits, in, n_blocks, block_size, block_freqs, true, chunk_syms, blob, blob_cap, offsets,
+                               blob_size, mem_kind);
+}
+
+extern "C" int rb200_blocks_coder_decode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* blob, size_t blob_size,
+                                         const uint64_t* offsets, const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size,
+                                         uint32_t chunk_syms, uint8_t* out, int mem_kind)
+{
+    const int rc = blocks_coder_args(coder, scale_bits, n_blocks, block_size, chunk_syms, nullptr, mem_kind);
+    if (rc != RB200_OK) return rc;
+    return blocks_decode_entry(ctx, coder, scale_bits, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out, mem_kind);
 }
 
 // ---------------------------------------------------------------------------
@@ -1374,10 +1444,11 @@ struct SliceCrc {
     }
 };
 
-// rb200_container_decode / rb200_container_blocks_decode once the buffers are checked: header, model and directory
-// validated by the shared parser for `version`, then the blob CRC, then the decode (a model and rb200_decode's kernels
-// for version 1, the per-block decoder reading its tables in place for version 2).  DEVICE: the prefix is read through
-// pinned memory, both CRCs are taken on the GPU, and nothing is decoded unless every check passes.
+// rb200_container_decode / rb200_container_blocks_decode / rb200_container_blocks_coder_decode once the buffers are
+// checked: header, model and directory validated by the shared parser for `version`, then the blob CRC, then the decode
+// (a model and rb200_decode's kernels for version 1, the per-block decoder of the header's coder reading its tables in
+// place for versions 2 and 3).  DEVICE: the prefix is read through pinned memory, both CRCs are taken on the GPU, and
+// nothing is decoded unless every check passes.
 int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap, uint64_t* n_symbols,
                           bool device, uint16_t version)
 {
@@ -1392,10 +1463,10 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
         RB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         rc = container_parse_header(reinterpret_cast<const uint8_t*>(ctx->h_dir), size, version, &h);
         if (rc != RB200_OK) return rc;
-        const size_t boff = container_blob_offset(h);
+        const size_t boff = container_blob_offset(container_layout(h));
         rc = reserve_dir(ctx, boff / sizeof(uint64_t));
         if (rc != RB200_OK) return rc;
-        const uint64_t covered = container_dir_end(h) - sizeof(ContainerHeader);     // model and directory: what the CRC covers after the header
+        const uint64_t covered = container_dir_end(container_layout(h)) - sizeof(ContainerHeader);     // model and directory: what the CRC covers after the header
         RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir, buf, boff, cudaMemcpyDeviceToHost, ctx->stream));
         rc = launch_crc(ctx, buf + sizeof(ContainerHeader), covered, nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK) rc = fetch_crc(ctx, 1);
@@ -1406,15 +1477,15 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
         rc = container_parse_header(buf, size, version, &h);
         if (rc == RB200_OK)
             rc = container_check_prefix(h, buf, container_meta_crc(h, buf + sizeof(ContainerHeader),
-                                                                   reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h))));
+                                                                   reinterpret_cast<const uint64_t*>(buf + container_dir_offset(container_layout(h)))));
     }
     if (rc != RB200_OK) return rc;
     if (n_symbols) *n_symbols = h.n_symbols;
     if (out_cap < h.n_symbols) return RB200_E_SPACE;
     if (h.n_symbols && !out) return RB200_E_ARG;
     if (!container_geometry_decodable(h.chunk_syms, h.blob_bytes)) return RB200_E_ARG;  // what rb200_decode accepts
-    const uint8_t* blob = buf + container_blob_offset(h);
-    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h));
+    const uint8_t* blob = buf + container_blob_offset(container_layout(h));
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(container_layout(h)));
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
     if (device && blob_crc) {
         rc = launch_crc(ctx, blob, h.blob_bytes, nullptr, 0, ctx->d_crc);
@@ -1436,12 +1507,16 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
         if (r == RB200_OK) r = container_check_blob(h, crc);
         return r;
     };
-    if (version == kContainerVersionBlocks) {
+    if (version != kContainerVersion) {       // per-block models: the word coder at 12 (version 2), byte / rans64 (version 3)
         const uint16_t* block_freqs = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));     // read in place
         return decode(
-            [&] { return blocks_decode_device(ctx, blob, h.blob_bytes, offsets, block_freqs, h.n_blocks, h.block_size, h.chunk_syms, out); },
+            [&] {
+                return blocks_decode_device(ctx, h.coder, h.scale_bits, blob, h.blob_bytes, offsets, block_freqs, h.n_blocks, h.block_size,
+                                            h.chunk_syms, out);
+            },
             [&](SliceCrc hook) {
-                return blocks_decode_host(ctx, blob, h.blob_bytes, offsets, block_freqs, h.n_blocks, h.block_size, h.chunk_syms, out, hook);
+                return blocks_decode_host(ctx, h.coder, h.scale_bits, blob, h.blob_bytes, offsets, block_freqs, h.n_blocks, h.block_size,
+                                          h.chunk_syms, out, hook);
             });
     }
     const uint32_t* freqs = reinterpret_cast<const uint32_t*>(prefix + sizeof(ContainerHeader));
@@ -1527,21 +1602,21 @@ extern "C" int rb200_container_decode(rb200_ctx* ctx, const uint8_t* buf, size_t
     return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, mem_kind == RB200_MEM_DEVICE, kContainerVersion);
 }
 
-// The per-block container: the block encoder writes every block's model (built, or the caller's tables copied in
-// first), the directory and the blob straight into their place in `out`; then as rb200_container_encode, except that
-// one CRC launch covers model and directory, which are contiguous.
-extern "C" int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
-                                             const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap,
-                                             size_t* out_size, int mem_kind)
+namespace {
+
+// The per-block containers (version 2: the word coder at 12; version 3: byte / rans64): the block encoder writes every
+// block's model (built, or the caller's tables copied in first), the directory and the blob straight into their place
+// in `out`; then as rb200_container_encode, except that one CRC launch covers model and directory, which are contiguous.
+// Arguments are checked by the caller.
+int container_blocks_encode_impl(rb200_ctx* ctx, ContainerHeader h, const uint8_t* in, const uint16_t* block_freqs, uint8_t* out,
+                                 size_t out_cap, size_t* out_size, int mem_kind)
 {
-    if (!ctx || !in || !out || !container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
-    if (!container_mem_ok(mem_kind, out, nullptr)) return RB200_E_ARG;
     const bool device = mem_kind == RB200_MEM_DEVICE, build = block_freqs == nullptr;
-    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
-    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
-    if (!build && !device && !container_block_models_ok(block_freqs, n_blocks)) return RB200_E_MODEL;
-    ContainerHeader h = container_blocks_header(n_blocks, block_size, chunk_syms, 0, flags);
-    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
+    const uint32_t n_blocks = h.n_blocks, block_size = h.block_size, chunk_syms = h.chunk_syms;
+    const uint64_t n_chunks = h.n_chunks;
+    if (!build && !device && !container_block_models_sum_to(block_freqs, n_blocks, 1u << h.scale_bits)) return RB200_E_MODEL;
+    const ContainerHeader l = container_layout(h);
+    const size_t dir_off = container_dir_offset(l), dir_end = container_dir_end(l), boff = container_blob_offset(l);
     if (out_cap < boff) return RB200_E_SPACE;
     DeviceGuard g(ctx->device);
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
@@ -1550,7 +1625,8 @@ extern "C" int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, 
     const size_t model_bytes = dir_off - sizeof(ContainerHeader);
     if (device) {            // asynchronous: model + directory CRC, blob CRC, then the header from blob_bytes = dir[n_chunks]
         if (!build) RB_CUDA(ctx, cudaMemcpyAsync(model, block_freqs, model_bytes, cudaMemcpyDeviceToDevice, ctx->stream));
-        int rc = blocks_encode_device(ctx, in, n_blocks, block_size, model, build, chunk_syms, out + boff, out_cap - boff, dir);
+        int rc = blocks_encode_device(ctx, h.coder, h.scale_bits, in, n_blocks, block_size, model, build, chunk_syms, out + boff, out_cap - boff,
+                                      dir);
         if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
         if (rc != RB200_OK) return rc;
@@ -1559,8 +1635,8 @@ extern "C" int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, 
     }
     if (!build) std::memcpy(model, block_freqs, model_bytes);
     size_t blob_bytes = 0, slices = 0;
-    int rc = blocks_encode_host(ctx, in, n_blocks, block_size, model, build, chunk_syms, out + boff, out_cap - boff, dir, &blob_bytes,
-                                SliceCrc{ctx, blob_crc, &slices});
+    int rc = blocks_encode_host(ctx, h.coder, h.scale_bits, in, n_blocks, block_size, model, build, chunk_syms, out + boff, out_cap - boff,
+                                dir, &blob_bytes, SliceCrc{ctx, blob_crc, &slices});
     if (rc == RB200_OK && blob_crc) rc = joined_slice_crc(ctx, slices, &h.blob_crc);
     if (rc != RB200_OK) return rc;
     h.blob_bytes = blob_bytes;
@@ -1571,6 +1647,32 @@ extern "C" int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, 
     return RB200_OK;
 }
 
+}  // namespace
+
+extern "C" int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                                             const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap,
+                                             size_t* out_size, int mem_kind)
+{
+    if (!ctx || !in || !out || !container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
+    if (!container_mem_ok(mem_kind, out, nullptr)) return RB200_E_ARG;
+    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
+    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    return container_blocks_encode_impl(ctx, container_blocks_header(n_blocks, block_size, chunk_syms, 0, flags), in, block_freqs, out,
+                                        out_cap, out_size, mem_kind);
+}
+
+extern "C" int rb200_container_blocks_coder_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
+                                                   uint32_t block_size, const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags,
+                                                   uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind)
+{
+    if (!ctx || !in || !out || coder < 0 || !container_blocks_coder_ok(static_cast<uint32_t>(coder), scale_bits)) return RB200_E_ARG;
+    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms) || !container_mem_ok(mem_kind, out, nullptr)) return RB200_E_ARG;
+    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
+    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    return container_blocks_encode_impl(ctx, container_blocks_coder_header(coder, scale_bits, n_blocks, block_size, chunk_syms, 0, flags), in,
+                                        block_freqs, out, out_cap, out_size, mem_kind);
+}
+
 extern "C" int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                              uint64_t* n_symbols, int mem_kind)
 {
@@ -1578,6 +1680,15 @@ extern "C" int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf,
     if (!container_mem_ok(mem_kind, buf, out)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
     return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, mem_kind == RB200_MEM_DEVICE, kContainerVersionBlocks);
+}
+
+extern "C" int rb200_container_blocks_coder_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                                   uint64_t* n_symbols, int mem_kind)
+{
+    if (!ctx || !buf || (!out && out_cap)) return RB200_E_ARG;
+    if (!container_mem_ok(mem_kind, buf, out)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, mem_kind == RB200_MEM_DEVICE, kContainerVersionBlocksCoder);
 }
 
 namespace {

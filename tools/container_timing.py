@@ -33,9 +33,19 @@ RB200_CONTAINER_CRC_BLOB, alternated:
   *d_n = n_max = 1 GiB against the fixed async call, and at *d_n = 64 MiB with n_max = 1 GiB against the fixed call at
   64 MiB (the cost of launch shapes sized for n_max), with a torch.profiler list of the varlen call's kernels.
 
+With --blocks-coder, per-block models for the byte and rans64 coders on 8192 blocks of 64 KiB, chunks of 8192, device
+buffers, on two data sets: "skewed" (per block one symbol at p = 0.90..0.99 and a Zipf-1.1 tail over the other 255,
+alphabet permuted per block) and "zipf" (the --blocks data):
+
+  rb200_blocks_coder_model_encode (byte and rans64 at scale_bits 14) against rb200_blocks_model_encode (word), alternated;
+  rb200_blocks_coder_decode against rb200_blocks_decode and against the single-model decoders of the byte and rans64
+  coders (K8 / K9) on the same number of bytes, alternated; the size of each output in bytes per symbol (512 B of model
+  per block included; single models at 1024 B) with byte and rans64 also at scale_bits 15 and every coder's single model
+  from the whole data; and a torch.profiler list of each per-block call's kernels.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
-    python tools/container_timing.py [--blocks | --single | --model] [--reps 10] [--json out.json]"""
+    python tools/container_timing.py [--blocks | --blocks-coder | --single | --model] [--reps 10] [--json out.json]"""
 import argparse
 import json
 import os
@@ -185,6 +195,104 @@ def blocks(args):
         "decode_call_host_ms": {k: stats(v) for k, v in host.items()},
         "checks": {**identical, **decode_ok},
     }
+    ctx.close()
+    return res
+
+
+def skewed_blocks_data(n_blocks, block_size, seed):
+    """per block one symbol at p = 0.90 + 0.01 (b % 10) and a Zipf-1.1 tail over the other 255, alphabet permuted per
+    block, generated on the GPU"""
+    import torch
+    g = torch.Generator(device="cuda")
+    g.manual_seed(seed)
+    tail = 1.0 / torch.arange(1, 256, device="cuda", dtype=torch.float64) ** 1.1
+    tail = tail / tail.sum()
+    probs = torch.stack([torch.cat([torch.tensor([0.90 + 0.01 * e], device="cuda", dtype=torch.float64), (0.10 - 0.01 * e) * tail])
+                         for e in range(10)])
+    out = torch.empty(n_blocks * block_size, dtype=torch.uint8, device="cuda")
+    step = 256
+    for b0 in range(0, n_blocks, step):
+        nb = min(step, n_blocks - b0)
+        p = probs[torch.arange(b0, b0 + nb, device="cuda") % 10]
+        r = torch.multinomial(p, block_size, replacement=True, generator=g)
+        perm = torch.argsort(torch.rand(nb, 256, device="cuda", generator=g), dim=1)
+        out[b0 * block_size:(b0 + nb) * block_size] = torch.gather(perm, 1, r).to(torch.uint8).reshape(-1)
+    return out
+
+
+def blocks_coder(args):
+    import torch
+    n_blocks, block_size, chunk, sb = 8192, 65536, 8192, 14
+    n = n_blocks * block_size
+    n_chunks = n // chunk
+    ctx = rb.Context(0)
+    bound = ctx.encode_bound(n, chunk)
+    sync = ctx.sync
+    res = {"card": card(), "workload": {"n_blocks": n_blocks, "block_size": block_size, "chunk_syms": chunk, "n": n, "scale_bits": sb},
+           "checks": {}}
+    coders = {"byte": rb.CODER_BYTE, "rans64": rb.CODER_RANS64}
+    for name, make in (("skewed", skewed_blocks_data), ("zipf", blocks_data)):
+        d_in = make(n_blocks, block_size, 1234)
+        bufs = {k: (torch.empty(bound + 16, dtype=torch.uint8, device="cuda"), torch.empty(n_chunks + 1, dtype=torch.int64, device="cuda"),
+                    torch.empty(n_blocks * 256, dtype=torch.int16, device="cuda")) for k in ("word", *coders)}
+        d_out = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+
+        def menc(k, s=sb):
+            b, o, f = bufs[k]
+            if k == "word":
+                return lambda: ctx.blocks_model_encode_device(d_in.data_ptr(), n_blocks, block_size, f.data_ptr(), chunk, b.data_ptr(), bound,
+                                                              o.data_ptr())
+            return lambda: ctx.blocks_coder_model_encode_device(coders[k], s, d_in.data_ptr(), n_blocks, block_size, f.data_ptr(), chunk,
+                                                                b.data_ptr(), bound, o.data_ptr())
+        enc = {f"{k}_blocks_model_encode": menc(k) for k in ("byte", "rans64", "word")}
+        etimes = alternate(enc, sync, args.warmup, args.reps)
+        for f in enc.values():
+            f()
+        sync()
+        blob_bytes = {k: int(bufs[k][1][n_chunks].item()) for k in bufs}
+        sizes = {f"{k}_per_block_sb{12 if k == 'word' else sb}": (blob_bytes[k] + 512 * n_blocks) / n for k in bufs}
+
+        def dec_blocks(k):
+            b, o, f = bufs[k]
+            if k == "word":
+                return lambda: ctx.blocks_decode_device(b.data_ptr(), blob_bytes[k], o.data_ptr(), f.data_ptr(), n_blocks, block_size, chunk,
+                                                        d_out.data_ptr())
+            return lambda: ctx.blocks_coder_decode_device(coders[k], sb, b.data_ptr(), blob_bytes[k], o.data_ptr(), f.data_ptr(), n_blocks,
+                                                          block_size, chunk, d_out.data_ptr())
+        dec = {f"{k}_blocks_decode": dec_blocks(k) for k in ("byte", "rans64", "word")}
+        # single models from the whole data (K8 / K9 and the word decoder), on the same bytes
+        single = {}
+        for k, coder, s in (("byte", rb.CODER_BYTE, sb), ("rans64", rb.CODER_RANS64, sb), ("word", rb.CODER_WORD, 12)):
+            m = rb.Model.from_data(ctx, coder, s, device_ptr=d_in.data_ptr(), n=n)
+            b = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+            o = torch.empty(n_chunks + 1, dtype=torch.int64, device="cuda")
+            ctx.encode_device(m, d_in.data_ptr(), n, chunk, b.data_ptr(), bound, o.data_ptr())
+            sync()
+            single[k] = (m, b, o, int(o[n_chunks].item()))
+            sizes[f"{k}_single_model_sb{s}"] = (single[k][3] + 1024) / n
+        for k in ("byte", "rans64"):
+            m, b, o, bb = single[k]
+            dec[f"{k}_single_model_decode"] = (lambda m=m, b=b, o=o, bb=bb:
+                                               ctx.decode_device(m, b.data_ptr(), bb, o.data_ptr(), chunk, d_out.data_ptr(), n))
+        dtimes = alternate(dec, sync, args.warmup, args.reps)
+        for k, f in dec.items():
+            d_out.zero_()
+            f()
+            sync()
+            res["checks"][f"{name}_{k}_equals_input"] = bool(torch.equal(d_out[:n], d_in))
+        for k in coders:                                               # sizes at scale_bits 15
+            menc(k, 15)()
+            sync()
+            sizes[f"{k}_per_block_sb15"] = (int(bufs[k][1][n_chunks].item()) + 512 * n_blocks) / n
+        profile = {k: kernel_times(f, sync, args.reps) for k, f in (("byte_blocks_model_encode", menc("byte")),
+                                                                     ("rans64_blocks_model_encode", menc("rans64")))}
+        for k in ("byte", "rans64"):                                   # the blobs at 14 again for the decode profile
+            menc(k)()
+            sync()
+        profile.update({k: kernel_times(dec[k], sync, args.reps) for k in ("byte_blocks_decode", "rans64_blocks_decode")})
+        for m, *_ in single.values():
+            m.close()
+        res[name] = {"encode": etimes, "decode": dtimes, "bytes_per_symbol": sizes, "kernels": profile}
     ctx.close()
     return res
 
@@ -444,6 +552,7 @@ def model_encode(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
+    ap.add_argument("--blocks-coder", action="store_true", help="per-block models for the byte and rans64 coders, 8192 blocks of 64 KiB")
     ap.add_argument("--single", action="store_true", help="the single-model container's decode calls on three workloads")
     ap.add_argument("--model", action="store_true", help="the single-model container's encode with the model built from the data")
     ap.add_argument("--reps", type=int, default=10)
@@ -452,7 +561,7 @@ def main():
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else single(args) if args.single else model_encode(args) if args.model else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else single(args) if args.single else model_encode(args) if args.model else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
