@@ -278,6 +278,20 @@ int rb200_container_blocks_coder_encode(rb200_ctx* ctx, int coder, uint32_t scal
                                         uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind);
 int rb200_container_blocks_coder_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                         uint64_t* n_symbols, int mem_kind);
+/* rb200_container_blocks_coder_decode(..., RB200_MEM_DEVICE) with nothing done on the host: the header, every block's
+ * model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, and the block decoder of the
+ * header's coder and scale_bits is picked on the GPU -- all enqueued on the context stream.  The rules of
+ * rb200_container_blocks_decode_async apply: DEVICE memory only, buf and out 16-byte aligned, d_n_symbols 8-byte
+ * aligned or NULL; the call never synchronises, copies to or from the host or allocates, so it can be captured in a
+ * CUDA graph, and returns only RB200_E_ARG (nothing launched) or RB200_E_CUDA.  *d_n_symbols receives n once header,
+ * models and directory pass (also when the blob CRC then fails).  rb200_sync gives the verdict: RB200_E_STREAM for
+ * anything rb200_container_blocks_coder_open rejects (version 1 and 2 containers among them), RB200_E_SPACE for
+ * n > out_cap, content errors first; in both cases out is untouched.  A corrupt stream that passes every check is
+ * RB200_E_STREAM, as from rb200_blocks_coder_decode.  One difference from rb200_container_blocks_coder_decode: a
+ * container that open accepts but the decoders refuse (a blob of 2^36 bytes or more), which that call reports as
+ * RB200_E_ARG, is RB200_E_STREAM here, out untouched. */
+int rb200_container_blocks_coder_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                              uint64_t* d_n_symbols);
 
 /* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
  * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's

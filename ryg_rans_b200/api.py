@@ -67,6 +67,7 @@ EXPORTS = [
     ("rb200_container_blocks_coder_encode", C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p,
                                                       C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int]),
     ("rb200_container_blocks_coder_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
+    ("rb200_container_blocks_coder_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_container_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_container_model_encode_async", C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_size_t, C.c_uint32,
                                                      C.c_uint32, C.c_void_p, C.c_size_t]),
@@ -524,6 +525,12 @@ class Context:
         self.lib.check(self.lib.dll.rb200_container_blocks_coder_decode(self.h, buf_ptr, size, out_ptr, out_cap, C.byref(n), MEM_DEVICE),
                        self.h)
         return n.value
+
+    def container_blocks_coder_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
+        """enqueue only (CUDA-graph capturable); n_ptr: device address of a u64 that receives n, or 0.  The verdict on
+        the container (-4 corrupt, -3 out_cap too small, output untouched) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_blocks_coder_decode_async(self.h, buf_ptr, size, out_ptr, out_cap, n_ptr or None),
+                       self.h)
 
     # ---- per-block models of the byte and rans64 coders (scale_bits 8..15)
     def blocks_coder_encode_device(self, coder, scale_bits, in_ptr, n_blocks, block_size, freqs_ptr, chunk_syms, blob_ptr, blob_cap,

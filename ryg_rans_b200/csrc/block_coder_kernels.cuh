@@ -89,22 +89,12 @@ block_coder_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, u
         encode_chunk_split(src, chunk_syms, chunk, Rans64Encoder{tab, sb}, wsm, scratch, slot_bytes, sizes, status);
 }
 
-template <uint32_t CODER, uint32_t SB>
-__global__ void __launch_bounds__(kMaxBlockWarps * 32)
-block_coder_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets,
-                          const uint16_t* __restrict__ block_freqs, uint32_t sb_rt, uint32_t block_size, uint32_t chunk_syms,
-                          uint8_t* __restrict__ out, uint32_t* __restrict__ status)
+// A block's decode table in shared memory at s_tab, from its cumulative frequencies (s_cum[257], M = 1 << sb): cum2sym[M],
+// then the symbol entries.  Every thread of the CTA takes part; the caller synchronises before the table is read.
+template <uint32_t CODER>
+__device__ __forceinline__ void block_coder_decode_table(const uint32_t* s_cum, uint8_t* s_tab, uint32_t M)
 {
-    extern __shared__ __align__(1024) uint8_t s_bdec[];         // [warps x 1 KiB rings][cum2sym[1 << sb]][symbol entries]
-    __shared__ uint32_t s_cum[257];
-    __shared__ uint32_t s_flag[1];
-    const uint32_t sb = SB ? SB : sb_rt, M = 1u << sb;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, warps = blockDim.x >> 5;
-    if (!block_prefix(block_freqs + static_cast<uint64_t>(blockIdx.x) * 256, s_cum, &s_flag[0], M)) {
-        if (tid == 0) atomicOr(status, kStatStream);
-        return;
-    }
-    uint8_t* s_tab = s_bdec + warps * kRingBytes;
+    const uint32_t tid = threadIdx.x;
     // cum2sym, 4 slots (one u32) at a time: one binary search per 4 slots for the largest s with cum[s] <= slot, then a
     // walk that also steps over zero-width symbols; the cost per slot does not depend on how skewed the model is, and
     // consecutive threads store consecutive words
@@ -133,6 +123,25 @@ block_coder_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, 
             syms[i] = make_uint2(s_cum[s], s_cum[s + 1] - s_cum[s]);
         }
     }
+}
+
+template <uint32_t CODER, uint32_t SB>
+__global__ void __launch_bounds__(kMaxBlockWarps * 32)
+block_coder_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets,
+                          const uint16_t* __restrict__ block_freqs, uint32_t sb_rt, uint32_t block_size, uint32_t chunk_syms,
+                          uint8_t* __restrict__ out, uint32_t* __restrict__ status)
+{
+    extern __shared__ __align__(1024) uint8_t s_bdec[];         // [warps x 1 KiB rings][cum2sym[1 << sb]][symbol entries]
+    __shared__ uint32_t s_cum[257];
+    __shared__ uint32_t s_flag[1];
+    const uint32_t sb = SB ? SB : sb_rt, M = 1u << sb;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, warps = blockDim.x >> 5;
+    if (!block_prefix(block_freqs + static_cast<uint64_t>(blockIdx.x) * 256, s_cum, &s_flag[0], M)) {
+        if (tid == 0) atomicOr(status, kStatStream);
+        return;
+    }
+    uint8_t* s_tab = s_bdec + warps * kRingBytes;
+    block_coder_decode_table<CODER>(s_cum, s_tab, M);
     __syncthreads();
 
     const uint32_t per_block = block_size / chunk_syms;

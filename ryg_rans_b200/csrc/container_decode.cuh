@@ -1,28 +1,36 @@
-// container_decode.cuh -- rb200_container_blocks_decode_async (version 2, per-block models) and
+// container_decode.cuh -- rb200_container_blocks_decode_async (version 2, per-block models),
+// rb200_container_blocks_coder_decode_async (version 3, per-block models of the byte or rans64 coder) and
 // rb200_container_decode_async (version 1, one model, any coder): a container in device memory, checked and decoded by
 // kernels alone, so that the call only enqueues work (and can be captured in a CUDA graph).
 //
 // The stages run in stream order; each reads what the one before it left in the context's BlocksAsyncWork (for
-// version 1 the first member of its SingleAsyncWork):
+// versions 1 and 3 the first member of their SingleAsyncWork / BlocksCoderAsyncWork):
 //   container_plan_kernel          one warp: container_header_ok on buf[0, 64) against size for the call's version ->
 //                                  the plan (version 1 also coder and scale_bits); clears the verdict words and the
 //                                  call's work counters, so that a call never depends on how the previous one ended
+//                                  (version 3: blocks_coder_plan_kernel, container_blocks_coder_header_ok)
 //   crc32_kernel x 2               meta CRC of buf + 64, length from the plan; blob CRC at buf + blob_off (both lengths
 //                                  are zero when the header is rejected, the blob's also when the flag is clear)
-//   container_prefix_check_kernel  container_block_model_ok for every block (version 2), container_dir_step_ok for
+//   container_prefix_check_kernel  container_block_model_sums_to(4096) for every block (version 2; version 3:
+//                                  blocks_coder_prefix_check_kernel, 1 << scale_bits), container_dir_step_ok for
 //                                  every directory entry, container_dir_ends_ok once
 //   container_table_kernel         version 1, one CTA: container_model_ok and container_model_decodable on the model,
 //                                  then the header coder's decode table, byte for byte what rb200_model_create uploads
 //   container_verdict_kernel       one warp: header CRC (crc fields zero) joined with the meta CRC, both CRCs compared;
 //                                  writes n_symbols, then sets go or ORs kStatStream / kStatSpace into the status word
+//                                  (version 3: blocks_coder_verdict_kernel)
 //   version 2: block_decode_planned_kernel
 //                                  a fixed grid that exits at once unless go; CTAs take block ids from a counter, build
 //                                  the block's slot table in shared memory and decode its chunks
+//   version 3: block_coder_decode_planned_kernel<CODER, SB>, one launch per instance of RB200_BLOCK_CODER_DISPATCH, each
+//              on a fixed grid; go holds the id of the one that runs, which decodes as block_decode_planned_kernel does
+//              with block_coder_decode_kernel's table
 //   version 1: one launch per decoder variant rb200_decode can pick (kDec*), each on a fixed grid; go holds the id of
 //              the one that runs, every other exits before it touches shared memory, TMA or its counter
 // The rules are the host parser's (container_format.h); they run in its order: content errors before kStatSpace.
 #pragma once
 #include "alias_kernels.cuh"
+#include "block_coder_kernels.cuh"
 #include "block_kernels.cuh"
 #include "container_format.h"
 #include "crc_kernels.cuh"
@@ -72,6 +80,49 @@ struct SingleAsyncWork {
     alignas(16) uint8_t table[kSingleTableBytes];   // the decode table of the header's coder, as rb200_model_create's
 };
 
+// rb200_container_blocks_coder_decode_async's workspace (version 3): version 2's, with the header's coder and scale_bits
+struct BlocksCoderAsyncWork {
+    BlocksAsyncWork c;          // plan, CRCs and verdict words; go is the decoder id (block_coder_decoder)
+    uint32_t coder, scale_bits; // from the header, when c.plan.ok
+};
+
+// The decoders of a version 3 container, one per instance of RB200_BLOCK_CODER_DISPATCH: the byte coder at scale_bits
+// 14, 12 or generic (ids 1, 2, 3), rans64 (4).  The verdict stores the id of the one to run in go.
+constexpr int kBlockCoderDecoders = 4;
+__host__ __device__ constexpr uint32_t block_coder_decoder(uint32_t coder, uint32_t sb)
+{
+    return coder == RB200_CODER_RANS64 ? 4 : sb == 14 ? 1 : sb == 12 ? 2 : 3;
+}
+
+// The plan of a header that passed its version's rules, into p (zero so far): l is the header the layout functions read
+// (for version 3 its version 2 shape); blocks: versions 2 and 3 (version 1 does not check n_blocks and block_size)
+__device__ __forceinline__ void container_plan(const ContainerHeader& l, bool blocks, BlocksPlan& p)
+{
+    p.ok = 1;
+    p.n_symbols = l.n_symbols;
+    p.n_chunks = l.n_chunks;
+    p.dir_off = container_dir_offset(l);
+    p.blob_off = container_blob_offset(l);
+    p.blob_bytes = l.blob_bytes;
+    p.meta_len = container_dir_end(l) - sizeof(ContainerHeader);
+    p.blob_len = (l.flags & RB200_CONTAINER_CRC_BLOB) ? l.blob_bytes : 0;
+    if (blocks) {
+        p.n_blocks = l.n_blocks;
+        p.block_size = l.block_size;
+    }
+    p.chunk_syms = l.chunk_syms;
+}
+
+// the plan, with the verdict words and the decoder's counters cleared
+__device__ __forceinline__ void container_plan_store(BlocksAsyncWork* w, const BlocksPlan& p)
+{
+    w->plan = p;
+    w->bad = 0;
+    w->go = 0;
+    w->next_block = 0;
+    w->ctas_done = 0;
+}
+
 // single: the version 1 call's workspace (w is then &single->c), or null for version 2
 __global__ void __launch_bounds__(32)
     container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, BlocksAsyncWork* w, SingleAsyncWork* single)
@@ -82,28 +133,12 @@ __global__ void __launch_bounds__(32)
     if (size >= sizeof(ContainerHeader)) {                           // a shorter buffer is not read at all
         const ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(buf);
         if (container_header_ok(h, size, static_cast<uint16_t>(version))) {
-            p.ok = 1;
-            p.n_symbols = h.n_symbols;
-            p.n_chunks = h.n_chunks;
-            p.dir_off = container_dir_offset(h);
-            p.blob_off = container_blob_offset(h);
-            p.blob_bytes = h.blob_bytes;
-            p.meta_len = container_dir_end(h) - sizeof(ContainerHeader);
-            p.blob_len = (h.flags & RB200_CONTAINER_CRC_BLOB) ? h.blob_bytes : 0;
-            if (version == kContainerVersionBlocks) {                // version 1 does not check these fields
-                p.n_blocks = h.n_blocks;
-                p.block_size = h.block_size;
-            }
-            p.chunk_syms = h.chunk_syms;
+            container_plan(h, version == kContainerVersionBlocks, p);
             coder = h.coder;
             scale_bits = h.scale_bits;
         }
     }
-    w->plan = p;
-    w->bad = 0;
-    w->go = 0;
-    w->next_block = 0;
-    w->ctas_done = 0;
+    container_plan_store(w, p);
     if (single) {
         single->coder = coder;
         single->scale_bits = scale_bits;
@@ -113,13 +148,33 @@ __global__ void __launch_bounds__(32)
     }
 }
 
+// Version 3: its header rule (container_blocks_coder_header_ok, the host parser's), then the plan of its version 2 shape
+__global__ void __launch_bounds__(32)
+    blocks_coder_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, BlocksCoderAsyncWork* w)
+{
+    if (threadIdx.x) return;
+    BlocksPlan p = {};
+    uint32_t coder = 0, scale_bits = 0;
+    if (size >= sizeof(ContainerHeader)) {                           // a shorter buffer is not read at all
+        const ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(buf);
+        if (container_blocks_coder_header_ok(h, size)) {
+            container_plan(container_layout(h), true, p);
+            coder = h.coder;
+            scale_bits = h.scale_bits;
+        }
+    }
+    container_plan_store(&w->c, p);
+    w->coder = coder;
+    w->scale_bits = scale_bits;
+}
+
 // The per-element rules of the prefix.  Each warp stages 32 block models (16 KiB, coalesced) in shared memory with
-// rows padded to 129 words, so that lane r checking row r reads a different bank from every other lane.
+// rows padded to 129 words, so that lane r checking row r reads a different bank from every other lane.  Every block
+// sums to total: 4096 (version 2), 1 << scale_bits (version 3).
 constexpr int kPrefixWarps = 2;
 constexpr uint32_t kPrefixRowWords = 129;
 
-__global__ void __launch_bounds__(kPrefixWarps * 32)
-    container_prefix_check_kernel(const uint8_t* __restrict__ buf, BlocksAsyncWork* w)
+__device__ __forceinline__ void container_prefix_check(const uint8_t* __restrict__ buf, BlocksAsyncWork* w, uint32_t total)
 {
     __shared__ uint32_t s_rows[kPrefixWarps][32 * kPrefixRowWords];
     const BlocksPlan p = w->plan;
@@ -141,7 +196,7 @@ __global__ void __launch_bounds__(kPrefixWarps * 32)
             d[3] = v.w;
         }
         __syncwarp();
-        if (lane < n) ok &= container_block_model_ok(reinterpret_cast<const uint16_t*>(rows + lane * kPrefixRowWords));
+        if (lane < n) ok &= container_block_model_sums_to(reinterpret_cast<const uint16_t*>(rows + lane * kPrefixRowWords), total);
         __syncwarp();
     }
     const uint64_t threads = static_cast<uint64_t>(gridDim.x) * blockDim.x;
@@ -149,6 +204,18 @@ __global__ void __launch_bounds__(kPrefixWarps * 32)
     for (uint64_t c = t; c < p.n_chunks; c += threads) ok &= container_dir_step_ok(offsets, c);
     if (t == 0) ok &= container_dir_ends_ok(offsets, p.n_chunks, p.blob_bytes);
     if (!ok) w->bad = 1;
+}
+
+__global__ void __launch_bounds__(kPrefixWarps * 32)
+    container_prefix_check_kernel(const uint8_t* __restrict__ buf, BlocksAsyncWork* w)
+{
+    container_prefix_check(buf, w, 4096);
+}
+
+__global__ void __launch_bounds__(kPrefixWarps * 32)
+    blocks_coder_prefix_check_kernel(const uint8_t* __restrict__ buf, BlocksCoderAsyncWork* w)
+{
+    container_prefix_check(buf, &w->c, 1u << w->scale_bits);
 }
 
 // The version 1 model (256 x u32 at buf + 64) checked and turned into the decode table of the header's coder in
@@ -241,11 +308,10 @@ __device__ inline uint32_t single_decoder(uint32_t coder, uint32_t scale_bits, u
 
 // One warp.  meta_crc covers the header with its crc fields zeroed, then meta_len bytes whose CRC is in crc[0];
 // the header's CRC is taken here with container_finish_kernel's warp helpers and joined (crc32_combine).
-// single: as for container_plan_kernel.  Version 1 also refuses what the decoders do not take (container_format.h),
-// as content, and its go is the id of the decoder to run.
-__global__ void __launch_bounds__(32)
-    container_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, BlocksAsyncWork* w,
-                             uint32_t* status, const SingleAsyncWork* single)
+// refused(): the decoders do not take what open accepted (content, as kStatStream); decoder(): the go of a pass.
+template <class Refused, class Decoder>
+__device__ __forceinline__ void container_verdict(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols,
+                                                  BlocksAsyncWork* w, uint32_t* status, Refused refused_of, Decoder decoder)
 {
     using namespace crc_detail;
     __shared__ uint4 s_head_v[sizeof(ContainerHeader) / 16];
@@ -275,13 +341,38 @@ __global__ void __launch_bounds__(32)
     if (lane) return;
     const bool prefix_ok = meta == meta_crc && !w->bad;
     if (prefix_ok && n_symbols) *n_symbols = p.n_symbols;
-    const bool refused = single && (single->refused || !container_geometry_decodable(p.chunk_syms, p.blob_bytes));
+    const bool refused = refused_of();
     if (!prefix_ok || refused || ((flags & RB200_CONTAINER_CRC_BLOB) && w->crc[1].crc != blob_crc))
         atomicOr(status, kStatStream);
     else if (p.n_symbols > out_cap)
         atomicOr(status, kStatSpace);
     else
-        w->go = single ? single_decoder(single->coder, single->scale_bits, single->wide) : 1;
+        w->go = decoder();
+}
+
+// Versions 1 and 2.  single: as for container_plan_kernel.  Version 1 also refuses what the decoders do not take
+// (container_format.h), and its go is the id of the decoder to run.
+__global__ void __launch_bounds__(32)
+    container_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, BlocksAsyncWork* w,
+                             uint32_t* status, const SingleAsyncWork* single)
+{
+    const BlocksPlan& p = w->plan;
+    container_verdict(
+        buf, out_cap, n_symbols, w, status,
+        [&] { return single && (single->refused || !container_geometry_decodable(p.chunk_syms, p.blob_bytes)); },
+        [&] { return single ? single_decoder(single->coder, single->scale_bits, single->wide) : 1u; });
+}
+
+// Version 3: the block decoders refuse a blob of 2^36 bytes or more (its chunk sizes are theirs by the header rule);
+// go is the id of the decoder of the header's coder and scale_bits.
+__global__ void __launch_bounds__(32)
+    blocks_coder_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, BlocksCoderAsyncWork* w,
+                                uint32_t* status)
+{
+    const BlocksPlan& p = w->c.plan;
+    container_verdict(
+        buf, out_cap, n_symbols, &w->c, status, [&] { return !container_geometry_decodable(p.chunk_syms, p.blob_bytes); },
+        [&] { return block_coder_decoder(w->coder, w->scale_bits); });
 }
 
 // The per-block decoder for a geometry only the device knows: a fixed grid of kPlannedWarps-warp CTAs (resident all at
@@ -337,6 +428,60 @@ __global__ void __launch_bounds__(kPlannedWarps * 32, 8)
     if (tid == 0 && atomicAdd(&w->ctas_done, 1u) == gridDim.x - 1) {
         w->next_block = 0;
         w->ctas_done = 0;
+    }
+}
+
+// The version 3 decoders, one per instance of RB200_BLOCK_CODER_DISPATCH, each on a fixed grid of kPlannedWarps-warp CTAs
+// (resident all at once).  Only the one whose id is in go runs; every other exits before it touches shared memory or
+// the counter.  CTAs take block ids from w->c.next_block; per block, block_coder_decode_kernel's table in shared memory,
+// then the warps take the block's 1..32 chunks in turn.
+template <uint32_t CODER, uint32_t SB>
+__global__ void __launch_bounds__(kPlannedWarps * 32)
+    block_coder_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, BlocksCoderAsyncWork* __restrict__ w,
+                                      uint32_t* __restrict__ status)
+{
+    if (w->c.go != block_coder_decoder(CODER, SB)) return;           // the same for the whole grid
+    extern __shared__ __align__(1024) uint8_t s_bdec[];             // [kPlannedWarps x 1 KiB rings][cum2sym[1 << sb]][symbol entries]
+    __shared__ uint32_t s_cum[257];
+    __shared__ uint32_t s_flag[1];
+    __shared__ uint32_t s_block;
+    const BlocksPlan& p = w->c.plan;
+    const uint32_t sb = SB ? SB : w->scale_bits, M = 1u << sb;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t n_blocks = p.n_blocks, block_size = p.block_size, chunk_syms = p.chunk_syms;
+    const uint32_t per_block = block_size / chunk_syms;
+    const uint64_t blob_bytes = p.blob_bytes;
+    const uint16_t* models = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + p.dir_off);
+    const uint8_t* blob = buf + p.blob_off;
+    uint8_t* s_tab = s_bdec + kPlannedWarps * kRingBytes;
+    const uint32_t ring = smem_addr(s_bdec) + warp * kRingBytes, tab = smem_addr_pinned(s_tab);
+    for (;;) {
+        __syncthreads();                                             // the previous block's table is no longer in use
+        if (tid == 0) s_block = atomicAdd(&w->c.next_block, 1u);
+        __syncthreads();
+        const uint32_t block = s_block;
+        if (block >= n_blocks) break;
+        if (!block_prefix(models + static_cast<uint64_t>(block) * 256, s_cum, &s_flag[0], M)) {   // checked before: not reached
+            if (tid == 0) atomicOr(status, kStatStream);
+            continue;
+        }
+        block_coder_decode_table<CODER>(s_cum, s_tab, M);
+        __syncthreads();
+        for (uint32_t k = warp; k < per_block; k += kPlannedWarps) {
+            const uint32_t chunk = block * per_block + k;
+            uint8_t* dst = out + static_cast<uint64_t>(block) * block_size + static_cast<uint64_t>(k) * chunk_syms;
+            if (CODER == RB200_CODER_BYTE)
+                decode_window_chunk(ByteDecoder<SB>{tab, sb}, blob, blob_bytes, offsets, chunk, ring, dst, chunk_syms, status);
+            else
+                decode_window_chunk(Rans64Decoder{tab, tab + M + (lane & (kRans64DecReplicas - 1)) * 8, sb}, blob, blob_bytes, offsets, chunk,
+                                    ring, dst, chunk_syms, status);
+        }
+    }
+    // every CTA has taken its last block id before it counts itself out: the last one re-arms the counter
+    if (tid == 0 && atomicAdd(&w->c.ctas_done, 1u) == gridDim.x - 1) {
+        w->c.next_block = 0;
+        w->c.ctas_done = 0;
     }
 }
 
@@ -525,6 +670,37 @@ inline void configure_single_decode(uint32_t sms, SingleDecodeLaunch* out)
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, l[i].kernel, static_cast<int>(l[i].threads), l[i].smem);
             out[i].grid = sms * static_cast<uint32_t>(per_sm < 1 ? 1 : per_sm);
         }
+    }
+}
+
+// One launch of a version 3 decoder: kernel, grid (every CTA that is resident at once), dynamic shared memory.
+struct BlockCoderDecodeLaunch {
+    void (*kernel)(const uint8_t*, uint8_t*, BlocksCoderAsyncWork*, uint32_t*);
+    uint32_t grid, smem;
+    const char* name;
+};
+
+// The version 3 decoders in id order; shared memory for the largest scale_bits each decodes (the generic ones: 15).
+inline void configure_blocks_coder_decode(uint32_t sms, BlockCoderDecodeLaunch* out)
+{
+    constexpr uint32_t threads = kPlannedWarps * 32;
+    const BlockCoderDecodeLaunch l[kBlockCoderDecoders] = {
+        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 14>, 0, block_coder_decode_smem(RB200_CODER_BYTE, 14, threads),
+         "block_coder_decode_planned_kernel<byte, 14>"},
+        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 12>, 0, block_coder_decode_smem(RB200_CODER_BYTE, 12, threads),
+         "block_coder_decode_planned_kernel<byte, 12>"},
+        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 0>, 0, block_coder_decode_smem(RB200_CODER_BYTE, kBlockCoderMaxScaleBits, threads),
+         "block_coder_decode_planned_kernel<byte, 0>"},
+        {block_coder_decode_planned_kernel<RB200_CODER_RANS64, 0>, 0,
+         block_coder_decode_smem(RB200_CODER_RANS64, kBlockCoderMaxScaleBits, threads), "block_coder_decode_planned_kernel<rans64, 0>"},
+    };
+    for (int i = 0; i < kBlockCoderDecoders; i++) {
+        out[i] = l[i];
+        cudaFuncSetAttribute(l[i].kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(l[i].kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(l[i].smem));
+        int per_sm = 0;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, l[i].kernel, static_cast<int>(threads), l[i].smem);
+        out[i].grid = sms * static_cast<uint32_t>(per_sm < 1 ? 1 : per_sm);
     }
 }
 

@@ -8,8 +8,8 @@
 #include "rans_b200.h"
 
 // The layout and the rules below are compiled for the host and, under nvcc, for the device too (RB200_HD): the kernels
-// of rb200_container_decode_async / rb200_container_blocks_decode_async (container_decode.cuh) apply the same functions
-// as the host parser.
+// of rb200_container_decode_async / rb200_container_blocks_decode_async / rb200_container_blocks_coder_decode_async
+// (container_decode.cuh) apply the same functions as the host parser.
 
 namespace rb200 {
 
@@ -53,14 +53,14 @@ RB200_HD inline uint64_t container_blob_offset(const ContainerHeader& h) { retur
 
 // Version 3 is version 2 with the header's own coder (byte or rans64) and scale_bits (8..15): the same layout, and every
 // rule of version 2 but the coder, scale_bits and the block total.  The layout functions above and container_header_ok
-// serve versions 1 and 2 (the kernels of container_decode.cuh call them); the host reads a version 3 header through
-// its version 2 shape.
+// serve versions 1 and 2; host and kernels read a version 3 header through its version 2 shape
+// (container_blocks_coder_header_ok below).
 RB200_HD inline bool container_blocks_coder_ok(uint32_t coder, uint32_t scale_bits)
 {
     return (coder == RB200_CODER_BYTE || coder == RB200_CODER_RANS64) && scale_bits >= 8 && scale_bits <= 15;
 }
 // the header the layout functions and version 2's rules read for h: h itself, or for version 3 its version 2 shape
-inline ContainerHeader container_layout(ContainerHeader h)
+RB200_HD inline ContainerHeader container_layout(ContainerHeader h)
 {
     if (h.version == kContainerVersionBlocksCoder) {
         h.version = kContainerVersionBlocks;
@@ -106,6 +106,12 @@ RB200_HD inline bool container_header_ok(const ContainerHeader& h, uint64_t size
     }
     const uint64_t boff = container_blob_offset(h);                 // < 2^42: n_chunks < 2^31, n_blocks < 2^32
     return boff <= size && h.blob_bytes <= size - boff;
+}
+// Every rule of a version 3 header: its coder and scale_bits, then version 2's rules on its version 2 shape.
+RB200_HD inline bool container_blocks_coder_header_ok(const ContainerHeader& h, uint64_t size)
+{
+    return h.version == kContainerVersionBlocksCoder && container_blocks_coder_ok(h.coder, h.scale_bits) &&
+           container_header_ok(container_layout(h), size, kContainerVersionBlocks);
 }
 
 // what rb200_model_create would accept: a known coder, its scale_bits range, frequencies that sum to 1 << scale_bits

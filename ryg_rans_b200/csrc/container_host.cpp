@@ -28,7 +28,8 @@
 // on one core: the blob CRC is optional for that reason).  rb200_container_encode / _decode and the _blocks_ forms
 // (rans_b200.cu) write and read the same bytes in host or device memory with the blob CRC on the GPU
 // (crc_kernels.cuh); they validate through the parser below, so both sides apply one set of rules.
-// rb200_container_decode_async and rb200_container_blocks_decode_async apply the same rules in kernels
+// rb200_container_decode_async, rb200_container_blocks_decode_async and rb200_container_blocks_coder_decode_async apply
+// the same rules in kernels
 // (container_decode.cuh): the header, model and per-element rules are the __host__ __device__ functions of
 // container_format.h that the parser below calls.
 #include "container_format.h"
@@ -154,10 +155,7 @@ int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, Co
     if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
     ContainerHeader h;
     std::memcpy(&h, hdr, sizeof h);
-    const bool ok = version == kContainerVersionBlocksCoder
-                        ? h.version == version && container_blocks_coder_ok(h.coder, h.scale_bits) &&
-                              container_header_ok(container_layout(h), size, kContainerVersionBlocks)
-                        : container_header_ok(h, size, version);
+    const bool ok = version == kContainerVersionBlocksCoder ? container_blocks_coder_header_ok(h, size) : container_header_ok(h, size, version);
     if (!ok) return RB200_E_STREAM;
     *out = h;
     return RB200_OK;

@@ -70,6 +70,9 @@ struct rb200_ctx {
     // rb200_container_decode_async: its fixed workspace (with the decode table) and its decoders' launches
     SingleAsyncWork* d_single_async = nullptr;
     SingleDecodeLaunch single_decoders[kSingleDecoders] = {};
+    // rb200_container_blocks_coder_decode_async: its fixed workspace and its decoders' launches
+    BlocksCoderAsyncWork* d_blocks_coder_async = nullptr;
+    BlockCoderDecodeLaunch blocks_coder_decoders[kBlockCoderDecoders] = {};
     // rb200_container_model_encode_async (model_kernels.cuh): the counts, the model and its encode tables
     ModelAsyncWork* d_model_async = nullptr;
 };
@@ -235,6 +238,8 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_async, 0, sizeof(BlocksAsyncWork));
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_single_async, sizeof(SingleAsyncWork));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_single_async, 0, sizeof(SingleAsyncWork));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_blocks_coder_async, sizeof(BlocksCoderAsyncWork));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_coder_async, 0, sizeof(BlocksCoderAsyncWork));
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_model_async, sizeof(ModelAsyncWork));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_model_async, 0, sizeof(ModelAsyncWork));
     if (e != cudaSuccess) {
@@ -251,6 +256,7 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     configure_crc_kernels();
     ctx->blocks_async = configure_container_decode(static_cast<uint32_t>(ctx->sms));
     configure_single_decode(static_cast<uint32_t>(ctx->sms), ctx->single_decoders);
+    configure_blocks_coder_decode(static_cast<uint32_t>(ctx->sms), ctx->blocks_coder_decoders);
     configure_model_kernels();
     cudaGetLastError();
     *out = ctx;
@@ -274,6 +280,7 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->h_crc) cudaFreeHost(ctx->h_crc);
     if (ctx->d_blocks_async) cudaFree(ctx->d_blocks_async);
     if (ctx->d_single_async) cudaFree(ctx->d_single_async);
+    if (ctx->d_blocks_coder_async) cudaFree(ctx->d_blocks_coder_async);
     if (ctx->d_model_async) cudaFree(ctx->d_model_async);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
@@ -1697,22 +1704,28 @@ namespace {
 // version 2): plan, meta CRC, blob CRC, the prefix check, version 1's model check and table build, then the verdict.
 // Lengths and positions the host cannot know come from the plan on the device; the host passes only bounds it knows
 // (size).
-int enqueue_container_checks(rb200_ctx* ctx, const uint8_t* buf, size_t size, size_t out_cap, uint64_t* d_n_symbols, uint16_t version,
-                             BlocksAsyncWork* w, SingleAsyncWork* single)
+// the meta and blob CRCs of the async decodes, lengths and blob position from the plan in w
+int enqueue_container_crcs(rb200_ctx* ctx, const uint8_t* buf, size_t size, BlocksAsyncWork* w)
 {
     const uint32_t sms = static_cast<uint32_t>(ctx->sms);
     const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
     cudaStream_t s = ctx->stream;
-    container_plan_kernel<<<1, 32, 0, s>>>(buf, size, version, w, single);
-    int rc = check_launch(ctx, "container_plan_kernel");
-    if (rc != RB200_OK) return rc;
     crc32_kernel<<<crc32_grid(sms, after_head), kCrcThreads, kCrcSmemBytes, s>>>(buf + sizeof(ContainerHeader), after_head, &w->plan.meta_len,
                                                                                  nullptr, 0, &w->crc_work, &w->crc[0]);
-    rc = check_launch(ctx, "crc32_kernel(meta)");
+    const int rc = check_launch(ctx, "crc32_kernel(meta)");
     if (rc != RB200_OK) return rc;
     crc32_kernel<<<crc32_grid(sms, size), kCrcThreads, kCrcSmemBytes, s>>>(buf, size, &w->plan.blob_len, &w->plan.blob_off, 0,
                                                                            &w->crc_work, &w->crc[1]);
-    rc = check_launch(ctx, "crc32_kernel(blob)");
+    return check_launch(ctx, "crc32_kernel(blob)");
+}
+
+int enqueue_container_checks(rb200_ctx* ctx, const uint8_t* buf, size_t size, size_t out_cap, uint64_t* d_n_symbols, uint16_t version,
+                             BlocksAsyncWork* w, SingleAsyncWork* single)
+{
+    cudaStream_t s = ctx->stream;
+    container_plan_kernel<<<1, 32, 0, s>>>(buf, size, version, w, single);
+    int rc = check_launch(ctx, "container_plan_kernel");
+    if (rc == RB200_OK) rc = enqueue_container_crcs(ctx, buf, size, w);
     if (rc != RB200_OK) return rc;
     container_prefix_check_kernel<<<ctx->blocks_async.check_grid, kPrefixWarps * 32, 0, s>>>(buf, w);
     rc = check_launch(ctx, "container_prefix_check_kernel");
@@ -1759,6 +1772,32 @@ extern "C" int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, 
     for (int i = 0; i < kSingleDecoders && rc == RB200_OK; i++) {
         const SingleDecodeLaunch& l = ctx->single_decoders[i];
         l.kernel<<<l.grid, l.threads, l.smem, ctx->stream>>>(buf, out, w, ctx->d_status);
+        rc = check_launch(ctx, l.name);
+    }
+    return rc;
+}
+
+// Version 3: its own plan, prefix check and verdict kernels around the same CRCs, then every block decoder variant on
+// its fixed grid: the verdict's go names the one that runs.  Nine launches, no copy, no synchronisation, no allocation.
+extern "C" int rb200_container_blocks_coder_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                                         uint64_t* d_n_symbols)
+{
+    if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    BlocksCoderAsyncWork* w = ctx->d_blocks_coder_async;
+    cudaStream_t s = ctx->stream;
+    blocks_coder_plan_kernel<<<1, 32, 0, s>>>(buf, size, w);
+    int rc = check_launch(ctx, "blocks_coder_plan_kernel");
+    if (rc == RB200_OK) rc = enqueue_container_crcs(ctx, buf, size, &w->c);
+    if (rc != RB200_OK) return rc;
+    blocks_coder_prefix_check_kernel<<<ctx->blocks_async.check_grid, kPrefixWarps * 32, 0, s>>>(buf, w);
+    rc = check_launch(ctx, "blocks_coder_prefix_check_kernel");
+    if (rc != RB200_OK) return rc;
+    blocks_coder_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status);
+    rc = check_launch(ctx, "blocks_coder_verdict_kernel");
+    for (int i = 0; i < kBlockCoderDecoders && rc == RB200_OK; i++) {
+        const BlockCoderDecodeLaunch& l = ctx->blocks_coder_decoders[i];
+        l.kernel<<<l.grid, kPlannedWarps * 32, l.smem, s>>>(buf, out, w, ctx->d_status);
         rc = check_launch(ctx, l.name);
     }
     return rc;

@@ -42,6 +42,9 @@ alphabet permuted per block) and "zipf" (the --blocks data):
   coders (K8 / K9) on the same number of bytes, alternated; the size of each output in bytes per symbol (512 B of model
   per block included; single models at 1024 B) with byte and rans64 also at scale_bits 15 and every coder's single model
   from the whole data; and a torch.profiler list of each per-block call's kernels.
+  The version 3 container of the same blocks (byte and rans64 at 14, models built, flags 0 and RB200_CONTAINER_CRC_BLOB):
+  rb200_blocks_coder_decode against rb200_container_blocks_coder_decode and rb200_container_blocks_coder_decode_async,
+  alternated; the host time each container call takes to return; and a torch.profiler list of the async call's kernels.
 
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
@@ -293,8 +296,54 @@ def blocks_coder(args):
         for m, *_ in single.values():
             m.close()
         res[name] = {"encode": etimes, "decode": dtimes, "bytes_per_symbol": sizes, "kernels": profile}
+        res[name].update(blocks_coder_containers(ctx, args, name, coders, sb, d_in, d_out, dec, res["checks"]))
     ctx.close()
     return res
+
+
+def blocks_coder_containers(ctx, args, name, coders, sb, d_in, d_out, dec, checks):
+    """The version 3 container of the same blocks (models built on the GPU), each coder with flags 0 and
+    RB200_CONTAINER_CRC_BLOB: rb200_blocks_coder_decode against rb200_container_blocks_coder_decode (DEVICE) and
+    rb200_container_blocks_coder_decode_async, alternated; the host time each container call takes to return; and a
+    torch.profiler list of the async call's kernels (the planned decoder and the gated-out launches)."""
+    import torch
+    n = d_in.numel()
+    n_blocks, block_size, chunk = 8192, 65536, 8192
+    cap = ctx.container_blocks_capacity(n_blocks, block_size, chunk)
+    sync = ctx.sync
+    conts = {}
+    for k, coder in coders.items():
+        for flags, tag in ((0, ""), (api.CONTAINER_CRC_BLOB, "_crc")):
+            d = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+            ctx.container_blocks_coder_encode_device(coder, sb, d_in.data_ptr(), n_blocks, block_size, None, chunk, flags, d.data_ptr(), cap)
+            sync()
+            blob_bytes = int(d[32:40].cpu().numpy().view(np.uint64)[0])
+            conts[k + tag] = (d, int(ctx.lib.dll.rb200_container_blocks_size(n_blocks, n // chunk, blob_bytes)))
+    calls = {}
+    for k in coders:
+        calls[f"{k}_blocks_decode"] = dec[f"{k}_blocks_decode"]
+        for tag in ("", "_crc"):
+            d, size = conts[k + tag]
+            calls[f"{k}_container_decode{tag}"] = lambda d=d, size=size: ctx.container_blocks_coder_decode_device(d.data_ptr(), size,
+                                                                                                                  d_out.data_ptr(), n)
+            calls[f"{k}_container_decode_async{tag}"] = lambda d=d, size=size: ctx.container_blocks_coder_decode_async(d.data_ptr(), size,
+                                                                                                                      d_out.data_ptr(), n)
+    times = alternate(calls, sync, args.warmup, args.reps)
+    host = {k: [] for k in calls if "container" in k}
+    for _ in range(args.reps):
+        for k in host:
+            t0 = time.perf_counter()
+            calls[k]()
+            host[k].append((time.perf_counter() - t0) * 1e3)
+            sync()
+    for k, f in calls.items():
+        d_out.zero_()
+        f()
+        sync()
+        checks[f"{name}_{k}_equals_input"] = bool(torch.equal(d_out[:n], d_in))
+    profile = {f"{k}_container_decode_async": kernel_times(calls[f"{k}_container_decode_async"], sync, args.reps) for k in coders}
+    return {"container_decode": times, "container_decode_call_host_ms": {k: stats(v) for k, v in host.items()},
+            "container_kernels": profile}
 
 
 def headline(args):
