@@ -481,8 +481,8 @@ int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* siz
 //   fused: ONE persistent launch -- workers encode, a scanner warp turns published sizes into end offsets
 //          in chunk order, workers place chunk k after encoding chunk k+1 (placement.cuh);
 //   ring:  the fused launch with every stream kept in its warp's shared-memory ring until it is placed with TMA bulk
-//          copies (K2r, encode_ring.cuh): no scratch; for chunks of <= kEncRingMaxChunk symbols, whose worst-case
-//          stream fits a ring, and models the host knows satisfy word_ring_model (so not for
+//          copies (K2r, encode_ring.cuh): what does not fit the ring goes to per-warp spill slots; for chunks of
+//          <= kEncRingMaxChunk symbols, whose worst-case stream fits a slot, and models the host knows satisfy word_ring_model (so not for
 //          rb200_container_model_encode_async, whose model is built on the GPU);
 //   split: three launches -- encode into per-chunk worst-case slots, tile scan, compaction.
 // fused is faster as long as the scanner keeps up, i.e. for chunks of >= 4096 symbols; below that the split path
@@ -507,12 +507,12 @@ bool use_fused_encode(uint32_t chunk_syms)
 }
 
 // How one encode call over n_chunks chunks runs, decided once: the path, the encode launch's shape, and the workspace
-// both need.  Fused: one launch of `grid` CTAs with `slots` scratch slots (slots per worker warp x the warps of the grid; none for ring);
+// both need.  Fused: one launch of `grid` CTAs with `slots` scratch slots (slots per worker warp x the warps of the grid; ring: a pair of spill slots per warp);
 // in ctx->sizes the chunk counter (16 bytes), then look[n_chunks] (placement.cuh).  Split: the encode launch into one
 // slot per chunk, then finish_encode; in ctx->sizes sizes[n_chunks], then the scan's tile sums.
 struct EncodePlan {
     bool fused;
-    bool ring;                         // word coder, fused: K2r instead of K2f (no scratch slots)
+    bool ring;                         // word coder, fused: K2r instead of K2f
     uint32_t grid, threads, smem;      // the encode launch (dynamic shared memory in bytes)
     size_t slots;
     uint32_t slot_bytes;
@@ -520,7 +520,8 @@ struct EncodePlan {
 };
 
 // A word model whose streams fit K2r's ring: no symbol holds all 4096 slots.  Such a symbol's x_max wraps to 0
-// (word_enc_expand), so every step emits a word: 2 * chunk_syms + 128 bytes per chunk, more than kWordStreamMax.
+// (word_enc_expand), so every step emits a word: 2 * chunk_syms + 128 bytes per chunk, so
+// every stream would go largely through K2r's spill slots; K2f takes those models.
 bool word_ring_model(const uint32_t freqs[256])
 {
     for (int s = 0; s < 256; s++)
@@ -545,7 +546,8 @@ EncodePlan plan_encode(const rb200_ctx* ctx, int coder, uint32_t scale_bits, uin
             p.threads = kEncRingWarps * 32;
             p.smem = kEncRingSmemBytes;
             p.grid = std::min((n_chunks + 1 + kEncRingWarps - 1) / kEncRingWarps, sms);
-            p.slots = 0;
+            p.slots = static_cast<size_t>(p.grid) * kEncRingWarps;     // one pair of spill slots per warp
+            p.slot_bytes = kEncRingSpillBytes;
         } else if (p.fused) {
             const uint32_t want = (n_chunks + 1 + kEncWarps - 1) / kEncWarps;     // + 1: one warp of the grid is the scanner
             p.grid = std::min(want, sms * RB200_FUSED_MINBLOCKS);
@@ -676,8 +678,8 @@ int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, si
             const WordEncEntry* table = t.word[t.word_r32 ? 1 : 0];
             if (p.ring) {
                 auto kernel = t.word_r32 ? word_encode_ring_kernel<true> : word_encode_ring_kernel<false>;
-                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.look, ws.counter, d_blob,
-                                                                   blob_cap, d_offsets, ctx->d_status);
+                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.scratch, ws.look, ws.counter,
+                                                                   d_blob, blob_cap, d_offsets, ctx->d_status);
                 return check_launch(ctx, "word_encode_ring_kernel");
             }
             if (p.fused) {

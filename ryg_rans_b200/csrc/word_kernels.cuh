@@ -193,7 +193,6 @@ word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t ch
 // offset is published and is then stored to the blob with TMA bulk copies, so no stream goes through global scratch.
 // The step loads its symbol 2 D steps and its table entry D steps ahead, so only the state arithmetic is on the chain.
 // ---------------------------------------------------------------------------
-constexpr uint32_t kWordStreamMax = 12480;   // worst-case stream of a chunk of 8192 symbols (DESIGN.md section 8)
 
 // shared address of ring position pos, pos in [-RING, RING) (as uint32_t)
 template <uint32_t RING>
@@ -277,13 +276,14 @@ __device__ __forceinline__ void word_ring_step(uint32_t& x, uint32_t& wpos, uint
 // downwards, modulo RING; the bytes of encode_stream's stream, preceded by zeros up to a 16-byte boundary.  Returns the
 // stream size in bytes (warp-uniform); the stream then fills [top - round_up_16(size), top) of the ring.
 //   stage = this warp's 512 B input stage; tab = the shared address of the 8x replicated uint4 table
-//   space.reserve(emitted, need): returns once `need` more bytes below the `emitted` ones are free to write
+//   space.reserve(emitted, need): returns once `need` more bytes below the `emitted` ones (counted modulo RING) are
+//   free to write; space.emitted(emitted): the stream's emitted bytes from their count modulo RING
 template <bool R32, uint32_t RING, uint32_t D, class Space>
 __device__ __forceinline__ uint32_t word_encode_stream_ring(const uint8_t* __restrict__ chunk_in, uint32_t m, uint32_t tab, uint32_t stage,
                                                             uint32_t ring, uint32_t top, Space& space, uint32_t* __restrict__ status)
 {
     static_assert(D == 1 || D == 2 || D == 4, "the prefetch registers rotate with the 16-step stage block");
-    static_assert(RING % 16 == 0 && RING >= kWordStreamMax + 16 && RING > 2048, "a worst-case stream fits the ring");
+    static_assert(RING % 16 == 0 && RING > 2048, "16-byte aligned stream ends; a 16-step block (<= 1 KiB) wraps at most once");
     constexpr uint32_t D2 = 2 * D;
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t tab_lane = tab + (lane & (kEncReplicas - 1)) * 16;
@@ -370,17 +370,31 @@ __device__ __forceinline__ uint32_t word_encode_stream_ring(const uint8_t* __res
     const uint32_t hpos = wpos - 4u * (31u - lane);
     sts_u16(ring_addr<RING>(ring, hpos), x >> 16);
     sts_u16(ring_addr<RING>(ring, hpos - 2u), x);
-    const uint32_t produced = emitted(wpos) + 32 * 4;
+    const uint32_t produced = space.emitted(emitted(wpos)) + 32 * 4;
     const uint32_t gap = ((produced + 15u) & ~15u) - produced;
-    if (2u * lane < gap) sts_u16(ring_addr<RING>(ring, top - produced - 2u - 2u * lane), 0);
+    if (2u * lane < gap) sts_u16(ring_addr<RING>(ring, wpos - 32u * 4 - 2u * lane), 0);     // wpos - 126 = top - produced, modulo RING
     if (__any_sync(0xffffffffu, (flags & kWordSlots) != 0) && lane == 0) atomicOr(status, kStatSymbol);
     return produced;
 }
 
 // K2r's shape: one CTA of RB200_RING_WARPS warps per SM, each with a ring of RB200_RING_BYTES and a 512 B stage, and the
-// table: 32 KiB + 15 x (12800 + 512) B = 227 KiB, all the shared memory a CTA can have.  A ring holds a worst-case stream
-// (12 480 B at chunks of 8192); with uniform bytes the pending stream (8.3 KB) leaves 4.5 KB for the next one.
-// H100 SXM at 400 W, 1 GiB uniform bytes, chunks of 8192, ms per call of the step alone (no placement:
+// table: 32 KiB + 20 x (9472 + 512) B = 227 KiB, all the shared memory a CTA can have.  The ring no longer holds a
+// worst-case stream (12 480 B at chunks of 8192) and the pending one before it: what does not fit goes to the warp's
+// spill slots (encode_ring.cuh).  Occupancy is what pays: 20 warps at 96 registers, no local-memory spills.  At 22 and
+// 24 warps ptxas allocates 80 registers (-Xptxas -v) and spills to local memory.
+// H100 80GB HBM3 at 700 W, 1 GiB, chunks of 8192, ms per call with placement (tools/encode_ring_lab.cu, two alternated
+// passes; D = prefetch distance; P = RB200_RING_PEND_PIECE, 16512 = a pending stream spilled whole, 0 = its offset
+// waited for; spilled = bytes per chunk that went through a spill slot):
+//   uniform bytes: {12800, 15, 2} 1.355-1.358 | {10240, 18, 1, P 16512} 1.259-1.270, 2.7 KB spilled |
+//   {9472, 20, 1, P 16512} 1.246-1.283, 4.4 KB spilled | {9472, 20, 1, P 2048} 1.237-1.241, 1.8 KB |
+//   {9472, 20, 1, P 1024} 1.212-1.214, 0.96 KB, a pending stream spilled from in 94 % of chunks |
+//   {9472, 20, 2, P 16512} 1.257-1.267 | {9472, 20, 1, P 0} 2.79-3.21 | {8560, 22, 2} 1.505 and {8560, 22, 1} 1.92
+//   (register spills); K2f 1.574.  The step alone: {12800, 15, 1} 1.158-1.166 | {10240, 18, 1} 1.039-1.050 |
+//   {9472, 20, 1} 0.981-0.988 | {8560, 22, 1} 0.942-0.950 | {7808, 24, 1} 0.908-0.917.
+//   text-like bytes (book1 histogram, nothing spilled at 20 warps): {12800, 15, 2} 1.358-1.365 | {10240, 18, 1}
+//   1.215-1.227 | {9472, 20, 1} 1.155-1.163 for every P but 0 (1.193-1.196) | {9472, 20, 2} 1.152-1.158 |
+//   {8560, 22, 2} 1.182-1.186 | {7808, 24, 2} 1.395-1.400 (with 12 480 B slots); K2f 1.200.
+// The sweep of the 15-warp design, H100 SXM at 400 W, 1 GiB uniform bytes, chunks of 8192, ms per call of the step alone (no placement:
 // tools/encode_ring_lab.cu), {ring bytes, warps, D}: {16384, 11, 1} 2.00 | {16384, 11, 2} 1.73 | {16384, 11, 4} 1.60 |
 // {14336, 13, 2} 1.32 | {14336, 13, 4} 1.33 | {13312, 14, 1} 1.23 | {13312, 14, 2} 1.24 | {13312, 14, 4} 1.26 |
 // {12800, 15, 1} 1.18 | {12800, 15, 2} 1.25 | {12800, 15, 4} 1.27; the split encoder (K2, 16 warps x 3 CTAs, streams
@@ -389,23 +403,35 @@ __device__ __forceinline__ uint32_t word_encode_stream_ring(const uint8_t* __res
 // (encode_ring.cuh) the order changes: {12800, 15, 2} 1.37-1.38 | {12800, 15, 1} 1.59-1.75 | {13312, 14, 1} 1.41-1.42 |
 // {14336, 13, 2} 1.50-1.51 | {16384, 11, 4} 1.76-1.77, against 1.70-1.71 for K2f in the same runs (two sessions).
 #ifndef RB200_RING_BYTES
-#define RB200_RING_BYTES 12800
+#define RB200_RING_BYTES 9472
 #endif
 #ifndef RB200_RING_WARPS
-#define RB200_RING_WARPS 15
+#define RB200_RING_WARPS 20
+#endif
+#ifndef RB200_RING_PEND_PIECE
+#define RB200_RING_PEND_PIECE 1024     // bytes of an unpublished pending stream spilled per step of making room (encode_ring.cuh)
 #endif
 #ifndef RB200_RING_AHEAD
-#define RB200_RING_AHEAD 2             // D: table entries loaded D steps ahead, symbols 2 D steps ahead
+#define RB200_RING_AHEAD 1             // D: table entries loaded D steps ahead, symbols 2 D steps ahead
 #endif
 constexpr uint32_t kEncRingStreamBytes = RB200_RING_BYTES, kEncRingWarps = RB200_RING_WARPS;
-constexpr uint32_t kEncRingMaxChunk = 8192;     // chunks of at most this many symbols have streams of at most kWordStreamMax bytes
+constexpr uint32_t kEncRingMaxChunk = 8192;     // chunks of at most this many symbols: a spill slot holds any of their streams
 constexpr uint32_t kEncRingSmemBytes = kEncTableBytes + kEncRingWarps * (kEncRingStreamBytes + kEncStageBytes);
 
+// Each worker warp's two spill slots (encode_ring.cuh), one worst-case stream each; the host sizes the workspace as
+// grid x kEncRingWarps of them (including the scanner warp's, unused).
+// A slot holds any stream of a chunk of kEncRingMaxChunk symbols, also one whose frequency-0 symbols make every step
+// emit a word (2 x 8192 + 128 B): such a call fails with kStatSymbol, but its spills stay inside the warp's own slots.
+constexpr uint32_t kEncRingSlotBytes = 2 * kEncRingMaxChunk + 128;
+constexpr uint32_t kEncRingSpillBytes = 2 * kEncRingSlotBytes;
+
 // The body of K2r at a given shape (the kernels below use RB200_RING_*): dynamic shared memory
-// [32 KiB table][W rings of RING bytes][W stages of 512 B].  Returns this warp's ring waits (encode_ring.cuh).
-template <bool R32, uint32_t RING, uint32_t W, uint32_t D>
-__device__ __forceinline__ uint32_t word_encode_ring(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms,
-                                                     const WordEncEntry* __restrict__ g_table, const PlaceOut& out, uint32_t* __restrict__ counter)
+// [32 KiB table][W rings of RING bytes][W stages of 512 B], and kEncRingSpillBytes per warp at `spill`.  Returns what
+// this warp's ring did (encode_ring.cuh).
+template <bool R32, uint32_t RING, uint32_t W, uint32_t D, uint32_t PEND_PIECE = RB200_RING_PEND_PIECE>
+__device__ __forceinline__ RingStats word_encode_ring(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms,
+                                                      const WordEncEntry* __restrict__ g_table, uint8_t* __restrict__ spill,
+                                                      const PlaceOut& out, uint32_t* __restrict__ counter)
 {
     extern __shared__ __align__(1024) uint8_t s_enc[];
     uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
@@ -413,21 +439,26 @@ __device__ __forceinline__ uint32_t word_encode_ring(const uint8_t* __restrict__
     __syncthreads();
     const uint32_t warp = threadIdx.x >> 5, tab = smem_addr(s_enc);
     const uint32_t ring = tab + kEncTableBytes + warp * RING, stage = tab + kEncTableBytes + W * RING + warp * kEncStageBytes;
+    uint8_t* slots = spill + (static_cast<uint64_t>(blockIdx.x) * W + warp) * kEncRingSpillBytes;
     uint32_t* status = out.status;
-    return encode_chunks_ring<RING>(in, n, chunk_syms, ring, out, counter, [=](const uint8_t* chunk_in, uint32_t m, StreamRing<RING>& q) {
+    using Ring = StreamRing<RING, kEncRingSlotBytes, PEND_PIECE>;
+    return encode_chunks_ring<RING, kEncRingSlotBytes, PEND_PIECE>(in, n, chunk_syms, ring, slots, out, counter,
+                                                                   [=](const uint8_t* chunk_in, uint32_t m, Ring& q) {
         return word_encode_stream_ring<R32, RING, D>(chunk_in, m, tab, stage, ring, q.top, q, status);
     });
 }
 
-// Grid = min(SMs, what the chunks need), sized by the host's encode plan; chunk_syms <= kEncRingMaxChunk.
+// Grid = min(SMs, what the chunks need), sized by the host's encode plan; chunk_syms <= kEncRingMaxChunk; spill: grid x
+// kEncRingWarps x kEncRingSpillBytes bytes.
 template <bool R32>
 __global__ void __launch_bounds__(kEncRingWarps * 32, 1)
 word_encode_ring_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
-                        const WordEncEntry* __restrict__ g_table, uint64_t* __restrict__ look, uint32_t* __restrict__ counter,
-                        uint8_t* __restrict__ blob, uint64_t blob_cap, uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
+                        const WordEncEntry* __restrict__ g_table, uint8_t* __restrict__ spill, uint64_t* __restrict__ look,
+                        uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap, uint64_t* __restrict__ offsets,
+                        uint32_t* __restrict__ status)
 {
-    word_encode_ring<R32, kEncRingStreamBytes, kEncRingWarps, RB200_RING_AHEAD>(in, n, chunk_syms, g_table,
-                                                                   PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
+    word_encode_ring<R32, kEncRingStreamBytes, kEncRingWarps, RB200_RING_AHEAD>(in, n, chunk_syms, g_table, spill,
+                                                                                PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
 }
 
 // ---------------------------------------------------------------------------

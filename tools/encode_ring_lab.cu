@@ -1,7 +1,10 @@
 // encode_ring_lab.cu -- timing bench for the fused word encoder with its streams in a shared-memory ring (K2r,
-// word_kernels.cuh) at several shapes {ring bytes, warps, prefetch distance D}, on 1 GiB of uniform bytes:
-//   ring_place:   K2r with placement; its blob and directory are checked against K2f's byte for byte, and the ring
-//                 waits (a pending stream placed before its offset was seen ready) are counted per chunk;
+// word_kernels.cuh) at several shapes {ring bytes, warps, prefetch distance D}, on 1 GiB of uniform bytes or of bytes
+// drawn from a histogram (--hist tests/golden/book1_hist.json: text-like):
+//   ring_place:   K2r with placement; its blob and directory are checked against K2f's byte for byte.  Per chunk: the
+//                 ring waits (a placement that waited for its offset), the pending streams spilled whole to the spill
+//                 slot (pieces of at most spill_pending bytes), and the bytes spilled.  spill_pending 0: a pending
+//                 stream waits for its offset instead;
 //   ring_noplace: the step alone: every warp encodes its chunks into its ring and only records their sizes (checked
 //                 against K2's), so the output is not a container.
 // Against them, in the same process on the same data: the split word encoder (K2, encode into global slots, no
@@ -10,9 +13,10 @@
 //
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Iinclude -Iryg_rans_b200/csrc \
 //        -o build/encode_ring_lab tools/encode_ring_lab.cu
-//   build/encode_ring_lab [--n BYTES] [--chunk SYMS] [--reps K]
+//   build/encode_ring_lab [--n BYTES] [--chunk SYMS] [--reps K] [--hist FILE]
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -37,14 +41,16 @@ __device__ __forceinline__ uint32_t mix32(uint64_t v)
     v ^= v >> 33; v *= 0xff51afd7ed558ccdull; v ^= v >> 33; v *= 0xc4ceb9fe1a85ec53ull; v ^= v >> 33;
     return static_cast<uint32_t>(v);
 }
-__global__ void gen_uniform_kernel(uint8_t* out, uint64_t n, uint64_t seed)
+// byte i = slot_sym[a 12-bit hash of i]: symbols drawn from the model's own distribution
+__global__ void gen_kernel(uint8_t* out, uint64_t n, uint64_t seed, const uint8_t* __restrict__ slot_sym)
 {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
-    for (uint64_t i = blockIdx.x * static_cast<uint64_t>(blockDim.x) + threadIdx.x; i < n; i += stride) out[i] = mix32(i + seed) >> 24;
+    for (uint64_t i = blockIdx.x * static_cast<uint64_t>(blockDim.x) + threadIdx.x; i < n; i += stride) out[i] = slot_sym[mix32(i + seed) >> 20];
 }
 
 struct NoSpace {
     __device__ __forceinline__ void reserve(uint32_t, uint32_t) {}
+    __device__ __forceinline__ uint32_t emitted(uint32_t e) const { return e; }
 };
 
 template <uint32_t RING, uint32_t W, uint32_t D>
@@ -74,22 +80,26 @@ ring_step_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms
     }
 }
 
-// K2r with placement at a given shape; adds up the warps' ring waits in *waits
-template <uint32_t RING, uint32_t W, uint32_t D>
+// K2r with placement at a given shape; adds up the warps' RingStats in stats[0..2]
+template <uint32_t RING, uint32_t W, uint32_t D, uint32_t SP>
 __global__ void __launch_bounds__(W * 32, 1)
 ring_place_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, const WordEncEntry* __restrict__ g_table,
-                  uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap,
-                  uint64_t* __restrict__ offsets, uint32_t* __restrict__ status, unsigned long long* __restrict__ waits)
+                  uint8_t* __restrict__ spill, uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob,
+                  uint64_t blob_cap, uint64_t* __restrict__ offsets, uint32_t* __restrict__ status, unsigned long long* __restrict__ stats)
 {
-    const uint32_t w = word_encode_ring<true, RING, W, D>(in, n, chunk_syms, g_table, PlaceOut{look, n_chunks, blob, blob_cap, offsets, status},
-                                                          counter);
-    if ((threadIdx.x & 31) == 0 && w) atomicAdd(waits, static_cast<unsigned long long>(w));
+    const RingStats s = word_encode_ring<true, RING, W, D, SP>(in, n, chunk_syms, g_table, spill,
+                                                               PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
+    if ((threadIdx.x & 31) == 0) {
+        if (s.waits) atomicAdd(stats, static_cast<unsigned long long>(s.waits));
+        if (s.pend_spills) atomicAdd(stats + 1, static_cast<unsigned long long>(s.pend_spills));
+        if (s.spilled_bytes) atomicAdd(stats + 2, static_cast<unsigned long long>(s.spilled_bytes));
+    }
 }
 
 struct Ctx {
     const uint8_t* in; uint64_t n; uint32_t chunk, n_chunks; const WordEncEntry* table; uint32_t* counter; uint32_t* sizes;
     uint32_t* ref_sizes; uint32_t* status; uint8_t* scratch; uint32_t slot; uint64_t* look; uint8_t* blob; uint64_t* offsets; int sms; int reps;
-    uint8_t* ref_blob; uint64_t* ref_offsets; unsigned long long* waits;
+    uint8_t* ref_blob; uint64_t* ref_offsets; unsigned long long* stats; uint8_t* spill;
 };
 
 template <class F>
@@ -149,24 +159,28 @@ bool same_container(const Ctx& c)
     return b == rb;
 }
 
-template <uint32_t RING, uint32_t W, uint32_t D>
+template <uint32_t RING, uint32_t W, uint32_t D, uint32_t SP>
 void run_place(const Ctx& c)
 {
+    static_assert(kEncTableBytes + W * (RING + kEncStageBytes) <= 227 * 1024, "shared memory");
     const uint32_t smem = kEncTableBytes + W * (RING + kEncStageBytes);
-    auto k = ring_place_kernel<RING, W, D>;
+    auto k = ring_place_kernel<RING, W, D, SP>;
     CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     CK(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     CK(cudaMemset(c.blob, 0, 2 * c.n));
     CK(cudaMemset(c.offsets, 0, (c.n_chunks + 1) * 8ull));
-    CK(cudaMemset(c.waits, 0, 8));
+    CK(cudaMemset(c.stats, 0, 24));
     const double ms = time_ms(c, [&] {
-        k<<<c.sms, W * 32, smem>>>(c.in, c.n, c.chunk, c.n_chunks, c.table, c.look, c.counter, c.blob, 2 * c.n, c.offsets, c.status, c.waits);
+        k<<<c.sms, W * 32, smem>>>(c.in, c.n, c.chunk, c.n_chunks, c.table, c.spill, c.look, c.counter, c.blob, 2 * c.n, c.offsets, c.status,
+                                   c.stats);
     }, true);
-    unsigned long long waits = 0;
-    CK(cudaMemcpy(&waits, c.waits, 8, cudaMemcpyDeviceToHost));
+    unsigned long long st[3] = {};
+    CK(cudaMemcpy(st, c.stats, 24, cudaMemcpyDeviceToHost));
     const bool ok = same_container(c);
-    std::printf("{\"variant\": \"ring_place\", \"ring\": %u, \"warps\": %u, \"D\": %u, \"ms\": %.4f, \"waits_per_chunk\": %.4f, "
-                "\"same_as_k2f\": %s}\n", RING, W, D, ms, static_cast<double>(waits) / (c.reps + 2) / c.n_chunks, ok ? "true" : "false");
+    const double per = 1.0 / (c.reps + 2) / c.n_chunks;
+    std::printf("{\"variant\": \"ring_place\", \"ring\": %u, \"warps\": %u, \"D\": %u, \"spill_pending\": %u, \"ms\": %.4f, "
+                "\"waits_per_chunk\": %.4f, \"pending_spills_per_chunk\": %.4f, \"spilled_bytes_per_chunk\": %.1f, \"same_as_k2f\": %s}\n",
+                RING, W, D, SP, ms, st[0] * per, st[1] * per, st[2] * per, ok ? "true" : "false");
     std::fflush(stdout);
 }
 
@@ -175,23 +189,64 @@ int main(int argc, char** argv)
     uint64_t n = 1ull << 30;
     uint32_t chunk = 8192;
     int reps = 10;
+    const char* hist = nullptr;
     for (int i = 1; i + 1 < argc; i += 2) {
         if (!std::strcmp(argv[i], "--n")) n = std::strtoull(argv[i + 1], nullptr, 0);
         else if (!std::strcmp(argv[i], "--chunk")) chunk = static_cast<uint32_t>(std::strtoul(argv[i + 1], nullptr, 0));
         else if (!std::strcmp(argv[i], "--reps")) reps = std::atoi(argv[i + 1]);
+        else if (!std::strcmp(argv[i], "--hist")) hist = argv[i + 1];
     }
     int dev = 0, sms = 0;
     CK(cudaGetDevice(&dev));
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, dev));
-    std::printf("{\"device\": \"%s\", \"sms\": %d, \"n\": %llu, \"chunk\": %u, \"reps\": %d}\n", prop.name, sms,
-                static_cast<unsigned long long>(n), chunk, reps);
+    // the card's power limit, read in the same process as the timings
+    char power[64] = "unknown";
+    if (FILE* smi = popen("nvidia-smi --query-gpu=power.limit,clocks.max.sm --format=csv,noheader -i 0", "r")) {
+        if (std::fgets(power, sizeof power, smi)) power[std::strcspn(power, "\n")] = 0;
+        pclose(smi);
+    }
+    std::printf("{\"power_limit_and_max_sm_clock\": \"%s\"}\n", power);
+    std::printf("{\"device\": \"%s\", \"sms\": %d, \"n\": %llu, \"chunk\": %u, \"reps\": %d, \"data\": \"%s\"}\n", prop.name, sms,
+                static_cast<unsigned long long>(n), chunk, reps, hist ? hist : "uniform");
 
-    // uniform model: every byte has frequency 4096 / 256
+    // the model: uniform (every byte 4096 / 256), or the "counts" of a histogram file scaled to 4096 (each seen byte
+    // at least 1, the rounding error on the most frequent one)
+    std::vector<uint32_t> freq(256, 16);
+    if (hist) {
+        FILE* f = std::fopen(hist, "rb");
+        if (!f) { std::fprintf(stderr, "cannot open %s\n", hist); return 2; }
+        std::string text;
+        char buf[4096];
+        for (size_t got; (got = std::fread(buf, 1, sizeof buf, f)) > 0;) text.append(buf, got);
+        std::fclose(f);
+        const size_t at = text.find("\"counts\"");
+        if (at == std::string::npos) { std::fprintf(stderr, "no counts in %s\n", hist); return 2; }
+        const char* q = std::strchr(text.c_str() + at, '[') + 1;
+        std::vector<double> cnt(256);
+        double total = 0;
+        for (int s = 0; s < 256; s++) {
+            char* e;
+            cnt[s] = std::strtod(q, &e);
+            q = e + 1;
+            total += cnt[s];
+        }
+        uint32_t sum = 0, top = 0;
+        for (int s = 0; s < 256; s++) {
+            freq[s] = cnt[s] > 0 ? std::max<uint32_t>(1, static_cast<uint32_t>(cnt[s] / total * 4096)) : 0;
+            sum += freq[s];
+            if (freq[s] > freq[top]) top = s;
+        }
+        freq[top] += 4096 - sum;
+    }
     std::vector<WordEncEntry> tab(256);
+    std::vector<uint8_t> slot_sym(4096);
     int exact = 1;
-    for (uint32_t s = 0; s < 256; s++) tab[s] = word_enc32_entry(16, s * 16, &exact);
+    for (uint32_t s = 0, cum = 0; s < 256; cum += freq[s], s++) {
+        tab[s] = word_enc32_entry(freq[s], cum, &exact);
+        for (uint32_t j = 0; j < freq[s]; j++) slot_sym[cum + j] = static_cast<uint8_t>(s);
+    }
 
     Ctx c = {};
     c.n = n; c.chunk = chunk; c.n_chunks = static_cast<uint32_t>((n + chunk - 1) / chunk); c.sms = sms; c.reps = reps;
@@ -201,7 +256,10 @@ int main(int argc, char** argv)
     CK(cudaMalloc(&d_in, n + 16));
     CK(cudaMalloc(&d_tab, 256 * sizeof(WordEncEntry)));
     CK(cudaMemcpy(d_tab, tab.data(), 256 * sizeof(WordEncEntry), cudaMemcpyHostToDevice));
-    gen_uniform_kernel<<<sms * 8, 256>>>(d_in, n, 12345);
+    uint8_t* d_slot_sym;
+    CK(cudaMalloc(&d_slot_sym, 4096));
+    CK(cudaMemcpy(d_slot_sym, slot_sym.data(), 4096, cudaMemcpyHostToDevice));
+    gen_kernel<<<sms * 8, 256>>>(d_in, n, 12345, d_slot_sym);
     CK(cudaGetLastError());
     c.in = d_in; c.table = d_tab;
     CK(cudaMalloc(&c.counter, 16));
@@ -215,7 +273,8 @@ int main(int argc, char** argv)
     CK(cudaMalloc(&c.offsets, (c.n_chunks + 1) * 8ull));
     CK(cudaMalloc(&c.ref_blob, n * 2));
     CK(cudaMalloc(&c.ref_offsets, (c.n_chunks + 1) * 8ull));
-    CK(cudaMalloc(&c.waits, 8));
+    CK(cudaMalloc(&c.stats, 24));
+    CK(cudaMalloc(&c.spill, static_cast<uint64_t>(sms) * 32 * kEncRingSpillBytes));     // up to 32 warps per CTA
 
     // K2, the split encoder: encode into global slots, no compaction
     configure_word_kernels();
@@ -237,22 +296,24 @@ int main(int argc, char** argv)
         CK(cudaMemcpy(c.ref_blob, c.blob, 2 * n, cudaMemcpyDeviceToDevice));
         CK(cudaMemcpy(c.ref_offsets, c.offsets, (c.n_chunks + 1) * 8ull, cudaMemcpyDeviceToDevice));
     }
-    run_place<12800, 15, 1>(c);
-    run_place<12800, 15, 2>(c);
-    run_place<13312, 14, 1>(c);
-    run_place<14336, 13, 2>(c);
-    run_place<16384, 11, 4>(c);
-    run_ring<16384, 11, 1>(c);
-    run_ring<16384, 11, 2>(c);
-    run_ring<16384, 11, 4>(c);
-    run_ring<14336, 13, 2>(c);
-    run_ring<14336, 13, 4>(c);
-    run_ring<13312, 14, 1>(c);
-    run_ring<13312, 14, 2>(c);
-    run_ring<13312, 14, 4>(c);
+    // shapes by occupancy (32 KiB + W x (ring + 512) <= 227 KiB; a ring of at least half a slot, so 20 warps at most)
+    // and how an unpublished pending stream is spilled (bytes per step of making room; 0: wait for its offset instead);
+    // two alternated passes with placement
+    for (int pass = 0; pass < 2; pass++) {
+        run_place<12800, 15, 2, kEncRingSlotBytes>(c);
+        run_place<10240, 18, 1, kEncRingSlotBytes>(c);
+        run_place<9472, 20, 1, kEncRingSlotBytes>(c);
+        run_place<9472, 20, 1, 2048>(c);
+        run_place<9472, 20, 1, 1024>(c);
+        run_place<9472, 20, 1, 0>(c);
+        run_place<9472, 20, 2, kEncRingSlotBytes>(c);
+    }
+    // the step alone.  A stream longer than the ring wraps over its own start (harmless here) and its size no longer
+    // matches K2's.
     run_ring<12800, 15, 1>(c);
-    run_ring<12800, 15, 2>(c);
-    run_ring<12800, 15, 4>(c);
+    run_ring<9472, 20, 1>(c);
+    run_ring<8560, 22, 1>(c);
+    run_ring<7808, 24, 1>(c);
     uint32_t st = 0;
     CK(cudaMemcpy(&st, c.status, 4, cudaMemcpyDeviceToHost));
     std::printf("{\"status\": %u}\n", st);
