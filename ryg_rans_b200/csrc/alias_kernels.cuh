@@ -464,33 +464,26 @@ __device__ __forceinline__ void alias_encode(const uint8_t* __restrict__ in, uin
                                                                  PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
 }
 
-template <bool ALIAS, uint32_t SB>
+// GEOM (rb200_container_model_encode_varlen_async): n, the chunk count, the blob's place in the container `blob` and
+// its capacity from the record, on the grid the host sized for n_max.  In split mode a CTA past the real chunks exits
+// before it stages its tables; in fused mode every CTA runs (CTA 0 holds the scanner, the others find no chunk and leave).
+template <bool ALIAS, uint32_t SB, bool GEOM = false>
 __global__ void __launch_bounds__(kAliasEncWarps * 32, 1)
 alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb_rt,
                     const AliasEncEntry* __restrict__ g_enc, const uint16_t* __restrict__ g_remap,
                     uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
                     uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap,
-                    uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
+                    uint64_t* __restrict__ offsets, uint32_t* __restrict__ status, const VarlenGeom* __restrict__ geom)
 {
+    if (GEOM) {
+        n_chunks = geom->n_chunks;
+        if (!geom->go || (!look && blockIdx.x * kAliasEncWarps >= n_chunks)) return;
+        n = geom->n;
+        blob += geom->blob_off;
+        blob_cap = geom->blob_cap;
+    }
     alias_encode<ALIAS, SB>(in, n, chunk_syms, n_chunks, sb_rt, g_enc, g_remap, scratch, slot_bytes, sizes, look, counter, blob, blob_cap,
                             offsets, status);
-}
-
-// rb200_container_model_encode_varlen_async: n, the chunk count, the blob's place in the container `out` and its
-// capacity from the record, on the grid the host sized for n_max.  In split mode a CTA past the real chunks exits before
-// it stages its tables; in fused mode every CTA runs (CTA 0 holds the scanner, the others find no chunk and leave).
-template <bool ALIAS, uint32_t SB>
-__global__ void __launch_bounds__(kAliasEncWarps * 32, 1)
-alias_encode_varlen_kernel(const uint8_t* __restrict__ in, uint32_t chunk_syms, const VarlenGeom* __restrict__ geom, uint32_t sb_rt,
-                           const AliasEncEntry* __restrict__ g_enc, const uint16_t* __restrict__ g_remap,
-                           uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
-                           uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ out,
-                           uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
-{
-    const uint32_t n_chunks = geom->n_chunks;
-    if (!geom->go || (!look && blockIdx.x * kAliasEncWarps >= n_chunks)) return;
-    alias_encode<ALIAS, SB>(in, geom->n, chunk_syms, n_chunks, sb_rt, g_enc, g_remap, scratch, slot_bytes, sizes, look, counter,
-                            out + geom->blob_off, geom->blob_cap, offsets, status);
 }
 
 // dynamic shared memory of the alias (remap != nullptr) or byte encoder at scale_bits sb
@@ -504,8 +497,8 @@ inline void configure_alias_encode()
 {
     cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, alias_encode_smem(ALIAS, 16));
-    cudaFuncSetAttribute(alias_encode_varlen_kernel<ALIAS, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(alias_encode_varlen_kernel<ALIAS, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, alias_encode_smem(ALIAS, 16));
+    cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, alias_encode_smem(ALIAS, 16));
 }
 template <uint32_t SB>
 inline void configure_byte_decode()
@@ -544,35 +537,21 @@ inline void configure_alias_kernels()
 
 // remap == nullptr selects the rans_byte cum2sym coder.  look == nullptr: split mode (sizes[] out, one slot per
 // chunk); otherwise fused mode (kAliasFusedSlots slots per worker warp; look/counter zeroed by the caller).
-// grid <= one CTA per SM (the kernel is persistent), smem = alias_encode_smem(remap != nullptr, sb).
+// grid <= one CTA per SM (the kernel is persistent), smem = alias_encode_smem(remap != nullptr, sb).  geom set: the
+// GEOM instance, with n, n_chunks and the grid those of n_max and blob the container.
 inline void launch_alias_encode(cudaStream_t stream, uint32_t grid, uint32_t smem, const uint8_t* d_in, uint64_t n, uint32_t chunk_syms,
                                 uint32_t n_chunks, uint32_t sb, const AliasEncEntry* enc, const uint16_t* remap, uint8_t* scratch,
                                 uint32_t slot, uint32_t* sizes, uint64_t* look, uint32_t* counter, uint8_t* blob, uint64_t blob_cap,
-                                uint64_t* offsets, uint32_t* status)
+                                uint64_t* offsets, uint32_t* status, const VarlenGeom* geom)
 {
+    auto kernel = alias_encode_kernel<false, 0>;
     if (remap) {
-        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_kernel<true, SB><<<grid, kAliasEncWarps * 32, smem, stream>>>(
-            d_in, n, chunk_syms, n_chunks, sb, enc, remap, scratch, slot, sizes, look, counter, blob, blob_cap, offsets, status)))
+        RB200_ALIAS_SB_DISPATCH(sb, (kernel = geom ? alias_encode_kernel<true, SB, true> : alias_encode_kernel<true, SB>))
     } else {
-        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_kernel<false, SB><<<grid, kAliasEncWarps * 32, smem, stream>>>(
-            d_in, n, chunk_syms, n_chunks, sb, enc, nullptr, scratch, slot, sizes, look, counter, blob, blob_cap, offsets, status)))
+        RB200_ALIAS_SB_DISPATCH(sb, (kernel = geom ? alias_encode_kernel<false, SB, true> : alias_encode_kernel<false, SB>))
     }
-}
-
-// launch_alias_encode for rb200_container_model_encode_varlen_async: n, n_chunks and the blob from `geom`, the blob in
-// `out`; grid and mode fixed by the host for n_max
-inline void launch_alias_encode_varlen(cudaStream_t stream, uint32_t grid, uint32_t smem, const uint8_t* d_in, uint32_t chunk_syms,
-                                       const VarlenGeom* geom, uint32_t sb, const AliasEncEntry* enc, const uint16_t* remap,
-                                       uint8_t* scratch, uint32_t slot, uint32_t* sizes, uint64_t* look, uint32_t* counter, uint8_t* out,
-                                       uint64_t* offsets, uint32_t* status)
-{
-    if (remap) {
-        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_varlen_kernel<true, SB><<<grid, kAliasEncWarps * 32, smem, stream>>>(
-            d_in, chunk_syms, geom, sb, enc, remap, scratch, slot, sizes, look, counter, out, offsets, status)))
-    } else {
-        RB200_ALIAS_SB_DISPATCH(sb, (alias_encode_varlen_kernel<false, SB><<<grid, kAliasEncWarps * 32, smem, stream>>>(
-            d_in, chunk_syms, geom, sb, enc, nullptr, scratch, slot, sizes, look, counter, out, offsets, status)))
-    }
+    kernel<<<grid, kAliasEncWarps * 32, smem, stream>>>(d_in, n, chunk_syms, n_chunks, sb, enc, remap, scratch, slot, sizes, look, counter,
+                                                        blob, blob_cap, offsets, status, geom);
 }
 
 // the persistent kernel: sms x 2 CTAs of 20 warps, chunk ids from the context's work counter

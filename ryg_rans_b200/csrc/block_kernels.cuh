@@ -26,8 +26,15 @@ constexpr int kHistWarps = 8;
 // The 32 lanes of a shared-memory atomic therefore never share a bank -- whatever the symbols are: uniform data no
 // longer pays the ~3.5 wavefronts of 32 random banks, skewed data no longer serialises on one hot counter (round 1's
 // per-warp copies did both and ran at 2.6 TB/s).  All warps of the CTA add into the same 32 KiB.
-__device__ __forceinline__ void histogram(const uint8_t* __restrict__ in, uint64_t n, unsigned long long* __restrict__ counts)
+// GEOM (rb200_container_model_encode_varlen_async): the length from the record (VarlenGeom), on the grid of n_max.
+template <bool GEOM = false>
+__global__ void __launch_bounds__(kHistWarps * 32)
+histogram_kernel(const uint8_t* __restrict__ in, uint64_t n, unsigned long long* __restrict__ counts, const VarlenGeom* __restrict__ geom)
 {
+    if (GEOM) {
+        if (!geom->go) return;
+        n = geom->n;
+    }
     __shared__ uint32_t s_h[256 * 32];
     for (uint32_t i = threadIdx.x; i < 256 * 32; i += blockDim.x) s_h[i] = 0;
     __syncthreads();
@@ -69,33 +76,16 @@ __device__ __forceinline__ void histogram(const uint8_t* __restrict__ in, uint64
     }
 }
 
-__global__ void __launch_bounds__(kHistWarps * 32)
-histogram_kernel(const uint8_t* __restrict__ in, uint64_t n, unsigned long long* __restrict__ counts)
-{
-    histogram(in, n, counts);
-}
-
-// rb200_container_model_encode_varlen_async: the length from the record (VarlenGeom), on the grid of n_max
-__global__ void __launch_bounds__(kHistWarps * 32)
-histogram_varlen_kernel(const uint8_t* __restrict__ in, const VarlenGeom* __restrict__ geom, unsigned long long* __restrict__ counts)
-{
-    if (!geom->go) return;
-    histogram(in, geom->n, counts);
-}
-
-// the histogram's grid for n symbols
-inline uint32_t histogram_grid(uint32_t sms, uint64_t n)
+// geom set: the GEOM instance, with n = n_max sizing the grid
+inline void launch_histogram(cudaStream_t stream, uint32_t sms, const uint8_t* d_in, uint64_t n, unsigned long long* d_counts,
+                             const VarlenGeom* geom = nullptr)
 {
     const uint64_t want = (n / 16 + kHistWarps * 32 - 1) / (kHistWarps * 32);
     // keep each block's per-bin count below 2^32: >= 1 block per 2^31 bytes is plenty
     uint64_t grid = static_cast<uint64_t>(sms) * 8;
     if (want < grid) grid = want ? want : 1;
-    return static_cast<uint32_t>(grid);
-}
-
-inline void launch_histogram(cudaStream_t stream, uint32_t sms, const uint8_t* d_in, uint64_t n, unsigned long long* d_counts)
-{
-    histogram_kernel<<<histogram_grid(sms, n), kHistWarps * 32, 0, stream>>>(d_in, n, d_counts);
+    auto kernel = geom ? histogram_kernel<true> : histogram_kernel<false>;
+    kernel<<<static_cast<uint32_t>(grid), kHistWarps * 32, 0, stream>>>(d_in, n, d_counts, geom);
 }
 
 // ---------------------------------------------------------------------------

@@ -270,9 +270,21 @@ inline uint32_t crc32_grid(uint32_t sms, uint64_t n)
 // the blob's CRC is in slots[1].  Reads blob_bytes from the directory, completes the header (h arrives with
 // blob_bytes and both CRCs zero), and writes the head and the zero pad in front of the blob -- only when the status
 // word is clear (an encoder error leaves the buffer as it is) and the blob fits out_cap (else it flags kStatSpace).
-__device__ __forceinline__ void container_finish(uint8_t* out, const ContainerHeader& h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
-                                                 const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status)
+// GEOM (rb200_container_model_encode_varlen_async, version 1): n_symbols, n_chunks and the blob offset from the record
+// (VarlenGeom); h arrives with coder, scale_bits, chunk_syms and flags.  Writes nothing when geom->go == 0.
+template <bool GEOM = false>
+__global__ void __launch_bounds__(32)
+    container_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
+                            const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status,
+                            const VarlenGeom* __restrict__ geom)
 {
+    if (GEOM) {
+        if (!geom->go) return;
+        h.n_symbols = geom->n;
+        h.n_chunks = geom->n_chunks;
+        dir_off = kContainerDirOffset;
+        blob_off = geom->blob_off;
+    }
     using namespace crc_detail;
     __shared__ uint4 sbuf_v[kContainerDirOffset / 16];
     uint32_t* sbuf = reinterpret_cast<uint32_t*>(sbuf_v);
@@ -308,25 +320,6 @@ __device__ __forceinline__ void container_finish(uint8_t* out, const ContainerHe
     uint4* dst = reinterpret_cast<uint4*>(out);
     for (uint32_t i = lane; i < head / 16; i += 32) dst[i] = sbuf_v[i];
     if (lane == 0 && blob_off > dir_end) *reinterpret_cast<uint64_t*>(out + dir_end) = 0;   // the 8-byte pad
-}
-
-__global__ void __launch_bounds__(32)
-    container_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
-                            const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status)
-{
-    container_finish(out, h, dir_off, blob_off, out_cap, freqs, slots, status);
-}
-
-// The same for rb200_container_model_encode_varlen_async (version 1): n_symbols, n_chunks and the blob offset from the
-// record (VarlenGeom); h arrives with coder, scale_bits, chunk_syms and flags.  Writes nothing when geom->go == 0.
-__global__ void __launch_bounds__(32)
-    container_finish_varlen_kernel(uint8_t* out, ContainerHeader h, const VarlenGeom* __restrict__ geom, uint64_t out_cap,
-                                   const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status)
-{
-    if (!geom->go) return;
-    h.n_symbols = geom->n;
-    h.n_chunks = geom->n_chunks;
-    container_finish(out, h, kContainerDirOffset, geom->blob_off, out_cap, freqs, slots, status);
 }
 
 }  // namespace rb200

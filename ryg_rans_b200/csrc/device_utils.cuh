@@ -16,8 +16,9 @@ constexpr uint32_t kStatArg    = 32u;  // a length read from device memory is ou
 constexpr uint32_t kHeaderBytes = 128; // 32 lanes x u32 final state (RansWordEncFlush / RansEncFlush x 32)
 
 // The geometry of rb200_container_model_encode_varlen_async, which reads the input length from device memory: written
-// by varlen_plan_kernel (model_kernels.cuh) from *d_n at every run, read at entry by every kernel after it, which all
-// exit when go == 0.  The launch shapes are the host's, sized for n_max; everything that depends on n is here.
+// by varlen_plan_kernel (model_kernels.cuh) from *d_n at every run, read at entry by every kernel after it (the GEOM
+// instances of the C4 kernels), which all exit when go == 0.  The launch shapes are the host's, sized for n_max;
+// everything that depends on n is here.
 struct VarlenGeom {
     uint64_t n;            // symbols, 1 <= n <= n_max
     uint64_t dir_len;      // directory bytes, 8 (n_chunks + 1)

@@ -8,15 +8,15 @@
 //                               (block_normalize); the checks of rb200_model_create (kStatModel on refusal); the coder's
 //                               encode tables, byte for byte what rb200_model_create uploads (tables.h formulas)
 //   the coder's encoder         the shipped kernel with its table pointers into the workspace.  The word coder runs
-//                               both instances of its gated wrappers below; r32 names the one that encodes, the other
-//                               exits before it touches the counter, look[] or scratch
+//                               both GATED instances of K2 or K2f (word_kernels.cuh); r32 names the one that encodes,
+//                               the other exits before it touches the counter, look[] or scratch
 //   crc32_kernel x 1-2, container_finish_kernel
 //                               as rb200_container_encode in device memory, with the model section from freqs[]
 //
 // rb200_container_model_encode_varlen_async runs the same stages on launch shapes the host sizes for a bound n_max,
 // and reads the length from device memory: varlen_plan_kernel checks *d_n and writes the geometry record (VarlenGeom,
-// device_utils.cuh) into geom; every later kernel takes n, the chunk count and the blob's place from there and exits
-// at entry when the checks failed.  The encoders are the *_varlen_kernel instances, which call the same drivers.
+// device_utils.cuh) into geom; every later kernel is the GEOM instance of the same kernel, which takes n, the chunk
+// count and the blob's place from there and exits at entry when the checks failed.
 #pragma once
 #include "block_kernels.cuh"
 #include "container_format.h"
@@ -47,9 +47,13 @@ constexpr int kModelThreads = 256;                // one thread per symbol
 // well-formed entries, and container_finish_kernel writes no header).  Normalisation itself cannot fail for targets
 // >= 256: a squashed symbol needs a donor of width > 1, and while any symbol is squashed the widths, which sum to the
 // target, cannot all be <= 1.  block_normalize keeps its check all the same, with kStatModel as the verdict.
-__device__ __forceinline__ void container_model(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w,
-                                                uint32_t* __restrict__ status)
+// GEOM (the device-length call): with *d_n == 0 the counts are all zero and normalisation has no total to scale, so it
+// runs only when the plan passed.
+template <bool GEOM = false>
+__global__ void __launch_bounds__(kModelThreads)
+    container_model_kernel(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w, uint32_t* __restrict__ status)
 {
+    if (GEOM && !w->geom.go) return;
     __shared__ uint32_t s_cnt[256], s_cum[257];
     __shared__ __align__(16) uint32_t s_w[256];
     __shared__ uint32_t s_divider[256], s_adjust[512], s_slot_freqs[512], s_rest[256], s_given[256];
@@ -107,22 +111,6 @@ __device__ __forceinline__ void container_model(uint32_t coder, uint32_t sb, uin
     }
 }
 
-__global__ void __launch_bounds__(kModelThreads)
-    container_model_kernel(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w, uint32_t* __restrict__ status)
-{
-    container_model(coder, sb, r32_allowed, w, status);
-}
-
-// The varlen call's instance: with *d_n == 0 the counts are all zero and normalisation has no total to scale, so it
-// runs only when the plan passed
-__global__ void __launch_bounds__(kModelThreads)
-    container_model_varlen_kernel(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w,
-                                  uint32_t* __restrict__ status)
-{
-    if (!w->geom.go) return;
-    container_model(coder, sb, r32_allowed, w, status);
-}
-
 // The first kernel of rb200_container_model_encode_varlen_async, one warp: reads n = *d_n, checks 1 <= n <= n_max
 // (n == 0 is kStatModel, as the fixed call's RB200_E_MODEL; n > n_max is kStatArg) and writes the geometry of a
 // version 1 container of n symbols into *g, with go = 1 when the checks pass.  On failure *g is zero: every later
@@ -153,103 +141,6 @@ __global__ void __launch_bounds__(32)
 __global__ void __launch_bounds__(32) varlen_blob_len_kernel(const uint64_t* __restrict__ dir, VarlenGeom* __restrict__ g)
 {
     if (threadIdx.x == 0 && g->go) g->blob_len = dir[g->n_chunks];
-}
-
-// The word encoders behind the gate: word_encode_kernel / word_encode_fused_kernel, run only when *gate (the model
-// kernel's r32) names this instance.  The host launches both instances of the call's path.
-template <bool R32>
-__global__ void __launch_bounds__(kEncWarps * 32, RB200_ENC_MINBLOCKS)
-word_encode_gated_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
-                         const WordEncEntry* __restrict__ g_table, const uint32_t* __restrict__ gate, uint8_t* __restrict__ scratch,
-                         uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
-{
-    if (*gate != (R32 ? 1u : 0u)) return;                          // the same for the whole grid
-    extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
-    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
-    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
-    __syncthreads();
-
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint32_t chunk = blockIdx.x * kEncWarps + warp;
-    if (chunk >= n_chunks) return;
-    const ChunkRange r = chunk_range(chunk, chunk_syms, n);
-    encode_chunk_split(in + r.first, r.m, chunk, WordEncoder<R32>{smem_addr(s_enc)}, smem_addr(s_enc) + kEncTableBytes + warp * kEncWarpSmem,
-                       scratch, slot_bytes, sizes, status);
-}
-
-template <bool R32>
-__global__ void __launch_bounds__(kEncWarps * 32, RB200_FUSED_MINBLOCKS)
-word_encode_fused_gated_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
-                               const WordEncEntry* __restrict__ g_table, const uint32_t* __restrict__ gate, uint8_t* __restrict__ scratch,
-                               uint32_t slot_bytes, uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob,
-                               uint64_t blob_cap, uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
-{
-    if (*gate != (R32 ? 1u : 0u)) return;                          // the same for the whole grid
-    extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
-    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
-    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
-    __syncthreads();
-
-    const uint32_t tab = smem_addr(s_enc), wsm = tab + kEncTableBytes + (threadIdx.x >> 5) * kEncWarpSmem;
-    encode_chunks_fused<kFusedSlots, kEncWarps, RB200_ENC_KEEP_HINT>(in, n, chunk_syms, WordEncoder<R32>{tab}, wsm, scratch, slot_bytes,
-                                                                     PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
-}
-
-// The varlen call's word encoders: the gated wrappers above with n, the chunk count and the blob's place (in the
-// container `out`) from the record, on the grid the host sized for n_max.  A split-path CTA past the real chunks exits
-// before it stages its table.
-template <bool R32>
-__global__ void __launch_bounds__(kEncWarps * 32, RB200_ENC_MINBLOCKS)
-word_encode_gated_varlen_kernel(const uint8_t* __restrict__ in, uint32_t chunk_syms, const VarlenGeom* __restrict__ geom,
-                                const WordEncEntry* __restrict__ g_table, const uint32_t* __restrict__ gate, uint8_t* __restrict__ scratch,
-                                uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
-{
-    const uint32_t n_chunks = geom->n_chunks;
-    if (!geom->go || *gate != (R32 ? 1u : 0u) || blockIdx.x * kEncWarps >= n_chunks) return;   // the same for the whole CTA
-    extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
-    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
-    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
-    __syncthreads();
-
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint32_t chunk = blockIdx.x * kEncWarps + warp;
-    if (chunk >= n_chunks) return;
-    const ChunkRange r = chunk_range(chunk, chunk_syms, geom->n);
-    encode_chunk_split(in + r.first, r.m, chunk, WordEncoder<R32>{smem_addr(s_enc)}, smem_addr(s_enc) + kEncTableBytes + warp * kEncWarpSmem,
-                       scratch, slot_bytes, sizes, status);
-}
-
-template <bool R32>
-__global__ void __launch_bounds__(kEncWarps * 32, RB200_FUSED_MINBLOCKS)
-word_encode_fused_gated_varlen_kernel(const uint8_t* __restrict__ in, uint32_t chunk_syms, const VarlenGeom* __restrict__ geom,
-                                      const WordEncEntry* __restrict__ g_table, const uint32_t* __restrict__ gate, uint8_t* __restrict__ scratch,
-                                      uint32_t slot_bytes, uint64_t* __restrict__ look, uint32_t* __restrict__ counter,
-                                      uint8_t* __restrict__ out, uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
-{
-    if (!geom->go || *gate != (R32 ? 1u : 0u)) return;             // the same for the whole grid
-    extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
-    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
-    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
-    __syncthreads();
-
-    const uint32_t tab = smem_addr(s_enc), wsm = tab + kEncTableBytes + (threadIdx.x >> 5) * kEncWarpSmem;
-    encode_chunks_fused<kFusedSlots, kEncWarps, RB200_ENC_KEEP_HINT>(
-        in, geom->n, chunk_syms, WordEncoder<R32>{tab}, wsm, scratch, slot_bytes,
-        PlaceOut{look, geom->n_chunks, out + geom->blob_off, geom->blob_cap, offsets, status}, counter);
-}
-
-inline void configure_model_kernels()
-{
-    for (const void* k : {reinterpret_cast<const void*>(word_encode_gated_kernel<false>), reinterpret_cast<const void*>(word_encode_gated_kernel<true>),
-                          reinterpret_cast<const void*>(word_encode_fused_gated_kernel<false>),
-                          reinterpret_cast<const void*>(word_encode_fused_gated_kernel<true>),
-                          reinterpret_cast<const void*>(word_encode_gated_varlen_kernel<false>),
-                          reinterpret_cast<const void*>(word_encode_gated_varlen_kernel<true>),
-                          reinterpret_cast<const void*>(word_encode_fused_gated_varlen_kernel<false>),
-                          reinterpret_cast<const void*>(word_encode_fused_gated_varlen_kernel<true>)}) {
-        cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
-    }
 }
 
 }  // namespace rb200

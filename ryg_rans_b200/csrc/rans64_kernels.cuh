@@ -129,13 +129,25 @@ struct Rans64Encoder {
     }
 };
 
+// GEOM (rb200_container_model_encode_varlen_async): n and the chunk count from the record, on a grid sized for n_max; a
+// CTA past the real chunks exits before it stages the table
+template <bool GEOM = false>
 __global__ void __launch_bounds__(kRans64Warps * 32, 2)
 rans64_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb,
                      const uint4* __restrict__ g_enc,      // 256 x 2 x uint4
-                     uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
+                     uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status,
+                     const VarlenGeom* __restrict__ geom)
 {
-    extern __shared__ __align__(1024) uint8_t s_r64e[];      // [16 x 1 KiB stage + ring][32 KiB table, 8 replicas]
-    uint4* s_tab = reinterpret_cast<uint4*>(s_r64e + kRans64Warps * kEncWarpSmem);
+    if (GEOM) {
+        n_chunks = geom->n_chunks;
+        if (!geom->go || blockIdx.x * kRans64Warps >= n_chunks) return;
+    }
+    // [16 x 1 KiB stage + ring][32 KiB table, 8 replicas].  Each instance has its own name for it: with one name for
+    // both, ptxas schedules the GEOM = false instance differently.
+    extern __shared__ __align__(1024) uint8_t s_r64e[];
+    extern __shared__ __align__(1024) uint8_t s_r64v[];
+    uint8_t* const s_enc = GEOM ? s_r64v : s_r64e;
+    uint4* s_tab = reinterpret_cast<uint4*>(s_enc + kRans64Warps * kEncWarpSmem);
     for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) {
         const uint4 a = g_enc[2 * (i / kEncReplicas)], b = g_enc[2 * (i / kEncReplicas) + 1];   // {rcp_lo, rcp_hi, freq, bias}, {cmpl, shift | bad, -, -}
         s_tab[i] = make_uint4(a.x, a.y, a.w, (b.x & 0xfffffu) | ((b.y & 63u) << 20) | (b.y & kEncBadSymbol));
@@ -145,33 +157,9 @@ rans64_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_
     const uint32_t warp = threadIdx.x >> 5;
     const uint32_t chunk = blockIdx.x * kRans64Warps + warp;
     if (chunk >= n_chunks) return;
+    if (GEOM) n = geom->n;
     const ChunkRange r = chunk_range(chunk, chunk_syms, n);
-    encode_chunk_split(in + r.first, r.m, chunk, Rans64Encoder{smem_addr(s_tab), sb}, smem_addr(s_r64e) + warp * kEncWarpSmem, scratch,
-                       slot_bytes, sizes, status);
-}
-
-// rb200_container_model_encode_varlen_async: n and the chunk count from the record, on a grid sized for n_max; a CTA
-// past the real chunks exits before it stages the table
-__global__ void __launch_bounds__(kRans64Warps * 32, 2)
-rans64_encode_varlen_kernel(const uint8_t* __restrict__ in, uint32_t chunk_syms, const VarlenGeom* __restrict__ geom, uint32_t sb,
-                            const uint4* __restrict__ g_enc, uint8_t* __restrict__ scratch, uint32_t slot_bytes,
-                            uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
-{
-    const uint32_t n_chunks = geom->n_chunks;
-    if (!geom->go || blockIdx.x * kRans64Warps >= n_chunks) return;
-    extern __shared__ __align__(1024) uint8_t s_r64v[];      // as rans64_encode_kernel (its own name: a second user of s_r64e reorders that kernel's code)
-    uint4* s_tab = reinterpret_cast<uint4*>(s_r64v + kRans64Warps * kEncWarpSmem);
-    for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) {
-        const uint4 a = g_enc[2 * (i / kEncReplicas)], b = g_enc[2 * (i / kEncReplicas) + 1];
-        s_tab[i] = make_uint4(a.x, a.y, a.w, (b.x & 0xfffffu) | ((b.y & 63u) << 20) | (b.y & kEncBadSymbol));
-    }
-    __syncthreads();
-
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint32_t chunk = blockIdx.x * kRans64Warps + warp;
-    if (chunk >= n_chunks) return;
-    const ChunkRange r = chunk_range(chunk, chunk_syms, geom->n);
-    encode_chunk_split(in + r.first, r.m, chunk, Rans64Encoder{smem_addr(s_tab), sb}, smem_addr(s_r64v) + warp * kEncWarpSmem, scratch,
+    encode_chunk_split(in + r.first, r.m, chunk, Rans64Encoder{smem_addr(s_tab), sb}, smem_addr(s_enc) + warp * kEncWarpSmem, scratch,
                        slot_bytes, sizes, status);
 }
 constexpr uint32_t kRans64EncSmemBytes = kRans64Warps * kEncWarpSmem + kEncTableBytes;     // dynamic shared memory of the encoder
@@ -180,10 +168,10 @@ inline void configure_rans64_kernels()
 {
     cudaFuncSetAttribute(rans64_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRans64Warps * kRingBytes + kRans64DecSymBytes + (1u << 16));
     cudaFuncSetAttribute(rans64_decode_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(rans64_encode_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(rans64_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRans64EncSmemBytes);
-    cudaFuncSetAttribute(rans64_encode_varlen_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(rans64_encode_varlen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRans64EncSmemBytes);
+    for (const void* k : {reinterpret_cast<const void*>(rans64_encode_kernel<false>), reinterpret_cast<const void*>(rans64_encode_kernel<true>)}) {
+        cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kRans64EncSmemBytes);
+    }
 }
 
 inline void launch_rans64_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets, uint32_t sb,

@@ -257,7 +257,6 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     ctx->blocks_async = configure_container_decode(static_cast<uint32_t>(ctx->sms));
     configure_single_decode(static_cast<uint32_t>(ctx->sms), ctx->single_decoders);
     configure_blocks_coder_decode(static_cast<uint32_t>(ctx->sms), ctx->blocks_coder_decoders);
-    configure_model_kernels();
     cudaGetLastError();
     *out = ctx;
     return RB200_OK;
@@ -453,27 +452,31 @@ extern "C" size_t rb200_encode_bound(size_t n, uint32_t chunk_syms)
 namespace {
 
 
-// directory + compaction after any encode kernel: sizes[] -> offsets[] + blob
+// directory + compaction after any encode kernel: sizes[] -> offsets[] + blob.  geom set: the GEOM instances, on grids
+// sized for n_chunks (the bound's), with d_blob the container.
 int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* sizes, uint64_t* tile_sums, uint32_t n_chunks,
-                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets)
+                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom)
 {
     if (!n_chunks) {
         RB_CUDA(ctx, cudaMemsetAsync(d_offsets, 0, sizeof(uint64_t), ctx->stream));
         return RB200_OK;
     }
     const uint32_t tiles = (n_chunks + kScanTile - 1) / kScanTile;
-    scan_tiles_kernel<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, d_offsets, tile_sums);
+    auto scan = geom ? scan_tiles_kernel<true> : scan_tiles_kernel<false>;
+    scan<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, d_offsets, tile_sums, geom);
     int rc = check_launch(ctx, "scan_tiles_kernel");
     if (rc != RB200_OK) return rc;
     const uint32_t prefixed = tiles > kTilePrefixThreshold ? 1u : 0u;
     if (prefixed) {
-        tile_prefix_kernel<<<1, 1024, 0, ctx->stream>>>(tile_sums, tiles);
+        auto prefix = geom ? tile_prefix_kernel<true> : tile_prefix_kernel<false>;
+        prefix<<<1, 1024, 0, ctx->stream>>>(tile_sums, tiles, geom);
         rc = check_launch(ctx, "tile_prefix_kernel");
         if (rc != RB200_OK) return rc;
     }
     const uint32_t grid = (n_chunks + kCopyWarps - 1) / kCopyWarps;
-    compact_kernel<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, d_offsets, tile_sums, prefixed, n_chunks, d_blob,
-                                                               blob_cap, ctx->d_status);
+    auto compact = geom ? compact_kernel<true> : compact_kernel<false>;
+    compact<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, d_offsets, tile_sums, prefixed, n_chunks, d_blob, blob_cap,
+                                                        ctx->d_status, geom);
     return check_launch(ctx, "compact_kernel");
 }
 
@@ -612,9 +615,10 @@ int prepare_workspace(rb200_ctx* ctx, const EncodePlan& p, EncodeWorkspace* ws)
 }
 
 // Runs a plan: prepare its workspace; fused: `launch(ws)`, the one kernel; split: `launch(ws)` encodes into the slots
-// (when there are chunks), then finish_encode.  `launch` returns check_launch's code.
+// (when there are chunks), then finish_encode (geom: as there).  `launch` returns check_launch's code.
 template <class Launch>
-int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, Launch launch)
+int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom,
+               Launch launch)
 {
     EncodeWorkspace ws = {};
     int rc = prepare_workspace(ctx, p, &ws);
@@ -624,11 +628,11 @@ int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob
         rc = launch(ws);
         if (rc != RB200_OK) return rc;
     }
-    return finish_encode(ctx, ws.scratch, p.slot_bytes, ws.sizes, ws.tile_sums, p.n_chunks, d_blob, blob_cap, d_offsets);
+    return finish_encode(ctx, ws.scratch, p.slot_bytes, ws.sizes, ws.tile_sums, p.n_chunks, d_blob, blob_cap, d_offsets, geom);
 }
 
 // The encode tables of one encode call, in device memory.  Word: `word_gate` null runs the instance word_r32 names on
-// word[word_r32]; set, both gated instances run (model_kernels.cuh), each on its own table, and *word_gate picks one.
+// word[word_r32]; set, both GATED instances run (word_kernels.cuh), each on its own table, and *word_gate picks one.
 struct EncodeTables {
     int coder;
     uint32_t scale_bits;
@@ -648,33 +652,17 @@ EncodeTables model_tables(const rb200_model* m)
                         word_ring_model(m->freqs)};
 }
 
+// geom set (rb200_container_model_encode_varlen_async): n is the bound n_max, which fixes the plan and every launch
+// shape, the GEOM instances read n, the chunk count and the blob's place from the record, and d_blob is the container.
 int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, size_t n, uint32_t chunk_syms, uint8_t* d_blob,
-                  size_t blob_cap, uint64_t* d_offsets)
+                  size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom = nullptr)
 {
     const size_t n_chunks_sz = rb200_chunk_count(n, chunk_syms);
     if (n_chunks_sz >= (1ull << 31)) return RB200_E_ARG;
     const uint32_t n_chunks = static_cast<uint32_t>(n_chunks_sz);
     const EncodePlan p = plan_encode(ctx, t.coder, t.scale_bits, n_chunks, chunk_syms, t.word_ring);
-    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, [&](const EncodeWorkspace& ws) {
+    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, geom, [&](const EncodeWorkspace& ws) {
         if (t.coder == RB200_CODER_WORD) {
-            if (t.word_gate) {
-                int rc = RB200_OK;
-                for (int r32 = 0; r32 < 2 && rc == RB200_OK; r32++) {
-                    if (p.fused) {
-                        auto kernel = r32 ? word_encode_fused_gated_kernel<true> : word_encode_fused_gated_kernel<false>;
-                        kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], t.word_gate, ws.scratch,
-                                                                           p.slot_bytes, ws.look, ws.counter, d_blob, blob_cap, d_offsets,
-                                                                           ctx->d_status);
-                        rc = check_launch(ctx, "word_encode_fused_gated_kernel");
-                    } else {
-                        auto kernel = r32 ? word_encode_gated_kernel<true> : word_encode_gated_kernel<false>;
-                        kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], t.word_gate, ws.scratch,
-                                                                           p.slot_bytes, ws.sizes, ctx->d_status);
-                        rc = check_launch(ctx, "word_encode_gated_kernel");
-                    }
-                }
-                return rc;
-            }
             const WordEncEntry* table = t.word[t.word_r32 ? 1 : 0];
             if (p.ring) {
                 auto kernel = t.word_r32 ? word_encode_ring_kernel<true> : word_encode_ring_kernel<false>;
@@ -682,80 +670,39 @@ int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, si
                                                                    d_blob, blob_cap, d_offsets, ctx->d_status);
                 return check_launch(ctx, "word_encode_ring_kernel");
             }
-            if (p.fused) {
-                auto kernel = t.word_r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>;
-                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.scratch, p.slot_bytes,
-                                                                   ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status);
-                return check_launch(ctx, "word_encode_fused_kernel");
+            // the instance word_r32 names, or both GATED ones
+            int rc = RB200_OK;
+            const int r32_first = t.word_gate ? 0 : t.word_r32, r32_last = t.word_gate ? 1 : t.word_r32;
+            for (int r32 = r32_first; r32 <= r32_last && rc == RB200_OK; r32++) {
+                if (p.fused) {
+                    auto kernel = !t.word_gate ? (r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>)
+                                  : !geom  ? (r32 ? word_encode_fused_kernel<true, true> : word_encode_fused_kernel<false, true>)
+                                           : (r32 ? word_encode_fused_kernel<true, true, true> : word_encode_fused_kernel<false, true, true>);
+                    kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], ws.scratch, p.slot_bytes, ws.look,
+                                                                       ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status, t.word_gate, geom);
+                    rc = check_launch(ctx, "word_encode_fused_kernel");
+                } else {
+                    auto kernel = !t.word_gate ? (r32 ? word_encode_kernel<true> : word_encode_kernel<false>)
+                                  : !geom  ? (r32 ? word_encode_kernel<true, true> : word_encode_kernel<false, true>)
+                                           : (r32 ? word_encode_kernel<true, true, true> : word_encode_kernel<false, true, true>);
+                    kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], ws.scratch, p.slot_bytes, ws.sizes,
+                                                                       ctx->d_status, t.word_gate, geom);
+                    rc = check_launch(ctx, "word_encode_kernel");
+                }
             }
-            auto kernel = t.word_r32 ? word_encode_kernel<true> : word_encode_kernel<false>;
-            kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.scratch, p.slot_bytes,
-                                                               ws.sizes, ctx->d_status);
-            return check_launch(ctx, "word_encode_kernel");
+            return rc;
         }
         if (t.coder == RB200_CODER_RANS64) {
-            rans64_encode_kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.scale_bits, t.r64,
-                                                                             ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status);
+            auto kernel = geom ? rans64_encode_kernel<true> : rans64_encode_kernel<false>;
+            kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.scale_bits, t.r64, ws.scratch, p.slot_bytes,
+                                                               ws.sizes, ctx->d_status, geom);
             return check_launch(ctx, "rans64_encode_kernel");
         }
         const bool alias = t.coder == RB200_CODER_ALIAS;
         launch_alias_encode(ctx->stream, p.grid, p.smem, d_in, n, chunk_syms, n_chunks, t.scale_bits, t.enc, alias ? t.remap : nullptr,
-                            ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status);
+                            ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status, geom);
         return check_launch(ctx, alias ? "alias_encode_kernel" : "byte_encode_kernel");
     });
-}
-
-// encode_device for rb200_container_model_encode_varlen_async, on a GPU-built model (t.word_gate set): the plan of
-// n_chunks_max chunks fixes the path and every launch shape, and each kernel reads n, the chunk count and the blob's
-// place in the container `out` from `geom`.  Split: the tile scan, the tile prefix when n_max's tiles pass the
-// threshold, and the compaction, all on the device's chunk count.
-int encode_device_varlen(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, uint32_t n_chunks_max, uint32_t chunk_syms,
-                         const VarlenGeom* geom, uint8_t* out, uint64_t* d_offsets)
-{
-    const EncodePlan p = plan_encode(ctx, t.coder, t.scale_bits, n_chunks_max, chunk_syms, false);
-    EncodeWorkspace ws = {};
-    int rc = prepare_workspace(ctx, p, &ws);
-    if (rc != RB200_OK) return rc;
-    cudaStream_t s = ctx->stream;
-    if (t.coder == RB200_CODER_WORD) {
-        for (int r32 = 0; r32 < 2 && rc == RB200_OK; r32++) {
-            if (p.fused) {
-                auto kernel = r32 ? word_encode_fused_gated_varlen_kernel<true> : word_encode_fused_gated_varlen_kernel<false>;
-                kernel<<<p.grid, p.threads, p.smem, s>>>(d_in, chunk_syms, geom, t.word[r32], t.word_gate, ws.scratch, p.slot_bytes, ws.look,
-                                                         ws.counter, out, d_offsets, ctx->d_status);
-                rc = check_launch(ctx, "word_encode_fused_gated_varlen_kernel");
-            } else {
-                auto kernel = r32 ? word_encode_gated_varlen_kernel<true> : word_encode_gated_varlen_kernel<false>;
-                kernel<<<p.grid, p.threads, p.smem, s>>>(d_in, chunk_syms, geom, t.word[r32], t.word_gate, ws.scratch, p.slot_bytes, ws.sizes,
-                                                         ctx->d_status);
-                rc = check_launch(ctx, "word_encode_gated_varlen_kernel");
-            }
-        }
-    } else if (t.coder == RB200_CODER_RANS64) {
-        rans64_encode_varlen_kernel<<<p.grid, p.threads, p.smem, s>>>(d_in, chunk_syms, geom, t.scale_bits, t.r64, ws.scratch, p.slot_bytes,
-                                                                      ws.sizes, ctx->d_status);
-        rc = check_launch(ctx, "rans64_encode_varlen_kernel");
-    } else {
-        const bool alias = t.coder == RB200_CODER_ALIAS;
-        launch_alias_encode_varlen(s, p.grid, p.smem, d_in, chunk_syms, geom, t.scale_bits, t.enc, alias ? t.remap : nullptr, ws.scratch,
-                                   p.slot_bytes, ws.sizes, ws.look, ws.counter, out, d_offsets, ctx->d_status);
-        rc = check_launch(ctx, "alias_encode_varlen_kernel");
-    }
-    if (rc != RB200_OK || p.fused) return rc;
-    const uint32_t tiles = (n_chunks_max + kScanTile - 1) / kScanTile;
-    scan_tiles_varlen_kernel<<<tiles, 1024, 0, s>>>(ws.sizes, geom, d_offsets, ws.tile_sums);
-    rc = check_launch(ctx, "scan_tiles_varlen_kernel");
-    if (rc != RB200_OK) return rc;
-    const uint32_t prefixed = tiles > kTilePrefixThreshold ? 1u : 0u;
-    if (prefixed) {
-        tile_prefix_varlen_kernel<<<1, 1024, 0, s>>>(ws.tile_sums, geom);
-        rc = check_launch(ctx, "tile_prefix_varlen_kernel");
-        if (rc != RB200_OK) return rc;
-    }
-    const uint32_t grid = (n_chunks_max + kCopyWarps - 1) / kCopyWarps;
-    compact_varlen_kernel<<<grid, kCopyWarps * 32, 0, s>>>(ws.scratch, p.slot_bytes, ws.sizes, d_offsets, ws.tile_sums, prefixed, geom, out,
-                                                           ctx->d_status);
-    return check_launch(ctx, "compact_varlen_kernel");
 }
 
 int decode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_blob, size_t blob_size, const uint64_t* d_offsets,
@@ -1239,7 +1186,7 @@ int blocks_encode_device(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* 
 {
     if (static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) >= (1ull << 31)) return RB200_E_ARG;
     const EncodePlan p = plan_blocks_encode(ctx, coder, n_blocks, block_size, chunk_syms, build_models);
-    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, [&](const EncodeWorkspace& ws) {
+    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, nullptr, [&](const EncodeWorkspace& ws) {
         if (coder != RB200_CODER_WORD) {
             launch_block_coder_encode(ctx->stream, static_cast<uint32_t>(coder), sb, build_models, p.grid, p.threads, p.smem, d_in, block_size,
                                       d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status);
@@ -1586,7 +1533,7 @@ extern "C" int rb200_container_encode(rb200_ctx* ctx, const rb200_model* model, 
         if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
         if (rc != RB200_OK) return rc;
-        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, model->d_freqs, ctx->d_crc, ctx->d_status);
+        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, model->d_freqs, ctx->d_crc, ctx->d_status, nullptr);
         return check_launch(ctx, "container_finish_kernel");
     }
     size_t blob_bytes = 0, slices = 0;
@@ -1639,7 +1586,7 @@ int container_blocks_encode_impl(rb200_ctx* ctx, ContainerHeader h, const uint8_
         if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
         if (rc != RB200_OK) return rc;
-        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, nullptr, ctx->d_crc, ctx->d_status);
+        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, nullptr, ctx->d_crc, ctx->d_status, nullptr);
         return check_launch(ctx, "container_finish_kernel");
     }
     if (!build) std::memcpy(model, block_freqs, model_bytes);
@@ -1825,83 +1772,75 @@ EncodeTables workspace_tables(ModelAsyncWork* w, int coder, uint32_t scale_bits)
                         coder == RB200_CODER_ALIAS ? w->alias_enc : w->byte_enc, w->alias_remap, w->r64_enc};
 }
 
+// The body of both model encodes (model_kernels.cuh): histogram, model kernel, the coder's encoder, the CRCs and the
+// header.  d_n null: n symbols, every length by value.  d_n set: n is the bound n_max, which sizes every launch; the plan
+// kernel reads *d_n into the record at every run, and every later kernel is its GEOM instance.
+int model_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, size_t n, const uint64_t* d_n, uint32_t chunk_syms,
+                 uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
+    const ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n, n_chunks, 0, flags);
+    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
+    if (out_cap < boff) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    cudaStream_t s = ctx->stream;
+    ModelAsyncWork* w = ctx->d_model_async;
+    VarlenGeom* geom = d_n ? &w->geom : nullptr;
+    int rc = RB200_OK;
+    if (geom) {
+        varlen_plan_kernel<<<1, 32, 0, s>>>(d_n, n, chunk_syms, out_cap, geom, ctx->d_status);
+        rc = check_launch(ctx, "varlen_plan_kernel");
+        if (rc != RB200_OK) return rc;
+    }
+    RB_CUDA(ctx, cudaMemsetAsync(w->counts, 0, sizeof w->counts, s));
+    launch_histogram(s, static_cast<uint32_t>(ctx->sms), in, n, w->counts, geom);
+    rc = check_launch(ctx, "histogram_kernel");
+    if (rc != RB200_OK) return rc;
+    auto model = geom ? container_model_kernel<true> : container_model_kernel<false>;
+    model<<<1, kModelThreads, 0, s>>>(static_cast<uint32_t>(coder), scale_bits, word_r32_allowed() ? 1u : 0u, w, ctx->d_status);
+    rc = check_launch(ctx, "container_model_kernel");
+    if (rc != RB200_OK) return rc;
+    const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
+    rc = encode_device(ctx, workspace_tables(w, coder, scale_bits), in, n, chunk_syms, geom ? out : out + boff, out_cap - boff, dir, geom);
+    if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, geom ? &geom->dir_len : nullptr, 0, ctx->d_crc);
+    if (rc == RB200_OK && blob_crc) {
+        if (geom) {
+            varlen_blob_len_kernel<<<1, 32, 0, s>>>(dir, geom);
+            rc = check_launch(ctx, "varlen_blob_len_kernel");
+            if (rc == RB200_OK) rc = launch_crc(ctx, out, out_cap, &geom->blob_len, 0, ctx->d_crc + 1, &geom->blob_off);
+        } else {
+            rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+        }
+    }
+    if (rc != RB200_OK) return rc;
+    auto finish = geom ? container_finish_kernel<true> : container_finish_kernel<false>;
+    finish<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, w->freqs, ctx->d_crc, ctx->d_status, geom);
+    return check_launch(ctx, "container_finish_kernel");
+}
+
 }  // namespace
 
-// rb200_model_from_data + rb200_container_encode (device memory) + rb200_model_destroy with kernels alone
-// (model_kernels.cuh): histogram, model kernel, the coder's encoder, the CRCs and the header.  Five to seven launches and
-// one memset, no copy, no synchronisation; the encode workspace grows as in rb200_container_encode.
+// rb200_model_from_data + rb200_container_encode (device memory) + rb200_model_destroy with kernels alone: five to seven
+// launches and one memset, no copy, no synchronisation; the encode workspace grows as in rb200_container_encode.
 extern "C" int rb200_container_model_encode_async(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, size_t n,
                                                   uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
 {
     if (!model_encode_args_ok(ctx, coder, scale_bits, in, n, chunk_syms, out)) return RB200_E_ARG;
-    const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
     if (n == 0) return RB200_E_MODEL;                                // normalize_freqs divides by the total
-    ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n, n_chunks, 0, flags);
-    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
-    if (out_cap < boff) return RB200_E_SPACE;
-    DeviceGuard g(ctx->device);
-    ModelAsyncWork* w = ctx->d_model_async;
-    RB_CUDA(ctx, cudaMemsetAsync(w->counts, 0, sizeof w->counts, ctx->stream));
-    launch_histogram(ctx->stream, static_cast<uint32_t>(ctx->sms), in, n, w->counts);
-    int rc = check_launch(ctx, "histogram_kernel");
-    if (rc != RB200_OK) return rc;
-    container_model_kernel<<<1, kModelThreads, 0, ctx->stream>>>(static_cast<uint32_t>(coder), scale_bits, word_r32_allowed() ? 1u : 0u, w,
-                                                                 ctx->d_status);
-    rc = check_launch(ctx, "container_model_kernel");
-    if (rc != RB200_OK) return rc;
-    const EncodeTables t = workspace_tables(w, coder, scale_bits);
-    const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
-    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
-    rc = encode_device(ctx, t, in, n, chunk_syms, out + boff, out_cap - boff, dir);
-    if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, nullptr, 0, ctx->d_crc);
-    if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
-    if (rc != RB200_OK) return rc;
-    container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, w->freqs, ctx->d_crc, ctx->d_status);
-    return check_launch(ctx, "container_finish_kernel");
+    return model_encode(ctx, coder, scale_bits, in, n, nullptr, chunk_syms, flags, out, out_cap);
 }
 
-// rb200_container_model_encode_async with the length read from device memory at every run (model_kernels.cuh): the plan
-// kernel, then the same stages on launch shapes sized for n_max, each taking the length from the plan's record.  Eight
-// to eleven launches and one or two memsets, no copy, no synchronisation; the workspace grows as the fixed call's for n_max.
+// rb200_container_model_encode_async with the length read from device memory at every run: the plan kernel, then the
+// same stages on launch shapes sized for n_max, each taking the length from the plan's record.  Eight to eleven launches
+// and one or two memsets, no copy, no synchronisation; the workspace grows as the fixed call's for n_max.
 extern "C" int rb200_container_model_encode_varlen_async(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in,
                                                          const uint64_t* d_n, size_t n_max, uint32_t chunk_syms, uint32_t flags,
                                                          uint8_t* out, size_t out_cap)
 {
     if (!d_n || (reinterpret_cast<uintptr_t>(d_n) & 7) || n_max == 0) return RB200_E_ARG;
     if (!model_encode_args_ok(ctx, coder, scale_bits, in, n_max, chunk_syms, out)) return RB200_E_ARG;
-    const uint32_t n_chunks_max = static_cast<uint32_t>(rb200_chunk_count(n_max, chunk_syms));
-    ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n_max, n_chunks_max, 0, flags);
-    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h);
-    if (out_cap < container_blob_offset(h)) return RB200_E_SPACE;
-    DeviceGuard g(ctx->device);
-    cudaStream_t s = ctx->stream;
-    ModelAsyncWork* w = ctx->d_model_async;
-    VarlenGeom* geom = &w->geom;
-    varlen_plan_kernel<<<1, 32, 0, s>>>(d_n, n_max, chunk_syms, out_cap, geom, ctx->d_status);
-    int rc = check_launch(ctx, "varlen_plan_kernel");
-    if (rc != RB200_OK) return rc;
-    RB_CUDA(ctx, cudaMemsetAsync(w->counts, 0, sizeof w->counts, s));
-    histogram_varlen_kernel<<<histogram_grid(static_cast<uint32_t>(ctx->sms), n_max), kHistWarps * 32, 0, s>>>(in, geom, w->counts);
-    rc = check_launch(ctx, "histogram_varlen_kernel");
-    if (rc != RB200_OK) return rc;
-    container_model_varlen_kernel<<<1, kModelThreads, 0, s>>>(static_cast<uint32_t>(coder), scale_bits, word_r32_allowed() ? 1u : 0u, w,
-                                                              ctx->d_status);
-    rc = check_launch(ctx, "container_model_varlen_kernel");
-    if (rc != RB200_OK) return rc;
-    const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
-    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
-    rc = encode_device_varlen(ctx, workspace_tables(w, coder, scale_bits), in, n_chunks_max, chunk_syms, geom, out, dir);
-    if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, &geom->dir_len, 0, ctx->d_crc);
-    if (rc == RB200_OK && blob_crc) {
-        varlen_blob_len_kernel<<<1, 32, 0, s>>>(dir, geom);
-        rc = check_launch(ctx, "varlen_blob_len_kernel");
-        if (rc == RB200_OK) rc = launch_crc(ctx, out, out_cap, &geom->blob_len, 0, ctx->d_crc + 1, &geom->blob_off);
-    }
-    if (rc != RB200_OK) return rc;
-    h.n_symbols = 0;                                   // the finish kernel fills in n and n_chunks from the record
-    h.n_chunks = 0;
-    container_finish_varlen_kernel<<<1, 32, 0, s>>>(out, h, geom, out_cap, w->freqs, ctx->d_crc, ctx->d_status);
-    return check_launch(ctx, "container_finish_varlen_kernel");
+    return model_encode(ctx, coder, scale_bits, in, n_max, d_n, chunk_syms, flags, out, out_cap);
 }
 
 // ---------------------------------------------------------------------------

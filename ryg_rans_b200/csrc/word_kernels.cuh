@@ -144,12 +144,22 @@ struct WordEncoder {
 #ifndef RB200_ENC_MINBLOCKS
 #define RB200_ENC_MINBLOCKS 3
 #endif
-template <bool R32>
+// The instances of rb200_container_model_encode_async and its device-length form (model_kernels.cuh), which the flags
+// select; with both off, gate and geom are unused.
+//   GATED: run only when *gate (the model kernel's r32) names this instance.  The host launches both instances, and
+//          the other one exits at entry, before it touches shared memory, the counter, look[] or scratch.
+//   GEOM:  n, the chunk count, and on the fused path the blob's place in the container `blob` and its capacity come from
+//          the record (VarlenGeom), on a grid sized for n_max; nothing runs when geom->go == 0.  A split-path CTA past
+//          the real chunks exits before it stages its table.
+template <bool R32, bool GATED = false, bool GEOM = false>
 __global__ void __launch_bounds__(kEncWarps * 32, RB200_ENC_MINBLOCKS)
 word_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
                    const WordEncEntry* __restrict__ g_table, uint8_t* __restrict__ scratch, uint32_t slot_bytes,
-                   uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
+                   uint32_t* __restrict__ sizes, uint32_t* __restrict__ status, const uint32_t* __restrict__ gate,
+                   const VarlenGeom* __restrict__ geom)
 {
+    if (GEOM) n_chunks = geom->n_chunks;
+    if ((GEOM && !geom->go) || (GATED && *gate != (R32 ? 1u : 0u)) || (GEOM && blockIdx.x * kEncWarps >= n_chunks)) return;
     extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
     uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
     for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
@@ -158,6 +168,7 @@ word_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_sy
     const uint32_t warp = threadIdx.x >> 5;
     const uint32_t chunk = blockIdx.x * kEncWarps + warp;
     if (chunk >= n_chunks) return;
+    if (GEOM) n = geom->n;
     const ChunkRange r = chunk_range(chunk, chunk_syms, n);
     encode_chunk_split(in + r.first, r.m, chunk, WordEncoder<R32>{smem_addr(s_enc)}, smem_addr(s_enc) + kEncTableBytes + warp * kEncWarpSmem,
                        scratch, slot_bytes, sizes, status);
@@ -169,20 +180,29 @@ constexpr uint32_t kEncSmemBytes = kEncTableBytes + kEncWarps * kEncWarpSmem;
 // K2f: persistent encode with the directory and the compaction fused in (the protocol: placement.cuh).
 // ---------------------------------------------------------------------------
 // Grid = resident capacity (SMs x RB200_FUSED_MINBLOCKS CTAs, sized by the host's encode plan).  Warp 0 of CTA 0 is the
-// scanner, every other warp is a worker with kFusedSlots scratch slots (encode_chunks_fused).
-template <bool R32>
+// scanner, every other warp is a worker with kFusedSlots scratch slots (encode_chunks_fused).  GATED, GEOM: as
+// word_encode_kernel; with GEOM every CTA runs.
+template <bool R32, bool GATED = false, bool GEOM = false>
 __global__ void __launch_bounds__(kEncWarps * 32, RB200_FUSED_MINBLOCKS)
 word_encode_fused_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks,
                          const WordEncEntry* __restrict__ g_table, uint8_t* __restrict__ scratch, uint32_t slot_bytes,
                          uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap,
-                         uint64_t* __restrict__ offsets, uint32_t* __restrict__ status)
+                         uint64_t* __restrict__ offsets, uint32_t* __restrict__ status, const uint32_t* __restrict__ gate,
+                         const VarlenGeom* __restrict__ geom)
 {
+    if ((GEOM && !geom->go) || (GATED && *gate != (R32 ? 1u : 0u))) return;     // the same for the whole grid
     extern __shared__ __align__(1024) uint8_t s_enc[];     // [32 KiB table][warps x 1 KiB]
     uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
     for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) s_tab[i] = word_enc_expand<R32>(g_table[i / kEncReplicas]);
     __syncthreads();
 
     const uint32_t tab = smem_addr(s_enc), wsm = tab + kEncTableBytes + (threadIdx.x >> 5) * kEncWarpSmem;
+    if (GEOM) {
+        n = geom->n;
+        n_chunks = geom->n_chunks;
+        blob += geom->blob_off;
+        blob_cap = geom->blob_cap;
+    }
     encode_chunks_fused<kFusedSlots, kEncWarps, RB200_ENC_KEEP_HINT>(in, n, chunk_syms, WordEncoder<R32>{tab}, wsm, scratch, slot_bytes,
                                                                      PlaceOut{look, n_chunks, blob, blob_cap, offsets, status}, counter);
 }
@@ -471,10 +491,19 @@ word_encode_ring_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chu
 // ---------------------------------------------------------------------------
 constexpr uint32_t kScanTile = 4096;
 
-// pass 1 for tile blockIdx.x (one CTA of 1024 threads)
-__device__ __forceinline__ void scan_tile(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
-                                          uint64_t* __restrict__ tile_sums)
+// GEOM (rb200_container_model_encode_varlen_async): grids sized for n_max, the chunk count, the blob's place in the
+// container `blob` and its capacity from the record (VarlenGeom, device_utils.cuh); CTAs past the real tiles or chunks
+// exit at entry.  The host fixes whether tile_prefix_kernel runs from n_max's tile count; the prefix and the compaction
+// then both use the device's, which gives the same sums as either choice.
+template <bool GEOM = false>
+__global__ void __launch_bounds__(1024)
+scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
+                  uint64_t* __restrict__ tile_sums, const VarlenGeom* __restrict__ geom)
 {
+    if (GEOM) {
+        n_chunks = geom->n_chunks;
+        if (!geom->go || blockIdx.x * kScanTile >= n_chunks) return;
+    }
     __shared__ uint64_t s_warp[32];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t c0 = blockIdx.x * kScanTile + tid * 4;
@@ -510,17 +539,15 @@ __device__ __forceinline__ void scan_tile(const uint32_t* __restrict__ sizes, ui
     if (tid == 1023) tile_sums[blockIdx.x] = s_warp[31];
 }
 
+// for very large directories: turn tile_sums into exclusive prefixes once, so compact CTAs read one value
+template <bool GEOM = false>
 __global__ void __launch_bounds__(1024)
-scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
-                  uint64_t* __restrict__ tile_sums)
+tile_prefix_kernel(uint64_t* __restrict__ tile_sums, uint32_t n_tiles, const VarlenGeom* __restrict__ geom)
 {
-    scan_tile(sizes, n_chunks, offsets, tile_sums);
-}
-
-// for very large directories: turn tile_sums into exclusive prefixes once, so compact CTAs read one value (one CTA of
-// 1024 threads)
-__device__ __forceinline__ void tile_prefix(uint64_t* __restrict__ tile_sums, uint32_t n_tiles)
-{
+    if (GEOM) {
+        if (!geom->go) return;
+        n_tiles = (geom->n_chunks + kScanTile - 1) / kScanTile;
+    }
     __shared__ uint64_t s_warp[32];
     __shared__ uint64_t s_carry;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -553,21 +580,23 @@ __device__ __forceinline__ void tile_prefix(uint64_t* __restrict__ tile_sums, ui
     }
 }
 
-__global__ void __launch_bounds__(1024)
-tile_prefix_kernel(uint64_t* __restrict__ tile_sums, uint32_t n_tiles)
-{
-    tile_prefix(tile_sums, n_tiles);
-}
-
 constexpr int kCopyWarps = 8;
 constexpr uint32_t kTilePrefixThreshold = 256;   // above this many tiles, tile_prefix_kernel runs first
 
 // one warp moves one chunk stream from the end of its scratch slot to blob[offsets[c]..E_c)
-__device__ __forceinline__ void compact_chunks(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
-                                               uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums,
-                                               uint32_t tiles_prefixed, uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap,
-                                               uint32_t* __restrict__ status)
+template <bool GEOM = false>
+__global__ void __launch_bounds__(kCopyWarps * 32)
+compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+               uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
+               uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status,
+               const VarlenGeom* __restrict__ geom)
 {
+    if (GEOM) {
+        n_chunks = geom->n_chunks;
+        if (!geom->go || blockIdx.x * kCopyWarps >= n_chunks) return;
+        blob += geom->blob_off;
+        blob_cap = geom->blob_cap;
+    }
     __shared__ uint64_t s_base;
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t chunk0 = blockIdx.x * kCopyWarps;
@@ -599,55 +628,23 @@ __device__ __forceinline__ void compact_chunks(const uint8_t* __restrict__ scrat
     if (end <= blob_cap) place_stream<false>(scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, size, blob, end, lane);
 }
 
-__global__ void __launch_bounds__(kCopyWarps * 32)
-compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
-               uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
-               uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status)
+// the K2 and K2f instances: (R32, GATED, GEOM) = (r32, 0, 0) for an rb200_model, (r32, 1, 0) and (r32, 1, 1) for the
+// model encodes
+template <bool R32, bool GATED, bool GEOM>
+inline void configure_word_encode()
 {
-    compact_chunks(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, blob, blob_cap, status);
-}
-
-// The split path's directory and compaction for rb200_container_model_encode_varlen_async: grids sized for n_max, the
-// chunk count, the blob's place and its capacity from the record (VarlenGeom, device_utils.cuh).  CTAs past the real
-// tiles or chunks exit at entry.  The host fixes whether tile_prefix runs from n_max's tile count; the prefix and the
-// compaction then both use the device's, which gives the same sums as either choice.
-__global__ void __launch_bounds__(1024)
-scan_tiles_varlen_kernel(const uint32_t* __restrict__ sizes, const VarlenGeom* __restrict__ geom, uint64_t* __restrict__ offsets,
-                         uint64_t* __restrict__ tile_sums)
-{
-    const uint32_t n_chunks = geom->n_chunks;
-    if (!geom->go || blockIdx.x * kScanTile >= n_chunks) return;
-    scan_tile(sizes, n_chunks, offsets, tile_sums);
-}
-
-__global__ void __launch_bounds__(1024)
-tile_prefix_varlen_kernel(uint64_t* __restrict__ tile_sums, const VarlenGeom* __restrict__ geom)
-{
-    if (!geom->go) return;
-    tile_prefix(tile_sums, (geom->n_chunks + kScanTile - 1) / kScanTile);
-}
-
-// out = the container: the blob starts geom->blob_off bytes into it
-__global__ void __launch_bounds__(kCopyWarps * 32)
-compact_varlen_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
-                      uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
-                      const VarlenGeom* __restrict__ geom, uint8_t* __restrict__ out, uint32_t* __restrict__ status)
-{
-    const uint32_t n_chunks = geom->n_chunks;
-    if (!geom->go || blockIdx.x * kCopyWarps >= n_chunks) return;
-    compact_chunks(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, out + geom->blob_off, geom->blob_cap, status);
+    for (const void* k : {reinterpret_cast<const void*>(word_encode_kernel<R32, GATED, GEOM>),
+                          reinterpret_cast<const void*>(word_encode_fused_kernel<R32, GATED, GEOM>)}) {
+        cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+    }
 }
 
 inline void configure_word_kernels()
 {
-    cudaFuncSetAttribute(word_encode_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_encode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
-    cudaFuncSetAttribute(word_encode_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_encode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
-    cudaFuncSetAttribute(word_encode_fused_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_encode_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
-    cudaFuncSetAttribute(word_encode_fused_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(word_encode_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+    configure_word_encode<false, false, false>(); configure_word_encode<true, false, false>();
+    configure_word_encode<false, true, false>(); configure_word_encode<true, true, false>();
+    configure_word_encode<false, true, true>(); configure_word_encode<true, true, true>();
     cudaFuncSetAttribute(word_encode_ring_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(word_encode_ring_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncRingSmemBytes);
     cudaFuncSetAttribute(word_encode_ring_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);

@@ -281,7 +281,7 @@ int main(int argc, char** argv)
     {
         const double ms = time_ms(c, [&] {
             word_encode_kernel<true><<<(c.n_chunks + kEncWarps - 1) / kEncWarps, kEncWarps * 32, kEncSmemBytes>>>(
-                c.in, c.n, c.chunk, c.n_chunks, c.table, c.scratch, c.slot, c.ref_sizes, c.status);
+                c.in, c.n, c.chunk, c.n_chunks, c.table, c.scratch, c.slot, c.ref_sizes, c.status, nullptr, nullptr);
         }, false);
         std::printf("{\"variant\": \"k2_split_encode\", \"ms\": %.4f}\n", ms);
     }
@@ -290,7 +290,7 @@ int main(int argc, char** argv)
         const uint32_t grid = sms * RB200_FUSED_MINBLOCKS;
         const double ms = time_ms(c, [&] {
             word_encode_fused_kernel<true><<<grid, kEncWarps * 32, kEncSmemBytes>>>(c.in, c.n, c.chunk, c.n_chunks, c.table, c.scratch, c.slot,
-                                                                                    c.look, c.counter, c.blob, 2 * n, c.offsets, c.status);
+                                                                                    c.look, c.counter, c.blob, 2 * n, c.offsets, c.status, nullptr, nullptr);
         }, true);
         std::printf("{\"variant\": \"k2f_fused_shipped\", \"ms\": %.4f}\n", ms);
         CK(cudaMemcpy(c.ref_blob, c.blob, 2 * n, cudaMemcpyDeviceToDevice));

@@ -42,9 +42,9 @@ def main():
     lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "ryg_rans_b200", "librans_b200.so")
     fns = functions(subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout)
     dec = next(v for k, v in fns.items() if "block_decode_kernel" in k)
-    enc = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1" in k)
-    enc_gated = next(v for k, v in fns.items() if "word_encode_fused_gated_kernelILb1" in k)
-    enc_varlen = next(v for k, v in fns.items() if "word_encode_fused_gated_varlen_kernelILb1" in k)
+    enc = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1ELb0ELb0E" in k)
+    enc_gated = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1ELb1ELb0E" in k)
+    enc_varlen = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1ELb1ELb1E" in k)
     tma = next(v for k, v in fns.items() if "word_decode_tma_kernel" in k and k.endswith("Lb0EEEvPKhmPKmPKjPhmjjPNS_10DecodeWorkEPjy"))
     ali = next(v for k, v in fns.items() if "alias_decode_persist_kernelILj16E" in k)
     tma_planned = next(v for k, v in fns.items() if "word_decode_planned_kernelILb0E" in k)
@@ -60,9 +60,9 @@ def main():
                         ("block_decode_kernel (round 1 window: decode_window_chunk with WordDecoder<false>): one step (vote to vote)",
                          step_between(dec, "VOTE.ANY", 5)),
                         ("word_encode_fused_kernel<R32>: one step (symbol load to symbol load)", step_between(enc, "LDS.U8", 8)),
-                        ("word_encode_fused_gated_kernel<R32> (rb200_container_model_encode_async): one step (symbol load to symbol load)",
-                         step_between(enc_gated, "LDS.U8", 8)),
-                        ("word_encode_fused_gated_varlen_kernel<R32> (rb200_container_model_encode_varlen_async): one step (symbol load "
+                        ("word_encode_fused_kernel<R32, GATED> (rb200_container_model_encode_async): one step (symbol load to symbol "
+                         "load)", step_between(enc_gated, "LDS.U8", 8)),
+                        ("word_encode_fused_kernel<R32, GATED, GEOM> (rb200_container_model_encode_varlen_async): one step (symbol load "
                          "to symbol load)", step_between(enc_varlen, "LDS.U8", 8))):
         print("## %s: %d instructions" % (title, len(step)))
         print("```")
