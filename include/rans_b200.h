@@ -337,6 +337,43 @@ int rb200_container_model_encode_varlen_async(rb200_ctx* ctx, int coder, uint32_
                                               const uint64_t* d_n, size_t n_max, uint32_t chunk_syms, uint32_t flags,
                                               uint8_t* out, size_t out_cap);
 
+/* Choosing the coder from the data.  A candidate is a pair (coder, scale_bits) that rb200_container_model_encode_async
+ * accepts -- word at 12; byte, alias or rans64 at 8..16 -- written RB200_CANDIDATE(coder, scale_bits).  A list holds 1 to
+ * 16 distinct candidates in the caller's order of preference.  The rule, the same integer steps on the host and the GPU:
+ *   f_i      = normalize_freqs(counts, 1 << sb_i), as rb200_model_from_data builds it;
+ *   feasible = rb200_model_create accepts f_i for the coder (so the byte coder at 16 on data of one symbol is not);
+ *   log2q(f) = log2 f in 16.16 fixed point: k = floor(log2 f), x = f << (31 - k), r = k << 16, then for i = 15 .. 0:
+ *              x = (x * x) >> 31 in 64 bits, and if x >= 2^32, x >>= 1 and r |= 1 << i;
+ *   bits_q   = sum over the symbols with counts[s] > 0 of counts[s] * ((sb_i << 16) - log2q(f_i[s]));
+ *   cost_i   = ceil(bits_q / 2^19) + n_chunks * H (H = 256 for rans64, 128 otherwise: the 32 final states of a chunk),
+ *              an estimate of the blob bytes; UINT64_MAX for an infeasible candidate.
+ * The choice is the first candidate in list order whose cost is at most min + floor(min * tolerance_ppm / 10^6), min the
+ * smallest cost.  {WORD 12, ALIAS 16} with 20000 ppm: the word coder unless alias at 16 is more than 2 % smaller. */
+#define RB200_CANDIDATE(coder, scale_bits) ((uint32_t)(coder) << 8 | (uint32_t)(scale_bits))
+
+/* The rule on the host, for counts[256] of n symbols (rb200_histogram's) cut into chunks of chunk_syms: costs[i]
+ * (may be NULL) receives every candidate's cost and *chosen the index of the choice; with it, a caller whose data is in
+ * host memory calls rb200_model_from_data and rb200_container_encode.  RB200_E_ARG for a null counts or chosen, an
+ * invalid list, tolerance_ppm > 10^6, chunk_syms outside 32 .. 2^24, n >= 2^32 or counts that do not sum to n;
+ * RB200_E_MODEL when no candidate is feasible (n == 0 included): costs are written, *chosen is not. */
+int rb200_choose_coder(const uint64_t counts[256], size_t n, uint32_t chunk_syms, const uint32_t* candidates,
+                       uint32_t n_candidates, uint32_t tolerance_ppm, uint64_t* costs, uint32_t* chosen);
+
+/* rb200_container_model_encode_async with (coder, scale_bits) chosen by the rule above on the GPU, from the data's
+ * histogram, at every run: one captured graph writes whichever coder suits the data it meets, and
+ * rb200_container_decode_async decodes it.  The container is byte for byte what rb200_container_model_encode_async
+ * writes for the chosen pair; the choice is recorded only in the header (bytes 6-7).  d_n == NULL encodes n symbols;
+ * otherwise n is n_max and the length is read from *d_n at every run, by the rules of
+ * rb200_container_model_encode_varlen_async.  The call returns RB200_E_ARG (nothing launched) for everything the fixed
+ * (or varlen) call refuses, checked for every candidate, for an invalid candidate list and for tolerance_ppm > 10^6;
+ * RB200_E_MODEL for n == 0 with d_n NULL; RB200_E_SPACE when out_cap is below the blob offset.  rb200_sync returns
+ * RB200_E_MODEL when no candidate is feasible, and otherwise what it returns for the fixed call with the chosen pair.
+ * On every error the header is not written.  The workspace grows for the largest encode plan over the candidates, so a
+ * call with the same list and geometry outside a capture must come first. */
+int rb200_container_model_encode_auto_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                            uint32_t tolerance_ppm, const uint8_t* in, const uint64_t* d_n, size_t n,
+                                            uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap);
+
 /* ---------------------------------------------------------------- multi-GPU: gathering the shards' blobs (NCCL) */
 
 /* Shards are independent (SURVEY 8e): every rank encodes / decodes its own contiguous range of symbols with no

@@ -73,6 +73,9 @@ EXPORTS = [
                                                      C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_container_model_encode_varlen_async", C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t,
                                                             C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_choose_coder", C.c_int, [_u64p, C.c_size_t, C.c_uint32, _u32p, C.c_uint32, C.c_uint32, _u64p, _u32p]),
+    ("rb200_container_model_encode_auto_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                          C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -88,6 +91,30 @@ EXPORTS = [
     ("rb200_container_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
 ]
 CONTAINER_CRC_BLOB = 1
+
+
+def CANDIDATE(coder, scale_bits):
+    """RB200_CANDIDATE: one (coder, scale_bits) pair of a coder-choice list"""
+    return (coder << 8) | scale_bits
+
+
+def _candidates(candidates):
+    return np.ascontiguousarray(candidates, dtype=np.uint32)
+
+
+def choose_coder(counts, n, chunk_syms, candidates, tolerance_ppm=0):
+    """rb200_choose_coder: the rule of the auto encode on the host.  counts: the 256 counts of n symbols (as
+    Context.histogram returns them); candidates: CANDIDATE values in order of preference.  Returns (index, costs), costs
+    as u64 with 2^64 - 1 for an infeasible candidate; RansError -2 when none is feasible."""
+    lib = load()
+    counts = np.ascontiguousarray(counts, dtype=np.uint64)
+    assert counts.size == 256
+    cands = _candidates(candidates)
+    costs = np.zeros(max(cands.size, 1), np.uint64)
+    chosen = C.c_uint32(0)
+    lib.check(lib.dll.rb200_choose_coder(counts.ctypes.data_as(_u64p), n, chunk_syms, cands.ctypes.data_as(_u32p), cands.size,
+                                         tolerance_ppm, costs.ctypes.data_as(_u64p), C.byref(chosen)))
+    return int(chosen.value), costs[:cands.size]
 
 
 class ContainerInfo(C.Structure):
@@ -434,6 +461,17 @@ class Context:
         container_model_encode_async) comes from sync()"""
         self.lib.check(self.lib.dll.rb200_container_model_encode_varlen_async(self.h, coder, scale_bits, in_ptr, n_ptr, n_max, chunk_syms,
                                                                               flags, out_ptr, out_cap), self.h)
+
+    def container_model_encode_auto_async(self, candidates, tolerance_ppm, in_ptr, n, chunk_syms, flags, out_ptr, out_cap, n_ptr=0):
+        """container_model_encode_async with (coder, scale_bits) chosen on the GPU from the data at every run, by the
+        rule of choose_coder over `candidates` (CANDIDATE values, in order of preference).  n_ptr: the device address of
+        a u64 length read when the work runs, with n its bound n_max (as container_model_encode_varlen_async), or 0.
+        The header records the choice.  The verdict (-2 when no candidate is feasible, otherwise as the fixed call for
+        the chosen pair) comes from sync()"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_model_encode_auto_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
+                                                                            in_ptr, n_ptr or None, n, chunk_syms, flags, out_ptr, out_cap),
+                       self.h)
 
     # ---- per-block containers (version 2): every block's model, the directory and the blob in one buffer
     def container_blocks_capacity(self, n_blocks, block_size, chunk_syms):

@@ -467,14 +467,21 @@ __device__ __forceinline__ void alias_encode(const uint8_t* __restrict__ in, uin
 // GEOM (rb200_container_model_encode_varlen_async): n, the chunk count, the blob's place in the container `blob` and
 // its capacity from the record, on the grid the host sized for n_max.  In split mode a CTA past the real chunks exits
 // before it stages its tables; in fused mode every CTA runs (CTA 0 holds the scanner, the others find no chunk and leave).
-template <bool ALIAS, uint32_t SB, bool GEOM = false>
+// GATED (rb200_container_model_encode_auto_async): runs only when the choice record names `group`, and then at the
+// recorded scale_bits; otherwise it exits at entry, before it touches shared memory, the counter, look[] or scratch.
+template <bool ALIAS, uint32_t SB, bool GEOM = false, bool GATED = false>
 __global__ void __launch_bounds__(kAliasEncWarps * 32, 1)
 alias_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb_rt,
                     const AliasEncEntry* __restrict__ g_enc, const uint16_t* __restrict__ g_remap,
                     uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
                     uint64_t* __restrict__ look, uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap,
-                    uint64_t* __restrict__ offsets, uint32_t* __restrict__ status, const VarlenGeom* __restrict__ geom)
+                    uint64_t* __restrict__ offsets, uint32_t* __restrict__ status, const VarlenGeom* __restrict__ geom,
+                    const CoderChoice* __restrict__ choice, uint32_t group)
 {
+    if (GATED) {
+        if (choice->group != group) return;
+        sb_rt = choice->scale_bits;
+    }
     if (GEOM) {
         n_chunks = geom->n_chunks;
         if (!geom->go || (!look && blockIdx.x * kAliasEncWarps >= n_chunks)) return;
@@ -495,10 +502,12 @@ inline uint32_t alias_encode_smem(bool alias, uint32_t sb) { return kAliasEncFix
 template <bool ALIAS, uint32_t SB>
 inline void configure_alias_encode()
 {
-    cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, alias_encode_smem(ALIAS, 16));
-    cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(alias_encode_kernel<ALIAS, SB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, alias_encode_smem(ALIAS, 16));
+    for (const void* k : {reinterpret_cast<const void*>(alias_encode_kernel<ALIAS, SB>), reinterpret_cast<const void*>(alias_encode_kernel<ALIAS, SB, true>),
+                          reinterpret_cast<const void*>(alias_encode_kernel<ALIAS, SB, false, true>),
+                          reinterpret_cast<const void*>(alias_encode_kernel<ALIAS, SB, true, true>)}) {
+        cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, alias_encode_smem(ALIAS, 16));
+    }
 }
 template <uint32_t SB>
 inline void configure_byte_decode()
@@ -538,20 +547,28 @@ inline void configure_alias_kernels()
 // remap == nullptr selects the rans_byte cum2sym coder.  look == nullptr: split mode (sizes[] out, one slot per
 // chunk); otherwise fused mode (kAliasFusedSlots slots per worker warp; look/counter zeroed by the caller).
 // grid <= one CTA per SM (the kernel is persistent), smem = alias_encode_smem(remap != nullptr, sb).  geom set: the
-// GEOM instance, with n, n_chunks and the grid those of n_max and blob the container.
+// GEOM instance, with n, n_chunks and the grid those of n_max and blob the container.  choice set: the GATED instance of
+// sb's SB, run when the record names `group` (smem then covers the largest scale_bits of the group).
 inline void launch_alias_encode(cudaStream_t stream, uint32_t grid, uint32_t smem, const uint8_t* d_in, uint64_t n, uint32_t chunk_syms,
                                 uint32_t n_chunks, uint32_t sb, const AliasEncEntry* enc, const uint16_t* remap, uint8_t* scratch,
                                 uint32_t slot, uint32_t* sizes, uint64_t* look, uint32_t* counter, uint8_t* blob, uint64_t blob_cap,
-                                uint64_t* offsets, uint32_t* status, const VarlenGeom* geom)
+                                uint64_t* offsets, uint32_t* status, const VarlenGeom* geom, const CoderChoice* choice = nullptr,
+                                uint32_t group = 0)
 {
     auto kernel = alias_encode_kernel<false, 0>;
-    if (remap) {
+    if (choice) {
+        if (remap) {
+            RB200_ALIAS_SB_DISPATCH(sb, (kernel = geom ? alias_encode_kernel<true, SB, true, true> : alias_encode_kernel<true, SB, false, true>))
+        } else {
+            RB200_ALIAS_SB_DISPATCH(sb, (kernel = geom ? alias_encode_kernel<false, SB, true, true> : alias_encode_kernel<false, SB, false, true>))
+        }
+    } else if (remap) {
         RB200_ALIAS_SB_DISPATCH(sb, (kernel = geom ? alias_encode_kernel<true, SB, true> : alias_encode_kernel<true, SB>))
     } else {
         RB200_ALIAS_SB_DISPATCH(sb, (kernel = geom ? alias_encode_kernel<false, SB, true> : alias_encode_kernel<false, SB>))
     }
     kernel<<<grid, kAliasEncWarps * 32, smem, stream>>>(d_in, n, chunk_syms, n_chunks, sb, enc, remap, scratch, slot, sizes, look, counter,
-                                                        blob, blob_cap, offsets, status, geom);
+                                                        blob, blob_cap, offsets, status, geom, choice, group);
 }
 
 // the persistent kernel: sms x 2 CTAs of 20 warps, chunk ids from the context's work counter

@@ -140,6 +140,66 @@ RB200_HD inline bool container_model_decodable(uint32_t coder, const uint32_t* f
     return true;
 }
 
+// The coder choice of rb200_choose_coder and rb200_container_model_encode_auto_async (coder_choice_kernel), the same
+// integer steps on host and device.  A candidate is RB200_CANDIDATE(coder, scale_bits).
+// a pair rb200_container_model_encode_async accepts: word at 12; byte, alias or rans64 at 8..16
+RB200_HD inline bool candidate_ok(uint32_t c)
+{
+    const uint32_t coder = c >> 8, sb = c & 0xffu;
+    if (coder == RB200_CODER_WORD) return sb == 12;
+    return coder <= RB200_CODER_RANS64 && sb >= 8 && sb <= 16;
+}
+// 1..16 valid candidates, no two alike
+inline bool candidate_list_ok(const uint32_t* c, uint32_t n)
+{
+    if (!c || n == 0 || n > 16) return false;
+    for (uint32_t i = 0; i < n; i++) {
+        if (!candidate_ok(c[i])) return false;
+        for (uint32_t j = 0; j < i; j++)
+            if (c[j] == c[i]) return false;
+    }
+    return true;
+}
+// log2(f) in 16.16 fixed point, by squaring the mantissa: x = f << (31 - k) holds f / 2^k in [1, 2) as x / 2^31; each
+// squaring that reaches 2 gives one fraction bit.  f <= 65536.
+RB200_HD inline uint32_t log2q(uint32_t f)
+{
+    uint32_t k = 0;
+    while ((f >> k) > 1) k++;
+    uint64_t x = static_cast<uint64_t>(f) << (31 - k);
+    uint32_t r = k << 16;
+    for (int i = 15; i >= 0; i--) {
+        x = (x * x) >> 31;
+        if (x >= (1ull << 32)) {
+            x >>= 1;
+            r |= 1u << i;
+        }
+    }
+    return r;
+}
+// symbol s's share of bits_q: count * -log2(f / 2^sb) in 16.16 (0 for a symbol that does not occur).  A symbol that
+// occurs has f >= 1 once normalised, so the term is at most count * 2^20 and bits_q stays below 2^52 for n < 2^32.
+RB200_HD inline uint64_t candidate_bits_q(uint32_t count, uint32_t f, uint32_t sb)
+{
+    return count ? static_cast<uint64_t>(count) * ((sb << 16) - log2q(f)) : 0;
+}
+// estimated container blob bytes: the coded bits, rounded up to bytes, and the 32 final states of every chunk
+RB200_HD inline uint64_t candidate_cost(uint64_t bits_q, uint64_t n_chunks, uint32_t coder)
+{
+    return ((bits_q + (1ull << 19) - 1) >> 19) + n_chunks * (coder == RB200_CODER_RANS64 ? 256u : 128u);
+}
+// the first candidate whose cost is within tolerance_ppm of the smallest, or -1 when every cost is UINT64_MAX
+RB200_HD inline int choose_candidate(const uint64_t* costs, uint32_t n, uint32_t tolerance_ppm)
+{
+    uint64_t min = ~0ull;
+    for (uint32_t i = 0; i < n; i++) min = costs[i] < min ? costs[i] : min;
+    if (min == ~0ull) return -1;
+    const uint64_t bound = min + min * tolerance_ppm / 1000000u;        // min < 2^40, tolerance_ppm <= 10^6
+    for (uint32_t i = 0; i < n; i++)
+        if (costs[i] <= bound) return static_cast<int>(i);
+    return -1;
+}
+
 // The per-element rules of a version 2 prefix, one block or one directory entry at a time.
 // one block's 256 frequencies sum to total (version 3: 1 << scale_bits)
 RB200_HD inline bool container_block_model_sums_to(const uint16_t* freqs, uint32_t total)

@@ -337,3 +337,31 @@ extern "C" int rb200_container_blocks_coder_open(const uint8_t* buf, size_t size
     info->blob = buf + container_blob_offset(l);
     return RB200_OK;
 }
+
+extern "C" int rb200_choose_coder(const uint64_t counts[256], size_t n, uint32_t chunk_syms, const uint32_t* candidates,
+                                  uint32_t n_candidates, uint32_t tolerance_ppm, uint64_t* costs, uint32_t* chosen)
+{
+    if (!counts || !chosen || !candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    if (!container_chunk_ok(chunk_syms) || (n >> 32)) return RB200_E_ARG;
+    uint64_t total = 0;
+    for (int s = 0; s < 256; s++) total += counts[s];                 // each count <= n < 2^32: no overflow
+    if (total != n) return RB200_E_ARG;
+    const uint64_t n_chunks = n / chunk_syms + (n % chunk_syms != 0);
+    uint64_t cost[16];
+    for (uint32_t i = 0; i < n_candidates; i++) {
+        const uint32_t coder = candidates[i] >> 8, sb = candidates[i] & 0xffu;
+        uint32_t f[256], cum[257];
+        for (int s = 0; s < 256; s++) f[s] = static_cast<uint32_t>(counts[s]);
+        cost[i] = ~0ull;
+        if (n == 0 || rb200_normalize_freqs(f, cum, 1u << sb) != RB200_OK) continue;
+        if (!container_model_ok(coder, sb, f) || !container_model_decodable(coder, f)) continue;
+        uint64_t bits_q = 0;
+        for (int s = 0; s < 256; s++) bits_q += candidate_bits_q(static_cast<uint32_t>(counts[s]), f[s], sb);
+        cost[i] = candidate_cost(bits_q, n_chunks, coder);
+    }
+    if (costs) std::memcpy(costs, cost, n_candidates * sizeof(uint64_t));
+    const int k = choose_candidate(cost, n_candidates, tolerance_ppm);
+    if (k < 0) return RB200_E_MODEL;
+    *chosen = static_cast<uint32_t>(k);
+    return RB200_OK;
+}

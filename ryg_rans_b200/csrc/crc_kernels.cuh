@@ -272,11 +272,12 @@ inline uint32_t crc32_grid(uint32_t sms, uint64_t n)
 // word is clear (an encoder error leaves the buffer as it is) and the blob fits out_cap (else it flags kStatSpace).
 // GEOM (rb200_container_model_encode_varlen_async, version 1): n_symbols, n_chunks and the blob offset from the record
 // (VarlenGeom); h arrives with coder, scale_bits, chunk_syms and flags.  Writes nothing when geom->go == 0.
-template <bool GEOM = false>
+// CHOSEN (rb200_container_model_encode_auto_async, version 1): coder and scale_bits from the choice record.
+template <bool GEOM = false, bool CHOSEN = false>
 __global__ void __launch_bounds__(32)
     container_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
                             const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status,
-                            const VarlenGeom* __restrict__ geom)
+                            const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice)
 {
     if (GEOM) {
         if (!geom->go) return;
@@ -284,6 +285,10 @@ __global__ void __launch_bounds__(32)
         h.n_chunks = geom->n_chunks;
         dir_off = kContainerDirOffset;
         blob_off = geom->blob_off;
+    }
+    if (CHOSEN) {
+        h.coder = static_cast<uint8_t>(choice->coder);
+        h.scale_bits = static_cast<uint8_t>(choice->scale_bits);
     }
     using namespace crc_detail;
     __shared__ uint4 sbuf_v[kContainerDirOffset / 16];

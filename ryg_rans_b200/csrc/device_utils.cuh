@@ -29,6 +29,17 @@ struct VarlenGeom {
     uint32_t go;           // 1: *d_n passed the checks; 0: nothing after the plan runs (dir_len, blob_off, blob_len are 0)
 };
 
+// The choice of rb200_container_model_encode_auto_async: written by coder_choice_kernel (model_kernels.cuh) at every
+// run, read by the CHOSEN / GATED instances after it.  The host launches one gated group of encode kernels per distinct
+// encoder instance the candidate list needs; only the group named here runs, the others exit at entry.
+constexpr uint32_t kMaxCandidates = 16;
+struct CoderChoice {
+    uint32_t coder, scale_bits;        // the chosen pair
+    uint32_t index;                    // its place in the caller's list (the first one when none is feasible)
+    uint32_t group;                    // the launch group that encodes
+    uint64_t costs[kMaxCandidates];    // every candidate's cost, UINT64_MAX when infeasible
+};
+
 __device__ __forceinline__ uint32_t lanemask_lt()
 {
     uint32_t m;

@@ -17,6 +17,13 @@
 // and reads the length from device memory: varlen_plan_kernel checks *d_n and writes the geometry record (VarlenGeom,
 // device_utils.cuh) into geom; every later kernel is the GEOM instance of the same kernel, which takes n, the chunk
 // count and the blob's place from there and exits at entry when the checks failed.
+//
+// rb200_container_model_encode_auto_async runs coder_choice_kernel after the histogram: it applies the rule of
+// rb200_choose_coder to the counts and writes the choice record (CoderChoice).  The CHOSEN instance of the model kernel
+// builds the chosen coder's tables from it; the host launches one gated group per distinct encoder instance the list
+// needs (word: both GATED instances, whose gate r32 the model kernel closes for other coders; alias/byte per SB
+// instance; rans64), each with its own directory and compaction when split, and only the recorded group runs; the
+// CHOSEN instance of container_finish_kernel writes the chosen coder and scale_bits into the header.
 #pragma once
 #include "block_kernels.cuh"
 #include "container_format.h"
@@ -25,7 +32,7 @@
 
 namespace rb200 {
 
-// The call's workspace: fixed-size (about 150 KiB), allocated with the context, so the call never allocates for the
+// The call's workspace: fixed-size (about 170 KiB), allocated with the context, so the call never allocates for the
 // model.  Every table has the layout of its rb200_model counterpart.
 struct ModelAsyncWork {
     unsigned long long counts[256];               // the histogram; zeroed in stream order before each call
@@ -38,7 +45,11 @@ struct ModelAsyncWork {
     alignas(16) uint4 r64_enc[256 * 2];           // Rans64EncSymbol images, 32 bytes each
     alignas(16) uint16_t alias_remap[1u << 16];   // the first 1 << scale_bits entries are the model's
     VarlenGeom geom;                              // rb200_container_model_encode_varlen_async: the length and layout of this run
+    CoderChoice choice;                           // rb200_container_model_encode_auto_async: the choice of this run
+    uint32_t cand_freqs[kMaxCandidates][256];     // its candidates' models; the chosen row is the container's
 };
+
+constexpr uint32_t kWordGateClosed = 2;          // r32 when the auto encode chose another coder: neither word instance runs
 
 constexpr int kModelThreads = 256;                // one thread per symbol
 
@@ -49,20 +60,30 @@ constexpr int kModelThreads = 256;                // one thread per symbol
 // target, cannot all be <= 1.  block_normalize keeps its check all the same, with kStatModel as the verdict.
 // GEOM (the device-length call): with *d_n == 0 the counts are all zero and normalisation has no total to scale, so it
 // runs only when the plan passed.
-template <bool GEOM = false>
+// CHOSEN (the auto encode): coder, scale_bits and the normalised model come from the choice record (coder_choice_kernel
+// normalised every candidate); the arguments coder and sb are unused.  Another coder than word closes both word gates.
+template <bool GEOM = false, bool CHOSEN = false>
 __global__ void __launch_bounds__(kModelThreads)
     container_model_kernel(uint32_t coder, uint32_t sb, uint32_t r32_allowed, ModelAsyncWork* __restrict__ w, uint32_t* __restrict__ status)
 {
     if (GEOM && !w->geom.go) return;
+    if (CHOSEN) {
+        coder = w->choice.coder;
+        sb = w->choice.scale_bits;
+    }
     __shared__ uint32_t s_cnt[256], s_cum[257];
     __shared__ __align__(16) uint32_t s_w[256];
     __shared__ uint32_t s_divider[256], s_adjust[512], s_slot_freqs[512], s_rest[256], s_given[256];
     __shared__ uint8_t s_sym_id[512];
     __shared__ uint32_t s_paired;
     const uint32_t tid = threadIdx.x, M = 1u << sb;
-    s_cnt[tid] = static_cast<uint32_t>(w->counts[tid]);        // n < 2^32, so every count and their sum fit
-    __syncthreads();
-    if (tid < 32) block_normalize(s_cnt, s_cum, s_w, w->freqs, M, kStatModel, status);
+    if (CHOSEN) {
+        s_w[tid] = w->freqs[tid] = w->cand_freqs[w->choice.index][tid];
+    } else {
+        s_cnt[tid] = static_cast<uint32_t>(w->counts[tid]);    // n < 2^32, so every count and their sum fit
+        __syncthreads();
+        if (tid < 32) block_normalize(s_cnt, s_cum, s_w, w->freqs, M, kStatModel, status);
+    }
     __syncthreads();
     if (tid == 0) {
         bool ok = container_model_ok(coder, sb, s_w) && container_model_decodable(coder, s_w);
@@ -82,6 +103,7 @@ __global__ void __launch_bounds__(kModelThreads)
     }
     __syncthreads();
     const uint32_t f = s_w[tid], cum = s_cum[tid];
+    if (CHOSEN && coder != RB200_CODER_WORD && tid == 0) w->r32 = kWordGateClosed;
     if (coder == RB200_CODER_WORD) {
         int exact = 1;
         w->word_enc[tid] = word_enc_entry(f, cum);
@@ -108,6 +130,68 @@ __global__ void __launch_bounds__(kModelThreads)
         rans64_enc_entry(f, cum, sb, e);
         w->r64_enc[2 * tid] = make_uint4(e[0], e[1], e[2], e[3]);
         w->r64_enc[2 * tid + 1] = make_uint4(e[4], e[5], e[6], e[7]);
+    }
+}
+
+// The candidate list of rb200_container_model_encode_auto_async, by value: the pairs (RB200_CANDIDATE) and the launch
+// group of each (the host's numbering: one group per distinct encoder instance).
+struct CandidateList {
+    uint32_t pair[kMaxCandidates];
+    uint32_t group[kMaxCandidates];
+    uint32_t n, tolerance_ppm;
+};
+
+// The rule of rb200_choose_coder (container_format.h) on the histogram, one CTA with one warp per candidate: warp i
+// normalises the counts to 1 << sb_i into cand_freqs[i] (block_normalize, bit-exact), checks the model as the fixed
+// call would, and sums its bits_q; thread 0 then applies the rule and writes the choice record.  No feasible candidate
+// sets kStatModel and records the first one, whose tables the model kernel then builds as the fixed call would (the
+// header is never written).  n_chunks is the fixed call's; geom set: the device-length call, which takes it from the
+// record and runs only when the plan passed.
+__global__ void __launch_bounds__(kMaxCandidates * 32)
+    coder_choice_kernel(CandidateList list, uint64_t n_chunks, ModelAsyncWork* __restrict__ w, const VarlenGeom* __restrict__ geom,
+                        uint32_t* __restrict__ status)
+{
+    if (geom) {
+        if (!geom->go) return;
+        n_chunks = geom->n_chunks;
+    }
+    __shared__ uint32_t s_cnt[256], s_cum[kMaxCandidates][257], s_fail[kMaxCandidates];
+    __shared__ __align__(16) uint32_t s_w[kMaxCandidates][256];
+    __shared__ uint64_t s_cost[kMaxCandidates];
+    const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    for (uint32_t s = tid; s < 256; s += blockDim.x) s_cnt[s] = static_cast<uint32_t>(w->counts[s]);   // n < 2^32
+    if (lane == 0) s_fail[warp] = 0;
+    __syncthreads();
+    const uint32_t coder = list.pair[warp] >> 8, sb = list.pair[warp] & 0xffu;
+    uint32_t* f = s_w[warp];
+    block_normalize(s_cnt, s_cum[warp], f, w->cand_freqs[warp], 1u << sb, 1u, &s_fail[warp]);
+    __syncwarp();
+    // container_model_ok and container_model_decodable, spread over the warp (the pair itself is valid): the model sums
+    // to 1 << sb, and the byte coder's frequencies stay below 65536
+    uint64_t bits_q = 0;
+    uint32_t sum = 0, top = 0;
+    for (uint32_t s = lane; s < 256; s += 32) {
+        bits_q += candidate_bits_q(s_cnt[s], f[s], sb);
+        sum += f[s];
+        top = max(top, f[s]);
+    }
+    for (int d = 16; d; d >>= 1) bits_q += __shfl_xor_sync(0xffffffffu, bits_q, d);
+    sum = __reduce_add_sync(0xffffffffu, sum);
+    top = __reduce_max_sync(0xffffffffu, top);
+    if (lane == 0) {
+        const bool ok = !s_fail[warp] && sum == (1u << sb) && (coder != RB200_CODER_BYTE || top < 65536u);
+        s_cost[warp] = ok ? candidate_cost(bits_q, n_chunks, coder) : ~0ull;
+    }
+    __syncthreads();
+    if (tid < list.n) w->choice.costs[tid] = s_cost[tid];
+    if (tid == 0) {
+        const int k = choose_candidate(s_cost, list.n, list.tolerance_ppm);
+        if (k < 0) atomicOr(status, kStatModel);
+        const uint32_t i = k < 0 ? 0u : static_cast<uint32_t>(k);
+        w->choice.coder = list.pair[i] >> 8;
+        w->choice.scale_bits = list.pair[i] & 0xffu;
+        w->choice.index = i;
+        w->choice.group = list.group[i];
     }
 }
 

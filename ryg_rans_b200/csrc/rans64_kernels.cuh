@@ -130,23 +130,29 @@ struct Rans64Encoder {
 };
 
 // GEOM (rb200_container_model_encode_varlen_async): n and the chunk count from the record, on a grid sized for n_max; a
-// CTA past the real chunks exits before it stages the table
-template <bool GEOM = false>
+// CTA past the real chunks exits before it stages the table.  GATED (rb200_container_model_encode_auto_async): runs only
+// when the choice record names `group`, at the recorded scale_bits; otherwise it exits at entry.
+template <bool GEOM = false, bool GATED = false>
 __global__ void __launch_bounds__(kRans64Warps * 32, 2)
 rans64_encode_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk_syms, uint32_t n_chunks, uint32_t sb,
                      const uint4* __restrict__ g_enc,      // 256 x 2 x uint4
                      uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status,
-                     const VarlenGeom* __restrict__ geom)
+                     const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
 {
+    if (GATED) {
+        if (choice->group != group) return;
+        sb = choice->scale_bits;
+    }
     if (GEOM) {
         n_chunks = geom->n_chunks;
         if (!geom->go || blockIdx.x * kRans64Warps >= n_chunks) return;
     }
-    // [16 x 1 KiB stage + ring][32 KiB table, 8 replicas].  Each instance has its own name for it: with one name for
-    // both, ptxas schedules the GEOM = false instance differently.
+    // [16 x 1 KiB stage + ring][32 KiB table, 8 replicas].  The instances name it differently: with one name for
+    // GEOM and not, or for GATED and not, ptxas schedules the shipped instances differently.
     extern __shared__ __align__(1024) uint8_t s_r64e[];
     extern __shared__ __align__(1024) uint8_t s_r64v[];
-    uint8_t* const s_enc = GEOM ? s_r64v : s_r64e;
+    extern __shared__ __align__(1024) uint8_t s_r64g[];
+    uint8_t* const s_enc = GATED ? s_r64g : (GEOM ? s_r64v : s_r64e);
     uint4* s_tab = reinterpret_cast<uint4*>(s_enc + kRans64Warps * kEncWarpSmem);
     for (uint32_t i = threadIdx.x; i < 256 * kEncReplicas; i += blockDim.x) {
         const uint4 a = g_enc[2 * (i / kEncReplicas)], b = g_enc[2 * (i / kEncReplicas) + 1];   // {rcp_lo, rcp_hi, freq, bias}, {cmpl, shift | bad, -, -}
@@ -168,7 +174,8 @@ inline void configure_rans64_kernels()
 {
     cudaFuncSetAttribute(rans64_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRans64Warps * kRingBytes + kRans64DecSymBytes + (1u << 16));
     cudaFuncSetAttribute(rans64_decode_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    for (const void* k : {reinterpret_cast<const void*>(rans64_encode_kernel<false>), reinterpret_cast<const void*>(rans64_encode_kernel<true>)}) {
+    for (const void* k : {reinterpret_cast<const void*>(rans64_encode_kernel<false>), reinterpret_cast<const void*>(rans64_encode_kernel<true>),
+                          reinterpret_cast<const void*>(rans64_encode_kernel<false, true>), reinterpret_cast<const void*>(rans64_encode_kernel<true, true>)}) {
         cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kRans64EncSmemBytes);
     }

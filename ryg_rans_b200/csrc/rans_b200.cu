@@ -453,30 +453,34 @@ namespace {
 
 
 // directory + compaction after any encode kernel: sizes[] -> offsets[] + blob.  geom set: the GEOM instances, on grids
-// sized for n_chunks (the bound's), with d_blob the container.
+// sized for n_chunks (the bound's), with d_blob the container.  choice set: the GATED instances, which run only when the
+// record names `group`.
 int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* sizes, uint64_t* tile_sums, uint32_t n_chunks,
-                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom)
+                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom, const CoderChoice* choice, uint32_t group)
 {
     if (!n_chunks) {
         RB_CUDA(ctx, cudaMemsetAsync(d_offsets, 0, sizeof(uint64_t), ctx->stream));
         return RB200_OK;
     }
     const uint32_t tiles = (n_chunks + kScanTile - 1) / kScanTile;
-    auto scan = geom ? scan_tiles_kernel<true> : scan_tiles_kernel<false>;
-    scan<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, d_offsets, tile_sums, geom);
+    auto scan = choice ? (geom ? scan_tiles_kernel<true, true> : scan_tiles_kernel<false, true>)
+                       : (geom ? scan_tiles_kernel<true> : scan_tiles_kernel<false>);
+    scan<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, d_offsets, tile_sums, geom, choice, group);
     int rc = check_launch(ctx, "scan_tiles_kernel");
     if (rc != RB200_OK) return rc;
     const uint32_t prefixed = tiles > kTilePrefixThreshold ? 1u : 0u;
     if (prefixed) {
-        auto prefix = geom ? tile_prefix_kernel<true> : tile_prefix_kernel<false>;
-        prefix<<<1, 1024, 0, ctx->stream>>>(tile_sums, tiles, geom);
+        auto prefix = choice ? (geom ? tile_prefix_kernel<true, true> : tile_prefix_kernel<false, true>)
+                             : (geom ? tile_prefix_kernel<true> : tile_prefix_kernel<false>);
+        prefix<<<1, 1024, 0, ctx->stream>>>(tile_sums, tiles, geom, choice, group);
         rc = check_launch(ctx, "tile_prefix_kernel");
         if (rc != RB200_OK) return rc;
     }
     const uint32_t grid = (n_chunks + kCopyWarps - 1) / kCopyWarps;
-    auto compact = geom ? compact_kernel<true> : compact_kernel<false>;
+    auto compact = choice ? (geom ? compact_kernel<true, true> : compact_kernel<false, true>)
+                          : (geom ? compact_kernel<true> : compact_kernel<false>);
     compact<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, d_offsets, tile_sums, prefixed, n_chunks, d_blob, blob_cap,
-                                                        ctx->d_status, geom);
+                                                        ctx->d_status, geom, choice, group);
     return check_launch(ctx, "compact_kernel");
 }
 
@@ -615,10 +619,10 @@ int prepare_workspace(rb200_ctx* ctx, const EncodePlan& p, EncodeWorkspace* ws)
 }
 
 // Runs a plan: prepare its workspace; fused: `launch(ws)`, the one kernel; split: `launch(ws)` encodes into the slots
-// (when there are chunks), then finish_encode (geom: as there).  `launch` returns check_launch's code.
+// (when there are chunks), then finish_encode (geom, choice, group: as there).  `launch` returns check_launch's code.
 template <class Launch>
 int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom,
-               Launch launch)
+               Launch launch, const CoderChoice* choice = nullptr, uint32_t group = 0)
 {
     EncodeWorkspace ws = {};
     int rc = prepare_workspace(ctx, p, &ws);
@@ -628,11 +632,14 @@ int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob
         rc = launch(ws);
         if (rc != RB200_OK) return rc;
     }
-    return finish_encode(ctx, ws.scratch, p.slot_bytes, ws.sizes, ws.tile_sums, p.n_chunks, d_blob, blob_cap, d_offsets, geom);
+    return finish_encode(ctx, ws.scratch, p.slot_bytes, ws.sizes, ws.tile_sums, p.n_chunks, d_blob, blob_cap, d_offsets, geom, choice,
+                         group);
 }
 
 // The encode tables of one encode call, in device memory.  Word: `word_gate` null runs the instance word_r32 names on
 // word[word_r32]; set, both GATED instances run (word_kernels.cuh), each on its own table, and *word_gate picks one.
+// choice set (the auto encode): the other coders' GATED instances, and those of the split path's directory and
+// compaction, which run only when the record names `group`; scale_bits is then the largest of the group.
 struct EncodeTables {
     int coder;
     uint32_t scale_bits;
@@ -643,6 +650,8 @@ struct EncodeTables {
     const uint16_t* remap;             // alias
     const uint4* r64;                  // rans64
     bool word_ring = false;            // word: the model satisfies word_ring_model
+    const CoderChoice* choice = nullptr;
+    uint32_t group = 0;
 };
 
 EncodeTables model_tables(const rb200_model* m)
@@ -693,16 +702,18 @@ int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, si
             return rc;
         }
         if (t.coder == RB200_CODER_RANS64) {
-            auto kernel = geom ? rans64_encode_kernel<true> : rans64_encode_kernel<false>;
+            auto kernel = t.choice ? (geom ? rans64_encode_kernel<true, true> : rans64_encode_kernel<false, true>)
+                                   : (geom ? rans64_encode_kernel<true> : rans64_encode_kernel<false>);
             kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.scale_bits, t.r64, ws.scratch, p.slot_bytes,
-                                                               ws.sizes, ctx->d_status, geom);
+                                                               ws.sizes, ctx->d_status, geom, t.choice, t.group);
             return check_launch(ctx, "rans64_encode_kernel");
         }
         const bool alias = t.coder == RB200_CODER_ALIAS;
         launch_alias_encode(ctx->stream, p.grid, p.smem, d_in, n, chunk_syms, n_chunks, t.scale_bits, t.enc, alias ? t.remap : nullptr,
-                            ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status, geom);
+                            ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status, geom,
+                            t.choice, t.group);
         return check_launch(ctx, alias ? "alias_encode_kernel" : "byte_encode_kernel");
-    });
+    }, t.choice, t.group);
 }
 
 int decode_device(rb200_ctx* ctx, const rb200_model* model, const uint8_t* d_blob, size_t blob_size, const uint64_t* d_offsets,
@@ -1533,7 +1544,8 @@ extern "C" int rb200_container_encode(rb200_ctx* ctx, const rb200_model* model, 
         if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
         if (rc != RB200_OK) return rc;
-        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, model->d_freqs, ctx->d_crc, ctx->d_status, nullptr);
+        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, model->d_freqs, ctx->d_crc, ctx->d_status, nullptr,
+                                                           nullptr);
         return check_launch(ctx, "container_finish_kernel");
     }
     size_t blob_bytes = 0, slices = 0;
@@ -1586,7 +1598,7 @@ int container_blocks_encode_impl(rb200_ctx* ctx, ContainerHeader h, const uint8_
         if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
         if (rc != RB200_OK) return rc;
-        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, nullptr, ctx->d_crc, ctx->d_status, nullptr);
+        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, nullptr, ctx->d_crc, ctx->d_status, nullptr, nullptr);
         return check_launch(ctx, "container_finish_kernel");
     }
     if (!build) std::memcpy(model, block_freqs, model_bytes);
@@ -1772,11 +1784,50 @@ EncodeTables workspace_tables(ModelAsyncWork* w, int coder, uint32_t scale_bits)
                         coder == RB200_CODER_ALIAS ? w->alias_enc : w->byte_enc, w->alias_remap, w->r64_enc};
 }
 
+// The launch groups of an auto encode, one per distinct encoder instance its candidates need: word (both GATED K2 or
+// K2f instances), alias and byte per SB instance of RB200_ALIAS_SB_DISPATCH, rans64.  A group's scale_bits is the
+// largest of its candidates': it sizes the alias encoder's shared memory (no other plan depends on it), and the GATED
+// kernels take the chosen one from the record.
+struct AutoPlan {
+    CandidateList list;
+    int coder[kMaxCandidates];
+    uint32_t sb[kMaxCandidates];
+    uint32_t n_groups;
+};
+
+AutoPlan plan_auto(const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm)
+{
+    AutoPlan a = {};
+    uint32_t key[kMaxCandidates];
+    a.list.n = n_candidates;
+    a.list.tolerance_ppm = tolerance_ppm;
+    for (uint32_t i = 0; i < n_candidates; i++) {
+        const int coder = static_cast<int>(candidates[i] >> 8);
+        const uint32_t sb = candidates[i] & 0xffu;
+        const bool by_sb = (coder == RB200_CODER_ALIAS || coder == RB200_CODER_BYTE) && (sb == 16 || sb == 14 || sb == 12);
+        const uint32_t k = static_cast<uint32_t>(coder) << 8 | (by_sb ? sb : 0u);
+        uint32_t g = 0;
+        while (g < a.n_groups && key[g] != k) g++;
+        if (g == a.n_groups) {
+            key[g] = k;
+            a.coder[g] = coder;
+            a.sb[g] = sb;
+            a.n_groups++;
+        }
+        a.sb[g] = std::max(a.sb[g], sb);
+        a.list.pair[i] = candidates[i];
+        a.list.group[i] = g;
+    }
+    return a;
+}
+
 // The body of both model encodes (model_kernels.cuh): histogram, model kernel, the coder's encoder, the CRCs and the
 // header.  d_n null: n symbols, every length by value.  d_n set: n is the bound n_max, which sizes every launch; the plan
-// kernel reads *d_n into the record at every run, and every later kernel is its GEOM instance.
+// kernel reads *d_n into the record at every run, and every later kernel is its GEOM instance.  a set (the auto encode):
+// the choice kernel, the CHOSEN model kernel, every group's gated encode, the CHOSEN header kernel; coder and
+// scale_bits are then the first candidate's, for the host-side layout only (it does not depend on them).
 int model_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, size_t n, const uint64_t* d_n, uint32_t chunk_syms,
-                 uint32_t flags, uint8_t* out, size_t out_cap)
+                 uint32_t flags, uint8_t* out, size_t out_cap, const AutoPlan* a = nullptr)
 {
     const size_t n_chunks = rb200_chunk_count(n, chunk_syms);
     const ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n, n_chunks, 0, flags);
@@ -1787,6 +1838,11 @@ int model_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* 
     ModelAsyncWork* w = ctx->d_model_async;
     VarlenGeom* geom = d_n ? &w->geom : nullptr;
     int rc = RB200_OK;
+    if (a) {                 // every group's workspace first, so that no group's launch is followed by a reallocation
+        for (uint32_t k = 0; k < a->n_groups && rc == RB200_OK; k++)
+            rc = reserve_plan(ctx, plan_encode(ctx, a->coder[k], a->sb[k], static_cast<uint32_t>(n_chunks), chunk_syms, false));
+        if (rc != RB200_OK) return rc;
+    }
     if (geom) {
         varlen_plan_kernel<<<1, 32, 0, s>>>(d_n, n, chunk_syms, out_cap, geom, ctx->d_status);
         rc = check_launch(ctx, "varlen_plan_kernel");
@@ -1796,13 +1852,29 @@ int model_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* 
     launch_histogram(s, static_cast<uint32_t>(ctx->sms), in, n, w->counts, geom);
     rc = check_launch(ctx, "histogram_kernel");
     if (rc != RB200_OK) return rc;
-    auto model = geom ? container_model_kernel<true> : container_model_kernel<false>;
+    if (a) {
+        coder_choice_kernel<<<1, a->list.n * 32, 0, s>>>(a->list, n_chunks, w, geom, ctx->d_status);
+        rc = check_launch(ctx, "coder_choice_kernel");
+        if (rc != RB200_OK) return rc;
+    }
+    auto model = a ? (geom ? container_model_kernel<true, true> : container_model_kernel<false, true>)
+                   : (geom ? container_model_kernel<true> : container_model_kernel<false>);
     model<<<1, kModelThreads, 0, s>>>(static_cast<uint32_t>(coder), scale_bits, word_r32_allowed() ? 1u : 0u, w, ctx->d_status);
     rc = check_launch(ctx, "container_model_kernel");
     if (rc != RB200_OK) return rc;
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
     uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
-    rc = encode_device(ctx, workspace_tables(w, coder, scale_bits), in, n, chunk_syms, geom ? out : out + boff, out_cap - boff, dir, geom);
+    uint8_t* blob = geom ? out : out + boff;
+    if (a) {
+        for (uint32_t k = 0; k < a->n_groups && rc == RB200_OK; k++) {
+            EncodeTables t = workspace_tables(w, a->coder[k], a->sb[k]);
+            t.choice = &w->choice;
+            t.group = k;
+            rc = encode_device(ctx, t, in, n, chunk_syms, blob, out_cap - boff, dir, geom);
+        }
+    } else {
+        rc = encode_device(ctx, workspace_tables(w, coder, scale_bits), in, n, chunk_syms, blob, out_cap - boff, dir, geom);
+    }
     if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, geom ? &geom->dir_len : nullptr, 0, ctx->d_crc);
     if (rc == RB200_OK && blob_crc) {
         if (geom) {
@@ -1814,8 +1886,9 @@ int model_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* 
         }
     }
     if (rc != RB200_OK) return rc;
-    auto finish = geom ? container_finish_kernel<true> : container_finish_kernel<false>;
-    finish<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, w->freqs, ctx->d_crc, ctx->d_status, geom);
+    auto finish = a ? (geom ? container_finish_kernel<true, true> : container_finish_kernel<false, true>)
+                    : (geom ? container_finish_kernel<true> : container_finish_kernel<false>);
+    finish<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, w->freqs, ctx->d_crc, ctx->d_status, geom, &w->choice);
     return check_launch(ctx, "container_finish_kernel");
 }
 
@@ -1841,6 +1914,22 @@ extern "C" int rb200_container_model_encode_varlen_async(rb200_ctx* ctx, int cod
     if (!d_n || (reinterpret_cast<uintptr_t>(d_n) & 7) || n_max == 0) return RB200_E_ARG;
     if (!model_encode_args_ok(ctx, coder, scale_bits, in, n_max, chunk_syms, out)) return RB200_E_ARG;
     return model_encode(ctx, coder, scale_bits, in, n_max, d_n, chunk_syms, flags, out, out_cap);
+}
+
+// Either call above with the pair chosen on the GPU at every run (coder_choice_kernel): the choice kernel, the CHOSEN
+// model kernel, one gated encode group per distinct encoder instance of the list, the CHOSEN header kernel.  No copy,
+// no synchronisation; the workspace grows for every group's plan.
+extern "C" int rb200_container_model_encode_auto_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                       uint32_t tolerance_ppm, const uint8_t* in, const uint64_t* d_n, size_t n,
+                                                       uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    if (!candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    if (d_n && ((reinterpret_cast<uintptr_t>(d_n) & 7) || n == 0)) return RB200_E_ARG;
+    for (uint32_t i = 0; i < n_candidates; i++)
+        if (!model_encode_args_ok(ctx, static_cast<int>(candidates[i] >> 8), candidates[i] & 0xffu, in, n, chunk_syms, out)) return RB200_E_ARG;
+    if (!d_n && n == 0) return RB200_E_MODEL;                        // normalize_freqs divides by the total
+    const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
+    return model_encode(ctx, static_cast<int>(candidates[0] >> 8), candidates[0] & 0xffu, in, n, d_n, chunk_syms, flags, out, out_cap, &a);
 }
 
 // ---------------------------------------------------------------------------

@@ -495,11 +495,15 @@ constexpr uint32_t kScanTile = 4096;
 // container `blob` and its capacity from the record (VarlenGeom, device_utils.cuh); CTAs past the real tiles or chunks
 // exit at entry.  The host fixes whether tile_prefix_kernel runs from n_max's tile count; the prefix and the compaction
 // then both use the device's, which gives the same sums as either choice.
-template <bool GEOM = false>
+// GATED (rb200_container_model_encode_auto_async): the three kernels run only when the choice record (CoderChoice,
+// device_utils.cuh) names `group`, the launch group whose split encoder they finish; otherwise they exit at entry.
+template <bool GEOM = false, bool GATED = false>
 __global__ void __launch_bounds__(1024)
 scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
-                  uint64_t* __restrict__ tile_sums, const VarlenGeom* __restrict__ geom)
+                  uint64_t* __restrict__ tile_sums, const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice,
+                  uint32_t group)
 {
+    if (GATED && choice->group != group) return;
     if (GEOM) {
         n_chunks = geom->n_chunks;
         if (!geom->go || blockIdx.x * kScanTile >= n_chunks) return;
@@ -540,10 +544,12 @@ scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_
 }
 
 // for very large directories: turn tile_sums into exclusive prefixes once, so compact CTAs read one value
-template <bool GEOM = false>
+template <bool GEOM = false, bool GATED = false>
 __global__ void __launch_bounds__(1024)
-tile_prefix_kernel(uint64_t* __restrict__ tile_sums, uint32_t n_tiles, const VarlenGeom* __restrict__ geom)
+tile_prefix_kernel(uint64_t* __restrict__ tile_sums, uint32_t n_tiles, const VarlenGeom* __restrict__ geom,
+                   const CoderChoice* __restrict__ choice, uint32_t group)
 {
+    if (GATED && choice->group != group) return;
     if (GEOM) {
         if (!geom->go) return;
         n_tiles = (geom->n_chunks + kScanTile - 1) / kScanTile;
@@ -584,13 +590,14 @@ constexpr int kCopyWarps = 8;
 constexpr uint32_t kTilePrefixThreshold = 256;   // above this many tiles, tile_prefix_kernel runs first
 
 // one warp moves one chunk stream from the end of its scratch slot to blob[offsets[c]..E_c)
-template <bool GEOM = false>
+template <bool GEOM = false, bool GATED = false>
 __global__ void __launch_bounds__(kCopyWarps * 32)
 compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
                uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
                uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status,
-               const VarlenGeom* __restrict__ geom)
+               const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
 {
+    if (GATED && choice->group != group) return;
     if (GEOM) {
         n_chunks = geom->n_chunks;
         if (!geom->go || blockIdx.x * kCopyWarps >= n_chunks) return;

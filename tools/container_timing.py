@@ -46,9 +46,14 @@ alphabet permuted per block) and "zipf" (the --blocks data):
   rb200_blocks_coder_decode against rb200_container_blocks_coder_decode and rb200_container_blocks_coder_decode_async,
   alternated; the host time each container call takes to return; and a torch.profiler list of the async call's kernels.
 
+With --auto, rb200_container_model_encode_auto_async over {word 12, alias 16, byte 14} with a 2 % tolerance, on 1 GiB of
+uniform bytes and of p = 0.99 data (symbol 0, a Zipf-1.1 tail over the rest), chunks of 8192: against the fixed call
+for the pair it chose, flags 0 and RB200_CONTAINER_CRC_BLOB, alternated; the costs, the bytes per symbol against the
+word coder's; and a torch.profiler list of the auto call's kernels (the choice kernel, the gated-out launches).
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
-    python tools/container_timing.py [--blocks | --blocks-coder | --single | --model] [--reps 10] [--json out.json]"""
+    python tools/container_timing.py [--blocks | --blocks-coder | --single | --model | --auto] [--reps 10] [--json out.json]"""
 import argparse
 import json
 import os
@@ -598,19 +603,95 @@ def model_encode(args):
     return res
 
 
+def skewed_data(n, seed, p_top=0.99):
+    """symbol 0 at p_top, a Zipf-1.1 tail over symbols 1..255, generated on the GPU in pieces"""
+    import torch
+    tail = zipf_data(n, seed + 1)
+    g = torch.Generator(device="cuda")
+    g.manual_seed(seed)
+    step = 1 << 26
+    for lo in range(0, n, step):
+        part = tail[lo:lo + step]
+        u = torch.rand(part.numel(), device="cuda", generator=g)
+        part.copy_(torch.where(u < p_top, torch.zeros_like(part), part % 255 + 1))
+    return tail
+
+
+def auto_encode(args):
+    """rb200_container_model_encode_auto_async over {word 12, alias 16, byte 14} (2 % tolerance) against the fixed call
+    for the pair it chose, on uniform bytes and on p = 0.99 data"""
+    import torch
+    n, chunk, tol = 1 << 30, 8192, 20000
+    cands = [api.CANDIDATE(rb.CODER_WORD, 12), api.CANDIDATE(rb.CODER_ALIAS, 16), api.CANDIDATE(rb.CODER_BYTE, 14)]
+    g = torch.Generator(device="cuda")
+    g.manual_seed(1234)
+    workloads = (("uniform", lambda: torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda", generator=g)),
+                 ("p = 0.99", lambda: skewed_data(n, 1236)))
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    crc = api.CONTAINER_CRC_BLOB
+    cap = ctx.container_capacity(n, chunk)
+    d_ref = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_out = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    res = {"card": card(), "candidates": ["word 12", "alias 16", "byte 14"], "tolerance_ppm": tol, "workloads": {}, "checks": {}}
+
+    def container_size(d):
+        head = d[:64].cpu().numpy()
+        return int(ctx.lib.dll.rb200_container_size(int(head[24:32].view(np.uint64)[0]), int(head[32:40].view(np.uint64)[0])))
+
+    for name, make in workloads:
+        d_in = make()
+        i, r, o = d_in.data_ptr(), d_ref.data_ptr(), d_out.data_ptr()
+        ctx.container_model_encode_auto_async(cands, tol, i, n, chunk, 0, o, cap)
+        sync()
+        head = d_out[:64].cpu().numpy()
+        coder, sb = int(head[6]), int(head[7])
+        blob_auto = int(head[32:40].view(np.uint64)[0])
+        k, costs = api.choose_coder(ctx.histogram_device(i, n), n, chunk, cands, tol)
+        res["checks"][f"{name}: header_is_the_rule's_choice"] = cands[k] == api.CANDIDATE(coder, sb)
+        calls = {}
+        for tag, flags in (("", 0), ("_crc", crc)):
+            calls["auto" + tag] = lambda flags=flags: ctx.container_model_encode_auto_async(cands, tol, i, n, chunk, flags, o, cap)
+            calls["fixed_chosen" + tag] = lambda flags=flags: ctx.container_model_encode_async(coder, sb, i, n, chunk, flags, r, cap)
+        times = alternate(calls, sync, args.warmup, args.reps)
+        for tag in ("", "_crc"):
+            calls["auto" + tag]()
+            calls["fixed_chosen" + tag]()
+            sync()
+            size = container_size(d_out)
+            res["checks"][f"{name}: auto{tag}_equals_fixed_call"] = bool(torch.equal(d_out[:size], d_ref[:size]))
+        ctx.container_model_encode_async(rb.CODER_WORD, 12, i, n, chunk, 0, r, cap)
+        sync()
+        blob_word = int(d_ref[32:40].cpu().numpy().view(np.uint64)[0])
+        kernels = {k: kernel_times(calls[k], sync, args.reps) for k in ("auto_crc", "fixed_chosen_crc")}
+        res["workloads"][name] = {
+            "n": n, "chunk_syms": chunk, "chosen": {"coder": coder, "scale_bits": sb},
+            "costs": [int(c) for c in costs], "blob_bytes": blob_auto,
+            "bytes_per_symbol": blob_auto / n, "word12_bytes_per_symbol": blob_word / n,
+            "encode": times,
+            "auto_minus_fixed_median_us": {tag or "flags 0": 1e3 * (times["auto" + tag]["median_ms"] - times["fixed_chosen" + tag]["median_ms"])
+                                           for tag in ("", "_crc")},
+            "kernels": kernels,
+        }
+        del d_in
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
     ap.add_argument("--blocks-coder", action="store_true", help="per-block models for the byte and rans64 coders, 8192 blocks of 64 KiB")
     ap.add_argument("--single", action="store_true", help="the single-model container's decode calls on three workloads")
     ap.add_argument("--model", action="store_true", help="the single-model container's encode with the model built from the data")
+    ap.add_argument("--auto", action="store_true", help="the model-building encode with the coder chosen on the GPU")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else single(args) if args.single else model_encode(args) if args.model else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:

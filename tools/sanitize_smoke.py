@@ -184,6 +184,26 @@ def main():
         except rb.RansError as e:
             assert e.code == code, e
         assert bool((d_v == 0x5C).all().item())
+    # the coder chosen on the GPU: every gated group of a list that spans all four coders, on data that picks each side,
+    # by value and from device memory; then a list with no feasible candidate
+    cands = [api.CANDIDATE(rb.CODER_WORD, 12), api.CANDIDATE(rb.CODER_ALIAS, 16), api.CANDIDATE(rb.CODER_BYTE, 11),
+             api.CANDIDATE(rb.CODER_RANS64, 14)]
+    d_skew = torch.where(d_in < 250, torch.zeros_like(d_in), d_in)
+    for src in (d_in, d_skew, d_one):
+        for d_len_ptr in (0, d_len.data_ptr()):
+            d_len.fill_(data.size)
+            ctx.container_model_encode_auto_async(cands, 20000, src.data_ptr(), n_max if d_len_ptr else data.size, 4096,
+                                                  api.CONTAINER_CRC_BLOB, d_v.data_ptr(), vcap, n_ptr=d_len_ptr)
+            d_out.zero_()
+            ctx.container_decode_async(d_v.data_ptr(), vcap, d_out.data_ptr(), data.size, d_n.data_ptr())
+            ctx.sync()
+            assert torch.equal(d_out[:data.size], src)
+    ctx.container_model_encode_auto_async([api.CANDIDATE(rb.CODER_BYTE, 16)], 0, d_one.data_ptr(), data.size, 4096, 0, d_c.data_ptr(), ccap)
+    try:
+        ctx.sync()
+        raise SystemExit("no feasible candidate not reported")
+    except rb.RansError as e:
+        assert e.code == -2, e
     print("sanitize smoke ok:", ctx.launches, "launches")
 
 
