@@ -227,7 +227,9 @@ int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf, size_t siz
  * accepted, as by rb200_container_blocks_open).  d_n_symbols (device memory, may be NULL) receives n once header,
  * models and directory pass.  The call returns only RB200_E_ARG (null / misaligned / bad mem) or RB200_E_CUDA;
  * every verdict on the container comes from rb200_sync: RB200_E_STREAM for anything rb200_container_blocks_open
- * rejects, RB200_E_SPACE for n > out_cap; in both cases out is untouched. */
+ * rejects, RB200_E_SPACE for n > out_cap; in both cases out is untouched.  One difference from
+ * rb200_container_blocks_decode: a container that open accepts but the decoder refuses (a blob of 2^36 bytes or more),
+ * which that call reports as RB200_E_ARG, is RB200_E_STREAM here, out untouched. */
 int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                         uint64_t* d_n_symbols);
 /* ---------------------------------------------------------------- per-block models for the byte and rans64 coders */
@@ -304,7 +306,7 @@ int rb200_container_blocks_coder_decode_async(rb200_ctx* ctx, const uint8_t* buf
  * first; in both cases out is untouched.  One difference from rb200_container_decode: a container that open accepts
  * but the decoders refuse (chunk_syms outside 32 .. 2^24, a blob of 2^36 bytes or more, a byte-coder frequency of
  * 65536), which that call reports as RB200_E_ARG or RB200_E_MODEL, is RB200_E_STREAM here, out untouched.  Version 2
- * containers are rejected (RB200_E_STREAM). */
+ * and 3 containers are rejected (RB200_E_STREAM). */
 int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                  uint64_t* d_n_symbols);
 

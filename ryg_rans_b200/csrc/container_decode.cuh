@@ -1,32 +1,29 @@
-// container_decode.cuh -- rb200_container_blocks_decode_async (version 2, per-block models),
-// rb200_container_blocks_coder_decode_async (version 3, per-block models of the byte or rans64 coder) and
-// rb200_container_decode_async (version 1, one model, any coder): a container in device memory, checked and decoded by
+// container_decode.cuh -- rb200_container_decode_async (version 1, one model, any coder),
+// rb200_container_blocks_decode_async (version 2, per-block models) and rb200_container_blocks_coder_decode_async
+// (version 3, per-block models of the byte or rans64 coder): a container in device memory, checked and decoded by
 // kernels alone, so that the call only enqueues work (and can be captured in a CUDA graph).
 //
-// The stages run in stream order; each reads what the one before it left in the context's BlocksAsyncWork (for
-// versions 1 and 3 the first member of their SingleAsyncWork / BlocksCoderAsyncWork):
+// The stages run in stream order; each reads what the one before it left in the call's ContainerAsyncWork (one per
+// version, allocated with the context):
 //   container_plan_kernel          one warp: container_header_ok on buf[0, 64) against size for the call's version ->
-//                                  the plan (version 1 also coder and scale_bits); clears the verdict words and the
-//                                  call's work counters, so that a call never depends on how the previous one ended
-//                                  (version 3: blocks_coder_plan_kernel, container_blocks_coder_header_ok)
+//                                  the plan, coder and scale_bits; clears the verdict words and the decoders' work
+//                                  counters, so that a call never depends on how the previous one ended
 //   crc32_kernel x 2               meta CRC of buf + 64, length from the plan; blob CRC at buf + blob_off (both lengths
 //                                  are zero when the header is rejected, the blob's also when the flag is clear)
-//   container_prefix_check_kernel  container_block_model_sums_to(4096) for every block (version 2; version 3:
-//                                  blocks_coder_prefix_check_kernel, 1 << scale_bits), container_dir_step_ok for
-//                                  every directory entry, container_dir_ends_ok once
+//   container_prefix_check_kernel  container_block_model_sums_to(1 << scale_bits) for every block (none in version 1),
+//                                  container_dir_step_ok for every directory entry, container_dir_ends_ok once
 //   container_table_kernel         version 1, one CTA: container_model_ok and container_model_decodable on the model,
 //                                  then the header coder's decode table, byte for byte what rb200_model_create uploads
-//   container_verdict_kernel       one warp: header CRC (crc fields zero) joined with the meta CRC, both CRCs compared;
-//                                  writes n_symbols, then sets go or ORs kStatStream / kStatSpace into the status word
-//                                  (version 3: blocks_coder_verdict_kernel)
-//   version 2: block_decode_planned_kernel
-//                                  a fixed grid that exits at once unless go; CTAs take block ids from a counter, build
-//                                  the block's slot table in shared memory and decode its chunks
-//   version 3: block_coder_decode_planned_kernel<CODER, SB>, one launch per instance of RB200_BLOCK_CODER_DISPATCH, each
-//              on a fixed grid; go holds the id of the one that runs, which decodes as block_decode_planned_kernel does
-//              with block_coder_decode_kernel's table
-//   version 1: one launch per decoder variant rb200_decode can pick (kDec*), each on a fixed grid; go holds the id of
-//              the one that runs, every other exits before it touches shared memory, TMA or its counter
+//   container_verdict_kernel       one warp: header CRC (crc fields zero) joined with the meta CRC, both CRCs compared,
+//                                  what the decoders refuse; writes n_symbols, then sets go to the id of the decoder to
+//                                  run (container_decoder) or ORs kStatStream / kStatSpace into the status word
+//   the version's decoders         one launch per decoder the version can need, each on a fixed grid of every CTA that
+//                                  is resident at once; only the one whose id is in go runs, every other exits before
+//                                  it touches shared memory, TMA or its counter.  Version 1: one per variant rb200_decode
+//                                  can pick (kDec*); version 2: block_decode_planned_kernel; version 3:
+//                                  block_coder_decode_planned_kernel<CODER, SB>, one per instance of
+//                                  RB200_BLOCK_CODER_DISPATCH.  The per-block ones take block ids from a counter, build
+//                                  the block's table in shared memory and decode its chunks.
 // The rules are the host parser's (container_format.h); they run in its order: content errors before kStatSpace.
 #pragma once
 #include "alias_kernels.cuh"
@@ -45,87 +42,55 @@ struct BlocksPlan {
     uint64_t n_symbols, n_chunks, dir_off, blob_off, blob_bytes;
     uint64_t meta_len;          // bytes meta_crc covers after the header: model section and directory
     uint64_t blob_len;          // blob_bytes with RB200_CONTAINER_CRC_BLOB, else 0
-    uint32_t ok, n_blocks, block_size, chunk_syms;
+    uint32_t ok, n_blocks, block_size, chunk_syms;   // n_blocks, block_size: per-block versions only (else zero)
 };
-
-// The call's workspace: fixed-size, allocated with the context, so the call never allocates.
-struct BlocksAsyncWork {
-    BlocksPlan plan;
-    CrcSlot crc[2];             // meta, blob
-    CrcWork crc_work;           // crc32_kernel's accumulator, zero between launches
-    uint32_t bad;               // a block model or a directory entry broke a rule
-    uint32_t go;                // the verdict: decode.  Private to the call, so that status bits left by earlier calls
-                                // that were not synchronised do not change this call's outcome
-    uint32_t next_block;        // the decoder's work counter; zero between launches (the last CTA out re-arms it)
-    uint32_t ctas_done;
-};
-
-// The decoders of a version 1 container, one per variant rb200_decode picks: the word coder narrow or WIDE (a frequency
-// of 4096), the alias and byte coders specialised for scale_bits 16, 14, 12 or generic (RB200_ALIAS_SB_DISPATCH), rans64.
-// The verdict stores the id of the one to run in go; kDecNone decodes nothing.
-constexpr uint32_t kDecNone = 0, kDecWord = 1, kDecWordWide = 2, kDecAlias = 3, kDecByte = 7, kDecRans64 = 11;
-// offset of a specialisation from kDecAlias / kDecByte
-__host__ __device__ constexpr uint32_t sb_variant(uint32_t sb) { return sb == 16 ? 0 : sb == 14 ? 1 : sb == 12 ? 2 : 3; }
 
 // the largest decode table: rans64's cum2sym at scale_bits 16 and its 256 x {start, freq}
 constexpr uint32_t kSingleTableBytes = (1u << 16) + 2048;
 
-// rb200_container_decode_async's workspace: fixed-size, allocated with the context.
-struct SingleAsyncWork {
-    BlocksAsyncWork c;          // plan (n_blocks 0: no block models), CRCs and verdict words; go is the decoder id
-    uint32_t coder, scale_bits; // from the header, when c.plan.ok
-    uint32_t wide;              // the word table has a slot of frequency 4096
-    uint32_t refused;           // the decoders refuse the model (container_model_decodable)
-    DecodeWork work;            // the decoder's chunk counter; zero between launches (the last warp out re-arms it)
-    alignas(16) uint8_t table[kSingleTableBytes];   // the decode table of the header's coder, as rb200_model_create's
+// The call's workspace: fixed-size, allocated with the context, so the call never allocates.
+struct ContainerAsyncWork {
+    BlocksPlan plan;
+    CrcSlot crc[2];             // meta, blob
+    CrcWork crc_work;           // crc32_kernel's accumulator, zero between launches
+    uint32_t bad;               // the model, a block model or a directory entry broke a rule
+    uint32_t go;                // the verdict: the id of the decoder to run, 0 for none.  Private to the call, so that
+                                // status bits left by earlier calls that were not synchronised do not change its outcome
+    uint32_t next_block;        // the per-block decoders' work counter; zero between launches (the last CTA out re-arms it)
+    uint32_t ctas_done;
+    uint32_t coder, scale_bits; // from the header, when plan.ok
+    uint32_t wide;              // version 1: the word table has a slot of frequency 4096
+    uint32_t refused;           // version 1: the decoders refuse the model (container_model_decodable)
+    DecodeWork work;            // version 1: the decoder's chunk counter; zero between launches (the last warp out re-arms it)
+    alignas(16) uint8_t table[kSingleTableBytes];   // version 1: the decode table of the header's coder, as rb200_model_create's
 };
 
-// rb200_container_blocks_coder_decode_async's workspace (version 3): version 2's, with the header's coder and scale_bits
-struct BlocksCoderAsyncWork {
-    BlocksAsyncWork c;          // plan, CRCs and verdict words; go is the decoder id (block_coder_decoder)
-    uint32_t coder, scale_bits; // from the header, when c.plan.ok
-};
+// The decoders of each version, with ids from 1 in the order of the version's range of the launch table
+// (configure_container_decode); the verdict stores the id of the one to run in go, kDecNone decodes nothing.
+// Version 1: one per variant rb200_decode picks, the word coder narrow or WIDE (a frequency of 4096), the alias and byte
+// coders specialised for scale_bits 16, 14, 12 or generic (RB200_ALIAS_SB_DISPATCH), rans64.  Version 2:
+// block_decode_planned_kernel.  Version 3: one per instance of RB200_BLOCK_CODER_DISPATCH, the byte coder at
+// scale_bits 14, 12 or generic (ids 1, 2, 3), rans64 (4).
+constexpr uint32_t kDecNone = 0, kDecWord = 1, kDecWordWide = 2, kDecAlias = 3, kDecByte = 7, kDecRans64 = 11;
+// offset of a specialisation from kDecAlias / kDecByte
+__host__ __device__ constexpr uint32_t sb_variant(uint32_t sb) { return sb == 16 ? 0 : sb == 14 ? 1 : sb == 12 ? 2 : 3; }
 
-// The decoders of a version 3 container, one per instance of RB200_BLOCK_CODER_DISPATCH: the byte coder at scale_bits
-// 14, 12 or generic (ids 1, 2, 3), rans64 (4).  The verdict stores the id of the one to run in go.
-constexpr int kBlockCoderDecoders = 4;
-__host__ __device__ constexpr uint32_t block_coder_decoder(uint32_t coder, uint32_t sb)
+// the id of the decoder a container of `version` needs for the header's coder and scale_bits (version 1: rb200_decode's
+// choice of kernel, decode_device; wide: the word table has a slot of frequency 4096)
+__host__ __device__ constexpr uint32_t container_decoder(uint32_t version, uint32_t coder, uint32_t sb, uint32_t wide)
 {
-    return coder == RB200_CODER_RANS64 ? 4 : sb == 14 ? 1 : sb == 12 ? 2 : 3;
+    if (version == kContainerVersionBlocks) return 1;
+    if (version == kContainerVersionBlocksCoder) return coder == RB200_CODER_RANS64 ? 4 : sb == 14 ? 1 : sb == 12 ? 2 : 3;
+    if (coder == RB200_CODER_WORD) return wide ? kDecWordWide : kDecWord;
+    if (coder == RB200_CODER_ALIAS) return kDecAlias + sb_variant(sb);
+    if (coder == RB200_CODER_BYTE) return kDecByte + sb_variant(sb);
+    return kDecRans64;
 }
 
-// The plan of a header that passed its version's rules, into p (zero so far): l is the header the layout functions read
-// (for version 3 its version 2 shape); blocks: versions 2 and 3 (version 1 does not check n_blocks and block_size)
-__device__ __forceinline__ void container_plan(const ContainerHeader& l, bool blocks, BlocksPlan& p)
-{
-    p.ok = 1;
-    p.n_symbols = l.n_symbols;
-    p.n_chunks = l.n_chunks;
-    p.dir_off = container_dir_offset(l);
-    p.blob_off = container_blob_offset(l);
-    p.blob_bytes = l.blob_bytes;
-    p.meta_len = container_dir_end(l) - sizeof(ContainerHeader);
-    p.blob_len = (l.flags & RB200_CONTAINER_CRC_BLOB) ? l.blob_bytes : 0;
-    if (blocks) {
-        p.n_blocks = l.n_blocks;
-        p.block_size = l.block_size;
-    }
-    p.chunk_syms = l.chunk_syms;
-}
-
-// the plan, with the verdict words and the decoder's counters cleared
-__device__ __forceinline__ void container_plan_store(BlocksAsyncWork* w, const BlocksPlan& p)
-{
-    w->plan = p;
-    w->bad = 0;
-    w->go = 0;
-    w->next_block = 0;
-    w->ctas_done = 0;
-}
-
-// single: the version 1 call's workspace (w is then &single->c), or null for version 2
+// One warp: the plan of a header that passes the rules of the call's version (a zero plan otherwise), with the verdict
+// words and the decoders' counters cleared
 __global__ void __launch_bounds__(32)
-    container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, BlocksAsyncWork* w, SingleAsyncWork* single)
+    container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, ContainerAsyncWork* w)
 {
     if (threadIdx.x) return;
     BlocksPlan p = {};
@@ -133,52 +98,48 @@ __global__ void __launch_bounds__(32)
     if (size >= sizeof(ContainerHeader)) {                           // a shorter buffer is not read at all
         const ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(buf);
         if (container_header_ok(h, size, static_cast<uint16_t>(version))) {
-            container_plan(h, version == kContainerVersionBlocks, p);
+            p.ok = 1;
+            p.n_symbols = h.n_symbols;
+            p.n_chunks = h.n_chunks;
+            p.dir_off = container_dir_offset(h);
+            p.blob_off = container_blob_offset(h);
+            p.blob_bytes = h.blob_bytes;
+            p.meta_len = container_dir_end(h) - sizeof(ContainerHeader);
+            p.blob_len = (h.flags & RB200_CONTAINER_CRC_BLOB) ? h.blob_bytes : 0;
+            if (container_per_block(h)) {                            // version 1 does not check n_blocks and block_size
+                p.n_blocks = h.n_blocks;
+                p.block_size = h.block_size;
+            }
+            p.chunk_syms = h.chunk_syms;
             coder = h.coder;
             scale_bits = h.scale_bits;
         }
     }
-    container_plan_store(w, p);
-    if (single) {
-        single->coder = coder;
-        single->scale_bits = scale_bits;
-        single->wide = 0;
-        single->refused = 0;
-        single->work = DecodeWork{0, 0};
-    }
-}
-
-// Version 3: its header rule (container_blocks_coder_header_ok, the host parser's), then the plan of its version 2 shape
-__global__ void __launch_bounds__(32)
-    blocks_coder_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, BlocksCoderAsyncWork* w)
-{
-    if (threadIdx.x) return;
-    BlocksPlan p = {};
-    uint32_t coder = 0, scale_bits = 0;
-    if (size >= sizeof(ContainerHeader)) {                           // a shorter buffer is not read at all
-        const ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(buf);
-        if (container_blocks_coder_header_ok(h, size)) {
-            container_plan(container_layout(h), true, p);
-            coder = h.coder;
-            scale_bits = h.scale_bits;
-        }
-    }
-    container_plan_store(&w->c, p);
+    w->plan = p;
+    w->bad = 0;
+    w->go = 0;
+    w->next_block = 0;
+    w->ctas_done = 0;
     w->coder = coder;
     w->scale_bits = scale_bits;
+    w->wide = 0;
+    w->refused = 0;
+    w->work = DecodeWork{0, 0};
 }
 
 // The per-element rules of the prefix.  Each warp stages 32 block models (16 KiB, coalesced) in shared memory with
 // rows padded to 129 words, so that lane r checking row r reads a different bank from every other lane.  Every block
-// sums to total: 4096 (version 2), 1 << scale_bits (version 3).
+// sums to 1 << scale_bits; version 1 has no blocks (n_blocks 0), so only the directory rules run.
 constexpr int kPrefixWarps = 2;
 constexpr uint32_t kPrefixRowWords = 129;
 
-__device__ __forceinline__ void container_prefix_check(const uint8_t* __restrict__ buf, BlocksAsyncWork* w, uint32_t total)
+__global__ void __launch_bounds__(kPrefixWarps * 32)
+    container_prefix_check_kernel(const uint8_t* __restrict__ buf, ContainerAsyncWork* w)
 {
     __shared__ uint32_t s_rows[kPrefixWarps][32 * kPrefixRowWords];
     const BlocksPlan p = w->plan;
     if (!p.ok) return;
+    const uint32_t total = 1u << w->scale_bits;
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint4* models = reinterpret_cast<const uint4*>(buf + sizeof(ContainerHeader));        // 32 vectors per block
     const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + p.dir_off);
@@ -206,39 +167,27 @@ __device__ __forceinline__ void container_prefix_check(const uint8_t* __restrict
     if (!ok) w->bad = 1;
 }
 
-__global__ void __launch_bounds__(kPrefixWarps * 32)
-    container_prefix_check_kernel(const uint8_t* __restrict__ buf, BlocksAsyncWork* w)
-{
-    container_prefix_check(buf, w, 4096);
-}
-
-__global__ void __launch_bounds__(kPrefixWarps * 32)
-    blocks_coder_prefix_check_kernel(const uint8_t* __restrict__ buf, BlocksCoderAsyncWork* w)
-{
-    container_prefix_check(buf, &w->c, 1u << w->scale_bits);
-}
-
 // The version 1 model (256 x u32 at buf + 64) checked and turned into the decode table of the header's coder in
 // s->table, byte for byte what rb200_model_create builds on the host (tables.h has the formats and the per-entry
 // formulas both sides call).  Slot-to-symbol is a binary search over cum, per slot (word) or per 4 slots (the cum2sym
 // bytes of the byte and rans64 coders, stored as one u32); the alias pairing runs on one thread.
 constexpr int kTableThreads = 512;
 
-__global__ void __launch_bounds__(kTableThreads) container_table_kernel(const uint8_t* __restrict__ buf, SingleAsyncWork* s)
+__global__ void __launch_bounds__(kTableThreads) container_table_kernel(const uint8_t* __restrict__ buf, ContainerAsyncWork* s)
 {
     __shared__ uint32_t s_freq[256], s_cum[257];
     __shared__ uint32_t s_divider[256], s_adjust[512], s_slot_freqs[512], s_rest[256], s_given[256];
     __shared__ uint8_t s_sym_id[512];
     __shared__ uint32_t s_build;
     const uint32_t tid = threadIdx.x;
-    if (!s->c.plan.ok) return;
+    if (!s->plan.ok) return;
     const uint32_t coder = s->coder, sb = s->scale_bits;
     if (tid < 256) s_freq[tid] = reinterpret_cast<const uint32_t*>(buf + sizeof(ContainerHeader))[tid];
     __syncthreads();
     if (tid == 0) {
         bool build = false;
         if (!container_model_ok(coder, sb, s_freq)) {
-            s->c.bad = 1;                                            // what rb200_container_open rejects
+            s->bad = 1;                                              // what rb200_container_open rejects
         } else if (!container_model_decodable(coder, s_freq)) {
             s->refused = 1;                                          // what rb200_container_decode refuses
         } else if (coder == RB200_CODER_ALIAS) {
@@ -297,21 +246,13 @@ __global__ void __launch_bounds__(kTableThreads) container_table_kernel(const ui
     }
 }
 
-// the decoder a version 1 container needs: rb200_decode's choice of kernel (decode_device)
-__device__ inline uint32_t single_decoder(uint32_t coder, uint32_t scale_bits, uint32_t wide)
-{
-    if (coder == RB200_CODER_WORD) return wide ? kDecWordWide : kDecWord;
-    if (coder == RB200_CODER_ALIAS) return kDecAlias + sb_variant(scale_bits);
-    if (coder == RB200_CODER_BYTE) return kDecByte + sb_variant(scale_bits);
-    return kDecRans64;
-}
-
 // One warp.  meta_crc covers the header with its crc fields zeroed, then meta_len bytes whose CRC is in crc[0];
-// the header's CRC is taken here with container_finish_kernel's warp helpers and joined (crc32_combine).
-// refused(): the decoders do not take what open accepted (content, as kStatStream); decoder(): the go of a pass.
-template <class Refused, class Decoder>
-__device__ __forceinline__ void container_verdict(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols,
-                                                  BlocksAsyncWork* w, uint32_t* status, Refused refused_of, Decoder decoder)
+// the header's CRC is taken here with container_finish_kernel's warp helpers and joined (crc32_combine).  What open
+// accepts but the decoders do not take is refused as content (kStatStream): a blob of 2^36 bytes or more and version 1's
+// chunk sizes outside 32 .. 2^24 (container_geometry_decodable), version 1's models that the table kernel refused.
+__global__ void __launch_bounds__(32)
+    container_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, ContainerAsyncWork* w,
+                             uint32_t* status, uint32_t version)
 {
     using namespace crc_detail;
     __shared__ uint4 s_head_v[sizeof(ContainerHeader) / 16];
@@ -341,38 +282,13 @@ __device__ __forceinline__ void container_verdict(const uint8_t* __restrict__ bu
     if (lane) return;
     const bool prefix_ok = meta == meta_crc && !w->bad;
     if (prefix_ok && n_symbols) *n_symbols = p.n_symbols;
-    const bool refused = refused_of();
+    const bool refused = w->refused || !container_geometry_decodable(p.chunk_syms, p.blob_bytes);
     if (!prefix_ok || refused || ((flags & RB200_CONTAINER_CRC_BLOB) && w->crc[1].crc != blob_crc))
         atomicOr(status, kStatStream);
     else if (p.n_symbols > out_cap)
         atomicOr(status, kStatSpace);
     else
-        w->go = decoder();
-}
-
-// Versions 1 and 2.  single: as for container_plan_kernel.  Version 1 also refuses what the decoders do not take
-// (container_format.h), and its go is the id of the decoder to run.
-__global__ void __launch_bounds__(32)
-    container_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, BlocksAsyncWork* w,
-                             uint32_t* status, const SingleAsyncWork* single)
-{
-    const BlocksPlan& p = w->plan;
-    container_verdict(
-        buf, out_cap, n_symbols, w, status,
-        [&] { return single && (single->refused || !container_geometry_decodable(p.chunk_syms, p.blob_bytes)); },
-        [&] { return single ? single_decoder(single->coder, single->scale_bits, single->wide) : 1u; });
-}
-
-// Version 3: the block decoders refuse a blob of 2^36 bytes or more (its chunk sizes are theirs by the header rule);
-// go is the id of the decoder of the header's coder and scale_bits.
-__global__ void __launch_bounds__(32)
-    blocks_coder_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, BlocksCoderAsyncWork* w,
-                                uint32_t* status)
-{
-    const BlocksPlan& p = w->c.plan;
-    container_verdict(
-        buf, out_cap, n_symbols, &w->c, status, [&] { return !container_geometry_decodable(p.chunk_syms, p.blob_bytes); },
-        [&] { return block_coder_decoder(w->coder, w->scale_bits); });
+        w->go = container_decoder(version, w->coder, w->scale_bits, w->wide);
 }
 
 // The per-block decoder for a geometry only the device knows: a fixed grid of kPlannedWarps-warp CTAs (resident all at
@@ -381,7 +297,7 @@ __global__ void __launch_bounds__(32)
 constexpr int kPlannedWarps = 8;
 
 __global__ void __launch_bounds__(kPlannedWarps * 32, 8)
-    block_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, BlocksAsyncWork* w, uint32_t* __restrict__ status)
+    block_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* w, uint32_t* __restrict__ status)
 {
     __shared__ __align__(1024) uint8_t s_ring[kPlannedWarps * kRingBytes];
     __shared__ __align__(16) uint32_t s_tab[kWordSlots];
@@ -433,19 +349,19 @@ __global__ void __launch_bounds__(kPlannedWarps * 32, 8)
 
 // The version 3 decoders, one per instance of RB200_BLOCK_CODER_DISPATCH, each on a fixed grid of kPlannedWarps-warp CTAs
 // (resident all at once).  Only the one whose id is in go runs; every other exits before it touches shared memory or
-// the counter.  CTAs take block ids from w->c.next_block; per block, block_coder_decode_kernel's table in shared memory,
+// the counter.  CTAs take block ids from w->next_block; per block, block_coder_decode_kernel's table in shared memory,
 // then the warps take the block's 1..32 chunks in turn.
 template <uint32_t CODER, uint32_t SB>
 __global__ void __launch_bounds__(kPlannedWarps * 32)
-    block_coder_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, BlocksCoderAsyncWork* __restrict__ w,
+    block_coder_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                       uint32_t* __restrict__ status)
 {
-    if (w->c.go != block_coder_decoder(CODER, SB)) return;           // the same for the whole grid
+    if (w->go != container_decoder(kContainerVersionBlocksCoder, CODER, SB, 0)) return;   // the same for the whole grid
     extern __shared__ __align__(1024) uint8_t s_bdec[];             // [kPlannedWarps x 1 KiB rings][cum2sym[1 << sb]][symbol entries]
     __shared__ uint32_t s_cum[257];
     __shared__ uint32_t s_flag[1];
     __shared__ uint32_t s_block;
-    const BlocksPlan& p = w->c.plan;
+    const BlocksPlan& p = w->plan;
     const uint32_t sb = SB ? SB : w->scale_bits, M = 1u << sb;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t n_blocks = p.n_blocks, block_size = p.block_size, chunk_syms = p.chunk_syms;
@@ -458,7 +374,7 @@ __global__ void __launch_bounds__(kPlannedWarps * 32)
     const uint32_t ring = smem_addr(s_bdec) + warp * kRingBytes, tab = smem_addr_pinned(s_tab);
     for (;;) {
         __syncthreads();                                             // the previous block's table is no longer in use
-        if (tid == 0) s_block = atomicAdd(&w->c.next_block, 1u);
+        if (tid == 0) s_block = atomicAdd(&w->next_block, 1u);
         __syncthreads();
         const uint32_t block = s_block;
         if (block >= n_blocks) break;
@@ -479,26 +395,26 @@ __global__ void __launch_bounds__(kPlannedWarps * 32)
         }
     }
     // every CTA has taken its last block id before it counts itself out: the last one re-arms the counter
-    if (tid == 0 && atomicAdd(&w->c.ctas_done, 1u) == gridDim.x - 1) {
-        w->c.next_block = 0;
-        w->c.ctas_done = 0;
+    if (tid == 0 && atomicAdd(&w->ctas_done, 1u) == gridDim.x - 1) {
+        w->next_block = 0;
+        w->ctas_done = 0;
     }
 }
 
-// The version 1 decoders.  Each takes the geometry, the table and its counter from the call's SingleAsyncWork and runs
+// The version 1 decoders.  Each takes the geometry, the table and its counter from the call's ContainerAsyncWork and runs
 // only when go is its id.  Word and alias: the shipped persistent kernels' CTA set-up around decode_persistent with the
 // shipped policies; byte and rans64: the shipped kernels' table staging around a counter-driven loop over
 // decode_window_chunk (their own kernels launch one warp per chunk, a grid only the host can size).
 
 template <bool WIDE>
 __global__ void __launch_bounds__(DecShip::kWarps * 32, DecShip::kMinBlocks)
-    word_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, SingleAsyncWork* __restrict__ w,
+    word_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                uint32_t* __restrict__ status)
 {
     using P = DecShip;
     static_assert(P::kRefill == kRefillCpAsync, "the ring's mbarriers are not initialised here: cp.async refill only");
-    if (w->c.go != (WIDE ? kDecWordWide : kDecWord)) return;        // the same for the whole grid
-    const BlocksPlan p = w->c.plan;
+    if (w->go != (WIDE ? kDecWordWide : kDecWord)) return;        // the same for the whole grid
+    const BlocksPlan p = w->plan;
     extern __shared__ __align__(1024) uint8_t s_dec[];     // [16 KiB table][table mbarrier][kWarps x (ring, mirror, mbarriers)]
     const uint32_t tab = smem_addr_pinned(s_dec);
     const uint32_t bar_tab = tab + kWordSlots * 4;
@@ -528,12 +444,12 @@ __global__ void __launch_bounds__(DecShip::kWarps * 32, DecShip::kMinBlocks)
 
 template <uint32_t SB>
 __global__ void __launch_bounds__(AliasDecShip::kWarps * 32, AliasDecShip::kMinBlocks)
-    alias_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, SingleAsyncWork* __restrict__ w,
+    alias_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                 uint32_t* __restrict__ status)
 {
     using P = AliasDecShip;
-    if (w->c.go != kDecAlias + sb_variant(SB)) return;
-    const BlocksPlan p = w->c.plan;
+    if (w->go != kDecAlias + sb_variant(SB)) return;
+    const BlocksPlan p = w->plan;
     const uint32_t sb_rt = w->scale_bits;
     const AliasDecEntry* g_dec = reinterpret_cast<const AliasDecEntry*>(w->table);
     extern __shared__ __align__(1024) uint8_t s_adec[];       // [32 KiB table][16 B][kWarps x (ring, mirror)]
@@ -558,9 +474,9 @@ __global__ void __launch_bounds__(AliasDecShip::kWarps * 32, AliasDecShip::kMinB
 // window at shared address `ring`; the last warp out re-arms the counter.
 template <class C>
 __device__ __forceinline__ void decode_window_planned(const C& coder, const uint8_t* __restrict__ buf, uint8_t* __restrict__ out,
-                                                      SingleAsyncWork* __restrict__ w, uint32_t ring, uint32_t* __restrict__ status)
+                                                      ContainerAsyncWork* __restrict__ w, uint32_t ring, uint32_t* __restrict__ status)
 {
-    const BlocksPlan p = w->c.plan;
+    const BlocksPlan p = w->plan;
     const uint8_t* blob = buf + p.blob_off;
     const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + p.dir_off);
     const uint32_t lane = threadIdx.x & 31, n_chunks = static_cast<uint32_t>(p.n_chunks);
@@ -585,10 +501,10 @@ __host__ __device__ constexpr uint32_t byte_planned_smem(uint32_t SB) { return k
 
 template <uint32_t SB>
 __global__ void __launch_bounds__(kAliasDecWarps * 32, 4)
-    byte_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, SingleAsyncWork* __restrict__ w,
+    byte_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                uint32_t* __restrict__ status)
 {
-    if (w->c.go != kDecByte + sb_variant(SB)) return;
+    if (w->go != kDecByte + sb_variant(SB)) return;
     const uint32_t sb = SB ? SB : w->scale_bits;
     extern __shared__ __align__(1024) uint8_t s_adec[];       // [16 x 1 KiB rings][table]
     uint4* s_tab = reinterpret_cast<uint4*>(s_adec + kAliasDecWarps * kRingBytes);
@@ -602,10 +518,10 @@ __global__ void __launch_bounds__(kAliasDecWarps * 32, 4)
 constexpr uint32_t kRans64PlannedSmem = kRans64Warps * kRingBytes + kRans64DecSymBytes + (1u << 16);
 
 __global__ void __launch_bounds__(kRans64Warps * 32, 2)
-    rans64_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, SingleAsyncWork* __restrict__ w,
+    rans64_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                  uint32_t* __restrict__ status)
 {
-    if (w->c.go != kDecRans64) return;
+    if (w->go != kDecRans64) return;
     const uint32_t sb = w->scale_bits;
     extern __shared__ __align__(1024) uint8_t s_r64[];        // [16 x 1 KiB rings][cum2sym][256 x 16 replicas x {start, freq}]
     uint4* s_tab = reinterpret_cast<uint4*>(s_r64 + kRans64Warps * kRingBytes);
@@ -623,32 +539,27 @@ __global__ void __launch_bounds__(kRans64Warps * 32, 2)
     decode_window_planned(coder, buf, out, w, smem_addr(s_r64) + warp * kRingBytes, status);
 }
 
-// The launch shapes, fixed per device: the decoder's grid is every CTA that is resident at once.
-struct BlocksAsyncShape {
-    uint32_t decode_grid, check_grid;
-};
-
-inline BlocksAsyncShape configure_container_decode(uint32_t sms)
-{
-    cudaFuncSetAttribute(block_decode_planned_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    int per_sm = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_decode_planned_kernel, kPlannedWarps * 32, 0);
-    return BlocksAsyncShape{sms * static_cast<uint32_t>(per_sm < 1 ? 1 : per_sm), sms * 8};
-}
-
-// One launch of a version 1 decoder: kernel, grid, threads, dynamic shared memory.
-struct SingleDecodeLaunch {
-    void (*kernel)(const uint8_t*, uint8_t*, SingleAsyncWork*, uint32_t*);
+// One launch of a decoder: kernel, grid, threads, dynamic shared memory.
+struct DecoderLaunch {
+    void (*kernel)(const uint8_t*, uint8_t*, ContainerAsyncWork*, uint32_t*);
     uint32_t grid, threads, smem;
     const char* name;
 };
-constexpr int kSingleDecoders = 11;
 
-// The version 1 decoders in id order, each with every CTA that is resident at once (the word and alias grids are the
-// shipped kernels' full grids).
-inline void configure_single_decode(uint32_t sms, SingleDecodeLaunch* out)
+// The decoders of every version in one launch table, each version's in id order: version v's are the entries
+// kDecoderFirst[v - 1] .. kDecoderFirst[v] - 1.
+constexpr int kDecoderFirst[] = {0, 11, 12, 16};
+constexpr int kContainerDecoders = kDecoderFirst[3];
+// the prefix check's grid: kPrefixCtasPerSm CTAs of kPrefixWarps warps per SM
+constexpr uint32_t kPrefixCtasPerSm = 8;
+
+// The launch table, fixed per device: each decoder's grid is every CTA that is resident at once (the version 1 word and
+// alias grids are the shipped kernels' full grids); the generic byte and rans64 decoders get shared memory for the
+// largest scale_bits they decode.
+inline void configure_container_decode(uint32_t sms, DecoderLaunch* out)
 {
-    const SingleDecodeLaunch l[kSingleDecoders] = {
+    constexpr uint32_t planned = kPlannedWarps * 32;
+    const DecoderLaunch l[kContainerDecoders] = {
         {word_decode_planned_kernel<false>, sms * DecShip::kMinBlocks, DecShip::kWarps * 32, DecShip::kSmemBytes, "word_decode_planned_kernel"},
         {word_decode_planned_kernel<true>, sms * DecShip::kMinBlocks, DecShip::kWarps * 32, DecShip::kSmemBytes, "word_decode_planned_kernel(wide)"},
         {alias_decode_planned_kernel<16>, sms * AliasDecShip::kMinBlocks, AliasDecShip::kWarps * 32, AliasDecShip::kSmemBytes, "alias_decode_planned_kernel<16>"},
@@ -660,8 +571,17 @@ inline void configure_single_decode(uint32_t sms, SingleDecodeLaunch* out)
         {byte_decode_planned_kernel<12>, 0, kAliasDecWarps * 32, byte_planned_smem(12), "byte_decode_planned_kernel<12>"},
         {byte_decode_planned_kernel<0>, 0, kAliasDecWarps * 32, byte_planned_smem(0), "byte_decode_planned_kernel<0>"},
         {rans64_decode_planned_kernel, 0, kRans64Warps * 32, kRans64PlannedSmem, "rans64_decode_planned_kernel"},
+        {block_decode_planned_kernel, 0, planned, 0, "block_decode_planned_kernel"},
+        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 14>, 0, planned, block_coder_decode_smem(RB200_CODER_BYTE, 14, planned),
+         "block_coder_decode_planned_kernel<byte, 14>"},
+        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 12>, 0, planned, block_coder_decode_smem(RB200_CODER_BYTE, 12, planned),
+         "block_coder_decode_planned_kernel<byte, 12>"},
+        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 0>, 0, planned,
+         block_coder_decode_smem(RB200_CODER_BYTE, kBlockCoderMaxScaleBits, planned), "block_coder_decode_planned_kernel<byte, 0>"},
+        {block_coder_decode_planned_kernel<RB200_CODER_RANS64, 0>, 0, planned,
+         block_coder_decode_smem(RB200_CODER_RANS64, kBlockCoderMaxScaleBits, planned), "block_coder_decode_planned_kernel<rans64, 0>"},
     };
-    for (int i = 0; i < kSingleDecoders; i++) {
+    for (int i = 0; i < kContainerDecoders; i++) {
         out[i] = l[i];
         cudaFuncSetAttribute(l[i].kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(l[i].kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(l[i].smem));
@@ -670,37 +590,6 @@ inline void configure_single_decode(uint32_t sms, SingleDecodeLaunch* out)
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, l[i].kernel, static_cast<int>(l[i].threads), l[i].smem);
             out[i].grid = sms * static_cast<uint32_t>(per_sm < 1 ? 1 : per_sm);
         }
-    }
-}
-
-// One launch of a version 3 decoder: kernel, grid (every CTA that is resident at once), dynamic shared memory.
-struct BlockCoderDecodeLaunch {
-    void (*kernel)(const uint8_t*, uint8_t*, BlocksCoderAsyncWork*, uint32_t*);
-    uint32_t grid, smem;
-    const char* name;
-};
-
-// The version 3 decoders in id order; shared memory for the largest scale_bits each decodes (the generic ones: 15).
-inline void configure_blocks_coder_decode(uint32_t sms, BlockCoderDecodeLaunch* out)
-{
-    constexpr uint32_t threads = kPlannedWarps * 32;
-    const BlockCoderDecodeLaunch l[kBlockCoderDecoders] = {
-        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 14>, 0, block_coder_decode_smem(RB200_CODER_BYTE, 14, threads),
-         "block_coder_decode_planned_kernel<byte, 14>"},
-        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 12>, 0, block_coder_decode_smem(RB200_CODER_BYTE, 12, threads),
-         "block_coder_decode_planned_kernel<byte, 12>"},
-        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 0>, 0, block_coder_decode_smem(RB200_CODER_BYTE, kBlockCoderMaxScaleBits, threads),
-         "block_coder_decode_planned_kernel<byte, 0>"},
-        {block_coder_decode_planned_kernel<RB200_CODER_RANS64, 0>, 0,
-         block_coder_decode_smem(RB200_CODER_RANS64, kBlockCoderMaxScaleBits, threads), "block_coder_decode_planned_kernel<rans64, 0>"},
-    };
-    for (int i = 0; i < kBlockCoderDecoders; i++) {
-        out[i] = l[i];
-        cudaFuncSetAttribute(l[i].kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        cudaFuncSetAttribute(l[i].kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(l[i].smem));
-        int per_sm = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, l[i].kernel, static_cast<int>(threads), l[i].smem);
-        out[i].grid = sms * static_cast<uint32_t>(per_sm < 1 ? 1 : per_sm);
     }
 }
 

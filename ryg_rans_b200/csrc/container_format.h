@@ -40,34 +40,27 @@ static_assert(sizeof(ContainerHeader) == 64, "container header must stay 64 byte
 constexpr size_t kContainerDirOffset = sizeof(ContainerHeader) + 256 * sizeof(uint32_t);   // version 1: 1088, 16-aligned
 constexpr size_t kBlockModelBytes = 256 * sizeof(uint16_t);                                 // one block's frequencies
 
+// versions 2 and 3: a model per block, n_blocks x 256 x u16 (version 1: one model, 256 x u32)
+RB200_HD inline bool container_per_block(const ContainerHeader& h)
+{
+    return h.version == kContainerVersionBlocks || h.version == kContainerVersionBlocksCoder;
+}
+
 // The layout, as functions of the (parsed) header: model section, directory, pad to 16, blob.  Version 1 keeps 1024
-// bytes of model, so its directory stays at 1088; version 2 has 512 bytes per block, so its directory starts at
-// 64 + 512 n_blocks, also 16-aligned.  64-bit throughout: n_blocks < 2^32 and n_chunks < 2^31 once parsed.
+// bytes of model, so its directory stays at 1088; the per-block versions have 512 bytes per block, so their directory
+// starts at 64 + 512 n_blocks, also 16-aligned.  64-bit throughout: n_blocks < 2^32 and n_chunks < 2^31 once parsed.
 RB200_HD inline uint64_t container_model_bytes(const ContainerHeader& h)
 {
-    return h.version == kContainerVersionBlocks ? kBlockModelBytes * h.n_blocks : 256 * sizeof(uint32_t);
+    return container_per_block(h) ? kBlockModelBytes * h.n_blocks : 256 * sizeof(uint32_t);
 }
 RB200_HD inline uint64_t container_dir_offset(const ContainerHeader& h) { return sizeof(ContainerHeader) + container_model_bytes(h); }
 RB200_HD inline uint64_t container_dir_end(const ContainerHeader& h) { return container_dir_offset(h) + (h.n_chunks + 1) * sizeof(uint64_t); }
 RB200_HD inline uint64_t container_blob_offset(const ContainerHeader& h) { return (container_dir_end(h) + 15) & ~15ull; }
 
-// Version 3 is version 2 with the header's own coder (byte or rans64) and scale_bits (8..15): the same layout, and every
-// rule of version 2 but the coder, scale_bits and the block total.  The layout functions above and container_header_ok
-// serve versions 1 and 2; host and kernels read a version 3 header through its version 2 shape
-// (container_blocks_coder_header_ok below).
+// version 3's coder and scale_bits: byte or rans64 at 8..15
 RB200_HD inline bool container_blocks_coder_ok(uint32_t coder, uint32_t scale_bits)
 {
     return (coder == RB200_CODER_BYTE || coder == RB200_CODER_RANS64) && scale_bits >= 8 && scale_bits <= 15;
-}
-// the header the layout functions and version 2's rules read for h: h itself, or for version 3 its version 2 shape
-RB200_HD inline ContainerHeader container_layout(ContainerHeader h)
-{
-    if (h.version == kContainerVersionBlocksCoder) {
-        h.version = kContainerVersionBlocks;
-        h.coder = RB200_CODER_WORD;
-        h.scale_bits = 12;
-    }
-    return h;
 }
 
 // a header with only what the layout depends on: for sizes computed before there is a header
@@ -89,14 +82,17 @@ RB200_HD inline bool container_blocks_geometry_ok(uint32_t n_blocks, uint32_t bl
 }
 
 // Every rule of a header (already read from the first 64 of `size` bytes) for the one `version` the caller accepts:
-// the fields agree with each other and with the geometry the decoders take, and every section fits `size`.
+// the fields agree with each other and with the geometry the decoders take, and every section fits `size`.  The
+// per-block versions share every rule but the coder and scale_bits: the word coder at 12 (version 2), byte or rans64
+// at 8..15 (version 3).
 RB200_HD inline bool container_header_ok(const ContainerHeader& h, uint64_t size, uint16_t version)
 {
     if (h.magic != kContainerMagic || h.version != version || h.lanes != RB200_LANES || !h.chunk_syms) return false;
-    if (version == kContainerVersionBlocks) {
-        // what rb200_blocks_decode accepts; n_blocks * block_size cannot overflow 64 bits
-        if (h.coder != RB200_CODER_WORD || h.scale_bits != 12 || !container_blocks_geometry_ok(h.n_blocks, h.block_size, h.chunk_syms))
-            return false;
+    if (container_per_block(h)) {
+        const bool coder_ok = version == kContainerVersionBlocks ? h.coder == RB200_CODER_WORD && h.scale_bits == 12
+                                                                 : container_blocks_coder_ok(h.coder, h.scale_bits);
+        // what rb200_blocks_decode / rb200_blocks_coder_decode accept; n_blocks * block_size cannot overflow 64 bits
+        if (!coder_ok || !container_blocks_geometry_ok(h.n_blocks, h.block_size, h.chunk_syms)) return false;
         if (h.n_symbols != static_cast<uint64_t>(h.n_blocks) * h.block_size || h.n_chunks != h.n_symbols / h.chunk_syms ||
             h.n_chunks >= (1ull << 31) || (h.blob_bytes & 15) || h.reserved || (h.flags & ~RB200_CONTAINER_CRC_BLOB))
             return false;
@@ -106,12 +102,6 @@ RB200_HD inline bool container_header_ok(const ContainerHeader& h, uint64_t size
     }
     const uint64_t boff = container_blob_offset(h);                 // < 2^42: n_chunks < 2^31, n_blocks < 2^32
     return boff <= size && h.blob_bytes <= size - boff;
-}
-// Every rule of a version 3 header: its coder and scale_bits, then version 2's rules on its version 2 shape.
-RB200_HD inline bool container_blocks_coder_header_ok(const ContainerHeader& h, uint64_t size)
-{
-    return h.version == kContainerVersionBlocksCoder && container_blocks_coder_ok(h.coder, h.scale_bits) &&
-           container_header_ok(container_layout(h), size, kContainerVersionBlocks);
 }
 
 // what rb200_model_create would accept: a known coder, its scale_bits range, frequencies that sum to 1 << scale_bits
@@ -200,16 +190,14 @@ RB200_HD inline int choose_candidate(const uint64_t* costs, uint32_t n, uint32_t
     return -1;
 }
 
-// The per-element rules of a version 2 prefix, one block or one directory entry at a time.
-// one block's 256 frequencies sum to total (version 3: 1 << scale_bits)
+// The per-element rules of a prefix, one block or one directory entry at a time.
+// one block's 256 frequencies sum to total: 1 << scale_bits (4096 in version 2)
 RB200_HD inline bool container_block_model_sums_to(const uint16_t* freqs, uint32_t total)
 {
     uint32_t sum = 0;
     for (int s = 0; s < 256; s++) sum += freqs[s];
     return sum == total;
 }
-// one block's 256 frequencies sum to 4096
-RB200_HD inline bool container_block_model_ok(const uint16_t* freqs) { return container_block_model_sums_to(freqs, 4096); }
 // entry c (< n_chunks) of the directory is not above the next one
 RB200_HD inline bool container_dir_step_ok(const uint64_t* offsets, uint64_t c) { return offsets[c] <= offsets[c + 1]; }
 // the first stream starts inside the first vector, the last entry is the blob size
@@ -226,8 +214,6 @@ ContainerHeader container_blocks_header(uint32_t n_blocks, uint32_t block_size, 
 // the header rb200_container_blocks_coder_pack writes (crc fields zero)
 ContainerHeader container_blocks_coder_header(int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
                                               uint64_t blob_bytes, uint32_t flags);
-// every block's 256 frequencies sum to 4096
-bool container_block_models_ok(const uint16_t* block_freqs, uint32_t n_blocks);
 // every block's 256 frequencies sum to total
 bool container_block_models_sum_to(const uint16_t* block_freqs, uint32_t n_blocks, uint32_t total);
 // the directory rules: the first stream starts inside the first vector, monotone, last entry == blob_bytes

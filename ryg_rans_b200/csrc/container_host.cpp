@@ -10,7 +10,7 @@
 //
 // All integers little-endian.  CRC-32 (zlib's: IEEE, reflected) over header (with the crc fields zeroed) + model +
 // offsets always (meta_crc); over the blob when RB200_CONTAINER_CRC_BLOB is set.  The header layout is the same in
-// both versions.  Version 1 has its directory at 1088; version 2 (word coder, scale_bits 12, 32 lanes) carries
+// every version.  Version 1 has its directory at 1088; version 2 (word coder, scale_bits 12, 32 lanes) carries
 // block_size at byte 52 and n_blocks at byte 56, its model section is 512 n_blocks bytes, so its directory starts at
 // 64 + 512 n_blocks, and the u32 at byte 60 is zero.  Its chunk order is the per-block calls': chunk = block *
 // (block_size / chunk_syms) + chunk-in-block, so each block's chunks are ordinary 32-way word streams under that
@@ -20,18 +20,16 @@
 // fits the buffer, no flag but RB200_CONTAINER_CRC_BLOB, meta_crc matches, every block's frequencies sum to 4096, the
 // directory rules of version 1 hold (offsets[0] < 16, monotone, offsets[n_chunks] == blob_bytes), and the blob CRC
 // matches when present.  Version 3 is version 2 with the header's own coder (RB200_CODER_BYTE or RB200_CODER_RANS64) and
-// scale_bits (8..15), every block's frequencies summing to 1 << scale_bits; every other rule is version 2's.  Each call
-// accepts exactly one version: rb200_container_* version 1, rb200_container_blocks_* version 2,
+// scale_bits (8..15); every other rule is version 2's, and in both every block's frequencies sum to 1 << scale_bits.
+// Each call accepts exactly one version: rb200_container_* version 1, rb200_container_blocks_* version 2,
 // rb200_container_blocks_coder_* version 3.
 //
 // rb200_container_pack / _open and the _blocks_ forms here work on host buffers with a host CRC (slicing-by-8, ~1 GB/s
 // on one core: the blob CRC is optional for that reason).  rb200_container_encode / _decode and the _blocks_ forms
 // (rans_b200.cu) write and read the same bytes in host or device memory with the blob CRC on the GPU
-// (crc_kernels.cuh); they validate through the parser below, so both sides apply one set of rules.
-// rb200_container_decode_async, rb200_container_blocks_decode_async and rb200_container_blocks_coder_decode_async apply
-// the same rules in kernels
-// (container_decode.cuh): the header, model and per-element rules are the __host__ __device__ functions of
-// container_format.h that the parser below calls.
+// (crc_kernels.cuh); they validate through the parser below, so both sides apply one set of rules.  The _decode_async
+// forms apply the same rules in kernels (container_decode.cuh): the header, model and per-element rules are the
+// __host__ __device__ functions of container_format.h that the parser below calls.
 #include "container_format.h"
 
 #include <cstring>
@@ -87,15 +85,8 @@ uint32_t container_header_crc(const ContainerHeader& h)
 uint32_t container_meta_crc(const ContainerHeader& h, const void* model, const uint64_t* offsets)
 {
     uint32_t c = container_header_crc(h);
-    c = container_crc32(c, model, container_model_bytes(container_layout(h)));
+    c = container_crc32(c, model, container_model_bytes(h));
     return container_crc32(c, offsets, (h.n_chunks + 1) * sizeof(uint64_t));
-}
-
-bool container_block_models_ok(const uint16_t* block_freqs, uint32_t n_blocks)
-{
-    for (uint64_t b = 0; b < n_blocks; b++)
-        if (!container_block_model_ok(block_freqs + b * 256)) return false;
-    return true;
 }
 
 bool container_block_models_sum_to(const uint16_t* block_freqs, uint32_t n_blocks, uint32_t total)
@@ -155,8 +146,7 @@ int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, Co
     if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
     ContainerHeader h;
     std::memcpy(&h, hdr, sizeof h);
-    const bool ok = version == kContainerVersionBlocksCoder ? container_blocks_coder_header_ok(h, size) : container_header_ok(h, size, version);
-    if (!ok) return RB200_E_STREAM;
+    if (!container_header_ok(h, size, version)) return RB200_E_STREAM;
     *out = h;
     return RB200_OK;
 }
@@ -164,12 +154,11 @@ int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, Co
 int container_check_prefix(const ContainerHeader& h, const uint8_t* prefix, uint32_t meta_crc)
 {
     const uint8_t* model = prefix + sizeof(ContainerHeader);
-    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(prefix + container_dir_offset(container_layout(h)));
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(prefix + container_dir_offset(h));
     if (meta_crc != h.meta_crc) return RB200_E_STREAM;
-    const uint16_t* block_freqs = reinterpret_cast<const uint16_t*>(model);
-    const bool model_ok = h.version == kContainerVersionBlocks        ? container_block_models_ok(block_freqs, h.n_blocks)
-                          : h.version == kContainerVersionBlocksCoder ? container_block_models_sum_to(block_freqs, h.n_blocks, 1u << h.scale_bits)
-                                                                      : container_model_ok(h.coder, h.scale_bits, reinterpret_cast<const uint32_t*>(model));
+    const bool model_ok = container_per_block(h)
+                              ? container_block_models_sum_to(reinterpret_cast<const uint16_t*>(model), h.n_blocks, 1u << h.scale_bits)
+                              : container_model_ok(h.coder, h.scale_bits, reinterpret_cast<const uint32_t*>(model));
     if (!model_ok) return RB200_E_STREAM;                                                  // CRC-valid but inconsistent
     return container_directory_ok(offsets, h.n_chunks, h.blob_bytes) ? RB200_OK : RB200_E_STREAM;
 }
@@ -186,10 +175,9 @@ void container_write(ContainerHeader h, const void* model, const uint64_t* offse
 {
     h.meta_crc = container_meta_crc(h, model, offsets);
     if (h.flags & RB200_CONTAINER_CRC_BLOB) h.blob_crc = container_crc32(0, blob, h.blob_bytes);
-    const ContainerHeader l = container_layout(h);
-    const uint64_t dir = container_dir_offset(l), dir_end = container_dir_end(l), boff = container_blob_offset(l);
+    const uint64_t dir = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
     std::memcpy(out, &h, sizeof h);
-    std::memcpy(out + sizeof h, model, container_model_bytes(l));
+    std::memcpy(out + sizeof h, model, container_model_bytes(h));
     std::memcpy(out + dir, offsets, dir_end - dir);
     std::memset(out + dir_end, 0, boff - dir_end);
     if (h.blob_bytes) std::memcpy(out + boff, blob, h.blob_bytes);
@@ -202,12 +190,46 @@ int container_open_checked(const uint8_t* buf, size_t size, uint16_t version, Co
     if (rc != RB200_OK) return rc;
     // model and offsets sit at 4- and 8-byte aligned positions when buf itself is 8-byte aligned (callers map or malloc it)
     if (reinterpret_cast<uintptr_t>(buf) & 7) return RB200_E_ARG;
-    const ContainerHeader l = container_layout(*h);
     rc = container_check_prefix(*h, buf, container_meta_crc(*h, buf + sizeof(ContainerHeader),
-                                                            reinterpret_cast<const uint64_t*>(buf + container_dir_offset(l))));
+                                                            reinterpret_cast<const uint64_t*>(buf + container_dir_offset(*h))));
     if (rc == RB200_OK && (h->flags & RB200_CONTAINER_CRC_BLOB))
-        rc = container_check_blob(*h, container_crc32(0, buf + container_blob_offset(l), h->blob_bytes));
+        rc = container_check_blob(*h, container_crc32(0, buf + container_blob_offset(*h), h->blob_bytes));
     return rc;
+}
+
+// The pack of both per-block versions, for the header h (crc fields zero) the caller built from a geometry it checked:
+// the other argument rules, every block summing to 1 << h.scale_bits, then the bytes.
+int container_blocks_pack(const ContainerHeader& h, const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob,
+                          uint8_t* out, size_t out_cap, size_t* out_size)
+{
+    if (!block_freqs || !offsets || (!blob && h.blob_bytes) || !out || h.n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    if (!container_block_models_sum_to(block_freqs, h.n_blocks, 1u << h.scale_bits)) return RB200_E_MODEL;   // never write what open rejects
+    if ((h.blob_bytes & 15) || !container_directory_ok(offsets, h.n_chunks, h.blob_bytes)) return RB200_E_ARG;
+    const size_t total = container_blob_offset(h) + h.blob_bytes;
+    if (total > out_cap) return RB200_E_SPACE;
+    container_write(h, block_freqs, offsets, blob, out);
+    if (out_size) *out_size = total;
+    return RB200_OK;
+}
+
+// The open of both per-block versions: the parser's steps for `version`, then the fields their info structs share.
+template <class Info>
+int container_blocks_open(const uint8_t* buf, size_t size, uint16_t version, Info* info, ContainerHeader* h)
+{
+    if (!buf || !info) return RB200_E_ARG;
+    const int rc = container_open_checked(buf, size, version, h);
+    if (rc != RB200_OK) return rc;
+    info->n_blocks = h->n_blocks;
+    info->block_size = h->block_size;
+    info->chunk_syms = h->chunk_syms;
+    info->flags = h->flags;
+    info->n_symbols = h->n_symbols;
+    info->n_chunks = h->n_chunks;
+    info->blob_bytes = h->blob_bytes;
+    info->block_freqs = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));
+    info->offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(*h));
+    info->blob = buf + container_blob_offset(*h);
+    return RB200_OK;
 }
 
 }  // namespace
@@ -264,77 +286,34 @@ extern "C" int rb200_container_blocks_pack(uint32_t n_blocks, uint32_t block_siz
                                            const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes, uint32_t flags, uint8_t* out,
                                            size_t out_cap, size_t* out_size)
 {
-    if (!block_freqs || !offsets || (!blob && blob_bytes) || !out) return RB200_E_ARG;
     if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
-    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
-    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
-    if (!container_block_models_ok(block_freqs, n_blocks)) return RB200_E_MODEL;          // never write what open rejects
-    if ((blob_bytes & 15) || !container_directory_ok(offsets, n_chunks, blob_bytes)) return RB200_E_ARG;
-    const ContainerHeader h = container_blocks_header(n_blocks, block_size, chunk_syms, blob_bytes, flags);
-    const size_t total = container_blob_offset(h) + blob_bytes;
-    if (total > out_cap) return RB200_E_SPACE;
-    container_write(h, block_freqs, offsets, blob, out);
-    if (out_size) *out_size = total;
-    return RB200_OK;
+    return container_blocks_pack(container_blocks_header(n_blocks, block_size, chunk_syms, blob_bytes, flags), block_freqs, offsets, blob,
+                                 out, out_cap, out_size);
 }
 
 extern "C" int rb200_container_blocks_open(const uint8_t* buf, size_t size, rb200_container_blocks_info* info)
 {
-    if (!buf || !info) return RB200_E_ARG;
     ContainerHeader h;
-    const int rc = container_open_checked(buf, size, kContainerVersionBlocks, &h);
-    if (rc != RB200_OK) return rc;
-    info->n_blocks = h.n_blocks;
-    info->block_size = h.block_size;
-    info->chunk_syms = h.chunk_syms;
-    info->flags = h.flags;
-    info->n_symbols = h.n_symbols;
-    info->n_chunks = h.n_chunks;
-    info->blob_bytes = h.blob_bytes;
-    info->block_freqs = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));
-    info->offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h));
-    info->blob = buf + container_blob_offset(h);
-    return RB200_OK;
+    return container_blocks_open(buf, size, kContainerVersionBlocks, info, &h);
 }
 
 extern "C" int rb200_container_blocks_coder_pack(int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
                                                  const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob,
                                                  size_t blob_bytes, uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size)
 {
-    if (!block_freqs || !offsets || (!blob && blob_bytes) || !out) return RB200_E_ARG;
     if (coder < 0 || !container_blocks_coder_ok(static_cast<uint32_t>(coder), scale_bits)) return RB200_E_ARG;
     if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
-    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
-    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
-    if (!container_block_models_sum_to(block_freqs, n_blocks, 1u << scale_bits)) return RB200_E_MODEL;   // never write what open rejects
-    if ((blob_bytes & 15) || !container_directory_ok(offsets, n_chunks, blob_bytes)) return RB200_E_ARG;
-    const ContainerHeader h = container_blocks_coder_header(coder, scale_bits, n_blocks, block_size, chunk_syms, blob_bytes, flags);
-    const size_t total = container_blob_offset(container_layout(h)) + blob_bytes;
-    if (total > out_cap) return RB200_E_SPACE;
-    container_write(h, block_freqs, offsets, blob, out);
-    if (out_size) *out_size = total;
-    return RB200_OK;
+    return container_blocks_pack(container_blocks_coder_header(coder, scale_bits, n_blocks, block_size, chunk_syms, blob_bytes, flags),
+                                 block_freqs, offsets, blob, out, out_cap, out_size);
 }
 
 extern "C" int rb200_container_blocks_coder_open(const uint8_t* buf, size_t size, rb200_container_blocks_coder_info* info)
 {
-    if (!buf || !info) return RB200_E_ARG;
     ContainerHeader h;
-    const int rc = container_open_checked(buf, size, kContainerVersionBlocksCoder, &h);
+    const int rc = container_blocks_open(buf, size, kContainerVersionBlocksCoder, info, &h);
     if (rc != RB200_OK) return rc;
-    const ContainerHeader l = container_layout(h);
     info->coder = h.coder;
     info->scale_bits = h.scale_bits;
-    info->n_blocks = h.n_blocks;
-    info->block_size = h.block_size;
-    info->chunk_syms = h.chunk_syms;
-    info->flags = h.flags;
-    info->n_symbols = h.n_symbols;
-    info->n_chunks = h.n_chunks;
-    info->blob_bytes = h.blob_bytes;
-    info->block_freqs = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));
-    info->offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(l));
-    info->blob = buf + container_blob_offset(l);
     return RB200_OK;
 }
 

@@ -64,15 +64,10 @@ struct rb200_ctx {
     CrcWork* d_crc_work = nullptr;
     CrcSlot* d_crc = nullptr;            // kMaxSlices entries
     CrcSlot* h_crc = nullptr;
-    // rb200_container_blocks_decode_async (container_decode.cuh): its fixed workspace and launch shapes
-    BlocksAsyncWork* d_blocks_async = nullptr;
-    BlocksAsyncShape blocks_async = {};
-    // rb200_container_decode_async: its fixed workspace (with the decode table) and its decoders' launches
-    SingleAsyncWork* d_single_async = nullptr;
-    SingleDecodeLaunch single_decoders[kSingleDecoders] = {};
-    // rb200_container_blocks_coder_decode_async: its fixed workspace and its decoders' launches
-    BlocksCoderAsyncWork* d_blocks_coder_async = nullptr;
-    BlockCoderDecodeLaunch blocks_coder_decoders[kBlockCoderDecoders] = {};
+    // the async container decodes (container_decode.cuh): one fixed workspace per version, so that calls of different
+    // versions never share state, and every version's decoder launches
+    ContainerAsyncWork* d_async[3] = {};
+    DecoderLaunch async_decoders[kContainerDecoders] = {};
     // rb200_container_model_encode_async (model_kernels.cuh): the counts, the model and its encode tables
     ModelAsyncWork* d_model_async = nullptr;
 };
@@ -234,12 +229,10 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     if (e == cudaSuccess) e = cudaMemset(ctx->d_crc_work, 0, sizeof(CrcWork));
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_crc, rb200_ctx::kMaxSlices * sizeof(CrcSlot));
     if (e == cudaSuccess) e = cudaMallocHost(&ctx->h_crc, rb200_ctx::kMaxSlices * sizeof(CrcSlot));
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_blocks_async, sizeof(BlocksAsyncWork));
-    if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_async, 0, sizeof(BlocksAsyncWork));
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_single_async, sizeof(SingleAsyncWork));
-    if (e == cudaSuccess) e = cudaMemset(ctx->d_single_async, 0, sizeof(SingleAsyncWork));
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_blocks_coder_async, sizeof(BlocksCoderAsyncWork));
-    if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_coder_async, 0, sizeof(BlocksCoderAsyncWork));
+    for (ContainerAsyncWork*& w : ctx->d_async) {
+        if (e == cudaSuccess) e = cudaMalloc(&w, sizeof(ContainerAsyncWork));
+        if (e == cudaSuccess) e = cudaMemset(w, 0, sizeof(ContainerAsyncWork));
+    }
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_model_async, sizeof(ModelAsyncWork));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_model_async, 0, sizeof(ModelAsyncWork));
     if (e != cudaSuccess) {
@@ -254,9 +247,7 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     configure_block_coder_kernels();
     configure_rans64_kernels();
     configure_crc_kernels();
-    ctx->blocks_async = configure_container_decode(static_cast<uint32_t>(ctx->sms));
-    configure_single_decode(static_cast<uint32_t>(ctx->sms), ctx->single_decoders);
-    configure_blocks_coder_decode(static_cast<uint32_t>(ctx->sms), ctx->blocks_coder_decoders);
+    configure_container_decode(static_cast<uint32_t>(ctx->sms), ctx->async_decoders);
     cudaGetLastError();
     *out = ctx;
     return RB200_OK;
@@ -277,9 +268,8 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->d_crc_work) cudaFree(ctx->d_crc_work);
     if (ctx->d_crc) cudaFree(ctx->d_crc);
     if (ctx->h_crc) cudaFreeHost(ctx->h_crc);
-    if (ctx->d_blocks_async) cudaFree(ctx->d_blocks_async);
-    if (ctx->d_single_async) cudaFree(ctx->d_single_async);
-    if (ctx->d_blocks_coder_async) cudaFree(ctx->d_blocks_coder_async);
+    for (ContainerAsyncWork* w : ctx->d_async)
+        if (w) cudaFree(w);
     if (ctx->d_model_async) cudaFree(ctx->d_model_async);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
@@ -1430,10 +1420,10 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
         RB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         rc = container_parse_header(reinterpret_cast<const uint8_t*>(ctx->h_dir), size, version, &h);
         if (rc != RB200_OK) return rc;
-        const size_t boff = container_blob_offset(container_layout(h));
+        const size_t boff = container_blob_offset(h);
         rc = reserve_dir(ctx, boff / sizeof(uint64_t));
         if (rc != RB200_OK) return rc;
-        const uint64_t covered = container_dir_end(container_layout(h)) - sizeof(ContainerHeader);     // model and directory: what the CRC covers after the header
+        const uint64_t covered = container_dir_end(h) - sizeof(ContainerHeader);     // model and directory: what the CRC covers after the header
         RB_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir, buf, boff, cudaMemcpyDeviceToHost, ctx->stream));
         rc = launch_crc(ctx, buf + sizeof(ContainerHeader), covered, nullptr, 0, ctx->d_crc);
         if (rc == RB200_OK) rc = fetch_crc(ctx, 1);
@@ -1444,15 +1434,15 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
         rc = container_parse_header(buf, size, version, &h);
         if (rc == RB200_OK)
             rc = container_check_prefix(h, buf, container_meta_crc(h, buf + sizeof(ContainerHeader),
-                                                                   reinterpret_cast<const uint64_t*>(buf + container_dir_offset(container_layout(h)))));
+                                                                   reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h))));
     }
     if (rc != RB200_OK) return rc;
     if (n_symbols) *n_symbols = h.n_symbols;
     if (out_cap < h.n_symbols) return RB200_E_SPACE;
     if (h.n_symbols && !out) return RB200_E_ARG;
     if (!container_geometry_decodable(h.chunk_syms, h.blob_bytes)) return RB200_E_ARG;  // what rb200_decode accepts
-    const uint8_t* blob = buf + container_blob_offset(container_layout(h));
-    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(container_layout(h)));
+    const uint8_t* blob = buf + container_blob_offset(h);
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(h));
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
     if (device && blob_crc) {
         rc = launch_crc(ctx, blob, h.blob_bytes, nullptr, 0, ctx->d_crc);
@@ -1583,8 +1573,7 @@ int container_blocks_encode_impl(rb200_ctx* ctx, ContainerHeader h, const uint8_
     const uint32_t n_blocks = h.n_blocks, block_size = h.block_size, chunk_syms = h.chunk_syms;
     const uint64_t n_chunks = h.n_chunks;
     if (!build && !device && !container_block_models_sum_to(block_freqs, n_blocks, 1u << h.scale_bits)) return RB200_E_MODEL;
-    const ContainerHeader l = container_layout(h);
-    const size_t dir_off = container_dir_offset(l), dir_end = container_dir_end(l), boff = container_blob_offset(l);
+    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
     if (out_cap < boff) return RB200_E_SPACE;
     DeviceGuard g(ctx->device);
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
@@ -1661,107 +1650,77 @@ extern "C" int rb200_container_blocks_coder_decode(rb200_ctx* ctx, const uint8_t
 
 namespace {
 
-// The async decodes' checks up to the verdict, for `version` (single: version 1's workspace, w == &single->c; null for
-// version 2): plan, meta CRC, blob CRC, the prefix check, version 1's model check and table build, then the verdict.
-// Lengths and positions the host cannot know come from the plan on the device; the host passes only bounds it knows
-// (size).
-// the meta and blob CRCs of the async decodes, lengths and blob position from the plan in w
-int enqueue_container_crcs(rb200_ctx* ctx, const uint8_t* buf, size_t size, BlocksAsyncWork* w)
-{
-    const uint32_t sms = static_cast<uint32_t>(ctx->sms);
-    const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
-    cudaStream_t s = ctx->stream;
-    crc32_kernel<<<crc32_grid(sms, after_head), kCrcThreads, kCrcSmemBytes, s>>>(buf + sizeof(ContainerHeader), after_head, &w->plan.meta_len,
-                                                                                 nullptr, 0, &w->crc_work, &w->crc[0]);
-    const int rc = check_launch(ctx, "crc32_kernel(meta)");
-    if (rc != RB200_OK) return rc;
-    crc32_kernel<<<crc32_grid(sms, size), kCrcThreads, kCrcSmemBytes, s>>>(buf, size, &w->plan.blob_len, &w->plan.blob_off, 0,
-                                                                           &w->crc_work, &w->crc[1]);
-    return check_launch(ctx, "crc32_kernel(blob)");
-}
-
-int enqueue_container_checks(rb200_ctx* ctx, const uint8_t* buf, size_t size, size_t out_cap, uint64_t* d_n_symbols, uint16_t version,
-                             BlocksAsyncWork* w, SingleAsyncWork* single)
-{
-    cudaStream_t s = ctx->stream;
-    container_plan_kernel<<<1, 32, 0, s>>>(buf, size, version, w, single);
-    int rc = check_launch(ctx, "container_plan_kernel");
-    if (rc == RB200_OK) rc = enqueue_container_crcs(ctx, buf, size, w);
-    if (rc != RB200_OK) return rc;
-    container_prefix_check_kernel<<<ctx->blocks_async.check_grid, kPrefixWarps * 32, 0, s>>>(buf, w);
-    rc = check_launch(ctx, "container_prefix_check_kernel");
-    if (rc != RB200_OK) return rc;
-    if (single) {
-        container_table_kernel<<<1, kTableThreads, 0, s>>>(buf, single);
-        rc = check_launch(ctx, "container_table_kernel");
-        if (rc != RB200_OK) return rc;
-    }
-    container_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status, single);
-    return check_launch(ctx, "container_verdict_kernel");
-}
-
-// the argument rules both async decodes share: device memory, buf and out 16-byte aligned, d_n_symbols 8-byte aligned
+// the argument rules the async decodes share: device memory, buf and out 16-byte aligned, d_n_symbols 8-byte aligned
 bool async_args_ok(const rb200_ctx* ctx, const uint8_t* buf, const uint8_t* out, const uint64_t* d_n_symbols)
 {
     return ctx && buf && out && !(reinterpret_cast<uintptr_t>(d_n_symbols) & 7) && container_mem_ok(RB200_MEM_DEVICE, buf, out);
 }
 
+// The async decode of a container of `version` (container_decode.cuh), in its own workspace: plan, meta CRC, blob CRC,
+// the prefix check, version 1's model check and table build, the verdict, then every decoder of the version on its
+// fixed grid; the verdict's go names the one that runs.  Lengths and positions the host cannot know come from the plan
+// on the device; the host passes only bounds it knows (size).  No copy, no synchronisation, no allocation.
+int container_decode_async(rb200_ctx* ctx, uint16_t version, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                           uint64_t* d_n_symbols)
+{
+    DeviceGuard g(ctx->device);
+    ContainerAsyncWork* w = ctx->d_async[version - 1];
+    const uint32_t sms = static_cast<uint32_t>(ctx->sms);
+    const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
+    cudaStream_t s = ctx->stream;
+    container_plan_kernel<<<1, 32, 0, s>>>(buf, size, version, w);
+    int rc = check_launch(ctx, "container_plan_kernel");
+    if (rc != RB200_OK) return rc;
+    crc32_kernel<<<crc32_grid(sms, after_head), kCrcThreads, kCrcSmemBytes, s>>>(buf + sizeof(ContainerHeader), after_head, &w->plan.meta_len,
+                                                                                 nullptr, 0, &w->crc_work, &w->crc[0]);
+    rc = check_launch(ctx, "crc32_kernel(meta)");
+    if (rc != RB200_OK) return rc;
+    crc32_kernel<<<crc32_grid(sms, size), kCrcThreads, kCrcSmemBytes, s>>>(buf, size, &w->plan.blob_len, &w->plan.blob_off, 0,
+                                                                           &w->crc_work, &w->crc[1]);
+    rc = check_launch(ctx, "crc32_kernel(blob)");
+    if (rc != RB200_OK) return rc;
+    container_prefix_check_kernel<<<sms * kPrefixCtasPerSm, kPrefixWarps * 32, 0, s>>>(buf, w);
+    rc = check_launch(ctx, "container_prefix_check_kernel");
+    if (rc != RB200_OK) return rc;
+    if (version == kContainerVersion) {
+        container_table_kernel<<<1, kTableThreads, 0, s>>>(buf, w);
+        rc = check_launch(ctx, "container_table_kernel");
+        if (rc != RB200_OK) return rc;
+    }
+    container_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status, version);
+    rc = check_launch(ctx, "container_verdict_kernel");
+    for (int i = kDecoderFirst[version - 1]; i < kDecoderFirst[version] && rc == RB200_OK; i++) {
+        const DecoderLaunch& l = ctx->async_decoders[i];
+        l.kernel<<<l.grid, l.threads, l.smem, s>>>(buf, out, w, ctx->d_status);
+        rc = check_launch(ctx, l.name);
+    }
+    return rc;
+}
+
 }  // namespace
 
-// The kernels of container_decode.cuh.  Six launches, no copy, no synchronisation, no allocation.
+// Six launches: the checks and the block decoder.
 extern "C" int rb200_container_blocks_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                                    uint64_t* d_n_symbols)
 {
     if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
-    DeviceGuard g(ctx->device);
-    BlocksAsyncWork* w = ctx->d_blocks_async;
-    int rc = enqueue_container_checks(ctx, buf, size, out_cap, d_n_symbols, kContainerVersionBlocks, w, nullptr);
-    if (rc != RB200_OK) return rc;
-    block_decode_planned_kernel<<<ctx->blocks_async.decode_grid, kPlannedWarps * 32, 0, ctx->stream>>>(buf, out, w, ctx->d_status);
-    return check_launch(ctx, "block_decode_planned_kernel");
+    return container_decode_async(ctx, kContainerVersionBlocks, buf, size, out, out_cap, d_n_symbols);
 }
 
-// The same checks for version 1, then every decoder variant on its fixed grid: the verdict's go names the one that
-// runs.  Seventeen launches, no copy, no synchronisation, no allocation.
+// Seventeen launches: the checks, the table kernel and every decoder variant rb200_decode can pick.
 extern "C" int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                             uint64_t* d_n_symbols)
 {
     if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
-    DeviceGuard g(ctx->device);
-    SingleAsyncWork* w = ctx->d_single_async;
-    int rc = enqueue_container_checks(ctx, buf, size, out_cap, d_n_symbols, kContainerVersion, &w->c, w);
-    for (int i = 0; i < kSingleDecoders && rc == RB200_OK; i++) {
-        const SingleDecodeLaunch& l = ctx->single_decoders[i];
-        l.kernel<<<l.grid, l.threads, l.smem, ctx->stream>>>(buf, out, w, ctx->d_status);
-        rc = check_launch(ctx, l.name);
-    }
-    return rc;
+    return container_decode_async(ctx, kContainerVersion, buf, size, out, out_cap, d_n_symbols);
 }
 
-// Version 3: its own plan, prefix check and verdict kernels around the same CRCs, then every block decoder variant on
-// its fixed grid: the verdict's go names the one that runs.  Nine launches, no copy, no synchronisation, no allocation.
+// Nine launches: the checks and every block decoder variant of RB200_BLOCK_CODER_DISPATCH.
 extern "C" int rb200_container_blocks_coder_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                                          uint64_t* d_n_symbols)
 {
     if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
-    DeviceGuard g(ctx->device);
-    BlocksCoderAsyncWork* w = ctx->d_blocks_coder_async;
-    cudaStream_t s = ctx->stream;
-    blocks_coder_plan_kernel<<<1, 32, 0, s>>>(buf, size, w);
-    int rc = check_launch(ctx, "blocks_coder_plan_kernel");
-    if (rc == RB200_OK) rc = enqueue_container_crcs(ctx, buf, size, &w->c);
-    if (rc != RB200_OK) return rc;
-    blocks_coder_prefix_check_kernel<<<ctx->blocks_async.check_grid, kPrefixWarps * 32, 0, s>>>(buf, w);
-    rc = check_launch(ctx, "blocks_coder_prefix_check_kernel");
-    if (rc != RB200_OK) return rc;
-    blocks_coder_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status);
-    rc = check_launch(ctx, "blocks_coder_verdict_kernel");
-    for (int i = 0; i < kBlockCoderDecoders && rc == RB200_OK; i++) {
-        const BlockCoderDecodeLaunch& l = ctx->blocks_coder_decoders[i];
-        l.kernel<<<l.grid, kPlannedWarps * 32, l.smem, s>>>(buf, out, w, ctx->d_status);
-        rc = check_launch(ctx, l.name);
-    }
-    return rc;
+    return container_decode_async(ctx, kContainerVersionBlocksCoder, buf, size, out, out_cap, d_n_symbols);
 }
 
 namespace {
