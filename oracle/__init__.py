@@ -95,7 +95,7 @@ class _Lib:
     # ---- N-way streams
     def encode(self, coder, data, freqs, cum, nlanes, scale_bits=12):
         data = _u8(data)
-        cap = 2 * data.size + 8 * nlanes + 64
+        cap = 4 * data.size + 8 * nlanes + 64          # rans64 moves up to one u32 per symbol (scale_bits 31: ~31 bits)
         out = np.zeros(cap, np.uint8)
         if coder == CODER_WORD:
             r = getattr(self.lib, f"{self.prefix}_word_encode")(_p(data, _u8p), data.size, _p(freqs, _u32p), _p(cum, _u32p),

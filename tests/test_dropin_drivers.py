@@ -43,25 +43,3 @@ def test_reference_driver_builds_unchanged_and_round_trips(tmp_path, book1, src,
     out = subprocess.run([exe], cwd=tmp_path, capture_output=True, text=True, timeout=120).stdout
     assert "ERROR" not in out and out.count("decode ok!") == len(sizes), out[-400:]
     assert [int(x) for x in re.findall(r"rANS: (\d+) bytes", out)] == sizes
-
-
-def test_headers_compile_for_device(tmp_path):
-    """The same step functions are usable inside sm_90a kernels."""
-    cu = tmp_path / "t.cu"
-    cu.write_text('''
-#include <assert.h>
-#include "rans_byte.h"
-#include "rans64.h"
-#include "rans_word_sse41.h"
-__global__ void k(uint8_t* b, uint32_t* w32, uint16_t* w16, RansWordTables* tab, RansEncSymbol* es, Rans64EncSymbol* e64)
-{
-    RansState r; RansEncInit(&r); uint8_t* p = b + 64; RansEncPutSymbol(&r, &p, es); RansEncFlush(&r, &p);
-    RansDecInit(&r, &p); RansDecAdvance(&r, &p, 0, 1, 12); RansDecRenorm(&r, &p);
-    Rans64State q; Rans64EncInit(&q); uint32_t* pw = w32 + 16; Rans64EncPutSymbol(&q, &pw, e64, 12); Rans64EncFlush(&q, &pw);
-    Rans64DecInit(&q, &pw); Rans64DecAdvance(&q, &pw, 0, 1, 12);
-    RansWordEnc e = RansWordEncInit(); uint16_t* ph = w16 + 32; RansWordEncPut(&e, &ph, 0, 1); RansWordEncFlush(&e, &ph);
-    RansWordDec d; RansWordDecInit(&d, &ph); b[0] = RansWordDecSym(&d, tab); RansWordDecRenorm(&d, &ph);
-}
-''')
-    subprocess.check_call(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-I" + os.path.join(ROOT, "include"), "-c",
-                           "-o", str(tmp_path / "t.o"), str(cu)])
