@@ -261,7 +261,8 @@ int rb200_blocks_coder_decode(rb200_ctx* ctx, int coder, uint32_t scale_bits, co
  * calls reject it.  pack: host only; RB200_E_ARG for a bad coder or scale_bits and as rb200_container_blocks_pack,
  * RB200_E_MODEL for a block that does not sum.  open: as rb200_container_blocks_open, with coder and scale_bits.
  * encode: block_freqs == NULL builds the models on the GPU straight into the model section; otherwise the rules of
- * rb200_container_blocks_encode with the total 1 << scale_bits.  decode: the rules of rb200_container_blocks_decode. */
+ * rb200_container_blocks_encode with the total 1 << scale_bits.  decode: the rules of rb200_container_blocks_decode.
+ * The alias coder's per-block container is version 4 (rb200_container_blocks_alias_*, below). */
 typedef struct rb200_container_blocks_coder_info {
     uint32_t coder, scale_bits;
     uint32_t n_blocks, block_size, chunk_syms, flags;
@@ -294,6 +295,37 @@ int rb200_container_blocks_coder_decode(rb200_ctx* ctx, const uint8_t* buf, size
  * RB200_E_ARG, is RB200_E_STREAM here, out untouched. */
 int rb200_container_blocks_coder_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                               uint64_t* d_n_symbols);
+
+/* ---------------------------------------------------------------- per-block models for the alias coder */
+
+/* The per-block calls of the byte and rans64 coders for RB200_CODER_ALIAS (main_alias.cpp: rans_byte + alias table) at
+ * scale_bits 8..15: the same geometry, memory kinds, HOST slice pipeline and error codes.  Each block's alias table
+ * (make_alias_table, main_alias.cpp:147-237, bit-exact with rb200_alias_tables_build) is built on the GPU from its
+ * row of block_freqs by the encoding or decoding CTA; every chunk is the alias coder's ordinary 32-way stream under its
+ * block's row, as rb200_encode writes it with that model.  RB200_E_ARG (nothing launched) for scale_bits outside 8..15,
+ * a bad geometry, a null pointer, a bad mem_kind or 2^31 chunks or more. */
+int rb200_blocks_alias_encode(rb200_ctx* ctx, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                              const uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap,
+                              uint64_t* offsets, size_t* blob_size, int mem_kind);
+int rb200_blocks_alias_model_encode(rb200_ctx* ctx, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                                    uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap,
+                                    uint64_t* offsets, size_t* blob_size, int mem_kind);
+int rb200_blocks_alias_decode(rb200_ctx* ctx, uint32_t scale_bits, const uint8_t* blob, size_t blob_size, const uint64_t* offsets,
+                              const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                              uint8_t* out, int mem_kind);
+
+/* Their container, version 4: version 3 with coder RB200_CODER_ALIAS (byte 6) at scale_bits 8..15 (byte 7); every other
+ * rule is version 3's.  The _alias_ calls accept only version 4, every other container call rejects it.  pack, open,
+ * encode and decode behave as the _coder_ calls; open fills the version 3 info struct. */
+int rb200_container_blocks_alias_pack(uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                      const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob,
+                                      size_t blob_bytes, uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size);
+int rb200_container_blocks_alias_open(const uint8_t* buf, size_t size, rb200_container_blocks_coder_info* info);
+int rb200_container_blocks_alias_encode(rb200_ctx* ctx, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
+                                        uint32_t block_size, const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags,
+                                        uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind);
+int rb200_container_blocks_alias_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                        uint64_t* n_symbols, int mem_kind);
 
 /* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
  * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's

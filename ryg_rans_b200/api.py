@@ -68,6 +68,18 @@ EXPORTS = [
                                                       C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int]),
     ("rb200_container_blocks_coder_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
     ("rb200_container_blocks_coder_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_blocks_alias_encode", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
+                                            C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t), C.c_int]),
+    ("rb200_blocks_alias_model_encode", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p,
+                                                  C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t), C.c_int]),
+    ("rb200_blocks_alias_decode", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32,
+                                            C.c_uint32, C.c_uint32, C.c_void_p, C.c_int]),
+    ("rb200_container_blocks_alias_pack", C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("rb200_container_blocks_alias_open", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_container_blocks_alias_encode", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p,
+                                                      C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int]),
+    ("rb200_container_blocks_alias_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
     ("rb200_container_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_container_model_encode_async", C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_size_t, C.c_uint32,
                                                      C.c_uint32, C.c_void_p, C.c_size_t]),
@@ -211,12 +223,32 @@ def container_blocks_coder_pack(coder, scale_bits, n_blocks, block_size, chunk_s
     return out[:size.value]
 
 
-def container_blocks_coder_open(buf):
+def container_blocks_alias_pack(scale_bits, n_blocks, block_size, chunk_syms, block_freqs, offsets, blob, flags=0):
+    """rb200_container_blocks_alias_pack: a version 4 container (alias coder, a model per block)"""
+    lib = load()
+    block_freqs = np.ascontiguousarray(block_freqs, dtype=np.uint16)
+    offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+    blob = np.ascontiguousarray(blob, dtype=np.uint8)
+    total = int(lib.dll.rb200_container_blocks_size(n_blocks, offsets.size - 1, blob.size))
+    out = np.zeros(total, np.uint8)
+    size = C.c_size_t(0)
+    lib.check(lib.dll.rb200_container_blocks_alias_pack(scale_bits, n_blocks, block_size, chunk_syms, block_freqs.ctypes.data,
+                                                        offsets.ctypes.data, blob.ctypes.data, blob.size, flags, out.ctypes.data, total,
+                                                        C.byref(size)))
+    return out[:size.value]
+
+
+def container_blocks_alias_open(buf):
+    """rb200_container_blocks_alias_open: as container_blocks_coder_open, for version 4"""
+    return container_blocks_coder_open(buf, _open="rb200_container_blocks_alias_open")
+
+
+def container_blocks_coder_open(buf, _open="rb200_container_blocks_coder_open"):
     """Returns (info dict, block_freqs [n_blocks, 256], offsets, blob) as numpy views into buf."""
     lib = load()
     buf = np.ascontiguousarray(buf, dtype=np.uint8)
     info = ContainerBlocksCoderInfo()
-    lib.check(lib.dll.rb200_container_blocks_coder_open(buf.ctypes.data, buf.size, C.byref(info)))
+    lib.check(getattr(lib.dll, _open)(buf.ctypes.data, buf.size, C.byref(info)))
     base = buf.ctypes.data
     f_off = C.addressof(info.block_freqs.contents) - base
     o_off = C.addressof(info.offsets.contents) - base
@@ -620,6 +652,93 @@ class Context:
                                                               _np_ptr(block_freqs), n_blocks, block_size, chunk_syms, _np_ptr(out),
                                                               MEM_HOST), self.h)
         return out
+
+    # ---- per-block models of the alias coder (scale_bits 8..15) and their container (version 4)
+    def blocks_alias_encode_device(self, scale_bits, in_ptr, n_blocks, block_size, freqs_ptr, chunk_syms, blob_ptr, blob_cap, offsets_ptr):
+        self.lib.check(self.lib.dll.rb200_blocks_alias_encode(self.h, scale_bits, in_ptr, n_blocks, block_size, freqs_ptr, chunk_syms,
+                                                              blob_ptr, blob_cap, offsets_ptr, None, MEM_DEVICE), self.h)
+
+    def blocks_alias_model_encode_device(self, scale_bits, in_ptr, n_blocks, block_size, freqs_ptr, chunk_syms, blob_ptr, blob_cap,
+                                         offsets_ptr):
+        self.lib.check(self.lib.dll.rb200_blocks_alias_model_encode(self.h, scale_bits, in_ptr, n_blocks, block_size, freqs_ptr,
+                                                                    chunk_syms, blob_ptr, blob_cap, offsets_ptr, None, MEM_DEVICE), self.h)
+
+    def blocks_alias_decode_device(self, scale_bits, blob_ptr, blob_size, offsets_ptr, freqs_ptr, n_blocks, block_size, chunk_syms, out_ptr):
+        self.lib.check(self.lib.dll.rb200_blocks_alias_decode(self.h, scale_bits, blob_ptr, blob_size, offsets_ptr, freqs_ptr, n_blocks,
+                                                              block_size, chunk_syms, out_ptr, MEM_DEVICE), self.h)
+
+    def blocks_alias_encode_host(self, scale_bits, data, n_blocks, block_size, block_freqs, chunk_syms, blob_cap=None):
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        block_freqs = np.ascontiguousarray(block_freqs, dtype=np.uint16)
+        cap = self.encode_bound(data.size, chunk_syms) if blob_cap is None else blob_cap
+        blob = np.zeros(max(cap, 16), np.uint8)
+        offsets = np.zeros(n_blocks * (block_size // chunk_syms) + 1, np.uint64)
+        size = C.c_size_t(0)
+        self.lib.check(self.lib.dll.rb200_blocks_alias_encode(self.h, scale_bits, _np_ptr(data), n_blocks, block_size, _np_ptr(block_freqs),
+                                                              chunk_syms, _np_ptr(blob), cap, _np_ptr(offsets), C.byref(size), MEM_HOST),
+                       self.h)
+        return blob[:size.value].copy(), offsets
+
+    def blocks_alias_model_encode_host(self, scale_bits, data, n_blocks, block_size, chunk_syms, blob_cap=None):
+        """models + encode in one call; returns (blob, offsets, block_freqs)"""
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        freqs = np.zeros((n_blocks, 256), np.uint16)
+        cap = self.encode_bound(data.size, chunk_syms) if blob_cap is None else blob_cap
+        blob = np.zeros(max(cap, 16), np.uint8)
+        offsets = np.zeros(n_blocks * (block_size // chunk_syms) + 1, np.uint64)
+        size = C.c_size_t(0)
+        self.lib.check(self.lib.dll.rb200_blocks_alias_model_encode(self.h, scale_bits, _np_ptr(data), n_blocks, block_size, _np_ptr(freqs),
+                                                                    chunk_syms, _np_ptr(blob), cap, _np_ptr(offsets), C.byref(size),
+                                                                    MEM_HOST), self.h)
+        return blob[:size.value].copy(), offsets, freqs
+
+    def blocks_alias_decode_host(self, scale_bits, blob, offsets, block_freqs, n_blocks, block_size, chunk_syms):
+        blob = np.ascontiguousarray(blob, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        block_freqs = np.ascontiguousarray(block_freqs, dtype=np.uint16)
+        out = np.zeros(n_blocks * block_size, np.uint8)
+        self.lib.check(self.lib.dll.rb200_blocks_alias_decode(self.h, scale_bits, _np_ptr(blob), blob.size, _np_ptr(offsets),
+                                                              _np_ptr(block_freqs), n_blocks, block_size, chunk_syms, _np_ptr(out), MEM_HOST),
+                       self.h)
+        return out
+
+    def container_blocks_alias_encode_host(self, scale_bits, data, n_blocks, block_size, chunk_syms, block_freqs=None, flags=0, out_cap=None):
+        """block_freqs None: the models (normalised to 1 << scale_bits) are built on the GPU; else the caller's tables"""
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        freqs = None if block_freqs is None else np.ascontiguousarray(block_freqs, dtype=np.uint16)
+        cap = self.container_blocks_capacity(n_blocks, block_size, chunk_syms) if out_cap is None else out_cap
+        out = np.zeros(max(cap, 16), np.uint8)
+        size = C.c_size_t(0)
+        self.lib.check(self.lib.dll.rb200_container_blocks_alias_encode(self.h, scale_bits, _np_ptr(data), n_blocks, block_size,
+                                                                        None if freqs is None else _np_ptr(freqs), chunk_syms, flags,
+                                                                        _np_ptr(out), cap, C.byref(size), MEM_HOST), self.h)
+        return out[:size.value].copy()
+
+    def container_blocks_alias_encode_device(self, scale_bits, in_ptr, n_blocks, block_size, freqs_ptr, chunk_syms, flags, out_ptr, out_cap):
+        """asynchronous; freqs_ptr None builds the models; errors come from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_blocks_alias_encode(self.h, scale_bits, in_ptr, n_blocks, block_size, freqs_ptr,
+                                                                        chunk_syms, flags, out_ptr, out_cap, None, MEM_DEVICE), self.h)
+
+    def container_blocks_alias_decode_host(self, buf, out_cap=None):
+        """returns the decoded symbols; out_cap defaults to the container's n"""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        n = C.c_uint64(0)
+        if out_cap is None:
+            rc = self.lib.dll.rb200_container_blocks_alias_decode(self.h, _np_ptr(buf), buf.size, None, 0, C.byref(n), MEM_HOST)
+            if rc not in (0, -3):
+                self.lib.check(rc, self.h)
+            out_cap = n.value
+        out = np.zeros(max(out_cap, 1), np.uint8)
+        self.lib.check(self.lib.dll.rb200_container_blocks_alias_decode(self.h, _np_ptr(buf), buf.size, _np_ptr(out), out_cap, C.byref(n),
+                                                                        MEM_HOST), self.h)
+        return out[:n.value]
+
+    def container_blocks_alias_decode_device(self, buf_ptr, size, out_ptr, out_cap):
+        """synchronous; returns the container's n"""
+        n = C.c_uint64(0)
+        self.lib.check(self.lib.dll.rb200_container_blocks_alias_decode(self.h, buf_ptr, size, out_ptr, out_cap, C.byref(n), MEM_DEVICE),
+                       self.h)
+        return n.value
 
     # ---- per-block models, device pointers (asynchronous)
     def blocks_build_models_device(self, in_ptr, n_blocks, block_size, freqs_ptr):

@@ -61,6 +61,14 @@ struct ByteDecoder {
             n1 = x < kByteL;
             n2 = x < (kByteL >> 8);
         }
+        renorm<FULL>(x, cursor, ring, lt, n1, n2);
+    }
+
+    // RansDecRenorm (rans_byte.h:307-318) for the warp on the stream window: 0, 1 or 2 bytes per lane, lane k's bytes
+    // before lane k+1's, most significant first; n1 / n2: this lane takes at least one / two bytes (false when inactive)
+    template <bool FULL>
+    static __device__ __forceinline__ void renorm(uint32_t& x, uint32_t& cursor, uint32_t ring, uint32_t lt, bool n1, bool n2)
+    {
         if (FULL) {
             // RansDecRenorm for the warp as one PTX sequence: two predicates feed the votes, the two ranked byte
             // loads and the state updates (the C++ below costs six more instructions and a branch per step)
@@ -178,33 +186,51 @@ struct AliasDecoder {
         return ByteDecoder<SB>{0, 0}.read_header(at, lane);
     }
 
+    // window step (decode_window_chunk): the lookup of step_p, then ByteDecoder's window renormalisation
+    template <bool FULL>
+    __device__ __forceinline__ void step(uint32_t& x, uint32_t& cursor, uint32_t ring, uint8_t* o, uint32_t lt, bool active) const
+    {
+        bool n1 = false, n2 = false;
+        if (active) {
+            get<true>(x, o);
+            n1 = x < kByteL;
+            n2 = x < (kByteL >> 8);
+        }
+        ByteDecoder<SB>::template renorm<FULL>(x, cursor, ring, lt, n1, n2);
+    }
+
+    // RansDecGetAlias (main_alias.cpp:252-267): the next state and, when STORE, the symbol
+    template <bool STORE>
+    __device__ __forceinline__ void get(uint32_t& x, uint8_t* o) const
+    {
+        const uint32_t sb = SB ? SB : sb_rt;
+        if (LEAN && SB > 8) {
+            constexpr uint32_t LB = SB > 8 ? SB - 8 : 1;
+            // bucket id: byte 1 of x by one PRMT at scale_bits 16, otherwise masked in place and scaled by the IMAD
+            const uint32_t addr = LB == 8 ? mad_u32(__byte_perm(x, 0u, 0x4441u), kAliasDecReplicas * 16, tab_lane)
+                                          : mad_u32(x & (0xffu << LB), (kAliasDecReplicas * 16) >> (LB & 7), tab_lane);
+            const uint4 e = lds_u128_ro(addr);
+            const bool own = mad_u32(x, 1u << (32 - LB), 0u) <= e.x;           // main_alias.cpp:261 on the bucket-local bits
+            const uint32_t fs = own ? e.y : e.z;
+            const uint32_t adj = own ? e.x : e.w;
+            x = mad_u32(fs >> 8, x >> SB, (x - adj) & ((1u << SB) - 1));       // :265
+            if (STORE) *o = static_cast<uint8_t>(fs);                          // :266
+        } else {
+            const uint32_t xm = x & ((1u << sb) - 1);                              // main_alias.cpp:258
+            const uint32_t bucket = xm >> (sb - 8);                                // :259
+            const uint4 e = lds_u128_ro(mad_u32(bucket, kAliasDecReplicas * 16, tab_lane));
+            const bool own = xm < e.x;                                             // :261 (bucket2 = 2 * bucket + 1)
+            const uint32_t fs = own ? e.z : e.y;                                   // slot_freqs << 8 | sym_id
+            const uint32_t adj = __byte_perm(e.w, 0u, own ? 0x4432u : 0x4410u);    // the taken half of the packed adjusts
+            x = mad_u32(fs >> 8, x >> sb, (xm - adj) & 0xffffu);                   // :265
+            if (STORE) *o = static_cast<uint8_t>(fs);                              // :266
+        }
+    }
+
     template <class P>
     __device__ __forceinline__ void step_p(uint32_t& x, uint32_t& cur, uint8_t* o, uint32_t lt, uint32_t lane, int j, bool active) const
     {
-        const uint32_t sb = SB ? SB : sb_rt;
-        if (active) {
-            if (LEAN && SB > 8) {
-                constexpr uint32_t LB = SB > 8 ? SB - 8 : 1;
-                // bucket id: byte 1 of x by one PRMT at scale_bits 16, otherwise masked in place and scaled by the IMAD
-                const uint32_t addr = LB == 8 ? mad_u32(__byte_perm(x, 0u, 0x4441u), kAliasDecReplicas * 16, tab_lane)
-                                              : mad_u32(x & (0xffu << LB), (kAliasDecReplicas * 16) >> (LB & 7), tab_lane);
-                const uint4 e = lds_u128_ro(addr);
-                const bool own = mad_u32(x, 1u << (32 - LB), 0u) <= e.x;           // main_alias.cpp:261 on the bucket-local bits
-                const uint32_t fs = own ? e.y : e.z;
-                const uint32_t adj = own ? e.x : e.w;
-                x = mad_u32(fs >> 8, x >> SB, (x - adj) & ((1u << SB) - 1));       // :265
-                if (!(P::kAblate & kAblNoSymbolStore)) *o = static_cast<uint8_t>(fs);     // :266
-            } else {
-                const uint32_t xm = x & ((1u << sb) - 1);                              // main_alias.cpp:258
-                const uint32_t bucket = xm >> (sb - 8);                                // :259
-                const uint4 e = lds_u128_ro(mad_u32(bucket, kAliasDecReplicas * 16, tab_lane));
-                const bool own = xm < e.x;                                             // :261 (bucket2 = 2 * bucket + 1)
-                const uint32_t fs = own ? e.z : e.y;                                   // slot_freqs << 8 | sym_id
-                const uint32_t adj = __byte_perm(e.w, 0u, own ? 0x4432u : 0x4410u);    // the taken half of the packed adjusts
-                x = mad_u32(fs >> 8, x >> sb, (xm - adj) & 0xffffu);                   // :265
-                if (!(P::kAblate & kAblNoSymbolStore)) *o = static_cast<uint8_t>(fs);         // :266
-            }
-        }
+        if (active) get<!(P::kAblate & kAblNoSymbolStore)>(x, o);
         // RansDecRenorm (rans_byte.h:307-318) for the warp: 0, 1 or 2 bytes per lane, lane k's bytes before lane k+1's,
         // most significant first.  Two predicates feed the votes, the ranked byte loads and the merges.
         const uint32_t xr = active ? x : kByteL;

@@ -1,4 +1,5 @@
-// block_coder_kernels.cuh -- per-block models for the byte (main.cpp) and rans64 (main64.cpp) coders at scale_bits 8..15:
+// block_coder_kernels.cuh -- per-block models for the byte (main.cpp), rans64 (main64.cpp) and alias (main_alias.cpp)
+// coders at scale_bits 8..15:
 // the version 2 geometry (one CTA per block, one warp per chunk, at most 32 chunks per block) with each block's model
 // normalised to 1 << scale_bits instead of 4096.
 //
@@ -12,6 +13,9 @@
 //                          the block's decode table in shared memory (cum2sym[1 << sb], then byte_dec_symbol x 256 or
 //                          rans64's 16x replicated {start, freq}), then decode_window_chunk per warp with ByteDecoder<SB> /
 //                          Rans64Decoder
+//   CODER = RB200_CODER_ALIAS  the block's alias table built by the CTA (block_alias_tables, over the coding table's place),
+//                          then AliasEncoder<true, SB> with the remap (block_alias_remap, after the warps' stages) or
+//                          AliasDecoder<SB, lean> on kAliasDecReplicas copies of the 256 bucket entries
 //
 // A block whose frequencies do not sum to 1 << sb: the encoder codes it with an empty model (every symbol flagged,
 // RB200_E_SYMBOL), the decoder flags kStatStream and decodes nothing of it, as K5 does for the word coder.
@@ -26,8 +30,141 @@ namespace rb200 {
 // the largest scale_bits of a per-block model: its frequencies are u16, and 1 << 15 holds a one-symbol block
 constexpr uint32_t kBlockCoderMaxScaleBits = 15;
 
-// dynamic shared memory of the per-block byte / rans64 encoder: the 32 KiB table, then 1 KiB per warp (as K5's)
+// ---------------------------------------------------------------------------
+// make_alias_table (main_alias.cpp:147-237) of one block, built by the CTA: bit-exact with alias_tables_core and
+// rb200_alias_tables_build (tables.h, model_host.cpp), which stay the host builders.
+// ---------------------------------------------------------------------------
+// The outputs of alias_tables_core, and the per-symbol records of the pairing that phase 2 turns into them.  12.5 KiB:
+// the per-block alias kernels place it over their (not yet built) 32 KiB coding table.
+struct AliasBuildSmem {
+    uint32_t divider[256];
+    uint32_t slot_adjust[512];
+    uint32_t slot_freqs[512];
+    uint32_t rest[256];         // phase 1: what each symbol still has to hand out (main_alias.cpp's rest)
+    uint32_t own[256];          // the part of bucket s that s keeps (divider[s] before :219)
+    uint32_t lend_base[256];    // taker s: what its donor had lent to earlier takers (= earlier buckets)
+    uint32_t own_base[256];     // what s had lent to buckets below s: given[s] when bucket s is handed out (:217)
+    uint32_t lent[256];         // everything s lent
+    uint32_t dst[512];          // remap: where bucket s's own part [2s] and its partner's part [2s + 1] start, minus k
+    uint8_t sym_id[512];
+};
+
+// Phase 1 (main_alias.cpp:159-204) on warp 0, phase 2 (:207-232) on the CTA, from the block's s_cum[257] (sum M, a
+// multiple of 256).  Every thread of the CTA calls it; it ends with a CTA barrier and returns what alias_tables_core
+// returns: false when some symbol is not handed exactly its frequency (never for a table that sums to M).
+//
+// Phase 1 is a chain of at most 256 (taker, donor) steps.  Each step needs "the first index >= p whose rest is below
+// (taker) / at least (donor) the bucket".  Lane l keeps bit k of `under` for symbol 32k + l, so one ballot over bit k
+// is word k of the 256-bit predicate rest < bucket, and a query is one ballot per word from p's word on (usually one).
+// Only the donor's rest changes in a step, so only its bit is updated.
+// Phase 2 needs given[] in bucket order.  A donor's run of steps is contiguous and its takers come in increasing bucket
+// order (the first may be the previous donor, which lies below the resume point; the rest come from the resume scan),
+// so what a donor lent before taker t is a running sum over its run (lend_base), and what it lent below its own bucket
+// is that sum at the first taker above it (own_base).  Then every bucket's entries are independent.
+__device__ __forceinline__ bool block_alias_tables(const uint32_t* s_cum, uint32_t M, AliasBuildSmem& a)
+{
+    const uint32_t tid = threadIdx.x, lane = tid & 31, bucket = M >> 8;
+    for (uint32_t s = tid; s < 256; s += blockDim.x) {
+        a.rest[s] = s_cum[s + 1] - s_cum[s];
+        a.own[s] = bucket;
+        a.lend_base[s] = 0;
+        a.own_base[s] = 0;
+        a.lent[s] = 0;
+        a.sym_id[2 * s] = a.sym_id[2 * s + 1] = static_cast<uint8_t>(s);
+    }
+    __syncthreads();
+    if (tid < 32) {
+        uint32_t under = 0;
+#pragma unroll
+        for (uint32_t k = 0; k < 8; k++) under |= static_cast<uint32_t>(a.rest[32 * k + lane] < bucket) << k;
+        // the first index >= p (p <= 257) with rest < bucket (want_under) or rest >= bucket, 256 if none
+        auto next = [&](uint32_t p, bool want_under) {
+            const uint32_t bits = want_under ? under : ~under;
+            for (uint32_t k = p >> 5; k < 8; k++) {
+                uint32_t w = __ballot_sync(0xffffffffu, (bits >> k) & 1u);
+                if (k == (p >> 5)) w &= ~0u << (p & 31);
+                if (w) return 32 * k + __ffs(w) - 1;
+            }
+            return 256u;
+        };
+        uint32_t donor = next(0, false), taker = next(0, true);   // :172-175
+        uint32_t resume = taker + 1;                              // :179
+        uint32_t rd = donor < 256 ? a.rest[donor] : 0;            // the donor's rest
+        uint32_t before = 0;                                      // what the donor lent in its earlier steps
+        bool crossed = false;                                     // the donor has had a taker above its own bucket
+        while (donor < 256 && taker < 256) {                      // :183
+            const uint32_t rt = a.rest[taker], give = bucket - rt;
+            if (lane == 0) {
+                a.sym_id[2 * taker] = static_cast<uint8_t>(donor);     // :185
+                a.own[taker] = rt;                                     // :186
+                a.lend_base[taker] = before;
+                if (!crossed && taker > donor) a.own_base[donor] = before;
+            }
+            crossed |= taker > donor;
+            before += give;
+            rd -= give;                                           // :189
+            a.rest[donor] = rd;                                   // every lane stores it, so every lane reads it back
+            const bool low = rd < bucket;
+            if (low && lane == (donor & 31)) under |= 1u << (donor >> 5);
+            if (!low || resume <= donor) {                        // :192
+                taker = next(resume, true);
+                resume = taker + 1;
+            } else {
+                taker = donor;                                    // :199 (donor became a taker behind us)
+            }
+            if (low) {                                            // :202-203: the donor's run ends
+                if (lane == 0) {
+                    if (!crossed) a.own_base[donor] = before;
+                    a.lent[donor] = before;
+                }
+                before = 0;
+                crossed = false;
+                donor = next(donor + 1, false);
+                rd = donor < 256 ? a.rest[donor] : 0;             // never a donor before: its rest is its frequency
+            }
+        }
+        if (donor < 256 && lane == 0) {
+            if (!crossed) a.own_base[donor] = before;
+            a.lent[donor] = before;
+        }
+    }
+    __syncthreads();
+    bool bad = false;
+    for (uint32_t s = tid; s < 256; s += blockDim.x) {            // :207-232, one bucket per thread
+        const uint32_t other = a.sym_id[2 * s], own = a.own[s], lo = s * bucket, f = s_cum[s + 1] - s_cum[s];
+        const uint32_t own_base = a.own_base[s];
+        const uint32_t other_base = other == s ? own_base : a.lend_base[s] + (other < s ? a.own[other] : 0);
+        a.divider[s] = lo + own;                                  // :219
+        a.slot_freqs[2 * s + 1] = f;                              // :221
+        a.slot_freqs[2 * s] = s_cum[other + 1] - s_cum[other];    // :222
+        a.slot_adjust[2 * s + 1] = lo - own_base;                 // :223
+        a.slot_adjust[2 * s] = lo - (other_base - own);           // :224
+        a.dst[2 * s] = s_cum[s] + own_base - lo;
+        a.dst[2 * s + 1] = s_cum[other] + other_base - lo - own;
+        bad |= own + a.lent[s] != f;                              // :235-236 (given[s] = own + what s lent)
+    }
+    return __syncthreads_or(bad) == 0;
+}
+
+// alias_remap (main_alias.cpp:225-228) as u16 from a pairing that block_alias_tables accepted, one slot per thread:
+// slot j of bucket s = j / bucket goes to s's own part or to its partner's, after what earlier buckets gave that
+// symbol.  The caller puts a CTA barrier between this and the first read of remap.
+__device__ __forceinline__ void block_alias_remap(const AliasBuildSmem& a, uint32_t M, uint16_t* remap)
+{
+    const uint32_t lb = __ffs(M >> 8) - 1;                        // log2(bucket)
+    for (uint32_t j = threadIdx.x; j < M; j += blockDim.x) {
+        const uint32_t s = j >> lb;
+        remap[a.dst[2 * s + (j - (s << lb) >= a.own[s])] + j] = static_cast<uint16_t>(j);
+    }
+}
+
+// dynamic shared memory of the per-block encoder: the 32 KiB table, then 1 KiB per warp (as K5's); the alias coder's
+// remap (u16, 1 << sb entries) after them
 inline uint32_t block_coder_encode_smem(uint32_t threads) { return block_encode_smem(threads); }
+inline uint32_t block_coder_encode_smem(uint32_t coder, uint32_t sb, uint32_t threads)
+{
+    return block_encode_smem(threads) + (coder == RB200_CODER_ALIAS ? (2u << sb) : 0u);
+}
 
 // dynamic shared memory of the per-block decoder: 1 KiB of stream window per warp, cum2sym, then the symbol entries
 __host__ __device__ constexpr uint32_t block_coder_sym_bytes(uint32_t coder)
@@ -36,6 +173,7 @@ __host__ __device__ constexpr uint32_t block_coder_sym_bytes(uint32_t coder)
 }
 inline uint32_t block_coder_decode_smem(uint32_t coder, uint32_t sb, uint32_t threads)
 {
+    if (coder == RB200_CODER_ALIAS) return (threads / 32) * kRingBytes + 256 * kAliasDecReplicas * 16;   // the bucket table
     return (threads / 32) * kRingBytes + (1u << sb) + block_coder_sym_bytes(coder);
 }
 
@@ -60,12 +198,25 @@ block_coder_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, u
     } else {
         ok = block_prefix(static_cast<const uint16_t*>(freqs), s_cum, &s_flag[0], M);
     }
+    const uint32_t warps = blockDim.x >> 5;
+    const uint32_t remap = smem_addr(s_benc) + kEncTableBytes + warps * kEncWarpSmem;
+    if (CODER == RB200_CODER_ALIAS && ok) {
+        // the pairing and the remap, in the table's place; a table that sums to M always pairs
+        AliasBuildSmem& a = *reinterpret_cast<AliasBuildSmem*>(s_benc);
+        ok = block_alias_tables(s_cum, M, a);
+        if (ok) block_alias_remap(a, M, reinterpret_cast<uint16_t*>(s_benc + kEncTableBytes + warps * kEncWarpSmem));
+        __syncthreads();
+    }
     // the encoder table as K8 / K9 stage theirs: one 16-byte entry per symbol, kEncReplicas copies
     uint4* s_tab = reinterpret_cast<uint4*>(s_benc);
     for (uint32_t s = tid; s < 256; s += blockDim.x) {
         const uint32_t f = ok ? s_cum[s + 1] - s_cum[s] : 0, cum = ok ? s_cum[s] : 0;
         uint4 x;
-        if (CODER == RB200_CODER_BYTE) {
+        if (CODER == RB200_CODER_ALIAS) {
+            // a symbol outside the model: freq 1 keeps the step well defined, the flag reports it (as K4 stages it)
+            const AliasEncEntry e = alias_enc_entry(f, cum);          // {magic, freq, cum, shift}
+            x = f ? make_uint4(e.magic, e.freq, e.cum, e.shift) : make_uint4(0, 1, 0, kEncBadSymbol);
+        } else if (CODER == RB200_CODER_BYTE) {
             const AliasEncEntry e = byte_enc_entry(f, cum, sb);       // {x_max, rcp_freq, bias, cmpl_freq | rcp_shift << 16}
             x = make_uint4(e.magic, e.freq, e.cum, e.shift);
         } else {
@@ -83,7 +234,9 @@ block_coder_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, u
     const uint32_t chunk = blockIdx.x * per_block + warp;
     const uint8_t* src = blk + static_cast<uint64_t>(warp) * chunk_syms;
     const uint32_t tab = smem_addr(s_benc), wsm = tab + kEncTableBytes + warp * kEncWarpSmem;
-    if (CODER == RB200_CODER_BYTE)
+    if (CODER == RB200_CODER_ALIAS)
+        encode_chunk_split(src, chunk_syms, chunk, AliasEncoder<true, SB>{tab, remap, sb}, wsm, scratch, slot_bytes, sizes, status);
+    else if (CODER == RB200_CODER_BYTE)
         encode_chunk_split(src, chunk_syms, chunk, AliasEncoder<false, SB>{tab, 0, sb}, wsm, scratch, slot_bytes, sizes, status);
     else
         encode_chunk_split(src, chunk_syms, chunk, Rans64Encoder{tab, sb}, wsm, scratch, slot_bytes, sizes, status);
@@ -141,7 +294,35 @@ block_coder_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, 
         return;
     }
     uint8_t* s_tab = s_bdec + warps * kRingBytes;
-    block_coder_decode_table<CODER>(s_cum, s_tab, M);
+    if (CODER == RB200_CODER_ALIAS) {
+        // the pairing in the table's place, each thread's bucket entries (at most 2: blockDim >= 128) in registers,
+        // then the kAliasDecReplicas copies over it
+        const AliasBuildSmem& a = *reinterpret_cast<AliasBuildSmem*>(s_tab);
+        if (!block_alias_tables(s_cum, M, *reinterpret_cast<AliasBuildSmem*>(s_tab))) {
+            if (tid == 0) atomicOr(status, kStatStream);
+            return;
+        }
+        uint4 e[2];
+#pragma unroll
+        for (uint32_t i = 0; i < 2; i++) {
+            const uint32_t b = tid + i * blockDim.x;
+            if (b >= 256) continue;
+            const AliasDecEntry d = alias_dec_entry(b, a.divider, a.slot_adjust, a.slot_freqs, a.sym_id);
+            if (kAliasLean && SB > 8) e[i] = alias_lean_entry<(SB > 8 ? SB : 9)>(d, b);
+            else e[i] = make_uint4(d.divider, d.alt0, d.alt1, d.adjust);
+        }
+        __syncthreads();
+        uint4* s_dec = reinterpret_cast<uint4*>(s_tab);
+#pragma unroll
+        for (uint32_t i = 0; i < 2; i++) {
+            const uint32_t b = tid + i * blockDim.x;
+            if (b >= 256) continue;
+#pragma unroll
+            for (uint32_t r = 0; r < kAliasDecReplicas; r++) s_dec[b * kAliasDecReplicas + r] = e[i];
+        }
+    } else {
+        block_coder_decode_table<CODER>(s_cum, s_tab, M);
+    }
     __syncthreads();
 
     const uint32_t per_block = block_size / chunk_syms;
@@ -149,7 +330,10 @@ block_coder_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, 
     const uint32_t chunk = blockIdx.x * per_block + warp;
     uint8_t* dst = out + static_cast<uint64_t>(blockIdx.x) * block_size + static_cast<uint64_t>(warp) * chunk_syms;
     const uint32_t ring = smem_addr(s_bdec) + warp * kRingBytes, tab = smem_addr_pinned(s_tab);
-    if (CODER == RB200_CODER_BYTE)
+    if (CODER == RB200_CODER_ALIAS)
+        decode_window_chunk(AliasDecoder<SB, kAliasLean>{tab + (lane & (kAliasDecReplicas - 1)) * 16, sb}, blob, blob_size, offsets, chunk,
+                            ring, dst, chunk_syms, status);
+    else if (CODER == RB200_CODER_BYTE)
         decode_window_chunk(ByteDecoder<SB>{tab, sb}, blob, blob_size, offsets, chunk, ring, dst, chunk_syms, status);
     else
         decode_window_chunk(Rans64Decoder{tab, tab + M + (lane & (kRans64DecReplicas - 1)) * 8, sb}, blob, blob_size, offsets, chunk, ring,
@@ -168,13 +352,32 @@ block_coder_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, 
         constexpr uint32_t CODER = RB200_CODER_BYTE, SB = 0; CALL;                       \
     }
 
+// The alias coder's instances (rb200_blocks_alias_*), the same scale_bits specialised: 14 (main.cpp's) and 12, generic
+// otherwise.  A dispatch of its own, so that RB200_BLOCK_CODER_DISPATCH stays the version 3 decoders' list.
+#define RB200_BLOCK_ALIAS_DISPATCH(sb, CALL)                                             \
+    if (sb == 14) {                                                                      \
+        constexpr uint32_t CODER = RB200_CODER_ALIAS, SB = 14; CALL;                     \
+    } else if (sb == 12) {                                                               \
+        constexpr uint32_t CODER = RB200_CODER_ALIAS, SB = 12; CALL;                     \
+    } else {                                                                             \
+        constexpr uint32_t CODER = RB200_CODER_ALIAS, SB = 0; CALL;                      \
+    }
+// every per-block coder instance
+#define RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, CALL)                                  \
+    if (coder == RB200_CODER_ALIAS) {                                                    \
+        RB200_BLOCK_ALIAS_DISPATCH(sb, CALL)                                             \
+    } else {                                                                             \
+        RB200_BLOCK_CODER_DISPATCH(coder, sb, CALL)                                      \
+    }
+
 template <uint32_t CODER, uint32_t SB>
 inline void configure_block_coder()
 {
     for (const void* k : {reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, true>),
                           reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, false>)}) {
         cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, block_coder_encode_smem(kMaxBlockWarps * 32));
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             block_coder_encode_smem(CODER, kBlockCoderMaxScaleBits, kMaxBlockWarps * 32));
     }
     cudaFuncSetAttribute(block_coder_decode_kernel<CODER, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(block_coder_decode_kernel<CODER, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -186,14 +389,17 @@ inline void configure_block_coder_kernels()
     configure_block_coder<RB200_CODER_BYTE, 12>();
     configure_block_coder<RB200_CODER_BYTE, 0>();
     configure_block_coder<RB200_CODER_RANS64, 0>();
+    configure_block_coder<RB200_CODER_ALIAS, 14>();
+    configure_block_coder<RB200_CODER_ALIAS, 12>();
+    configure_block_coder<RB200_CODER_ALIAS, 0>();
 }
 
-// one CTA per block of block_threads() threads; smem = block_coder_encode_smem(threads)
+// one CTA per block of block_threads() threads; smem = block_coder_encode_smem(coder, sb, threads)
 inline void launch_block_coder_encode(cudaStream_t stream, uint32_t coder, uint32_t sb, bool build, uint32_t n_blocks, uint32_t threads,
                                       uint32_t smem, const uint8_t* d_in, uint32_t block_size, uint16_t* d_freqs, uint32_t chunk_syms,
                                       uint8_t* scratch, uint32_t slot_bytes, uint32_t* sizes, uint32_t* status)
 {
-    RB200_BLOCK_CODER_DISPATCH(coder, sb, ((build ? block_coder_encode_kernel<CODER, SB, true> : block_coder_encode_kernel<CODER, SB, false>)
+    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, ((build ? block_coder_encode_kernel<CODER, SB, true> : block_coder_encode_kernel<CODER, SB, false>)
                                            <<<n_blocks, threads, smem, stream>>>(d_in, block_size, d_freqs, sb, chunk_syms, scratch,
                                                                                  slot_bytes, sizes, status)))
 }
@@ -204,7 +410,7 @@ inline void launch_block_coder_decode(cudaStream_t stream, uint32_t coder, uint3
 {
     const uint32_t threads = block_threads(block_size, chunk_syms);
     const uint32_t smem = block_coder_decode_smem(coder, sb, threads);
-    RB200_BLOCK_CODER_DISPATCH(coder, sb, (block_coder_decode_kernel<CODER, SB><<<n_blocks, threads, smem, stream>>>(
+    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, (block_coder_decode_kernel<CODER, SB><<<n_blocks, threads, smem, stream>>>(
                                               blob, blob_size, offsets, d_freqs, sb, block_size, chunk_syms, out, status)))
 }
 

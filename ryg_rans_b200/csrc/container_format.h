@@ -17,6 +17,7 @@ constexpr uint32_t kContainerMagic = 0x43324252u;   // "RB2C"
 constexpr uint16_t kContainerVersion = 1;           // one model: 256 x u32
 constexpr uint16_t kContainerVersionBlocks = 2;     // one model per block: n_blocks x 256 x u16, word coder
 constexpr uint16_t kContainerVersionBlocksCoder = 3;  // version 2's layout with the byte or rans64 coder at scale_bits 8..15
+constexpr uint16_t kContainerVersionBlocksAlias = 4;  // version 2's layout with the alias coder at scale_bits 8..15
 
 struct ContainerHeader {        // 64 bytes
     uint32_t magic;
@@ -31,19 +32,19 @@ struct ContainerHeader {        // 64 bytes
     uint32_t flags;
     uint32_t meta_crc;          // header (crc fields zero) + model + offsets
     uint32_t blob_crc;          // valid when flags & RB200_CONTAINER_CRC_BLOB
-    uint32_t block_size;        // versions 2, 3: symbols per block (version 1: zero, not checked)
-    uint32_t n_blocks;          // versions 2, 3: blocks, >= 1 (version 1: zero, not checked)
-    uint32_t reserved;          // versions 2, 3: zero
+    uint32_t block_size;        // versions 2-4: symbols per block (version 1: zero, not checked)
+    uint32_t n_blocks;          // versions 2-4: blocks, >= 1 (version 1: zero, not checked)
+    uint32_t reserved;          // versions 2-4: zero
 };
 static_assert(sizeof(ContainerHeader) == 64, "container header must stay 64 bytes");
 
 constexpr size_t kContainerDirOffset = sizeof(ContainerHeader) + 256 * sizeof(uint32_t);   // version 1: 1088, 16-aligned
 constexpr size_t kBlockModelBytes = 256 * sizeof(uint16_t);                                 // one block's frequencies
 
-// versions 2 and 3: a model per block, n_blocks x 256 x u16 (version 1: one model, 256 x u32)
+// versions 2, 3 and 4: a model per block, n_blocks x 256 x u16 (version 1: one model, 256 x u32)
 RB200_HD inline bool container_per_block(const ContainerHeader& h)
 {
-    return h.version == kContainerVersionBlocks || h.version == kContainerVersionBlocksCoder;
+    return h.version >= kContainerVersionBlocks && h.version <= kContainerVersionBlocksAlias;
 }
 
 // The layout, as functions of the (parsed) header: model section, directory, pad to 16, blob.  Version 1 keeps 1024
@@ -57,10 +58,14 @@ RB200_HD inline uint64_t container_dir_offset(const ContainerHeader& h) { return
 RB200_HD inline uint64_t container_dir_end(const ContainerHeader& h) { return container_dir_offset(h) + (h.n_chunks + 1) * sizeof(uint64_t); }
 RB200_HD inline uint64_t container_blob_offset(const ContainerHeader& h) { return (container_dir_end(h) + 15) & ~15ull; }
 
-// version 3's coder and scale_bits: byte or rans64 at 8..15
-RB200_HD inline bool container_blocks_coder_ok(uint32_t coder, uint32_t scale_bits)
+// The coder and scale_bits of each per-block version, for its headers and for the arguments of its calls: the word
+// coder at 12 (version 2), byte or rans64 at 8..15 (version 3), alias at 8..15 (version 4)
+RB200_HD inline bool container_blocks_coder_ok(uint16_t version, uint32_t coder, uint32_t scale_bits)
 {
-    return (coder == RB200_CODER_BYTE || coder == RB200_CODER_RANS64) && scale_bits >= 8 && scale_bits <= 15;
+    if (version == kContainerVersionBlocks) return coder == RB200_CODER_WORD && scale_bits == 12;
+    const bool coder_ok = version == kContainerVersionBlocksCoder ? coder == RB200_CODER_BYTE || coder == RB200_CODER_RANS64
+                                                                  : version == kContainerVersionBlocksAlias && coder == RB200_CODER_ALIAS;
+    return coder_ok && scale_bits >= 8 && scale_bits <= 15;
 }
 
 // a header with only what the layout depends on: for sizes computed before there is a header
@@ -83,16 +88,14 @@ RB200_HD inline bool container_blocks_geometry_ok(uint32_t n_blocks, uint32_t bl
 
 // Every rule of a header (already read from the first 64 of `size` bytes) for the one `version` the caller accepts:
 // the fields agree with each other and with the geometry the decoders take, and every section fits `size`.  The
-// per-block versions share every rule but the coder and scale_bits: the word coder at 12 (version 2), byte or rans64
-// at 8..15 (version 3).
+// per-block versions share every rule but the coder and scale_bits (container_blocks_coder_ok).
 RB200_HD inline bool container_header_ok(const ContainerHeader& h, uint64_t size, uint16_t version)
 {
     if (h.magic != kContainerMagic || h.version != version || h.lanes != RB200_LANES || !h.chunk_syms) return false;
     if (container_per_block(h)) {
-        const bool coder_ok = version == kContainerVersionBlocks ? h.coder == RB200_CODER_WORD && h.scale_bits == 12
-                                                                 : container_blocks_coder_ok(h.coder, h.scale_bits);
-        // what rb200_blocks_decode / rb200_blocks_coder_decode accept; n_blocks * block_size cannot overflow 64 bits
-        if (!coder_ok || !container_blocks_geometry_ok(h.n_blocks, h.block_size, h.chunk_syms)) return false;
+        // what rb200_blocks_decode / rb200_blocks_coder_decode / rb200_blocks_alias_decode accept; n_blocks * block_size
+        // cannot overflow 64 bits
+        if (!container_blocks_coder_ok(version, h.coder, h.scale_bits) || !container_blocks_geometry_ok(h.n_blocks, h.block_size, h.chunk_syms)) return false;
         if (h.n_symbols != static_cast<uint64_t>(h.n_blocks) * h.block_size || h.n_chunks != h.n_symbols / h.chunk_syms ||
             h.n_chunks >= (1ull << 31) || (h.blob_bytes & 15) || h.reserved || (h.flags & ~RB200_CONTAINER_CRC_BLOB))
             return false;
@@ -211,8 +214,9 @@ ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_
                                  uint64_t blob_bytes, uint32_t flags);
 // the header rb200_container_blocks_pack writes (crc fields zero)
 ContainerHeader container_blocks_header(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint64_t blob_bytes, uint32_t flags);
-// the header rb200_container_blocks_coder_pack writes (crc fields zero)
-ContainerHeader container_blocks_coder_header(int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+// the header rb200_container_blocks_coder_pack (version 3) or rb200_container_blocks_alias_pack (version 4) writes (crc
+// fields zero)
+ContainerHeader container_blocks_coder_header(uint16_t version, int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
                                               uint64_t blob_bytes, uint32_t flags);
 // every block's 256 frequencies sum to total
 bool container_block_models_sum_to(const uint16_t* block_freqs, uint32_t n_blocks, uint32_t total);
@@ -228,8 +232,8 @@ uint32_t container_meta_crc(const ContainerHeader& h, const void* model, const u
 // The parser, in the order rb200_container_open applies it.  Each step returns RB200_OK or RB200_E_STREAM; the CRC
 // values are the caller's, computed wherever the bytes live.
 //  1. the 64-byte header against the buffer size (`size` bytes in all; `hdr` holds at least 64 of them); `version`
-//     is the one the caller accepts (kContainerVersion, kContainerVersionBlocks or kContainerVersionBlocksCoder), any
-//     other is rejected
+//     is the one the caller accepts (kContainerVersion, kContainerVersionBlocks, kContainerVersionBlocksCoder or
+//     kContainerVersionBlocksAlias), any other is rejected
 int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, ContainerHeader* h);
 //  2. header + model + directory (`prefix`: container_blob_offset(h) bytes), given their CRC
 int container_check_prefix(const ContainerHeader& h, const uint8_t* prefix, uint32_t meta_crc);

@@ -7,6 +7,7 @@
 //   version 1 (one model):       [ 64-byte header ][ freqs: 256 x u32 ][ offsets: (n_chunks + 1) x u64 ][ pad to 16 ][ blob ]
 //   version 2 (a model per block): [ 64-byte header ][ block_freqs: n_blocks x 256 x u16 ][ offsets ][ pad to 16 ][ blob ]
 //   version 3 (a model per block, byte or rans64 coder): version 2's layout
+//   version 4 (a model per block, alias coder): version 2's layout
 //
 // All integers little-endian.  CRC-32 (zlib's: IEEE, reflected) over header (with the crc fields zeroed) + model +
 // offsets always (meta_crc); over the blob when RB200_CONTAINER_CRC_BLOB is set.  The header layout is the same in
@@ -21,8 +22,9 @@
 // directory rules of version 1 hold (offsets[0] < 16, monotone, offsets[n_chunks] == blob_bytes), and the blob CRC
 // matches when present.  Version 3 is version 2 with the header's own coder (RB200_CODER_BYTE or RB200_CODER_RANS64) and
 // scale_bits (8..15); every other rule is version 2's, and in both every block's frequencies sum to 1 << scale_bits.
-// Each call accepts exactly one version: rb200_container_* version 1, rb200_container_blocks_* version 2,
-// rb200_container_blocks_coder_* version 3.
+// Version 4 is version 3 with RB200_CODER_ALIAS (the per-block main_alias.cpp coder), also at 8..15.  Each call accepts
+// exactly one version: rb200_container_* version 1, rb200_container_blocks_* version 2, rb200_container_blocks_coder_*
+// version 3, rb200_container_blocks_alias_* version 4.
 //
 // rb200_container_pack / _open and the _blocks_ forms here work on host buffers with a host CRC (slicing-by-8, ~1 GB/s
 // on one core: the blob CRC is optional for that reason).  rb200_container_encode / _decode and the _blocks_ forms
@@ -131,11 +133,11 @@ ContainerHeader container_blocks_header(uint32_t n_blocks, uint32_t block_size, 
     return h;
 }
 
-ContainerHeader container_blocks_coder_header(int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
-                                              uint64_t blob_bytes, uint32_t flags)
+ContainerHeader container_blocks_coder_header(uint16_t version, int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size,
+                                              uint32_t chunk_syms, uint64_t blob_bytes, uint32_t flags)
 {
     ContainerHeader h = container_blocks_header(n_blocks, block_size, chunk_syms, blob_bytes, flags);
-    h.version = kContainerVersionBlocksCoder;
+    h.version = version;
     h.coder = static_cast<uint8_t>(coder);
     h.scale_bits = static_cast<uint8_t>(scale_bits);
     return h;
@@ -197,7 +199,7 @@ int container_open_checked(const uint8_t* buf, size_t size, uint16_t version, Co
     return rc;
 }
 
-// The pack of both per-block versions, for the header h (crc fields zero) the caller built from a geometry it checked:
+// The pack of every per-block version, for the header h (crc fields zero) the caller built from a geometry it checked:
 // the other argument rules, every block summing to 1 << h.scale_bits, then the bytes.
 int container_blocks_pack(const ContainerHeader& h, const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob,
                           uint8_t* out, size_t out_cap, size_t* out_size)
@@ -212,7 +214,7 @@ int container_blocks_pack(const ContainerHeader& h, const uint16_t* block_freqs,
     return RB200_OK;
 }
 
-// The open of both per-block versions: the parser's steps for `version`, then the fields their info structs share.
+// The open of every per-block version: the parser's steps for `version`, then the fields their info structs share.
 template <class Info>
 int container_blocks_open(const uint8_t* buf, size_t size, uint16_t version, Info* info, ContainerHeader* h)
 {
@@ -229,6 +231,28 @@ int container_blocks_open(const uint8_t* buf, size_t size, uint16_t version, Inf
     info->block_freqs = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));
     info->offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(*h));
     info->blob = buf + container_blob_offset(*h);
+    return RB200_OK;
+}
+
+// The pack of versions 3 and 4: the version's coder rule, the geometry, then the shared pack
+int container_blocks_coder_pack(uint16_t version, int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes, uint32_t flags,
+                                uint8_t* out, size_t out_cap, size_t* out_size)
+{
+    if (coder < 0 || !container_blocks_coder_ok(version, static_cast<uint32_t>(coder), scale_bits)) return RB200_E_ARG;
+    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
+    return container_blocks_pack(container_blocks_coder_header(version, coder, scale_bits, n_blocks, block_size, chunk_syms, blob_bytes, flags),
+                                 block_freqs, offsets, blob, out, out_cap, out_size);
+}
+
+// The open of versions 3 and 4, which also report the header's coder and scale_bits
+int container_blocks_coder_open(const uint8_t* buf, size_t size, uint16_t version, rb200_container_blocks_coder_info* info)
+{
+    ContainerHeader h;
+    const int rc = container_blocks_open(buf, size, version, info, &h);
+    if (rc != RB200_OK) return rc;
+    info->coder = h.coder;
+    info->scale_bits = h.scale_bits;
     return RB200_OK;
 }
 
@@ -301,20 +325,26 @@ extern "C" int rb200_container_blocks_coder_pack(int coder, uint32_t scale_bits,
                                                  const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob,
                                                  size_t blob_bytes, uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size)
 {
-    if (coder < 0 || !container_blocks_coder_ok(static_cast<uint32_t>(coder), scale_bits)) return RB200_E_ARG;
-    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
-    return container_blocks_pack(container_blocks_coder_header(coder, scale_bits, n_blocks, block_size, chunk_syms, blob_bytes, flags),
-                                 block_freqs, offsets, blob, out, out_cap, out_size);
+    return container_blocks_coder_pack(kContainerVersionBlocksCoder, coder, scale_bits, n_blocks, block_size, chunk_syms, block_freqs, offsets,
+                                       blob, blob_bytes, flags, out, out_cap, out_size);
 }
 
 extern "C" int rb200_container_blocks_coder_open(const uint8_t* buf, size_t size, rb200_container_blocks_coder_info* info)
 {
-    ContainerHeader h;
-    const int rc = container_blocks_open(buf, size, kContainerVersionBlocksCoder, info, &h);
-    if (rc != RB200_OK) return rc;
-    info->coder = h.coder;
-    info->scale_bits = h.scale_bits;
-    return RB200_OK;
+    return container_blocks_coder_open(buf, size, kContainerVersionBlocksCoder, info);
+}
+
+extern "C" int rb200_container_blocks_alias_pack(uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                                 const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob,
+                                                 size_t blob_bytes, uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size)
+{
+    return container_blocks_coder_pack(kContainerVersionBlocksAlias, RB200_CODER_ALIAS, scale_bits, n_blocks, block_size, chunk_syms,
+                                       block_freqs, offsets, blob, blob_bytes, flags, out, out_cap, out_size);
+}
+
+extern "C" int rb200_container_blocks_alias_open(const uint8_t* buf, size_t size, rb200_container_blocks_coder_info* info)
+{
+    return container_blocks_coder_open(buf, size, kContainerVersionBlocksAlias, info);
 }
 
 extern "C" int rb200_choose_coder(const uint64_t counts[256], size_t n, uint32_t chunk_syms, const uint32_t* candidates,

@@ -1156,15 +1156,17 @@ constexpr size_t kBlockFreqBytes = 256 * sizeof(uint16_t);     // one block's fr
 // The plan of a per-block encode over n_blocks blocks (n_blocks x block_size / chunk_syms < 2^31 chunks).  The word
 // coder: the fused kernel (CTA 0 the scanner, then as many worker CTAs as are resident at once, at most one per block)
 // whenever it builds the models, or the split sequence (one CTA per block) when use_fused_encode says so.  The byte and
-// rans64 coders: the split sequence (block_coder_encode_kernel), in slots of the same worst case as plan_encode's.
-EncodePlan plan_blocks_encode(const rb200_ctx* ctx, int coder, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, bool build)
+// rans64 and alias coders: the split sequence (block_coder_encode_kernel), in slots of the same worst case as
+// plan_encode's.
+EncodePlan plan_blocks_encode(const rb200_ctx* ctx, int coder, uint32_t sb, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                              bool build)
 {
     EncodePlan p = {};
     p.n_chunks = n_blocks * (block_size / chunk_syms);
     p.slot_bytes = slot_bytes_for(chunk_syms);
     p.fused = coder == RB200_CODER_WORD && (build || use_fused_encode(chunk_syms));
     p.threads = block_threads(block_size, chunk_syms);
-    p.smem = block_encode_smem(p.threads);
+    p.smem = coder == RB200_CODER_WORD ? block_encode_smem(p.threads) : block_coder_encode_smem(static_cast<uint32_t>(coder), sb, p.threads);
     if (!p.fused) {
         p.grid = n_blocks;
         p.slots = p.n_chunks;
@@ -1181,12 +1183,12 @@ EncodePlan plan_blocks_encode(const rb200_ctx* ctx, int coder, uint32_t n_blocks
 // Per-block encode.  The word coder (scale_bits 12), default: ONE persistent launch (block_encode_fused_kernel: [model,]
 // tables, encode, directory, placement); build_models makes the kernel run count_freqs + normalize_freqs per block first
 // and write d_freqs.  RB200_ENCODE_PATH=split keeps the round-1 sequence (encode into per-chunk slots, tile scan,
-// compaction), which the byte and rans64 coders always run (block_coder_encode_kernel, models of 1 << sb).
+// compaction), which the byte, rans64 and alias coders always run (block_coder_encode_kernel, models of 1 << sb).
 int blocks_encode_device(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* d_in, uint32_t n_blocks, uint32_t block_size,
                          uint16_t* d_freqs, bool build_models, uint32_t chunk_syms, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets)
 {
     if (static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) >= (1ull << 31)) return RB200_E_ARG;
-    const EncodePlan p = plan_blocks_encode(ctx, coder, n_blocks, block_size, chunk_syms, build_models);
+    const EncodePlan p = plan_blocks_encode(ctx, coder, sb, n_blocks, block_size, chunk_syms, build_models);
     return run_encode(ctx, p, d_blob, blob_cap, d_offsets, nullptr, [&](const EncodeWorkspace& ws) {
         if (coder != RB200_CODER_WORD) {
             launch_block_coder_encode(ctx->stream, static_cast<uint32_t>(coder), sb, build_models, p.grid, p.threads, p.smem, d_in, block_size,
@@ -1215,7 +1217,7 @@ int blocks_encode_host(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* in
     const UnitTable freqs = build ? UnitTable{nullptr, block_freqs, kBlockFreqBytes} : UnitTable{block_freqs, nullptr, kBlockFreqBytes};
     return encode_pipeline(
         ctx, in, static_cast<size_t>(n_blocks) * block_size, chunk_syms, block_size / chunk_syms, freqs,
-        [&](const Slice& s) { return plan_blocks_encode(ctx, coder, static_cast<uint32_t>(s.units), block_size, chunk_syms, build); },
+        [&](const Slice& s) { return plan_blocks_encode(ctx, coder, sb, static_cast<uint32_t>(s.units), block_size, chunk_syms, build); },
         [&](const Slice& s, const uint8_t* d_in, uint8_t* d_freqs, uint8_t* d_blob, size_t cap, uint64_t* d_off) {
             return blocks_encode_device(ctx, coder, sb, d_in, static_cast<uint32_t>(s.units), block_size, reinterpret_cast<uint16_t*>(d_freqs),
                                         build, chunk_syms, d_blob, cap, d_off);
@@ -1279,12 +1281,13 @@ int blocks_decode_entry(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* b
         [&] { return blocks_decode_host(ctx, coder, sb, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out); });
 }
 
-// The byte / rans64 per-block calls' own checks before the shared entries: the coder, scale_bits 8..15 and fewer than
-// 2^31 chunks (RB200_E_ARG, nothing launched); a HOST-mode caller table that does not sum to 1 << sb (RB200_E_MODEL).
-int blocks_coder_args(int coder, uint32_t sb, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, const uint16_t* caller_freqs,
-                      int mem_kind)
+// The byte / rans64 (version 3) and alias (version 4) per-block calls' own checks before the shared entries: the coder
+// and scale_bits of `version`, fewer than 2^31 chunks (RB200_E_ARG, nothing launched); a HOST-mode caller table that
+// does not sum to 1 << sb (RB200_E_MODEL).
+int blocks_coder_args(uint16_t version, int coder, uint32_t sb, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                      const uint16_t* caller_freqs, int mem_kind)
 {
-    if (coder < 0 || !container_blocks_coder_ok(static_cast<uint32_t>(coder), sb)) return RB200_E_ARG;
+    if (coder < 0 || !container_blocks_coder_ok(version, static_cast<uint32_t>(coder), sb)) return RB200_E_ARG;
     if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
     if (static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) >= (1ull << 31)) return RB200_E_ARG;
     if (caller_freqs && mem_kind == RB200_MEM_HOST && !container_block_models_sum_to(caller_freqs, n_blocks, 1u << sb)) return RB200_E_MODEL;
@@ -1322,7 +1325,7 @@ extern "C" int rb200_blocks_coder_encode(rb200_ctx* ctx, int coder, uint32_t sca
                                          size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind)
 {
     if (!block_freqs) return RB200_E_ARG;
-    const int rc = blocks_coder_args(coder, scale_bits, n_blocks, block_size, chunk_syms, block_freqs, mem_kind);
+    const int rc = blocks_coder_args(kContainerVersionBlocksCoder, coder, scale_bits, n_blocks, block_size, chunk_syms, block_freqs, mem_kind);
     if (rc != RB200_OK) return rc;
     return blocks_encode_entry(ctx, coder, scale_bits, in, n_blocks, block_size, const_cast<uint16_t*>(block_freqs), false, chunk_syms,
                                blob, blob_cap, offsets, blob_size, mem_kind);
@@ -1332,7 +1335,7 @@ extern "C" int rb200_blocks_coder_model_encode(rb200_ctx* ctx, int coder, uint32
                                                uint32_t block_size, uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob,
                                                size_t blob_cap, uint64_t* offsets, size_t* blob_size, int mem_kind)
 {
-    const int rc = blocks_coder_args(coder, scale_bits, n_blocks, block_size, chunk_syms, nullptr, mem_kind);
+    const int rc = blocks_coder_args(kContainerVersionBlocksCoder, coder, scale_bits, n_blocks, block_size, chunk_syms, nullptr, mem_kind);
     if (rc != RB200_OK) return rc;
     return blocks_encode_entry(ctx, coder, scale_bits, in, n_blocks, block_size, block_freqs, true, chunk_syms, blob, blob_cap, offsets,
                                blob_size, mem_kind);
@@ -1342,9 +1345,43 @@ extern "C" int rb200_blocks_coder_decode(rb200_ctx* ctx, int coder, uint32_t sca
                                          const uint64_t* offsets, const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size,
                                          uint32_t chunk_syms, uint8_t* out, int mem_kind)
 {
-    const int rc = blocks_coder_args(coder, scale_bits, n_blocks, block_size, chunk_syms, nullptr, mem_kind);
+    const int rc = blocks_coder_args(kContainerVersionBlocksCoder, coder, scale_bits, n_blocks, block_size, chunk_syms, nullptr, mem_kind);
     if (rc != RB200_OK) return rc;
     return blocks_decode_entry(ctx, coder, scale_bits, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms, out, mem_kind);
+}
+
+extern "C" int rb200_blocks_alias_encode(rb200_ctx* ctx, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                                         const uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap,
+                                         uint64_t* offsets, size_t* blob_size, int mem_kind)
+{
+    if (!block_freqs) return RB200_E_ARG;
+    const int rc = blocks_coder_args(kContainerVersionBlocksAlias, RB200_CODER_ALIAS, scale_bits, n_blocks, block_size, chunk_syms,
+                                     block_freqs, mem_kind);
+    if (rc != RB200_OK) return rc;
+    return blocks_encode_entry(ctx, RB200_CODER_ALIAS, scale_bits, in, n_blocks, block_size, const_cast<uint16_t*>(block_freqs), false,
+                               chunk_syms, blob, blob_cap, offsets, blob_size, mem_kind);
+}
+
+extern "C" int rb200_blocks_alias_model_encode(rb200_ctx* ctx, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                                               uint16_t* block_freqs, uint32_t chunk_syms, uint8_t* blob, size_t blob_cap,
+                                               uint64_t* offsets, size_t* blob_size, int mem_kind)
+{
+    const int rc = blocks_coder_args(kContainerVersionBlocksAlias, RB200_CODER_ALIAS, scale_bits, n_blocks, block_size, chunk_syms, nullptr,
+                                     mem_kind);
+    if (rc != RB200_OK) return rc;
+    return blocks_encode_entry(ctx, RB200_CODER_ALIAS, scale_bits, in, n_blocks, block_size, block_freqs, true, chunk_syms, blob, blob_cap,
+                               offsets, blob_size, mem_kind);
+}
+
+extern "C" int rb200_blocks_alias_decode(rb200_ctx* ctx, uint32_t scale_bits, const uint8_t* blob, size_t blob_size,
+                                         const uint64_t* offsets, const uint16_t* block_freqs, uint32_t n_blocks, uint32_t block_size,
+                                         uint32_t chunk_syms, uint8_t* out, int mem_kind)
+{
+    const int rc = blocks_coder_args(kContainerVersionBlocksAlias, RB200_CODER_ALIAS, scale_bits, n_blocks, block_size, chunk_syms, nullptr,
+                                     mem_kind);
+    if (rc != RB200_OK) return rc;
+    return blocks_decode_entry(ctx, RB200_CODER_ALIAS, scale_bits, blob, blob_size, offsets, block_freqs, n_blocks, block_size, chunk_syms,
+                               out, mem_kind);
 }
 
 // ---------------------------------------------------------------------------
@@ -1464,7 +1501,7 @@ int container_decode_impl(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8
         if (r == RB200_OK) r = container_check_blob(h, crc);
         return r;
     };
-    if (version != kContainerVersion) {       // per-block models: the word coder at 12 (version 2), byte / rans64 (version 3)
+    if (version != kContainerVersion) {       // per-block models: word at 12 (version 2), byte / rans64 (3), alias (4)
         const uint16_t* block_freqs = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));     // read in place
         return decode(
             [&] {
@@ -1562,7 +1599,7 @@ extern "C" int rb200_container_decode(rb200_ctx* ctx, const uint8_t* buf, size_t
 
 namespace {
 
-// The per-block containers (version 2: the word coder at 12; version 3: byte / rans64): the block encoder writes every
+// The per-block containers (version 2: the word coder at 12; version 3: byte / rans64; version 4: alias): the block encoder writes every
 // block's model (built, or the caller's tables copied in first), the directory and the blob straight into their place
 // in `out`; then as rb200_container_encode, except that one CRC launch covers model and directory, which are contiguous.
 // Arguments are checked by the caller.
@@ -1618,16 +1655,38 @@ extern "C" int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, 
                                         out_cap, out_size, mem_kind);
 }
 
+namespace {
+
+// rb200_container_blocks_coder_encode (version 3) and rb200_container_blocks_alias_encode (version 4)
+int container_blocks_coder_encode(rb200_ctx* ctx, uint16_t version, int coder, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
+                                  uint32_t block_size, const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags, uint8_t* out,
+                                  size_t out_cap, size_t* out_size, int mem_kind)
+{
+    if (!ctx || !in || !out || coder < 0 || !container_blocks_coder_ok(version, static_cast<uint32_t>(coder), scale_bits)) return RB200_E_ARG;
+    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms) || !container_mem_ok(mem_kind, out, nullptr)) return RB200_E_ARG;
+    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
+    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    return container_blocks_encode_impl(
+        ctx, container_blocks_coder_header(version, coder, scale_bits, n_blocks, block_size, chunk_syms, 0, flags), in, block_freqs, out,
+        out_cap, out_size, mem_kind);
+}
+
+}  // namespace
+
 extern "C" int rb200_container_blocks_coder_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
                                                    uint32_t block_size, const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags,
                                                    uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind)
 {
-    if (!ctx || !in || !out || coder < 0 || !container_blocks_coder_ok(static_cast<uint32_t>(coder), scale_bits)) return RB200_E_ARG;
-    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms) || !container_mem_ok(mem_kind, out, nullptr)) return RB200_E_ARG;
-    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
-    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
-    return container_blocks_encode_impl(ctx, container_blocks_coder_header(coder, scale_bits, n_blocks, block_size, chunk_syms, 0, flags), in,
-                                        block_freqs, out, out_cap, out_size, mem_kind);
+    return container_blocks_coder_encode(ctx, kContainerVersionBlocksCoder, coder, scale_bits, in, n_blocks, block_size, block_freqs,
+                                         chunk_syms, flags, out, out_cap, out_size, mem_kind);
+}
+
+extern "C" int rb200_container_blocks_alias_encode(rb200_ctx* ctx, uint32_t scale_bits, const uint8_t* in, uint32_t n_blocks,
+                                                   uint32_t block_size, const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags,
+                                                   uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind)
+{
+    return container_blocks_coder_encode(ctx, kContainerVersionBlocksAlias, RB200_CODER_ALIAS, scale_bits, in, n_blocks, block_size,
+                                         block_freqs, chunk_syms, flags, out, out_cap, out_size, mem_kind);
 }
 
 extern "C" int rb200_container_blocks_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
@@ -1646,6 +1705,15 @@ extern "C" int rb200_container_blocks_coder_decode(rb200_ctx* ctx, const uint8_t
     if (!container_mem_ok(mem_kind, buf, out)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
     return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, mem_kind == RB200_MEM_DEVICE, kContainerVersionBlocksCoder);
+}
+
+extern "C" int rb200_container_blocks_alias_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                                   uint64_t* n_symbols, int mem_kind)
+{
+    if (!ctx || !buf || (!out && out_cap)) return RB200_E_ARG;
+    if (!container_mem_ok(mem_kind, buf, out)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    return container_decode_impl(ctx, buf, size, out, out_cap, n_symbols, mem_kind == RB200_MEM_DEVICE, kContainerVersionBlocksAlias);
 }
 
 namespace {

@@ -46,6 +46,12 @@ alphabet permuted per block) and "zipf" (the --blocks data):
   rb200_blocks_coder_decode against rb200_container_blocks_coder_decode and rb200_container_blocks_coder_decode_async,
   alternated; the host time each container call takes to return; and a torch.profiler list of the async call's kernels.
 
+With --blocks-alias, per-block models for the alias coder on the --blocks-coder workloads (8192 blocks of 64 KiB, chunks
+of 8192, device buffers, "skewed" and "zipf"): rb200_blocks_alias_model_encode against rb200_blocks_coder_model_encode
+(byte) and rb200_blocks_alias_decode against rb200_blocks_coder_decode (byte), at scale_bits 14 and 15, all four in one
+alternated run; the size of each output in bytes per symbol (512 B of model per block included); and a torch.profiler
+list of each call's kernels.
+
 With --auto, rb200_container_model_encode_auto_async over {word 12, alias 16, byte 14} with a 2 % tolerance, on 1 GiB of
 uniform bytes and of p = 0.99 data (symbol 0, a Zipf-1.1 tail over the rest), chunks of 8192: against the fixed call
 for the pair it chose, flags 0 and RB200_CONTAINER_CRC_BLOB, alternated; the costs, the bytes per symbol against the
@@ -53,7 +59,8 @@ word coder's; and a torch.profiler list of the auto call's kernels (the choice k
 
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
-    python tools/container_timing.py [--blocks | --blocks-coder | --single | --model | --auto] [--reps 10] [--json out.json]"""
+    python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto] [--reps 10]
+                                     [--json out.json]"""
 import argparse
 import json
 import os
@@ -302,6 +309,59 @@ def blocks_coder(args):
             m.close()
         res[name] = {"encode": etimes, "decode": dtimes, "bytes_per_symbol": sizes, "kernels": profile}
         res[name].update(blocks_coder_containers(ctx, args, name, coders, sb, d_in, d_out, dec, res["checks"]))
+    ctx.close()
+    return res
+
+
+def blocks_alias(args):
+    import torch
+    n_blocks, block_size, chunk = 8192, 65536, 8192
+    n = n_blocks * block_size
+    n_chunks = n // chunk
+    ctx = rb.Context(0)
+    bound = ctx.encode_bound(n, chunk)
+    sync = ctx.sync
+    res = {"card": card(), "workload": {"n_blocks": n_blocks, "block_size": block_size, "chunk_syms": chunk, "n": n}, "checks": {}}
+    arms = [(c, sb) for sb in (14, 15) for c in ("alias", "byte")]
+    for name, make in (("skewed", skewed_blocks_data), ("zipf", blocks_data)):
+        d_in = make(n_blocks, block_size, 1234)
+        d_out = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+        bufs = {a: (torch.empty(bound + 16, dtype=torch.uint8, device="cuda"), torch.empty(n_chunks + 1, dtype=torch.int64, device="cuda"),
+                    torch.empty(n_blocks * 256, dtype=torch.int16, device="cuda")) for a in arms}
+
+        def menc(a):
+            (c, sb), (b, o, f) = a, bufs[a]
+            if c == "alias":
+                return lambda: ctx.blocks_alias_model_encode_device(sb, d_in.data_ptr(), n_blocks, block_size, f.data_ptr(), chunk, b.data_ptr(),
+                                                                    bound, o.data_ptr())
+            return lambda: ctx.blocks_coder_model_encode_device(rb.CODER_BYTE, sb, d_in.data_ptr(), n_blocks, block_size, f.data_ptr(), chunk,
+                                                                b.data_ptr(), bound, o.data_ptr())
+
+        def dec(a, bb):
+            (c, sb), (b, o, f) = a, bufs[a]
+            if c == "alias":
+                return lambda: ctx.blocks_alias_decode_device(sb, b.data_ptr(), bb, o.data_ptr(), f.data_ptr(), n_blocks, block_size, chunk,
+                                                              d_out.data_ptr())
+            return lambda: ctx.blocks_coder_decode_device(rb.CODER_BYTE, sb, b.data_ptr(), bb, o.data_ptr(), f.data_ptr(), n_blocks,
+                                                          block_size, chunk, d_out.data_ptr())
+        enc = {f"{c}_sb{sb}_blocks_model_encode": menc((c, sb)) for c, sb in arms}
+        etimes = alternate(enc, sync, args.warmup, args.reps)
+        for f in enc.values():
+            f()
+        sync()
+        blob_bytes = {a: int(bufs[a][1][n_chunks].item()) for a in arms}
+        sizes = {f"{c}_sb{sb}_per_block": (blob_bytes[(c, sb)] + 512 * n_blocks) / n for c, sb in arms}
+        for sb in (14, 15):                                            # both coders normalise every block the same way
+            res["checks"][f"{name}_sb{sb}_models_equal_byte"] = bool(torch.equal(bufs[("alias", sb)][2], bufs[("byte", sb)][2]))
+        decs = {f"{c}_sb{sb}_blocks_decode": dec((c, sb), blob_bytes[(c, sb)]) for c, sb in arms}
+        dtimes = alternate(decs, sync, args.warmup, args.reps)
+        for k, f in decs.items():
+            d_out.zero_()
+            f()
+            sync()
+            res["checks"][f"{name}_{k}_equals_input"] = bool(torch.equal(d_out[:n], d_in))
+        profile = {k: kernel_times(f, sync, args.reps) for k, f in {**enc, **decs}.items()}
+        res[name] = {"encode": etimes, "decode": dtimes, "bytes_per_symbol": sizes, "kernels": profile}
     ctx.close()
     return res
 
@@ -682,6 +742,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
     ap.add_argument("--blocks-coder", action="store_true", help="per-block models for the byte and rans64 coders, 8192 blocks of 64 KiB")
+    ap.add_argument("--blocks-alias", action="store_true", help="per-block models for the alias coder against byte, 8192 blocks of 64 KiB")
     ap.add_argument("--single", action="store_true", help="the single-model container's decode calls on three workloads")
     ap.add_argument("--model", action="store_true", help="the single-model container's encode with the model built from the data")
     ap.add_argument("--auto", action="store_true", help="the model-building encode with the coder chosen on the GPU")
@@ -691,7 +752,7 @@ def main():
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
