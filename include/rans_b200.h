@@ -288,7 +288,7 @@ int rb200_container_blocks_coder_decode(rb200_ctx* ctx, const uint8_t* buf, size
  * aligned or NULL; the call never synchronises, copies to or from the host or allocates, so it can be captured in a
  * CUDA graph, and returns only RB200_E_ARG (nothing launched) or RB200_E_CUDA.  *d_n_symbols receives n once header,
  * models and directory pass (also when the blob CRC then fails).  rb200_sync gives the verdict: RB200_E_STREAM for
- * anything rb200_container_blocks_coder_open rejects (version 1 and 2 containers among them), RB200_E_SPACE for
+ * anything rb200_container_blocks_coder_open rejects (version 1, 2 and 4 containers among them), RB200_E_SPACE for
  * n > out_cap, content errors first; in both cases out is untouched.  A corrupt stream that passes every check is
  * RB200_E_STREAM, as from rb200_blocks_coder_decode.  One difference from rb200_container_blocks_coder_decode: a
  * container that open accepts but the decoders refuse (a blob of 2^36 bytes or more), which that call reports as
@@ -315,8 +315,9 @@ int rb200_blocks_alias_decode(rb200_ctx* ctx, uint32_t scale_bits, const uint8_t
                               uint8_t* out, int mem_kind);
 
 /* Their container, version 4: version 3 with coder RB200_CODER_ALIAS (byte 6) at scale_bits 8..15 (byte 7); every other
- * rule is version 3's.  The _alias_ calls accept only version 4, every other container call rejects it.  pack, open,
- * encode and decode behave as the _coder_ calls; open fills the version 3 info struct. */
+ * rule is version 3's.  The _alias_ calls accept only version 4, every other container call (the version 1-3 async
+ * decodes included) rejects it.  pack, open, encode and decode behave as the _coder_ calls; open fills the version 3
+ * info struct. */
 int rb200_container_blocks_alias_pack(uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
                                       const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob,
                                       size_t blob_bytes, uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size);
@@ -326,6 +327,19 @@ int rb200_container_blocks_alias_encode(rb200_ctx* ctx, uint32_t scale_bits, con
                                         uint8_t* out, size_t out_cap, size_t* out_size, int mem_kind);
 int rb200_container_blocks_alias_decode(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                         uint64_t* n_symbols, int mem_kind);
+/* rb200_container_blocks_alias_decode(..., RB200_MEM_DEVICE) with nothing done on the host: the header, every block's
+ * model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the block decoder of the
+ * header's scale_bits is picked on the GPU, and each decoding CTA builds its block's alias table -- all enqueued on the
+ * context stream.  Exactly the contract of rb200_container_blocks_coder_decode_async with version 4 in place of
+ * version 3: DEVICE memory only, buf and out 16-byte aligned, d_n_symbols 8-byte aligned or NULL; the call never
+ * synchronises, copies to or from the host or allocates, so it can be captured in a CUDA graph, and returns only
+ * RB200_E_ARG (nothing launched) or RB200_E_CUDA.  *d_n_symbols receives n once header, models and directory pass.
+ * rb200_sync gives the verdict: RB200_E_STREAM for anything rb200_container_blocks_alias_open rejects (version 1, 2 and
+ * 3 containers among them), RB200_E_SPACE for n > out_cap, content errors first; in both cases out is untouched.  A
+ * corrupt stream that passes every check is RB200_E_STREAM, as from rb200_blocks_alias_decode.  A blob of 2^36 bytes or
+ * more, which rb200_container_blocks_alias_decode reports as RB200_E_ARG, is RB200_E_STREAM here, out untouched. */
+int rb200_container_blocks_alias_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                              uint64_t* d_n_symbols);
 
 /* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
  * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's
@@ -337,8 +351,8 @@ int rb200_container_blocks_alias_decode(rb200_ctx* ctx, const uint8_t* buf, size
  * the verdict: RB200_E_STREAM for anything rb200_container_open rejects, RB200_E_SPACE for n > out_cap, content errors
  * first; in both cases out is untouched.  One difference from rb200_container_decode: a container that open accepts
  * but the decoders refuse (chunk_syms outside 32 .. 2^24, a blob of 2^36 bytes or more, a byte-coder frequency of
- * 65536), which that call reports as RB200_E_ARG or RB200_E_MODEL, is RB200_E_STREAM here, out untouched.  Version 2
- * and 3 containers are rejected (RB200_E_STREAM). */
+ * 65536), which that call reports as RB200_E_ARG or RB200_E_MODEL, is RB200_E_STREAM here, out untouched.  Version 2,
+ * 3 and 4 containers are rejected (RB200_E_STREAM). */
 int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                  uint64_t* d_n_symbols);
 

@@ -80,6 +80,7 @@ EXPORTS = [
     ("rb200_container_blocks_alias_encode", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p,
                                                       C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int]),
     ("rb200_container_blocks_alias_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
+    ("rb200_container_blocks_alias_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_container_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_container_model_encode_async", C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_size_t, C.c_uint32,
                                                      C.c_uint32, C.c_void_p, C.c_size_t]),
@@ -739,6 +740,12 @@ class Context:
         self.lib.check(self.lib.dll.rb200_container_blocks_alias_decode(self.h, buf_ptr, size, out_ptr, out_cap, C.byref(n), MEM_DEVICE),
                        self.h)
         return n.value
+
+    def container_blocks_alias_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
+        """enqueue only (CUDA-graph capturable); n_ptr: device address of a u64 that receives n, or 0.  The verdict on
+        the container (-4 corrupt, -3 out_cap too small, output untouched) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_blocks_alias_decode_async(self.h, buf_ptr, size, out_ptr, out_cap, n_ptr or None),
+                       self.h)
 
     # ---- per-block models, device pointers (asynchronous)
     def blocks_build_models_device(self, in_ptr, n_blocks, block_size, freqs_ptr):

@@ -278,6 +278,38 @@ __device__ __forceinline__ void block_coder_decode_table(const uint32_t* s_cum, 
     }
 }
 
+// A block's alias decode table in shared memory at s_tab, from its cumulative frequencies (s_cum[257], M = 1 << sb): the
+// pairing (block_alias_tables) in the table's place, each thread's bucket entries (at most 2: blockDim >= 128) in
+// registers, then kAliasDecReplicas copies of the 256 entries over it (lean for SB > 8).  Every thread of the CTA takes
+// part and gets the same result: false when the pairing fails (never for a table that sums to M), with nothing written
+// over the pairing.  The caller synchronises before the table is read.
+template <uint32_t SB>
+__device__ __forceinline__ bool block_alias_decode_table(const uint32_t* s_cum, uint8_t* s_tab, uint32_t M)
+{
+    const uint32_t tid = threadIdx.x;
+    const AliasBuildSmem& a = *reinterpret_cast<AliasBuildSmem*>(s_tab);
+    if (!block_alias_tables(s_cum, M, *reinterpret_cast<AliasBuildSmem*>(s_tab))) return false;
+    uint4 e[2];
+#pragma unroll
+    for (uint32_t i = 0; i < 2; i++) {
+        const uint32_t b = tid + i * blockDim.x;
+        if (b >= 256) continue;
+        const AliasDecEntry d = alias_dec_entry(b, a.divider, a.slot_adjust, a.slot_freqs, a.sym_id);
+        if (kAliasLean && SB > 8) e[i] = alias_lean_entry<(SB > 8 ? SB : 9)>(d, b);
+        else e[i] = make_uint4(d.divider, d.alt0, d.alt1, d.adjust);
+    }
+    __syncthreads();
+    uint4* s_dec = reinterpret_cast<uint4*>(s_tab);
+#pragma unroll
+    for (uint32_t i = 0; i < 2; i++) {
+        const uint32_t b = tid + i * blockDim.x;
+        if (b >= 256) continue;
+#pragma unroll
+        for (uint32_t r = 0; r < kAliasDecReplicas; r++) s_dec[b * kAliasDecReplicas + r] = e[i];
+    }
+    return true;
+}
+
 template <uint32_t CODER, uint32_t SB>
 __global__ void __launch_bounds__(kMaxBlockWarps * 32)
 block_coder_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets,
@@ -295,30 +327,9 @@ block_coder_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, 
     }
     uint8_t* s_tab = s_bdec + warps * kRingBytes;
     if (CODER == RB200_CODER_ALIAS) {
-        // the pairing in the table's place, each thread's bucket entries (at most 2: blockDim >= 128) in registers,
-        // then the kAliasDecReplicas copies over it
-        const AliasBuildSmem& a = *reinterpret_cast<AliasBuildSmem*>(s_tab);
-        if (!block_alias_tables(s_cum, M, *reinterpret_cast<AliasBuildSmem*>(s_tab))) {
+        if (!block_alias_decode_table<SB>(s_cum, s_tab, M)) {
             if (tid == 0) atomicOr(status, kStatStream);
             return;
-        }
-        uint4 e[2];
-#pragma unroll
-        for (uint32_t i = 0; i < 2; i++) {
-            const uint32_t b = tid + i * blockDim.x;
-            if (b >= 256) continue;
-            const AliasDecEntry d = alias_dec_entry(b, a.divider, a.slot_adjust, a.slot_freqs, a.sym_id);
-            if (kAliasLean && SB > 8) e[i] = alias_lean_entry<(SB > 8 ? SB : 9)>(d, b);
-            else e[i] = make_uint4(d.divider, d.alt0, d.alt1, d.adjust);
-        }
-        __syncthreads();
-        uint4* s_dec = reinterpret_cast<uint4*>(s_tab);
-#pragma unroll
-        for (uint32_t i = 0; i < 2; i++) {
-            const uint32_t b = tid + i * blockDim.x;
-            if (b >= 256) continue;
-#pragma unroll
-            for (uint32_t r = 0; r < kAliasDecReplicas; r++) s_dec[b * kAliasDecReplicas + r] = e[i];
         }
     } else {
         block_coder_decode_table<CODER>(s_cum, s_tab, M);

@@ -1,7 +1,8 @@
 // container_decode.cuh -- rb200_container_decode_async (version 1, one model, any coder),
-// rb200_container_blocks_decode_async (version 2, per-block models) and rb200_container_blocks_coder_decode_async
-// (version 3, per-block models of the byte or rans64 coder): a container in device memory, checked and decoded by
-// kernels alone, so that the call only enqueues work (and can be captured in a CUDA graph).
+// rb200_container_blocks_decode_async (version 2, per-block models), rb200_container_blocks_coder_decode_async
+// (version 3, per-block models of the byte or rans64 coder) and rb200_container_blocks_alias_decode_async (version 4,
+// per-block models of the alias coder): a container in device memory, checked and decoded by kernels alone, so that the
+// call only enqueues work (and can be captured in a CUDA graph).
 //
 // The stages run in stream order; each reads what the one before it left in the call's ContainerAsyncWork (one per
 // version, allocated with the context):
@@ -20,10 +21,11 @@
 //   the version's decoders         one launch per decoder the version can need, each on a fixed grid of every CTA that
 //                                  is resident at once; only the one whose id is in go runs, every other exits before
 //                                  it touches shared memory, TMA or its counter.  Version 1: one per variant rb200_decode
-//                                  can pick (kDec*); version 2: block_decode_planned_kernel; version 3:
+//                                  can pick (kDec*); version 2: block_decode_planned_kernel; versions 3 and 4:
 //                                  block_coder_decode_planned_kernel<CODER, SB>, one per instance of
-//                                  RB200_BLOCK_CODER_DISPATCH.  The per-block ones take block ids from a counter, build
-//                                  the block's table in shared memory and decode its chunks.
+//                                  RB200_BLOCK_CODER_DISPATCH (version 3) or RB200_BLOCK_ALIAS_DISPATCH (version 4).  The
+//                                  per-block ones take block ids from a counter, build the block's table in shared
+//                                  memory (version 4: the block's alias pairing first) and decode its chunks.
 // The rules are the host parser's (container_format.h); they run in its order: content errors before kStatSpace.
 #pragma once
 #include "alias_kernels.cuh"
@@ -70,7 +72,8 @@ struct ContainerAsyncWork {
 // Version 1: one per variant rb200_decode picks, the word coder narrow or WIDE (a frequency of 4096), the alias and byte
 // coders specialised for scale_bits 16, 14, 12 or generic (RB200_ALIAS_SB_DISPATCH), rans64.  Version 2:
 // block_decode_planned_kernel.  Version 3: one per instance of RB200_BLOCK_CODER_DISPATCH, the byte coder at
-// scale_bits 14, 12 or generic (ids 1, 2, 3), rans64 (4).
+// scale_bits 14, 12 or generic (ids 1, 2, 3), rans64 (4).  Version 4: one per instance of RB200_BLOCK_ALIAS_DISPATCH, the
+// alias coder at scale_bits 14, 12 or generic (ids 1, 2, 3).
 constexpr uint32_t kDecNone = 0, kDecWord = 1, kDecWordWide = 2, kDecAlias = 3, kDecByte = 7, kDecRans64 = 11;
 // offset of a specialisation from kDecAlias / kDecByte
 __host__ __device__ constexpr uint32_t sb_variant(uint32_t sb) { return sb == 16 ? 0 : sb == 14 ? 1 : sb == 12 ? 2 : 3; }
@@ -80,7 +83,7 @@ __host__ __device__ constexpr uint32_t sb_variant(uint32_t sb) { return sb == 16
 __host__ __device__ constexpr uint32_t container_decoder(uint32_t version, uint32_t coder, uint32_t sb, uint32_t wide)
 {
     if (version == kContainerVersionBlocks) return 1;
-    if (version == kContainerVersionBlocksCoder) return coder == RB200_CODER_RANS64 ? 4 : sb == 14 ? 1 : sb == 12 ? 2 : 3;
+    if (version >= kContainerVersionBlocksCoder) return coder == RB200_CODER_RANS64 ? 4 : sb == 14 ? 1 : sb == 12 ? 2 : 3;
     if (coder == RB200_CODER_WORD) return wide ? kDecWordWide : kDecWord;
     if (coder == RB200_CODER_ALIAS) return kDecAlias + sb_variant(sb);
     if (coder == RB200_CODER_BYTE) return kDecByte + sb_variant(sb);
@@ -347,17 +350,21 @@ __global__ void __launch_bounds__(kPlannedWarps * 32, 8)
     }
 }
 
-// The version 3 decoders, one per instance of RB200_BLOCK_CODER_DISPATCH, each on a fixed grid of kPlannedWarps-warp CTAs
-// (resident all at once).  Only the one whose id is in go runs; every other exits before it touches shared memory or
-// the counter.  CTAs take block ids from w->next_block; per block, block_coder_decode_kernel's table in shared memory,
-// then the warps take the block's 1..32 chunks in turn.
+// The version 3 and 4 decoders, one per instance of RB200_BLOCK_CODER_DISPATCH (version 3) and of
+// RB200_BLOCK_ALIAS_DISPATCH (version 4), each on a fixed grid of kPlannedWarps-warp CTAs (resident all at once).  Only
+// the one whose id is in go runs; every other exits before it touches shared memory or the counter.  CTAs take block
+// ids from w->next_block; per block, block_coder_decode_kernel's table in shared memory, then the warps take the block's
+// 1..32 chunks in turn.  The alias coder's pairing overlays the table the previous block's warps read: the barrier at
+// the loop's top keeps it behind their last chunk.
 template <uint32_t CODER, uint32_t SB>
 __global__ void __launch_bounds__(kPlannedWarps * 32)
     block_coder_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                       uint32_t* __restrict__ status)
 {
-    if (w->go != container_decoder(kContainerVersionBlocksCoder, CODER, SB, 0)) return;   // the same for the whole grid
-    extern __shared__ __align__(1024) uint8_t s_bdec[];             // [kPlannedWarps x 1 KiB rings][cum2sym[1 << sb]][symbol entries]
+    constexpr uint32_t version = CODER == RB200_CODER_ALIAS ? kContainerVersionBlocksAlias : kContainerVersionBlocksCoder;
+    if (w->go != container_decoder(version, CODER, SB, 0)) return;   // the same for the whole grid
+    // [kPlannedWarps x 1 KiB rings][cum2sym[1 << sb]][symbol entries], alias: [rings][256 x kAliasDecReplicas bucket entries]
+    extern __shared__ __align__(1024) uint8_t s_bdec[];
     __shared__ uint32_t s_cum[257];
     __shared__ uint32_t s_flag[1];
     __shared__ uint32_t s_block;
@@ -382,12 +389,22 @@ __global__ void __launch_bounds__(kPlannedWarps * 32)
             if (tid == 0) atomicOr(status, kStatStream);
             continue;
         }
-        block_coder_decode_table<CODER>(s_cum, s_tab, M);
+        if (CODER == RB200_CODER_ALIAS) {
+            if (!block_alias_decode_table<SB>(s_cum, s_tab, M)) {   // a block that sums always pairs: not reached
+                if (tid == 0) atomicOr(status, kStatStream);
+                continue;
+            }
+        } else {
+            block_coder_decode_table<CODER>(s_cum, s_tab, M);
+        }
         __syncthreads();
         for (uint32_t k = warp; k < per_block; k += kPlannedWarps) {
             const uint32_t chunk = block * per_block + k;
             uint8_t* dst = out + static_cast<uint64_t>(block) * block_size + static_cast<uint64_t>(k) * chunk_syms;
-            if (CODER == RB200_CODER_BYTE)
+            if (CODER == RB200_CODER_ALIAS)
+                decode_window_chunk(AliasDecoder<SB, kAliasLean>{tab + (lane & (kAliasDecReplicas - 1)) * 16, sb}, blob, blob_bytes, offsets,
+                                    chunk, ring, dst, chunk_syms, status);
+            else if (CODER == RB200_CODER_BYTE)
                 decode_window_chunk(ByteDecoder<SB>{tab, sb}, blob, blob_bytes, offsets, chunk, ring, dst, chunk_syms, status);
             else
                 decode_window_chunk(Rans64Decoder{tab, tab + M + (lane & (kRans64DecReplicas - 1)) * 8, sb}, blob, blob_bytes, offsets, chunk,
@@ -548,14 +565,14 @@ struct DecoderLaunch {
 
 // The decoders of every version in one launch table, each version's in id order: version v's are the entries
 // kDecoderFirst[v - 1] .. kDecoderFirst[v] - 1.
-constexpr int kDecoderFirst[] = {0, 11, 12, 16};
-constexpr int kContainerDecoders = kDecoderFirst[3];
+constexpr int kDecoderFirst[] = {0, 11, 12, 16, 19};
+constexpr int kContainerDecoders = kDecoderFirst[4];
 // the prefix check's grid: kPrefixCtasPerSm CTAs of kPrefixWarps warps per SM
 constexpr uint32_t kPrefixCtasPerSm = 8;
 
 // The launch table, fixed per device: each decoder's grid is every CTA that is resident at once (the version 1 word and
 // alias grids are the shipped kernels' full grids); the generic byte and rans64 decoders get shared memory for the
-// largest scale_bits they decode.
+// largest scale_bits they decode, the version 4 ones the alias bucket table, whose size does not depend on scale_bits.
 inline void configure_container_decode(uint32_t sms, DecoderLaunch* out)
 {
     constexpr uint32_t planned = kPlannedWarps * 32;
@@ -580,6 +597,12 @@ inline void configure_container_decode(uint32_t sms, DecoderLaunch* out)
          block_coder_decode_smem(RB200_CODER_BYTE, kBlockCoderMaxScaleBits, planned), "block_coder_decode_planned_kernel<byte, 0>"},
         {block_coder_decode_planned_kernel<RB200_CODER_RANS64, 0>, 0, planned,
          block_coder_decode_smem(RB200_CODER_RANS64, kBlockCoderMaxScaleBits, planned), "block_coder_decode_planned_kernel<rans64, 0>"},
+        {block_coder_decode_planned_kernel<RB200_CODER_ALIAS, 14>, 0, planned, block_coder_decode_smem(RB200_CODER_ALIAS, 14, planned),
+         "block_coder_decode_planned_kernel<alias, 14>"},
+        {block_coder_decode_planned_kernel<RB200_CODER_ALIAS, 12>, 0, planned, block_coder_decode_smem(RB200_CODER_ALIAS, 12, planned),
+         "block_coder_decode_planned_kernel<alias, 12>"},
+        {block_coder_decode_planned_kernel<RB200_CODER_ALIAS, 0>, 0, planned,
+         block_coder_decode_smem(RB200_CODER_ALIAS, kBlockCoderMaxScaleBits, planned), "block_coder_decode_planned_kernel<alias, 0>"},
     };
     for (int i = 0; i < kContainerDecoders; i++) {
         out[i] = l[i];

@@ -66,7 +66,7 @@ struct rb200_ctx {
     CrcSlot* h_crc = nullptr;
     // the async container decodes (container_decode.cuh): one fixed workspace per version, so that calls of different
     // versions never share state, and every version's decoder launches
-    ContainerAsyncWork* d_async[3] = {};
+    ContainerAsyncWork* d_async[4] = {};
     DecoderLaunch async_decoders[kContainerDecoders] = {};
     // rb200_container_model_encode_async (model_kernels.cuh): the counts, the model and its encode tables
     ModelAsyncWork* d_model_async = nullptr;
@@ -1789,6 +1789,14 @@ extern "C" int rb200_container_blocks_coder_decode_async(rb200_ctx* ctx, const u
 {
     if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
     return container_decode_async(ctx, kContainerVersionBlocksCoder, buf, size, out, out_cap, d_n_symbols);
+}
+
+// Eight launches: the checks and every block decoder variant of RB200_BLOCK_ALIAS_DISPATCH.
+extern "C" int rb200_container_blocks_alias_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                                         uint64_t* d_n_symbols)
+{
+    if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    return container_decode_async(ctx, kContainerVersionBlocksAlias, buf, size, out, out_cap, d_n_symbols);
 }
 
 namespace {

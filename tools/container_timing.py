@@ -50,7 +50,10 @@ With --blocks-alias, per-block models for the alias coder on the --blocks-coder 
 of 8192, device buffers, "skewed" and "zipf"): rb200_blocks_alias_model_encode against rb200_blocks_coder_model_encode
 (byte) and rb200_blocks_alias_decode against rb200_blocks_coder_decode (byte), at scale_bits 14 and 15, all four in one
 alternated run; the size of each output in bytes per symbol (512 B of model per block included); and a torch.profiler
-list of each call's kernels.
+list of each call's kernels.  Then the --blocks-coder container rows for the version 4 (alias) and version 3 (byte)
+containers of the same blocks at 14 and 15, in one alternated run: rb200_blocks_{alias,coder}_decode against
+rb200_container_blocks_{alias,coder}_decode (DEVICE) and the async call, flags 0 and RB200_CONTAINER_CRC_BLOB; the
+host time each container call takes to return; and a torch.profiler list of each async call's kernels.
 
 With --auto, rb200_container_model_encode_auto_async over {word 12, alias 16, byte 14} with a 2 % tolerance, on 1 GiB of
 uniform bytes and of p = 0.99 data (symbol 0, a Zipf-1.1 tail over the rest), chunks of 8192: against the fixed call
@@ -308,7 +311,10 @@ def blocks_coder(args):
         for m, *_ in single.values():
             m.close()
         res[name] = {"encode": etimes, "decode": dtimes, "bytes_per_symbol": sizes, "kernels": profile}
-        res[name].update(blocks_coder_containers(ctx, args, name, coders, sb, d_in, d_out, dec, res["checks"]))
+        arms = {k: (lambda flags, p, cap, c=c: ctx.container_blocks_coder_encode_device(c, sb, d_in.data_ptr(), n_blocks, block_size, None,
+                                                                                        chunk, flags, p, cap),
+                    ctx.container_blocks_coder_decode_device, ctx.container_blocks_coder_decode_async) for k, c in coders.items()}
+        res[name].update(blocks_coder_containers(ctx, args, name, arms, d_in, d_out, dec, res["checks"]))
     ctx.close()
     return res
 
@@ -362,37 +368,50 @@ def blocks_alias(args):
             res["checks"][f"{name}_{k}_equals_input"] = bool(torch.equal(d_out[:n], d_in))
         profile = {k: kernel_times(f, sync, args.reps) for k, f in {**enc, **decs}.items()}
         res[name] = {"encode": etimes, "decode": dtimes, "bytes_per_symbol": sizes, "kernels": profile}
+
+        def cenc(c, sb):
+            """the encode of the version 4 (alias) or version 3 (byte) container of the same blocks, so that both planned
+            decoders run side by side"""
+            if c == "alias":
+                return lambda flags, p, cap: ctx.container_blocks_alias_encode_device(sb, d_in.data_ptr(), n_blocks, block_size, None, chunk,
+                                                                                      flags, p, cap)
+            return lambda flags, p, cap: ctx.container_blocks_coder_encode_device(rb.CODER_BYTE, sb, d_in.data_ptr(), n_blocks, block_size,
+                                                                                  None, chunk, flags, p, cap)
+        decodes = {"alias": (ctx.container_blocks_alias_decode_device, ctx.container_blocks_alias_decode_async),
+                   "byte": (ctx.container_blocks_coder_decode_device, ctx.container_blocks_coder_decode_async)}
+        carms = {f"{c}_sb{sb}": (cenc(c, sb), *decodes[c]) for c, sb in arms}
+        res[name].update(blocks_coder_containers(ctx, args, name, carms, d_in, d_out, decs, res["checks"]))
     ctx.close()
     return res
 
 
-def blocks_coder_containers(ctx, args, name, coders, sb, d_in, d_out, dec, checks):
-    """The version 3 container of the same blocks (models built on the GPU), each coder with flags 0 and
-    RB200_CONTAINER_CRC_BLOB: rb200_blocks_coder_decode against rb200_container_blocks_coder_decode (DEVICE) and
-    rb200_container_blocks_coder_decode_async, alternated; the host time each container call takes to return; and a
-    torch.profiler list of the async call's kernels (the planned decoder and the gated-out launches)."""
+def blocks_coder_containers(ctx, args, name, arms, d_in, d_out, dec, checks):
+    """The per-block container (version 3 or 4) of the same blocks, models built on the GPU, each arm with flags 0 and
+    RB200_CONTAINER_CRC_BLOB: the plain per-block decode dec[f"{arm}_blocks_decode"] against the container's DEVICE
+    decode and its async decode, alternated; the host time each container call takes to return; and a torch.profiler
+    list of the async call's kernels (the planned decoder and the gated-out launches).  arms: {arm: (encode, decode,
+    decode_async)}, encode(flags, out_ptr, out_cap) writes the container of d_in, decode and decode_async take
+    (buf_ptr, size, out_ptr, out_cap)."""
     import torch
     n = d_in.numel()
     n_blocks, block_size, chunk = 8192, 65536, 8192
     cap = ctx.container_blocks_capacity(n_blocks, block_size, chunk)
     sync = ctx.sync
     conts = {}
-    for k, coder in coders.items():
+    for k, (encode, _, _) in arms.items():
         for flags, tag in ((0, ""), (api.CONTAINER_CRC_BLOB, "_crc")):
             d = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
-            ctx.container_blocks_coder_encode_device(coder, sb, d_in.data_ptr(), n_blocks, block_size, None, chunk, flags, d.data_ptr(), cap)
+            encode(flags, d.data_ptr(), cap)
             sync()
             blob_bytes = int(d[32:40].cpu().numpy().view(np.uint64)[0])
             conts[k + tag] = (d, int(ctx.lib.dll.rb200_container_blocks_size(n_blocks, n // chunk, blob_bytes)))
     calls = {}
-    for k in coders:
+    for k, (_, decode, decode_async) in arms.items():
         calls[f"{k}_blocks_decode"] = dec[f"{k}_blocks_decode"]
         for tag in ("", "_crc"):
             d, size = conts[k + tag]
-            calls[f"{k}_container_decode{tag}"] = lambda d=d, size=size: ctx.container_blocks_coder_decode_device(d.data_ptr(), size,
-                                                                                                                  d_out.data_ptr(), n)
-            calls[f"{k}_container_decode_async{tag}"] = lambda d=d, size=size: ctx.container_blocks_coder_decode_async(d.data_ptr(), size,
-                                                                                                                      d_out.data_ptr(), n)
+            calls[f"{k}_container_decode{tag}"] = lambda d=d, size=size, f=decode: f(d.data_ptr(), size, d_out.data_ptr(), n)
+            calls[f"{k}_container_decode_async{tag}"] = lambda d=d, size=size, f=decode_async: f(d.data_ptr(), size, d_out.data_ptr(), n)
     times = alternate(calls, sync, args.warmup, args.reps)
     host = {k: [] for k in calls if "container" in k}
     for _ in range(args.reps):
@@ -406,7 +425,7 @@ def blocks_coder_containers(ctx, args, name, coders, sb, d_in, d_out, dec, check
         f()
         sync()
         checks[f"{name}_{k}_equals_input"] = bool(torch.equal(d_out[:n], d_in))
-    profile = {f"{k}_container_decode_async": kernel_times(calls[f"{k}_container_decode_async"], sync, args.reps) for k in coders}
+    profile = {f"{k}_container_decode_async": kernel_times(calls[f"{k}_container_decode_async"], sync, args.reps) for k in arms}
     return {"container_decode": times, "container_decode_call_host_ms": {k: stats(v) for k, v in host.items()},
             "container_kernels": profile}
 

@@ -81,29 +81,35 @@ def main():
     except rb.RansError:
         pass
     m.close()
-    # the per-block container decoded by kernels alone: valid, then a corrupt model and a corrupt blob (both rejected
-    # before any decode)
+    # the per-block containers decoded by kernels alone, version 2 (word) and version 4 (alias at 14, each block's alias
+    # table built by its decoding CTA): valid, then a corrupt model and a corrupt blob (both rejected before any decode)
     cap = ctx.container_blocks_capacity(nb, bs, chunk)
     d_cb = torch.zeros(cap + 16, dtype=torch.uint8, device="cuda")
     d_n = torch.zeros(1, dtype=torch.int64, device="cuda")
-    ctx.container_blocks_encode_device(d_in.data_ptr(), nb, bs, None, chunk, api.CONTAINER_CRC_BLOB, d_cb.data_ptr(), cap)
-    d_out.zero_()
-    ctx.container_blocks_decode_async(d_cb.data_ptr(), cap, d_out.data_ptr(), data.size, d_n.data_ptr())
-    ctx.sync()
-    assert int(d_n.item()) == data.size and torch.equal(d_out[:data.size], d_in)
-    h_cb = d_cb[:cap].cpu().numpy()
-    boff = api.container_blocks_open(h_cb)[3].ctypes.data - h_cb.ctypes.data
-    for pos in (64 + 3, boff + 1000):
-        d_cb[pos] ^= 1
+    crc = api.CONTAINER_CRC_BLOB
+    for encode, decode_async, open_ in (
+            (lambda: ctx.container_blocks_encode_device(d_in.data_ptr(), nb, bs, None, chunk, crc, d_cb.data_ptr(), cap),
+             ctx.container_blocks_decode_async, api.container_blocks_open),
+            (lambda: ctx.container_blocks_alias_encode_device(14, d_in.data_ptr(), nb, bs, None, chunk, crc, d_cb.data_ptr(), cap),
+             ctx.container_blocks_alias_decode_async, api.container_blocks_alias_open)):
+        encode()
         d_out.zero_()
-        ctx.container_blocks_decode_async(d_cb.data_ptr(), cap, d_out.data_ptr(), data.size, d_n.data_ptr())
-        try:
-            ctx.sync()
-            raise SystemExit("per-block container corruption not reported")
-        except rb.RansError:
-            pass
-        assert not d_out.any().item()
-        d_cb[pos] ^= 1
+        decode_async(d_cb.data_ptr(), cap, d_out.data_ptr(), data.size, d_n.data_ptr())
+        ctx.sync()
+        assert int(d_n.item()) == data.size and torch.equal(d_out[:data.size], d_in)
+        h_cb = d_cb[:cap].cpu().numpy()
+        boff = open_(h_cb)[3].ctypes.data - h_cb.ctypes.data
+        for pos in (64 + 3, boff + 1000):
+            d_cb[pos] ^= 1
+            d_out.zero_()
+            decode_async(d_cb.data_ptr(), cap, d_out.data_ptr(), data.size, d_n.data_ptr())
+            try:
+                ctx.sync()
+                raise SystemExit("per-block container corruption not reported")
+            except rb.RansError:
+                pass
+            assert not d_out.any().item()
+            d_cb[pos] ^= 1
     # the single-model container decoded by kernels alone: a valid container of each coder, then (alias) a corrupt
     # model and a corrupt blob, rejected before any decode, and a corrupt stream with flags 0, which the decoder reports
     for coder, sb in ((rb.CODER_WORD, 12), (rb.CODER_ALIAS, 16), (rb.CODER_BYTE, 14), (rb.CODER_RANS64, 12)):
