@@ -1154,10 +1154,19 @@ namespace {
 constexpr size_t kBlockFreqBytes = 256 * sizeof(uint16_t);     // one block's frequency table
 
 // The plan of a per-block encode over n_blocks blocks (n_blocks x block_size / chunk_syms < 2^31 chunks).  The word
-// coder: the fused kernel (CTA 0 the scanner, then as many worker CTAs as are resident at once, at most one per block)
+// coder: the fused kernel (CTA 0 the scanner, then as many worker CTAs as are resident at once, at most one per block
+// and as many as kBlockFusedScratchMax holds)
 // whenever it builds the models, or the split sequence (one CTA per block) when use_fused_encode says so.  The byte and
 // rans64 and alias coders: the split sequence (block_coder_encode_kernel), in slots of the same worst case as
 // plan_encode's.
+// K5f holds kBlockFusedSlots worst-case slots (2 x chunk_syms + 512 bytes) per warp of every CTA: about 4x a block's
+// bytes per CTA.  The flat path leaves the fused kernel above 64 Ki symbols per chunk (use_fused_encode), but K5f is
+// the only per-block path that builds models, so it takes any chunk; its worker CTAs are capped instead, so that the
+// scratch stays within kBlockFusedScratchMax (one worker at least).  Up to 64 Ki symbols per chunk the cap binds only
+// at 32 chunks of 64 Ki per block, by a few of ~260 CTAs on an H100; without it, 64 blocks of 2^24 symbols would take
+// 65 x 256 MiB of scratch where the split path takes 2 GiB.
+constexpr uint64_t kBlockFusedScratchMax = 2ull << 30;
+
 EncodePlan plan_blocks_encode(const rb200_ctx* ctx, int coder, uint32_t sb, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
                               bool build)
 {
@@ -1174,7 +1183,10 @@ EncodePlan plan_blocks_encode(const rb200_ctx* ctx, int coder, uint32_t sb, uint
     }
     int per_sm = 0;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_encode_fused_for(build, p.threads), static_cast<int>(p.threads), p.smem);
-    const uint64_t workers = static_cast<uint64_t>(ctx->sms) * std::max(per_sm, 1) - 1;      // the scanner CTA takes one slot
+    const uint64_t cta_scratch = static_cast<uint64_t>(p.threads / 32) * kBlockFusedSlots * p.slot_bytes;
+    const uint64_t fit = kBlockFusedScratchMax / cta_scratch;                                  // CTAs, the scanner's included
+    const uint64_t workers = std::min<uint64_t>(static_cast<uint64_t>(ctx->sms) * std::max(per_sm, 1) - 1,   // the scanner CTA takes one slot
+                                                std::max<uint64_t>(fit, 2) - 1);
     p.grid = static_cast<uint32_t>(std::max<uint64_t>(std::min<uint64_t>(workers, n_blocks), 1) + 1);
     p.slots = static_cast<size_t>(p.grid) * (p.threads / 32) * kBlockFusedSlots;
     return p;
