@@ -422,6 +422,56 @@ int rb200_container_model_encode_auto_async(rb200_ctx* ctx, const uint32_t* cand
                                             uint32_t tolerance_ppm, const uint8_t* in, const uint64_t* d_n, size_t n,
                                             uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap);
 
+/* Choosing the coder of a per-block container (versions 2-4) from the blocks.  A candidate is RB200_CANDIDATE(coder,
+ * scale_bits) with a pair some per-block version takes: word at 12 (version 2), byte or rans64 at 8..15 (version 3),
+ * alias at 8..15 (version 4); a list holds 1 to 16 distinct candidates in order of preference.  The rule above, per
+ * block b (counts c_b, block_size / chunk_syms chunks) and summed over the blocks:
+ *   f          = normalize_freqs(c_b, 1 << sb_i): the block's model exactly as the model-building per-block encode
+ *                writes it for (coder_i, sb_i);
+ *   block_cost = ceil(bits_q / 2^19) + (block_size / chunk_syms) * H, bits_q and H as above; except for the word coder
+ *                on a block of one symbol (f holds 4096), which costs what its encoder writes: 2 * block_size + 128 per
+ *                chunk (every step emits a 16-bit word);
+ *   cost_i     = the sum of block_cost over the blocks (the 512-byte model of each block is the same in every version
+ *                and is not counted).
+ * Every candidate is feasible on every block, so every cost is finite.  The choice is the first candidate whose cost is
+ * at most min + floor(min * tolerance_ppm / 10^6).
+ * rb200_choose_blocks_coder applies it on the host to block_counts (n_blocks x 256 counts, each row summing to
+ * block_size): costs (may be NULL) receives every cost, *chosen the index of the choice.  RB200_E_ARG for a null
+ * block_counts or chosen, an invalid list or a candidate no per-block version takes, a geometry the per-block calls
+ * refuse, tolerance_ppm > 10^6, or a row that does not sum to block_size. */
+int rb200_choose_blocks_coder(const uint32_t* block_counts, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                              const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm, uint64_t* costs,
+                              uint32_t* chosen);
+
+/* rb200_container_blocks_encode, rb200_container_blocks_coder_encode or rb200_container_blocks_alias_encode in DEVICE
+ * memory with the models built (block_freqs NULL), for the pair the rule above picks on the GPU from the blocks at
+ * every run: one captured graph writes a version 2, 3 or 4 container, whichever suits the data it meets, byte for byte
+ * (header included) what the fixed call writes for the chosen pair.  in and out are device memory, out 16-byte aligned;
+ * the geometry rules are the per-block calls'.  The call only enqueues work: a memset and one choice kernel, one gated
+ * encode group per distinct encoder instance the list needs (only the chosen group runs), the CRCs and the header
+ * kernel.  It returns RB200_E_ARG (nothing launched) for a null ctx, in or out, a misaligned out, an invalid list or
+ * candidate, tolerance_ppm > 10^6, a bad geometry or 2^31 chunks or more; RB200_E_SPACE when out_cap is below the blob
+ * offset (64 + 512 n_blocks + the directory, rounded to 16).  rb200_sync returns RB200_E_SPACE when the chosen blob does
+ * not fit out_cap, with the header not written, as for the fixed call.  The workspace grows for every group's plan, so
+ * a call with the same list and geometry outside a capture must come first.  rb200_container_blocks_auto_costs copies
+ * the costs of the last run's choice (n <= 16 of them, the list's order) to host memory; it synchronises. */
+int rb200_container_blocks_model_encode_auto_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                   uint32_t tolerance_ppm, const uint8_t* in, uint32_t n_blocks,
+                                                   uint32_t block_size, uint32_t chunk_syms, uint32_t flags, uint8_t* out,
+                                                   size_t out_cap);
+int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n);
+
+/* The async decode of a per-block container of any version: the header's version field (bytes 4-5) picks version 2, 3
+ * or 4, and the call then reaches the verdict, status and output of rb200_container_blocks_decode_async,
+ * rb200_container_blocks_coder_decode_async or rb200_container_blocks_alias_decode_async on it, under the same rules
+ * (DEVICE memory only, buf and out 16-byte aligned, d_n_symbols 8-byte aligned or NULL, enqueue only, RB200_E_ARG or
+ * RB200_E_CUDA from the call, the verdict from rb200_sync).  Any other version, version 1 included, is RB200_E_STREAM.
+ * Thirteen launches: the checks, then the decoders of all three versions, of which only the header version's can run.
+ * A host caller that does not capture can read the version field itself and call the synchronous decode of that
+ * version. */
+int rb200_container_blocks_any_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                            uint64_t* d_n_symbols);
+
 /* ---------------------------------------------------------------- multi-GPU: gathering the shards' blobs (NCCL) */
 
 /* Shards are independent (SURVEY 8e): every rank encodes / decodes its own contiguous range of symbols with no

@@ -89,6 +89,11 @@ EXPORTS = [
     ("rb200_choose_coder", C.c_int, [_u64p, C.c_size_t, C.c_uint32, _u32p, C.c_uint32, C.c_uint32, _u64p, _u32p]),
     ("rb200_container_model_encode_auto_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t,
                                                           C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_choose_blocks_coder", C.c_int, [_u32p, C.c_uint32, C.c_uint32, C.c_uint32, _u32p, C.c_uint32, C.c_uint32, _u64p, _u32p]),
+    ("rb200_container_blocks_model_encode_auto_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
+                                                                 C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_container_blocks_auto_costs", C.c_int, [C.c_void_p, _u64p, C.c_uint32]),
+    ("rb200_container_blocks_any_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -127,6 +132,21 @@ def choose_coder(counts, n, chunk_syms, candidates, tolerance_ppm=0):
     chosen = C.c_uint32(0)
     lib.check(lib.dll.rb200_choose_coder(counts.ctypes.data_as(_u64p), n, chunk_syms, cands.ctypes.data_as(_u32p), cands.size,
                                          tolerance_ppm, costs.ctypes.data_as(_u64p), C.byref(chosen)))
+    return int(chosen.value), costs[:cands.size]
+
+
+def choose_blocks_coder(block_counts, block_size, chunk_syms, candidates, tolerance_ppm=0):
+    """rb200_choose_blocks_coder: the rule of the per-block auto encode on the host.  block_counts: n_blocks x 256 counts,
+    each row summing to block_size; candidates: CANDIDATE values of per-block pairs (word 12; byte, rans64 or alias at
+    8..15), in order of preference.  Returns (index, costs), costs as u64 in list order."""
+    lib = load()
+    counts = np.ascontiguousarray(block_counts, dtype=np.uint32).reshape(-1, 256)
+    cands = _candidates(candidates)
+    costs = np.zeros(max(cands.size, 1), np.uint64)
+    chosen = C.c_uint32(0)
+    lib.check(lib.dll.rb200_choose_blocks_coder(counts.ctypes.data_as(_u32p), counts.shape[0], block_size, chunk_syms,
+                                                cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm, costs.ctypes.data_as(_u64p),
+                                                C.byref(chosen)))
     return int(chosen.value), costs[:cands.size]
 
 
@@ -740,6 +760,29 @@ class Context:
         self.lib.check(self.lib.dll.rb200_container_blocks_alias_decode(self.h, buf_ptr, size, out_ptr, out_cap, C.byref(n), MEM_DEVICE),
                        self.h)
         return n.value
+
+    def container_blocks_model_encode_auto_async(self, candidates, tolerance_ppm, in_ptr, n_blocks, block_size, chunk_syms, flags, out_ptr,
+                                                 out_cap):
+        """the per-block container encode (DEVICE, models built) with (coder, scale_bits) chosen on the GPU from the blocks
+        at every run, by the rule of choose_blocks_coder over `candidates`: a version 2, 3 or 4 container, byte for byte
+        the fixed call's for the chosen pair.  The verdict (-3 when the chosen blob does not fit, header unwritten) comes
+        from sync()"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_blocks_model_encode_auto_async(self.h, cands.ctypes.data_as(_u32p), cands.size,
+                                                                                   tolerance_ppm, in_ptr, n_blocks, block_size, chunk_syms,
+                                                                                   flags, out_ptr, out_cap), self.h)
+
+    def container_blocks_auto_costs(self, n):
+        """the n candidate costs of the last container_blocks_model_encode_auto_async run (synchronises)"""
+        costs = np.zeros(max(n, 1), np.uint64)
+        self.lib.check(self.lib.dll.rb200_container_blocks_auto_costs(self.h, costs.ctypes.data_as(_u64p), n), self.h)
+        return costs[:n]
+
+    def container_blocks_any_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
+        """the async decode of a per-block container of version 2, 3 or 4, whichever the header names; enqueue only
+        (CUDA-graph capturable).  The verdict (-4 corrupt or another version, -3 out_cap too small, output untouched)
+        comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_blocks_any_decode_async(self.h, buf_ptr, size, out_ptr, out_cap, n_ptr or None), self.h)
 
     def container_blocks_alias_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
         """enqueue only (CUDA-graph capturable); n_ptr: device address of a u64 that receives n, or 0.  The verdict on

@@ -178,10 +178,9 @@ inline uint32_t block_coder_decode_smem(uint32_t coder, uint32_t sb, uint32_t th
 }
 
 template <uint32_t CODER, uint32_t SB, bool BUILD>
-__global__ void __launch_bounds__(kMaxBlockWarps * 32)
-block_coder_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t sb_rt,
-                          uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
-                          uint32_t* __restrict__ status)
+__device__ __forceinline__ void block_coder_encode(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs,
+                                                   uint32_t sb_rt, uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes,
+                                                   uint32_t* __restrict__ sizes, uint32_t* __restrict__ status)
 {
     extern __shared__ __align__(1024) uint8_t s_benc[];         // [32 KiB: histogram copies (BUILD), then the table][warps x 1 KiB]
     __shared__ uint32_t s_cnt[256], s_cum[257];
@@ -240,6 +239,28 @@ block_coder_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, u
         encode_chunk_split(src, chunk_syms, chunk, AliasEncoder<false, SB>{tab, 0, sb}, wsm, scratch, slot_bytes, sizes, status);
     else
         encode_chunk_split(src, chunk_syms, chunk, Rans64Encoder{tab, sb}, wsm, scratch, slot_bytes, sizes, status);
+}
+
+template <uint32_t CODER, uint32_t SB, bool BUILD>
+__global__ void __launch_bounds__(kMaxBlockWarps * 32)
+block_coder_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t sb_rt,
+                          uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
+                          uint32_t* __restrict__ status)
+{
+    block_coder_encode<CODER, SB, BUILD>(in, block_size, block_freqs, sb_rt, chunk_syms, scratch, slot_bytes, sizes, status);
+}
+
+// The model-building instances for rb200_container_blocks_model_encode_auto_async: run only when the choice record
+// (CoderChoice, device_utils.cuh) names `group`, and then at the record's scale_bits (the generic instances; the
+// specialised ones are only ever named at their own)
+template <uint32_t CODER, uint32_t SB>
+__global__ void __launch_bounds__(kMaxBlockWarps * 32)
+block_coder_encode_gated_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t chunk_syms,
+                                uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status,
+                                const CoderChoice* __restrict__ choice, uint32_t group)
+{
+    if (choice->group != group) return;                          // the same for the whole grid
+    block_coder_encode<CODER, SB, true>(in, block_size, block_freqs, choice->scale_bits, chunk_syms, scratch, slot_bytes, sizes, status);
 }
 
 // A block's decode table in shared memory at s_tab, from its cumulative frequencies (s_cum[257], M = 1 << sb): cum2sym[M],
@@ -385,7 +406,8 @@ template <uint32_t CODER, uint32_t SB>
 inline void configure_block_coder()
 {
     for (const void* k : {reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, true>),
-                          reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, false>)}) {
+                          reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, false>),
+                          reinterpret_cast<const void*>(block_coder_encode_gated_kernel<CODER, SB>)}) {
         cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              block_coder_encode_smem(CODER, kBlockCoderMaxScaleBits, kMaxBlockWarps * 32));
@@ -413,6 +435,16 @@ inline void launch_block_coder_encode(cudaStream_t stream, uint32_t coder, uint3
     RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, ((build ? block_coder_encode_kernel<CODER, SB, true> : block_coder_encode_kernel<CODER, SB, false>)
                                            <<<n_blocks, threads, smem, stream>>>(d_in, block_size, d_freqs, sb, chunk_syms, scratch,
                                                                                  slot_bytes, sizes, status)))
+}
+
+// the gated instance of (coder, sb)'s dispatch (rb200_container_blocks_model_encode_auto_async): sb is the largest
+// scale_bits of the launch group, which sizes the alias coder's remap; the kernel takes the chosen one from the record
+inline void launch_block_coder_encode_gated(cudaStream_t stream, uint32_t coder, uint32_t sb, uint32_t n_blocks, uint32_t threads, uint32_t smem,
+                                            const uint8_t* d_in, uint32_t block_size, uint16_t* d_freqs, uint32_t chunk_syms, uint8_t* scratch,
+                                            uint32_t slot_bytes, uint32_t* sizes, uint32_t* status, const CoderChoice* choice, uint32_t group)
+{
+    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, (block_coder_encode_gated_kernel<CODER, SB><<<n_blocks, threads, smem, stream>>>(
+                                              d_in, block_size, d_freqs, chunk_syms, scratch, slot_bytes, sizes, status, choice, group)))
 }
 
 inline void launch_block_coder_decode(cudaStream_t stream, uint32_t coder, uint32_t sb, const uint8_t* blob, uint64_t blob_size,

@@ -202,14 +202,12 @@ __device__ __forceinline__ void block_model_build(const uint8_t* __restrict__ bl
     __syncthreads();
 }
 
-// The same with the bank-private histogram of histogram_kernel (one copy per lane, 32 KiB at `hist`): no bank
-// conflicts and no hot-counter serialisation.  Used by the fused per-block encoder, where the 32 KiB are the (not yet
-// built) encoder table.  s_cnt / s_cum / s_w: 256 / 257 / 256 words.  target as for block_model_build.
-__device__ __forceinline__ void block_model_build_wide(const uint8_t* __restrict__ blk, uint32_t block_size, uint32_t* hist, uint32_t* s_cnt,
-                                                       uint32_t* s_cum, uint32_t* s_w, uint16_t* __restrict__ dst,
-                                                       uint32_t* __restrict__ status, uint32_t target)
+// count_freqs of one block by the whole CTA with the bank-private histogram of histogram_kernel (one copy per lane, 32
+// KiB at `hist`): no bank conflicts and no hot-counter serialisation.  The CTA must call it convergently; on return
+// (after a CTA barrier) s_cnt[0..256) holds the counts and `hist` is free.
+__device__ __forceinline__ void block_histogram_wide(const uint8_t* __restrict__ blk, uint32_t block_size, uint32_t* hist, uint32_t* s_cnt)
 {
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t tid = threadIdx.x, lane = tid & 31;
     for (uint32_t i = tid; i < 256 * 32; i += blockDim.x) hist[i] = 0;
     __syncthreads();
     {   // count_freqs, main.cpp:59-66
@@ -239,6 +237,17 @@ __device__ __forceinline__ void block_model_build_wide(const uint8_t* __restrict
         s_cnt[s] = t;
     }
     __syncthreads();
+}
+
+// block_model_build on the bank-private histogram (block_histogram_wide).  Used by the fused per-block encoder, where
+// the 32 KiB are the (not yet built) encoder table.  s_cnt / s_cum / s_w: 256 / 257 / 256 words.  target as for
+// block_model_build.
+__device__ __forceinline__ void block_model_build_wide(const uint8_t* __restrict__ blk, uint32_t block_size, uint32_t* hist, uint32_t* s_cnt,
+                                                       uint32_t* s_cum, uint32_t* s_w, uint16_t* __restrict__ dst,
+                                                       uint32_t* __restrict__ status, uint32_t target)
+{
+    const uint32_t warp = threadIdx.x >> 5;
+    block_histogram_wide(blk, block_size, hist, s_cnt);
     if (warp == 0) block_normalize(s_cnt, s_cum, s_w, dst, target, kStatStream, status);
     __syncthreads();
 }
@@ -422,12 +431,12 @@ block_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, const u
 // place the chunk of the PREVIOUS block once the scanner has turned the published sizes into end offsets.  The second
 // pass over the block's 64 KiB (histogram first, then encode) is served by the L2.
 constexpr uint32_t kBlockFusedSlots = 2;        // scratch slots per worker warp
-template <bool BUILD, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32, WARPS <= 8 ? 5 : 1)
-block_encode_fused_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uint32_t block_size, uint16_t* __restrict__ block_freqs,
-                          uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint64_t* __restrict__ look,
-                          uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap, uint64_t* __restrict__ offsets,
-                          uint32_t* __restrict__ status)
+template <bool BUILD>
+__device__ __forceinline__ void block_encode_fused(const uint8_t* __restrict__ in, uint32_t n_blocks, uint32_t block_size,
+                                                   uint16_t* __restrict__ block_freqs, uint32_t chunk_syms, uint8_t* __restrict__ scratch,
+                                                   uint32_t slot_bytes, uint64_t* __restrict__ look, uint32_t* __restrict__ counter,
+                                                   uint8_t* __restrict__ blob, uint64_t blob_cap, uint64_t* __restrict__ offsets,
+                                                   uint32_t* __restrict__ status)
 {
     extern __shared__ __align__(1024) uint8_t s_enc[];          // [32 KiB: histogram copies, then the table][warps x 1 KiB stage + ring]
     __shared__ uint32_t s_cnt[256], s_cum[257];
@@ -472,6 +481,32 @@ block_encode_fused_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uin
     q.drain(out, lane);
 }
 
+template <bool BUILD, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32, WARPS <= 8 ? 5 : 1)
+block_encode_fused_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uint32_t block_size, uint16_t* __restrict__ block_freqs,
+                          uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint64_t* __restrict__ look,
+                          uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap, uint64_t* __restrict__ offsets,
+                          uint32_t* __restrict__ status)
+{
+    block_encode_fused<BUILD>(in, n_blocks, block_size, block_freqs, chunk_syms, scratch, slot_bytes, look, counter, blob, blob_cap, offsets,
+                              status);
+}
+
+// The model-building instance for rb200_container_blocks_model_encode_auto_async: runs only when the choice record
+// (CoderChoice, device_utils.cuh) names `group`; otherwise every CTA, the scanner's included, exits at entry, before it
+// touches the counter, look[] or scratch, which the host zeroes before every launch all the same.
+template <int WARPS>
+__global__ void __launch_bounds__(WARPS * 32, WARPS <= 8 ? 5 : 1)
+block_encode_fused_gated_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uint32_t block_size, uint16_t* __restrict__ block_freqs,
+                                uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint64_t* __restrict__ look,
+                                uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap, uint64_t* __restrict__ offsets,
+                                uint32_t* __restrict__ status, const CoderChoice* __restrict__ choice, uint32_t group)
+{
+    if (choice->group != group) return;                         // the same for the whole grid
+    block_encode_fused<true>(in, n_blocks, block_size, block_freqs, chunk_syms, scratch, slot_bytes, look, counter, blob, blob_cap, offsets,
+                             status);
+}
+
 inline uint32_t block_threads(uint32_t block_size, uint32_t chunk_syms)
 {
     uint32_t warps = 4;                // table construction wants a few warps even for 1-chunk blocks;
@@ -489,6 +524,11 @@ inline BlockEncodeFusedKernel block_encode_fused_for(bool build, uint32_t thread
     if (threads <= 256) return build ? block_encode_fused_kernel<true, 8> : block_encode_fused_kernel<false, 8>;
     return build ? block_encode_fused_kernel<true, 32> : block_encode_fused_kernel<false, 32>;
 }
+using BlockEncodeFusedGatedKernel = decltype(&block_encode_fused_gated_kernel<8>);
+inline BlockEncodeFusedGatedKernel block_encode_fused_gated_for(uint32_t threads)
+{
+    return threads <= 256 ? block_encode_fused_gated_kernel<8> : block_encode_fused_gated_kernel<32>;
+}
 
 inline void configure_block_kernels()
 {
@@ -503,6 +543,10 @@ inline void configure_block_kernels()
                                  cudaSharedmemCarveoutMaxShared);
             cudaFuncSetAttribute(block_encode_fused_for(build, threads), cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
         }
+    for (const uint32_t threads : {8u * 32, 32u * 32}) {
+        cudaFuncSetAttribute(block_encode_fused_gated_for(threads), cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(block_encode_fused_gated_for(threads), cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
+    }
 }
 
 inline void launch_block_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets,

@@ -27,6 +27,11 @@
 //                                  per-block ones take block ids from a counter, build the block's table in shared
 //                                  memory (version 4: the block's alias pairing first) and decode its chunks.
 // The rules are the host parser's (container_format.h); they run in its order: content errors before kStatSpace.
+//
+// rb200_container_blocks_any_decode_async runs the same stages for whichever per-block version the header names:
+// container_any_plan_kernel and container_any_verdict_kernel (the plan and verdict bodies with the header's version)
+// on the call's own workspace, and the verdict hands plan and go to the workspace of that version, whose decoders then
+// run; the other versions' decoders see go == 0 in theirs.
 #pragma once
 #include "alias_kernels.cuh"
 #include "block_coder_kernels.cuh"
@@ -92,10 +97,8 @@ __host__ __device__ constexpr uint32_t container_decoder(uint32_t version, uint3
 
 // One warp: the plan of a header that passes the rules of the call's version (a zero plan otherwise), with the verdict
 // words and the decoders' counters cleared
-__global__ void __launch_bounds__(32)
-    container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, ContainerAsyncWork* w)
+__device__ __forceinline__ void container_plan(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, ContainerAsyncWork* w)
 {
-    if (threadIdx.x) return;
     BlocksPlan p = {};
     uint32_t coder = 0, scale_bits = 0;
     if (size >= sizeof(ContainerHeader)) {                           // a shorter buffer is not read at all
@@ -128,6 +131,37 @@ __global__ void __launch_bounds__(32)
     w->wide = 0;
     w->refused = 0;
     w->work = DecodeWork{0, 0};
+}
+
+__global__ void __launch_bounds__(32)
+    container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, ContainerAsyncWork* w)
+{
+    if (threadIdx.x) return;
+    container_plan(buf, size, version, w);
+}
+
+// The per-block container of any version (rb200_container_blocks_any_decode_async) takes the call's workspace `w` for
+// its checks and hands the plan to the workspace of the header's version, whose decoders then run.  vw[0..2]: the
+// workspaces of versions 2, 3 and 4.
+struct BlocksAnyWork {
+    ContainerAsyncWork* vw[3];
+};
+
+// container_plan with the version the header names when that is 2, 3 or 4; any other version, or fewer than 64 bytes,
+// gets the zero plan.  The three version workspaces' go and decoder counters are cleared, as the plan kernel clears
+// its own: no decoder runs unless the verdict hands it this call's plan.
+__global__ void __launch_bounds__(32)
+    container_any_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, ContainerAsyncWork* w, BlocksAnyWork any)
+{
+    if (threadIdx.x) return;
+    const uint32_t version = size >= sizeof(ContainerHeader) ? reinterpret_cast<const ContainerHeader*>(buf)->version : 0u;
+    const bool per_block = version >= kContainerVersionBlocks && version <= kContainerVersionBlocksAlias;
+    container_plan(buf, per_block ? size : 0, per_block ? version : kContainerVersionBlocks, w);
+    for (ContainerAsyncWork* v : any.vw) {
+        v->go = 0;
+        v->next_block = 0;
+        v->ctas_done = 0;
+    }
 }
 
 // The per-element rules of the prefix.  Each warp stages 32 block models (16 KiB, coalesced) in shared memory with
@@ -253,9 +287,8 @@ __global__ void __launch_bounds__(kTableThreads) container_table_kernel(const ui
 // the header's CRC is taken here with container_finish_kernel's warp helpers and joined (crc32_combine).  What open
 // accepts but the decoders do not take is refused as content (kStatStream): a blob of 2^36 bytes or more and version 1's
 // chunk sizes outside 32 .. 2^24 (container_geometry_decodable), version 1's models that the table kernel refused.
-__global__ void __launch_bounds__(32)
-    container_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, ContainerAsyncWork* w,
-                             uint32_t* status, uint32_t version)
+__device__ __forceinline__ void container_verdict(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols,
+                                                  ContainerAsyncWork* w, uint32_t* status, uint32_t version)
 {
     using namespace crc_detail;
     __shared__ uint4 s_head_v[sizeof(ContainerHeader) / 16];
@@ -292,6 +325,30 @@ __global__ void __launch_bounds__(32)
         atomicOr(status, kStatSpace);
     else
         w->go = container_decoder(version, w->coder, w->scale_bits, w->wide);
+}
+
+__global__ void __launch_bounds__(32)
+    container_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, ContainerAsyncWork* w,
+                             uint32_t* status, uint32_t version)
+{
+    container_verdict(buf, out_cap, n_symbols, w, status, version);
+}
+
+// The verdict of rb200_container_blocks_any_decode_async: container_verdict for the header's version (the plan accepted
+// it, so it is 2, 3 or 4), then plan, coder, scale_bits and go handed to that version's workspace, whose decoders
+// alone can see a nonzero go (the plan kernel cleared the others')
+__global__ void __launch_bounds__(32)
+    container_any_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, ContainerAsyncWork* w,
+                                 uint32_t* status, BlocksAnyWork any)
+{
+    const uint32_t version = w->plan.ok ? reinterpret_cast<const ContainerHeader*>(buf)->version : kContainerVersionBlocks;
+    container_verdict(buf, out_cap, n_symbols, w, status, version);
+    if (threadIdx.x || !w->go) return;                           // lane 0 wrote go
+    ContainerAsyncWork* v = any.vw[version - kContainerVersionBlocks];
+    v->plan = w->plan;
+    v->coder = w->coder;
+    v->scale_bits = w->scale_bits;
+    v->go = w->go;
 }
 
 // The per-block decoder for a geometry only the device knows: a fixed grid of kPlannedWarps-warp CTAs (resident all at

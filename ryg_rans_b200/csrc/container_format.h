@@ -193,6 +193,38 @@ RB200_HD inline int choose_candidate(const uint64_t* costs, uint32_t n, uint32_t
     return -1;
 }
 
+// The per-block coder choice of rb200_choose_blocks_coder and rb200_container_blocks_model_encode_auto_async
+// (blocks_choice_kernel): C7's steps per block, summed over the blocks.  A candidate is a pair some per-block version
+// takes (container_blocks_coder_ok): word at 12, byte, rans64 or alias at 8..15.
+// the per-block version of a coder: word 2, byte and rans64 3, alias 4
+RB200_HD inline uint16_t container_blocks_version(uint32_t coder)
+{
+    return coder == RB200_CODER_WORD ? kContainerVersionBlocks : coder == RB200_CODER_ALIAS ? kContainerVersionBlocksAlias
+                                                                                         : kContainerVersionBlocksCoder;
+}
+RB200_HD inline bool blocks_candidate_ok(uint32_t c)
+{
+    const uint32_t coder = c >> 8, sb = c & 0xffu;
+    return coder <= RB200_CODER_RANS64 && container_blocks_coder_ok(container_blocks_version(coder), coder, sb);
+}
+// 1..16 valid candidates, no two alike
+inline bool blocks_candidate_list_ok(const uint32_t* c, uint32_t n)
+{
+    if (!candidate_list_ok(c, n)) return false;
+    for (uint32_t i = 0; i < n; i++)
+        if (!blocks_candidate_ok(c[i])) return false;
+    return true;
+}
+// One block's cost under a candidate: candidate_cost of the block's bits_q and chunks, except for the word coder on a
+// block of one symbol (one_symbol: a frequency of 4096), where K5's WIDE step writes a 16-bit word per symbol, so every
+// chunk is 2 x chunk_syms + 128 bytes; rule C7 counts 0 bits there.
+RB200_HD inline uint64_t blocks_candidate_cost(uint64_t bits_q, uint32_t block_size, uint32_t chunk_syms, uint32_t coder, bool one_symbol)
+{
+    const uint32_t per_block = block_size / chunk_syms;
+    if (coder == RB200_CODER_WORD && one_symbol) return 2ull * block_size + 128ull * per_block;
+    return candidate_cost(bits_q, per_block, coder);
+}
+
 // The per-element rules of a prefix, one block or one directory entry at a time.
 // one block's 256 frequencies sum to total: 1 << scale_bits (4096 in version 2)
 RB200_HD inline bool container_block_model_sums_to(const uint16_t* freqs, uint32_t total)

@@ -374,3 +374,36 @@ extern "C" int rb200_choose_coder(const uint64_t counts[256], size_t n, uint32_t
     *chosen = static_cast<uint32_t>(k);
     return RB200_OK;
 }
+
+extern "C" int rb200_choose_blocks_coder(const uint32_t* block_counts, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                         const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm, uint64_t* costs,
+                                         uint32_t* chosen)
+{
+    if (!block_counts || !chosen || !blocks_candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
+    for (uint32_t b = 0; b < n_blocks; b++) {
+        uint64_t total = 0;
+        for (int s = 0; s < 256; s++) total += block_counts[static_cast<size_t>(b) * 256 + s];
+        if (total != block_size) return RB200_E_ARG;
+    }
+    uint64_t cost[16] = {};
+    for (uint32_t b = 0; b < n_blocks; b++) {
+        const uint32_t* counts = block_counts + static_cast<size_t>(b) * 256;
+        for (uint32_t i = 0; i < n_candidates; i++) {
+            const uint32_t coder = candidates[i] >> 8, sb = candidates[i] & 0xffu;
+            uint32_t f[256], cum[257];
+            std::memcpy(f, counts, sizeof f);
+            if (rb200_normalize_freqs(f, cum, 1u << sb) != RB200_OK) return RB200_E_MODEL;   // not reached: targets >= 256
+            uint64_t bits_q = 0;
+            bool one_symbol = false;
+            for (int s = 0; s < 256; s++) {
+                bits_q += candidate_bits_q(counts[s], f[s], sb);
+                one_symbol |= f[s] == (1u << sb);
+            }
+            cost[i] += blocks_candidate_cost(bits_q, block_size, chunk_syms, coder, one_symbol);
+        }
+    }
+    if (costs) std::memcpy(costs, cost, n_candidates * sizeof(uint64_t));
+    *chosen = static_cast<uint32_t>(choose_candidate(cost, n_candidates, tolerance_ppm));   // every cost is finite
+    return RB200_OK;
+}

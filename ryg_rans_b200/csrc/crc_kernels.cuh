@@ -273,11 +273,10 @@ inline uint32_t crc32_grid(uint32_t sms, uint64_t n)
 // GEOM (rb200_container_model_encode_varlen_async, version 1): n_symbols, n_chunks and the blob offset from the record
 // (VarlenGeom); h arrives with coder, scale_bits, chunk_syms and flags.  Writes nothing when geom->go == 0.
 // CHOSEN (rb200_container_model_encode_auto_async, version 1): coder and scale_bits from the choice record.
-template <bool GEOM = false, bool CHOSEN = false>
-__global__ void __launch_bounds__(32)
-    container_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
-                            const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status,
-                            const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice)
+template <bool GEOM, bool CHOSEN>
+__device__ __forceinline__ void container_finish(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
+                                                 const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status,
+                                                 const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice)
 {
     if (GEOM) {
         if (!geom->go) return;
@@ -325,6 +324,26 @@ __global__ void __launch_bounds__(32)
     uint4* dst = reinterpret_cast<uint4*>(out);
     for (uint32_t i = lane; i < head / 16; i += 32) dst[i] = sbuf_v[i];
     if (lane == 0 && blob_off > dir_end) *reinterpret_cast<uint64_t*>(out + dir_end) = 0;   // the 8-byte pad
+}
+
+template <bool GEOM = false, bool CHOSEN = false>
+__global__ void __launch_bounds__(32)
+    container_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
+                            const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status,
+                            const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice)
+{
+    container_finish<GEOM, CHOSEN>(out, h, dir_off, blob_off, out_cap, freqs, slots, status, geom, choice);
+}
+
+// The CHOSEN per-block instance (rb200_container_blocks_model_encode_auto_async, versions 2-4): version, coder and
+// scale_bits from the choice record; the layout of the three versions is the same, so h carries the rest.
+__global__ void __launch_bounds__(32)
+    container_blocks_finish_chosen_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
+                                          const CrcSlot* __restrict__ slots, uint32_t* status, const CoderChoice* __restrict__ choice,
+                                          const uint32_t* __restrict__ version)
+{
+    h.version = static_cast<uint16_t>(*version);
+    container_finish<false, true>(out, h, dir_off, blob_off, out_cap, nullptr, slots, status, nullptr, choice);
 }
 
 }  // namespace rb200

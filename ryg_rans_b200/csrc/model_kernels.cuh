@@ -24,6 +24,12 @@
 // needs (word: both GATED instances, whose gate r32 the model kernel closes for other coders; alias/byte per SB
 // instance; rans64), each with its own directory and compaction when split, and only the recorded group runs; the
 // CHOSEN instance of container_finish_kernel writes the chosen coder and scale_bits into the header.
+//
+// rb200_container_blocks_model_encode_auto_async does the same for the per-block containers (versions 2-4):
+// blocks_choice_kernel applies the rule of rb200_choose_blocks_coder block by block and writes BlocksChoice; one gated
+// group per distinct per-block encoder instance follows (block_encode_fused_gated_kernel, block_coder_encode_gated_kernel
+// with C7's GATED scan, prefix and compaction), then the CRCs and container_blocks_finish_chosen_kernel, which writes
+// version, coder and scale_bits from the record.
 #pragma once
 #include "block_kernels.cuh"
 #include "container_format.h"
@@ -192,6 +198,75 @@ __global__ void __launch_bounds__(kMaxCandidates * 32)
         w->choice.scale_bits = list.pair[i] & 0xffu;
         w->choice.index = i;
         w->choice.group = list.group[i];
+    }
+}
+
+// The choice of rb200_container_blocks_model_encode_auto_async: the record the gated encode groups read (choice: pair,
+// index, group and every candidate's cost) and the container version the header kernel writes, with the running sums
+// of blocks_choice_kernel, which the host zeroes (one memset from `done` on) before every launch.
+struct BlocksChoice {
+    CoderChoice choice;
+    uint32_t version;
+    uint32_t done;                                // CTAs that have added their costs
+    unsigned long long sums[kMaxCandidates];      // the costs so far
+};
+
+constexpr int kBlocksChoiceWarps = 8;
+constexpr uint32_t kBlocksChoiceRowWords = 784;  // a warp's rows over the free histogram: widths, model, cumulative (16-byte aligned)
+
+// The rule of rb200_choose_blocks_coder, one CTA per block: count_freqs with the bank-private histogram
+// (block_histogram_wide, as K5f's model build), then warp w takes candidates w, w + 8: block_normalize to 1 << sb_i
+// (the device normaliser every per-block encoder uses, bit-exact), bits_q by warp reduction, and the block's cost
+// (blocks_candidate_cost) added into sums[i].  Every candidate is feasible on every block (byte at <= 15 stays below
+// 65536, a model that sums always pairs, word takes 4096 through WIDE), so there is no infeasible cost.  The last CTA
+// out applies choose_candidate and writes the record.
+__global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
+    blocks_choice_kernel(CandidateList list, const uint8_t* __restrict__ in, uint32_t block_size, uint32_t chunk_syms, BlocksChoice* r,
+                         uint32_t* __restrict__ status)
+{
+    __shared__ __align__(16) uint32_t s_hist[256 * 32];          // the histogram copies, then the warps' rows
+    __shared__ uint32_t s_cnt[256];
+    __shared__ uint64_t s_cost[kMaxCandidates];
+    __shared__ uint32_t s_last;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    block_histogram_wide(in + static_cast<uint64_t>(blockIdx.x) * block_size, block_size, s_hist, s_cnt);
+    static_assert(kBlocksChoiceWarps * kBlocksChoiceRowWords <= 256 * 32, "the rows fit the histogram's place");
+    uint32_t* s_w = s_hist + warp * kBlocksChoiceRowWords;       // 256 widths, 256 frequencies, 257 cumulative
+    uint32_t* s_f = s_w + 256;
+    uint32_t* s_cum = s_w + 512;
+    for (uint32_t i = warp; i < list.n; i += kBlocksChoiceWarps) {
+        const uint32_t coder = list.pair[i] >> 8, sb = list.pair[i] & 0xffu;
+        block_normalize(s_cnt, s_cum, s_w, s_f, 1u << sb, kStatStream, status);
+        __syncwarp();
+        uint64_t bits_q = 0;
+        bool one_symbol = false;
+        for (uint32_t s = lane; s < 256; s += 32) {
+            bits_q += candidate_bits_q(s_cnt[s], s_f[s], sb);
+            one_symbol |= s_f[s] == (1u << sb);
+        }
+        for (int d = 16; d; d >>= 1) bits_q += __shfl_xor_sync(0xffffffffu, bits_q, d);
+        one_symbol = __any_sync(0xffffffffu, one_symbol);
+        if (lane == 0) atomicAdd(&r->sums[i], static_cast<unsigned long long>(blocks_candidate_cost(bits_q, block_size, chunk_syms, coder, one_symbol)));
+        __syncwarp();
+    }
+    __syncthreads();
+    if (tid == 0) {
+        __threadfence();                                         // this CTA's sums before its count
+        s_last = atomicAdd(&r->done, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    if (tid < list.n) s_cost[tid] = r->choice.costs[tid] = __ldcg(&r->sums[tid]);
+    __syncthreads();
+    if (tid == 0) {
+        const int k = choose_candidate(s_cost, list.n, list.tolerance_ppm);   // every cost is finite: k >= 0
+        const uint32_t i = k < 0 ? 0u : static_cast<uint32_t>(k);
+        r->choice.coder = list.pair[i] >> 8;
+        r->choice.scale_bits = list.pair[i] & 0xffu;
+        r->choice.index = i;
+        r->choice.group = list.group[i];
+        r->version = container_blocks_version(r->choice.coder);
     }
 }
 

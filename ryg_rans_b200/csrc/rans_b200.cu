@@ -68,8 +68,12 @@ struct rb200_ctx {
     // versions never share state, and every version's decoder launches
     ContainerAsyncWork* d_async[4] = {};
     DecoderLaunch async_decoders[kContainerDecoders] = {};
+    // rb200_container_blocks_any_decode_async: the checks' own workspace; its decoders run on d_async[1..3]
+    ContainerAsyncWork* d_async_any = nullptr;
     // rb200_container_model_encode_async (model_kernels.cuh): the counts, the model and its encode tables
     ModelAsyncWork* d_model_async = nullptr;
+    // rb200_container_blocks_model_encode_auto_async (model_kernels.cuh): the choice record and its running sums
+    BlocksChoice* d_blocks_choice = nullptr;
 };
 
 struct rb200_model {
@@ -235,6 +239,10 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     }
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_model_async, sizeof(ModelAsyncWork));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_model_async, 0, sizeof(ModelAsyncWork));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_async_any, sizeof(ContainerAsyncWork));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_async_any, 0, sizeof(ContainerAsyncWork));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_blocks_choice, sizeof(BlocksChoice));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_choice, 0, sizeof(BlocksChoice));
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -271,6 +279,8 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     for (ContainerAsyncWork* w : ctx->d_async)
         if (w) cudaFree(w);
     if (ctx->d_model_async) cudaFree(ctx->d_model_async);
+    if (ctx->d_async_any) cudaFree(ctx->d_async_any);
+    if (ctx->d_blocks_choice) cudaFree(ctx->d_blocks_choice);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -1811,6 +1821,47 @@ extern "C" int rb200_container_blocks_alias_decode_async(rb200_ctx* ctx, const u
     return container_decode_async(ctx, kContainerVersionBlocksAlias, buf, size, out, out_cap, d_n_symbols);
 }
 
+// Thirteen launches: the any plan, both CRCs and the prefix check on the call's own workspace, the any verdict, then
+// the decoders of versions 2, 3 and 4 (1 + 4 + 3), each on its own version's workspace.  Only the header version's
+// workspace can hold a nonzero go, so the version-local decoder ids, which overlap across versions, never collide.
+extern "C" int rb200_container_blocks_any_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                                       uint64_t* d_n_symbols)
+{
+    if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    ContainerAsyncWork* w = ctx->d_async_any;
+    const BlocksAnyWork any = {{ctx->d_async[kContainerVersionBlocks - 1], ctx->d_async[kContainerVersionBlocksCoder - 1],
+                                ctx->d_async[kContainerVersionBlocksAlias - 1]}};
+    const uint32_t sms = static_cast<uint32_t>(ctx->sms);
+    const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
+    cudaStream_t s = ctx->stream;
+    container_any_plan_kernel<<<1, 32, 0, s>>>(buf, size, w, any);
+    int rc = check_launch(ctx, "container_any_plan_kernel");
+    if (rc != RB200_OK) return rc;
+    crc32_kernel<<<crc32_grid(sms, after_head), kCrcThreads, kCrcSmemBytes, s>>>(buf + sizeof(ContainerHeader), after_head, &w->plan.meta_len,
+                                                                                 nullptr, 0, &w->crc_work, &w->crc[0]);
+    rc = check_launch(ctx, "crc32_kernel(meta)");
+    if (rc != RB200_OK) return rc;
+    crc32_kernel<<<crc32_grid(sms, size), kCrcThreads, kCrcSmemBytes, s>>>(buf, size, &w->plan.blob_len, &w->plan.blob_off, 0,
+                                                                           &w->crc_work, &w->crc[1]);
+    rc = check_launch(ctx, "crc32_kernel(blob)");
+    if (rc != RB200_OK) return rc;
+    container_prefix_check_kernel<<<sms * kPrefixCtasPerSm, kPrefixWarps * 32, 0, s>>>(buf, w);
+    rc = check_launch(ctx, "container_prefix_check_kernel");
+    if (rc != RB200_OK) return rc;
+    container_any_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status, any);
+    rc = check_launch(ctx, "container_any_verdict_kernel");
+    for (int i = kDecoderFirst[kContainerVersionBlocks - 1]; i < kDecoderFirst[kContainerVersionBlocksAlias] && rc == RB200_OK; i++) {
+        const DecoderLaunch& l = ctx->async_decoders[i];
+        const int version = i < kDecoderFirst[kContainerVersionBlocks] ? kContainerVersionBlocks
+                            : i < kDecoderFirst[kContainerVersionBlocksCoder] ? kContainerVersionBlocksCoder
+                                                                              : kContainerVersionBlocksAlias;
+        l.kernel<<<l.grid, l.threads, l.smem, s>>>(buf, out, ctx->d_async[version - 1], ctx->d_status);
+        rc = check_launch(ctx, l.name);
+    }
+    return rc;
+}
+
 namespace {
 
 // the argument rules of both model encodes, with n the length (fixed call) or its bound n_max (varlen call)
@@ -1977,6 +2028,79 @@ extern "C" int rb200_container_model_encode_auto_async(rb200_ctx* ctx, const uin
     if (!d_n && n == 0) return RB200_E_MODEL;                        // normalize_freqs divides by the total
     const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
     return model_encode(ctx, static_cast<int>(candidates[0] >> 8), candidates[0] & 0xffu, in, n, d_n, chunk_syms, flags, out, out_cap, &a);
+}
+
+namespace {
+
+// The per-block encode of one launch group of an auto encode, with models built: the gated K5f instance (word), or the
+// gated K5c instance of the group's dispatch followed by the GATED tile scan, prefix and compaction (byte, rans64,
+// alias).  The plan is the fixed model-building call's for the group's coder and largest scale_bits.
+int blocks_encode_gated(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* d_in, uint32_t n_blocks, uint32_t block_size,
+                        uint16_t* d_freqs, uint32_t chunk_syms, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets,
+                        const CoderChoice* choice, uint32_t group)
+{
+    const EncodePlan p = plan_blocks_encode(ctx, coder, sb, n_blocks, block_size, chunk_syms, true);
+    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, nullptr, [&](const EncodeWorkspace& ws) {
+        if (coder != RB200_CODER_WORD) {
+            launch_block_coder_encode_gated(ctx->stream, static_cast<uint32_t>(coder), sb, p.grid, p.threads, p.smem, d_in, block_size, d_freqs,
+                                            chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status, choice, group);
+            return check_launch(ctx, "block_coder_encode_gated_kernel");
+        }
+        block_encode_fused_gated_for(p.threads)<<<p.grid, p.threads, p.smem, ctx->stream>>>(
+            d_in, n_blocks, block_size, d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.look, ws.counter, d_blob, blob_cap, d_offsets,
+            ctx->d_status, choice, group);
+        return check_launch(ctx, "block_encode_fused_gated_kernel");
+    }, choice, group);
+}
+
+}  // namespace
+
+// rb200_container_blocks_encode / _coder_encode / _alias_encode (DEVICE, models built) with the pair chosen on the GPU
+// at every run: the choice kernel (after a memset of its sums), one gated encode group per distinct encoder instance
+// of the list, the model + directory CRC, the optional blob CRC, the CHOSEN per-block header kernel.  The layout of
+// versions 2-4 is the same, so the host lays the container out without knowing the choice.
+extern "C" int rb200_container_blocks_model_encode_auto_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                              uint32_t tolerance_ppm, const uint8_t* in, uint32_t n_blocks,
+                                                              uint32_t block_size, uint32_t chunk_syms, uint32_t flags, uint8_t* out,
+                                                              size_t out_cap)
+{
+    if (!ctx || !in || !out || !blocks_candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms) || !container_mem_ok(RB200_MEM_DEVICE, out, nullptr)) return RB200_E_ARG;
+    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
+    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    const ContainerHeader h = container_blocks_header(n_blocks, block_size, chunk_syms, 0, flags);
+    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
+    if (out_cap < boff) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
+    int rc = RB200_OK;
+    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++)    // every group's workspace before the first launch
+        rc = reserve_plan(ctx, plan_blocks_encode(ctx, a.coder[k], a.sb[k], n_blocks, block_size, chunk_syms, true));
+    if (rc != RB200_OK) return rc;
+    cudaStream_t s = ctx->stream;
+    BlocksChoice* r = ctx->d_blocks_choice;
+    RB_CUDA(ctx, cudaMemsetAsync(&r->done, 0, sizeof(BlocksChoice) - offsetof(BlocksChoice, done), s));
+    blocks_choice_kernel<<<n_blocks, kBlocksChoiceWarps * 32, 0, s>>>(a.list, in, block_size, chunk_syms, r, ctx->d_status);
+    rc = check_launch(ctx, "blocks_choice_kernel");
+    uint16_t* model = reinterpret_cast<uint16_t*>(out + sizeof(ContainerHeader));
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
+    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++)
+        rc = blocks_encode_gated(ctx, a.coder[k], a.sb[k], in, n_blocks, block_size, model, chunk_syms, out + boff, out_cap - boff, dir,
+                                 &r->choice, k);
+    if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), nullptr, 0, ctx->d_crc);
+    if (rc == RB200_OK && (h.flags & RB200_CONTAINER_CRC_BLOB)) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+    if (rc != RB200_OK) return rc;
+    container_blocks_finish_chosen_kernel<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, ctx->d_crc, ctx->d_status, &r->choice, &r->version);
+    return check_launch(ctx, "container_blocks_finish_chosen_kernel");
+}
+
+extern "C" int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n)
+{
+    if (!ctx || !costs || n > kMaxCandidates) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    RB_CUDA(ctx, cudaMemcpyAsync(costs, ctx->d_blocks_choice->choice.costs, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    RB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return RB200_OK;
 }
 
 // ---------------------------------------------------------------------------

@@ -60,9 +60,17 @@ uniform bytes and of p = 0.99 data (symbol 0, a Zipf-1.1 tail over the rest), ch
 for the pair it chose, flags 0 and RB200_CONTAINER_CRC_BLOB, alternated; the costs, the bytes per symbol against the
 word coder's; and a torch.profiler list of the auto call's kernels (the choice kernel, the gated-out launches).
 
+With --blocks-auto, rb200_container_blocks_model_encode_auto_async over {word 12, byte 14, alias 14} with a 2 %
+tolerance on the --blocks-coder workloads (8192 blocks of 64 KiB, chunks of 8192, "skewed" and "zipf"): against the
+fixed model-building container call for the pair it chose, flags 0 and RB200_CONTAINER_CRC_BLOB, alternated; the
+device costs against rb200_choose_blocks_coder's; every candidate's blob in bytes per symbol; a torch.profiler list of
+the auto call's kernels and the fixed call's; and rb200_container_blocks_any_decode_async against the chosen version's
+own async decode, alternated, with its kernel list.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
-    python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto] [--reps 10]
+    python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto | --blocks-auto]
+                                     [--reps 10]
                                      [--json out.json]"""
 import argparse
 import json
@@ -757,6 +765,95 @@ def auto_encode(args):
     return res
 
 
+def blocks_auto(args):
+    """rb200_container_blocks_model_encode_auto_async over {word 12, byte 14, alias 14} (2 % tolerance) against the fixed
+    model-building call for the pair it chose, on the --blocks-coder workloads; every candidate's bytes per symbol; a
+    kernel split of the auto call; rb200_container_blocks_any_decode_async against the version's own async decode"""
+    import torch
+    n_blocks, block_size, chunk, tol = 8192, 65536, 8192, 20000
+    n = n_blocks * block_size
+    W, B, A = rb.CODER_WORD, rb.CODER_BYTE, rb.CODER_ALIAS
+    cands = [api.CANDIDATE(W, 12), api.CANDIDATE(B, 14), api.CANDIDATE(A, 14)]
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    crc = api.CONTAINER_CRC_BLOB
+    cap = ctx.container_blocks_capacity(n_blocks, block_size, chunk)
+    d_ref = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_out = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_dec = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+    res = {"card": card(), "workload": {"n_blocks": n_blocks, "block_size": block_size, "chunk_syms": chunk, "n": n},
+           "candidates": ["word 12", "byte 14", "alias 14"], "tolerance_ppm": tol, "workloads": {}, "checks": {}}
+
+    def fixed(coder, sb, i, o, flags):
+        if coder == W:
+            return lambda: ctx.container_blocks_encode_device(i, n_blocks, block_size, None, chunk, flags, o, cap)
+        if coder == A:
+            return lambda: ctx.container_blocks_alias_encode_device(sb, i, n_blocks, block_size, None, chunk, flags, o, cap)
+        return lambda: ctx.container_blocks_coder_encode_device(coder, sb, i, n_blocks, block_size, None, chunk, flags, o, cap)
+
+    def head(d):
+        h = d[:64].cpu().numpy()
+        return int(h[4:6].view(np.uint16)[0]), int(h[6]), int(h[7]), int(h[32:40].view(np.uint64)[0])
+
+    boff = (64 + 512 * n_blocks + 8 * (n // chunk + 1) + 15) & ~15
+    for name, make in (("skewed", skewed_blocks_data), ("zipf", blocks_data)):
+        d_in = make(n_blocks, block_size, 4321)
+        i, r, o = d_in.data_ptr(), d_ref.data_ptr(), d_out.data_ptr()
+        ctx.container_blocks_model_encode_auto_async(cands, tol, i, n_blocks, block_size, chunk, 0, o, cap)
+        sync()
+        version, coder, sb, blob_auto = head(d_out)
+        costs = [int(c) for c in ctx.container_blocks_auto_costs(len(cands))]
+        counts = torch.stack([torch.bincount(d_in[b * block_size:(b + 1) * block_size].long(), minlength=256) for b in range(n_blocks)])
+        k, host_costs = api.choose_blocks_coder(counts.cpu().numpy().astype(np.uint32), block_size, chunk, cands, tol)
+        res["checks"][f"{name}: choice_and_costs_are_the_host_rule's"] = cands[k] == api.CANDIDATE(coder, sb) and costs == [int(c) for c in host_costs]
+        calls = {}
+        for tag, flags in (("", 0), ("_crc", crc)):
+            calls["auto" + tag] = lambda flags=flags: ctx.container_blocks_model_encode_auto_async(cands, tol, i, n_blocks, block_size, chunk,
+                                                                                                  flags, o, cap)
+            calls["fixed_chosen" + tag] = fixed(coder, sb, i, r, flags)
+        times = alternate(calls, sync, args.warmup, args.reps)
+        for tag in ("", "_crc"):
+            calls["auto" + tag]()
+            calls["fixed_chosen" + tag]()
+            sync()
+            size = boff + head(d_out)[3]
+            res["checks"][f"{name}: auto{tag}_equals_fixed_call"] = bool(torch.equal(d_out[:size], d_ref[:size]))
+        per_candidate = {}
+        for c, cost in zip(cands, costs):
+            fixed(c >> 8, c & 0xFF, i, r, 0)()
+            sync()
+            per_candidate[f"{c >> 8}/{c & 0xFF}"] = {"bytes_per_symbol": head(d_ref)[3] / n, "cost_per_symbol": cost / n}
+        kernels = kernel_times(calls["auto_crc"], sync, args.reps)
+        kernels_fixed = kernel_times(calls["fixed_chosen_crc"], sync, args.reps)
+        # decode: the container of the chosen version, by the any call and by the version's own async decode
+        calls["auto_crc"]()
+        sync()
+        own = {2: ctx.container_blocks_decode_async, 3: ctx.container_blocks_coder_decode_async, 4: ctx.container_blocks_alias_decode_async}[version]
+        dec = {"any_decode_async": lambda: ctx.container_blocks_any_decode_async(o, cap, d_dec.data_ptr(), n),
+               "own_decode_async": lambda: own(o, cap, d_dec.data_ptr(), n)}
+        dtimes = alternate(dec, sync, args.warmup, args.reps)
+        for k, f in dec.items():
+            d_dec.zero_()
+            f()
+            sync()
+            res["checks"][f"{name}: {k}_round_trip"] = bool(torch.equal(d_dec[:n], d_in[:n]))
+        dkernels = kernel_times(dec["any_decode_async"], sync, args.reps)
+        res["workloads"][name] = {
+            "chosen": {"version": version, "coder": coder, "scale_bits": sb}, "costs": costs,
+            "bytes_per_symbol": blob_auto / n, "candidates": per_candidate,
+            "encode": times,
+            "auto_minus_fixed_median_us": {tag or "flags 0": 1e3 * (times["auto" + tag]["median_ms"] - times["fixed_chosen" + tag]["median_ms"])
+                                           for tag in ("", "_crc")},
+            "auto_crc_kernels": kernels, "fixed_chosen_crc_kernels": kernels_fixed,
+            "decode": dtimes,
+            "any_minus_own_median_us": 1e3 * (dtimes["any_decode_async"]["median_ms"] - dtimes["own_decode_async"]["median_ms"]),
+            "any_decode_kernels": dkernels,
+        }
+        del d_in
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
@@ -765,13 +862,14 @@ def main():
     ap.add_argument("--single", action="store_true", help="the single-model container's decode calls on three workloads")
     ap.add_argument("--model", action="store_true", help="the single-model container's encode with the model built from the data")
     ap.add_argument("--auto", action="store_true", help="the model-building encode with the coder chosen on the GPU")
+    ap.add_argument("--blocks-auto", action="store_true", help="the per-block model-building encode with the coder chosen on the GPU")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
