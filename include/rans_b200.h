@@ -461,6 +461,26 @@ int rb200_container_blocks_model_encode_auto_async(rb200_ctx* ctx, const uint32_
                                                    size_t out_cap);
 int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n);
 
+/* rb200_container_blocks_model_encode_auto_async with the block count read from device memory when the work runs: for
+ * 1 <= *d_n_blocks <= n_blocks_max the container is byte for byte what the fixed call writes for n_blocks =
+ * *d_n_blocks, so one captured graph takes any count up to n_blocks_max.  Only the first *d_n_blocks blocks of in are
+ * read and nothing past the container's end is written.  n_blocks_max fixes the launch shapes and the workspace, and the
+ * host checks it: the geometry, fewer than 2^31 chunks, and out_cap at least its blob offset (RB200_E_SPACE below it);
+ * the layout offsets and the encode bound grow with the count, so rb200_container_blocks_size for n_blocks_max holds
+ * every smaller count.  RB200_E_ARG (nothing launched) also for a null, or not 4-byte aligned, d_n_blocks and for
+ * n_blocks_max == 0.  rb200_sync returns RB200_E_ARG when *d_n_blocks is 0 or above n_blocks_max (zero blocks is the
+ * fixed call's RB200_E_ARG too), and then out is not written at all; the other verdicts are the fixed call's.  The call
+ * only enqueues work: the plan kernel, the choice kernel on a grid of n_blocks_max (its CTAs past the count exit), one
+ * gated encode group per distinct encoder instance, the CRCs and the header kernel.  With one candidate the pair is
+ * known, so the choice kernel is not launched: the plan kernel writes the choice, and rb200_container_blocks_auto_costs
+ * is then undefined (it reads the costs of the last call that ran the choice kernel, one with two or more candidates).
+ * The workspace grows for every group's plan at n_blocks_max, so a call with the same list and bounds outside a
+ * capture must come first. */
+int rb200_container_blocks_model_encode_varlen_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                     uint32_t tolerance_ppm, const uint8_t* in, const uint32_t* d_n_blocks,
+                                                     uint32_t n_blocks_max, uint32_t block_size, uint32_t chunk_syms, uint32_t flags,
+                                                     uint8_t* out, size_t out_cap);
+
 /* The async decode of a per-block container of any version: the header's version field (bytes 4-5) picks version 2, 3
  * or 4, and the call then reaches the verdict, status and output of rb200_container_blocks_decode_async,
  * rb200_container_blocks_coder_decode_async or rb200_container_blocks_alias_decode_async on it, under the same rules

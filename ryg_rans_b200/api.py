@@ -93,6 +93,8 @@ EXPORTS = [
     ("rb200_container_blocks_model_encode_auto_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
                                                                  C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_container_blocks_auto_costs", C.c_int, [C.c_void_p, _u64p, C.c_uint32]),
+    ("rb200_container_blocks_model_encode_varlen_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                                   C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_container_blocks_any_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
@@ -771,6 +773,19 @@ class Context:
         self.lib.check(self.lib.dll.rb200_container_blocks_model_encode_auto_async(self.h, cands.ctypes.data_as(_u32p), cands.size,
                                                                                    tolerance_ppm, in_ptr, n_blocks, block_size, chunk_syms,
                                                                                    flags, out_ptr, out_cap), self.h)
+
+    def container_blocks_model_encode_varlen_async(self, candidates, tolerance_ppm, in_ptr, n_blocks_ptr, n_blocks_max, block_size, chunk_syms,
+                                                   flags, out_ptr, out_cap):
+        """container_blocks_model_encode_auto_async with the block count read from device memory when the work runs:
+        n_blocks_ptr is the device address of a u32 count, 1 <= count <= n_blocks_max.  n_blocks_max fixes the launch
+        shapes and the workspace, so one captured call serves every such count; out_cap =
+        container_blocks_capacity(n_blocks_max, ...) holds every one.  With one candidate no choice kernel runs and
+        container_blocks_auto_costs is undefined after it.  The verdict (-1 for a count of 0 or above n_blocks_max, with
+        out untouched; otherwise as the fixed call) comes from sync()"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_blocks_model_encode_varlen_async(self.h, cands.ctypes.data_as(_u32p), cands.size,
+                                                                                     tolerance_ppm, in_ptr, n_blocks_ptr, n_blocks_max,
+                                                                                     block_size, chunk_syms, flags, out_ptr, out_cap), self.h)
 
     def container_blocks_auto_costs(self, n):
         """the n candidate costs of the last container_blocks_model_encode_auto_async run (synchronises)"""

@@ -263,6 +263,18 @@ block_coder_encode_gated_kernel(const uint8_t* __restrict__ in, uint32_t block_s
     block_coder_encode<CODER, SB, true>(in, block_size, block_freqs, choice->scale_bits, chunk_syms, scratch, slot_bytes, sizes, status);
 }
 
+// The same for rb200_container_blocks_model_encode_varlen_async, on the grid of n_blocks_max: the CTAs at or past the
+// record's count (BlocksVarlenGeom) exit at entry, as every CTA does when the plan failed (the count is then 0)
+template <uint32_t CODER, uint32_t SB>
+__global__ void __launch_bounds__(kMaxBlockWarps * 32)
+block_coder_encode_varlen_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t chunk_syms,
+                                 uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status,
+                                 const CoderChoice* __restrict__ choice, uint32_t group, const BlocksVarlenGeom* __restrict__ geom)
+{
+    if (choice->group != group || blockIdx.x >= geom->n_blocks) return;     // the group is the same for the whole grid
+    block_coder_encode<CODER, SB, true>(in, block_size, block_freqs, choice->scale_bits, chunk_syms, scratch, slot_bytes, sizes, status);
+}
+
 // A block's decode table in shared memory at s_tab, from its cumulative frequencies (s_cum[257], M = 1 << sb): cum2sym[M],
 // then the symbol entries.  Every thread of the CTA takes part; the caller synchronises before the table is read.
 template <uint32_t CODER>
@@ -407,7 +419,8 @@ inline void configure_block_coder()
 {
     for (const void* k : {reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, true>),
                           reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, false>),
-                          reinterpret_cast<const void*>(block_coder_encode_gated_kernel<CODER, SB>)}) {
+                          reinterpret_cast<const void*>(block_coder_encode_gated_kernel<CODER, SB>),
+                          reinterpret_cast<const void*>(block_coder_encode_varlen_kernel<CODER, SB>)}) {
         cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              block_coder_encode_smem(CODER, kBlockCoderMaxScaleBits, kMaxBlockWarps * 32));
@@ -445,6 +458,17 @@ inline void launch_block_coder_encode_gated(cudaStream_t stream, uint32_t coder,
 {
     RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, (block_coder_encode_gated_kernel<CODER, SB><<<n_blocks, threads, smem, stream>>>(
                                               d_in, block_size, d_freqs, chunk_syms, scratch, slot_bytes, sizes, status, choice, group)))
+}
+
+// the varlen instance of (coder, sb)'s dispatch (rb200_container_blocks_model_encode_varlen_async): as the gated one,
+// on a grid of n_blocks_max CTAs
+inline void launch_block_coder_encode_varlen(cudaStream_t stream, uint32_t coder, uint32_t sb, uint32_t n_blocks_max, uint32_t threads,
+                                             uint32_t smem, const uint8_t* d_in, uint32_t block_size, uint16_t* d_freqs, uint32_t chunk_syms,
+                                             uint8_t* scratch, uint32_t slot_bytes, uint32_t* sizes, uint32_t* status, const CoderChoice* choice,
+                                             uint32_t group, const BlocksVarlenGeom* geom)
+{
+    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, (block_coder_encode_varlen_kernel<CODER, SB><<<n_blocks_max, threads, smem, stream>>>(
+                                              d_in, block_size, d_freqs, chunk_syms, scratch, slot_bytes, sizes, status, choice, group, geom)))
 }
 
 inline void launch_block_coder_decode(cudaStream_t stream, uint32_t coder, uint32_t sb, const uint8_t* blob, uint64_t blob_size,

@@ -507,6 +507,28 @@ block_encode_fused_gated_kernel(const uint8_t* __restrict__ in, uint32_t n_block
                              status);
 }
 
+// The model-building instance for rb200_container_blocks_model_encode_varlen_async: gated as the one above, on the
+// grid the host plans for n_blocks_max, with the block count from the record (BlocksVarlenGeom).  The body takes the
+// count as an argument, so the scanner warp follows the record's chunks and workers past the count find no block and
+// drain.  The directory and the blob's place in the container `out` are worked out here from the count and the
+// parameters (per_block = block_size / chunk_syms), as the plan kernel lays them out, rather than read from the
+// record: values this cheap to derive from one register are recomputed where they are used instead of held, which
+// keeps the 8-warp instance at the spill of the shipped one whose body it runs.
+template <int WARPS>
+__global__ void __launch_bounds__(WARPS * 32, WARPS <= 8 ? 5 : 1)
+block_encode_fused_varlen_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t chunk_syms,
+                                 uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint64_t* __restrict__ look, uint32_t* __restrict__ counter,
+                                 uint8_t* __restrict__ out, uint64_t out_cap, uint32_t per_block, uint32_t* __restrict__ status,
+                                 const CoderChoice* __restrict__ choice, uint32_t group, const BlocksVarlenGeom* __restrict__ geom)
+{
+    const uint32_t n_blocks = geom->n_blocks;                   // 0 when the plan failed
+    if (!n_blocks || choice->group != group) return;            // the same for the whole grid
+    const uint64_t entries = static_cast<uint64_t>(n_blocks) * per_block + 1;     // the directory's
+    const uint64_t dir_off = 64 + 512ull * n_blocks, blob_off = dir_off + ((entries + 1) >> 1) * 16;
+    block_encode_fused<true>(in, n_blocks, block_size, block_freqs, chunk_syms, scratch, slot_bytes, look, counter, out + blob_off,
+                             out_cap - blob_off, reinterpret_cast<uint64_t*>(out + dir_off), status);
+}
+
 inline uint32_t block_threads(uint32_t block_size, uint32_t chunk_syms)
 {
     uint32_t warps = 4;                // table construction wants a few warps even for 1-chunk blocks;
@@ -529,6 +551,11 @@ inline BlockEncodeFusedGatedKernel block_encode_fused_gated_for(uint32_t threads
 {
     return threads <= 256 ? block_encode_fused_gated_kernel<8> : block_encode_fused_gated_kernel<32>;
 }
+using BlockEncodeFusedVarlenKernel = decltype(&block_encode_fused_varlen_kernel<8>);
+inline BlockEncodeFusedVarlenKernel block_encode_fused_varlen_for(uint32_t threads)
+{
+    return threads <= 256 ? block_encode_fused_varlen_kernel<8> : block_encode_fused_varlen_kernel<32>;
+}
 
 inline void configure_block_kernels()
 {
@@ -546,6 +573,8 @@ inline void configure_block_kernels()
     for (const uint32_t threads : {8u * 32, 32u * 32}) {
         cudaFuncSetAttribute(block_encode_fused_gated_for(threads), cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(block_encode_fused_gated_for(threads), cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
+        cudaFuncSetAttribute(block_encode_fused_varlen_for(threads), cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(block_encode_fused_varlen_for(threads), cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
     }
 }
 

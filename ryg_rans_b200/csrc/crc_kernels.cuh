@@ -346,4 +346,20 @@ __global__ void __launch_bounds__(32)
     container_finish<false, true>(out, h, dir_off, blob_off, out_cap, nullptr, slots, status, nullptr, choice);
 }
 
+// The same for rb200_container_blocks_model_encode_varlen_async: n_blocks, n_symbols, n_chunks, the directory and the
+// blob offset from the record (BlocksVarlenGeom); h arrives with block_size, chunk_syms and flags.  Writes nothing when
+// geom->v.go == 0.
+__global__ void __launch_bounds__(32)
+    container_blocks_finish_varlen_kernel(uint8_t* out, ContainerHeader h, uint64_t out_cap, const CrcSlot* __restrict__ slots, uint32_t* status,
+                                          const CoderChoice* __restrict__ choice, const uint32_t* __restrict__ version,
+                                          const BlocksVarlenGeom* __restrict__ geom)
+{
+    if (!geom->v.go) return;
+    h.version = static_cast<uint16_t>(*version);
+    h.n_blocks = geom->n_blocks;
+    h.n_symbols = geom->v.n;
+    h.n_chunks = geom->v.n_chunks;
+    container_finish<false, true>(out, h, geom->dir_off, geom->v.blob_off, out_cap, nullptr, slots, status, nullptr, choice);
+}
+
 }  // namespace rb200

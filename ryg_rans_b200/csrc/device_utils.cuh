@@ -29,6 +29,18 @@ struct VarlenGeom {
     uint32_t go;           // 1: *d_n passed the checks; 0: nothing after the plan runs (dir_len, blob_off, blob_len are 0)
 };
 
+// The geometry of rb200_container_blocks_model_encode_varlen_async, which reads the block count from device memory:
+// written by blocks_varlen_plan_kernel (model_kernels.cuh) from *d_n_blocks at every run.  v is the VarlenGeom of the
+// container's symbols and chunks (n = n_blocks x block_size), so the GEOM instances of C5 read it as they are; the
+// directory, which sits after the n_blocks models and so moves with the count, and the meta CRC's length follow it.
+struct BlocksVarlenGeom {
+    VarlenGeom v;          // v.blob_off = round16(dir_off + v.dir_len)
+    uint64_t dir_off;      // 64 + 512 n_blocks
+    uint64_t meta_len;     // 512 n_blocks + v.dir_len: models and directory, the bytes the meta CRC's kernel covers
+    uint32_t n_blocks;     // 1 <= n_blocks <= n_blocks_max; 0 when v.go == 0
+    uint32_t reserved;
+};
+
 // The choice of rb200_container_model_encode_auto_async: written by coder_choice_kernel (model_kernels.cuh) at every
 // run, read by the CHOSEN / GATED instances after it.  The host launches one gated group of encode kernels per distinct
 // encoder instance the candidate list needs; only the group named here runs, the others exit at entry.

@@ -30,6 +30,11 @@
 // group per distinct per-block encoder instance follows (block_encode_fused_gated_kernel, block_coder_encode_gated_kernel
 // with C7's GATED scan, prefix and compaction), then the CRCs and container_blocks_finish_chosen_kernel, which writes
 // version, coder and scale_bits from the record.
+//
+// rb200_container_blocks_model_encode_varlen_async runs those stages on launch shapes sized for n_blocks_max:
+// blocks_varlen_plan_kernel reads *d_n_blocks into BlocksVarlenGeom (device_utils.cuh), and the choice kernel, the
+// encoders, the scan and compaction and the header kernel are varlen instances around the same bodies, which take the
+// count, the directory's place (after the count's models) and the blob's from it.
 #pragma once
 #include "block_kernels.cuh"
 #include "container_format.h"
@@ -220,10 +225,14 @@ constexpr uint32_t kBlocksChoiceRowWords = 784;  // a warp's rows over the free 
 // (blocks_candidate_cost) added into sums[i].  Every candidate is feasible on every block (byte at <= 15 stays below
 // 65536, a model that sums always pairs, word takes 4096 through WIDE), so there is no infeasible cost.  The last CTA
 // out applies choose_candidate and writes the record.
-__global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
-    blocks_choice_kernel(CandidateList list, const uint8_t* __restrict__ in, uint32_t block_size, uint32_t chunk_syms, BlocksChoice* r,
-                         uint32_t* __restrict__ status)
+// GEOM (rb200_container_blocks_model_encode_varlen_async): the block count from the record (BlocksVarlenGeom), on the
+// grid of n_blocks_max; the CTAs at or past it exit at entry, before they count, so the last of the device count's CTAs
+// is the last out (none runs when the plan failed: n_blocks is then 0).
+template <bool GEOM>
+__device__ __forceinline__ void blocks_choice(CandidateList list, const uint8_t* __restrict__ in, uint32_t block_size, uint32_t chunk_syms,
+                                              BlocksChoice* r, uint32_t* __restrict__ status, const BlocksVarlenGeom* __restrict__ geom)
 {
+    if (GEOM && blockIdx.x >= geom->n_blocks) return;            // the same for the whole CTA
     __shared__ __align__(16) uint32_t s_hist[256 * 32];          // the histogram copies, then the warps' rows
     __shared__ uint32_t s_cnt[256];
     __shared__ uint64_t s_cost[kMaxCandidates];
@@ -252,7 +261,7 @@ __global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
     __syncthreads();
     if (tid == 0) {
         __threadfence();                                         // this CTA's sums before its count
-        s_last = atomicAdd(&r->done, 1u) == gridDim.x - 1;
+        s_last = atomicAdd(&r->done, 1u) == (GEOM ? geom->n_blocks : gridDim.x) - 1;
     }
     __syncthreads();
     if (!s_last) return;
@@ -268,6 +277,20 @@ __global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
         r->choice.group = list.group[i];
         r->version = container_blocks_version(r->choice.coder);
     }
+}
+
+__global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
+    blocks_choice_kernel(CandidateList list, const uint8_t* __restrict__ in, uint32_t block_size, uint32_t chunk_syms, BlocksChoice* r,
+                         uint32_t* __restrict__ status)
+{
+    blocks_choice<false>(list, in, block_size, chunk_syms, r, status, nullptr);
+}
+
+__global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
+    blocks_choice_geom_kernel(CandidateList list, const uint8_t* __restrict__ in, uint32_t block_size, uint32_t chunk_syms, BlocksChoice* r,
+                              uint32_t* __restrict__ status, const BlocksVarlenGeom* __restrict__ geom)
+{
+    blocks_choice<true>(list, in, block_size, chunk_syms, r, status, geom);
 }
 
 // The first kernel of rb200_container_model_encode_varlen_async, one warp: reads n = *d_n, checks 1 <= n <= n_max
@@ -300,6 +323,52 @@ __global__ void __launch_bounds__(32)
 __global__ void __launch_bounds__(32) varlen_blob_len_kernel(const uint64_t* __restrict__ dir, VarlenGeom* __restrict__ g)
 {
     if (threadIdx.x == 0 && g->go) g->blob_len = dir[g->n_chunks];
+}
+
+// The first kernel of rb200_container_blocks_model_encode_varlen_async, one warp: reads n_blocks = *d_n_blocks, checks
+// 1 <= n_blocks <= n_blocks_max (both failures are kStatArg: zero blocks is the fixed call's RB200_E_ARG) and writes the
+// geometry of a per-block container of n_blocks blocks into *g, with v.go = 1 when the checks pass.  On failure *g is
+// zero: every later kernel exits at entry and the CRC kernels, which read their lengths from *g, cover nothing.  out_cap
+// is at least the blob offset of n_blocks_max (the host checks it), and the offset grows with the count, so blob_cap
+// does not wrap.  one_pair set (a list of one candidate, for which the host launches no choice kernel): the choice
+// record the gated groups and the header kernel read, that pair as group 0; its costs are left as they are.
+__global__ void __launch_bounds__(32)
+    blocks_varlen_plan_kernel(const uint32_t* __restrict__ d_n_blocks, uint32_t n_blocks_max, uint32_t block_size, uint32_t chunk_syms,
+                              uint64_t out_cap, uint32_t one_pair, BlocksVarlenGeom* __restrict__ g, BlocksChoice* __restrict__ r,
+                              uint32_t* __restrict__ status)
+{
+    if (threadIdx.x) return;
+    const uint32_t n_blocks = *d_n_blocks;
+    BlocksVarlenGeom q = {};
+    if (n_blocks == 0 || n_blocks > n_blocks_max) {
+        atomicOr(status, kStatArg);
+    } else {
+        const uint64_t chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
+        q.n_blocks = n_blocks;
+        q.dir_off = sizeof(ContainerHeader) + kBlockModelBytes * n_blocks;
+        q.v.n = static_cast<uint64_t>(n_blocks) * block_size;
+        q.v.n_chunks = static_cast<uint32_t>(chunks);
+        q.v.dir_len = (chunks + 1) * sizeof(uint64_t);
+        q.v.blob_off = (q.dir_off + q.v.dir_len + 15) & ~15ull;
+        q.v.blob_cap = out_cap - q.v.blob_off;
+        q.meta_len = q.dir_off + q.v.dir_len - sizeof(ContainerHeader);
+        q.v.go = 1;
+    }
+    *g = q;
+    if (one_pair) {
+        r->choice.coder = one_pair >> 8;
+        r->choice.scale_bits = one_pair & 0xffu;
+        r->choice.index = 0;
+        r->choice.group = 0;
+        r->version = container_blocks_version(r->choice.coder);
+    }
+}
+
+// After the encoder, one thread: v.blob_len = the directory's last entry, the length of the blob CRC (crc32_kernel's
+// n_dev); the directory is at out + dir_off, which moves with the count
+__global__ void __launch_bounds__(32) blocks_varlen_blob_len_kernel(const uint8_t* __restrict__ out, BlocksVarlenGeom* __restrict__ g)
+{
+    if (threadIdx.x == 0 && g->v.go) g->v.blob_len = reinterpret_cast<const uint64_t*>(out + g->dir_off)[g->v.n_chunks];
 }
 
 }  // namespace rb200

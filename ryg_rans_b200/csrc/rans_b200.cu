@@ -74,6 +74,8 @@ struct rb200_ctx {
     ModelAsyncWork* d_model_async = nullptr;
     // rb200_container_blocks_model_encode_auto_async (model_kernels.cuh): the choice record and its running sums
     BlocksChoice* d_blocks_choice = nullptr;
+    // rb200_container_blocks_model_encode_varlen_async: the geometry of the count its plan kernel read
+    BlocksVarlenGeom* d_blocks_geom = nullptr;
 };
 
 struct rb200_model {
@@ -243,6 +245,8 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     if (e == cudaSuccess) e = cudaMemset(ctx->d_async_any, 0, sizeof(ContainerAsyncWork));
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_blocks_choice, sizeof(BlocksChoice));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_choice, 0, sizeof(BlocksChoice));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_blocks_geom, sizeof(BlocksVarlenGeom));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_geom, 0, sizeof(BlocksVarlenGeom));
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -281,6 +285,7 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->d_model_async) cudaFree(ctx->d_model_async);
     if (ctx->d_async_any) cudaFree(ctx->d_async_any);
     if (ctx->d_blocks_choice) cudaFree(ctx->d_blocks_choice);
+    if (ctx->d_blocks_geom) cudaFree(ctx->d_blocks_geom);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -454,18 +459,25 @@ namespace {
 
 // directory + compaction after any encode kernel: sizes[] -> offsets[] + blob.  geom set: the GEOM instances, on grids
 // sized for n_chunks (the bound's), with d_blob the container.  choice set: the GATED instances, which run only when the
-// record names `group`.
+// record names `group`.  bgeom set (with choice; geom is then ignored): the per-block varlen encode, whose scan and
+// compaction also take the directory's place from the record, with d_blob the container and d_offsets unused.
 int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* sizes, uint64_t* tile_sums, uint32_t n_chunks,
-                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom, const CoderChoice* choice, uint32_t group)
+                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom, const CoderChoice* choice, uint32_t group,
+                  const BlocksVarlenGeom* bgeom = nullptr)
 {
     if (!n_chunks) {
         RB_CUDA(ctx, cudaMemsetAsync(d_offsets, 0, sizeof(uint64_t), ctx->stream));
         return RB200_OK;
     }
+    if (bgeom) geom = &bgeom->v;
     const uint32_t tiles = (n_chunks + kScanTile - 1) / kScanTile;
-    auto scan = choice ? (geom ? scan_tiles_kernel<true, true> : scan_tiles_kernel<false, true>)
-                       : (geom ? scan_tiles_kernel<true> : scan_tiles_kernel<false>);
-    scan<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, d_offsets, tile_sums, geom, choice, group);
+    if (bgeom) {
+        scan_tiles_blocks_kernel<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, d_blob, tile_sums, bgeom, choice, group);
+    } else {
+        auto scan = choice ? (geom ? scan_tiles_kernel<true, true> : scan_tiles_kernel<false, true>)
+                           : (geom ? scan_tiles_kernel<true> : scan_tiles_kernel<false>);
+        scan<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, d_offsets, tile_sums, geom, choice, group);
+    }
     int rc = check_launch(ctx, "scan_tiles_kernel");
     if (rc != RB200_OK) return rc;
     const uint32_t prefixed = tiles > kTilePrefixThreshold ? 1u : 0u;
@@ -477,6 +489,11 @@ int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* siz
         if (rc != RB200_OK) return rc;
     }
     const uint32_t grid = (n_chunks + kCopyWarps - 1) / kCopyWarps;
+    if (bgeom) {
+        compact_blocks_kernel<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, tile_sums, prefixed, n_chunks, d_blob,
+                                                                         ctx->d_status, bgeom, choice, group);
+        return check_launch(ctx, "compact_blocks_kernel");
+    }
     auto compact = choice ? (geom ? compact_kernel<true, true> : compact_kernel<false, true>)
                           : (geom ? compact_kernel<true> : compact_kernel<false>);
     compact<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, d_offsets, tile_sums, prefixed, n_chunks, d_blob, blob_cap,
@@ -619,10 +636,10 @@ int prepare_workspace(rb200_ctx* ctx, const EncodePlan& p, EncodeWorkspace* ws)
 }
 
 // Runs a plan: prepare its workspace; fused: `launch(ws)`, the one kernel; split: `launch(ws)` encodes into the slots
-// (when there are chunks), then finish_encode (geom, choice, group: as there).  `launch` returns check_launch's code.
+// (when there are chunks), then finish_encode (geom, choice, group, bgeom: as there).  `launch` returns check_launch's code.
 template <class Launch>
 int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom,
-               Launch launch, const CoderChoice* choice = nullptr, uint32_t group = 0)
+               Launch launch, const CoderChoice* choice = nullptr, uint32_t group = 0, const BlocksVarlenGeom* bgeom = nullptr)
 {
     EncodeWorkspace ws = {};
     int rc = prepare_workspace(ctx, p, &ws);
@@ -633,7 +650,7 @@ int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob
         if (rc != RB200_OK) return rc;
     }
     return finish_encode(ctx, ws.scratch, p.slot_bytes, ws.sizes, ws.tile_sums, p.n_chunks, d_blob, blob_cap, d_offsets, geom, choice,
-                         group);
+                         group, bgeom);
 }
 
 // The encode tables of one encode call, in device memory.  Word: `word_gate` null runs the instance word_r32 names on
@@ -2092,6 +2109,79 @@ extern "C" int rb200_container_blocks_model_encode_auto_async(rb200_ctx* ctx, co
     if (rc != RB200_OK) return rc;
     container_blocks_finish_chosen_kernel<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, ctx->d_crc, ctx->d_status, &r->choice, &r->version);
     return check_launch(ctx, "container_blocks_finish_chosen_kernel");
+}
+
+namespace {
+
+// The per-block encode of one launch group of a varlen auto encode: blocks_encode_gated's plan for n_blocks_max, which
+// fixes every launch shape, with the varlen instances, which take the count, the directory and the blob's place in the
+// container `out` from the record
+int blocks_encode_varlen(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* d_in, uint32_t n_blocks_max, uint32_t block_size,
+                         uint32_t chunk_syms, uint8_t* out, size_t out_cap, const CoderChoice* choice, uint32_t group,
+                         const BlocksVarlenGeom* geom)
+{
+    const EncodePlan p = plan_blocks_encode(ctx, coder, sb, n_blocks_max, block_size, chunk_syms, true);
+    uint16_t* model = reinterpret_cast<uint16_t*>(out + sizeof(ContainerHeader));
+    return run_encode(ctx, p, out, 0, nullptr, nullptr, [&](const EncodeWorkspace& ws) {
+        if (coder != RB200_CODER_WORD) {
+            launch_block_coder_encode_varlen(ctx->stream, static_cast<uint32_t>(coder), sb, n_blocks_max, p.threads, p.smem, d_in, block_size,
+                                             model, chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status, choice, group, geom);
+            return check_launch(ctx, "block_coder_encode_varlen_kernel");
+        }
+        block_encode_fused_varlen_for(p.threads)<<<p.grid, p.threads, p.smem, ctx->stream>>>(
+            d_in, block_size, model, chunk_syms, ws.scratch, p.slot_bytes, ws.look, ws.counter, out, out_cap, block_size / chunk_syms, ctx->d_status, choice, group, geom);
+        return check_launch(ctx, "block_encode_fused_varlen_kernel");
+    }, choice, group, geom);
+}
+
+}  // namespace
+
+// rb200_container_blocks_model_encode_auto_async with the block count read from device memory at every run: the plan
+// kernel, then the same stages on launch shapes sized for n_blocks_max, each taking the count, the directory's and the
+// blob's places and the CRC lengths from the plan's record.  One candidate: the plan kernel writes the choice record and
+// no choice kernel runs.
+extern "C" int rb200_container_blocks_model_encode_varlen_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                                uint32_t tolerance_ppm, const uint8_t* in, const uint32_t* d_n_blocks,
+                                                                uint32_t n_blocks_max, uint32_t block_size, uint32_t chunk_syms,
+                                                                uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    if (!ctx || !in || !out || !d_n_blocks || (reinterpret_cast<uintptr_t>(d_n_blocks) & 3) || n_blocks_max == 0) return RB200_E_ARG;
+    if (!blocks_candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    if (!container_blocks_geometry_ok(n_blocks_max, block_size, chunk_syms) || !container_mem_ok(RB200_MEM_DEVICE, out, nullptr)) return RB200_E_ARG;
+    const uint64_t n_chunks_max = static_cast<uint64_t>(n_blocks_max) * (block_size / chunk_syms);
+    if (n_chunks_max >= (1ull << 31)) return RB200_E_ARG;
+    const ContainerHeader h = container_blocks_header(n_blocks_max, block_size, chunk_syms, 0, flags);
+    const size_t dir_end_max = container_dir_end(h), boff_max = container_blob_offset(h);
+    if (out_cap < boff_max) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
+    int rc = RB200_OK;
+    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++)    // every group's workspace before the first launch
+        rc = reserve_plan(ctx, plan_blocks_encode(ctx, a.coder[k], a.sb[k], n_blocks_max, block_size, chunk_syms, true));
+    if (rc != RB200_OK) return rc;
+    cudaStream_t s = ctx->stream;
+    BlocksChoice* r = ctx->d_blocks_choice;
+    BlocksVarlenGeom* geom = ctx->d_blocks_geom;
+    const bool one = n_candidates == 1;
+    if (!one) RB_CUDA(ctx, cudaMemsetAsync(&r->done, 0, sizeof(BlocksChoice) - offsetof(BlocksChoice, done), s));
+    blocks_varlen_plan_kernel<<<1, 32, 0, s>>>(d_n_blocks, n_blocks_max, block_size, chunk_syms, out_cap, one ? candidates[0] : 0u, geom, r,
+                                               ctx->d_status);
+    rc = check_launch(ctx, "blocks_varlen_plan_kernel");
+    if (rc == RB200_OK && !one) {
+        blocks_choice_geom_kernel<<<n_blocks_max, kBlocksChoiceWarps * 32, 0, s>>>(a.list, in, block_size, chunk_syms, r, ctx->d_status, geom);
+        rc = check_launch(ctx, "blocks_choice_geom_kernel");
+    }
+    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++)
+        rc = blocks_encode_varlen(ctx, a.coder[k], a.sb[k], in, n_blocks_max, block_size, chunk_syms, out, out_cap, &r->choice, k, geom);
+    if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end_max - sizeof(ContainerHeader), &geom->meta_len, 0, ctx->d_crc);
+    if (rc == RB200_OK && (h.flags & RB200_CONTAINER_CRC_BLOB)) {
+        blocks_varlen_blob_len_kernel<<<1, 32, 0, s>>>(out, geom);
+        rc = check_launch(ctx, "blocks_varlen_blob_len_kernel");
+        if (rc == RB200_OK) rc = launch_crc(ctx, out, out_cap, &geom->v.blob_len, 0, ctx->d_crc + 1, &geom->v.blob_off);
+    }
+    if (rc != RB200_OK) return rc;
+    container_blocks_finish_varlen_kernel<<<1, 32, 0, s>>>(out, h, out_cap, ctx->d_crc, ctx->d_status, &r->choice, &r->version, geom);
+    return check_launch(ctx, "container_blocks_finish_varlen_kernel");
 }
 
 extern "C" int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n)

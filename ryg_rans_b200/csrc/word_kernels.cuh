@@ -497,11 +497,10 @@ constexpr uint32_t kScanTile = 4096;
 // then both use the device's, which gives the same sums as either choice.
 // GATED (rb200_container_model_encode_auto_async): the three kernels run only when the choice record (CoderChoice,
 // device_utils.cuh) names `group`, the launch group whose split encoder they finish; otherwise they exit at entry.
-template <bool GEOM = false, bool GATED = false>
-__global__ void __launch_bounds__(1024)
-scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
-                  uint64_t* __restrict__ tile_sums, const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice,
-                  uint32_t group)
+template <bool GEOM, bool GATED>
+__device__ __forceinline__ void scan_tiles(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
+                                           uint64_t* __restrict__ tile_sums, const VarlenGeom* __restrict__ geom,
+                                           const CoderChoice* __restrict__ choice, uint32_t group)
 {
     if (GATED && choice->group != group) return;
     if (GEOM) {
@@ -541,6 +540,24 @@ scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_
         if (c0 + j < n_chunks) offsets[c0 + j] = run;
     }
     if (tid == 1023) tile_sums[blockIdx.x] = s_warp[31];
+}
+
+template <bool GEOM = false, bool GATED = false>
+__global__ void __launch_bounds__(1024)
+scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t* __restrict__ offsets,
+                  uint64_t* __restrict__ tile_sums, const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice,
+                  uint32_t group)
+{
+    scan_tiles<GEOM, GATED>(sizes, n_chunks, offsets, tile_sums, geom, choice, group);
+}
+
+// The GEOM and GATED scan of rb200_container_blocks_model_encode_varlen_async, whose directory sits after the models
+// of the record's count: at out + geom->dir_off (BlocksVarlenGeom)
+__global__ void __launch_bounds__(1024)
+scan_tiles_blocks_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint8_t* __restrict__ out, uint64_t* __restrict__ tile_sums,
+                         const BlocksVarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
+{
+    scan_tiles<true, true>(sizes, n_chunks, reinterpret_cast<uint64_t*>(out + geom->dir_off), tile_sums, &geom->v, choice, group);
 }
 
 // for very large directories: turn tile_sums into exclusive prefixes once, so compact CTAs read one value
@@ -590,12 +607,11 @@ constexpr int kCopyWarps = 8;
 constexpr uint32_t kTilePrefixThreshold = 256;   // above this many tiles, tile_prefix_kernel runs first
 
 // one warp moves one chunk stream from the end of its scratch slot to blob[offsets[c]..E_c)
-template <bool GEOM = false, bool GATED = false>
-__global__ void __launch_bounds__(kCopyWarps * 32)
-compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
-               uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
-               uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status,
-               const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
+template <bool GEOM, bool GATED>
+__device__ __forceinline__ void compact(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+                                        uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
+                                        uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status,
+                                        const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
 {
     if (GATED && choice->group != group) return;
     if (GEOM) {
@@ -633,6 +649,28 @@ compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const u
         }
     }
     if (end <= blob_cap) place_stream<false>(scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, size, blob, end, lane);
+}
+
+template <bool GEOM = false, bool GATED = false>
+__global__ void __launch_bounds__(kCopyWarps * 32)
+compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+               uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
+               uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status,
+               const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
+{
+    compact<GEOM, GATED>(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, blob, blob_cap, status, geom, choice, group);
+}
+
+// The GEOM and GATED compaction of rb200_container_blocks_model_encode_varlen_async: the directory at out +
+// geom->dir_off, the blob at out + geom->v.blob_off (BlocksVarlenGeom)
+__global__ void __launch_bounds__(kCopyWarps * 32)
+compact_blocks_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+                      const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed, uint32_t n_chunks, uint8_t* __restrict__ out,
+                      uint32_t* __restrict__ status, const BlocksVarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice,
+                      uint32_t group)
+{
+    compact<true, true>(scratch, slot_bytes, sizes, reinterpret_cast<uint64_t*>(out + geom->dir_off), tile_sums, tiles_prefixed, n_chunks, out,
+                        0, status, &geom->v, choice, group);
 }
 
 // the K2 and K2f instances: (R32, GATED, GEOM) = (r32, 0, 0) for an rb200_model, (r32, 1, 0) and (r32, 1, 1) for the

@@ -67,10 +67,15 @@ device costs against rb200_choose_blocks_coder's; every candidate's blob in byte
 the auto call's kernels and the fixed call's; and rb200_container_blocks_any_decode_async against the chosen version's
 own async decode, alternated, with its kernel list.
 
+With --blocks-varlen, rb200_container_blocks_model_encode_varlen_async on the --blocks-auto workloads with n_blocks_max =
+8192, flags 0, alternated: at *d_n_blocks = 8192 against the fixed auto call, at *d_n_blocks = 1024 against the fixed
+auto call at 1024 blocks, and with the chosen pair as its one candidate against the fixed model-building container call
+of that pair; a torch.profiler list of the varlen calls' kernels and their fixed twins'.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
-    python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto | --blocks-auto]
-                                     [--reps 10]
+    python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto | --blocks-auto
+                                      | --blocks-varlen] [--reps 10]
                                      [--json out.json]"""
 import argparse
 import json
@@ -854,6 +859,63 @@ def blocks_auto(args):
     return res
 
 
+def blocks_varlen(args):
+    """rb200_container_blocks_model_encode_varlen_async (n_blocks_max 8192) against the fixed calls: the auto call at 8192
+    and at 1024 blocks, and, with one candidate, the fixed model-building call of the pair the auto call chose"""
+    import torch
+    nb_max, block_size, chunk, tol = 8192, 65536, 8192, 20000
+    W, B, A = rb.CODER_WORD, rb.CODER_BYTE, rb.CODER_ALIAS
+    cands = [api.CANDIDATE(W, 12), api.CANDIDATE(B, 14), api.CANDIDATE(A, 14)]
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    cap = ctx.container_blocks_capacity(nb_max, block_size, chunk)
+    d_ref = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_out = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_nb = torch.tensor([nb_max, 1024], dtype=torch.int32, device="cuda")
+    res = {"card": card(), "workload": {"n_blocks_max": nb_max, "block_size": block_size, "chunk_syms": chunk},
+           "candidates": ["word 12", "byte 14", "alias 14"], "tolerance_ppm": tol, "workloads": {}, "checks": {}}
+
+    def size(d):
+        h = d[:64].cpu().numpy()
+        nb, blob = int(h[56:60].view(np.uint32)[0]), int(h[32:40].view(np.uint64)[0])
+        return ((64 + 512 * nb + 8 * (nb * block_size // chunk + 1) + 15) & ~15) + blob
+
+    for name, make in (("skewed", skewed_blocks_data), ("zipf", blocks_data)):
+        d_in = make(nb_max, block_size, 4321)
+        i, r, o = d_in.data_ptr(), d_ref.data_ptr(), d_out.data_ptr()
+        ctx.container_blocks_model_encode_auto_async(cands, tol, i, nb_max, block_size, chunk, 0, r, cap)
+        sync()
+        h = d_ref[:8].cpu().numpy()
+        coder, sb = int(h[6]), int(h[7])
+        fixed_pair = {W: lambda: ctx.container_blocks_encode_device(i, nb_max, block_size, None, chunk, 0, r, cap),
+                      A: lambda: ctx.container_blocks_alias_encode_device(sb, i, nb_max, block_size, None, chunk, 0, r, cap)}.get(
+            coder, lambda: ctx.container_blocks_coder_encode_device(coder, sb, i, nb_max, block_size, None, chunk, 0, r, cap))
+        arms = {  # (varlen call, fixed call)
+            "max": (lambda: ctx.container_blocks_model_encode_varlen_async(cands, tol, i, d_nb.data_ptr(), nb_max, block_size, chunk, 0, o, cap),
+                    lambda: ctx.container_blocks_model_encode_auto_async(cands, tol, i, nb_max, block_size, chunk, 0, r, cap)),
+            "1024": (lambda: ctx.container_blocks_model_encode_varlen_async(cands, tol, i, d_nb[1:].data_ptr(), nb_max, block_size, chunk, 0, o,
+                                                                            cap),
+                     lambda: ctx.container_blocks_model_encode_auto_async(cands, tol, i, 1024, block_size, chunk, 0, r, cap)),
+            "one_candidate": (lambda: ctx.container_blocks_model_encode_varlen_async([api.CANDIDATE(coder, sb)], 0, i, d_nb.data_ptr(), nb_max,
+                                                                                     block_size, chunk, 0, o, cap),
+                              fixed_pair),
+        }
+        out = {"chosen": {"coder": coder, "scale_bits": sb}}
+        for arm, (varlen, fixed) in arms.items():
+            times = alternate({"varlen": varlen, "fixed": fixed}, sync, args.warmup, args.reps)
+            varlen()
+            fixed()
+            sync()
+            n = size(d_ref)
+            res["checks"][f"{name} {arm}: varlen_equals_fixed_call"] = size(d_out) == n and bool(torch.equal(d_out[:n], d_ref[:n]))
+            out[arm] = {"encode": times, "varlen_minus_fixed_median_us": 1e3 * (times["varlen"]["median_ms"] - times["fixed"]["median_ms"]),
+                        "varlen_kernels": kernel_times(varlen, sync, args.reps), "fixed_kernels": kernel_times(fixed, sync, args.reps)}
+        res["workloads"][name] = out
+        del d_in
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
@@ -863,13 +925,14 @@ def main():
     ap.add_argument("--model", action="store_true", help="the single-model container's encode with the model built from the data")
     ap.add_argument("--auto", action="store_true", help="the model-building encode with the coder chosen on the GPU")
     ap.add_argument("--blocks-auto", action="store_true", help="the per-block model-building encode with the coder chosen on the GPU")
+    ap.add_argument("--blocks-varlen", action="store_true", help="the per-block auto encode with the block count in device memory")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
