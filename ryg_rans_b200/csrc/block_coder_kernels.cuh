@@ -241,38 +241,21 @@ __device__ __forceinline__ void block_coder_encode(const uint8_t* __restrict__ i
         encode_chunk_split(src, chunk_syms, chunk, Rans64Encoder{tab, sb}, wsm, scratch, slot_bytes, sizes, status);
 }
 
-template <uint32_t CODER, uint32_t SB, bool BUILD>
+// GATED (rb200_container_blocks_model_encode_auto_async, with BUILD): runs only when the choice record (CoderChoice,
+// device_utils.cuh) names `group`, and then at the record's scale_bits (the generic instances; the specialised ones are
+// only ever named at their own).
+// GEOM (rb200_container_blocks_model_encode_varlen_async, with GATED): on the grid of n_blocks_max, the CTAs at or past
+// the record's count (BlocksVarlenGeom) exit at entry, as every CTA does when the plan failed (the count is then 0).
+template <uint32_t CODER, uint32_t SB, bool BUILD, bool GATED = false, bool GEOM = false>
 __global__ void __launch_bounds__(kMaxBlockWarps * 32)
 block_coder_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t sb_rt,
                           uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
-                          uint32_t* __restrict__ status)
+                          uint32_t* __restrict__ status, const CoderChoice* __restrict__ choice, uint32_t group,
+                          const BlocksVarlenGeom* __restrict__ geom)
 {
-    block_coder_encode<CODER, SB, BUILD>(in, block_size, block_freqs, sb_rt, chunk_syms, scratch, slot_bytes, sizes, status);
-}
-
-// The model-building instances for rb200_container_blocks_model_encode_auto_async: run only when the choice record
-// (CoderChoice, device_utils.cuh) names `group`, and then at the record's scale_bits (the generic instances; the
-// specialised ones are only ever named at their own)
-template <uint32_t CODER, uint32_t SB>
-__global__ void __launch_bounds__(kMaxBlockWarps * 32)
-block_coder_encode_gated_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t chunk_syms,
-                                uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status,
-                                const CoderChoice* __restrict__ choice, uint32_t group)
-{
-    if (choice->group != group) return;                          // the same for the whole grid
-    block_coder_encode<CODER, SB, true>(in, block_size, block_freqs, choice->scale_bits, chunk_syms, scratch, slot_bytes, sizes, status);
-}
-
-// The same for rb200_container_blocks_model_encode_varlen_async, on the grid of n_blocks_max: the CTAs at or past the
-// record's count (BlocksVarlenGeom) exit at entry, as every CTA does when the plan failed (the count is then 0)
-template <uint32_t CODER, uint32_t SB>
-__global__ void __launch_bounds__(kMaxBlockWarps * 32)
-block_coder_encode_varlen_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t chunk_syms,
-                                 uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes, uint32_t* __restrict__ status,
-                                 const CoderChoice* __restrict__ choice, uint32_t group, const BlocksVarlenGeom* __restrict__ geom)
-{
-    if (choice->group != group || blockIdx.x >= geom->n_blocks) return;     // the group is the same for the whole grid
-    block_coder_encode<CODER, SB, true>(in, block_size, block_freqs, choice->scale_bits, chunk_syms, scratch, slot_bytes, sizes, status);
+    if ((GATED && choice->group != group) || (GEOM && blockIdx.x >= geom->n_blocks)) return;   // the group is the same for the whole grid
+    block_coder_encode<CODER, SB, BUILD>(in, block_size, block_freqs, GATED ? choice->scale_bits : sb_rt, chunk_syms, scratch, slot_bytes,
+                                         sizes, status);
 }
 
 // A block's decode table in shared memory at s_tab, from its cumulative frequencies (s_cum[257], M = 1 << sb): cum2sym[M],
@@ -419,8 +402,8 @@ inline void configure_block_coder()
 {
     for (const void* k : {reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, true>),
                           reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, false>),
-                          reinterpret_cast<const void*>(block_coder_encode_gated_kernel<CODER, SB>),
-                          reinterpret_cast<const void*>(block_coder_encode_varlen_kernel<CODER, SB>)}) {
+                          reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, true, true>),
+                          reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, true, true, true>)}) {
         cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              block_coder_encode_smem(CODER, kBlockCoderMaxScaleBits, kMaxBlockWarps * 32));
@@ -440,35 +423,21 @@ inline void configure_block_coder_kernels()
     configure_block_coder<RB200_CODER_ALIAS, 0>();
 }
 
-// one CTA per block of block_threads() threads; smem = block_coder_encode_smem(coder, sb, threads)
+// one CTA per block of block_threads() threads; smem = block_coder_encode_smem(coder, sb, threads).  choice set: the
+// GATED instance of (coder, sb)'s dispatch, with models built, where sb is the largest scale_bits of the launch group,
+// which sizes the alias coder's remap, and the kernel takes the chosen one from the record; geom set as well: the GEOM
+// instance, on a grid of n_blocks = n_blocks_max CTAs.
 inline void launch_block_coder_encode(cudaStream_t stream, uint32_t coder, uint32_t sb, bool build, uint32_t n_blocks, uint32_t threads,
                                       uint32_t smem, const uint8_t* d_in, uint32_t block_size, uint16_t* d_freqs, uint32_t chunk_syms,
-                                      uint8_t* scratch, uint32_t slot_bytes, uint32_t* sizes, uint32_t* status)
+                                      uint8_t* scratch, uint32_t slot_bytes, uint32_t* sizes, uint32_t* status,
+                                      const CoderChoice* choice = nullptr, uint32_t group = 0, const BlocksVarlenGeom* geom = nullptr)
 {
-    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, ((build ? block_coder_encode_kernel<CODER, SB, true> : block_coder_encode_kernel<CODER, SB, false>)
+    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, ((geom     ? block_coder_encode_kernel<CODER, SB, true, true, true>
+                                                : choice ? block_coder_encode_kernel<CODER, SB, true, true>
+                                                : build  ? block_coder_encode_kernel<CODER, SB, true>
+                                                         : block_coder_encode_kernel<CODER, SB, false>)
                                            <<<n_blocks, threads, smem, stream>>>(d_in, block_size, d_freqs, sb, chunk_syms, scratch,
-                                                                                 slot_bytes, sizes, status)))
-}
-
-// the gated instance of (coder, sb)'s dispatch (rb200_container_blocks_model_encode_auto_async): sb is the largest
-// scale_bits of the launch group, which sizes the alias coder's remap; the kernel takes the chosen one from the record
-inline void launch_block_coder_encode_gated(cudaStream_t stream, uint32_t coder, uint32_t sb, uint32_t n_blocks, uint32_t threads, uint32_t smem,
-                                            const uint8_t* d_in, uint32_t block_size, uint16_t* d_freqs, uint32_t chunk_syms, uint8_t* scratch,
-                                            uint32_t slot_bytes, uint32_t* sizes, uint32_t* status, const CoderChoice* choice, uint32_t group)
-{
-    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, (block_coder_encode_gated_kernel<CODER, SB><<<n_blocks, threads, smem, stream>>>(
-                                              d_in, block_size, d_freqs, chunk_syms, scratch, slot_bytes, sizes, status, choice, group)))
-}
-
-// the varlen instance of (coder, sb)'s dispatch (rb200_container_blocks_model_encode_varlen_async): as the gated one,
-// on a grid of n_blocks_max CTAs
-inline void launch_block_coder_encode_varlen(cudaStream_t stream, uint32_t coder, uint32_t sb, uint32_t n_blocks_max, uint32_t threads,
-                                             uint32_t smem, const uint8_t* d_in, uint32_t block_size, uint16_t* d_freqs, uint32_t chunk_syms,
-                                             uint8_t* scratch, uint32_t slot_bytes, uint32_t* sizes, uint32_t* status, const CoderChoice* choice,
-                                             uint32_t group, const BlocksVarlenGeom* geom)
-{
-    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, (block_coder_encode_varlen_kernel<CODER, SB><<<n_blocks_max, threads, smem, stream>>>(
-                                              d_in, block_size, d_freqs, chunk_syms, scratch, slot_bytes, sizes, status, choice, group, geom)))
+                                                                                 slot_bytes, sizes, status, choice, group, geom)))
 }
 
 inline void launch_block_coder_decode(cudaStream_t stream, uint32_t coder, uint32_t sb, const uint8_t* blob, uint64_t blob_size,

@@ -481,52 +481,35 @@ __device__ __forceinline__ void block_encode_fused(const uint8_t* __restrict__ i
     q.drain(out, lane);
 }
 
-template <bool BUILD, int WARPS>
+// GATED (rb200_container_blocks_model_encode_auto_async, with BUILD): runs only when the choice record (CoderChoice,
+// device_utils.cuh) names `group`; otherwise every CTA, the scanner's included, exits at entry, before it touches the
+// counter, look[] or scratch, which the host zeroes before every launch all the same.
+// GEOM (rb200_container_blocks_model_encode_varlen_async, with GATED): on the grid the host plans for n_blocks_max, with
+// the block count from the record (BlocksVarlenGeom; 0 when the plan failed, and then every CTA exits at entry).  The
+// body takes the count as an argument, so the scanner warp follows the record's chunks and workers past the count find
+// no block and drain.  `blob` is the container and blob_cap its capacity; the directory and the blob's place in it are
+// worked out here from the count and per_block (= block_size / chunk_syms), as the plan kernel lays them out, rather
+// than read from the record: values this cheap to derive from one register are recomputed where they are used instead
+// of held, which keeps the 8-warp instance at the spill of the shipped one whose body it runs.
+template <bool BUILD, int WARPS, bool GATED = false, bool GEOM = false>
 __global__ void __launch_bounds__(WARPS * 32, WARPS <= 8 ? 5 : 1)
 block_encode_fused_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uint32_t block_size, uint16_t* __restrict__ block_freqs,
                           uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint64_t* __restrict__ look,
                           uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap, uint64_t* __restrict__ offsets,
-                          uint32_t* __restrict__ status)
+                          uint32_t* __restrict__ status, const CoderChoice* __restrict__ choice, uint32_t group,
+                          const BlocksVarlenGeom* __restrict__ geom, uint32_t per_block)
 {
+    if (GEOM) n_blocks = geom->n_blocks;
+    if ((GEOM && !n_blocks) || (GATED && choice->group != group)) return;      // the same for the whole grid
+    if (GEOM) {
+        const uint64_t entries = static_cast<uint64_t>(n_blocks) * per_block + 1;     // the directory's
+        const uint64_t dir_off = 64 + 512ull * n_blocks, blob_off = dir_off + ((entries + 1) >> 1) * 16;
+        offsets = reinterpret_cast<uint64_t*>(blob + dir_off);
+        blob += blob_off;
+        blob_cap -= blob_off;
+    }
     block_encode_fused<BUILD>(in, n_blocks, block_size, block_freqs, chunk_syms, scratch, slot_bytes, look, counter, blob, blob_cap, offsets,
                               status);
-}
-
-// The model-building instance for rb200_container_blocks_model_encode_auto_async: runs only when the choice record
-// (CoderChoice, device_utils.cuh) names `group`; otherwise every CTA, the scanner's included, exits at entry, before it
-// touches the counter, look[] or scratch, which the host zeroes before every launch all the same.
-template <int WARPS>
-__global__ void __launch_bounds__(WARPS * 32, WARPS <= 8 ? 5 : 1)
-block_encode_fused_gated_kernel(const uint8_t* __restrict__ in, uint32_t n_blocks, uint32_t block_size, uint16_t* __restrict__ block_freqs,
-                                uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint64_t* __restrict__ look,
-                                uint32_t* __restrict__ counter, uint8_t* __restrict__ blob, uint64_t blob_cap, uint64_t* __restrict__ offsets,
-                                uint32_t* __restrict__ status, const CoderChoice* __restrict__ choice, uint32_t group)
-{
-    if (choice->group != group) return;                         // the same for the whole grid
-    block_encode_fused<true>(in, n_blocks, block_size, block_freqs, chunk_syms, scratch, slot_bytes, look, counter, blob, blob_cap, offsets,
-                             status);
-}
-
-// The model-building instance for rb200_container_blocks_model_encode_varlen_async: gated as the one above, on the
-// grid the host plans for n_blocks_max, with the block count from the record (BlocksVarlenGeom).  The body takes the
-// count as an argument, so the scanner warp follows the record's chunks and workers past the count find no block and
-// drain.  The directory and the blob's place in the container `out` are worked out here from the count and the
-// parameters (per_block = block_size / chunk_syms), as the plan kernel lays them out, rather than read from the
-// record: values this cheap to derive from one register are recomputed where they are used instead of held, which
-// keeps the 8-warp instance at the spill of the shipped one whose body it runs.
-template <int WARPS>
-__global__ void __launch_bounds__(WARPS * 32, WARPS <= 8 ? 5 : 1)
-block_encode_fused_varlen_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t chunk_syms,
-                                 uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint64_t* __restrict__ look, uint32_t* __restrict__ counter,
-                                 uint8_t* __restrict__ out, uint64_t out_cap, uint32_t per_block, uint32_t* __restrict__ status,
-                                 const CoderChoice* __restrict__ choice, uint32_t group, const BlocksVarlenGeom* __restrict__ geom)
-{
-    const uint32_t n_blocks = geom->n_blocks;                   // 0 when the plan failed
-    if (!n_blocks || choice->group != group) return;            // the same for the whole grid
-    const uint64_t entries = static_cast<uint64_t>(n_blocks) * per_block + 1;     // the directory's
-    const uint64_t dir_off = 64 + 512ull * n_blocks, blob_off = dir_off + ((entries + 1) >> 1) * 16;
-    block_encode_fused<true>(in, n_blocks, block_size, block_freqs, chunk_syms, scratch, slot_bytes, look, counter, out + blob_off,
-                             out_cap - blob_off, reinterpret_cast<uint64_t*>(out + dir_off), status);
 }
 
 inline uint32_t block_threads(uint32_t block_size, uint32_t chunk_syms)
@@ -539,22 +522,19 @@ inline uint32_t block_threads(uint32_t block_size, uint32_t chunk_syms)
 // dynamic shared memory of both per-block encoders (K5, K5f) at `threads` threads: the table, then 1 KiB per warp
 inline uint32_t block_encode_smem(uint32_t threads) { return kEncTableBytes + (threads / 32) * kEncWarpSmem; }
 
-// the instance of the fused per-block encoder for blocks of block_threads() = `threads`
+// the instance of the fused per-block encoder for blocks of block_threads() = `threads`: (BUILD, GATED, GEOM) =
+// (build, 0, 0) for the fixed calls, (1, 1, 0) for the auto encode, (1, 1, 1) for the device-count encode
 using BlockEncodeFusedKernel = decltype(&block_encode_fused_kernel<true, 8>);
-inline BlockEncodeFusedKernel block_encode_fused_for(bool build, uint32_t threads)
+template <int WARPS>
+inline BlockEncodeFusedKernel block_encode_fused_warps(bool build, bool gated, bool geom)
 {
-    if (threads <= 256) return build ? block_encode_fused_kernel<true, 8> : block_encode_fused_kernel<false, 8>;
-    return build ? block_encode_fused_kernel<true, 32> : block_encode_fused_kernel<false, 32>;
+    if (geom) return block_encode_fused_kernel<true, WARPS, true, true>;
+    if (gated) return block_encode_fused_kernel<true, WARPS, true>;
+    return build ? block_encode_fused_kernel<true, WARPS> : block_encode_fused_kernel<false, WARPS>;
 }
-using BlockEncodeFusedGatedKernel = decltype(&block_encode_fused_gated_kernel<8>);
-inline BlockEncodeFusedGatedKernel block_encode_fused_gated_for(uint32_t threads)
+inline BlockEncodeFusedKernel block_encode_fused_for(bool build, bool gated, bool geom, uint32_t threads)
 {
-    return threads <= 256 ? block_encode_fused_gated_kernel<8> : block_encode_fused_gated_kernel<32>;
-}
-using BlockEncodeFusedVarlenKernel = decltype(&block_encode_fused_varlen_kernel<8>);
-inline BlockEncodeFusedVarlenKernel block_encode_fused_varlen_for(uint32_t threads)
-{
-    return threads <= 256 ? block_encode_fused_varlen_kernel<8> : block_encode_fused_varlen_kernel<32>;
+    return threads <= 256 ? block_encode_fused_warps<8>(build, gated, geom) : block_encode_fused_warps<32>(build, gated, geom);
 }
 
 inline void configure_block_kernels()
@@ -564,18 +544,12 @@ inline void configure_block_kernels()
     cudaFuncSetAttribute(block_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxBlockWarps * kRingBytes);
     cudaFuncSetAttribute(block_encode_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(block_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(kMaxBlockWarps * 32));
-    for (const bool build : {true, false})
-        for (const uint32_t threads : {8u * 32, 32u * 32}) {
-            cudaFuncSetAttribute(block_encode_fused_for(build, threads), cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 cudaSharedmemCarveoutMaxShared);
-            cudaFuncSetAttribute(block_encode_fused_for(build, threads), cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
+    for (const uint32_t threads : {8u * 32, 32u * 32})
+        for (const BlockEncodeFusedKernel k : {block_encode_fused_for(true, false, false, threads), block_encode_fused_for(false, false, false, threads),
+                                               block_encode_fused_for(true, true, false, threads), block_encode_fused_for(true, true, true, threads)}) {
+            cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
         }
-    for (const uint32_t threads : {8u * 32, 32u * 32}) {
-        cudaFuncSetAttribute(block_encode_fused_gated_for(threads), cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        cudaFuncSetAttribute(block_encode_fused_gated_for(threads), cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
-        cudaFuncSetAttribute(block_encode_fused_varlen_for(threads), cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        cudaFuncSetAttribute(block_encode_fused_varlen_for(threads), cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
-    }
 }
 
 inline void launch_block_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets,

@@ -335,31 +335,27 @@ __global__ void __launch_bounds__(32)
     container_finish<GEOM, CHOSEN>(out, h, dir_off, blob_off, out_cap, freqs, slots, status, geom, choice);
 }
 
-// The CHOSEN per-block instance (rb200_container_blocks_model_encode_auto_async, versions 2-4): version, coder and
-// scale_bits from the choice record; the layout of the three versions is the same, so h carries the rest.
-__global__ void __launch_bounds__(32)
-    container_blocks_finish_chosen_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
-                                          const CrcSlot* __restrict__ slots, uint32_t* status, const CoderChoice* __restrict__ choice,
-                                          const uint32_t* __restrict__ version)
-{
-    h.version = static_cast<uint16_t>(*version);
-    container_finish<false, true>(out, h, dir_off, blob_off, out_cap, nullptr, slots, status, nullptr, choice);
-}
-
-// The same for rb200_container_blocks_model_encode_varlen_async: n_blocks, n_symbols, n_chunks, the directory and the
-// blob offset from the record (BlocksVarlenGeom); h arrives with block_size, chunk_syms and flags.  Writes nothing when
+// The per-block header kernel of rb200_container_blocks_model_encode_auto_async (versions 2-4): version, coder and
+// scale_bits from the choice record r; the layout of the three versions is the same, so h carries the rest.
+// GEOM (rb200_container_blocks_model_encode_varlen_async): n_blocks, n_symbols, n_chunks, the directory and the blob
+// offset from the record (BlocksVarlenGeom); h arrives with block_size, chunk_syms and flags.  Writes nothing when
 // geom->v.go == 0.
+template <bool GEOM>
 __global__ void __launch_bounds__(32)
-    container_blocks_finish_varlen_kernel(uint8_t* out, ContainerHeader h, uint64_t out_cap, const CrcSlot* __restrict__ slots, uint32_t* status,
-                                          const CoderChoice* __restrict__ choice, const uint32_t* __restrict__ version,
-                                          const BlocksVarlenGeom* __restrict__ geom)
+    container_blocks_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
+                                   const CrcSlot* __restrict__ slots, uint32_t* status, const BlocksChoice* __restrict__ r,
+                                   const BlocksVarlenGeom* __restrict__ geom)
 {
-    if (!geom->v.go) return;
-    h.version = static_cast<uint16_t>(*version);
-    h.n_blocks = geom->n_blocks;
-    h.n_symbols = geom->v.n;
-    h.n_chunks = geom->v.n_chunks;
-    container_finish<false, true>(out, h, geom->dir_off, geom->v.blob_off, out_cap, nullptr, slots, status, nullptr, choice);
+    if (GEOM && !geom->v.go) return;
+    h.version = static_cast<uint16_t>(r->version);
+    if (GEOM) {
+        h.n_blocks = geom->n_blocks;
+        h.n_symbols = geom->v.n;
+        h.n_chunks = geom->v.n_chunks;
+        dir_off = geom->v.dir_off;
+        blob_off = geom->v.blob_off;
+    }
+    container_finish<false, true>(out, h, dir_off, blob_off, out_cap, nullptr, slots, status, nullptr, &r->choice);
 }
 
 }  // namespace rb200

@@ -22,20 +22,20 @@ constexpr uint32_t kHeaderBytes = 128; // 32 lanes x u32 final state (RansWordEn
 struct VarlenGeom {
     uint64_t n;            // symbols, 1 <= n <= n_max
     uint64_t dir_len;      // directory bytes, 8 (n_chunks + 1)
-    uint64_t blob_off;     // offset of the blob in the container, round16(1088 + dir_len)
+    uint64_t blob_off;     // offset of the blob in the container, round16(dir_off + dir_len)
     uint64_t blob_cap;     // out_cap - blob_off
     uint64_t blob_len;     // dir[n_chunks], copied after the encoder (the blob CRC's length)
     uint32_t n_chunks;
     uint32_t go;           // 1: *d_n passed the checks; 0: nothing after the plan runs (dir_len, blob_off, blob_len are 0)
+    uint64_t dir_off;      // offset of the directory in the container: 1088 (version 1), 64 + 512 n_blocks (per-block)
 };
 
 // The geometry of rb200_container_blocks_model_encode_varlen_async, which reads the block count from device memory:
 // written by blocks_varlen_plan_kernel (model_kernels.cuh) from *d_n_blocks at every run.  v is the VarlenGeom of the
 // container's symbols and chunks (n = n_blocks x block_size), so the GEOM instances of C5 read it as they are; the
-// directory, which sits after the n_blocks models and so moves with the count, and the meta CRC's length follow it.
+// meta CRC's length follows it.
 struct BlocksVarlenGeom {
-    VarlenGeom v;          // v.blob_off = round16(dir_off + v.dir_len)
-    uint64_t dir_off;      // 64 + 512 n_blocks
+    VarlenGeom v;
     uint64_t meta_len;     // 512 n_blocks + v.dir_len: models and directory, the bytes the meta CRC's kernel covers
     uint32_t n_blocks;     // 1 <= n_blocks <= n_blocks_max; 0 when v.go == 0
     uint32_t reserved;
@@ -50,6 +50,16 @@ struct CoderChoice {
     uint32_t index;                    // its place in the caller's list (the first one when none is feasible)
     uint32_t group;                    // the launch group that encodes
     uint64_t costs[kMaxCandidates];    // every candidate's cost, UINT64_MAX when infeasible
+};
+
+// The choice of rb200_container_blocks_model_encode_auto_async: the record the gated encode groups read (choice: pair,
+// index, group and every candidate's cost) and the container version the header kernel writes, with the running sums
+// of blocks_choice_kernel (model_kernels.cuh), which the host zeroes (one memset from `done` on) before every launch.
+struct BlocksChoice {
+    CoderChoice choice;
+    uint32_t version;
+    uint32_t done;                                // CTAs that have added their costs
+    unsigned long long sums[kMaxCandidates];      // the costs so far
 };
 
 __device__ __forceinline__ uint32_t lanemask_lt()

@@ -16,7 +16,7 @@
 // rb200_container_model_encode_varlen_async runs the same stages on launch shapes the host sizes for a bound n_max,
 // and reads the length from device memory: varlen_plan_kernel checks *d_n and writes the geometry record (VarlenGeom,
 // device_utils.cuh) into geom; every later kernel is the GEOM instance of the same kernel, which takes n, the chunk
-// count and the blob's place from there and exits at entry when the checks failed.
+// count and the directory's and blob's places from there and exits at entry when the checks failed.
 //
 // rb200_container_model_encode_auto_async runs coder_choice_kernel after the histogram: it applies the rule of
 // rb200_choose_coder to the counts and writes the choice record (CoderChoice).  The CHOSEN instance of the model kernel
@@ -26,15 +26,15 @@
 // CHOSEN instance of container_finish_kernel writes the chosen coder and scale_bits into the header.
 //
 // rb200_container_blocks_model_encode_auto_async does the same for the per-block containers (versions 2-4):
-// blocks_choice_kernel applies the rule of rb200_choose_blocks_coder block by block and writes BlocksChoice; one gated
-// group per distinct per-block encoder instance follows (block_encode_fused_gated_kernel, block_coder_encode_gated_kernel
-// with C7's GATED scan, prefix and compaction), then the CRCs and container_blocks_finish_chosen_kernel, which writes
-// version, coder and scale_bits from the record.
+// blocks_choice_kernel applies the rule of rb200_choose_blocks_coder block by block and writes BlocksChoice
+// (device_utils.cuh); one gated group per distinct per-block encoder instance follows (the GATED instances of
+// block_encode_fused_kernel and block_coder_encode_kernel, with C7's GATED scan, prefix and compaction), then the CRCs
+// and container_blocks_finish_kernel, which writes version, coder and scale_bits from the record.
 //
 // rb200_container_blocks_model_encode_varlen_async runs those stages on launch shapes sized for n_blocks_max:
 // blocks_varlen_plan_kernel reads *d_n_blocks into BlocksVarlenGeom (device_utils.cuh), and the choice kernel, the
-// encoders, the scan and compaction and the header kernel are varlen instances around the same bodies, which take the
-// count, the directory's place (after the count's models) and the blob's from it.
+// encoders, the scan and compaction, the blob length and the header kernel are the GEOM instances of the same kernels,
+// which take the count, the directory's place (after the count's models) and the blob's from it.
 #pragma once
 #include "block_kernels.cuh"
 #include "container_format.h"
@@ -56,7 +56,7 @@ struct ModelAsyncWork {
     alignas(16) uint4 r64_enc[256 * 2];           // Rans64EncSymbol images, 32 bytes each
     alignas(16) uint16_t alias_remap[1u << 16];   // the first 1 << scale_bits entries are the model's
     VarlenGeom geom;                              // rb200_container_model_encode_varlen_async: the length and layout of this run
-    CoderChoice choice;                           // rb200_container_model_encode_auto_async: the choice of this run
+    alignas(16) CoderChoice choice;               // rb200_container_model_encode_auto_async: the choice of this run
     uint32_t cand_freqs[kMaxCandidates][256];     // its candidates' models; the chosen row is the container's
 };
 
@@ -206,16 +206,6 @@ __global__ void __launch_bounds__(kMaxCandidates * 32)
     }
 }
 
-// The choice of rb200_container_blocks_model_encode_auto_async: the record the gated encode groups read (choice: pair,
-// index, group and every candidate's cost) and the container version the header kernel writes, with the running sums
-// of blocks_choice_kernel, which the host zeroes (one memset from `done` on) before every launch.
-struct BlocksChoice {
-    CoderChoice choice;
-    uint32_t version;
-    uint32_t done;                                // CTAs that have added their costs
-    unsigned long long sums[kMaxCandidates];      // the costs so far
-};
-
 constexpr int kBlocksChoiceWarps = 8;
 constexpr uint32_t kBlocksChoiceRowWords = 784;  // a warp's rows over the free histogram: widths, model, cumulative (16-byte aligned)
 
@@ -228,9 +218,10 @@ constexpr uint32_t kBlocksChoiceRowWords = 784;  // a warp's rows over the free 
 // GEOM (rb200_container_blocks_model_encode_varlen_async): the block count from the record (BlocksVarlenGeom), on the
 // grid of n_blocks_max; the CTAs at or past it exit at entry, before they count, so the last of the device count's CTAs
 // is the last out (none runs when the plan failed: n_blocks is then 0).
-template <bool GEOM>
-__device__ __forceinline__ void blocks_choice(CandidateList list, const uint8_t* __restrict__ in, uint32_t block_size, uint32_t chunk_syms,
-                                              BlocksChoice* r, uint32_t* __restrict__ status, const BlocksVarlenGeom* __restrict__ geom)
+template <bool GEOM = false>
+__global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
+    blocks_choice_kernel(CandidateList list, const uint8_t* __restrict__ in, uint32_t block_size, uint32_t chunk_syms, BlocksChoice* r,
+                         uint32_t* __restrict__ status, const BlocksVarlenGeom* __restrict__ geom)
 {
     if (GEOM && blockIdx.x >= geom->n_blocks) return;            // the same for the whole CTA
     __shared__ __align__(16) uint32_t s_hist[256 * 32];          // the histogram copies, then the warps' rows
@@ -279,20 +270,6 @@ __device__ __forceinline__ void blocks_choice(CandidateList list, const uint8_t*
     }
 }
 
-__global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
-    blocks_choice_kernel(CandidateList list, const uint8_t* __restrict__ in, uint32_t block_size, uint32_t chunk_syms, BlocksChoice* r,
-                         uint32_t* __restrict__ status)
-{
-    blocks_choice<false>(list, in, block_size, chunk_syms, r, status, nullptr);
-}
-
-__global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
-    blocks_choice_geom_kernel(CandidateList list, const uint8_t* __restrict__ in, uint32_t block_size, uint32_t chunk_syms, BlocksChoice* r,
-                              uint32_t* __restrict__ status, const BlocksVarlenGeom* __restrict__ geom)
-{
-    blocks_choice<true>(list, in, block_size, chunk_syms, r, status, geom);
-}
-
 // The first kernel of rb200_container_model_encode_varlen_async, one warp: reads n = *d_n, checks 1 <= n <= n_max
 // (n == 0 is kStatModel, as the fixed call's RB200_E_MODEL; n > n_max is kStatArg) and writes the geometry of a
 // version 1 container of n symbols into *g, with go = 1 when the checks pass.  On failure *g is zero: every later
@@ -312,6 +289,7 @@ __global__ void __launch_bounds__(32)
         r.n = n;
         r.n_chunks = static_cast<uint32_t>(chunks);
         r.dir_len = (chunks + 1) * sizeof(uint64_t);
+        r.dir_off = kContainerDirOffset;
         r.blob_off = (kContainerDirOffset + r.dir_len + 15) & ~15ull;
         r.blob_cap = out_cap - r.blob_off;
         r.go = 1;
@@ -319,10 +297,11 @@ __global__ void __launch_bounds__(32)
     *g = r;
 }
 
-// After the encoder, one thread: blob_len = dir[n_chunks], the length of the blob CRC (crc32_kernel's n_dev)
-__global__ void __launch_bounds__(32) varlen_blob_len_kernel(const uint64_t* __restrict__ dir, VarlenGeom* __restrict__ g)
+// After the encoder, one thread: blob_len = the directory's last entry, the length of the blob CRC (crc32_kernel's
+// n_dev); the directory is at out + dir_off in the container `out`
+__global__ void __launch_bounds__(32) varlen_blob_len_kernel(const uint8_t* __restrict__ out, VarlenGeom* __restrict__ g)
 {
-    if (threadIdx.x == 0 && g->go) g->blob_len = dir[g->n_chunks];
+    if (threadIdx.x == 0 && g->go) g->blob_len = reinterpret_cast<const uint64_t*>(out + g->dir_off)[g->n_chunks];
 }
 
 // The first kernel of rb200_container_blocks_model_encode_varlen_async, one warp: reads n_blocks = *d_n_blocks, checks
@@ -345,13 +324,13 @@ __global__ void __launch_bounds__(32)
     } else {
         const uint64_t chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
         q.n_blocks = n_blocks;
-        q.dir_off = sizeof(ContainerHeader) + kBlockModelBytes * n_blocks;
+        q.v.dir_off = sizeof(ContainerHeader) + kBlockModelBytes * n_blocks;
         q.v.n = static_cast<uint64_t>(n_blocks) * block_size;
         q.v.n_chunks = static_cast<uint32_t>(chunks);
         q.v.dir_len = (chunks + 1) * sizeof(uint64_t);
-        q.v.blob_off = (q.dir_off + q.v.dir_len + 15) & ~15ull;
+        q.v.blob_off = (q.v.dir_off + q.v.dir_len + 15) & ~15ull;
         q.v.blob_cap = out_cap - q.v.blob_off;
-        q.meta_len = q.dir_off + q.v.dir_len - sizeof(ContainerHeader);
+        q.meta_len = q.v.dir_off + q.v.dir_len - sizeof(ContainerHeader);
         q.v.go = 1;
     }
     *g = q;
@@ -362,13 +341,6 @@ __global__ void __launch_bounds__(32)
         r->choice.group = 0;
         r->version = container_blocks_version(r->choice.coder);
     }
-}
-
-// After the encoder, one thread: v.blob_len = the directory's last entry, the length of the blob CRC (crc32_kernel's
-// n_dev); the directory is at out + dir_off, which moves with the count
-__global__ void __launch_bounds__(32) blocks_varlen_blob_len_kernel(const uint8_t* __restrict__ out, BlocksVarlenGeom* __restrict__ g)
-{
-    if (threadIdx.x == 0 && g->v.go) g->v.blob_len = reinterpret_cast<const uint64_t*>(out + g->dir_off)[g->v.n_chunks];
 }
 
 }  // namespace rb200

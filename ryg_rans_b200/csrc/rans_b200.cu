@@ -458,26 +458,20 @@ namespace {
 
 
 // directory + compaction after any encode kernel: sizes[] -> offsets[] + blob.  geom set: the GEOM instances, on grids
-// sized for n_chunks (the bound's), with d_blob the container.  choice set: the GATED instances, which run only when the
-// record names `group`.  bgeom set (with choice; geom is then ignored): the per-block varlen encode, whose scan and
-// compaction also take the directory's place from the record, with d_blob the container and d_offsets unused.
+// sized for n_chunks (the bound's), with d_blob the container, in which they find the directory and the blob from the
+// record (d_offsets unused).  choice set: the GATED instances, which run only when the record names `group`.
 int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* sizes, uint64_t* tile_sums, uint32_t n_chunks,
-                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom, const CoderChoice* choice, uint32_t group,
-                  const BlocksVarlenGeom* bgeom = nullptr)
+                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom, const CoderChoice* choice, uint32_t group)
 {
     if (!n_chunks) {
         RB_CUDA(ctx, cudaMemsetAsync(d_offsets, 0, sizeof(uint64_t), ctx->stream));
         return RB200_OK;
     }
-    if (bgeom) geom = &bgeom->v;
     const uint32_t tiles = (n_chunks + kScanTile - 1) / kScanTile;
-    if (bgeom) {
-        scan_tiles_blocks_kernel<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, d_blob, tile_sums, bgeom, choice, group);
-    } else {
-        auto scan = choice ? (geom ? scan_tiles_kernel<true, true> : scan_tiles_kernel<false, true>)
-                           : (geom ? scan_tiles_kernel<true> : scan_tiles_kernel<false>);
-        scan<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, d_offsets, tile_sums, geom, choice, group);
-    }
+    auto scan = choice ? (geom ? scan_tiles_kernel<true, true> : scan_tiles_kernel<false, true>)
+                       : (geom ? scan_tiles_kernel<true> : scan_tiles_kernel<false>);
+    scan<<<tiles, 1024, 0, ctx->stream>>>(sizes, n_chunks, geom ? reinterpret_cast<uint64_t*>(d_blob) : d_offsets, tile_sums, geom, choice,
+                                          group);
     int rc = check_launch(ctx, "scan_tiles_kernel");
     if (rc != RB200_OK) return rc;
     const uint32_t prefixed = tiles > kTilePrefixThreshold ? 1u : 0u;
@@ -489,11 +483,6 @@ int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* siz
         if (rc != RB200_OK) return rc;
     }
     const uint32_t grid = (n_chunks + kCopyWarps - 1) / kCopyWarps;
-    if (bgeom) {
-        compact_blocks_kernel<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, tile_sums, prefixed, n_chunks, d_blob,
-                                                                         ctx->d_status, bgeom, choice, group);
-        return check_launch(ctx, "compact_blocks_kernel");
-    }
     auto compact = choice ? (geom ? compact_kernel<true, true> : compact_kernel<false, true>)
                           : (geom ? compact_kernel<true> : compact_kernel<false>);
     compact<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, d_offsets, tile_sums, prefixed, n_chunks, d_blob, blob_cap,
@@ -636,10 +625,10 @@ int prepare_workspace(rb200_ctx* ctx, const EncodePlan& p, EncodeWorkspace* ws)
 }
 
 // Runs a plan: prepare its workspace; fused: `launch(ws)`, the one kernel; split: `launch(ws)` encodes into the slots
-// (when there are chunks), then finish_encode (geom, choice, group, bgeom: as there).  `launch` returns check_launch's code.
+// (when there are chunks), then finish_encode (geom, choice, group: as there).  `launch` returns check_launch's code.
 template <class Launch>
 int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom,
-               Launch launch, const CoderChoice* choice = nullptr, uint32_t group = 0, const BlocksVarlenGeom* bgeom = nullptr)
+               Launch launch, const CoderChoice* choice = nullptr, uint32_t group = 0)
 {
     EncodeWorkspace ws = {};
     int rc = prepare_workspace(ctx, p, &ws);
@@ -650,7 +639,7 @@ int run_encode(rb200_ctx* ctx, const EncodePlan& p, uint8_t* d_blob, size_t blob
         if (rc != RB200_OK) return rc;
     }
     return finish_encode(ctx, ws.scratch, p.slot_bytes, ws.sizes, ws.tile_sums, p.n_chunks, d_blob, blob_cap, d_offsets, geom, choice,
-                         group, bgeom);
+                         group);
 }
 
 // The encode tables of one encode call, in device memory.  Word: `word_gate` null runs the instance word_r32 names on
@@ -1209,7 +1198,7 @@ EncodePlan plan_blocks_encode(const rb200_ctx* ctx, int coder, uint32_t sb, uint
         return p;
     }
     int per_sm = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_encode_fused_for(build, p.threads), static_cast<int>(p.threads), p.smem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, block_encode_fused_for(build, false, false, p.threads), static_cast<int>(p.threads), p.smem);
     const uint64_t cta_scratch = static_cast<uint64_t>(p.threads / 32) * kBlockFusedSlots * p.slot_bytes;
     const uint64_t fit = kBlockFusedScratchMax / cta_scratch;                                  // CTAs, the scanner's included
     const uint64_t workers = std::min<uint64_t>(static_cast<uint64_t>(ctx->sms) * std::max(per_sm, 1) - 1,   // the scanner CTA takes one slot
@@ -1223,27 +1212,33 @@ EncodePlan plan_blocks_encode(const rb200_ctx* ctx, int coder, uint32_t sb, uint
 // tables, encode, directory, placement); build_models makes the kernel run count_freqs + normalize_freqs per block first
 // and write d_freqs.  RB200_ENCODE_PATH=split keeps the round-1 sequence (encode into per-chunk slots, tile scan,
 // compaction), which the byte, rans64 and alias coders always run (block_coder_encode_kernel, models of 1 << sb).
+// choice set (with build_models; an auto encode's launch group): the GATED instances of the encoder, the scan, prefix
+// and compaction, which run only when the record names `group`; sb is then the largest scale_bits of the group.  geom
+// set as well (the device-count encode): n_blocks is the bound n_blocks_max, which fixes the plan and every launch
+// shape, the GEOM instances take the count, the directory's and the blob's places from the record, and d_blob is the
+// container, of capacity blob_cap.
 int blocks_encode_device(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* d_in, uint32_t n_blocks, uint32_t block_size,
-                         uint16_t* d_freqs, bool build_models, uint32_t chunk_syms, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets)
+                         uint16_t* d_freqs, bool build_models, uint32_t chunk_syms, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets,
+                         const CoderChoice* choice = nullptr, uint32_t group = 0, const BlocksVarlenGeom* geom = nullptr)
 {
     if (static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) >= (1ull << 31)) return RB200_E_ARG;
     const EncodePlan p = plan_blocks_encode(ctx, coder, sb, n_blocks, block_size, chunk_syms, build_models);
-    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, nullptr, [&](const EncodeWorkspace& ws) {
+    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, geom ? &geom->v : nullptr, [&](const EncodeWorkspace& ws) {
         if (coder != RB200_CODER_WORD) {
             launch_block_coder_encode(ctx->stream, static_cast<uint32_t>(coder), sb, build_models, p.grid, p.threads, p.smem, d_in, block_size,
-                                      d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status);
+                                      d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status, choice, group, geom);
             return check_launch(ctx, "block_coder_encode_kernel");
         }
         if (p.fused) {
-            block_encode_fused_for(build_models, p.threads)<<<p.grid, p.threads, p.smem, ctx->stream>>>(
+            block_encode_fused_for(build_models, choice != nullptr, geom != nullptr, p.threads)<<<p.grid, p.threads, p.smem, ctx->stream>>>(
                 d_in, n_blocks, block_size, d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.look, ws.counter, d_blob, blob_cap, d_offsets,
-                ctx->d_status);
+                ctx->d_status, choice, group, geom, block_size / chunk_syms);
             return check_launch(ctx, "block_encode_fused_kernel");
         }
         block_encode_kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, block_size, d_freqs, chunk_syms, ws.scratch, p.slot_bytes,
                                                                         ws.sizes, ctx->d_status);
         return check_launch(ctx, "block_encode_kernel");
-    });
+    }, choice, group);
 }
 
 // Host mode runs the slice pipeline over whole blocks; the frequency tables go in with each slice when the caller supplies
@@ -1638,35 +1633,138 @@ extern "C" int rb200_container_decode(rb200_ctx* ctx, const uint8_t* buf, size_t
 
 namespace {
 
-// The per-block containers (version 2: the word coder at 12; version 3: byte / rans64; version 4: alias): the block encoder writes every
-// block's model (built, or the caller's tables copied in first), the directory and the blob straight into their place
-// in `out`; then as rb200_container_encode, except that one CRC launch covers model and directory, which are contiguous.
-// Arguments are checked by the caller.
+// The launch groups of an auto encode, one per distinct encoder instance its candidates need: word (both GATED K2 or
+// K2f instances), alias and byte per SB instance of RB200_ALIAS_SB_DISPATCH, rans64.  A group's scale_bits is the
+// largest of its candidates': it sizes the alias encoder's shared memory (no other plan depends on it), and the GATED
+// kernels take the chosen one from the record.
+struct AutoPlan {
+    CandidateList list;
+    int coder[kMaxCandidates];
+    uint32_t sb[kMaxCandidates];
+    uint32_t n_groups;
+};
+
+AutoPlan plan_auto(const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm)
+{
+    AutoPlan a = {};
+    uint32_t key[kMaxCandidates];
+    a.list.n = n_candidates;
+    a.list.tolerance_ppm = tolerance_ppm;
+    for (uint32_t i = 0; i < n_candidates; i++) {
+        const int coder = static_cast<int>(candidates[i] >> 8);
+        const uint32_t sb = candidates[i] & 0xffu;
+        const bool by_sb = (coder == RB200_CODER_ALIAS || coder == RB200_CODER_BYTE) && (sb == 16 || sb == 14 || sb == 12);
+        const uint32_t k = static_cast<uint32_t>(coder) << 8 | (by_sb ? sb : 0u);
+        uint32_t g = 0;
+        while (g < a.n_groups && key[g] != k) g++;
+        if (g == a.n_groups) {
+            key[g] = k;
+            a.coder[g] = coder;
+            a.sb[g] = sb;
+            a.n_groups++;
+        }
+        a.sb[g] = std::max(a.sb[g], sb);
+        a.list.pair[i] = candidates[i];
+        a.list.group[i] = g;
+    }
+    return a;
+}
+
+// the argument rules of every per-block container encode, with n_blocks the count (fixed calls) or its bound
+// n_blocks_max (device-count call)
+bool blocks_container_args_ok(const rb200_ctx* ctx, const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                              const uint8_t* out, int mem_kind)
+{
+    if (!ctx || !in || !out || !container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return false;
+    if (!container_mem_ok(mem_kind, out, nullptr)) return false;
+    return static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) < (1ull << 31);
+}
+
+// The per-block containers (version 2: the word coder at 12; version 3: byte / rans64; version 4: alias) in device
+// memory, enqueue only: the block encoder writes every block's model (built, or the caller's tables copied in first),
+// the directory and the blob straight into their place in `out`; then as rb200_container_encode, except that one CRC
+// launch covers model and directory, which are contiguous, and the header kernel reads blob_bytes = dir[n_chunks].
+// a set (the auto encode, with models built): the choice kernel (after a memset of its sums), one gated encode group per
+// distinct encoder instance of the list, then the CRCs and the per-block header kernel, which writes the chosen
+// version, coder and scale_bits; the layout of versions 2-4 is the same, so the host lays the container out without
+// knowing the choice.  d_n_blocks set as well: h.n_blocks is the bound n_blocks_max, which sizes every launch; the plan
+// kernel reads *d_n_blocks into the record at every run (for a list of one it also writes the choice record, and no
+// choice kernel runs), and every later kernel is its GEOM instance.  Arguments are checked by the caller.
+int blocks_container_encode(rb200_ctx* ctx, const ContainerHeader& h, const uint8_t* in, const uint16_t* caller_freqs,
+                            const uint32_t* d_n_blocks, uint8_t* out, size_t out_cap, const AutoPlan* a = nullptr)
+{
+    const uint32_t n_blocks = h.n_blocks, block_size = h.block_size, chunk_syms = h.chunk_syms;
+    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
+    if (out_cap < boff) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    cudaStream_t s = ctx->stream;
+    BlocksChoice* r = ctx->d_blocks_choice;
+    BlocksVarlenGeom* geom = d_n_blocks ? ctx->d_blocks_geom : nullptr;
+    uint16_t* model = reinterpret_cast<uint16_t*>(out + sizeof(ContainerHeader));
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
+    uint8_t* blob = geom ? out : out + boff;                 // GEOM: the container, in which the kernels place the blob
+    const size_t blob_cap = geom ? out_cap : out_cap - boff;
+    int rc = RB200_OK;
+    if (caller_freqs) RB_CUDA(ctx, cudaMemcpyAsync(model, caller_freqs, dir_off - sizeof(ContainerHeader), cudaMemcpyDeviceToDevice, s));
+    if (a) {
+        for (uint32_t k = 0; k < a->n_groups && rc == RB200_OK; k++)    // every group's workspace before the first launch
+            rc = reserve_plan(ctx, plan_blocks_encode(ctx, a->coder[k], a->sb[k], n_blocks, block_size, chunk_syms, true));
+        if (rc != RB200_OK) return rc;
+        const bool one = geom && a->list.n == 1;
+        if (!one) RB_CUDA(ctx, cudaMemsetAsync(&r->done, 0, sizeof(BlocksChoice) - offsetof(BlocksChoice, done), s));
+        if (geom) {
+            blocks_varlen_plan_kernel<<<1, 32, 0, s>>>(d_n_blocks, n_blocks, block_size, chunk_syms, out_cap, one ? a->list.pair[0] : 0u, geom,
+                                                       r, ctx->d_status);
+            rc = check_launch(ctx, "blocks_varlen_plan_kernel");
+        }
+        if (rc == RB200_OK && !one) {
+            auto choice = geom ? blocks_choice_kernel<true> : blocks_choice_kernel<false>;
+            choice<<<n_blocks, kBlocksChoiceWarps * 32, 0, s>>>(a->list, in, block_size, chunk_syms, r, ctx->d_status, geom);
+            rc = check_launch(ctx, "blocks_choice_kernel");
+        }
+        for (uint32_t k = 0; k < a->n_groups && rc == RB200_OK; k++)
+            rc = blocks_encode_device(ctx, a->coder[k], a->sb[k], in, n_blocks, block_size, model, true, chunk_syms, blob, blob_cap, dir,
+                                      &r->choice, k, geom);
+    } else {
+        rc = blocks_encode_device(ctx, h.coder, h.scale_bits, in, n_blocks, block_size, model, !caller_freqs, chunk_syms, blob, blob_cap, dir);
+    }
+    if (rc == RB200_OK)
+        rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), geom ? &geom->meta_len : nullptr, 0, ctx->d_crc);
+    if (rc == RB200_OK && (h.flags & RB200_CONTAINER_CRC_BLOB)) {
+        if (geom) {
+            varlen_blob_len_kernel<<<1, 32, 0, s>>>(out, &geom->v);
+            rc = check_launch(ctx, "varlen_blob_len_kernel");
+            if (rc == RB200_OK) rc = launch_crc(ctx, out, out_cap, &geom->v.blob_len, 0, ctx->d_crc + 1, &geom->v.blob_off);
+        } else {
+            rc = launch_crc(ctx, out + boff, out_cap - boff, dir + h.n_chunks, 0, ctx->d_crc + 1);
+        }
+    }
+    if (rc != RB200_OK) return rc;
+    if (!a) {
+        container_finish_kernel<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, nullptr, ctx->d_crc, ctx->d_status, nullptr, nullptr);
+        return check_launch(ctx, "container_finish_kernel");
+    }
+    auto finish = geom ? container_blocks_finish_kernel<true> : container_blocks_finish_kernel<false>;
+    finish<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, ctx->d_crc, ctx->d_status, r, geom);
+    return check_launch(ctx, "container_blocks_finish_kernel");
+}
+
+// The fixed per-block container encodes: in device memory blocks_container_encode; in host memory the slice pipeline,
+// then the CRCs and the header on the host.  Arguments are checked by the caller.
 int container_blocks_encode_impl(rb200_ctx* ctx, ContainerHeader h, const uint8_t* in, const uint16_t* block_freqs, uint8_t* out,
                                  size_t out_cap, size_t* out_size, int mem_kind)
 {
-    const bool device = mem_kind == RB200_MEM_DEVICE, build = block_freqs == nullptr;
+    if (mem_kind == RB200_MEM_DEVICE) return blocks_container_encode(ctx, h, in, block_freqs, nullptr, out, out_cap);
+    const bool build = block_freqs == nullptr;
     const uint32_t n_blocks = h.n_blocks, block_size = h.block_size, chunk_syms = h.chunk_syms;
-    const uint64_t n_chunks = h.n_chunks;
-    if (!build && !device && !container_block_models_sum_to(block_freqs, n_blocks, 1u << h.scale_bits)) return RB200_E_MODEL;
+    if (!build && !container_block_models_sum_to(block_freqs, n_blocks, 1u << h.scale_bits)) return RB200_E_MODEL;
     const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
     if (out_cap < boff) return RB200_E_SPACE;
     DeviceGuard g(ctx->device);
     const bool blob_crc = (h.flags & RB200_CONTAINER_CRC_BLOB) != 0;
     uint16_t* model = reinterpret_cast<uint16_t*>(out + sizeof(ContainerHeader));
     uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
-    const size_t model_bytes = dir_off - sizeof(ContainerHeader);
-    if (device) {            // asynchronous: model + directory CRC, blob CRC, then the header from blob_bytes = dir[n_chunks]
-        if (!build) RB_CUDA(ctx, cudaMemcpyAsync(model, block_freqs, model_bytes, cudaMemcpyDeviceToDevice, ctx->stream));
-        int rc = blocks_encode_device(ctx, h.coder, h.scale_bits, in, n_blocks, block_size, model, build, chunk_syms, out + boff, out_cap - boff,
-                                      dir);
-        if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), nullptr, 0, ctx->d_crc);
-        if (rc == RB200_OK && blob_crc) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
-        if (rc != RB200_OK) return rc;
-        container_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_off, boff, out_cap, nullptr, ctx->d_crc, ctx->d_status, nullptr, nullptr);
-        return check_launch(ctx, "container_finish_kernel");
-    }
-    if (!build) std::memcpy(model, block_freqs, model_bytes);
+    if (!build) std::memcpy(model, block_freqs, dir_off - sizeof(ContainerHeader));
     size_t blob_bytes = 0, slices = 0;
     int rc = blocks_encode_host(ctx, h.coder, h.scale_bits, in, n_blocks, block_size, model, build, chunk_syms, out + boff, out_cap - boff,
                                 dir, &blob_bytes, SliceCrc{ctx, blob_crc, &slices});
@@ -1686,10 +1784,7 @@ extern "C" int rb200_container_blocks_encode(rb200_ctx* ctx, const uint8_t* in, 
                                              const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap,
                                              size_t* out_size, int mem_kind)
 {
-    if (!ctx || !in || !out || !container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
-    if (!container_mem_ok(mem_kind, out, nullptr)) return RB200_E_ARG;
-    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
-    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    if (!blocks_container_args_ok(ctx, in, n_blocks, block_size, chunk_syms, out, mem_kind)) return RB200_E_ARG;
     return container_blocks_encode_impl(ctx, container_blocks_header(n_blocks, block_size, chunk_syms, 0, flags), in, block_freqs, out,
                                         out_cap, out_size, mem_kind);
 }
@@ -1701,10 +1796,8 @@ int container_blocks_coder_encode(rb200_ctx* ctx, uint16_t version, int coder, u
                                   uint32_t block_size, const uint16_t* block_freqs, uint32_t chunk_syms, uint32_t flags, uint8_t* out,
                                   size_t out_cap, size_t* out_size, int mem_kind)
 {
-    if (!ctx || !in || !out || coder < 0 || !container_blocks_coder_ok(version, static_cast<uint32_t>(coder), scale_bits)) return RB200_E_ARG;
-    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms) || !container_mem_ok(mem_kind, out, nullptr)) return RB200_E_ARG;
-    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
-    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    if (coder < 0 || !container_blocks_coder_ok(version, static_cast<uint32_t>(coder), scale_bits)) return RB200_E_ARG;
+    if (!blocks_container_args_ok(ctx, in, n_blocks, block_size, chunk_syms, out, mem_kind)) return RB200_E_ARG;
     return container_blocks_encode_impl(
         ctx, container_blocks_coder_header(version, coder, scale_bits, n_blocks, block_size, chunk_syms, 0, flags), in, block_freqs, out,
         out_cap, out_size, mem_kind);
@@ -1899,43 +1992,6 @@ EncodeTables workspace_tables(ModelAsyncWork* w, int coder, uint32_t scale_bits)
                         coder == RB200_CODER_ALIAS ? w->alias_enc : w->byte_enc, w->alias_remap, w->r64_enc};
 }
 
-// The launch groups of an auto encode, one per distinct encoder instance its candidates need: word (both GATED K2 or
-// K2f instances), alias and byte per SB instance of RB200_ALIAS_SB_DISPATCH, rans64.  A group's scale_bits is the
-// largest of its candidates': it sizes the alias encoder's shared memory (no other plan depends on it), and the GATED
-// kernels take the chosen one from the record.
-struct AutoPlan {
-    CandidateList list;
-    int coder[kMaxCandidates];
-    uint32_t sb[kMaxCandidates];
-    uint32_t n_groups;
-};
-
-AutoPlan plan_auto(const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm)
-{
-    AutoPlan a = {};
-    uint32_t key[kMaxCandidates];
-    a.list.n = n_candidates;
-    a.list.tolerance_ppm = tolerance_ppm;
-    for (uint32_t i = 0; i < n_candidates; i++) {
-        const int coder = static_cast<int>(candidates[i] >> 8);
-        const uint32_t sb = candidates[i] & 0xffu;
-        const bool by_sb = (coder == RB200_CODER_ALIAS || coder == RB200_CODER_BYTE) && (sb == 16 || sb == 14 || sb == 12);
-        const uint32_t k = static_cast<uint32_t>(coder) << 8 | (by_sb ? sb : 0u);
-        uint32_t g = 0;
-        while (g < a.n_groups && key[g] != k) g++;
-        if (g == a.n_groups) {
-            key[g] = k;
-            a.coder[g] = coder;
-            a.sb[g] = sb;
-            a.n_groups++;
-        }
-        a.sb[g] = std::max(a.sb[g], sb);
-        a.list.pair[i] = candidates[i];
-        a.list.group[i] = g;
-    }
-    return a;
-}
-
 // The body of both model encodes (model_kernels.cuh): histogram, model kernel, the coder's encoder, the CRCs and the
 // header.  d_n null: n symbols, every length by value.  d_n set: n is the bound n_max, which sizes every launch; the plan
 // kernel reads *d_n into the record at every run, and every later kernel is its GEOM instance.  a set (the auto encode):
@@ -1993,7 +2049,7 @@ int model_encode(rb200_ctx* ctx, int coder, uint32_t scale_bits, const uint8_t* 
     if (rc == RB200_OK) rc = launch_crc(ctx, out + dir_off, dir_end - dir_off, geom ? &geom->dir_len : nullptr, 0, ctx->d_crc);
     if (rc == RB200_OK && blob_crc) {
         if (geom) {
-            varlen_blob_len_kernel<<<1, 32, 0, s>>>(dir, geom);
+            varlen_blob_len_kernel<<<1, 32, 0, s>>>(out, geom);
             rc = check_launch(ctx, "varlen_blob_len_kernel");
             if (rc == RB200_OK) rc = launch_crc(ctx, out, out_cap, &geom->blob_len, 0, ctx->d_crc + 1, &geom->blob_off);
         } else {
@@ -2047,94 +2103,20 @@ extern "C" int rb200_container_model_encode_auto_async(rb200_ctx* ctx, const uin
     return model_encode(ctx, static_cast<int>(candidates[0] >> 8), candidates[0] & 0xffu, in, n, d_n, chunk_syms, flags, out, out_cap, &a);
 }
 
-namespace {
-
-// The per-block encode of one launch group of an auto encode, with models built: the gated K5f instance (word), or the
-// gated K5c instance of the group's dispatch followed by the GATED tile scan, prefix and compaction (byte, rans64,
-// alias).  The plan is the fixed model-building call's for the group's coder and largest scale_bits.
-int blocks_encode_gated(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* d_in, uint32_t n_blocks, uint32_t block_size,
-                        uint16_t* d_freqs, uint32_t chunk_syms, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets,
-                        const CoderChoice* choice, uint32_t group)
-{
-    const EncodePlan p = plan_blocks_encode(ctx, coder, sb, n_blocks, block_size, chunk_syms, true);
-    return run_encode(ctx, p, d_blob, blob_cap, d_offsets, nullptr, [&](const EncodeWorkspace& ws) {
-        if (coder != RB200_CODER_WORD) {
-            launch_block_coder_encode_gated(ctx->stream, static_cast<uint32_t>(coder), sb, p.grid, p.threads, p.smem, d_in, block_size, d_freqs,
-                                            chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status, choice, group);
-            return check_launch(ctx, "block_coder_encode_gated_kernel");
-        }
-        block_encode_fused_gated_for(p.threads)<<<p.grid, p.threads, p.smem, ctx->stream>>>(
-            d_in, n_blocks, block_size, d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.look, ws.counter, d_blob, blob_cap, d_offsets,
-            ctx->d_status, choice, group);
-        return check_launch(ctx, "block_encode_fused_gated_kernel");
-    }, choice, group);
-}
-
-}  // namespace
-
 // rb200_container_blocks_encode / _coder_encode / _alias_encode (DEVICE, models built) with the pair chosen on the GPU
 // at every run: the choice kernel (after a memset of its sums), one gated encode group per distinct encoder instance
-// of the list, the model + directory CRC, the optional blob CRC, the CHOSEN per-block header kernel.  The layout of
-// versions 2-4 is the same, so the host lays the container out without knowing the choice.
+// of the list, the model + directory CRC, the optional blob CRC, the per-block header kernel.
 extern "C" int rb200_container_blocks_model_encode_auto_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
                                                               uint32_t tolerance_ppm, const uint8_t* in, uint32_t n_blocks,
                                                               uint32_t block_size, uint32_t chunk_syms, uint32_t flags, uint8_t* out,
                                                               size_t out_cap)
 {
-    if (!ctx || !in || !out || !blocks_candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
-    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms) || !container_mem_ok(RB200_MEM_DEVICE, out, nullptr)) return RB200_E_ARG;
-    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
-    if (n_chunks >= (1ull << 31)) return RB200_E_ARG;
-    const ContainerHeader h = container_blocks_header(n_blocks, block_size, chunk_syms, 0, flags);
-    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
-    if (out_cap < boff) return RB200_E_SPACE;
-    DeviceGuard g(ctx->device);
+    if (!blocks_candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    if (!blocks_container_args_ok(ctx, in, n_blocks, block_size, chunk_syms, out, RB200_MEM_DEVICE)) return RB200_E_ARG;
     const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
-    int rc = RB200_OK;
-    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++)    // every group's workspace before the first launch
-        rc = reserve_plan(ctx, plan_blocks_encode(ctx, a.coder[k], a.sb[k], n_blocks, block_size, chunk_syms, true));
-    if (rc != RB200_OK) return rc;
-    cudaStream_t s = ctx->stream;
-    BlocksChoice* r = ctx->d_blocks_choice;
-    RB_CUDA(ctx, cudaMemsetAsync(&r->done, 0, sizeof(BlocksChoice) - offsetof(BlocksChoice, done), s));
-    blocks_choice_kernel<<<n_blocks, kBlocksChoiceWarps * 32, 0, s>>>(a.list, in, block_size, chunk_syms, r, ctx->d_status);
-    rc = check_launch(ctx, "blocks_choice_kernel");
-    uint16_t* model = reinterpret_cast<uint16_t*>(out + sizeof(ContainerHeader));
-    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
-    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++)
-        rc = blocks_encode_gated(ctx, a.coder[k], a.sb[k], in, n_blocks, block_size, model, chunk_syms, out + boff, out_cap - boff, dir,
-                                 &r->choice, k);
-    if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), nullptr, 0, ctx->d_crc);
-    if (rc == RB200_OK && (h.flags & RB200_CONTAINER_CRC_BLOB)) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
-    if (rc != RB200_OK) return rc;
-    container_blocks_finish_chosen_kernel<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, ctx->d_crc, ctx->d_status, &r->choice, &r->version);
-    return check_launch(ctx, "container_blocks_finish_chosen_kernel");
+    return blocks_container_encode(ctx, container_blocks_header(n_blocks, block_size, chunk_syms, 0, flags), in, nullptr, nullptr, out,
+                                   out_cap, &a);
 }
-
-namespace {
-
-// The per-block encode of one launch group of a varlen auto encode: blocks_encode_gated's plan for n_blocks_max, which
-// fixes every launch shape, with the varlen instances, which take the count, the directory and the blob's place in the
-// container `out` from the record
-int blocks_encode_varlen(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* d_in, uint32_t n_blocks_max, uint32_t block_size,
-                         uint32_t chunk_syms, uint8_t* out, size_t out_cap, const CoderChoice* choice, uint32_t group,
-                         const BlocksVarlenGeom* geom)
-{
-    const EncodePlan p = plan_blocks_encode(ctx, coder, sb, n_blocks_max, block_size, chunk_syms, true);
-    uint16_t* model = reinterpret_cast<uint16_t*>(out + sizeof(ContainerHeader));
-    return run_encode(ctx, p, out, 0, nullptr, nullptr, [&](const EncodeWorkspace& ws) {
-        if (coder != RB200_CODER_WORD) {
-            launch_block_coder_encode_varlen(ctx->stream, static_cast<uint32_t>(coder), sb, n_blocks_max, p.threads, p.smem, d_in, block_size,
-                                             model, chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status, choice, group, geom);
-            return check_launch(ctx, "block_coder_encode_varlen_kernel");
-        }
-        block_encode_fused_varlen_for(p.threads)<<<p.grid, p.threads, p.smem, ctx->stream>>>(
-            d_in, block_size, model, chunk_syms, ws.scratch, p.slot_bytes, ws.look, ws.counter, out, out_cap, block_size / chunk_syms, ctx->d_status, choice, group, geom);
-        return check_launch(ctx, "block_encode_fused_varlen_kernel");
-    }, choice, group, geom);
-}
-
-}  // namespace
 
 // rb200_container_blocks_model_encode_auto_async with the block count read from device memory at every run: the plan
 // kernel, then the same stages on launch shapes sized for n_blocks_max, each taking the count, the directory's and the
@@ -2145,43 +2127,12 @@ extern "C" int rb200_container_blocks_model_encode_varlen_async(rb200_ctx* ctx, 
                                                                 uint32_t n_blocks_max, uint32_t block_size, uint32_t chunk_syms,
                                                                 uint32_t flags, uint8_t* out, size_t out_cap)
 {
-    if (!ctx || !in || !out || !d_n_blocks || (reinterpret_cast<uintptr_t>(d_n_blocks) & 3) || n_blocks_max == 0) return RB200_E_ARG;
+    if (!d_n_blocks || (reinterpret_cast<uintptr_t>(d_n_blocks) & 3) || n_blocks_max == 0) return RB200_E_ARG;
     if (!blocks_candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
-    if (!container_blocks_geometry_ok(n_blocks_max, block_size, chunk_syms) || !container_mem_ok(RB200_MEM_DEVICE, out, nullptr)) return RB200_E_ARG;
-    const uint64_t n_chunks_max = static_cast<uint64_t>(n_blocks_max) * (block_size / chunk_syms);
-    if (n_chunks_max >= (1ull << 31)) return RB200_E_ARG;
-    const ContainerHeader h = container_blocks_header(n_blocks_max, block_size, chunk_syms, 0, flags);
-    const size_t dir_end_max = container_dir_end(h), boff_max = container_blob_offset(h);
-    if (out_cap < boff_max) return RB200_E_SPACE;
-    DeviceGuard g(ctx->device);
+    if (!blocks_container_args_ok(ctx, in, n_blocks_max, block_size, chunk_syms, out, RB200_MEM_DEVICE)) return RB200_E_ARG;
     const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
-    int rc = RB200_OK;
-    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++)    // every group's workspace before the first launch
-        rc = reserve_plan(ctx, plan_blocks_encode(ctx, a.coder[k], a.sb[k], n_blocks_max, block_size, chunk_syms, true));
-    if (rc != RB200_OK) return rc;
-    cudaStream_t s = ctx->stream;
-    BlocksChoice* r = ctx->d_blocks_choice;
-    BlocksVarlenGeom* geom = ctx->d_blocks_geom;
-    const bool one = n_candidates == 1;
-    if (!one) RB_CUDA(ctx, cudaMemsetAsync(&r->done, 0, sizeof(BlocksChoice) - offsetof(BlocksChoice, done), s));
-    blocks_varlen_plan_kernel<<<1, 32, 0, s>>>(d_n_blocks, n_blocks_max, block_size, chunk_syms, out_cap, one ? candidates[0] : 0u, geom, r,
-                                               ctx->d_status);
-    rc = check_launch(ctx, "blocks_varlen_plan_kernel");
-    if (rc == RB200_OK && !one) {
-        blocks_choice_geom_kernel<<<n_blocks_max, kBlocksChoiceWarps * 32, 0, s>>>(a.list, in, block_size, chunk_syms, r, ctx->d_status, geom);
-        rc = check_launch(ctx, "blocks_choice_geom_kernel");
-    }
-    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++)
-        rc = blocks_encode_varlen(ctx, a.coder[k], a.sb[k], in, n_blocks_max, block_size, chunk_syms, out, out_cap, &r->choice, k, geom);
-    if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end_max - sizeof(ContainerHeader), &geom->meta_len, 0, ctx->d_crc);
-    if (rc == RB200_OK && (h.flags & RB200_CONTAINER_CRC_BLOB)) {
-        blocks_varlen_blob_len_kernel<<<1, 32, 0, s>>>(out, geom);
-        rc = check_launch(ctx, "blocks_varlen_blob_len_kernel");
-        if (rc == RB200_OK) rc = launch_crc(ctx, out, out_cap, &geom->v.blob_len, 0, ctx->d_crc + 1, &geom->v.blob_off);
-    }
-    if (rc != RB200_OK) return rc;
-    container_blocks_finish_varlen_kernel<<<1, 32, 0, s>>>(out, h, out_cap, ctx->d_crc, ctx->d_status, &r->choice, &r->version, geom);
-    return check_launch(ctx, "container_blocks_finish_varlen_kernel");
+    return blocks_container_encode(ctx, container_blocks_header(n_blocks_max, block_size, chunk_syms, 0, flags), in, nullptr, d_n_blocks,
+                                   out, out_cap, &a);
 }
 
 extern "C" int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n)

@@ -491,10 +491,11 @@ word_encode_ring_kernel(const uint8_t* __restrict__ in, uint64_t n, uint32_t chu
 // ---------------------------------------------------------------------------
 constexpr uint32_t kScanTile = 4096;
 
-// GEOM (rb200_container_model_encode_varlen_async): grids sized for n_max, the chunk count, the blob's place in the
-// container `blob` and its capacity from the record (VarlenGeom, device_utils.cuh); CTAs past the real tiles or chunks
-// exit at entry.  The host fixes whether tile_prefix_kernel runs from n_max's tile count; the prefix and the compaction
-// then both use the device's, which gives the same sums as either choice.
+// GEOM (the device-length and device-count encodes): grids sized for the bound, the chunk count and the directory's and
+// blob's places in the container from the record (VarlenGeom, device_utils.cuh), with `offsets` (scan) and `blob`
+// (compaction) the container; CTAs past the real tiles or chunks exit at entry.  The host fixes whether
+// tile_prefix_kernel runs from the bound's tile count; the prefix and the compaction then both use the device's, which
+// gives the same sums as either choice.
 // GATED (rb200_container_model_encode_auto_async): the three kernels run only when the choice record (CoderChoice,
 // device_utils.cuh) names `group`, the launch group whose split encoder they finish; otherwise they exit at entry.
 template <bool GEOM, bool GATED>
@@ -506,6 +507,7 @@ __device__ __forceinline__ void scan_tiles(const uint32_t* __restrict__ sizes, u
     if (GEOM) {
         n_chunks = geom->n_chunks;
         if (!geom->go || blockIdx.x * kScanTile >= n_chunks) return;
+        offsets = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(offsets) + geom->dir_off);
     }
     __shared__ uint64_t s_warp[32];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -549,15 +551,6 @@ scan_tiles_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_
                   uint32_t group)
 {
     scan_tiles<GEOM, GATED>(sizes, n_chunks, offsets, tile_sums, geom, choice, group);
-}
-
-// The GEOM and GATED scan of rb200_container_blocks_model_encode_varlen_async, whose directory sits after the models
-// of the record's count: at out + geom->dir_off (BlocksVarlenGeom)
-__global__ void __launch_bounds__(1024)
-scan_tiles_blocks_kernel(const uint32_t* __restrict__ sizes, uint32_t n_chunks, uint8_t* __restrict__ out, uint64_t* __restrict__ tile_sums,
-                         const BlocksVarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
-{
-    scan_tiles<true, true>(sizes, n_chunks, reinterpret_cast<uint64_t*>(out + geom->dir_off), tile_sums, &geom->v, choice, group);
 }
 
 // for very large directories: turn tile_sums into exclusive prefixes once, so compact CTAs read one value
@@ -617,6 +610,7 @@ __device__ __forceinline__ void compact(const uint8_t* __restrict__ scratch, uin
     if (GEOM) {
         n_chunks = geom->n_chunks;
         if (!geom->go || blockIdx.x * kCopyWarps >= n_chunks) return;
+        offsets = reinterpret_cast<uint64_t*>(blob + geom->dir_off);
         blob += geom->blob_off;
         blob_cap = geom->blob_cap;
     }
@@ -659,18 +653,6 @@ compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const u
                const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
 {
     compact<GEOM, GATED>(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, blob, blob_cap, status, geom, choice, group);
-}
-
-// The GEOM and GATED compaction of rb200_container_blocks_model_encode_varlen_async: the directory at out +
-// geom->dir_off, the blob at out + geom->v.blob_off (BlocksVarlenGeom)
-__global__ void __launch_bounds__(kCopyWarps * 32)
-compact_blocks_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
-                      const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed, uint32_t n_chunks, uint8_t* __restrict__ out,
-                      uint32_t* __restrict__ status, const BlocksVarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice,
-                      uint32_t group)
-{
-    compact<true, true>(scratch, slot_bytes, sizes, reinterpret_cast<uint64_t*>(out + geom->dir_off), tile_sums, tiles_prefixed, n_chunks, out,
-                        0, status, &geom->v, choice, group);
 }
 
 // the K2 and K2f instances: (R32, GATED, GEOM) = (r32, 0, 0) for an rb200_model, (r32, 1, 0) and (r32, 1, 1) for the

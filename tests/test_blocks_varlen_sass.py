@@ -1,6 +1,7 @@
-"""The kernels of rb200_container_blocks_model_encode_varlen_async spill no more than the shipped kernels they are built
-around: every new function has no more local-memory stores and loads in its SASS than its twin of the fixed auto encode
-(the 8-warp K5f instance keeps the shipped body's spill; every other one has none).  No GPU needed."""
+"""The GATED and GEOM instances of the per-block container encodes (rb200_container_blocks_model_encode_auto_async and
+its device-count form rb200_container_blocks_model_encode_varlen_async) spill no more than the flags-off instance of
+the same stage: every such function has no more local-memory stores and loads in its SASS than the instance the fixed
+calls run (the 8-warp K5f instances keep the shipped body's spill; every other one has none).  No GPU needed."""
 import os
 import re
 import shutil
@@ -16,18 +17,21 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
 
-# (new function, the shipped twin it is built around); a twin of None: the function has no twin and must not spill
-TWINS = [
-    ("blocks_varlen_plan_kernel", None),
-    ("blocks_varlen_blob_len_kernel", None),
-    ("blocks_choice_geom_kernel", "blocks_choice_kernel"),
-    ("block_encode_fused_varlen_kernelILi8E", "block_encode_fused_gated_kernelILi8E"),
-    ("block_encode_fused_varlen_kernelILi32E", "block_encode_fused_gated_kernelILi32E"),
-    ("scan_tiles_blocks_kernel", "scan_tiles_kernelILb1ELb1E"),
-    ("compact_blocks_kernel", "compact_kernelILb1ELb1E"),
-    ("container_blocks_finish_varlen_kernel", "container_blocks_finish_chosen_kernel"),
-] + [(f"block_coder_encode_varlen_kernelILj{c}ELj{sb}E", f"block_coder_encode_gated_kernelILj{c}ELj{sb}E")
-     for c, sb in ((1, 0), (1, 12), (1, 14), (2, 0), (2, 12), (2, 14), (3, 0))]
+# (GATED or GEOM instance, the flags-off instance of the same stage); None: the function has no flags-off instance and
+# must not spill
+CODER_SB = ((1, 0), (1, 12), (1, 14), (2, 0), (2, 12), (2, 14), (3, 0))
+TWINS = (
+    [("blocks_varlen_plan_kernel", None),
+     ("varlen_blob_len_kernel", None),
+     ("blocks_choice_kernelILb1E", "blocks_choice_kernelILb0E")]
+    + [(f"block_encode_fused_kernelILb1ELi{w}ELb1ELb{geom}E", f"block_encode_fused_kernelILb1ELi{w}ELb0ELb0E")
+       for w in (8, 32) for geom in (0, 1)]
+    + [(f"{k}ILb{geom}ELb{gated}E", f"{k}ILb0ELb0E")
+       for k in ("scan_tiles_kernel", "tile_prefix_kernel", "compact_kernel") for geom, gated in ((0, 1), (1, 0), (1, 1))]
+    + [(f"container_blocks_finish_kernelILb{geom}E", "container_finish_kernelILb0ELb0E") for geom in (0, 1)]
+    + [(f"block_coder_encode_kernelILj{c}ELj{sb}ELb1ELb1ELb{geom}E", f"block_coder_encode_kernelILj{c}ELj{sb}ELb1ELb0ELb0E")
+       for c, sb in CODER_SB for geom in (0, 1)]
+)
 
 
 @pytest.fixture(scope="module")
