@@ -1,24 +1,28 @@
-// block_coder_kernels.cuh -- per-block models for the byte (main.cpp), rans64 (main64.cpp) and alias (main_alias.cpp)
-// coders at scale_bits 8..15:
-// the version 2 geometry (one CTA per block, one warp per chunk, at most 32 chunks per block) with each block's model
-// normalised to 1 << scale_bits instead of 4096.
+// block_coder_kernels.cuh -- the split encoder and the decoder of every per-block coder: the word coder
+// (rans_word_sse41.h) at scale_bits 12, and the byte (main.cpp), rans64 (main64.cpp) and alias (main_alias.cpp) coders
+// at scale_bits 8..15.  One CTA per block, one warp per chunk, at most 32 chunks per block, each block's model
+// normalised to 1 << scale_bits.
 //
 //   block_coder_encode_kernel<CODER, SB, BUILD>
 //                          BUILD: count_freqs + normalize_freqs(1 << sb) of the block (block_model_build_wide, bit-exact,
 //                          written to block_freqs); else the caller's row.  Then the block's encoder table in shared
-//                          memory from the tables.h formulas (byte_enc_entry / rans64_enc_entry, 8x replicated as K8 / K9
-//                          stage it), and encode_chunk_split per warp with AliasEncoder<false, SB> / Rans64Encoder: the
-//                          split path's slots, followed by K6's tile scan and compaction
-//   block_coder_decode_kernel<CODER, SB>
-//                          the block's decode table in shared memory (cum2sym[1 << sb], then byte_dec_symbol x 256 or
-//                          rans64's 16x replicated {start, freq}), then decode_window_chunk per warp with ByteDecoder<SB> /
-//                          Rans64Decoder
+//                          memory: the word coder's reciprocal table (block_build_enc_table, WordEncoder<r32>), or the
+//                          tables.h formulas (byte_enc_entry / rans64_enc_entry, 8x replicated as K8 / K9 stage it), and
+//                          encode_chunk_split per warp with AliasEncoder<false, SB> / Rans64Encoder: the split path's
+//                          slots, followed by K6's tile scan and compaction.  The word coder has the flags-off instance
+//                          only: a word encode that builds its models runs K5f (block_encode_fused_kernel).
+//   block_decode_kernel<CODER, SB>
+//                          the block's decode table in shared memory (block_decode_table: the word coder's 4096 slot
+//                          entries, RansWordTablesInitSymbol of rans_word_sse41.h:64-72; cum2sym[1 << sb], then
+//                          byte_dec_symbol x 256 or rans64's 16x replicated {start, freq}), then each warp's chunk
+//                          (block_decode_chunk: decode_window_chunk with WordDecoder<WIDE> / ByteDecoder<SB> / Rans64Decoder).
+//                          container_decode.cuh's block_decode_planned_kernel runs the same two steps per block.
 //   CODER = RB200_CODER_ALIAS  the block's alias table built by the CTA (block_alias_tables, over the coding table's place),
 //                          then AliasEncoder<true, SB> with the remap (block_alias_remap, after the warps' stages) or
 //                          AliasDecoder<SB, lean> on kAliasDecReplicas copies of the 256 bucket entries
 //
 // A block whose frequencies do not sum to 1 << sb: the encoder codes it with an empty model (every symbol flagged,
-// RB200_E_SYMBOL), the decoder flags kStatStream and decodes nothing of it, as K5 does for the word coder.
+// RB200_E_SYMBOL), the decoder flags kStatStream and decodes nothing of it.
 #pragma once
 #include "alias_kernels.cuh"
 #include "block_kernels.cuh"
@@ -158,21 +162,22 @@ __device__ __forceinline__ void block_alias_remap(const AliasBuildSmem& a, uint3
     }
 }
 
-// dynamic shared memory of the per-block encoder: the 32 KiB table, then 1 KiB per warp (as K5's); the alias coder's
-// remap (u16, 1 << sb entries) after them
-inline uint32_t block_coder_encode_smem(uint32_t threads) { return block_encode_smem(threads); }
+// dynamic shared memory of the split per-block encoder: the 32 KiB table, then 1 KiB per warp (as K5f's); the alias
+// coder's remap (u16, 1 << sb entries) after them
 inline uint32_t block_coder_encode_smem(uint32_t coder, uint32_t sb, uint32_t threads)
 {
     return block_encode_smem(threads) + (coder == RB200_CODER_ALIAS ? (2u << sb) : 0u);
 }
 
-// dynamic shared memory of the per-block decoder: 1 KiB of stream window per warp, cum2sym, then the symbol entries
+// dynamic shared memory of the per-block decoders: 1 KiB of stream window per warp, then the table: the word coder's
+// 4096 slot entries, the alias coder's bucket entries, or cum2sym and the symbol entries
 __host__ __device__ constexpr uint32_t block_coder_sym_bytes(uint32_t coder)
 {
     return coder == RB200_CODER_BYTE ? 256 * 4 : kRans64DecSymBytes;
 }
 inline uint32_t block_coder_decode_smem(uint32_t coder, uint32_t sb, uint32_t threads)
 {
+    if (coder == RB200_CODER_WORD) return (threads / 32) * kRingBytes + kWordSlots * 4;
     if (coder == RB200_CODER_ALIAS) return (threads / 32) * kRingBytes + 256 * kAliasDecReplicas * 16;   // the bucket table
     return (threads / 32) * kRingBytes + (1u << sb) + block_coder_sym_bytes(coder);
 }
@@ -190,13 +195,7 @@ __device__ __forceinline__ void block_coder_encode(const uint8_t* __restrict__ i
     const uint32_t tid = threadIdx.x, warp = tid >> 5;
     const uint8_t* blk = in + static_cast<uint64_t>(blockIdx.x) * block_size;
     uint16_t* freqs = block_freqs + static_cast<uint64_t>(blockIdx.x) * 256;
-    bool ok;
-    if (BUILD) {
-        block_model_build_wide(blk, block_size, reinterpret_cast<uint32_t*>(s_benc), s_cnt, s_cum, s_w, freqs, status, M);
-        ok = block_prefix(s_w, s_cum, &s_flag[0], M);                // the widths are still in shared memory
-    } else {
-        ok = block_prefix(static_cast<const uint16_t*>(freqs), s_cum, &s_flag[0], M);
-    }
+    bool ok = block_model_prefix<BUILD>(blk, block_size, freqs, reinterpret_cast<uint32_t*>(s_benc), s_cnt, s_cum, s_w, &s_flag[0], status, M);
     const uint32_t warps = blockDim.x >> 5;
     const uint32_t remap = smem_addr(s_benc) + kEncTableBytes + warps * kEncWarpSmem;
     if (CODER == RB200_CODER_ALIAS && ok) {
@@ -206,34 +205,43 @@ __device__ __forceinline__ void block_coder_encode(const uint8_t* __restrict__ i
         if (ok) block_alias_remap(a, M, reinterpret_cast<uint16_t*>(s_benc + kEncTableBytes + warps * kEncWarpSmem));
         __syncthreads();
     }
-    // the encoder table as K8 / K9 stage theirs: one 16-byte entry per symbol, kEncReplicas copies
     uint4* s_tab = reinterpret_cast<uint4*>(s_benc);
-    for (uint32_t s = tid; s < 256; s += blockDim.x) {
-        const uint32_t f = ok ? s_cum[s + 1] - s_cum[s] : 0, cum = ok ? s_cum[s] : 0;
-        uint4 x;
-        if (CODER == RB200_CODER_ALIAS) {
-            // a symbol outside the model: freq 1 keeps the step well defined, the flag reports it (as K4 stages it)
-            const AliasEncEntry e = alias_enc_entry(f, cum);          // {magic, freq, cum, shift}
-            x = f ? make_uint4(e.magic, e.freq, e.cum, e.shift) : make_uint4(0, 1, 0, kEncBadSymbol);
-        } else if (CODER == RB200_CODER_BYTE) {
-            const AliasEncEntry e = byte_enc_entry(f, cum, sb);       // {x_max, rcp_freq, bias, cmpl_freq | rcp_shift << 16}
-            x = make_uint4(e.magic, e.freq, e.cum, e.shift);
-        } else {
-            uint32_t e[8];
-            rans64_enc_entry(f, cum, sb, e);                          // {rcp_lo, rcp_hi, freq, bias}, {cmpl_freq, shift | bad}
-            x = make_uint4(e[0], e[1], e[3], (e[4] & 0xfffffu) | ((e[5] & 63u) << 20) | (e[5] & kEncBadSymbol));
-        }
+    bool r32 = false;
+    if (CODER == RB200_CODER_WORD) {
+        r32 = block_build_enc_table(s_cum, ok, s_tab);              // ends with a CTA barrier
+    } else {
+        // the encoder table as K8 / K9 stage theirs: one 16-byte entry per symbol, kEncReplicas copies
+        for (uint32_t s = tid; s < 256; s += blockDim.x) {
+            const uint32_t f = ok ? s_cum[s + 1] - s_cum[s] : 0, cum = ok ? s_cum[s] : 0;
+            uint4 x;
+            if (CODER == RB200_CODER_ALIAS) {
+                // a symbol outside the model: freq 1 keeps the step well defined, the flag reports it (as K4 stages it)
+                const AliasEncEntry e = alias_enc_entry(f, cum);      // {magic, freq, cum, shift}
+                x = f ? make_uint4(e.magic, e.freq, e.cum, e.shift) : make_uint4(0, 1, 0, kEncBadSymbol);
+            } else if (CODER == RB200_CODER_BYTE) {
+                const AliasEncEntry e = byte_enc_entry(f, cum, sb);   // {x_max, rcp_freq, bias, cmpl_freq | rcp_shift << 16}
+                x = make_uint4(e.magic, e.freq, e.cum, e.shift);
+            } else {
+                uint32_t e[8];
+                rans64_enc_entry(f, cum, sb, e);                      // {rcp_lo, rcp_hi, freq, bias}, {cmpl_freq, shift | bad}
+                x = make_uint4(e[0], e[1], e[3], (e[4] & 0xfffffu) | ((e[5] & 63u) << 20) | (e[5] & kEncBadSymbol));
+            }
 #pragma unroll
-        for (uint32_t r = 0; r < kEncReplicas; r++) s_tab[s * kEncReplicas + r] = x;
+            for (uint32_t r = 0; r < kEncReplicas; r++) s_tab[s * kEncReplicas + r] = x;
+        }
+        __syncthreads();
     }
-    __syncthreads();
 
     const uint32_t per_block = block_size / chunk_syms;
     if (warp >= per_block) return;
     const uint32_t chunk = blockIdx.x * per_block + warp;
     const uint8_t* src = blk + static_cast<uint64_t>(warp) * chunk_syms;
     const uint32_t tab = smem_addr(s_benc), wsm = tab + kEncTableBytes + warp * kEncWarpSmem;
-    if (CODER == RB200_CODER_ALIAS)
+    if (CODER == RB200_CODER_WORD && r32)
+        encode_chunk_split(src, chunk_syms, chunk, WordEncoder<true>{tab}, wsm, scratch, slot_bytes, sizes, status);
+    else if (CODER == RB200_CODER_WORD)
+        encode_chunk_split(src, chunk_syms, chunk, WordEncoder<false>{tab}, wsm, scratch, slot_bytes, sizes, status);
+    else if (CODER == RB200_CODER_ALIAS)
         encode_chunk_split(src, chunk_syms, chunk, AliasEncoder<true, SB>{tab, remap, sb}, wsm, scratch, slot_bytes, sizes, status);
     else if (CODER == RB200_CODER_BYTE)
         encode_chunk_split(src, chunk_syms, chunk, AliasEncoder<false, SB>{tab, 0, sb}, wsm, scratch, slot_bytes, sizes, status);
@@ -249,9 +257,9 @@ __device__ __forceinline__ void block_coder_encode(const uint8_t* __restrict__ i
 template <uint32_t CODER, uint32_t SB, bool BUILD, bool GATED = false, bool GEOM = false>
 __global__ void __launch_bounds__(kMaxBlockWarps * 32)
 block_coder_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, uint16_t* __restrict__ block_freqs, uint32_t sb_rt,
-                          uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
-                          uint32_t* __restrict__ status, const CoderChoice* __restrict__ choice, uint32_t group,
-                          const BlocksVarlenGeom* __restrict__ geom)
+                    uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
+                    uint32_t* __restrict__ status, const CoderChoice* __restrict__ choice, uint32_t group,
+                    const BlocksVarlenGeom* __restrict__ geom)
 {
     if ((GATED && choice->group != group) || (GEOM && blockIdx.x >= geom->n_blocks)) return;   // the group is the same for the whole grid
     block_coder_encode<CODER, SB, BUILD>(in, block_size, block_freqs, GATED ? choice->scale_bits : sb_rt, chunk_syms, scratch, slot_bytes,
@@ -326,94 +334,129 @@ __device__ __forceinline__ bool block_alias_decode_table(const uint32_t* s_cum, 
     return true;
 }
 
+// A block's decode table in dynamic shared memory after the `warps` 1 KiB stream windows at s_dyn, from its model (freqs:
+// 256 x u16, summing to M = 1 << sb), for block_decode_chunk:
+// the word coder's slot table, with s_flag[1] set when one symbol takes all 4096 slots (the WIDE decoder); the alias
+// coder's bucket entries; cum2sym and the symbol entries otherwise.  s_flag[0] is block_prefix's.  Every thread of the
+// CTA takes part and gets the same result: false when the model does not sum to M (or, alias, does not pair), with no
+// table built; true after a CTA barrier.
 template <uint32_t CODER, uint32_t SB>
-__global__ void __launch_bounds__(kMaxBlockWarps * 32)
-block_coder_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets,
-                          const uint16_t* __restrict__ block_freqs, uint32_t sb_rt, uint32_t block_size, uint32_t chunk_syms,
-                          uint8_t* __restrict__ out, uint32_t* __restrict__ status)
+__device__ __forceinline__ bool block_decode_table(const uint16_t* freqs, uint32_t M, uint32_t* s_cum, uint32_t* s_flag, uint8_t* s_dyn,
+                                                   uint32_t warps)
 {
-    extern __shared__ __align__(1024) uint8_t s_bdec[];         // [warps x 1 KiB rings][cum2sym[1 << sb]][symbol entries]
-    __shared__ uint32_t s_cum[257];
-    __shared__ uint32_t s_flag[1];
-    const uint32_t sb = SB ? SB : sb_rt, M = 1u << sb;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, warps = blockDim.x >> 5;
-    if (!block_prefix(block_freqs + static_cast<uint64_t>(blockIdx.x) * 256, s_cum, &s_flag[0], M)) {
-        if (tid == 0) atomicOr(status, kStatStream);
-        return;
-    }
-    uint8_t* s_tab = s_bdec + warps * kRingBytes;
-    if (CODER == RB200_CODER_ALIAS) {
-        if (!block_alias_decode_table<SB>(s_cum, s_tab, M)) {
-            if (tid == 0) atomicOr(status, kStatStream);
-            return;
-        }
-    } else {
+    if (CODER == RB200_CODER_WORD && threadIdx.x == 0) s_flag[1] = 0;
+    if (!block_prefix(freqs, s_cum, &s_flag[0], M)) return false;
+    uint8_t* s_tab = s_dyn + warps * kRingBytes;
+    if (CODER == RB200_CODER_WORD)
+        block_fill_slots(s_cum, reinterpret_cast<uint32_t*>(s_tab), &s_flag[1]);
+    else if (CODER == RB200_CODER_ALIAS && !block_alias_decode_table<SB>(s_cum, s_tab, M))
+        return false;
+    else if (CODER != RB200_CODER_ALIAS)
         block_coder_decode_table<CODER>(s_cum, s_tab, M);
-    }
     __syncthreads();
+    return true;
+}
 
-    const uint32_t per_block = block_size / chunk_syms;
-    if (warp >= per_block) return;
-    const uint32_t chunk = blockIdx.x * per_block + warp;
-    uint8_t* dst = out + static_cast<uint64_t>(blockIdx.x) * block_size + static_cast<uint64_t>(warp) * chunk_syms;
-    const uint32_t ring = smem_addr(s_bdec) + warp * kRingBytes, tab = smem_addr_pinned(s_tab);
-    if (CODER == RB200_CODER_ALIAS)
+// One chunk of a block through the warp's 1 KiB stream window at shared address ring, on the table block_decode_table
+// built at shared address tab; wide: its s_flag[1] (word coder only).
+template <uint32_t CODER, uint32_t SB>
+__device__ __forceinline__ void block_decode_chunk(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets,
+                                                   uint32_t chunk, uint32_t ring, uint32_t tab, uint32_t sb, bool wide, uint8_t* __restrict__ dst,
+                                                   uint32_t chunk_syms, uint32_t* __restrict__ status)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    if (CODER == RB200_CODER_WORD && wide)
+        decode_window_chunk(WordDecoder<true>{tab, 0}, blob, blob_size, offsets, chunk, ring, dst, chunk_syms, status);
+    else if (CODER == RB200_CODER_WORD)
+        decode_window_chunk(WordDecoder<false>{tab, 0}, blob, blob_size, offsets, chunk, ring, dst, chunk_syms, status);
+    else if (CODER == RB200_CODER_ALIAS)
         decode_window_chunk(AliasDecoder<SB, kAliasLean>{tab + (lane & (kAliasDecReplicas - 1)) * 16, sb}, blob, blob_size, offsets, chunk,
                             ring, dst, chunk_syms, status);
     else if (CODER == RB200_CODER_BYTE)
         decode_window_chunk(ByteDecoder<SB>{tab, sb}, blob, blob_size, offsets, chunk, ring, dst, chunk_syms, status);
     else
-        decode_window_chunk(Rans64Decoder{tab, tab + M + (lane & (kRans64DecReplicas - 1)) * 8, sb}, blob, blob_size, offsets, chunk, ring,
-                            dst, chunk_syms, status);
+        decode_window_chunk(Rans64Decoder{tab, tab + (1u << sb) + (lane & (kRans64DecReplicas - 1)) * 8, sb}, blob, blob_size, offsets, chunk,
+                            ring, dst, chunk_syms, status);
 }
 
-// The instances: the byte coder specialised for scale_bits 14 (main.cpp) and 12, generic otherwise, as K8; rans64 generic
-#define RB200_BLOCK_CODER_DISPATCH(coder, sb, CALL)                                      \
-    if (coder == RB200_CODER_RANS64) {                                                   \
-        constexpr uint32_t CODER = RB200_CODER_RANS64, SB = 0; CALL;                     \
-    } else if (sb == 14) {                                                               \
-        constexpr uint32_t CODER = RB200_CODER_BYTE, SB = 14; CALL;                      \
+// K5: one CTA per block, launched by the host
+template <uint32_t CODER, uint32_t SB>
+__global__ void __launch_bounds__(kMaxBlockWarps * 32)
+block_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets,
+                    const uint16_t* __restrict__ block_freqs, uint32_t sb_rt, uint32_t block_size, uint32_t chunk_syms,
+                    uint8_t* __restrict__ out, uint32_t* __restrict__ status)
+{
+    extern __shared__ __align__(1024) uint8_t s_bdec[];         // [warps x 1 KiB rings][the block's decode table]
+    __shared__ uint32_t s_cum[257];
+    __shared__ uint32_t s_flag[2];                              // [0] bad model, [1] wide (word coder)
+    const uint32_t sb = SB ? SB : sb_rt;
+    const uint32_t tid = threadIdx.x, warp = tid >> 5, warps = blockDim.x >> 5;
+    if (!block_decode_table<CODER, SB>(block_freqs + static_cast<uint64_t>(blockIdx.x) * 256, 1u << sb, s_cum, s_flag, s_bdec, warps)) {
+        if (tid == 0) atomicOr(status, kStatStream);
+        return;
+    }
+    const uint32_t per_block = block_size / chunk_syms;
+    if (warp >= per_block) return;
+    uint8_t* dst = out + static_cast<uint64_t>(blockIdx.x) * block_size + static_cast<uint64_t>(warp) * chunk_syms;
+    block_decode_chunk<CODER, SB>(blob, blob_size, offsets, blockIdx.x * per_block + warp, smem_addr(s_bdec) + warp * kRingBytes,
+                                  smem_addr_pinned(s_bdec + warps * kRingBytes), sb, CODER == RB200_CODER_WORD && s_flag[1], dst, chunk_syms,
+                                  status);
+}
+
+// Every per-block instance, in the order of the planned decoders' ids (container_decoder): the word coder at scale_bits
+// 12; the byte coder specialised for scale_bits 14 (main.cpp) and 12, generic otherwise, as K8; rans64 generic; the
+// alias coder at the byte coder's scale_bits.
+#define RB200_BLOCK_SB_DISPATCH(C, sb, CALL)                                             \
+    if (sb == 14) {                                                                      \
+        constexpr uint32_t CODER = C, SB = 14; CALL;                                     \
     } else if (sb == 12) {                                                               \
-        constexpr uint32_t CODER = RB200_CODER_BYTE, SB = 12; CALL;                      \
+        constexpr uint32_t CODER = C, SB = 12; CALL;                                     \
     } else {                                                                             \
-        constexpr uint32_t CODER = RB200_CODER_BYTE, SB = 0; CALL;                       \
+        constexpr uint32_t CODER = C, SB = 0; CALL;                                      \
+    }
+#define RB200_BLOCK_DISPATCH(coder, sb, CALL)                                            \
+    if (coder == RB200_CODER_WORD) {                                                     \
+        constexpr uint32_t CODER = RB200_CODER_WORD, SB = kWordScaleBits; CALL;          \
+    } else if (coder == RB200_CODER_RANS64) {                                            \
+        constexpr uint32_t CODER = RB200_CODER_RANS64, SB = 0; CALL;                     \
+    } else if (coder == RB200_CODER_ALIAS) {                                             \
+        RB200_BLOCK_SB_DISPATCH(RB200_CODER_ALIAS, sb, CALL)                             \
+    } else {                                                                             \
+        RB200_BLOCK_SB_DISPATCH(RB200_CODER_BYTE, sb, CALL)                              \
     }
 
-// The alias coder's instances (rb200_blocks_alias_*), the same scale_bits specialised: 14 (main.cpp's) and 12, generic
-// otherwise.  A dispatch of its own, so that RB200_BLOCK_CODER_DISPATCH stays the version 3 decoders' list.
-#define RB200_BLOCK_ALIAS_DISPATCH(sb, CALL)                                             \
-    if (sb == 14) {                                                                      \
-        constexpr uint32_t CODER = RB200_CODER_ALIAS, SB = 14; CALL;                     \
-    } else if (sb == 12) {                                                               \
-        constexpr uint32_t CODER = RB200_CODER_ALIAS, SB = 12; CALL;                     \
-    } else {                                                                             \
-        constexpr uint32_t CODER = RB200_CODER_ALIAS, SB = 0; CALL;                      \
-    }
-// every per-block coder instance
-#define RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, CALL)                                  \
-    if (coder == RB200_CODER_ALIAS) {                                                    \
-        RB200_BLOCK_ALIAS_DISPATCH(sb, CALL)                                             \
-    } else {                                                                             \
-        RB200_BLOCK_CODER_DISPATCH(coder, sb, CALL)                                      \
-    }
+// The split encoder instance of (CODER, SB): (BUILD, GATED, GEOM) = (build, 0, 0) for the fixed calls, (1, 1, 0) for the
+// auto encode, (1, 1, 1) for the device-count encode.  The word coder has only (0, 0, 0), null for any other flags: its
+// model-building encodes run K5f (plan_blocks_encode).
+using BlockEncodeKernel = decltype(&block_coder_encode_kernel<RB200_CODER_BYTE, 0, false>);
+template <uint32_t CODER, uint32_t SB>
+inline BlockEncodeKernel block_encode_for(bool build, bool gated, bool geom)
+{
+    if constexpr (CODER == RB200_CODER_WORD) return build || gated || geom ? nullptr : block_coder_encode_kernel<CODER, SB, false>;
+    else if (geom) return block_coder_encode_kernel<CODER, SB, true, true, true>;
+    else if (gated) return block_coder_encode_kernel<CODER, SB, true, true>;
+    else return build ? block_coder_encode_kernel<CODER, SB, true> : block_coder_encode_kernel<CODER, SB, false>;
+}
 
 template <uint32_t CODER, uint32_t SB>
 inline void configure_block_coder()
 {
-    for (const void* k : {reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, true>),
-                          reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, false>),
-                          reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, true, true>),
-                          reinterpret_cast<const void*>(block_coder_encode_kernel<CODER, SB, true, true, true>)}) {
+    for (const BlockEncodeKernel k : {block_encode_for<CODER, SB>(true, false, false), block_encode_for<CODER, SB>(false, false, false),
+                                      block_encode_for<CODER, SB>(true, true, false), block_encode_for<CODER, SB>(true, true, true)}) {
+        if (!k) continue;
         cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              block_coder_encode_smem(CODER, kBlockCoderMaxScaleBits, kMaxBlockWarps * 32));
     }
-    cudaFuncSetAttribute(block_coder_decode_kernel<CODER, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(block_coder_decode_kernel<CODER, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaFuncSetAttribute(block_decode_kernel<CODER, SB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(block_decode_kernel<CODER, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          block_coder_decode_smem(CODER, kBlockCoderMaxScaleBits, kMaxBlockWarps * 32));
 }
-inline void configure_block_coder_kernels()
+
+// every per-block kernel: the instances of RB200_BLOCK_DISPATCH and K5f's
+inline void configure_block_kernels()
 {
+    configure_block_coder<RB200_CODER_WORD, kWordScaleBits>();
     configure_block_coder<RB200_CODER_BYTE, 14>();
     configure_block_coder<RB200_CODER_BYTE, 12>();
     configure_block_coder<RB200_CODER_BYTE, 0>();
@@ -421,33 +464,36 @@ inline void configure_block_coder_kernels()
     configure_block_coder<RB200_CODER_ALIAS, 14>();
     configure_block_coder<RB200_CODER_ALIAS, 12>();
     configure_block_coder<RB200_CODER_ALIAS, 0>();
+    for (const uint32_t threads : {8u * 32, 32u * 32})
+        for (const BlockEncodeFusedKernel k : {block_encode_fused_for(true, false, false, threads), block_encode_fused_for(false, false, false, threads),
+                                               block_encode_fused_for(true, true, false, threads), block_encode_fused_for(true, true, true, threads)}) {
+            cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
+        }
 }
 
 // one CTA per block of block_threads() threads; smem = block_coder_encode_smem(coder, sb, threads).  choice set: the
 // GATED instance of (coder, sb)'s dispatch, with models built, where sb is the largest scale_bits of the launch group,
 // which sizes the alias coder's remap, and the kernel takes the chosen one from the record; geom set as well: the GEOM
 // instance, on a grid of n_blocks = n_blocks_max CTAs.
-inline void launch_block_coder_encode(cudaStream_t stream, uint32_t coder, uint32_t sb, bool build, uint32_t n_blocks, uint32_t threads,
-                                      uint32_t smem, const uint8_t* d_in, uint32_t block_size, uint16_t* d_freqs, uint32_t chunk_syms,
-                                      uint8_t* scratch, uint32_t slot_bytes, uint32_t* sizes, uint32_t* status,
-                                      const CoderChoice* choice = nullptr, uint32_t group = 0, const BlocksVarlenGeom* geom = nullptr)
+inline void launch_block_encode(cudaStream_t stream, uint32_t coder, uint32_t sb, bool build, uint32_t n_blocks, uint32_t threads,
+                                uint32_t smem, const uint8_t* d_in, uint32_t block_size, uint16_t* d_freqs, uint32_t chunk_syms,
+                                uint8_t* scratch, uint32_t slot_bytes, uint32_t* sizes, uint32_t* status,
+                                const CoderChoice* choice = nullptr, uint32_t group = 0, const BlocksVarlenGeom* geom = nullptr)
 {
-    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, ((geom     ? block_coder_encode_kernel<CODER, SB, true, true, true>
-                                                : choice ? block_coder_encode_kernel<CODER, SB, true, true>
-                                                : build  ? block_coder_encode_kernel<CODER, SB, true>
-                                                         : block_coder_encode_kernel<CODER, SB, false>)
-                                           <<<n_blocks, threads, smem, stream>>>(d_in, block_size, d_freqs, sb, chunk_syms, scratch,
-                                                                                 slot_bytes, sizes, status, choice, group, geom)))
+    RB200_BLOCK_DISPATCH(coder, sb, (block_encode_for<CODER, SB>(build, choice != nullptr, geom != nullptr)
+                                     <<<n_blocks, threads, smem, stream>>>(d_in, block_size, d_freqs, sb, chunk_syms, scratch, slot_bytes, sizes,
+                                                                           status, choice, group, geom)))
 }
 
-inline void launch_block_coder_decode(cudaStream_t stream, uint32_t coder, uint32_t sb, const uint8_t* blob, uint64_t blob_size,
-                                      const uint64_t* offsets, const uint16_t* d_freqs, uint32_t n_blocks, uint32_t block_size,
-                                      uint32_t chunk_syms, uint8_t* out, uint32_t* status)
+inline void launch_block_decode(cudaStream_t stream, uint32_t coder, uint32_t sb, const uint8_t* blob, uint64_t blob_size,
+                                const uint64_t* offsets, const uint16_t* d_freqs, uint32_t n_blocks, uint32_t block_size,
+                                uint32_t chunk_syms, uint8_t* out, uint32_t* status)
 {
     const uint32_t threads = block_threads(block_size, chunk_syms);
     const uint32_t smem = block_coder_decode_smem(coder, sb, threads);
-    RB200_BLOCK_ANY_CODER_DISPATCH(coder, sb, (block_coder_decode_kernel<CODER, SB><<<n_blocks, threads, smem, stream>>>(
-                                              blob, blob_size, offsets, d_freqs, sb, block_size, chunk_syms, out, status)))
+    RB200_BLOCK_DISPATCH(coder, sb, (block_decode_kernel<CODER, SB><<<n_blocks, threads, smem, stream>>>(
+                                        blob, blob_size, offsets, d_freqs, sb, block_size, chunk_syms, out, status)))
 }
 
 }  // namespace rb200

@@ -6,9 +6,9 @@
 //   block_model_kernel     count_freqs + calc_cum_freqs + normalize_freqs (main.cpp:59-129)
 //                          per block, bit-exact, one warp running the order-dependent
 //                          "steal a slot" loop with a warp-wide arg-min
-//   block_decode_kernel    RansWordTablesInitSymbol (rans_word_sse41.h:64-72) in shared
-//                          memory, then the 32-way decode of each of the block's chunks
-//   block_encode_kernel    encoder reciprocal table in shared memory, then 32-way encode
+//   block_encode_fused_kernel  K5f: model (optional), encoder reciprocal table in shared memory, 32-way encode,
+//                          directory and placement in one persistent launch
+// The split per-block encoder and the per-block decoders of every coder are in block_coder_kernels.cuh.
 #pragma once
 #include "device_utils.cuh"
 #include "tables.h"
@@ -270,7 +270,7 @@ inline void launch_block_models(cudaStream_t stream, const uint8_t* d_in, uint32
 }
 
 // ---------------------------------------------------------------------------
-// K5: per-block decode / encode.  One CTA per block, one warp per chunk of the block.
+// K5: per-block decode / encode.  One CTA per block, one warp per chunk of the block (block_coder_kernels.cuh).
 // ---------------------------------------------------------------------------
 constexpr int kMaxBlockWarps = 32;
 
@@ -323,38 +323,6 @@ __device__ __forceinline__ void block_fill_slots(const uint32_t* s_cum, uint32_t
     }
 }
 
-__global__ void __launch_bounds__(kMaxBlockWarps * 32)
-block_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const uint64_t* __restrict__ offsets,
-                    const uint16_t* __restrict__ block_freqs, uint32_t block_size, uint32_t chunk_syms,
-                    uint8_t* __restrict__ out, uint32_t* __restrict__ status)
-{
-    extern __shared__ __align__(1024) uint8_t s_dyn[];           // [warps][1 KiB] rings
-    __shared__ __align__(16) uint32_t s_tab[kWordSlots];
-    __shared__ uint32_t s_cum[257];
-    __shared__ uint32_t s_flag[2];                               // [0] bad model, [1] wide (a freq of 4096)
-
-    const uint32_t tid = threadIdx.x, warp = tid >> 5;
-    const uint16_t* freqs = block_freqs + static_cast<uint64_t>(blockIdx.x) * 256;
-    if (tid == 0) s_flag[1] = 0;
-    const bool ok = block_prefix(freqs, s_cum, &s_flag[0], kWordSlots);
-    if (!ok) {
-        if (tid == 0) atomicOr(status, kStatStream);
-        return;
-    }
-    block_fill_slots(s_cum, s_tab, &s_flag[1]);
-    __syncthreads();
-
-    const uint32_t per_block = block_size / chunk_syms;
-    if (warp >= per_block) return;
-    const uint32_t chunk = blockIdx.x * per_block + warp;
-    uint8_t* dst = out + static_cast<uint64_t>(blockIdx.x) * block_size + static_cast<uint64_t>(warp) * chunk_syms;
-    const uint32_t ring = smem_addr(s_dyn) + warp * kRingBytes;
-    if (s_flag[1])
-        decode_window_chunk(WordDecoder<true>{smem_addr_pinned(s_tab), 0}, blob, blob_size, offsets, chunk, ring, dst, chunk_syms, status);
-    else
-        decode_window_chunk(WordDecoder<false>{smem_addr_pinned(s_tab), 0}, blob, blob_size, offsets, chunk, ring, dst, chunk_syms, status);
-}
-
 // The block's encoder table (8x replicated {magic, x_max | shift, start, 4096 - freq}) from its cumulative table in
 // s_cum; returns whether the 32-bit reciprocal is exact for every symbol of this model (tables.h: enc32), which
 // selects the kernel variant for the block.  Ends with a CTA barrier.
@@ -398,28 +366,16 @@ __device__ __forceinline__ bool block_build_enc_table(const uint32_t* s_cum, boo
     return r32;
 }
 
-__global__ void __launch_bounds__(kMaxBlockWarps * 32)
-block_encode_kernel(const uint8_t* __restrict__ in, uint32_t block_size, const uint16_t* __restrict__ block_freqs,
-                    uint32_t chunk_syms, uint8_t* __restrict__ scratch, uint32_t slot_bytes, uint32_t* __restrict__ sizes,
-                    uint32_t* __restrict__ status)
+// The block's model in s_cum: BUILD, count_freqs + normalize_freqs(M) of the block (block_model_build_wide over the 32
+// KiB at hist, written to freqs); else freqs, the caller's row.  Returns block_prefix's verdict (s_bad its flag).
+template <bool BUILD>
+__device__ __forceinline__ bool block_model_prefix(const uint8_t* __restrict__ blk, uint32_t block_size, uint16_t* __restrict__ freqs,
+                                                   uint32_t* hist, uint32_t* s_cnt, uint32_t* s_cum, uint32_t* s_w, uint32_t* s_bad,
+                                                   uint32_t* __restrict__ status, uint32_t M)
 {
-    extern __shared__ __align__(1024) uint8_t s_enc[];          // [32 KiB table][warps x 1 KiB stage + ring]
-    __shared__ uint32_t s_cum[257];
-    __shared__ uint32_t s_flag[1];
-    uint4* s_tab = reinterpret_cast<uint4*>(s_enc);
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint16_t* freqs = block_freqs + static_cast<uint64_t>(blockIdx.x) * 256;
-    const uint32_t per_block = block_size / chunk_syms;
-    const bool ok = block_prefix(freqs, s_cum, &s_flag[0], kWordSlots);
-    const bool r32 = block_build_enc_table(s_cum, ok, s_tab);
-    if (warp >= per_block) return;
-    const uint32_t chunk = blockIdx.x * per_block + warp;
-    const uint8_t* src = in + static_cast<uint64_t>(blockIdx.x) * block_size + static_cast<uint64_t>(warp) * chunk_syms;
-    const uint32_t wsm = smem_addr(s_enc) + kEncTableBytes + warp * kEncWarpSmem;
-    if (r32)
-        encode_chunk_split(src, chunk_syms, chunk, WordEncoder<true>{smem_addr(s_enc)}, wsm, scratch, slot_bytes, sizes, status);
-    else
-        encode_chunk_split(src, chunk_syms, chunk, WordEncoder<false>{smem_addr(s_enc)}, wsm, scratch, slot_bytes, sizes, status);
+    if (!BUILD) return block_prefix(static_cast<const uint16_t*>(freqs), s_cum, s_bad, M);
+    block_model_build_wide(blk, block_size, hist, s_cnt, s_cum, s_w, freqs, status, M);
+    return block_prefix(s_w, s_cum, s_bad, M);                    // the widths are still in shared memory
 }
 
 // K5f: per-block encode in ONE persistent launch -- model (optional), tables, encode, directory, placement.
@@ -463,13 +419,8 @@ __device__ __forceinline__ void block_encode_fused(const uint8_t* __restrict__ i
         if (block >= n_blocks) break;
         const uint8_t* blk = in + static_cast<uint64_t>(block) * block_size;
         uint16_t* freqs = block_freqs + static_cast<uint64_t>(block) * 256;
-        bool ok;
-        if (BUILD) {
-            block_model_build_wide(blk, block_size, reinterpret_cast<uint32_t*>(s_enc), s_cnt, s_cum, s_w, freqs, status, kWordSlots);
-            ok = block_prefix(s_w, s_cum, &s_flag[0], kWordSlots);    // the widths are still in shared memory
-        } else {
-            ok = block_prefix(static_cast<const uint16_t*>(freqs), s_cum, &s_flag[0], kWordSlots);
-        }
+        const bool ok = block_model_prefix<BUILD>(blk, block_size, freqs, reinterpret_cast<uint32_t*>(s_enc), s_cnt, s_cum, s_w, &s_flag[0],
+                                                  status, kWordSlots);
         const bool r32 = block_build_enc_table(s_cum, ok, s_tab);
         if (warp < per_block) {
             const uint8_t* src = blk + static_cast<uint64_t>(warp) * chunk_syms;
@@ -519,7 +470,8 @@ inline uint32_t block_threads(uint32_t block_size, uint32_t chunk_syms)
     return warps * 32;
 }
 
-// dynamic shared memory of both per-block encoders (K5, K5f) at `threads` threads: the table, then 1 KiB per warp
+// dynamic shared memory of the per-block encoders (K5f; K5 adds the alias coder's remap) at `threads` threads: the
+// table, then 1 KiB per warp
 inline uint32_t block_encode_smem(uint32_t threads) { return kEncTableBytes + (threads / 32) * kEncWarpSmem; }
 
 // the instance of the fused per-block encoder for blocks of block_threads() = `threads`: (BUILD, GATED, GEOM) =
@@ -535,30 +487,6 @@ inline BlockEncodeFusedKernel block_encode_fused_warps(bool build, bool gated, b
 inline BlockEncodeFusedKernel block_encode_fused_for(bool build, bool gated, bool geom, uint32_t threads)
 {
     return threads <= 256 ? block_encode_fused_warps<8>(build, gated, geom) : block_encode_fused_warps<32>(build, gated, geom);
-}
-
-inline void configure_block_kernels()
-{
-    cudaFuncSetAttribute(block_decode_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    // ~17.4 KiB static (table, cumulative, flag) + 1 KiB of ring per warp: above 48 KiB from 31 warps on, so opt in
-    cudaFuncSetAttribute(block_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxBlockWarps * kRingBytes);
-    cudaFuncSetAttribute(block_encode_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(block_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(kMaxBlockWarps * 32));
-    for (const uint32_t threads : {8u * 32, 32u * 32})
-        for (const BlockEncodeFusedKernel k : {block_encode_fused_for(true, false, false, threads), block_encode_fused_for(false, false, false, threads),
-                                               block_encode_fused_for(true, true, false, threads), block_encode_fused_for(true, true, true, threads)}) {
-            cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, block_encode_smem(threads));
-        }
-}
-
-inline void launch_block_decode(cudaStream_t stream, const uint8_t* blob, uint64_t blob_size, const uint64_t* offsets,
-                                const uint16_t* d_freqs, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
-                                uint8_t* out, uint32_t* status)
-{
-    const uint32_t threads = block_threads(block_size, chunk_syms);
-    block_decode_kernel<<<n_blocks, threads, (threads / 32) * kRingBytes, stream>>>(blob, blob_size, offsets, d_freqs, block_size,
-                                                                                    chunk_syms, out, status);
 }
 
 }  // namespace rb200

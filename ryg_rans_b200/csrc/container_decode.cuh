@@ -21,17 +21,15 @@
 //   the version's decoders         one launch per decoder the version can need, each on a fixed grid of every CTA that
 //                                  is resident at once; only the one whose id is in go runs, every other exits before
 //                                  it touches shared memory, TMA or its counter.  Version 1: one per variant rb200_decode
-//                                  can pick (kDec*); version 2: block_decode_planned_kernel; versions 3 and 4:
-//                                  block_coder_decode_planned_kernel<CODER, SB>, one per instance of
-//                                  RB200_BLOCK_CODER_DISPATCH (version 3) or RB200_BLOCK_ALIAS_DISPATCH (version 4).  The
-//                                  per-block ones take block ids from a counter, build the block's table in shared
-//                                  memory (version 4: the block's alias pairing first) and decode its chunks.
+//                                  can pick (kDec*); versions 2, 3 and 4: block_decode_planned_kernel<CODER, SB>, one per
+//                                  instance of RB200_BLOCK_DISPATCH of the version's coders.  The per-block ones take
+//                                  block ids from a counter, build the block's table in shared memory (block_decode_table;
+//                                  version 4: the block's alias pairing first) and decode its chunks.
 // The rules are the host parser's (container_format.h); they run in its order: content errors before kStatSpace.
 //
-// rb200_container_blocks_any_decode_async runs the same stages for whichever per-block version the header names:
-// container_any_plan_kernel and container_any_verdict_kernel (the plan and verdict bodies with the header's version)
-// on the call's own workspace, and the verdict hands plan and go to the workspace of that version, whose decoders then
-// run; the other versions' decoders see go == 0 in theirs.
+// rb200_container_blocks_any_decode_async runs the same stages on its own workspace for whichever per-block version the
+// header names (kContainerVersionAnyBlocks), then the decoders of versions 2, 3 and 4: their ids are unique across
+// those versions.
 #pragma once
 #include "alias_kernels.cuh"
 #include "block_coder_kernels.cuh"
@@ -72,14 +70,16 @@ struct ContainerAsyncWork {
     alignas(16) uint8_t table[kSingleTableBytes];   // version 1: the decode table of the header's coder, as rb200_model_create's
 };
 
-// The decoders of each version, with ids from 1 in the order of the version's range of the launch table
-// (configure_container_decode); the verdict stores the id of the one to run in go, kDecNone decodes nothing.
-// Version 1: one per variant rb200_decode picks, the word coder narrow or WIDE (a frequency of 4096), the alias and byte
-// coders specialised for scale_bits 16, 14, 12 or generic (RB200_ALIAS_SB_DISPATCH), rans64.  Version 2:
-// block_decode_planned_kernel.  Version 3: one per instance of RB200_BLOCK_CODER_DISPATCH, the byte coder at
-// scale_bits 14, 12 or generic (ids 1, 2, 3), rans64 (4).  Version 4: one per instance of RB200_BLOCK_ALIAS_DISPATCH, the
-// alias coder at scale_bits 14, 12 or generic (ids 1, 2, 3).
+// The decoders, with ids from 1 in the order of the launch table (configure_container_decode); the verdict stores the id
+// of the one to run in go, kDecNone decodes nothing.  Version 1: one per variant rb200_decode picks, the word coder
+// narrow or WIDE (a frequency of 4096), the alias and byte coders specialised for scale_bits 16, 14, 12 or generic
+// (RB200_ALIAS_SB_DISPATCH), rans64.  Versions 2, 3 and 4, numbered once across them: one per instance of
+// RB200_BLOCK_DISPATCH, the word coder (1), the byte coder at scale_bits 14, 12 or generic (2, 3, 4), rans64 (5), the
+// alias coder at scale_bits 14, 12 or generic (6, 7, 8).
 constexpr uint32_t kDecNone = 0, kDecWord = 1, kDecWordWide = 2, kDecAlias = 3, kDecByte = 7, kDecRans64 = 11;
+// the version argument of rb200_container_blocks_any_decode_async's plan and verdict: whichever of versions 2, 3 and 4
+// the header names
+constexpr uint16_t kContainerVersionAnyBlocks = 0;
 // offset of a specialisation from kDecAlias / kDecByte
 __host__ __device__ constexpr uint32_t sb_variant(uint32_t sb) { return sb == 16 ? 0 : sb == 14 ? 1 : sb == 12 ? 2 : 3; }
 
@@ -87,8 +87,11 @@ __host__ __device__ constexpr uint32_t sb_variant(uint32_t sb) { return sb == 16
 // choice of kernel, decode_device; wide: the word table has a slot of frequency 4096)
 __host__ __device__ constexpr uint32_t container_decoder(uint32_t version, uint32_t coder, uint32_t sb, uint32_t wide)
 {
-    if (version == kContainerVersionBlocks) return 1;
-    if (version >= kContainerVersionBlocksCoder) return coder == RB200_CODER_RANS64 ? 4 : sb == 14 ? 1 : sb == 12 ? 2 : 3;
+    if (version != kContainerVersion) {                              // the per-block versions
+        if (coder == RB200_CODER_WORD) return 1;
+        if (coder == RB200_CODER_RANS64) return 5;
+        return (coder == RB200_CODER_ALIAS ? 6 : 2) + (sb == 14 ? 0 : sb == 12 ? 1 : 2);
+    }
     if (coder == RB200_CODER_WORD) return wide ? kDecWordWide : kDecWord;
     if (coder == RB200_CODER_ALIAS) return kDecAlias + sb_variant(sb);
     if (coder == RB200_CODER_BYTE) return kDecByte + sb_variant(sb);
@@ -96,9 +99,16 @@ __host__ __device__ constexpr uint32_t container_decoder(uint32_t version, uint3
 }
 
 // One warp: the plan of a header that passes the rules of the call's version (a zero plan otherwise), with the verdict
-// words and the decoders' counters cleared
-__device__ __forceinline__ void container_plan(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, ContainerAsyncWork* w)
+// words and the decoders' counters cleared.  kContainerVersionAnyBlocks: the version the header names when that is 2, 3
+// or 4; any other version, or fewer than 64 bytes, gets the zero plan.
+__global__ void __launch_bounds__(32)
+    container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, ContainerAsyncWork* w)
 {
+    if (threadIdx.x) return;
+    if (version == kContainerVersionAnyBlocks) {
+        version = size >= sizeof(ContainerHeader) ? reinterpret_cast<const ContainerHeader*>(buf)->version : 0u;
+        if (version < kContainerVersionBlocks || version > kContainerVersionBlocksAlias) size = 0;
+    }
     BlocksPlan p = {};
     uint32_t coder = 0, scale_bits = 0;
     if (size >= sizeof(ContainerHeader)) {                           // a shorter buffer is not read at all
@@ -131,37 +141,6 @@ __device__ __forceinline__ void container_plan(const uint8_t* __restrict__ buf, 
     w->wide = 0;
     w->refused = 0;
     w->work = DecodeWork{0, 0};
-}
-
-__global__ void __launch_bounds__(32)
-    container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, ContainerAsyncWork* w)
-{
-    if (threadIdx.x) return;
-    container_plan(buf, size, version, w);
-}
-
-// The per-block container of any version (rb200_container_blocks_any_decode_async) takes the call's workspace `w` for
-// its checks and hands the plan to the workspace of the header's version, whose decoders then run.  vw[0..2]: the
-// workspaces of versions 2, 3 and 4.
-struct BlocksAnyWork {
-    ContainerAsyncWork* vw[3];
-};
-
-// container_plan with the version the header names when that is 2, 3 or 4; any other version, or fewer than 64 bytes,
-// gets the zero plan.  The three version workspaces' go and decoder counters are cleared, as the plan kernel clears
-// its own: no decoder runs unless the verdict hands it this call's plan.
-__global__ void __launch_bounds__(32)
-    container_any_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, ContainerAsyncWork* w, BlocksAnyWork any)
-{
-    if (threadIdx.x) return;
-    const uint32_t version = size >= sizeof(ContainerHeader) ? reinterpret_cast<const ContainerHeader*>(buf)->version : 0u;
-    const bool per_block = version >= kContainerVersionBlocks && version <= kContainerVersionBlocksAlias;
-    container_plan(buf, per_block ? size : 0, per_block ? version : kContainerVersionBlocks, w);
-    for (ContainerAsyncWork* v : any.vw) {
-        v->go = 0;
-        v->next_block = 0;
-        v->ctas_done = 0;
-    }
 }
 
 // The per-element rules of the prefix.  Each warp stages 32 block models (16 KiB, coalesced) in shared memory with
@@ -287,8 +266,9 @@ __global__ void __launch_bounds__(kTableThreads) container_table_kernel(const ui
 // the header's CRC is taken here with container_finish_kernel's warp helpers and joined (crc32_combine).  What open
 // accepts but the decoders do not take is refused as content (kStatStream): a blob of 2^36 bytes or more and version 1's
 // chunk sizes outside 32 .. 2^24 (container_geometry_decodable), version 1's models that the table kernel refused.
-__device__ __forceinline__ void container_verdict(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols,
-                                                  ContainerAsyncWork* w, uint32_t* status, uint32_t version)
+__global__ void __launch_bounds__(32)
+    container_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, ContainerAsyncWork* w,
+                             uint32_t* status, uint32_t version)
 {
     using namespace crc_detail;
     __shared__ uint4 s_head_v[sizeof(ContainerHeader) / 16];
@@ -327,145 +307,57 @@ __device__ __forceinline__ void container_verdict(const uint8_t* __restrict__ bu
         w->go = container_decoder(version, w->coder, w->scale_bits, w->wide);
 }
 
-__global__ void __launch_bounds__(32)
-    container_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, ContainerAsyncWork* w,
-                             uint32_t* status, uint32_t version)
-{
-    container_verdict(buf, out_cap, n_symbols, w, status, version);
-}
-
-// The verdict of rb200_container_blocks_any_decode_async: container_verdict for the header's version (the plan accepted
-// it, so it is 2, 3 or 4), then plan, coder, scale_bits and go handed to that version's workspace, whose decoders
-// alone can see a nonzero go (the plan kernel cleared the others')
-__global__ void __launch_bounds__(32)
-    container_any_verdict_kernel(const uint8_t* __restrict__ buf, uint64_t out_cap, uint64_t* __restrict__ n_symbols, ContainerAsyncWork* w,
-                                 uint32_t* status, BlocksAnyWork any)
-{
-    const uint32_t version = w->plan.ok ? reinterpret_cast<const ContainerHeader*>(buf)->version : kContainerVersionBlocks;
-    container_verdict(buf, out_cap, n_symbols, w, status, version);
-    if (threadIdx.x || !w->go) return;                           // lane 0 wrote go
-    ContainerAsyncWork* v = any.vw[version - kContainerVersionBlocks];
-    v->plan = w->plan;
-    v->coder = w->coder;
-    v->scale_bits = w->scale_bits;
-    v->go = w->go;
-}
-
-// The per-block decoder for a geometry only the device knows: a fixed grid of kPlannedWarps-warp CTAs (resident all at
-// once) takes block ids from w->next_block; per block, the slot table as block_decode_kernel builds it (the WIDE
-// variant chosen per block), then the warps take the block's 1..32 chunks in turn.
+// The per-block decoders for a geometry only the device knows, one per instance of RB200_BLOCK_DISPATCH, each on a fixed
+// grid of kPlannedWarps-warp CTAs (resident all at once).  Only the one whose id is in go runs; every other exits before
+// it touches shared memory or the counter.  CTAs take block ids from w->next_block; per block, block_decode_kernel's two
+// steps: the table in shared memory (block_decode_table), then the warps take the block's 1..32 chunks in turn
+// (block_decode_chunk).  The alias coder's pairing overlays the table the previous block's warps read: the barrier at
+// the loop's top keeps it behind their last chunk.  The word instance keeps 8 CTAs per SM (32 registers).
 constexpr int kPlannedWarps = 8;
 
-__global__ void __launch_bounds__(kPlannedWarps * 32, 8)
-    block_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* w, uint32_t* __restrict__ status)
-{
-    __shared__ __align__(1024) uint8_t s_ring[kPlannedWarps * kRingBytes];
-    __shared__ __align__(16) uint32_t s_tab[kWordSlots];
-    __shared__ uint32_t s_cum[257];
-    __shared__ uint32_t s_flag[2];                               // [0] bad model, [1] wide (a freq of 4096)
-    __shared__ uint32_t s_block;
-    const uint32_t tid = threadIdx.x, warp = tid >> 5;
-    if (w->go) {                                                 // the same for the whole grid
-        const BlocksPlan& p = w->plan;
-        const uint32_t n_blocks = p.n_blocks, block_size = p.block_size, chunk_syms = p.chunk_syms;
-        const uint32_t per_block = block_size / chunk_syms;
-        const uint64_t blob_bytes = p.blob_bytes;
-        const uint16_t* models = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));
-        const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + p.dir_off);
-        const uint8_t* blob = buf + p.blob_off;
-        const uint32_t ring = smem_addr(s_ring) + warp * kRingBytes;
-        for (;;) {
-            __syncthreads();                                     // the previous block's table is no longer in use
-            if (tid == 0) {
-                s_block = atomicAdd(&w->next_block, 1u);
-                s_flag[1] = 0;
-            }
-            __syncthreads();
-            const uint32_t block = s_block;
-            if (block >= n_blocks) break;
-            if (!block_prefix(models + static_cast<uint64_t>(block) * 256, s_cum, &s_flag[0], kWordSlots)) {   // checked before: not reached
-                if (tid == 0) atomicOr(status, kStatStream);
-                continue;
-            }
-            block_fill_slots(s_cum, s_tab, &s_flag[1]);
-            __syncthreads();
-            const bool wide = s_flag[1] != 0;
-            for (uint32_t k = warp; k < per_block; k += kPlannedWarps) {
-                const uint32_t chunk = block * per_block + k;
-                uint8_t* dst = out + static_cast<uint64_t>(block) * block_size + static_cast<uint64_t>(k) * chunk_syms;
-                if (wide)
-                    decode_window_chunk(WordDecoder<true>{smem_addr_pinned(s_tab), 0}, blob, blob_bytes, offsets, chunk, ring, dst, chunk_syms, status);
-                else
-                    decode_window_chunk(WordDecoder<false>{smem_addr_pinned(s_tab), 0}, blob, blob_bytes, offsets, chunk, ring, dst, chunk_syms, status);
-            }
-        }
-    }
-    // every CTA has taken its last block id before it counts itself out: the last one re-arms the counter
-    if (tid == 0 && atomicAdd(&w->ctas_done, 1u) == gridDim.x - 1) {
-        w->next_block = 0;
-        w->ctas_done = 0;
-    }
-}
-
-// The version 3 and 4 decoders, one per instance of RB200_BLOCK_CODER_DISPATCH (version 3) and of
-// RB200_BLOCK_ALIAS_DISPATCH (version 4), each on a fixed grid of kPlannedWarps-warp CTAs (resident all at once).  Only
-// the one whose id is in go runs; every other exits before it touches shared memory or the counter.  CTAs take block
-// ids from w->next_block; per block, block_coder_decode_kernel's table in shared memory, then the warps take the block's
-// 1..32 chunks in turn.  The alias coder's pairing overlays the table the previous block's warps read: the barrier at
-// the loop's top keeps it behind their last chunk.
 template <uint32_t CODER, uint32_t SB>
-__global__ void __launch_bounds__(kPlannedWarps * 32)
-    block_coder_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
-                                      uint32_t* __restrict__ status)
+__global__ void __launch_bounds__(kPlannedWarps * 32, CODER == RB200_CODER_WORD ? 8 : 0)
+    block_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
+                                uint32_t* __restrict__ status)
 {
-    constexpr uint32_t version = CODER == RB200_CODER_ALIAS ? kContainerVersionBlocksAlias : kContainerVersionBlocksCoder;
-    if (w->go != container_decoder(version, CODER, SB, 0)) return;   // the same for the whole grid
-    // [kPlannedWarps x 1 KiB rings][cum2sym[1 << sb]][symbol entries], alias: [rings][256 x kAliasDecReplicas bucket entries]
-    extern __shared__ __align__(1024) uint8_t s_bdec[];
+    if (w->go != container_decoder(kContainerVersionBlocks, CODER, SB, 0)) return;   // the same for the whole grid
+    // [kPlannedWarps x 1 KiB rings][the block's decode table]: dynamic, but static for the word coder, whose decode
+    // step ptxas schedules better with the table at a fixed address
+    extern __shared__ __align__(1024) uint8_t s_dyn[];
+    __shared__ __align__(1024) uint8_t s_word[CODER == RB200_CODER_WORD ? kPlannedWarps * kRingBytes + kWordSlots * 4 : 1];
     __shared__ uint32_t s_cum[257];
-    __shared__ uint32_t s_flag[1];
+    __shared__ uint32_t s_flag[2];                              // [0] bad model, [1] wide (word coder)
     __shared__ uint32_t s_block;
+    uint8_t* s_bdec = CODER == RB200_CODER_WORD ? s_word : s_dyn;
     const BlocksPlan& p = w->plan;
-    const uint32_t sb = SB ? SB : w->scale_bits, M = 1u << sb;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t sb = SB ? SB : w->scale_bits;
+    const uint32_t tid = threadIdx.x, warp = tid >> 5;
     const uint32_t n_blocks = p.n_blocks, block_size = p.block_size, chunk_syms = p.chunk_syms;
     const uint32_t per_block = block_size / chunk_syms;
     const uint64_t blob_bytes = p.blob_bytes;
     const uint16_t* models = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));
     const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + p.dir_off);
     const uint8_t* blob = buf + p.blob_off;
-    uint8_t* s_tab = s_bdec + kPlannedWarps * kRingBytes;
-    const uint32_t ring = smem_addr(s_bdec) + warp * kRingBytes, tab = smem_addr_pinned(s_tab);
+    // the word coder takes its table's address per chunk: hoisted, it goes to a uniform register and the step changes
+    const uint32_t ring = smem_addr(s_bdec) + warp * kRingBytes;
+    const uint32_t tab = CODER == RB200_CODER_WORD ? 0 : smem_addr_pinned(s_bdec + kPlannedWarps * kRingBytes);
     for (;;) {
         __syncthreads();                                             // the previous block's table is no longer in use
         if (tid == 0) s_block = atomicAdd(&w->next_block, 1u);
         __syncthreads();
         const uint32_t block = s_block;
         if (block >= n_blocks) break;
-        if (!block_prefix(models + static_cast<uint64_t>(block) * 256, s_cum, &s_flag[0], M)) {   // checked before: not reached
+        // a model that does not sum was refused by the prefix check: not reached
+        if (!block_decode_table<CODER, SB>(models + static_cast<uint64_t>(block) * 256, 1u << sb, s_cum, s_flag, s_bdec, kPlannedWarps)) {
             if (tid == 0) atomicOr(status, kStatStream);
             continue;
         }
-        if (CODER == RB200_CODER_ALIAS) {
-            if (!block_alias_decode_table<SB>(s_cum, s_tab, M)) {   // a block that sums always pairs: not reached
-                if (tid == 0) atomicOr(status, kStatStream);
-                continue;
-            }
-        } else {
-            block_coder_decode_table<CODER>(s_cum, s_tab, M);
-        }
-        __syncthreads();
+        const bool wide = CODER == RB200_CODER_WORD && s_flag[1];
         for (uint32_t k = warp; k < per_block; k += kPlannedWarps) {
-            const uint32_t chunk = block * per_block + k;
             uint8_t* dst = out + static_cast<uint64_t>(block) * block_size + static_cast<uint64_t>(k) * chunk_syms;
-            if (CODER == RB200_CODER_ALIAS)
-                decode_window_chunk(AliasDecoder<SB, kAliasLean>{tab + (lane & (kAliasDecReplicas - 1)) * 16, sb}, blob, blob_bytes, offsets,
-                                    chunk, ring, dst, chunk_syms, status);
-            else if (CODER == RB200_CODER_BYTE)
-                decode_window_chunk(ByteDecoder<SB>{tab, sb}, blob, blob_bytes, offsets, chunk, ring, dst, chunk_syms, status);
-            else
-                decode_window_chunk(Rans64Decoder{tab, tab + M + (lane & (kRans64DecReplicas - 1)) * 8, sb}, blob, blob_bytes, offsets, chunk,
-                                    ring, dst, chunk_syms, status);
+            block_decode_chunk<CODER, SB>(blob, blob_bytes, offsets, block * per_block + k, ring,
+                                          CODER == RB200_CODER_WORD ? smem_addr_pinned(s_bdec + kPlannedWarps * kRingBytes) : tab, sb, wide, dst,
+                                          chunk_syms, status);
         }
     }
     // every CTA has taken its last block id before it counts itself out: the last one re-arms the counter
@@ -645,21 +537,21 @@ inline void configure_container_decode(uint32_t sms, DecoderLaunch* out)
         {byte_decode_planned_kernel<12>, 0, kAliasDecWarps * 32, byte_planned_smem(12), "byte_decode_planned_kernel<12>"},
         {byte_decode_planned_kernel<0>, 0, kAliasDecWarps * 32, byte_planned_smem(0), "byte_decode_planned_kernel<0>"},
         {rans64_decode_planned_kernel, 0, kRans64Warps * 32, kRans64PlannedSmem, "rans64_decode_planned_kernel"},
-        {block_decode_planned_kernel, 0, planned, 0, "block_decode_planned_kernel"},
-        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 14>, 0, planned, block_coder_decode_smem(RB200_CODER_BYTE, 14, planned),
-         "block_coder_decode_planned_kernel<byte, 14>"},
-        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 12>, 0, planned, block_coder_decode_smem(RB200_CODER_BYTE, 12, planned),
-         "block_coder_decode_planned_kernel<byte, 12>"},
-        {block_coder_decode_planned_kernel<RB200_CODER_BYTE, 0>, 0, planned,
-         block_coder_decode_smem(RB200_CODER_BYTE, kBlockCoderMaxScaleBits, planned), "block_coder_decode_planned_kernel<byte, 0>"},
-        {block_coder_decode_planned_kernel<RB200_CODER_RANS64, 0>, 0, planned,
-         block_coder_decode_smem(RB200_CODER_RANS64, kBlockCoderMaxScaleBits, planned), "block_coder_decode_planned_kernel<rans64, 0>"},
-        {block_coder_decode_planned_kernel<RB200_CODER_ALIAS, 14>, 0, planned, block_coder_decode_smem(RB200_CODER_ALIAS, 14, planned),
-         "block_coder_decode_planned_kernel<alias, 14>"},
-        {block_coder_decode_planned_kernel<RB200_CODER_ALIAS, 12>, 0, planned, block_coder_decode_smem(RB200_CODER_ALIAS, 12, planned),
-         "block_coder_decode_planned_kernel<alias, 12>"},
-        {block_coder_decode_planned_kernel<RB200_CODER_ALIAS, 0>, 0, planned,
-         block_coder_decode_smem(RB200_CODER_ALIAS, kBlockCoderMaxScaleBits, planned), "block_coder_decode_planned_kernel<alias, 0>"},
+        {block_decode_planned_kernel<RB200_CODER_WORD, kWordScaleBits>, 0, planned, 0, "block_decode_planned_kernel<word, 12>"},
+        {block_decode_planned_kernel<RB200_CODER_BYTE, 14>, 0, planned, block_coder_decode_smem(RB200_CODER_BYTE, 14, planned),
+         "block_decode_planned_kernel<byte, 14>"},
+        {block_decode_planned_kernel<RB200_CODER_BYTE, 12>, 0, planned, block_coder_decode_smem(RB200_CODER_BYTE, 12, planned),
+         "block_decode_planned_kernel<byte, 12>"},
+        {block_decode_planned_kernel<RB200_CODER_BYTE, 0>, 0, planned,
+         block_coder_decode_smem(RB200_CODER_BYTE, kBlockCoderMaxScaleBits, planned), "block_decode_planned_kernel<byte, 0>"},
+        {block_decode_planned_kernel<RB200_CODER_RANS64, 0>, 0, planned,
+         block_coder_decode_smem(RB200_CODER_RANS64, kBlockCoderMaxScaleBits, planned), "block_decode_planned_kernel<rans64, 0>"},
+        {block_decode_planned_kernel<RB200_CODER_ALIAS, 14>, 0, planned, block_coder_decode_smem(RB200_CODER_ALIAS, 14, planned),
+         "block_decode_planned_kernel<alias, 14>"},
+        {block_decode_planned_kernel<RB200_CODER_ALIAS, 12>, 0, planned, block_coder_decode_smem(RB200_CODER_ALIAS, 12, planned),
+         "block_decode_planned_kernel<alias, 12>"},
+        {block_decode_planned_kernel<RB200_CODER_ALIAS, 0>, 0, planned,
+         block_coder_decode_smem(RB200_CODER_ALIAS, kBlockCoderMaxScaleBits, planned), "block_decode_planned_kernel<alias, 0>"},
     };
     for (int i = 0; i < kContainerDecoders; i++) {
         out[i] = l[i];

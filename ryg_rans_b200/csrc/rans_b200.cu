@@ -68,7 +68,7 @@ struct rb200_ctx {
     // versions never share state, and every version's decoder launches
     ContainerAsyncWork* d_async[4] = {};
     DecoderLaunch async_decoders[kContainerDecoders] = {};
-    // rb200_container_blocks_any_decode_async: the checks' own workspace; its decoders run on d_async[1..3]
+    // rb200_container_blocks_any_decode_async: its own workspace, for its checks and the decoders of versions 2-4
     ContainerAsyncWork* d_async_any = nullptr;
     // rb200_container_model_encode_async (model_kernels.cuh): the counts, the model and its encode tables
     ModelAsyncWork* d_model_async = nullptr;
@@ -256,7 +256,6 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     configure_word_kernels();
     configure_alias_kernels();
     configure_block_kernels();
-    configure_block_coder_kernels();
     configure_rans64_kernels();
     configure_crc_kernels();
     configure_container_decode(static_cast<uint32_t>(ctx->sms), ctx->async_decoders);
@@ -1191,7 +1190,7 @@ EncodePlan plan_blocks_encode(const rb200_ctx* ctx, int coder, uint32_t sb, uint
     p.slot_bytes = slot_bytes_for(chunk_syms);
     p.fused = coder == RB200_CODER_WORD && (build || use_fused_encode(chunk_syms));
     p.threads = block_threads(block_size, chunk_syms);
-    p.smem = coder == RB200_CODER_WORD ? block_encode_smem(p.threads) : block_coder_encode_smem(static_cast<uint32_t>(coder), sb, p.threads);
+    p.smem = block_coder_encode_smem(static_cast<uint32_t>(coder), sb, p.threads);
     if (!p.fused) {
         p.grid = n_blocks;
         p.slots = p.n_chunks;
@@ -1223,21 +1222,18 @@ int blocks_encode_device(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* 
 {
     if (static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) >= (1ull << 31)) return RB200_E_ARG;
     const EncodePlan p = plan_blocks_encode(ctx, coder, sb, n_blocks, block_size, chunk_syms, build_models);
+    // the word coder's split encoder has no model-building, GATED or GEOM instance
+    if (!p.fused && coder == RB200_CODER_WORD && (build_models || choice || geom)) return RB200_E_ARG;
     return run_encode(ctx, p, d_blob, blob_cap, d_offsets, geom ? &geom->v : nullptr, [&](const EncodeWorkspace& ws) {
-        if (coder != RB200_CODER_WORD) {
-            launch_block_coder_encode(ctx->stream, static_cast<uint32_t>(coder), sb, build_models, p.grid, p.threads, p.smem, d_in, block_size,
-                                      d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status, choice, group, geom);
-            return check_launch(ctx, "block_coder_encode_kernel");
-        }
         if (p.fused) {
             block_encode_fused_for(build_models, choice != nullptr, geom != nullptr, p.threads)<<<p.grid, p.threads, p.smem, ctx->stream>>>(
                 d_in, n_blocks, block_size, d_freqs, chunk_syms, ws.scratch, p.slot_bytes, ws.look, ws.counter, d_blob, blob_cap, d_offsets,
                 ctx->d_status, choice, group, geom, block_size / chunk_syms);
             return check_launch(ctx, "block_encode_fused_kernel");
         }
-        block_encode_kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, block_size, d_freqs, chunk_syms, ws.scratch, p.slot_bytes,
-                                                                        ws.sizes, ctx->d_status);
-        return check_launch(ctx, "block_encode_kernel");
+        launch_block_encode(ctx->stream, static_cast<uint32_t>(coder), sb, build_models, p.grid, p.threads, p.smem, d_in, block_size, d_freqs,
+                            chunk_syms, ws.scratch, p.slot_bytes, ws.sizes, ctx->d_status, choice, group, geom);
+        return check_launch(ctx, "block_coder_encode_kernel");
     }, choice, group);
 }
 
@@ -1277,12 +1273,8 @@ int blocks_encode_entry(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* i
 int blocks_decode_device(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* d_blob, size_t blob_size, const uint64_t* d_off,
                          const uint16_t* d_freqs, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms, uint8_t* d_out)
 {
-    if (coder != RB200_CODER_WORD) {
-        launch_block_coder_decode(ctx->stream, static_cast<uint32_t>(coder), sb, d_blob, blob_size, d_off, d_freqs, n_blocks, block_size,
-                                  chunk_syms, d_out, ctx->d_status);
-        return check_launch(ctx, "block_coder_decode_kernel");
-    }
-    launch_block_decode(ctx->stream, d_blob, blob_size, d_off, d_freqs, n_blocks, block_size, chunk_syms, d_out, ctx->d_status);
+    launch_block_decode(ctx->stream, static_cast<uint32_t>(coder), sb, d_blob, blob_size, d_off, d_freqs, n_blocks, block_size, chunk_syms,
+                        d_out, ctx->d_status);
     return check_launch(ctx, "block_decode_kernel");
 }
 
@@ -1856,15 +1848,19 @@ bool async_args_ok(const rb200_ctx* ctx, const uint8_t* buf, const uint8_t* out,
     return ctx && buf && out && !(reinterpret_cast<uintptr_t>(d_n_symbols) & 7) && container_mem_ok(RB200_MEM_DEVICE, buf, out);
 }
 
-// The async decode of a container of `version` (container_decode.cuh), in its own workspace: plan, meta CRC, blob CRC,
-// the prefix check, version 1's model check and table build, the verdict, then every decoder of the version on its
-// fixed grid; the verdict's go names the one that runs.  Lengths and positions the host cannot know come from the plan
-// on the device; the host passes only bounds it knows (size).  No copy, no synchronisation, no allocation.
+// The async decode of a container of `version` (container_decode.cuh), or of any per-block version
+// (kContainerVersionAnyBlocks), in its own workspace: plan, meta CRC, blob CRC, the prefix check, version 1's model
+// check and table build, the verdict, then every decoder of the version (of versions 2-4) on its fixed grid; the
+// verdict's go names the one that runs.  Lengths and positions the host cannot know come from the plan on the device;
+// the host passes only bounds it knows (size).  No copy, no synchronisation, no allocation.
 int container_decode_async(rb200_ctx* ctx, uint16_t version, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                            uint64_t* d_n_symbols)
 {
     DeviceGuard g(ctx->device);
-    ContainerAsyncWork* w = ctx->d_async[version - 1];
+    const bool any = version == kContainerVersionAnyBlocks;
+    ContainerAsyncWork* w = any ? ctx->d_async_any : ctx->d_async[version - 1];
+    const int first = kDecoderFirst[any ? kContainerVersionBlocks - 1 : version - 1];
+    const int last = kDecoderFirst[any ? kContainerVersionBlocksAlias : version];
     const uint32_t sms = static_cast<uint32_t>(ctx->sms);
     const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
     cudaStream_t s = ctx->stream;
@@ -1889,7 +1885,7 @@ int container_decode_async(rb200_ctx* ctx, uint16_t version, const uint8_t* buf,
     }
     container_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status, version);
     rc = check_launch(ctx, "container_verdict_kernel");
-    for (int i = kDecoderFirst[version - 1]; i < kDecoderFirst[version] && rc == RB200_OK; i++) {
+    for (int i = first; i < last && rc == RB200_OK; i++) {
         const DecoderLaunch& l = ctx->async_decoders[i];
         l.kernel<<<l.grid, l.threads, l.smem, s>>>(buf, out, w, ctx->d_status);
         rc = check_launch(ctx, l.name);
@@ -1915,7 +1911,7 @@ extern "C" int rb200_container_decode_async(rb200_ctx* ctx, const uint8_t* buf, 
     return container_decode_async(ctx, kContainerVersion, buf, size, out, out_cap, d_n_symbols);
 }
 
-// Nine launches: the checks and every block decoder variant of RB200_BLOCK_CODER_DISPATCH.
+// Nine launches: the checks and the block decoder variants of the byte and rans64 coders (RB200_BLOCK_DISPATCH).
 extern "C" int rb200_container_blocks_coder_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                                          uint64_t* d_n_symbols)
 {
@@ -1923,7 +1919,7 @@ extern "C" int rb200_container_blocks_coder_decode_async(rb200_ctx* ctx, const u
     return container_decode_async(ctx, kContainerVersionBlocksCoder, buf, size, out, out_cap, d_n_symbols);
 }
 
-// Eight launches: the checks and every block decoder variant of RB200_BLOCK_ALIAS_DISPATCH.
+// Eight launches: the checks and the block decoder variants of the alias coder (RB200_BLOCK_DISPATCH).
 extern "C" int rb200_container_blocks_alias_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                                          uint64_t* d_n_symbols)
 {
@@ -1931,45 +1927,12 @@ extern "C" int rb200_container_blocks_alias_decode_async(rb200_ctx* ctx, const u
     return container_decode_async(ctx, kContainerVersionBlocksAlias, buf, size, out, out_cap, d_n_symbols);
 }
 
-// Thirteen launches: the any plan, both CRCs and the prefix check on the call's own workspace, the any verdict, then
-// the decoders of versions 2, 3 and 4 (1 + 4 + 3), each on its own version's workspace.  Only the header version's
-// workspace can hold a nonzero go, so the version-local decoder ids, which overlap across versions, never collide.
+// Thirteen launches: the checks and every block decoder variant of RB200_BLOCK_DISPATCH (versions 2, 3 and 4).
 extern "C" int rb200_container_blocks_any_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                                        uint64_t* d_n_symbols)
 {
     if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
-    DeviceGuard g(ctx->device);
-    ContainerAsyncWork* w = ctx->d_async_any;
-    const BlocksAnyWork any = {{ctx->d_async[kContainerVersionBlocks - 1], ctx->d_async[kContainerVersionBlocksCoder - 1],
-                                ctx->d_async[kContainerVersionBlocksAlias - 1]}};
-    const uint32_t sms = static_cast<uint32_t>(ctx->sms);
-    const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
-    cudaStream_t s = ctx->stream;
-    container_any_plan_kernel<<<1, 32, 0, s>>>(buf, size, w, any);
-    int rc = check_launch(ctx, "container_any_plan_kernel");
-    if (rc != RB200_OK) return rc;
-    crc32_kernel<<<crc32_grid(sms, after_head), kCrcThreads, kCrcSmemBytes, s>>>(buf + sizeof(ContainerHeader), after_head, &w->plan.meta_len,
-                                                                                 nullptr, 0, &w->crc_work, &w->crc[0]);
-    rc = check_launch(ctx, "crc32_kernel(meta)");
-    if (rc != RB200_OK) return rc;
-    crc32_kernel<<<crc32_grid(sms, size), kCrcThreads, kCrcSmemBytes, s>>>(buf, size, &w->plan.blob_len, &w->plan.blob_off, 0,
-                                                                           &w->crc_work, &w->crc[1]);
-    rc = check_launch(ctx, "crc32_kernel(blob)");
-    if (rc != RB200_OK) return rc;
-    container_prefix_check_kernel<<<sms * kPrefixCtasPerSm, kPrefixWarps * 32, 0, s>>>(buf, w);
-    rc = check_launch(ctx, "container_prefix_check_kernel");
-    if (rc != RB200_OK) return rc;
-    container_any_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status, any);
-    rc = check_launch(ctx, "container_any_verdict_kernel");
-    for (int i = kDecoderFirst[kContainerVersionBlocks - 1]; i < kDecoderFirst[kContainerVersionBlocksAlias] && rc == RB200_OK; i++) {
-        const DecoderLaunch& l = ctx->async_decoders[i];
-        const int version = i < kDecoderFirst[kContainerVersionBlocks] ? kContainerVersionBlocks
-                            : i < kDecoderFirst[kContainerVersionBlocksCoder] ? kContainerVersionBlocksCoder
-                                                                              : kContainerVersionBlocksAlias;
-        l.kernel<<<l.grid, l.threads, l.smem, s>>>(buf, out, ctx->d_async[version - 1], ctx->d_status);
-        rc = check_launch(ctx, l.name);
-    }
-    return rc;
+    return container_decode_async(ctx, kContainerVersionAnyBlocks, buf, size, out, out_cap, d_n_symbols);
 }
 
 namespace {

@@ -50,13 +50,15 @@ __global__ void __launch_bounds__(kMaxBlockWarps * 32)
                            target);
 }
 
-// block_prefix + block_fill_slots with block_decode_kernel's shared arrays; the slot table is pre-filled with a
-// sentinel so that a slot the fill misses shows.  flags[2i] = block_prefix's verdict, flags[2i + 1] = wide.
+// block_prefix + block_fill_slots with block_decode_kernel's shared memory layout (rings, then the table); the slot table
+// is pre-filled with a sentinel so that a slot the fill misses shows.  flags[2i] = block_prefix's verdict,
+// flags[2i + 1] = wide.
 __global__ void __launch_bounds__(kMaxBlockWarps * 32) batch_fill_slots(const uint16_t* rows, uint32_t* tab, uint32_t* flags)
 {
-    __shared__ __align__(16) uint32_t s_tab[kWordSlots];
+    extern __shared__ __align__(1024) uint8_t s_bdec[];
     __shared__ uint32_t s_cum[257];
     __shared__ uint32_t s_flag[2];
+    uint32_t* s_tab = reinterpret_cast<uint32_t*>(s_bdec + (blockDim.x >> 5) * kRingBytes);
     const uint32_t tid = threadIdx.x;
     for (uint32_t i = tid; i < kWordSlots; i += blockDim.x) s_tab[i] = 0xdeadbeefu;
     if (tid == 0) s_flag[1] = 0;
@@ -70,7 +72,7 @@ __global__ void __launch_bounds__(kMaxBlockWarps * 32) batch_fill_slots(const ui
     }
 }
 
-// block_prefix + block_build_enc_table with block_encode_kernel's shared arrays (the table at the start of the
+// block_prefix + block_build_enc_table with block_coder_encode_kernel<word>'s shared arrays (the table at the start of the
 // 1024-aligned dynamic shared memory).  flags[2i] = block_prefix's verdict, flags[2i + 1] = r32.
 __global__ void __launch_bounds__(kMaxBlockWarps * 32) batch_enc_table(const uint16_t* rows, uint4* out, uint32_t* flags)
 {
@@ -94,7 +96,7 @@ __global__ void __launch_bounds__(256) batch_enc_expand(const WordEncEntry* e, c
     out[i] = r32[blockIdx.x] ? word_enc_expand<true>(e[i]) : word_enc_expand<false>(e[i]);
 }
 
-// block_prefix + block_coder_decode_table<CODER> with block_coder_decode_kernel's dynamic shared memory layout (rings,
+// block_prefix + block_coder_decode_table<CODER> with block_decode_kernel's dynamic shared memory layout (rings,
 // then the table); the table is pre-filled with a sentinel.  A row block_prefix rejects gets no table (ok[i] = 0), as
 // in the shipped callers.
 template <uint32_t CODER>
@@ -210,7 +212,9 @@ int md_block_build(int wide, uint32_t threads, uint32_t n, const uint8_t* in, co
 
 int md_fill_slots(uint32_t threads, uint32_t n, const uint16_t* rows, uint32_t* tab, uint32_t* flags)
 {
-    batch_fill_slots<<<n, threads>>>(rows, tab, flags);
+    const uint32_t smem = block_coder_decode_smem(RB200_CODER_WORD, kWordScaleBits, threads);
+    cudaFuncSetAttribute(batch_fill_slots, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    batch_fill_slots<<<n, threads, smem>>>(rows, tab, flags);
     return finish();
 }
 

@@ -2,7 +2,7 @@
 blocks that do not start 16-byte aligned, 2-3 and 9-16 chunks per block (the 4-warp CTA with idle warps, the 512-thread
 CTA), 32-symbol chunks, tens of thousands of 32-symbol blocks, chunks above 64 Ki and the largest legal chunk, 2^24.
 
-For every instance of RB200_BLOCK_CODER_DISPATCH and RB200_BLOCK_ALIAS_DISPATCH and for the word coder, against the
+For every instance of RB200_BLOCK_DISPATCH (the word coder's included), against the
 oracle: the models built on the GPU, blob and directory with built and with caller models in both memory kinds, decode
 of the oracle's streams and of the GPU's own, the plain DEVICE-mode calls on input and output pointers that are not
 16-byte aligned (nothing written outside the output, past blob_bytes or past the last directory entry), the containers
@@ -583,7 +583,7 @@ def test_host_slice_pipeline(cuda_box):
     assert _child("child_slices", {"RB200_SLICE_MIB": str(SLICE_MIB)}).count("slices ok") == 4 * len(SLICED)
 
 
-# ---- rejects of block_coder_decode_kernel
+# ---- rejects of block_decode_kernel
 
 def _bad_inputs(blob, offs, unit, flip_chunks):
     """(what, blob, offsets, chunk whose output must stay untouched or None): a flipped byte inside each chunk of

@@ -197,7 +197,7 @@ def test_async_calls_reject_each_others_versions(gpu_ctx, oracle_lib, gen, base)
 
 
 def test_launches_per_call(gpu_ctx, base):
-    """plan, meta CRC, blob CRC, prefix check, verdict and the three decoders of RB200_BLOCK_ALIAS_DISPATCH"""
+    """plan, meta CRC, blob CRC, prefix check, verdict and the three alias decoders of RB200_BLOCK_DISPATCH"""
     torch = _torch()
     data, (nb, bs, ch, sb, freqs, offs, blob) = base
     good = api.container_blocks_alias_pack(sb, nb, bs, ch, freqs, offs, blob, CRC_BLOB)

@@ -238,7 +238,7 @@ def test_launch_counts(gpu_ctx):
     d_in = gbc._dev(data)
     d_buf = torch.zeros(cap + 16, dtype=torch.uint8, device="cuda")
     d_out = torch.zeros(data.size + 16, dtype=torch.uint8, device="cuda")
-    # choice + word (K5f) + byte 14 (K5c, scan, compaction) + alias 14 (the same) + CRCs + header
+    # choice + word (K5f) + byte 14 (K5, scan, compaction) + alias 14 (the same) + CRCs + header
     for flags, want in ((0, 10), (CRC_BLOB, 11)):
         before = gpu_ctx.launches
         gpu_ctx.container_blocks_model_encode_auto_async(THREE, 20000, d_in.data_ptr(), nb, bs, ch, flags, d_buf.data_ptr(), cap)

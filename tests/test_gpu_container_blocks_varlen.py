@@ -224,7 +224,7 @@ def test_argument_space_errors_and_launch_counts(gpu_ctx):
         assert call(THREE, nbp=nbp, out_cap=boff + 64) == 0
         assert lib.rb200_sync(gpu_ctx.h) == -3
         assert (d_buf[:64].cpu().numpy() == SENTINEL).all()
-    # launches: plan, choice, K5f (word), K5c + scan + compaction (byte 14, alias 14), the CRCs, the header; with the
+    # launches: plan, choice, K5f (word), K5 + scan + compaction (byte 14, alias 14), the CRCs, the header; with the
     # blob CRC also the blob length kernel.  One candidate: no choice kernel.
     for cands, flags, want in ((THREE, 0, 11), (THREE, CRC_BLOB, 13), ([CAND(WORD, 12)], 0, 4), ([CAND(BYTE, 14)], 0, 6),
                                ([CAND(ALIAS, 14)], CRC_BLOB, 8)):

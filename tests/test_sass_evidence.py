@@ -63,3 +63,24 @@ def test_main_loop_step_lengths(kernels):
     ali = next(v for k, v in kernels.items() if "alias_decode_persist_kernelILj16E" in k)
     assert len(sass_steps.step_between(tma, "STG.E.U8", 2)) <= 17
     assert len(sass_steps.step_between(ali, "STG.E.U8", 2)) <= 30
+
+
+# The word coder's per-block decode step (vote to vote), opcodes in issue order.  block_decode_planned_kernel<word, 12>
+# keeps the order of the one-CTA-per-block kernel it replaced only with its table in static shared memory and the table
+# address taken per chunk (container_decode.cuh); a change to the shared per-block body that moves either step shows here.
+WORD_BLOCK_STEP = {
+    "block_decode_kernelILj0ELj12E": [
+        "VOTE.ANY", "LOP3.LUT", "POPC", "IMAD", "LOP3.LUT", "LDS.U16", "PRMT", "LOP3.LUT", "SHF.R.U32.HI", "IMAD", "LDS",
+        "SHF.R.U32.HI", "STG.E.U8", "SHF.R.U32.HI", "LOP3.LUT", "IMAD", "POPC", "ISETP.GE.U32.AND", "IMAD"],
+    "block_decode_planned_kernelILj0ELj12E": [
+        "VOTE.ANY", "LOP3.LUT", "POPC", "POPC", "IMAD", "IMAD", "LOP3.LUT", "LDS.U16", "PRMT", "LOP3.LUT", "SHF.R.U32.HI",
+        "IMAD", "LDS", "SHF.R.U32.HI", "STG.E.U8", "SHF.R.U32.HI", "LOP3.LUT", "IMAD", "ISETP.GE.U32.AND"],
+}
+
+
+@pytest.mark.parametrize("name", sorted(WORD_BLOCK_STEP))
+def test_word_block_decode_step(kernels, name):
+    import sass_steps
+    body = next(v for k, v in kernels.items() if name in k)
+    step = sass_steps.step_between(body, "VOTE.ANY", 5)
+    assert [re.match(r"(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)", ins).group(1) for _, ins in step] == WORD_BLOCK_STEP[name]

@@ -41,7 +41,7 @@ def step_between(instrs, opcode, skip, max_len=60):
 def main():
     lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "ryg_rans_b200", "librans_b200.so")
     fns = functions(subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout)
-    dec = next(v for k, v in fns.items() if "block_decode_kernel" in k)
+    dec = next(v for k, v in fns.items() if "block_decode_kernelILj0ELj12E" in k)
     enc = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1ELb0ELb0E" in k)
     enc_gated = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1ELb1ELb0E" in k)
     enc_varlen = next(v for k, v in fns.items() if "word_encode_fused_kernelILb1ELb1ELb1E" in k)
@@ -57,7 +57,7 @@ def main():
                          step_between(ali, "STG.E.U8", 2)),
                         ("alias_decode_planned_kernel<16> (rb200_container_decode_async): one step (symbol store to symbol store)",
                          step_between(ali_planned, "STG.E.U8", 2)),
-                        ("block_decode_kernel (round 1 window: decode_window_chunk with WordDecoder<false>): one step (vote to vote)",
+                        ("block_decode_kernel<word, 12> (round 1 window: decode_window_chunk with WordDecoder<false>): one step (vote to vote)",
                          step_between(dec, "VOTE.ANY", 5)),
                         ("word_encode_fused_kernel<R32>: one step (symbol load to symbol load)", step_between(enc, "LDS.U8", 8)),
                         ("word_encode_fused_kernel<R32, GATED> (rb200_container_model_encode_async): one step (symbol load to symbol "
