@@ -341,6 +341,52 @@ int rb200_container_blocks_alias_decode(rb200_ctx* ctx, const uint8_t* buf, size
 int rb200_container_blocks_alias_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                               uint64_t* d_n_symbols);
 
+/* ---------------------------------------------------------------- per-block containers with stored blocks */
+
+/* Version 5: the layout of versions 2-4 (rb200_container_blocks_size gives its size) with the header of the per-block
+ * version of its pair (bytes 6-7: word at 12; byte, rans64 or alias at 8..15) and the version field 5.  A block whose
+ * row of block_freqs is all zero is STORED: each of its chunks is a stream of round16(chunk_syms) bytes, the chunk's
+ * symbols and then zero bytes, placed in the blob and the directory by the rules of a coded stream of that length
+ * (so the chunk's directory step, (offsets[c + 1] & ~15) - offsets[c], is exactly round16(chunk_syms)).  Every other
+ * row sums to 1 << scale_bits and its block is coded as in versions 2-4.  Only the _stored_ calls accept version 5;
+ * every other container call, rb200_container_blocks_any_decode_async included, rejects it (RB200_E_STREAM).
+ *   bound: header + models + directory + n_chunks x round16(chunk_syms): the most any version 5 container of that
+ *          geometry takes (0 for a geometry the per-block calls refuse).
+ *   pack:  host only; block_freqs with zero rows for stored blocks.  RB200_E_ARG for a bad pair or geometry, a null
+ *          pointer, and a directory that disagrees with the blob or gives a stored chunk the wrong step or nonzero
+ *          padding; RB200_E_MODEL for a row that is neither zero nor sums to 1 << scale_bits; RB200_E_SPACE when out_cap
+ *          is below the container.
+ *   open:  as rb200_container_blocks_coder_open (the version 3 info struct), with the rules above and those of the
+ *          twin version; RB200_E_STREAM for anything else, versions 1-4 among them. */
+size_t rb200_container_blocks_stored_bound(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms);
+int rb200_container_blocks_stored_pack(int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                       const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes,
+                                       uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size);
+int rb200_container_blocks_stored_open(const uint8_t* buf, size_t size, rb200_container_blocks_coder_info* info);
+/* A version 5 container of the blocks at `in`, in DEVICE memory with the models built on the GPU, enqueued only: the
+ * pair is rb200_choose_blocks_coder's choice over `candidates` (every block counted, stored or not; one candidate is
+ * encoded as it is, with no choice kernel), every block is encoded with it, and then a block is stored when its coded
+ * chunks take more than (block_size / chunk_syms) x round16(chunk_syms) bytes of blob (each stream rounded up to 16).
+ * The decision is made from the streams the encoder wrote, so out_cap >= rb200_container_blocks_stored_bound(n_blocks,
+ * block_size, chunk_syms) always suffices.  Arguments, space and sync verdicts are those of
+ * rb200_container_blocks_model_encode_auto_async: RB200_E_ARG (nothing launched) for a null ctx, in or out, a misaligned
+ * out, an invalid list or candidate, tolerance_ppm > 10^6, a bad geometry or 2^31 chunks or more; RB200_E_SPACE when
+ * out_cap is below the blob offset; rb200_sync returns RB200_E_SPACE when the blob does not fit out_cap, header
+ * unwritten.  Capturable in a CUDA graph after one call with the same list and geometry outside the capture. */
+int rb200_container_blocks_stored_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                               const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                               uint32_t flags, uint8_t* out, size_t out_cap);
+/* The contract of rb200_container_blocks_alias_decode_async with version 5 in place of version 4: kernels check the
+ * header, every row (zero or summing), the directory, every stored chunk's step and padding, meta_crc and the optional
+ * blob CRC, then the block decoder of the header's pair runs, copying stored blocks and decoding the others.  DEVICE
+ * memory only, buf and out 16-byte aligned, d_n_symbols 8-byte aligned or NULL; enqueue only; RB200_E_ARG (nothing
+ * launched) or RB200_E_CUDA from the call.  rb200_sync gives the verdict: RB200_E_STREAM for anything
+ * rb200_container_blocks_stored_open rejects (versions 1-4 among them) and for a blob of 2^36 bytes or more,
+ * RB200_E_SPACE for n > out_cap, content errors first; in both cases out is untouched.  A corrupt coded stream that
+ * passes every check is RB200_E_STREAM. */
+int rb200_container_blocks_stored_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                               uint64_t* d_n_symbols);
+
 /* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
  * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's
  * decode table is built on the GPU into the context, and the decoder the header calls for is picked on the GPU -- all

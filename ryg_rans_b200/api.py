@@ -96,6 +96,13 @@ EXPORTS = [
     ("rb200_container_blocks_model_encode_varlen_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
                                                                    C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_container_blocks_any_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_container_blocks_stored_bound", C.c_size_t, [C.c_uint32, C.c_uint32, C.c_uint32]),
+    ("rb200_container_blocks_stored_pack", C.c_int, [C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                     C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("rb200_container_blocks_stored_open", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_container_blocks_stored_encode_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
+                                                             C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_container_blocks_stored_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -264,6 +271,33 @@ def container_blocks_alias_pack(scale_bits, n_blocks, block_size, chunk_syms, bl
 def container_blocks_alias_open(buf):
     """rb200_container_blocks_alias_open: as container_blocks_coder_open, for version 4"""
     return container_blocks_coder_open(buf, _open="rb200_container_blocks_alias_open")
+
+
+def container_blocks_stored_bound(n_blocks, block_size, chunk_syms):
+    """rb200_container_blocks_stored_bound: the most bytes a version 5 container of this geometry takes (0 for a geometry
+    the per-block calls refuse)"""
+    return int(load().dll.rb200_container_blocks_stored_bound(n_blocks, block_size, chunk_syms))
+
+
+def container_blocks_stored_pack(coder, scale_bits, n_blocks, block_size, chunk_syms, block_freqs, offsets, blob, flags=0):
+    """rb200_container_blocks_stored_pack: a version 5 container (any per-block pair; a zero row of block_freqs marks a
+    stored block, whose chunks are round16(chunk_syms)-byte streams of their symbols and zero padding)"""
+    lib = load()
+    block_freqs = np.ascontiguousarray(block_freqs, dtype=np.uint16)
+    offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+    blob = np.ascontiguousarray(blob, dtype=np.uint8)
+    total = int(lib.dll.rb200_container_blocks_size(n_blocks, offsets.size - 1, blob.size))
+    out = np.zeros(total, np.uint8)
+    size = C.c_size_t(0)
+    lib.check(lib.dll.rb200_container_blocks_stored_pack(coder, scale_bits, n_blocks, block_size, chunk_syms, block_freqs.ctypes.data,
+                                                         offsets.ctypes.data, blob.ctypes.data, blob.size, flags, out.ctypes.data, total,
+                                                         C.byref(size)))
+    return out[:size.value]
+
+
+def container_blocks_stored_open(buf):
+    """rb200_container_blocks_stored_open: as container_blocks_coder_open, for version 5"""
+    return container_blocks_coder_open(buf, _open="rb200_container_blocks_stored_open")
 
 
 def container_blocks_coder_open(buf, _open="rb200_container_blocks_coder_open"):
@@ -798,6 +832,22 @@ class Context:
         (CUDA-graph capturable).  The verdict (-4 corrupt or another version, -3 out_cap too small, output untouched)
         comes from sync()"""
         self.lib.check(self.lib.dll.rb200_container_blocks_any_decode_async(self.h, buf_ptr, size, out_ptr, out_cap, n_ptr or None), self.h)
+
+    def container_blocks_stored_encode_async(self, candidates, tolerance_ppm, in_ptr, n_blocks, block_size, chunk_syms, flags, out_ptr,
+                                             out_cap):
+        """container_blocks_model_encode_auto_async's choice and encoders, then every block whose coded chunks take more
+        than its stored size is stored: a version 5 container of at most container_blocks_stored_bound bytes.  The
+        verdict (-3 when the blob does not fit, header unwritten) comes from sync()"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_blocks_stored_encode_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
+                                                                               in_ptr, n_blocks, block_size, chunk_syms, flags, out_ptr,
+                                                                               out_cap), self.h)
+
+    def container_blocks_stored_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
+        """the async decode of a version 5 container; enqueue only (CUDA-graph capturable).  The verdict (-4 corrupt or
+        another version, -3 out_cap too small, output untouched) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_blocks_stored_decode_async(self.h, buf_ptr, size, out_ptr, out_cap, n_ptr or None),
+                       self.h)
 
     def container_blocks_alias_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
         """enqueue only (CUDA-graph capturable); n_ptr: device address of a u64 that receives n, or 0.  The verdict on

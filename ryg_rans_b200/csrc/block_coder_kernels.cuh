@@ -10,7 +10,8 @@
 //                          tables.h formulas (byte_enc_entry / rans64_enc_entry, 8x replicated as K8 / K9 stage it), and
 //                          encode_chunk_split per warp with AliasEncoder<false, SB> / Rans64Encoder: the split path's
 //                          slots, followed by K6's tile scan and compaction.  The word coder has the flags-off instance
-//                          only: a word encode that builds its models runs K5f (block_encode_fused_kernel).
+//                          and the GATED one of rb200_container_blocks_stored_encode_async, which needs every stream's
+//                          size before anything is placed; its other model-building encodes run K5f (block_encode_fused_kernel).
 //   block_decode_kernel<CODER, SB>
 //                          the block's decode table in shared memory (block_decode_table: the word coder's 4096 slot
 //                          entries, RansWordTablesInitSymbol of rans_word_sse41.h:64-72; cum2sym[1 << sb], then
@@ -426,13 +427,14 @@ block_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const 
     }
 
 // The split encoder instance of (CODER, SB): (BUILD, GATED, GEOM) = (build, 0, 0) for the fixed calls, (1, 1, 0) for the
-// auto encode, (1, 1, 1) for the device-count encode.  The word coder has only (0, 0, 0), null for any other flags: its
-// model-building encodes run K5f (plan_blocks_encode).
+// auto and the stored encodes, (1, 1, 1) for the device-count encode.  The word coder has only (0, 0, 0) and (1, 1, 0),
+// null for any other flags: its other model-building encodes run K5f (plan_blocks_encode).
 using BlockEncodeKernel = decltype(&block_coder_encode_kernel<RB200_CODER_BYTE, 0, false>);
 template <uint32_t CODER, uint32_t SB>
 inline BlockEncodeKernel block_encode_for(bool build, bool gated, bool geom)
 {
-    if constexpr (CODER == RB200_CODER_WORD) return build || gated || geom ? nullptr : block_coder_encode_kernel<CODER, SB, false>;
+    if constexpr (CODER == RB200_CODER_WORD)
+        return gated && !geom ? block_coder_encode_kernel<CODER, SB, true, true> : build || geom ? nullptr : block_coder_encode_kernel<CODER, SB, false>;
     else if (geom) return block_coder_encode_kernel<CODER, SB, true, true, true>;
     else if (gated) return block_coder_encode_kernel<CODER, SB, true, true>;
     else return build ? block_coder_encode_kernel<CODER, SB, true> : block_coder_encode_kernel<CODER, SB, false>;

@@ -30,6 +30,10 @@
 // rb200_container_blocks_any_decode_async runs the same stages on its own workspace for whichever per-block version the
 // header names (kContainerVersionAnyBlocks), then the decoders of versions 2, 3 and 4: their ids are unique across
 // those versions.
+//
+// rb200_container_blocks_stored_decode_async (version 5) runs the STORED instances of the plan (version 5 planned as
+// its twin version), of the prefix check (zero rows, stored chunks' steps and padding) and of the eight per-block
+// decoders, which copy a stored block's chunks and decode every other block as versions 2-4 do, with the same ids.
 #pragma once
 #include "alias_kernels.cuh"
 #include "block_coder_kernels.cuh"
@@ -101,6 +105,9 @@ __host__ __device__ constexpr uint32_t container_decoder(uint32_t version, uint3
 // One warp: the plan of a header that passes the rules of the call's version (a zero plan otherwise), with the verdict
 // words and the decoders' counters cleared.  kContainerVersionAnyBlocks: the version the header names when that is 2, 3
 // or 4; any other version, or fewer than 64 bytes, gets the zero plan.
+// STORED (rb200_container_blocks_stored_decode_async): version 5 alone (container_stored_header_ok), planned as its
+// twin, whose layout it has; `version` is unused.
+template <bool STORED = false>
 __global__ void __launch_bounds__(32)
     container_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t version, ContainerAsyncWork* w)
 {
@@ -112,8 +119,15 @@ __global__ void __launch_bounds__(32)
     BlocksPlan p = {};
     uint32_t coder = 0, scale_bits = 0;
     if (size >= sizeof(ContainerHeader)) {                           // a shorter buffer is not read at all
-        const ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(buf);
-        if (container_header_ok(h, size, static_cast<uint16_t>(version))) {
+        ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(buf);
+        bool ok;
+        if (STORED) {
+            ok = container_stored_header_ok(h, size);
+            h = container_stored_twin(h);
+        } else {
+            ok = container_header_ok(h, size, static_cast<uint16_t>(version));
+        }
+        if (ok) {
             p.ok = 1;
             p.n_symbols = h.n_symbols;
             p.n_chunks = h.n_chunks;
@@ -146,9 +160,12 @@ __global__ void __launch_bounds__(32)
 // The per-element rules of the prefix.  Each warp stages 32 block models (16 KiB, coalesced) in shared memory with
 // rows padded to 129 words, so that lane r checking row r reads a different bank from every other lane.  Every block
 // sums to 1 << scale_bits; version 1 has no blocks (n_blocks 0), so only the directory rules run.
+// STORED (version 5): a row may also be all zero, and then lane r checks the step and the zero padding of each of that
+// block's chunks (container_stored_step_ok, container_stored_pad_ok), reading the padding only inside the blob.
 constexpr int kPrefixWarps = 2;
 constexpr uint32_t kPrefixRowWords = 129;
 
+template <bool STORED = false>
 __global__ void __launch_bounds__(kPrefixWarps * 32)
     container_prefix_check_kernel(const uint8_t* __restrict__ buf, ContainerAsyncWork* w)
 {
@@ -173,7 +190,14 @@ __global__ void __launch_bounds__(kPrefixWarps * 32)
             d[3] = v.w;
         }
         __syncwarp();
-        if (lane < n) ok &= container_block_model_sums_to(reinterpret_cast<const uint16_t*>(rows + lane * kPrefixRowWords), total);
+        if (STORED && lane < n && container_block_model_stored(reinterpret_cast<const uint16_t*>(rows + lane * kPrefixRowWords))) {
+            const uint32_t per_block = p.block_size / p.chunk_syms;
+            const uint8_t* blob = buf + p.blob_off;
+            for (uint64_t c = (b0 + lane) * per_block; c < (b0 + lane + 1) * per_block; c++)
+                ok &= container_stored_step_ok(offsets, c, p.chunk_syms, p.blob_bytes) && container_stored_pad_ok(blob + offsets[c], p.chunk_syms);
+        } else if (lane < n) {
+            ok &= container_block_model_sums_to(reinterpret_cast<const uint16_t*>(rows + lane * kPrefixRowWords), total);
+        }
         __syncwarp();
     }
     const uint64_t threads = static_cast<uint64_t>(gridDim.x) * blockDim.x;
@@ -313,9 +337,30 @@ __global__ void __launch_bounds__(32)
 // steps: the table in shared memory (block_decode_table), then the warps take the block's 1..32 chunks in turn
 // (block_decode_chunk).  The alias coder's pairing overlays the table the previous block's warps read: the barrier at
 // the loop's top keeps it behind their last chunk.  The word instance keeps 8 CTAs per SM (32 registers).
+// STORED (rb200_container_blocks_stored_decode_async, version 5): a block whose row is all zero is stored, and the warps
+// copy its chunks from the blob (block_copy_stored) in place of the table and the decode.
 constexpr int kPlannedWarps = 8;
+static_assert(kPlannedWarps * 32 == 256, "STORED: one thread per frequency of a row");
 
-template <uint32_t CODER, uint32_t SB>
+// One chunk of a stored block, one warp: chunk_syms symbols from src (16-byte aligned: a stored stream starts a vector)
+// to dst, with 16-byte loads; whole 16-byte stores where dst and the length allow them, bytes otherwise.
+__device__ __forceinline__ void block_copy_stored(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t chunk_syms, uint32_t lane)
+{
+    const bool vec = ((reinterpret_cast<uintptr_t>(dst) | chunk_syms) & 15) == 0;
+    for (uint32_t v = lane; v < (chunk_syms + 15) / 16; v += 32) {
+        const uint4 q = ldg_stream_u128(reinterpret_cast<const uint4*>(src) + v);
+        if (vec) {
+            stg_stream_u128(reinterpret_cast<uint4*>(dst) + v, q);
+        } else {
+            const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+            for (uint32_t j = 0; j < 16; j++)
+                if (16 * v + j < chunk_syms) dst[16 * v + j] = static_cast<uint8_t>(w[j >> 2] >> (8 * (j & 3)));
+        }
+    }
+}
+
+template <uint32_t CODER, uint32_t SB, bool STORED = false>
 __global__ void __launch_bounds__(kPlannedWarps * 32, CODER == RB200_CODER_WORD ? 8 : 0)
     block_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                 uint32_t* __restrict__ status)
@@ -348,6 +393,13 @@ __global__ void __launch_bounds__(kPlannedWarps * 32, CODER == RB200_CODER_WORD 
         const uint32_t block = s_block;
         if (block >= n_blocks) break;
         // a model that does not sum was refused by the prefix check: not reached
+        // a stored block: its row is all zero (256 threads, one frequency each); the prefix check saw its chunks
+        if (STORED && !__syncthreads_or(models[static_cast<uint64_t>(block) * 256 + tid] != 0)) {
+            for (uint32_t k = warp; k < per_block; k += kPlannedWarps)
+                block_copy_stored(blob + offsets[block * per_block + k],
+                                  out + static_cast<uint64_t>(block) * block_size + static_cast<uint64_t>(k) * chunk_syms, chunk_syms, tid & 31);
+            continue;
+        }
         if (!block_decode_table<CODER, SB>(models + static_cast<uint64_t>(block) * 256, 1u << sb, s_cum, s_flag, s_bdec, kPlannedWarps)) {
             if (tid == 0) atomicOr(status, kStatStream);
             continue;
@@ -513,9 +565,9 @@ struct DecoderLaunch {
 };
 
 // The decoders of every version in one launch table, each version's in id order: version v's are the entries
-// kDecoderFirst[v - 1] .. kDecoderFirst[v] - 1.
-constexpr int kDecoderFirst[] = {0, 11, 12, 16, 19};
-constexpr int kContainerDecoders = kDecoderFirst[4];
+// kDecoderFirst[v - 1] .. kDecoderFirst[v] - 1.  Version 5's are the STORED twins of versions 2-4's, with their ids.
+constexpr int kDecoderFirst[] = {0, 11, 12, 16, 19, 27};
+constexpr int kContainerDecoders = kDecoderFirst[5];
 // the prefix check's grid: kPrefixCtasPerSm CTAs of kPrefixWarps warps per SM
 constexpr uint32_t kPrefixCtasPerSm = 8;
 
@@ -552,6 +604,21 @@ inline void configure_container_decode(uint32_t sms, DecoderLaunch* out)
          "block_decode_planned_kernel<alias, 12>"},
         {block_decode_planned_kernel<RB200_CODER_ALIAS, 0>, 0, planned,
          block_coder_decode_smem(RB200_CODER_ALIAS, kBlockCoderMaxScaleBits, planned), "block_decode_planned_kernel<alias, 0>"},
+        {block_decode_planned_kernel<RB200_CODER_WORD, kWordScaleBits, true>, 0, planned, 0, "block_decode_planned_kernel<word, 12, stored>"},
+        {block_decode_planned_kernel<RB200_CODER_BYTE, 14, true>, 0, planned, block_coder_decode_smem(RB200_CODER_BYTE, 14, planned),
+         "block_decode_planned_kernel<byte, 14, stored>"},
+        {block_decode_planned_kernel<RB200_CODER_BYTE, 12, true>, 0, planned, block_coder_decode_smem(RB200_CODER_BYTE, 12, planned),
+         "block_decode_planned_kernel<byte, 12, stored>"},
+        {block_decode_planned_kernel<RB200_CODER_BYTE, 0, true>, 0, planned,
+         block_coder_decode_smem(RB200_CODER_BYTE, kBlockCoderMaxScaleBits, planned), "block_decode_planned_kernel<byte, 0, stored>"},
+        {block_decode_planned_kernel<RB200_CODER_RANS64, 0, true>, 0, planned,
+         block_coder_decode_smem(RB200_CODER_RANS64, kBlockCoderMaxScaleBits, planned), "block_decode_planned_kernel<rans64, 0, stored>"},
+        {block_decode_planned_kernel<RB200_CODER_ALIAS, 14, true>, 0, planned, block_coder_decode_smem(RB200_CODER_ALIAS, 14, planned),
+         "block_decode_planned_kernel<alias, 14, stored>"},
+        {block_decode_planned_kernel<RB200_CODER_ALIAS, 12, true>, 0, planned, block_coder_decode_smem(RB200_CODER_ALIAS, 12, planned),
+         "block_decode_planned_kernel<alias, 12, stored>"},
+        {block_decode_planned_kernel<RB200_CODER_ALIAS, 0, true>, 0, planned,
+         block_coder_decode_smem(RB200_CODER_ALIAS, kBlockCoderMaxScaleBits, planned), "block_decode_planned_kernel<alias, 0, stored>"},
     };
     for (int i = 0; i < kContainerDecoders; i++) {
         out[i] = l[i];

@@ -18,6 +18,7 @@ constexpr uint16_t kContainerVersion = 1;           // one model: 256 x u32
 constexpr uint16_t kContainerVersionBlocks = 2;     // one model per block: n_blocks x 256 x u16, word coder
 constexpr uint16_t kContainerVersionBlocksCoder = 3;  // version 2's layout with the byte or rans64 coder at scale_bits 8..15
 constexpr uint16_t kContainerVersionBlocksAlias = 4;  // version 2's layout with the alias coder at scale_bits 8..15
+constexpr uint16_t kContainerVersionBlocksStored = 5; // the layout of versions 2-4 for any of their pairs, with stored blocks
 
 struct ContainerHeader {        // 64 bytes
     uint32_t magic;
@@ -57,6 +58,13 @@ RB200_HD inline uint64_t container_model_bytes(const ContainerHeader& h)
 RB200_HD inline uint64_t container_dir_offset(const ContainerHeader& h) { return sizeof(ContainerHeader) + container_model_bytes(h); }
 RB200_HD inline uint64_t container_dir_end(const ContainerHeader& h) { return container_dir_offset(h) + (h.n_chunks + 1) * sizeof(uint64_t); }
 RB200_HD inline uint64_t container_blob_offset(const ContainerHeader& h) { return (container_dir_end(h) + 15) & ~15ull; }
+
+// the per-block version of a coder: word 2, byte and rans64 3, alias 4
+RB200_HD inline uint16_t container_blocks_version(uint32_t coder)
+{
+    return coder == RB200_CODER_WORD ? kContainerVersionBlocks : coder == RB200_CODER_ALIAS ? kContainerVersionBlocksAlias
+                                                                                         : kContainerVersionBlocksCoder;
+}
 
 // The coder and scale_bits of each per-block version, for its headers and for the arguments of its calls: the word
 // coder at 12 (version 2), byte or rans64 at 8..15 (version 3), alias at 8..15 (version 4)
@@ -105,6 +113,25 @@ RB200_HD inline bool container_header_ok(const ContainerHeader& h, uint64_t size
     }
     const uint64_t boff = container_blob_offset(h);                 // < 2^42: n_chunks < 2^31, n_blocks < 2^32
     return boff <= size && h.blob_bytes <= size - boff;
+}
+
+// Version 5 (stored blocks) is the header of its twin -- the per-block version of its coder (2, 3 or 4) -- with the
+// version field 5: every header rule and the layout are the twin's, so the twin's header is what the layout functions
+// above take.  A coder past rans64 has no twin (version 0, which no rule accepts).
+RB200_HD inline ContainerHeader container_stored_twin(ContainerHeader h)
+{
+    h.version = h.coder <= RB200_CODER_RANS64 ? container_blocks_version(h.coder) : 0;
+    return h;
+}
+RB200_HD inline bool container_stored_header_ok(const ContainerHeader& h, uint64_t size)
+{
+    const ContainerHeader t = container_stored_twin(h);
+    return h.version == kContainerVersionBlocksStored && t.version && container_header_ok(t, size, t.version);
+}
+// the header whose layout a header has (host): version 5's twin, any other version itself
+inline ContainerHeader container_layout(const ContainerHeader& h)
+{
+    return h.version == kContainerVersionBlocksStored ? container_stored_twin(h) : h;
 }
 
 // what rb200_model_create would accept: a known coder, its scale_bits range, frequencies that sum to 1 << scale_bits
@@ -196,12 +223,6 @@ RB200_HD inline int choose_candidate(const uint64_t* costs, uint32_t n, uint32_t
 // The per-block coder choice of rb200_choose_blocks_coder and rb200_container_blocks_model_encode_auto_async
 // (blocks_choice_kernel): C7's steps per block, summed over the blocks.  A candidate is a pair some per-block version
 // takes (container_blocks_coder_ok): word at 12, byte, rans64 or alias at 8..15.
-// the per-block version of a coder: word 2, byte and rans64 3, alias 4
-RB200_HD inline uint16_t container_blocks_version(uint32_t coder)
-{
-    return coder == RB200_CODER_WORD ? kContainerVersionBlocks : coder == RB200_CODER_ALIAS ? kContainerVersionBlocksAlias
-                                                                                         : kContainerVersionBlocksCoder;
-}
 RB200_HD inline bool blocks_candidate_ok(uint32_t c)
 {
     const uint32_t coder = c >> 8, sb = c & 0xffu;
@@ -241,6 +262,25 @@ RB200_HD inline bool container_dir_ends_ok(const uint64_t* offsets, uint64_t n_c
     return offsets[n_chunks] == blob_bytes && (!n_chunks || offsets[0] < 16);
 }
 
+// Version 5: a block whose row is all zero is stored; every other row sums to 1 << scale_bits (container_block_model_sums_to)
+RB200_HD inline bool container_block_model_stored(const uint16_t* freqs) { return container_block_model_sums_to(freqs, 0); }
+// the stream of a stored chunk: its chunk_syms symbols, then zero bytes up to a multiple of 16
+RB200_HD inline uint64_t container_stored_bytes(uint32_t chunk_syms) { return (chunk_syms + 15ull) & ~15ull; }
+// chunk c of a stored block: its stream [offsets[c], offsets[c + 1] & ~15) is container_stored_bytes long and lies in the
+// blob (so its bytes can be read once this holds, whatever the other entries say)
+RB200_HD inline bool container_stored_step_ok(const uint64_t* offsets, uint64_t c, uint32_t chunk_syms, uint64_t blob_bytes)
+{
+    const uint64_t end = offsets[c + 1] & ~15ull;
+    return end >= offsets[c] && end - offsets[c] == container_stored_bytes(chunk_syms) && end <= blob_bytes;
+}
+// and its padding, the bytes after the symbols, is zero
+RB200_HD inline bool container_stored_pad_ok(const uint8_t* stream, uint32_t chunk_syms)
+{
+    for (uint64_t i = chunk_syms; i < container_stored_bytes(chunk_syms); i++)
+        if (stream[i]) return false;
+    return true;
+}
+
 // the header rb200_container_pack writes (crc fields zero)
 ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_syms, uint64_t n, uint64_t n_chunks,
                                  uint64_t blob_bytes, uint32_t flags);
@@ -250,6 +290,9 @@ ContainerHeader container_blocks_header(uint32_t n_blocks, uint32_t block_size, 
 // fields zero)
 ContainerHeader container_blocks_coder_header(uint16_t version, int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
                                               uint64_t blob_bytes, uint32_t flags);
+// version 5: every row is stored or sums to 1 << h.scale_bits, and every chunk of a stored block has its step and zero
+// padding (container_stored_step_ok, container_stored_pad_ok); the directory rules hold already
+bool container_stored_rows_ok(const ContainerHeader& h, const uint16_t* rows, const uint64_t* offsets, const uint8_t* blob);
 // every block's 256 frequencies sum to total
 bool container_block_models_sum_to(const uint16_t* block_freqs, uint32_t n_blocks, uint32_t total);
 // the directory rules: the first stream starts inside the first vector, monotone, last entry == blob_bytes
@@ -264,10 +307,11 @@ uint32_t container_meta_crc(const ContainerHeader& h, const void* model, const u
 // The parser, in the order rb200_container_open applies it.  Each step returns RB200_OK or RB200_E_STREAM; the CRC
 // values are the caller's, computed wherever the bytes live.
 //  1. the 64-byte header against the buffer size (`size` bytes in all; `hdr` holds at least 64 of them); `version`
-//     is the one the caller accepts (kContainerVersion, kContainerVersionBlocks, kContainerVersionBlocksCoder or
-//     kContainerVersionBlocksAlias), any other is rejected
+//     is the one the caller accepts (kContainerVersion, kContainerVersionBlocks, kContainerVersionBlocksCoder,
+//     kContainerVersionBlocksAlias or kContainerVersionBlocksStored), any other is rejected
 int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, ContainerHeader* h);
-//  2. header + model + directory (`prefix`: container_blob_offset(h) bytes), given their CRC
+//  2. header + model + directory (`prefix`: container_blob_offset(h) bytes), given their CRC; version 5 (`buf`, its
+//     blob included): the stored chunks' steps and padding as well
 int container_check_prefix(const ContainerHeader& h, const uint8_t* prefix, uint32_t meta_crc);
 //  3. the blob, given its CRC (only consulted when the header carries one)
 int container_check_blob(const ContainerHeader& h, uint32_t blob_crc);

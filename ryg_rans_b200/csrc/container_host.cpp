@@ -87,7 +87,7 @@ uint32_t container_header_crc(const ContainerHeader& h)
 uint32_t container_meta_crc(const ContainerHeader& h, const void* model, const uint64_t* offsets)
 {
     uint32_t c = container_header_crc(h);
-    c = container_crc32(c, model, container_model_bytes(h));
+    c = container_crc32(c, model, container_model_bytes(container_layout(h)));
     return container_crc32(c, offsets, (h.n_chunks + 1) * sizeof(uint64_t));
 }
 
@@ -95,6 +95,22 @@ bool container_block_models_sum_to(const uint16_t* block_freqs, uint32_t n_block
 {
     for (uint64_t b = 0; b < n_blocks; b++)
         if (!container_block_model_sums_to(block_freqs + b * 256, total)) return false;
+    return true;
+}
+
+bool container_stored_rows_ok(const ContainerHeader& h, const uint16_t* rows, const uint64_t* offsets, const uint8_t* blob)
+{
+    const uint32_t per_block = h.block_size / h.chunk_syms;
+    for (uint64_t b = 0; b < h.n_blocks; b++) {
+        const uint16_t* row = rows + b * 256;
+        if (!container_block_model_stored(row)) {
+            if (!container_block_model_sums_to(row, 1u << h.scale_bits)) return false;
+            continue;
+        }
+        for (uint64_t c = b * per_block; c < (b + 1) * per_block; c++)
+            if (!container_stored_step_ok(offsets, c, h.chunk_syms, h.blob_bytes) || !container_stored_pad_ok(blob + offsets[c], h.chunk_syms))
+                return false;
+    }
     return true;
 }
 
@@ -148,7 +164,8 @@ int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, Co
     if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
     ContainerHeader h;
     std::memcpy(&h, hdr, sizeof h);
-    if (!container_header_ok(h, size, version)) return RB200_E_STREAM;
+    const bool ok = version == kContainerVersionBlocksStored ? container_stored_header_ok(h, size) : container_header_ok(h, size, version);
+    if (!ok) return RB200_E_STREAM;
     *out = h;
     return RB200_OK;
 }
@@ -156,8 +173,13 @@ int container_parse_header(const uint8_t* hdr, size_t size, uint16_t version, Co
 int container_check_prefix(const ContainerHeader& h, const uint8_t* prefix, uint32_t meta_crc)
 {
     const uint8_t* model = prefix + sizeof(ContainerHeader);
-    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(prefix + container_dir_offset(h));
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(prefix + container_dir_offset(container_layout(h)));
     if (meta_crc != h.meta_crc) return RB200_E_STREAM;
+    if (h.version == kContainerVersionBlocksStored) {
+        const uint16_t* rows = reinterpret_cast<const uint16_t*>(model);
+        if (!container_directory_ok(offsets, h.n_chunks, h.blob_bytes)) return RB200_E_STREAM;
+        return container_stored_rows_ok(h, rows, offsets, prefix + container_blob_offset(container_layout(h))) ? RB200_OK : RB200_E_STREAM;
+    }
     const bool model_ok = container_per_block(h)
                               ? container_block_models_sum_to(reinterpret_cast<const uint16_t*>(model), h.n_blocks, 1u << h.scale_bits)
                               : container_model_ok(h.coder, h.scale_bits, reinterpret_cast<const uint32_t*>(model));
@@ -177,9 +199,10 @@ void container_write(ContainerHeader h, const void* model, const uint64_t* offse
 {
     h.meta_crc = container_meta_crc(h, model, offsets);
     if (h.flags & RB200_CONTAINER_CRC_BLOB) h.blob_crc = container_crc32(0, blob, h.blob_bytes);
-    const uint64_t dir = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
+    const ContainerHeader l = container_layout(h);
+    const uint64_t dir = container_dir_offset(l), dir_end = container_dir_end(l), boff = container_blob_offset(l);
     std::memcpy(out, &h, sizeof h);
-    std::memcpy(out + sizeof h, model, container_model_bytes(h));
+    std::memcpy(out + sizeof h, model, container_model_bytes(l));
     std::memcpy(out + dir, offsets, dir_end - dir);
     std::memset(out + dir_end, 0, boff - dir_end);
     if (h.blob_bytes) std::memcpy(out + boff, blob, h.blob_bytes);
@@ -192,10 +215,11 @@ int container_open_checked(const uint8_t* buf, size_t size, uint16_t version, Co
     if (rc != RB200_OK) return rc;
     // model and offsets sit at 4- and 8-byte aligned positions when buf itself is 8-byte aligned (callers map or malloc it)
     if (reinterpret_cast<uintptr_t>(buf) & 7) return RB200_E_ARG;
+    const ContainerHeader l = container_layout(*h);
     rc = container_check_prefix(*h, buf, container_meta_crc(*h, buf + sizeof(ContainerHeader),
-                                                            reinterpret_cast<const uint64_t*>(buf + container_dir_offset(*h))));
+                                                            reinterpret_cast<const uint64_t*>(buf + container_dir_offset(l))));
     if (rc == RB200_OK && (h->flags & RB200_CONTAINER_CRC_BLOB))
-        rc = container_check_blob(*h, container_crc32(0, buf + container_blob_offset(*h), h->blob_bytes));
+        rc = container_check_blob(*h, container_crc32(0, buf + container_blob_offset(l), h->blob_bytes));
     return rc;
 }
 
@@ -207,7 +231,7 @@ int container_blocks_pack(const ContainerHeader& h, const uint16_t* block_freqs,
     if (!block_freqs || !offsets || (!blob && h.blob_bytes) || !out || h.n_chunks >= (1ull << 31)) return RB200_E_ARG;
     if (!container_block_models_sum_to(block_freqs, h.n_blocks, 1u << h.scale_bits)) return RB200_E_MODEL;   // never write what open rejects
     if ((h.blob_bytes & 15) || !container_directory_ok(offsets, h.n_chunks, h.blob_bytes)) return RB200_E_ARG;
-    const size_t total = container_blob_offset(h) + h.blob_bytes;
+    const size_t total = container_blob_offset(container_layout(h)) + h.blob_bytes;
     if (total > out_cap) return RB200_E_SPACE;
     container_write(h, block_freqs, offsets, blob, out);
     if (out_size) *out_size = total;
@@ -229,8 +253,8 @@ int container_blocks_open(const uint8_t* buf, size_t size, uint16_t version, Inf
     info->n_chunks = h->n_chunks;
     info->blob_bytes = h->blob_bytes;
     info->block_freqs = reinterpret_cast<const uint16_t*>(buf + sizeof(ContainerHeader));
-    info->offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(*h));
-    info->blob = buf + container_blob_offset(*h);
+    info->offsets = reinterpret_cast<const uint64_t*>(buf + container_dir_offset(container_layout(*h)));
+    info->blob = buf + container_blob_offset(container_layout(*h));
     return RB200_OK;
 }
 
@@ -345,6 +369,41 @@ extern "C" int rb200_container_blocks_alias_pack(uint32_t scale_bits, uint32_t n
 extern "C" int rb200_container_blocks_alias_open(const uint8_t* buf, size_t size, rb200_container_blocks_coder_info* info)
 {
     return container_blocks_coder_open(buf, size, kContainerVersionBlocksAlias, info);
+}
+
+extern "C" size_t rb200_container_blocks_stored_bound(uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms)
+{
+    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return 0;
+    const uint64_t n_chunks = static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms);
+    return container_blob_offset(container_shape(kContainerVersionBlocks, n_blocks, n_chunks)) + n_chunks * container_stored_bytes(chunk_syms);
+}
+
+extern "C" int rb200_container_blocks_stored_pack(int coder, uint32_t scale_bits, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                                                  const uint16_t* block_freqs, const uint64_t* offsets, const uint8_t* blob,
+                                                  size_t blob_bytes, uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size)
+{
+    if (coder < 0 || !blocks_candidate_ok(RB200_CANDIDATE(coder, scale_bits))) return RB200_E_ARG;
+    if (!container_blocks_geometry_ok(n_blocks, block_size, chunk_syms)) return RB200_E_ARG;
+    if (!block_freqs || !offsets || (!blob && blob_bytes) || !out) return RB200_E_ARG;
+    ContainerHeader h = container_blocks_coder_header(container_blocks_version(static_cast<uint32_t>(coder)), coder, scale_bits, n_blocks,
+                                                      block_size, chunk_syms, blob_bytes, flags);
+    h.version = kContainerVersionBlocksStored;
+    if (h.n_chunks >= (1ull << 31)) return RB200_E_ARG;
+    for (uint64_t b = 0; b < n_blocks; b++)                          // never write what open rejects
+        if (!container_block_model_stored(block_freqs + b * 256) && !container_block_model_sums_to(block_freqs + b * 256, 1u << scale_bits))
+            return RB200_E_MODEL;
+    if ((blob_bytes & 15) || !container_directory_ok(offsets, h.n_chunks, blob_bytes) || !container_stored_rows_ok(h, block_freqs, offsets, blob))
+        return RB200_E_ARG;
+    const size_t total = container_blob_offset(container_layout(h)) + blob_bytes;
+    if (total > out_cap) return RB200_E_SPACE;
+    container_write(h, block_freqs, offsets, blob, out);
+    if (out_size) *out_size = total;
+    return RB200_OK;
+}
+
+extern "C" int rb200_container_blocks_stored_open(const uint8_t* buf, size_t size, rb200_container_blocks_coder_info* info)
+{
+    return container_blocks_coder_open(buf, size, kContainerVersionBlocksStored, info);
 }
 
 extern "C" int rb200_choose_coder(const uint64_t counts[256], size_t n, uint32_t chunk_syms, const uint32_t* candidates,

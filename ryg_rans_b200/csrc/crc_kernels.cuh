@@ -358,4 +358,14 @@ __global__ void __launch_bounds__(32)
     container_finish<false, true>(out, h, dir_off, blob_off, out_cap, nullptr, slots, status, nullptr, &r->choice);
 }
 
+// The header kernel of rb200_container_blocks_stored_encode_async: container_blocks_finish_kernel's with version 5 (coder
+// and scale_bits from the record)
+__global__ void __launch_bounds__(32)
+    container_blocks_stored_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
+                                          const CrcSlot* __restrict__ slots, uint32_t* status, const BlocksChoice* __restrict__ r)
+{
+    h.version = kContainerVersionBlocksStored;
+    container_finish<false, true>(out, h, dir_off, blob_off, out_cap, nullptr, slots, status, nullptr, &r->choice);
+}
+
 }  // namespace rb200

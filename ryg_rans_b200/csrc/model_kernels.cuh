@@ -35,6 +35,10 @@
 // blocks_varlen_plan_kernel reads *d_n_blocks into BlocksVarlenGeom (device_utils.cuh), and the choice kernel, the
 // encoders, the scan and compaction, the blob length and the header kernel are the GEOM instances of the same kernels,
 // which take the count, the directory's place (after the count's models) and the blob's from it.
+//
+// rb200_container_blocks_stored_encode_async (version 5) runs the choice kernel (blocks_one_pair_kernel for one
+// candidate) and one GATED split encoder per group into one workspace, then blocks_store_kernel, which stores every
+// block whose coded chunks take more blob than its symbols, and one ungated scan and compact_stored_kernel.
 #pragma once
 #include "block_kernels.cuh"
 #include "container_format.h"
@@ -268,6 +272,42 @@ __global__ void __launch_bounds__(kBlocksChoiceWarps * 32)
         r->choice.group = list.group[i];
         r->version = container_blocks_version(r->choice.coder);
     }
+}
+
+// rb200_container_blocks_stored_encode_async with one candidate, one thread: the choice record of that pair as group 0,
+// which the gated encoders and the header kernel read (no choice kernel runs; its costs are left as they are)
+__global__ void __launch_bounds__(32) blocks_one_pair_kernel(uint32_t pair, BlocksChoice* __restrict__ r)
+{
+    if (threadIdx.x) return;
+    r->choice.coder = pair >> 8;
+    r->choice.scale_bits = pair & 0xffu;
+    r->choice.index = 0;
+    r->choice.group = 0;
+    r->version = container_blocks_version(r->choice.coder);
+}
+
+// The store rule of rb200_container_blocks_stored_encode_async, one warp per block, after the encoder wrote every chunk's
+// stream size to sizes[]: the blob bytes of the block's chunks (each stream rounded up to 16, as the compaction places
+// it) against per_block x round16(chunk_syms), its size stored.  Above that the block is stored: its model row in the
+// container is zeroed, every chunk's size becomes round16(chunk_syms), and stored[block] = 1 has the compaction copy
+// the chunk's symbols in place of its stream; otherwise stored[block] = 0.  Stream sizes stay below 2^26 (a slot), so
+// a block's sum fits 32 bits.
+constexpr int kStoreWarps = 8;
+
+__global__ void __launch_bounds__(kStoreWarps * 32)
+    blocks_store_kernel(uint32_t* __restrict__ sizes, uint32_t n_blocks, uint32_t per_block, uint32_t chunk_syms, uint16_t* __restrict__ models,
+                        uint32_t* __restrict__ stored)
+{
+    const uint32_t lane = threadIdx.x & 31, block = blockIdx.x * kStoreWarps + (threadIdx.x >> 5);
+    if (block >= n_blocks) return;                               // the same for the whole warp
+    const uint32_t raw = static_cast<uint32_t>(container_stored_bytes(chunk_syms));
+    uint32_t* s = sizes + static_cast<uint64_t>(block) * per_block;
+    const uint32_t coded = __reduce_add_sync(0xffffffffu, lane < per_block ? (s[lane] + 15u) & ~15u : 0u);
+    const bool store = coded > per_block * raw;
+    if (lane == 0) stored[block] = store;
+    if (!store) return;
+    if (lane < per_block) s[lane] = raw;
+    reinterpret_cast<uint4*>(models + static_cast<uint64_t>(block) * 256)[lane] = make_uint4(0, 0, 0, 0);   // 32 x 16 bytes
 }
 
 // The first kernel of rb200_container_model_encode_varlen_async, one warp: reads n = *d_n, checks 1 <= n <= n_max

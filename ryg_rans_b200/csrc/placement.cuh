@@ -71,6 +71,26 @@ __device__ __forceinline__ void place_stream(const uint8_t* src_end, uint32_t si
     for (; v < nvec; v += 32) stg_stream_u128(d4 + v, ld(s4 + v));
 }
 
+// A stored chunk (rb200_container_blocks_stored_encode_async): its m symbols at src, then zero bytes up to a multiple of
+// 16, to dst (16-byte aligned), one warp.  Whole 16-byte loads where src and m allow them, bytes otherwise.
+__device__ __forceinline__ void place_stored(const uint8_t* __restrict__ src, uint32_t m, uint8_t* __restrict__ dst, uint32_t lane)
+{
+    const bool vec = ((reinterpret_cast<uintptr_t>(src) | m) & 15) == 0;
+    for (uint32_t v = lane; v < (m + 15) / 16; v += 32) {
+        uint4 q;
+        if (vec) {
+            q = ldg_stream_u128(reinterpret_cast<const uint4*>(src) + v);
+        } else {
+            uint32_t w[4] = {0, 0, 0, 0};
+#pragma unroll
+            for (uint32_t j = 0; j < 16; j++)
+                if (16 * v + j < m) w[j >> 2] |= static_cast<uint32_t>(src[16 * v + j]) << (8 * (j & 3));
+            q = make_uint4(w[0], w[1], w[2], w[3]);
+        }
+        stg_stream_u128(reinterpret_cast<uint4*>(dst) + v, q);
+    }
+}
+
 // The scanner: ONE warp of the grid walks the status array in chunk order and rewrites every published
 // size (kLookAgg | padded size) into the inclusive end offset E_c (kLookPrefix | E_c).  Chunks are handed
 // out in order, so the entry it waits for always belongs to a chunk some resident warp is encoding.

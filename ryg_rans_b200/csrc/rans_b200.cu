@@ -66,7 +66,7 @@ struct rb200_ctx {
     CrcSlot* h_crc = nullptr;
     // the async container decodes (container_decode.cuh): one fixed workspace per version, so that calls of different
     // versions never share state, and every version's decoder launches
-    ContainerAsyncWork* d_async[4] = {};
+    ContainerAsyncWork* d_async[5] = {};
     DecoderLaunch async_decoders[kContainerDecoders] = {};
     // rb200_container_blocks_any_decode_async: its own workspace, for its checks and the decoders of versions 2-4
     ContainerAsyncWork* d_async_any = nullptr;
@@ -458,9 +458,11 @@ namespace {
 
 // directory + compaction after any encode kernel: sizes[] -> offsets[] + blob.  geom set: the GEOM instances, on grids
 // sized for n_chunks (the bound's), with d_blob the container, in which they find the directory and the blob from the
-// record (d_offsets unused).  choice set: the GATED instances, which run only when the record names `group`.
+// record (d_offsets unused).  choice set: the GATED instances, which run only when the record names `group`.  stored
+// set (the stored encode, ungated): compact_stored_kernel, which copies the stored blocks' chunks from the input.
 int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* sizes, uint64_t* tile_sums, uint32_t n_chunks,
-                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom, const CoderChoice* choice, uint32_t group)
+                  uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom, const CoderChoice* choice, uint32_t group,
+                  const StoredBlocks* stored = nullptr)
 {
     if (!n_chunks) {
         RB_CUDA(ctx, cudaMemsetAsync(d_offsets, 0, sizeof(uint64_t), ctx->stream));
@@ -482,6 +484,11 @@ int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* siz
         if (rc != RB200_OK) return rc;
     }
     const uint32_t grid = (n_chunks + kCopyWarps - 1) / kCopyWarps;
+    if (stored) {
+        compact_stored_kernel<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, d_offsets, tile_sums, prefixed, n_chunks, d_blob,
+                                                                         blob_cap, ctx->d_status, *stored);
+        return check_launch(ctx, "compact_stored_kernel");
+    }
     auto compact = choice ? (geom ? compact_kernel<true, true> : compact_kernel<false, true>)
                           : (geom ? compact_kernel<true> : compact_kernel<false>);
     compact<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, d_offsets, tile_sums, prefixed, n_chunks, d_blob, blob_cap,
@@ -1859,12 +1866,14 @@ int container_decode_async(rb200_ctx* ctx, uint16_t version, const uint8_t* buf,
     DeviceGuard g(ctx->device);
     const bool any = version == kContainerVersionAnyBlocks;
     ContainerAsyncWork* w = any ? ctx->d_async_any : ctx->d_async[version - 1];
+    const bool stored = version == kContainerVersionBlocksStored;
     const int first = kDecoderFirst[any ? kContainerVersionBlocks - 1 : version - 1];
     const int last = kDecoderFirst[any ? kContainerVersionBlocksAlias : version];
     const uint32_t sms = static_cast<uint32_t>(ctx->sms);
     const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
     cudaStream_t s = ctx->stream;
-    container_plan_kernel<<<1, 32, 0, s>>>(buf, size, version, w);
+    auto plan = stored ? container_plan_kernel<true> : container_plan_kernel<false>;
+    plan<<<1, 32, 0, s>>>(buf, size, version, w);
     int rc = check_launch(ctx, "container_plan_kernel");
     if (rc != RB200_OK) return rc;
     crc32_kernel<<<crc32_grid(sms, after_head), kCrcThreads, kCrcSmemBytes, s>>>(buf + sizeof(ContainerHeader), after_head, &w->plan.meta_len,
@@ -1875,7 +1884,8 @@ int container_decode_async(rb200_ctx* ctx, uint16_t version, const uint8_t* buf,
                                                                            &w->crc_work, &w->crc[1]);
     rc = check_launch(ctx, "crc32_kernel(blob)");
     if (rc != RB200_OK) return rc;
-    container_prefix_check_kernel<<<sms * kPrefixCtasPerSm, kPrefixWarps * 32, 0, s>>>(buf, w);
+    auto prefix = stored ? container_prefix_check_kernel<true> : container_prefix_check_kernel<false>;
+    prefix<<<sms * kPrefixCtasPerSm, kPrefixWarps * 32, 0, s>>>(buf, w);
     rc = check_launch(ctx, "container_prefix_check_kernel");
     if (rc != RB200_OK) return rc;
     if (version == kContainerVersion) {
@@ -1925,6 +1935,14 @@ extern "C" int rb200_container_blocks_alias_decode_async(rb200_ctx* ctx, const u
 {
     if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
     return container_decode_async(ctx, kContainerVersionBlocksAlias, buf, size, out, out_cap, d_n_symbols);
+}
+
+// Thirteen launches: the checks and the STORED block decoder variants of RB200_BLOCK_DISPATCH (version 5).
+extern "C" int rb200_container_blocks_stored_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                                          uint64_t* d_n_symbols)
+{
+    if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    return container_decode_async(ctx, kContainerVersionBlocksStored, buf, size, out, out_cap, d_n_symbols);
 }
 
 // Thirteen launches: the checks and every block decoder variant of RB200_BLOCK_DISPATCH (versions 2, 3 and 4).
@@ -2096,6 +2114,81 @@ extern "C" int rb200_container_blocks_model_encode_varlen_async(rb200_ctx* ctx, 
     const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
     return blocks_container_encode(ctx, container_blocks_header(n_blocks_max, block_size, chunk_syms, 0, flags), in, nullptr, d_n_blocks,
                                    out, out_cap, &a);
+}
+
+namespace {
+
+// rb200_container_blocks_stored_encode_async: the choice kernel (after a memset of its sums) or, for one candidate,
+// blocks_one_pair_kernel; one GATED split encoder per launch group of the list, all into one workspace of one
+// worst-case slot per chunk (slot_bytes_for does not depend on the coder), so that every stream's size is known before
+// anything is placed; blocks_store_kernel; the scan, the tile prefix and compact_stored_kernel, ungated; the model +
+// directory CRC, the optional blob CRC and container_blocks_stored_finish_kernel (version 5).  The workspace: the split plan's, then the
+// per-block verdicts after its tile sums.  Arguments are checked by the caller.
+int blocks_stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
+                         uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    const ContainerHeader h = container_blocks_header(n_blocks, block_size, chunk_syms, 0, flags);
+    const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
+    if (out_cap < boff) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    cudaStream_t s = ctx->stream;
+    BlocksChoice* r = ctx->d_blocks_choice;
+    const uint32_t per_block = block_size / chunk_syms, n_chunks = static_cast<uint32_t>(h.n_chunks);
+    EncodePlan p = {};
+    p.n_chunks = n_chunks;
+    p.slots = n_chunks;
+    p.slot_bytes = slot_bytes_for(chunk_syms);
+    p.threads = block_threads(block_size, chunk_syms);
+    const size_t longs = (n_chunks + kScanTile - 1) / kScanTile + 1;
+    int rc = reserve(ctx, ctx->scratch, p.slots * p.slot_bytes + 16);
+    if (rc == RB200_OK) rc = reserve(ctx, ctx->sizes, plan_head_bytes(p) + longs * sizeof(uint64_t) + n_blocks * sizeof(uint32_t));
+    if (rc != RB200_OK) return rc;
+    uint8_t* scratch = static_cast<uint8_t*>(ctx->scratch.p);
+    uint32_t* sizes = static_cast<uint32_t*>(ctx->sizes.p);
+    uint64_t* tile_sums = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + plan_head_bytes(p));
+    uint32_t* stored = reinterpret_cast<uint32_t*>(tile_sums + longs);
+    uint16_t* model = reinterpret_cast<uint16_t*>(out + sizeof(ContainerHeader));
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
+    if (a.list.n == 1) {
+        blocks_one_pair_kernel<<<1, 32, 0, s>>>(a.list.pair[0], r);
+        rc = check_launch(ctx, "blocks_one_pair_kernel");
+    } else {
+        RB_CUDA(ctx, cudaMemsetAsync(&r->done, 0, sizeof(BlocksChoice) - offsetof(BlocksChoice, done), s));
+        blocks_choice_kernel<false><<<n_blocks, kBlocksChoiceWarps * 32, 0, s>>>(a.list, in, block_size, chunk_syms, r, ctx->d_status, nullptr);
+        rc = check_launch(ctx, "blocks_choice_kernel");
+    }
+    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++) {
+        launch_block_encode(s, static_cast<uint32_t>(a.coder[k]), a.sb[k], true, n_blocks, p.threads,
+                            block_coder_encode_smem(static_cast<uint32_t>(a.coder[k]), a.sb[k], p.threads), in, block_size, model, chunk_syms,
+                            scratch, p.slot_bytes, sizes, ctx->d_status, &r->choice, k);
+        rc = check_launch(ctx, "block_coder_encode_kernel");
+    }
+    if (rc != RB200_OK) return rc;
+    blocks_store_kernel<<<(n_blocks + kStoreWarps - 1) / kStoreWarps, kStoreWarps * 32, 0, s>>>(sizes, n_blocks, per_block, chunk_syms, model,
+                                                                                                stored);
+    rc = check_launch(ctx, "blocks_store_kernel");
+    const StoredBlocks st = {in, stored, per_block, chunk_syms};
+    if (rc == RB200_OK)
+        rc = finish_encode(ctx, scratch, p.slot_bytes, sizes, tile_sums, n_chunks, out + boff, out_cap - boff, dir, nullptr, nullptr, 0, &st);
+    if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), nullptr, 0, ctx->d_crc);
+    if (rc == RB200_OK && (flags & RB200_CONTAINER_CRC_BLOB)) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+    if (rc != RB200_OK) return rc;
+    container_blocks_stored_finish_kernel<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, ctx->d_crc, ctx->d_status, r);
+    return check_launch(ctx, "container_blocks_stored_finish_kernel");
+}
+
+}  // namespace
+
+// The auto encode's choice and model-building encoders, with every block whose coded chunks would take more than its
+// stored size stored verbatim (version 5).  Eight to eleven launches and one memset, no copy, no synchronisation.
+extern "C" int rb200_container_blocks_stored_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                          uint32_t tolerance_ppm, const uint8_t* in, uint32_t n_blocks, uint32_t block_size,
+                                                          uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    if (!blocks_candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    if (!blocks_container_args_ok(ctx, in, n_blocks, block_size, chunk_syms, out, RB200_MEM_DEVICE)) return RB200_E_ARG;
+    return blocks_stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n_blocks, block_size, chunk_syms, flags, out,
+                                out_cap);
 }
 
 extern "C" int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n)

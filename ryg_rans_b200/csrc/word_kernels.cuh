@@ -599,12 +599,23 @@ tile_prefix_kernel(uint64_t* __restrict__ tile_sums, uint32_t n_tiles, const Var
 constexpr int kCopyWarps = 8;
 constexpr uint32_t kTilePrefixThreshold = 256;   // above this many tiles, tile_prefix_kernel runs first
 
+// The blocks rb200_container_blocks_stored_encode_async stores: the input, chunks of chunk_syms symbols, per_block to a
+// block, and blocks_store_kernel's verdict per block (nonzero: stored).
+struct StoredBlocks {
+    const uint8_t* in;
+    const uint32_t* stored;
+    uint32_t per_block, chunk_syms;
+};
+
 // one warp moves one chunk stream from the end of its scratch slot to blob[offsets[c]..E_c)
-template <bool GEOM, bool GATED>
+// STORED (rb200_container_blocks_stored_encode_async): a chunk of a stored block is its symbols from the input instead,
+// with zero padding (place_stored); its size is already round16(chunk_syms)
+template <bool GEOM, bool GATED, bool STORED = false>
 __device__ __forceinline__ void compact(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
                                         uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
                                         uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status,
-                                        const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
+                                        const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group,
+                                        const StoredBlocks& st = StoredBlocks{})
 {
     if (GATED && choice->group != group) return;
     if (GEOM) {
@@ -642,7 +653,12 @@ __device__ __forceinline__ void compact(const uint8_t* __restrict__ scratch, uin
             if (end > blob_cap) atomicOr(status, kStatSpace);
         }
     }
-    if (end <= blob_cap) place_stream<false>(scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, size, blob, end, lane);
+    if (end <= blob_cap) {
+        if (STORED && st.stored[chunk / st.per_block])
+            place_stored(st.in + static_cast<uint64_t>(chunk) * st.chunk_syms, st.chunk_syms, blob + (end - size), lane);
+        else
+            place_stream<false>(scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, size, blob, end, lane);
+    }
 }
 
 template <bool GEOM = false, bool GATED = false>
@@ -653,6 +669,16 @@ compact_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const u
                const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice, uint32_t group)
 {
     compact<GEOM, GATED>(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, blob, blob_cap, status, geom, choice, group);
+}
+
+// the STORED compaction of rb200_container_blocks_stored_encode_async (ungated, every length by value)
+__global__ void __launch_bounds__(kCopyWarps * 32)
+compact_stored_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+                      uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
+                      uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status, StoredBlocks st)
+{
+    compact<false, false, true>(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, blob, blob_cap, status, nullptr,
+                                nullptr, 0, st);
 }
 
 // the K2 and K2f instances: (R32, GATED, GEOM) = (r32, 0, 0) for an rb200_model, (r32, 1, 0) and (r32, 1, 1) for the

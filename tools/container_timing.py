@@ -72,10 +72,16 @@ With --blocks-varlen, rb200_container_blocks_model_encode_varlen_async on the --
 auto call at 1024 blocks, and with the chosen pair as its one candidate against the fixed model-building container call
 of that pair; a torch.profiler list of the varlen calls' kernels and their fixed twins'.
 
+With --blocks-stored, rb200_container_blocks_stored_encode_async (version 5, incompressible blocks stored) over the
+--blocks-auto candidates against rb200_container_blocks_model_encode_auto_async on uniform, Zipf, skewed and half-uniform
+/ half-Zipf blocks, flags 0, alternated: bytes per symbol of both containers, encode times, and
+rb200_container_blocks_stored_decode_async against rb200_container_blocks_any_decode_async on the auto container; a
+torch.profiler list of the version 5 calls' kernels.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
     python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto | --blocks-auto
-                                      | --blocks-varlen] [--reps 10]
+                                      | --blocks-varlen | --blocks-stored] [--reps 10]
                                      [--json out.json]"""
 import argparse
 import json
@@ -916,6 +922,79 @@ def blocks_varlen(args):
     return res
 
 
+def blocks_stored(args):
+    """rb200_container_blocks_stored_encode_async (version 5) over {word 12, byte 14, alias 14} (2 % tolerance) against
+    rb200_container_blocks_model_encode_auto_async, on uniform, Zipf, skewed and half-uniform / half-Zipf blocks: bytes
+    per symbol of both containers, encode times, the version 5 decode against rb200_container_blocks_any_decode_async on
+    the auto container, and a kernel split of both version 5 calls"""
+    import torch
+    n_blocks, block_size, chunk, tol = 8192, 65536, 8192, 20000
+    n = n_blocks * block_size
+    W, B, A = rb.CODER_WORD, rb.CODER_BYTE, rb.CODER_ALIAS
+    cands = [api.CANDIDATE(W, 12), api.CANDIDATE(B, 14), api.CANDIDATE(A, 14)]
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    cap = ctx.container_blocks_capacity(n_blocks, block_size, chunk)
+    bound = api.container_blocks_stored_bound(n_blocks, block_size, chunk)
+    d_auto = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_st = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+    d_dec = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+    res = {"card": card(), "workload": {"n_blocks": n_blocks, "block_size": block_size, "chunk_syms": chunk, "n": n},
+           "candidates": ["word 12", "byte 14", "alias 14"], "tolerance_ppm": tol, "bound_bytes_per_symbol": bound / n,
+           "workloads": {}, "checks": {}}
+
+    def size(d):
+        h = d[:64].cpu().numpy()
+        return ((64 + 512 * n_blocks + 8 * (n // chunk + 1) + 15) & ~15) + int(h[32:40].view(np.uint64)[0]), int(h[6]), int(h[7])
+
+    def uniform(nb, bs, seed):
+        g = torch.Generator(device="cuda")
+        g.manual_seed(seed)
+        return torch.randint(0, 256, (nb * bs,), dtype=torch.uint8, device="cuda", generator=g)
+
+    def half(nb, bs, seed):
+        d = blocks_data(nb, bs, seed).view(nb, bs)
+        d[0::2] = uniform(nb // 2, bs, seed + 1).view(nb // 2, bs)
+        return d.reshape(-1)
+
+    for name, make in (("uniform", uniform), ("zipf", blocks_data), ("skewed", skewed_blocks_data), ("half_uniform_zipf", half)):
+        d_in = make(n_blocks, block_size, 4321)
+        i, a, o = d_in.data_ptr(), d_auto.data_ptr(), d_st.data_ptr()
+        enc = {"stored_encode": lambda: ctx.container_blocks_stored_encode_async(cands, tol, i, n_blocks, block_size, chunk, 0, o, bound),
+               "auto_encode": lambda: ctx.container_blocks_model_encode_auto_async(cands, tol, i, n_blocks, block_size, chunk, 0, a, cap)}
+        times = alternate(enc, sync, args.warmup, args.reps)
+        for f in enc.values():
+            f()
+        sync()
+        st_size, coder, sb = size(d_st)
+        auto_size = size(d_auto)[0]
+        rows = d_st[64:64 + 512 * n_blocks].view(torch.int16).view(n_blocks, 256)
+        stored = int((rows == 0).all(dim=1).sum().item())
+        res["checks"][f"{name}: stored_container_within_bound"] = st_size <= bound
+        dec = {"stored_decode_async": lambda: ctx.container_blocks_stored_decode_async(o, bound, d_dec.data_ptr(), n),
+               "any_decode_async_on_auto": lambda: ctx.container_blocks_any_decode_async(a, cap, d_dec.data_ptr(), n)}
+        dtimes = alternate(dec, sync, args.warmup, args.reps)
+        for k, f in dec.items():
+            d_dec.zero_()
+            f()
+            sync()
+            res["checks"][f"{name}: {k}_round_trip"] = bool(torch.equal(d_dec[:n], d_in[:n]))
+        res["workloads"][name] = {
+            "chosen": {"coder": coder, "scale_bits": sb}, "stored_blocks": stored,
+            "bytes_per_symbol": {"stored": st_size / n, "auto": auto_size / n},
+            "encode": times, "stored_minus_auto_encode_median_us": 1e3 * (times["stored_encode"]["median_ms"] - times["auto_encode"]["median_ms"]),
+            "decode": dtimes,
+            "stored_minus_any_decode_median_us": 1e3 * (dtimes["stored_decode_async"]["median_ms"] - dtimes["any_decode_async_on_auto"]["median_ms"]),
+            "stored_encode_kernels": kernel_times(enc["stored_encode"], sync, args.reps),
+            "auto_encode_kernels": kernel_times(enc["auto_encode"], sync, args.reps),
+            "stored_decode_kernels": kernel_times(dec["stored_decode_async"], sync, args.reps),
+            "any_decode_kernels": kernel_times(dec["any_decode_async_on_auto"], sync, args.reps),
+        }
+        del d_in
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
@@ -926,13 +1005,14 @@ def main():
     ap.add_argument("--auto", action="store_true", help="the model-building encode with the coder chosen on the GPU")
     ap.add_argument("--blocks-auto", action="store_true", help="the per-block model-building encode with the coder chosen on the GPU")
     ap.add_argument("--blocks-varlen", action="store_true", help="the per-block auto encode with the block count in device memory")
+    ap.add_argument("--blocks-stored", action="store_true", help="the per-block encode and decode with incompressible blocks stored (version 5)")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
