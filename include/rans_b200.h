@@ -387,6 +387,49 @@ int rb200_container_blocks_stored_encode_async(rb200_ctx* ctx, const uint32_t* c
 int rb200_container_blocks_stored_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                                uint64_t* d_n_symbols);
 
+/* ---------------------------------------------------------------- single-model containers with stored chunks */
+
+/* Version 6: version 1's header (version field 6; block_size, n_blocks and reserved zero, which is checked), model and
+ * directory at 1088, then from the next 16-byte boundary a stored-chunk bitmap, ceil(n_chunks / 32) u32 words with bit
+ * c % 32 of word c / 32 set when chunk c is stored, zero-padded to 16 bytes, then the blob.  Bits at or past n_chunks
+ * and the padding are zero.  meta_crc covers every byte before the blob: header (crc fields zero), model, directory,
+ * the zero pad after it and the bitmap.  A stored chunk of m_c symbols (chunk_syms, or fewer for a ragged last chunk)
+ * is a stream of round16(m_c) bytes, its symbols and then zero bytes, placed by the rules of a coded stream of that
+ * length: its directory step, (offsets[c + 1] & ~15) - offsets[c], is exactly round16(m_c).  The model is always
+ * present and valid, even when every chunk is stored.  Only the _stored_ calls below accept version 6; every other
+ * container call rejects it (RB200_E_STREAM), and they reject versions 1-5.
+ *   bound: the blob offset + the sum of round16(m_c): the most any version 6 container of n symbols takes (0 for n == 0,
+ *          n >= 2^32 or chunk_syms outside 32 .. 2^24).
+ *   pack:  host only; stored_bits holds ceil(n_chunks / 32) words.  RB200_E_ARG for a bad pair (as
+ *          rb200_container_model_encode_async takes it) or length, a null pointer, a bit at or past n_chunks, and a
+ *          directory that disagrees with the blob or gives a stored chunk the wrong step or nonzero padding;
+ *          RB200_E_MODEL for a model that does not sum to 1 << scale_bits; RB200_E_SPACE when out_cap is below the
+ *          container.
+ *   open:  as rb200_container_open, with the rules above; *stored_bits points at the bitmap in buf. */
+struct rb200_container_info;   /* defined with rb200_container_open below */
+size_t rb200_container_stored_bound(size_t n, uint32_t chunk_syms);
+int rb200_container_stored_pack(int coder, uint32_t scale_bits, uint32_t chunk_syms, size_t n, const uint32_t freqs[256],
+                                const uint32_t* stored_bits, const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes,
+                                uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size);
+int rb200_container_stored_open(const uint8_t* buf, size_t size, struct rb200_container_info* info, const uint32_t** stored_bits);
+/* A version 6 container of n symbols at `in`, DEVICE memory, enqueued only: the pair is the choice of
+ * rb200_container_model_encode_auto_async (d_n NULL) over `candidates`, every chunk is encoded with it, and then chunk c
+ * is stored when its stream, rounded up to 16, is longer than round16(m_c).  The decision is made from the streams the
+ * encoder wrote, so out_cap >= rb200_container_stored_bound(n, chunk_syms) always suffices.  Arguments and verdicts are
+ * those of rb200_container_model_encode_auto_async with d_n NULL: RB200_E_ARG (nothing launched), RB200_E_MODEL for
+ * n == 0, RB200_E_SPACE when out_cap is below the blob offset; rb200_sync returns RB200_E_MODEL when no candidate is
+ * feasible and RB200_E_SPACE when the blob does not fit out_cap, header unwritten.  Capturable in a CUDA graph after one
+ * call with the same list and geometry outside the capture. */
+int rb200_container_stored_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                        const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap);
+/* The contract of rb200_container_decode_async with version 6 in place of version 1: kernels check the header, the
+ * model, the directory, the bitmap, every stored chunk's step and padding, meta_crc and the optional blob CRC; then the
+ * decoder of the header's coder runs, copying stored chunks and decoding the others.  rb200_sync gives RB200_E_STREAM
+ * for anything rb200_container_stored_open rejects (versions 1-5 among them) or the decoders refuse, RB200_E_SPACE for
+ * n > out_cap, content errors first; in both cases out is untouched. */
+int rb200_container_stored_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                        uint64_t* d_n_symbols);
+
 /* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
  * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's
  * decode table is built on the GPU into the context, and the decoder the header calls for is picked on the GPU -- all

@@ -103,6 +103,13 @@ EXPORTS = [
     ("rb200_container_blocks_stored_encode_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
                                                              C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_container_blocks_stored_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_container_stored_bound", C.c_size_t, [C.c_size_t, C.c_uint32]),
+    ("rb200_container_stored_pack", C.c_int, [C.c_int, C.c_uint32, C.c_uint32, C.c_size_t, _u32p, _u32p, C.c_void_p, C.c_void_p,
+                                              C.c_size_t, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("rb200_container_stored_open", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(_u32p)]),
+    ("rb200_container_stored_encode_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_uint32,
+                                                      C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_container_stored_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -193,6 +200,51 @@ def container_open(buf):
     blob = buf[b_off:b_off + info.blob_bytes]
     meta = {k: int(getattr(info, k)) for k in ("coder", "scale_bits", "chunk_syms", "flags", "n_symbols", "n_chunks", "blob_bytes")}
     return meta, freqs, offsets, blob
+
+
+def container_stored_bound(n, chunk_syms):
+    """rb200_container_stored_bound: the most bytes a version 6 container of n symbols takes (0 for a length or chunk size
+    the calls refuse)"""
+    return int(load().dll.rb200_container_stored_bound(n, chunk_syms))
+
+
+def container_stored_pack(coder, scale_bits, chunk_syms, n, freqs, stored_bits, offsets, blob, flags=0):
+    """rb200_container_stored_pack: a version 6 container (one model; bit c of stored_bits, ceil(n_chunks / 32) u32 words,
+    marks chunk c stored, its stream round16(m_c) bytes of its symbols and zero padding)"""
+    lib = load()
+    freqs = np.ascontiguousarray(freqs, dtype=np.uint32)
+    bits = np.ascontiguousarray(stored_bits, dtype=np.uint32)
+    offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+    blob = np.ascontiguousarray(blob, dtype=np.uint8)
+    n_chunks = offsets.size - 1
+    bitmap = (1088 + 8 * (n_chunks + 1) + 15) // 16 * 16                  # the layout of include/rans_b200.h
+    out = np.zeros(bitmap + 16 * ((n_chunks + 127) // 128) + blob.size, np.uint8)
+    size = C.c_size_t(0)
+    lib.check(lib.dll.rb200_container_stored_pack(coder, scale_bits, chunk_syms, n, freqs.ctypes.data_as(_u32p), bits.ctypes.data_as(_u32p),
+                                                  offsets.ctypes.data, blob.ctypes.data, blob.size, flags, out.ctypes.data, out.size,
+                                                  C.byref(size)))
+    return out[:size.value].copy()
+
+
+def container_stored_open(buf):
+    """Returns (info dict, freqs, stored_bits, offsets, blob) as numpy views into buf (stored_bits: ceil(n_chunks / 32)
+    u32 words)."""
+    lib = load()
+    buf = np.ascontiguousarray(buf, dtype=np.uint8)
+    info = ContainerInfo()
+    bits_p = _u32p()
+    lib.check(lib.dll.rb200_container_stored_open(buf.ctypes.data, buf.size, C.byref(info), C.byref(bits_p)))
+    base = buf.ctypes.data
+    f_off = C.addressof(info.freqs.contents) - base
+    o_off = C.addressof(info.offsets.contents) - base
+    s_off = C.addressof(bits_p.contents) - base
+    b_off = (C.addressof(info.blob.contents) - base) if info.blob_bytes else buf.size
+    freqs = buf[f_off:f_off + 1024].view(np.uint32)
+    offsets = buf[o_off:o_off + 8 * (info.n_chunks + 1)].view(np.uint64)
+    bits = buf[s_off:s_off + 4 * ((info.n_chunks + 31) // 32)].view(np.uint32)
+    blob = buf[b_off:b_off + info.blob_bytes]
+    meta = {k: int(getattr(info, k)) for k in ("coder", "scale_bits", "chunk_syms", "flags", "n_symbols", "n_chunks", "blob_bytes")}
+    return meta, freqs, bits, offsets, blob
 
 
 class ContainerBlocksInfo(C.Structure):
@@ -561,6 +613,19 @@ class Context:
         self.lib.check(self.lib.dll.rb200_container_model_encode_auto_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
                                                                             in_ptr, n_ptr or None, n, chunk_syms, flags, out_ptr, out_cap),
                        self.h)
+
+    def container_stored_encode_async(self, candidates, tolerance_ppm, in_ptr, n, chunk_syms, flags, out_ptr, out_cap):
+        """container_model_encode_auto_async's choice, model and (split) encoders, then every chunk whose stream is
+        longer than its symbols is stored: a version 6 container of at most container_stored_bound bytes.  The verdict
+        (-2 when no candidate is feasible, -3 when the blob does not fit, header unwritten) comes from sync()"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_stored_encode_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
+                                                                        in_ptr, n, chunk_syms, flags, out_ptr, out_cap), self.h)
+
+    def container_stored_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
+        """the async decode of a version 6 container; enqueue only (CUDA-graph capturable).  The verdict (-4 corrupt or
+        another version, -3 out_cap too small, output untouched) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_stored_decode_async(self.h, buf_ptr, size, out_ptr, out_cap, n_ptr or None), self.h)
 
     # ---- per-block containers (version 2): every block's model, the directory and the blob in one buffer
     def container_blocks_capacity(self, n_blocks, block_size, chunk_syms):

@@ -31,6 +31,10 @@
 // header names (kContainerVersionAnyBlocks), then the decoders of versions 2, 3 and 4: their ids are unique across
 // those versions.
 //
+// rb200_container_stored_decode_async (version 6) runs container_stored_plan_kernel and container_stored_check_kernel
+// (the bitmap, stored chunks' steps and padding) in place of the plan and prefix check, the CRCs, the table kernel and
+// the verdict of version 1, then the STORED instances of the eleven version 1 decoders, with version 1's ids.
+//
 // rb200_container_blocks_stored_decode_async (version 5) runs the STORED instances of the plan (version 5 planned as
 // its twin version), of the prefix check (zero rows, stored chunks' steps and padding) and of the eight per-block
 // decoders, which copy a stored block's chunks and decode every other block as versions 2-4 do, with the same ids.
@@ -207,6 +211,64 @@ __global__ void __launch_bounds__(kPrefixWarps * 32)
     if (!ok) w->bad = 1;
 }
 
+// Version 6 (rb200_container_stored_decode_async), one warp: container_plan_kernel's plan and cleared words for a header
+// that passes container_chunks_stored_header_ok, with the blob after the bitmap and meta_len up to it
+// (container_bitmap_blob_offset); a zero plan otherwise.
+__global__ void __launch_bounds__(32)
+    container_stored_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, ContainerAsyncWork* w)
+{
+    if (threadIdx.x) return;
+    BlocksPlan p = {};
+    uint32_t coder = 0, scale_bits = 0;
+    if (size >= sizeof(ContainerHeader)) {                           // a shorter buffer is not read at all
+        const ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(buf);
+        if (container_chunks_stored_header_ok(h, size)) {
+            p.ok = 1;
+            p.n_symbols = h.n_symbols;
+            p.n_chunks = h.n_chunks;
+            p.dir_off = kContainerDirOffset;
+            p.blob_off = container_bitmap_blob_offset(h.n_chunks);
+            p.blob_bytes = h.blob_bytes;
+            p.meta_len = p.blob_off - sizeof(ContainerHeader);
+            p.blob_len = (h.flags & RB200_CONTAINER_CRC_BLOB) ? h.blob_bytes : 0;
+            p.chunk_syms = h.chunk_syms;
+            coder = h.coder;
+            scale_bits = h.scale_bits;
+        }
+    }
+    w->plan = p;
+    w->bad = 0;
+    w->go = 0;
+    w->next_block = 0;
+    w->ctas_done = 0;
+    w->coder = coder;
+    w->scale_bits = scale_bits;
+    w->wide = 0;
+    w->refused = 0;
+    w->work = DecodeWork{0, 0};
+}
+
+// Version 6's per-element rules, a thread per chunk and per bitmap word (grid-stride): container_v6_chunk_ok (the
+// directory step; a stored chunk's step and padding, read only inside the blob), container_bitmap_word_ok on every word
+// of the bitmap and its padding, container_dir_ends_ok once.
+__global__ void __launch_bounds__(kPrefixWarps * 32)
+    container_stored_check_kernel(const uint8_t* __restrict__ buf, ContainerAsyncWork* w)
+{
+    const BlocksPlan p = w->plan;
+    if (!p.ok) return;
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + p.dir_off);
+    const uint32_t* bits = reinterpret_cast<const uint32_t*>(buf + container_bitmap_offset(p.n_chunks));
+    const uint8_t* blob = buf + p.blob_off;
+    const uint64_t threads = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    const uint64_t t = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    bool ok = true;
+    for (uint64_t c = t; c < p.n_chunks; c += threads)
+        ok &= container_v6_chunk_ok(offsets, bits, blob, c, p.chunk_syms, p.n_symbols, p.blob_bytes);
+    for (uint64_t i = t; i < container_bitmap_words(p.n_chunks); i += threads) ok &= container_bitmap_word_ok(bits, i, p.n_chunks);
+    if (t == 0) ok &= container_dir_ends_ok(offsets, p.n_chunks, p.blob_bytes);
+    if (!ok) w->bad = 1;
+}
+
 // The version 1 model (256 x u32 at buf + 64) checked and turned into the decode table of the header's coder in
 // s->table, byte for byte what rb200_model_create builds on the host (tables.h has the formats and the per-entry
 // formulas both sides call).  Slot-to-symbol is a binary search over cum, per slot (word) or per 4 slots (the cum2sym
@@ -342,23 +404,6 @@ __global__ void __launch_bounds__(32)
 constexpr int kPlannedWarps = 8;
 static_assert(kPlannedWarps * 32 == 256, "STORED: one thread per frequency of a row");
 
-// One chunk of a stored block, one warp: chunk_syms symbols from src (16-byte aligned: a stored stream starts a vector)
-// to dst, with 16-byte loads; whole 16-byte stores where dst and the length allow them, bytes otherwise.
-__device__ __forceinline__ void block_copy_stored(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t chunk_syms, uint32_t lane)
-{
-    const bool vec = ((reinterpret_cast<uintptr_t>(dst) | chunk_syms) & 15) == 0;
-    for (uint32_t v = lane; v < (chunk_syms + 15) / 16; v += 32) {
-        const uint4 q = ldg_stream_u128(reinterpret_cast<const uint4*>(src) + v);
-        if (vec) {
-            stg_stream_u128(reinterpret_cast<uint4*>(dst) + v, q);
-        } else {
-            const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-            for (uint32_t j = 0; j < 16; j++)
-                if (16 * v + j < chunk_syms) dst[16 * v + j] = static_cast<uint8_t>(w[j >> 2] >> (8 * (j & 3)));
-        }
-    }
-}
 
 template <uint32_t CODER, uint32_t SB, bool STORED = false>
 __global__ void __launch_bounds__(kPlannedWarps * 32, CODER == RB200_CODER_WORD ? 8 : 0)
@@ -423,8 +468,16 @@ __global__ void __launch_bounds__(kPlannedWarps * 32, CODER == RB200_CODER_WORD 
 // only when go is its id.  Word and alias: the shipped persistent kernels' CTA set-up around decode_persistent with the
 // shipped policies; byte and rans64: the shipped kernels' table staging around a counter-driven loop over
 // decode_window_chunk (their own kernels launch one warp per chunk, a grid only the host can size).
+// STORED (rb200_container_stored_decode_async, version 6, with version 1's ids): the chunk loops copy every chunk whose
+// bit is set in the bitmap and decode the others.
 
-template <bool WIDE>
+// version 6's stored-chunk bitmap (STORED only)
+__device__ __forceinline__ const uint32_t* planned_stored_bits(const uint8_t* buf, const BlocksPlan& p)
+{
+    return reinterpret_cast<const uint32_t*>(buf + container_bitmap_offset(p.n_chunks));
+}
+
+template <bool WIDE, bool STORED = false>
 __global__ void __launch_bounds__(DecShip::kWarps * 32, DecShip::kMinBlocks)
     word_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                uint32_t* __restrict__ status)
@@ -456,11 +509,12 @@ __global__ void __launch_bounds__(DecShip::kWarps * 32, DecShip::kMinBlocks)
             }
     }
     __syncwarp();
-    decode_persistent<P>(WordDecoder<WIDE>{tab, 0}, ring, buf + p.blob_off, p.blob_bytes, reinterpret_cast<const uint64_t*>(buf + p.dir_off),
-                         out, p.n_symbols, p.chunk_syms, static_cast<uint32_t>(p.n_chunks), &w->work, lane, status);
+    decode_persistent<P, STORED>(WordDecoder<WIDE>{tab, 0}, ring, buf + p.blob_off, p.blob_bytes, reinterpret_cast<const uint64_t*>(buf + p.dir_off),
+                                 out, p.n_symbols, p.chunk_syms, static_cast<uint32_t>(p.n_chunks), &w->work, lane, status,
+                                 STORED ? planned_stored_bits(buf, p) : nullptr);
 }
 
-template <uint32_t SB>
+template <uint32_t SB, bool STORED = false>
 __global__ void __launch_bounds__(AliasDecShip::kWarps * 32, AliasDecShip::kMinBlocks)
     alias_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                 uint32_t* __restrict__ status)
@@ -483,14 +537,15 @@ __global__ void __launch_bounds__(AliasDecShip::kWarps * 32, AliasDecShip::kMinB
     const uint32_t warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
     const uint32_t lane = threadIdx.x & 31;
     const AliasDecoder<SB, kAliasLean> coder = {base + (lane & (kAliasDecReplicas - 1)) * 16, sb_rt};
-    decode_persistent<P>(coder, base + P::kWarpsOff + warp * P::kWarpStride, buf + p.blob_off, p.blob_bytes,
-                         reinterpret_cast<const uint64_t*>(buf + p.dir_off), out, p.n_symbols, p.chunk_syms, static_cast<uint32_t>(p.n_chunks),
-                         &w->work, lane, status);
+    decode_persistent<P, STORED>(coder, base + P::kWarpsOff + warp * P::kWarpStride, buf + p.blob_off, p.blob_bytes,
+                                 reinterpret_cast<const uint64_t*>(buf + p.dir_off), out, p.n_symbols, p.chunk_syms,
+                                 static_cast<uint32_t>(p.n_chunks), &w->work, lane, status, STORED ? planned_stored_bits(buf, p) : nullptr);
 }
 
 // Every warp of the grid takes chunk ids from w->work until none is left and decodes each through its 1 KiB stream
-// window at shared address `ring`; the last warp out re-arms the counter.
-template <class C>
+// window at shared address `ring`; the last warp out re-arms the counter.  STORED: a chunk whose bit is set is copied
+// (block_copy_stored) in place of the window and the decode.
+template <bool STORED = false, class C>
 __device__ __forceinline__ void decode_window_planned(const C& coder, const uint8_t* __restrict__ buf, uint8_t* __restrict__ out,
                                                       ContainerAsyncWork* __restrict__ w, uint32_t ring, uint32_t* __restrict__ status)
 {
@@ -505,6 +560,10 @@ __device__ __forceinline__ void decode_window_planned(const C& coder, const uint
         if (chunk >= n_chunks) break;
         const uint64_t first = static_cast<uint64_t>(chunk) * p.chunk_syms;
         const uint32_t m = static_cast<uint32_t>(min(static_cast<uint64_t>(p.chunk_syms), p.n_symbols - first));
+        if (STORED && container_chunk_stored(planned_stored_bits(buf, p), chunk)) {
+            block_copy_stored(blob + offsets[chunk], out + first, m, lane);
+            continue;
+        }
         decode_window_chunk(coder, blob, p.blob_bytes, offsets, chunk, ring, out + first, m, status);
     }
     if (lane == 0 && atomicAdd(&w->work.warps_done, 1u) == gridDim.x * (blockDim.x / 32) - 1) {
@@ -517,7 +576,7 @@ __device__ __forceinline__ void decode_window_planned(const C& coder, const uint
 // variant decodes (the generic one: 15)
 __host__ __device__ constexpr uint32_t byte_planned_smem(uint32_t SB) { return kAliasDecWarps * kRingBytes + 1024 + (1u << (SB ? SB : 15)); }
 
-template <uint32_t SB>
+template <uint32_t SB, bool STORED = false>
 __global__ void __launch_bounds__(kAliasDecWarps * 32, 4)
     byte_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
                                uint32_t* __restrict__ status)
@@ -530,14 +589,14 @@ __global__ void __launch_bounds__(kAliasDecWarps * 32, 4)
     for (uint32_t i = threadIdx.x; i < vecs; i += blockDim.x) s_tab[i] = reinterpret_cast<const uint4*>(w->table)[i];
     __syncthreads();
     const uint32_t warp = threadIdx.x >> 5;
-    decode_window_planned(ByteDecoder<SB>{smem_addr_pinned(s_tab), sb}, buf, out, w, smem_addr(s_adec) + warp * kRingBytes, status);
+    decode_window_planned<STORED>(ByteDecoder<SB>{smem_addr_pinned(s_tab), sb}, buf, out, w, smem_addr(s_adec) + warp * kRingBytes, status);
 }
 
 constexpr uint32_t kRans64PlannedSmem = kRans64Warps * kRingBytes + kRans64DecSymBytes + (1u << 16);
 
-__global__ void __launch_bounds__(kRans64Warps * 32, 2)
-    rans64_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
-                                 uint32_t* __restrict__ status)
+template <bool STORED>
+__device__ __forceinline__ void rans64_decode_planned(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
+                                                      uint32_t* __restrict__ status)
 {
     if (w->go != kDecRans64) return;
     const uint32_t sb = w->scale_bits;
@@ -554,7 +613,21 @@ __global__ void __launch_bounds__(kRans64Warps * 32, 2)
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t tab = smem_addr(s_tab);
     const Rans64Decoder coder = {tab, tab + (1u << sb) + (lane & (kRans64DecReplicas - 1)) * 8, sb};
-    decode_window_planned(coder, buf, out, w, smem_addr(s_r64) + warp * kRingBytes, status);
+    decode_window_planned<STORED>(coder, buf, out, w, smem_addr(s_r64) + warp * kRingBytes, status);
+}
+
+__global__ void __launch_bounds__(kRans64Warps * 32, 2)
+    rans64_decode_planned_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
+                                 uint32_t* __restrict__ status)
+{
+    rans64_decode_planned<false>(buf, out, w, status);
+}
+
+__global__ void __launch_bounds__(kRans64Warps * 32, 2)
+    rans64_decode_planned_stored_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ out, ContainerAsyncWork* __restrict__ w,
+                                        uint32_t* __restrict__ status)
+{
+    rans64_decode_planned<true>(buf, out, w, status);
 }
 
 // One launch of a decoder: kernel, grid, threads, dynamic shared memory.
@@ -565,9 +638,10 @@ struct DecoderLaunch {
 };
 
 // The decoders of every version in one launch table, each version's in id order: version v's are the entries
-// kDecoderFirst[v - 1] .. kDecoderFirst[v] - 1.  Version 5's are the STORED twins of versions 2-4's, with their ids.
-constexpr int kDecoderFirst[] = {0, 11, 12, 16, 19, 27};
-constexpr int kContainerDecoders = kDecoderFirst[5];
+// kDecoderFirst[v - 1] .. kDecoderFirst[v] - 1.  Version 5's are the STORED twins of versions 2-4's, with their ids;
+// version 6's the STORED twins of version 1's, with theirs.
+constexpr int kDecoderFirst[] = {0, 11, 12, 16, 19, 27, 38};
+constexpr int kContainerDecoders = kDecoderFirst[6];
 // the prefix check's grid: kPrefixCtasPerSm CTAs of kPrefixWarps warps per SM
 constexpr uint32_t kPrefixCtasPerSm = 8;
 
@@ -619,6 +693,23 @@ inline void configure_container_decode(uint32_t sms, DecoderLaunch* out)
          "block_decode_planned_kernel<alias, 12, stored>"},
         {block_decode_planned_kernel<RB200_CODER_ALIAS, 0, true>, 0, planned,
          block_coder_decode_smem(RB200_CODER_ALIAS, kBlockCoderMaxScaleBits, planned), "block_decode_planned_kernel<alias, 0, stored>"},
+        {word_decode_planned_kernel<false, true>, sms * DecShip::kMinBlocks, DecShip::kWarps * 32, DecShip::kSmemBytes,
+         "word_decode_planned_kernel(stored)"},
+        {word_decode_planned_kernel<true, true>, sms * DecShip::kMinBlocks, DecShip::kWarps * 32, DecShip::kSmemBytes,
+         "word_decode_planned_kernel(wide, stored)"},
+        {alias_decode_planned_kernel<16, true>, sms * AliasDecShip::kMinBlocks, AliasDecShip::kWarps * 32, AliasDecShip::kSmemBytes,
+         "alias_decode_planned_kernel<16, stored>"},
+        {alias_decode_planned_kernel<14, true>, sms * AliasDecShip::kMinBlocks, AliasDecShip::kWarps * 32, AliasDecShip::kSmemBytes,
+         "alias_decode_planned_kernel<14, stored>"},
+        {alias_decode_planned_kernel<12, true>, sms * AliasDecShip::kMinBlocks, AliasDecShip::kWarps * 32, AliasDecShip::kSmemBytes,
+         "alias_decode_planned_kernel<12, stored>"},
+        {alias_decode_planned_kernel<0, true>, sms * AliasDecShip::kMinBlocks, AliasDecShip::kWarps * 32, AliasDecShip::kSmemBytes,
+         "alias_decode_planned_kernel<0, stored>"},
+        {byte_decode_planned_kernel<16, true>, 0, kAliasDecWarps * 32, byte_planned_smem(16), "byte_decode_planned_kernel<16, stored>"},
+        {byte_decode_planned_kernel<14, true>, 0, kAliasDecWarps * 32, byte_planned_smem(14), "byte_decode_planned_kernel<14, stored>"},
+        {byte_decode_planned_kernel<12, true>, 0, kAliasDecWarps * 32, byte_planned_smem(12), "byte_decode_planned_kernel<12, stored>"},
+        {byte_decode_planned_kernel<0, true>, 0, kAliasDecWarps * 32, byte_planned_smem(0), "byte_decode_planned_kernel<0, stored>"},
+        {rans64_decode_planned_stored_kernel, 0, kRans64Warps * 32, kRans64PlannedSmem, "rans64_decode_planned_stored_kernel"},
     };
     for (int i = 0; i < kContainerDecoders; i++) {
         out[i] = l[i];

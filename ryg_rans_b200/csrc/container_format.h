@@ -19,6 +19,7 @@ constexpr uint16_t kContainerVersionBlocks = 2;     // one model per block: n_bl
 constexpr uint16_t kContainerVersionBlocksCoder = 3;  // version 2's layout with the byte or rans64 coder at scale_bits 8..15
 constexpr uint16_t kContainerVersionBlocksAlias = 4;  // version 2's layout with the alias coder at scale_bits 8..15
 constexpr uint16_t kContainerVersionBlocksStored = 5; // the layout of versions 2-4 for any of their pairs, with stored blocks
+constexpr uint16_t kContainerVersionStored = 6;       // version 1's layout with a stored-chunk bitmap before the blob
 
 struct ContainerHeader {        // 64 bytes
     uint32_t magic;
@@ -279,6 +280,53 @@ RB200_HD inline bool container_stored_pad_ok(const uint8_t* stream, uint32_t chu
     for (uint64_t i = chunk_syms; i < container_stored_bytes(chunk_syms); i++)
         if (stream[i]) return false;
     return true;
+}
+
+// Version 6 (single model, stored chunks): version 1's header, model and directory at 1088, then, from the next
+// 16-byte boundary, the stored-chunk bitmap -- ceil(n_chunks / 32) u32 words, bit c % 32 of word c / 32 set when chunk c
+// is stored, zero-padded to 16 bytes -- then the blob.  meta_crc covers every byte before the blob: the header (crc
+// fields zero), the model, the directory, the zero pad after it and the bitmap with its padding.
+RB200_HD inline uint64_t container_bitmap_offset(uint64_t n_chunks) { return (kContainerDirOffset + (n_chunks + 1) * sizeof(uint64_t) + 15) & ~15ull; }
+// the bitmap's words with its padding: a multiple of 4
+RB200_HD inline uint64_t container_bitmap_words(uint64_t n_chunks) { return ((n_chunks + 31) / 32 + 3) & ~3ull; }
+RB200_HD inline uint64_t container_bitmap_blob_offset(uint64_t n_chunks)
+{
+    return container_bitmap_offset(n_chunks) + container_bitmap_words(n_chunks) * sizeof(uint32_t);
+}
+// version 6's header rules: version 1's, with block_size, n_blocks and reserved zero and the bitmap's blob offset
+RB200_HD inline bool container_chunks_stored_header_ok(const ContainerHeader& h, uint64_t size)
+{
+    if (h.version != kContainerVersionStored || h.block_size || h.n_blocks || h.reserved) return false;
+    ContainerHeader v1 = h;
+    v1.version = kContainerVersion;
+    if (!container_header_ok(v1, size, kContainerVersion)) return false;
+    const uint64_t boff = container_bitmap_blob_offset(h.n_chunks);
+    return boff <= size && h.blob_bytes <= size - boff;
+}
+// m_c: the symbols of chunk c, chunk_syms but for a ragged last chunk
+RB200_HD inline uint32_t container_chunk_symbols(uint64_t c, uint32_t chunk_syms, uint64_t n_symbols)
+{
+    const uint64_t left = n_symbols - c * chunk_syms;
+    return left < chunk_syms ? static_cast<uint32_t>(left) : chunk_syms;
+}
+// chunk c's bit
+RB200_HD inline bool container_chunk_stored(const uint32_t* bits, uint64_t c) { return (bits[c >> 5] >> (c & 31)) & 1u; }
+// word w of the bitmap (padding included) has no bit at or past n_chunks
+RB200_HD inline bool container_bitmap_word_ok(const uint32_t* bits, uint64_t w, uint64_t n_chunks)
+{
+    if (32 * w >= n_chunks) return bits[w] == 0;
+    return n_chunks - 32 * w >= 32 || (bits[w] >> (n_chunks - 32 * w)) == 0;
+}
+// chunk c of version 6 is well formed: its directory step (every entry), and when its bit is set the step and zero
+// padding of a stored stream of m_c symbols (container_stored_step_ok, container_stored_pad_ok: the padding is read
+// only once the step puts the stream inside the blob)
+RB200_HD inline bool container_v6_chunk_ok(const uint64_t* offsets, const uint32_t* bits, const uint8_t* blob, uint64_t c, uint32_t chunk_syms,
+                                        uint64_t n_symbols, uint64_t blob_bytes)
+{
+    if (!container_dir_step_ok(offsets, c)) return false;
+    if (!container_chunk_stored(bits, c)) return true;
+    const uint32_t m = container_chunk_symbols(c, chunk_syms, n_symbols);
+    return container_stored_step_ok(offsets, c, m, blob_bytes) && container_stored_pad_ok(blob + offsets[c], m);
 }
 
 // the header rb200_container_pack writes (crc fields zero)

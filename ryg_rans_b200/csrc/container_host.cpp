@@ -35,6 +35,7 @@
 #include "container_format.h"
 
 #include <cstring>
+#include <vector>
 
 namespace rb200 {
 
@@ -404,6 +405,95 @@ extern "C" int rb200_container_blocks_stored_pack(int coder, uint32_t scale_bits
 extern "C" int rb200_container_blocks_stored_open(const uint8_t* buf, size_t size, rb200_container_blocks_coder_info* info)
 {
     return container_blocks_coder_open(buf, size, kContainerVersionBlocksStored, info);
+}
+
+namespace {
+
+// Version 6's prefix rules past the header, on a host buffer holding the whole container: meta_crc over [0, blob
+// offset), the model, the directory's ends, every chunk (container_v6_chunk_ok) and every bitmap word.
+int container_v6_check(const ContainerHeader& h, const uint8_t* buf)
+{
+    const uint64_t boff = container_bitmap_blob_offset(h.n_chunks);
+    const uint32_t meta = container_crc32(container_header_crc(h), buf + sizeof(ContainerHeader), boff - sizeof(ContainerHeader));
+    if (meta != h.meta_crc) return RB200_E_STREAM;
+    if (!container_model_ok(h.coder, h.scale_bits, reinterpret_cast<const uint32_t*>(buf + sizeof(ContainerHeader)))) return RB200_E_STREAM;
+    const uint64_t* offsets = reinterpret_cast<const uint64_t*>(buf + kContainerDirOffset);
+    const uint32_t* bits = reinterpret_cast<const uint32_t*>(buf + container_bitmap_offset(h.n_chunks));
+    if (!container_dir_ends_ok(offsets, h.n_chunks, h.blob_bytes)) return RB200_E_STREAM;
+    for (uint64_t w = 0; w < container_bitmap_words(h.n_chunks); w++)
+        if (!container_bitmap_word_ok(bits, w, h.n_chunks)) return RB200_E_STREAM;
+    for (uint64_t c = 0; c < h.n_chunks; c++)
+        if (!container_v6_chunk_ok(offsets, bits, buf + boff, c, h.chunk_syms, h.n_symbols, h.blob_bytes)) return RB200_E_STREAM;
+    return RB200_OK;
+}
+
+}  // namespace
+
+extern "C" size_t rb200_container_stored_bound(size_t n, uint32_t chunk_syms)
+{
+    if (n == 0 || (n >> 32) || !container_chunk_ok(chunk_syms)) return 0;
+    const uint64_t n_chunks = rb200_chunk_count(n, chunk_syms), tail = n % chunk_syms;
+    return container_bitmap_blob_offset(n_chunks) + (n / chunk_syms) * container_stored_bytes(chunk_syms) +
+           (tail ? container_stored_bytes(static_cast<uint32_t>(tail)) : 0);
+}
+
+extern "C" int rb200_container_stored_pack(int coder, uint32_t scale_bits, uint32_t chunk_syms, size_t n, const uint32_t freqs[256],
+                                           const uint32_t* stored_bits, const uint64_t* offsets, const uint8_t* blob, size_t blob_bytes,
+                                           uint32_t flags, uint8_t* out, size_t out_cap, size_t* out_size)
+{
+    if (coder < 0 || !candidate_ok(RB200_CANDIDATE(coder, scale_bits)) || !rb200_container_stored_bound(n, chunk_syms)) return RB200_E_ARG;
+    if (!freqs || !stored_bits || !offsets || (!blob && blob_bytes) || !out) return RB200_E_ARG;
+    if (!container_model_ok(static_cast<uint32_t>(coder), scale_bits, freqs)) return RB200_E_MODEL;   // never write what open rejects
+    const uint64_t n_chunks = rb200_chunk_count(n, chunk_syms);
+    const uint64_t words = (n_chunks + 31) / 32;
+    if (!container_bitmap_word_ok(stored_bits, words - 1, n_chunks) || (blob_bytes & 15) ||
+        !container_dir_ends_ok(offsets, n_chunks, blob_bytes))
+        return RB200_E_ARG;
+    std::vector<uint32_t> bits(container_bitmap_words(n_chunks), 0u);
+    std::memcpy(bits.data(), stored_bits, words * sizeof(uint32_t));
+    for (uint64_t c = 0; c < n_chunks; c++)
+        if (!container_v6_chunk_ok(offsets, bits.data(), blob, c, chunk_syms, n, blob_bytes)) return RB200_E_ARG;
+    const uint64_t boff = container_bitmap_blob_offset(n_chunks), bitmap = container_bitmap_offset(n_chunks);
+    const size_t total = boff + blob_bytes;
+    if (total > out_cap) return RB200_E_SPACE;
+    ContainerHeader h = container_header(coder, scale_bits, chunk_syms, n, n_chunks, blob_bytes, flags);
+    h.version = kContainerVersionStored;
+    std::memset(out, 0, boff);
+    std::memcpy(out + sizeof h, freqs, 256 * sizeof(uint32_t));
+    std::memcpy(out + kContainerDirOffset, offsets, (n_chunks + 1) * sizeof(uint64_t));
+    std::memcpy(out + bitmap, bits.data(), bits.size() * sizeof(uint32_t));
+    h.meta_crc = container_crc32(container_header_crc(h), out + sizeof h, boff - sizeof h);
+    if (h.flags & RB200_CONTAINER_CRC_BLOB) h.blob_crc = container_crc32(0, blob, blob_bytes);
+    std::memcpy(out, &h, sizeof h);
+    if (blob_bytes) std::memcpy(out + boff, blob, blob_bytes);
+    if (out_size) *out_size = total;
+    return RB200_OK;
+}
+
+extern "C" int rb200_container_stored_open(const uint8_t* buf, size_t size, rb200_container_info* info, const uint32_t** stored_bits)
+{
+    if (!buf || !info || !stored_bits) return RB200_E_ARG;
+    if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
+    ContainerHeader h;
+    std::memcpy(&h, buf, sizeof h);
+    if (!container_chunks_stored_header_ok(h, size)) return RB200_E_STREAM;
+    if (reinterpret_cast<uintptr_t>(buf) & 7) return RB200_E_ARG;
+    int rc = container_v6_check(h, buf);
+    if (rc == RB200_OK && (h.flags & RB200_CONTAINER_CRC_BLOB))
+        rc = container_check_blob(h, container_crc32(0, buf + container_bitmap_blob_offset(h.n_chunks), h.blob_bytes));
+    if (rc != RB200_OK) return rc;
+    info->coder = h.coder;
+    info->scale_bits = h.scale_bits;
+    info->chunk_syms = h.chunk_syms;
+    info->flags = h.flags;
+    info->n_symbols = h.n_symbols;
+    info->n_chunks = h.n_chunks;
+    info->blob_bytes = h.blob_bytes;
+    info->freqs = reinterpret_cast<const uint32_t*>(buf + sizeof(ContainerHeader));
+    info->offsets = reinterpret_cast<const uint64_t*>(buf + kContainerDirOffset);
+    info->blob = buf + container_bitmap_blob_offset(h.n_chunks);
+    *stored_bits = reinterpret_cast<const uint32_t*>(buf + container_bitmap_offset(h.n_chunks));
+    return RB200_OK;
 }
 
 extern "C" int rb200_choose_coder(const uint64_t counts[256], size_t n, uint32_t chunk_syms, const uint32_t* candidates,

@@ -273,7 +273,9 @@ inline uint32_t crc32_grid(uint32_t sms, uint64_t n)
 // GEOM (rb200_container_model_encode_varlen_async, version 1): n_symbols, n_chunks and the blob offset from the record
 // (VarlenGeom); h arrives with coder, scale_bits, chunk_syms and flags.  Writes nothing when geom->go == 0.
 // CHOSEN (rb200_container_model_encode_auto_async, version 1): coder and scale_bits from the choice record.
-template <bool GEOM, bool CHOSEN>
+// BITMAP (rb200_container_stored_encode_async, version 6): slots[0] covers out[head, blob_off) -- directory, the pad
+// after it and the stored-chunk bitmap, all written by then -- so meta_crc spans everything before the blob.
+template <bool GEOM, bool CHOSEN, bool BITMAP = false>
 __device__ __forceinline__ void container_finish(uint8_t* out, ContainerHeader h, uint64_t dir_off, uint64_t blob_off, uint64_t out_cap,
                                                  const uint32_t* __restrict__ freqs, const CrcSlot* __restrict__ slots, uint32_t* status,
                                                  const VarlenGeom* __restrict__ geom, const CoderChoice* __restrict__ choice)
@@ -314,7 +316,8 @@ __device__ __forceinline__ void container_finish(uint8_t* out, ContainerHeader h
     c = __reduce_xor_sync(0xffffffffu, crc32_shift(c, head - piece * (lane + 1)));
     const uint32_t head_crc = finish_warp(0, head, c);
     const uint64_t dir_end = dir_off + (h.n_chunks + 1) * sizeof(uint64_t);
-    const uint32_t meta = crc32_mulmod(head_crc, x8pow_warp(dir_end - head)) ^ slots[0].crc;      // crc32_combine
+    const uint64_t meta_end = BITMAP ? blob_off : dir_end;
+    const uint32_t meta = crc32_mulmod(head_crc, x8pow_warp(meta_end - head)) ^ slots[0].crc;     // crc32_combine
     __syncwarp();
     if (lane == 0) {
         sbuf[offsetof(ContainerHeader, meta_crc) / 4] = meta;
@@ -323,7 +326,7 @@ __device__ __forceinline__ void container_finish(uint8_t* out, ContainerHeader h
     __syncwarp();
     uint4* dst = reinterpret_cast<uint4*>(out);
     for (uint32_t i = lane; i < head / 16; i += 32) dst[i] = sbuf_v[i];
-    if (lane == 0 && blob_off > dir_end) *reinterpret_cast<uint64_t*>(out + dir_end) = 0;   // the 8-byte pad
+    if (!BITMAP && lane == 0 && blob_off > dir_end) *reinterpret_cast<uint64_t*>(out + dir_end) = 0;   // the 8-byte pad
 }
 
 template <bool GEOM = false, bool CHOSEN = false>
@@ -366,6 +369,16 @@ __global__ void __launch_bounds__(32)
 {
     h.version = kContainerVersionBlocksStored;
     container_finish<false, true>(out, h, dir_off, blob_off, out_cap, nullptr, slots, status, nullptr, &r->choice);
+}
+
+// The header kernel of rb200_container_stored_encode_async: container_finish_kernel's CHOSEN instance with version 6,
+// meta_crc over the bitmap as well (BITMAP), and the model section from freqs
+__global__ void __launch_bounds__(32)
+    container_stored_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t blob_off, uint64_t out_cap, const uint32_t* __restrict__ freqs,
+                                   const CrcSlot* __restrict__ slots, uint32_t* status, const CoderChoice* __restrict__ choice)
+{
+    h.version = kContainerVersionStored;
+    container_finish<false, true, true>(out, h, kContainerDirOffset, blob_off, out_cap, freqs, slots, status, nullptr, choice);
 }
 
 }  // namespace rb200

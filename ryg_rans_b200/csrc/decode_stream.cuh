@@ -337,14 +337,35 @@ __device__ __forceinline__ void tma_advance(TmaWindow& w, uint32_t lane, uint32_
     w.limit += P::kUnit;
 }
 
+// One stored chunk, one warp (block_decode_planned_kernel's stored blocks, the version 6 decoders' stored chunks):
+// chunk_syms symbols from src (16-byte aligned: a stored stream starts a vector) to dst, with 16-byte loads; whole
+// 16-byte stores where dst and the length allow them, bytes otherwise.
+__device__ __forceinline__ void block_copy_stored(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t chunk_syms, uint32_t lane)
+{
+    const bool vec = ((reinterpret_cast<uintptr_t>(dst) | chunk_syms) & 15) == 0;
+    for (uint32_t v = lane; v < (chunk_syms + 15) / 16; v += 32) {
+        const uint4 q = ldg_stream_u128(reinterpret_cast<const uint4*>(src) + v);
+        if (vec) {
+            stg_stream_u128(reinterpret_cast<uint4*>(dst) + v, q);
+        } else {
+            const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+            for (uint32_t j = 0; j < 16; j++)
+                if (16 * v + j < chunk_syms) dst[16 * v + j] = static_cast<uint8_t>(w[j >> 2] >> (8 * (j & 3)));
+        }
+    }
+}
+
 // The persistent chunk loop of one warp: pull chunk ids from work->next_chunk until none is left, decode each into
 // out[chunk * chunk_syms, ...) through the warp's TmaWindow at shared address `ring`; the last warp out re-arms `work`
 // for the next launch.  With kRefillTma the caller has initialised the ring's mbarriers behind a CTA barrier.
-template <class P, class C>
+// STORED (the version 6 decoders): a chunk whose bit is set in stored_bits is copied from blob + offsets[chunk]
+// (block_copy_stored; the container's checks saw its step and padding), with no window set-up.
+template <class P, bool STORED = false, class C>
 __device__ __forceinline__ void decode_persistent(const C& coder, uint32_t ring, const uint8_t* __restrict__ blob, uint64_t blob_size,
                                                   const uint64_t* __restrict__ offsets, uint8_t* __restrict__ out, uint64_t n,
                                                   uint32_t chunk_syms, uint32_t n_chunks, DecodeWork* __restrict__ work,
-                                                  uint32_t lane, uint32_t* __restrict__ status)
+                                                  uint32_t lane, uint32_t* __restrict__ status, const uint32_t* __restrict__ stored_bits = nullptr)
 {
     static_assert(C::kMaxBytes <= 2, "DecPolicy::kNeed and the mirror are sized for at most 2 bytes per lane per step");
     TmaWindow win;
@@ -360,6 +381,10 @@ __device__ __forceinline__ void decode_persistent(const C& coder, uint32_t ring,
         const uint64_t first = static_cast<uint64_t>(chunk) * chunk_syms;
         const uint64_t left = n - first;
         const uint32_t m = left < chunk_syms ? static_cast<uint32_t>(left) : chunk_syms;
+        if (STORED && ((stored_bits[chunk >> 5] >> (chunk & 31)) & 1u)) {
+            block_copy_stored(blob + offsets[chunk], out + first, m, lane);
+            continue;
+        }
         const uint64_t off = offsets[chunk];
         const uint64_t end = offsets[chunk + 1] & ~static_cast<uint64_t>(15);
         if (__shfl_sync(0xffffffffu, dir_entry_bad<C>(off, end, blob_size) ? 1u : 0u, 0)) {

@@ -39,6 +39,10 @@
 // rb200_container_blocks_stored_encode_async (version 5) runs the choice kernel (blocks_one_pair_kernel for one
 // candidate) and one GATED split encoder per group into one workspace, then blocks_store_kernel, which stores every
 // block whose coded chunks take more blob than its symbols, and one ungated scan and compact_stored_kernel.
+//
+// rb200_container_stored_encode_async (version 6) runs the histogram, the choice and the CHOSEN model kernel of the auto
+// encode, then one GATED split encoder per group into one workspace, chunks_store_kernel, which stores every chunk whose
+// stream is longer than its symbols and writes the bitmap, one ungated scan and chunks_stored_compaction_kernel.
 #pragma once
 #include "block_kernels.cuh"
 #include "container_format.h"
@@ -308,6 +312,32 @@ __global__ void __launch_bounds__(kStoreWarps * 32)
     if (!store) return;
     if (lane < per_block) s[lane] = raw;
     reinterpret_cast<uint4*>(models + static_cast<uint64_t>(block) * 256)[lane] = make_uint4(0, 0, 0, 0);   // 32 x 16 bytes
+}
+
+// The store rule of rb200_container_stored_encode_async (version 6), one thread per chunk, after the encoder wrote every
+// chunk's stream size to sizes[]: chunk c is stored when its stream, rounded up to 16 as the compaction places it, is
+// longer than round16(m_c), its symbols' stored size; ties stay coded.  A stored chunk's size becomes round16(m_c) and
+// stored[c] = 1 has the compaction copy its symbols in place of its stream; otherwise stored[c] = 0.  Each warp's ballot
+// is one word of the container's bitmap: the grid covers the padding words too, which it writes zero, and thread 0
+// zeroes the pad between the directory and the bitmap, both of which meta_crc covers.
+constexpr int kChunkStoreThreads = 256;
+
+__global__ void __launch_bounds__(kChunkStoreThreads)
+    chunks_store_kernel(uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t n, uint32_t chunk_syms, uint8_t* __restrict__ out,
+                        uint32_t* __restrict__ stored)
+{
+    const uint64_t c = static_cast<uint64_t>(blockIdx.x) * kChunkStoreThreads + threadIdx.x;
+    bool store = false;
+    if (c < n_chunks) {
+        const uint32_t raw = static_cast<uint32_t>(container_stored_bytes(container_chunk_symbols(c, chunk_syms, n)));
+        store = ((sizes[c] + 15u) & ~15u) > raw;
+        stored[c] = store;
+        if (store) sizes[c] = raw;
+    }
+    const uint32_t word = __ballot_sync(0xffffffffu, store);
+    const uint64_t bitmap = container_bitmap_offset(n_chunks), dir_end = kContainerDirOffset + (n_chunks + 1) * sizeof(uint64_t);
+    if ((threadIdx.x & 31) == 0 && c / 32 < container_bitmap_words(n_chunks)) reinterpret_cast<uint32_t*>(out + bitmap)[c / 32] = word;
+    if (c == 0 && bitmap > dir_end) *reinterpret_cast<uint64_t*>(out + dir_end) = 0;
 }
 
 // The first kernel of rb200_container_model_encode_varlen_async, one warp: reads n = *d_n, checks 1 <= n <= n_max

@@ -66,7 +66,7 @@ struct rb200_ctx {
     CrcSlot* h_crc = nullptr;
     // the async container decodes (container_decode.cuh): one fixed workspace per version, so that calls of different
     // versions never share state, and every version's decoder launches
-    ContainerAsyncWork* d_async[5] = {};
+    ContainerAsyncWork* d_async[6] = {};
     DecoderLaunch async_decoders[kContainerDecoders] = {};
     // rb200_container_blocks_any_decode_async: its own workspace, for its checks and the decoders of versions 2-4
     ContainerAsyncWork* d_async_any = nullptr;
@@ -549,12 +549,14 @@ bool word_ring_model(const uint32_t freqs[256])
 }
 
 // ring_model: the word model is known to satisfy word_ring_model (a model built on the GPU is not known to)
-EncodePlan plan_encode(const rb200_ctx* ctx, int coder, uint32_t scale_bits, uint32_t n_chunks, uint32_t chunk_syms, bool ring_model)
+// split: the split path whatever the chunk size (rb200_container_stored_encode_async needs every stream's size first)
+EncodePlan plan_encode(const rb200_ctx* ctx, int coder, uint32_t scale_bits, uint32_t n_chunks, uint32_t chunk_syms, bool ring_model,
+                       bool split = false)
 {
     EncodePlan p = {};
     p.n_chunks = n_chunks;
     p.slot_bytes = slot_bytes_for(chunk_syms);
-    p.fused = n_chunks && coder != RB200_CODER_RANS64 && use_fused_encode(chunk_syms);
+    p.fused = !split && n_chunks && coder != RB200_CODER_RANS64 && use_fused_encode(chunk_syms);
     p.slots = n_chunks;
     const uint32_t sms = static_cast<uint32_t>(ctx->sms);
     if (coder == RB200_CODER_WORD) {
@@ -673,6 +675,54 @@ EncodeTables model_tables(const rb200_model* m)
                         word_ring_model(m->freqs)};
 }
 
+// The encode launch of plan p with tables t on workspace ws (split: into the slots; fused: the one kernel).
+int launch_encoder(rb200_ctx* ctx, const EncodeTables& t, const EncodePlan& p, const uint8_t* d_in, size_t n, uint32_t chunk_syms,
+                   uint32_t n_chunks, const EncodeWorkspace& ws, uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom)
+{
+    if (t.coder == RB200_CODER_WORD) {
+        const WordEncEntry* table = t.word[t.word_r32 ? 1 : 0];
+        if (p.ring) {
+            auto kernel = t.word_r32 ? word_encode_ring_kernel<true> : word_encode_ring_kernel<false>;
+            kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.scratch, ws.look, ws.counter,
+                                                               d_blob, blob_cap, d_offsets, ctx->d_status);
+            return check_launch(ctx, "word_encode_ring_kernel");
+        }
+        // the instance word_r32 names, or both GATED ones
+        int rc = RB200_OK;
+        const int r32_first = t.word_gate ? 0 : t.word_r32, r32_last = t.word_gate ? 1 : t.word_r32;
+        for (int r32 = r32_first; r32 <= r32_last && rc == RB200_OK; r32++) {
+            if (p.fused) {
+                auto kernel = !t.word_gate ? (r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>)
+                              : !geom  ? (r32 ? word_encode_fused_kernel<true, true> : word_encode_fused_kernel<false, true>)
+                                       : (r32 ? word_encode_fused_kernel<true, true, true> : word_encode_fused_kernel<false, true, true>);
+                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], ws.scratch, p.slot_bytes, ws.look,
+                                                                   ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status, t.word_gate, geom);
+                rc = check_launch(ctx, "word_encode_fused_kernel");
+            } else {
+                auto kernel = !t.word_gate ? (r32 ? word_encode_kernel<true> : word_encode_kernel<false>)
+                              : !geom  ? (r32 ? word_encode_kernel<true, true> : word_encode_kernel<false, true>)
+                                       : (r32 ? word_encode_kernel<true, true, true> : word_encode_kernel<false, true, true>);
+                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], ws.scratch, p.slot_bytes, ws.sizes,
+                                                                   ctx->d_status, t.word_gate, geom);
+                rc = check_launch(ctx, "word_encode_kernel");
+            }
+        }
+        return rc;
+    }
+    if (t.coder == RB200_CODER_RANS64) {
+        auto kernel = t.choice ? (geom ? rans64_encode_kernel<true, true> : rans64_encode_kernel<false, true>)
+                               : (geom ? rans64_encode_kernel<true> : rans64_encode_kernel<false>);
+        kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.scale_bits, t.r64, ws.scratch, p.slot_bytes,
+                                                           ws.sizes, ctx->d_status, geom, t.choice, t.group);
+        return check_launch(ctx, "rans64_encode_kernel");
+    }
+    const bool alias = t.coder == RB200_CODER_ALIAS;
+    launch_alias_encode(ctx->stream, p.grid, p.smem, d_in, n, chunk_syms, n_chunks, t.scale_bits, t.enc, alias ? t.remap : nullptr,
+                        ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status, geom,
+                        t.choice, t.group);
+    return check_launch(ctx, alias ? "alias_encode_kernel" : "byte_encode_kernel");
+}
+
 // geom set (rb200_container_model_encode_varlen_async): n is the bound n_max, which fixes the plan and every launch
 // shape, the GEOM instances read n, the chunk count and the blob's place from the record, and d_blob is the container.
 int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, size_t n, uint32_t chunk_syms, uint8_t* d_blob,
@@ -683,48 +733,7 @@ int encode_device(rb200_ctx* ctx, const EncodeTables& t, const uint8_t* d_in, si
     const uint32_t n_chunks = static_cast<uint32_t>(n_chunks_sz);
     const EncodePlan p = plan_encode(ctx, t.coder, t.scale_bits, n_chunks, chunk_syms, t.word_ring);
     return run_encode(ctx, p, d_blob, blob_cap, d_offsets, geom, [&](const EncodeWorkspace& ws) {
-        if (t.coder == RB200_CODER_WORD) {
-            const WordEncEntry* table = t.word[t.word_r32 ? 1 : 0];
-            if (p.ring) {
-                auto kernel = t.word_r32 ? word_encode_ring_kernel<true> : word_encode_ring_kernel<false>;
-                kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, table, ws.scratch, ws.look, ws.counter,
-                                                                   d_blob, blob_cap, d_offsets, ctx->d_status);
-                return check_launch(ctx, "word_encode_ring_kernel");
-            }
-            // the instance word_r32 names, or both GATED ones
-            int rc = RB200_OK;
-            const int r32_first = t.word_gate ? 0 : t.word_r32, r32_last = t.word_gate ? 1 : t.word_r32;
-            for (int r32 = r32_first; r32 <= r32_last && rc == RB200_OK; r32++) {
-                if (p.fused) {
-                    auto kernel = !t.word_gate ? (r32 ? word_encode_fused_kernel<true> : word_encode_fused_kernel<false>)
-                                  : !geom  ? (r32 ? word_encode_fused_kernel<true, true> : word_encode_fused_kernel<false, true>)
-                                           : (r32 ? word_encode_fused_kernel<true, true, true> : word_encode_fused_kernel<false, true, true>);
-                    kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], ws.scratch, p.slot_bytes, ws.look,
-                                                                       ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status, t.word_gate, geom);
-                    rc = check_launch(ctx, "word_encode_fused_kernel");
-                } else {
-                    auto kernel = !t.word_gate ? (r32 ? word_encode_kernel<true> : word_encode_kernel<false>)
-                                  : !geom  ? (r32 ? word_encode_kernel<true, true> : word_encode_kernel<false, true>)
-                                           : (r32 ? word_encode_kernel<true, true, true> : word_encode_kernel<false, true, true>);
-                    kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.word[r32], ws.scratch, p.slot_bytes, ws.sizes,
-                                                                       ctx->d_status, t.word_gate, geom);
-                    rc = check_launch(ctx, "word_encode_kernel");
-                }
-            }
-            return rc;
-        }
-        if (t.coder == RB200_CODER_RANS64) {
-            auto kernel = t.choice ? (geom ? rans64_encode_kernel<true, true> : rans64_encode_kernel<false, true>)
-                                   : (geom ? rans64_encode_kernel<true> : rans64_encode_kernel<false>);
-            kernel<<<p.grid, p.threads, p.smem, ctx->stream>>>(d_in, n, chunk_syms, n_chunks, t.scale_bits, t.r64, ws.scratch, p.slot_bytes,
-                                                               ws.sizes, ctx->d_status, geom, t.choice, t.group);
-            return check_launch(ctx, "rans64_encode_kernel");
-        }
-        const bool alias = t.coder == RB200_CODER_ALIAS;
-        launch_alias_encode(ctx->stream, p.grid, p.smem, d_in, n, chunk_syms, n_chunks, t.scale_bits, t.enc, alias ? t.remap : nullptr,
-                            ws.scratch, p.slot_bytes, ws.sizes, ws.look, ws.counter, d_blob, blob_cap, d_offsets, ctx->d_status, geom,
-                            t.choice, t.group);
-        return check_launch(ctx, alias ? "alias_encode_kernel" : "byte_encode_kernel");
+        return launch_encoder(ctx, t, p, d_in, n, chunk_syms, n_chunks, ws, d_blob, blob_cap, d_offsets, geom);
     }, t.choice, t.group);
 }
 
@@ -1866,14 +1875,18 @@ int container_decode_async(rb200_ctx* ctx, uint16_t version, const uint8_t* buf,
     DeviceGuard g(ctx->device);
     const bool any = version == kContainerVersionAnyBlocks;
     ContainerAsyncWork* w = any ? ctx->d_async_any : ctx->d_async[version - 1];
-    const bool stored = version == kContainerVersionBlocksStored;
+    const bool stored = version == kContainerVersionBlocksStored, v6 = version == kContainerVersionStored;
     const int first = kDecoderFirst[any ? kContainerVersionBlocks - 1 : version - 1];
     const int last = kDecoderFirst[any ? kContainerVersionBlocksAlias : version];
     const uint32_t sms = static_cast<uint32_t>(ctx->sms);
     const uint64_t after_head = size > sizeof(ContainerHeader) ? size - sizeof(ContainerHeader) : 0;
     cudaStream_t s = ctx->stream;
-    auto plan = stored ? container_plan_kernel<true> : container_plan_kernel<false>;
-    plan<<<1, 32, 0, s>>>(buf, size, version, w);
+    if (v6) {
+        container_stored_plan_kernel<<<1, 32, 0, s>>>(buf, size, w);
+    } else {
+        auto plan = stored ? container_plan_kernel<true> : container_plan_kernel<false>;
+        plan<<<1, 32, 0, s>>>(buf, size, version, w);
+    }
     int rc = check_launch(ctx, "container_plan_kernel");
     if (rc != RB200_OK) return rc;
     crc32_kernel<<<crc32_grid(sms, after_head), kCrcThreads, kCrcSmemBytes, s>>>(buf + sizeof(ContainerHeader), after_head, &w->plan.meta_len,
@@ -1884,16 +1897,21 @@ int container_decode_async(rb200_ctx* ctx, uint16_t version, const uint8_t* buf,
                                                                            &w->crc_work, &w->crc[1]);
     rc = check_launch(ctx, "crc32_kernel(blob)");
     if (rc != RB200_OK) return rc;
-    auto prefix = stored ? container_prefix_check_kernel<true> : container_prefix_check_kernel<false>;
-    prefix<<<sms * kPrefixCtasPerSm, kPrefixWarps * 32, 0, s>>>(buf, w);
+    if (v6) {
+        container_stored_check_kernel<<<sms * kPrefixCtasPerSm, kPrefixWarps * 32, 0, s>>>(buf, w);
+    } else {
+        auto prefix = stored ? container_prefix_check_kernel<true> : container_prefix_check_kernel<false>;
+        prefix<<<sms * kPrefixCtasPerSm, kPrefixWarps * 32, 0, s>>>(buf, w);
+    }
     rc = check_launch(ctx, "container_prefix_check_kernel");
     if (rc != RB200_OK) return rc;
-    if (version == kContainerVersion) {
+    if (version == kContainerVersion || v6) {
         container_table_kernel<<<1, kTableThreads, 0, s>>>(buf, w);
         rc = check_launch(ctx, "container_table_kernel");
         if (rc != RB200_OK) return rc;
     }
-    container_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status, version);
+    // version 6 runs the STORED twins of version 1's decoders, with version 1's ids
+    container_verdict_kernel<<<1, 32, 0, s>>>(buf, out_cap, d_n_symbols, w, ctx->d_status, v6 ? kContainerVersion : version);
     rc = check_launch(ctx, "container_verdict_kernel");
     for (int i = first; i < last && rc == RB200_OK; i++) {
         const DecoderLaunch& l = ctx->async_decoders[i];
@@ -1943,6 +1961,14 @@ extern "C" int rb200_container_blocks_stored_decode_async(rb200_ctx* ctx, const 
 {
     if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
     return container_decode_async(ctx, kContainerVersionBlocksStored, buf, size, out, out_cap, d_n_symbols);
+}
+
+// Seventeen launches: version 6's checks, the table kernel and the STORED twin of every decoder variant of version 1.
+extern "C" int rb200_container_stored_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
+                                                   uint64_t* d_n_symbols)
+{
+    if (!async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    return container_decode_async(ctx, kContainerVersionStored, buf, size, out, out_cap, d_n_symbols);
 }
 
 // Thirteen launches: the checks and every block decoder variant of RB200_BLOCK_DISPATCH (versions 2, 3 and 4).
@@ -2189,6 +2215,96 @@ extern "C" int rb200_container_blocks_stored_encode_async(rb200_ctx* ctx, const 
     if (!blocks_container_args_ok(ctx, in, n_blocks, block_size, chunk_syms, out, RB200_MEM_DEVICE)) return RB200_E_ARG;
     return blocks_stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n_blocks, block_size, chunk_syms, flags, out,
                                 out_cap);
+}
+
+namespace {
+
+// rb200_container_stored_encode_async (version 6): the histogram, coder_choice_kernel and the CHOSEN model kernel of the
+// auto encode; one GATED split encoder per launch group of the list, all into one workspace of one worst-case slot per
+// chunk (slot_bytes_for does not depend on the coder), so that every stream's size is known before anything is placed;
+// chunks_store_kernel (the bitmap and the per-chunk verdicts); the scan, the tile prefix and
+// chunks_stored_compaction_kernel, ungated; the CRC of everything between the model and the blob, the optional blob CRC
+// and container_stored_finish_kernel.  The workspace: the split plan's, then the verdicts after its tile sums.
+// Arguments are checked by the caller.
+int stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags, uint8_t* out,
+                  size_t out_cap)
+{
+    const uint32_t n_chunks = static_cast<uint32_t>(rb200_chunk_count(n, chunk_syms));
+    const ContainerHeader h = container_header(static_cast<int>(a.list.pair[0] >> 8), a.list.pair[0] & 0xffu, chunk_syms, n, n_chunks, 0, flags);
+    const size_t boff = container_bitmap_blob_offset(n_chunks);
+    if (out_cap < boff) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    cudaStream_t s = ctx->stream;
+    ModelAsyncWork* w = ctx->d_model_async;
+    EncodePlan p = {};
+    p.n_chunks = n_chunks;
+    p.slots = n_chunks;
+    p.slot_bytes = slot_bytes_for(chunk_syms);
+    const size_t longs = (n_chunks + kScanTile - 1) / kScanTile + 1;
+    int rc = reserve(ctx, ctx->scratch, p.slots * p.slot_bytes + 16);
+    if (rc == RB200_OK) rc = reserve(ctx, ctx->sizes, plan_head_bytes(p) + longs * sizeof(uint64_t) + n_chunks * sizeof(uint32_t));
+    if (rc != RB200_OK) return rc;
+    uint8_t* scratch = static_cast<uint8_t*>(ctx->scratch.p);
+    uint32_t* sizes = static_cast<uint32_t*>(ctx->sizes.p);
+    uint64_t* tile_sums = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(ctx->sizes.p) + plan_head_bytes(p));
+    uint32_t* stored = reinterpret_cast<uint32_t*>(tile_sums + longs);
+    const EncodeWorkspace ws = {scratch, nullptr, nullptr, sizes, tile_sums};
+    uint64_t* dir = reinterpret_cast<uint64_t*>(out + kContainerDirOffset);
+    RB_CUDA(ctx, cudaMemsetAsync(w->counts, 0, sizeof w->counts, s));
+    launch_histogram(s, static_cast<uint32_t>(ctx->sms), in, n, w->counts, nullptr);
+    rc = check_launch(ctx, "histogram_kernel");
+    if (rc != RB200_OK) return rc;
+    coder_choice_kernel<<<1, a.list.n * 32, 0, s>>>(a.list, n_chunks, w, nullptr, ctx->d_status);
+    rc = check_launch(ctx, "coder_choice_kernel");
+    if (rc != RB200_OK) return rc;
+    container_model_kernel<false, true><<<1, kModelThreads, 0, s>>>(h.coder, h.scale_bits, word_r32_allowed() ? 1u : 0u, w, ctx->d_status);
+    rc = check_launch(ctx, "container_model_kernel");
+    for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++) {
+        EncodeTables t = workspace_tables(w, a.coder[k], a.sb[k]);
+        t.choice = &w->choice;
+        t.group = k;
+        const EncodePlan pk = plan_encode(ctx, a.coder[k], a.sb[k], n_chunks, chunk_syms, false, true);
+        rc = launch_encoder(ctx, t, pk, in, n, chunk_syms, n_chunks, ws, nullptr, 0, nullptr, nullptr);
+    }
+    if (rc != RB200_OK) return rc;
+    chunks_store_kernel<<<static_cast<uint32_t>((container_bitmap_words(n_chunks) * 32 + kChunkStoreThreads - 1) / kChunkStoreThreads),
+                          kChunkStoreThreads, 0, s>>>(sizes, n_chunks, n, chunk_syms, out, stored);
+    rc = check_launch(ctx, "chunks_store_kernel");
+    if (rc != RB200_OK) return rc;
+    // the scan and the tile prefix ungated; the compaction copies stored chunks from the input
+    const uint32_t tiles = (n_chunks + kScanTile - 1) / kScanTile;
+    scan_tiles_kernel<false><<<tiles, 1024, 0, s>>>(sizes, n_chunks, dir, tile_sums, nullptr, nullptr, 0);
+    rc = check_launch(ctx, "scan_tiles_kernel");
+    const uint32_t prefixed = tiles > kTilePrefixThreshold ? 1u : 0u;
+    if (rc == RB200_OK && prefixed) {
+        tile_prefix_kernel<false><<<1, 1024, 0, s>>>(tile_sums, tiles, nullptr, nullptr, 0);
+        rc = check_launch(ctx, "tile_prefix_kernel");
+    }
+    if (rc != RB200_OK) return rc;
+    const StoredBlocks st = {in, stored, 1, chunk_syms, n};
+    chunks_stored_compaction_kernel<<<(n_chunks + kCopyWarps - 1) / kCopyWarps, kCopyWarps * 32, 0, s>>>(
+        scratch, p.slot_bytes, sizes, dir, tile_sums, prefixed, n_chunks, out + boff, out_cap - boff, ctx->d_status, st);
+    rc = check_launch(ctx, "chunks_stored_compaction_kernel");
+    if (rc == RB200_OK) rc = launch_crc(ctx, out + kContainerDirOffset, boff - kContainerDirOffset, nullptr, 0, ctx->d_crc);
+    if (rc == RB200_OK && (flags & RB200_CONTAINER_CRC_BLOB)) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+    if (rc != RB200_OK) return rc;
+    container_stored_finish_kernel<<<1, 32, 0, s>>>(out, h, boff, out_cap, w->freqs, ctx->d_crc, ctx->d_status, &w->choice);
+    return check_launch(ctx, "container_stored_finish_kernel");
+}
+
+}  // namespace
+
+// The auto encode's choice, model and split encoders, with every chunk whose stream is longer than its symbols stored
+// verbatim (version 6).  Ten to fourteen launches and one memset, no copy, no synchronisation.
+extern "C" int rb200_container_stored_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                                   const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags, uint8_t* out,
+                                                   size_t out_cap)
+{
+    if (!candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    for (uint32_t i = 0; i < n_candidates; i++)
+        if (!model_encode_args_ok(ctx, static_cast<int>(candidates[i] >> 8), candidates[i] & 0xffu, in, n, chunk_syms, out)) return RB200_E_ARG;
+    if (n == 0) return RB200_E_MODEL;                                // normalize_freqs divides by the total
+    return stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n, chunk_syms, flags, out, out_cap);
 }
 
 extern "C" int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n)

@@ -9,6 +9,7 @@
 //   RansWordEncPut    (rans_word_sse41.h:81-93)    -> ballot + popc(mask & lanemask_gt),
 //                                                     exact division by reciprocal multiply
 #pragma once
+#include "container_format.h"
 #include "device_utils.cuh"
 #include "encode_ring.cuh"
 #include "encode_stream.cuh"
@@ -600,17 +601,21 @@ constexpr int kCopyWarps = 8;
 constexpr uint32_t kTilePrefixThreshold = 256;   // above this many tiles, tile_prefix_kernel runs first
 
 // The blocks rb200_container_blocks_stored_encode_async stores: the input, chunks of chunk_syms symbols, per_block to a
-// block, and blocks_store_kernel's verdict per block (nonzero: stored).
+// block, and blocks_store_kernel's verdict per block (nonzero: stored).  rb200_container_stored_encode_async: one chunk
+// per "block" and chunks_store_kernel's verdicts, with the input's length n for its ragged last chunk.
 struct StoredBlocks {
     const uint8_t* in;
     const uint32_t* stored;
     uint32_t per_block, chunk_syms;
+    uint64_t n;
 };
 
 // one warp moves one chunk stream from the end of its scratch slot to blob[offsets[c]..E_c)
 // STORED (rb200_container_blocks_stored_encode_async): a chunk of a stored block is its symbols from the input instead,
-// with zero padding (place_stored); its size is already round16(chunk_syms)
-template <bool GEOM, bool GATED, bool STORED = false>
+// with zero padding (place_stored); its size is already round16(chunk_syms).  RAGGED (with STORED,
+// rb200_container_stored_encode_async): a stored chunk has m_c symbols, fewer than chunk_syms when it is the last of
+// st.n, and its size is round16(m_c); nothing at or past in + n is read.
+template <bool GEOM, bool GATED, bool STORED = false, bool RAGGED = false>
 __device__ __forceinline__ void compact(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
                                         uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
                                         uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status,
@@ -655,7 +660,8 @@ __device__ __forceinline__ void compact(const uint8_t* __restrict__ scratch, uin
     }
     if (end <= blob_cap) {
         if (STORED && st.stored[chunk / st.per_block])
-            place_stored(st.in + static_cast<uint64_t>(chunk) * st.chunk_syms, st.chunk_syms, blob + (end - size), lane);
+            place_stored(st.in + static_cast<uint64_t>(chunk) * st.chunk_syms,
+                         RAGGED ? container_chunk_symbols(chunk, st.chunk_syms, st.n) : st.chunk_syms, blob + (end - size), lane);
         else
             place_stream<false>(scratch + static_cast<uint64_t>(chunk + 1) * slot_bytes, size, blob, end, lane);
     }
@@ -679,6 +685,17 @@ compact_stored_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, 
 {
     compact<false, false, true>(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, blob, blob_cap, status, nullptr,
                                 nullptr, 0, st);
+}
+
+// the compaction of rb200_container_stored_encode_async: STORED and RAGGED, one chunk per verdict (ungated, every length
+// by value)
+__global__ void __launch_bounds__(kCopyWarps * 32)
+chunks_stored_compaction_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+                                uint64_t* __restrict__ offsets, const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed,
+                                uint32_t n_chunks, uint8_t* __restrict__ blob, uint64_t blob_cap, uint32_t* __restrict__ status, StoredBlocks st)
+{
+    compact<false, false, true, true>(scratch, slot_bytes, sizes, offsets, tile_sums, tiles_prefixed, n_chunks, blob, blob_cap, status,
+                                      nullptr, nullptr, 0, st);
 }
 
 // the K2 and K2f instances: (R32, GATED, GEOM) = (r32, 0, 0) for an rb200_model, (r32, 1, 0) and (r32, 1, 1) for the

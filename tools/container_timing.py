@@ -78,10 +78,16 @@ With --blocks-stored, rb200_container_blocks_stored_encode_async (version 5, inc
 rb200_container_blocks_stored_decode_async against rb200_container_blocks_any_decode_async on the auto container; a
 torch.profiler list of the version 5 calls' kernels.
 
+With --stored, rb200_container_stored_encode_async (version 6, incompressible chunks stored) over the --auto candidates
+against rb200_container_model_encode_auto_async on 1 GiB of uniform, p = 0.99 skewed and half-uniform / half-Zipf data,
+chunks of 8192, flags 0, alternated: bytes per symbol of both containers and the bytes after the header, encode times,
+and rb200_container_stored_decode_async against rb200_container_decode_async on the auto container; a torch.profiler
+list of the four calls' kernels.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
     python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto | --blocks-auto
-                                      | --blocks-varlen | --blocks-stored] [--reps 10]
+                                      | --blocks-varlen | --blocks-stored | --stored] [--reps 10]
                                      [--json out.json]"""
 import argparse
 import json
@@ -995,6 +1001,88 @@ def blocks_stored(args):
     return res
 
 
+def stored(args):
+    """rb200_container_stored_encode_async (version 6) over {word 12, alias 16, byte 14} (2 % tolerance) against
+    rb200_container_model_encode_auto_async, on uniform, p = 0.99 skewed and half-uniform / half-Zipf data: bytes per
+    symbol of both containers, encode times, the version 6 decode against rb200_container_decode_async on the auto
+    container, and a kernel split of all four calls"""
+    import torch
+    n, chunk, tol = 1 << 30, 8192, 20000
+    n_chunks = n // chunk
+    cands = [api.CANDIDATE(rb.CODER_WORD, 12), api.CANDIDATE(rb.CODER_ALIAS, 16), api.CANDIDATE(rb.CODER_BYTE, 14)]
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    cap = ctx.container_capacity(n, chunk)
+    bound = api.container_stored_bound(n, chunk)
+    d_auto = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+    d_st = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+    d_dec = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+    bitmap = (1088 + 8 * (n_chunks + 1) + 15) & ~15
+    v6_boff, v1_boff = bitmap + 16 * ((n_chunks + 127) // 128), bitmap
+    res = {"card": card(), "workload": {"n": n, "chunk_syms": chunk}, "candidates": ["word 12", "alias 16", "byte 14"], "tolerance_ppm": tol,
+           "bound_bytes_per_symbol": bound / n, "workloads": {}, "checks": {}}
+
+    def blob_bytes(d):
+        h = d[:64].cpu().numpy()
+        return int(h[32:40].view(np.uint64)[0]), int(h[6]), int(h[7])
+
+    def uniform(seed):
+        g = torch.Generator(device="cuda")
+        g.manual_seed(seed)
+        return torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda", generator=g)
+
+    def half(seed):
+        """runs of 3 chunks + 1000 symbols, uniform and Zipf in turn: every boundary falls inside a chunk"""
+        run = 3 * chunk + 1000
+        m = -(-n // (2 * run)) * 2 * run
+        d = zipf_data(m, seed).view(-1, 2, run)
+        g = torch.Generator(device="cuda")
+        g.manual_seed(seed + 1)
+        d[:, 0, :] = torch.randint(0, 256, (d.shape[0], run), dtype=torch.uint8, device="cuda", generator=g)
+        return d.reshape(-1)[:n]
+
+    for name, make in (("uniform", uniform), ("p = 0.99", lambda seed: skewed_data(n, seed)), ("half_uniform_zipf", half)):
+        d_in = make(4321)[:n].contiguous()
+        i, a, o = d_in.data_ptr(), d_auto.data_ptr(), d_st.data_ptr()
+        enc = {"stored_encode": lambda: ctx.container_stored_encode_async(cands, tol, i, n, chunk, 0, o, bound),
+               "auto_encode": lambda: ctx.container_model_encode_auto_async(cands, tol, i, n, chunk, 0, a, cap)}
+        times = alternate(enc, sync, args.warmup, args.reps)
+        for f in enc.values():
+            f()
+        sync()
+        st_blob, coder, sb = blob_bytes(d_st)
+        auto_blob = blob_bytes(d_auto)[0]
+        bits = d_st[bitmap:bitmap + 4 * ((n_chunks + 31) // 32)].cpu().numpy().view(np.uint32)
+        stored_chunks = int(sum(bin(int(w)).count("1") for w in bits))
+        res["checks"][f"{name}: stored_container_within_bound"] = v6_boff + st_blob <= bound
+        if stored_chunks == 0:
+            res["checks"][f"{name}: nothing_stored_blob_equals_auto"] = bool(
+                torch.equal(d_st[v6_boff:v6_boff + st_blob], d_auto[v1_boff:v1_boff + auto_blob]))
+        dec = {"stored_decode_async": lambda: ctx.container_stored_decode_async(o, bound, d_dec.data_ptr(), n),
+               "decode_async_on_auto": lambda: ctx.container_decode_async(a, cap, d_dec.data_ptr(), n)}
+        dtimes = alternate(dec, sync, args.warmup, args.reps)
+        for k, f in dec.items():
+            d_dec.zero_()
+            f()
+            sync()
+            res["checks"][f"{name}: {k}_round_trip"] = bool(torch.equal(d_dec[:n], d_in[:n]))
+        res["workloads"][name] = {
+            "chosen": {"coder": coder, "scale_bits": sb}, "stored_chunks": stored_chunks, "n_chunks": n_chunks,
+            "bytes_per_symbol": {"stored": (v6_boff + st_blob) / n, "auto": (v1_boff + auto_blob) / n},
+            "bytes_after_header": {"stored": v6_boff + st_blob - 64, "auto": v1_boff + auto_blob - 64},
+            "encode": times, "stored_minus_auto_encode_median_us": 1e3 * (times["stored_encode"]["median_ms"] - times["auto_encode"]["median_ms"]),
+            "decode": dtimes,
+            "stored_minus_v1_decode_median_us": 1e3 * (dtimes["stored_decode_async"]["median_ms"] - dtimes["decode_async_on_auto"]["median_ms"]),
+            "stored_encode_kernels": kernel_times(enc["stored_encode"], sync, args.reps),
+            "auto_encode_kernels": kernel_times(enc["auto_encode"], sync, args.reps),
+            "stored_decode_kernels": kernel_times(dec["stored_decode_async"], sync, args.reps),
+            "v1_decode_kernels": kernel_times(dec["decode_async_on_auto"], sync, args.reps),
+        }
+        del d_in
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
@@ -1006,13 +1094,14 @@ def main():
     ap.add_argument("--blocks-auto", action="store_true", help="the per-block model-building encode with the coder chosen on the GPU")
     ap.add_argument("--blocks-varlen", action="store_true", help="the per-block auto encode with the block count in device memory")
     ap.add_argument("--blocks-stored", action="store_true", help="the per-block encode and decode with incompressible blocks stored (version 5)")
+    ap.add_argument("--stored", action="store_true", help="the single-model encode and decode with incompressible chunks stored (version 6)")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
