@@ -376,6 +376,22 @@ int rb200_container_blocks_stored_open(const uint8_t* buf, size_t size, rb200_co
 int rb200_container_blocks_stored_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
                                                const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
                                                uint32_t flags, uint8_t* out, size_t out_cap);
+/* rb200_container_blocks_stored_encode_async with the block count read from device memory when the work runs: for
+ * 1 <= *d_n_blocks <= n_blocks_max the container is byte for byte (header included) what the fixed call writes for
+ * n_blocks = *d_n_blocks, so one captured graph writes a bounded container of any count up to n_blocks_max.  Only the
+ * first *d_n_blocks blocks of in are read and nothing at or past the container's end is written.  n_blocks_max fixes
+ * the launch shapes and the workspace; the bound grows with the count, so out_cap >=
+ * rb200_container_blocks_stored_bound(n_blocks_max, block_size, chunk_syms) means rb200_sync never returns
+ * RB200_E_SPACE, whatever the count.  The call returns RB200_E_ARG (nothing launched) for everything the fixed call
+ * refuses, checked with n_blocks_max, for a null or not 4-byte aligned d_n_blocks and for n_blocks_max == 0;
+ * RB200_E_SPACE when out_cap is below the blob offset for n_blocks_max.  rb200_sync returns RB200_E_ARG when
+ * *d_n_blocks is 0 or above n_blocks_max, and then out is not written at all; every other verdict is the fixed call's,
+ * with the header unwritten on every error.  The call only enqueues work (no copy, synchronisation or allocation); the
+ * workspace grows for n_blocks_max, so a call with the same list, geometry and bound outside a capture must come first. */
+int rb200_container_blocks_stored_encode_varlen_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                      uint32_t tolerance_ppm, const uint8_t* in, const uint32_t* d_n_blocks,
+                                                      uint32_t n_blocks_max, uint32_t block_size, uint32_t chunk_syms,
+                                                      uint32_t flags, uint8_t* out, size_t out_cap);
 /* The contract of rb200_container_blocks_alias_decode_async with version 5 in place of version 4: kernels check the
  * header, every row (zero or summing), the directory, every stored chunk's step and padding, meta_crc and the optional
  * blob CRC, then the block decoder of the header's pair runs, copying stored blocks and decoding the others.  DEVICE
@@ -422,6 +438,21 @@ int rb200_container_stored_open(const uint8_t* buf, size_t size, struct rb200_co
  * call with the same list and geometry outside the capture. */
 int rb200_container_stored_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
                                         const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap);
+/* rb200_container_stored_encode_async with the length read from device memory when the work runs: for
+ * 1 <= *d_n <= n_max the container is byte for byte (header included) what the fixed call writes for n = *d_n, so one
+ * captured graph writes a bounded container of any length up to n_max.  Only the first *d_n symbols of in are read
+ * and nothing at or past the container's end is written.  n_max fixes the launch shapes and the workspace; the bound
+ * grows with the length, so out_cap >= rb200_container_stored_bound(n_max, chunk_syms) means rb200_sync never returns
+ * RB200_E_SPACE, whatever the length.  d_n is device memory, 8-byte aligned.  The call returns RB200_E_ARG (nothing
+ * launched) for everything the fixed call refuses, checked with n_max and for every candidate, for a null or misaligned
+ * d_n and for n_max == 0; RB200_E_SPACE when out_cap is below the blob offset for n_max.  rb200_sync returns
+ * RB200_E_MODEL for *d_n == 0 (the fixed call's verdict for n == 0) and RB200_E_ARG for *d_n > n_max, and then out is
+ * not written at all; every other verdict is the fixed call's, with the header unwritten on every error.  The call only
+ * enqueues work (no copy, synchronisation or allocation); the workspace grows for n_max, so a call with the same list,
+ * chunk_syms and n_max outside a capture must come first. */
+int rb200_container_stored_encode_varlen_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                               uint32_t tolerance_ppm, const uint8_t* in, const uint64_t* d_n, size_t n_max,
+                                               uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap);
 /* The contract of rb200_container_decode_async with version 6 in place of version 1: kernels check the header, the
  * model, the directory, the bitmap, every stored chunk's step and padding, meta_crc and the optional blob CRC; then the
  * decoder of the header's coder runs, copying stored chunks and decoding the others.  rb200_sync gives RB200_E_STREAM

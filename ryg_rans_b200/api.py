@@ -110,6 +110,11 @@ EXPORTS = [
     ("rb200_container_stored_encode_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_uint32,
                                                       C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_container_stored_decode_async", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_container_stored_encode_varlen_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                             C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_container_blocks_stored_encode_varlen_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                                    C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
+                                                                    C.c_size_t]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -622,6 +627,16 @@ class Context:
         self.lib.check(self.lib.dll.rb200_container_stored_encode_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
                                                                         in_ptr, n, chunk_syms, flags, out_ptr, out_cap), self.h)
 
+    def container_stored_encode_varlen_async(self, candidates, tolerance_ppm, in_ptr, n_ptr, n_max, chunk_syms, flags, out_ptr, out_cap):
+        """container_stored_encode_async with the length read from device memory when the work runs: n_ptr is the device
+        address of a u64 n, 1 <= n <= n_max.  n_max fixes the launch shapes and the workspace, so one captured call serves
+        every such n, and out_cap = container_stored_bound(n_max, chunk_syms) holds every one.  The verdict (-2 for n == 0,
+        -1 for n > n_max, both with out untouched; otherwise as container_stored_encode_async) comes from sync()"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_stored_encode_varlen_async(self.h, cands.ctypes.data_as(_u32p), cands.size,
+                                                                               tolerance_ppm, in_ptr, n_ptr, n_max, chunk_syms, flags,
+                                                                               out_ptr, out_cap), self.h)
+
     def container_stored_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
         """the async decode of a version 6 container; enqueue only (CUDA-graph capturable).  The verdict (-4 corrupt or
         another version, -3 out_cap too small, output untouched) comes from sync()"""
@@ -907,6 +922,19 @@ class Context:
         self.lib.check(self.lib.dll.rb200_container_blocks_stored_encode_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
                                                                                in_ptr, n_blocks, block_size, chunk_syms, flags, out_ptr,
                                                                                out_cap), self.h)
+
+    def container_blocks_stored_encode_varlen_async(self, candidates, tolerance_ppm, in_ptr, n_blocks_ptr, n_blocks_max, block_size,
+                                                    chunk_syms, flags, out_ptr, out_cap):
+        """container_blocks_stored_encode_async with the block count read from device memory when the work runs:
+        n_blocks_ptr is the device address of a u32 count, 1 <= count <= n_blocks_max.  n_blocks_max fixes the launch
+        shapes and the workspace, so one captured call serves every such count, and out_cap =
+        container_blocks_stored_bound(n_blocks_max, ...) holds every one.  The verdict (-1 for a count of 0 or above
+        n_blocks_max, with out untouched; otherwise as container_blocks_stored_encode_async) comes from sync()"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_blocks_stored_encode_varlen_async(self.h, cands.ctypes.data_as(_u32p), cands.size,
+                                                                                      tolerance_ppm, in_ptr, n_blocks_ptr, n_blocks_max,
+                                                                                      block_size, chunk_syms, flags, out_ptr, out_cap),
+                       self.h)
 
     def container_blocks_stored_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
         """the async decode of a version 5 container; enqueue only (CUDA-graph capturable).  The verdict (-4 corrupt or

@@ -427,14 +427,15 @@ block_decode_kernel(const uint8_t* __restrict__ blob, uint64_t blob_size, const 
     }
 
 // The split encoder instance of (CODER, SB): (BUILD, GATED, GEOM) = (build, 0, 0) for the fixed calls, (1, 1, 0) for the
-// auto and the stored encodes, (1, 1, 1) for the device-count encode.  The word coder has only (0, 0, 0) and (1, 1, 0),
-// null for any other flags: its other model-building encodes run K5f (plan_blocks_encode).
+// auto and the stored encodes, (1, 1, 1) for the device-count encodes.  The word coder has only (0, 0, 0), (1, 1, 0) and
+// (1, 1, 1) (the stored encodes'), null for any other flags: its other model-building encodes run K5f (plan_blocks_encode).
 using BlockEncodeKernel = decltype(&block_coder_encode_kernel<RB200_CODER_BYTE, 0, false>);
 template <uint32_t CODER, uint32_t SB>
 inline BlockEncodeKernel block_encode_for(bool build, bool gated, bool geom)
 {
     if constexpr (CODER == RB200_CODER_WORD)
-        return gated && !geom ? block_coder_encode_kernel<CODER, SB, true, true> : build || geom ? nullptr : block_coder_encode_kernel<CODER, SB, false>;
+        return gated ? (geom ? block_coder_encode_kernel<CODER, SB, true, true, true> : block_coder_encode_kernel<CODER, SB, true, true>)
+                     : build || geom ? nullptr : block_coder_encode_kernel<CODER, SB, false>;
     else if (geom) return block_coder_encode_kernel<CODER, SB, true, true, true>;
     else if (gated) return block_coder_encode_kernel<CODER, SB, true, true>;
     else return build ? block_coder_encode_kernel<CODER, SB, true> : block_coder_encode_kernel<CODER, SB, false>;

@@ -381,4 +381,31 @@ __global__ void __launch_bounds__(32)
     container_finish<false, true, true>(out, h, kContainerDirOffset, blob_off, out_cap, freqs, slots, status, nullptr, choice);
 }
 
+// The GEOM header kernels of the two device-size stored encodes: n_symbols, n_chunks (version 5: n_blocks and the
+// directory's place too) and the blob offset from the record; h arrives with the bound's geometry, chunk_syms and flags.
+// Write nothing when the plan failed.
+__global__ void __launch_bounds__(32)
+    container_blocks_stored_finish_varlen_kernel(uint8_t* out, ContainerHeader h, uint64_t out_cap, const CrcSlot* __restrict__ slots,
+                                                 uint32_t* status, const BlocksChoice* __restrict__ r, const BlocksVarlenGeom* __restrict__ geom)
+{
+    if (!geom->v.go) return;
+    h.version = kContainerVersionBlocksStored;
+    h.n_blocks = geom->n_blocks;
+    h.n_symbols = geom->v.n;
+    h.n_chunks = geom->v.n_chunks;
+    container_finish<false, true>(out, h, geom->v.dir_off, geom->v.blob_off, out_cap, nullptr, slots, status, nullptr, &r->choice);
+}
+
+__global__ void __launch_bounds__(32)
+    container_stored_finish_varlen_kernel(uint8_t* out, ContainerHeader h, uint64_t out_cap, const uint32_t* __restrict__ freqs,
+                                          const CrcSlot* __restrict__ slots, uint32_t* status, const CoderChoice* __restrict__ choice,
+                                          const StoredVarlenGeom* __restrict__ geom)
+{
+    if (!geom->v.go) return;
+    h.version = kContainerVersionStored;
+    h.n_symbols = geom->v.n;
+    h.n_chunks = geom->v.n_chunks;
+    container_finish<false, true, true>(out, h, kContainerDirOffset, geom->v.blob_off, out_cap, freqs, slots, status, nullptr, choice);
+}
+
 }  // namespace rb200

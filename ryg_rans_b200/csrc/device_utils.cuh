@@ -41,6 +41,15 @@ struct BlocksVarlenGeom {
     uint32_t reserved;
 };
 
+// The geometry of rb200_container_stored_encode_varlen_async (version 6), which reads the input length from device
+// memory: written by stored_varlen_plan_kernel (model_kernels.cuh) from *d_n at every run.  v is the VarlenGeom of the
+// container's symbols and chunks with v.blob_off past the stored-chunk bitmap (container_bitmap_blob_offset), so the
+// GEOM instances of C5 read it as they are; the meta CRC's length follows it.
+struct StoredVarlenGeom {
+    VarlenGeom v;
+    uint64_t meta_len;     // v.blob_off - 1088: directory, pad and bitmap, the bytes the meta CRC's kernel covers
+};
+
 // The choice of rb200_container_model_encode_auto_async: written by coder_choice_kernel (model_kernels.cuh) at every
 // run, read by the CHOSEN / GATED instances after it.  The host launches one gated group of encode kernels per distinct
 // encoder instance the candidate list needs; only the group named here runs, the others exit at entry.

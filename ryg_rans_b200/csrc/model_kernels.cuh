@@ -43,6 +43,11 @@
 // rb200_container_stored_encode_async (version 6) runs the histogram, the choice and the CHOSEN model kernel of the auto
 // encode, then one GATED split encoder per group into one workspace, chunks_store_kernel, which stores every chunk whose
 // stream is longer than its symbols and writes the bitmap, one ungated scan and chunks_stored_compaction_kernel.
+//
+// rb200_container_stored_encode_varlen_async and rb200_container_blocks_stored_encode_varlen_async run those two on
+// launch shapes sized for the bound: stored_varlen_plan_kernel (StoredVarlenGeom, device_utils.cuh) or
+// blocks_varlen_plan_kernel reads the size, and every later kernel is the GEOM instance of the same stage
+// (chunks_store_varlen_kernel, blocks_store_varlen_kernel and the *_varlen_kernel compactions and header kernels).
 #pragma once
 #include "block_kernels.cuh"
 #include "container_format.h"
@@ -296,12 +301,16 @@ __global__ void __launch_bounds__(32) blocks_one_pair_kernel(uint32_t pair, Bloc
 // container is zeroed, every chunk's size becomes round16(chunk_syms), and stored[block] = 1 has the compaction copy
 // the chunk's symbols in place of its stream; otherwise stored[block] = 0.  Stream sizes stay below 2^26 (a slot), so
 // a block's sum fits 32 bits.
+// GEOM (rb200_container_blocks_stored_encode_varlen_async): on the grid of n_blocks_max, the count from the record
+// (BlocksVarlenGeom, 0 when the plan failed); the models stay at out + 64, so nothing else moves.
 constexpr int kStoreWarps = 8;
 
-__global__ void __launch_bounds__(kStoreWarps * 32)
-    blocks_store_kernel(uint32_t* __restrict__ sizes, uint32_t n_blocks, uint32_t per_block, uint32_t chunk_syms, uint16_t* __restrict__ models,
-                        uint32_t* __restrict__ stored)
+template <bool GEOM>
+__device__ __forceinline__ void blocks_store(uint32_t* __restrict__ sizes, uint32_t n_blocks, uint32_t per_block, uint32_t chunk_syms,
+                                             uint16_t* __restrict__ models, uint32_t* __restrict__ stored,
+                                             const BlocksVarlenGeom* __restrict__ geom)
 {
+    if (GEOM) n_blocks = geom->n_blocks;
     const uint32_t lane = threadIdx.x & 31, block = blockIdx.x * kStoreWarps + (threadIdx.x >> 5);
     if (block >= n_blocks) return;                               // the same for the whole warp
     const uint32_t raw = static_cast<uint32_t>(container_stored_bytes(chunk_syms));
@@ -314,18 +323,41 @@ __global__ void __launch_bounds__(kStoreWarps * 32)
     reinterpret_cast<uint4*>(models + static_cast<uint64_t>(block) * 256)[lane] = make_uint4(0, 0, 0, 0);   // 32 x 16 bytes
 }
 
+__global__ void __launch_bounds__(kStoreWarps * 32)
+    blocks_store_kernel(uint32_t* __restrict__ sizes, uint32_t n_blocks, uint32_t per_block, uint32_t chunk_syms, uint16_t* __restrict__ models,
+                        uint32_t* __restrict__ stored)
+{
+    blocks_store<false>(sizes, n_blocks, per_block, chunk_syms, models, stored, nullptr);
+}
+
+__global__ void __launch_bounds__(kStoreWarps * 32)
+    blocks_store_varlen_kernel(uint32_t* __restrict__ sizes, uint32_t per_block, uint32_t chunk_syms, uint16_t* __restrict__ models,
+                               uint32_t* __restrict__ stored, const BlocksVarlenGeom* __restrict__ geom)
+{
+    blocks_store<true>(sizes, 0, per_block, chunk_syms, models, stored, geom);
+}
+
 // The store rule of rb200_container_stored_encode_async (version 6), one thread per chunk, after the encoder wrote every
 // chunk's stream size to sizes[]: chunk c is stored when its stream, rounded up to 16 as the compaction places it, is
 // longer than round16(m_c), its symbols' stored size; ties stay coded.  A stored chunk's size becomes round16(m_c) and
 // stored[c] = 1 has the compaction copy its symbols in place of its stream; otherwise stored[c] = 0.  Each warp's ballot
 // is one word of the container's bitmap: the grid covers the padding words too, which it writes zero, and thread 0
 // zeroes the pad between the directory and the bitmap, both of which meta_crc covers.
+// GEOM (rb200_container_stored_encode_varlen_async): on the grid of n_max's bitmap words, n and the chunk count from the
+// record (VarlenGeom); the bitmap's place and its words follow that count, and the CTAs past its words exit at entry,
+// so nothing is written for the bound's extra words.  Every CTA exits when the plan failed.
 constexpr int kChunkStoreThreads = 256;
 
-__global__ void __launch_bounds__(kChunkStoreThreads)
-    chunks_store_kernel(uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t n, uint32_t chunk_syms, uint8_t* __restrict__ out,
-                        uint32_t* __restrict__ stored)
+template <bool GEOM>
+__device__ __forceinline__ void chunks_store(uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t n, uint32_t chunk_syms,
+                                             uint8_t* __restrict__ out, uint32_t* __restrict__ stored, const VarlenGeom* __restrict__ geom)
 {
+    if (GEOM) {
+        if (!geom->go) return;
+        n_chunks = geom->n_chunks;
+        n = geom->n;
+        if (static_cast<uint64_t>(blockIdx.x) * kChunkStoreThreads >= container_bitmap_words(n_chunks) * 32) return;
+    }
     const uint64_t c = static_cast<uint64_t>(blockIdx.x) * kChunkStoreThreads + threadIdx.x;
     bool store = false;
     if (c < n_chunks) {
@@ -338,6 +370,20 @@ __global__ void __launch_bounds__(kChunkStoreThreads)
     const uint64_t bitmap = container_bitmap_offset(n_chunks), dir_end = kContainerDirOffset + (n_chunks + 1) * sizeof(uint64_t);
     if ((threadIdx.x & 31) == 0 && c / 32 < container_bitmap_words(n_chunks)) reinterpret_cast<uint32_t*>(out + bitmap)[c / 32] = word;
     if (c == 0 && bitmap > dir_end) *reinterpret_cast<uint64_t*>(out + dir_end) = 0;
+}
+
+__global__ void __launch_bounds__(kChunkStoreThreads)
+    chunks_store_kernel(uint32_t* __restrict__ sizes, uint32_t n_chunks, uint64_t n, uint32_t chunk_syms, uint8_t* __restrict__ out,
+                        uint32_t* __restrict__ stored)
+{
+    chunks_store<false>(sizes, n_chunks, n, chunk_syms, out, stored, nullptr);
+}
+
+__global__ void __launch_bounds__(kChunkStoreThreads)
+    chunks_store_varlen_kernel(uint32_t* __restrict__ sizes, uint32_t chunk_syms, uint8_t* __restrict__ out, uint32_t* __restrict__ stored,
+                               const VarlenGeom* __restrict__ geom)
+{
+    chunks_store<true>(sizes, 0, 0, chunk_syms, out, stored, geom);
 }
 
 // The first kernel of rb200_container_model_encode_varlen_async, one warp: reads n = *d_n, checks 1 <= n <= n_max
@@ -365,6 +411,34 @@ __global__ void __launch_bounds__(32)
         r.go = 1;
     }
     *g = r;
+}
+
+// The first kernel of rb200_container_stored_encode_varlen_async, one warp: varlen_plan_kernel's checks and verdicts,
+// with the geometry of a version 6 container of n symbols (the blob after the stored-chunk bitmap, the meta CRC over
+// directory, pad and bitmap) written into *g.  The same VarlenGeom goes to *model_geom, the record the GEOM model
+// kernel reads its gate from (ModelAsyncWork::geom).  On failure both are zero.
+__global__ void __launch_bounds__(32)
+    stored_varlen_plan_kernel(const uint64_t* __restrict__ d_n, uint64_t n_max, uint32_t chunk_syms, uint64_t out_cap,
+                              StoredVarlenGeom* __restrict__ g, VarlenGeom* __restrict__ model_geom, uint32_t* __restrict__ status)
+{
+    if (threadIdx.x) return;
+    const uint64_t n = *d_n;
+    StoredVarlenGeom r = {};
+    if (n == 0 || n > n_max) {
+        atomicOr(status, n == 0 ? kStatModel : kStatArg);
+    } else {
+        const uint64_t chunks = n / chunk_syms + (n % chunk_syms != 0);
+        r.v.n = n;
+        r.v.n_chunks = static_cast<uint32_t>(chunks);
+        r.v.dir_len = (chunks + 1) * sizeof(uint64_t);
+        r.v.dir_off = kContainerDirOffset;
+        r.v.blob_off = container_bitmap_blob_offset(chunks);
+        r.v.blob_cap = out_cap - r.v.blob_off;
+        r.meta_len = r.v.blob_off - kContainerDirOffset;
+        r.v.go = 1;
+    }
+    *g = r;
+    *model_geom = r.v;
 }
 
 // After the encoder, one thread: blob_len = the directory's last entry, the length of the blob CRC (crc32_kernel's

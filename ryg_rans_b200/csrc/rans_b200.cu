@@ -76,6 +76,8 @@ struct rb200_ctx {
     BlocksChoice* d_blocks_choice = nullptr;
     // rb200_container_blocks_model_encode_varlen_async: the geometry of the count its plan kernel read
     BlocksVarlenGeom* d_blocks_geom = nullptr;
+    // rb200_container_stored_encode_varlen_async: the geometry of the length its plan kernel read
+    StoredVarlenGeom* d_stored_geom = nullptr;
 };
 
 struct rb200_model {
@@ -247,6 +249,8 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_choice, 0, sizeof(BlocksChoice));
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_blocks_geom, sizeof(BlocksVarlenGeom));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_geom, 0, sizeof(BlocksVarlenGeom));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_stored_geom, sizeof(StoredVarlenGeom));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_stored_geom, 0, sizeof(StoredVarlenGeom));
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -285,6 +289,7 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->d_async_any) cudaFree(ctx->d_async_any);
     if (ctx->d_blocks_choice) cudaFree(ctx->d_blocks_choice);
     if (ctx->d_blocks_geom) cudaFree(ctx->d_blocks_geom);
+    if (ctx->d_stored_geom) cudaFree(ctx->d_stored_geom);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -459,7 +464,8 @@ namespace {
 // directory + compaction after any encode kernel: sizes[] -> offsets[] + blob.  geom set: the GEOM instances, on grids
 // sized for n_chunks (the bound's), with d_blob the container, in which they find the directory and the blob from the
 // record (d_offsets unused).  choice set: the GATED instances, which run only when the record names `group`.  stored
-// set (the stored encode, ungated): compact_stored_kernel, which copies the stored blocks' chunks from the input.
+// set (the stored encode, ungated): compact_stored_kernel, which copies the stored blocks' chunks from the input
+// (with geom: compact_stored_varlen_kernel).
 int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* sizes, uint64_t* tile_sums, uint32_t n_chunks,
                   uint8_t* d_blob, size_t blob_cap, uint64_t* d_offsets, const VarlenGeom* geom, const CoderChoice* choice, uint32_t group,
                   const StoredBlocks* stored = nullptr)
@@ -484,6 +490,11 @@ int finish_encode(rb200_ctx* ctx, uint8_t* scratch, uint32_t slot, uint32_t* siz
         if (rc != RB200_OK) return rc;
     }
     const uint32_t grid = (n_chunks + kCopyWarps - 1) / kCopyWarps;
+    if (stored && geom) {
+        compact_stored_varlen_kernel<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, tile_sums, prefixed, d_blob, ctx->d_status,
+                                                                                geom, *stored);
+        return check_launch(ctx, "compact_stored_varlen_kernel");
+    }
     if (stored) {
         compact_stored_kernel<<<grid, kCopyWarps * 32, 0, ctx->stream>>>(scratch, slot, sizes, d_offsets, tile_sums, prefixed, n_chunks, d_blob,
                                                                          blob_cap, ctx->d_status, *stored);
@@ -1238,7 +1249,7 @@ int blocks_encode_device(rb200_ctx* ctx, int coder, uint32_t sb, const uint8_t* 
 {
     if (static_cast<uint64_t>(n_blocks) * (block_size / chunk_syms) >= (1ull << 31)) return RB200_E_ARG;
     const EncodePlan p = plan_blocks_encode(ctx, coder, sb, n_blocks, block_size, chunk_syms, build_models);
-    // the word coder's split encoder has no model-building, GATED or GEOM instance
+    // the word coder's model-building encodes run K5f: its split GATED and GEOM instances serve the stored encodes only
     if (!p.fused && coder == RB200_CODER_WORD && (build_models || choice || geom)) return RB200_E_ARG;
     return run_encode(ctx, p, d_blob, blob_cap, d_offsets, geom ? &geom->v : nullptr, [&](const EncodeWorkspace& ws) {
         if (p.fused) {
@@ -2149,9 +2160,12 @@ namespace {
 // worst-case slot per chunk (slot_bytes_for does not depend on the coder), so that every stream's size is known before
 // anything is placed; blocks_store_kernel; the scan, the tile prefix and compact_stored_kernel, ungated; the model +
 // directory CRC, the optional blob CRC and container_blocks_stored_finish_kernel (version 5).  The workspace: the split plan's, then the
-// per-block verdicts after its tile sums.  Arguments are checked by the caller.
-int blocks_stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, uint32_t n_blocks, uint32_t block_size, uint32_t chunk_syms,
-                         uint32_t flags, uint8_t* out, size_t out_cap)
+// per-block verdicts after its tile sums.  d_n_blocks set (rb200_container_blocks_stored_encode_varlen_async): n_blocks
+// is the bound n_blocks_max, which sizes the workspace and every launch; blocks_varlen_plan_kernel reads *d_n_blocks into
+// the record at every run (for one candidate it also writes the choice record), and every later kernel is its GEOM
+// instance.  Arguments are checked by the caller.
+int blocks_stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, uint32_t n_blocks, const uint32_t* d_n_blocks,
+                         uint32_t block_size, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
 {
     const ContainerHeader h = container_blocks_header(n_blocks, block_size, chunk_syms, 0, flags);
     const size_t dir_off = container_dir_offset(h), dir_end = container_dir_end(h), boff = container_blob_offset(h);
@@ -2159,6 +2173,7 @@ int blocks_stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, u
     DeviceGuard g(ctx->device);
     cudaStream_t s = ctx->stream;
     BlocksChoice* r = ctx->d_blocks_choice;
+    BlocksVarlenGeom* geom = d_n_blocks ? ctx->d_blocks_geom : nullptr;
     const uint32_t per_block = block_size / chunk_syms, n_chunks = static_cast<uint32_t>(h.n_chunks);
     EncodePlan p = {};
     p.n_chunks = n_chunks;
@@ -2175,30 +2190,56 @@ int blocks_stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, u
     uint32_t* stored = reinterpret_cast<uint32_t*>(tile_sums + longs);
     uint16_t* model = reinterpret_cast<uint16_t*>(out + sizeof(ContainerHeader));
     uint64_t* dir = reinterpret_cast<uint64_t*>(out + dir_off);
-    if (a.list.n == 1) {
+    const bool one = a.list.n == 1;
+    if (!one) RB_CUDA(ctx, cudaMemsetAsync(&r->done, 0, sizeof(BlocksChoice) - offsetof(BlocksChoice, done), s));
+    if (geom) {
+        blocks_varlen_plan_kernel<<<1, 32, 0, s>>>(d_n_blocks, n_blocks, block_size, chunk_syms, out_cap, one ? a.list.pair[0] : 0u, geom, r,
+                                                   ctx->d_status);
+        rc = check_launch(ctx, "blocks_varlen_plan_kernel");
+    } else if (one) {
         blocks_one_pair_kernel<<<1, 32, 0, s>>>(a.list.pair[0], r);
         rc = check_launch(ctx, "blocks_one_pair_kernel");
-    } else {
-        RB_CUDA(ctx, cudaMemsetAsync(&r->done, 0, sizeof(BlocksChoice) - offsetof(BlocksChoice, done), s));
-        blocks_choice_kernel<false><<<n_blocks, kBlocksChoiceWarps * 32, 0, s>>>(a.list, in, block_size, chunk_syms, r, ctx->d_status, nullptr);
+    }
+    if (rc == RB200_OK && !one) {
+        auto choice = geom ? blocks_choice_kernel<true> : blocks_choice_kernel<false>;
+        choice<<<n_blocks, kBlocksChoiceWarps * 32, 0, s>>>(a.list, in, block_size, chunk_syms, r, ctx->d_status, geom);
         rc = check_launch(ctx, "blocks_choice_kernel");
     }
     for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++) {
         launch_block_encode(s, static_cast<uint32_t>(a.coder[k]), a.sb[k], true, n_blocks, p.threads,
                             block_coder_encode_smem(static_cast<uint32_t>(a.coder[k]), a.sb[k], p.threads), in, block_size, model, chunk_syms,
-                            scratch, p.slot_bytes, sizes, ctx->d_status, &r->choice, k);
+                            scratch, p.slot_bytes, sizes, ctx->d_status, &r->choice, k, geom);
         rc = check_launch(ctx, "block_coder_encode_kernel");
     }
     if (rc != RB200_OK) return rc;
-    blocks_store_kernel<<<(n_blocks + kStoreWarps - 1) / kStoreWarps, kStoreWarps * 32, 0, s>>>(sizes, n_blocks, per_block, chunk_syms, model,
-                                                                                                stored);
-    rc = check_launch(ctx, "blocks_store_kernel");
+    const uint32_t store_grid = (n_blocks + kStoreWarps - 1) / kStoreWarps;
+    if (geom) {
+        blocks_store_varlen_kernel<<<store_grid, kStoreWarps * 32, 0, s>>>(sizes, per_block, chunk_syms, model, stored, geom);
+        rc = check_launch(ctx, "blocks_store_varlen_kernel");
+    } else {
+        blocks_store_kernel<<<store_grid, kStoreWarps * 32, 0, s>>>(sizes, n_blocks, per_block, chunk_syms, model, stored);
+        rc = check_launch(ctx, "blocks_store_kernel");
+    }
     const StoredBlocks st = {in, stored, per_block, chunk_syms};
     if (rc == RB200_OK)
-        rc = finish_encode(ctx, scratch, p.slot_bytes, sizes, tile_sums, n_chunks, out + boff, out_cap - boff, dir, nullptr, nullptr, 0, &st);
-    if (rc == RB200_OK) rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), nullptr, 0, ctx->d_crc);
-    if (rc == RB200_OK && (flags & RB200_CONTAINER_CRC_BLOB)) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+        rc = geom ? finish_encode(ctx, scratch, p.slot_bytes, sizes, tile_sums, n_chunks, out, out_cap, nullptr, &geom->v, nullptr, 0, &st)
+                  : finish_encode(ctx, scratch, p.slot_bytes, sizes, tile_sums, n_chunks, out + boff, out_cap - boff, dir, nullptr, nullptr, 0, &st);
+    if (rc == RB200_OK)
+        rc = launch_crc(ctx, out + sizeof(ContainerHeader), dir_end - sizeof(ContainerHeader), geom ? &geom->meta_len : nullptr, 0, ctx->d_crc);
+    if (rc == RB200_OK && (flags & RB200_CONTAINER_CRC_BLOB)) {
+        if (geom) {
+            varlen_blob_len_kernel<<<1, 32, 0, s>>>(out, &geom->v);
+            rc = check_launch(ctx, "varlen_blob_len_kernel");
+            if (rc == RB200_OK) rc = launch_crc(ctx, out, out_cap, &geom->v.blob_len, 0, ctx->d_crc + 1, &geom->v.blob_off);
+        } else {
+            rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+        }
+    }
     if (rc != RB200_OK) return rc;
+    if (geom) {
+        container_blocks_stored_finish_varlen_kernel<<<1, 32, 0, s>>>(out, h, out_cap, ctx->d_crc, ctx->d_status, r, geom);
+        return check_launch(ctx, "container_blocks_stored_finish_varlen_kernel");
+    }
     container_blocks_stored_finish_kernel<<<1, 32, 0, s>>>(out, h, dir_off, boff, out_cap, ctx->d_crc, ctx->d_status, r);
     return check_launch(ctx, "container_blocks_stored_finish_kernel");
 }
@@ -2213,8 +2254,23 @@ extern "C" int rb200_container_blocks_stored_encode_async(rb200_ctx* ctx, const 
 {
     if (!blocks_candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
     if (!blocks_container_args_ok(ctx, in, n_blocks, block_size, chunk_syms, out, RB200_MEM_DEVICE)) return RB200_E_ARG;
-    return blocks_stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n_blocks, block_size, chunk_syms, flags, out,
-                                out_cap);
+    return blocks_stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n_blocks, nullptr, block_size, chunk_syms, flags,
+                                out, out_cap);
+}
+
+// rb200_container_blocks_stored_encode_async with the block count read from device memory at every run: the plan kernel,
+// then the same stages on launch shapes sized for n_blocks_max, each taking the count, the directory's and the blob's
+// places and the CRC lengths from the plan's record.  One candidate: the plan kernel writes the choice record.
+extern "C" int rb200_container_blocks_stored_encode_varlen_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                                 uint32_t tolerance_ppm, const uint8_t* in, const uint32_t* d_n_blocks,
+                                                                 uint32_t n_blocks_max, uint32_t block_size, uint32_t chunk_syms,
+                                                                 uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    if (!d_n_blocks || (reinterpret_cast<uintptr_t>(d_n_blocks) & 3) || n_blocks_max == 0) return RB200_E_ARG;
+    if (!blocks_candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    if (!blocks_container_args_ok(ctx, in, n_blocks_max, block_size, chunk_syms, out, RB200_MEM_DEVICE)) return RB200_E_ARG;
+    return blocks_stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n_blocks_max, d_n_blocks, block_size, chunk_syms,
+                                flags, out, out_cap);
 }
 
 namespace {
@@ -2225,9 +2281,11 @@ namespace {
 // chunks_store_kernel (the bitmap and the per-chunk verdicts); the scan, the tile prefix and
 // chunks_stored_compaction_kernel, ungated; the CRC of everything between the model and the blob, the optional blob CRC
 // and container_stored_finish_kernel.  The workspace: the split plan's, then the verdicts after its tile sums.
-// Arguments are checked by the caller.
-int stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags, uint8_t* out,
-                  size_t out_cap)
+// d_n set (rb200_container_stored_encode_varlen_async): n is the bound n_max, which sizes the workspace and every
+// launch; stored_varlen_plan_kernel reads *d_n into the record at every run, and every later kernel is its GEOM
+// instance.  Arguments are checked by the caller.
+int stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, size_t n, const uint64_t* d_n, uint32_t chunk_syms, uint32_t flags,
+                  uint8_t* out, size_t out_cap)
 {
     const uint32_t n_chunks = static_cast<uint32_t>(rb200_chunk_count(n, chunk_syms));
     const ContainerHeader h = container_header(static_cast<int>(a.list.pair[0] >> 8), a.list.pair[0] & 0xffu, chunk_syms, n, n_chunks, 0, flags);
@@ -2236,6 +2294,8 @@ int stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, size_t n
     DeviceGuard g(ctx->device);
     cudaStream_t s = ctx->stream;
     ModelAsyncWork* w = ctx->d_model_async;
+    StoredVarlenGeom* sg = d_n ? ctx->d_stored_geom : nullptr;
+    const VarlenGeom* geom = sg ? &sg->v : nullptr;
     EncodePlan p = {};
     p.n_chunks = n_chunks;
     p.slots = n_chunks;
@@ -2250,44 +2310,79 @@ int stored_encode(rb200_ctx* ctx, const AutoPlan& a, const uint8_t* in, size_t n
     uint32_t* stored = reinterpret_cast<uint32_t*>(tile_sums + longs);
     const EncodeWorkspace ws = {scratch, nullptr, nullptr, sizes, tile_sums};
     uint64_t* dir = reinterpret_cast<uint64_t*>(out + kContainerDirOffset);
+    if (sg) {
+        stored_varlen_plan_kernel<<<1, 32, 0, s>>>(d_n, n, chunk_syms, out_cap, sg, &w->geom, ctx->d_status);
+        rc = check_launch(ctx, "stored_varlen_plan_kernel");
+        if (rc != RB200_OK) return rc;
+    }
     RB_CUDA(ctx, cudaMemsetAsync(w->counts, 0, sizeof w->counts, s));
-    launch_histogram(s, static_cast<uint32_t>(ctx->sms), in, n, w->counts, nullptr);
+    launch_histogram(s, static_cast<uint32_t>(ctx->sms), in, n, w->counts, geom);
     rc = check_launch(ctx, "histogram_kernel");
     if (rc != RB200_OK) return rc;
-    coder_choice_kernel<<<1, a.list.n * 32, 0, s>>>(a.list, n_chunks, w, nullptr, ctx->d_status);
+    coder_choice_kernel<<<1, a.list.n * 32, 0, s>>>(a.list, n_chunks, w, geom, ctx->d_status);
     rc = check_launch(ctx, "coder_choice_kernel");
     if (rc != RB200_OK) return rc;
-    container_model_kernel<false, true><<<1, kModelThreads, 0, s>>>(h.coder, h.scale_bits, word_r32_allowed() ? 1u : 0u, w, ctx->d_status);
+    auto model = geom ? container_model_kernel<true, true> : container_model_kernel<false, true>;
+    model<<<1, kModelThreads, 0, s>>>(h.coder, h.scale_bits, word_r32_allowed() ? 1u : 0u, w, ctx->d_status);
     rc = check_launch(ctx, "container_model_kernel");
     for (uint32_t k = 0; k < a.n_groups && rc == RB200_OK; k++) {
         EncodeTables t = workspace_tables(w, a.coder[k], a.sb[k]);
         t.choice = &w->choice;
         t.group = k;
         const EncodePlan pk = plan_encode(ctx, a.coder[k], a.sb[k], n_chunks, chunk_syms, false, true);
-        rc = launch_encoder(ctx, t, pk, in, n, chunk_syms, n_chunks, ws, nullptr, 0, nullptr, nullptr);
+        rc = launch_encoder(ctx, t, pk, in, n, chunk_syms, n_chunks, ws, nullptr, 0, nullptr, geom);
     }
     if (rc != RB200_OK) return rc;
-    chunks_store_kernel<<<static_cast<uint32_t>((container_bitmap_words(n_chunks) * 32 + kChunkStoreThreads - 1) / kChunkStoreThreads),
-                          kChunkStoreThreads, 0, s>>>(sizes, n_chunks, n, chunk_syms, out, stored);
-    rc = check_launch(ctx, "chunks_store_kernel");
+    const uint32_t store_grid = static_cast<uint32_t>((container_bitmap_words(n_chunks) * 32 + kChunkStoreThreads - 1) / kChunkStoreThreads);
+    if (geom) {
+        chunks_store_varlen_kernel<<<store_grid, kChunkStoreThreads, 0, s>>>(sizes, chunk_syms, out, stored, geom);
+        rc = check_launch(ctx, "chunks_store_varlen_kernel");
+    } else {
+        chunks_store_kernel<<<store_grid, kChunkStoreThreads, 0, s>>>(sizes, n_chunks, n, chunk_syms, out, stored);
+        rc = check_launch(ctx, "chunks_store_kernel");
+    }
     if (rc != RB200_OK) return rc;
-    // the scan and the tile prefix ungated; the compaction copies stored chunks from the input
+    // the scan and the tile prefix ungated; the compaction copies stored chunks from the input.  GEOM: the scan writes
+    // the directory into the container `out` at the record's place, and the prefix and the compaction use the record's
+    // tile count, whichever the host chose from the bound's
     const uint32_t tiles = (n_chunks + kScanTile - 1) / kScanTile;
-    scan_tiles_kernel<false><<<tiles, 1024, 0, s>>>(sizes, n_chunks, dir, tile_sums, nullptr, nullptr, 0);
+    auto scan = geom ? scan_tiles_kernel<true> : scan_tiles_kernel<false>;
+    scan<<<tiles, 1024, 0, s>>>(sizes, n_chunks, geom ? reinterpret_cast<uint64_t*>(out) : dir, tile_sums, geom, nullptr, 0);
     rc = check_launch(ctx, "scan_tiles_kernel");
     const uint32_t prefixed = tiles > kTilePrefixThreshold ? 1u : 0u;
     if (rc == RB200_OK && prefixed) {
-        tile_prefix_kernel<false><<<1, 1024, 0, s>>>(tile_sums, tiles, nullptr, nullptr, 0);
+        auto prefix = geom ? tile_prefix_kernel<true> : tile_prefix_kernel<false>;
+        prefix<<<1, 1024, 0, s>>>(tile_sums, tiles, geom, nullptr, 0);
         rc = check_launch(ctx, "tile_prefix_kernel");
     }
     if (rc != RB200_OK) return rc;
     const StoredBlocks st = {in, stored, 1, chunk_syms, n};
-    chunks_stored_compaction_kernel<<<(n_chunks + kCopyWarps - 1) / kCopyWarps, kCopyWarps * 32, 0, s>>>(
-        scratch, p.slot_bytes, sizes, dir, tile_sums, prefixed, n_chunks, out + boff, out_cap - boff, ctx->d_status, st);
-    rc = check_launch(ctx, "chunks_stored_compaction_kernel");
-    if (rc == RB200_OK) rc = launch_crc(ctx, out + kContainerDirOffset, boff - kContainerDirOffset, nullptr, 0, ctx->d_crc);
-    if (rc == RB200_OK && (flags & RB200_CONTAINER_CRC_BLOB)) rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+    const uint32_t copy_grid = (n_chunks + kCopyWarps - 1) / kCopyWarps;
+    if (geom) {
+        chunks_stored_compaction_varlen_kernel<<<copy_grid, kCopyWarps * 32, 0, s>>>(scratch, p.slot_bytes, sizes, tile_sums, prefixed, out,
+                                                                                     ctx->d_status, geom, st);
+        rc = check_launch(ctx, "chunks_stored_compaction_varlen_kernel");
+    } else {
+        chunks_stored_compaction_kernel<<<copy_grid, kCopyWarps * 32, 0, s>>>(scratch, p.slot_bytes, sizes, dir, tile_sums, prefixed, n_chunks,
+                                                                              out + boff, out_cap - boff, ctx->d_status, st);
+        rc = check_launch(ctx, "chunks_stored_compaction_kernel");
+    }
+    if (rc == RB200_OK)
+        rc = launch_crc(ctx, out + kContainerDirOffset, boff - kContainerDirOffset, sg ? &sg->meta_len : nullptr, 0, ctx->d_crc);
+    if (rc == RB200_OK && (flags & RB200_CONTAINER_CRC_BLOB)) {
+        if (sg) {
+            varlen_blob_len_kernel<<<1, 32, 0, s>>>(out, &sg->v);
+            rc = check_launch(ctx, "varlen_blob_len_kernel");
+            if (rc == RB200_OK) rc = launch_crc(ctx, out, out_cap, &sg->v.blob_len, 0, ctx->d_crc + 1, &sg->v.blob_off);
+        } else {
+            rc = launch_crc(ctx, out + boff, out_cap - boff, dir + n_chunks, 0, ctx->d_crc + 1);
+        }
+    }
     if (rc != RB200_OK) return rc;
+    if (sg) {
+        container_stored_finish_varlen_kernel<<<1, 32, 0, s>>>(out, h, out_cap, w->freqs, ctx->d_crc, ctx->d_status, &w->choice, sg);
+        return check_launch(ctx, "container_stored_finish_varlen_kernel");
+    }
     container_stored_finish_kernel<<<1, 32, 0, s>>>(out, h, boff, out_cap, w->freqs, ctx->d_crc, ctx->d_status, &w->choice);
     return check_launch(ctx, "container_stored_finish_kernel");
 }
@@ -2304,7 +2399,22 @@ extern "C" int rb200_container_stored_encode_async(rb200_ctx* ctx, const uint32_
     for (uint32_t i = 0; i < n_candidates; i++)
         if (!model_encode_args_ok(ctx, static_cast<int>(candidates[i] >> 8), candidates[i] & 0xffu, in, n, chunk_syms, out)) return RB200_E_ARG;
     if (n == 0) return RB200_E_MODEL;                                // normalize_freqs divides by the total
-    return stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n, chunk_syms, flags, out, out_cap);
+    return stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n, nullptr, chunk_syms, flags, out, out_cap);
+}
+
+// rb200_container_stored_encode_async with the length read from device memory at every run: the plan kernel, then the
+// same stages on launch shapes sized for n_max, each taking the length, the chunk count, the bitmap's and the blob's
+// places and the CRC lengths from the plan's record.
+extern "C" int rb200_container_stored_encode_varlen_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                          uint32_t tolerance_ppm, const uint8_t* in, const uint64_t* d_n, size_t n_max,
+                                                          uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    if (!d_n || (reinterpret_cast<uintptr_t>(d_n) & 7) || n_max == 0) return RB200_E_ARG;
+    if (!candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    for (uint32_t i = 0; i < n_candidates; i++)
+        if (!model_encode_args_ok(ctx, static_cast<int>(candidates[i] >> 8), candidates[i] & 0xffu, in, n_max, chunk_syms, out))
+            return RB200_E_ARG;
+    return stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n_max, d_n, chunk_syms, flags, out, out_cap);
 }
 
 extern "C" int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n)

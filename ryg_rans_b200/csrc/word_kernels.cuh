@@ -698,6 +698,28 @@ chunks_stored_compaction_kernel(const uint8_t* __restrict__ scratch, uint32_t sl
                                       nullptr, nullptr, 0, st);
 }
 
+// The GEOM instances of the two stored compactions (rb200_container_blocks_stored_encode_varlen_async and
+// rb200_container_stored_encode_varlen_async): on the grid of the bound, with `blob` the container, the chunk count,
+// the directory and the blob from the record; the version 6 one also takes the input's length, for its ragged last
+// chunk, from there.
+__global__ void __launch_bounds__(kCopyWarps * 32)
+compact_stored_varlen_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+                             const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed, uint8_t* __restrict__ blob,
+                             uint32_t* __restrict__ status, const VarlenGeom* __restrict__ geom, StoredBlocks st)
+{
+    compact<true, false, true>(scratch, slot_bytes, sizes, nullptr, tile_sums, tiles_prefixed, 0, blob, 0, status, geom, nullptr, 0, st);
+}
+
+__global__ void __launch_bounds__(kCopyWarps * 32)
+chunks_stored_compaction_varlen_kernel(const uint8_t* __restrict__ scratch, uint32_t slot_bytes, const uint32_t* __restrict__ sizes,
+                                       const uint64_t* __restrict__ tile_sums, uint32_t tiles_prefixed, uint8_t* __restrict__ blob,
+                                       uint32_t* __restrict__ status, const VarlenGeom* __restrict__ geom, StoredBlocks st)
+{
+    st.n = geom->n;
+    compact<true, false, true, true>(scratch, slot_bytes, sizes, nullptr, tile_sums, tiles_prefixed, 0, blob, 0, status, geom, nullptr, 0,
+                                     st);
+}
+
 // the K2 and K2f instances: (R32, GATED, GEOM) = (r32, 0, 0) for an rb200_model, (r32, 1, 0) and (r32, 1, 1) for the
 // model encodes
 template <bool R32, bool GATED, bool GEOM>

@@ -84,10 +84,17 @@ chunks of 8192, flags 0, alternated: bytes per symbol of both containers and the
 and rb200_container_stored_decode_async against rb200_container_decode_async on the auto container; a torch.profiler
 list of the four calls' kernels.
 
+With --stored-varlen, rb200_container_stored_encode_varlen_async (n_max = 1 GiB) on the --stored workloads, flags 0 and
+RB200_CONTAINER_CRC_BLOB, alternated: at *d_n = n_max against the fixed stored call, with the candidates and with the
+chosen pair alone, and at *d_n = n_max / 16 against the fixed call at that length; a torch.profiler list of both calls'
+kernels.  With --blocks-stored-varlen, the same for rb200_container_blocks_stored_encode_varlen_async (n_blocks_max =
+8192 blocks of 64 KiB, the sixteenth at 512 blocks) on the --blocks-stored workloads.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
     python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto | --blocks-auto
-                                      | --blocks-varlen | --blocks-stored | --stored] [--reps 10]
+                                      | --blocks-varlen | --blocks-stored | --stored | --stored-varlen
+                                      | --blocks-stored-varlen] [--reps 10]
                                      [--json out.json]"""
 import argparse
 import json
@@ -928,6 +935,38 @@ def blocks_varlen(args):
     return res
 
 
+def uniform_blocks(nb, bs, seed):
+    import torch
+    g = torch.Generator(device="cuda")
+    g.manual_seed(seed)
+    return torch.randint(0, 256, (nb * bs,), dtype=torch.uint8, device="cuda", generator=g)
+
+
+def half_blocks(nb, bs, seed):
+    """uniform blocks between per-block Zipf ones"""
+    d = blocks_data(nb, bs, seed).view(nb, bs)
+    d[0::2] = uniform_blocks(nb // 2, bs, seed + 1).view(nb // 2, bs)
+    return d.reshape(-1)
+
+
+def half_data(n, chunk, seed):
+    """runs of 3 chunks + 1000 symbols, uniform and Zipf in turn: every boundary falls inside a chunk"""
+    import torch
+    run = 3 * chunk + 1000
+    m = -(-n // (2 * run)) * 2 * run
+    d = zipf_data(m, seed).view(-1, 2, run)
+    g = torch.Generator(device="cuda")
+    g.manual_seed(seed + 1)
+    d[:, 0, :] = torch.randint(0, 256, (d.shape[0], run), dtype=torch.uint8, device="cuda", generator=g)
+    return d.reshape(-1)[:n]
+
+
+# the stored encodes' workloads: (name, make(n_blocks, block_size, seed)) and (name, make(n, chunk_syms, seed))
+STORED_BLOCKS_WORKLOADS = (("uniform", uniform_blocks), ("zipf", blocks_data), ("skewed", skewed_blocks_data), ("half_uniform_zipf", half_blocks))
+STORED_WORKLOADS = (("uniform", lambda n, chunk, seed: uniform_blocks(1, n, seed)), ("p = 0.99", lambda n, chunk, seed: skewed_data(n, seed)),
+                    ("half_uniform_zipf", half_data))
+
+
 def blocks_stored(args):
     """rb200_container_blocks_stored_encode_async (version 5) over {word 12, byte 14, alias 14} (2 % tolerance) against
     rb200_container_blocks_model_encode_auto_async, on uniform, Zipf, skewed and half-uniform / half-Zipf blocks: bytes
@@ -953,17 +992,7 @@ def blocks_stored(args):
         h = d[:64].cpu().numpy()
         return ((64 + 512 * n_blocks + 8 * (n // chunk + 1) + 15) & ~15) + int(h[32:40].view(np.uint64)[0]), int(h[6]), int(h[7])
 
-    def uniform(nb, bs, seed):
-        g = torch.Generator(device="cuda")
-        g.manual_seed(seed)
-        return torch.randint(0, 256, (nb * bs,), dtype=torch.uint8, device="cuda", generator=g)
-
-    def half(nb, bs, seed):
-        d = blocks_data(nb, bs, seed).view(nb, bs)
-        d[0::2] = uniform(nb // 2, bs, seed + 1).view(nb // 2, bs)
-        return d.reshape(-1)
-
-    for name, make in (("uniform", uniform), ("zipf", blocks_data), ("skewed", skewed_blocks_data), ("half_uniform_zipf", half)):
+    for name, make in STORED_BLOCKS_WORKLOADS:
         d_in = make(n_blocks, block_size, 4321)
         i, a, o = d_in.data_ptr(), d_auto.data_ptr(), d_st.data_ptr()
         enc = {"stored_encode": lambda: ctx.container_blocks_stored_encode_async(cands, tol, i, n_blocks, block_size, chunk, 0, o, bound),
@@ -1026,23 +1055,8 @@ def stored(args):
         h = d[:64].cpu().numpy()
         return int(h[32:40].view(np.uint64)[0]), int(h[6]), int(h[7])
 
-    def uniform(seed):
-        g = torch.Generator(device="cuda")
-        g.manual_seed(seed)
-        return torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda", generator=g)
-
-    def half(seed):
-        """runs of 3 chunks + 1000 symbols, uniform and Zipf in turn: every boundary falls inside a chunk"""
-        run = 3 * chunk + 1000
-        m = -(-n // (2 * run)) * 2 * run
-        d = zipf_data(m, seed).view(-1, 2, run)
-        g = torch.Generator(device="cuda")
-        g.manual_seed(seed + 1)
-        d[:, 0, :] = torch.randint(0, 256, (d.shape[0], run), dtype=torch.uint8, device="cuda", generator=g)
-        return d.reshape(-1)[:n]
-
-    for name, make in (("uniform", uniform), ("p = 0.99", lambda seed: skewed_data(n, seed)), ("half_uniform_zipf", half)):
-        d_in = make(4321)[:n].contiguous()
+    for name, make in STORED_WORKLOADS:
+        d_in = make(n, chunk, 4321)[:n].contiguous()
         i, a, o = d_in.data_ptr(), d_auto.data_ptr(), d_st.data_ptr()
         enc = {"stored_encode": lambda: ctx.container_stored_encode_async(cands, tol, i, n, chunk, 0, o, bound),
                "auto_encode": lambda: ctx.container_model_encode_auto_async(cands, tol, i, n, chunk, 0, a, cap)}
@@ -1083,6 +1097,122 @@ def stored(args):
     return res
 
 
+def varlen_arms(res, name, arms, sync, args, same):
+    """times every arm's (varlen, fixed) pair, alternated, at flags 0 and with the blob CRC; checks that the varlen
+    call wrote the fixed call's container (same()) and profiles both calls of every flags-0 arm"""
+    out = {}
+    for arm, (varlen, fixed) in arms.items():
+        for tag, flags in (("", 0), ("_crc", api.CONTAINER_CRC_BLOB)):
+            v, f = (lambda v=varlen, flags=flags: v(flags)), (lambda f=fixed, flags=flags: f(flags))
+            times = alternate({"varlen": v, "fixed": f}, sync, args.warmup, args.reps)
+            v()
+            f()
+            sync()
+            res["checks"][f"{name} {arm}{tag}: varlen_equals_fixed_call"] = same()
+            out[arm + tag] = {"encode": times, "varlen_minus_fixed_median_us": 1e3 * (times["varlen"]["median_ms"] - times["fixed"]["median_ms"])}
+            if not tag:
+                out[arm]["varlen_kernels"] = kernel_times(v, sync, args.reps)
+                out[arm]["fixed_kernels"] = kernel_times(f, sync, args.reps)
+    return out
+
+
+def stored_varlen(args):
+    """rb200_container_stored_encode_varlen_async (n_max = 1 GiB, chunks of 8192) against the fixed stored call on the
+    --stored workloads: at *d_n = n_max with the list and with the pair it chose as the one candidate, and at
+    *d_n = n_max / 16 against the fixed call at that length"""
+    import torch
+    n_max, chunk, tol = 1 << 30, 8192, 20000
+    cands = [api.CANDIDATE(rb.CODER_WORD, 12), api.CANDIDATE(rb.CODER_ALIAS, 16), api.CANDIDATE(rb.CODER_BYTE, 14)]
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    bound = api.container_stored_bound(n_max, chunk)
+    d_ref = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+    d_out = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+    d_n = torch.tensor([n_max, n_max // 16], dtype=torch.int64, device="cuda")
+    res = {"card": card(), "workload": {"n_max": n_max, "chunk_syms": chunk}, "candidates": ["word 12", "alias 16", "byte 14"],
+           "tolerance_ppm": tol, "workloads": {}, "checks": {}}
+
+    def size(d):
+        h = d[:64].cpu().numpy()
+        n_chunks = int(h[24:32].view(np.uint64)[0])
+        bitmap = (1088 + 8 * (n_chunks + 1) + 15) & ~15
+        return bitmap + 16 * ((n_chunks + 127) // 128) + int(h[32:40].view(np.uint64)[0])
+
+    def same():
+        n = size(d_ref)
+        return size(d_out) == n and bool(torch.equal(d_out[:n], d_ref[:n]))
+
+    for name, make in STORED_WORKLOADS:
+        d_in = make(n_max, chunk, 4321)[:n_max].contiguous()
+        i, r, o = d_in.data_ptr(), d_ref.data_ptr(), d_out.data_ptr()
+        ctx.container_stored_encode_async(cands, tol, i, n_max, chunk, 0, r, bound)
+        sync()
+        one = [api.CANDIDATE(int(d_ref[6].item()), int(d_ref[7].item()))]
+        arms = {  # (varlen call, fixed call), each taking flags
+            "bound": (lambda fl: ctx.container_stored_encode_varlen_async(cands, tol, i, d_n.data_ptr(), n_max, chunk, fl, o, bound),
+                      lambda fl: ctx.container_stored_encode_async(cands, tol, i, n_max, chunk, fl, r, bound)),
+            "bound_one_candidate": (lambda fl: ctx.container_stored_encode_varlen_async(one, 0, i, d_n.data_ptr(), n_max, chunk, fl, o, bound),
+                                    lambda fl: ctx.container_stored_encode_async(one, 0, i, n_max, chunk, fl, r, bound)),
+            "sixteenth": (lambda fl: ctx.container_stored_encode_varlen_async(cands, tol, i, d_n[1:].data_ptr(), n_max, chunk, fl, o, bound),
+                          lambda fl: ctx.container_stored_encode_async(cands, tol, i, n_max // 16, chunk, fl, r, bound)),
+        }
+        res["workloads"][name] = {"chosen": {"coder": one[0] >> 8, "scale_bits": one[0] & 0xFF},
+                                  **varlen_arms(res, name, arms, sync, args, same)}
+        del d_in
+    ctx.close()
+    return res
+
+
+def blocks_stored_varlen(args):
+    """rb200_container_blocks_stored_encode_varlen_async (n_blocks_max = 8192 blocks of 64 KiB, chunks of 8192) against
+    the fixed stored call on the --blocks-stored workloads: at *d_n_blocks = 8192 with the list and with the pair it
+    chose as the one candidate, and at *d_n_blocks = 512 against the fixed call at 512 blocks"""
+    import torch
+    nb_max, block_size, chunk, tol = 8192, 65536, 8192, 20000
+    W, B, A = rb.CODER_WORD, rb.CODER_BYTE, rb.CODER_ALIAS
+    cands = [api.CANDIDATE(W, 12), api.CANDIDATE(B, 14), api.CANDIDATE(A, 14)]
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    bound = api.container_blocks_stored_bound(nb_max, block_size, chunk)
+    d_ref = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+    d_out = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+    d_nb = torch.tensor([nb_max, nb_max // 16], dtype=torch.int32, device="cuda")
+    res = {"card": card(), "workload": {"n_blocks_max": nb_max, "block_size": block_size, "chunk_syms": chunk},
+           "candidates": ["word 12", "byte 14", "alias 14"], "tolerance_ppm": tol, "workloads": {}, "checks": {}}
+
+    def size(d):
+        h = d[:64].cpu().numpy()
+        nb, blob = int(h[56:60].view(np.uint32)[0]), int(h[32:40].view(np.uint64)[0])
+        return ((64 + 512 * nb + 8 * (nb * block_size // chunk + 1) + 15) & ~15) + blob
+
+    def same():
+        n = size(d_ref)
+        return size(d_out) == n and bool(torch.equal(d_out[:n], d_ref[:n]))
+
+    for name, make in STORED_BLOCKS_WORKLOADS:
+        d_in = make(nb_max, block_size, 4321)
+        i, r, o = d_in.data_ptr(), d_ref.data_ptr(), d_out.data_ptr()
+        ctx.container_blocks_stored_encode_async(cands, tol, i, nb_max, block_size, chunk, 0, r, bound)
+        sync()
+        one = [api.CANDIDATE(int(d_ref[6].item()), int(d_ref[7].item()))]
+        arms = {
+            "bound": (lambda fl: ctx.container_blocks_stored_encode_varlen_async(cands, tol, i, d_nb.data_ptr(), nb_max, block_size, chunk, fl,
+                                                                                 o, bound),
+                      lambda fl: ctx.container_blocks_stored_encode_async(cands, tol, i, nb_max, block_size, chunk, fl, r, bound)),
+            "bound_one_candidate": (lambda fl: ctx.container_blocks_stored_encode_varlen_async(one, 0, i, d_nb.data_ptr(), nb_max, block_size,
+                                                                                               chunk, fl, o, bound),
+                                    lambda fl: ctx.container_blocks_stored_encode_async(one, 0, i, nb_max, block_size, chunk, fl, r, bound)),
+            "sixteenth": (lambda fl: ctx.container_blocks_stored_encode_varlen_async(cands, tol, i, d_nb[1:].data_ptr(), nb_max, block_size,
+                                                                                     chunk, fl, o, bound),
+                          lambda fl: ctx.container_blocks_stored_encode_async(cands, tol, i, nb_max // 16, block_size, chunk, fl, r, bound)),
+        }
+        res["workloads"][name] = {"chosen": {"coder": one[0] >> 8, "scale_bits": one[0] & 0xFF},
+                                  **varlen_arms(res, name, arms, sync, args, same)}
+        del d_in
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
@@ -1095,13 +1225,15 @@ def main():
     ap.add_argument("--blocks-varlen", action="store_true", help="the per-block auto encode with the block count in device memory")
     ap.add_argument("--blocks-stored", action="store_true", help="the per-block encode and decode with incompressible blocks stored (version 5)")
     ap.add_argument("--stored", action="store_true", help="the single-model encode and decode with incompressible chunks stored (version 6)")
+    ap.add_argument("--stored-varlen", action="store_true", help="the version 6 encode with the length in device memory")
+    ap.add_argument("--blocks-stored-varlen", action="store_true", help="the version 5 encode with the block count in device memory")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else stored_varlen(args) if args.stored_varlen else blocks_stored_varlen(args) if args.blocks_stored_varlen else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
