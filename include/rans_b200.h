@@ -461,6 +461,56 @@ int rb200_container_stored_encode_varlen_async(rb200_ctx* ctx, const uint32_t* c
 int rb200_container_stored_decode_async(rb200_ctx* ctx, const uint8_t* buf, size_t size, uint8_t* out, size_t out_cap,
                                         uint64_t* d_n_symbols);
 
+/* ---------------------------------------------------------------- byte-plane containers */
+
+/* Version 7: the n bytes of a tensor of w-byte elements (w = elem_bytes, 2, 4 or 8) as w byte planes, plane p holding
+ * byte p of every element in element order (little-endian, as the tensor lies in memory), each plane a complete version
+ * 6 container of n / w symbols.  Layout: a 64-byte header (version 7, coder and scale_bits 0, lanes 32, chunk_syms, n
+ * in n_symbols, n_chunks 0, blob_bytes = the bytes after the plane table, the caller's flags, meta_crc over the header
+ * (crc fields zero) and the table, blob_crc 0, block_size = n_blocks = w, reserved 0), then w table entries {u64 offset,
+ * u64 size}, then the planes with no gaps: offset[0] = 64 + 16 w, offset[p + 1] = offset[p] + size[p], size[p] the
+ * plane's exact size.  Every plane has the header's chunk_syms (32 .. 2^24) and flags.  n is a nonzero multiple of w
+ * with n / w < 2^32.  Only the _planes_ calls accept version 7, and they accept no other version.
+ *   bound: 64 + 16 w + w * rb200_container_stored_bound(n / w, chunk_syms); 0 for arguments the encode refuses.
+ *   pack:  host only, from w version 6 containers (each exactly sizes[p] bytes, 8-byte aligned) that agree on n,
+ *          chunk_syms and flags.  RB200_E_ARG for a bad elem_bytes, a null pointer or a plane that
+ *          rb200_container_stored_open rejects or that disagrees; RB200_E_SPACE when out_cap is below the container.
+ *   open:  checks the header, the table, meta_crc and every plane by rb200_container_stored_open's rules; RB200_E_STREAM
+ *          for anything else (versions 1-6 among them), RB200_E_ARG for a null pointer or a buf that is not 8-byte
+ *          aligned.  info->planes[p] / sizes[p] are views into buf that rb200_container_stored_open accepts. */
+typedef struct rb200_container_planes_info {
+    uint32_t elem_bytes, chunk_syms, flags, reserved;
+    uint64_t n;
+    const uint8_t* planes[8];
+    size_t sizes[8];
+} rb200_container_planes_info;
+size_t rb200_container_planes_bound(size_t n, uint32_t elem_bytes, uint32_t chunk_syms);
+int rb200_container_planes_pack(uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint8_t* out, size_t out_cap,
+                                size_t* out_size);
+int rb200_container_planes_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info);
+/* A version 7 container of the n bytes at `in`, DEVICE memory, enqueued only: plane p is byte for byte what
+ * rb200_container_stored_encode_async writes for plane p's bytes with the same candidates, tolerance_ppm, chunk_syms
+ * and flags, so each plane picks its own coder.  in and out 16-byte aligned.  The call returns RB200_E_ARG (nothing
+ * launched) for everything rb200_container_stored_encode_async refuses for n / w symbols, an elem_bytes other than 2, 4
+ * or 8, n == 0 or not a multiple of it, n / w >= 2^32, and a misaligned in; RB200_E_SPACE (nothing launched) when
+ * out_cap is below rb200_container_planes_bound.  rb200_sync gives the first failing plane's verdict (RB200_E_MODEL when
+ * no candidate is feasible for a plane), and the version 7 header is then not written.  Capturable in a CUDA graph
+ * after one call with the same list and geometry outside the capture (the workspaces grow). */
+int rb200_container_planes_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                        uint32_t elem_bytes, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags,
+                                        uint8_t* out, size_t out_cap);
+/* The contract of rb200_container_stored_decode_async for version 7, with the element width the caller expects: kernels
+ * check the header (its w must be elem_bytes), the table and meta_crc, and every plane through version 6's checks and
+ * decoders, into a workspace of min(out_cap, w * 2^32) bytes; only when every check has passed does one kernel
+ * interleave the planes into out.  *d_n_symbols receives n once the header, the table and the planes' headers pass.
+ * rb200_sync gives RB200_E_STREAM for anything rb200_container_planes_open rejects, a w other than elem_bytes or a
+ * plane that fails its checks, and RB200_E_SPACE for n > out_cap once the header and table pass (whatever the planes
+ * hold); in both cases out is untouched.  A corrupt coded stream that passes every check is RB200_E_STREAM.
+ * RB200_E_ARG (nothing launched) for a bad elem_bytes or the arguments rb200_container_stored_decode_async refuses.
+ * Capturable after one call of the same size and out_cap outside the capture (the workspaces grow). */
+int rb200_container_planes_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size, uint8_t* out,
+                                        size_t out_cap, uint64_t* d_n_symbols);
+
 /* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
  * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's
  * decode table is built on the GPU into the context, and the decoder the header calls for is picked on the GPU -- all

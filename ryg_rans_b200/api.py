@@ -115,6 +115,13 @@ EXPORTS = [
     ("rb200_container_blocks_stored_encode_varlen_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
                                                                     C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
                                                                     C.c_size_t]),
+    ("rb200_container_planes_bound", C.c_size_t, [C.c_size_t, C.c_uint32, C.c_uint32]),
+    ("rb200_container_planes_pack", C.c_int, [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("rb200_container_planes_open", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("rb200_container_planes_encode_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,
+                                                      C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_container_planes_decode_async", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
+                                                      C.c_void_p]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -250,6 +257,43 @@ def container_stored_open(buf):
     blob = buf[b_off:b_off + info.blob_bytes]
     meta = {k: int(getattr(info, k)) for k in ("coder", "scale_bits", "chunk_syms", "flags", "n_symbols", "n_chunks", "blob_bytes")}
     return meta, freqs, bits, offsets, blob
+
+
+def container_planes_bound(n, elem_bytes, chunk_syms):
+    """rb200_container_planes_bound: the most bytes a version 7 container of n bytes of elem_bytes-byte elements takes
+    (0 for arguments the encode refuses)"""
+    return int(load().dll.rb200_container_planes_bound(n, elem_bytes, chunk_syms))
+
+
+class ContainerPlanesInfo(C.Structure):
+    _fields_ = [("elem_bytes", C.c_uint32), ("chunk_syms", C.c_uint32), ("flags", C.c_uint32), ("reserved", C.c_uint32),
+                ("n", C.c_uint64), ("planes", C.c_void_p * 8), ("sizes", C.c_size_t * 8)]
+
+
+def container_planes_pack(planes):
+    """rb200_container_planes_pack: a version 7 container from w = len(planes) version 6 containers (uint8 arrays, one
+    per byte plane, agreeing on n, chunk_syms and flags)"""
+    lib = load()
+    planes = [np.ascontiguousarray(p, dtype=np.uint8) for p in planes]
+    w = len(planes)
+    ptrs = (C.c_void_p * max(w, 1))(*[p.ctypes.data for p in planes])
+    sizes = (C.c_size_t * max(w, 1))(*[p.size for p in planes])
+    out = np.zeros(64 + 16 * w + sum(p.size for p in planes), np.uint8)
+    size = C.c_size_t(0)
+    lib.check(lib.dll.rb200_container_planes_pack(w, ptrs, sizes, out.ctypes.data, out.size, C.byref(size)))
+    return out[:size.value]
+
+
+def container_planes_open(buf):
+    """Returns (info dict, planes): planes[p] is a view into buf of plane p's version 6 container."""
+    lib = load()
+    buf = np.ascontiguousarray(buf, dtype=np.uint8)
+    info = ContainerPlanesInfo()
+    lib.check(lib.dll.rb200_container_planes_open(buf.ctypes.data, buf.size, C.byref(info)))
+    base = buf.ctypes.data
+    planes = [buf[info.planes[p] - base:info.planes[p] - base + info.sizes[p]] for p in range(info.elem_bytes)]
+    meta = {k: int(getattr(info, k)) for k in ("elem_bytes", "chunk_syms", "flags", "n")}
+    return meta, planes
 
 
 class ContainerBlocksInfo(C.Structure):
@@ -636,6 +680,21 @@ class Context:
         self.lib.check(self.lib.dll.rb200_container_stored_encode_varlen_async(self.h, cands.ctypes.data_as(_u32p), cands.size,
                                                                                tolerance_ppm, in_ptr, n_ptr, n_max, chunk_syms, flags,
                                                                                out_ptr, out_cap), self.h)
+
+    def container_planes_encode_async(self, candidates, tolerance_ppm, elem_bytes, in_ptr, n, chunk_syms, flags, out_ptr, out_cap):
+        """A version 7 container of n bytes of elem_bytes-byte elements (2, 4 or 8): byte plane p of every element is a
+        version 6 container, byte for byte what container_stored_encode_async writes for it.  out_cap >=
+        container_planes_bound.  The verdict (the first failing plane's, header unwritten) comes from sync()"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_planes_encode_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
+                                                                        elem_bytes, in_ptr, n, chunk_syms, flags, out_ptr, out_cap), self.h)
+
+    def container_planes_decode_async(self, elem_bytes, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
+        """enqueue only (CUDA-graph capturable once a call of the same size and out_cap has grown the workspaces): a
+        version 7 container of elem_bytes-byte elements.  The verdict (-4 corrupt, -3 out_cap too small, output
+        untouched) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_planes_decode_async(self.h, elem_bytes, buf_ptr, size, out_ptr, out_cap, n_ptr or None),
+                       self.h)
 
     def container_stored_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
         """the async decode of a version 6 container; enqueue only (CUDA-graph capturable).  The verdict (-4 corrupt or

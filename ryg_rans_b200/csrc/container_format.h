@@ -329,6 +329,48 @@ RB200_HD inline bool container_v6_chunk_ok(const uint64_t* offsets, const uint32
     return container_stored_step_ok(offsets, c, m, blob_bytes) && container_stored_pad_ok(blob + offsets[c], m);
 }
 
+// Version 7 (byte planes): a 64-byte header, a table of w {offset, size} entries, then w version 6 containers with no
+// gaps, plane p holding byte p of every w-byte element.  The header: coder and scale_bits 0, lanes 32, chunk_syms, n
+// input bytes (a nonzero multiple of w, n / w < 2^32), n_chunks 0, blob_bytes the bytes after the table, the caller's
+// flags, meta_crc over the header (crc fields zero) and the table, blob_crc 0, block_size = n_blocks = w, reserved 0.
+// Every plane is a version 6 container of n / w symbols with the header's chunk_syms and flags.
+constexpr uint16_t kContainerVersionPlanes = 7;
+struct PlaneEntry {
+    uint64_t offset, size;
+};
+static_assert(sizeof(PlaneEntry) == 16, "plane table entries are 16 bytes");
+RB200_HD inline bool container_planes_w_ok(uint32_t w) { return w == 2 || w == 4 || w == 8; }
+// the end of the table: plane 0's offset, 16-aligned
+RB200_HD inline uint64_t container_planes_table_end(uint32_t w) { return sizeof(ContainerHeader) + sizeof(PlaneEntry) * w; }
+// version 7's header rules; the table and the planes fit `size`
+RB200_HD inline bool container_planes_header_ok(const ContainerHeader& h, uint64_t size)
+{
+    if (h.magic != kContainerMagic || h.version != kContainerVersionPlanes || h.coder || h.scale_bits || h.lanes != RB200_LANES) return false;
+    if (!container_planes_w_ok(h.block_size) || h.n_blocks != h.block_size || h.n_chunks || h.reserved || h.blob_crc) return false;
+    if (!container_chunk_ok(h.chunk_syms) || !h.n_symbols || h.n_symbols % h.block_size || ((h.n_symbols / h.block_size) >> 32)) return false;
+    const uint64_t t = container_planes_table_end(h.block_size);
+    return t <= size && h.blob_bytes <= size - t;
+}
+// the table: plane 0 right after it, every plane right after the previous one, each at least a header long and a
+// multiple of 16, and the last one ending where the blob does
+RB200_HD inline bool container_planes_table_ok(const ContainerHeader& h, const PlaneEntry* t)
+{
+    uint64_t end = container_planes_table_end(h.block_size);
+    const uint64_t last = end + h.blob_bytes;
+    for (uint32_t p = 0; p < h.block_size; p++) {
+        if (t[p].offset != end || (t[p].size & 15) || t[p].size < sizeof(ContainerHeader) || t[p].size > last - end) return false;
+        end += t[p].size;
+    }
+    return end == last;
+}
+// plane p's header (ph, read from the start of its size bytes): version 6 with n / w symbols, the header's chunk_syms
+// and flags, and exactly size bytes long
+RB200_HD inline bool container_planes_plane_ok(const ContainerHeader& h, const ContainerHeader& ph, uint64_t size)
+{
+    return ph.n_symbols == h.n_symbols / h.block_size && ph.chunk_syms == h.chunk_syms && ph.flags == h.flags &&
+           container_chunks_stored_header_ok(ph, size) && container_bitmap_blob_offset(ph.n_chunks) + ph.blob_bytes == size;
+}
+
 // the header rb200_container_pack writes (crc fields zero)
 ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_syms, uint64_t n, uint64_t n_chunks,
                                  uint64_t blob_bytes, uint32_t flags);

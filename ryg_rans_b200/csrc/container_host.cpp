@@ -26,6 +26,11 @@
 // exactly one version: rb200_container_* version 1, rb200_container_blocks_* version 2, rb200_container_blocks_coder_*
 // version 3, rb200_container_blocks_alias_* version 4.
 //
+//   version 7 (byte planes):     [ 64-byte header ][ w x {u64 offset, u64 size} ][ plane 0: a version 6 container ] ... [ plane w-1 ]
+//
+// Plane p holds byte p of every w-byte element; the rules are container_planes_* in container_format.h, and each plane
+// is checked by rb200_container_stored_open's.
+//
 // rb200_container_pack / _open and the _blocks_ forms here work on host buffers with a host CRC (slicing-by-8, ~1 GB/s
 // on one core: the blob CRC is optional for that reason).  rb200_container_encode / _decode and the _blocks_ forms
 // (rans_b200.cu) write and read the same bytes in host or device memory with the blob CRC on the GPU
@@ -493,6 +498,93 @@ extern "C" int rb200_container_stored_open(const uint8_t* buf, size_t size, rb20
     info->offsets = reinterpret_cast<const uint64_t*>(buf + kContainerDirOffset);
     info->blob = buf + container_bitmap_blob_offset(h.n_chunks);
     *stored_bits = reinterpret_cast<const uint32_t*>(buf + container_bitmap_offset(h.n_chunks));
+    return RB200_OK;
+}
+
+extern "C" size_t rb200_container_planes_bound(size_t n, uint32_t elem_bytes, uint32_t chunk_syms)
+{
+    if (!container_planes_w_ok(elem_bytes) || n % elem_bytes) return 0;
+    const size_t plane = rb200_container_stored_bound(n / elem_bytes, chunk_syms);
+    return plane ? container_planes_table_end(elem_bytes) + elem_bytes * plane : 0;
+}
+
+namespace {
+
+// a version 6 container that rb200_container_stored_open accepts, exactly `size` bytes long: its header in *h
+int planes_plane_open(const uint8_t* plane, size_t size, ContainerHeader* h)
+{
+    rb200_container_info info;
+    const uint32_t* bits = nullptr;
+    const int rc = rb200_container_stored_open(plane, size, &info, &bits);
+    if (rc != RB200_OK) return rc;
+    std::memcpy(h, plane, sizeof *h);
+    return container_bitmap_blob_offset(h->n_chunks) + h->blob_bytes == size ? RB200_OK : RB200_E_STREAM;
+}
+
+}  // namespace
+
+extern "C" int rb200_container_planes_pack(uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint8_t* out,
+                                           size_t out_cap, size_t* out_size)
+{
+    if (!container_planes_w_ok(elem_bytes) || !planes || !sizes || !out) return RB200_E_ARG;
+    ContainerHeader first{};
+    PlaneEntry table[8];
+    uint64_t end = container_planes_table_end(elem_bytes);
+    for (uint32_t p = 0; p < elem_bytes; p++) {
+        ContainerHeader ph;
+        if (!planes[p] || planes_plane_open(planes[p], sizes[p], &ph) != RB200_OK) return RB200_E_ARG;
+        if (p == 0) first = ph;
+        else if (ph.n_symbols != first.n_symbols || ph.chunk_syms != first.chunk_syms || ph.flags != first.flags) return RB200_E_ARG;
+        table[p] = PlaneEntry{end, sizes[p]};
+        end += sizes[p];
+    }
+    if (!container_chunk_ok(first.chunk_syms)) return RB200_E_ARG;          // the v7 rules take the encodes' chunk sizes
+    if (end > out_cap) return RB200_E_SPACE;
+    ContainerHeader h{};
+    h.magic = kContainerMagic;
+    h.version = kContainerVersionPlanes;
+    h.lanes = RB200_LANES;
+    h.chunk_syms = first.chunk_syms;
+    h.n_symbols = first.n_symbols * elem_bytes;
+    h.blob_bytes = end - container_planes_table_end(elem_bytes);
+    h.flags = first.flags;
+    h.block_size = h.n_blocks = elem_bytes;
+    h.meta_crc = container_crc32(container_header_crc(h), table, sizeof(PlaneEntry) * elem_bytes);
+    std::memcpy(out, &h, sizeof h);
+    std::memcpy(out + sizeof h, table, sizeof(PlaneEntry) * elem_bytes);
+    for (uint32_t p = 0; p < elem_bytes; p++) std::memcpy(out + table[p].offset, planes[p], sizes[p]);
+    if (out_size) *out_size = end;
+    return RB200_OK;
+}
+
+extern "C" int rb200_container_planes_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info)
+{
+    if (!buf || !info) return RB200_E_ARG;
+    if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
+    ContainerHeader h;
+    std::memcpy(&h, buf, sizeof h);
+    if (!container_planes_header_ok(h, size)) return RB200_E_STREAM;
+    if (reinterpret_cast<uintptr_t>(buf) & 7) return RB200_E_ARG;
+    const uint32_t w = h.block_size;
+    PlaneEntry table[8];
+    std::memcpy(table, buf + sizeof h, sizeof(PlaneEntry) * w);
+    if (container_crc32(container_header_crc(h), table, sizeof(PlaneEntry) * w) != h.meta_crc || !container_planes_table_ok(h, table))
+        return RB200_E_STREAM;
+    for (uint32_t p = 0; p < w; p++) {
+        ContainerHeader ph;
+        std::memcpy(&ph, buf + table[p].offset, sizeof ph);
+        if (!container_planes_plane_ok(h, ph, table[p].size) || planes_plane_open(buf + table[p].offset, table[p].size, &ph) != RB200_OK)
+            return RB200_E_STREAM;
+    }
+    std::memset(info, 0, sizeof *info);
+    info->elem_bytes = w;
+    info->chunk_syms = h.chunk_syms;
+    info->flags = h.flags;
+    info->n = h.n_symbols;
+    for (uint32_t p = 0; p < w; p++) {
+        info->planes[p] = buf + table[p].offset;
+        info->sizes[p] = table[p].size;
+    }
     return RB200_OK;
 }
 

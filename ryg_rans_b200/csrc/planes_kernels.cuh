@@ -1,0 +1,288 @@
+// planes_kernels.cuh -- the byte-plane container (version 7): rb200_container_planes_encode_async and
+// rb200_container_planes_decode_async (rans_b200.cu).  Every plane is a version 6 container written and read by the
+// version 6 calls' own stages; the kernels here only move bytes between the element layout and the planes, place the
+// planes and write or check the version 7 header and table.
+//
+// Encode, in stream order on the context's stream:
+//   planes_split_kernel<W>      the n input bytes into W planes of m = n / W bytes, at a stride of round16(m), in a
+//                               context workspace: 16 elements per thread, W 16-byte loads, the byte transpose in
+//                               registers (PRMT), one 16-byte store per plane
+//   plane 0's version 6 encode  in place, at 64 + 16 W
+//   planes_place_kernel(0)      plane 0's verdict (the status word is clear: its header was written) and table entry
+//   for p = 1 .. W-1: plane p's version 6 encode into a staging area, then planes_place_kernel(p): its verdict, its size
+//                               from its header, its offset from entry p - 1, the copy to there and its table entry
+//   planes_finish_kernel        the version 7 header and meta_crc, only when every plane was placed
+// Decode:
+//   planes_plan_kernel          the header (its W must be the caller's), the table, every plane's header and meta_crc,
+//                               into the call's record
+//   plane 0's version 6 decode  in place from 64 + 16 W, into plane 0 of a workspace; planes_record_kernel(0)
+//   for p = 1 .. W-1: planes_fetch_kernel(p) copies [offset, offset + size) into staging when the record passed (else a
+//                               zero header, which version 6's plan rejects), plane p's version 6 decode from there,
+//                               planes_record_kernel(p)
+//   planes_verdict_kernel       *d_n_symbols, then kStatStream / kStatSpace or the record's go
+//   planes_interleave_kernel<W> the planes into out, only when go is set
+#pragma once
+#include "container_decode.cuh"
+#include "container_format.h"
+#include "crc_kernels.cuh"
+
+namespace rb200 {
+
+// The call-private record of a byte-plane call (one for the encode, one for the decode): the outcome of the call's own
+// checks, so that status bits left by earlier calls that were not synchronised do not change what it writes.
+struct PlanesWork {
+    PlaneEntry table[8];        // decode: the table, when ok
+    uint64_t n;                 // decode: the header's n, when ok
+    uint32_t ok;                // decode: the header, the table, every plane's header and meta_crc passed
+    uint32_t go;                // decode: every check passed; the interleave runs
+    uint32_t plane_go[8];       // encode: plane p was written and placed; decode: plane p's version 6 verdict passed
+};
+
+constexpr uint32_t kPlanesThreads = 256;
+constexpr uint32_t kPlanesCtasPerSm = 8;
+
+// 16 elements of W bytes in x (4 W words, element e at bytes e W .. e W + W - 1) -> y[4 k + j] = byte k of elements
+// 4 j .. 4 j + 3: three PRMTs per output word, every index a constant once unrolled
+template <int W>
+__device__ __forceinline__ void planes_transpose(const uint32_t (&x)[4 * W], uint32_t (&y)[4 * W])
+{
+#pragma unroll
+    for (int k = 0; k < W; k++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int b0 = 4 * j * W + k, b1 = b0 + W, b2 = b1 + W, b3 = b2 + W;
+            const uint32_t lo = __byte_perm(x[b0 >> 2], x[b1 >> 2], (b0 & 3) | ((b1 & 3) + 4) << 4);
+            const uint32_t hi = __byte_perm(x[b2 >> 2], x[b3 >> 2], (b2 & 3) | ((b3 & 3) + 4) << 4);
+            y[4 * k + j] = __byte_perm(lo, hi, 0x5410);
+        }
+}
+
+// the inverse: byte b of x is byte b % W of element b / W, which is byte (b / W) % 4 of y[4 (b % W) + b / W / 4]
+template <int W>
+__device__ __forceinline__ void planes_untranspose(const uint32_t (&y)[4 * W], uint32_t (&x)[4 * W])
+{
+#pragma unroll
+    for (int t = 0; t < 4 * W; t++) {
+        int word[4], sel[4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const int b = 4 * t + i, e = b / W;
+            word[i] = 4 * (b % W) + (e >> 2);
+            sel[i] = e & 3;
+        }
+        const uint32_t lo = __byte_perm(y[word[0]], y[word[1]], sel[0] | (sel[1] + 4) << 4);
+        const uint32_t hi = __byte_perm(y[word[2]], y[word[3]], sel[2] | (sel[3] + 4) << 4);
+        x[t] = __byte_perm(lo, hi, 0x5410);
+    }
+}
+
+// in (m elements of W bytes, 16-byte aligned) -> plane k at planes + k * stride (stride a multiple of 16).  Grid-stride
+// over groups of 16 elements; the ragged end (fewer than 16 elements) a byte per thread.
+template <int W>
+__global__ void __launch_bounds__(kPlanesThreads)
+    planes_split_kernel(const uint8_t* __restrict__ in, uint64_t m, uint8_t* __restrict__ planes, uint64_t stride)
+{
+    const uint64_t groups = m / 16, step = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    const uint64_t tid = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    for (uint64_t g = tid; g < groups; g += step) {
+        const uint4* src = reinterpret_cast<const uint4*>(in) + g * W;
+        uint32_t x[4 * W], y[4 * W];
+#pragma unroll
+        for (int i = 0; i < W; i++) {
+            const uint4 v = __ldcs(src + i);
+            x[4 * i] = v.x;
+            x[4 * i + 1] = v.y;
+            x[4 * i + 2] = v.z;
+            x[4 * i + 3] = v.w;
+        }
+        planes_transpose<W>(x, y);
+#pragma unroll
+        for (int k = 0; k < W; k++)
+            *reinterpret_cast<uint4*>(planes + k * stride + g * 16) = make_uint4(y[4 * k], y[4 * k + 1], y[4 * k + 2], y[4 * k + 3]);
+    }
+    const uint64_t tail = groups * 16;
+    if (tid < (m - tail) * W) {
+        const uint64_t e = tail + tid / W, k = tid % W;
+        planes[k * stride + e] = in[e * W + k];
+    }
+}
+
+// The inverse, from the decode workspace into out: n from the record, and nothing unless every check passed.
+template <int W>
+__global__ void __launch_bounds__(kPlanesThreads)
+    planes_interleave_kernel(const uint8_t* __restrict__ planes, uint64_t stride, uint8_t* __restrict__ out, const PlanesWork* __restrict__ r)
+{
+    if (!r->go) return;
+    const uint64_t m = r->n / W, groups = m / 16, step = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    const uint64_t tid = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    for (uint64_t g = tid; g < groups; g += step) {
+        uint32_t x[4 * W], y[4 * W];
+#pragma unroll
+        for (int k = 0; k < W; k++) {
+            const uint4 v = __ldcs(reinterpret_cast<const uint4*>(planes + k * stride + g * 16));
+            y[4 * k] = v.x;
+            y[4 * k + 1] = v.y;
+            y[4 * k + 2] = v.z;
+            y[4 * k + 3] = v.w;
+        }
+        planes_untranspose<W>(y, x);
+        uint4* dst = reinterpret_cast<uint4*>(out) + g * W;
+#pragma unroll
+        for (int i = 0; i < W; i++) dst[i] = make_uint4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
+    }
+    const uint64_t tail = groups * 16;
+    if (tid < (m - tail) * W) {
+        const uint64_t e = tail + tid / W, k = tid % W;
+        out[e * W + k] = planes[k * stride + e];
+    }
+}
+
+// Encode: plane p's verdict and place.  Its container is complete (header included) at src -- out + 64 + 16 W for
+// plane 0, the staging area for the others -- exactly when the status word is clear, since version 6's header kernel
+// writes only then.  Entry p: the offset right after plane p - 1 (entry p - 1, written by the previous launch), the
+// size from the plane's header.  Plane 0 is in place; the others are copied, 16 bytes per thread and step.
+__global__ void __launch_bounds__(kPlanesThreads)
+    planes_place_kernel(uint8_t* __restrict__ out, const uint8_t* __restrict__ src, uint32_t p, uint32_t w, uint64_t out_cap,
+                        PlanesWork* __restrict__ r, uint32_t* status)
+{
+    const bool ok = *status == 0;
+    const bool first = blockIdx.x == 0 && threadIdx.x == 0;
+    if (first) r->plane_go[p] = 0;
+    if (!ok) return;
+    PlaneEntry* table = reinterpret_cast<PlaneEntry*>(out + sizeof(ContainerHeader));
+    const ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(src);
+    const uint64_t size = container_bitmap_blob_offset(h.n_chunks) + h.blob_bytes;
+    const uint64_t offset = p ? table[p - 1].offset + table[p - 1].size : container_planes_table_end(w);
+    if (offset > out_cap || size > out_cap - offset) {                // not reached: the host checked the bound
+        if (first) atomicOr(status, kStatSpace);
+        return;
+    }
+    if (first) {
+        table[p] = PlaneEntry{offset, size};
+        r->plane_go[p] = 1;
+    }
+    if (p == 0) return;
+    const uint4* s = reinterpret_cast<const uint4*>(src);
+    uint4* d = reinterpret_cast<uint4*>(out + offset);
+    const uint64_t step = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < size / 16; i += step) d[i] = s[i];
+}
+
+// CRC-32 of the header (crc fields zero) and the table, staged in shared memory at s (bytes = 64 + 16 W, a multiple
+// of 32): one warp, bytes / 32 per lane, each shifted past the bytes after it
+__device__ __forceinline__ uint32_t planes_meta_crc(const uint8_t* s, uint32_t bytes)
+{
+    using namespace crc_detail;
+    const uint32_t lane = threadIdx.x & 31, piece = bytes / 32;
+    uint32_t c = raw_bytes_bitwise(s + lane * piece, piece);
+    c = __reduce_xor_sync(0xffffffffu, crc32_shift(c, bytes - piece * (lane + 1)));
+    return finish_warp(0, bytes, c);
+}
+
+// Encode: the version 7 header, when every plane was placed and the status word is still clear.  h arrives complete
+// but for blob_bytes and meta_crc.
+__global__ void __launch_bounds__(32)
+    planes_finish_kernel(uint8_t* out, ContainerHeader h, const PlanesWork* __restrict__ r, const uint32_t* status)
+{
+    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
+    uint8_t* s = reinterpret_cast<uint8_t*>(s_v);
+    const uint32_t lane = threadIdx.x, w = h.block_size;
+    bool all = *status == 0;
+    for (uint32_t p = 0; p < w; p++) all = all && r->plane_go[p];
+    if (!all) return;
+    const PlaneEntry* table = reinterpret_cast<const PlaneEntry*>(out + sizeof(ContainerHeader));
+    const uint64_t end = container_planes_table_end(w);
+    h.blob_bytes = table[w - 1].offset + table[w - 1].size - end;
+    h.meta_crc = 0;
+    h.blob_crc = 0;
+    if (lane == 0) *reinterpret_cast<ContainerHeader*>(s) = h;
+    if (lane < w) s_v[4 + lane] = reinterpret_cast<const uint4*>(table)[lane];
+    __syncwarp();
+    const uint32_t meta = planes_meta_crc(s, static_cast<uint32_t>(end));
+    if (lane == 0) reinterpret_cast<ContainerHeader*>(s)->meta_crc = meta;
+    __syncwarp();
+    if (lane < 4) reinterpret_cast<uint4*>(out)[lane] = s_v[lane];
+}
+
+// Decode: every version 7 rule on the header, the table and the planes' headers, and meta_crc; the record is reset
+// for the call.  One warp: lanes 0..3 stage the header, lanes 4.. the table, lane p < W checks plane p's header.
+__global__ void __launch_bounds__(32)
+    planes_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, PlanesWork* __restrict__ r)
+{
+    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
+    uint8_t* s = reinterpret_cast<uint8_t*>(s_v);
+    const uint32_t lane = threadIdx.x;
+    ContainerHeader h = {};
+    if (size >= sizeof(ContainerHeader)) h = *reinterpret_cast<const ContainerHeader*>(buf);   // a shorter buffer is not read
+    bool ok = size >= sizeof(ContainerHeader) && container_planes_header_ok(h, size) && h.block_size == w;
+    const uint32_t meta_crc = h.meta_crc;
+    if (ok) {                                                         // the table lies in size (header rule)
+        h.meta_crc = 0;
+        h.blob_crc = 0;
+        if (lane == 0) *reinterpret_cast<ContainerHeader*>(s) = h;
+        if (lane < w) s_v[4 + lane] = reinterpret_cast<const uint4*>(buf + sizeof(ContainerHeader))[lane];
+        __syncwarp();
+        const PlaneEntry* table = reinterpret_cast<const PlaneEntry*>(s + sizeof(ContainerHeader));
+        ok = planes_meta_crc(s, static_cast<uint32_t>(container_planes_table_end(w))) == meta_crc && container_planes_table_ok(h, table);
+        // each plane's header lies in size once the table passes
+        const bool plane = !ok || lane >= w ||
+                           container_planes_plane_ok(h, *reinterpret_cast<const ContainerHeader*>(buf + table[lane].offset), table[lane].size);
+        ok = __all_sync(0xffffffffu, plane) && ok;
+    }
+    if (lane < 8) {
+        r->plane_go[lane] = 0;
+        r->table[lane] = ok && lane < w ? reinterpret_cast<const PlaneEntry*>(s + sizeof(ContainerHeader))[lane] : PlaneEntry{0, 0};
+    }
+    if (lane == 0) {
+        r->ok = ok;
+        r->go = 0;
+        r->n = ok ? h.n_symbols : 0;
+    }
+}
+
+// Decode: plane p's bytes into staging, when the record passed and the plane fits it; otherwise a zero header, which
+// version 6's plan rejects.
+__global__ void __launch_bounds__(kPlanesThreads)
+    planes_fetch_kernel(const uint8_t* __restrict__ buf, uint8_t* __restrict__ stage, uint64_t stage_cap, uint32_t p,
+                        const PlanesWork* __restrict__ r)
+{
+    const PlaneEntry e = r->table[p];
+    const uint64_t tid = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (!r->ok || e.size > stage_cap) {
+        if (tid < sizeof(ContainerHeader) / 16) reinterpret_cast<uint4*>(stage)[tid] = make_uint4(0, 0, 0, 0);
+        return;
+    }
+    const uint4* s = reinterpret_cast<const uint4*>(buf + e.offset);
+    uint4* d = reinterpret_cast<uint4*>(stage);
+    const uint64_t step = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    for (uint64_t i = tid; i < e.size / 16; i += step) d[i] = s[i];
+}
+
+// Decode: plane p's version 6 verdict (its workspace's go) into the record
+__global__ void __launch_bounds__(32) planes_record_kernel(uint32_t p, const ContainerAsyncWork* __restrict__ w6, PlanesWork* __restrict__ r)
+{
+    if (threadIdx.x == 0) r->plane_go[p] = w6->go != 0;
+}
+
+// Decode: the call's verdict.  The header and table rejected: kStatStream.  Otherwise n is written, then n > out_cap
+// is kStatSpace, a plane that failed its checks kStatStream, and a call that passed everything sets go.
+__global__ void __launch_bounds__(32)
+    planes_verdict_kernel(uint32_t w, uint64_t out_cap, uint64_t* __restrict__ n_symbols, PlanesWork* __restrict__ r, uint32_t* status)
+{
+    if (threadIdx.x) return;
+    if (!r->ok) {
+        atomicOr(status, kStatStream);
+        return;
+    }
+    if (n_symbols) *n_symbols = r->n;
+    bool all = true;
+    for (uint32_t p = 0; p < w; p++) all = all && r->plane_go[p];
+    if (r->n > out_cap)
+        atomicOr(status, kStatSpace);
+    else if (!all)
+        atomicOr(status, kStatStream);
+    else
+        r->go = 1;
+}
+
+}  // namespace rb200

@@ -23,6 +23,7 @@
 #include "container_format.h"
 #include "crc_kernels.cuh"
 #include "model_kernels.cuh"
+#include "planes_kernels.cuh"
 #include "rans64_kernels.cuh"
 #include "tables.h"
 #include "word_kernels.cuh"
@@ -78,6 +79,11 @@ struct rb200_ctx {
     BlocksVarlenGeom* d_blocks_geom = nullptr;
     // rb200_container_stored_encode_varlen_async: the geometry of the length its plan kernel read
     StoredVarlenGeom* d_stored_geom = nullptr;
+    // the byte-plane calls (planes_kernels.cuh): each call's record, the encode's split planes and staging area, the
+    // decode's decoded planes and staging area
+    PlanesWork* d_planes_enc = nullptr;
+    PlanesWork* d_planes_dec = nullptr;
+    DevBuf planes_in, planes_enc_stage, planes_out, planes_dec_stage;
 };
 
 struct rb200_model {
@@ -251,6 +257,10 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     if (e == cudaSuccess) e = cudaMemset(ctx->d_blocks_geom, 0, sizeof(BlocksVarlenGeom));
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_stored_geom, sizeof(StoredVarlenGeom));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_stored_geom, 0, sizeof(StoredVarlenGeom));
+    for (PlanesWork** r : {&ctx->d_planes_enc, &ctx->d_planes_dec}) {
+        if (e == cudaSuccess) e = cudaMalloc(r, sizeof(PlanesWork));
+        if (e == cudaSuccess) e = cudaMemset(*r, 0, sizeof(PlanesWork));
+    }
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -275,6 +285,7 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     cudaStreamSynchronize(ctx->stream);
     release(ctx->scratch); release(ctx->sizes);
     release(ctx->st_in); release(ctx->st_blob); release(ctx->st_offsets); release(ctx->st_out); release(ctx->st_aux);
+    release(ctx->planes_in); release(ctx->planes_enc_stage); release(ctx->planes_out); release(ctx->planes_dec_stage);
     if (ctx->d_status) cudaFree(ctx->d_status);
     if (ctx->d_work) cudaFree(ctx->d_work);
     if (ctx->h_status) cudaFreeHost(ctx->h_status);
@@ -290,6 +301,8 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->d_blocks_choice) cudaFree(ctx->d_blocks_choice);
     if (ctx->d_blocks_geom) cudaFree(ctx->d_blocks_geom);
     if (ctx->d_stored_geom) cudaFree(ctx->d_stored_geom);
+    if (ctx->d_planes_enc) cudaFree(ctx->d_planes_enc);
+    if (ctx->d_planes_dec) cudaFree(ctx->d_planes_dec);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -2415,6 +2428,114 @@ extern "C" int rb200_container_stored_encode_varlen_async(rb200_ctx* ctx, const 
         if (!model_encode_args_ok(ctx, static_cast<int>(candidates[i] >> 8), candidates[i] & 0xffu, in, n_max, chunk_syms, out))
             return RB200_E_ARG;
     return stored_encode(ctx, plan_auto(candidates, n_candidates, tolerance_ppm), in, n_max, d_n, chunk_syms, flags, out, out_cap);
+}
+
+namespace {
+
+// a grid of every CTA of the byte-plane kernels that is resident at once: they stride over what they move
+uint32_t planes_grid(const rb200_ctx* ctx) { return static_cast<uint32_t>(ctx->sms) * kPlanesCtasPerSm; }
+
+int launch_split(rb200_ctx* ctx, uint32_t w, const uint8_t* in, uint64_t m, uint8_t* planes, uint64_t stride)
+{
+    auto split = w == 2 ? planes_split_kernel<2> : w == 4 ? planes_split_kernel<4> : planes_split_kernel<8>;
+    split<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(in, m, planes, stride);
+    return check_launch(ctx, "planes_split_kernel");
+}
+
+int launch_interleave(rb200_ctx* ctx, uint32_t w, const uint8_t* planes, uint64_t stride, uint8_t* out, const PlanesWork* r)
+{
+    auto interleave = w == 2 ? planes_interleave_kernel<2> : w == 4 ? planes_interleave_kernel<4> : planes_interleave_kernel<8>;
+    interleave<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(planes, stride, out, r);
+    return check_launch(ctx, "planes_interleave_kernel");
+}
+
+}  // namespace
+
+// The split, then per plane the whole version 6 encode (stored_encode, unchanged) and a place kernel, then the version
+// 7 header: 2 + w * (11 to 15) launches and w memsets, no copy, no synchronisation.  Plane 0 is encoded in place; the
+// others into one staging area of rb200_container_stored_bound(n / w) bytes, from which their place kernel copies them
+// to the end of the previous plane, whose size only the device knows.
+extern "C" int rb200_container_planes_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                                   uint32_t elem_bytes, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags,
+                                                   uint8_t* out, size_t out_cap)
+{
+    const uint32_t w = elem_bytes;
+    if (!container_planes_w_ok(w) || n == 0 || n % w || ((n / w) >> 32) || (reinterpret_cast<uintptr_t>(in) & 15)) return RB200_E_ARG;
+    const size_t m = n / w;
+    if (!candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
+    for (uint32_t i = 0; i < n_candidates; i++)
+        if (!model_encode_args_ok(ctx, static_cast<int>(candidates[i] >> 8), candidates[i] & 0xffu, in, m, chunk_syms, out)) return RB200_E_ARG;
+    const size_t plane_cap = rb200_container_stored_bound(m, chunk_syms), table_end = container_planes_table_end(w);
+    if (out_cap < rb200_container_planes_bound(n, w, chunk_syms)) return RB200_E_SPACE;
+    DeviceGuard g(ctx->device);
+    const uint64_t stride = round16(m);
+    int rc = reserve(ctx, ctx->planes_in, w * stride);
+    if (rc == RB200_OK) rc = reserve(ctx, ctx->planes_enc_stage, plane_cap);
+    if (rc != RB200_OK) return rc;
+    uint8_t* planes = static_cast<uint8_t*>(ctx->planes_in.p);
+    uint8_t* stage = static_cast<uint8_t*>(ctx->planes_enc_stage.p);
+    const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
+    rc = launch_split(ctx, w, in, m, planes, stride);
+    for (uint32_t p = 0; p < w && rc == RB200_OK; p++) {
+        uint8_t* dst = p ? stage : out + table_end;
+        rc = stored_encode(ctx, a, planes + p * stride, m, nullptr, chunk_syms, flags, dst, plane_cap);
+        if (rc != RB200_OK) break;
+        planes_place_kernel<<<p ? planes_grid(ctx) : 1, kPlanesThreads, 0, ctx->stream>>>(out, dst, p, w, out_cap, ctx->d_planes_enc,
+                                                                                         ctx->d_status);
+        rc = check_launch(ctx, "planes_place_kernel");
+    }
+    if (rc != RB200_OK) return rc;
+    ContainerHeader h{};
+    h.magic = kContainerMagic;
+    h.version = kContainerVersionPlanes;
+    h.lanes = RB200_LANES;
+    h.chunk_syms = chunk_syms;
+    h.n_symbols = n;
+    h.flags = flags;
+    h.block_size = h.n_blocks = w;
+    planes_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, ctx->d_planes_enc, ctx->d_status);
+    return check_launch(ctx, "planes_finish_kernel");
+}
+
+// The plan kernel, then per plane the whole version 6 async decode (container_decode_async, unchanged) into a
+// workspace -- plane 0 in place, the others after a fetch into staging -- and a record kernel, then the verdict and the
+// interleave: 2 + 19 w launches, no copy, no synchronisation.
+extern "C" int rb200_container_planes_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size, uint8_t* out,
+                                                   size_t out_cap, uint64_t* d_n_symbols)
+{
+    const uint32_t w = elem_bytes;
+    if (!container_planes_w_ok(w) || !async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    DeviceGuard g(ctx->device);
+    const uint64_t table_end = container_planes_table_end(w);
+    // every plane of n <= out_cap bytes has n / w <= out_cap / w symbols, and fewer than 2^32
+    const uint64_t stride = round16(std::min<uint64_t>(out_cap / w, 0xffffffffull));
+    const uint64_t stage_cap = round16(std::max<uint64_t>(size > table_end ? size - table_end : 0, sizeof(ContainerHeader)));
+    int rc = reserve(ctx, ctx->planes_out, std::max<uint64_t>(w * stride, 16));
+    if (rc == RB200_OK) rc = reserve(ctx, ctx->planes_dec_stage, stage_cap);
+    if (rc != RB200_OK) return rc;
+    uint8_t* planes = static_cast<uint8_t*>(ctx->planes_out.p);
+    uint8_t* stage = static_cast<uint8_t*>(ctx->planes_dec_stage.p);
+    PlanesWork* r = ctx->d_planes_dec;
+    cudaStream_t s = ctx->stream;
+    planes_plan_kernel<<<1, 32, 0, s>>>(buf, size, w, r);
+    rc = check_launch(ctx, "planes_plan_kernel");
+    for (uint32_t p = 0; p < w && rc == RB200_OK; p++) {
+        if (p) {
+            planes_fetch_kernel<<<planes_grid(ctx), kPlanesThreads, 0, s>>>(buf, stage, stage_cap, p, r);
+            rc = check_launch(ctx, "planes_fetch_kernel");
+            if (rc == RB200_OK) rc = container_decode_async(ctx, kContainerVersionStored, stage, stage_cap, planes + p * stride, stride, nullptr);
+        } else {
+            rc = container_decode_async(ctx, kContainerVersionStored, buf + table_end, size > table_end ? size - table_end : 0, planes, stride,
+                                        nullptr);
+        }
+        if (rc != RB200_OK) break;
+        planes_record_kernel<<<1, 32, 0, s>>>(p, ctx->d_async[kContainerVersionStored - 1], r);
+        rc = check_launch(ctx, "planes_record_kernel");
+    }
+    if (rc != RB200_OK) return rc;
+    planes_verdict_kernel<<<1, 32, 0, s>>>(w, out_cap, d_n_symbols, r, ctx->d_status);
+    rc = check_launch(ctx, "planes_verdict_kernel");
+    return rc == RB200_OK ? launch_interleave(ctx, w, planes, stride, out, r) : rc;
 }
 
 extern "C" int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n)

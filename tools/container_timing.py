@@ -90,11 +90,18 @@ chosen pair alone, and at *d_n = n_max / 16 against the fixed call at that lengt
 kernels.  With --blocks-stored-varlen, the same for rb200_container_blocks_stored_encode_varlen_async (n_blocks_max =
 8192 blocks of 64 KiB, the sixteenth at 512 blocks) on the --blocks-stored workloads.
 
+With --planes, rb200_container_planes_encode_async and rb200_container_planes_decode_async (version 7, one version 6
+container per byte plane) against rb200_container_stored_encode_async and rb200_container_stored_decode_async (version 6)
+on the same 1 GiB of bf16 and of fp32 N(0, 0.02) data in device memory, chunks of 8192, {word 12, alias 16, byte 14} at
+2 %, flags 0, alternated: bytes per input byte, encode and decode times, the version 7 minus version 6 time per GiB, a
+torch.profiler list of the version 7 calls' kernels, and the split and interleave kernels' rate (2n bytes moved each)
+against 3.35 TB/s.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
     python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto | --blocks-auto
                                       | --blocks-varlen | --blocks-stored | --stored | --stored-varlen
-                                      | --blocks-stored-varlen] [--reps 10]
+                                      | --blocks-stored-varlen | --planes] [--reps 10]
                                      [--json out.json]"""
 import argparse
 import json
@@ -1213,6 +1220,66 @@ def blocks_stored_varlen(args):
     return res
 
 
+def planes(args):
+    """version 7 against version 6 on the same bytes: bf16 and fp32 N(0, 0.02), 1 GiB each"""
+    import torch
+    n, chunk, tol = 1 << 30, 8192, 20000
+    cands = [api.CANDIDATE(rb.CODER_WORD, 12), api.CANDIDATE(rb.CODER_ALIAS, 16), api.CANDIDATE(rb.CODER_BYTE, 14)]
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    v6_bound = api.container_stored_bound(n, chunk)
+    d_v6 = torch.empty(v6_bound + 16, dtype=torch.uint8, device="cuda")
+    d_dec = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+    res = {"card": card(), "workload": {"n": n, "chunk_syms": chunk}, "candidates": ["word 12", "alias 16", "byte 14"], "tolerance_ppm": tol,
+           "workloads": {}, "checks": {}}
+    gen = torch.Generator(device="cuda").manual_seed(4321)
+    for name, dtype, w in (("bf16", torch.bfloat16, 2), ("fp32", torch.float32, 4)):
+        d_in = (torch.randn(n // w, device="cuda", generator=gen) * 0.02).to(dtype).view(torch.uint8)
+        bound = api.container_planes_bound(n, w, chunk)
+        d_v7 = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+        i, o6, o7, dd = d_in.data_ptr(), d_v6.data_ptr(), d_v7.data_ptr(), d_dec.data_ptr()
+        enc = {"v7_encode": lambda: ctx.container_planes_encode_async(cands, tol, w, i, n, chunk, 0, o7, bound),
+               "v6_encode": lambda: ctx.container_stored_encode_async(cands, tol, i, n, chunk, 0, o6, v6_bound)}
+        times = alternate(enc, sync, args.warmup, args.reps)
+        for f in enc.values():
+            f()
+        sync()
+        h7, h6 = d_v7[:64 + 16 * w].cpu().numpy(), d_v6[:64].cpu().numpy()
+        size7 = 64 + 16 * w + int(h7[32:40].view(np.uint64)[0])
+        n_chunks = int(h6[24:32].view(np.uint64)[0])
+        size6 = ((1088 + 8 * (n_chunks + 1) + 15) & ~15) + 16 * ((n_chunks + 127) // 128) + int(h6[32:40].view(np.uint64)[0])
+        table = h7[64:].view(np.uint64).reshape(w, 2)
+        res["checks"][f"{name}: v7_within_bound"] = size7 <= bound
+        dec = {"v7_decode": lambda: ctx.container_planes_decode_async(w, o7, size7, dd, n),
+               "v6_decode": lambda: ctx.container_stored_decode_async(o6, size6, dd, n)}
+        dtimes = alternate(dec, sync, args.warmup, args.reps)
+        for k, f in dec.items():
+            d_dec.zero_()
+            f()
+            sync()
+            res["checks"][f"{name}: {k}_round_trip"] = bool(torch.equal(d_dec[:n], d_in))
+        ek = kernel_times(enc["v7_encode"], sync, args.reps)
+        dk = kernel_times(dec["v7_decode"], sync, args.reps)
+
+        def rate(kernels, part):
+            us = sum(v["median_us"] * v["launches_per_call"] for k, v in kernels.items() if part in k)
+            return {"us": us, "TB_per_s": 2 * n / us / 1e6 if us else None, "share_of_3.35_TB_per_s": 2 * n / us / 1e6 / 3.35 if us else None}
+
+        res["workloads"][name] = {
+            "bytes_per_input_byte": {"v7": size7 / n, "v6": size6 / n},
+            "plane_bytes_per_symbol": [int(table[p, 1]) / (n // w) for p in range(w)],
+            "plane_coders": [int(h) for h in (d_v7[int(table[p, 0]) + 6].item() for p in range(w))],
+            "encode": times, "decode": dtimes,
+            "v7_minus_v6_encode_ms_per_GiB": times["v7_encode"]["median_ms"] - times["v6_encode"]["median_ms"],
+            "v7_minus_v6_decode_ms_per_GiB": dtimes["v7_decode"]["median_ms"] - dtimes["v6_decode"]["median_ms"],
+            "split_kernel": rate(ek, "planes_split_kernel"), "interleave_kernel": rate(dk, "planes_interleave_kernel"),
+            "v7_encode_kernels": ek, "v7_decode_kernels": dk,
+        }
+        del d_in, d_v7
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
@@ -1227,13 +1294,14 @@ def main():
     ap.add_argument("--stored", action="store_true", help="the single-model encode and decode with incompressible chunks stored (version 6)")
     ap.add_argument("--stored-varlen", action="store_true", help="the version 6 encode with the length in device memory")
     ap.add_argument("--blocks-stored-varlen", action="store_true", help="the version 5 encode with the block count in device memory")
+    ap.add_argument("--planes", action="store_true", help="the byte-plane container (version 7) against version 6 on bf16 and fp32")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else stored_varlen(args) if args.stored_varlen else blocks_stored_varlen(args) if args.blocks_stored_varlen else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else stored_varlen(args) if args.stored_varlen else blocks_stored_varlen(args) if args.blocks_stored_varlen else planes(args) if args.planes else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
