@@ -499,6 +499,26 @@ int rb200_container_planes_open(const uint8_t* buf, size_t size, rb200_container
 int rb200_container_planes_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
                                         uint32_t elem_bytes, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags,
                                         uint8_t* out, size_t out_cap);
+/* rb200_container_planes_encode_async with the length in bytes read from device memory when the work runs: for
+ * 1 <= *d_n <= n_max with *d_n a multiple of w = elem_bytes, the container is byte for byte (header included) what the
+ * fixed call writes for n = *d_n with the same arguments, so one captured graph writes a version 7 container of any
+ * such length.  Only the first *d_n bytes of in are read and nothing at or past the container's end (64 + 16 w +
+ * blob_bytes) is written.  n_max fixes the launch shapes and the workspaces; rb200_container_planes_bound is monotone
+ * in n, so out_cap >= rb200_container_planes_bound(n_max, w, chunk_syms) means rb200_sync never returns
+ * RB200_E_SPACE, whatever the length.  d_n is device memory, 8-byte aligned.  The call returns RB200_E_ARG (nothing
+ * launched) for everything the fixed call refuses, checked with n_max for n (n_max not a multiple of w, n_max / w >=
+ * 2^32, every candidate at n_max / w symbols, a misaligned in), for a null or misaligned d_n and for n_max == 0;
+ * RB200_E_SPACE (nothing launched) when out_cap is below rb200_container_planes_bound(n_max, w, chunk_syms).
+ * rb200_sync returns RB200_E_ARG when *d_n is 0, not a multiple of w or above n_max (the fixed call's verdict for such
+ * an n), and then out is not written at all; every other verdict is the fixed call's, the first failing plane's with
+ * the version 7 header unwritten.  The call only enqueues work (no copy, synchronisation or allocation); the
+ * workspaces grow for n_max, so a call with the same list, elem_bytes, chunk_syms and n_max outside a capture must
+ * come first.  The version 7 decode needs no device-length form: captured with size = the bound, it reads every
+ * shorter container. */
+int rb200_container_planes_encode_varlen_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                               uint32_t tolerance_ppm, uint32_t elem_bytes, const uint8_t* in,
+                                               const uint64_t* d_n, size_t n_max, uint32_t chunk_syms, uint32_t flags,
+                                               uint8_t* out, size_t out_cap);
 /* The contract of rb200_container_stored_decode_async for version 7, with the element width the caller expects: kernels
  * check the header (its w must be elem_bytes), the table and meta_crc, and every plane through version 6's checks and
  * decoders, into a workspace of min(out_cap, w * 2^32) bytes; only when every check has passed does one kernel

@@ -120,6 +120,8 @@ EXPORTS = [
     ("rb200_container_planes_open", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
     ("rb200_container_planes_encode_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,
                                                       C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_container_planes_encode_varlen_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
+                                                             C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_container_planes_decode_async", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
                                                       C.c_void_p]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
@@ -688,6 +690,19 @@ class Context:
         cands = _candidates(candidates)
         self.lib.check(self.lib.dll.rb200_container_planes_encode_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
                                                                         elem_bytes, in_ptr, n, chunk_syms, flags, out_ptr, out_cap), self.h)
+
+    def container_planes_encode_varlen_async(self, candidates, tolerance_ppm, elem_bytes, in_ptr, n_ptr, n_max, chunk_syms, flags, out_ptr,
+                                             out_cap):
+        """container_planes_encode_async with the length in bytes read from device memory when the work runs: n_ptr is
+        the device address of a u64 n, 1 <= n <= n_max and a multiple of elem_bytes.  n_max fixes the launch shapes and
+        the workspaces, so one captured call serves every such n, and out_cap = container_planes_bound(n_max,
+        elem_bytes, chunk_syms) holds every one (never -3 from sync()).  The verdict comes from sync(): -1 for an n of
+        0, not a multiple of elem_bytes or above n_max, with out untouched; otherwise container_planes_encode_async's
+        (the first failing plane's, header unwritten)"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_planes_encode_varlen_async(self.h, cands.ctypes.data_as(_u32p), cands.size,
+                                                                               tolerance_ppm, elem_bytes, in_ptr, n_ptr, n_max, chunk_syms,
+                                                                               flags, out_ptr, out_cap), self.h)
 
     def container_planes_decode_async(self, elem_bytes, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
         """enqueue only (CUDA-graph capturable once a call of the same size and out_cap has grown the workspaces): a

@@ -12,6 +12,12 @@
 //   for p = 1 .. W-1: plane p's version 6 encode into a staging area, then planes_place_kernel(p): its verdict, its size
 //                               from its header, its offset from entry p - 1, the copy to there and its table entry
 //   planes_finish_kernel        the version 7 header and meta_crc, only when every plane was placed
+// Encode with the length in device memory (rb200_container_planes_encode_varlen_async), launch shapes and workspaces
+// sized for n_max:
+//   planes_varlen_plan_kernel   *d_n checked, n and the plane length m into the context's PlanesVarlenGeom
+//   planes_split_varlen_kernel<W>  the split body with m from the record, at the stride round16(n_max / W)
+//   per plane: version 6's varlen encode with &geom->m as its length, then planes_place_kernel, as above
+//   planes_finish_varlen_kernel the finish body with n from the record
 // Decode:
 //   planes_plan_kernel          the header (its W must be the caller's), the table, every plane's header and meta_crc,
 //                               into the call's record
@@ -36,6 +42,15 @@ struct PlanesWork {
     uint32_t ok;                // decode: the header, the table, every plane's header and meta_crc passed
     uint32_t go;                // decode: every check passed; the interleave runs
     uint32_t plane_go[8];       // encode: plane p was written and placed; decode: plane p's version 6 verdict passed
+};
+
+// The length of rb200_container_planes_encode_varlen_async, in device memory: written by planes_varlen_plan_kernel from
+// *d_n at every run, read by the split, by every plane's version 6 varlen encode (m is its length) and by the finish.
+// For a bad *d_n, n is 0 and m is UINT64_MAX, above every plane's bound: version 6's plan then refuses it (kStatArg)
+// and writes nothing, so no plane is placed and no header written.
+struct PlanesVarlenGeom {
+    uint64_t n;                 // input bytes, 1 <= n <= n_max and a multiple of w; 0 for a bad *d_n
+    uint64_t m;                 // symbols per plane, n / w; UINT64_MAX for a bad *d_n
 };
 
 constexpr uint32_t kPlanesThreads = 256;
@@ -79,8 +94,7 @@ __device__ __forceinline__ void planes_untranspose(const uint32_t (&y)[4 * W], u
 // in (m elements of W bytes, 16-byte aligned) -> plane k at planes + k * stride (stride a multiple of 16).  Grid-stride
 // over groups of 16 elements; the ragged end (fewer than 16 elements) a byte per thread.
 template <int W>
-__global__ void __launch_bounds__(kPlanesThreads)
-    planes_split_kernel(const uint8_t* __restrict__ in, uint64_t m, uint8_t* __restrict__ planes, uint64_t stride)
+__device__ __forceinline__ void planes_split(const uint8_t* __restrict__ in, uint64_t m, uint8_t* __restrict__ planes, uint64_t stride)
 {
     const uint64_t groups = m / 16, step = static_cast<uint64_t>(gridDim.x) * blockDim.x;
     const uint64_t tid = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -105,6 +119,24 @@ __global__ void __launch_bounds__(kPlanesThreads)
         const uint64_t e = tail + tid / W, k = tid % W;
         planes[k * stride + e] = in[e * W + k];
     }
+}
+
+template <int W>
+__global__ void __launch_bounds__(kPlanesThreads)
+    planes_split_kernel(const uint8_t* __restrict__ in, uint64_t m, uint8_t* __restrict__ planes, uint64_t stride)
+{
+    planes_split<W>(in, m, planes, stride);
+}
+
+// The split of the varlen encode: m from the record, nothing for a bad length.  The grid is the fixed call's, so a
+// short length costs no extra CTAs.
+template <int W>
+__global__ void __launch_bounds__(kPlanesThreads)
+    planes_split_varlen_kernel(const uint8_t* __restrict__ in, const PlanesVarlenGeom* __restrict__ g, uint8_t* __restrict__ planes,
+                               uint64_t stride)
+{
+    if (g->n == 0) return;
+    planes_split<W>(in, g->m, planes, stride);
 }
 
 // The inverse, from the decode workspace into out: n from the record, and nothing unless every check passed.
@@ -180,11 +212,10 @@ __device__ __forceinline__ uint32_t planes_meta_crc(const uint8_t* s, uint32_t b
 }
 
 // Encode: the version 7 header, when every plane was placed and the status word is still clear.  h arrives complete
-// but for blob_bytes and meta_crc.
-__global__ void __launch_bounds__(32)
-    planes_finish_kernel(uint8_t* out, ContainerHeader h, const PlanesWork* __restrict__ r, const uint32_t* status)
+// but for blob_bytes and meta_crc; s_v is the kernel's shared staging of header and table.
+__device__ __forceinline__ void planes_finish(uint4* s_v, uint8_t* out, ContainerHeader h, const PlanesWork* __restrict__ r,
+                                              const uint32_t* status)
 {
-    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
     uint8_t* s = reinterpret_cast<uint8_t*>(s_v);
     const uint32_t lane = threadIdx.x, w = h.block_size;
     bool all = *status == 0;
@@ -202,6 +233,35 @@ __global__ void __launch_bounds__(32)
     if (lane == 0) reinterpret_cast<ContainerHeader*>(s)->meta_crc = meta;
     __syncwarp();
     if (lane < 4) reinterpret_cast<uint4*>(out)[lane] = s_v[lane];
+}
+
+__global__ void __launch_bounds__(32)
+    planes_finish_kernel(uint8_t* out, ContainerHeader h, const PlanesWork* __restrict__ r, const uint32_t* status)
+{
+    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
+    planes_finish(s_v, out, h, r, status);
+}
+
+// The finish of the varlen encode: n from the record.  A bad length left the status word set, so nothing is written.
+__global__ void __launch_bounds__(32)
+    planes_finish_varlen_kernel(uint8_t* out, ContainerHeader h, const PlanesVarlenGeom* __restrict__ g, const PlanesWork* __restrict__ r,
+                                const uint32_t* status)
+{
+    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
+    h.n_symbols = g->n;
+    planes_finish(s_v, out, h, r, status);
+}
+
+// The first kernel of the varlen encode, one thread: reads n = *d_n and writes n and m = n / w into *g when
+// 1 <= n <= n_max and w divides n; otherwise n = 0 and m = UINT64_MAX, which every plane's version 6 varlen plan
+// refuses as above its bound (kStatArg, the fixed call's RB200_E_ARG for n == 0 or n % w != 0), writing nothing.
+__global__ void __launch_bounds__(32)
+    planes_varlen_plan_kernel(const uint64_t* __restrict__ d_n, uint64_t n_max, uint32_t w, PlanesVarlenGeom* __restrict__ g)
+{
+    if (threadIdx.x) return;
+    const uint64_t n = *d_n;
+    const bool ok = n != 0 && n <= n_max && n % w == 0;
+    *g = ok ? PlanesVarlenGeom{n, n / w} : PlanesVarlenGeom{0, UINT64_MAX};
 }
 
 // Decode: every version 7 rule on the header, the table and the planes' headers, and meta_crc; the record is reset

@@ -84,6 +84,8 @@ struct rb200_ctx {
     PlanesWork* d_planes_enc = nullptr;
     PlanesWork* d_planes_dec = nullptr;
     DevBuf planes_in, planes_enc_stage, planes_out, planes_dec_stage;
+    // rb200_container_planes_encode_varlen_async: the length its plan kernel read
+    PlanesVarlenGeom* d_planes_geom = nullptr;
 };
 
 struct rb200_model {
@@ -261,6 +263,8 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
         if (e == cudaSuccess) e = cudaMalloc(r, sizeof(PlanesWork));
         if (e == cudaSuccess) e = cudaMemset(*r, 0, sizeof(PlanesWork));
     }
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_planes_geom, sizeof(PlanesVarlenGeom));
+    if (e == cudaSuccess) e = cudaMemset(ctx->d_planes_geom, 0, sizeof(PlanesVarlenGeom));
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -303,6 +307,7 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->d_stored_geom) cudaFree(ctx->d_stored_geom);
     if (ctx->d_planes_enc) cudaFree(ctx->d_planes_enc);
     if (ctx->d_planes_dec) cudaFree(ctx->d_planes_dec);
+    if (ctx->d_planes_geom) cudaFree(ctx->d_planes_geom);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -2435,8 +2440,14 @@ namespace {
 // a grid of every CTA of the byte-plane kernels that is resident at once: they stride over what they move
 uint32_t planes_grid(const rb200_ctx* ctx) { return static_cast<uint32_t>(ctx->sms) * kPlanesCtasPerSm; }
 
-int launch_split(rb200_ctx* ctx, uint32_t w, const uint8_t* in, uint64_t m, uint8_t* planes, uint64_t stride)
+// geom set: the varlen split, m from the record
+int launch_split(rb200_ctx* ctx, uint32_t w, const uint8_t* in, uint64_t m, const PlanesVarlenGeom* geom, uint8_t* planes, uint64_t stride)
 {
+    if (geom) {
+        auto split = w == 2 ? planes_split_varlen_kernel<2> : w == 4 ? planes_split_varlen_kernel<4> : planes_split_varlen_kernel<8>;
+        split<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(in, geom, planes, stride);
+        return check_launch(ctx, "planes_split_varlen_kernel");
+    }
     auto split = w == 2 ? planes_split_kernel<2> : w == 4 ? planes_split_kernel<4> : planes_split_kernel<8>;
     split<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(in, m, planes, stride);
     return check_launch(ctx, "planes_split_kernel");
@@ -2449,17 +2460,16 @@ int launch_interleave(rb200_ctx* ctx, uint32_t w, const uint8_t* planes, uint64_
     return check_launch(ctx, "planes_interleave_kernel");
 }
 
-}  // namespace
-
 // The split, then per plane the whole version 6 encode (stored_encode, unchanged) and a place kernel, then the version
-// 7 header: 2 + w * (11 to 15) launches and w memsets, no copy, no synchronisation.  Plane 0 is encoded in place; the
-// others into one staging area of rb200_container_stored_bound(n / w) bytes, from which their place kernel copies them
-// to the end of the previous plane, whose size only the device knows.
-extern "C" int rb200_container_planes_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
-                                                   uint32_t elem_bytes, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags,
-                                                   uint8_t* out, size_t out_cap)
+// 7 header.  Plane 0 is encoded in place; the others into one staging area of rb200_container_stored_bound(n / w)
+// bytes, from which their place kernel copies them to the end of the previous plane, whose size only the device knows.
+// d_n set (rb200_container_planes_encode_varlen_async): n is the bound n_max, which sizes the workspaces, the planes'
+// stride and every version 6 encode's bound; planes_varlen_plan_kernel reads *d_n into the context's PlanesVarlenGeom
+// first, the split and the finish are their varlen forms, and every plane's version 6 encode is the varlen one, with
+// the record's m as its length.  Arguments are checked here, with n_max for n.
+int planes_encode(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm, uint32_t w, const uint8_t* in,
+                  size_t n, const uint64_t* d_n, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
 {
-    const uint32_t w = elem_bytes;
     if (!container_planes_w_ok(w) || n == 0 || n % w || ((n / w) >> 32) || (reinterpret_cast<uintptr_t>(in) & 15)) return RB200_E_ARG;
     const size_t m = n / w;
     if (!candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
@@ -2474,11 +2484,17 @@ extern "C" int rb200_container_planes_encode_async(rb200_ctx* ctx, const uint32_
     if (rc != RB200_OK) return rc;
     uint8_t* planes = static_cast<uint8_t*>(ctx->planes_in.p);
     uint8_t* stage = static_cast<uint8_t*>(ctx->planes_enc_stage.p);
+    PlanesVarlenGeom* geom = d_n ? ctx->d_planes_geom : nullptr;
     const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
-    rc = launch_split(ctx, w, in, m, planes, stride);
+    if (geom) {
+        planes_varlen_plan_kernel<<<1, 32, 0, ctx->stream>>>(d_n, n, w, geom);
+        rc = check_launch(ctx, "planes_varlen_plan_kernel");
+        if (rc != RB200_OK) return rc;
+    }
+    rc = launch_split(ctx, w, in, m, geom, planes, stride);
     for (uint32_t p = 0; p < w && rc == RB200_OK; p++) {
         uint8_t* dst = p ? stage : out + table_end;
-        rc = stored_encode(ctx, a, planes + p * stride, m, nullptr, chunk_syms, flags, dst, plane_cap);
+        rc = stored_encode(ctx, a, planes + p * stride, m, geom ? &geom->m : nullptr, chunk_syms, flags, dst, plane_cap);
         if (rc != RB200_OK) break;
         planes_place_kernel<<<p ? planes_grid(ctx) : 1, kPlanesThreads, 0, ctx->stream>>>(out, dst, p, w, out_cap, ctx->d_planes_enc,
                                                                                          ctx->d_status);
@@ -2493,8 +2509,34 @@ extern "C" int rb200_container_planes_encode_async(rb200_ctx* ctx, const uint32_
     h.n_symbols = n;
     h.flags = flags;
     h.block_size = h.n_blocks = w;
+    if (geom) {
+        planes_finish_varlen_kernel<<<1, 32, 0, ctx->stream>>>(out, h, geom, ctx->d_planes_enc, ctx->d_status);
+        return check_launch(ctx, "planes_finish_varlen_kernel");
+    }
     planes_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, ctx->d_planes_enc, ctx->d_status);
     return check_launch(ctx, "planes_finish_kernel");
+}
+
+}  // namespace
+
+// planes_encode without a device length: 2 + w * (11 to 15) launches and w memsets, no copy, no synchronisation.
+extern "C" int rb200_container_planes_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                                   uint32_t elem_bytes, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags,
+                                                   uint8_t* out, size_t out_cap)
+{
+    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, n, nullptr, chunk_syms, flags, out, out_cap);
+}
+
+// rb200_container_planes_encode_async with the length read from device memory at every run: the plan kernel, the
+// varlen split, per plane version 6's varlen encode and the place kernel, the varlen finish, all sized for n_max: the
+// fixed call's launches plus the plan kernel, plus w version 6 plan kernels, plus w blob-length kernels with the blob
+// CRC.
+extern "C" int rb200_container_planes_encode_varlen_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates,
+                                                          uint32_t tolerance_ppm, uint32_t elem_bytes, const uint8_t* in, const uint64_t* d_n,
+                                                          size_t n_max, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    if (!d_n || (reinterpret_cast<uintptr_t>(d_n) & 7) || n_max == 0) return RB200_E_ARG;
+    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, n_max, d_n, chunk_syms, flags, out, out_cap);
 }
 
 // The plan kernel, then per plane the whole version 6 async decode (container_decode_async, unchanged) into a

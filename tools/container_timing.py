@@ -97,11 +97,16 @@ on the same 1 GiB of bf16 and of fp32 N(0, 0.02) data in device memory, chunks o
 torch.profiler list of the version 7 calls' kernels, and the split and interleave kernels' rate (2n bytes moved each)
 against 3.35 TB/s.
 
+With --planes-varlen, rb200_container_planes_encode_varlen_async (n_max = 1 GiB) against rb200_container_planes_encode_async
+on the --planes data, flags 0 and RB200_CONTAINER_CRC_BLOB, alternated: at *d_n = n_max and at *d_n = n_max / 16, each
+against the fixed call at that length, after checking that both wrote the same bytes; varlen minus fixed in total and
+per plane, and a torch.profiler list of both calls' kernels.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
     python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto | --blocks-auto
                                       | --blocks-varlen | --blocks-stored | --stored | --stored-varlen
-                                      | --blocks-stored-varlen | --planes] [--reps 10]
+                                      | --blocks-stored-varlen | --planes | --planes-varlen] [--reps 10]
                                      [--json out.json]"""
 import argparse
 import json
@@ -1280,6 +1285,57 @@ def planes(args):
     return res
 
 
+def planes_varlen(args):
+    """rb200_container_planes_encode_varlen_async (n_max = 1 GiB, chunks of 8192) against the fixed plane call on bf16
+    and fp32 N(0, 0.02): at *d_n = n_max and at *d_n = n_max / 16 against the fixed call at that length"""
+    import torch
+    n_max, chunk, tol = 1 << 30, 8192, 20000
+    cands = [api.CANDIDATE(rb.CODER_WORD, 12), api.CANDIDATE(rb.CODER_ALIAS, 16), api.CANDIDATE(rb.CODER_BYTE, 14)]
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    d_n = torch.tensor([n_max, n_max // 16], dtype=torch.int64, device="cuda")
+    res = {"card": card(), "workload": {"n_max": n_max, "chunk_syms": chunk}, "candidates": ["word 12", "alias 16", "byte 14"],
+           "tolerance_ppm": tol, "workloads": {}, "checks": {}}
+    gen = torch.Generator(device="cuda").manual_seed(4321)
+    for name, dtype, w in (("bf16", torch.bfloat16, 2), ("fp32", torch.float32, 4)):
+        d_in = (torch.randn(n_max // w, device="cuda", generator=gen) * 0.02).to(dtype).view(torch.uint8)
+        bound = api.container_planes_bound(n_max, w, chunk)
+        d_ref = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+        d_out = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+        i, r, o = d_in.data_ptr(), d_ref.data_ptr(), d_out.data_ptr()
+
+        def size(d, w=w):
+            return 64 + 16 * w + int(d[32:40].cpu().numpy().view(np.uint64)[0])
+
+        def same(d_ref=d_ref, d_out=d_out):
+            n = size(d_ref)
+            return size(d_out) == n and bool(torch.equal(d_out[:n], d_ref[:n]))
+
+        arms = {  # (varlen call, fixed call), each taking flags
+            "bound": (lambda fl: ctx.container_planes_encode_varlen_async(cands, tol, w, i, d_n.data_ptr(), n_max, chunk, fl, o, bound),
+                      lambda fl: ctx.container_planes_encode_async(cands, tol, w, i, n_max, chunk, fl, r, bound)),
+            "sixteenth": (lambda fl: ctx.container_planes_encode_varlen_async(cands, tol, w, i, d_n[1:].data_ptr(), n_max, chunk, fl, o, bound),
+                          lambda fl: ctx.container_planes_encode_async(cands, tol, w, i, n_max // 16, chunk, fl, r, bound)),
+        }
+        for arm, (varlen, fixed) in arms.items():                     # equal bytes before anything is timed
+            for tag, flags in (("", 0), ("_crc", api.CONTAINER_CRC_BLOB)):
+                d_out.fill_(0x5C)
+                torch.cuda.synchronize()
+                varlen(flags)
+                fixed(flags)
+                sync()
+                res["checks"][f"{name} {arm}{tag}: varlen_equals_fixed_call_before_timing"] = same()
+        res["workloads"][name] = varlen_arms(res, name, arms, sync, args, same)
+        for arm in arms:
+            for tag in ("", "_crc"):
+                res["workloads"][name][arm + tag]["varlen_minus_fixed_per_plane_us"] = (
+                    res["workloads"][name][arm + tag]["varlen_minus_fixed_median_us"] / w)
+        del d_in, d_ref, d_out
+        torch.cuda.empty_cache()
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
@@ -1295,13 +1351,14 @@ def main():
     ap.add_argument("--stored-varlen", action="store_true", help="the version 6 encode with the length in device memory")
     ap.add_argument("--blocks-stored-varlen", action="store_true", help="the version 5 encode with the block count in device memory")
     ap.add_argument("--planes", action="store_true", help="the byte-plane container (version 7) against version 6 on bf16 and fp32")
+    ap.add_argument("--planes-varlen", action="store_true", help="the byte-plane encode with the length in device memory, on bf16 and fp32")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else stored_varlen(args) if args.stored_varlen else blocks_stored_varlen(args) if args.blocks_stored_varlen else planes(args) if args.planes else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else stored_varlen(args) if args.stored_varlen else blocks_stored_varlen(args) if args.blocks_stored_varlen else planes(args) if args.planes else planes_varlen(args) if args.planes_varlen else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
