@@ -44,6 +44,7 @@ extern "C" {
 #define RB200_E_NCCL     -8   /* NCCL missing or an NCCL call failed, see rb200_last_cuda_error */
 #define RB200_E_STALL    -9   /* a bounded wait inside a kernel (8 s without progress) expired: a bug or a wedged
                                  device, never bad input -- the kernels give up instead of hanging the GPU            */
+#define RB200_E_BASE    -10   /* a delta container's base is not the tensor it was encoded against (its CRC differs)  */
 
 /* which memory the data pointers of a bulk call live in */
 #define RB200_MEM_HOST    0   /* host pointers; the call copies H2D/D2H and is synchronous */
@@ -530,6 +531,40 @@ int rb200_container_planes_encode_varlen_async(rb200_ctx* ctx, const uint32_t* c
  * Capturable after one call of the same size and out_cap outside the capture (the workspaces grow). */
 int rb200_container_planes_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size, uint8_t* out,
                                         size_t out_cap, uint64_t* d_n_symbols);
+
+/* ---------------------------------------------------------------- delta byte-plane containers */
+
+/* Version 8: a tensor of w-byte elements (w = elem_bytes, 2, 4 or 8) as its difference from a base tensor of the same n
+ * bytes that the receiver already holds (the previous checkpoint or weight sync).  The layout and every rule are
+ * version 7's, but for two header fields: version 8, and reserved = the CRC-32 (rb200_crc32's) of the base's n bytes,
+ * which meta_crc covers.  The planes hold d, not the input: for element i, with x and b the w-byte little-endian
+ * unsigned integers of the input and the base, s = (x - b) mod 2^(8w) read as signed and d = (s << 1) ^ (s >> (8w - 1))
+ * (arithmetic shift, mod 2^(8w)); byte k of d is in plane k.  The inverse x = b + ((d >> 1) ^ -(d & 1)) mod 2^(8w) is
+ * exact for every bit pattern (NaNs, infinities, sign changes, integer extremes).  An unchanged tensor gives constant
+ * zero planes.  Only the _delta_ calls accept version 8, and they accept no other version: a delta is never decoded
+ * as a whole tensor.  The size bound is rb200_container_planes_bound's.
+ *   pack / open: rb200_container_planes_pack / _open for version 8, with the base CRC as an argument / output. */
+int rb200_container_delta_pack(uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint32_t base_crc, uint8_t* out,
+                               size_t out_cap, size_t* out_size);
+int rb200_container_delta_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info, uint32_t* base_crc);
+/* rb200_container_planes_encode_async of the difference of in from base (both n bytes, DEVICE memory, 16-byte aligned):
+ * plane p is byte for byte what rb200_container_stored_encode_async writes for plane p of d.  The same refusals as that
+ * call, and RB200_E_ARG (nothing launched) for a null or misaligned base; out_cap >= rb200_container_planes_bound(n, w,
+ * chunk_syms).  Enqueue only, capturable in a CUDA graph after one call with the same list and geometry outside the
+ * capture (the workspaces grow). */
+int rb200_container_delta_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                       uint32_t elem_bytes, const uint8_t* in, const uint8_t* base, size_t n, uint32_t chunk_syms,
+                                       uint32_t flags, uint8_t* out, size_t out_cap);
+/* The contract of rb200_container_planes_decode_async for version 8, applying the delta to base (DEVICE memory, 16-byte
+ * aligned): out = base is allowed and applies it in place, so the receiver needs no second copy of its tensor.  Any
+ * other overlap of [out, out + out_cap) and [base, base + out_cap) is RB200_E_ARG, nothing launched.  After the
+ * header, the table and every plane pass, and n <= out_cap, a kernel takes the CRC of base's n bytes; a CRC other than
+ * the header's is RB200_E_BASE from rb200_sync.  out is written only after every check, the base's included, has
+ * passed, so a rejected buffer or a wrong base leaves out (and so an in-place base) untouched.  base is never read past
+ * the header's n, and not at all when the container is rejected or n > out_cap.  A corrupt container is
+ * RB200_E_STREAM and n > out_cap RB200_E_SPACE, as for version 7. */
+int rb200_container_delta_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size, const uint8_t* base,
+                                       uint8_t* out, size_t out_cap, uint64_t* d_n_symbols);
 
 /* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
  * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's

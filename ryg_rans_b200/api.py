@@ -124,6 +124,13 @@ EXPORTS = [
                                                              C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_container_planes_decode_async", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
                                                       C.c_void_p]),
+    ("rb200_container_delta_pack", C.c_int, [C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t,
+                                             C.POINTER(C.c_size_t)]),
+    ("rb200_container_delta_open", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, _u32p]),
+    ("rb200_container_delta_encode_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                     C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_container_delta_decode_async", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                     C.c_size_t, C.c_void_p]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -139,6 +146,8 @@ EXPORTS = [
     ("rb200_container_decode", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_int]),
 ]
 CONTAINER_CRC_BLOB = 1
+# status codes (include/rans_b200.h); rb200_strerror has the message of each
+E_ARG, E_MODEL, E_SPACE, E_STREAM, E_CUDA, E_NOMEM, E_SYMBOL, E_NCCL, E_STALL, E_BASE = range(-1, -11, -1)
 
 
 def CANDIDATE(coder, scale_bits):
@@ -295,6 +304,35 @@ def container_planes_open(buf):
     base = buf.ctypes.data
     planes = [buf[info.planes[p] - base:info.planes[p] - base + info.sizes[p]] for p in range(info.elem_bytes)]
     meta = {k: int(getattr(info, k)) for k in ("elem_bytes", "chunk_syms", "flags", "n")}
+    return meta, planes
+
+
+def container_delta_pack(planes, base_crc):
+    """rb200_container_delta_pack: a version 8 container from w = len(planes) version 6 containers of the planes of the
+    difference d (as container_planes_pack) and the CRC-32 of the base tensor's n bytes"""
+    lib = load()
+    planes = [np.ascontiguousarray(p, dtype=np.uint8) for p in planes]
+    w = len(planes)
+    ptrs = (C.c_void_p * max(w, 1))(*[p.ctypes.data for p in planes])
+    sizes = (C.c_size_t * max(w, 1))(*[p.size for p in planes])
+    out = np.zeros(64 + 16 * w + sum(p.size for p in planes), np.uint8)
+    size = C.c_size_t(0)
+    lib.check(lib.dll.rb200_container_delta_pack(w, ptrs, sizes, base_crc, out.ctypes.data, out.size, C.byref(size)))
+    return out[:size.value]
+
+
+def container_delta_open(buf):
+    """Returns (info dict with base_crc, planes) of a version 8 container: planes[p] is a view into buf of the version 6
+    container of plane p of the difference."""
+    lib = load()
+    buf = np.ascontiguousarray(buf, dtype=np.uint8)
+    info = ContainerPlanesInfo()
+    crc = C.c_uint32(0)
+    lib.check(lib.dll.rb200_container_delta_open(buf.ctypes.data, buf.size, C.byref(info), C.byref(crc)))
+    base = buf.ctypes.data
+    planes = [buf[info.planes[p] - base:info.planes[p] - base + info.sizes[p]] for p in range(info.elem_bytes)]
+    meta = {k: int(getattr(info, k)) for k in ("elem_bytes", "chunk_syms", "flags", "n")}
+    meta["base_crc"] = int(crc.value)
     return meta, planes
 
 
@@ -710,6 +748,24 @@ class Context:
         untouched) comes from sync()"""
         self.lib.check(self.lib.dll.rb200_container_planes_decode_async(self.h, elem_bytes, buf_ptr, size, out_ptr, out_cap, n_ptr or None),
                        self.h)
+
+    def container_delta_encode_async(self, candidates, tolerance_ppm, elem_bytes, in_ptr, base_ptr, n, chunk_syms, flags, out_ptr,
+                                     out_cap):
+        """A version 8 container of the n bytes at in_ptr as their difference from the n bytes at base_ptr (both 16-byte
+        aligned): container_planes_encode_async of the zigzag difference, with the base's CRC in the header.  out_cap >=
+        container_planes_bound.  The verdict (the first failing plane's, header unwritten) comes from sync()"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_delta_encode_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
+                                                                       elem_bytes, in_ptr, base_ptr, n, chunk_syms, flags, out_ptr,
+                                                                       out_cap), self.h)
+
+    def container_delta_decode_async(self, elem_bytes, buf_ptr, size, base_ptr, out_ptr, out_cap, n_ptr=0):
+        """enqueue only (CUDA-graph capturable once a call of the same size and out_cap has grown the workspaces): a
+        version 8 container applied to the base at base_ptr, into out_ptr; out_ptr == base_ptr applies it in place, any
+        other overlap is -1.  The verdict (-4 corrupt, -3 out_cap too small, -10 a base with another CRC; out untouched
+        in every case) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_delta_decode_async(self.h, elem_bytes, buf_ptr, size, base_ptr, out_ptr, out_cap,
+                                                                       n_ptr or None), self.h)
 
     def container_stored_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
         """the async decode of a version 6 container; enqueue only (CUDA-graph capturable).  The verdict (-4 corrupt or

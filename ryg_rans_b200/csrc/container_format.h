@@ -342,14 +342,27 @@ static_assert(sizeof(PlaneEntry) == 16, "plane table entries are 16 bytes");
 RB200_HD inline bool container_planes_w_ok(uint32_t w) { return w == 2 || w == 4 || w == 8; }
 // the end of the table: plane 0's offset, 16-aligned
 RB200_HD inline uint64_t container_planes_table_end(uint32_t w) { return sizeof(ContainerHeader) + sizeof(PlaneEntry) * w; }
-// version 7's header rules; the table and the planes fit `size`
-RB200_HD inline bool container_planes_header_ok(const ContainerHeader& h, uint64_t size)
+// Version 8 (a delta from a base tensor): version 7's layout and rules but for two header fields, version 8 and
+// reserved = the CRC-32 of the base tensor's n bytes (covered by meta_crc, which zeroes only the two crc fields).  The
+// planes hold d, not the input: for element i with x and b the w-byte little-endian integers of the input and the
+// base, s = (x - b) mod 2^(8w) read as signed, d = (s << 1) ^ (s >> (8w - 1)) (arithmetic shift), byte k of d in plane
+// k; the inverse x = b + ((d >> 1) ^ -(d & 1)) mod 2^(8w) is exact for every bit pattern.
+constexpr uint16_t kContainerVersionDelta = 8;
+// the header rules of version 7 or 8 (`version`, the one the caller accepts); the table and the planes fit `size`.
+// Only version 7 requires reserved == 0.
+RB200_HD inline bool container_planes_header_version_ok(const ContainerHeader& h, uint64_t size, uint16_t version)
 {
-    if (h.magic != kContainerMagic || h.version != kContainerVersionPlanes || h.coder || h.scale_bits || h.lanes != RB200_LANES) return false;
-    if (!container_planes_w_ok(h.block_size) || h.n_blocks != h.block_size || h.n_chunks || h.reserved || h.blob_crc) return false;
+    if (h.magic != kContainerMagic || h.version != version || h.coder || h.scale_bits || h.lanes != RB200_LANES) return false;
+    if (!container_planes_w_ok(h.block_size) || h.n_blocks != h.block_size || h.n_chunks || h.blob_crc) return false;
+    if (version == kContainerVersionPlanes && h.reserved) return false;
     if (!container_chunk_ok(h.chunk_syms) || !h.n_symbols || h.n_symbols % h.block_size || ((h.n_symbols / h.block_size) >> 32)) return false;
     const uint64_t t = container_planes_table_end(h.block_size);
     return t <= size && h.blob_bytes <= size - t;
+}
+// version 7's header rules; the table and the planes fit `size`
+RB200_HD inline bool container_planes_header_ok(const ContainerHeader& h, uint64_t size)
+{
+    return container_planes_header_version_ok(h, size, kContainerVersionPlanes);
 }
 // the table: plane 0 right after it, every plane right after the previous one, each at least a header long and a
 // multiple of 16, and the last one ending where the blob does

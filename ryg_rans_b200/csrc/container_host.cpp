@@ -31,6 +31,10 @@
 // Plane p holds byte p of every w-byte element; the rules are container_planes_* in container_format.h, and each plane
 // is checked by rb200_container_stored_open's.
 //
+//   version 8 (a delta from a base tensor): version 7's layout, version 8, reserved = CRC-32 of the base's n bytes
+//
+// Its planes hold the zigzag difference from the base (container_format.h); the _delta_ calls accept only version 8.
+//
 // rb200_container_pack / _open and the _blocks_ forms here work on host buffers with a host CRC (slicing-by-8, ~1 GB/s
 // on one core: the blob CRC is optional for that reason).  rb200_container_encode / _decode and the _blocks_ forms
 // (rans_b200.cu) write and read the same bytes in host or device memory with the blob CRC on the GPU
@@ -521,10 +525,9 @@ int planes_plane_open(const uint8_t* plane, size_t size, ContainerHeader* h)
     return container_bitmap_blob_offset(h->n_chunks) + h->blob_bytes == size ? RB200_OK : RB200_E_STREAM;
 }
 
-}  // namespace
-
-extern "C" int rb200_container_planes_pack(uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint8_t* out,
-                                           size_t out_cap, size_t* out_size)
+// the pack of version 7 (reserved 0) or version 8 (reserved the base tensor's CRC)
+int planes_pack(uint16_t version, uint32_t reserved, uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint8_t* out,
+                size_t out_cap, size_t* out_size)
 {
     if (!container_planes_w_ok(elem_bytes) || !planes || !sizes || !out) return RB200_E_ARG;
     ContainerHeader first{};
@@ -542,13 +545,14 @@ extern "C" int rb200_container_planes_pack(uint32_t elem_bytes, const uint8_t* c
     if (end > out_cap) return RB200_E_SPACE;
     ContainerHeader h{};
     h.magic = kContainerMagic;
-    h.version = kContainerVersionPlanes;
+    h.version = version;
     h.lanes = RB200_LANES;
     h.chunk_syms = first.chunk_syms;
     h.n_symbols = first.n_symbols * elem_bytes;
     h.blob_bytes = end - container_planes_table_end(elem_bytes);
     h.flags = first.flags;
     h.block_size = h.n_blocks = elem_bytes;
+    h.reserved = reserved;
     h.meta_crc = container_crc32(container_header_crc(h), table, sizeof(PlaneEntry) * elem_bytes);
     std::memcpy(out, &h, sizeof h);
     std::memcpy(out + sizeof h, table, sizeof(PlaneEntry) * elem_bytes);
@@ -557,13 +561,14 @@ extern "C" int rb200_container_planes_pack(uint32_t elem_bytes, const uint8_t* c
     return RB200_OK;
 }
 
-extern "C" int rb200_container_planes_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info)
+// the open of version 7 or 8 (`version`, the one the caller accepts); *reserved receives the header's reserved word
+int planes_open(uint16_t version, const uint8_t* buf, size_t size, rb200_container_planes_info* info, uint32_t* reserved)
 {
     if (!buf || !info) return RB200_E_ARG;
     if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
     ContainerHeader h;
     std::memcpy(&h, buf, sizeof h);
-    if (!container_planes_header_ok(h, size)) return RB200_E_STREAM;
+    if (!container_planes_header_version_ok(h, size, version)) return RB200_E_STREAM;
     if (reinterpret_cast<uintptr_t>(buf) & 7) return RB200_E_ARG;
     const uint32_t w = h.block_size;
     PlaneEntry table[8];
@@ -585,7 +590,34 @@ extern "C" int rb200_container_planes_open(const uint8_t* buf, size_t size, rb20
         info->planes[p] = buf + table[p].offset;
         info->sizes[p] = table[p].size;
     }
+    *reserved = h.reserved;
     return RB200_OK;
+}
+
+}  // namespace
+
+extern "C" int rb200_container_planes_pack(uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint8_t* out,
+                                           size_t out_cap, size_t* out_size)
+{
+    return planes_pack(kContainerVersionPlanes, 0, elem_bytes, planes, sizes, out, out_cap, out_size);
+}
+
+extern "C" int rb200_container_planes_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info)
+{
+    uint32_t reserved;
+    return planes_open(kContainerVersionPlanes, buf, size, info, &reserved);
+}
+
+extern "C" int rb200_container_delta_pack(uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint32_t base_crc,
+                                          uint8_t* out, size_t out_cap, size_t* out_size)
+{
+    return planes_pack(kContainerVersionDelta, base_crc, elem_bytes, planes, sizes, out, out_cap, out_size);
+}
+
+extern "C" int rb200_container_delta_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info, uint32_t* base_crc)
+{
+    if (!base_crc) return RB200_E_ARG;
+    return planes_open(kContainerVersionDelta, buf, size, info, base_crc);
 }
 
 extern "C" int rb200_choose_coder(const uint64_t counts[256], size_t n, uint32_t chunk_syms, const uint32_t* candidates,

@@ -12,6 +12,7 @@ constexpr uint32_t kStatSpace  = 4u;   // compacted blob does not fit blob_cap
 constexpr uint32_t kStatStall  = 8u;   // a bounded wait inside a kernel expired (a bug or a wedged GPU, not bad input)
 constexpr uint32_t kStatModel  = 16u;  // the model built from the data is one rb200_model_create refuses
 constexpr uint32_t kStatArg    = 32u;  // a length read from device memory is outside what the call was enqueued for
+constexpr uint32_t kStatBase   = 64u;  // a delta container's base has another CRC than the one it was encoded against
 
 constexpr uint32_t kHeaderBytes = 128; // 32 lanes x u32 final state (RansWordEncFlush / RansEncFlush x 32)
 

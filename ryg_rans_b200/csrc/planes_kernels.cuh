@@ -27,6 +27,13 @@
 //                               planes_record_kernel(p)
 //   planes_verdict_kernel       *d_n_symbols, then kStatStream / kStatSpace or the record's go
 //   planes_interleave_kernel<W> the planes into out, only when go is set
+// The delta container (version 8, rb200_container_delta_encode_async / _decode_async) runs the same host bodies with a
+// base tensor; its kernels are thin wrappers around the bodies above, or the version 7 kernels themselves:
+//   encode: delta_split_kernel<W> (the split of d, the zigzag difference from base), crc32_kernel over base into the
+//           call's DeltaWork, every plane as above, delta_finish_kernel (the finish with version 8, reserved = the CRC)
+//   decode: delta_plan_kernel (the plan with version 8's rules), every plane as above, delta_verdict_kernel (the verdict,
+//           then the base's length: n when go, else 0), crc32_kernel over that many bytes of base, delta_check_kernel
+//           (a CRC other than the header's: kStatBase, go cleared), delta_interleave_kernel<W> (d and base into out)
 #pragma once
 #include "container_decode.cuh"
 #include "container_format.h"
@@ -51,6 +58,13 @@ struct PlanesWork {
 struct PlanesVarlenGeom {
     uint64_t n;                 // input bytes, 1 <= n <= n_max and a multiple of w; 0 for a bad *d_n
     uint64_t m;                 // symbols per plane, n / w; UINT64_MAX for a bad *d_n
+};
+
+// The base tensor's CRC of a delta call (one for the encode, one for the decode): crc32_kernel's result, and on decode
+// the length it covers (the header's n once every check passed, else 0: the base is then not read).
+struct DeltaWork {
+    CrcSlot crc;
+    uint64_t base_n;
 };
 
 constexpr uint32_t kPlanesThreads = 256;
@@ -91,23 +105,91 @@ __device__ __forceinline__ void planes_untranspose(const uint32_t (&y)[4 * W], u
     }
 }
 
-// in (m elements of W bytes, 16-byte aligned) -> plane k at planes + k * stride (stride a multiple of 16).  Grid-stride
-// over groups of 16 elements; the ragged end (fewer than 16 elements) a byte per thread.
+// The version 8 transform of one element of W bytes (the low 8 W bits of x and b): d = zigzag((x - b) mod 2^(8 W)), and
+// its inverse x = b + unzigzag(d).  For the ragged ends; the groups of 16 take the lane forms below.
 template <int W>
-__device__ __forceinline__ void planes_split(const uint8_t* __restrict__ in, uint64_t m, uint8_t* __restrict__ planes, uint64_t stride)
+__device__ __forceinline__ uint64_t delta_zigzag(uint64_t x, uint64_t b)
+{
+    const uint64_t s = (x - b) << (64 - 8 * W);                      // the difference in the top 8 W bits
+    return ((s << 1) ^ static_cast<uint64_t>(static_cast<int64_t>(s) >> 63)) >> (64 - 8 * W);
+}
+template <int W>
+__device__ __forceinline__ uint64_t delta_unzigzag(uint64_t d, uint64_t b)
+{
+    const uint64_t x = b + ((d >> 1) ^ (0ull - (d & 1)));
+    return W == 8 ? x : x & ((1ull << (8 * W)) - 1);
+}
+
+// The transform on 4 W words of element data (element e at bytes e W .. e W + W - 1), in place: 16-bit lanes of a word
+// for W = 2, the word for W = 4, pairs of words for W = 8.  forward: x -> d from x and b; inverse: d -> x from d and b.
+template <int W>
+__device__ __forceinline__ void delta_forward(uint32_t (&x)[4 * W], const uint32_t (&b)[4 * W])
+{
+#pragma unroll
+    for (int i = 0; i < 4 * W; i += W == 8 ? 2 : 1) {
+        if (W == 2) {
+            const uint32_t s = __vsub2(x[i], b[i]);
+            x[i] = ((s << 1) & 0xfffefffeu) ^ (((s >> 15) & 0x00010001u) * 0xffffu);
+        } else if (W == 4) {
+            const uint32_t s = x[i] - b[i];
+            x[i] = (s << 1) ^ static_cast<uint32_t>(static_cast<int32_t>(s) >> 31);
+        } else {
+            const uint64_t s = (static_cast<uint64_t>(x[i + 1]) << 32 | x[i]) - (static_cast<uint64_t>(b[i + 1]) << 32 | b[i]);
+            const uint64_t d = (s << 1) ^ static_cast<uint64_t>(static_cast<int64_t>(s) >> 63);
+            x[i] = static_cast<uint32_t>(d);
+            x[i + 1] = static_cast<uint32_t>(d >> 32);
+        }
+    }
+}
+template <int W>
+__device__ __forceinline__ void delta_inverse(uint32_t (&x)[4 * W], const uint32_t (&b)[4 * W])
+{
+#pragma unroll
+    for (int i = 0; i < 4 * W; i += W == 8 ? 2 : 1) {
+        if (W == 2) {
+            x[i] = __vadd2(b[i], ((x[i] >> 1) & 0x7fff7fffu) ^ ((x[i] & 0x00010001u) * 0xffffu));
+        } else if (W == 4) {
+            x[i] = b[i] + ((x[i] >> 1) ^ (0u - (x[i] & 1u)));
+        } else {
+            const uint64_t d = static_cast<uint64_t>(x[i + 1]) << 32 | x[i];
+            const uint64_t v = (static_cast<uint64_t>(b[i + 1]) << 32 | b[i]) + ((d >> 1) ^ (0ull - (d & 1)));
+            x[i] = static_cast<uint32_t>(v);
+            x[i + 1] = static_cast<uint32_t>(v >> 32);
+        }
+    }
+}
+
+// W 16-byte loads of 16 elements into 4 W words
+template <int W>
+__device__ __forceinline__ void planes_load_group(const uint4* src, uint32_t (&x)[4 * W])
+{
+#pragma unroll
+    for (int i = 0; i < W; i++) {
+        const uint4 v = __ldcs(src + i);
+        x[4 * i] = v.x;
+        x[4 * i + 1] = v.y;
+        x[4 * i + 2] = v.z;
+        x[4 * i + 3] = v.w;
+    }
+}
+
+// in (m elements of W bytes, 16-byte aligned) -> plane k at planes + k * stride (stride a multiple of 16).  Grid-stride
+// over groups of 16 elements; the ragged end (fewer than 16 elements) a byte per thread.  DELTA (version 8): the planes
+// of d, the difference of in from base (16-byte aligned too), W more loads per group; the ragged end an element per
+// thread.
+template <int W, bool DELTA = false>
+__device__ __forceinline__ void planes_split(const uint8_t* __restrict__ in, const uint8_t* __restrict__ base, uint64_t m,
+                                             uint8_t* __restrict__ planes, uint64_t stride)
 {
     const uint64_t groups = m / 16, step = static_cast<uint64_t>(gridDim.x) * blockDim.x;
     const uint64_t tid = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     for (uint64_t g = tid; g < groups; g += step) {
-        const uint4* src = reinterpret_cast<const uint4*>(in) + g * W;
         uint32_t x[4 * W], y[4 * W];
-#pragma unroll
-        for (int i = 0; i < W; i++) {
-            const uint4 v = __ldcs(src + i);
-            x[4 * i] = v.x;
-            x[4 * i + 1] = v.y;
-            x[4 * i + 2] = v.z;
-            x[4 * i + 3] = v.w;
+        planes_load_group<W>(reinterpret_cast<const uint4*>(in) + g * W, x);
+        if (DELTA) {
+            uint32_t b[4 * W];
+            planes_load_group<W>(reinterpret_cast<const uint4*>(base) + g * W, b);
+            delta_forward<W>(x, b);
         }
         planes_transpose<W>(x, y);
 #pragma unroll
@@ -115,7 +197,20 @@ __device__ __forceinline__ void planes_split(const uint8_t* __restrict__ in, uin
             *reinterpret_cast<uint4*>(planes + k * stride + g * 16) = make_uint4(y[4 * k], y[4 * k + 1], y[4 * k + 2], y[4 * k + 3]);
     }
     const uint64_t tail = groups * 16;
-    if (tid < (m - tail) * W) {
+    if (DELTA) {
+        if (tid < m - tail) {
+            const uint64_t e = tail + tid;
+            uint64_t x = 0, b = 0;
+#pragma unroll
+            for (int k = 0; k < W; k++) {
+                x |= static_cast<uint64_t>(in[e * W + k]) << (8 * k);
+                b |= static_cast<uint64_t>(base[e * W + k]) << (8 * k);
+            }
+            const uint64_t d = delta_zigzag<W>(x, b);
+#pragma unroll
+            for (int k = 0; k < W; k++) planes[k * stride + e] = static_cast<uint8_t>(d >> (8 * k));
+        }
+    } else if (tid < (m - tail) * W) {
         const uint64_t e = tail + tid / W, k = tid % W;
         planes[k * stride + e] = in[e * W + k];
     }
@@ -125,7 +220,7 @@ template <int W>
 __global__ void __launch_bounds__(kPlanesThreads)
     planes_split_kernel(const uint8_t* __restrict__ in, uint64_t m, uint8_t* __restrict__ planes, uint64_t stride)
 {
-    planes_split<W>(in, m, planes, stride);
+    planes_split<W>(in, nullptr, m, planes, stride);
 }
 
 // The split of the varlen encode: m from the record, nothing for a bad length.  The grid is the fixed call's, so a
@@ -136,13 +231,24 @@ __global__ void __launch_bounds__(kPlanesThreads)
                                uint64_t stride)
 {
     if (g->n == 0) return;
-    planes_split<W>(in, g->m, planes, stride);
+    planes_split<W>(in, nullptr, g->m, planes, stride);
 }
 
-// The inverse, from the decode workspace into out: n from the record, and nothing unless every check passed.
+// The split of the delta encode: the planes of d = zigzag(in - base)
 template <int W>
 __global__ void __launch_bounds__(kPlanesThreads)
-    planes_interleave_kernel(const uint8_t* __restrict__ planes, uint64_t stride, uint8_t* __restrict__ out, const PlanesWork* __restrict__ r)
+    delta_split_kernel(const uint8_t* __restrict__ in, const uint8_t* __restrict__ base, uint64_t m, uint8_t* __restrict__ planes,
+                       uint64_t stride)
+{
+    planes_split<W, true>(in, base, m, planes, stride);
+}
+
+// The inverse, from the decode workspace into out: n from the record, and nothing unless every check passed.  DELTA
+// (version 8): the planes hold d, and out = base + unzigzag(d), base 16-byte aligned; each thread reads exactly the base
+// bytes it writes to out, so out == base (the delta applied in place) is correct, and neither pointer is __restrict__.
+template <int W, bool DELTA>
+__device__ __forceinline__ void planes_interleave(const uint8_t* __restrict__ planes, uint64_t stride, const uint8_t* base, uint8_t* out,
+                                                  const PlanesWork* __restrict__ r)
 {
     if (!r->go) return;
     const uint64_t m = r->n / W, groups = m / 16, step = static_cast<uint64_t>(gridDim.x) * blockDim.x;
@@ -158,15 +264,48 @@ __global__ void __launch_bounds__(kPlanesThreads)
             y[4 * k + 3] = v.w;
         }
         planes_untranspose<W>(y, x);
+        if (DELTA) {
+            uint32_t b[4 * W];
+            planes_load_group<W>(reinterpret_cast<const uint4*>(base) + g * W, b);
+            delta_inverse<W>(x, b);
+        }
         uint4* dst = reinterpret_cast<uint4*>(out) + g * W;
 #pragma unroll
         for (int i = 0; i < W; i++) dst[i] = make_uint4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
     }
     const uint64_t tail = groups * 16;
-    if (tid < (m - tail) * W) {
+    if (DELTA) {
+        if (tid < m - tail) {
+            const uint64_t e = tail + tid;
+            uint64_t d = 0, b = 0;
+#pragma unroll
+            for (int k = 0; k < W; k++) {
+                d |= static_cast<uint64_t>(planes[k * stride + e]) << (8 * k);
+                b |= static_cast<uint64_t>(base[e * W + k]) << (8 * k);
+            }
+            const uint64_t x = delta_unzigzag<W>(d, b);
+#pragma unroll
+            for (int k = 0; k < W; k++) out[e * W + k] = static_cast<uint8_t>(x >> (8 * k));
+        }
+    } else if (tid < (m - tail) * W) {
         const uint64_t e = tail + tid / W, k = tid % W;
         out[e * W + k] = planes[k * stride + e];
     }
+}
+
+template <int W>
+__global__ void __launch_bounds__(kPlanesThreads)
+    planes_interleave_kernel(const uint8_t* __restrict__ planes, uint64_t stride, uint8_t* __restrict__ out, const PlanesWork* __restrict__ r)
+{
+    planes_interleave<W, false>(planes, stride, nullptr, out, r);
+}
+
+template <int W>
+__global__ void __launch_bounds__(kPlanesThreads)
+    delta_interleave_kernel(const uint8_t* __restrict__ planes, uint64_t stride, const uint8_t* base, uint8_t* out,
+                            const PlanesWork* __restrict__ r)
+{
+    planes_interleave<W, true>(planes, stride, base, out, r);
 }
 
 // Encode: plane p's verdict and place.  Its container is complete (header included) at src -- out + 64 + 16 W for
@@ -242,6 +381,16 @@ __global__ void __launch_bounds__(32)
     planes_finish(s_v, out, h, r, status);
 }
 
+// The finish of the delta encode: version 8, reserved the base's CRC
+__global__ void __launch_bounds__(32)
+    delta_finish_kernel(uint8_t* out, ContainerHeader h, const DeltaWork* __restrict__ d, const PlanesWork* __restrict__ r, const uint32_t* status)
+{
+    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
+    h.version = kContainerVersionDelta;
+    h.reserved = d->crc.crc;
+    planes_finish(s_v, out, h, r, status);
+}
+
 // The finish of the varlen encode: n from the record.  A bad length left the status word set, so nothing is written.
 __global__ void __launch_bounds__(32)
     planes_finish_varlen_kernel(uint8_t* out, ContainerHeader h, const PlanesVarlenGeom* __restrict__ g, const PlanesWork* __restrict__ r,
@@ -264,17 +413,17 @@ __global__ void __launch_bounds__(32)
     *g = ok ? PlanesVarlenGeom{n, n / w} : PlanesVarlenGeom{0, UINT64_MAX};
 }
 
-// Decode: every version 7 rule on the header, the table and the planes' headers, and meta_crc; the record is reset
-// for the call.  One warp: lanes 0..3 stage the header, lanes 4.. the table, lane p < W checks plane p's header.
-__global__ void __launch_bounds__(32)
-    planes_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, PlanesWork* __restrict__ r)
+// Decode: every rule of version 7 (VERSION 8: version 8's) on the header, the table and the planes' headers, and
+// meta_crc; the record is reset for the call.  One warp: lanes 0..3 stage the header, lanes 4.. the table, lane p < W
+// checks plane p's header.
+template <uint16_t VERSION>
+__device__ __forceinline__ void planes_plan(uint4* s_v, const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, PlanesWork* __restrict__ r)
 {
-    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
     uint8_t* s = reinterpret_cast<uint8_t*>(s_v);
     const uint32_t lane = threadIdx.x;
     ContainerHeader h = {};
     if (size >= sizeof(ContainerHeader)) h = *reinterpret_cast<const ContainerHeader*>(buf);   // a shorter buffer is not read
-    bool ok = size >= sizeof(ContainerHeader) && container_planes_header_ok(h, size) && h.block_size == w;
+    bool ok = size >= sizeof(ContainerHeader) && container_planes_header_version_ok(h, size, VERSION) && h.block_size == w;
     const uint32_t meta_crc = h.meta_crc;
     if (ok) {                                                         // the table lies in size (header rule)
         h.meta_crc = 0;
@@ -298,6 +447,20 @@ __global__ void __launch_bounds__(32)
         r->go = 0;
         r->n = ok ? h.n_symbols : 0;
     }
+}
+
+__global__ void __launch_bounds__(32)
+    planes_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, PlanesWork* __restrict__ r)
+{
+    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
+    planes_plan<kContainerVersionPlanes>(s_v, buf, size, w, r);
+}
+
+__global__ void __launch_bounds__(32)
+    delta_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, PlanesWork* __restrict__ r)
+{
+    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
+    planes_plan<kContainerVersionDelta>(s_v, buf, size, w, r);
 }
 
 // Decode: plane p's bytes into staging, when the record passed and the plane fits it; otherwise a zero header, which
@@ -326,10 +489,9 @@ __global__ void __launch_bounds__(32) planes_record_kernel(uint32_t p, const Con
 
 // Decode: the call's verdict.  The header and table rejected: kStatStream.  Otherwise n is written, then n > out_cap
 // is kStatSpace, a plane that failed its checks kStatStream, and a call that passed everything sets go.
-__global__ void __launch_bounds__(32)
-    planes_verdict_kernel(uint32_t w, uint64_t out_cap, uint64_t* __restrict__ n_symbols, PlanesWork* __restrict__ r, uint32_t* status)
+__device__ __forceinline__ void planes_verdict(uint32_t w, uint64_t out_cap, uint64_t* __restrict__ n_symbols, PlanesWork* __restrict__ r,
+                                               uint32_t* status)
 {
-    if (threadIdx.x) return;
     if (!r->ok) {
         atomicOr(status, kStatStream);
         return;
@@ -343,6 +505,36 @@ __global__ void __launch_bounds__(32)
         atomicOr(status, kStatStream);
     else
         r->go = 1;
+}
+
+__global__ void __launch_bounds__(32)
+    planes_verdict_kernel(uint32_t w, uint64_t out_cap, uint64_t* __restrict__ n_symbols, PlanesWork* __restrict__ r, uint32_t* status)
+{
+    if (threadIdx.x) return;
+    planes_verdict(w, out_cap, n_symbols, r, status);
+}
+
+// Decode, version 8: the verdict, then the length of base the CRC covers: n once every check passed (so n <= out_cap),
+// otherwise 0, and the base is not read
+__global__ void __launch_bounds__(32)
+    delta_verdict_kernel(uint32_t w, uint64_t out_cap, uint64_t* __restrict__ n_symbols, PlanesWork* __restrict__ r, uint32_t* status,
+                         DeltaWork* __restrict__ d)
+{
+    if (threadIdx.x) return;
+    planes_verdict(w, out_cap, n_symbols, r, status);
+    d->base_n = r->go ? r->n : 0;
+}
+
+// Decode, version 8: when every other check passed, the base's CRC against the header's reserved word (the header
+// passed, so buf holds it); a different base clears go, so the interleave writes nothing, and flags kStatBase.
+__global__ void __launch_bounds__(32)
+    delta_check_kernel(const uint8_t* __restrict__ buf, const DeltaWork* __restrict__ d, PlanesWork* __restrict__ r, uint32_t* status)
+{
+    if (threadIdx.x || !r->go) return;
+    if (d->crc.crc != reinterpret_cast<const ContainerHeader*>(buf)->reserved) {
+        r->go = 0;
+        atomicOr(status, kStatBase);
+    }
 }
 
 }  // namespace rb200

@@ -86,6 +86,9 @@ struct rb200_ctx {
     DevBuf planes_in, planes_enc_stage, planes_out, planes_dec_stage;
     // rb200_container_planes_encode_varlen_async: the length its plan kernel read
     PlanesVarlenGeom* d_planes_geom = nullptr;
+    // the delta calls (version 8): the base's CRC, one record for the encode, one for the decode
+    DeltaWork* d_delta_enc = nullptr;
+    DeltaWork* d_delta_dec = nullptr;
 };
 
 struct rb200_model {
@@ -159,6 +162,7 @@ int status_to_code(uint32_t bits)
     if (bits & kStatSymbol) return RB200_E_SYMBOL;
     if (bits & kStatSpace) return RB200_E_SPACE;
     if (bits & kStatStream) return RB200_E_STREAM;
+    if (bits & kStatBase) return RB200_E_BASE;
     if (bits & kStatStall) return RB200_E_STALL;
     return RB200_OK;
 }
@@ -204,6 +208,7 @@ extern "C" const char* rb200_strerror(int code)
     case RB200_E_SYMBOL: return "symbol with zero model frequency";
     case RB200_E_NCCL: return "NCCL error";
     case RB200_E_STALL: return "a bounded wait inside a kernel expired";
+    case RB200_E_BASE: return "the base is not the tensor the delta was encoded against";
     }
     return "unknown";
 }
@@ -265,6 +270,10 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
     }
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_planes_geom, sizeof(PlanesVarlenGeom));
     if (e == cudaSuccess) e = cudaMemset(ctx->d_planes_geom, 0, sizeof(PlanesVarlenGeom));
+    for (DeltaWork** d : {&ctx->d_delta_enc, &ctx->d_delta_dec}) {
+        if (e == cudaSuccess) e = cudaMalloc(d, sizeof(DeltaWork));
+        if (e == cudaSuccess) e = cudaMemset(*d, 0, sizeof(DeltaWork));
+    }
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -308,6 +317,8 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->d_planes_enc) cudaFree(ctx->d_planes_enc);
     if (ctx->d_planes_dec) cudaFree(ctx->d_planes_dec);
     if (ctx->d_planes_geom) cudaFree(ctx->d_planes_geom);
+    if (ctx->d_delta_enc) cudaFree(ctx->d_delta_enc);
+    if (ctx->d_delta_dec) cudaFree(ctx->d_delta_dec);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -2440,9 +2451,15 @@ namespace {
 // a grid of every CTA of the byte-plane kernels that is resident at once: they stride over what they move
 uint32_t planes_grid(const rb200_ctx* ctx) { return static_cast<uint32_t>(ctx->sms) * kPlanesCtasPerSm; }
 
-// geom set: the varlen split, m from the record
-int launch_split(rb200_ctx* ctx, uint32_t w, const uint8_t* in, uint64_t m, const PlanesVarlenGeom* geom, uint8_t* planes, uint64_t stride)
+// geom set: the varlen split, m from the record; base set: the delta split
+int launch_split(rb200_ctx* ctx, uint32_t w, const uint8_t* in, const uint8_t* base, uint64_t m, const PlanesVarlenGeom* geom, uint8_t* planes,
+                 uint64_t stride)
 {
+    if (base) {
+        auto split = w == 2 ? delta_split_kernel<2> : w == 4 ? delta_split_kernel<4> : delta_split_kernel<8>;
+        split<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(in, base, m, planes, stride);
+        return check_launch(ctx, "delta_split_kernel");
+    }
     if (geom) {
         auto split = w == 2 ? planes_split_varlen_kernel<2> : w == 4 ? planes_split_varlen_kernel<4> : planes_split_varlen_kernel<8>;
         split<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(in, geom, planes, stride);
@@ -2453,8 +2470,14 @@ int launch_split(rb200_ctx* ctx, uint32_t w, const uint8_t* in, uint64_t m, cons
     return check_launch(ctx, "planes_split_kernel");
 }
 
-int launch_interleave(rb200_ctx* ctx, uint32_t w, const uint8_t* planes, uint64_t stride, uint8_t* out, const PlanesWork* r)
+// base set: the delta interleave, out = base + the decoded difference
+int launch_interleave(rb200_ctx* ctx, uint32_t w, const uint8_t* planes, uint64_t stride, const uint8_t* base, uint8_t* out, const PlanesWork* r)
 {
+    if (base) {
+        auto interleave = w == 2 ? delta_interleave_kernel<2> : w == 4 ? delta_interleave_kernel<4> : delta_interleave_kernel<8>;
+        interleave<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(planes, stride, base, out, r);
+        return check_launch(ctx, "delta_interleave_kernel");
+    }
     auto interleave = w == 2 ? planes_interleave_kernel<2> : w == 4 ? planes_interleave_kernel<4> : planes_interleave_kernel<8>;
     interleave<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(planes, stride, out, r);
     return check_launch(ctx, "planes_interleave_kernel");
@@ -2467,8 +2490,10 @@ int launch_interleave(rb200_ctx* ctx, uint32_t w, const uint8_t* planes, uint64_
 // stride and every version 6 encode's bound; planes_varlen_plan_kernel reads *d_n into the context's PlanesVarlenGeom
 // first, the split and the finish are their varlen forms, and every plane's version 6 encode is the varlen one, with
 // the record's m as its length.  Arguments are checked here, with n_max for n.
+// base set (rb200_container_delta_encode_async, never with d_n): the delta split, the base's CRC (crc32_kernel into the
+// call's DeltaWork) right after it, and the delta finish, which writes version 8 with the CRC in reserved.
 int planes_encode(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm, uint32_t w, const uint8_t* in,
-                  size_t n, const uint64_t* d_n, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
+                  const uint8_t* base, size_t n, const uint64_t* d_n, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
 {
     if (!container_planes_w_ok(w) || n == 0 || n % w || ((n / w) >> 32) || (reinterpret_cast<uintptr_t>(in) & 15)) return RB200_E_ARG;
     const size_t m = n / w;
@@ -2491,7 +2516,8 @@ int planes_encode(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candida
         rc = check_launch(ctx, "planes_varlen_plan_kernel");
         if (rc != RB200_OK) return rc;
     }
-    rc = launch_split(ctx, w, in, m, geom, planes, stride);
+    rc = launch_split(ctx, w, in, base, m, geom, planes, stride);
+    if (rc == RB200_OK && base) rc = launch_crc(ctx, base, n, nullptr, 0, &ctx->d_delta_enc->crc);
     for (uint32_t p = 0; p < w && rc == RB200_OK; p++) {
         uint8_t* dst = p ? stage : out + table_end;
         rc = stored_encode(ctx, a, planes + p * stride, m, geom ? &geom->m : nullptr, chunk_syms, flags, dst, plane_cap);
@@ -2509,6 +2535,10 @@ int planes_encode(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candida
     h.n_symbols = n;
     h.flags = flags;
     h.block_size = h.n_blocks = w;
+    if (base) {
+        delta_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, ctx->d_delta_enc, ctx->d_planes_enc, ctx->d_status);
+        return check_launch(ctx, "delta_finish_kernel");
+    }
     if (geom) {
         planes_finish_varlen_kernel<<<1, 32, 0, ctx->stream>>>(out, h, geom, ctx->d_planes_enc, ctx->d_status);
         return check_launch(ctx, "planes_finish_varlen_kernel");
@@ -2524,7 +2554,7 @@ extern "C" int rb200_container_planes_encode_async(rb200_ctx* ctx, const uint32_
                                                    uint32_t elem_bytes, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags,
                                                    uint8_t* out, size_t out_cap)
 {
-    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, n, nullptr, chunk_syms, flags, out, out_cap);
+    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, nullptr, n, nullptr, chunk_syms, flags, out, out_cap);
 }
 
 // rb200_container_planes_encode_async with the length read from device memory at every run: the plan kernel, the
@@ -2536,17 +2566,20 @@ extern "C" int rb200_container_planes_encode_varlen_async(rb200_ctx* ctx, const 
                                                           size_t n_max, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
 {
     if (!d_n || (reinterpret_cast<uintptr_t>(d_n) & 7) || n_max == 0) return RB200_E_ARG;
-    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, n_max, d_n, chunk_syms, flags, out, out_cap);
+    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, nullptr, n_max, d_n, chunk_syms, flags, out, out_cap);
 }
+
+namespace {
 
 // The plan kernel, then per plane the whole version 6 async decode (container_decode_async, unchanged) into a
 // workspace -- plane 0 in place, the others after a fetch into staging -- and a record kernel, then the verdict and the
 // interleave: 2 + 19 w launches, no copy, no synchronisation.
-extern "C" int rb200_container_planes_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size, uint8_t* out,
-                                                   size_t out_cap, uint64_t* d_n_symbols)
+// base set (rb200_container_delta_decode_async): version 8's plan, and between the verdict (delta_verdict_kernel, which
+// also writes the base's length) and the delta interleave the base's CRC and its check: 4 + 19 w launches.  Arguments
+// are checked by the callers.
+int planes_decode(rb200_ctx* ctx, uint32_t w, const uint8_t* buf, size_t size, const uint8_t* base, uint8_t* out, size_t out_cap,
+                  uint64_t* d_n_symbols)
 {
-    const uint32_t w = elem_bytes;
-    if (!container_planes_w_ok(w) || !async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
     DeviceGuard g(ctx->device);
     const uint64_t table_end = container_planes_table_end(w);
     // every plane of n <= out_cap bytes has n / w <= out_cap / w symbols, and fewer than 2^32
@@ -2559,8 +2592,11 @@ extern "C" int rb200_container_planes_decode_async(rb200_ctx* ctx, uint32_t elem
     uint8_t* stage = static_cast<uint8_t*>(ctx->planes_dec_stage.p);
     PlanesWork* r = ctx->d_planes_dec;
     cudaStream_t s = ctx->stream;
-    planes_plan_kernel<<<1, 32, 0, s>>>(buf, size, w, r);
-    rc = check_launch(ctx, "planes_plan_kernel");
+    if (base)
+        delta_plan_kernel<<<1, 32, 0, s>>>(buf, size, w, r);
+    else
+        planes_plan_kernel<<<1, 32, 0, s>>>(buf, size, w, r);
+    rc = check_launch(ctx, base ? "delta_plan_kernel" : "planes_plan_kernel");
     for (uint32_t p = 0; p < w && rc == RB200_OK; p++) {
         if (p) {
             planes_fetch_kernel<<<planes_grid(ctx), kPlanesThreads, 0, s>>>(buf, stage, stage_cap, p, r);
@@ -2575,9 +2611,50 @@ extern "C" int rb200_container_planes_decode_async(rb200_ctx* ctx, uint32_t elem
         rc = check_launch(ctx, "planes_record_kernel");
     }
     if (rc != RB200_OK) return rc;
-    planes_verdict_kernel<<<1, 32, 0, s>>>(w, out_cap, d_n_symbols, r, ctx->d_status);
-    rc = check_launch(ctx, "planes_verdict_kernel");
-    return rc == RB200_OK ? launch_interleave(ctx, w, planes, stride, out, r) : rc;
+    if (base) {
+        DeltaWork* d = ctx->d_delta_dec;
+        delta_verdict_kernel<<<1, 32, 0, s>>>(w, out_cap, d_n_symbols, r, ctx->d_status, d);
+        rc = check_launch(ctx, "delta_verdict_kernel");
+        if (rc == RB200_OK) rc = launch_crc(ctx, base, out_cap, &d->base_n, 0, &d->crc);
+        if (rc != RB200_OK) return rc;
+        delta_check_kernel<<<1, 32, 0, s>>>(buf, d, r, ctx->d_status);
+        rc = check_launch(ctx, "delta_check_kernel");
+    } else {
+        planes_verdict_kernel<<<1, 32, 0, s>>>(w, out_cap, d_n_symbols, r, ctx->d_status);
+        rc = check_launch(ctx, "planes_verdict_kernel");
+    }
+    return rc == RB200_OK ? launch_interleave(ctx, w, planes, stride, base, out, r) : rc;
+}
+
+}  // namespace
+
+extern "C" int rb200_container_planes_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size, uint8_t* out,
+                                                   size_t out_cap, uint64_t* d_n_symbols)
+{
+    if (!container_planes_w_ok(elem_bytes) || !async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    return planes_decode(ctx, elem_bytes, buf, size, nullptr, out, out_cap, d_n_symbols);
+}
+
+// The version 7 encode of the difference from base: planes_encode with base set, 3 + w * (11 to 15) launches.
+extern "C" int rb200_container_delta_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                                  uint32_t elem_bytes, const uint8_t* in, const uint8_t* base, size_t n, uint32_t chunk_syms,
+                                                  uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    if (!base || (reinterpret_cast<uintptr_t>(base) & 15)) return RB200_E_ARG;
+    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, base, n, nullptr, chunk_syms, flags, out, out_cap);
+}
+
+// The version 7 decode applied to base: planes_decode with base set.  out == base applies the delta in place; any other
+// overlap of the two, each taken as out_cap bytes long (the most the decode writes, and the most of base it reads), is
+// refused, since the interleave's threads would read base bytes that others have already written.
+extern "C" int rb200_container_delta_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size, const uint8_t* base,
+                                                  uint8_t* out, size_t out_cap, uint64_t* d_n_symbols)
+{
+    if (!container_planes_w_ok(elem_bytes) || !async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
+    if (!base || (reinterpret_cast<uintptr_t>(base) & 15)) return RB200_E_ARG;
+    const uintptr_t o = reinterpret_cast<uintptr_t>(out), b = reinterpret_cast<uintptr_t>(base);
+    if (o != b && o < b + out_cap && b < o + out_cap) return RB200_E_ARG;
+    return planes_decode(ctx, elem_bytes, buf, size, base, out, out_cap, d_n_symbols);
 }
 
 extern "C" int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n)

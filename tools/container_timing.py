@@ -102,11 +102,19 @@ on the --planes data, flags 0 and RB200_CONTAINER_CRC_BLOB, alternated: at *d_n 
 against the fixed call at that length, after checking that both wrote the same bytes; varlen minus fixed in total and
 per plane, and a torch.profiler list of both calls' kernels.
 
+With --delta, rb200_container_delta_encode_async and rb200_container_delta_decode_async (version 8, the difference from a
+base tensor) against the version 7 calls on the same tensor: 1 GiB of bf16 and of fp32, base = fp32 master weights of
+N(0, 0.02), in = the same after one step of 1e-4 * sign * U(0, 1), as the kind; chunks of 8192, {byte 14, word 12,
+alias 16} at 2 %, flags 0, alternated.  Sizes of both, encode and decode times and the version 8 minus version 7 time
+per GiB, a torch.profiler list of the version 8 calls' kernels, and the delta split and interleave kernels' rate (3n
+bytes moved each) beside the version 7 interleave's (2n bytes) in the same run.  The decodes write to a separate
+output, so every repetition sees the same base.
+
 Device calls are timed with CUDA events after a warm-up; the card's name and power limit are printed with the
 numbers.  Every output is checked against the plain calls plus rb200_container_pack / rb200_container_blocks_pack.
     python tools/container_timing.py [--blocks | --blocks-coder | --blocks-alias | --single | --model | --auto | --blocks-auto
                                       | --blocks-varlen | --blocks-stored | --stored | --stored-varlen
-                                      | --blocks-stored-varlen | --planes | --planes-varlen] [--reps 10]
+                                      | --blocks-stored-varlen | --planes | --planes-varlen | --delta] [--reps 10]
                                      [--json out.json]"""
 import argparse
 import json
@@ -1336,6 +1344,71 @@ def planes_varlen(args):
     return res
 
 
+def delta(args):
+    """version 8 against version 7 on the same tensor: bf16 and fp32 after one synthetic training step, 1 GiB each"""
+    import torch
+    n, chunk, tol = 1 << 30, 8192, 20000
+    cands = [api.CANDIDATE(rb.CODER_BYTE, 14), api.CANDIDATE(rb.CODER_WORD, 12), api.CANDIDATE(rb.CODER_ALIAS, 16)]
+    ctx = rb.Context(0)
+    sync = ctx.sync
+    d_dec = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+    res = {"card": card(), "workload": {"n": n, "chunk_syms": chunk, "step": "lr 1e-4, one step"},
+           "candidates": ["byte 14", "word 12", "alias 16"], "tolerance_ppm": tol, "workloads": {}, "checks": {}}
+    gen = torch.Generator(device="cuda").manual_seed(4321)
+    for name, dtype, w in (("bf16", torch.bfloat16, 2), ("fp32", torch.float32, 4)):
+        master = torch.randn(n // w, device="cuda", generator=gen) * 0.02
+        d_base = master.to(dtype, copy=True).view(torch.uint8)        # a copy also for fp32: the step below moves master
+        sign = torch.randint(0, 2, (n // w,), device="cuda", generator=gen, dtype=torch.int8).float() * 2 - 1
+        master += 1e-4 * sign * torch.rand(n // w, device="cuda", generator=gen)
+        d_in = master.to(dtype, copy=True).view(torch.uint8)
+        del master, sign
+        torch.cuda.empty_cache()
+        bound = api.container_planes_bound(n, w, chunk)
+        d_v7 = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+        d_v8 = torch.empty(bound + 16, dtype=torch.uint8, device="cuda")
+        i, b, o7, o8, dd = d_in.data_ptr(), d_base.data_ptr(), d_v7.data_ptr(), d_v8.data_ptr(), d_dec.data_ptr()
+        enc = {"v8_encode": lambda: ctx.container_delta_encode_async(cands, tol, w, i, b, n, chunk, 0, o8, bound),
+               "v7_encode": lambda: ctx.container_planes_encode_async(cands, tol, w, i, n, chunk, 0, o7, bound)}
+        times = alternate(enc, sync, args.warmup, args.reps)
+        for f in enc.values():
+            f()
+        sync()
+        h7, h8 = d_v7[:64].cpu().numpy(), d_v8[:64].cpu().numpy()
+        size7 = 64 + 16 * w + int(h7[32:40].view(np.uint64)[0])
+        size8 = 64 + 16 * w + int(h8[32:40].view(np.uint64)[0])
+        res["checks"][f"{name}: v8_within_bound"] = size8 <= bound
+        dec = {"v8_decode": lambda: ctx.container_delta_decode_async(w, o8, size8, b, dd, n),
+               "v7_decode": lambda: ctx.container_planes_decode_async(w, o7, size7, dd, n)}
+        dtimes = alternate(dec, sync, args.warmup, args.reps)
+        for k, f in dec.items():
+            d_dec.zero_()
+            f()
+            sync()
+            res["checks"][f"{name}: {k}_round_trip"] = bool(torch.equal(d_dec[:n], d_in))
+        ek = kernel_times(enc["v8_encode"], sync, args.reps)
+        dk = kernel_times(dec["v8_decode"], sync, args.reps)
+        dk7 = kernel_times(dec["v7_decode"], sync, args.reps)
+
+        def rate(kernels, part, moved):
+            us = sum(v["median_us"] * v["launches_per_call"] for k, v in kernels.items() if part in k)
+            return {"us": us, "TB_per_s": moved / us / 1e6 if us else None}
+
+        res["workloads"][name] = {
+            "bytes_per_input_byte": {"v8": size8 / n, "v7": size7 / n},
+            "encode": times, "decode": dtimes,
+            "v8_minus_v7_encode_ms_per_GiB": times["v8_encode"]["median_ms"] - times["v7_encode"]["median_ms"],
+            "v8_minus_v7_decode_ms_per_GiB": dtimes["v8_decode"]["median_ms"] - dtimes["v7_decode"]["median_ms"],
+            "delta_split_kernel": rate(ek, "delta_split_kernel", 3 * n),
+            "delta_interleave_kernel": rate(dk, "delta_interleave_kernel", 3 * n),
+            "v7_interleave_kernel": rate(dk7, "planes_interleave_kernel", 2 * n),
+            "v8_encode_kernels": ek, "v8_decode_kernels": dk,
+        }
+        del d_in, d_base, d_v7, d_v8
+        torch.cuda.empty_cache()
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
@@ -1352,13 +1425,14 @@ def main():
     ap.add_argument("--blocks-stored-varlen", action="store_true", help="the version 5 encode with the block count in device memory")
     ap.add_argument("--planes", action="store_true", help="the byte-plane container (version 7) against version 6 on bf16 and fp32")
     ap.add_argument("--planes-varlen", action="store_true", help="the byte-plane encode with the length in device memory, on bf16 and fp32")
+    ap.add_argument("--delta", action="store_true", help="the delta byte-plane container (version 8) against version 7 on bf16 and fp32")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else stored_varlen(args) if args.stored_varlen else blocks_stored_varlen(args) if args.blocks_stored_varlen else planes(args) if args.planes else planes_varlen(args) if args.planes_varlen else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else stored_varlen(args) if args.stored_varlen else blocks_stored_varlen(args) if args.blocks_stored_varlen else planes(args) if args.planes else planes_varlen(args) if args.planes_varlen else delta(args) if args.delta else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
