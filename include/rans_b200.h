@@ -566,6 +566,60 @@ int rb200_container_delta_encode_async(rb200_ctx* ctx, const uint32_t* candidate
 int rb200_container_delta_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size, const uint8_t* base,
                                        uint8_t* out, size_t out_cap, uint64_t* d_n_symbols);
 
+/* ---------------------------------------------------------------- tensor-list containers */
+
+/* Version 9: a list of T tensors of one element width w (elem_bytes, 2, 4 or 8), such as the bf16 or the fp32 tensors of
+ * a state dict, as one container: version 7 of the concatenation of their bytes, in list order with no padding, plus a
+ * directory of their lengths.  Layout: the 64-byte header (version 7's fields but for version 9, n_blocks = T with
+ * 1 <= T <= 2^20, n_symbols = the total n, blob_bytes = the planes' bytes, reserved = the CRC-32 of the directory's 8 T
+ * bytes, which meta_crc covers), w table entries {u64 offset, u64 size}, the directory (T u64 byte lengths, zero-padded
+ * to a multiple of 16), then the w version 6 planes with no gaps from offset 64 + 16 w + round16(8 T).  Every length is
+ * a multiple of w (zero allowed), and they sum to n, a nonzero multiple of w with n / w < 2^32.  Plane p is byte for
+ * byte plane p of a version 7 container of the concatenated bytes.  Only the _tensors_ calls accept version 9, and
+ * they accept no other version.
+ *   bound: rb200_container_planes_bound(n_max, w, chunk_syms) + round16(8 count); 0 for a count outside 1..2^20 or
+ *          arguments the planes bound refuses.
+ *   pack:  host only: rb200_container_planes_pack's rules, and RB200_E_ARG for a null lengths, a count outside 1..2^20
+ *          or lengths that are not multiples of w summing to the planes' n.
+ *   open:  rb200_container_planes_open's checks, and the directory's CRC and rules (RB200_E_STREAM); *count and
+ *          *lengths (a view into buf) receive the directory. */
+typedef struct rb200_tensor_ref {
+    uint64_t ptr;     /* device address of the tensor's bytes */
+    uint64_t bytes;   /* encode: its length; decode: its capacity */
+} rb200_tensor_ref;
+size_t rb200_container_tensors_bound(size_t n_max, uint32_t count, uint32_t elem_bytes, uint32_t chunk_syms);
+int rb200_container_tensors_pack(uint32_t elem_bytes, const uint64_t* lengths, uint32_t count, const uint8_t* const* planes,
+                                 const size_t* sizes, uint8_t* out, size_t out_cap, size_t* out_size);
+int rb200_container_tensors_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info, uint32_t* count,
+                                 const uint64_t** lengths);
+/* A version 9 container of the count tensors that d_refs names, DEVICE memory, enqueued only.  d_refs (count entries, 16
+ * bytes each, 16-byte aligned) lives in device memory and is read when the work runs, so one captured graph encodes
+ * whatever tensors the list names at each replay: their addresses and lengths may change between replays, as long as
+ * the count stays and the total stays within n_max.  Each entry's bytes is a multiple of w (zero allowed) and its ptr
+ * is aligned to w when bytes is not zero (element alignment is enough: views into a flat buffer work); the total is
+ * 1 .. n_max.  A list that breaks any of these is RB200_E_ARG from rb200_sync, and not one byte of out is written.
+ * The container is byte for byte rb200_container_tensors_pack of the lengths and of the planes that
+ * rb200_container_planes_encode_async writes for the concatenated bytes with the same arguments.  The call returns
+ * RB200_E_ARG (nothing launched) for everything rb200_container_planes_encode_varlen_async refuses at n_max, a count
+ * outside 1..2^20 and a null or misaligned d_refs, and RB200_E_SPACE (nothing launched) when out_cap is below
+ * rb200_container_tensors_bound(n_max, count, w, chunk_syms).  Every other verdict is the version 7 call's, the
+ * header then unwritten.  Capturable after one call with the same list, elem_bytes, count, chunk_syms and n_max
+ * outside the capture (the workspaces grow). */
+int rb200_container_tensors_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                         uint32_t elem_bytes, const rb200_tensor_ref* d_refs, uint32_t count, size_t n_max,
+                                         uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap);
+/* The decode of a version 9 container into the count outputs d_refs names (DEVICE memory, 16-byte aligned, read when
+ * the work runs: each entry's ptr and its capacity in bytes).  Tensor i goes to refs[i].ptr; its length comes from
+ * the directory.  rb200_sync gives RB200_E_STREAM for anything rb200_container_tensors_open rejects, a w other than
+ * elem_bytes, a container T other than count or a plane that fails its checks, and RB200_E_SPACE for a stored length
+ * above its ref's capacity or a total above n_max; in every one of these cases no output is touched.  d_lengths (NULL
+ * or count u64, 8-byte aligned) receives the directory once it passes (also when a capacity then fails).  Outputs that
+ * overlap each other or buf are a precondition violation, as for memcpy.  The call returns RB200_E_ARG (nothing
+ * launched) for a bad elem_bytes, a null or misaligned buf, d_refs or d_lengths, n_max == 0 and a count outside
+ * 1..2^20.  Enqueue only; capturable after one call of the same size, count and n_max outside the capture. */
+int rb200_container_tensors_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size,
+                                         const rb200_tensor_ref* d_refs, uint32_t count, size_t n_max, uint64_t* d_lengths);
+
 /* rb200_container_decode(..., RB200_MEM_DEVICE) for a version 1 container of any coder, with nothing done on the host:
  * the header, the model, the directory, meta_crc and (when flagged) the blob CRC are checked by kernels, the model's
  * decode table is built on the GPU into the context, and the decoder the header calls for is picked on the GPU -- all

@@ -131,6 +131,14 @@ EXPORTS = [
                                                      C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
     ("rb200_container_delta_decode_async", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
                                                      C.c_size_t, C.c_void_p]),
+    ("rb200_container_tensors_bound", C.c_size_t, [C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32]),
+    ("rb200_container_tensors_pack", C.c_int, [C.c_uint32, _u64p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                               C.POINTER(C.c_size_t)]),
+    ("rb200_container_tensors_open", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, _u32p, C.POINTER(_u64p)]),
+    ("rb200_container_tensors_encode_async", C.c_int, [C.c_void_p, _u32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
+                                                       C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("rb200_container_tensors_decode_async", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32,
+                                                       C.c_size_t, C.c_void_p]),
     ("rb200_comm_unique_id", C.c_int, [C.c_void_p]),
     ("rb200_comm_create", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("rb200_comm_destroy", None, [C.c_void_p]),
@@ -334,6 +342,46 @@ def container_delta_open(buf):
     meta = {k: int(getattr(info, k)) for k in ("elem_bytes", "chunk_syms", "flags", "n")}
     meta["base_crc"] = int(crc.value)
     return meta, planes
+
+
+def container_tensors_bound(n_max, count, elem_bytes, chunk_syms):
+    """rb200_container_tensors_bound: the most bytes a version 9 container of count tensors of elem_bytes-byte elements,
+    n_max bytes in all, takes (0 for arguments the encode refuses)"""
+    return int(load().dll.rb200_container_tensors_bound(n_max, count, elem_bytes, chunk_syms))
+
+
+def container_tensors_pack(lengths, planes):
+    """rb200_container_tensors_pack: a version 9 container of a list of tensors with these byte lengths, from the w =
+    len(planes) version 6 containers of the byte planes of their concatenated bytes (as container_planes_pack)"""
+    lib = load()
+    lengths = np.ascontiguousarray(lengths, dtype=np.uint64)
+    planes = [np.ascontiguousarray(p, dtype=np.uint8) for p in planes]
+    w = len(planes)
+    ptrs = (C.c_void_p * max(w, 1))(*[p.ctypes.data for p in planes])
+    sizes = (C.c_size_t * max(w, 1))(*[p.size for p in planes])
+    out = np.zeros(64 + 16 * w + 8 * lengths.size + 16 + sum(p.size for p in planes), np.uint8)
+    size = C.c_size_t(0)
+    lib.check(lib.dll.rb200_container_tensors_pack(w, lengths.ctypes.data_as(_u64p), lengths.size, ptrs, sizes, out.ctypes.data,
+                                                   out.size, C.byref(size)))
+    return out[:size.value]
+
+
+def container_tensors_open(buf):
+    """Returns (info dict, lengths, planes) of a version 9 container: lengths (uint64, one per tensor) and planes[p] (plane
+    p's version 6 container) are views into buf."""
+    lib = load()
+    buf = np.ascontiguousarray(buf, dtype=np.uint8)
+    info = ContainerPlanesInfo()
+    count = C.c_uint32(0)
+    dir_ptr = _u64p()
+    lib.check(lib.dll.rb200_container_tensors_open(buf.ctypes.data, buf.size, C.byref(info), C.byref(count), C.byref(dir_ptr)))
+    base = buf.ctypes.data
+    d_off = C.addressof(dir_ptr.contents) - base
+    lengths = buf[d_off:d_off + 8 * count.value].view(np.uint64)
+    planes = [buf[info.planes[p] - base:info.planes[p] - base + info.sizes[p]] for p in range(info.elem_bytes)]
+    meta = {k: int(getattr(info, k)) for k in ("elem_bytes", "chunk_syms", "flags", "n")}
+    meta["count"] = int(count.value)
+    return meta, lengths, planes
 
 
 class ContainerBlocksInfo(C.Structure):
@@ -766,6 +814,27 @@ class Context:
         in every case) comes from sync()"""
         self.lib.check(self.lib.dll.rb200_container_delta_decode_async(self.h, elem_bytes, buf_ptr, size, base_ptr, out_ptr, out_cap,
                                                                        n_ptr or None), self.h)
+
+    def container_tensors_encode_async(self, candidates, tolerance_ppm, elem_bytes, refs_ptr, count, n_max, chunk_syms, flags, out_ptr,
+                                       out_cap):
+        """A version 9 container of the count tensors named by the rb200_tensor_ref list at refs_ptr (device memory, 16
+        bytes per entry {u64 ptr, u64 bytes}, 16-byte aligned), read when the work runs: each bytes a multiple of
+        elem_bytes, each ptr aligned to elem_bytes, the total 1 .. n_max.  out_cap >= container_tensors_bound(n_max, count,
+        elem_bytes, chunk_syms).  The verdict comes from sync(): -1 for a bad list, with out untouched; otherwise
+        container_planes_encode_async's of the concatenated bytes (the first failing plane's, header unwritten)"""
+        cands = _candidates(candidates)
+        self.lib.check(self.lib.dll.rb200_container_tensors_encode_async(self.h, cands.ctypes.data_as(_u32p), cands.size, tolerance_ppm,
+                                                                         elem_bytes, refs_ptr, count, n_max, chunk_syms, flags, out_ptr,
+                                                                         out_cap), self.h)
+
+    def container_tensors_decode_async(self, elem_bytes, buf_ptr, size, refs_ptr, count, n_max, lengths_ptr=0):
+        """enqueue only (CUDA-graph capturable once a call of the same size, count and n_max has grown the workspaces): a
+        version 9 container of count tensors into the outputs of the rb200_tensor_ref list at refs_ptr (device memory:
+        each entry's ptr and capacity in bytes).  lengths_ptr (device, count u64, or 0) receives the directory.  The
+        verdict (-4 corrupt or another count, -3 a length above its capacity or a total above n_max; every output
+        untouched) comes from sync()"""
+        self.lib.check(self.lib.dll.rb200_container_tensors_decode_async(self.h, elem_bytes, buf_ptr, size, refs_ptr, count, n_max,
+                                                                         lengths_ptr or None), self.h)
 
     def container_stored_decode_async(self, buf_ptr, size, out_ptr, out_cap, n_ptr=0):
         """the async decode of a version 6 container; enqueue only (CUDA-graph capturable).  The verdict (-4 corrupt or

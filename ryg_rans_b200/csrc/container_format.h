@@ -340,23 +340,42 @@ struct PlaneEntry {
 };
 static_assert(sizeof(PlaneEntry) == 16, "plane table entries are 16 bytes");
 RB200_HD inline bool container_planes_w_ok(uint32_t w) { return w == 2 || w == 4 || w == 8; }
-// the end of the table: plane 0's offset, 16-aligned
-RB200_HD inline uint64_t container_planes_table_end(uint32_t w) { return sizeof(ContainerHeader) + sizeof(PlaneEntry) * w; }
+// plane 0's offset, 16-aligned: the end of the table, and of the directory of dir_bytes after it (version 9; 0 for
+// versions 7 and 8)
+RB200_HD inline uint64_t container_planes_table_end(uint32_t w, uint64_t dir_bytes)
+{
+    return sizeof(ContainerHeader) + sizeof(PlaneEntry) * w + dir_bytes;
+}
 // Version 8 (a delta from a base tensor): version 7's layout and rules but for two header fields, version 8 and
 // reserved = the CRC-32 of the base tensor's n bytes (covered by meta_crc, which zeroes only the two crc fields).  The
 // planes hold d, not the input: for element i with x and b the w-byte little-endian integers of the input and the
 // base, s = (x - b) mod 2^(8w) read as signed, d = (s << 1) ^ (s >> (8w - 1)) (arithmetic shift), byte k of d in plane
 // k; the inverse x = b + ((d >> 1) ^ -(d & 1)) mod 2^(8w) is exact for every bit pattern.
 constexpr uint16_t kContainerVersionDelta = 8;
-// the header rules of version 7 or 8 (`version`, the one the caller accepts); the table and the planes fit `size`.
-// Only version 7 requires reserved == 0.
+// Version 9 (a list of tensors of one element width): version 7 of the concatenation of the T tensors' bytes, in list
+// order with no padding, with a directory of the tensors' byte lengths between the table and plane 0.  The header
+// differs from version 7's in n_blocks = T (1 <= T <= 2^20) and reserved = the CRC-32 of the directory's 8 T bytes
+// (covered by meta_crc); n_symbols is the total n.  The directory is T u64 lengths, each a multiple of w (zero
+// allowed), summing to n, zero-padded to 16 bytes; blob_bytes counts the planes' bytes, from plane 0's offset.
+constexpr uint16_t kContainerVersionTensors = 9;
+constexpr uint32_t kContainerTensorsMax = 1u << 20;
+// the directory's bytes with its padding
+RB200_HD inline uint64_t container_tensors_dir_bytes(uint32_t count) { return (8ull * count + 15) & ~15ull; }
+// the directory bytes of a header of `version` (none for versions 7 and 8)
+RB200_HD inline uint64_t container_planes_dir_bytes(const ContainerHeader& h, uint16_t version)
+{
+    return version == kContainerVersionTensors ? container_tensors_dir_bytes(h.n_blocks) : 0;
+}
+// the header rules of version 7, 8 or 9 (`version`, the one the caller accepts); the table, the directory and the
+// planes fit `size`.  Only version 7 requires reserved == 0; only version 9 has n_blocks other than w.
 RB200_HD inline bool container_planes_header_version_ok(const ContainerHeader& h, uint64_t size, uint16_t version)
 {
     if (h.magic != kContainerMagic || h.version != version || h.coder || h.scale_bits || h.lanes != RB200_LANES) return false;
-    if (!container_planes_w_ok(h.block_size) || h.n_blocks != h.block_size || h.n_chunks || h.blob_crc) return false;
+    const bool list_ok = version == kContainerVersionTensors ? h.n_blocks && h.n_blocks <= kContainerTensorsMax : h.n_blocks == h.block_size;
+    if (!container_planes_w_ok(h.block_size) || !list_ok || h.n_chunks || h.blob_crc) return false;
     if (version == kContainerVersionPlanes && h.reserved) return false;
     if (!container_chunk_ok(h.chunk_syms) || !h.n_symbols || h.n_symbols % h.block_size || ((h.n_symbols / h.block_size) >> 32)) return false;
-    const uint64_t t = container_planes_table_end(h.block_size);
+    const uint64_t t = container_planes_table_end(h.block_size, container_planes_dir_bytes(h, version));
     return t <= size && h.blob_bytes <= size - t;
 }
 // version 7's header rules; the table and the planes fit `size`
@@ -364,11 +383,11 @@ RB200_HD inline bool container_planes_header_ok(const ContainerHeader& h, uint64
 {
     return container_planes_header_version_ok(h, size, kContainerVersionPlanes);
 }
-// the table: plane 0 right after it, every plane right after the previous one, each at least a header long and a
-// multiple of 16, and the last one ending where the blob does
-RB200_HD inline bool container_planes_table_ok(const ContainerHeader& h, const PlaneEntry* t)
+// the table: plane 0 right after it and the directory of dir_bytes (0 but for version 9), every plane right after the
+// previous one, each at least a header long and a multiple of 16, and the last one ending where the blob does
+RB200_HD inline bool container_planes_table_ok(const ContainerHeader& h, const PlaneEntry* t, uint64_t dir_bytes)
 {
-    uint64_t end = container_planes_table_end(h.block_size);
+    uint64_t end = container_planes_table_end(h.block_size, dir_bytes);
     const uint64_t last = end + h.blob_bytes;
     for (uint32_t p = 0; p < h.block_size; p++) {
         if (t[p].offset != end || (t[p].size & 15) || t[p].size < sizeof(ContainerHeader) || t[p].size > last - end) return false;
@@ -383,6 +402,20 @@ RB200_HD inline bool container_planes_plane_ok(const ContainerHeader& h, const C
     return ph.n_symbols == h.n_symbols / h.block_size && ph.chunk_syms == h.chunk_syms && ph.flags == h.flags &&
            container_chunks_stored_header_ok(ph, size) && container_bitmap_blob_offset(ph.n_chunks) + ph.blob_bytes == size;
 }
+// Version 9's directory rule, on entries [begin, end) of the T lengths `dir` of a header with w and n: each a
+// multiple of w (2, 4 or 8) and at most n (so the sum of all T, below 2^20 n, cannot overflow); *sum accumulates them.  The
+// directory passes when every part passes, the parts' sums add up to n and the padding word (dir[T], when T is odd) is
+// zero.
+RB200_HD inline bool container_tensors_dir_part_ok(const uint64_t* dir, uint32_t begin, uint32_t end, uint32_t w, uint64_t n, uint64_t* sum)
+{
+    bool ok = true;
+    for (uint32_t i = begin; i < end; i++) {
+        ok = ok && (dir[i] & (w - 1)) == 0 && dir[i] <= n;
+        *sum += dir[i] <= n ? dir[i] : 0;
+    }
+    return ok;
+}
+RB200_HD inline bool container_tensors_dir_pad_ok(const uint64_t* dir, uint32_t count) { return count % 2 == 0 || dir[count] == 0; }
 
 // the header rb200_container_pack writes (crc fields zero)
 ContainerHeader container_header(int coder, uint32_t scale_bits, uint32_t chunk_syms, uint64_t n, uint64_t n_chunks,

@@ -35,6 +35,11 @@
 //
 // Its planes hold the zigzag difference from the base (container_format.h); the _delta_ calls accept only version 8.
 //
+//   version 9 (a list of tensors): [ 64-byte header ][ w x {u64 offset, u64 size} ][ T x u64 lengths, pad to 16 ][ plane 0 ] ...
+//
+// Version 7 of the tensors' concatenated bytes, with n_blocks = T and reserved = CRC-32 of the directory's 8 T bytes
+// (container_format.h); the _tensors_ calls accept only version 9.
+//
 // rb200_container_pack / _open and the _blocks_ forms here work on host buffers with a host CRC (slicing-by-8, ~1 GB/s
 // on one core: the blob CRC is optional for that reason).  rb200_container_encode / _decode and the _blocks_ forms
 // (rans_b200.cu) write and read the same bytes in host or device memory with the blob CRC on the GPU
@@ -509,7 +514,14 @@ extern "C" size_t rb200_container_planes_bound(size_t n, uint32_t elem_bytes, ui
 {
     if (!container_planes_w_ok(elem_bytes) || n % elem_bytes) return 0;
     const size_t plane = rb200_container_stored_bound(n / elem_bytes, chunk_syms);
-    return plane ? container_planes_table_end(elem_bytes) + elem_bytes * plane : 0;
+    return plane ? container_planes_table_end(elem_bytes, 0) + elem_bytes * plane : 0;
+}
+
+extern "C" size_t rb200_container_tensors_bound(size_t n_max, uint32_t count, uint32_t elem_bytes, uint32_t chunk_syms)
+{
+    if (!count || count > kContainerTensorsMax) return 0;
+    const size_t b = rb200_container_planes_bound(n_max, elem_bytes, chunk_syms);
+    return b ? b + container_tensors_dir_bytes(count) : 0;
 }
 
 namespace {
@@ -525,14 +537,18 @@ int planes_plane_open(const uint8_t* plane, size_t size, ContainerHeader* h)
     return container_bitmap_blob_offset(h->n_chunks) + h->blob_bytes == size ? RB200_OK : RB200_E_STREAM;
 }
 
-// the pack of version 7 (reserved 0) or version 8 (reserved the base tensor's CRC)
-int planes_pack(uint16_t version, uint32_t reserved, uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint8_t* out,
-                size_t out_cap, size_t* out_size)
+// the pack of version 7 (reserved 0), version 8 (reserved the base tensor's CRC) or version 9 (`lengths`: the
+// directory of `count` tensors; reserved its CRC)
+int planes_pack(uint16_t version, uint32_t reserved, uint32_t elem_bytes, const uint64_t* lengths, uint32_t count, const uint8_t* const* planes,
+                const size_t* sizes, uint8_t* out, size_t out_cap, size_t* out_size)
 {
     if (!container_planes_w_ok(elem_bytes) || !planes || !sizes || !out) return RB200_E_ARG;
+    const bool list = version == kContainerVersionTensors;
+    if (list && (!lengths || !count || count > kContainerTensorsMax)) return RB200_E_ARG;
+    const uint64_t dir_bytes = list ? container_tensors_dir_bytes(count) : 0;
     ContainerHeader first{};
     PlaneEntry table[8];
-    uint64_t end = container_planes_table_end(elem_bytes);
+    uint64_t end = container_planes_table_end(elem_bytes, dir_bytes);
     for (uint32_t p = 0; p < elem_bytes; p++) {
         ContainerHeader ph;
         if (!planes[p] || planes_plane_open(planes[p], sizes[p], &ph) != RB200_OK) return RB200_E_ARG;
@@ -542,27 +558,39 @@ int planes_pack(uint16_t version, uint32_t reserved, uint32_t elem_bytes, const 
         end += sizes[p];
     }
     if (!container_chunk_ok(first.chunk_syms)) return RB200_E_ARG;          // the v7 rules take the encodes' chunk sizes
+    const uint64_t n = first.n_symbols * elem_bytes;
+    std::vector<uint64_t> dir(dir_bytes / sizeof(uint64_t), 0);
+    if (list) {
+        std::memcpy(dir.data(), lengths, sizeof(uint64_t) * count);
+        uint64_t sum = 0;
+        if (!container_tensors_dir_part_ok(dir.data(), 0, count, elem_bytes, n, &sum) || sum != n) return RB200_E_ARG;
+        reserved = container_crc32(0, dir.data(), sizeof(uint64_t) * count);
+    }
     if (end > out_cap) return RB200_E_SPACE;
     ContainerHeader h{};
     h.magic = kContainerMagic;
     h.version = version;
     h.lanes = RB200_LANES;
     h.chunk_syms = first.chunk_syms;
-    h.n_symbols = first.n_symbols * elem_bytes;
-    h.blob_bytes = end - container_planes_table_end(elem_bytes);
+    h.n_symbols = n;
+    h.blob_bytes = end - container_planes_table_end(elem_bytes, dir_bytes);
     h.flags = first.flags;
-    h.block_size = h.n_blocks = elem_bytes;
+    h.block_size = elem_bytes;
+    h.n_blocks = list ? count : elem_bytes;
     h.reserved = reserved;
     h.meta_crc = container_crc32(container_header_crc(h), table, sizeof(PlaneEntry) * elem_bytes);
     std::memcpy(out, &h, sizeof h);
     std::memcpy(out + sizeof h, table, sizeof(PlaneEntry) * elem_bytes);
+    if (dir_bytes) std::memcpy(out + container_planes_table_end(elem_bytes, 0), dir.data(), dir_bytes);
     for (uint32_t p = 0; p < elem_bytes; p++) std::memcpy(out + table[p].offset, planes[p], sizes[p]);
     if (out_size) *out_size = end;
     return RB200_OK;
 }
 
-// the open of version 7 or 8 (`version`, the one the caller accepts); *reserved receives the header's reserved word
-int planes_open(uint16_t version, const uint8_t* buf, size_t size, rb200_container_planes_info* info, uint32_t* reserved)
+// the open of version 7, 8 or 9 (`version`, the one the caller accepts); *reserved receives the header's reserved word,
+// and for version 9 *count and *lengths the directory, once its CRC (reserved) and rules pass
+int planes_open(uint16_t version, const uint8_t* buf, size_t size, rb200_container_planes_info* info, uint32_t* reserved,
+                uint32_t* count = nullptr, const uint64_t** lengths = nullptr)
 {
     if (!buf || !info) return RB200_E_ARG;
     if (size < sizeof(ContainerHeader)) return RB200_E_STREAM;
@@ -571,10 +599,21 @@ int planes_open(uint16_t version, const uint8_t* buf, size_t size, rb200_contain
     if (!container_planes_header_version_ok(h, size, version)) return RB200_E_STREAM;
     if (reinterpret_cast<uintptr_t>(buf) & 7) return RB200_E_ARG;
     const uint32_t w = h.block_size;
+    const uint64_t dir_bytes = container_planes_dir_bytes(h, version);
     PlaneEntry table[8];
     std::memcpy(table, buf + sizeof h, sizeof(PlaneEntry) * w);
-    if (container_crc32(container_header_crc(h), table, sizeof(PlaneEntry) * w) != h.meta_crc || !container_planes_table_ok(h, table))
+    if (container_crc32(container_header_crc(h), table, sizeof(PlaneEntry) * w) != h.meta_crc || !container_planes_table_ok(h, table, dir_bytes))
         return RB200_E_STREAM;
+    if (version == kContainerVersionTensors) {                        // the directory lies in size (header rule)
+        const uint64_t* dir = reinterpret_cast<const uint64_t*>(buf + container_planes_table_end(w, 0));
+        uint64_t sum = 0;
+        if (container_crc32(0, dir, sizeof(uint64_t) * h.n_blocks) != h.reserved ||
+            !container_tensors_dir_part_ok(dir, 0, h.n_blocks, w, h.n_symbols, &sum) || sum != h.n_symbols ||
+            !container_tensors_dir_pad_ok(dir, h.n_blocks))
+            return RB200_E_STREAM;
+        *count = h.n_blocks;
+        *lengths = dir;
+    }
     for (uint32_t p = 0; p < w; p++) {
         ContainerHeader ph;
         std::memcpy(&ph, buf + table[p].offset, sizeof ph);
@@ -599,7 +638,7 @@ int planes_open(uint16_t version, const uint8_t* buf, size_t size, rb200_contain
 extern "C" int rb200_container_planes_pack(uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint8_t* out,
                                            size_t out_cap, size_t* out_size)
 {
-    return planes_pack(kContainerVersionPlanes, 0, elem_bytes, planes, sizes, out, out_cap, out_size);
+    return planes_pack(kContainerVersionPlanes, 0, elem_bytes, nullptr, 0, planes, sizes, out, out_cap, out_size);
 }
 
 extern "C" int rb200_container_planes_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info)
@@ -611,13 +650,27 @@ extern "C" int rb200_container_planes_open(const uint8_t* buf, size_t size, rb20
 extern "C" int rb200_container_delta_pack(uint32_t elem_bytes, const uint8_t* const* planes, const size_t* sizes, uint32_t base_crc,
                                           uint8_t* out, size_t out_cap, size_t* out_size)
 {
-    return planes_pack(kContainerVersionDelta, base_crc, elem_bytes, planes, sizes, out, out_cap, out_size);
+    return planes_pack(kContainerVersionDelta, base_crc, elem_bytes, nullptr, 0, planes, sizes, out, out_cap, out_size);
 }
 
 extern "C" int rb200_container_delta_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info, uint32_t* base_crc)
 {
     if (!base_crc) return RB200_E_ARG;
     return planes_open(kContainerVersionDelta, buf, size, info, base_crc);
+}
+
+extern "C" int rb200_container_tensors_pack(uint32_t elem_bytes, const uint64_t* lengths, uint32_t count, const uint8_t* const* planes,
+                                            const size_t* sizes, uint8_t* out, size_t out_cap, size_t* out_size)
+{
+    return planes_pack(kContainerVersionTensors, 0, elem_bytes, lengths, count, planes, sizes, out, out_cap, out_size);
+}
+
+extern "C" int rb200_container_tensors_open(const uint8_t* buf, size_t size, rb200_container_planes_info* info, uint32_t* count,
+                                            const uint64_t** lengths)
+{
+    if (!count || !lengths) return RB200_E_ARG;
+    uint32_t reserved;
+    return planes_open(kContainerVersionTensors, buf, size, info, &reserved, count, lengths);
 }
 
 extern "C" int rb200_choose_coder(const uint64_t counts[256], size_t n, uint32_t chunk_syms, const uint32_t* candidates,

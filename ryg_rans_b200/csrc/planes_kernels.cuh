@@ -34,6 +34,18 @@
 //   decode: delta_plan_kernel (the plan with version 8's rules), every plane as above, delta_verdict_kernel (the verdict,
 //           then the base's length: n when go, else 0), crc32_kernel over that many bytes of base, delta_check_kernel
 //           (a CRC other than the header's: kStatBase, go cleared), delta_interleave_kernel<W> (d and base into out)
+// The tensor-list container (version 9, rb200_container_tensors_encode_async / _decode_async) runs the same host bodies
+// with a list of rb200_tensor_ref in device memory in place of in / out:
+//   encode: tensors_plan_kernel (one CTA: the list checked, the exclusive prefix of its element counts into a context
+//           workspace, PlanesVarlenGeom {n, m} -- {0, UINT64_MAX} for a bad list, which every plane's version 6 varlen
+//           plan refuses -- and, only for a good list, the directory into out), tensors_split_kernel<W> (the segmented
+//           split), crc32_kernel over the directory into the call's TensorsWork, every plane as the varlen encode's,
+//           tensors_finish_kernel (the finish with version 9, n_blocks = T, reserved = the directory's CRC)
+//   decode: tensors_open_kernel (the plan with version 9's rules and T == count), every plane as above,
+//           planes_verdict_kernel with n_max for out_cap, crc32_kernel over the directory (its length 8 T from the
+//           plan, 0 for a rejected header), tensors_check_kernel (the CRC against reserved, the directory's rules and
+//           every length against its ref's capacity, else go cleared; then the directory's prefix into a workspace),
+//           tensors_interleave_kernel<W> (the segmented inverse scatter into the refs)
 #pragma once
 #include "container_decode.cuh"
 #include "container_format.h"
@@ -65,6 +77,13 @@ struct PlanesVarlenGeom {
 struct DeltaWork {
     CrcSlot crc;
     uint64_t base_n;
+};
+
+// The directory's CRC of a tensor-list call (one for the encode, one for the decode): crc32_kernel's result, and on
+// decode the length it covers (8 T once the header passed, else 0: the directory is then not read).
+struct TensorsWork {
+    CrcSlot crc;
+    uint64_t dir_len;
 };
 
 constexpr uint32_t kPlanesThreads = 256;
@@ -308,12 +327,14 @@ __global__ void __launch_bounds__(kPlanesThreads)
     planes_interleave<W, true>(planes, stride, base, out, r);
 }
 
-// Encode: plane p's verdict and place.  Its container is complete (header included) at src -- out + 64 + 16 W for
+// Encode: plane p's verdict and place.  Its container is complete (header included) at src -- out + 64 + 16 units for
 // plane 0, the staging area for the others -- exactly when the status word is clear, since version 6's header kernel
-// writes only then.  Entry p: the offset right after plane p - 1 (entry p - 1, written by the previous launch), the
-// size from the plane's header.  Plane 0 is in place; the others are copied, 16 bytes per thread and step.
+// writes only then.  units counts the 16-byte units between the header and plane 0: W table entries, and in version 9
+// round16(8 T) / 16 more for the directory.  Entry p: the offset right after plane p - 1 (entry p - 1, written by the
+// previous launch), the size from the plane's header.  Plane 0 is in place; the others are copied, 16 bytes per thread
+// and step.
 __global__ void __launch_bounds__(kPlanesThreads)
-    planes_place_kernel(uint8_t* __restrict__ out, const uint8_t* __restrict__ src, uint32_t p, uint32_t w, uint64_t out_cap,
+    planes_place_kernel(uint8_t* __restrict__ out, const uint8_t* __restrict__ src, uint32_t p, uint32_t units, uint64_t out_cap,
                         PlanesWork* __restrict__ r, uint32_t* status)
 {
     const bool ok = *status == 0;
@@ -323,7 +344,7 @@ __global__ void __launch_bounds__(kPlanesThreads)
     PlaneEntry* table = reinterpret_cast<PlaneEntry*>(out + sizeof(ContainerHeader));
     const ContainerHeader h = *reinterpret_cast<const ContainerHeader*>(src);
     const uint64_t size = container_bitmap_blob_offset(h.n_chunks) + h.blob_bytes;
-    const uint64_t offset = p ? table[p - 1].offset + table[p - 1].size : container_planes_table_end(w);
+    const uint64_t offset = p ? table[p - 1].offset + table[p - 1].size : sizeof(ContainerHeader) + sizeof(PlaneEntry) * units;
     if (offset > out_cap || size > out_cap - offset) {                // not reached: the host checked the bound
         if (first) atomicOr(status, kStatSpace);
         return;
@@ -351,8 +372,9 @@ __device__ __forceinline__ uint32_t planes_meta_crc(const uint8_t* s, uint32_t b
 }
 
 // Encode: the version 7 header, when every plane was placed and the status word is still clear.  h arrives complete
-// but for blob_bytes and meta_crc; s_v is the kernel's shared staging of header and table.
-__device__ __forceinline__ void planes_finish(uint4* s_v, uint8_t* out, ContainerHeader h, const PlanesWork* __restrict__ r,
+// but for blob_bytes and meta_crc; s_v is the kernel's shared staging of header and table; dir_bytes the directory's
+// (version 9; 0 otherwise), between the table and plane 0.
+__device__ __forceinline__ void planes_finish(uint4* s_v, uint8_t* out, ContainerHeader h, uint64_t dir_bytes, const PlanesWork* __restrict__ r,
                                               const uint32_t* status)
 {
     uint8_t* s = reinterpret_cast<uint8_t*>(s_v);
@@ -361,8 +383,8 @@ __device__ __forceinline__ void planes_finish(uint4* s_v, uint8_t* out, Containe
     for (uint32_t p = 0; p < w; p++) all = all && r->plane_go[p];
     if (!all) return;
     const PlaneEntry* table = reinterpret_cast<const PlaneEntry*>(out + sizeof(ContainerHeader));
-    const uint64_t end = container_planes_table_end(w);
-    h.blob_bytes = table[w - 1].offset + table[w - 1].size - end;
+    const uint64_t end = container_planes_table_end(w, 0);
+    h.blob_bytes = table[w - 1].offset + table[w - 1].size - end - dir_bytes;
     h.meta_crc = 0;
     h.blob_crc = 0;
     if (lane == 0) *reinterpret_cast<ContainerHeader*>(s) = h;
@@ -378,7 +400,7 @@ __global__ void __launch_bounds__(32)
     planes_finish_kernel(uint8_t* out, ContainerHeader h, const PlanesWork* __restrict__ r, const uint32_t* status)
 {
     __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
-    planes_finish(s_v, out, h, r, status);
+    planes_finish(s_v, out, h, 0, r, status);
 }
 
 // The finish of the delta encode: version 8, reserved the base's CRC
@@ -388,7 +410,7 @@ __global__ void __launch_bounds__(32)
     __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
     h.version = kContainerVersionDelta;
     h.reserved = d->crc.crc;
-    planes_finish(s_v, out, h, r, status);
+    planes_finish(s_v, out, h, 0, r, status);
 }
 
 // The finish of the varlen encode: n from the record.  A bad length left the status word set, so nothing is written.
@@ -398,7 +420,7 @@ __global__ void __launch_bounds__(32)
 {
     __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
     h.n_symbols = g->n;
-    planes_finish(s_v, out, h, r, status);
+    planes_finish(s_v, out, h, 0, r, status);
 }
 
 // The first kernel of the varlen encode, one thread: reads n = *d_n and writes n and m = n / w into *g when
@@ -413,17 +435,19 @@ __global__ void __launch_bounds__(32)
     *g = ok ? PlanesVarlenGeom{n, n / w} : PlanesVarlenGeom{0, UINT64_MAX};
 }
 
-// Decode: every rule of version 7 (VERSION 8: version 8's) on the header, the table and the planes' headers, and
-// meta_crc; the record is reset for the call.  One warp: lanes 0..3 stage the header, lanes 4.. the table, lane p < W
-// checks plane p's header.
+// Decode: every rule of version 7 (VERSION 8 or 9: that version's, and for 9 a T of count) on the header, the table
+// and the planes' headers, and meta_crc; the record is reset for the call.  One warp: lanes 0..3 stage the header,
+// lanes 4.. the table, lane p < W checks plane p's header.
 template <uint16_t VERSION>
-__device__ __forceinline__ void planes_plan(uint4* s_v, const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, PlanesWork* __restrict__ r)
+__device__ __forceinline__ void planes_plan(uint4* s_v, const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, uint32_t count,
+                                            PlanesWork* __restrict__ r)
 {
     uint8_t* s = reinterpret_cast<uint8_t*>(s_v);
     const uint32_t lane = threadIdx.x;
     ContainerHeader h = {};
     if (size >= sizeof(ContainerHeader)) h = *reinterpret_cast<const ContainerHeader*>(buf);   // a shorter buffer is not read
-    bool ok = size >= sizeof(ContainerHeader) && container_planes_header_version_ok(h, size, VERSION) && h.block_size == w;
+    bool ok = size >= sizeof(ContainerHeader) && container_planes_header_version_ok(h, size, VERSION) && h.block_size == w &&
+              (VERSION != kContainerVersionTensors || h.n_blocks == count);
     const uint32_t meta_crc = h.meta_crc;
     if (ok) {                                                         // the table lies in size (header rule)
         h.meta_crc = 0;
@@ -432,7 +456,8 @@ __device__ __forceinline__ void planes_plan(uint4* s_v, const uint8_t* __restric
         if (lane < w) s_v[4 + lane] = reinterpret_cast<const uint4*>(buf + sizeof(ContainerHeader))[lane];
         __syncwarp();
         const PlaneEntry* table = reinterpret_cast<const PlaneEntry*>(s + sizeof(ContainerHeader));
-        ok = planes_meta_crc(s, static_cast<uint32_t>(container_planes_table_end(w))) == meta_crc && container_planes_table_ok(h, table);
+        ok = planes_meta_crc(s, static_cast<uint32_t>(container_planes_table_end(w, 0))) == meta_crc &&
+             container_planes_table_ok(h, table, container_planes_dir_bytes(h, VERSION));
         // each plane's header lies in size once the table passes
         const bool plane = !ok || lane >= w ||
                            container_planes_plane_ok(h, *reinterpret_cast<const ContainerHeader*>(buf + table[lane].offset), table[lane].size);
@@ -453,14 +478,14 @@ __global__ void __launch_bounds__(32)
     planes_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, PlanesWork* __restrict__ r)
 {
     __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
-    planes_plan<kContainerVersionPlanes>(s_v, buf, size, w, r);
+    planes_plan<kContainerVersionPlanes>(s_v, buf, size, w, 0, r);
 }
 
 __global__ void __launch_bounds__(32)
     delta_plan_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, PlanesWork* __restrict__ r)
 {
     __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
-    planes_plan<kContainerVersionDelta>(s_v, buf, size, w, r);
+    planes_plan<kContainerVersionDelta>(s_v, buf, size, w, 0, r);
 }
 
 // Decode: plane p's bytes into staging, when the record passed and the plane fits it; otherwise a zero header, which
@@ -534,6 +559,313 @@ __global__ void __launch_bounds__(32)
     if (d->crc.crc != reinterpret_cast<const ContainerHeader*>(buf)->reserved) {
         r->go = 0;
         atomicOr(status, kStatBase);
+    }
+}
+
+// ---- version 9: a list of tensors
+
+constexpr uint32_t kTensorsPlanThreads = 1024;   // the plan and check kernels: one CTA, 32 warps
+
+// Thread t of a kTensorsPlanThreads CTA takes the entries [begin, end) of count: a run of ceil(count / threads)
+__device__ __forceinline__ void tensors_run(uint32_t count, uint32_t& begin, uint32_t& end)
+{
+    const uint32_t k = (count + kTensorsPlanThreads - 1) / kTensorsPlanThreads;
+    begin = min(threadIdx.x * k, count);
+    end = min(begin + k, count);
+}
+
+// The CTA's exclusive scan of one value per thread (the sum of its run): returns the sum of the threads before this
+// one, and *total the sum of all.  s_warp: 32 words of shared memory.
+__device__ __forceinline__ uint64_t tensors_block_scan(uint64_t v, uint64_t* s_warp, uint64_t* total)
+{
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint64_t x = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint64_t y = __shfl_up_sync(0xffffffffu, x, d);
+        if (lane >= d) x += y;
+    }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        uint64_t t = s_warp[lane];
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint64_t y = __shfl_up_sync(0xffffffffu, t, d);
+            if (lane >= d) t += y;
+        }
+        s_warp[lane] = t;
+    }
+    __syncthreads();
+    *total = s_warp[31];
+    return (warp ? s_warp[warp - 1] : 0) + x - v;
+}
+
+// Encode, the first kernel: every entry of the list -- bytes a multiple of w and at most n_max (so the sum of the
+// count entries cannot overflow), ptr nonzero and aligned to w unless bytes is 0 -- and the total, 1 .. n_max.  Writes
+// the exclusive prefix of the element counts, prefix[0 .. count], and *g: {n, n / w}, or {0, UINT64_MAX} for a bad list
+// (which every plane's version 6 varlen plan refuses as kStatArg, so nothing is written).  Only a good list's lengths
+// go to the directory at dir, with its zero padding.
+__global__ void __launch_bounds__(kTensorsPlanThreads)
+    tensors_plan_kernel(const rb200_tensor_ref* __restrict__ refs, uint32_t count, uint32_t w, uint64_t n_max, uint64_t* __restrict__ prefix,
+                        PlanesVarlenGeom* __restrict__ g, uint64_t* __restrict__ dir)
+{
+    __shared__ uint64_t s_warp[32];
+    const uint32_t shift = __ffs(w) - 1;                               // w is 2, 4 or 8
+    uint32_t begin, end;
+    tensors_run(count, begin, end);
+    bool ok = true;
+    uint64_t sum = 0;                                                  // elements
+    for (uint32_t i = begin; i < end; i++) {
+        const rb200_tensor_ref t = refs[i];
+        const bool fits = t.bytes <= n_max;
+        ok = ok && fits && !(t.bytes & (w - 1)) && (t.bytes == 0 || (t.ptr && !(t.ptr & (w - 1))));
+        sum += fits ? t.bytes >> shift : 0;
+    }
+    ok = __syncthreads_and(ok);
+    uint64_t total;
+    uint64_t e = tensors_block_scan(sum, s_warp, &total);
+    ok = ok && total && total <= n_max >> shift;
+    for (uint32_t i = begin; i < end; i++) {
+        const uint64_t bytes = refs[i].bytes;
+        prefix[i] = e;
+        e += bytes <= n_max ? bytes >> shift : 0;
+        if (ok) dir[i] = bytes;
+    }
+    if (threadIdx.x == 0) {
+        prefix[count] = total;
+        if (ok && count % 2) dir[count] = 0;
+        *g = ok ? PlanesVarlenGeom{total << shift, total} : PlanesVarlenGeom{0, UINT64_MAX};
+    }
+}
+
+// A thread's place in the list: tensor i holds the elements [lo, hi) of the concatenation, at ptr
+struct TensorCursor {
+    uint32_t i;
+    uint64_t lo, hi, ptr;
+};
+
+// Moves c to the tensor that holds element e < prefix[count]; e never decreases along a thread's walk, so c stays while
+// e < hi and otherwise a binary search over prefix[c.i .. count] finds the last tensor that starts at or before e, which
+// is never one of zero length.
+__device__ __forceinline__ void tensors_seek(const uint64_t* __restrict__ prefix, const rb200_tensor_ref* __restrict__ refs, uint32_t count,
+                                             uint64_t e, TensorCursor& c)
+{
+    if (e < c.hi) return;
+    uint32_t a = c.i, b = count;                                       // prefix[a] <= e < prefix[b]
+    while (b - a > 1) {
+        const uint32_t mid = (a + b) / 2;
+        if (prefix[mid] <= e) a = mid;
+        else b = mid;
+    }
+    c.i = a;
+    c.lo = prefix[a];
+    c.hi = prefix[a + 1];
+    c.ptr = refs[a].ptr;
+}
+
+// Element j (0..15) of 16 in 4 W words, as planes_load_group leaves them
+template <int W>
+__device__ __forceinline__ void tensors_put(uint32_t (&x)[4 * W], int j, uint64_t v)
+{
+    if (W == 2) {
+        if (j & 1) x[j >> 1] |= static_cast<uint32_t>(v) << 16;
+        else x[j >> 1] = static_cast<uint32_t>(v);
+    } else if (W == 4) {
+        x[j] = static_cast<uint32_t>(v);
+    } else {
+        x[2 * j] = static_cast<uint32_t>(v);
+        x[2 * j + 1] = static_cast<uint32_t>(v >> 32);
+    }
+}
+template <int W>
+__device__ __forceinline__ uint64_t tensors_get(const uint32_t (&x)[4 * W], int j)
+{
+    if (W == 2) return (x[j >> 1] >> (16 * (j & 1))) & 0xffffu;
+    if (W == 4) return x[j];
+    return static_cast<uint64_t>(x[2 * j + 1]) << 32 | x[2 * j];
+}
+
+// One element at a w-aligned address (the encode's list rule)
+template <int W>
+__device__ __forceinline__ uint64_t tensors_load(uint64_t addr)
+{
+    if (W == 2) return *reinterpret_cast<const uint16_t*>(addr);
+    if (W == 4) return *reinterpret_cast<const uint32_t*>(addr);
+    return *reinterpret_cast<const uint64_t*>(addr);
+}
+// One element at any address: the decode's outputs need no alignment
+template <int W>
+__device__ __forceinline__ void tensors_store(uint64_t addr, uint64_t v)
+{
+    if (addr % W) {
+#pragma unroll
+        for (int k = 0; k < W; k++) reinterpret_cast<uint8_t*>(addr)[k] = static_cast<uint8_t>(v >> (8 * k));
+    } else if (W == 2) {
+        *reinterpret_cast<uint16_t*>(addr) = static_cast<uint16_t>(v);
+    } else if (W == 4) {
+        *reinterpret_cast<uint32_t*>(addr) = static_cast<uint32_t>(v);
+    } else {
+        *reinterpret_cast<uint64_t*>(addr) = v;
+    }
+}
+
+// The segmented split: the concatenation of the list's tensors (m elements, from the record) into W planes, as
+// planes_split_kernel would split the concatenated bytes.  Groups of 16 elements; a group that lies in one tensor at a
+// 16-byte-aligned address takes W 16-byte loads, any other (across tensors, or in an element-aligned view) one load
+// per element.  The ragged end (fewer than 16 elements) an element per thread.  Nothing for a bad list.
+template <int W>
+__global__ void __launch_bounds__(kPlanesThreads)
+    tensors_split_kernel(const rb200_tensor_ref* __restrict__ refs, const uint64_t* __restrict__ prefix, uint32_t count,
+                         const PlanesVarlenGeom* __restrict__ geom, uint8_t* __restrict__ planes, uint64_t stride)
+{
+    if (geom->n == 0) return;
+    const uint64_t m = geom->m, groups = m / 16, step = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    const uint64_t tid = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    TensorCursor c = {0, 0, 0, 0};
+    for (uint64_t g = tid; g < groups; g += step) {
+        const uint64_t e = g * 16;
+        tensors_seek(prefix, refs, count, e, c);
+        uint32_t x[4 * W], y[4 * W];
+        const uint64_t src = c.ptr + (e - c.lo) * W;
+        if (e + 16 <= c.hi && !(src & 15)) {
+            planes_load_group<W>(reinterpret_cast<const uint4*>(src), x);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                tensors_seek(prefix, refs, count, e + j, c);
+                tensors_put<W>(x, j, tensors_load<W>(c.ptr + (e + j - c.lo) * W));
+            }
+        }
+        planes_transpose<W>(x, y);
+#pragma unroll
+        for (int k = 0; k < W; k++)
+            *reinterpret_cast<uint4*>(planes + k * stride + g * 16) = make_uint4(y[4 * k], y[4 * k + 1], y[4 * k + 2], y[4 * k + 3]);
+    }
+    const uint64_t tail = groups * 16;
+    if (tid < m - tail) {
+        const uint64_t e = tail + tid;
+        tensors_seek(prefix, refs, count, e, c);
+        const uint64_t v = tensors_load<W>(c.ptr + (e - c.lo) * W);
+#pragma unroll
+        for (int k = 0; k < W; k++) planes[k * stride + e] = static_cast<uint8_t>(v >> (8 * k));
+    }
+}
+
+// Its inverse, from the decode workspace into the refs' outputs, only when every check passed: the groups' 16-byte
+// stores where a group lies in one tensor at a 16-byte-aligned address, element stores otherwise.
+template <int W>
+__global__ void __launch_bounds__(kPlanesThreads)
+    tensors_interleave_kernel(const uint8_t* __restrict__ planes, uint64_t stride, const rb200_tensor_ref* __restrict__ refs,
+                              const uint64_t* __restrict__ prefix, uint32_t count, const PlanesWork* __restrict__ r)
+{
+    if (!r->go) return;
+    const uint64_t m = r->n / W, groups = m / 16, step = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    const uint64_t tid = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    TensorCursor c = {0, 0, 0, 0};
+    for (uint64_t g = tid; g < groups; g += step) {
+        uint32_t x[4 * W], y[4 * W];
+#pragma unroll
+        for (int k = 0; k < W; k++) {
+            const uint4 v = __ldcs(reinterpret_cast<const uint4*>(planes + k * stride + g * 16));
+            y[4 * k] = v.x;
+            y[4 * k + 1] = v.y;
+            y[4 * k + 2] = v.z;
+            y[4 * k + 3] = v.w;
+        }
+        planes_untranspose<W>(y, x);
+        const uint64_t e = g * 16;
+        tensors_seek(prefix, refs, count, e, c);
+        const uint64_t dst = c.ptr + (e - c.lo) * W;
+        if (e + 16 <= c.hi && !(dst & 15)) {
+            uint4* d = reinterpret_cast<uint4*>(dst);
+#pragma unroll
+            for (int i = 0; i < W; i++) d[i] = make_uint4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                tensors_seek(prefix, refs, count, e + j, c);
+                tensors_store<W>(c.ptr + (e + j - c.lo) * W, tensors_get<W>(x, j));
+            }
+        }
+    }
+    const uint64_t tail = groups * 16;
+    if (tid < m - tail) {
+        const uint64_t e = tail + tid;
+        uint64_t v = 0;
+#pragma unroll
+        for (int k = 0; k < W; k++) v |= static_cast<uint64_t>(planes[k * stride + e]) << (8 * k);
+        tensors_seek(prefix, refs, count, e, c);
+        tensors_store<W>(c.ptr + (e - c.lo) * W, v);
+    }
+}
+
+// Encode, last: the version 9 header (h arrives with version 9 and n_blocks = T), with n from the record and reserved
+// the directory's CRC.  A bad list left the status word set, so nothing is written.
+__global__ void __launch_bounds__(32)
+    tensors_finish_kernel(uint8_t* out, ContainerHeader h, uint64_t dir_bytes, const PlanesVarlenGeom* __restrict__ g,
+                          const TensorsWork* __restrict__ t, const PlanesWork* __restrict__ r, const uint32_t* status)
+{
+    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
+    h.n_symbols = g->n;
+    h.reserved = t->crc.crc;
+    planes_finish(s_v, out, h, dir_bytes, r, status);
+}
+
+// Decode, first: the plan with version 9's rules and T == count, and the directory's length for its CRC (8 T once the
+// header and table passed, so the directory lies in size; else 0)
+__global__ void __launch_bounds__(32)
+    tensors_open_kernel(const uint8_t* __restrict__ buf, uint64_t size, uint32_t w, uint32_t count, PlanesWork* __restrict__ r,
+                        TensorsWork* __restrict__ t)
+{
+    __shared__ uint4 s_v[(sizeof(ContainerHeader) + 8 * sizeof(PlaneEntry)) / 16];
+    planes_plan<kContainerVersionTensors>(s_v, buf, size, w, count, r);
+    if (threadIdx.x == 0) t->dir_len = r->ok ? 8ull * count : 0;
+}
+
+// Decode, after the verdict, when every other check passed: the directory's CRC against the header's reserved word,
+// its rules (container_tensors_dir_part_ok over every thread's run, the sum n, the zero padding) -- a failure is
+// kStatStream -- then d_lengths and the directory's exclusive prefix in elements, prefix[0 .. count], and every length
+// against its ref's capacity -- a failure is kStatSpace.  Either clears go, so the interleave writes nothing.
+__global__ void __launch_bounds__(kTensorsPlanThreads)
+    tensors_check_kernel(const uint8_t* __restrict__ buf, uint32_t w, uint32_t count, const rb200_tensor_ref* __restrict__ refs,
+                         uint64_t* __restrict__ prefix, uint64_t* __restrict__ d_lengths, const TensorsWork* __restrict__ t,
+                         PlanesWork* __restrict__ r, uint32_t* status)
+{
+    __shared__ uint64_t s_warp[32];
+    if (!r->go) return;                  // every thread reads go before any clears it: the clears follow the barriers below
+    const uint64_t* dir = reinterpret_cast<const uint64_t*>(buf + container_planes_table_end(w, 0));
+    const uint64_t n = r->n;
+    const uint32_t shift = __ffs(w) - 1;                               // w is 2, 4 or 8
+    uint32_t begin, end;
+    tensors_run(count, begin, end);
+    uint64_t sum = 0;
+    bool ok = container_tensors_dir_part_ok(dir, begin, end, w, n, &sum);
+    if (threadIdx.x == 0)
+        ok = ok && t->crc.crc == reinterpret_cast<const ContainerHeader*>(buf)->reserved && container_tensors_dir_pad_ok(dir, count);
+    ok = __syncthreads_and(ok);
+    uint64_t total;
+    uint64_t e = tensors_block_scan(sum, s_warp, &total);
+    if (!ok || total != n) {
+        if (threadIdx.x == 0) {
+            r->go = 0;
+            atomicOr(status, kStatStream);
+        }
+        return;
+    }
+    bool fits = true;
+    for (uint32_t i = begin; i < end; i++) {
+        const uint64_t bytes = dir[i];
+        if (d_lengths) d_lengths[i] = bytes;
+        prefix[i] = e >> shift;
+        e += bytes;
+        fits = fits && bytes <= refs[i].bytes;
+    }
+    if (threadIdx.x == 0) prefix[count] = n >> shift;
+    fits = __syncthreads_and(fits);
+    if (!fits && threadIdx.x == 0) {
+        r->go = 0;
+        atomicOr(status, kStatSpace);
     }
 }
 

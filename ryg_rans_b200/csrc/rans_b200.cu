@@ -89,6 +89,11 @@ struct rb200_ctx {
     // the delta calls (version 8): the base's CRC, one record for the encode, one for the decode
     DeltaWork* d_delta_enc = nullptr;
     DeltaWork* d_delta_dec = nullptr;
+    // the tensor-list calls (version 9): the directory's CRC and the list's prefix, one of each for the encode and the
+    // decode
+    TensorsWork* d_tensors_enc = nullptr;
+    TensorsWork* d_tensors_dec = nullptr;
+    DevBuf tensors_enc_prefix, tensors_dec_prefix;
 };
 
 struct rb200_model {
@@ -274,6 +279,10 @@ extern "C" int rb200_ctx_create(rb200_ctx** out, int device, void* stream)
         if (e == cudaSuccess) e = cudaMalloc(d, sizeof(DeltaWork));
         if (e == cudaSuccess) e = cudaMemset(*d, 0, sizeof(DeltaWork));
     }
+    for (TensorsWork** t : {&ctx->d_tensors_enc, &ctx->d_tensors_dec}) {
+        if (e == cudaSuccess) e = cudaMalloc(t, sizeof(TensorsWork));
+        if (e == cudaSuccess) e = cudaMemset(*t, 0, sizeof(TensorsWork));
+    }
     if (e != cudaSuccess) {
         rb200_ctx_destroy(ctx);
         return RB200_E_CUDA;
@@ -299,6 +308,7 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     release(ctx->scratch); release(ctx->sizes);
     release(ctx->st_in); release(ctx->st_blob); release(ctx->st_offsets); release(ctx->st_out); release(ctx->st_aux);
     release(ctx->planes_in); release(ctx->planes_enc_stage); release(ctx->planes_out); release(ctx->planes_dec_stage);
+    release(ctx->tensors_enc_prefix); release(ctx->tensors_dec_prefix);
     if (ctx->d_status) cudaFree(ctx->d_status);
     if (ctx->d_work) cudaFree(ctx->d_work);
     if (ctx->h_status) cudaFreeHost(ctx->h_status);
@@ -319,6 +329,8 @@ extern "C" void rb200_ctx_destroy(rb200_ctx* ctx)
     if (ctx->d_planes_geom) cudaFree(ctx->d_planes_geom);
     if (ctx->d_delta_enc) cudaFree(ctx->d_delta_enc);
     if (ctx->d_delta_dec) cudaFree(ctx->d_delta_dec);
+    if (ctx->d_tensors_enc) cudaFree(ctx->d_tensors_enc);
+    if (ctx->d_tensors_dec) cudaFree(ctx->d_tensors_dec);
     for (int i = 0; i < rb200_ctx::kMaxSlices; i++) {
         if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
@@ -2451,10 +2463,22 @@ namespace {
 // a grid of every CTA of the byte-plane kernels that is resident at once: they stride over what they move
 uint32_t planes_grid(const rb200_ctx* ctx) { return static_cast<uint32_t>(ctx->sms) * kPlanesCtasPerSm; }
 
-// geom set: the varlen split, m from the record; base set: the delta split
-int launch_split(rb200_ctx* ctx, uint32_t w, const uint8_t* in, const uint8_t* base, uint64_t m, const PlanesVarlenGeom* geom, uint8_t* planes,
-                 uint64_t stride)
+// The list a tensor-list call reads, in device memory, with its prefix workspace (count + 1 u64)
+struct TensorList {
+    const rb200_tensor_ref* refs;
+    uint32_t count;
+    uint64_t* prefix;
+};
+
+// geom set: the varlen split, m from the record; base set: the delta split; list set: the segmented split (geom set too)
+int launch_split(rb200_ctx* ctx, uint32_t w, const uint8_t* in, const uint8_t* base, uint64_t m, const PlanesVarlenGeom* geom, const TensorList* list,
+                 uint8_t* planes, uint64_t stride)
 {
+    if (list) {
+        auto split = w == 2 ? tensors_split_kernel<2> : w == 4 ? tensors_split_kernel<4> : tensors_split_kernel<8>;
+        split<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(list->refs, list->prefix, list->count, geom, planes, stride);
+        return check_launch(ctx, "tensors_split_kernel");
+    }
     if (base) {
         auto split = w == 2 ? delta_split_kernel<2> : w == 4 ? delta_split_kernel<4> : delta_split_kernel<8>;
         split<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(in, base, m, planes, stride);
@@ -2470,9 +2494,15 @@ int launch_split(rb200_ctx* ctx, uint32_t w, const uint8_t* in, const uint8_t* b
     return check_launch(ctx, "planes_split_kernel");
 }
 
-// base set: the delta interleave, out = base + the decoded difference
-int launch_interleave(rb200_ctx* ctx, uint32_t w, const uint8_t* planes, uint64_t stride, const uint8_t* base, uint8_t* out, const PlanesWork* r)
+// base set: the delta interleave, out = base + the decoded difference; list set: the segmented interleave into its refs
+int launch_interleave(rb200_ctx* ctx, uint32_t w, const uint8_t* planes, uint64_t stride, const uint8_t* base, const TensorList* list, uint8_t* out,
+                      const PlanesWork* r)
 {
+    if (list) {
+        auto interleave = w == 2 ? tensors_interleave_kernel<2> : w == 4 ? tensors_interleave_kernel<4> : tensors_interleave_kernel<8>;
+        interleave<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(planes, stride, list->refs, list->prefix, list->count, r);
+        return check_launch(ctx, "tensors_interleave_kernel");
+    }
     if (base) {
         auto interleave = w == 2 ? delta_interleave_kernel<2> : w == 4 ? delta_interleave_kernel<4> : delta_interleave_kernel<8>;
         interleave<<<planes_grid(ctx), kPlanesThreads, 0, ctx->stream>>>(planes, stride, base, out, r);
@@ -2492,37 +2522,54 @@ int launch_interleave(rb200_ctx* ctx, uint32_t w, const uint8_t* planes, uint64_
 // the record's m as its length.  Arguments are checked here, with n_max for n.
 // base set (rb200_container_delta_encode_async, never with d_n): the delta split, the base's CRC (crc32_kernel into the
 // call's DeltaWork) right after it, and the delta finish, which writes version 8 with the CRC in reserved.
+// refs set (rb200_container_tensors_encode_async, with n = n_max): the varlen encode with tensors_plan_kernel in place
+// of its plan (the list checked, its prefix, the record, the directory), the segmented split, the directory's CRC
+// (crc32_kernel into the call's TensorsWork) right after it, plane 0 after the directory, and the tensors finish, which
+// writes version 9.  Arguments are checked here, with n_max for n and the list for in.
 int planes_encode(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm, uint32_t w, const uint8_t* in,
-                  const uint8_t* base, size_t n, const uint64_t* d_n, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
+                  const uint8_t* base, size_t n, const uint64_t* d_n, const rb200_tensor_ref* refs, uint32_t count, uint32_t chunk_syms,
+                  uint32_t flags, uint8_t* out, size_t out_cap)
 {
-    if (!container_planes_w_ok(w) || n == 0 || n % w || ((n / w) >> 32) || (reinterpret_cast<uintptr_t>(in) & 15)) return RB200_E_ARG;
+    const uint8_t* src = refs ? reinterpret_cast<const uint8_t*>(refs) : in;
+    if (!container_planes_w_ok(w) || n == 0 || n % w || ((n / w) >> 32) || (reinterpret_cast<uintptr_t>(src) & 15)) return RB200_E_ARG;
     const size_t m = n / w;
     if (!candidate_list_ok(candidates, n_candidates) || tolerance_ppm > 1000000u) return RB200_E_ARG;
     for (uint32_t i = 0; i < n_candidates; i++)
-        if (!model_encode_args_ok(ctx, static_cast<int>(candidates[i] >> 8), candidates[i] & 0xffu, in, m, chunk_syms, out)) return RB200_E_ARG;
-    const size_t plane_cap = rb200_container_stored_bound(m, chunk_syms), table_end = container_planes_table_end(w);
-    if (out_cap < rb200_container_planes_bound(n, w, chunk_syms)) return RB200_E_SPACE;
+        if (!model_encode_args_ok(ctx, static_cast<int>(candidates[i] >> 8), candidates[i] & 0xffu, src, m, chunk_syms, out)) return RB200_E_ARG;
+    const uint64_t dir_bytes = refs ? container_tensors_dir_bytes(count) : 0;
+    const size_t plane_cap = rb200_container_stored_bound(m, chunk_syms), table_end = container_planes_table_end(w, dir_bytes);
+    if (out_cap < rb200_container_planes_bound(n, w, chunk_syms) + dir_bytes) return RB200_E_SPACE;
     DeviceGuard g(ctx->device);
     const uint64_t stride = round16(m);
     int rc = reserve(ctx, ctx->planes_in, w * stride);
     if (rc == RB200_OK) rc = reserve(ctx, ctx->planes_enc_stage, plane_cap);
+    if (rc == RB200_OK && refs) rc = reserve(ctx, ctx->tensors_enc_prefix, (count + 1ull) * sizeof(uint64_t));
     if (rc != RB200_OK) return rc;
     uint8_t* planes = static_cast<uint8_t*>(ctx->planes_in.p);
     uint8_t* stage = static_cast<uint8_t*>(ctx->planes_enc_stage.p);
-    PlanesVarlenGeom* geom = d_n ? ctx->d_planes_geom : nullptr;
+    PlanesVarlenGeom* geom = d_n || refs ? ctx->d_planes_geom : nullptr;
+    const TensorList list = {refs, count, static_cast<uint64_t*>(ctx->tensors_enc_prefix.p)};
     const AutoPlan a = plan_auto(candidates, n_candidates, tolerance_ppm);
-    if (geom) {
+    if (refs) {
+        tensors_plan_kernel<<<1, kTensorsPlanThreads, 0, ctx->stream>>>(refs, count, w, n, list.prefix, geom,
+                                                                        reinterpret_cast<uint64_t*>(out + container_planes_table_end(w, 0)));
+        rc = check_launch(ctx, "tensors_plan_kernel");
+        if (rc != RB200_OK) return rc;
+    } else if (geom) {
         planes_varlen_plan_kernel<<<1, 32, 0, ctx->stream>>>(d_n, n, w, geom);
         rc = check_launch(ctx, "planes_varlen_plan_kernel");
         if (rc != RB200_OK) return rc;
     }
-    rc = launch_split(ctx, w, in, base, m, geom, planes, stride);
+    rc = launch_split(ctx, w, in, base, m, geom, refs ? &list : nullptr, planes, stride);
     if (rc == RB200_OK && base) rc = launch_crc(ctx, base, n, nullptr, 0, &ctx->d_delta_enc->crc);
+    if (rc == RB200_OK && refs)
+        rc = launch_crc(ctx, out + container_planes_table_end(w, 0), 8ull * count, nullptr, 0, &ctx->d_tensors_enc->crc);
+    const uint32_t units = w + static_cast<uint32_t>(dir_bytes / 16);
     for (uint32_t p = 0; p < w && rc == RB200_OK; p++) {
         uint8_t* dst = p ? stage : out + table_end;
         rc = stored_encode(ctx, a, planes + p * stride, m, geom ? &geom->m : nullptr, chunk_syms, flags, dst, plane_cap);
         if (rc != RB200_OK) break;
-        planes_place_kernel<<<p ? planes_grid(ctx) : 1, kPlanesThreads, 0, ctx->stream>>>(out, dst, p, w, out_cap, ctx->d_planes_enc,
+        planes_place_kernel<<<p ? planes_grid(ctx) : 1, kPlanesThreads, 0, ctx->stream>>>(out, dst, p, units, out_cap, ctx->d_planes_enc,
                                                                                          ctx->d_status);
         rc = check_launch(ctx, "planes_place_kernel");
     }
@@ -2535,6 +2582,12 @@ int planes_encode(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candida
     h.n_symbols = n;
     h.flags = flags;
     h.block_size = h.n_blocks = w;
+    if (refs) {
+        h.version = kContainerVersionTensors;
+        h.n_blocks = count;
+        tensors_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, dir_bytes, geom, ctx->d_tensors_enc, ctx->d_planes_enc, ctx->d_status);
+        return check_launch(ctx, "tensors_finish_kernel");
+    }
     if (base) {
         delta_finish_kernel<<<1, 32, 0, ctx->stream>>>(out, h, ctx->d_delta_enc, ctx->d_planes_enc, ctx->d_status);
         return check_launch(ctx, "delta_finish_kernel");
@@ -2554,7 +2607,8 @@ extern "C" int rb200_container_planes_encode_async(rb200_ctx* ctx, const uint32_
                                                    uint32_t elem_bytes, const uint8_t* in, size_t n, uint32_t chunk_syms, uint32_t flags,
                                                    uint8_t* out, size_t out_cap)
 {
-    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, nullptr, n, nullptr, chunk_syms, flags, out, out_cap);
+    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, nullptr, n, nullptr, nullptr, 0, chunk_syms, flags, out,
+                         out_cap);
 }
 
 // rb200_container_planes_encode_async with the length read from device memory at every run: the plan kernel, the
@@ -2566,7 +2620,8 @@ extern "C" int rb200_container_planes_encode_varlen_async(rb200_ctx* ctx, const 
                                                           size_t n_max, uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
 {
     if (!d_n || (reinterpret_cast<uintptr_t>(d_n) & 7) || n_max == 0) return RB200_E_ARG;
-    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, nullptr, n_max, d_n, chunk_syms, flags, out, out_cap);
+    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, nullptr, n_max, d_n, nullptr, 0, chunk_syms, flags, out,
+                         out_cap);
 }
 
 namespace {
@@ -2575,28 +2630,35 @@ namespace {
 // workspace -- plane 0 in place, the others after a fetch into staging -- and a record kernel, then the verdict and the
 // interleave: 2 + 19 w launches, no copy, no synchronisation.
 // base set (rb200_container_delta_decode_async): version 8's plan, and between the verdict (delta_verdict_kernel, which
-// also writes the base's length) and the delta interleave the base's CRC and its check: 4 + 19 w launches.  Arguments
-// are checked by the callers.
-int planes_decode(rb200_ctx* ctx, uint32_t w, const uint8_t* buf, size_t size, const uint8_t* base, uint8_t* out, size_t out_cap,
-                  uint64_t* d_n_symbols)
+// also writes the base's length) and the delta interleave the base's CRC and its check: 4 + 19 w launches.
+// refs set (rb200_container_tensors_decode_async, with out_cap = n_max and no out): version 9's plan (tensors_open_kernel,
+// with count; plane 0 after the directory), and between the verdict and the segmented interleave the directory's CRC
+// and its check (tensors_check_kernel, which also writes d_lengths and the prefix): 4 + 19 w launches.  Arguments are
+// checked by the callers.
+int planes_decode(rb200_ctx* ctx, uint32_t w, const uint8_t* buf, size_t size, const uint8_t* base, const rb200_tensor_ref* refs, uint32_t count,
+                  uint8_t* out, size_t out_cap, uint64_t* d_n_symbols)
 {
     DeviceGuard g(ctx->device);
-    const uint64_t table_end = container_planes_table_end(w);
+    const uint64_t table_end = container_planes_table_end(w, refs ? container_tensors_dir_bytes(count) : 0);
     // every plane of n <= out_cap bytes has n / w <= out_cap / w symbols, and fewer than 2^32
     const uint64_t stride = round16(std::min<uint64_t>(out_cap / w, 0xffffffffull));
     const uint64_t stage_cap = round16(std::max<uint64_t>(size > table_end ? size - table_end : 0, sizeof(ContainerHeader)));
     int rc = reserve(ctx, ctx->planes_out, std::max<uint64_t>(w * stride, 16));
     if (rc == RB200_OK) rc = reserve(ctx, ctx->planes_dec_stage, stage_cap);
+    if (rc == RB200_OK && refs) rc = reserve(ctx, ctx->tensors_dec_prefix, (count + 1ull) * sizeof(uint64_t));
     if (rc != RB200_OK) return rc;
     uint8_t* planes = static_cast<uint8_t*>(ctx->planes_out.p);
     uint8_t* stage = static_cast<uint8_t*>(ctx->planes_dec_stage.p);
     PlanesWork* r = ctx->d_planes_dec;
+    const TensorList list = {refs, count, static_cast<uint64_t*>(ctx->tensors_dec_prefix.p)};
     cudaStream_t s = ctx->stream;
-    if (base)
+    if (refs)
+        tensors_open_kernel<<<1, 32, 0, s>>>(buf, size, w, count, r, ctx->d_tensors_dec);
+    else if (base)
         delta_plan_kernel<<<1, 32, 0, s>>>(buf, size, w, r);
     else
         planes_plan_kernel<<<1, 32, 0, s>>>(buf, size, w, r);
-    rc = check_launch(ctx, base ? "delta_plan_kernel" : "planes_plan_kernel");
+    rc = check_launch(ctx, refs ? "tensors_open_kernel" : base ? "delta_plan_kernel" : "planes_plan_kernel");
     for (uint32_t p = 0; p < w && rc == RB200_OK; p++) {
         if (p) {
             planes_fetch_kernel<<<planes_grid(ctx), kPlanesThreads, 0, s>>>(buf, stage, stage_cap, p, r);
@@ -2620,10 +2682,17 @@ int planes_decode(rb200_ctx* ctx, uint32_t w, const uint8_t* buf, size_t size, c
         delta_check_kernel<<<1, 32, 0, s>>>(buf, d, r, ctx->d_status);
         rc = check_launch(ctx, "delta_check_kernel");
     } else {
-        planes_verdict_kernel<<<1, 32, 0, s>>>(w, out_cap, d_n_symbols, r, ctx->d_status);
+        planes_verdict_kernel<<<1, 32, 0, s>>>(w, out_cap, refs ? nullptr : d_n_symbols, r, ctx->d_status);
         rc = check_launch(ctx, "planes_verdict_kernel");
     }
-    return rc == RB200_OK ? launch_interleave(ctx, w, planes, stride, base, out, r) : rc;
+    if (rc == RB200_OK && refs) {
+        TensorsWork* t = ctx->d_tensors_dec;
+        rc = launch_crc(ctx, buf + container_planes_table_end(w, 0), 8ull * count, &t->dir_len, 0, &t->crc);
+        if (rc != RB200_OK) return rc;
+        tensors_check_kernel<<<1, kTensorsPlanThreads, 0, s>>>(buf, w, count, refs, list.prefix, d_n_symbols, t, r, ctx->d_status);
+        rc = check_launch(ctx, "tensors_check_kernel");
+    }
+    return rc == RB200_OK ? launch_interleave(ctx, w, planes, stride, base, refs ? &list : nullptr, out, r) : rc;
 }
 
 }  // namespace
@@ -2632,7 +2701,7 @@ extern "C" int rb200_container_planes_decode_async(rb200_ctx* ctx, uint32_t elem
                                                    size_t out_cap, uint64_t* d_n_symbols)
 {
     if (!container_planes_w_ok(elem_bytes) || !async_args_ok(ctx, buf, out, d_n_symbols)) return RB200_E_ARG;
-    return planes_decode(ctx, elem_bytes, buf, size, nullptr, out, out_cap, d_n_symbols);
+    return planes_decode(ctx, elem_bytes, buf, size, nullptr, nullptr, 0, out, out_cap, d_n_symbols);
 }
 
 // The version 7 encode of the difference from base: planes_encode with base set, 3 + w * (11 to 15) launches.
@@ -2641,7 +2710,8 @@ extern "C" int rb200_container_delta_encode_async(rb200_ctx* ctx, const uint32_t
                                                   uint32_t flags, uint8_t* out, size_t out_cap)
 {
     if (!base || (reinterpret_cast<uintptr_t>(base) & 15)) return RB200_E_ARG;
-    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, base, n, nullptr, chunk_syms, flags, out, out_cap);
+    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, in, base, n, nullptr, nullptr, 0, chunk_syms, flags, out,
+                         out_cap);
 }
 
 // The version 7 decode applied to base: planes_decode with base set.  out == base applies the delta in place; any other
@@ -2654,7 +2724,30 @@ extern "C" int rb200_container_delta_decode_async(rb200_ctx* ctx, uint32_t elem_
     if (!base || (reinterpret_cast<uintptr_t>(base) & 15)) return RB200_E_ARG;
     const uintptr_t o = reinterpret_cast<uintptr_t>(out), b = reinterpret_cast<uintptr_t>(base);
     if (o != b && o < b + out_cap && b < o + out_cap) return RB200_E_ARG;
-    return planes_decode(ctx, elem_bytes, buf, size, base, out, out_cap, d_n_symbols);
+    return planes_decode(ctx, elem_bytes, buf, size, base, nullptr, 0, out, out_cap, d_n_symbols);
+}
+
+// The version 7 varlen encode of a list's concatenated bytes, read through the list: planes_encode with refs set.
+// Launches: the version 7 varlen call's (1 + 1 + w x (the version 6 varlen encode + 1) + 1), with tensors_plan_kernel
+// and tensors_finish_kernel in place of its plan and finish kernels, plus one for the directory's CRC -- whatever T is.
+extern "C" int rb200_container_tensors_encode_async(rb200_ctx* ctx, const uint32_t* candidates, uint32_t n_candidates, uint32_t tolerance_ppm,
+                                                    uint32_t elem_bytes, const rb200_tensor_ref* d_refs, uint32_t count, size_t n_max,
+                                                    uint32_t chunk_syms, uint32_t flags, uint8_t* out, size_t out_cap)
+{
+    if (!d_refs || !count || count > kContainerTensorsMax) return RB200_E_ARG;
+    return planes_encode(ctx, candidates, n_candidates, tolerance_ppm, elem_bytes, nullptr, nullptr, n_max, nullptr, d_refs, count, chunk_syms,
+                         flags, out, out_cap);
+}
+
+// The version 7 decode into a list's outputs: planes_decode with refs set, with n_max as the workspaces' bound.
+// Launches: version 7's 2 + 19 w, plus the directory's CRC and tensors_check_kernel -- whatever T is.
+extern "C" int rb200_container_tensors_decode_async(rb200_ctx* ctx, uint32_t elem_bytes, const uint8_t* buf, size_t size,
+                                                    const rb200_tensor_ref* d_refs, uint32_t count, size_t n_max, uint64_t* d_lengths)
+{
+    if (!container_planes_w_ok(elem_bytes) || !d_refs || !async_args_ok(ctx, buf, reinterpret_cast<const uint8_t*>(d_refs), d_lengths))
+        return RB200_E_ARG;
+    if (!count || count > kContainerTensorsMax || n_max == 0) return RB200_E_ARG;
+    return planes_decode(ctx, elem_bytes, buf, size, nullptr, d_refs, count, nullptr, n_max, d_lengths);
 }
 
 extern "C" int rb200_container_blocks_auto_costs(rb200_ctx* ctx, uint64_t* costs, uint32_t n)

@@ -1409,6 +1409,126 @@ def delta(args):
     return res
 
 
+def tensor_list_shapes(name):
+    """(a) 8 transformer layers at hidden size 2048 (q, k, v, o 2048 x 2048; gate, up, down 2048 x 8192; two norms of
+    2048): 72 tensors, 1 GiB in bf16; (b) a LoRA-like list of 448 tensors of 64 Ki elements (128 KiB in bf16)"""
+    if name == "lora":
+        return [1 << 16] * 448
+    layer = [2048 * 2048] * 4 + [2048 * 8192] * 3 + [2048, 2048]
+    return layer * 8
+
+
+def tensors(args):
+    """version 9 on three lists -- (a) 8 layers at hidden 2048 in bf16, (b) 448 LoRA-like bf16 tensors of 128 KiB, (c)
+    list (a) in fp32 -- against T version 7 calls (looped, and as one captured graph) and one version 7 call on the
+    already-concatenated bytes (the floor)"""
+    import torch
+    chunk, tol = 8192, 20000
+    cands = [api.CANDIDATE(rb.CODER_WORD, 12), api.CANDIDATE(rb.CODER_ALIAS, 16), api.CANDIDATE(rb.CODER_BYTE, 14)]
+    stream = torch.cuda.Stream()
+    ctx = rb.Context(0, stream=stream.cuda_stream)
+    sync = ctx.sync
+    res = {"card": card(), "workload": {"chunk_syms": chunk, "data": "N(0, 0.02) per tensor"}, "candidates": ["word 12", "alias 16", "byte 14"],
+           "tolerance_ppm": tol, "workloads": {}, "checks": {}}
+    gen = torch.Generator(device="cuda").manual_seed(99)
+    for name, shape, dtype, w in (("a_layers_bf16", "layers", torch.bfloat16, 2), ("b_lora_bf16", "lora", torch.bfloat16, 2),
+                                  ("c_layers_fp32", "layers", torch.float32, 4)):
+        counts = tensor_list_shapes(shape)
+        t_count = len(counts)
+        ts = [(torch.randn(c, device="cuda", generator=gen) * 0.02).to(dtype).view(torch.uint8) for c in counts]
+        lengths = [t.numel() for t in ts]
+        n = sum(lengths)
+        cat = torch.cat(ts)
+        refs = torch.tensor([[t.data_ptr(), t.numel()] for t in ts], dtype=torch.int64, device="cuda")
+        bound9 = api.container_tensors_bound(n, t_count, w, chunk)
+        bound7 = api.container_planes_bound(n, w, chunk)
+        d_v9 = torch.empty(bound9, dtype=torch.uint8, device="cuda")
+        d_v7 = torch.empty(bound7, dtype=torch.uint8, device="cuda")
+        b7 = [api.container_planes_bound(b, w, chunk) for b in lengths]
+        offs = np.concatenate([[0], np.cumsum([(b + 15) // 16 * 16 for b in b7])]).astype(np.int64)
+        d_each = torch.empty(int(offs[-1]), dtype=torch.uint8, device="cuda")
+        outs = [torch.empty_like(t) for t in ts]
+        orefs = torch.tensor([[o.data_ptr(), o.numel()] for o in outs], dtype=torch.int64, device="cuda")
+        d_dec = torch.empty(n + 16, dtype=torch.uint8, device="cuda")
+        o9, o7, oe, dd = d_v9.data_ptr(), d_v7.data_ptr(), d_each.data_ptr(), d_dec.data_ptr()
+
+        def enc_each():
+            for t, o, b in zip(ts, offs, b7):
+                ctx.container_planes_encode_async(cands, tol, w, t.data_ptr(), t.numel(), chunk, 0, oe + int(o), b)
+
+        with torch.cuda.stream(stream):
+            ctx.container_tensors_encode_async(cands, tol, w, refs.data_ptr(), t_count, n, chunk, 0, o9, bound9)
+            ctx.container_planes_encode_async(cands, tol, w, cat.data_ptr(), n, chunk, 0, o7, bound7)
+            enc_each()
+            sync()
+            size9 = 64 + 16 * w + (8 * t_count + 15) // 16 * 16 + int(d_v9[:64].cpu().numpy()[32:40].view(np.uint64)[0])
+            size7 = 64 + 16 * w + int(d_v7[:64].cpu().numpy()[32:40].view(np.uint64)[0])
+            sizes_each = []
+            for o in offs[:-1]:
+                h = d_each[int(o):int(o) + 64].cpu().numpy()
+                sizes_each.append(64 + 16 * w + int(h[32:40].view(np.uint64)[0]))
+            # the version 9 planes are the concatenation's version 7 planes
+            res["checks"][f"{name}: v9_planes_equal_v7_of_concatenation"] = bool(torch.equal(
+                d_v9[64 + 16 * w + (8 * t_count + 15) // 16 * 16:size9], d_v7[64 + 16 * w:size7]))
+
+            def dec_each():
+                at = 0
+                for o, s_, b in zip(offs, sizes_each, lengths):
+                    ctx.container_planes_decode_async(w, oe + int(o), s_, dd + at, b)
+                    at += b
+
+            dec_each()
+            ctx.container_tensors_decode_async(w, o9, size9, orefs.data_ptr(), t_count, n)
+            ctx.container_planes_decode_async(w, o7, size7, dd, n)
+            sync()
+            g_enc, g_dec = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g_enc, stream=stream):
+                enc_each()
+            with torch.cuda.graph(g_dec, stream=stream):
+                dec_each()
+            enc = {"v9_one_call": lambda: ctx.container_tensors_encode_async(cands, tol, w, refs.data_ptr(), t_count, n, chunk, 0, o9, bound9),
+                   "v7_T_calls_looped": enc_each,
+                   "v7_T_calls_graph": g_enc.replay,
+                   "v7_concatenated_floor": lambda: ctx.container_planes_encode_async(cands, tol, w, cat.data_ptr(), n, chunk, 0, o7, bound7)}
+            dec = {"v9_one_call": lambda: ctx.container_tensors_decode_async(w, o9, size9, orefs.data_ptr(), t_count, n),
+                   "v7_T_calls_looped": dec_each,
+                   "v7_T_calls_graph": g_dec.replay,
+                   "v7_concatenated_floor": lambda: ctx.container_planes_decode_async(w, o7, size7, dd, n)}
+            etimes = alternate(enc, sync, args.warmup, args.reps)
+            dtimes = alternate(dec, sync, args.warmup, args.reps)
+            for o in outs:
+                o.zero_()
+            dec["v9_one_call"]()
+            sync()
+            res["checks"][f"{name}: v9_round_trip"] = all(bool(torch.equal(o, t)) for o, t in zip(outs, ts))
+            ek9 = kernel_times(enc["v9_one_call"], sync, args.reps)
+            ek7 = kernel_times(enc["v7_concatenated_floor"], sync, args.reps)
+            dk9 = kernel_times(dec["v9_one_call"], sync, args.reps)
+            dk7 = kernel_times(dec["v7_concatenated_floor"], sync, args.reps)
+            del g_enc, g_dec
+
+        def rate(kernels, part):
+            us = sum(v["median_us"] * v["launches_per_call"] for k, v in kernels.items() if part in k)
+            return {"us": us, "TB_per_s": 2 * n / us / 1e6 if us else None}
+
+        res["workloads"][name] = {
+            "tensors": t_count, "n": n,
+            "bytes_per_input_byte": {"v9": size9 / n, "v7_T_containers": sum(sizes_each) / n, "v7_concatenated": size7 / n},
+            "encode": etimes, "decode": dtimes,
+            "v9_minus_floor_encode_ms": etimes["v9_one_call"]["median_ms"] - etimes["v7_concatenated_floor"]["median_ms"],
+            "v9_minus_floor_decode_ms": dtimes["v9_one_call"]["median_ms"] - dtimes["v7_concatenated_floor"]["median_ms"],
+            "tensors_split_kernel": rate(ek9, "tensors_split_kernel"), "planes_split_kernel": rate(ek7, "planes_split_kernel"),
+            "tensors_interleave_kernel": rate(dk9, "tensors_interleave_kernel"),
+            "planes_interleave_kernel": rate(dk7, "planes_interleave_kernel"),
+            "launches_per_call": {"v9_encode": sum(v["launches_per_call"] for v in ek9.values()),
+                                  "v9_decode": sum(v["launches_per_call"] for v in dk9.values())},
+        }
+        del ts, cat, refs, d_v9, d_v7, d_each, outs, orefs, d_dec
+        torch.cuda.empty_cache()
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", action="store_true", help="the per-block container on 8192 blocks of 64 KiB")
@@ -1426,13 +1546,14 @@ def main():
     ap.add_argument("--planes", action="store_true", help="the byte-plane container (version 7) against version 6 on bf16 and fp32")
     ap.add_argument("--planes-varlen", action="store_true", help="the byte-plane encode with the length in device memory, on bf16 and fp32")
     ap.add_argument("--delta", action="store_true", help="the delta byte-plane container (version 8) against version 7 on bf16 and fp32")
+    ap.add_argument("--tensors", action="store_true", help="the tensor-list container (version 9) against T version 7 calls and the concatenation")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "needs a CUDA device"
-    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else stored_varlen(args) if args.stored_varlen else blocks_stored_varlen(args) if args.blocks_stored_varlen else planes(args) if args.planes else planes_varlen(args) if args.planes_varlen else delta(args) if args.delta else headline(args)
+    res = blocks(args) if args.blocks else blocks_coder(args) if args.blocks_coder else blocks_alias(args) if args.blocks_alias else single(args) if args.single else model_encode(args) if args.model else auto_encode(args) if args.auto else blocks_auto(args) if args.blocks_auto else blocks_varlen(args) if args.blocks_varlen else blocks_stored(args) if args.blocks_stored else stored(args) if args.stored else stored_varlen(args) if args.stored_varlen else blocks_stored_varlen(args) if args.blocks_stored_varlen else planes(args) if args.planes else planes_varlen(args) if args.planes_varlen else delta(args) if args.delta else tensors(args) if args.tensors else headline(args)
     print(json.dumps(res, indent=1))
     if args.json:
         with open(args.json, "w") as f:
